@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — groupby-agg rows/sec on B200 (BASELINE.json metric), roofline and CPU baseline.
+"""bench.py — groupby-agg rows/sec on H100 (BASELINE.json metric), roofline and CPU baseline.
 
 Workload (config.workload): BASELINE.json configs[1] "2B-row int64 2-col, 1M-group groupby SUM/COUNT on
-1xB200"; with --gpus N > 1 it is configs[3] (the same 2B rows sharded across N GPUs, strong scaling, one
+1xH100"; with --gpus N > 1 it is configs[3] (the same 2B rows sharded across N GPUs, strong scaling, one
 hash-partition exchange of the partial aggregates over NCCL).  One step = one whole operator lifetime over
 the batch: init state -> consume all local rows -> (exchange) -> finalize -> produce.
 
@@ -11,6 +11,9 @@ the batch: init state -> consume all local rows -> (exchange) -> finalize -> pro
   roofline  consume kernel: 16 B/row (8 B key + 8 B value, SURVEY.md §8d) / its mean launch time, measured with
             CUDA events on the kernel's stream, against MEASURED_PEAKS.json hbm_gbs
   cpu_baseline  the CPU oracle (reference algorithm shape, one rank per host thread) on a bounded sample
+
+`--dump-outputs DIR` writes what the last timed step returned (key, sum, count; rows ordered by key, as float64) to
+DIR/<name>.npy, so that two builds can be compared output for output on the same seeded input.
 
 `--impl reference` times only that CPU restatement (the reference runtime cannot be built here: no MPI).
 
@@ -37,17 +40,11 @@ sys.path.insert(0, ROOT)
 METRIC = "groupby-agg rows/sec"
 UNIT = "rows/s"
 BYTES_PER_ROW = 16  # algorithmic bytes of the hash-aggregate scan (SURVEY.md §8d)
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu --set full captures (profiles/):
-# filled in from profiles/r01_*.txt for the 2^26-row launch of the default workload; None = not captured
-# spg: profiles/r01_spg_ncu_summary.txt, K1 1.074+1.019 GB + K2 1.123+0.004 GB per 2^26-row launch pair (3x the
-# algorithmic 1.074 GB by design: rows are written to and re-read from owner buckets).
-# direct: profiles/r01_direct_ncu_summary.txt (2^27-row launch, bucketized variant): 10.99 + 0.18 GB.
-# Both are DRAM bytes per ROW of a launch (measured bytes / rows of the captured launch); one launch of the timed run
-# moves that figure x its own row count (launches are 2^27 rows now, the captures above were taken on 2^26 / 2^27).
-# spgn (narrow bucket rows, the path the default workload takes since round 2): profiles/r02_launches.txt (105 launches of the
-# shipping 2^27-row kernels): K1n 2.133 + 1.029 GB, K2n 1.116 + 0.000 GB = 4.279 GB = 31.9 B/row (16 read + 8 bucket write +
-# 8 bucket read by design).
-TRAFFIC_PER_ROW = {"spg": 3.220e9 / (1 << 26), "spgn": 4.279e9 / (1 << 27), "direct": 11.17e9 / (1 << 27)}
+# HBM bytes per row the SM-partitioned kernels move by design (not a measurement): spgn reads the 16-byte row, writes and
+# re-reads an 8-byte owner-bucket row; spg does the same with 16-byte bucket rows.  The direct kernel's traffic depends on
+# how much of its hash table the L2 holds, so it has no design figure.
+TRAFFIC_PER_ROW = {"spg": 48.0, "spgn": 32.0, "direct": None}
+DUMP_MAX_BYTES = 64 << 20  # --dump-outputs: larger outputs are written as a fixed, seeded sample of rows
 
 
 def parse_args():
@@ -77,6 +74,8 @@ def parse_args():
     ap.add_argument("--probe-batch", type=int, default=250_000_000)
     ap.add_argument("--sample-lo", type=int, default=1000, help="join parity: sorted row-set equality for keys in [lo, hi)")
     ap.add_argument("--sample-hi", type=int, default=1400)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float64; flagship groupby workload only)")
     return ap.parse_args()
 
 
@@ -87,7 +86,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "fallback"  # H100 SXM data-sheet HBM3 bandwidth, not a measurement
 
 
 class ClockSampler:
@@ -219,13 +218,34 @@ def reference_arm(args):
 
 def workload_name(args):
     if args.gpus == 1:
-        return f"{args.rows}-row int64 2-col, {args.groups}-group groupby SUM/COUNT on 1xB200 (BASELINE.json configs[1])"
-    return (f"{args.rows}-row {args.groups}-group groupby SUM/COUNT sharded across {args.gpus}xB200, hash-partition "
+        return f"{args.rows}-row int64 2-col, {args.groups}-group groupby SUM/COUNT on 1xH100 (BASELINE.json configs[1])"
+    return (f"{args.rows}-row {args.groups}-group groupby SUM/COUNT sharded across {args.gpus}xH100, hash-partition "
             f"exchange of partial aggregates over NCCL (BASELINE.json configs[3])")
+
+
+def dump_outputs(out_dir, arrays, rank, world):
+    """Writes the named output columns (rows ordered by key) as float64 .npy files; above DUMP_MAX_BYTES, a fixed seeded
+    sample of rows.  With several ranks every rank writes its own part (<name>_rank<r>.npy)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    cols = {name: a.cpu().numpy() for name, a in arrays.items()}
+    order = np.argsort(cols["key"], kind="stable")
+    n = len(order)
+    cap = DUMP_MAX_BYTES // (8 * len(cols) * max(world, 1))
+    if n > cap:
+        order = order[np.sort(np.random.default_rng(0).choice(n, cap, replace=False))]
+    for name, a in cols.items():
+        fn = f"{name}.npy" if world == 1 else f"{name}_rank{rank}.npy"
+        np.save(os.path.join(out_dir, fn), a[order].astype(np.float64))
 
 
 def main():
     args = parse_args()
+    flagship = (args.workload == "groupby" and args.impl == "b200" and args.aggs.replace(" ", "") == "sum,count" and not args.nullable
+                and args.key_dtype == "int64" and args.val_dtype == "int64")
+    if args.dump_outputs is not None and (not flagship or args.steps < 1):
+        raise SystemExit("--dump-outputs needs the flagship groupby workload (--impl b200, sum,count over int64) and --steps >= 1")
     if args.workload == "join":
         from benchmarks import join_bench
 
@@ -280,7 +300,7 @@ def main():
 
     stats = {}
 
-    def one_step(tab, collect=False, profile=False, to_host=False, hint=None):
+    def one_step(tab, collect=False, profile=False, to_host=False, hint=None, keep=False):
         st = G.init_groupby_state(-1, (0,), ("sum", "count"), (0, 1, 2), (1, 1), parallel=world > 1,
                                   expected_groups=exp_groups_local if hint is None else hint,
                                   output_batch_size=1 << 40, device=local_rank, stream=stream_ptr)
@@ -294,6 +314,9 @@ def main():
         if to_host:
             res = [c.values_numpy(stream_ptr) for c in out.columns]
             stats["d2h"] = sum(a.nbytes for a in res)
+        if keep:  # the state owns the output columns: copy them before it is deleted
+            stats["dump"] = {name: torch.as_tensor(c.data, device=dev)[:out.n_rows].clone()
+                             for name, c in zip(("key", "sum", "count"), out.columns)}
         if collect:
             cols = [torch.as_tensor(c.data, device=dev) for c in out.columns]
             stats["n_out"] = out.n_rows
@@ -358,12 +381,14 @@ def main():
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     ev0.record(stream)
-    for _ in range(args.steps):
-        one_step(table)
+    for i in range(args.steps):
+        one_step(table, keep=args.dump_outputs is not None and i == args.steps - 1)
     ev1.record(stream)
     barrier()
     ms = ev0.elapsed_time(ev1)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs is not None:
+        dump_outputs(args.dump_outputs, stats.pop("dump"), rank, world)
 
     # the same steps WITHOUT the expected_groups hint (the reference's API has no such argument: a drop-in caller gets this
     # route — the state learns the cardinality from a 2^20-row prefix through the direct kernel, then takes the same kernels)
@@ -402,8 +427,9 @@ def main():
     kern_us = stats.get("consume_us", 0)
     n_launch = max(stats.get("consume_launches", 1), 1)
     achieved = (BYTES_PER_ROW * n_local / 1e9) / (kern_us * 1e-6) if kern_us else None
+    design_bpr = TRAFFIC_PER_ROW["spgn" if stats.get("spgn_launches") else "spg" if stats.get("spg_launches") else "direct"]
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": (achieved / peak) if achieved else None,
-                "traffic": TRAFFIC_PER_ROW["spgn" if stats.get("spgn_launches") else "spg" if stats.get("spg_launches") else "direct"] * n_local / n_launch,
+                "traffic": design_bpr * n_local / n_launch if design_bpr else None,
                 "peak_kind": peak_kind,
                 "kernel": ("spgn_partition_kernel<true,true> + spgn_aggregate_kernel<true,true> (narrow bucket rows; one launch = the pair)"
                            if stats.get("spgn_launches") else
@@ -464,7 +490,7 @@ def main():
             "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
             "dtype": "int64", "data": "synthetic",
             "config": {"workload": workload_name(args), "rows": args.rows, "groups": args.groups, "aggs": ["sum", "count"],
-                       "rows_per_gpu": n_local, "l2": "inputs (16 B/row x rows_per_gpu) exceed the 126 MB L2; no flush needed",
+                       "rows_per_gpu": n_local, "l2": "inputs (16 B/row x rows_per_gpu) exceed the 50 MB L2; no flush needed",
                        "step": "init state + consume + exchange + finalize + produce", "result_groups": n_groups_total,
                        "expected_groups_hint": exp_groups_local,
                        "no_hint": {"value": args.rows * args.steps / (no_hint_ms * 1e-3), "ms_per_step": no_hint_ms / args.steps,

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Secondary benchmark (not the bench.py contract): the Zipf variant of BASELINE.json configs[1] named in SURVEY.md §8(d) —
 hash-aggregate SUM+COUNT over int64 (key, value) rows whose keys follow Zipf(s) over n_groups groups (a few hot keys
-carry most of the rows), 1 x B200, inputs resident in HBM.
+carry most of the rows), 1 x H100, inputs resident in HBM.
 
     python benchmarks/bench_skew.py [--rows 536870912] [--groups 1000000] [--s 1.1] [--batch 134217728]
 
@@ -81,7 +81,7 @@ def main():
     ms = min(times)
     print(json.dumps({"metric": "groupby_agg_rows_per_sec_zipf", "value": n / ms * 1e3, "unit": "rows/s", "ms": ms, "all_ms": times,
                       "config": {"workload": f"{n} rows, {g} groups, Zipf(s={args.s}) keys, SUM+COUNT int64", "top_key_share": top_share},
-                      "result_check": "ok" if ok else "MISMATCH", "metrics": metrics, "roofline_frac": n * 16 / ms / 1e6 / 6574.8}))
+                      "result_check": "ok" if ok else "MISMATCH", "metrics": metrics, "roofline_frac": n * 16 / ms / 1e6 / 3350.0}))
 
 
 if __name__ == "__main__":

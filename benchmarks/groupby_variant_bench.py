@@ -1,6 +1,6 @@
 """bench.py --aggs ... [--nullable] [--key-dtype int32] [--val-dtype int32]: the groupby hot path on signatures OTHER than the
 headline one (BASELINE.json configs[1] shape — `--rows` rows, `--groups` groups — with other aggregate functions, nullable
-columns, 4-byte columns), 1 x B200.
+columns, 4-byte columns), 1 x H100.
 
 One step = init state -> consume one device-resident batch -> finalize -> produce, as bench.py's headline step.
   value     rows/s with the inputs resident in HBM (CUDA events around `--steps` steps)
@@ -184,10 +184,10 @@ def run(args, ClockSampler, peaks):
         "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
         "dtype": f"{args.key_dtype} key / {args.val_dtype} value", "data": "synthetic",
         "config": {"workload": f"{n}-row {ng}-group groupby {','.join(aggs)} ({'nullable' if args.nullable else 'non-null'} "
-                               f"{args.key_dtype} key, {args.val_dtype} value{', 1 % NA keys, 10 % NA values' if args.nullable else ''}) on 1xB200 "
+                               f"{args.key_dtype} key, {args.val_dtype} value{', 1 % NA keys, 10 % NA values' if args.nullable else ''}) on 1xH100 "
                                "— a VARIANT of BASELINE.json configs[1], not the headline signature",
                    "rows": n, "groups": ng, "aggs": list(aggs), "nullable": bool(args.nullable), "expected_groups_hint": hint,
-                   "l2": "inputs exceed the 126 MB L2; no flush needed", "step": "init state + consume + finalize + produce",
+                   "l2": "inputs exceed the 50 MB L2; no flush needed", "step": "init state + consume + finalize + produce",
                    "result_groups": stats["out"].n_rows,
                    "result_check": ("per-group ok: every group's aggregates equal an independent device recomputation" if ok
                                     else f"MISMATCH ({n_bad} bad groups, {n_expected} expected)")},

@@ -1,5 +1,5 @@
 """bench.py --workload join: BASELINE.json configs[2] — hash inner join 1 B x 100 M int64 key, 4 payload columns (2 per side)
-on 1 x B200, through the streaming join operator API (bodo_b200.streaming.join).
+on 1 x H100, through the streaming join operator API (bodo_b200.streaming.join).
 
 One step = one whole operator lifetime: init state -> build (one 100 M-row batch) -> probe in `--probe-batch`-row batches,
 every batch materialising its joined rows (kept columns: k, b1, b2 of the build side, p1, p2 of the probe side).
@@ -29,7 +29,7 @@ UNIT = "rows/s"
 
 
 def workload_name(args):
-    return (f"hash inner join {args.probe_rows} x {args.build_rows} int64 key, 2 payload cols per side on 1xB200 "
+    return (f"hash inner join {args.probe_rows} x {args.build_rows} int64 key, 2 payload cols per side on 1xH100 "
             "(BASELINE.json configs[2])")
 
 
@@ -232,7 +232,7 @@ def run(args, ClockSampler, peaks):
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps,
         "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "int64", "data": "synthetic",
         "config": {"workload": workload_name(args), "build_rows": nb, "probe_rows": npr, "probe_batch": batch, "out_rows": out_rows,
-                   "l2": "inputs and outputs (66 GB per step) exceed the 126 MB L2; no flush needed",
+                   "l2": "inputs and outputs (66 GB per step) exceed the 50 MB L2; no flush needed",
                    "step": "init state + build (insert, CSR, payload pack) + probe batches with output materialisation",
                    "result_check": ("ok: row count, sum mod 2^64 of all 5 output columns vs inverse-permutation gathers, sorted row-set equality for keys in "
                                     f"[{args.sample_lo}, {args.sample_hi}) ({got_s.shape[0]} rows)") if check_ok else "MISMATCH"},

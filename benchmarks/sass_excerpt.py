@@ -1,8 +1,8 @@
 """Disassemble bodo_b200/libbodo_b200.so (cuobjdump -sass) and list, per kernel, the instructions that prove which hardware
 paths it uses: UBLKCP (TMA bulk copy, cp.async.bulk), SYNCS (mbarrier), REDUX (warp reduce), ATOMS / ATOMG / RED (shared /
-global atomics), LDG.E.128 / STG.E.128 (16-byte global accesses), plus the register count.  Output: profiles/rNN_sass_excerpt.txt
+global atomics), LDG.E.128 / STG.E.128 (16-byte global accesses), plus the register count.  Output: stdout
 
-    python benchmarks/sass_excerpt.py > profiles/r02_sass_excerpt.txt
+    python benchmarks/sass_excerpt.py > sass_excerpt.txt
 """
 import collections
 import os
@@ -54,7 +54,7 @@ def main():
             if p in ins.split()[0] or (ins.startswith("@") and len(ins.split()) > 1 and p in ins.split()[1]):
                 counts[cur][p] += 1
                 first[cur].setdefault(p, ins)
-    print(f"# SASS excerpt of {os.path.relpath(LIB, ROOT)} (cuobjdump -sass, sm_100a only); counts are static instruction sites")
+    print(f"# SASS excerpt of {os.path.relpath(LIB, ROOT)} (cuobjdump -sass, sm_90a only); counts are static instruction sites")
     arch = set(re.findall(r"arch = (sm_\w+)", sass))
     print(f"# architectures in the fatbin: {sorted(arch)}")
     for fn, c in counts.items():

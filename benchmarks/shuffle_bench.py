@@ -134,10 +134,10 @@ def run(args, ClockSampler, peaks):
             "metric": METRIC, "value": args.rows * args.steps / (ms * 1e-3), "unit": UNIT, "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
             "dtype": "int64", "data": "synthetic",
-            "config": {"workload": f"raw-row hash shuffle of a {args.rows}-row int64 2-col table over {world}xB200 "
+            "config": {"workload": f"raw-row hash shuffle of a {args.rows}-row int64 2-col table over {world}xH100 "
                                    f"({'partition into ' + str(n_dest) + ' destinations, no exchange' if world == 1 else 'radix partition + NCCL all-to-all-v'}; "
                                    "raw-row variant of BASELINE.json configs[3])",
-                       "rows": args.rows, "rows_per_gpu": n, "n_dest": n_dest, "l2": "inputs exceed the 126 MB L2; no flush needed",
+                       "rows": args.rows, "rows_per_gpu": n, "n_dest": n_dest, "l2": "inputs exceed the 50 MB L2; no flush needed",
                        "step": "partition (hist + scan + scatter)" + (" + count exchange + all-to-all-v of 2 buffers" if world > 1 else ""),
                        "result_check": "counts, per-destination key/value sums, stable order, placement ok" if ok else "MISMATCH"},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,

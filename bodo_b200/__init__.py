@@ -1,6 +1,6 @@
-"""bodo_b200 — B200-native streaming hash groupby / hash join / row->rank shuffle behind Bodo's operator API.
+"""bodo_b200 — CUDA-native (H100) streaming hash groupby / hash join / row->rank shuffle behind Bodo's operator API.
 
-The compute path is libbodo_b200.so (hand-written sm_100a CUDA, include/bodo_b200.h); this package is the
+The compute path is libbodo_b200.so (hand-written sm_90a CUDA, include/bodo_b200.h); this package is the
 thin Python host layer that mirrors the reference's operator interface (bodo/libs/streaming/groupby.py,
 join.py, bodo/libs/array.py shuffle_table).  There is no CPU fallback.
 """

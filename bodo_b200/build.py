@@ -1,4 +1,4 @@
-"""In-tree build of libbodo_b200.so (nvcc, sm_100a only). Used by __graft_entry__.build() and `python -m bodo_b200.build`."""
+"""In-tree build of libbodo_b200.so (nvcc, sm_90a only). Used by __graft_entry__.build() and `python -m bodo_b200.build`."""
 
 from __future__ import annotations
 
@@ -11,8 +11,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbodo_b200.so")
 SOURCES = ["misc.cu", "groupby.cu", "shuffle.cu", "join.cu", "expr.cu"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper); the kernels use sm_90a TMA / mbarrier PTX
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    *GENCODE, "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function", "--expt-relaxed-constexpr",
 ]
 
@@ -28,7 +29,8 @@ def needs_build() -> bool:
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "bodo_b200.h")]
+    # build.py itself counts: a library built with other flags (another target architecture) is rebuilt
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "bodo_b200.h"), os.path.abspath(__file__)]
     return any(os.path.getmtime(d) > t for d in deps)
 
 
@@ -53,7 +55,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if verbose and out:
             print(out)
         objs.append(obj)
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, *GENCODE]
     subprocess.check_call(cmd)
     return LIB
 

@@ -1,4 +1,4 @@
-// common.cuh — shared device/host helpers for libbodo_b200.so (sm_100a only).
+// common.cuh — shared device/host helpers for libbodo_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -205,7 +205,7 @@ __host__ __device__ __forceinline__ uint64_t mix64(uint64_t x) {
 inline int num_sms(int device) {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device);
-    return n > 0 ? n : 148;
+    return n > 0 ? n : 132;  // H100 SXM
 }
 
 // Scratch buffers (bucket / retry / fail lists: up to GBs) come from a process-wide per-device pool and go back to

@@ -1,4 +1,4 @@
-// expr.cu — fused filter + projection front end of the aggregate / join pipelines (sm_100a).
+// expr.cu — fused filter + projection front end of the aggregate / join pipelines (sm_90a).
 //
 // Replaces PhysicalFilter + PhysicalProjection with their expression trees (bodo/pandas/physical/filter.h, project.h,
 // expression.{h,cpp}; GPU twins: cudf::ast expressions + cudf::apply_boolean_mask, gpu_expression.cpp:601+, gpu_filter.h:143)

@@ -1,4 +1,4 @@
-// groupby.cu — streaming hash groupby/aggregate on one B200 (sm_100a).
+// groupby.cu — streaming hash groupby/aggregate on one GPU (H100, sm_90a).
 //
 // Replaces GroupbyState + groupby_agg_build_consume_batch + FinalizeBuild of the reference
 // (bodo/libs/streaming/_groupby.cpp:2554-3031, 4325-4457, 4062-4256) and the aggregate kernels of
@@ -67,8 +67,8 @@ struct ConsumeArgs {
 
 // find-or-insert with linear probing over 8-byte key slots; returns the slot, or UINT64_MAX when the table is at
 // its group limit (group_limit < 0 disables the limit: rehash into a table that is known to be large enough).
-// Measured on B200 (scratch/ubench2.cu, profiles/r01_ubench2.txt): a 4-key bucket fetched with one 256-bit load
-// is SLOWER than this (29 vs 40 Grows/s) — L2 random-request rate, not probe-chain latency, is the limit.
+// Bucketed 4-key variants of this probe (scratch/ubench2.cu) issue more L2 requests per row; the L2 random-request rate,
+// not probe-chain latency, is what limits this path.
 __device__ __forceinline__ uint64_t find_or_insert(long long* __restrict__ tkeys, uint64_t cap, long long key,
                                                    long long* counters, long long group_limit) {
     uint64_t mask = cap - 1;
@@ -979,8 +979,8 @@ __global__ void eval_mk_keys_kernel(const __grid_constant__ EvalMkKeysArgs a) {
 
 // ================================================================================================
 // SM-partitioned groupby (SPG): the fast path for cardinalities whose accumulators fit the chip's
-// aggregate shared memory (≈148 x 10k groups).  Motivation (profiles/r01_ubench*.txt): two global `red`s per
-// row cap the direct kernel at ≈85 Grows/s and the key probe halves that again (L2 random-request rate), while
+// aggregate shared memory (≈ SMs x 10k groups).  Motivation (scratch/ubench*.cu): two global `red`s per
+// row cap the direct kernel well below the HBM stream rate and the key probe halves that again (L2 random-request rate), while
 // 32-bit shared-memory atomics sustain the full HBM stream rate.  So rows travel to the SM that owns their key:
 //
 //   K1 spg_partition_kernel : every CTA counting-sorts TILE-row tiles by owner (= mulhi(hash, n_owners)) in
@@ -990,8 +990,8 @@ __global__ void eval_mk_keys_kernel(const __grid_constant__ EvalMkKeysArgs a) {
 //        SUM = two native 32-bit atomics with carry, COUNT = one), then flushes the table into the state's
 //        global table with the ordinary find-or-insert + `red` (each key has one owner: <= n_groups per launch).
 //   Algorithmic HBM traffic: 16 B/row read + 16 B/row bucket write + 16 B/row bucket read.
-// A persistent single-kernel variant (L2-resident inboxes, inter-CTA barriers) was measured slower
-// (profiles/r01_spg_persistent.txt): per-chunk work per SM is too small to amortise the barrier latency.
+// A persistent single-kernel variant (L2-resident inboxes, inter-CTA barriers) is not used: per-chunk work per SM is
+// too small to amortise the barrier latency.
 // Rows that do not fit (bucket overflow under skew, shared table full, marker key) take the direct global path
 // inside the same kernels; rows that cannot even be inserted there (global table at its limit) are appended to
 // a retry list in the partial-aggregate wire format and replayed by combine_partials_kernel after the table grew.
@@ -1001,8 +1001,8 @@ constexpr int SPG_PCTAS = 4;        // K1 CTAs per SM (more independent CTAs = b
 constexpr int SPG_TILE = 2048;
 constexpr int SPG_MAX_OWNERS = 256;
 // K1 reserves one run per owner per tile with a global atomic on the owner's row counter: ~10^7 atomics per launch.  With
-// the 148 counters packed into ten cache lines K1's speed depended on where the array happened to land (0.80 ms against
-// 1.00 ms per 2^27 rows for the same SASS after an unrelated allocation moved it), so every counter gets its own line.
+// the per-owner counters packed into a few cache lines K1's speed depended on where the array happened to land (same SASS,
+// slower after an unrelated allocation moved it), so every counter gets its own line.
 #ifdef SPG_CNT_STRIDE_OVERRIDE  // scratch/spg_harness experiments only
 constexpr int SPG_CNT_STRIDE = SPG_CNT_STRIDE_OVERRIDE;
 #else
@@ -1420,8 +1420,8 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPG_TCTAS) spg_partition_tma_ker
 //
 // Shared table = two-choice bucketed hash table + stash: every key has two candidate buckets of two slots (one 16-byte
 // shared load each), so the hot lookup is two unconditional loads + four compares, no probe loop and no divergence
-// (a linear-probing table spent > 50 % of its issue slots on loop control with ~15 of 32 lanes active,
-// profiles/r01_spg_ncu_summary.txt; a collision-free key set runs the same loop 1.65x faster, scratch/ubench3.cu).
+// (a linear-probing table spends much of its issue slots on loop control with about half the lanes active; compare a
+// collision-free key set with scratch/ubench3.cu).
 // Everything else — first appearance of a key (CAS into a free candidate slot), keys whose four candidates are taken
 // (~2 % at this load: linear-probing stash behind the buckets), a full stash (direct global path), a non-zero high word
 // of the sum — is parked and handled once per iteration behind the hot path.  Two racing inserts may put one key into
@@ -2235,7 +2235,9 @@ class GroupbyState {
             if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)LC_SLOTS_BIG * 20 + 64)) != cudaSuccess) { cudaGetLastError(); return false; }
         { const char* e3 = getenv("B200_LC"); lc_enabled = !(e3 && e3[0] == '0'); }
         spg_owners = sms;  // one owner (bucket + shared table) per SM
-        d_bucket_cnt.alloc((size_t)std::max(2 * spg_owners, GEN_CLS) * SPG_CNT_STRIDE * 8);  // SPG-G: one counter per class of K1g
+        // SPG-G: one counter per class of K1g.  consume_spg_gen clears n_vo + owners counters, and n_vo (owners x passes) may
+        // fill all GEN_CLS classes when the value column has no bitmap (e.g. 3 passes x 132 owners on an H100)
+        d_bucket_cnt.alloc((size_t)(GEN_CLS + spg_owners) * SPG_CNT_STRIDE * 8);
         spg_state = 1;
         return true;
     }

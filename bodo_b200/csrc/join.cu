@@ -1,4 +1,4 @@
-// join.cu — streaming hash join on one B200 (sm_100a).
+// join.cu — streaming hash join on one GPU (H100, sm_90a).
 //
 // Replaces HashJoinState / JoinPartition of the reference (bodo/libs/streaming/_join.cpp):
 //   build  : join_build_consume_batch (:3134-3443) appends batches to device-resident build columns; on the
@@ -502,6 +502,13 @@ __global__ void join_slots16_from32_kernel(const Slot32* in, uint64_t n_slots, S
         out[s] = e;
     }
 }
+// One Slot32 (one 32-byte sector) through the read-only path.  sm_90 has no 256-bit load: two 128-bit loads of the same
+// aligned sector, issued back to back, still cost one sector of L2 / HBM traffic.
+__device__ __forceinline__ void ld_slot32(const Slot32* p, unsigned long long& w0, unsigned long long& w1, unsigned long long& w2,
+                                          unsigned long long& w3) {
+    asm volatile("ld.global.nc.v2.u64 {%0, %1}, [%4];\n\tld.global.nc.v2.u64 {%2, %3}, [%4+16];"
+                 : "=l"(w0), "=l"(w1), "=l"(w2), "=l"(w3) : "l"(p));
+}
 template <int NF, int NPK>
 __global__ void __launch_bounds__(256) join_probe_inline_kernel(const __grid_constant__ InlineProbeArgs a) {
     constexpr int R = 4, NW = 8, TILE = 256 * R;
@@ -524,14 +531,14 @@ __global__ void __launch_bounds__(256) join_probe_inline_kernel(const __grid_con
 #pragma unroll
             for (int c = 0; c < NPK; c++) pv[c][r] = in ? __ldcs(a.p[c] + i) : 0ull;
         }
-        // first probe of all R rows: the R random 256-bit slot loads (one sector, one request each) are in flight together;
+        // first probe of all R rows: the R random 32-byte slot loads (one sector each) are in flight together;
         // a data-dependent probe loop per row would serialise them
         uint64_t sl[R];
         unsigned long long w0[R], w1[R], w2[R], w3[R];
 #pragma unroll
         for (int r = 0; r < R; r++) {
             sl[r] = key[r] == J_EMPTY ? a.cap + 1 : j_hash_slot(key[r], mask);
-            asm volatile("ld.global.nc.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(w0[r]), "=l"(w1[r]), "=l"(w2[r]), "=l"(w3[r]) : "l"(a.slots + sl[r]));
+            ld_slot32(a.slots + sl[r], w0[r], w1[r], w2[r], w3[r]);
         }
 #pragma unroll
         for (int r = 0; r < R; r++) {
@@ -547,7 +554,7 @@ __global__ void __launch_bounds__(256) join_probe_inline_kernel(const __grid_con
                 }
                 if ((long long)w0[r] == J_EMPTY || sl[r] > mask) break;  // free slot, or the marker-key slot (cap + 1) without a build row
                 sl[r] = (sl[r] + 1) & mask;  // collision (about one row in four at this load factor): next slot
-                asm volatile("ld.global.nc.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(w0[r]), "=l"(w1[r]), "=l"(w2[r]), "=l"(w3[r]) : "l"(a.slots + sl[r]));
+                ld_slot32(a.slots + sl[r], w0[r], w1[r], w2[r], w3[r]);
             }
         }
 #pragma unroll

@@ -1,4 +1,4 @@
-// shuffle.cu — row -> rank radix partition of a columnar table (sm_100a).
+// shuffle.cu — row -> rank radix partition of a columnar table (sm_90a).
 //
 // Replaces hash_keys_table(SEED_HASH_PARTITION) + mpi_comm_info::set_send_count + fill_send_array of the
 // reference's shuffle_table (bodo/libs/_shuffle.cpp:94-163, 345-368, 477+, 1593-1642) and the

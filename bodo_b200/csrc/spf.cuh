@@ -18,13 +18,14 @@
 //       consumer (19 warps) polls the heads of the rings it reads, takes lines as they arrive (four lines = 32 rows per warp
 //                          instruction, from whichever rings have them) and aggregates them into a shared-memory cuckoo hash
 //                          table that lives for the whole launch (flushed into the state's global table ONCE, at the end).
-//     A first version with a counting sort per 2048-row tile (three producer barriers per tile, 8 producer warps) ran at
-//     0.12 of the roofline: every phase waited for the slowest warp and the consumers starved (profiles/r02_spf_notes.txt).
-//   * every (producer SM p, owner SM o) pair has a private ring of SPF_RL lines (148 x 148 x 2 KB = 45 MB, L2 resident).  A
+//     A first version with a counting sort per 2048-row tile (three producer barriers per tile, 8 producer warps) was far
+//     slower: every phase waited for the slowest warp and the consumers starved.
+//   * every (producer SM p, owner SM o) pair has a private ring of SPF_RL lines (SMs x SMs x 2 KB:
+//     132 x 132 x 2 KB = 35 MB on an H100, inside its 50 MB L2).  A
 //     private ring needs no reservation atomics: p's flusher owns the head, o's consumer owns the tail; cursors are
 //     monotonically increasing line counts in pub[p][o] / cons[o][p];
-//   * measured ceiling of this data flow (scratch/ubench4.cu, profiles/r02_ubench4.txt): HBM stream + L2-resident ring
-//     write + ring read sustain 235 Grows/s of 16-byte rows (57 % of the roofline) against 129 when the ring lives in HBM.
+//   * scratch/ubench4.cu measures the ceiling of this data flow: HBM stream + L2-resident ring write + ring read, against
+//     the same ring in HBM.
 //
 // Shared-memory table: two-choice cuckoo, two-slot buckets (two 16-byte loads + four compares per lookup), two native
 // 32-bit atomics per row (low word of the sum with carry detection; count).  First appearances claim a free candidate slot

@@ -4,7 +4,7 @@ Same four verbs, same argument meaning and the same calling protocol as the refe
 (init_groupby_state :702-715, groupby_build_consume_batch :1295-1395, groupby_produce_output_batch
 :1502-1600, delete_groupby_state), so the reference's streaming test loops
 (bodo/tests/test_streaming/test_groupby.py:51-81) run unchanged against this module.  The work happens in
-libbodo_b200.so (CUDA, sm_100a); there is no CPU implementation behind these calls.
+libbodo_b200.so (CUDA, sm_90a); there is no CPU implementation behind these calls.
 
 Differences: the reference types the state at Numba compile time; here the build-table schema is taken
 from the first consumed batch.  With parallel=True the state is one shard of a torch.distributed process

@@ -1,5 +1,5 @@
 /*
- * bodo_b200.h — C ABI of libbodo_b200.so: the B200-native replacement for Bodo's streaming
+ * bodo_b200.h — C ABI of libbodo_b200.so: the CUDA-native (H100) replacement for Bodo's streaming
  * hash groupby / hash join / row->rank shuffle hot path.
  *
  * Every entry point mirrors one reference FFI symbol (cited per function, paths relative to the

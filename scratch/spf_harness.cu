@@ -2,7 +2,7 @@
 // the operator state machine: CUDA-event time per launch, achieved fraction of the 16 B/row roofline, and an EXACT per-group
 // check against a dense reference built with plain global atomics.  Development tool, not part of the library.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -I bodo_b200/csrc \
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -I bodo_b200/csrc \
 //        scratch/spf_harness.cu bodo_b200/csrc/misc.cu -o scratch/spf_harness
 //   scratch/spf_harness [log2_rows=27] [groups=1000000] [reps=3] [extra_rows=0] [zipf=0]
 #include <algorithm>
@@ -128,7 +128,7 @@ int main(int argc, char** argv) {
     const float med = t[t.size() / 2];
     printf("{\"rows\": %lld, \"groups\": %llu, \"skew_pct\": %d, \"ms\": {\"min\": %.4f, \"median\": %.4f}, \"grows_per_s\": %.2f, \"roofline_frac\": %.4f, "
            "\"groups_ok\": %llu, \"groups_bad\": %llu, \"groups_expected\": %llu, \"table_groups\": %lld, \"retry_rows\": %lld, \"tiles_claimed\": %llu, \"abort\": %llu, \"check\": \"%s\"}\n",
-           (long long)rows, (unsigned long long)groups, skew, t[0], med, rows / (med * 1e-3) / 1e9, rows * 16.0 / (med * 1e-3) / 6574.8e9,
+           (long long)rows, (unsigned long long)groups, skew, t[0], med, rows / (med * 1e-3) / 1e9, rows * 16.0 / (med * 1e-3) / 3350e9 /* H100 SXM data-sheet HBM bandwidth */,
            h[0], h[1], h[2], hc[0], hc[1], tc[0], tc[1], ok ? "ok" : "MISMATCH");
 #ifdef SPF_STATS
     unsigned long long st[64]; CK(cudaMemcpy(st, stats, 512, cudaMemcpyDeviceToHost));

@@ -1,5 +1,5 @@
 // Calibration microbenchmarks for the hash-aggregate design (scratch; not product code).
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o scratch/ubench scratch/ubench.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o scratch/ubench scratch/ubench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
@@ -252,7 +252,7 @@ int main(int argc, char** argv) {
     cudaDeviceProp prop; CK(cudaGetDeviceProperties(&prop, 0));
     printf("dev %s SMs %d L2 %d MB smem/blk optin %zu clock %d\n", prop.name, prop.multiProcessorCount, prop.l2CacheSize >> 20, prop.sharedMemPerBlockOptin, prop.clockRate);
     int64_t *keys, *vals; CK(cudaMalloc(&keys, n * 8)); CK(cudaMalloc(&vals, n * 8));
-    gen<<<148 * 8, 256>>>(keys, vals, n, ng); CK(cudaDeviceSynchronize());
+    gen<<<132 * 8, 256>>>(keys, vals, n, ng); CK(cudaDeviceSynchronize());
     uint32_t cap = 1; while (cap < 2 * ng) cap <<= 1; uint32_t mask = cap - 1;
     unsigned long long *sum, *cnt, *out; long long* tkeys; Slot32* tab;
     CK(cudaMalloc(&sum, cap * 8ull)); CK(cudaMalloc(&cnt, cap * 8ull)); CK(cudaMalloc(&tkeys, cap * 8ull)); CK(cudaMalloc(&tab, cap * 32ull)); CK(cudaMalloc(&out, 8));
@@ -260,7 +260,7 @@ int main(int argc, char** argv) {
     double gb = n * 16.0 / 1e9;
     auto rep = [&](const char* name, float ms) { printf("%-28s %8.3f ms  %8.1f GB/s  %7.2f Grows/s\n", name, ms, gb / (ms * 1e-3), n / (ms * 1e-3) / 1e9); fflush(stdout); };
     for (int bps : {4, 8}) {
-        int grid = 148 * bps, blk = 256;
+        int grid = 132 * bps, blk = 256;
         printf("-- grid %d x %d, n=%lld groups=%lld cap=%u\n", grid, blk, (long long)n, (long long)ng, cap);
         rep("A stream", timeit([&] { k_stream<<<grid, blk>>>(keys, vals, n, out); }));
         rep("B soa 1 red", timeit([&] { k_soa<1><<<grid, blk>>>(keys, vals, n, sum, cnt, mask); }));
@@ -277,7 +277,7 @@ int main(int argc, char** argv) {
         CK(cudaFuncSetAttribute(k_smem<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smb));
         CK(cudaFuncSetAttribute(k_smem32, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smb));
         for (int blk : {512, 1024}) {
-            int grid = 148;
+            int grid = 132;
             printf("-- smem table %d slots, grid %d x %d\n", smslots, grid, blk);
             rep("F smem 2x atom64", timeit([&] { k_smem<0><<<grid, blk, smb>>>(keys, vals, n, out, smslots); }));
             rep("F smem ld/st rmw", timeit([&] { k_smem<1><<<grid, blk, smb>>>(keys, vals, n, out, smslots); }));
@@ -286,7 +286,7 @@ int main(int argc, char** argv) {
         }
     }
     {
-        constexpr int TILE = 4096, NB = 148;
+        constexpr int TILE = 4096, NB = 132;
         int64_t capb = (int64_t)(n / NB * 1.05) + 4096;
         // limit n for partition test so inbox fits: use first 64M rows
         int64_t np = n < (1ll << 26) ? n : (1ll << 26);
@@ -296,13 +296,13 @@ int main(int argc, char** argv) {
         size_t smb = TILE * 16;
         CK(cudaFuncSetAttribute(k_partition<TILE, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smb));
         for (int bps : {1, 2}) {
-            float ms = timeit([&] { cudaMemsetAsync(cursors, 0, NB * 4); k_partition<TILE, NB><<<148 * bps, 512, smb>>>(keys, vals, np, inbox, cursors, capb); });
+            float ms = timeit([&] { cudaMemsetAsync(cursors, 0, NB * 4); k_partition<TILE, NB><<<132 * bps, 512, smb>>>(keys, vals, np, inbox, cursors, capb); });
             printf("H partition %d/SM  %8.3f ms  %7.2f Grows/s (n=%lld, HBM-sized inbox)\n", bps, ms, np / (ms * 1e-3) / 1e9, (long long)np);
         }
         // L2-sized: 2M rows repeatedly into the same 32MB inbox
         int64_t nl = 1ll << 21; capb = (int64_t)(nl / NB * 1.2) + 1024;
         for (int bps : {1, 2}) {
-            float ms = timeit([&] { for (int r = 0; r < 16; r++) { cudaMemsetAsync(cursors, 0, NB * 4); k_partition<TILE, NB><<<148 * bps, 512, smb>>>(keys + r * nl, vals + r * nl, nl, inbox, cursors, capb); } });
+            float ms = timeit([&] { for (int r = 0; r < 16; r++) { cudaMemsetAsync(cursors, 0, NB * 4); k_partition<TILE, NB><<<132 * bps, 512, smb>>>(keys + r * nl, vals + r * nl, nl, inbox, cursors, capb); } });
             printf("H partition L2 %d/SM  %8.3f ms  %7.2f Grows/s (16 x 2M rows, incl launch gaps)\n", bps, ms, 16 * nl / (ms * 1e-3) / 1e9);
         }
     }

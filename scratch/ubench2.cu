@@ -14,15 +14,18 @@ __global__ void gen(long long* keys, long long* vals, int64_t n, uint64_t ng) {
     for (; i < n; i += st) { keys[i] = (long long)(mix64(i ^ 0x9e3779b97f4a7c15ULL) % ng); vals[i] = (long long)(mix64(i ^ 0x1234567ull) % 1000) - 500; }
 }
 template <int MODE> __device__ __forceinline__ void loadb(const long long* t, uint64_t b, long long (&k)[4]) {
-    if (MODE == 0) asm volatile("ld.global.cg.v4.s64 {%0,%1,%2,%3}, [%4];" : "=l"(k[0]), "=l"(k[1]), "=l"(k[2]), "=l"(k[3]) : "l"(t + 4 * b));
-    else if (MODE == 1) {
+    // (sm_90 has no 256-bit load: a 32-byte bucket is two 128-bit loads)
+    if (MODE == 1) {
         asm volatile("ld.global.cg.v2.s64 {%0,%1}, [%2];" : "=l"(k[0]), "=l"(k[1]) : "l"(t + 4 * b));
         asm volatile("ld.global.cg.v2.s64 {%0,%1}, [%2];" : "=l"(k[2]), "=l"(k[3]) : "l"(t + 4 * b + 2));
     } else if (MODE == 2) {
         asm volatile("ld.global.ca.v2.s64 {%0,%1}, [%2];" : "=l"(k[0]), "=l"(k[1]) : "l"(t + 4 * b));
         asm volatile("ld.global.ca.v2.s64 {%0,%1}, [%2];" : "=l"(k[2]), "=l"(k[3]) : "l"(t + 4 * b + 2));
     } else {
-        asm volatile("ld.global.L2::evict_last.v4.s64 {%0,%1,%2,%3}, [%4];" : "=l"(k[0]), "=l"(k[1]), "=l"(k[2]), "=l"(k[3]) : "l"(t + 4 * b));
+        uint64_t pol;
+        asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+        asm volatile("ld.global.L2::cache_hint.v2.s64 {%0,%1}, [%2], %3;" : "=l"(k[0]), "=l"(k[1]) : "l"(t + 4 * b), "l"(pol));
+        asm volatile("ld.global.L2::cache_hint.v2.s64 {%0,%1}, [%2], %3;" : "=l"(k[2]), "=l"(k[3]) : "l"(t + 4 * b + 2), "l"(pol));
     }
 }
 template <int MODE> __device__ __forceinline__ uint64_t foi(long long* t, uint64_t cap, long long key) {
@@ -142,13 +145,13 @@ int main(int argc, char** argv) {
     int capmul = argc > 3 ? atoi(argv[3]) : 2;
     long long *keys, *vals, *t; unsigned long long *sum, *cnt;
     CK(cudaMalloc(&keys, n * 8)); CK(cudaMalloc(&vals, n * 8));
-    gen<<<148 * 8, 256>>>(keys, vals, n, ng);
+    gen<<<132 * 8, 256>>>(keys, vals, n, ng);
     uint64_t cap = 1; while (cap < capmul * ng) cap <<= 1;
     CK(cudaMalloc(&t, cap * 8)); CK(cudaMalloc(&sum, cap * 8)); CK(cudaMalloc(&cnt, cap * 8));
     CK(cudaDeviceSynchronize());
     auto reset = [&] { fill<<<1184, 256>>>(t, cap, EMPTY); cudaMemset(sum, 0, cap * 8); cudaMemset(cnt, 0, cap * 8); };
     auto rep = [&](const char* name, float ms) { printf("%-34s %8.3f ms %7.2f Grows/s\n", name, ms, n / (ms * 1e-3) / 1e9); fflush(stdout); };
-    int g = 148 * 8;
+    int g = 132 * 8;
     printf("n=%lld groups=%llu cap=%llu\n", (long long)n, (unsigned long long)ng, (unsigned long long)cap);
     reset(); rep("nocheck xxh3 (2 red only)", timeit([&] { agg_nocheck<0><<<g, 256>>>(keys, vals, n, cap, sum, cnt); }));
     reset(); rep("nocheck fib (2 red only)", timeit([&] { agg_nocheck<1><<<g, 256>>>(keys, vals, n, cap, sum, cnt); }));
@@ -158,12 +161,11 @@ int main(int argc, char** argv) {
     reset(); rep("linear fib  ilp2", timeit([&] { agg_lin2<1, 1><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
     reset(); rep("linear 64b, ldcs stream", timeit([&] { agg_lin<0><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
     reset(); rep("linear 64b, plain stream", timeit([&] { agg_lin<1><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
-    reset(); rep("bucket 256b cg, ldcs", timeit([&] { agg<0, 0><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
     reset(); rep("bucket 2x128b cg, ldcs", timeit([&] { agg<1, 0><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
     reset(); rep("bucket 2x128b cg, plain", timeit([&] { agg<1, 1><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
     reset(); rep("bucket 2x128b ca, ldcs", timeit([&] { agg<2, 0><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
-    reset(); rep("bucket 256b evict_last, ldcs", timeit([&] { agg<3, 0><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
-    reset(); rep("bucket 256b evict_last, nc ef", timeit([&] { agg<3, 2><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
-    reset(); rep("bucket 256b cg, nc evict_first", timeit([&] { agg<0, 2><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
+    reset(); rep("bucket 2x128b evict_last, ldcs", timeit([&] { agg<3, 0><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
+    reset(); rep("bucket 2x128b evict_last, nc ef", timeit([&] { agg<3, 2><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
+    reset(); rep("bucket 2x128b cg, nc evict_first", timeit([&] { agg<1, 2><<<g, 256>>>(keys, vals, n, t, cap, sum, cnt); }));
     return 0;
 }

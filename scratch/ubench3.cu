@@ -67,11 +67,11 @@ int main() {
     int64_t n = 1ll << 26; uint64_t ng = 6757;  // per CTA the same ~6.7k distinct keys (like one SPG owner)
     longlong2* rows; unsigned long long* out;
     CK(cudaMalloc(&rows, n * 16)); CK(cudaMalloc(&out, 8));
-    gen<<<148 * 8, 256>>>(rows, n, ng); CK(cudaDeviceSynchronize());
-    int64_t per = n / 148;
+    gen<<<132 * 8, 256>>>(rows, n, ng); CK(cudaDeviceSynchronize());
+    int64_t per = n / 132;
     int ns = 14000; size_t smb = (size_t)ns * 16 + 64;
     auto rep = [&](const char* name, float ms) { printf("%-44s %8.3f ms %7.2f Grows/s\n", name, ms, n / (ms * 1e-3) / 1e9); fflush(stdout); };
-#define RUN(MODE, T, name) { CK(cudaFuncSetAttribute(agg<MODE, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smb)); rep(name, timeit([&] { agg<MODE, T><<<148, T, smb>>>(rows, per, ns, out); })); }
+#define RUN(MODE, T, name) { CK(cudaFuncSetAttribute(agg<MODE, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smb)); rep(name, timeit([&] { agg<MODE, T><<<132, T, smb>>>(rows, per, ns, out); })); }
     RUN(0, 1024, "2 atomics, no probe, no return");
     RUN(2, 1024, "2 atomics, returning + carry");
     RUN(1, 1024, "probe (no insert) + 2 atomics");

@@ -1,4 +1,4 @@
-"""Full-size parity checks (BASELINE.json configs[1]: 2 B rows, 1 M groups, SUM+COUNT on one B200).
+"""Full-size parity checks (BASELINE.json configs[1]: 2 B rows, 1 M groups, SUM+COUNT on one H100).
 
 The CPU oracle cannot finish 2 B rows inside a test, so the result is pinned two ways that do not depend on size:
   * an independent device-side recomputation with torch (bincount / index_add_ per 2^28-row chunk) — every group's COUNT and
