@@ -48,6 +48,19 @@ struct OpDesc {
     void* a1;  // second accumulator (mean count, min/max seen-count) or nullptr
 };
 
+// The words of a state's device counter block (GroupbyState::d_counters), mirrored to the host by read_counters().
+enum CounterSlot : int {
+    CTR_GROUPS = 0,         // groups in the table (the tickets find_or_insert takes against the group limit)
+    CTR_FAIL = 1,           // rows in the fail list (direct / multi-key / combine), or in the slot-0 retry list (SPG, SPG-G)
+    CTR_OUT = 2,            // output cursor of the compaction
+    CTR_NA = 3,             // the NA key is present (slot cap)
+    CTR_MARKER = 4,         // the marker key EMPTY_KEY is present (slot cap + 1)
+    CTR_WIDE = 5,           // SPG-N: rows that did not fit the narrow (int32 key, int32 value) format
+    CTR_RETRY1 = 6,         // rows in the slot-1 retry list (SPG)
+    CTR_XCHG_OVERFLOW = 7,  // fused exchange: some rank's share overflowed its slab segment, nobody combined
+    N_COUNTERS = 8
+};
+
 struct ConsumeArgs {
     const void* key_data;
     const uint8_t* key_valid;
@@ -57,7 +70,7 @@ struct ConsumeArgs {
     const uint32_t* index_list;  // nullptr: rows [0, n_rows); else replay of the listed rows
     long long* tkeys;
     uint64_t cap;  // power of two; slot cap = NA key, slot cap + 1 = the key equal to EMPTY_KEY
-    long long* counters;  // [0] groups in table, [1] failed rows, [2] cursor, [3] NA present, [4] EMPTY_KEY present
+    long long* counters;  // the state's counter block (CounterSlot)
     long long group_limit;
     uint32_t* fail_list;
     unsigned long long seq_base;  // first / last: sequence number of row 0 of this launch, minus 1 (rank << 44 | rows consumed so far)
@@ -83,17 +96,17 @@ __device__ __forceinline__ uint64_t find_or_insert(long long* __restrict__ tkeys
             if (group_limit >= 0) {
                 const cooperative_groups::coalesced_group cgp = cooperative_groups::coalesced_threads();
                 long long t = 0;
-                if (cgp.thread_rank() == 0) t = (long long)atomicAdd((unsigned long long*)&counters[0], (unsigned long long)cgp.size());
+                if (cgp.thread_rank() == 0) t = (long long)atomicAdd((unsigned long long*)&counters[CTR_GROUPS], (unsigned long long)cgp.size());
                 t = cgp.shfl(t, 0) + (long long)cgp.thread_rank();
                 if (t >= group_limit) {
-                    atomicAdd((unsigned long long*)&counters[0], (unsigned long long)-1ll);
+                    atomicAdd((unsigned long long*)&counters[CTR_GROUPS], (unsigned long long)-1ll);
                     return ~0ull;
                 }
             }
             long long prev = atomicCAS((unsigned long long*)(tkeys + s), (unsigned long long)EMPTY_KEY,
                                        (unsigned long long)key);
             if (prev == EMPTY_KEY) return s;
-            if (group_limit >= 0) atomicAdd((unsigned long long*)&counters[0], (unsigned long long)-1ll);  // lost the race
+            if (group_limit >= 0) atomicAdd((unsigned long long*)&counters[CTR_GROUPS], (unsigned long long)-1ll);  // lost the race
             if (prev == key) return s;
         }
         s = (s + 1) & mask;
@@ -209,16 +222,16 @@ __global__ void __launch_bounds__(256) groupby_consume_kernel(const __grid_const
         if (!kvalid) {
             if (a.dropna) continue;  // filter_na_keys (_groupby.cpp:4278-4309)
             slot = a.cap;
-            a.counters[3] = 1;
+            a.counters[CTR_NA] = 1;
         } else {
             long long key = load_int_as_i64(a.key_data, a.key_ctype, row);
             if (key == EMPTY_KEY) {
                 slot = a.cap + 1;
-                a.counters[4] = 1;
+                a.counters[CTR_MARKER] = 1;
             } else {
                 slot = find_or_insert(a.tkeys, a.cap, key, a.counters, a.group_limit);
                 if (slot == ~0ull) {
-                    unsigned long long f = atomicAdd((unsigned long long*)&a.counters[1], 1ull);
+                    unsigned long long f = atomicAdd((unsigned long long*)&a.counters[CTR_FAIL], 1ull);
                     a.fail_list[f] = (uint32_t)row;
                     continue;
                 }
@@ -279,11 +292,11 @@ __global__ void __launch_bounds__(256) groupby_consume_i64_sumcount_kernel(
             uint64_t sl;
             if (k[r] == EMPTY_KEY) {
                 sl = cap + 1;
-                counters[4] = 1;
+                counters[CTR_MARKER] = 1;
             } else {
                 sl = find_or_insert(tkeys, cap, k[r], counters, group_limit);
                 if (sl == ~0ull) {
-                    unsigned long long f = atomicAdd((unsigned long long*)&counters[1], 1ull);
+                    unsigned long long f = atomicAdd((unsigned long long*)&counters[CTR_FAIL], 1ull);
                     fail_list[f] = (uint32_t)(i + r);
                     continue;
                 }
@@ -330,7 +343,7 @@ __global__ void rehash_kernel(const __grid_constant__ RehashArgs a) {
 // carry keys this rank owns)
 __global__ void compact_slots_kernel(const long long* __restrict__ tkeys, uint64_t cap, const long long* counters,
                                      long long* cursor, uint64_t* slot_of_out, int n_pes, int rank) {
-    const bool na_present = counters[3] != 0, empty_present = counters[4] != 0;
+    const bool na_present = counters[CTR_NA] != 0, empty_present = counters[CTR_MARKER] != 0;
     const uint32_t na_hash = (uint32_t)xxh3_64_short(1ull, 8, SEED_HASH_PARTITION);  // hash_na_val (_array_hash.cpp:22-29)
     uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
     for (uint64_t s0 = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s0 < ((cap + 2 + 31) & ~31ull); s0 += stride) {
@@ -577,12 +590,12 @@ __device__ __forceinline__ void combine_one_row(const CombineArgs& a, int64_t ro
     long long key = (long long)r[0];
     bool kvalid = r[1] & 1;
     uint64_t slot;
-    if (!kvalid) { slot = a.cap; a.counters[3] = 1; }
-    else if (key == EMPTY_KEY) { slot = a.cap + 1; a.counters[4] = 1; }
+    if (!kvalid) { slot = a.cap; a.counters[CTR_NA] = 1; }
+    else if (key == EMPTY_KEY) { slot = a.cap + 1; a.counters[CTR_MARKER] = 1; }
     else {
         slot = find_or_insert(a.tkeys, a.cap, key, a.counters, a.group_limit);
         if (slot == ~0ull) {
-            unsigned long long f = atomicAdd((unsigned long long*)&a.counters[1], 1ull);
+            unsigned long long f = atomicAdd((unsigned long long*)&a.counters[CTR_FAIL], 1ull);
             a.fail_list[f] = (uint32_t)row;
             return;
         }
@@ -646,7 +659,7 @@ struct XchgPackArgs {
     long long cap_rows;
 };
 __global__ void xchg_pack_remote_kernel(const __grid_constant__ XchgPackArgs a) {
-    const bool na_present = a.counters[3] != 0, empty_present = a.counters[4] != 0;
+    const bool na_present = a.counters[CTR_NA] != 0, empty_present = a.counters[CTR_MARKER] != 0;
     const uint32_t na_hash = (uint32_t)xxh3_64_short(1ull, 8, SEED_HASH_PARTITION);
     const int lane = threadIdx.x & 31;
     uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
@@ -688,7 +701,7 @@ __global__ void xchg_combine_slab_kernel(const __grid_constant__ CombineArgs a, 
     // a.in = first row of segment 0; flat row index = source * cap_rows + r (also what the fail list records)
     bool over = false;
     for (int s = 0; s < n_pes; s++) over |= (hdr[s] & XCHG_OVERFLOW) != 0;
-    if (over) { if (blockIdx.x == 0 && threadIdx.x == 0) a.counters[7] = 1; return; }  // every rank sees the same flags: nobody combines
+    if (over) { if (blockIdx.x == 0 && threadIdx.x == 0) a.counters[CTR_XCHG_OVERFLOW] = 1; return; }  // every rank sees the same flags: nobody combines
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int s = 0; s < n_pes; s++) {
         const int64_t n = (int64_t)(hdr[s] & ~XCHG_OVERFLOW);
@@ -747,8 +760,8 @@ __device__ __forceinline__ uint64_t find_or_insert_mk(const A& a, const long lon
             if (eq) return s;
         } else if (t == TAG_EMPTY) {
             if (a.group_limit >= 0) {
-                long long tk = atomicAdd((unsigned long long*)&a.counters[0], 1ull);
-                if (tk >= a.group_limit) { atomicAdd((unsigned long long*)&a.counters[0], (unsigned long long)-1ll); return ~0ull; }
+                long long tk = atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], 1ull);
+                if (tk >= a.group_limit) { atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], (unsigned long long)-1ll); return ~0ull; }
             }
             unsigned long long old = atomicCAS(a.tags + s, TAG_EMPTY, TAG_LOCKED);
             if (old == TAG_EMPTY) {
@@ -758,7 +771,7 @@ __device__ __forceinline__ uint64_t find_or_insert_mk(const A& a, const long lon
                 atomicExch(a.tags + s, tag);  // publish
                 return s;
             }
-            if (a.group_limit >= 0) atomicAdd((unsigned long long*)&a.counters[0], (unsigned long long)-1ll);
+            if (a.group_limit >= 0) atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], (unsigned long long)-1ll);
             continue;  // somebody else took the slot: look at it again
         } else if (t == TAG_LOCKED) {
             continue;  // being written: re-read
@@ -783,7 +796,7 @@ __global__ void __launch_bounds__(256) groupby_consume_mk_kernel(const __grid_co
         if (a.dropna && mask != (1u << a.nk) - 1u) continue;  // any NA key column drops the row (pandas dropna=True)
         uint64_t slot = find_or_insert_mk(a, keys, mask, mk_tag(keys, mask, a.nk));
         if (slot == ~0ull) {
-            unsigned long long f = atomicAdd((unsigned long long*)&a.counters[1], 1ull);
+            unsigned long long f = atomicAdd((unsigned long long*)&a.counters[CTR_FAIL], 1ull);
             a.fail_list[f] = (uint32_t)row;
             continue;
         }
@@ -849,10 +862,10 @@ __global__ void nunique_count_kernel(const __grid_constant__ NuniqueArgs a) {
         const unsigned int m = a.pmask[s];
         if (!(m & 2u)) continue;  // NA value
         uint64_t slot;
-        if (!(m & 1u)) { if (a.dropna) continue; slot = a.cap; a.counters[3] = 1; }
+        if (!(m & 1u)) { if (a.dropna) continue; slot = a.cap; a.counters[CTR_NA] = 1; }
         else {
             const long long key = a.pk[s];
-            if (key == EMPTY_KEY) { slot = a.cap + 1; a.counters[4] = 1; }
+            if (key == EMPTY_KEY) { slot = a.cap + 1; a.counters[CTR_MARKER] = 1; }
             else { slot = find_only(a.tkeys, a.cap, key); if (slot == ~0ull) continue; }  // (every key of a pair is a group of the outer table)
         }
         for (int j = 0; j < a.n_acc; j++) atomicAdd(a.acc[j] + slot, 1ull);
@@ -929,7 +942,7 @@ __global__ void xchg_combine_mk_kernel(const __grid_constant__ MkArgs m, const _
         const unsigned int mask = (unsigned int)r[m.nk];
         const uint64_t slot = find_or_insert_mk(m, keys, mask, mk_tag(keys, mask, m.nk));
         if (slot == ~0ull) {
-            unsigned long long f = atomicAdd((unsigned long long*)&c.counters[1], 1ull);
+            unsigned long long f = atomicAdd((unsigned long long*)&c.counters[CTR_FAIL], 1ull);
             c.fail_list[f] = (uint32_t)row;
             return;
         }
@@ -942,7 +955,7 @@ __global__ void xchg_combine_mk_kernel(const __grid_constant__ MkArgs m, const _
     }
     bool over = false;
     for (int s = 0; s < n_pes; s++) over |= (hdr[s] & XCHG_OVERFLOW) != 0;
-    if (over) { if (blockIdx.x == 0 && threadIdx.x == 0) c.counters[7] = 1; return; }
+    if (over) { if (blockIdx.x == 0 && threadIdx.x == 0) c.counters[CTR_XCHG_OVERFLOW] = 1; return; }
     for (int s = 0; s < n_pes; s++) {
         const int64_t n = (int64_t)(hdr[s] & ~XCHG_OVERFLOW);
         for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) one((int64_t)s * cap_rows + i);
@@ -1014,7 +1027,7 @@ struct SpgArgs {
     uint64_t cap;
     unsigned long long* acc_sum;
     unsigned long long* acc_cnt;
-    long long* counters;  // [0] groups, [1] retry rows, [4] marker key present
+    long long* counters;  // the state's counter block (CounterSlot); the retry list is counted in retry_ctr
     long long group_limit;
     // owner buckets
     longlong2* bucket;            // [n_owners][bucket_cap]
@@ -1052,7 +1065,7 @@ __device__ __forceinline__ void spg_retry_row(const SpgArgs& a, long long key, u
 template <bool HAS_SUM, bool HAS_CNT>
 __device__ __forceinline__ void spg_direct_apply(const SpgArgs& a, long long key, unsigned long long sum, unsigned long long cnt) {
     uint64_t sl;
-    if (key == EMPTY_KEY) { sl = a.cap + 1; a.counters[4] = 1; }
+    if (key == EMPTY_KEY) { sl = a.cap + 1; a.counters[CTR_MARKER] = 1; }
     else {
         sl = find_or_insert(a.tkeys, a.cap, key, a.counters, a.group_limit);
         if (sl == ~0ull) { spg_retry_row<HAS_SUM, HAS_CNT>(a, key, sum, cnt); return; }
@@ -1575,6 +1588,45 @@ struct FuncSpec {
     unsigned long long init1 = 0;  // initial value of the second accumulator
 };
 
+// ---- kernel-variant dispatch ----
+// for_each_X(f) calls f once per instantiation of kernel family X that a launch can pick, with its template arguments as
+// std::integral_constant values: spg_probe() sets the shared-memory limits through it.  with_X(..., f) calls f for the one
+// instantiation the runtime arguments select, found by the same enumeration, so a launch never picks a kernel whose limit
+// was not set.
+template <bool V> using bool_c = std::bool_constant<V>;
+template <int V> using int_c = std::integral_constant<int, V>;
+// sum / count kernels <HAS_SUM, HAS_CNT> (LC, K1, K1-hot, K2, K1n, K2n, the direct int64 kernel): <false, false> does not exist
+constexpr auto for_each_sum_cnt = [](auto&& f) {
+    f(bool_c<true>{}, bool_c<true>{}); f(bool_c<true>{}, bool_c<false>{}); f(bool_c<false>{}, bool_c<true>{});
+};
+// K1g spgg_partition_kernel<KEY_BYTES, VALUE_BYTES> (0 value bytes: size only)
+constexpr auto for_each_spgg_part = [](auto&& f) {
+    f(int_c<8>{}, int_c<8>{}); f(int_c<8>{}, int_c<4>{}); f(int_c<8>{}, int_c<0>{});
+    f(int_c<4>{}, int_c<8>{}); f(int_c<4>{}, int_c<4>{}); f(int_c<4>{}, int_c<0>{});
+};
+// K2g spgg_aggregate_kernel<HAS_SUM, HAS_MM, HAS_NN>: all eight
+constexpr auto for_each_spgg_agg = [](auto&& f) {
+    auto both_sums = [&](auto m, auto n) { f(bool_c<false>{}, m, n); f(bool_c<true>{}, m, n); };
+    both_sums(bool_c<false>{}, bool_c<false>{}); both_sums(bool_c<true>{}, bool_c<false>{});
+    both_sums(bool_c<false>{}, bool_c<true>{}); both_sums(bool_c<true>{}, bool_c<true>{});
+};
+template <typename Each, typename F, typename... W>
+void with_variant(Each&& each, F&& f, W... want) {
+    bool found = false;
+    each([&](auto... c) { if (((c == want) && ...)) { found = true; f(c...); } });
+    B200_REQUIRE(found, "internal: no kernel instantiation for this aggregate signature");
+}
+template <typename F> void with_sum_cnt(bool s, bool c, F&& f) { with_variant(for_each_sum_cnt, f, s, c); }
+template <typename F> void with_spgg_part(int ks, int vs, F&& f) { with_variant(for_each_spgg_part, f, ks, vs); }
+template <typename F> void with_spgg_agg(bool s, bool m, bool n, F&& f) { with_variant(for_each_spgg_agg, f, s, m, n); }
+
+// raises a kernel's dynamic shared-memory limit; false (error cleared) when the device refuses
+static bool set_smem_limit(const void* fn, size_t bytes) {
+    if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) == cudaSuccess) return true;
+    cudaGetLastError();
+    return false;
+}
+
 class GroupbyState {
    public:
     int device;
@@ -1625,6 +1677,7 @@ class GroupbyState {
     // host-side time accounting (printed at delete when B200_TRACE is set)
     double t_ctor = 0, t_grow = 0, t_alloc = 0, t_spg = 0, t_finalize = 0;
     static double now() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+    struct ScopedTimer { double& t; double t0 = now(); ~ScopedTimer() { t += now() - t0; } };  // adds its scope's time to t
     // metrics
     int64_t rows_consumed = 0, rebuilds = 0, launches = 0, fail_rows = 0;
     bool build_done = false;
@@ -1639,6 +1692,19 @@ class GroupbyState {
             if (cudaEventSynchronize(pr.second) == cudaSuccess && cudaEventElapsedTime(&ms, pr.first, pr.second) == cudaSuccess) us += ms * 1000.0;
         }
         return us;
+    }
+    using ProfEvents = std::pair<cudaEvent_t, cudaEvent_t>;
+    ProfEvents prof_begin(bool on) {  // (nullptr, nullptr) unless `on`
+        ProfEvents ev{nullptr, nullptr};
+        if (!on) return ev;
+        B200_CUDA(cudaEventCreate(&ev.first)); B200_CUDA(cudaEventCreate(&ev.second));
+        B200_CUDA(cudaEventRecord(ev.first, stream));
+        return ev;
+    }
+    void prof_end(ProfEvents ev) {
+        if (!ev.first) return;
+        B200_CUDA(cudaEventRecord(ev.second, stream));
+        prof_events.push_back(ev);
     }
 
     GroupbyState(const int8_t* ct, const int8_t* at, int n_arrs, const int32_t* ftypes, const int32_t* f_in_offsets,
@@ -1747,9 +1813,9 @@ class GroupbyState {
         B200_REQUIRE(n_funcs <= MAX_OPS, "b200 groupby: too many aggregate functions (composite ones count their accumulator columns)");
         d_a0.resize(n_funcs); d_a1.resize(n_funcs);
         d_out_data.resize(n_outs); d_out_valid.resize(n_outs);
-        d_counters.alloc(8 * sizeof(long long));
-        B200_CUDA(cudaMemsetAsync(d_counters.p, 0, 8 * sizeof(long long), stream));
-        h_counters = (long long*)pinned_acquire(8 * sizeof(long long));
+        d_counters.alloc(N_COUNTERS * sizeof(long long));
+        B200_CUDA(cudaMemsetAsync(d_counters.p, 0, N_COUNTERS * sizeof(long long), stream));
+        h_counters = (long long*)pinned_acquire(N_COUNTERS * sizeof(long long));
         expected_groups_hint = expected_groups > 0 ? expected_groups : 0;
         uint64_t want = 1ull << 16;
         if (expected_groups > 0) { while (want < (uint64_t)expected_groups * 2) want <<= 1; }
@@ -1777,7 +1843,7 @@ class GroupbyState {
                     t_ctor * 1e3, t_grow * 1e3, (long long)rebuilds, t_alloc * 1e3, t_spg * 1e3, t_finalize * 1e3, (unsigned long long)cap);
         if (copy_stream) { cudaStreamSynchronize(copy_stream); cudaStreamDestroy(copy_stream); }
         for (int b = 0; b < 2; b++) { if (stage_free[b]) cudaEventDestroy(stage_free[b]); if (stage_ready[b]) cudaEventDestroy(stage_ready[b]); }
-        pinned_release(h_counters, 8 * sizeof(long long));
+        pinned_release(h_counters, N_COUNTERS * sizeof(long long));
         pinned_release(h_spg, 24 * sizeof(long long));
         for (int b = 0; b < 2; b++) if (spg_ev[b]) cudaEventDestroy(spg_ev[b]);
         for (auto& pr : prof_events) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
@@ -1809,25 +1875,39 @@ class GroupbyState {
     }
 
     void read_counters() {
-        B200_CUDA(cudaMemcpyAsync(h_counters, d_counters.p, 8 * sizeof(long long), cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaMemcpyAsync(h_counters, d_counters.p, N_COUNTERS * sizeof(long long), cudaMemcpyDeviceToHost, stream));
         B200_CUDA(cudaStreamSynchronize(stream));
-        n_groups = h_counters[0];
+        n_groups = h_counters[CTR_GROUPS];
+    }
+
+    // the accumulator columns in wire order (per function a0, then a1 if it has one) into `out`; returns their number, acc_count()
+    template <typename P>
+    int wire_accs(const std::vector<DevBuf>& a0, const std::vector<DevBuf>& a1, P* out) const {
+        int n = 0;
+        for (int j = 0; j < n_funcs; j++) {
+            out[n++] = a0[j].as<unsigned long long>();
+            if (funcs[j].has_a1) out[n++] = a1[j].as<unsigned long long>();
+        }
+        return n;
+    }
+
+    // next power of two >= 2 x (groups + pending rows + headroom), and at least double
+    void grow_to_fit(int64_t pending, int64_t headroom = 0) {
+        uint64_t nc = cap;
+        while (nc < 2ull * (uint64_t)(n_groups + pending + headroom)) nc <<= 1;
+        if (nc == cap) nc <<= 1;
+        grow(nc);
     }
 
     void grow(uint64_t new_cap) {
-        double t0 = now();
-        struct Acc { double& t; double t0; ~Acc() { t += now() - t0; } } acc{t_grow, t0};
+        ScopedTimer timer{t_grow};
         if (nk > 1) { grow_mk(new_cap); return; }
         DevBuf nkeys; std::vector<DevBuf> na0(n_funcs), na1(n_funcs);
         alloc_table(new_cap, nkeys, na0, na1);
         RehashArgs ra{};
         ra.old_keys = d_keys.as<long long>(); ra.old_cap = cap; ra.new_keys = nkeys.as<long long>(); ra.new_cap = new_cap;
-        int n = 0;
-        for (int j = 0; j < n_funcs; j++) {
-            ra.old_acc[n] = d_a0[j].as<unsigned long long>(); ra.new_acc[n++] = na0[j].as<unsigned long long>();
-            if (funcs[j].has_a1) { ra.old_acc[n] = d_a1[j].as<unsigned long long>(); ra.new_acc[n++] = na1[j].as<unsigned long long>(); }
-        }
-        ra.n_acc = n;
+        ra.n_acc = wire_accs(d_a0, d_a1, ra.old_acc);
+        wire_accs(na0, na1, ra.new_acc);
         rehash_kernel<<<grid_for((int64_t)cap + 2), 256, 0, stream>>>(ra);
         launches++;
         B200_CUDA(cudaGetLastError());
@@ -1855,12 +1935,8 @@ class GroupbyState {
         ra.tags = ntags.as<unsigned long long>(); ra.mkmask = nmask.as<unsigned char>(); ra.cap = new_cap;
         ra.counters = d_counters.as<long long>(); ra.group_limit = -1;
         for (int j = 0; j < nk; j++) { ra.old_mk[j] = d_mk[j].as<long long>(); ra.mk[j] = nmk[j].as<long long>(); }
-        int n = 0;
-        for (int j = 0; j < n_funcs; j++) {
-            ra.old_acc[n] = d_a0[j].as<unsigned long long>(); ra.new_acc[n++] = na0[j].as<unsigned long long>();
-            if (funcs[j].has_a1) { ra.old_acc[n] = d_a1[j].as<unsigned long long>(); ra.new_acc[n++] = na1[j].as<unsigned long long>(); }
-        }
-        ra.n_acc = n;
+        ra.n_acc = wire_accs(d_a0, d_a1, ra.old_acc);
+        wire_accs(na0, na1, ra.new_acc);
         rehash_mk_kernel<<<grid_for((int64_t)cap), 256, 0, stream>>>(ra);
         launches++;
         B200_CUDA(cudaGetLastError());
@@ -1875,50 +1951,36 @@ class GroupbyState {
         bool could_fail = (int64_t)(cap / 2) - n_groups_bound < n;
         if (could_fail) d_fail.ensure(device, (size_t)n * 4);
         auto launch = [&](const uint32_t* index_list, int64_t rows) {
-            MkArgs a{};
-            a.nk = nk; a.dropna = dropna ? 1 : 0; a.n_rows = rows; a.index_list = index_list;
-            for (int j = 0; j < nk; j++) { a.key_data[j] = data[j]; a.key_valid[j] = valid[j]; a.key_ctype[j] = c_types[j]; a.mk[j] = d_mk[j].as<long long>(); }
-            a.tags = d_tags.as<unsigned long long>(); a.mkmask = d_mkmask.as<unsigned char>(); a.cap = cap;
-            a.counters = d_counters.as<long long>(); a.group_limit = (long long)(cap / 2); a.fail_list = d_fail.as<uint32_t>();
+            MkArgs a = mk_table_args();
+            a.dropna = dropna ? 1 : 0; a.n_rows = rows; a.index_list = index_list;
+            for (int j = 0; j < nk; j++) { a.key_data[j] = data[j]; a.key_valid[j] = valid[j]; a.key_ctype[j] = c_types[j]; }
             a.n_ops = n_funcs;
-            for (int j = 0; j < n_funcs; j++) {
-                const FuncSpec& f = funcs[j];
-                a.ops[j].kind = f.kind; a.ops[j].in_ctype = f.in_ctype;
-                a.ops[j].in_data = f.in_col >= 0 ? data[f.in_col] : nullptr;
-                a.ops[j].in_valid = f.in_col >= 0 ? valid[f.in_col] : nullptr;
-                a.ops[j].a0 = d_a0[j].p; a.ops[j].a1 = f.has_a1 ? d_a1[j].p : nullptr;
-            }
+            fill_ops(a.ops, data, valid);
             groupby_consume_mk_kernel<<<grid_for(rows), 256, 0, stream>>>(a);
             launches++; consume_launches += index_list == nullptr;
             B200_CUDA(cudaGetLastError());
         };
         launch(nullptr, n);
-        settle(n, could_fail, launch);
+        if (could_fail) settle<uint32_t>(d_fail, 1, fail_rows, launch);
         if (!could_fail) n_groups_bound += n; else n_groups_bound = n_groups;
         rows_consumed += n;
     }
 
-    // After a launch that may have failed rows: grow + replay until every row is in.
-    template <typename Replay>
-    void settle(int64_t chunk_rows, bool could_fail, Replay replay) {
-        if (!could_fail) return;
-        read_counters();
-        while (h_counters[1] > 0) {
-            int64_t nf = h_counters[1];
-            fail_rows += nf;
-            uint64_t nc = cap;
-            while (nc < 2ull * (uint64_t)(n_groups + nf)) nc <<= 1;
-            if (nc == cap) nc <<= 1;
-            grow(nc);
-            // the fail list becomes the index list of the replay; it cannot fail again (room for nf new groups)
+    // After a launch that may have failed rows: grow + replay until every row is in.  `list` holds counters[CTR_FAIL] entries
+    // of `words` T each (row indices, or rows of a wire format); `replayed` counts them.  The replay reads a copy of the list:
+    // it appends the entries that fail again to `list` itself.  The grown table has room for every pending entry.
+    template <typename T, typename Replay>
+    void settle(const DevBuf& list, size_t words, int64_t& replayed, Replay replay) {
+        for (read_counters(); h_counters[CTR_FAIL] > 0; read_counters()) {
+            const int64_t nf = h_counters[CTR_FAIL];
+            replayed += nf;
+            grow_to_fit(nf);
             DevBuf replay_list;
-            replay_list.alloc((size_t)nf * 4);
-            B200_CUDA(cudaMemcpyAsync(replay_list.p, d_fail.p, (size_t)nf * 4, cudaMemcpyDeviceToDevice, stream));
-            B200_CUDA(cudaMemsetAsync((char*)d_counters.p + 8, 0, 8, stream));
-            replay(replay_list.as<uint32_t>(), nf);
-            read_counters();
+            replay_list.alloc((size_t)nf * words * sizeof(T));
+            B200_CUDA(cudaMemcpyAsync(replay_list.p, list.p, (size_t)nf * words * sizeof(T), cudaMemcpyDeviceToDevice, stream));
+            B200_CUDA(cudaMemsetAsync((char*)d_counters.p + CTR_FAIL * 8, 0, 8, stream));
+            replay(replay_list.as<T>(), nf);
         }
-        (void)chunk_rows;
     }
 
     // ---- SM-partitioned fast path (SPG) ----
@@ -1941,56 +2003,45 @@ class GroupbyState {
         if (sms > SPG_MAX_OWNERS - 1 || max_smem < 64 * 1024) return false;
         spg_ns = ((int)(((size_t)max_smem - 64) / 16) - SPG_STASH) & ~1;
         spg_smem = (size_t)(spg_ns + SPG_STASH) * 16 + 16;
-        const void* fns[3] = {(const void*)spg_aggregate_kernel<true, true>, (const void*)spg_aggregate_kernel<true, false>,
-                              (const void*)spg_aggregate_kernel<false, true>};
-        for (auto f : fns)
-            if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spg_smem) != cudaSuccess) { cudaGetLastError(); return false; }
-        const void* tf[3] = {(const void*)spg_partition_tma_kernel<true, true>, (const void*)spg_partition_tma_kernel<true, false>,
-                             (const void*)spg_partition_tma_kernel<false, true>};
-        for (auto f : tf)
-            if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spg_tma_smem()) != cudaSuccess) { cudaGetLastError(); return false; }
-        const void* hf[3] = {(const void*)spg_partition_tma_kernel<true, true, true>, (const void*)spg_partition_tma_kernel<true, false, true>,
-                             (const void*)spg_partition_tma_kernel<false, true, true>};
-        for (auto f : hf)
-            if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spg_tma_smem(true)) != cudaSuccess) { cudaGetLastError(); return false; }
+        // K1 / K1-hot / K2 and the big LC kernel: SPG is off when one of them cannot get its shared memory
+        bool ok = true;
+        for_each_sum_cnt([&](auto s, auto c) {
+            ok = ok && set_smem_limit((const void*)spg_aggregate_kernel<s, c>, spg_smem)
+                    && set_smem_limit((const void*)spg_partition_tma_kernel<s, c>, spg_tma_smem())
+                    && set_smem_limit((const void*)spg_partition_tma_kernel<s, c, true>, spg_tma_smem(true))
+                    && set_smem_limit((const void*)groupby_lowcard_kernel<s, c, LC_SLOTS_BIG, 2>, (size_t)LC_SLOTS_BIG * 20 + 64);
+        });
+        if (!ok) return false;
         {   // SPG-N (spgn.cuh): narrow bucket rows
             spgn_ns = ((int)(((size_t)max_smem - 256) / 12) - SPG_STASH) & ~1;  // (K2n also has a few static shared words)
             spgn_smem = (size_t)(spgn_ns + SPG_STASH) * 12 + 16;
-            const void* nk1[3] = {(const void*)spgn_partition_kernel<true, true>, (const void*)spgn_partition_kernel<true, false>, (const void*)spgn_partition_kernel<false, true>};
-            const void* nk2[3] = {(const void*)spgn_aggregate_kernel<true, true>, (const void*)spgn_aggregate_kernel<true, false>, (const void*)spgn_aggregate_kernel<false, true>};
             spgn_enabled = true;
-            for (auto f : nk1) if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spgn_part_smem()) != cudaSuccess) { cudaGetLastError(); spgn_enabled = false; }
-            for (auto f : nk2) if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spgn_smem) != cudaSuccess) { cudaGetLastError(); spgn_enabled = false; }
+            for_each_sum_cnt([&](auto s, auto c) {
+                if (!set_smem_limit((const void*)spgn_partition_kernel<s, c>, spgn_part_smem())) spgn_enabled = false;
+                if (!set_smem_limit((const void*)spgn_aggregate_kernel<s, c>, spgn_smem)) spgn_enabled = false;
+            });
             const char* e8 = getenv("B200_SPG_NARROW");
             if (e8 && e8[0] == '0') spgn_enabled = false;
         }
         {   // SPG-G (spgg.cuh): generic signatures
             spgg_enabled = 2 * sms <= GEN_CLS;  // classes of K1g's counting sort: at least owners + owners
-            const void* gp[6] = {(const void*)spgg_partition_kernel<8, 8>, (const void*)spgg_partition_kernel<8, 4>, (const void*)spgg_partition_kernel<8, 0>,
-                                 (const void*)spgg_partition_kernel<4, 8>, (const void*)spgg_partition_kernel<4, 4>, (const void*)spgg_partition_kernel<4, 0>};
-            for (auto f : gp)
-                if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GEN_K1_SMEM) != cudaSuccess) { cudaGetLastError(); spgg_enabled = false; }
+            for_each_spgg_part([&](auto ks, auto vs) {
+                if (!set_smem_limit((const void*)spgg_partition_kernel<ks, vs>, GEN_K1_SMEM)) spgg_enabled = false;
+            });
             for (int v = 0; v < 4; v++) {  // v = mm + 2 * nn
                 const int sb = 16 + ((v & 1) ? 16 : 0) + ((v & 2) ? 4 : 0);
                 spgg_ns[v] = ((int)(((size_t)max_smem - 64) / sb) - SPG_STASH) & ~1;
                 spgg_smem[v] = (size_t)(spgg_ns[v] + SPG_STASH) * sb + 16;
             }
-            const void* ga[8] = {(const void*)spgg_aggregate_kernel<false, false, false>, (const void*)spgg_aggregate_kernel<true, false, false>,
-                                 (const void*)spgg_aggregate_kernel<false, true, false>, (const void*)spgg_aggregate_kernel<true, true, false>,
-                                 (const void*)spgg_aggregate_kernel<false, false, true>, (const void*)spgg_aggregate_kernel<true, false, true>,
-                                 (const void*)spgg_aggregate_kernel<false, true, true>, (const void*)spgg_aggregate_kernel<true, true, true>};
-            for (int q = 0; q < 8; q++)  // q = sum + 2 * mm + 4 * nn
-                if (cudaFuncSetAttribute(ga[q], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spgg_smem[q >> 1]) != cudaSuccess) { cudaGetLastError(); spgg_enabled = false; }
+            for_each_spgg_agg([&](auto s, auto mm, auto nn) {
+                if (!set_smem_limit((const void*)spgg_aggregate_kernel<s, mm, nn>, spgg_smem[mm + 2 * nn])) spgg_enabled = false;
+            });
             const char* e7 = getenv("B200_SPG_GEN");
             if (e7 && e7[0] == '0') spgg_enabled = false;
         }
-        if (cudaFuncSetAttribute((const void*)spg_hot_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SPG_HOT_SAMPLE_SMEM) != cudaSuccess) { cudaGetLastError(); return false; }
+        if (!set_smem_limit((const void*)spg_hot_sample_kernel, SPG_HOT_SAMPLE_SMEM)) return false;
         { const char* e4 = getenv("B200_SPG_HOT"); spg_hot_enabled = !(e4 && e4[0] == '0'); }
         d_hot.alloc((size_t)SPG_HOT_SLOTS * 8 + 16);
-        const void* lf[3] = {(const void*)groupby_lowcard_kernel<true, true, LC_SLOTS_BIG, 2>, (const void*)groupby_lowcard_kernel<true, false, LC_SLOTS_BIG, 2>,
-                             (const void*)groupby_lowcard_kernel<false, true, LC_SLOTS_BIG, 2>};
-        for (auto f : lf)
-            if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)LC_SLOTS_BIG * 20 + 64)) != cudaSuccess) { cudaGetLastError(); return false; }
         { const char* e3 = getenv("B200_LC"); lc_enabled = !(e3 && e3[0] == '0'); }
         spg_owners = sms;  // one owner (bucket + shared table) per SM
         // SPG-G: one counter per class of K1g.  consume_spg_gen clears n_vo + owners counters, and n_vo (owners x passes) may
@@ -2034,47 +2085,43 @@ class GroupbyState {
     long long* h_spg = nullptr;  // pinned: [slot][8] counter snapshots
     cudaEvent_t spg_ev[2] = {nullptr, nullptr};
 
-    int64_t spgn_wide_rows = 0;  // rows that did not fit the narrow format so far (device counter 5)
+    int64_t spgn_wide_rows = 0;  // rows that did not fit the narrow format so far (counters[CTR_WIDE])
+    static int spg_retry_slot(int slot) { return slot == 0 ? CTR_FAIL : CTR_RETRY1; }  // counter of launch slot `slot`'s retry list
     void spg_finish(int slot, int sum_j, int cnt_j) {
         B200_CUDA(cudaEventSynchronize(spg_ev[slot]));
-        const long long* hc = h_spg + slot * 8;
-        n_groups = hc[0];
-        spgn_wide_rows = hc[5];
-        int64_t nr = hc[1 + 5 * slot];  // retry rows of that launch: counters[1] (slot 0) / counters[6] (slot 1)
-        while (nr > 0) {
-            // rows / partials that found the global table full: grow, then merge them like received partial rows
-            spg_retry_rows += nr;
-            B200_CUDA(cudaStreamSynchronize(stream));  // the other in-flight launch uses the table we are about to replace
-            read_counters();
-            uint64_t nc = cap;
-            int64_t pending = h_counters[1] + h_counters[6];
-            // the snapshot this call was made on may be stale: the other slot's spg_finish already grew the table and merged
-            // BOTH retry lists (their live counters are 0 then) — nothing left to do, and no second grow
-            if (pending == 0) break;
-            while (nc < 2ull * (uint64_t)(n_groups + pending + (int64_t)spg_owners * spg_ns)) nc <<= 1;
-            if (nc == cap) nc <<= 1;
-            grow(nc);
-            for (int sl = 0; sl < 2; sl++) {
-                int64_t cnt = h_counters[1 + 5 * sl];
-                if (cnt == 0) continue;
-                B200_CUDA(cudaMemsetAsync((char*)d_counters.p + 8 * (1 + 5 * sl), 0, 8, stream));
-                CombineArgs c{};
-                c.in = d_retry2[sl].as<unsigned long long>(); c.n_rows = cnt; c.row_words = 4;
-                d_fail.ensure(device, (size_t)cnt * 4);
-                c.tkeys = d_keys.as<long long>(); c.cap = cap; c.counters = d_counters.as<long long>(); c.group_limit = (long long)(cap / 2);
-                c.fail_list = d_fail.as<uint32_t>(); c.index_list = nullptr; c.n_ops = 0;  // cannot fail: the table was grown for all pending rows
-                // wire order = function order of the (at most two) accumulators
-                int order[2] = {sum_j, cnt_j};
-                if (sum_j >= 0 && cnt_j >= 0 && cnt_j < sum_j) std::swap(order[0], order[1]);
-                if (order[0] < 0) std::swap(order[0], order[1]);
-                for (int q = 0; q < 2; q++) if (order[q] >= 0) { c.kinds[c.n_ops] = K_SUM_I64; c.a0[c.n_ops] = d_a0[order[q]].p; c.a1[c.n_ops] = nullptr; c.n_ops++; }
-                combine_partials_kernel<<<grid_for(cnt), 256, 0, stream>>>(c);
-                launches++;
-                B200_CUDA(cudaGetLastError());
-            }
-            read_counters();
-            nr = 0;
+        const long long* hc = h_spg + slot * N_COUNTERS;
+        n_groups = hc[CTR_GROUPS];
+        spgn_wide_rows = hc[CTR_WIDE];
+        const int64_t nr = hc[spg_retry_slot(slot)];  // retry rows of that launch
+        if (nr == 0) return;
+        // rows / partials that found the global table full: grow, then merge them like received partial rows
+        spg_retry_rows += nr;
+        B200_CUDA(cudaStreamSynchronize(stream));  // the other in-flight launch uses the table we are about to replace
+        read_counters();
+        const int64_t pending = h_counters[CTR_FAIL] + h_counters[CTR_RETRY1];
+        // the snapshot this call was made on may be stale: the other slot's spg_finish already grew the table and merged
+        // BOTH retry lists (their live counters are 0 then) — nothing left to do, and no second grow
+        if (pending == 0) return;
+        grow_to_fit(pending, (int64_t)spg_owners * spg_ns);
+        for (int sl = 0; sl < 2; sl++) {
+            int64_t cnt = h_counters[spg_retry_slot(sl)];
+            if (cnt == 0) continue;
+            B200_CUDA(cudaMemsetAsync((char*)d_counters.p + spg_retry_slot(sl) * 8, 0, 8, stream));
+            CombineArgs c{};
+            c.in = d_retry2[sl].as<unsigned long long>(); c.n_rows = cnt; c.row_words = 4;
+            d_fail.ensure(device, (size_t)cnt * 4);
+            c.tkeys = d_keys.as<long long>(); c.cap = cap; c.counters = d_counters.as<long long>(); c.group_limit = (long long)(cap / 2);
+            c.fail_list = d_fail.as<uint32_t>(); c.index_list = nullptr; c.n_ops = 0;  // cannot fail: the table was grown for all pending rows
+            // wire order = function order of the (at most two) accumulators
+            int order[2] = {sum_j, cnt_j};
+            if (sum_j >= 0 && cnt_j >= 0 && cnt_j < sum_j) std::swap(order[0], order[1]);
+            if (order[0] < 0) std::swap(order[0], order[1]);
+            for (int q = 0; q < 2; q++) if (order[q] >= 0) { c.kinds[c.n_ops] = K_SUM_I64; c.a0[c.n_ops] = d_a0[order[q]].p; c.a1[c.n_ops] = nullptr; c.n_ops++; }
+            combine_partials_kernel<<<grid_for(cnt), 256, 0, stream>>>(c);
+            launches++;
+            B200_CUDA(cudaGetLastError());
         }
+        read_counters();
     }
 
     void consume_spg(const long long* keys, const long long* vals, int64_t n, int sum_j, int cnt_j, bool lowcard = false, int64_t est_groups = 0) {
@@ -2084,8 +2131,7 @@ class GroupbyState {
             h_spg = (long long*)pinned_acquire(24 * sizeof(long long));  // [slot][8] counter snapshots + n_hot read-back
             for (int b = 0; b < 2; b++) B200_CUDA(cudaEventCreateWithFlags(&spg_ev[b], cudaEventDisableTiming));
         }
-        double tspg0 = now();
-        struct Acc2 { double& t; double t0; ~Acc2() { t += now() - t0; } } acc2{t_spg, tspg0};
+        ScopedTimer timer{t_spg};
         read_counters();  // exact group count before the first launch
         n_groups_bound = n_groups;
         if (!lowcard && !spg_hot_sampled) {
@@ -2123,25 +2169,19 @@ class GroupbyState {
             a.acc_sum = sum_j >= 0 ? d_a0[sum_j].as<unsigned long long>() : nullptr;
             a.acc_cnt = cnt_j >= 0 ? d_a0[cnt_j].as<unsigned long long>() : nullptr;
             a.counters = d_counters.as<long long>(); a.group_limit = (long long)(cap / 2);
-            a.retry_ctr = d_counters.as<long long>() + 1 + 5 * slot;
+            a.retry_ctr = d_counters.as<long long>() + spg_retry_slot(slot);
             a.bucket = d_bucket.as<longlong2>(); a.bucket_cnt = d_bucket_cnt.as<unsigned long long>(); a.bucket_cap = bucket_cap;
             a.retry = d_retry2[slot].as<unsigned long long>();
             a.sum_first = (sum_j >= 0 && cnt_j >= 0 && sum_j < cnt_j) ? 1 : 0; a.ns = spg_ns; a.n_pass = spg_passes;
-            cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-            if (profiling) { B200_CUDA(cudaEventCreate(&ev0)); B200_CUDA(cudaEventCreate(&ev1)); B200_CUDA(cudaEventRecord(ev0, stream)); }
+            const ProfEvents prof = prof_begin(profiling);
             if (lowcard) {
                 const bool small = lowcard_small;
                 int gl = (int)std::min<int64_t>((int64_t)sms * (small ? 3 : 2), (rows + LC_THREADS * 2 - 1) / (LC_THREADS * 2));
                 size_t lsm = (size_t)(small ? LC_SLOTS_SMALL : LC_SLOTS_BIG) * 20 + 64;
-                if (small) {
-                    if (sum_j >= 0 && cnt_j >= 0) groupby_lowcard_kernel<true, true, LC_SLOTS_SMALL, 3><<<gl, LC_THREADS, lsm, stream>>>(a);
-                    else if (sum_j >= 0) groupby_lowcard_kernel<true, false, LC_SLOTS_SMALL, 3><<<gl, LC_THREADS, lsm, stream>>>(a);
-                    else groupby_lowcard_kernel<false, true, LC_SLOTS_SMALL, 3><<<gl, LC_THREADS, lsm, stream>>>(a);
-                } else {
-                    if (sum_j >= 0 && cnt_j >= 0) groupby_lowcard_kernel<true, true, LC_SLOTS_BIG, 2><<<gl, LC_THREADS, lsm, stream>>>(a);
-                    else if (sum_j >= 0) groupby_lowcard_kernel<true, false, LC_SLOTS_BIG, 2><<<gl, LC_THREADS, lsm, stream>>>(a);
-                    else groupby_lowcard_kernel<false, true, LC_SLOTS_BIG, 2><<<gl, LC_THREADS, lsm, stream>>>(a);
-                }
+                with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
+                    if (small) groupby_lowcard_kernel<s, c, LC_SLOTS_SMALL, 3><<<gl, LC_THREADS, lsm, stream>>>(a);
+                    else groupby_lowcard_kernel<s, c, LC_SLOTS_BIG, 2><<<gl, LC_THREADS, lsm, stream>>>(a);
+                });
                 lc_launches++;
             } else {
                 int g2 = (int)std::min<int64_t>((int64_t)sms * SPG_TCTAS, (rows + SPG_TILE - 1) / SPG_TILE);
@@ -2162,27 +2202,22 @@ class GroupbyState {
                     a.bucket_cap = bucket_cap & ~1ll;
                     const size_t nsm = spgn_part_smem();
                     const int g2 = (int)std::min<int64_t>((int64_t)sms * SPGN_CTAS, (rows + SPGN_TILE - 1) / SPGN_TILE);
-                    if (sum_j >= 0 && cnt_j >= 0) { spgn_partition_kernel<true, true><<<g2, SPG_TTHREADS, nsm, stream>>>(a); spgn_aggregate_kernel<true, true><<<spg_owners, SPG_THREADS, spgn_smem, stream>>>(a); }
-                    else if (sum_j >= 0) { spgn_partition_kernel<true, false><<<g2, SPG_TTHREADS, nsm, stream>>>(a); spgn_aggregate_kernel<true, false><<<spg_owners, SPG_THREADS, spgn_smem, stream>>>(a); }
-                    else { spgn_partition_kernel<false, true><<<g2, SPG_TTHREADS, nsm, stream>>>(a); spgn_aggregate_kernel<false, true><<<spg_owners, SPG_THREADS, spgn_smem, stream>>>(a); }
+                    with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
+                        spgn_partition_kernel<s, c><<<g2, SPG_TTHREADS, nsm, stream>>>(a);
+                        spgn_aggregate_kernel<s, c><<<spg_owners, SPG_THREADS, spgn_smem, stream>>>(a);
+                    });
                     spgn_launches++;
-                } else if (sum_j >= 0 && cnt_j >= 0) {
-                    if (hot) spg_partition_tma_kernel<true, true, true><<<g2, SPG_TTHREADS, tsm, stream>>>(a);
-                    else spg_partition_tma_kernel<true, true><<<g2, SPG_TTHREADS, tsm, stream>>>(a);
-                    spg_aggregate_kernel<true, true><<<spg_owners, SPG_THREADS, spg_smem, stream>>>(a);
-                } else if (sum_j >= 0) {
-                    if (hot) spg_partition_tma_kernel<true, false, true><<<g2, SPG_TTHREADS, tsm, stream>>>(a);
-                    else spg_partition_tma_kernel<true, false><<<g2, SPG_TTHREADS, tsm, stream>>>(a);
-                    spg_aggregate_kernel<true, false><<<spg_owners, SPG_THREADS, spg_smem, stream>>>(a);
                 } else {
-                    if (hot) spg_partition_tma_kernel<false, true, true><<<g2, SPG_TTHREADS, tsm, stream>>>(a);
-                    else spg_partition_tma_kernel<false, true><<<g2, SPG_TTHREADS, tsm, stream>>>(a);
-                    spg_aggregate_kernel<false, true><<<spg_owners, SPG_THREADS, spg_smem, stream>>>(a);
+                    with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
+                        if (hot) spg_partition_tma_kernel<s, c, true><<<g2, SPG_TTHREADS, tsm, stream>>>(a);
+                        else spg_partition_tma_kernel<s, c><<<g2, SPG_TTHREADS, tsm, stream>>>(a);
+                        spg_aggregate_kernel<s, c><<<spg_owners, SPG_THREADS, spg_smem, stream>>>(a);
+                    });
                 }
             }
             B200_CUDA(cudaGetLastError());
-            if (ev0) { B200_CUDA(cudaEventRecord(ev1, stream)); prof_events.emplace_back(ev0, ev1); }
-            B200_CUDA(cudaMemcpyAsync(h_spg + slot * 8, d_counters.p, 8 * sizeof(long long), cudaMemcpyDeviceToHost, stream));
+            prof_end(prof);
+            B200_CUDA(cudaMemcpyAsync(h_spg + slot * N_COUNTERS, d_counters.p, N_COUNTERS * sizeof(long long), cudaMemcpyDeviceToHost, stream));
             B200_CUDA(cudaEventRecord(spg_ev[slot], stream));
             launches += 2; consume_launches++; spg_launches++;
             rows_consumed += rows;
@@ -2227,8 +2262,7 @@ class GroupbyState {
     PooledBuf d_nbucket;  // key-only buckets of the rows whose value is NA
 
     void consume_spg_gen(const std::vector<const void*>& data, const std::vector<const uint8_t*>& valid, int64_t n, const GenSig& gs, int passes) {
-        double tspg0 = now();
-        struct Acc2 { double& t; double t0; ~Acc2() { t += now() - t0; } } acc2{t_spg, tspg0};
+        ScopedTimer timer{t_spg};
         const int kct = c_types[0], vct = gs.vcol >= 0 ? c_types[gs.vcol] : CT_INT64;
         const int ks = ctype_size(kct), vs = gs.vcol >= 0 ? ctype_size(vct) : 0;
         const int mm = gs.layout;
@@ -2249,7 +2283,7 @@ class GroupbyState {
                 SpgGenArgs g{};
                 g.s.n_rows = rows; g.s.n_owners = spg_owners;
                 g.s.tkeys = d_keys.as<long long>(); g.s.cap = cap; g.s.counters = d_counters.as<long long>(); g.s.group_limit = (long long)(cap / 2);
-                g.s.retry_ctr = d_counters.as<long long>() + 1; g.s.retry = d_retry2[0].as<unsigned long long>();
+                g.s.retry_ctr = d_counters.as<long long>() + CTR_FAIL; g.s.retry = d_retry2[0].as<unsigned long long>();
                 g.s.bucket = d_bucket.as<longlong2>(); g.s.bucket_cnt = d_bucket_cnt.as<unsigned long long>(); g.s.bucket_cap = bucket_cap;
                 g.s.ns = spgg_ns[mm]; g.s.n_pass = passes;
                 g.nbucket = v_nullable ? d_nbucket.as<long long>() : nullptr; g.n_vo = n_vo;
@@ -2265,50 +2299,23 @@ class GroupbyState {
                 }
                 return g;
             };
-            SpgGenArgs g = make_args();
-            cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-            if (profiling) { B200_CUDA(cudaEventCreate(&ev0)); B200_CUDA(cudaEventCreate(&ev1)); B200_CUDA(cudaEventRecord(ev0, stream)); }
+            const SpgGenArgs g = make_args();
+            const ProfEvents prof = prof_begin(profiling);
             const int g1 = (int)std::min<int64_t>((int64_t)sms * SPG_TCTAS, (rows + SPG_TILE - 1) / SPG_TILE);
-            const size_t psm = GEN_K1_SMEM;
-            if (ks == 8 && vs == 8) spgg_partition_kernel<8, 8><<<g1, SPG_TTHREADS, psm, stream>>>(g);
-            else if (ks == 8 && vs == 4) spgg_partition_kernel<8, 4><<<g1, SPG_TTHREADS, psm, stream>>>(g);
-            else if (ks == 8) spgg_partition_kernel<8, 0><<<g1, SPG_TTHREADS, psm, stream>>>(g);
-            else if (vs == 8) spgg_partition_kernel<4, 8><<<g1, SPG_TTHREADS, psm, stream>>>(g);
-            else if (vs == 4) spgg_partition_kernel<4, 4><<<g1, SPG_TTHREADS, psm, stream>>>(g);
-            else spgg_partition_kernel<4, 0><<<g1, SPG_TTHREADS, psm, stream>>>(g);
-#define B200_SPGG_K2(S, M, N) spgg_aggregate_kernel<S, M, N><<<spg_owners, SPG_THREADS, spgg_smem[mm], stream>>>(g)
-            switch ((gs.has_sum ? 1 : 0) + (gs.has_mm ? 2 : 0) + (gs.has_nn ? 4 : 0)) {
-                case 0: B200_SPGG_K2(false, false, false); break;
-                case 1: B200_SPGG_K2(true, false, false); break;
-                case 2: B200_SPGG_K2(false, true, false); break;
-                case 3: B200_SPGG_K2(true, true, false); break;
-                case 4: B200_SPGG_K2(false, false, true); break;
-                case 5: B200_SPGG_K2(true, false, true); break;
-                case 6: B200_SPGG_K2(false, true, true); break;
-                default: B200_SPGG_K2(true, true, true); break;
-            }
-#undef B200_SPGG_K2
+            with_spgg_part(ks, vs, [&](auto k, auto v) { spgg_partition_kernel<k, v><<<g1, SPG_TTHREADS, GEN_K1_SMEM, stream>>>(g); });
+            with_spgg_agg(gs.has_sum, gs.has_mm, gs.has_nn, [&](auto s, auto m, auto nn) {
+                spgg_aggregate_kernel<s, m, nn><<<spg_owners, SPG_THREADS, spgg_smem[mm], stream>>>(g);
+            });
             B200_CUDA(cudaGetLastError());
-            if (ev0) { B200_CUDA(cudaEventRecord(ev1, stream)); prof_events.emplace_back(ev0, ev1); }
+            prof_end(prof);
             launches += 2; consume_launches++; spg_launches++; spgg_launches++;
             rows_consumed += rows;
-            read_counters();
-            while (h_counters[1] > 0) {  // partials that found the global table at its limit: grow, replay them
-                const int64_t nr = h_counters[1];
-                spg_retry_rows += nr;
-                uint64_t nc = cap;
-                while (nc < 2ull * (uint64_t)(n_groups + nr)) nc <<= 1;
-                if (nc == cap) nc <<= 1;
-                grow(nc);
-                d_retry2[1].ensure(device, (size_t)nr * GEN_RETRY_WORDS * 8);
-                B200_CUDA(cudaMemcpyAsync(d_retry2[1].p, d_retry2[0].p, (size_t)nr * GEN_RETRY_WORDS * 8, cudaMemcpyDeviceToDevice, stream));
-                B200_CUDA(cudaMemsetAsync((char*)d_counters.p + 8, 0, 8, stream));
-                SpgGenArgs g2 = make_args();
-                spgg_replay_kernel<<<grid_for(nr), 256, 0, stream>>>(g2, d_retry2[1].as<unsigned long long>(), (long long)nr);
+            // partials that found the global table at its limit: grow, replay them
+            settle<unsigned long long>(d_retry2[0], GEN_RETRY_WORDS, spg_retry_rows, [&](const unsigned long long* list, int64_t nr) {
+                spgg_replay_kernel<<<grid_for(nr), 256, 0, stream>>>(make_args(), list, (long long)nr);
                 launches++;
                 B200_CUDA(cudaGetLastError());
-                read_counters();
-            }
+            });
         }
         n_groups_bound = n_groups;
     }
@@ -2331,57 +2338,43 @@ class GroupbyState {
             }
         }
         if (fast && (((uintptr_t)data[0] & 15) || (vcol >= 0 && ((uintptr_t)data[vcol] & 15)))) fast = false;
-        // SM-partitioned path: big batches whose (estimated) cardinality fits the chip's shared memory
-        if (fast && n >= (1 << 20) && spg_probe()) {
-            const char* env = getenv("B200_SPG");
-            bool force = env && env[0] == '1';
-            int64_t est = std::max(expected_groups_hint, n_groups);
-            if (!force && est == 0 && rows_consumed == 0) {
-                // cardinality unknown: learn it from a prefix through the direct kernel
-                int64_t prefix = std::min<int64_t>(n, 1 << 20);
-                std::vector<const void*> d2(data); std::vector<const uint8_t*> v2(valid);
-                consume_direct(d2, v2, prefix, fast, sum_j, cnt_j, vcol, /*force_count=*/true);
-                est = n_groups;
-                if (prefix == n) return;
-                for (int c = 0; c < n_cols; c++) if (data[c]) d2[c] = (const char*)data[c] + prefix * ctype_size(c_types[c]);
-                if (spg_pass_count(est) > 0) { spg_passes = spg_pass_count(est); consume_spg((const long long*)d2[0], vcol >= 0 ? (const long long*)d2[vcol] : nullptr, n - prefix, sum_j, cnt_j, lc_pick(est), est); }
-                else consume_direct(d2, v2, n - prefix, fast, sum_j, cnt_j, vcol, false);
-                return;
+        // SM-partitioned paths for big batches whose (estimated) cardinality fits the chip's shared memory: SPG for the fast-path
+        // signature, SPG-G for generic ones (nullable / 4-byte keys or values / mean / min / max over one integer column)
+        const bool spg = n >= (1 << 20) && spg_probe();
+        GenSig gs;
+        const bool gen = !fast && spg && spgg_enabled && gen_signature(data, valid, gs);
+        if (!(fast && spg) && !gen) { consume_direct(data, valid, n, fast, sum_j, cnt_j, vcol, false); return; }
+        const char* env = getenv("B200_SPG");
+        const bool force = fast && env && env[0] == '1';
+        int64_t est = std::max(expected_groups_hint, n_groups);
+        std::vector<const void*> d2(data); std::vector<const uint8_t*> v2(valid);
+        int64_t left = n;
+        const bool learned = !force && est == 0 && rows_consumed == 0;
+        if (learned) {  // cardinality unknown: learn it from a prefix through the direct kernel
+            const int64_t prefix = std::min<int64_t>(n, 1 << 20);
+            consume_direct(data, valid, prefix, fast, sum_j, cnt_j, vcol, /*force_count=*/true);
+            est = n_groups;
+            if (prefix == n) return;
+            for (int c = 0; c < n_cols; c++) {  // (the fast-path signature has no validity bitmaps)
+                if (data[c]) d2[c] = (const char*)data[c] + prefix * ctype_size(c_types[c]);
+                if (valid[c]) v2[c] = valid[c] + prefix / 8;
             }
+            left = n - prefix;
+        }
+        if (fast) {
             if (force || spg_pass_count(est) > 0) {
                 spg_passes = std::max(1, spg_pass_count(est));
-                consume_spg((const long long*)data[0], vcol >= 0 ? (const long long*)data[vcol] : nullptr, n, sum_j, cnt_j, est > 0 && lc_pick(est), est);
+                // LC only on an estimate: a hint, groups already in the table, or a prefix (even one that found none)
+                const bool lowcard = (learned || est > 0) && lc_pick(est);
+                consume_spg((const long long*)d2[0], vcol >= 0 ? (const long long*)d2[vcol] : nullptr, left, sum_j, cnt_j, lowcard, est);
                 return;
             }
+        } else if (est > LC_SLOTS_BIG / 4 && spgg_pass_count(est, gs.layout) > 0 && left >= (1 << 16)) {
+            // (below ~1000 groups the owners are unevenly loaded, and there is no low-cardinality generic kernel: direct path)
+            consume_spg_gen(d2, v2, left, gs, spgg_pass_count(est, gs.layout));
+            return;
         }
-        // generic signatures (nullable / 4-byte keys or values / mean / min / max over one integer column): same two-kernel path
-        if (!fast && n >= (1 << 20) && spg_probe() && spgg_enabled) {
-            GenSig gs;
-            if (gen_signature(data, valid, gs)) {
-                int64_t est = std::max(expected_groups_hint, n_groups);
-                std::vector<const void*> d2(data); std::vector<const uint8_t*> v2(valid);
-                int64_t left = n;
-                if (est == 0 && rows_consumed == 0) {  // cardinality unknown: learn it from a prefix through the direct kernel
-                    const int64_t prefix = std::min<int64_t>(n, 1 << 20);
-                    consume_direct(data, valid, prefix, false, -1, -1, -1, /*force_count=*/true);
-                    est = n_groups;
-                    if (prefix == n) return;
-                    for (int c = 0; c < n_cols; c++) {
-                        if (data[c]) d2[c] = (const char*)data[c] + prefix * ctype_size(c_types[c]);
-                        if (valid[c]) v2[c] = valid[c] + prefix / 8;
-                    }
-                    left = n - prefix;
-                }
-                // below ~1000 groups the owners are unevenly loaded (and there is no low-cardinality generic kernel): direct path
-                if (est > LC_SLOTS_BIG / 4 && spgg_pass_count(est, gs.layout) > 0 && left >= (1 << 16)) {
-                    consume_spg_gen(d2, v2, left, gs, spgg_pass_count(est, gs.layout));
-                    return;
-                }
-                consume_direct(d2, v2, left, false, -1, -1, -1, false);
-                return;
-            }
-        }
-        consume_direct(data, valid, n, fast, sum_j, cnt_j, vcol, false);
+        consume_direct(d2, v2, left, fast, sum_j, cnt_j, vcol, false);
     }
 
     void consume_direct(const std::vector<const void*>& data, const std::vector<const uint8_t*>& valid, int64_t n, bool fast, int sum_j,
@@ -2390,36 +2383,27 @@ class GroupbyState {
         if (could_fail) d_fail.ensure(device, (size_t)n * 4);
         // table pointers are looked up at launch time: grow() replaces them between a launch and its replay
         auto launch = [&](const uint32_t* index_list, int64_t rows) {
-            long long* ctr = d_counters.as<long long>();
-            long long limit = (long long)(cap / 2);
-            cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-            if (profiling && index_list == nullptr) {
-                B200_CUDA(cudaEventCreate(&ev0)); B200_CUDA(cudaEventCreate(&ev1));
-                B200_CUDA(cudaEventRecord(ev0, stream));
-            }
+            const ProfEvents prof = prof_begin(profiling && index_list == nullptr);
             if (fast && index_list == nullptr) {
-                int g = grid_for(rows, 2);
                 const long long* k = (const long long*)data[0];
                 const long long* v = vcol >= 0 ? (const long long*)data[vcol] : nullptr;
                 unsigned long long* as = sum_j >= 0 ? d_a0[sum_j].as<unsigned long long>() : nullptr;
                 unsigned long long* ac = cnt_j >= 0 ? d_a0[cnt_j].as<unsigned long long>() : nullptr;
-                if (sum_j >= 0 && cnt_j >= 0)
-                    groupby_consume_i64_sumcount_kernel<true, true><<<g, 256, 0, stream>>>(k, v, rows, d_keys.as<long long>(), cap, as, ac, ctr, limit, d_fail.as<uint32_t>());
-                else if (sum_j >= 0)
-                    groupby_consume_i64_sumcount_kernel<true, false><<<g, 256, 0, stream>>>(k, v, rows, d_keys.as<long long>(), cap, as, ac, ctr, limit, d_fail.as<uint32_t>());
-                else
-                    groupby_consume_i64_sumcount_kernel<false, true><<<g, 256, 0, stream>>>(k, v, rows, d_keys.as<long long>(), cap, as, ac, ctr, limit, d_fail.as<uint32_t>());
+                with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
+                    groupby_consume_i64_sumcount_kernel<s, c><<<grid_for(rows, 2), 256, 0, stream>>>(
+                        k, v, rows, d_keys.as<long long>(), cap, as, ac, d_counters.as<long long>(), (long long)(cap / 2), d_fail.as<uint32_t>());
+                });
             } else {
                 ConsumeArgs a = generic_args(data, valid, index_list, rows);
                 groupby_consume_kernel<<<grid_for(rows), 256, 0, stream>>>(a);
             }
             launches++;
             if (index_list == nullptr) consume_launches++;
-            if (ev0) { B200_CUDA(cudaEventRecord(ev1, stream)); prof_events.emplace_back(ev0, ev1); }
+            prof_end(prof);
             B200_CUDA(cudaGetLastError());
         };
         launch(nullptr, n);
-        settle(n, could_fail, launch);
+        if (could_fail) settle<uint32_t>(d_fail, 1, fail_rows, launch);
         if (has_firstlast) {  // every row is in (replays included): the rows that won first / last write their values
             groupby_firstlast_fix_kernel<<<grid_for(n), 256, 0, stream>>>(generic_args(data, valid, nullptr, n));
             launches++;
@@ -2436,14 +2420,18 @@ class GroupbyState {
         a.counters = d_counters.as<long long>(); a.group_limit = (long long)(cap / 2); a.fail_list = d_fail.as<uint32_t>(); a.n_ops = n_funcs;
         // rank-major sequence numbers: rows of a lower rank come first (the reference's row-block distribution), then row order
         a.seq_base = ((unsigned long long)rank << 44) + (unsigned long long)rows_consumed;
+        fill_ops(a.ops, data, valid);
+        return a;
+    }
+    // the n_funcs aggregate updates of a consume launch (ConsumeArgs / MkArgs)
+    void fill_ops(OpDesc* ops, const std::vector<const void*>& data, const std::vector<const uint8_t*>& valid) const {
         for (int j = 0; j < n_funcs; j++) {
             const FuncSpec& f = funcs[j];
-            a.ops[j].kind = f.kind; a.ops[j].in_ctype = f.in_ctype;
-            a.ops[j].in_data = f.in_col >= 0 ? data[f.in_col] : nullptr;
-            a.ops[j].in_valid = f.in_col >= 0 ? valid[f.in_col] : nullptr;
-            a.ops[j].a0 = d_a0[j].p; a.ops[j].a1 = f.has_a1 ? d_a1[j].p : nullptr;
+            ops[j].kind = f.kind; ops[j].in_ctype = f.in_ctype;
+            ops[j].in_data = f.in_col >= 0 ? data[f.in_col] : nullptr;
+            ops[j].in_valid = f.in_col >= 0 ? valid[f.in_col] : nullptr;
+            ops[j].a0 = d_a0[j].p; ops[j].a1 = f.has_a1 ? d_a1[j].p : nullptr;
         }
-        return a;
     }
 
     int64_t n_groups_bound = 0;  // upper bound on groups in the table known to the host
@@ -2574,22 +2562,22 @@ class GroupbyState {
 
     // ---- finalize ----
     // Compacts the occupied slots (owned_only: of the groups this rank owns).  No host synchronisation: the output is sized by
-    // the table's group limit (cap / 2 + the two special slots), the count stays on the device (counters[2]).
+    // the table's group limit (cap / 2 + the two special slots), the count stays on the device (counters[CTR_OUT]).
     int64_t max_out_bound() const { return (int64_t)(cap / 2) + 2; }
     void compact(bool owned_only = false) {
         int64_t max_out = max_out_bound();
         d_slot_of_out.ensure((size_t)max_out * 8);
-        B200_CUDA(cudaMemsetAsync((char*)d_counters.p + 16, 0, 8, stream));
+        B200_CUDA(cudaMemsetAsync((char*)d_counters.p + CTR_OUT * 8, 0, 8, stream));
         if (nk > 1)
-            compact_mk_kernel<<<grid_for((int64_t)cap), 256, 0, stream>>>(d_tags.as<unsigned long long>(), cap, d_counters.as<long long>() + 2, d_slot_of_out.as<uint64_t>(),
+            compact_mk_kernel<<<grid_for((int64_t)cap), 256, 0, stream>>>(d_tags.as<unsigned long long>(), cap, d_counters.as<long long>() + CTR_OUT, d_slot_of_out.as<uint64_t>(),
                                                                            mk_owner(owned_only));
         else
             compact_slots_kernel<<<grid_for((int64_t)cap + 2), 256, 0, stream>>>(d_keys.as<long long>(), cap, d_counters.as<long long>(),
-                                                                                      d_counters.as<long long>() + 2, d_slot_of_out.as<uint64_t>(),
+                                                                                      d_counters.as<long long>() + CTR_OUT, d_slot_of_out.as<uint64_t>(),
                                                                                       owned_only ? n_pes : 1, rank);
         launches++;
         B200_CUDA(cudaGetLastError());
-        n_out = -1;  // known on the device (counters[2]); the host learns it with the next counter read-back
+        n_out = -1;  // known on the device (counters[CTR_OUT]); the host learns it with the next counter read-back
     }
 
     // nunique: count the distinct (key, value) pairs of every nested state into the outer table.  On the sharded path the host
@@ -2619,15 +2607,14 @@ class GroupbyState {
 
     int64_t finalize() {
         if (finalized) return n_out;
-        double tf0 = now();
-        struct Acc3 { double& t; double t0; ~Acc3() { t += now() - t0; } } acc3{t_finalize, tf0};
+        ScopedTimer timer{t_finalize};
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
         flush_coalesced();
         apply_nunique();
         compact(/*owned_only=*/parallel && n_pes > 1);
         const int64_t max_out = max_out_bound();
         EvalArgs e{};
-        e.tkeys = nk == 1 ? d_keys.as<long long>() : nullptr; e.cap = cap; e.slot_of_out = d_slot_of_out.as<uint64_t>(); e.n_out_ptr = d_counters.as<long long>() + 2;
+        e.tkeys = nk == 1 ? d_keys.as<long long>() : nullptr; e.cap = cap; e.slot_of_out = d_slot_of_out.as<uint64_t>(); e.n_out_ptr = d_counters.as<long long>() + CTR_OUT;
         e.key_ctype = c_types[0];
         size_t words = (size_t)((max_out + 31) / 32 + 1);
         if (nk == 1) {
@@ -2637,7 +2624,7 @@ class GroupbyState {
             if (key_nullable) { d_out_key_valid.ensure(words * 4); e.out_key_valid = d_out_key_valid.as<uint32_t>(); }
         } else {
             EvalMkKeysArgs k{};
-            k.nk = nk; k.mkmask = d_mkmask.as<unsigned char>(); k.slot_of_out = d_slot_of_out.as<uint64_t>(); k.n_out_ptr = d_counters.as<long long>() + 2;
+            k.nk = nk; k.mkmask = d_mkmask.as<unsigned char>(); k.slot_of_out = d_slot_of_out.as<uint64_t>(); k.n_out_ptr = d_counters.as<long long>() + CTR_OUT;
             for (int j = 0; j < nk; j++) {
                 k.mk[j] = d_mk[j].as<long long>(); k.key_ctype[j] = c_types[j];
                 d_out_mk[j].ensure((size_t)(max_out + 32) * ctype_size(c_types[j]));
@@ -2663,39 +2650,32 @@ class GroupbyState {
         B200_CUDA(cudaGetLastError());
         read_counters();  // one synchronisation: the output is complete and n_out is known
         if (xchg_fused) {
-            if (h_counters[7] != 0) {  // some rank's share did not fit its slab segment: nobody combined, the NCCL exchange takes over
-                B200_CUDA(cudaMemsetAsync((char*)d_counters.p + 56, 0, 8, stream));
+            if (h_counters[CTR_XCHG_OVERFLOW] != 0) {  // some rank's share did not fit its slab segment: nobody combined, the NCCL exchange takes over
+                B200_CUDA(cudaMemsetAsync((char*)d_counters.p + CTR_XCHG_OVERFLOW * 8, 0, 8, stream));
                 xchg_fused = false;
                 return -2;
             }
-            if (h_counters[1] > 0) {
+            if (h_counters[CTR_FAIL] > 0) {
                 // received rows that found the table at its group limit: grow, merge them from the slab (still intact), evaluate again
-                int64_t nf = h_counters[1];
-                fail_rows += nf;
-                uint64_t nc = cap;
-                while (nc < 2ull * (uint64_t)(n_groups + nf)) nc <<= 1;
-                if (nc == cap) nc <<= 1;
-                grow(nc);
-                DevBuf replay_list;
-                replay_list.alloc((size_t)nf * 4);
-                B200_CUDA(cudaMemcpyAsync(replay_list.p, d_fail.p, (size_t)nf * 4, cudaMemcpyDeviceToDevice, stream));
-                B200_CUDA(cudaMemsetAsync((char*)d_counters.p + 8, 0, 8, stream));
-                CombineArgs c = combine_args((const unsigned long long*)((const char*)xchg_slab + XCHG_HDR_BYTES), nf, /*group_limit=*/-1);
-                c.index_list = replay_list.as<uint32_t>();
-                if (nk > 1) { c.row_words = nk + 1 + acc_count(); MkArgs m = mk_table_args(); m.group_limit = -1; xchg_combine_mk_kernel<<<grid_for(nf), 256, 0, stream>>>(m, c, nullptr, n_pes, 0); }
-                else
-                combine_partials_kernel<<<grid_for(nf), 256, 0, stream>>>(c);
+                const unsigned long long* rows = (const unsigned long long*)((const char*)xchg_slab + XCHG_HDR_BYTES);
+                settle<uint32_t>(d_fail, 1, fail_rows, [&](const uint32_t* list, int64_t nf) {
+                    CombineArgs c = combine_args(rows, nf, /*group_limit=*/-1);
+                    c.index_list = list;
+                    if (nk > 1) { c.row_words = nk + 1 + acc_count(); MkArgs m = mk_table_args(); m.group_limit = -1; xchg_combine_mk_kernel<<<grid_for(nf), 256, 0, stream>>>(m, c, nullptr, n_pes, 0); }
+                    else
+                    combine_partials_kernel<<<grid_for(nf), 256, 0, stream>>>(c);
+                    launches++;
+                    B200_CUDA(cudaGetLastError());
+                });
                 if (has_firstlast) {  // over the whole slab again (idempotent): the table moved when it grew
-                    CombineArgs cf = combine_args((const unsigned long long*)((const char*)xchg_slab + XCHG_HDR_BYTES), 0, -1);
-                    combine_firstlast_fix_kernel<<<grid_for(1 << 20), 256, 0, stream>>>(cf, (const unsigned long long*)xchg_slab, n_pes, xchg_cap_rows);
+                    combine_firstlast_fix_kernel<<<grid_for(1 << 20), 256, 0, stream>>>(combine_args(rows, 0, -1), (const unsigned long long*)xchg_slab, n_pes, xchg_cap_rows);
+                    B200_CUDA(cudaGetLastError());
                 }
-                launches++;
-                B200_CUDA(cudaGetLastError());
                 B200_CUDA(cudaStreamSynchronize(stream));
                 return finalize();
             }
         }
-        n_out = h_counters[2];
+        n_out = h_counters[CTR_OUT];
         finalized = true;
         out_cursor = 0;
         return n_out;
@@ -2737,12 +2717,7 @@ class GroupbyState {
         if (nk > 1) {
             XchgPackMkArgs p{};
             p.ow = mk_owner(true); p.tags = d_tags.as<unsigned long long>(); p.cap = cap;
-            int n = 0;
-            for (int j = 0; j < n_funcs; j++) {
-                p.acc[n++] = d_a0[j].as<unsigned long long>();
-                if (funcs[j].has_a1) p.acc[n++] = d_a1[j].as<unsigned long long>();
-            }
-            p.n_acc = n; p.row_words = nk + 1 + n; p.cursors = d_xchg_cursors.as<unsigned long long>(); p.peer_slabs = peer_slabs_dev; p.cap_rows = cap_rows;
+            p.n_acc = wire_accs(d_a0, d_a1, p.acc); p.row_words = nk + 1 + p.n_acc; p.cursors = d_xchg_cursors.as<unsigned long long>(); p.peer_slabs = peer_slabs_dev; p.cap_rows = cap_rows;
             xchg_pack_remote_mk_kernel<<<grid_for((int64_t)cap), 256, 0, stream>>>(p);
             xchg_post_counts_kernel<<<1, 32, 0, stream>>>(d_xchg_cursors.as<unsigned long long>(), peer_slabs_dev, n_pes, rank, cap_rows);
             launches += 2;
@@ -2751,12 +2726,7 @@ class GroupbyState {
         }
         XchgPackArgs p{};
         p.tkeys = d_keys.as<long long>(); p.cap = cap; p.counters = d_counters.as<long long>(); p.n_pes = n_pes; p.rank = rank;
-        int n = 0;
-        for (int j = 0; j < n_funcs; j++) {
-            p.acc[n++] = d_a0[j].as<unsigned long long>();
-            if (funcs[j].has_a1) p.acc[n++] = d_a1[j].as<unsigned long long>();
-        }
-        p.n_acc = n; p.row_words = 2 + n; p.cursors = d_xchg_cursors.as<unsigned long long>(); p.peer_slabs = peer_slabs_dev; p.cap_rows = cap_rows;
+        p.n_acc = wire_accs(d_a0, d_a1, p.acc); p.row_words = 2 + p.n_acc; p.cursors = d_xchg_cursors.as<unsigned long long>(); p.peer_slabs = peer_slabs_dev; p.cap_rows = cap_rows;
         xchg_pack_remote_kernel<<<grid_for((int64_t)cap + 2), 256, 0, stream>>>(p);
         xchg_post_counts_kernel<<<1, 32, 0, stream>>>(d_xchg_cursors.as<unsigned long long>(), peer_slabs_dev, n_pes, rank, cap_rows);
         launches += 2;
@@ -2787,7 +2757,7 @@ class GroupbyState {
         build_done = true;
         compact(/*owned_only=*/false);
         read_counters();
-        n_out = h_counters[2];
+        n_out = h_counters[CTR_OUT];
         d_dest_count.ensure((size_t)n_pes * 8);
         B200_CUDA(cudaMemsetAsync(d_dest_count.p, 0, (size_t)n_pes * 8, stream));
         PackArgs p = pack_args();
@@ -2803,12 +2773,7 @@ class GroupbyState {
     PackArgs pack_args() {
         PackArgs p{};
         p.tkeys = d_keys.as<long long>(); p.cap = cap; p.slot_of_out = d_slot_of_out.as<uint64_t>(); p.n_out = n_out; p.n_pes = n_pes;
-        int n = 0;
-        for (int j = 0; j < n_funcs; j++) {
-            p.acc[n++] = d_a0[j].as<unsigned long long>();
-            if (funcs[j].has_a1) p.acc[n++] = d_a1[j].as<unsigned long long>();
-        }
-        p.n_acc = n; p.row_words = 2 + n; p.dest_count = d_dest_count.as<long long>();
+        p.n_acc = wire_accs(d_a0, d_a1, p.acc); p.row_words = 2 + p.n_acc; p.dest_count = d_dest_count.as<long long>();
         return p;
     }
     void shuffle_pack(void* send_buf) {
@@ -2825,7 +2790,7 @@ class GroupbyState {
         B200_CUDA(cudaStreamSynchronize(stream));  // offs is a stack buffer
         fill(d_keys.p, cap + 2, (unsigned long long)EMPTY_KEY);
         for (int j = 0; j < n_funcs; j++) { fill(d_a0[j].p, cap + 2, funcs[j].init0); if (funcs[j].has_a1) fill(d_a1[j].p, cap + 2, funcs[j].init1); }
-        B200_CUDA(cudaMemsetAsync(d_counters.p, 0, 8 * sizeof(long long), stream));
+        B200_CUDA(cudaMemsetAsync(d_counters.p, 0, N_COUNTERS * sizeof(long long), stream));
         n_groups = 0; n_groups_bound = 0; untracked_groups = 0;
     }
     void shuffle_combine(const void* recv, int64_t n_rows) {
@@ -2835,19 +2800,16 @@ class GroupbyState {
         bool could_fail = (int64_t)(cap / 2) - n_groups_bound < n_rows;
         if (could_fail) d_fail.ensure(device, (size_t)n_rows * 4);
         auto launch = [&](const uint32_t* index_list, int64_t rows) {
-            CombineArgs c{};
-            c.in = (const unsigned long long*)recv; c.n_rows = rows; c.row_words = 2 + acc_count();
             // with room guaranteed the per-insert ticket (one atomic on a single counter per new group: ~170 us for 1 M
             // groups) is skipped; the groups are accounted for as `untracked_groups` until the next compaction counts them
-            c.tkeys = d_keys.as<long long>(); c.cap = cap; c.counters = d_counters.as<long long>(); c.group_limit = could_fail ? (long long)(cap / 2) : -1;
-            c.fail_list = d_fail.as<uint32_t>(); c.index_list = index_list; c.n_ops = n_funcs;
-            for (int j = 0; j < n_funcs; j++) { c.kinds[j] = funcs[j].kind; c.a0[j] = d_a0[j].p; c.a1[j] = funcs[j].has_a1 ? d_a1[j].p : nullptr; }
+            CombineArgs c = combine_args((const unsigned long long*)recv, rows, could_fail ? (long long)(cap / 2) : -1);
+            c.index_list = index_list;
             combine_partials_kernel<<<grid_for(rows), 256, 0, stream>>>(c);
             launches++;
             B200_CUDA(cudaGetLastError());
         };
         launch(nullptr, n_rows);
-        settle(n_rows, could_fail, launch);
+        if (could_fail) settle<uint32_t>(d_fail, 1, fail_rows, launch);
         if (has_firstlast) {
             CombineArgs c = combine_args((const unsigned long long*)recv, n_rows, -1);
             combine_firstlast_fix_kernel<<<grid_for(n_rows), 256, 0, stream>>>(c, nullptr, 0, 0);

@@ -72,7 +72,7 @@ __device__ __forceinline__ void gen_direct_apply(const SpgGenArgs& g, long long 
                                               unsigned long long nnull, long long mn, long long mx) {
     const SpgArgs& a = g.s;
     uint64_t sl;
-    if (key == EMPTY_KEY) { sl = a.cap + 1; a.counters[4] = 1; }
+    if (key == EMPTY_KEY) { sl = a.cap + 1; a.counters[CTR_MARKER] = 1; }
     else {
         sl = find_or_insert(a.tkeys, a.cap, key, a.counters, a.group_limit);
         if (sl == ~0ull) {  // global table at its limit: park the partial, the host grows the table and replays it
@@ -231,7 +231,7 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPG_TCTAS) spgg_partition_kernel
         __syncthreads();
     }
     if (tid == 0 && (na_cnt[0] | na_cnt[1])) {  // NA-key group (slot cap of the state's table)
-        a.counters[3] = 1;
+        a.counters[CTR_NA] = 1;
         gen_apply_slot(g.fl, a.cap, *na_sum, (unsigned long long)na_cnt[0], (unsigned long long)na_cnt[1], *na_min, *na_max);
     }
 }

@@ -7,7 +7,7 @@
 // and copies out half the bytes, and K2n's shared table shrinks to 12-byte slots (int32 key, low sum word, count) whose
 // two-slot buckets are ONE 8-byte shared load each, with 32-bit key compares.  Rows that do not fit (either value outside
 // int32, or the key INT32_MIN, which marks a free slot) take the direct global path inside K1n, so the result is exact for any
-// input; a.counters[5] counts them and the host drops back to the 16-byte kernels when they are not rare.
+// input; a.counters[CTR_WIDE] counts them and the host drops back to the 16-byte kernels when they are not rare.
 // Sums stay exact mod 2^64: the sign-extended value is added as (low word, high word + carry) exactly as in spg_aggregate_kernel.
 #pragma once
 
@@ -159,7 +159,7 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPGN_CTAS) spgn_partition_kernel
         if (tid == 0) *tile_over = 0;
         __syncthreads();
     }
-    if (wide) atomicAdd((unsigned long long*)&a.counters[5], (unsigned long long)wide);
+    if (wide) atomicAdd((unsigned long long*)&a.counters[CTR_WIDE], (unsigned long long)wide);
 }
 
 // K2n's two candidate buckets of a key (two slots each) among the NB buckets of the shared table
@@ -318,9 +318,9 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgn_aggregate_kernel(const __
             if ((tid & 31) == 0 && mine) atomicAdd(&fl_occ, mine);
             __syncthreads();
             if (tid == 0 && fl_occ) {
-                const long long t = (long long)atomicAdd((unsigned long long*)&a.counters[0], (unsigned long long)fl_occ);
+                const long long t = (long long)atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], (unsigned long long)fl_occ);
                 if (t + (long long)fl_occ <= a.group_limit) fl_reserved = 1;
-                else atomicAdd((unsigned long long*)&a.counters[0], (unsigned long long)(-(long long)fl_occ));  // no room: per-insert tickets
+                else atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], (unsigned long long)(-(long long)fl_occ));  // no room: per-insert tickets
             }
             __syncthreads();
         }
@@ -342,7 +342,7 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgn_aggregate_kernel(const __
             for (int d = 16; d; d >>= 1) dup += __shfl_xor_sync(0xffffffffu, dup, d);
             if ((tid & 31) == 0 && dup) atomicAdd(&fl_dup, dup);
             __syncthreads();
-            if (tid == 0 && fl_dup) atomicAdd((unsigned long long*)&a.counters[0], (unsigned long long)(-(long long)fl_dup));
+            if (tid == 0 && fl_dup) atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], (unsigned long long)(-(long long)fl_dup));
         }
         __syncthreads();
     }
