@@ -125,12 +125,39 @@ __host__ __device__ inline int64_t py_hash_double(double v) {
     return r == -1 ? -2 : r;
 }
 
+// Float groupby keys live in the int64 tables as this encoding of their double value (a float32 key is widened first,
+// exactly): the bit pattern, with -0.0 folded onto +0.0 (one group, as in pandas) and every NaN mapped to INT64_MIN.  INT64_MIN
+// is the pattern of -0.0, so no other key produces it, and it is the tables' marker key: NaN keys land in the marker slot,
+// one group without a validity bitmap.  Integer equality of two encodings is equality of the keys.
+__host__ __device__ __forceinline__ long long canon_float_key(double d) {
+    if (isnan(d)) return (long long)0x8000000000000000ULL;
+    if (d == 0.0) return 0;
+#ifdef __CUDA_ARCH__
+    return __double_as_longlong(d);
+#else
+    long long b; memcpy(&b, &d, 8); return b;
+#endif
+}
+__host__ __device__ __forceinline__ double canon_float_decode(long long k) {
+    if (k == (long long)0x8000000000000000ULL) return NAN;
+#ifdef __CUDA_ARCH__
+    return __longlong_as_double(k);
+#else
+    double d; memcpy(&d, &k, 8); return d;
+#endif
+}
+
 // hash_to_rank (reference: bodo/libs/_shuffle.h:5-7): (uint32) hash % n_pes.
 __host__ __device__ __forceinline__ int hash_to_rank_u32(uint32_t h, int n_pes) { return (int)(h % (uint32_t)n_pes); }
 
 // Table-slot hash: the same xxh3 value (one hash per row); ranks use the low 32 bits, slots the high 32
 // bits, so the two are independent (a rank's keys all share low32 % P).
 __device__ __forceinline__ uint64_t key_hash(int64_t key) { return xxh3_64_short((uint64_t)key, 8, SEED_HASH_PARTITION); }
+// Owner-rank hash of a valid table key: the hash shuffle_table gives its rows (hash_key_column).  A float key's encoding
+// (canon_float_key) goes through _Py_HashDouble of its value first; NaN hashes as 0, as a NaN row does there.
+__device__ __forceinline__ uint32_t owner_key_hash(int64_t key, bool is_float) {
+    return (uint32_t)(is_float ? xxh3_64_short((uint64_t)py_hash_double(canon_float_decode(key)), 8, SEED_HASH_PARTITION) : key_hash(key));
+}
 
 __device__ __forceinline__ int64_t load_int_as_i64(const void* __restrict__ p, int ct, int64_t i) {
     switch (ct) {

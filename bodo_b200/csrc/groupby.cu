@@ -3,8 +3,8 @@
 // Replaces GroupbyState + groupby_agg_build_consume_batch + FinalizeBuild of the reference
 // (bodo/libs/streaming/_groupby.cpp:2554-3031, 4325-4457, 4062-4256) and the aggregate kernels of
 // bodo/libs/groupby/_groupby_agg_funcs.h.  Design (see DESIGN.md):
-//   * one persistent open-addressing table per state (linear probing, load <= 0.5, int64 keys,
-//     SoA accumulator columns), instead of the reference's per-batch update table + combine;
+//   * one persistent open-addressing table per state (linear probing, load <= 0.5, int64 keys — float keys as
+//     canon_float_key, see canon_keys — SoA accumulator columns), instead of the reference's per-batch update table + combine;
 //   * the consume kernel fuses hash + find-or-insert + every aggregate update of a row;
 //   * rows whose insert would overfill the table are appended to a fail list; the host grows/rehashes
 //     the table and replays only those rows (the reference's transactional retry,
@@ -307,6 +307,30 @@ __global__ void __launch_bounds__(256) groupby_consume_i64_sumcount_kernel(
     }
 }
 
+// Float key column -> its int64 table keys (canon_float_key), before any consume kernel reads the chunk.  A pure stream:
+// 8 (float64) or 4 (float32) bytes read and 8 written per row, four rows per thread through 16-byte loads and stores when
+// both columns are 16-byte aligned; the rest (or everything, when they are not) goes row by row.
+template <typename F>
+__global__ void __launch_bounds__(256) canon_float_key_kernel(const F* __restrict__ in, long long* __restrict__ out, int64_t n) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    const int64_t t0 = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const int64_t n4 = (((uintptr_t)in | (uintptr_t)out) & 15) == 0 ? n / 4 : 0;
+    for (int64_t q = t0; q < n4; q += stride) {
+        double v[4];
+        if constexpr (sizeof(F) == 8) {
+            const double2 a = __ldcs(reinterpret_cast<const double2*>(in) + 2 * q), b = __ldcs(reinterpret_cast<const double2*>(in) + 2 * q + 1);
+            v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
+        } else {
+            const float4 a = __ldcs(reinterpret_cast<const float4*>(in) + q);
+            v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w;
+        }
+        longlong2* o = reinterpret_cast<longlong2*>(out) + 2 * q;
+        o[0] = make_longlong2(canon_float_key(v[0]), canon_float_key(v[1]));
+        o[1] = make_longlong2(canon_float_key(v[2]), canon_float_key(v[3]));
+    }
+    for (int64_t i = 4 * n4 + t0; i < n; i += stride) out[i] = canon_float_key((double)in[i]);
+}
+
 __global__ void fill_u64_kernel(unsigned long long* p, uint64_t n, unsigned long long v) {
     uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += stride) p[i] = v;
@@ -340,10 +364,11 @@ __global__ void rehash_kernel(const __grid_constant__ RehashArgs a) {
 // ---- finalize: compact occupied slots, then evaluate output columns ----
 // n_pes > 1: only the groups this rank OWNS (hash_to_rank(key) == rank) are output — after the fused exchange the table still
 // holds the partial aggregates of groups that were sent to their owners (they are never touched again: received rows only
-// carry keys this rank owns)
+// carry keys this rank owns).  key_float: the key is a float column (canon_float_key), so the marker group is the NaN group
+// and dropna drops it.
 __global__ void compact_slots_kernel(const long long* __restrict__ tkeys, uint64_t cap, const long long* counters,
-                                     long long* cursor, uint64_t* slot_of_out, int n_pes, int rank) {
-    const bool na_present = counters[CTR_NA] != 0, empty_present = counters[CTR_MARKER] != 0;
+                                     long long* cursor, uint64_t* slot_of_out, int n_pes, int rank, bool key_float, bool dropna) {
+    const bool na_present = counters[CTR_NA] != 0, empty_present = counters[CTR_MARKER] != 0 && !(key_float && dropna);
     const uint32_t na_hash = (uint32_t)xxh3_64_short(1ull, 8, SEED_HASH_PARTITION);  // hash_na_val (_array_hash.cpp:22-29)
     uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
     for (uint64_t s0 = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s0 < ((cap + 2 + 31) & ~31ull); s0 += stride) {
@@ -352,7 +377,7 @@ __global__ void compact_slots_kernel(const long long* __restrict__ tkeys, uint64
         else if (s0 == cap) occ = na_present;
         else if (s0 == cap + 1) occ = empty_present;
         if (occ && n_pes > 1) {
-            const uint32_t h = s0 == cap ? na_hash : (uint32_t)key_hash(s0 < cap ? tkeys[s0] : EMPTY_KEY);
+            const uint32_t h = s0 == cap ? na_hash : owner_key_hash(s0 < cap ? tkeys[s0] : EMPTY_KEY, key_float);
             occ = hash_to_rank_u32(h, n_pes) == rank;
         }
         unsigned m = __ballot_sync(0xffffffffu, occ);
@@ -411,7 +436,8 @@ __global__ void eval_output_kernel(const __grid_constant__ EvalArgs a) {
         if (in && a.tkeys) {  // single-key tables only (multi-key tables write their key columns in eval_mk_keys_kernel)
             long long key = s < a.cap ? a.tkeys[s] : (s == a.cap ? 0 : EMPTY_KEY);
             key_ok = s != a.cap;
-            store_int_typed(a.out_keys, a.key_ctype, p, key);
+            if (ctype_is_float(a.key_ctype)) store_f_typed(a.out_keys, a.key_ctype, p, canon_float_decode(key));
+            else store_int_typed(a.out_keys, a.key_ctype, p, key);
         }
         if (a.out_key_valid) {
             unsigned m = __ballot_sync(0xffffffffu, in && key_ok);
@@ -512,6 +538,7 @@ struct PackArgs {
     unsigned long long* out; // packed rows
     int row_words;
     int pass;                // 0 = histogram, 1 = scatter
+    bool key_float;          // owner_key_hash of a float key
 };
 __global__ void pack_partials_kernel(const __grid_constant__ PackArgs a) {
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -523,7 +550,7 @@ __global__ void pack_partials_kernel(const __grid_constant__ PackArgs a) {
         uint64_t s = in ? a.slot_of_out[p] : 0;
         long long key = s < a.cap ? a.tkeys[s] : (s == a.cap ? 0 : EMPTY_KEY);
         bool kvalid = s != a.cap;
-        uint32_t h = kvalid ? (uint32_t)key_hash(key) : na_hash;
+        uint32_t h = kvalid ? owner_key_hash(key, a.key_float) : na_hash;
         int d = in ? hash_to_rank_u32(h, a.n_pes) : -1;
         // warp-aggregated cursor: one atomic per (warp, destination) instead of one per row
         unsigned peers = __match_any_sync(0xffffffffu, d);
@@ -657,6 +684,7 @@ struct XchgPackArgs {
     unsigned long long* cursors;      // [n_pes] rows packed per destination (device)
     void* const* peer_slabs;          // [n_pes] device pointers to every rank's slab (own slab included)
     long long cap_rows;
+    bool key_float;                   // owner_key_hash of a float key
 };
 __global__ void xchg_pack_remote_kernel(const __grid_constant__ XchgPackArgs a) {
     const bool na_present = a.counters[CTR_NA] != 0, empty_present = a.counters[CTR_MARKER] != 0;
@@ -670,7 +698,7 @@ __global__ void xchg_pack_remote_kernel(const __grid_constant__ XchgPackArgs a) 
         else if (s == a.cap + 1) occ = empty_present;
         const long long key = s < a.cap ? (occ ? a.tkeys[s] : 0) : (s == a.cap ? 0 : EMPTY_KEY);
         const bool kvalid = s != a.cap;
-        const uint32_t h = kvalid ? (uint32_t)key_hash(key) : na_hash;
+        const uint32_t h = kvalid ? owner_key_hash(key, a.key_float) : na_hash;
         int d = occ ? hash_to_rank_u32(h, a.n_pes) : -1;
         if (d == a.rank) d = -1;  // owned here: stays in the table
         // warp-aggregated cursor: one atomic per (warp, destination)
@@ -709,7 +737,7 @@ __global__ void xchg_combine_slab_kernel(const __grid_constant__ CombineArgs a, 
     }
 }
 
-// ---- multi-column keys (2..4 integer key columns; SURVEY.md §8f "next" row 1, the reference's select-distinct /
+// ---- multi-column keys (2..4 integer / float key columns; SURVEY.md §8f "next" row 1, the reference's select-distinct /
 // multi-key groupby: bodo/tests/test_streaming/test_groupby.py:111-177) -----------------------------------------
 // A slot is claimed through a 64-bit tag word (hash of the key tuple, bit 63 set; 0 = empty, 1 = being written): the
 // claiming thread CASes empty -> locked, writes the key columns + NA mask of the slot, fences and publishes the tag.
@@ -825,21 +853,23 @@ __global__ void rehash_mk_kernel(const __grid_constant__ RehashMkArgs a) {
     }
 }
 // Ownership of a multi-column key: hash_keys of the tuple exactly as the reference computes it on the original columns
-// (sizeof(T) raw bytes per integer column, NA -> hash_na_val, hash_combine_boost for the further columns), from the
-// widened int64 values the table stores.
+// (sizeof(T) raw bytes per integer column, _Py_HashDouble per float column, NA -> hash_na_val, hash_combine_boost for the
+// further columns), from the widened int64 values (float columns: canon_float_key) the table stores.
 struct MkOwner {
     int nk, n_pes, rank;
     int own_nk;  // 0: ownership by the hash of all key columns (the reference's hash_keys); 1: by the FIRST key column alone, hashed
                  // like a single-key state's key (nunique's nested (key, value) state: a key's pairs live where the key lives)
     const long long* mk[MAX_KEYS];
     const unsigned char* mkmask;
-    int key_ctype[MAX_KEYS];
+    int key_ctype[MAX_KEYS];  // the input column types
+    unsigned int drop_nan;    // compact_mk_kernel: bit j = drop groups whose float key column j is NaN (dropna)
 };
 __device__ __forceinline__ uint32_t mk_ref_hash(const long long* keys, unsigned int mask, int nk, const int* ctypes) {
     const uint32_t na_hash = (uint32_t)xxh3_64_short(1ull, 8, SEED_HASH_PARTITION);
     uint32_t h = 0;
     for (int j = 0; j < nk; j++) {
         const uint32_t hj = !((mask >> j) & 1u) ? na_hash
+                           : ctype_is_float(ctypes[j]) ? owner_key_hash(keys[j], true)
                            : ctype_size(ctypes[j]) == 8 ? (uint32_t)xxh3_64_short((uint64_t)keys[j], 8, SEED_HASH_PARTITION)
                                                         : (uint32_t)xxh3_64_short((uint64_t)(uint32_t)keys[j], 4, SEED_HASH_PARTITION);
         h = j == 0 ? hj : hash_combine_boost(h, hj);
@@ -847,20 +877,23 @@ __device__ __forceinline__ uint32_t mk_ref_hash(const long long* keys, unsigned 
     return h;
 }
 __device__ __forceinline__ uint32_t mk_owner_hash(const MkOwner& ow, const long long* keys, unsigned int mask) {
-    if (ow.own_nk == 1) return (mask & 1u) ? (uint32_t)key_hash(keys[0]) : (uint32_t)xxh3_64_short(1ull, 8, SEED_HASH_PARTITION);
+    if (ow.own_nk == 1) return (mask & 1u) ? owner_key_hash(keys[0], ctype_is_float(ow.key_ctype[0])) : (uint32_t)xxh3_64_short(1ull, 8, SEED_HASH_PARTITION);
     return mk_ref_hash(keys, mask, ow.nk, ow.key_ctype);
 }
-// nunique: one thread per distinct (key, value) pair of the nested state; pairs whose value is NA do not count
+// nunique: one thread per distinct (key, value) pair of the nested state; pairs whose value is NA do not count, nor (float
+// value column: canon_float_key) do pairs whose value is NaN, the marker key
 struct NuniqueArgs {
     const long long* pk; const long long* pv; const unsigned char* pmask; const uint64_t* slot_of_out; long long n_pairs;
     long long* tkeys; uint64_t cap; long long* counters; int dropna;
     int n_acc; unsigned long long* acc[MAX_OPS];
+    int value_float;
 };
 __global__ void nunique_count_kernel(const __grid_constant__ NuniqueArgs a) {
     for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < a.n_pairs; p += (long long)gridDim.x * blockDim.x) {
         const uint64_t s = a.slot_of_out[p];
         const unsigned int m = a.pmask[s];
         if (!(m & 2u)) continue;  // NA value
+        if (a.value_float && a.pv[s] == EMPTY_KEY) continue;  // NaN value
         uint64_t slot;
         if (!(m & 1u)) { if (a.dropna) continue; slot = a.cap; a.counters[CTR_NA] = 1; }
         else {
@@ -876,6 +909,11 @@ __global__ void compact_mk_kernel(const unsigned long long* __restrict__ tags, u
     uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
     for (uint64_t s0 = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s0 < ((cap + 31) & ~31ull); s0 += stride) {
         bool occ = s0 < cap && (tags[s0] >> 63);
+        if (occ && ow.drop_nan) {  // dropna: a NaN in a float key column is NA (it is not in the mask: the table holds the marker)
+            const unsigned int mask = ow.mkmask[s0];
+            for (int j = 0; j < ow.nk; j++)
+                if (((ow.drop_nan & mask) >> j) & 1u) occ = occ && ow.mk[j][s0] != EMPTY_KEY;
+        }
         if (occ && ow.n_pes > 1) {  // only the groups this rank owns (see compact_slots_kernel)
             long long keys[MAX_KEYS];
             for (int j = 0; j < ow.nk; j++) keys[j] = ow.mk[j][s0];
@@ -981,7 +1019,10 @@ __global__ void eval_mk_keys_kernel(const __grid_constant__ EvalMkKeysArgs a) {
         uint64_t s = in ? a.slot_of_out[p] : 0;
         unsigned int mask = in ? a.mkmask[s] : 0;
         for (int j = 0; j < a.nk; j++) {
-            if (in) store_int_typed(a.out_keys[j], a.key_ctype[j], p, a.mk[j][s]);
+            if (in) {
+                if (ctype_is_float(a.key_ctype[j])) store_f_typed(a.out_keys[j], a.key_ctype[j], p, canon_float_decode(a.mk[j][s]));
+                else store_int_typed(a.out_keys[j], a.key_ctype[j], p, a.mk[j][s]);
+            }
             if (a.out_key_valid[j]) {
                 unsigned m = __ballot_sync(0xffffffffu, in && ((mask >> j) & 1));
                 if ((threadIdx.x & 31) == 0) a.out_key_valid[j][p >> 5] = m;
@@ -1633,7 +1674,10 @@ class GroupbyState {
     cudaStream_t stream;
     cudaStream_t copy_stream = nullptr;
     int n_cols;
-    std::vector<int8_t> c_types, arr_types;
+    // Two types per column.  in_types: the caller's (batch validation, output typing, owner hashing).  c_types: what the table
+    // and every consume path read — a float key column is consumed as its canonical int64 column (canon_keys), so it is CT_INT64
+    // here; every other column has its input type.
+    std::vector<int8_t> in_types, c_types, arr_types;
     int n_funcs;                  // primitive accumulator functions (what the kernels, the table and the exchange see)
     std::vector<FuncSpec> funcs;
     int n_outs = 0;               // aggregates the caller asked for (output columns)
@@ -1716,13 +1760,14 @@ class GroupbyState {
         nk = (int)n_keys;
         B200_REQUIRE(n_arrs >= 1, "b200 groupby: empty build schema");
         B200_REQUIRE(n_funcs_ <= 2 * MAX_OPS, "b200 groupby: too many aggregate functions");
-        c_types.assign(ct, ct + n_arrs);
+        in_types.assign(ct, ct + n_arrs);
+        c_types = in_types;
         arr_types.assign(at, at + n_arrs);
         B200_REQUIRE(n_arrs >= nk, "b200 groupby: fewer columns than keys");
         for (int kc = 0; kc < nk; kc++) {
-            int kct = c_types[kc];
-            B200_REQUIRE(ctype_size(kct) > 0 && !ctype_is_float(kct), "b200 groupby: key columns must be integer/date typed");
+            B200_REQUIRE(ctype_size(in_types[kc]) > 0, "b200 groupby: key columns must be integer, date or float typed");
             B200_REQUIRE(arr_types[kc] == ARR_NUMPY || arr_types[kc] == ARR_NULLABLE, "b200 groupby: unsupported key array type");
+            if (ctype_is_float(in_types[kc])) c_types[kc] = CT_INT64;
         }
         if (!parallel) { n_pes = 1; rank = 0; }
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
@@ -1764,7 +1809,6 @@ class GroupbyState {
                 case FT_NUNIQUE: {
                     // nunique_computation (bodo/libs/groupby/_groupby_col_set.cpp:1771-1810): distinct non-NA values per group
                     B200_REQUIRE(nk == 1, "b200 groupby: nunique is supported for single-column keys");
-                    B200_REQUIRE(!isf, "b200 groupby: nunique of a float column is not supported (integer / date / bool value columns)");
                     f.kind = K_NUNIQUE; f.out_ctype = CT_INT64; f.out_arrtype = ARR_NUMPY;
                     size_t q = 0;
                     while (q < nu_inner.size() && nu_inner[q].in_col != f.in_col) q++;
@@ -1825,7 +1869,7 @@ class GroupbyState {
         if (nk > 1) alloc_mk(want, d_tags, d_mk, d_mkmask);
         cap = want;
         for (auto& ni : nu_inner) {  // nested distinct states over (key, value); their groups are owned where the KEY is owned
-            const int8_t ict[2] = {c_types[0], c_types[ni.in_col]}, iat[2] = {arr_types[0], arr_types[ni.in_col]};
+            const int8_t ict[2] = {in_types[0], in_types[ni.in_col]}, iat[2] = {arr_types[0], arr_types[ni.in_col]};
             const int32_t no_off[1] = {0};
             ni.st.reset(new GroupbyState(ict, iat, 2, nullptr, no_off, nullptr, 0, 2, 1ll << 40, parallel, /*dropna=*/false, device, n_pes, rank,
                                          expected_groups > 0 ? expected_groups * 4 : 0, stream));
@@ -2438,6 +2482,27 @@ class GroupbyState {
     int64_t untracked_groups = 0;  // upper bound of groups inserted without ticket counting (combine with guaranteed room)
     bool stage_recorded[2] = {false, false};
 
+    // ---- float keys: canonicalisation pre-pass ----
+    bool float_key(int kc) const { return ctype_is_float(in_types[kc]); }
+    DevBuf d_canon[MAX_KEYS];  // canonical int64 column of each float key column (pooled: 16-byte aligned, as SPG needs)
+    void canon_launch(const void* in, int ct, long long* out, int64_t n) {
+        if (n == 0) return;
+        const int g = grid_for((n + 3) / 4);
+        if (ct == CT_FLOAT64) canon_float_key_kernel<double><<<g, 256, 0, stream>>>((const double*)in, out, n);
+        else canon_float_key_kernel<float><<<g, 256, 0, stream>>>((const float*)in, out, n);
+        launches++;
+        B200_CUDA(cudaGetLastError());
+    }
+    // points the float key columns of a device-resident chunk at their canonical int64 columns
+    void canon_keys(std::vector<const void*>& data, int64_t n) {
+        for (int kc = 0; kc < nk; kc++) {
+            if (!float_key(kc)) continue;
+            d_canon[kc].ensure((size_t)n * 8);
+            canon_launch(data[kc], in_types[kc], d_canon[kc].as<long long>(), n);
+            data[kc] = d_canon[kc].p;
+        }
+    }
+
     void consume(const b200_table* t) {
         B200_REQUIRE(!build_done, "b200 groupby: consume after the build was finished");
         B200_REQUIRE(t->n_cols == n_cols, "b200 groupby: batch has a different number of columns than the build schema");
@@ -2448,7 +2513,7 @@ class GroupbyState {
         for (auto& f : funcs) if (f.in_col >= 0) used[f.in_col] = true;
         for (int c = 0; c < n_cols; c++) {
             if (!used[c]) continue;
-            B200_REQUIRE(t->cols[c].c_type == c_types[c], "b200 groupby: batch column dtype differs from the build schema");
+            B200_REQUIRE(t->cols[c].c_type == in_types[c], "b200 groupby: batch column dtype differs from the build schema");
             B200_REQUIRE(n == 0 || t->cols[c].data != nullptr, "b200 groupby: null data pointer");
         }
         for (auto& ni : nu_inner) {  // nunique: the (key, value) pairs of this batch go to the nested distinct state
@@ -2469,9 +2534,10 @@ class GroupbyState {
                 std::vector<const uint8_t*> valid(n_cols, nullptr);
                 for (int c = 0; c < n_cols; c++) {
                     if (!used[c]) continue;
-                    data[c] = (const char*)t->cols[c].data + r0 * ctype_size(c_types[c]);
+                    data[c] = (const char*)t->cols[c].data + r0 * ctype_size(in_types[c]);
                     valid[c] = t->cols[c].validity ? t->cols[c].validity + r0 / 8 : nullptr;
                 }
+                canon_keys(data, rows);
                 consume_device_chunk(data, valid, rows);
             }
             return;
@@ -2497,7 +2563,7 @@ class GroupbyState {
             std::vector<const uint8_t*> valid(n_cols, nullptr);
             for (int c = 0; c < n_cols; c++) {
                 if (!used[c]) continue;
-                size_t isz = ctype_size(c_types[c]);
+                size_t isz = ctype_size(in_types[c]);
                 stage[b][2 * c].ensure((size_t)std::min(HCHUNK, n) * isz);
                 B200_CUDA(cudaMemcpyAsync(stage[b][2 * c].p, (const char*)t->cols[c].data + r0 * isz, rows * isz, cudaMemcpyHostToDevice, copy_stream));
                 data[c] = stage[b][2 * c].p;
@@ -2509,6 +2575,7 @@ class GroupbyState {
             }
             B200_CUDA(cudaEventRecord(stage_ready[b], copy_stream));
             B200_CUDA(cudaStreamWaitEvent(stream, stage_ready[b], 0));
+            canon_keys(data, rows);
             consume_device_chunk(data, valid, rows);
             B200_CUDA(cudaEventRecord(stage_free[b], stream));
             stage_recorded[b] = true;
@@ -2517,8 +2584,8 @@ class GroupbyState {
 
     // ---- coalescing of small streaming batches ----
     // The reference streams 32 768-row batches (bodo/libs/streaming/_shuffle.h:27-31); the SM-partitioned and low-cardinality
-    // kernels want >= 2^20 rows per launch.  Batches of the fast-path signature (non-null int64 key, SUM / COUNT / SIZE over one
-    // non-null int64 value column) below that size are appended to a device-side buffer (one D2D or H2D copy per column) and
+    // kernels want >= 2^20 rows per launch.  Batches of the fast-path signature (non-null int64 or float key, SUM / COUNT / SIZE over
+    // one non-null int64 value column) below that size are appended to a device-side buffer (one D2D or H2D copy per column) and
     // consumed together when the buffer is full, when a batch of another shape arrives, or when the build ends.
     static constexpr int64_t CO_MIN_BATCH = 1ll << 20, CO_ROWS = 1ll << 22;
     DevBuf co_key, co_val;
@@ -2541,7 +2608,17 @@ class GroupbyState {
         if (vcol >= 0) co_val.ensure((size_t)CO_ROWS * 8);
         const cudaMemcpyKind kind = t->device >= 0 ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
         if (t->device >= 0) B200_REQUIRE(t->device == device, "b200 groupby: batch lives on a different device than the state");
-        B200_CUDA(cudaMemcpyAsync(co_key.as<long long>() + co_n, t->cols[0].data, (size_t)n * 8, kind, stream));
+        if (float_key(0)) {  // the buffer holds canonical keys (a host batch is copied over first)
+            const void* k = t->cols[0].data;
+            if (kind == cudaMemcpyHostToDevice) {
+                const size_t kb = (size_t)n * ctype_size(in_types[0]);
+                d_canon[0].ensure(kb);
+                B200_CUDA(cudaMemcpyAsync(d_canon[0].p, k, kb, kind, stream));
+                k = d_canon[0].p;
+            }
+            canon_launch(k, in_types[0], co_key.as<long long>() + co_n, n);
+        } else
+            B200_CUDA(cudaMemcpyAsync(co_key.as<long long>() + co_n, t->cols[0].data, (size_t)n * 8, kind, stream));
         if (vcol >= 0) B200_CUDA(cudaMemcpyAsync(co_val.as<long long>() + co_n, t->cols[vcol].data, (size_t)n * 8, kind, stream));
         if (kind == cudaMemcpyHostToDevice) B200_CUDA(cudaStreamSynchronize(stream));  // the caller may reuse its host batch right away
         co_n += n;
@@ -2574,7 +2651,7 @@ class GroupbyState {
         else
             compact_slots_kernel<<<grid_for((int64_t)cap + 2), 256, 0, stream>>>(d_keys.as<long long>(), cap, d_counters.as<long long>(),
                                                                                       d_counters.as<long long>() + CTR_OUT, d_slot_of_out.as<uint64_t>(),
-                                                                                      owned_only ? n_pes : 1, rank);
+                                                                                      owned_only ? n_pes : 1, rank, float_key(0), dropna);
         launches++;
         B200_CUDA(cudaGetLastError());
         n_out = -1;  // known on the device (counters[CTR_OUT]); the host learns it with the next counter read-back
@@ -2598,6 +2675,7 @@ class GroupbyState {
             a.tkeys = d_keys.as<long long>(); a.cap = cap; a.counters = d_counters.as<long long>(); a.dropna = dropna ? 1 : 0;
             a.n_acc = (int)ni.prims.size();
             for (int j = 0; j < a.n_acc; j++) a.acc[j] = d_a0[ni.prims[j]].as<unsigned long long>();
+            a.value_float = in.float_key(1) ? 1 : 0;
             nunique_count_kernel<<<grid_for(n_pairs), 256, 0, stream>>>(a);
             launches++;
             B200_CUDA(cudaGetLastError());
@@ -2615,10 +2693,10 @@ class GroupbyState {
         const int64_t max_out = max_out_bound();
         EvalArgs e{};
         e.tkeys = nk == 1 ? d_keys.as<long long>() : nullptr; e.cap = cap; e.slot_of_out = d_slot_of_out.as<uint64_t>(); e.n_out_ptr = d_counters.as<long long>() + CTR_OUT;
-        e.key_ctype = c_types[0];
+        e.key_ctype = in_types[0];
         size_t words = (size_t)((max_out + 31) / 32 + 1);
         if (nk == 1) {
-            d_out_keys.ensure((size_t)(max_out + 32) * ctype_size(c_types[0]));
+            d_out_keys.ensure((size_t)(max_out + 32) * ctype_size(in_types[0]));
             e.out_keys = d_out_keys.p;
             bool key_nullable = arr_types[0] == ARR_NULLABLE;
             if (key_nullable) { d_out_key_valid.ensure(words * 4); e.out_key_valid = d_out_key_valid.as<uint32_t>(); }
@@ -2626,8 +2704,8 @@ class GroupbyState {
             EvalMkKeysArgs k{};
             k.nk = nk; k.mkmask = d_mkmask.as<unsigned char>(); k.slot_of_out = d_slot_of_out.as<uint64_t>(); k.n_out_ptr = d_counters.as<long long>() + CTR_OUT;
             for (int j = 0; j < nk; j++) {
-                k.mk[j] = d_mk[j].as<long long>(); k.key_ctype[j] = c_types[j];
-                d_out_mk[j].ensure((size_t)(max_out + 32) * ctype_size(c_types[j]));
+                k.mk[j] = d_mk[j].as<long long>(); k.key_ctype[j] = in_types[j];
+                d_out_mk[j].ensure((size_t)(max_out + 32) * ctype_size(in_types[j]));
                 k.out_keys[j] = d_out_mk[j].p;
                 if (arr_types[j] == ARR_NULLABLE) { d_out_mk_valid[j].ensure(words * 4); k.out_key_valid[j] = d_out_mk_valid[j].as<uint32_t>(); }
             }
@@ -2684,7 +2762,10 @@ class GroupbyState {
     MkOwner mk_owner(bool owned_only) {
         MkOwner o{};
         o.nk = nk; o.n_pes = owned_only ? n_pes : 1; o.rank = rank; o.mkmask = d_mkmask.as<unsigned char>(); o.own_nk = owner_nk;
-        for (int j = 0; j < nk; j++) { o.mk[j] = d_mk[j].as<long long>(); o.key_ctype[j] = c_types[j]; }
+        for (int j = 0; j < nk; j++) {
+            o.mk[j] = d_mk[j].as<long long>(); o.key_ctype[j] = in_types[j];
+            if (dropna && float_key(j)) o.drop_nan |= 1u << j;
+        }
         return o;
     }
     MkArgs mk_table_args() {
@@ -2727,6 +2808,7 @@ class GroupbyState {
         XchgPackArgs p{};
         p.tkeys = d_keys.as<long long>(); p.cap = cap; p.counters = d_counters.as<long long>(); p.n_pes = n_pes; p.rank = rank;
         p.n_acc = wire_accs(d_a0, d_a1, p.acc); p.row_words = 2 + p.n_acc; p.cursors = d_xchg_cursors.as<unsigned long long>(); p.peer_slabs = peer_slabs_dev; p.cap_rows = cap_rows;
+        p.key_float = float_key(0);
         xchg_pack_remote_kernel<<<grid_for((int64_t)cap + 2), 256, 0, stream>>>(p);
         xchg_post_counts_kernel<<<1, 32, 0, stream>>>(d_xchg_cursors.as<unsigned long long>(), peer_slabs_dev, n_pes, rank, cap_rows);
         launches += 2;
@@ -2774,6 +2856,7 @@ class GroupbyState {
         PackArgs p{};
         p.tkeys = d_keys.as<long long>(); p.cap = cap; p.slot_of_out = d_slot_of_out.as<uint64_t>(); p.n_out = n_out; p.n_pes = n_pes;
         p.n_acc = wire_accs(d_a0, d_a1, p.acc); p.row_words = 2 + p.n_acc; p.dest_count = d_dest_count.as<long long>();
+        p.key_float = float_key(0);
         return p;
     }
     void shuffle_pack(void* send_buf) {
@@ -2832,9 +2915,9 @@ class GroupbyState {
             b200_column& k = out->cols[kc];
             const DevBuf& kd = nk == 1 ? d_out_keys : d_out_mk[kc];
             const DevBuf& kv = nk == 1 ? d_out_key_valid : d_out_mk_valid[kc];
-            k.data = (char*)kd.p + off * ctype_size(c_types[kc]);
+            k.data = (char*)kd.p + off * ctype_size(in_types[kc]);
             k.validity = arr_types[kc] == ARR_NULLABLE ? kv.as<uint8_t>() + off / 8 : nullptr;
-            k.length = rows; k.c_type = c_types[kc]; k.arr_type = arr_types[kc];
+            k.length = rows; k.c_type = in_types[kc]; k.arr_type = arr_types[kc];
         }
         for (int j = 0; j < n_outs; j++) {
             b200_column& c = out->cols[nk + j];
