@@ -248,6 +248,12 @@ void scratch_trim(int device, size_t keep_bytes);
 void* pinned_acquire(size_t bytes);   // small pinned host blocks (counter mirrors), pooled for the same reason
 void pinned_release(void* p, size_t bytes);
 
+// Kernels every operator uses, launched with `grid` CTAs of 256 threads on `st` (misc.cu).
+// words[i / 32] bit (i % 32) = bytes[i] != 0 for i < n; the last word's bits past n are 0.
+void launch_pack_bitmap(const uint8_t* bytes, int64_t n, uint32_t* words, int grid, cudaStream_t st);
+// n 64-bit words at p set to v
+void launch_fill_u64(void* p, uint64_t n, unsigned long long v, int grid, cudaStream_t st);
+
 // RAII device buffer drawn from the pool of the CURRENT device (states call cudaSetDevice first).
 struct DevBuf {
     void* p = nullptr;

@@ -182,15 +182,6 @@ __global__ void __launch_bounds__(FP_THREADS) filter_project_kernel(const __grid
     }
 }
 
-__global__ void fp_pack_bitmap_kernel(const uint8_t* bytes, int64_t n, uint32_t* words) {
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    int64_t n_round = (n + 31) & ~31ll;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n_round; i += stride) {
-        unsigned m = __ballot_sync(0xffffffffu, i < n && bytes[i]);
-        if ((threadIdx.x & 31) == 0) words[i >> 5] = m;
-    }
-}
-
 __global__ void remap_i32_kernel(const int32_t* in, const uint8_t* valid, int64_t n, const int32_t* map, int32_t map_len, int32_t* out) {
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
@@ -260,7 +251,7 @@ int64_t b200_filter_project(const b200_table* in_table, const void* program, int
             n_keep = (int64_t)*h;
             pinned_release(h, 8);
             for (int j = 0; j < n_out; j++)
-                if (a.out_valid_bytes[j] && n_keep > 0) fp_pack_bitmap_kernel<<<sms * 4, 256, 0, st>>>(a.out_valid_bytes[j], n_keep, (uint32_t*)out->cols[j].validity);
+                if (a.out_valid_bytes[j] && n_keep > 0) launch_pack_bitmap(a.out_valid_bytes[j], n_keep, (uint32_t*)out->cols[j].validity, sms * 4, st);
             B200_CUDA(cudaGetLastError());
             B200_CUDA(cudaStreamSynchronize(st));
         }

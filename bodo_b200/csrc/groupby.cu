@@ -331,11 +331,6 @@ __global__ void __launch_bounds__(256) canon_float_key_kernel(const F* __restric
     for (int64_t i = 4 * n4 + t0; i < n; i += stride) out[i] = canon_float_key((double)in[i]);
 }
 
-__global__ void fill_u64_kernel(unsigned long long* p, uint64_t n, unsigned long long v) {
-    uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += stride) p[i] = v;
-}
-
 struct RehashArgs {
     const long long* old_keys;
     uint64_t old_cap;
@@ -1901,7 +1896,7 @@ class GroupbyState {
 
     void fill(void* p, uint64_t n, unsigned long long v) {
         if (v == 0) { B200_CUDA(cudaMemsetAsync(p, 0, n * 8, stream)); return; }
-        fill_u64_kernel<<<grid_for((int64_t)n), 256, 0, stream>>>((unsigned long long*)p, n, v);
+        launch_fill_u64(p, n, v, grid_for((int64_t)n), stream);
         launches++;
     }
 

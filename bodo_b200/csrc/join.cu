@@ -284,18 +284,6 @@ __global__ void expand_bitmap_kernel(const uint8_t* bitmap, int64_t n, uint8_t* 
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) bytes[i] = bit_valid(bitmap, i) ? 1 : 0;
 }
-__global__ void pack_bitmap_kernel(const uint8_t* bytes, int64_t n, uint32_t* words) {
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    int64_t n_round = (n + 31) & ~31ll;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n_round; i += stride) {
-        unsigned m = __ballot_sync(0xffffffffu, i < n && bytes[i]);
-        if ((threadIdx.x & 31) == 0) words[i >> 5] = m;
-    }
-}
-__global__ void fill_i64_kernel(long long* p, uint64_t n, long long v) {
-    uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += stride) p[i] = v;
-}
 
 // ---- fast path: unique build keys + inner join --------------------------------------------------
 // One 16-byte slot {key, first_row, cnt} (one 32-byte sector per lookup instead of two), the non-key build columns
@@ -641,18 +629,24 @@ __global__ void join_runtime_filter_kernel(const void* key_data, int key_ctype, 
 }
 
 // ================================================================================================
+// When `buf` holds fewer than `need` bytes, replaces it by a buffer of max(need, alloc) bytes that keeps its first `keep` bytes.
+static void grow_keep(DevBuf& buf, size_t need, size_t keep, cudaStream_t st, size_t alloc = 0) {
+    if (need <= buf.bytes) return;
+    DevBuf nb;
+    nb.alloc(std::max(need, alloc));
+    if (keep) {
+        B200_CUDA(cudaMemcpyAsync(nb.p, buf.p, keep, cudaMemcpyDeviceToDevice, st));
+        B200_CUDA(cudaStreamSynchronize(st));
+    }
+    buf = std::move(nb);
+}
+
 struct GrowCol {  // growable device column (geometric growth, copy on grow)
     DevBuf buf;
     size_t used = 0;
-    void append(const void* src, size_t nbytes, bool src_is_host, cudaStream_t st) {
-        if (used + nbytes > buf.bytes) {
-            DevBuf nb;
-            nb.alloc(std::max<size_t>((used + nbytes) * 2, 1 << 16));
-            if (used) B200_CUDA(cudaMemcpyAsync(nb.p, buf.p, used, cudaMemcpyDeviceToDevice, st));
-            B200_CUDA(cudaStreamSynchronize(st));
-            buf = std::move(nb);
-        }
-        if (nbytes) B200_CUDA(cudaMemcpyAsync((char*)buf.p + used, src, nbytes, src_is_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st));
+    void append(const void* src, size_t nbytes, cudaStream_t st) {
+        grow_keep(buf, used + nbytes, used, st, std::max<size_t>((used + nbytes) * 2, 1 << 16));
+        if (nbytes) B200_CUDA(cudaMemcpyAsync((char*)buf.p + used, src, nbytes, cudaMemcpyDeviceToDevice, st));
         used += nbytes;
     }
     void reserve(size_t n) { if (n > buf.bytes) { B200_REQUIRE(used == 0, "internal: reserve after append"); buf.alloc(n); } }
@@ -672,10 +666,12 @@ class JoinState {
     int64_t n_build = 0;
     bool build_final = false;
     uint64_t cap = 0;
+    // the table the probe reads, chosen by finalize_build: the CSR key table of the general path; for unique build keys of an
+    // inner join, Slot16 (+ packed payload) built from the key table, or Slot32 (inline payload) with Slot16 derived on demand
+    enum class TableForm { CSR, SLOT16, SLOT32 } form = TableForm::CSR;
     DevBuf d_tkeys, d_info, d_row_slot, d_cnt_multi, d_goffs, d_groups, d_fill, d_bmatched;
     DevBuf d_slots16, d_bpack, d_cursor;  // fast path (unique build keys, inner join)
     DevBuf d_slots32;                      // inline-payload table (all-8-byte bitmap-free build schema, <= 2 payload columns)
-    bool fast_ready = false, inline_ready = false;
     int64_t inline_probes = 0, inline_builds = 0;
     // join kind (set_kind, before the first build batch): mark join / probe-side anti join (reference: is_mark_join member,
     // is_anti_join template argument of the probe)
@@ -686,7 +682,7 @@ class JoinState {
     uint64_t bloom_blocks = 0;
     long long key_min = INT64_MAX, key_max = INT64_MIN;
     int64_t filter_rows_in = 0, filter_rows_kept = 0;
-    unsigned long long* h_cursor = nullptr;
+    void* h_word = nullptr;  // pinned mirror of read_word
     int64_t fast_probes = 0;
     Scanner scan;
     // probe scratch + output
@@ -723,9 +719,18 @@ class JoinState {
         out_data.resize(n_b + np); out_vbytes.resize(n_b + np); out_bitmap.resize(n_b + np);
         if ((int)stage_data.size() < std::max(n_b, np)) { stage_data.resize(std::max(n_b, np)); stage_valid.resize(std::max(n_b, np)); }
     }
-    ~JoinState() { cudaSetDevice(device); scratch_set_stream(stream); cudaStreamSynchronize(stream); pinned_release(h_cursor, 8); }
+    ~JoinState() { cudaSetDevice(device); scratch_set_stream(stream); cudaStreamSynchronize(stream); pinned_release(h_word, 8); }
 
     int grid_for(int64_t n) const { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sms * 8)); }
+    const uint8_t* build_valid(int c) const { return b_has_valid[c] ? bvalid[c].buf.as<uint8_t>() : nullptr; }
+    // the device word at `dev` (synchronises the stream)
+    template <typename T> T read_word(const T* dev) {
+        static_assert(sizeof(T) <= 8, "one pinned 8-byte mirror");
+        if (!h_word) h_word = pinned_acquire(8);
+        B200_CUDA(cudaMemcpyAsync(h_word, dev, sizeof(T), cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaStreamSynchronize(stream));
+        return *(const T*)h_word;
+    }
 
     void set_kind(bool is_mark, bool is_anti) {
         B200_REQUIRE(n_build == 0 && !build_final, "b200 join: the join kind must be set before the first build batch");
@@ -747,7 +752,7 @@ class JoinState {
         const long long init[2] = {INT64_MAX, INT64_MIN};
         B200_CUDA(cudaMemcpyAsync(d_minmax.p, init, 16, cudaMemcpyHostToDevice, stream));
         if (n_build > 0) {
-            join_bloom_add_kernel<<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], b_has_valid[0] ? bvalid[0].buf.as<uint8_t>() : nullptr, n_build,
+            join_bloom_add_kernel<<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], build_valid(0), n_build,
                                                                         d_bloom.as<uint32_t>(), bloom_blocks, d_minmax.as<long long>());
             launches++;
             B200_CUDA(cudaGetLastError());
@@ -807,17 +812,17 @@ class JoinState {
             std::vector<const void*> data; std::vector<const uint8_t*> valid;
             stage_batch(t, n_b, b_ct, data, valid);
             for (int c = 0; c < n_b; c++) {
-                bcol[c].append(data[c], (size_t)n * ctype_size(b_ct[c]), false, stream);
+                bcol[c].append(data[c], (size_t)n * ctype_size(b_ct[c]), stream);
                 bool has = valid[c] != nullptr;
                 if (has && !b_has_valid[c]) {  // first batch with a bitmap: earlier rows were all valid
                     b_has_valid[c] = true;
-                    if (n_build) { DevBuf ones; ones.alloc((size_t)n_build); B200_CUDA(cudaMemsetAsync(ones.p, 1, (size_t)n_build, stream)); bvalid[c].append(ones.p, (size_t)n_build, false, stream); B200_CUDA(cudaStreamSynchronize(stream)); }
+                    if (n_build) { DevBuf ones; ones.alloc((size_t)n_build); B200_CUDA(cudaMemsetAsync(ones.p, 1, (size_t)n_build, stream)); bvalid[c].append(ones.p, (size_t)n_build, stream); B200_CUDA(cudaStreamSynchronize(stream)); }
                 }
                 if (b_has_valid[c]) {
                     d_stage_valid.ensure((size_t)n);
                     if (has) { expand_bitmap_kernel<<<grid_for(n), 256, 0, stream>>>(valid[c], n, d_stage_valid.as<uint8_t>()); launches++; }
                     else B200_CUDA(cudaMemsetAsync(d_stage_valid.p, 1, (size_t)n, stream));
-                    bvalid[c].append(d_stage_valid.p, (size_t)n, false, stream);
+                    bvalid[c].append(d_stage_valid.p, (size_t)n, stream);
                 }
             }
             B200_CUDA(cudaStreamSynchronize(stream));  // staging buffers are reused by the next batch
@@ -834,27 +839,27 @@ class JoinState {
         for (int c = 0; c < n_b; c++) ok = ok && ctype_size(b_ct[c]) == 8 && !b_has_valid[c];
         if (!ok) return false;
         d_slots32.alloc(n_slots * sizeof(Slot32));
-        d_cursor.alloc(8);
-        B200_CUDA(cudaMemsetAsync(d_cursor.p, 0, 8, stream));
+        DevBuf dup;  // raised by the second row of any key
+        dup.alloc(4);
+        B200_CUDA(cudaMemsetAsync(dup.p, 0, 4, stream));
         join_fill_slots32_kernel<<<grid_for((int64_t)n_slots), 256, 0, stream>>>(d_slots32.as<Slot32>(), n_slots);
         join_build_inline_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>((n_build + 1023) / 1024, (int64_t)sms * 8)), 256, 0, stream>>>(bcol[0].buf.as<long long>(), nf > 0 ? bcol[1].buf.as<unsigned long long>() : nullptr,
                                                                        nf > 1 ? bcol[2].buf.as<unsigned long long>() : nullptr, n_build, 0, d_slots32.as<Slot32>(), cap,
-                                                                       (int*)d_cursor.p);
+                                                                       dup.as<int>());
         launches += 2;
         B200_CUDA(cudaGetLastError());
-        if (!h_cursor) h_cursor = (unsigned long long*)pinned_acquire(8);
-        B200_CUDA(cudaMemcpyAsync(h_cursor, d_cursor.p, 8, cudaMemcpyDeviceToHost, stream));
-        B200_CUDA(cudaStreamSynchronize(stream));
-        if (*h_cursor != 0) { d_slots32.release(); return false; }  // duplicate build keys
+        if (read_word(dup.as<int>()) != 0) { d_slots32.release(); return false; }  // duplicate build keys
         return true;
     }
-    // Slot16 table + packed payload of the two-sector fast kernel, derived on demand when a probe batch does not qualify for the
-    // inline kernel (bitmaps, narrow columns) after an inline build
-    void ensure_fast_tables() {
-        if (d_slots16.p) return;
+    // Slot16 table + packed payload of the two-sector fast kernel: from the key table when finalize_build finds unique keys, or
+    // on demand from the Slot32 table when a probe batch does not qualify for the inline kernel (bitmaps, narrow columns)
+    void setup_slot16() {
         const uint64_t n_slots = cap + 2;
         d_slots16.alloc(n_slots * sizeof(Slot16));
-        join_slots16_from32_kernel<<<grid_for((int64_t)n_slots), 256, 0, stream>>>(d_slots32.as<Slot32>(), n_slots, d_slots16.as<Slot16>());
+        if (form == TableForm::SLOT32)
+            join_slots16_from32_kernel<<<grid_for((int64_t)n_slots), 256, 0, stream>>>(d_slots32.as<Slot32>(), n_slots, d_slots16.as<Slot16>());
+        else
+            join_make_slots16_kernel<<<grid_for((int64_t)n_slots), 256, 0, stream>>>(d_tkeys.as<long long>(), d_info.as<SlotInfo>(), n_slots, d_slots16.as<Slot16>());
         const int nf = n_b - 1;
         d_bpack.alloc((size_t)std::max<int64_t>(n_build * std::max(nf, 1), 1) * 8);
         if (nf > 0) {
@@ -872,19 +877,18 @@ class JoinState {
         while (cap < 2ull * (uint64_t)n_build) cap <<= 1;
         uint64_t n_slots = cap + 2;
         if (!mark && !anti && try_inline_build(n_slots)) {
-            d_goffs.alloc(8); d_groups.alloc(8);
-            fast_ready = true; inline_ready = true; inline_builds++;
+            form = TableForm::SLOT32; inline_builds++;
             build_final = true;
             return;
         }
         d_tkeys.alloc(n_slots * 8);
-        fill_i64_kernel<<<grid_for((int64_t)n_slots), 256, 0, stream>>>(d_tkeys.as<long long>(), n_slots, J_EMPTY);
+        launch_fill_u64(d_tkeys.p, n_slots, (unsigned long long)J_EMPTY, grid_for((int64_t)n_slots), stream);
         d_info.alloc(n_slots * sizeof(SlotInfo));
         B200_CUDA(cudaMemsetAsync(d_info.p, 0, n_slots * sizeof(SlotInfo), stream));
         d_row_slot.alloc((size_t)std::max<int64_t>(n_build, 1) * 4);
         launches++;
         if (n_build > 0) {
-            join_insert_count_kernel<<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], b_has_valid[0] ? bvalid[0].buf.as<uint8_t>() : nullptr,
+            join_insert_count_kernel<<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], build_valid(0),
                                                                            n_build, d_tkeys.as<long long>(), cap, d_info.as<SlotInfo>(), d_row_slot.as<uint32_t>(), na_equal ? 1 : 0);
             d_cnt_multi.alloc(n_slots * 4);
             join_slot_counts_kernel<<<grid_for((int64_t)n_slots), 256, 0, stream>>>(d_info.as<SlotInfo>(), n_slots, d_cnt_multi.as<uint32_t>());
@@ -900,26 +904,12 @@ class JoinState {
                 launches++;
             }
             d_cnt_multi.release(); d_fill.release(); d_row_slot.release();
-            if (n_multi == 0 && !build_outer && !probe_outer && !mark && !anti && n_b >= 1) {
+            if (n_multi == 0 && !build_outer && !probe_outer && !mark && !anti) {
                 // every key (incl. the NA / marker groups) has exactly one build row: set up the fused probe path
-                d_slots16.alloc(n_slots * sizeof(Slot16));
-                join_make_slots16_kernel<<<grid_for((int64_t)n_slots), 256, 0, stream>>>(d_tkeys.as<long long>(), d_info.as<SlotInfo>(), n_slots, d_slots16.as<Slot16>());
-                int nf = n_b - 1;
-                d_bpack.alloc((size_t)std::max<int64_t>(n_build * std::max(nf, 1), 1) * 8);
-                if (nf > 0) {
-                    PackPayloadArgs pa{};
-                    pa.n_build = n_build; pa.n_fields = nf; pa.out = d_bpack.as<unsigned long long>();
-                    for (int c = 1; c < n_b; c++) { pa.src[c - 1] = bcol[c].buf.p; pa.size[c - 1] = ctype_size(b_ct[c]); }
-                    join_pack_payload_kernel<<<grid_for(n_build), 256, 0, stream>>>(pa);
-                }
-                d_cursor.alloc(8);
-                if (!h_cursor) h_cursor = (unsigned long long*)pinned_acquire(8);
-                launches += 2;
-                fast_ready = true;
+                form = TableForm::SLOT16;
+                setup_slot16();
                 d_tkeys.release(); d_info.release();  // the general-path table is not needed any more
             }
-        } else {
-            d_goffs.alloc(8); d_groups.alloc(8);
         }
         if (build_outer) { d_bmatched.alloc((size_t)std::max<int64_t>(n_build, 1)); B200_CUDA(cudaMemsetAsync(d_bmatched.p, 0, (size_t)std::max<int64_t>(n_build, 1), stream)); }
         B200_CUDA(cudaGetLastError());
@@ -927,91 +917,169 @@ class JoinState {
         build_final = true;
     }
 
-    // describes output column k (0..n_kb-1 build, then probe) in `out`
-    void describe_out(b200_table* out, const std::vector<int>& kb, const std::vector<int>& kp, int64_t rows) {
-        out->n_rows = rows; out->n_cols = (int)(kb.size() + kp.size()); out->device = device;
-        for (size_t k = 0; k < kb.size() + kp.size(); k++) {
-            bool is_b = k < kb.size();
-            int src = is_b ? kb[k] : kp[k - kb.size()];
-            b200_column& c = out->cols[k];
-            c.data = out_data[k].p; c.length = rows;
-            c.c_type = is_b ? b_ct[src] : p_ct[src];
-            bool nullable = out_vbytes[k].p != nullptr && out_has_valid[k];
-            c.validity = nullable ? out_bitmap[k].as<uint8_t>() : nullptr;
-            c.arr_type = nullable ? ARR_NULLABLE : (is_b ? b_at[src] : p_at[src]);
+    // One output column of a probe batch: the kept build columns come first, then the kept probe columns.
+    struct OutCol {
+        bool is_b;      // build side, else probe side
+        int src;        // column of that side
+        int size;       // item bytes
+        bool nullable;  // has validity: one byte per row while the kernels write it, a bitmap in the output
+    };
+    // A column is nullable when its input has a bitmap or a nullable array type, or when an outer / anti join NULL-extends its side.
+    std::vector<OutCol> plan_out(const std::vector<int>& kb, const std::vector<int>& kp, const std::vector<const uint8_t*>& valid) const {
+        std::vector<OutCol> cols;
+        for (int src : kb) {
+            // the unique-key kernels write the probe's key value into the build key column, so it takes the probe key's bitmap
+            const bool has_bitmap = (src == 0 && form != TableForm::CSR) ? valid[0] != nullptr : b_has_valid[src];
+            cols.push_back({true, src, ctype_size(b_ct[src]), has_bitmap || b_at[src] == ARR_NULLABLE || probe_outer || anti});
+        }
+        for (int src : kp) cols.push_back({false, src, ctype_size(p_ct[src]), valid[src] != nullptr || p_at[src] == ARR_NULLABLE || build_outer});
+        return cols;
+    }
+    // room for `rows` output rows; the first `keep` rows already written survive a regrowth
+    void size_outputs(const std::vector<OutCol>& cols, int64_t rows, int64_t keep = 0) {
+        for (size_t k = 0; k < cols.size(); k++) {
+            grow_keep(out_data[k], (size_t)(rows + 32) * cols[k].size, (size_t)keep * cols[k].size, stream);
+            if (cols[k].nullable) {
+                grow_keep(out_vbytes[k], (size_t)rows + 32, (size_t)keep, stream);
+                out_bitmap[k].ensure((size_t)((rows + 31) / 32 + 1) * 4);
+            }
         }
     }
-    std::vector<bool> out_has_valid;
-
-    int64_t probe_fast(const b200_table* t, const std::vector<int>& kb, const std::vector<int>& kp, const std::vector<const void*>& data,
-                       const std::vector<const uint8_t*>& valid, b200_table* out) {
-        int64_t n = t->n_rows;
-        int n_out_cols = (int)(kb.size() + kp.size());
-        out_has_valid.assign(n_out_cols, false);
-        for (int k = 0; k < n_out_cols; k++) {
-            bool is_b = k < (int)kb.size();
-            int src = is_b ? kb[k] : kp[k - kb.size()];
-            out_has_valid[k] = is_b ? (src == 0 ? (valid[0] != nullptr || b_at[0] == ARR_NULLABLE) : (b_has_valid[src] || b_at[src] == ARR_NULLABLE))
-                                    : (valid[src] != nullptr || p_at[src] == ARR_NULLABLE);
-            out_data[k].ensure((size_t)(n + 32) * ctype_size(is_b ? b_ct[src] : p_ct[src]));  // matches <= probe rows
-            if (out_has_valid[k]) { out_vbytes[k].ensure((size_t)n + 32); out_bitmap[k].ensure((size_t)((n + 31) / 32 + 1) * 4); }
+    uint8_t* out_valid(const std::vector<OutCol>& cols, size_t k) const { return cols[k].nullable ? out_vbytes[k].as<uint8_t>() : nullptr; }
+    void describe_out(b200_table* out, const std::vector<OutCol>& cols, int64_t rows) {
+        out->n_rows = rows; out->n_cols = (int)cols.size(); out->device = device;
+        for (size_t k = 0; k < cols.size(); k++) {
+            const OutCol& oc = cols[k];
+            b200_column& c = out->cols[k];
+            c.data = out_data[k].p; c.length = rows;
+            c.c_type = oc.is_b ? b_ct[oc.src] : p_ct[oc.src];
+            c.validity = oc.nullable ? out_bitmap[k].as<uint8_t>() : nullptr;
+            c.arr_type = oc.nullable ? ARR_NULLABLE : (oc.is_b ? b_at[oc.src] : p_at[oc.src]);
         }
-        int64_t rows = 0;
-        if (n > 0) {
+    }
+
+    // unique build keys, inner join: one fused lookup + gather kernel, the inline-payload one when the batch qualifies
+    int64_t probe_unique(int64_t n, const std::vector<OutCol>& cols, int nkb, const std::vector<const void*>& data,
+                         const std::vector<const uint8_t*>& valid) {
+        size_outputs(cols, n);  // matches <= probe rows
+        if (n == 0) return 0;
+        const int nkp = (int)cols.size() - nkb;
+        d_cursor.ensure(8);
+        B200_CUDA(cudaMemsetAsync(d_cursor.p, 0, 8, stream));
+        // inline-payload variant: every column of this batch 8 bytes wide and bitmap-free, 1..4 kept probe columns
+        // (a nullable-typed column without a bitmap still gets one)
+        bool inl = form == TableForm::SLOT32 && valid[0] == nullptr && nkp >= 1 && nkp <= J_INL_MAX_P && nkb <= 4;
+        for (const OutCol& c : cols) inl = inl && c.size == 8 && !c.nullable;
+        const int gridp = (int)std::min<int64_t>((int64_t)sms * 8, (n + 1023) / 1024);
+        if (inl) {
+            InlineProbeArgs ia{};
+            ia.n_probe = n; ia.key = (const long long*)data[0]; ia.slots = d_slots32.as<Slot32>(); ia.cap = cap;
+            ia.cursor = d_cursor.as<unsigned long long>(); ia.n_b = nkb;
+            for (int k = 0; k < (int)cols.size(); k++) {
+                if (cols[k].is_b) { ia.b_field[k] = cols[k].src - 1; ia.ob[k] = out_data[k].as<unsigned long long>(); }
+                else { ia.p[k - nkb] = (const unsigned long long*)data[cols[k].src]; ia.op[k - nkb] = out_data[k].as<unsigned long long>(); }
+            }
+            const int nf = n_b - 1;
+#define B200_INL(NF, NPK) join_probe_inline_kernel<NF, NPK><<<gridp, 256, 0, stream>>>(ia)
+#define B200_INL_NF(NF) do { switch (nkp) { case 1: B200_INL(NF, 1); break; case 2: B200_INL(NF, 2); break; case 3: B200_INL(NF, 3); break; default: B200_INL(NF, 4); break; } } while (0)
+            if (nf <= 0) B200_INL_NF(0); else if (nf == 1) B200_INL_NF(1); else B200_INL_NF(2);
+#undef B200_INL_NF
+#undef B200_INL
+            inline_probes++;
+        } else {
+            if (!d_slots16.p) setup_slot16();
             FastProbeArgs f{};
             f.n_probe = n; f.key_data = data[0]; f.key_ctype = p_ct[0]; f.key_valid = valid[0];
             f.slots = d_slots16.as<Slot16>(); f.cap = cap; f.bpack = d_bpack.as<unsigned long long>(); f.n_fields = std::max(n_b - 1, 1);
-            f.cursor = d_cursor.as<unsigned long long>(); f.n_b = (int)kb.size(); f.n_p = (int)kp.size(); f.na_equal = na_equal ? 1 : 0;
-            for (int k = 0; k < n_out_cols; k++) {
-                bool is_b = k < (int)kb.size();
-                int src = is_b ? kb[k] : kp[k - kb.size()];
-                if (is_b) {
-                    f.b_field[k] = src - 1; f.b_size[k] = ctype_size(b_ct[src]);
-                    f.b_valid[k] = (src > 0 && b_has_valid[src]) ? bvalid[src].buf.as<uint8_t>() : nullptr;
-                    f.ob_data[k] = out_data[k].p; f.ob_valid[k] = out_has_valid[k] ? out_vbytes[k].as<uint8_t>() : nullptr;
+            f.cursor = d_cursor.as<unsigned long long>(); f.n_b = nkb; f.n_p = nkp; f.na_equal = na_equal ? 1 : 0;
+            for (int k = 0; k < (int)cols.size(); k++) {
+                const OutCol& c = cols[k];
+                if (c.is_b) {
+                    f.b_field[k] = c.src - 1; f.b_size[k] = c.size; f.b_valid[k] = c.src > 0 ? build_valid(c.src) : nullptr;
+                    f.ob_data[k] = out_data[k].p; f.ob_valid[k] = out_valid(cols, k);
                 } else {
-                    int j = k - (int)kb.size();
-                    f.p_data[j] = data[src]; f.p_valid[j] = valid[src]; f.p_size[j] = ctype_size(p_ct[src]);
-                    f.op_data[j] = out_data[k].p; f.op_valid[j] = out_has_valid[k] ? out_vbytes[k].as<uint8_t>() : nullptr;
+                    const int j = k - nkb;
+                    f.p_data[j] = data[c.src]; f.p_valid[j] = valid[c.src]; f.p_size[j] = c.size;
+                    f.op_data[j] = out_data[k].p; f.op_valid[j] = out_valid(cols, k);
                 }
             }
-            B200_CUDA(cudaMemsetAsync(d_cursor.p, 0, 8, stream));
-            // inline-payload variant: every column of this batch 8 bytes wide and bitmap-free, 1..4 kept probe columns
-            bool inl = inline_ready && valid[0] == nullptr && kp.size() >= 1 && kp.size() <= (size_t)J_INL_MAX_P && kb.size() <= 4;
-            for (int src : kp) inl = inl && ctype_size(p_ct[src]) == 8 && valid[src] == nullptr;
-            for (int k = 0; k < n_out_cols; k++) inl = inl && !out_has_valid[k];  // (a nullable-typed column without a bitmap still gets one)
-            const int gridp = (int)std::min<int64_t>((int64_t)sms * 8, (n + 1023) / 1024);
-            if (inl) {
-                InlineProbeArgs ia{};
-                ia.n_probe = n; ia.key = (const long long*)data[0]; ia.slots = d_slots32.as<Slot32>(); ia.cap = cap;
-                ia.cursor = d_cursor.as<unsigned long long>(); ia.n_b = (int)kb.size();
-                for (size_t k = 0; k < kb.size(); k++) { ia.b_field[k] = kb[k] - 1; ia.ob[k] = out_data[k].as<unsigned long long>(); }
-                for (size_t j = 0; j < kp.size(); j++) { ia.p[j] = (const unsigned long long*)data[kp[j]]; ia.op[j] = out_data[kb.size() + j].as<unsigned long long>(); }
-                const int nf = n_b - 1;
-#define B200_INL(NF, NPK) join_probe_inline_kernel<NF, NPK><<<gridp, 256, 0, stream>>>(ia)
-#define B200_INL_NF(NF) do { switch (kp.size()) { case 1: B200_INL(NF, 1); break; case 2: B200_INL(NF, 2); break; case 3: B200_INL(NF, 3); break; default: B200_INL(NF, 4); break; } } while (0)
-                if (nf <= 0) B200_INL_NF(0); else if (nf == 1) B200_INL_NF(1); else B200_INL_NF(2);
-#undef B200_INL_NF
-#undef B200_INL
-                inline_probes++;
-            } else {
-                ensure_fast_tables();
-                f.slots = d_slots16.as<Slot16>(); f.bpack = d_bpack.as<unsigned long long>();
-                join_probe_fast_kernel<<<gridp, 256, 0, stream>>>(f);
-            }
-            launches++; fast_probes++;
-            B200_CUDA(cudaGetLastError());
-            B200_CUDA(cudaMemcpyAsync(h_cursor, d_cursor.p, 8, cudaMemcpyDeviceToHost, stream));
-            B200_CUDA(cudaStreamSynchronize(stream));
-            rows = (int64_t)*h_cursor;
-            for (int k = 0; k < n_out_cols; k++)
-                if (out_has_valid[k] && rows > 0) { pack_bitmap_kernel<<<grid_for(rows), 256, 0, stream>>>(out_vbytes[k].as<uint8_t>(), rows, out_bitmap[k].as<uint32_t>()); launches++; }
-            B200_CUDA(cudaGetLastError());
-            B200_CUDA(cudaStreamSynchronize(stream));
+            join_probe_fast_kernel<<<gridp, 256, 0, stream>>>(f);
         }
-        describe_out(out, kb, kp, rows);
-        probe_rows += n; out_rows_total += rows;
-        return rows;
+        launches++; fast_probes++;
+        B200_CUDA(cudaGetLastError());
+        return (int64_t)read_word(d_cursor.as<unsigned long long>());
+    }
+
+    // general path (CSR groups: duplicate keys, outer, anti and mark joins): count + scan, then expand and gather; the unmatched
+    // build rows of a build-outer join follow the last probe batch
+    int64_t probe_general(int64_t n, const std::vector<OutCol>& cols, int nkb, const std::vector<const void*>& data,
+                          const std::vector<const uint8_t*>& valid, bool is_last) {
+        // pass A + scan
+        unsigned long long n_match = 0;
+        d_pslot.ensure((size_t)(n + 1) * 4); d_pcnt.ensure((size_t)(n + 1) * 4); d_poff.ensure((size_t)(n + 2) * 8);
+        if (n > 0) {
+            if (mark) { d_mark.ensure((size_t)n + 32); d_mark_valid.ensure((size_t)(n + 7) / 8 + 32); B200_CUDA(cudaMemsetAsync(d_mark_valid.p, 0xff, (size_t)(n + 7) / 8 + 8, stream)); }
+            join_probe_count_kernel<<<grid_for(n), 256, 0, stream>>>(data[0], p_ct[0], valid[0], n, d_tkeys.as<long long>(), cap, d_info.as<SlotInfo>(),
+                                                                     probe_outer ? 1 : 0, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(), na_equal ? 1 : 0,
+                                                                     anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr);
+            launches++;
+            B200_CUDA(cudaMemsetAsync(d_pcnt.as<uint32_t>() + n, 0, 4, stream));
+            n_match = scan.run(d_pcnt.as<uint32_t>(), n + 1, d_poff.as<unsigned long long>(), stream, &launches);
+        }
+        // unmatched build rows go out with the last probe batch
+        unsigned long long n_tail = 0;
+        DevBuf tail_flags, tail_off;
+        if (is_last && build_outer && !tail_emitted && n_build > 0) {
+            tail_flags.alloc((size_t)(n_build + 1) * 4); tail_off.alloc((size_t)(n_build + 2) * 8);
+        }
+        // pass B needs bmatched complete before the tail is computed, so: gather first, then the tail
+        size_outputs(cols, (int64_t)n_match);
+        GatherArgs g{};
+        g.n_probe = n; g.pslot = d_pslot.as<uint32_t>(); g.poff = d_poff.as<unsigned long long>(); g.info = d_info.as<SlotInfo>();
+        g.goffs = d_goffs.as<unsigned long long>(); g.groups = d_groups.as<uint32_t>(); g.bmatched = build_outer ? d_bmatched.as<uint8_t>() : nullptr;
+        g.n_b = nkb; g.n_p = (int)cols.size() - nkb;
+        for (int k = 0; k < (int)cols.size(); k++) {
+            const OutCol& c = cols[k];
+            if (c.is_b) {
+                g.b_data[k] = bcol[c.src].buf.p; g.b_valid[k] = build_valid(c.src); g.b_size[k] = c.size;
+                g.ob_data[k] = out_data[k].p; g.ob_valid[k] = out_valid(cols, k);
+            } else {
+                const int j = k - nkb;
+                g.p_data[j] = data[c.src]; g.p_valid[j] = valid[c.src]; g.p_size[j] = c.size;
+                g.op_data[j] = out_data[k].p; g.op_valid[j] = out_valid(cols, k);
+            }
+        }
+        if (n > 0 && n_match > 0) { join_probe_gather_kernel<<<grid_for(n), 256, 0, stream>>>(g); launches++; B200_CUDA(cudaGetLastError()); }
+        if (tail_flags.p) {
+            join_unmatched_flags_kernel<<<grid_for(n_build), 256, 0, stream>>>(d_bmatched.as<uint8_t>(), n_build, tail_flags.as<uint32_t>());
+            B200_CUDA(cudaMemsetAsync(tail_flags.as<uint32_t>() + n_build, 0, 4, stream));
+            launches++;
+            n_tail = scan.run(tail_flags.as<uint32_t>(), n_build + 1, tail_off.as<unsigned long long>(), stream, &launches);
+            tail_emitted = true;
+            if (n_tail > 0) {
+                // the tail size is only known after the gather: grow the outputs, keeping the gathered rows
+                size_outputs(cols, (int64_t)(n_match + n_tail), (int64_t)n_match);
+                TailArgs ta{};
+                ta.n_build = n_build; ta.flags = tail_flags.as<uint32_t>(); ta.off = tail_off.as<unsigned long long>();
+                ta.n_b = nkb; ta.n_p = (int)cols.size() - nkb;
+                for (int k = 0; k < (int)cols.size(); k++) {
+                    const OutCol& c = cols[k];
+                    void* od = (char*)out_data[k].p + n_match * c.size;
+                    uint8_t* ov = c.nullable ? out_vbytes[k].as<uint8_t>() + n_match : nullptr;
+                    if (c.is_b) {
+                        ta.b_data[k] = bcol[c.src].buf.p; ta.b_valid[k] = build_valid(c.src); ta.b_size[k] = c.size;
+                        ta.ob_data[k] = od; ta.ob_valid[k] = ov;
+                    } else {
+                        const int j = k - nkb;
+                        ta.p_size[j] = c.size; ta.op_data[j] = od; ta.op_valid[j] = ov;
+                    }
+                }
+                join_unmatched_emit_kernel<<<grid_for(n_build), 256, 0, stream>>>(ta);
+                launches++;
+                B200_CUDA(cudaGetLastError());
+            }
+        }
+        return (int64_t)(n_match + n_tail);
     }
 
     int64_t probe_consume(const b200_table* t, const uint64_t* kept_b, int64_t n_kb, const uint64_t* kept_p, int64_t n_kp,
@@ -1035,119 +1103,14 @@ class JoinState {
         int64_t n = t->n_rows;
         std::vector<const void*> data; std::vector<const uint8_t*> valid;
         stage_batch(t, n_p, p_ct, data, valid);
-        if (fast_ready) return probe_fast(t, kb, kp, data, valid, out);
-        // pass A + scan
-        unsigned long long n_match = 0;
-        d_pslot.ensure((size_t)(n + 1) * 4); d_pcnt.ensure((size_t)(n + 1) * 4); d_poff.ensure((size_t)(n + 2) * 8);
-        if (n > 0) {
-            if (mark) { d_mark.ensure((size_t)n + 32); d_mark_valid.ensure((size_t)(n + 7) / 8 + 32); B200_CUDA(cudaMemsetAsync(d_mark_valid.p, 0xff, (size_t)(n + 7) / 8 + 8, stream)); }
-            join_probe_count_kernel<<<grid_for(n), 256, 0, stream>>>(data[0], p_ct[0], valid[0], n, d_tkeys.as<long long>(), cap, d_info.as<SlotInfo>(),
-                                                                     probe_outer ? 1 : 0, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(), na_equal ? 1 : 0,
-                                                                     anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr);
-            launches++;
-            B200_CUDA(cudaMemsetAsync(d_pcnt.as<uint32_t>() + n, 0, 4, stream));
-            n_match = scan.run(d_pcnt.as<uint32_t>(), n + 1, d_poff.as<unsigned long long>(), stream, &launches);
-        }
-        // unmatched build rows go out with the last probe batch
-        unsigned long long n_tail = 0;
-        DevBuf tail_flags, tail_off;
-        if (is_last && build_outer && !tail_emitted && n_build > 0) {
-            tail_flags.alloc((size_t)(n_build + 1) * 4); tail_off.alloc((size_t)(n_build + 2) * 8);
-        }
-        // which output columns carry validity: nullable inputs, NULL-extended sides of an outer join
-        out_has_valid.assign(n_out_cols, false);
-        for (int k = 0; k < n_out_cols; k++) {
-            bool is_b = k < (int)kb.size();
-            int src = is_b ? kb[k] : kp[k - kb.size()];
-            out_has_valid[k] = is_b ? (b_has_valid[src] || b_at[src] == ARR_NULLABLE || probe_outer || anti)
-                                    : (valid[src] != nullptr || p_at[src] == ARR_NULLABLE || build_outer);
-        }
-        auto ensure_out = [&](int64_t rows) {
-            for (int k = 0; k < n_out_cols; k++) {
-                bool is_b = k < (int)kb.size();
-                int src = is_b ? kb[k] : kp[k - kb.size()];
-                out_data[k].ensure((size_t)(rows + 32) * ctype_size(is_b ? b_ct[src] : p_ct[src]));
-                if (out_has_valid[k]) { out_vbytes[k].ensure((size_t)rows + 32); out_bitmap[k].ensure((size_t)((rows + 31) / 32 + 1) * 4); }
-            }
-        };
-        // pass B needs bmatched complete before the tail is computed, so: gather first, then the tail
-        GatherArgs g{};
-        g.n_probe = n; g.pslot = d_pslot.as<uint32_t>(); g.poff = d_poff.as<unsigned long long>(); g.info = d_info.as<SlotInfo>();
-        g.goffs = d_goffs.as<unsigned long long>(); g.groups = d_groups.as<uint32_t>(); g.bmatched = build_outer ? d_bmatched.as<uint8_t>() : nullptr;
-        g.n_b = (int)kb.size(); g.n_p = (int)kp.size();
-        // the tail size is only known after the gather; grow the output (keeping the gathered rows) if needed
-        ensure_out((int64_t)n_match);
-        for (int k = 0; k < n_out_cols; k++) {
-            bool is_b = k < (int)kb.size();
-            int src = is_b ? kb[k] : kp[k - kb.size()];
-            if (is_b) {
-                int j = k;
-                g.b_data[j] = bcol[src].buf.p; g.b_valid[j] = b_has_valid[src] ? bvalid[src].buf.as<uint8_t>() : nullptr; g.b_size[j] = ctype_size(b_ct[src]);
-                g.ob_data[j] = out_data[k].p; g.ob_valid[j] = out_has_valid[k] ? out_vbytes[k].as<uint8_t>() : nullptr;
-            } else {
-                int j = k - (int)kb.size();
-                g.p_data[j] = data[src]; g.p_valid[j] = valid[src]; g.p_size[j] = ctype_size(p_ct[src]);
-                g.op_data[j] = out_data[k].p; g.op_valid[j] = out_has_valid[k] ? out_vbytes[k].as<uint8_t>() : nullptr;
-            }
-        }
-        if (n > 0 && n_match > 0) { join_probe_gather_kernel<<<grid_for(n), 256, 0, stream>>>(g); launches++; B200_CUDA(cudaGetLastError()); }
-        if (tail_flags.p) {
-            join_unmatched_flags_kernel<<<grid_for(n_build), 256, 0, stream>>>(d_bmatched.as<uint8_t>(), n_build, tail_flags.as<uint32_t>());
-            B200_CUDA(cudaMemsetAsync(tail_flags.as<uint32_t>() + n_build, 0, 4, stream));
-            launches++;
-            n_tail = scan.run(tail_flags.as<uint32_t>(), n_build + 1, tail_off.as<unsigned long long>(), stream, &launches);
-            tail_emitted = true;
-            if (n_tail > 0) {
-                // grow output columns, preserving the rows already gathered
-                for (int k = 0; k < n_out_cols; k++) {
-                    bool is_b = k < (int)kb.size();
-                    int src = is_b ? kb[k] : kp[k - kb.size()];
-                    size_t isz = ctype_size(is_b ? b_ct[src] : p_ct[src]);
-                    size_t need = (size_t)(n_match + n_tail + 32) * isz;
-                    if (need > out_data[k].bytes) {
-                        DevBuf nb; nb.alloc(need);
-                        B200_CUDA(cudaMemcpyAsync(nb.p, out_data[k].p, (size_t)n_match * isz, cudaMemcpyDeviceToDevice, stream));
-                        B200_CUDA(cudaStreamSynchronize(stream));
-                        out_data[k] = std::move(nb);
-                    }
-                    if (out_has_valid[k]) {
-                        size_t needv = (size_t)(n_match + n_tail) + 32;
-                        if (needv > out_vbytes[k].bytes) {
-                            DevBuf nb; nb.alloc(needv);
-                            B200_CUDA(cudaMemcpyAsync(nb.p, out_vbytes[k].p, (size_t)n_match, cudaMemcpyDeviceToDevice, stream));
-                            B200_CUDA(cudaStreamSynchronize(stream));
-                            out_vbytes[k] = std::move(nb);
-                        }
-                        out_bitmap[k].ensure((size_t)((n_match + n_tail + 31) / 32 + 1) * 4);
-                    }
-                }
-                TailArgs ta{};
-                ta.n_build = n_build; ta.flags = tail_flags.as<uint32_t>(); ta.off = tail_off.as<unsigned long long>();
-                ta.n_b = (int)kb.size(); ta.n_p = (int)kp.size();
-                for (int k = 0; k < n_out_cols; k++) {
-                    bool is_b = k < (int)kb.size();
-                    int src = is_b ? kb[k] : kp[k - kb.size()];
-                    size_t isz = ctype_size(is_b ? b_ct[src] : p_ct[src]);
-                    if (is_b) {
-                        ta.b_data[k] = bcol[src].buf.p; ta.b_valid[k] = b_has_valid[src] ? bvalid[src].buf.as<uint8_t>() : nullptr; ta.b_size[k] = (int)isz;
-                        ta.ob_data[k] = (char*)out_data[k].p + n_match * isz; ta.ob_valid[k] = out_has_valid[k] ? out_vbytes[k].as<uint8_t>() + n_match : nullptr;
-                    } else {
-                        int j = k - (int)kb.size();
-                        ta.p_size[j] = (int)isz;
-                        ta.op_data[j] = (char*)out_data[k].p + n_match * isz; ta.op_valid[j] = out_vbytes[k].as<uint8_t>() + n_match;
-                    }
-                }
-                join_unmatched_emit_kernel<<<grid_for(n_build), 256, 0, stream>>>(ta);
-                launches++;
-                B200_CUDA(cudaGetLastError());
-            }
-        }
-        int64_t rows = (int64_t)(n_match + n_tail);
+        const std::vector<OutCol> cols = plan_out(kb, kp, valid);
+        const int64_t rows = form == TableForm::CSR ? probe_general(n, cols, (int)kb.size(), data, valid, is_last)
+                                                    : probe_unique(n, cols, (int)kb.size(), data, valid);
         for (int k = 0; k < n_out_cols; k++)
-            if (out_has_valid[k] && rows > 0) { pack_bitmap_kernel<<<grid_for(rows), 256, 0, stream>>>(out_vbytes[k].as<uint8_t>(), rows, out_bitmap[k].as<uint32_t>()); launches++; }
+            if (cols[k].nullable && rows > 0) { launch_pack_bitmap(out_vbytes[k].as<uint8_t>(), rows, out_bitmap[k].as<uint32_t>(), grid_for(rows), stream); launches++; }
         B200_CUDA(cudaGetLastError());
         B200_CUDA(cudaStreamSynchronize(stream));
-        describe_out(out, kb, kp, rows);
+        describe_out(out, cols, rows);
         if (mark) {  // the mark column: BOOL, nullable array type, every row valid; output row i is probe row i
             b200_column& c = out->cols[n_out_cols];
             c.data = d_mark.p; c.validity = d_mark_valid.as<uint8_t>(); c.length = rows; c.c_type = CT_BOOL; c.arr_type = ARR_NULLABLE;

@@ -1,4 +1,5 @@
-// misc.cu — error reporting, runtime probes, raw memory helpers and the synthetic-table generator.
+// misc.cu — error reporting, runtime probes, raw memory helpers, the shared bitmap-pack and fill kernels and the
+// synthetic-table generator.
 #include <cstdlib>
 #include <mutex>
 #include <vector>
@@ -120,6 +121,26 @@ void pinned_release(void* p, size_t bytes) {
 
 static thread_local std::string g_last_error;
 void set_last_error(const std::string& msg) { g_last_error = msg; }
+
+__global__ void pack_bitmap_kernel(const uint8_t* bytes, int64_t n, uint32_t* words) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    int64_t n_round = (n + 31) & ~31ll;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n_round; i += stride) {
+        unsigned m = __ballot_sync(0xffffffffu, i < n && bytes[i]);
+        if ((threadIdx.x & 31) == 0) words[i >> 5] = m;
+    }
+}
+void launch_pack_bitmap(const uint8_t* bytes, int64_t n, uint32_t* words, int grid, cudaStream_t st) {
+    pack_bitmap_kernel<<<grid, 256, 0, st>>>(bytes, n, words);
+}
+
+__global__ void fill_u64_kernel(unsigned long long* p, uint64_t n, unsigned long long v) {
+    uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += stride) p[i] = v;
+}
+void launch_fill_u64(void* p, uint64_t n, unsigned long long v, int grid, cudaStream_t st) {
+    fill_u64_kernel<<<grid, 256, 0, st>>>((unsigned long long*)p, n, v);
+}
 
 // key = mix64(row ^ seed-derived salt) % n_groups ; val = (mix64(...) % 1000) - 500 (INT64) or u01 (FLOAT64).
 // Same arithmetic as oracle_synth_fill (oracle/bodo_oracle.c) and bodo_b200/synth.py.
