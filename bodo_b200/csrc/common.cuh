@@ -211,6 +211,9 @@ __host__ __device__ __forceinline__ uint64_t f64_to_ordered(double d) {
 #endif
     return b ^ ((b >> 63) ? 0xFFFFFFFFFFFFFFFFULL : 0x8000000000000000ULL);
 }
+// order-preserving signed form of a canon_float_key encoding of a non-NaN key (the join's runtime-filter bounds, so they stay
+// int64 min / max): a negative double's magnitude bits are flipped.  Its own inverse.
+__host__ __device__ __forceinline__ long long canon_float_ordered(long long k) { return k < 0 ? k ^ 0x7FFFFFFFFFFFFFFFLL : k; }
 __host__ __device__ __forceinline__ double ordered_to_f64(uint64_t e) {
     uint64_t b = e ^ ((e >> 63) ? 0x8000000000000000ULL : 0xFFFFFFFFFFFFFFFFULL);
 #ifdef __CUDA_ARCH__

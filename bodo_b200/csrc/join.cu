@@ -18,6 +18,8 @@
 // with an NA key never match — they are filtered from the build table unless it is the outer side
 // (_join.cpp:3180 filter_na_values) and only survive as NULL-extended rows of an outer join.
 #include <algorithm>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "common.cuh"
@@ -134,18 +136,37 @@ __device__ __forceinline__ uint32_t j_find(const long long* __restrict__ tkeys, 
     }
 }
 
+// One key row as the tables hold it, loaded once per row.  An integer key is its value.  A float key (FK: both key columns are
+// float64, or both float32) is the canon_float_key encoding of its value, and a NaN key is an NA key: it joins NaN and NA keys
+// exactly when NA joins NA (is_na_equal).  A non-NaN float never encodes to J_EMPTY, so float keys never use the marker-key slot
+// cap + 1.  `bits` is the input's bit pattern (zero-extended), which the unique-key kernels write to the build key column.  The
+// data of a row that is not `valid` is not read.
+struct JoinKey { long long key; unsigned long long bits; bool na; };
+template <bool FK>
+__device__ __forceinline__ JoinKey load_join_key(const void* __restrict__ p, int ct, int64_t i, bool valid) {
+    if constexpr (FK) {
+        const unsigned long long b = !valid ? 0ull : ct == CT_FLOAT64 ? ((const unsigned long long*)p)[i] : ((const unsigned int*)p)[i];
+        const long long k = canon_float_key(ct == CT_FLOAT64 ? __longlong_as_double((long long)b) : (double)__uint_as_float((unsigned int)b));
+        return {k, b, !valid || k == J_EMPTY};
+    } else {
+        const long long k = valid ? load_int_as_i64(p, ct, i) : 0;
+        return {k, (unsigned long long)k, !valid};
+    }
+}
+
 // BuildHashTable: slot per distinct key, num_rows_in_group, build_row_to_group_map (= row_slot)
+template <bool FK>
 __global__ void join_insert_count_kernel(const void* key_data, int key_ctype, const uint8_t* key_valid_bytes, int64_t n,
                                          long long* tkeys, uint64_t cap, SlotInfo* info, uint32_t* row_slot, int na_equal) {
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
         uint32_t s;
-        if (key_valid_bytes && !key_valid_bytes[i]) {
+        const JoinKey jk = load_join_key<FK>(key_data, key_ctype, i, !key_valid_bytes || key_valid_bytes[i]);
+        if (jk.na) {
             if (!na_equal) { row_slot[i] = J_NONE; continue; }  // never matches: belongs to no group
             s = (uint32_t)cap;  // NA group
         } else {
-            long long key = load_int_as_i64(key_data, key_ctype, i);
-            s = key == J_EMPTY ? (uint32_t)cap + 1 : j_find_or_insert(tkeys, cap, key);
+            s = jk.key == J_EMPTY ? (uint32_t)cap + 1 : j_find_or_insert(tkeys, cap, jk.key);
         }
         row_slot[i] = s;
         atomicAdd(&info[s].cnt, 1u);
@@ -174,17 +195,16 @@ __global__ void join_fill_groups_kernel(const uint32_t* row_slot, int64_t n, con
 // mode 0: inner / outer join; 1: anti join (a probe row goes out, once and with NULL build columns, iff it has NO match:
 // the is_anti_join template of the reference's probe, _join.cpp:763-767); 2: mark join (every probe row goes out once, without
 // build columns; mark[i] says whether it has a match, _join.cpp:3668-3693)
+template <bool FK>
 __global__ void join_probe_count_kernel(const void* key_data, int key_ctype, const uint8_t* key_valid, int64_t n,
                                         const long long* tkeys, uint64_t cap, const SlotInfo* info, int probe_outer,
                                         uint32_t* pslot, uint32_t* pcnt, int na_equal, int mode, uint8_t* mark) {
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
         uint32_t s;
-        if (!bit_valid(key_valid, i)) s = na_equal ? (uint32_t)cap : J_NONE;
-        else {
-            long long key = load_int_as_i64(key_data, key_ctype, i);
-            s = key == J_EMPTY ? (uint32_t)cap + 1 : j_find(tkeys, cap, key);
-        }
+        const JoinKey jk = load_join_key<FK>(key_data, key_ctype, i, bit_valid(key_valid, i));
+        if (jk.na) s = na_equal ? (uint32_t)cap : J_NONE;
+        else s = jk.key == J_EMPTY ? (uint32_t)cap + 1 : j_find(tkeys, cap, jk.key);
         uint32_t c = s == J_NONE ? 0 : info[s].cnt;
         if (c == 0) s = J_NONE;
         if (mode == 1) { pslot[i] = J_NONE; pcnt[i] = c ? 0u : 1u; continue; }
@@ -342,6 +362,7 @@ __device__ __forceinline__ void store_sized(void* dst, int64_t d, unsigned long 
         default: ((uint8_t*)dst)[d] = (uint8_t)v; break;
     }
 }
+template <bool FK>
 __global__ void __launch_bounds__(256) join_probe_fast_kernel(const __grid_constant__ FastProbeArgs a) {
     // tile = 1024 probe rows per CTA iteration (4 per thread); ONE global cursor atomic per tile (a cursor atomic per
     // warp serialises on a single L2 address: measured 117 ms for 1e9 probe rows, dominated by that atomic)
@@ -354,17 +375,19 @@ __global__ void __launch_bounds__(256) join_probe_fast_kernel(const __grid_const
     const int64_t n_tiles = (a.n_probe + TILE - 1) / TILE;
     for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
         long long key[R];
+        unsigned long long bits[R];  // the probe key's bit pattern: the build key column's value on a match
         uint32_t brow[R];
         unsigned int rank[R];
         bool match[R], kvalid[R];
 #pragma unroll
         for (int r = 0; r < R; r++) {
             const int64_t i = t * TILE + r * 256 + threadIdx.x;
-            match[r] = false; kvalid[r] = true; key[r] = 0; brow[r] = 0;
+            match[r] = false; kvalid[r] = true; key[r] = 0; bits[r] = 0; brow[r] = 0;
             if (i < a.n_probe) {
                 kvalid[r] = bit_valid(a.key_valid, i);
-                key[r] = load_int_as_i64(a.key_data, a.key_ctype, i);
-                if (!kvalid[r]) { if (a.na_equal) { Slot16 e = a.slots[a.cap]; match[r] = e.cnt > 0; brow[r] = e.first; } }
+                const JoinKey jk = load_join_key<FK>(a.key_data, a.key_ctype, i, true);  // bits under a NULL too: the output's validity hides them
+                key[r] = jk.key; bits[r] = jk.bits;
+                if (!kvalid[r] || jk.na) { if (a.na_equal) { Slot16 e = a.slots[a.cap]; match[r] = e.cnt > 0; brow[r] = e.first; } }
                 else if (key[r] == J_EMPTY) { Slot16 e = a.slots[a.cap + 1]; match[r] = e.cnt > 0; brow[r] = e.first; }
                 else {
                     uint64_t s = j_hash_slot(key[r], mask);
@@ -402,7 +425,7 @@ __global__ void __launch_bounds__(256) join_probe_fast_kernel(const __grid_const
             const unsigned long long* fields = a.bpack + (size_t)brow[r] * a.n_fields;
             for (int k2 = 0; k2 < a.n_b; k2++) {
                 int f = a.b_field[k2];
-                unsigned long long v = f < 0 ? (unsigned long long)key[r] : __ldg(fields + f);
+                unsigned long long v = f < 0 ? bits[r] : __ldg(fields + f);
                 store_sized(a.ob_data[k2], orow, v, a.b_size[k2]);
                 if (a.ob_valid[k2]) a.ob_valid[k2][orow] = f < 0 ? (kvalid[r] ? 1 : 0) : (a.b_valid[k2] ? a.b_valid[k2][brow[r]] : 1);
             }
@@ -431,17 +454,21 @@ struct InlineProbeArgs {
     unsigned long long* ob[4];
     const unsigned long long* p[J_INL_MAX_P];  // kept probe columns (the key column included when kept)
     unsigned long long* op[J_INL_MAX_P];
+    int na_equal;                  // float64 keys: a NaN probe key looks up the NA slot cap
 };
 // Direct build of the Slot32 table (no separate key table / slot-info / CSR passes): one random 32-byte sector per build row.
 // A row claims its slot with a CAS on the key word, counts itself in the slot and, when it is the first row of that key,
 // writes the payload.  A second row of any key raises *dup: the host then falls back to the general build (CSR groups).
+// Float64 keys (FK) are stored as their canon_float_key encoding; a NaN row takes the NA slot cap under na_equal (the marker
+// slot's scheme: the key word stays the free-slot pattern) and belongs to no group otherwise.
 __global__ void join_fill_slots32_kernel(Slot32* slots, uint64_t n_slots) {
     uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
     const ulonglong4 e = make_ulonglong4((unsigned long long)J_EMPTY, 0ull, 0ull, 0ull);
     for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < n_slots; s += stride) reinterpret_cast<ulonglong4*>(slots)[s] = e;
 }
+template <bool FK>
 __global__ void __launch_bounds__(256) join_build_inline_kernel(const long long* __restrict__ keys, const unsigned long long* __restrict__ f0, const unsigned long long* __restrict__ f1,
-                                                                int64_t n, int64_t row0, Slot32* slots, uint64_t cap, int* dup) {
+                                                                int64_t n, int64_t row0, Slot32* slots, uint64_t cap, int* dup, int na_equal) {
     constexpr int R = 4;
     const uint64_t mask = cap - 1;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x * R;
@@ -449,16 +476,21 @@ __global__ void __launch_bounds__(256) join_build_inline_kernel(const long long*
         long long key[R], k0[R];
         uint64_t s[R];
 #pragma unroll
-        for (int r = 0; r < R; r++) { const int64_t i = i0 + r * 256; key[r] = i < n ? __ldcs(keys + i) : 0; }
+        for (int r = 0; r < R; r++) {
+            const int64_t i = i0 + r * 256;
+            key[r] = i < n ? __ldcs(keys + i) : 0;
+            if constexpr (FK) key[r] = canon_float_key(__longlong_as_double(key[r]));
+        }
 #pragma unroll
         for (int r = 0; r < R; r++) {  // the R first probes are in flight together
-            s[r] = key[r] == J_EMPTY ? cap + 1 : j_hash_slot(key[r], mask);
+            s[r] = key[r] == J_EMPTY ? (FK ? cap : cap + 1) : j_hash_slot(key[r], mask);
             k0[r] = __ldcg(&slots[s[r]].key);
         }
 #pragma unroll
         for (int r = 0; r < R; r++) {
             const int64_t i = i0 + r * 256;
             if (i >= n) continue;
+            if (FK && key[r] == J_EMPTY && !na_equal) continue;  // a NaN key that never matches
             bool won = false;  // this row claimed a free slot (it is the first row of its key)
             if (key[r] != J_EMPTY) {
                 long long k = k0[r];
@@ -497,7 +529,9 @@ __device__ __forceinline__ void ld_slot32(const Slot32* p, unsigned long long& w
     asm volatile("ld.global.nc.v2.u64 {%0, %1}, [%4];\n\tld.global.nc.v2.u64 {%2, %3}, [%4+16];"
                  : "=l"(w0), "=l"(w1), "=l"(w2), "=l"(w3) : "l"(p));
 }
-template <int NF, int NPK>
+// Float64 keys (FK): the slots hold canon_float_key encodings.  A NaN probe key looks up the NA slot cap under na_equal and
+// otherwise the marker slot cap + 1, which float keys leave empty.  The build key column gets the probe key's bits.
+template <bool FK, int NF, int NPK>
 __global__ void __launch_bounds__(256) join_probe_inline_kernel(const __grid_constant__ InlineProbeArgs a) {
     constexpr int R = 4, NW = 8, TILE = 256 * R;
     __shared__ unsigned int wcnt[R * NW];
@@ -507,7 +541,7 @@ __global__ void __launch_bounds__(256) join_probe_inline_kernel(const __grid_con
     const uint64_t mask = a.cap - 1;
     const int64_t n_tiles = (a.n_probe + TILE - 1) / TILE;
     for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        long long key[R];
+        long long key[R], ck[R];  // the probe key's bits; its table key
         unsigned long long pv[NPK][R], f0[R], f1[R];
         unsigned int rank[R];
         bool match[R];
@@ -516,6 +550,7 @@ __global__ void __launch_bounds__(256) join_probe_inline_kernel(const __grid_con
             const int64_t i = t * TILE + r * 256 + threadIdx.x;
             const bool in = i < a.n_probe;
             key[r] = in ? __ldcs(a.key + i) : 0;
+            ck[r] = FK ? canon_float_key(__longlong_as_double(key[r])) : key[r];
 #pragma unroll
             for (int c = 0; c < NPK; c++) pv[c][r] = in ? __ldcs(a.p[c] + i) : 0ull;
         }
@@ -525,7 +560,7 @@ __global__ void __launch_bounds__(256) join_probe_inline_kernel(const __grid_con
         unsigned long long w0[R], w1[R], w2[R], w3[R];
 #pragma unroll
         for (int r = 0; r < R; r++) {
-            sl[r] = key[r] == J_EMPTY ? a.cap + 1 : j_hash_slot(key[r], mask);
+            sl[r] = ck[r] == J_EMPTY ? (FK && a.na_equal ? a.cap : a.cap + 1) : j_hash_slot(ck[r], mask);
             ld_slot32(a.slots + sl[r], w0[r], w1[r], w2[r], w3[r]);
         }
 #pragma unroll
@@ -534,7 +569,7 @@ __global__ void __launch_bounds__(256) join_probe_inline_kernel(const __grid_con
             match[r] = false; f0[r] = 0; f1[r] = 0;
             if (i >= a.n_probe) continue;
             while (true) {
-                if ((long long)w0[r] == key[r]) {
+                if ((long long)w0[r] == ck[r]) {
                     if (NF >= 1) f0[r] = w1[r];
                     if (NF >= 2) f1[r] = w2[r];
                     match[r] = (unsigned int)(w3[r] >> 32) > 0;
@@ -585,14 +620,18 @@ __device__ __forceinline__ void bloom_masks(uint32_t h, uint32_t (&m)[8]) {
 #pragma unroll
     for (int j = 0; j < 8; j++) m[j] = 1u << ((h * salt[j]) >> 27);
 }
+// Float keys (FK): the bloom filter hashes the table key (canon_float_key), and min / max are canon_float_ordered of it, over the
+// keys that are neither NA nor NaN.
+template <bool FK>
 __global__ void join_bloom_add_kernel(const void* key_data, int key_ctype, const uint8_t* key_valid_bytes, int64_t n, uint32_t* bloom, uint64_t n_blocks,
                                       long long* minmax) {
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     long long mn = INT64_MAX, mx = INT64_MIN;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
-        if (key_valid_bytes && !key_valid_bytes[i]) continue;
-        const long long key = load_int_as_i64(key_data, key_ctype, i);
-        mn = key < mn ? key : mn; mx = key > mx ? key : mx;
+        const JoinKey jk = load_join_key<FK>(key_data, key_ctype, i, !key_valid_bytes || key_valid_bytes[i]);
+        if (jk.na) continue;
+        const long long key = jk.key, ord = FK ? canon_float_ordered(key) : key;
+        mn = ord < mn ? ord : mn; mx = ord > mx ? ord : mx;
         const uint64_t h = xxh3_64_short((uint64_t)key, 8, SEED_HASH_JOIN);
         uint32_t m[8];
         bloom_masks((uint32_t)h, m);
@@ -606,15 +645,17 @@ __global__ void join_bloom_add_kernel(const void* key_data, int key_ctype, const
     }
     if ((threadIdx.x & 31) == 0 && mn <= mx) { atomicMin(minmax, mn); atomicMax(minmax + 1, mx); }
 }
-// keep[i] = 1 iff row i can still find a partner: key not NA, inside [min, max] of the build keys, bloom hit
+// keep[i] = 1 iff row i can still find a partner: key not NA (nor NaN), inside [min, max] of the build keys, bloom hit
+template <bool FK>
 __global__ void join_runtime_filter_kernel(const void* key_data, int key_ctype, const uint8_t* key_valid, int64_t n, const uint32_t* bloom, uint64_t n_blocks,
                                            long long mn, long long mx, int use_minmax, int use_bloom, uint8_t* keep) {
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
         bool k = bit_valid(key_valid, i);
         if (k) {
-            const long long key = load_int_as_i64(key_data, key_ctype, i);
-            if (use_minmax && (key < mn || key > mx)) k = false;
+            const JoinKey jk = load_join_key<FK>(key_data, key_ctype, i, true);
+            const long long key = jk.key, ord = FK ? canon_float_ordered(key) : key;
+            if (jk.na || (use_minmax && (ord < mn || ord > mx))) k = false;  // NaN, or outside the bounds
             if (k && use_bloom) {
                 const uint64_t h = xxh3_64_short((uint64_t)key, 8, SEED_HASH_JOIN);
                 uint32_t m[8];
@@ -652,6 +693,23 @@ struct GrowCol {  // growable device column (geometric growth, copy on grow)
     void reserve(size_t n) { if (n > buf.bytes) { B200_REQUIRE(used == 0, "internal: reserve after append"); buf.alloc(n); } }
 };
 
+static const char* ctype_name(int ct) {
+    switch (ct) {
+        case CT_INT8: return "int8"; case CT_UINT8: return "uint8"; case CT_INT16: return "int16"; case CT_UINT16: return "uint16";
+        case CT_INT32: return "int32"; case CT_UINT32: return "uint32"; case CT_INT64: return "int64"; case CT_UINT64: return "uint64";
+        case CT_FLOAT32: return "float32"; case CT_FLOAT64: return "float64"; case CT_BOOL: return "bool"; case CT_DATE: return "date";
+        case CT_DATETIME: return "datetime"; case CT_TIMEDELTA: return "timedelta"; default: return "unknown";
+    }
+}
+// f(std::integral_constant<int, v>) for the one v in [0, N) equal to `v`: the kernel instantiation a runtime argument selects
+template <typename F, int... I> void with_int_seq(int v, F&& f, std::integer_sequence<int, I...>) {
+    ((v == I ? f(std::integral_constant<int, I>{}) : void()), ...);
+}
+template <int N, typename F> void with_int(int v, F&& f) {
+    B200_REQUIRE(v >= 0 && v < N, "internal: no kernel instantiation for this argument");
+    with_int_seq(v, f, std::make_integer_sequence<int, N>{});
+}
+
 class JoinState {
    public:
     int device; cudaStream_t stream; int sms;
@@ -659,6 +717,7 @@ class JoinState {
     int n_b, n_p;
     bool build_outer, probe_outer;
     bool na_equal = false;  // is_na_equal of the reference's HashJoinState
+    bool float_key = false; // float64 or float32 key columns: every key kernel runs its FK instantiation
     int64_t output_batch_size;
     // build side
     std::vector<GrowCol> bcol, bvalid;  // data; validity as one byte per row (empty when the column has none so far)
@@ -699,7 +758,7 @@ class JoinState {
         B200_REQUIRE(nb >= 1 && np >= 0 && nb <= J_MAX_COLS && np <= J_MAX_COLS, "b200 join: between 1 and 32 columns per side");
         b_ct.assign(bct, bct + nb); b_at.assign(bat, bat + nb);
         for (int c = 0; c < nb; c++) B200_REQUIRE(ctype_size(b_ct[c]) > 0, "b200 join: unsupported build column dtype");
-        B200_REQUIRE(!ctype_is_float(b_ct[0]), "b200 join: key columns must be integer/date typed");
+        float_key = ctype_is_float(b_ct[0]);
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
         sms = num_sms(device);
         bcol.resize(nb); bvalid.resize(nb); b_has_valid.assign(nb, false);
@@ -714,12 +773,24 @@ class JoinState {
         B200_REQUIRE(np >= 1 && np <= J_MAX_COLS, "b200 join: between 1 and 32 columns per side");
         p_ct.assign(pct, pct + np); p_at.assign(pat, pat + np); n_p = np;
         for (int c = 0; c < np; c++) B200_REQUIRE(ctype_size(p_ct[c]) > 0, "b200 join: unsupported probe column dtype");
-        B200_REQUIRE(!ctype_is_float(p_ct[0]), "b200 join: key columns must be integer/date typed");
+        require_key_type(p_ct[0], "probe");
         B200_REQUIRE(ctype_size(b_ct[0]) == ctype_size(p_ct[0]), "b200 join: build and probe key widths differ");
         out_data.resize(n_b + np); out_vbytes.resize(n_b + np); out_bitmap.resize(n_b + np);
         if ((int)stage_data.size() < std::max(n_b, np)) { stage_data.resize(std::max(n_b, np)); stage_valid.resize(std::max(n_b, np)); }
     }
     ~JoinState() { cudaSetDevice(device); scratch_set_stream(stream); cudaStreamSynchronize(stream); pinned_release(h_word, 8); }
+
+    // A float key joins a float key of the same type only (integer keys keep their width rule)
+    void require_key_type(int ct, const char* what) const {
+        if (float_key || ctype_is_float(ct))
+            B200_REQUIRE(ct == b_ct[0], std::string("b200 join: the ") + what + " key column is " + ctype_name(ct) + " and the build key column is " +
+                                            ctype_name(b_ct[0]) + "; float keys join float keys of the same type");
+    }
+    // f(std::bool_constant<FK>): the instantiation of a key kernel for this join's key type
+    template <typename F> void with_key(F&& f) const {
+        if (float_key) f(std::true_type{});
+        else f(std::false_type{});
+    }
 
     int grid_for(int64_t n) const { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sms * 8)); }
     const uint8_t* build_valid(int c) const { return b_has_valid[c] ? bvalid[c].buf.as<uint8_t>() : nullptr; }
@@ -752,8 +823,10 @@ class JoinState {
         const long long init[2] = {INT64_MAX, INT64_MIN};
         B200_CUDA(cudaMemcpyAsync(d_minmax.p, init, 16, cudaMemcpyHostToDevice, stream));
         if (n_build > 0) {
-            join_bloom_add_kernel<<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], build_valid(0), n_build,
-                                                                        d_bloom.as<uint32_t>(), bloom_blocks, d_minmax.as<long long>());
+            with_key([&](auto fk) {
+                join_bloom_add_kernel<fk><<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], build_valid(0), n_build,
+                                                                                d_bloom.as<uint32_t>(), bloom_blocks, d_minmax.as<long long>());
+            });
             launches++;
             B200_CUDA(cudaGetLastError());
         }
@@ -765,13 +838,17 @@ class JoinState {
     void runtime_filter(const b200_table* t, int key_col, bool use_minmax, bool use_bloom, uint8_t* keep) {
         B200_REQUIRE(t->device == device, "b200 join: runtime_filter takes a device-resident table on the state's device");
         B200_REQUIRE(key_col >= 0 && key_col < t->n_cols, "b200 join: runtime_filter: bad key column");
-        B200_REQUIRE(ctype_size(t->cols[key_col].c_type) == ctype_size(b_ct[0]) && !ctype_is_float(t->cols[key_col].c_type), "b200 join: runtime_filter: key column type differs from the build key");
+        require_key_type(t->cols[key_col].c_type, "runtime_filter");
+        B200_REQUIRE(ctype_size(t->cols[key_col].c_type) == ctype_size(b_ct[0]), "b200 join: runtime_filter: key column type differs from the build key");
         if (!d_bloom.p) build_filter(0);
         B200_CUDA(cudaSetDevice(device));
         const int64_t n = t->n_rows;
         if (n == 0) return;
-        join_runtime_filter_kernel<<<grid_for(n), 256, 0, stream>>>(t->cols[key_col].data, t->cols[key_col].c_type, t->cols[key_col].validity, n, d_bloom.as<uint32_t>(),
-                                                                   bloom_blocks, key_min, key_max, use_minmax ? 1 : 0, use_bloom ? 1 : 0, keep);
+        with_key([&](auto fk) {
+            join_runtime_filter_kernel<fk><<<grid_for(n), 256, 0, stream>>>(t->cols[key_col].data, t->cols[key_col].c_type, t->cols[key_col].validity, n,
+                                                                           d_bloom.as<uint32_t>(), bloom_blocks, key_min, key_max, use_minmax ? 1 : 0,
+                                                                           use_bloom ? 1 : 0, keep);
+        });
         launches++;
         B200_CUDA(cudaGetLastError());
         filter_rows_in += n;
@@ -843,9 +920,11 @@ class JoinState {
         dup.alloc(4);
         B200_CUDA(cudaMemsetAsync(dup.p, 0, 4, stream));
         join_fill_slots32_kernel<<<grid_for((int64_t)n_slots), 256, 0, stream>>>(d_slots32.as<Slot32>(), n_slots);
-        join_build_inline_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>((n_build + 1023) / 1024, (int64_t)sms * 8)), 256, 0, stream>>>(bcol[0].buf.as<long long>(), nf > 0 ? bcol[1].buf.as<unsigned long long>() : nullptr,
-                                                                       nf > 1 ? bcol[2].buf.as<unsigned long long>() : nullptr, n_build, 0, d_slots32.as<Slot32>(), cap,
-                                                                       dup.as<int>());
+        with_key([&](auto fk) {
+            join_build_inline_kernel<fk><<<(int)std::max<int64_t>(1, std::min<int64_t>((n_build + 1023) / 1024, (int64_t)sms * 8)), 256, 0, stream>>>(
+                bcol[0].buf.as<long long>(), nf > 0 ? bcol[1].buf.as<unsigned long long>() : nullptr, nf > 1 ? bcol[2].buf.as<unsigned long long>() : nullptr,
+                n_build, 0, d_slots32.as<Slot32>(), cap, dup.as<int>(), na_equal ? 1 : 0);
+        });
         launches += 2;
         B200_CUDA(cudaGetLastError());
         if (read_word(dup.as<int>()) != 0) { d_slots32.release(); return false; }  // duplicate build keys
@@ -888,8 +967,10 @@ class JoinState {
         d_row_slot.alloc((size_t)std::max<int64_t>(n_build, 1) * 4);
         launches++;
         if (n_build > 0) {
-            join_insert_count_kernel<<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], build_valid(0),
-                                                                           n_build, d_tkeys.as<long long>(), cap, d_info.as<SlotInfo>(), d_row_slot.as<uint32_t>(), na_equal ? 1 : 0);
+            with_key([&](auto fk) {
+                join_insert_count_kernel<fk><<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], build_valid(0), n_build, d_tkeys.as<long long>(), cap,
+                                                                                   d_info.as<SlotInfo>(), d_row_slot.as<uint32_t>(), na_equal ? 1 : 0);
+            });
             d_cnt_multi.alloc(n_slots * 4);
             join_slot_counts_kernel<<<grid_for((int64_t)n_slots), 256, 0, stream>>>(d_info.as<SlotInfo>(), n_slots, d_cnt_multi.as<uint32_t>());
             launches += 2;
@@ -974,17 +1055,17 @@ class JoinState {
         if (inl) {
             InlineProbeArgs ia{};
             ia.n_probe = n; ia.key = (const long long*)data[0]; ia.slots = d_slots32.as<Slot32>(); ia.cap = cap;
-            ia.cursor = d_cursor.as<unsigned long long>(); ia.n_b = nkb;
+            ia.cursor = d_cursor.as<unsigned long long>(); ia.n_b = nkb; ia.na_equal = na_equal ? 1 : 0;
             for (int k = 0; k < (int)cols.size(); k++) {
                 if (cols[k].is_b) { ia.b_field[k] = cols[k].src - 1; ia.ob[k] = out_data[k].as<unsigned long long>(); }
                 else { ia.p[k - nkb] = (const unsigned long long*)data[cols[k].src]; ia.op[k - nkb] = out_data[k].as<unsigned long long>(); }
             }
-            const int nf = n_b - 1;
-#define B200_INL(NF, NPK) join_probe_inline_kernel<NF, NPK><<<gridp, 256, 0, stream>>>(ia)
-#define B200_INL_NF(NF) do { switch (nkp) { case 1: B200_INL(NF, 1); break; case 2: B200_INL(NF, 2); break; case 3: B200_INL(NF, 3); break; default: B200_INL(NF, 4); break; } } while (0)
-            if (nf <= 0) B200_INL_NF(0); else if (nf == 1) B200_INL_NF(1); else B200_INL_NF(2);
-#undef B200_INL_NF
-#undef B200_INL
+            // <FK, NF = build payload columns (0..2), NPK = kept probe columns (1..4)>
+            with_key([&](auto fk) {
+                with_int<3>(n_b - 1, [&](auto nf) {
+                    with_int<J_INL_MAX_P>(nkp - 1, [&](auto npk) { join_probe_inline_kernel<fk, nf, npk + 1><<<gridp, 256, 0, stream>>>(ia); });
+                });
+            });
             inline_probes++;
         } else {
             if (!d_slots16.p) setup_slot16();
@@ -1003,7 +1084,7 @@ class JoinState {
                     f.op_data[j] = out_data[k].p; f.op_valid[j] = out_valid(cols, k);
                 }
             }
-            join_probe_fast_kernel<<<gridp, 256, 0, stream>>>(f);
+            with_key([&](auto fk) { join_probe_fast_kernel<fk><<<gridp, 256, 0, stream>>>(f); });
         }
         launches++; fast_probes++;
         B200_CUDA(cudaGetLastError());
@@ -1019,9 +1100,11 @@ class JoinState {
         d_pslot.ensure((size_t)(n + 1) * 4); d_pcnt.ensure((size_t)(n + 1) * 4); d_poff.ensure((size_t)(n + 2) * 8);
         if (n > 0) {
             if (mark) { d_mark.ensure((size_t)n + 32); d_mark_valid.ensure((size_t)(n + 7) / 8 + 32); B200_CUDA(cudaMemsetAsync(d_mark_valid.p, 0xff, (size_t)(n + 7) / 8 + 8, stream)); }
-            join_probe_count_kernel<<<grid_for(n), 256, 0, stream>>>(data[0], p_ct[0], valid[0], n, d_tkeys.as<long long>(), cap, d_info.as<SlotInfo>(),
-                                                                     probe_outer ? 1 : 0, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(), na_equal ? 1 : 0,
-                                                                     anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr);
+            with_key([&](auto fk) {
+                join_probe_count_kernel<fk><<<grid_for(n), 256, 0, stream>>>(data[0], p_ct[0], valid[0], n, d_tkeys.as<long long>(), cap, d_info.as<SlotInfo>(),
+                                                                             probe_outer ? 1 : 0, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(), na_equal ? 1 : 0,
+                                                                             anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr);
+            });
             launches++;
             B200_CUDA(cudaMemsetAsync(d_pcnt.as<uint32_t>() + n, 0, 4, stream));
             n_match = scan.run(d_pcnt.as<uint32_t>(), n + 1, d_poff.as<unsigned long long>(), stream, &launches);

@@ -144,6 +144,9 @@ int64_t b200_groupby_get_metric(void* state, int32_t which);
  * build_table_outer / probe_table_outer select right/left/full-outer semantics. `is_na_equal` is the
  * HashJoinState option of the same name: 0 (what join_state_init_py_entry constructs: NA keys never match,
  * _join.cpp:3180) or 1 (what bodo/pandas/physical/join.h:267 passes: NA joins NA, pandas merge semantics).
+ * Key columns: integer / date / time types of one width on both sides, or float64 on both sides, or float32 on both sides
+ * (a float key against any other key type is an error).  Float keys: -0.0 and 0.0 are one key, and a NaN key is an NA key
+ * (is_na_equal decides whether it joins NaN and NA keys); output columns keep the input bits.
  * n_probe_arrs may be 0: the probe schema is then taken from the first probe batch. */
 void* b200_join_state_init(int64_t operator_id, const int8_t* build_arr_c_types,
                            const int8_t* build_arr_array_types, int32_t n_build_arrs,
@@ -182,7 +185,10 @@ int b200_join_set_kind(void* state, int32_t is_mark_join, int32_t is_anti_join);
  * join can OR their filters together in place (all ranks pass the same n_bloom_blocks; b200_join_set_key_bounds installs the
  * reduced bounds).  b200_join_runtime_filter writes keep_out[i] = 1 for the rows of a DEVICE-resident table that can still find a
  * partner (key not NA, inside the bounds, bloom hit): the rows a probe-side scan may drop before they are shuffled or probed
- * (inner and build-outer joins only — an outer probe side must keep its rows). */
+ * (inner and build-outer joins only — an outer probe side must keep its rows).
+ * Bounds of float keys cover the keys that are neither NA nor NaN, as an order-preserving int64 encoding: the double's bit
+ * pattern (a float32 key widened first, -0.0 as +0.0), with bits 0..62 flipped when the sign bit is set.  int64 min / max of
+ * encodings is the encoding of the float min / max, so ranks reduce them as they reduce integer bounds. */
 int b200_join_build_filter(void* state, int64_t n_bloom_blocks, void** bloom_words_dev, int64_t* n_blocks_out, int64_t* key_min_max);
 int b200_join_set_key_bounds(void* state, int64_t key_min, int64_t key_max);
 int b200_join_runtime_filter(void* state, const b200_table* in_table, int32_t key_col, int32_t use_min_max, int32_t use_bloom,
