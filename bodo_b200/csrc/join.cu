@@ -17,6 +17,8 @@
 // bodo/pandas/physical/join.h:267): NA joins NA.  false (the default of join_state_init_py_entry, SQL semantics): rows
 // with an NA key never match — they are filtered from the build table unless it is the outer side
 // (_join.cpp:3180 filter_na_values) and only survive as NULL-extended rows of an outer join.
+// Keys: the first n_keys (1..4) columns of each side.  One key column can take the unique-key tables (Slot16 / Slot32); a
+// multi-column key always takes the CSR form, whose key table holds (tuple-hash tag, first build row) words (the _mk kernels).
 #include <algorithm>
 #include <type_traits>
 #include <utility>
@@ -669,6 +671,160 @@ __global__ void join_runtime_filter_kernel(const void* key_data, int key_ctype, 
     }
 }
 
+// ---- multi-column keys (n_keys 2..4): the key table and the key-reading kernels of the general (CSR) path ----
+// Key columns are a KeySet in key order: build validity is one byte per row (nullptr = all valid), probe validity an Arrow bitmap.
+// The key table holds one 8-byte word per slot: the 32-bit tag of the row's tuple hash in the high half, the first build row that
+// claimed the slot in the low half; MK_EMPTY (row J_NONE) is a free slot.  Slot index and tag are independent bits of the hash.
+// Two rows are one key when the tags match and every key column compares equal (build rows are complete before finalize_build,
+// so the insert compares against the occupant's row without a race).  NA (and NaN) is part of the tuple: the NA slot cap and the
+// marker slot cap + 1 stay unused.  From the slot id on, the single-key general path runs unchanged.
+constexpr unsigned long long MK_EMPTY = ~0ull;
+// One tuple in canonical form: per column the load_join_key value (0 under an NA), and bit j of `na` set when column j is NA
+struct MKRow { long long key[MAX_HASH_KEYS]; uint32_t na; };
+template <bool BYTES>  // BYTES: validity is one byte per row (build side), else a bitmap
+__device__ __forceinline__ MKRow mk_row(const KeySet& k, int64_t i) {
+    MKRow r;
+    r.na = 0;
+#pragma unroll
+    for (int j = 0; j < MAX_HASH_KEYS; j++) {
+        r.key[j] = 0;
+        if (j < k.n_keys && k.data[j]) {  // a runtime filter's absent column (data nullptr) reads as a valid 0
+            const bool v = BYTES ? (!k.valid[j] || k.valid[j][i]) : bit_valid(k.valid[j], i);
+            const JoinKey jk = ctype_is_float(k.ctype[j]) ? load_join_key<true>(k.data[j], k.ctype[j], i, v)
+                                                          : load_join_key<false>(k.data[j], k.ctype[j], i, v);
+            if (jk.na) r.na |= 1u << j;
+            else r.key[j] = jk.key;
+        }
+    }
+    return r;
+}
+__device__ __forceinline__ uint64_t mk_hash(const MKRow& r, int n_keys) {
+    uint64_t h = SEED_HASH_JOIN;
+#pragma unroll
+    for (int j = 0; j < MAX_HASH_KEYS; j++)
+        if (j < n_keys) h = mix64(h ^ (uint64_t)r.key[j]);
+    return mix64(h ^ r.na);
+}
+__device__ __forceinline__ bool mk_equal_build(const KeySet& bk, uint32_t row, const MKRow& r) {
+    const MKRow o = mk_row<true>(bk, row);
+    bool eq = o.na == r.na;
+#pragma unroll
+    for (int j = 0; j < MAX_HASH_KEYS; j++) eq = eq && (j >= bk.n_keys || o.key[j] == r.key[j]);
+    return eq;
+}
+__device__ __forceinline__ uint64_t mk_slot(uint64_t h, uint64_t mask) { return (h >> 32) & mask; }
+__device__ __forceinline__ uint32_t mk_tag(uint64_t h) { return (uint32_t)h; }
+
+// join_insert_count_kernel for a multi-column key: same outputs (row_slot, info[s].cnt, info[s].first)
+__global__ void join_insert_count_mk_kernel(const KeySet bk, int64_t n, unsigned long long* table, uint64_t cap, SlotInfo* info,
+                                            uint32_t* row_slot, int na_equal) {
+    const uint64_t mask = cap - 1;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
+        const MKRow r = mk_row<true>(bk, i);
+        if (r.na && !na_equal) { row_slot[i] = J_NONE; continue; }  // never matches: belongs to no group
+        const uint64_t h = mk_hash(r, bk.n_keys);
+        const unsigned long long mine = ((unsigned long long)mk_tag(h) << 32) | (uint32_t)i;
+        uint64_t s = mk_slot(h, mask);
+        while (true) {
+            unsigned long long w = __ldcg(table + s);
+            if (w == MK_EMPTY) {
+                w = atomicCAS(table + s, MK_EMPTY, mine);
+                if (w == MK_EMPTY) break;  // claimed
+            }
+            if ((uint32_t)(w >> 32) == mk_tag(h) && mk_equal_build(bk, (uint32_t)w, r)) break;
+            s = (s + 1) & mask;
+        }
+        row_slot[i] = (uint32_t)s;
+        atomicAdd(&info[s].cnt, 1u);
+        info[s].first = (uint32_t)i;  // any row of the group; exact when cnt == 1
+    }
+}
+// join_probe_count_kernel for a multi-column key: same outputs (pslot, pcnt, mark) in modes 0, 1 and 2
+__global__ void join_probe_count_mk_kernel(const KeySet pk, const KeySet bk, int64_t n, const unsigned long long* __restrict__ table,
+                                           uint64_t cap, const SlotInfo* info, int probe_outer, uint32_t* pslot, uint32_t* pcnt,
+                                           int na_equal, int mode, uint8_t* mark) {
+    const uint64_t mask = cap - 1;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
+        const MKRow r = mk_row<false>(pk, i);
+        uint32_t s = J_NONE;
+        if (!r.na || na_equal) {
+            const uint64_t h = mk_hash(r, pk.n_keys);
+            for (uint64_t t = mk_slot(h, mask);; t = (t + 1) & mask) {
+                const unsigned long long w = __ldg(table + t);
+                if (w == MK_EMPTY) break;
+                if ((uint32_t)(w >> 32) == mk_tag(h) && mk_equal_build(bk, (uint32_t)w, r)) { s = (uint32_t)t; break; }
+            }
+        }
+        uint32_t c = s == J_NONE ? 0 : info[s].cnt;
+        if (c == 0) s = J_NONE;
+        if (mode == 1) { pslot[i] = J_NONE; pcnt[i] = c ? 0u : 1u; continue; }
+        if (mode == 2) { pslot[i] = J_NONE; pcnt[i] = 1u; mark[i] = c ? 1 : 0; continue; }
+        pslot[i] = s;
+        pcnt[i] = c ? c : (probe_outer ? 1u : 0u);
+    }
+}
+// Runtime filter of a multi-column key: one bloom filter over the tuple hash of the build rows that belong to a group, and min / max
+// per key column over its non-NA values (canon_float_ordered for float columns).  minmax[2j], minmax[2j + 1]: column j.
+__global__ void join_bloom_add_mk_kernel(const KeySet bk, int64_t n, int na_equal, uint32_t* bloom, uint64_t n_blocks, long long* minmax) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    long long mn[MAX_HASH_KEYS], mx[MAX_HASH_KEYS];
+#pragma unroll
+    for (int j = 0; j < MAX_HASH_KEYS; j++) { mn[j] = INT64_MAX; mx[j] = INT64_MIN; }
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
+        const MKRow r = mk_row<true>(bk, i);
+        if (r.na && !na_equal) continue;  // in no group
+#pragma unroll
+        for (int j = 0; j < MAX_HASH_KEYS; j++) {
+            if (j >= bk.n_keys || (r.na >> j & 1)) continue;
+            const long long ord = ctype_is_float(bk.ctype[j]) ? canon_float_ordered(r.key[j]) : r.key[j];
+            mn[j] = ord < mn[j] ? ord : mn[j]; mx[j] = ord > mx[j] ? ord : mx[j];
+        }
+        const uint64_t h = mk_hash(r, bk.n_keys);
+        uint32_t m[8];
+        bloom_masks((uint32_t)h, m);
+        uint32_t* blk = bloom + (size_t)(__umul64hi(h, n_blocks)) * 8;
+#pragma unroll
+        for (int j = 0; j < 8; j++) atomicOr(blk + j, m[j]);
+    }
+#pragma unroll
+    for (int j = 0; j < MAX_HASH_KEYS; j++) {
+        for (int d = 16; d; d >>= 1) {
+            const long long a = __shfl_xor_sync(0xffffffffu, mn[j], d), b = __shfl_xor_sync(0xffffffffu, mx[j], d);
+            mn[j] = a < mn[j] ? a : mn[j]; mx[j] = b > mx[j] ? b : mx[j];
+        }
+        if ((threadIdx.x & 31) == 0 && j < bk.n_keys && mn[j] <= mx[j]) { atomicMin(minmax + 2 * j, mn[j]); atomicMax(minmax + 2 * j + 1, mx[j]); }
+    }
+}
+struct MKBounds { long long v[2 * MAX_HASH_KEYS]; };
+// keep[i] = 1 iff probe row i can still find a partner.  A column absent from the probe table has pk.data[j] == nullptr; the host
+// clears its use_minmax bit and use_bloom.  An NA column drops the row unless NA joins NA; then it skips the bounds and is hashed
+// into the bloom test as the build side hashes it.
+__global__ void join_runtime_filter_mk_kernel(const KeySet pk, int64_t n, int na_equal, const uint32_t* bloom, uint64_t n_blocks,
+                                              const MKBounds b, uint32_t use_minmax, int use_bloom, uint8_t* keep) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
+        const MKRow r = mk_row<false>(pk, i);
+        bool k = !r.na || na_equal;
+#pragma unroll
+        for (int j = 0; j < MAX_HASH_KEYS; j++) {
+            if (j >= pk.n_keys || !(use_minmax >> j & 1) || (r.na >> j & 1)) continue;
+            const long long ord = ctype_is_float(pk.ctype[j]) ? canon_float_ordered(r.key[j]) : r.key[j];
+            if (ord < b.v[2 * j] || ord > b.v[2 * j + 1]) k = false;
+        }
+        if (k && use_bloom) {
+            const uint64_t h = mk_hash(r, pk.n_keys);
+            uint32_t m[8];
+            bloom_masks((uint32_t)h, m);
+            const uint4* blk = reinterpret_cast<const uint4*>(bloom + (size_t)(__umul64hi(h, n_blocks)) * 8);
+            const uint4 lo = __ldg(blk), hi = __ldg(blk + 1);
+            k = (lo.x & m[0]) && (lo.y & m[1]) && (lo.z & m[2]) && (lo.w & m[3]) && (hi.x & m[4]) && (hi.y & m[5]) && (hi.z & m[6]) && (hi.w & m[7]);
+        }
+        keep[i] = k ? 1 : 0;
+    }
+}
+
 // ================================================================================================
 // When `buf` holds fewer than `need` bytes, replaces it by a buffer of max(need, alloc) bytes that keeps its first `keep` bytes.
 static void grow_keep(DevBuf& buf, size_t need, size_t keep, cudaStream_t st, size_t alloc = 0) {
@@ -717,7 +873,8 @@ class JoinState {
     int n_b, n_p;
     bool build_outer, probe_outer;
     bool na_equal = false;  // is_na_equal of the reference's HashJoinState
-    bool float_key = false; // float64 or float32 key columns: every key kernel runs its FK instantiation
+    int n_keys = 1;         // key columns: the first n_keys of each side; more than one always takes the CSR form (the _mk kernels)
+    bool float_key = false; // float64 or float32 key column (n_keys == 1): every key kernel runs its FK instantiation
     int64_t output_batch_size;
     // build side
     std::vector<GrowCol> bcol, bvalid;  // data; validity as one byte per row (empty when the column has none so far)
@@ -739,7 +896,7 @@ class JoinState {
     // runtime join filter, built on demand from the build keys
     DevBuf d_bloom, d_minmax;
     uint64_t bloom_blocks = 0;
-    long long key_min = INT64_MAX, key_max = INT64_MIN;
+    long long key_bounds[2 * MAX_HASH_KEYS];  // min, max of key column 0, then of column 1, ...
     int64_t filter_rows_in = 0, filter_rows_kept = 0;
     void* h_word = nullptr;  // pinned mirror of read_word
     int64_t fast_probes = 0;
@@ -751,14 +908,17 @@ class JoinState {
     int64_t launches = 0, probe_rows = 0, out_rows_total = 0;
     bool tail_emitted = false;
 
-    JoinState(const int8_t* bct, const int8_t* bat, int nb, const int8_t* pct, const int8_t* pat, int np, uint64_t n_keys,
+    JoinState(const int8_t* bct, const int8_t* bat, int nb, const int8_t* pct, const int8_t* pat, int np, uint64_t nk,
               bool bo, bool po, bool na_eq, int64_t obs, int dev, int64_t expected_build_rows, cudaStream_t st)
         : device(dev), stream(st), n_b(nb), n_p(0), build_outer(bo), probe_outer(po), na_equal(na_eq), output_batch_size(obs) {
-        B200_REQUIRE(n_keys == 1, "b200 join: exactly one key column is supported (multi-key is a 'next' row, SURVEY.md §8f)");
+        B200_REQUIRE(nk >= 1 && nk <= MAX_HASH_KEYS, "b200 join: between 1 and 4 key columns (n_keys) per side");
+        n_keys = (int)nk;
+        for (int j = 0; j < 2 * MAX_HASH_KEYS; j++) key_bounds[j] = j % 2 ? INT64_MIN : INT64_MAX;
         B200_REQUIRE(nb >= 1 && np >= 0 && nb <= J_MAX_COLS && np <= J_MAX_COLS, "b200 join: between 1 and 32 columns per side");
+        B200_REQUIRE(nb >= n_keys && (np == 0 || np >= n_keys), "b200 join: fewer columns than key columns");
         b_ct.assign(bct, bct + nb); b_at.assign(bat, bat + nb);
         for (int c = 0; c < nb; c++) B200_REQUIRE(ctype_size(b_ct[c]) > 0, "b200 join: unsupported build column dtype");
-        float_key = ctype_is_float(b_ct[0]);
+        float_key = n_keys == 1 && ctype_is_float(b_ct[0]);
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
         sms = num_sms(device);
         bcol.resize(nb); bvalid.resize(nb); b_has_valid.assign(nb, false);
@@ -773,18 +933,34 @@ class JoinState {
         B200_REQUIRE(np >= 1 && np <= J_MAX_COLS, "b200 join: between 1 and 32 columns per side");
         p_ct.assign(pct, pct + np); p_at.assign(pat, pat + np); n_p = np;
         for (int c = 0; c < np; c++) B200_REQUIRE(ctype_size(p_ct[c]) > 0, "b200 join: unsupported probe column dtype");
-        require_key_type(p_ct[0], "probe");
+        B200_REQUIRE(np >= n_keys, "b200 join: fewer columns than key columns");
+        for (int j = 0; j < n_keys; j++) require_key_type(j, p_ct[j], "probe");
         B200_REQUIRE(ctype_size(b_ct[0]) == ctype_size(p_ct[0]), "b200 join: build and probe key widths differ");
         out_data.resize(n_b + np); out_vbytes.resize(n_b + np); out_bitmap.resize(n_b + np);
         if ((int)stage_data.size() < std::max(n_b, np)) { stage_data.resize(std::max(n_b, np)); stage_valid.resize(std::max(n_b, np)); }
     }
     ~JoinState() { cudaSetDevice(device); scratch_set_stream(stream); cudaStreamSynchronize(stream); pinned_release(h_word, 8); }
 
-    // A float key joins a float key of the same type only (integer keys keep their width rule)
-    void require_key_type(int ct, const char* what) const {
-        if (float_key || ctype_is_float(ct))
-            B200_REQUIRE(ct == b_ct[0], std::string("b200 join: the ") + what + " key column is " + ctype_name(ct) + " and the build key column is " +
-                                            ctype_name(b_ct[0]) + "; float keys join float keys of the same type");
+    // Key position j: a float key joins a float key of the same type only; integer keys join integer keys of the same width (for
+    // one key column the callers check the width with their own message)
+    void require_key_type(int j, int ct, const char* what) const {
+        const std::string pos = n_keys > 1 ? "key position " + std::to_string(j) + ": " : "";
+        const std::string types = std::string("the ") + what + " key column is " + ctype_name(ct) + " and the build key column is " + ctype_name(b_ct[j]);
+        if (ctype_is_float(b_ct[j]) || ctype_is_float(ct))
+            B200_REQUIRE(ct == b_ct[j], "b200 join: " + pos + types + "; float keys join float keys of the same type");
+        if (n_keys > 1) B200_REQUIRE(ctype_size(ct) == ctype_size(b_ct[j]), "b200 join: " + pos + types + "; integer keys join integer keys of the same width");
+    }
+    KeySet build_keys() const {
+        KeySet k{};
+        k.n_keys = n_keys;
+        for (int j = 0; j < n_keys; j++) { k.data[j] = bcol[j].buf.p; k.valid[j] = build_valid(j); k.ctype[j] = b_ct[j]; }
+        return k;
+    }
+    KeySet probe_keys(const std::vector<const void*>& data, const std::vector<const uint8_t*>& valid) const {
+        KeySet k{};
+        k.n_keys = n_keys;
+        for (int j = 0; j < n_keys; j++) { k.data[j] = data[j]; k.valid[j] = valid[j]; k.ctype[j] = p_ct[j]; }
+        return k;
     }
     // f(std::bool_constant<FK>): the instantiation of a key kernel for this join's key type
     template <typename F> void with_key(F&& f) const {
@@ -812,33 +988,43 @@ class JoinState {
 
     // ---- runtime join filter ----
     // n_blocks: 32-byte bloom blocks (0 = one per 32 build rows, ~8 bits per key); ranks that will OR their filters together
-    // pass the same value.  Also computes the min / max of the (non-NA) build keys.
+    // pass the same value.  Also computes the min / max of the (non-NA) build keys, per key column.
     void build_filter(uint64_t n_blocks) {
         B200_REQUIRE(build_final, "b200 join: runtime filter before the build side was finished");
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
         bloom_blocks = n_blocks ? n_blocks : (uint64_t)n_build / 32 + 1;
         d_bloom.alloc(bloom_blocks * 32);
         B200_CUDA(cudaMemsetAsync(d_bloom.p, 0, bloom_blocks * 32, stream));
-        d_minmax.alloc(16);
-        const long long init[2] = {INT64_MAX, INT64_MIN};
-        B200_CUDA(cudaMemcpyAsync(d_minmax.p, init, 16, cudaMemcpyHostToDevice, stream));
+        const size_t mm_bytes = 16 * (size_t)n_keys;
+        d_minmax.alloc(mm_bytes);
+        long long h[2 * MAX_HASH_KEYS];
+        for (int j = 0; j < 2 * n_keys; j++) h[j] = j % 2 ? INT64_MIN : INT64_MAX;
+        B200_CUDA(cudaMemcpyAsync(d_minmax.p, h, mm_bytes, cudaMemcpyHostToDevice, stream));
         if (n_build > 0) {
-            with_key([&](auto fk) {
-                join_bloom_add_kernel<fk><<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], build_valid(0), n_build,
-                                                                                d_bloom.as<uint32_t>(), bloom_blocks, d_minmax.as<long long>());
-            });
+            if (n_keys > 1)
+                join_bloom_add_mk_kernel<<<grid_for(n_build), 256, 0, stream>>>(build_keys(), n_build, na_equal ? 1 : 0, d_bloom.as<uint32_t>(), bloom_blocks,
+                                                                                d_minmax.as<long long>());
+            else
+                with_key([&](auto fk) {
+                    join_bloom_add_kernel<fk><<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], build_valid(0), n_build,
+                                                                                    d_bloom.as<uint32_t>(), bloom_blocks, d_minmax.as<long long>());
+                });
             launches++;
             B200_CUDA(cudaGetLastError());
         }
-        long long h[2];
-        B200_CUDA(cudaMemcpyAsync(h, d_minmax.p, 16, cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaMemcpyAsync(h, d_minmax.p, mm_bytes, cudaMemcpyDeviceToHost, stream));
         B200_CUDA(cudaStreamSynchronize(stream));
-        key_min = h[0]; key_max = h[1];
+        std::copy(h, h + 2 * n_keys, key_bounds);
+    }
+    void require_one_key(const char* entry) const {
+        B200_REQUIRE(n_keys == 1, std::string("b200 join: ") + entry + " takes one key column and this join has " + std::to_string(n_keys) +
+                                      "; use " + entry + "_n");
     }
     void runtime_filter(const b200_table* t, int key_col, bool use_minmax, bool use_bloom, uint8_t* keep) {
+        require_one_key("b200_join_runtime_filter");
         B200_REQUIRE(t->device == device, "b200 join: runtime_filter takes a device-resident table on the state's device");
         B200_REQUIRE(key_col >= 0 && key_col < t->n_cols, "b200 join: runtime_filter: bad key column");
-        require_key_type(t->cols[key_col].c_type, "runtime_filter");
+        require_key_type(0, t->cols[key_col].c_type, "runtime_filter");
         B200_REQUIRE(ctype_size(t->cols[key_col].c_type) == ctype_size(b_ct[0]), "b200 join: runtime_filter: key column type differs from the build key");
         if (!d_bloom.p) build_filter(0);
         B200_CUDA(cudaSetDevice(device));
@@ -846,9 +1032,44 @@ class JoinState {
         if (n == 0) return;
         with_key([&](auto fk) {
             join_runtime_filter_kernel<fk><<<grid_for(n), 256, 0, stream>>>(t->cols[key_col].data, t->cols[key_col].c_type, t->cols[key_col].validity, n,
-                                                                           d_bloom.as<uint32_t>(), bloom_blocks, key_min, key_max, use_minmax ? 1 : 0,
+                                                                           d_bloom.as<uint32_t>(), bloom_blocks, key_bounds[0], key_bounds[1], use_minmax ? 1 : 0,
                                                                            use_bloom ? 1 : 0, keep);
         });
+        launches++;
+        B200_CUDA(cudaGetLastError());
+        filter_rows_in += n;
+    }
+    // Any key count.  key_cols[j] < 0: key column j is absent from `t`; the bounds then apply to the present columns and the bloom
+    // filter only when every column is present.  One key column: runtime_filter, or keep every row when that column is absent.
+    void runtime_filter_n(const b200_table* t, const int32_t* key_cols, int nk, const int32_t* use_minmax, bool use_bloom, uint8_t* keep) {
+        B200_REQUIRE(nk == n_keys, "b200 join: runtime_filter_n: n_keys is " + std::to_string(nk) + " and this join has " + std::to_string(n_keys) + " key columns");
+        B200_REQUIRE(t->device == device, "b200 join: runtime_filter takes a device-resident table on the state's device");
+        if (n_keys == 1) {
+            if (key_cols[0] >= 0) return runtime_filter(t, key_cols[0], use_minmax[0] != 0, use_bloom, keep);
+            B200_CUDA(cudaSetDevice(device));
+            if (t->n_rows) B200_CUDA(cudaMemsetAsync(keep, 1, (size_t)t->n_rows, stream));
+            return;
+        }
+        KeySet pk{};
+        pk.n_keys = n_keys;
+        uint32_t mm = 0;
+        bool all = true;
+        for (int j = 0; j < n_keys; j++) {
+            const int c = key_cols[j];
+            if (c < 0) { all = false; continue; }
+            B200_REQUIRE(c < t->n_cols, "b200 join: runtime_filter: bad key column");
+            require_key_type(j, t->cols[c].c_type, "runtime_filter");
+            pk.data[j] = t->cols[c].data; pk.valid[j] = t->cols[c].validity; pk.ctype[j] = t->cols[c].c_type;
+            if (use_minmax[j]) mm |= 1u << j;
+        }
+        if (!d_bloom.p) build_filter(0);
+        B200_CUDA(cudaSetDevice(device));
+        const int64_t n = t->n_rows;
+        if (n == 0) return;
+        MKBounds b;
+        std::copy(key_bounds, key_bounds + 2 * MAX_HASH_KEYS, b.v);
+        join_runtime_filter_mk_kernel<<<grid_for(n), 256, 0, stream>>>(pk, n, na_equal ? 1 : 0, d_bloom.as<uint32_t>(), bloom_blocks, b, mm,
+                                                                       use_bloom && all ? 1 : 0, keep);
         launches++;
         B200_CUDA(cudaGetLastError());
         filter_rows_in += n;
@@ -955,22 +1176,27 @@ class JoinState {
         cap = 1024;
         while (cap < 2ull * (uint64_t)n_build) cap <<= 1;
         uint64_t n_slots = cap + 2;
-        if (!mark && !anti && try_inline_build(n_slots)) {
+        // the unique-key tables (Slot32, Slot16) hold one int64 key: a multi-column key always takes the CSR form
+        if (n_keys == 1 && !mark && !anti && try_inline_build(n_slots)) {
             form = TableForm::SLOT32; inline_builds++;
             build_final = true;
             return;
         }
-        d_tkeys.alloc(n_slots * 8);
-        launch_fill_u64(d_tkeys.p, n_slots, (unsigned long long)J_EMPTY, grid_for((int64_t)n_slots), stream);
+        d_tkeys.alloc(n_slots * 8);  // int64 keys, or the multi-column key table's (tag, row) words
+        launch_fill_u64(d_tkeys.p, n_slots, n_keys > 1 ? MK_EMPTY : (unsigned long long)J_EMPTY, grid_for((int64_t)n_slots), stream);
         d_info.alloc(n_slots * sizeof(SlotInfo));
         B200_CUDA(cudaMemsetAsync(d_info.p, 0, n_slots * sizeof(SlotInfo), stream));
         d_row_slot.alloc((size_t)std::max<int64_t>(n_build, 1) * 4);
         launches++;
         if (n_build > 0) {
-            with_key([&](auto fk) {
-                join_insert_count_kernel<fk><<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], build_valid(0), n_build, d_tkeys.as<long long>(), cap,
+            if (n_keys > 1)
+                join_insert_count_mk_kernel<<<grid_for(n_build), 256, 0, stream>>>(build_keys(), n_build, d_tkeys.as<unsigned long long>(), cap,
                                                                                    d_info.as<SlotInfo>(), d_row_slot.as<uint32_t>(), na_equal ? 1 : 0);
-            });
+            else
+                with_key([&](auto fk) {
+                    join_insert_count_kernel<fk><<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], build_valid(0), n_build, d_tkeys.as<long long>(), cap,
+                                                                                       d_info.as<SlotInfo>(), d_row_slot.as<uint32_t>(), na_equal ? 1 : 0);
+                });
             d_cnt_multi.alloc(n_slots * 4);
             join_slot_counts_kernel<<<grid_for((int64_t)n_slots), 256, 0, stream>>>(d_info.as<SlotInfo>(), n_slots, d_cnt_multi.as<uint32_t>());
             launches += 2;
@@ -985,7 +1211,7 @@ class JoinState {
                 launches++;
             }
             d_cnt_multi.release(); d_fill.release(); d_row_slot.release();
-            if (n_multi == 0 && !build_outer && !probe_outer && !mark && !anti) {
+            if (n_keys == 1 && n_multi == 0 && !build_outer && !probe_outer && !mark && !anti) {
                 // every key (incl. the NA / marker groups) has exactly one build row: set up the fused probe path
                 form = TableForm::SLOT16;
                 setup_slot16();
@@ -1100,11 +1326,16 @@ class JoinState {
         d_pslot.ensure((size_t)(n + 1) * 4); d_pcnt.ensure((size_t)(n + 1) * 4); d_poff.ensure((size_t)(n + 2) * 8);
         if (n > 0) {
             if (mark) { d_mark.ensure((size_t)n + 32); d_mark_valid.ensure((size_t)(n + 7) / 8 + 32); B200_CUDA(cudaMemsetAsync(d_mark_valid.p, 0xff, (size_t)(n + 7) / 8 + 8, stream)); }
-            with_key([&](auto fk) {
-                join_probe_count_kernel<fk><<<grid_for(n), 256, 0, stream>>>(data[0], p_ct[0], valid[0], n, d_tkeys.as<long long>(), cap, d_info.as<SlotInfo>(),
-                                                                             probe_outer ? 1 : 0, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(), na_equal ? 1 : 0,
-                                                                             anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr);
-            });
+            if (n_keys > 1)
+                join_probe_count_mk_kernel<<<grid_for(n), 256, 0, stream>>>(probe_keys(data, valid), build_keys(), n, d_tkeys.as<unsigned long long>(), cap,
+                                                                            d_info.as<SlotInfo>(), probe_outer ? 1 : 0, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(),
+                                                                            na_equal ? 1 : 0, anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr);
+            else
+                with_key([&](auto fk) {
+                    join_probe_count_kernel<fk><<<grid_for(n), 256, 0, stream>>>(data[0], p_ct[0], valid[0], n, d_tkeys.as<long long>(), cap, d_info.as<SlotInfo>(),
+                                                                                 probe_outer ? 1 : 0, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(), na_equal ? 1 : 0,
+                                                                                 anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr);
+                });
             launches++;
             B200_CUDA(cudaMemsetAsync(d_pcnt.as<uint32_t>() + n, 0, 4, stream));
             n_match = scan.run(d_pcnt.as<uint32_t>(), n + 1, d_poff.as<unsigned long long>(), stream, &launches);
@@ -1262,7 +1493,7 @@ int b200_join_build_filter(void* state, int64_t n_bloom_blocks, void** bloom_wor
         s->build_filter((uint64_t)n_bloom_blocks);
         if (bloom_words_dev) *bloom_words_dev = s->d_bloom.p;
         if (n_blocks_out) *n_blocks_out = (int64_t)s->bloom_blocks;
-        if (key_min_max) { key_min_max[0] = s->key_min; key_min_max[1] = s->key_max; }
+        if (key_min_max) std::copy(s->key_bounds, s->key_bounds + 2 * s->n_keys, key_min_max);
         return 0;
     } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
 }
@@ -1270,7 +1501,20 @@ int b200_join_build_filter(void* state, int64_t n_bloom_blocks, void** bloom_wor
 int b200_join_set_key_bounds(void* state, int64_t key_min, int64_t key_max) {
     try {
         B200_REQUIRE(state, "b200 join: null state");
-        ((JoinState*)state)->key_min = key_min; ((JoinState*)state)->key_max = key_max;
+        auto* s = (JoinState*)state;
+        s->require_one_key("b200_join_set_key_bounds");
+        s->key_bounds[0] = key_min; s->key_bounds[1] = key_max;
+        return 0;
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
+}
+
+int b200_join_set_key_bounds_n(void* state, const int64_t* key_min_max, int32_t n_keys) {
+    try {
+        B200_REQUIRE(state && key_min_max, "b200 join: null argument");
+        auto* s = (JoinState*)state;
+        B200_REQUIRE(n_keys == s->n_keys, "b200 join: set_key_bounds_n: n_keys is " + std::to_string(n_keys) + " and this join has " +
+                                              std::to_string(s->n_keys) + " key columns");
+        std::copy(key_min_max, key_min_max + 2 * n_keys, s->key_bounds);
         return 0;
     } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
 }
@@ -1279,6 +1523,15 @@ int b200_join_runtime_filter(void* state, const b200_table* in_table, int32_t ke
     try {
         B200_REQUIRE(state && in_table && keep_out, "b200 join: null argument");
         ((JoinState*)state)->runtime_filter(in_table, key_col, use_min_max != 0, use_bloom != 0, keep_out);
+        return 0;
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
+}
+
+int b200_join_runtime_filter_n(void* state, const b200_table* in_table, const int32_t* key_cols, int32_t n_keys, const int32_t* use_min_max,
+                               int32_t use_bloom, uint8_t* keep_out) {
+    try {
+        B200_REQUIRE(state && in_table && key_cols && use_min_max && keep_out, "b200 join: null argument");
+        ((JoinState*)state)->runtime_filter_n(in_table, key_cols, n_keys, use_min_max, use_bloom != 0, keep_out);
         return 0;
     } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
 }

@@ -244,7 +244,9 @@ class PhysicalAggregate:
 class PhysicalJoin:
     """Hash join: sink for build batches, ProcessBatch for probe batches (join.h:58-744)."""
 
-    def __init__(self, build_key: int, probe_key: int, build_names, probe_names, how: str = "inner", **kw):
+    def __init__(self, build_key, probe_key, build_names, probe_names, how: str = "inner", **kw):
+        """build_key / probe_key: a column index, or a sequence of 1..4 indices (a multi-column key, in key order)."""
+        keys = lambda k: tuple(k) if isinstance(k, (list, tuple)) else (k,)
         build_outer = how in ("right", "outer")   # the build side is the RIGHT table (reference convention)
         probe_outer = how in ("left", "outer")
         if how == "anti":   # LEFT ANTI: probe rows without a partner (physical/join.h:151: no build columns in the output)
@@ -252,7 +254,7 @@ class PhysicalJoin:
         elif how == "mark":
             kw["is_mark_join"] = True
         kw.setdefault("is_na_equal", True)  # pandas merge semantics: NA joins NA (bodo/pandas/physical/join.h:267)
-        self.state = J.init_join_state(-1, (build_key,), (probe_key,), tuple(build_names), tuple(probe_names), build_outer, probe_outer, **kw)
+        self.state = J.init_join_state(-1, keys(build_key), keys(probe_key), tuple(build_names), tuple(probe_names), build_outer, probe_outer, **kw)
 
     def ConsumeBatch(self, batch: Table, prev: OperatorResult) -> OperatorResult:
         is_last = prev == OperatorResult.FINISHED
@@ -343,11 +345,16 @@ def groupby_agg_parquet(path: str, by, aggs: Sequence[tuple], dropna: bool = Tru
     return out
 
 
-def merge(left, right, left_on: str, right_on: str, how: str = "inner", batch_size: int = STREAMING_BATCH_SIZE, **kw):
-    """left.merge(right, left_on=..., right_on=..., how=...) through the streaming join (right = build side).
+def merge(left, right, left_on, right_on, how: str = "inner", batch_size: int = STREAMING_BATCH_SIZE, **kw):
+    """left.merge(right, left_on=..., right_on=..., how=...) through the streaming join (right = build side).  left_on / right_on:
+    a column name, or equal-length lists of 1..4 names (a multi-column key).
     Output columns: right's columns then left's columns (the reference's build-then-probe order), renamed on clashes."""
     rcols, lcols = list(right.columns), list(left.columns)
-    op = PhysicalJoin(rcols.index(right_on), lcols.index(left_on), rcols, lcols, how=how, **kw)
+    lo = [left_on] if isinstance(left_on, str) else list(left_on)
+    ro = [right_on] if isinstance(right_on, str) else list(right_on)
+    if len(lo) != len(ro):
+        raise ValueError(f"merge: len(right_on) ({len(ro)}) must equal len(left_on) ({len(lo)})")
+    op = PhysicalJoin([rcols.index(c) for c in ro], [lcols.index(c) for c in lo], rcols, lcols, how=how, **kw)
     run_pipeline(PhysicalReadPandas(right, batch_size), [], op)
     coll = ResultCollector()
     run_pipeline(PhysicalReadPandas(left, batch_size), [op], coll)

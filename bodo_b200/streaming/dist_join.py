@@ -18,7 +18,10 @@ Here, per rank (one process per GPU, torch.distributed / NCCL for the plumbing):
 
 The calls are collective, as in the reference: every rank calls build / probe the same number of times (ranks that ran out of
 input keep calling with empty batches until the is_last call, bodo/pandas/_pipeline.cpp:453-457).
-Placement is the reference's: (uint32) XXH3_64(key, SEED_HASH_PARTITION) % n_pes.
+Placement is the reference's: (uint32) XXH3_64(key, SEED_HASH_PARTITION) % n_pes, and for a multi-column key hash_keys over the
+key columns in key order (hash_combine_boost folding, what shuffle_table does with n_keys).  Known limitation of float key
+columns, per column: a numpy NaN (hashed as a value) and a nullable NA (hashed as hash_na_val) can go to different ranks, so under
+is_na_equal=True they may not meet.
 """
 
 from __future__ import annotations
@@ -150,8 +153,8 @@ class DistJoinState:
         self.filter_ready = False
         self._build_batches = []
         self.is_broadcast = False
-        self.build_key = self.local.build_key_inds[0]
-        self.probe_key = self.local.probe_key_inds[0]
+        self.build_keys = self.local.build_key_inds
+        self.probe_keys = self.local.probe_key_inds
         self.metrics = {"build_rows_in": 0, "build_rows_local": 0, "probe_rows_in": 0, "probe_rows_local": 0, "broadcast": 0}
 
     # handle / metrics pass-throughs so get_metric / delete work on both kinds of state
@@ -159,27 +162,28 @@ class DistJoinState:
     def handle(self):
         return self.local.handle
 
-    def _keys_first(self, table: Table, key: int) -> Table:
-        order = [key] + [i for i in range(table.n_cols) if i != key]
+    def _keys_first(self, table: Table, keys) -> Table:
+        order = list(keys) + [i for i in range(table.n_cols) if i not in keys]
         return table.select(order), order
 
-    def _shuffle(self, table: Table, key: int) -> Table:
-        """Rows to their owners; returns the rows this rank owns, in the table's original column order."""
+    def _shuffle(self, table: Table, keys) -> Table:
+        """Rows to their owners (hash_keys over all key columns, in key order); returns the rows this rank owns, in the table's
+        original column order."""
         import torch
 
-        kf, order = self._keys_first(to_device(table, self.device), key)
-        part, counts = partition_device(with_schema_validity(kf), 1, self.n_pes)
+        kf, order = self._keys_first(to_device(table, self.device), keys)
+        part, counts = partition_device(with_schema_validity(kf), len(keys), self.n_pes)
         torch.cuda.current_stream().synchronize()
         recv = exchange_table(part, counts, self.group)
         inv = [order.index(i) for i in range(len(order))]
         return recv.select(inv)
 
-    def _owned_only(self, table: Table, key: int) -> Table:
+    def _owned_only(self, table: Table, keys) -> Table:
         """Replicated input against a partitioned other side: keep the rows whose key this rank owns (no exchange)."""
         import torch
 
-        kf, order = self._keys_first(to_device(table, self.device), key)
-        part, counts = partition_device(with_schema_validity(kf), 1, self.n_pes)
+        kf, order = self._keys_first(to_device(table, self.device), keys)
+        part, counts = partition_device(with_schema_validity(kf), len(keys), self.n_pes)
         torch.cuda.current_stream().synchronize()
         lo = sum(counts[: self.rank])
         n = counts[self.rank]
@@ -216,7 +220,7 @@ class DistJoinState:
             self.is_broadcast = True
             self.metrics["broadcast"] = 1
         else:
-            mine = self._shuffle(whole, self.build_key)
+            mine = self._shuffle(whole, self.build_keys)
         self.metrics["build_rows_local"] = mine.n_rows
         res = J.join_build_consume_batch(self.local, mine, True)
         if self.use_filter and self.probe_parallel and not self.is_broadcast:
@@ -224,26 +228,30 @@ class DistJoinState:
         return res
 
     def _build_global_filter(self):
-        """Union of the ranks' bloom filters (same block count everywhere) and the global key bounds."""
+        """Union of the ranks' bloom filters (same block count everywhere) and the global key bounds, per key column."""
         import torch
         import torch.distributed as dist
+
+        from .._lib import ffi
 
         dev = torch.device("cuda", self.device)
         tot = torch.tensor([self.metrics["build_rows_local"]], dtype=torch.int64, device=dev)
         dist.all_reduce(tot, group=self.group)
         n_blocks = int(tot.item()) // 32 + 1
-        words, (mn, mx) = J.build_runtime_filter(self.local, n_blocks)
+        words, bounds = J.build_runtime_filter(self.local, n_blocks)
+        bounds = [bounds] if len(self.build_keys) == 1 else bounds
         gathered = torch.empty(self.n_pes * words.numel(), dtype=words.dtype, device=dev)
         dist.all_gather_into_tensor(gathered, words, group=self.group)  # NCCL has no bitwise-or reduction
         acc = gathered.view(self.n_pes, -1)[0].clone()
         for r in range(1, self.n_pes):
             acc |= gathered.view(self.n_pes, -1)[r]
         words.copy_(acc)
-        lo = torch.tensor([mn], dtype=torch.int64, device=dev)
-        hi = torch.tensor([mx], dtype=torch.int64, device=dev)
+        lo = torch.tensor([mn for mn, _ in bounds], dtype=torch.int64, device=dev)
+        hi = torch.tensor([mx for _, mx in bounds], dtype=torch.int64, device=dev)
         dist.all_reduce(lo, op=dist.ReduceOp.MIN, group=self.group)
         dist.all_reduce(hi, op=dist.ReduceOp.MAX, group=self.group)
-        _lib.check(_lib.lib().b200_join_set_key_bounds(self.local.handle, int(lo.item()), int(hi.item())), "runtime_join_filter")
+        mm = [v for pair in zip(lo.tolist(), hi.tolist()) for v in pair]
+        _lib.check(_lib.lib().b200_join_set_key_bounds_n(self.local.handle, ffi.new("int64_t[]", mm), len(bounds)), "runtime_join_filter")
         self.filter_ready = True
         self.metrics["filter"] = 1
 
@@ -252,10 +260,10 @@ class DistJoinState:
         partitioned_build = self.build_parallel and not self.is_broadcast
         if partitioned_build and self.probe_parallel:
             if self.filter_ready and table.n_rows:
-                table = J.runtime_join_filter((self,), to_device(table, self.device), ((self.probe_key,),))
+                table = J.runtime_join_filter((self,), to_device(table, self.device), (self.probe_keys,))
                 self.metrics["probe_rows_after_filter"] = self.metrics.get("probe_rows_after_filter", 0) + table.n_rows
-            table = self._shuffle(table, self.probe_key)
+            table = self._shuffle(table, self.probe_keys)
         elif partitioned_build:
-            table = self._owned_only(table, self.probe_key)
+            table = self._owned_only(table, self.probe_keys)
         self.metrics["probe_rows_local"] += table.n_rows
         return J.join_probe_consume_batch(self.local, table, is_last, produce_output, used_cols)

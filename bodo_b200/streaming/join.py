@@ -24,8 +24,9 @@ class JoinState:
         self.is_anti_join = bool(is_anti_join)
         self.build_key_inds = tuple(int(k) for k in build_key_inds)
         self.probe_key_inds = tuple(int(k) for k in probe_key_inds)
-        if len(self.build_key_inds) != 1 or len(self.probe_key_inds) != 1:
-            raise _lib.B200Error("Streaming Join: exactly one equi-join key per side is supported")
+        if not 1 <= len(self.build_key_inds) <= 4 or len(self.probe_key_inds) != len(self.build_key_inds):
+            raise _lib.B200Error("Streaming Join: 1 to 4 equi-join keys per side, the same number on both sides "
+                                 f"(got {len(self.build_key_inds)} build and {len(self.probe_key_inds)} probe keys)")
         self.build_colnames = list(build_colnames) if build_colnames is not None else None
         self.probe_colnames = list(probe_colnames) if probe_colnames is not None else None
         self.build_outer = bool(build_outer)
@@ -59,7 +60,7 @@ class JoinState:
 
             self.device = build.device if build.device >= 0 else torch.cuda.current_device()
         h = L.b200_join_state_init(self.operator_id, ffi.new("int8_t[]", bct), ffi.new("int8_t[]", bat), len(bct),
-                                   ffi.NULL, ffi.NULL, 0, 1, int(self.build_outer), int(self.probe_outer), int(self.is_na_equal),
+                                   ffi.NULL, ffi.NULL, 0, len(self.build_key_inds), int(self.build_outer), int(self.probe_outer), int(self.is_na_equal),
                                    self.output_batch_size, self.device, self.expected_build_rows, ffi.cast("void*", self.stream))
         self.handle = _lib.check_ptr(h, "init_join_state")
         if self.is_mark_join or self.is_anti_join:
@@ -177,27 +178,31 @@ def delete_join_state(join_state: JoinState) -> None:
 
 def build_runtime_filter(join_state, n_bloom_blocks: int = 0):
     """Build the bloom filter + key bounds of a finished build side; returns (bloom words as a device tensor aliasing the
-    state's memory, (key_min, key_max)).  Sharded joins OR / min / max these across ranks (dist_join.DistJoinState does)."""
+    state's memory, (key_min, key_max)), or for a multi-column key [(min, max) of each key column].  Sharded joins OR / min / max
+    these across ranks (dist_join.DistJoinState does)."""
     import torch
 
     st = getattr(join_state, "local", join_state)
     L = _lib.lib()
+    nk = len(st.build_key_inds)
     ptr = ffi.new("void**")
     nb = ffi.new("int64_t*")
-    mm = ffi.new("int64_t[2]")
+    mm = ffi.new("int64_t[]", 2 * nk)
     _lib.check(L.b200_join_build_filter(st.handle, int(n_bloom_blocks), ptr, nb, mm), "runtime_join_filter")
     from ..table import DeviceArray
 
     words = torch.as_tensor(DeviceArray(int(ffi.cast("uintptr_t", ptr[0])), int(nb[0]) * 8, "int32", st.device, owner=st), device=torch.device("cuda", st.device))
-    return words, (int(mm[0]), int(mm[1]))
+    bounds = [(int(mm[2 * j]), int(mm[2 * j + 1])) for j in range(nk)]
+    return words, (bounds[0] if nk == 1 else bounds)
 
 
 def runtime_join_filter(join_states, table: Table, join_keys_idxs, process_col_bitmasks=None) -> Table:
     """Mirror of bodo.libs.streaming.join.runtime_join_filter (join.py:1392-1415; C++ HashJoinState::RuntimeFilter): drop the
     rows of `table` that cannot find a partner in the (finished) build sides of `join_states`.  join_keys_idxs[k] = (index of the
-    column of `table` that corresponds to the join key of state k,), -1 = no such column (no filter for that state);
-    process_col_bitmasks[k] = (apply the column-level min / max filter,).  The bloom filter is applied whenever the key column
-    is present, as in the reference.  Device-resident tables only (host batches: bodo_b200.table.to_device first)."""
+    column of `table` that corresponds to each join key of state k, in key order), -1 = no such column (no filter for that state
+    when every entry is -1); process_col_bitmasks[k] = (apply the column-level min / max filter, per key column).  The bloom
+    filter is applied whenever every key column is present, as in the reference.  Device-resident tables only (host batches:
+    bodo_b200.table.to_device first)."""
     import torch
 
     from ..expr import col
@@ -210,13 +215,16 @@ def runtime_join_filter(join_states, table: Table, join_keys_idxs, process_col_b
     keep_all = None
     for k, js in enumerate(join_states):
         st = getattr(js, "local", js)
-        kc = int(join_keys_idxs[k][0])
-        if kc < 0 or st.probe_outer:
+        kcs = [int(c) for c in join_keys_idxs[k]]
+        if all(c < 0 for c in kcs) or st.probe_outer:
             continue
-        use_mm = True if process_col_bitmasks is None else bool(process_col_bitmasks[k][0])
+        use_mm = [1] * len(kcs) if process_col_bitmasks is None else [int(bool(b)) for b in process_col_bitmasks[k]]
+        if len(use_mm) != len(kcs):
+            raise _lib.B200Error("runtime_join_filter: process_col_bitmasks[k] needs one entry per key column")
         keep = torch.empty(table.n_rows + 8, dtype=torch.uint8, device=dev)
         ct = CTable(table)
-        _lib.check(L.b200_join_runtime_filter(st.handle, ct.ptr, kc, int(use_mm), 1, ffi.cast("uint8_t*", keep.data_ptr())), "runtime_join_filter")
+        _lib.check(L.b200_join_runtime_filter_n(st.handle, ct.ptr, ffi.new("int32_t[]", kcs), len(kcs), ffi.new("int32_t[]", use_mm), 1,
+                                                ffi.cast("uint8_t*", keep.data_ptr())), "runtime_join_filter")
         keep_all = keep if keep_all is None else keep_all & keep
     if keep_all is None:
         return table
