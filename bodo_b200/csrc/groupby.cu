@@ -2052,8 +2052,8 @@ class GroupbyState {
         });
         if (!ok) return false;
         {   // SPG-N (spgn.cuh): narrow bucket rows
-            spgn_ns = ((int)(((size_t)max_smem - 256) / 12) - SPG_STASH) & ~1;  // (K2n also has a few static shared words)
-            spgn_smem = (size_t)(spgn_ns + SPG_STASH) * 12 + 16;
+            spgn_ns = ((int)(((size_t)max_smem - 256 - SPGN_QUEUE_BYTES) / 12) - SPG_STASH) & ~1;  // (K2n also has a few static shared words)
+            spgn_smem = (size_t)(spgn_ns + SPG_STASH) * 12 + SPGN_QUEUE_BYTES + 16;
             spgn_enabled = true;
             for_each_sum_cnt([&](auto s, auto c) {
                 if (!set_smem_limit((const void*)spgn_partition_kernel<s, c>, spgn_part_smem())) spgn_enabled = false;

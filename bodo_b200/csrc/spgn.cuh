@@ -17,6 +17,8 @@ constexpr int SPGN_EMPTY = (int)0x80000000;
 #endif
 constexpr int SPGN_TILE = SPGN_TILE_ROWS;            // rows per K1n tile (8-byte staged rows leave room for twice the 16-byte kernels' tile)
 constexpr int SPGN_CTAS = SPGN_TILE == 4096 ? 2 : 3;  // K1n CTAs per SM
+constexpr int SPGN_QUEUE = 32;                                          // K2n: cold rows a warp queues before it handles them together
+constexpr int SPGN_QUEUE_BYTES = SPG_THREADS / 32 * SPGN_QUEUE * 9;     // 8-byte row + one flag byte per queued row: 9 KB
 
 // find-or-insert for a caller that already holds a group ticket: `inserted` says whether THIS call created the group (else the
 // ticket goes back).  The table cannot be full: tickets bound the number of groups by cap / 2.
@@ -169,23 +171,24 @@ __device__ __forceinline__ void spgn_buckets(uint64_t h, unsigned int NB, unsign
     b2 = b2 == b1 ? (b1 + 1 == NB ? 0u : b1 + 1) : b2;
 }
 
-// K2n's rare per-row work.  s < 0: the key is not in its two buckets (first appearance: CAS into the emptier bucket, else the
-// stash, else the direct path), then the row is added.  s >= 0: the row was added already and `old` is the low sum word before
-// that add.  Either way a carry into the high sum word goes to the global table.
-// Out of line on purpose: inlined at each of the loop's call sites this code made K2n 4096 SASS instructions long, and on an
-// H100 it ran 4.5 ms per 2^28 rows at 1 M groups against 3.0 ms out of line (scratch/spg_harness.cu), with no change at 200 k
-// groups.
+// K2n's rare per-row work, for one queued row.  !added: the key is not in its two buckets (first appearance: CAS into the emptier
+// bucket, else the stash, else the direct path), then the row is added.  added: the row was added already and the low sum word
+// wrapped, so the high sum word takes the sign extension plus the carry: +1 for a value >= 0, -1 for a negative one.  Either way
+// a carry into the high sum word goes to the global table.
+// Out of line on purpose: inlined into the row loop it made K2n slower per 2^28 rows on an H100 (scratch/spg_harness.cu): at
+// eight call sites 4.5 against 3.0 ms at 1 M groups, at one call site 2.8 against 1.0 ms at 200 k groups.
 template <bool HAS_SUM, bool HAS_CNT>
 __device__ __noinline__ void spgn_cold_row(const SpgArgs& a, int* skeys, unsigned int* slo, unsigned int* scnt, unsigned int NB, int key, int val,
-                                           int s, unsigned int old) {
-    if (s < 0) {
+                                           bool added) {
+    unsigned int old = 0;
+    if (!added) {
         const unsigned int NS = 2 * NB;
         unsigned int b1, b2;
         spgn_buckets(spg_hash((long long)key), NB, b1, b2);
         const int2 c1 = *reinterpret_cast<const int2*>(skeys + 2 * b1);
         const int2 c2 = *reinterpret_cast<const int2*>(skeys + 2 * b2);
         const int f1 = (c1.x == SPGN_EMPTY) + (c1.y == SPGN_EMPTY), f2 = (c2.x == SPGN_EMPTY) + (c2.y == SPGN_EMPTY);
-        s = c1.x == key ? (int)(2 * b1) : c1.y == key ? (int)(2 * b1 + 1) : c2.x == key ? (int)(2 * b2) : c2.y == key ? (int)(2 * b2 + 1) : -1;
+        int s = c1.x == key ? (int)(2 * b1) : c1.y == key ? (int)(2 * b1 + 1) : c2.x == key ? (int)(2 * b2) : c2.y == key ? (int)(2 * b2 + 1) : -1;
         if (s < 0 && f1 + f2 > 0) {
             const unsigned int first = f2 > f1 ? b2 : b1, second = f2 > f1 ? b1 : b2;
             const unsigned int cand[4] = {2 * first, 2 * first + 1, 2 * second, 2 * second + 1};
@@ -214,19 +217,37 @@ __device__ __noinline__ void spgn_cold_row(const SpgArgs& a, int* skeys, unsigne
     }
     if (HAS_SUM) {
         const unsigned int lo = (unsigned int)val;
-        const unsigned int hi = (val < 0 ? 0xffffffffu : 0u) + (old + lo < old ? 1u : 0u);
+        const unsigned int hi = added ? (val < 0 ? 0xffffffffu : 1u) : (val < 0 ? 0xffffffffu : 0u) + (old + lo < old ? 1u : 0u);
         if (hi) spg_direct_apply<HAS_SUM, HAS_CNT>(a, (long long)key, (unsigned long long)hi << 32, 0ull);
     }
 }
+
+// scratch/spg_harness.cu builds K2n with SPGN_PHASE_CLOCKS to see where a launch's time goes: per CTA, the SM clocks of table
+// init, the row loop and the flush, summed over passes.  SPGN_SKIP_FLUSH (harness ablation, wrong results) drops the flush.
+#ifdef SPGN_PHASE_CLOCKS
+__device__ unsigned long long spgn_phase_clocks[SPG_MAX_OWNERS * 4];  // per CTA: 3 spans, then the clock of the last mark
+#define SPGN_PHASE(i)                                                                                                      \
+    do {                                                                                                                   \
+        if (threadIdx.x == 0) {                                                                                            \
+            unsigned long long* c_ = spgn_phase_clocks + blockIdx.x * 4;                                                   \
+            const unsigned long long t_ = clock64();                                                                       \
+            if ((i) >= 0) c_[(i)] += t_ - c_[3];                                                                           \
+            c_[3] = t_;                                                                                                    \
+        }                                                                                                                  \
+    } while (0)
+#else
+#define SPGN_PHASE(i) do {} while (0)
+#endif
 
 // K2n: slot = int32 key, low sum word (biased by 2^31), count.
 template <bool HAS_SUM, bool HAS_CNT>
 __global__ void __launch_bounds__(SPG_THREADS, 1) spgn_aggregate_kernel(const __grid_constant__ SpgArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
+    SPGN_PHASE(-1);
     const int NS = a.ns, NT = a.ns + SPG_STASH, tid = threadIdx.x, me = blockIdx.x;
     int* skeys = (int*)smem_raw;                      // NT x 4
     unsigned int* slo = (unsigned int*)(skeys + NT);  // NT x 4
-    unsigned int* scnt = slo + NT;
+    unsigned int* scnt = slo + NT;                    // NT x 4, then the warps' cold-row queues (SPGN_QUEUE_BYTES)
     const unsigned int NB = (unsigned int)NS / 2;
     const unsigned int NP = (unsigned int)a.n_pass, GP = (unsigned int)gridDim.x * NP;
 
@@ -248,6 +269,25 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgn_aggregate_kernel(const __
             } else if (r < n_in) row[2 * j] = __ldcs(src + r);
         }
     };
+    // Rows that need spgn_cold_row (a key not in its two buckets, a low sum word that wrapped) do not call it where they are found:
+    // they go to their warp's queue in shared memory, and the warp drains a full queue with one call on all lanes.  At 1 M groups a
+    // warp meets such a row in most iterations (first appearances, then stashed keys: about 14 k per CTA and 2^28-row launch), and
+    // calling it per row took K2n from 1.1 to 3.0 ms per launch (H100 at 400 W, scratch/spg_harness.cu), most likely because a call
+    // first waits for every load in flight, the next iteration's bucket rows included.
+    // queue slot i of this warp: row at q_row(i), flag "added already" at q_added(i) (computed where used: the loop has no
+    // register to spare for the two addresses)
+    auto q_row = [&](unsigned int i) { return reinterpret_cast<int2*>(scnt + NT) + (threadIdx.x >> 5) * SPGN_QUEUE + i; };
+    auto q_added = [&](unsigned int i) {
+        return reinterpret_cast<unsigned char*>(reinterpret_cast<int2*>(scnt + NT) + SPG_THREADS / 32 * SPGN_QUEUE) + (threadIdx.x >> 5) * SPGN_QUEUE + i;
+    };
+    unsigned int qn = 0;  // rows in this warp's queue (the same in every lane)
+    auto drain = [&]() {
+        __syncwarp();
+        const unsigned int lane = threadIdx.x & 31;
+        if (lane < qn) spgn_cold_row<HAS_SUM, HAS_CNT>(a, skeys, slo, scnt, NB, q_row(lane)->x, q_row(lane)->y, *q_added(lane) != 0);
+        __syncwarp();
+        qn = 0;
+    };
     auto process = [&](const int2 (&row)[U], unsigned int pass, auto full_tag) {
         constexpr bool FULL = decltype(full_tag)::value;
         int sl[U];
@@ -263,29 +303,44 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgn_aggregate_kernel(const __
             if (!FULL && key == SPGN_EMPTY) sl[u] = -2;  // padding lane (INT32_MIN never reaches a bucket)
             if (NP > 1 && __umulhi((unsigned int)(h >> 32), GP) - (unsigned int)me * NP != pass) sl[u] = -2;
         }
-        int pk = 0, pv = 0;
-        bool parked = false;
+        unsigned int cold = 0;  // bit u: row u goes to the queue; bit U + u: its row was added already (the low sum word wrapped)
 #pragma unroll
         for (int u = 0; u < U; u++) {
             if (sl[u] >= 0) {
                 if (HAS_SUM) {
                     const unsigned int lo = (unsigned int)row[u].y, old = atomicAdd(&slo[sl[u]], lo);
                     // high sum word = sign extension + carry of the low-word add: nonzero only when the biased low word wraps
-                    if ((row[u].y < 0 ? 0xffffffffu : 0u) + (old + lo < old ? 1u : 0u)) spgn_cold_row<HAS_SUM, HAS_CNT>(a, skeys, slo, scnt, NB, row[u].x, row[u].y, sl[u], old);
+                    if ((row[u].y < 0 ? 0xffffffffu : 0u) + (old + lo < old ? 1u : 0u)) cold |= (1u << u) | (1u << (U + u));
                 }
                 if (HAS_CNT) atomicAdd(&scnt[sl[u]], 1u);
-            } else if (sl[u] == -1) {
-                if (!parked) { pk = row[u].x; pv = row[u].y; parked = true; }
-                else spgn_cold_row<HAS_SUM, HAS_CNT>(a, skeys, slo, scnt, NB, row[u].x, row[u].y, -1, 0u);
+            } else if (sl[u] == -1) cold |= 1u << u;
+        }
+        if (__any_sync(0xffffffffu, cold != 0)) {
+#pragma unroll 1
+            for (int u = 0; u < U; u++) {
+                const bool mine = (cold >> u) & 1u;
+                const unsigned int m = __ballot_sync(0xffffffffu, mine);
+                if (!m) continue;
+                if (qn + __popc(m) > SPGN_QUEUE) drain();
+                if (mine) {
+                    int2 r = row[0];
+#pragma unroll
+                    for (int v = 1; v < U; v++)
+                        if (u == v) r = row[v];
+                    const unsigned int p = qn + __popc(m & ((1u << (threadIdx.x & 31)) - 1u));
+                    *q_row(p) = r;
+                    *q_added(p) = (cold >> (U + u)) & 1u;
+                }
+                qn += __popc(m);
             }
         }
-        if (parked) spgn_cold_row<HAS_SUM, HAS_CNT>(a, skeys, slo, scnt, NB, pk, pv, -1, 0u);
     };
     const unsigned long long ustep = (unsigned long long)(U / 2) * SPG_THREADS;   // units per CTA iteration
     const unsigned long long full_units = n_in / (2 * ustep) * ustep;              // iterations whose rows are all in range
     for (unsigned int pass = 0; pass < NP; pass++) {
         for (int s = tid; s < NT; s += SPG_THREADS) { skeys[s] = SPGN_EMPTY; slo[s] = 0x80000000u; scnt[s] = 0; }
         __syncthreads();
+        SPGN_PHASE(0);
         // software pipeline: the next iteration's bucket rows are in flight while the current ones are aggregated (the wait for these
         // loads was the largest single stall of the unpipelined loop, 20 % of the samples)
         if (full_units > 0) {
@@ -303,7 +358,12 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgn_aggregate_kernel(const __
             load_rows(ub + tid, tail, std::false_type{});
             process(tail, pass, std::false_type{});
         }
+        if (qn) drain();
         __syncthreads();
+        SPGN_PHASE(1);
+#ifdef SPGN_SKIP_FLUSH
+        continue;
+#endif
         // flush.  First flush of a state (empty global table, a.reserve_tickets): every occupied slot is a NEW group, and 10^6
         // per-insert tickets on one counter cost ~0.2 ms — the CTA takes the tickets of all its slots with ONE atomic and returns
         // the few it did not need (a key that sits in two slots, or that the direct path inserted meanwhile).
@@ -345,5 +405,6 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgn_aggregate_kernel(const __
             if (tid == 0 && fl_dup) atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], (unsigned long long)(-(long long)fl_dup));
         }
         __syncthreads();
+        SPGN_PHASE(2);
     }
 }

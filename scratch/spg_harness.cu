@@ -4,30 +4,36 @@
 //
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -I bodo_b200/csrc \
 //        scratch/spg_harness.cu bodo_b200/csrc/misc.cu -o scratch/spg_harness
-//   scratch/spg_harness [pair=n] [log2_rows=28] [groups=1000000] [reps=5] [cnt_stride_pad_bytes=0]
+//   scratch/spg_harness [pair=n] [log2_rows=28] [groups=1000000] [reps=5] [cnt_stride_pad_bytes=0] [keys=d]
 //
 // pair n: the narrow-row pair (K1n spgn_partition_kernel + K2n spgn_aggregate_kernel), launched as GroupbyState::consume_spg
 //         launches it for the flagship (SpgArgs as the host fills them, 2^28 rows = one launch, first launch with ticket
 //         reservation).  pair w: the 16-byte pair (K1 spg_partition_tma_kernel + K2 spg_aggregate_kernel) that the heavy-hitter and
 //         wide-row paths run.
-// Keys are uniform over `groups`, values uniform in [-500, 500), as bodo_b200/synth.py produces them.  Prints per-kernel
+// Keys are uniform over `groups`, values uniform in [-500, 500), as bodo_b200/synth.py produces them.  keys=s scrambles them:
+// each key k becomes mix64(k) truncated to 31 bits (still narrow), so the buckets see keys that a dense range does not model.  Prints per-kernel
 // CUDA-event times (min / median over reps, the first, cold repetition excluded), each kernel's design bytes over its median
 // time, a plain device copy (read the 16-byte row, write an 8-byte row) timed in the same process as the practical bandwidth
 // ceiling, and checks SUM/COUNT totals against the input (the result must be exact).
+// K2n is built with SPGN_PHASE_CLOCKS: the output also gives, per launch, where K2n's CTAs spend their SM clocks (table init,
+// row loop, flush; mean and max over CTAs, medians over reps).  Building with -DSPGN_SKIP_FLUSH times K2n without its flush
+// (the check then fails by design).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
 
+#define SPGN_PHASE_CLOCKS
 #include "../bodo_b200/csrc/groupby.cu"
 
 using namespace b200;
 
-__global__ void harness_fill_kernel(long long* keys, long long* vals, int64_t n, uint64_t n_groups) {
+__global__ void harness_fill_kernel(long long* keys, long long* vals, int64_t n, uint64_t n_groups, bool scramble) {
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
-        keys[i] = (long long)(mix64((uint64_t)i ^ 0x9e3779b97f4a7c15ULL) % n_groups);
+        const uint64_t k = mix64((uint64_t)i ^ 0x9e3779b97f4a7c15ULL) % n_groups;
+        keys[i] = (long long)(scramble ? mix64(k) & 0x7fffffffULL : k);
         vals[i] = (long long)(mix64((uint64_t)i ^ 0xd1b54a32d192ed03ULL * 2) % 1000) - 500;
     }
 }
@@ -58,6 +64,7 @@ int main(int argc, char** argv) {
     const uint64_t groups = argc > 3 ? strtoull(argv[3], nullptr, 10) : 1000000ull;
     const int reps = argc > 4 ? atoi(argv[4]) : 5;
     const size_t pad = argc > 5 ? strtoull(argv[5], nullptr, 10) : 0;  // shifts the owner row counters inside their allocation
+    const bool scramble = argc > 6 && strcmp(argv[6], "s") == 0;
     const int64_t rows = 1ll << lg;
     int dev = 0, sms = 0, max_smem = 0;
     CK(cudaSetDevice(dev));
@@ -66,9 +73,9 @@ int main(int argc, char** argv) {
     const int owners = sms;
     // shared-table sizes and K1 shapes exactly as GroupbyState::spg_probe / consume_spg compute them
     const int spg_ns = ((int)(((size_t)max_smem - 64) / 16) - SPG_STASH) & ~1;
-    const int spgn_ns = ((int)(((size_t)max_smem - 256) / 12) - SPG_STASH) & ~1;
+    const int spgn_ns = ((int)(((size_t)max_smem - 256 - SPGN_QUEUE_BYTES) / 12) - SPG_STASH) & ~1;
     const int ns = narrow ? spgn_ns : spg_ns;
-    const size_t k2_smem = narrow ? (size_t)(spgn_ns + SPG_STASH) * 12 + 16 : (size_t)(spg_ns + SPG_STASH) * 16 + 16;
+    const size_t k2_smem = narrow ? (size_t)(spgn_ns + SPG_STASH) * 12 + SPGN_QUEUE_BYTES + 16 : (size_t)(spg_ns + SPG_STASH) * 16 + 16;
     const size_t k1_smem = narrow ? GroupbyState::spgn_part_smem() : GroupbyState::spg_tma_smem();
     const int tile = narrow ? SPGN_TILE : SPG_TILE, k1_threads = SPG_TTHREADS, k1_ctas = narrow ? SPGN_CTAS : SPG_TCTAS;
     const int g1 = (int)std::min<int64_t>((int64_t)sms * k1_ctas, (rows + tile - 1) / tile);
@@ -87,7 +94,7 @@ int main(int argc, char** argv) {
     CK(cudaMalloc(&bucket_cnt_raw, (size_t)owners * SPG_CNT_STRIDE * 8 + pad + 256));
     CK(cudaMalloc(&retry, ((size_t)rows + (size_t)owners * spg_ns) * 32));
     unsigned long long* bucket_cnt = (unsigned long long*)((char*)bucket_cnt_raw + pad);
-    harness_fill_kernel<<<sms * 8, 256>>>(keys, vals, rows, groups);
+    harness_fill_kernel<<<sms * 8, 256>>>(keys, vals, rows, groups, scramble);
     harness_fill_u64<<<sms * 8, 256>>>((unsigned long long*)tkeys, cap + 2, (unsigned long long)EMPTY_KEY);
     CK(cudaMemset(acc_sum, 0, (cap + 2) * 8)); CK(cudaMemset(acc_cnt, 0, (cap + 2) * 8)); CK(cudaMemset(counters, 0, 64));
     CK(cudaDeviceSynchronize());
@@ -104,12 +111,15 @@ int main(int argc, char** argv) {
     CK(cudaFuncSetAttribute(k2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
 
     std::vector<float> t1, t2, tc;
+    std::vector<float> ph_mean[3], ph_max[3];  // K2n phase clocks per launch
+    std::vector<unsigned long long> ph((size_t)SPG_MAX_OWNERS * 4);
     cudaEvent_t e0, e1, e2;
     CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1)); CK(cudaEventCreate(&e2));
     for (int r = 0; r < reps + 1; r++) {  // the first repetition (table inserts, cold) is not reported
         // the host reserves group tickets only for the first flush into an empty table
         a.reserve_tickets = narrow && r == 0 && (int64_t)groups + (int64_t)groups / 4 <= (int64_t)(cap / 2) ? 1 : 0;
         CK(cudaMemsetAsync(bucket_cnt, 0, (size_t)owners * SPG_CNT_STRIDE * 8));
+        if (narrow) { std::fill(ph.begin(), ph.end(), 0ull); CK(cudaMemcpyToSymbol(spgn_phase_clocks, ph.data(), ph.size() * 8)); }
         CK(cudaEventRecord(e0));
         if (narrow) {
             spgn_partition_kernel<true, true><<<g1, k1_threads, k1_smem>>>(a);
@@ -126,6 +136,14 @@ int main(int argc, char** argv) {
         float a1 = 0, a2 = 0;
         CK(cudaEventElapsedTime(&a1, e0, e1)); CK(cudaEventElapsedTime(&a2, e1, e2));
         if (r > 0) { t1.push_back(a1); t2.push_back(a2); }
+        if (narrow && r > 0) {
+            CK(cudaMemcpyFromSymbol(ph.data(), spgn_phase_clocks, ph.size() * 8));
+            for (int i = 0; i < 3; i++) {
+                double sum = 0, mx = 0;
+                for (int c = 0; c < owners; c++) { sum += (double)ph[c * 4 + i]; mx = std::max(mx, (double)ph[c * 4 + i]); }
+                ph_mean[i].push_back((float)(sum / owners)); ph_max[i].push_back((float)mx);
+            }
+        }
     }
     // totals: SUM of sums and SUM of counts over the table must equal (reps + 1) x the input totals
     CK(cudaMemset(chk, 0, 16));
@@ -154,11 +172,14 @@ int main(int argc, char** argv) {
     const double b1 = narrow ? 24.0 : 48.0, b2 = narrow ? 8.0 : 16.0;  // design bytes per row: K1 reads the row and writes the bucket row, K2 reads it
     const float m1 = median(t1), m2 = median(t2), mc = median(tc);
     const double gbs1 = rows * b1 / (m1 * 1e-3) / 1e9, gbs2 = rows * b2 / (m2 * 1e-3) / 1e9, gbsc = rows * 24.0 / (mc * 1e-3) / 1e9;
-    printf("{\"pair\": \"%s\", \"rows\": %lld, \"groups\": %llu, \"n_pass\": %d, \"k1_shape\": {\"tile\": %d, \"threads\": %d, \"ctas_per_sm\": %d, \"smem\": %zu}, "
+    if (narrow)
+        printf("{\"k2n_phase_kclk\": {\"init\": [%.1f, %.1f], \"rows\": [%.1f, %.1f], \"flush\": [%.1f, %.1f]}, \"k2n_phase_note\": \"[mean, max] over CTAs, thousands of SM clocks\"}\n",
+               median(ph_mean[0]) / 1e3, median(ph_max[0]) / 1e3, median(ph_mean[1]) / 1e3, median(ph_max[1]) / 1e3, median(ph_mean[2]) / 1e3, median(ph_max[2]) / 1e3);
+    printf("{\"pair\": \"%s\", \"keys\": \"%s\", \"rows\": %lld, \"groups\": %llu, \"n_pass\": %d, \"k1_shape\": {\"tile\": %d, \"threads\": %d, \"ctas_per_sm\": %d, \"smem\": %zu}, "
            "\"k1_ms\": {\"min\": %.4f, \"median\": %.4f}, \"k2_ms\": {\"min\": %.4f, \"median\": %.4f}, \"copy_ms\": {\"min\": %.4f, \"median\": %.4f}, "
            "\"k1_gbs\": %.1f, \"k2_gbs\": %.1f, \"copy_gbs\": %.1f, \"k1_of_copy\": %.3f, \"k2_of_copy\": %.3f, "
            "\"pair_grows_per_s\": %.2f, \"table_groups\": %lld, \"retry_rows\": %lld, \"wide_rows\": %lld, \"check\": \"%s\"}\n",
-           narrow ? "spgn" : "spg", (long long)rows, (unsigned long long)groups, a.n_pass, tile, k1_threads, k1_ctas, k1_smem,
+           narrow ? "spgn" : "spg", scramble ? "scrambled" : "dense", (long long)rows, (unsigned long long)groups, a.n_pass, tile, k1_threads, k1_ctas, k1_smem,
            minimum(t1), m1, minimum(t2), m2, minimum(tc), mc, gbs1, gbs2, gbsc, gbs1 / gbsc, gbs2 / gbsc,
            rows / ((m1 + m2) * 1e-3) / 1e9, hc[0], hc[1], hc[5], ok ? "ok" : "MISMATCH");
     return ok ? 0 : 3;
