@@ -58,7 +58,8 @@ enum CounterSlot : int {
     CTR_WIDE = 5,           // SPG-N: rows that did not fit the narrow (int32 key, int32 value) format
     CTR_RETRY1 = 6,         // rows in the slot-1 retry list (SPG)
     CTR_XCHG_OVERFLOW = 7,  // fused exchange: some rank's share overflowed its slab segment, nobody combined
-    N_COUNTERS = 8
+    CTR_RETRY_OVERFLOW = 8, // SPG / SPG-G: an entry did not fit its retry list and was dropped (the host raises an error)
+    N_COUNTERS = 9
 };
 
 struct ConsumeArgs {
@@ -1072,6 +1073,7 @@ struct SpgArgs {
     long long bucket_cap;
     unsigned long long* retry;  // partial-aggregate rows [key][1][a0 of func 0][a0 of func 1]
     long long* retry_ctr;       // number of rows in `retry`
+    long long retry_cap;        // rows `retry` holds: an entry past it is dropped and raises counters[CTR_RETRY_OVERFLOW]
     int sum_first;              // order of the two accumulators in the wire format
     int ns;                     // shared-memory table slots (K2)
     int n_pass;                 // K2 passes over each owner bucket (pass p keeps the keys of sub-range p): > 1 when the
@@ -1093,6 +1095,7 @@ __device__ __forceinline__ unsigned int spg_slot(uint64_t h, int ns) { return __
 template <bool HAS_SUM, bool HAS_CNT>
 __device__ __forceinline__ void spg_retry_row(const SpgArgs& a, long long key, unsigned long long sum, unsigned long long cnt) {
     unsigned long long f = atomicAdd((unsigned long long*)a.retry_ctr, 1ull);
+    if (f >= (unsigned long long)a.retry_cap) { a.counters[CTR_RETRY_OVERFLOW] = 1; return; }
     unsigned long long* r = a.retry + f * 4;
     r[0] = (unsigned long long)key; r[1] = 1ull;
     if (HAS_SUM && HAS_CNT) { r[2] = a.sum_first ? sum : cnt; r[3] = a.sum_first ? cnt : sum; }
@@ -1883,7 +1886,7 @@ class GroupbyState {
         if (copy_stream) { cudaStreamSynchronize(copy_stream); cudaStreamDestroy(copy_stream); }
         for (int b = 0; b < 2; b++) { if (stage_free[b]) cudaEventDestroy(stage_free[b]); if (stage_ready[b]) cudaEventDestroy(stage_ready[b]); }
         pinned_release(h_counters, N_COUNTERS * sizeof(long long));
-        pinned_release(h_spg, 24 * sizeof(long long));
+        pinned_release(h_spg, H_SPG_WORDS * sizeof(long long));
         for (int b = 0; b < 2; b++) if (spg_ev[b]) cudaEventDestroy(spg_ev[b]);
         for (auto& pr : prof_events) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
     }
@@ -2011,6 +2014,7 @@ class GroupbyState {
     template <typename T, typename Replay>
     void settle(const DevBuf& list, size_t words, int64_t& replayed, Replay replay) {
         for (read_counters(); h_counters[CTR_FAIL] > 0; read_counters()) {
+            B200_REQUIRE(h_counters[CTR_RETRY_OVERFLOW] == 0, "SM-partitioned groupby: a retry list overflowed its buffer (internal sizing error)");
             const int64_t nf = h_counters[CTR_FAIL];
             replayed += nf;
             grow_to_fit(nf);
@@ -2096,7 +2100,7 @@ class GroupbyState {
     size_t spgn_smem = 0;
     bool spgn_enabled = false;
     int spg_sample_wide = -1;  // sampled rows of the first launch that do NOT fit (int32 key, int32 value); -1 = not sampled
-    int64_t spgn_launches = 0;
+    int64_t spgn_launches = 0, spg16_launches = 0;  // launches of the narrow-row pair, of the 16-byte pair
     static size_t spgn_part_smem() { return (size_t)SPGN_TILE * (16 + 8 + 1) + SPG_MAX_OWNERS * 16 + 16 + (2 * SPG_MAX_OWNERS + 4) * 4 + 256; }
     int64_t spgn_group_capacity() const { return (int64_t)spg_owners * (spgn_ns * 7 / 10); }
     int spgg_ns[4] = {0, 0, 0, 0};  // K2g table slots, by slot layout v = (min/max fields) + 2 * (NA-value counter)
@@ -2121,7 +2125,8 @@ class GroupbyState {
     // One SPG launch pair in flight while the host inspects the previous one (two retry lists / counter slots), so
     // the GPU never idles on the host's counter read-back.
     PooledBuf d_retry2[2];
-    long long* h_spg = nullptr;  // pinned: [slot][8] counter snapshots
+    static constexpr int H_SPG_WORDS = 2 * N_COUNTERS + 1;
+    long long* h_spg = nullptr;  // pinned: [slot][N_COUNTERS] counter snapshots, then the two ints of the sample verdict
     cudaEvent_t spg_ev[2] = {nullptr, nullptr};
 
     int64_t spgn_wide_rows = 0;  // rows that did not fit the narrow format so far (counters[CTR_WIDE])
@@ -2137,6 +2142,8 @@ class GroupbyState {
         spg_retry_rows += nr;
         B200_CUDA(cudaStreamSynchronize(stream));  // the other in-flight launch uses the table we are about to replace
         read_counters();
+        // (the flag is shared by both slots: a list that overflowed has entries, so its own or the other slot's call gets here)
+        B200_REQUIRE(h_counters[CTR_RETRY_OVERFLOW] == 0, "SM-partitioned groupby: a retry list overflowed its buffer (internal sizing error)");
         const int64_t pending = h_counters[CTR_FAIL] + h_counters[CTR_RETRY1];
         // the snapshot this call was made on may be stale: the other slot's spg_finish already grew the table and merged
         // BOTH retry lists (their live counters are 0 then) — nothing left to do, and no second grow
@@ -2167,7 +2174,7 @@ class GroupbyState {
         // K1 and K1n fetch their tiles with TMA bulk copies and LC reads row pairs with 16-byte loads: all need aligned columns
         B200_REQUIRE(((uintptr_t)keys & 15) == 0 && ((uintptr_t)vals & 15) == 0, "SM-partitioned groupby: key and value columns must be 16-byte aligned");
         if (!h_spg) {
-            h_spg = (long long*)pinned_acquire(24 * sizeof(long long));  // [slot][8] counter snapshots + n_hot read-back
+            h_spg = (long long*)pinned_acquire(H_SPG_WORDS * sizeof(long long));  // [slot][N_COUNTERS] counter snapshots + n_hot read-back
             for (int b = 0; b < 2; b++) B200_CUDA(cudaEventCreateWithFlags(&spg_ev[b], cudaEventDisableTiming));
         }
         ScopedTimer timer{t_spg};
@@ -2178,10 +2185,10 @@ class GroupbyState {
             // format; the host reads back both verdicts
             int* d_nhot = (int*)(d_hot.as<long long>() + SPG_HOT_SLOTS);
             spg_hot_sample_kernel<<<1, 1024, SPG_HOT_SAMPLE_SMEM, stream>>>(keys, vals, n, d_hot.as<long long>(), d_nhot);
-            B200_CUDA(cudaMemcpyAsync(h_spg + 16, d_nhot, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+            B200_CUDA(cudaMemcpyAsync(h_spg + 2 * N_COUNTERS, d_nhot, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
             B200_CUDA(cudaStreamSynchronize(stream));
-            spg_n_hot = spg_hot_enabled ? ((int*)(h_spg + 16))[0] : 0;
-            spg_sample_wide = ((int*)(h_spg + 16))[1];
+            spg_n_hot = spg_hot_enabled ? ((int*)(h_spg + 2 * N_COUNTERS))[0] : 0;
+            spg_sample_wide = ((int*)(h_spg + 2 * N_COUNTERS))[1];
             spg_hot_sampled = true;
             launches++;
         }
@@ -2197,9 +2204,23 @@ class GroupbyState {
             // uniform keys put rows / owners rows in every bucket (sd = sqrt of that); 12.5 % + 4096 rows head room,
             // anything beyond (skew) takes the direct path inside K1
             const int64_t bucket_cap = (rows / spg_owners) + (rows / spg_owners) / 8 + 4096;
+            const bool small = lowcard_small;
+            const int gl = (int)std::min<int64_t>((int64_t)sms * (small ? 3 : 2), (rows + LC_THREADS * 2 - 1) / (LC_THREADS * 2));
+            const int g2 = (int)std::min<int64_t>((int64_t)sms * SPG_TCTAS, (rows + SPG_TILE - 1) / SPG_TILE);
+            const bool hot = !lowcard && spg_hot_enabled && spg_n_hot > 0;
+            // SPG-N: the sample found only rows that fit (int32 key, int32 value), and the rows that did not so far are rare
+            const bool narrow = !lowcard && spgn_enabled && !hot && spg_sample_wide == 0 && spgn_wide_rows * 64 <= rows_consumed;
+            const int64_t est_n = std::max<int64_t>(est_groups, 1);
+            const int n_pass = narrow ? (int)std::min<int64_t>(SPG_MAX_PASSES, std::max<int64_t>(1, (est_n + spgn_group_capacity() - 1) / spgn_group_capacity()))
+                                      : spg_passes;
+            // retry entries: at most one per row (K1's direct rows; in K2 a carry or a row without a slot), plus one per partial of
+            // the per-CTA tables: LC's slots, or every occupied K2 slot (buckets and stash) in every pass and K1's heavy hitters
+            const int64_t retry_cap = rows + (lowcard ? (int64_t)gl * (small ? LC_SLOTS_SMALL : LC_SLOTS_BIG)
+                                                      : (int64_t)spg_owners * ((narrow ? spgn_ns : spg_ns) + SPG_STASH) * n_pass
+                                                        + (hot ? (int64_t)g2 * SPG_HOT_SLOTS : 0));
             double ta = now();
             d_bucket.ensure(device, (size_t)spg_owners * bucket_cap * 16);  // K2 of the previous launch precedes K1 of this one in stream order
-            d_retry2[slot].ensure(device, ((size_t)rows + (size_t)spg_owners * spg_ns) * 32);
+            d_retry2[slot].ensure(device, (size_t)retry_cap * 32);
             t_alloc += now() - ta;
             B200_CUDA(cudaMemsetAsync(d_bucket_cnt.p, 0, (size_t)spg_owners * SPG_CNT_STRIDE * 8, stream));
             SpgArgs a{};
@@ -2210,12 +2231,10 @@ class GroupbyState {
             a.counters = d_counters.as<long long>(); a.group_limit = (long long)(cap / 2);
             a.retry_ctr = d_counters.as<long long>() + spg_retry_slot(slot);
             a.bucket = d_bucket.as<longlong2>(); a.bucket_cnt = d_bucket_cnt.as<unsigned long long>(); a.bucket_cap = bucket_cap;
-            a.retry = d_retry2[slot].as<unsigned long long>();
-            a.sum_first = (sum_j >= 0 && cnt_j >= 0 && sum_j < cnt_j) ? 1 : 0; a.ns = spg_ns; a.n_pass = spg_passes;
+            a.retry = d_retry2[slot].as<unsigned long long>(); a.retry_cap = retry_cap;
+            a.sum_first = (sum_j >= 0 && cnt_j >= 0 && sum_j < cnt_j) ? 1 : 0; a.ns = spg_ns; a.n_pass = n_pass;
             const ProfEvents prof = prof_begin(profiling);
             if (lowcard) {
-                const bool small = lowcard_small;
-                int gl = (int)std::min<int64_t>((int64_t)sms * (small ? 3 : 2), (rows + LC_THREADS * 2 - 1) / (LC_THREADS * 2));
                 size_t lsm = (size_t)(small ? LC_SLOTS_SMALL : LC_SLOTS_BIG) * 20 + 64;
                 with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
                     if (small) groupby_lowcard_kernel<s, c, LC_SLOTS_SMALL, 3><<<gl, LC_THREADS, lsm, stream>>>(a);
@@ -2223,12 +2242,8 @@ class GroupbyState {
                 });
                 lc_launches++;
             } else {
-                int g2 = (int)std::min<int64_t>((int64_t)sms * SPG_TCTAS, (rows + SPG_TILE - 1) / SPG_TILE);
-                const bool hot = spg_hot_enabled && spg_n_hot > 0;
                 if (hot) { a.hot_tab = d_hot.as<long long>(); a.n_hot = (const int*)(d_hot.as<long long>() + SPG_HOT_SLOTS); }
                 const size_t tsm = spg_tma_smem(hot);
-                // SPG-N: the sample found only rows that fit (int32 key, int32 value), and the rows that did not so far are rare
-                const bool narrow = spgn_enabled && !hot && spg_sample_wide == 0 && spgn_wide_rows * 64 <= rows_consumed;
                 if (narrow) {
                     a.ns = spgn_ns;
                     // first flush into an empty table: per-CTA ticket reservation, but only with >= 25 % head room under the group
@@ -2236,13 +2251,11 @@ class GroupbyState {
                     // limit reached would send its groups to the retry list and make the host grow the table for nothing (seen on
                     // 8 GPUs: 1 M groups against a limit of 2^20 cost 1.4 ms per state in some runs)
                     a.reserve_tickets = (n_groups_bound == 0 && li == 0 && est_groups > 0 && est_groups + est_groups / 4 <= (int64_t)(cap / 2)) ? 1 : 0;
-                    const int64_t est_n = std::max<int64_t>(est_groups, 1);
-                    a.n_pass = (int)std::min<int64_t>(SPG_MAX_PASSES, std::max<int64_t>(1, (est_n + spgn_group_capacity() - 1) / spgn_group_capacity()));
                     a.bucket_cap = bucket_cap & ~1ll;
                     const size_t nsm = spgn_part_smem();
-                    const int g2 = (int)std::min<int64_t>((int64_t)sms * SPGN_CTAS, (rows + SPGN_TILE - 1) / SPGN_TILE);
+                    const int gn = (int)std::min<int64_t>((int64_t)sms * SPGN_CTAS, (rows + SPGN_TILE - 1) / SPGN_TILE);
                     with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
-                        spgn_partition_kernel<s, c><<<g2, SPG_TTHREADS, nsm, stream>>>(a);
+                        spgn_partition_kernel<s, c><<<gn, SPG_TTHREADS, nsm, stream>>>(a);
                         spgn_aggregate_kernel<s, c><<<spg_owners, SPG_THREADS, spgn_smem, stream>>>(a);
                     });
                     spgn_launches++;
@@ -2252,6 +2265,7 @@ class GroupbyState {
                         else spg_partition_tma_kernel<s, c><<<g2, SPG_TTHREADS, tsm, stream>>>(a);
                         spg_aggregate_kernel<s, c><<<spg_owners, SPG_THREADS, spg_smem, stream>>>(a);
                     });
+                    spg16_launches++;
                 }
             }
             B200_CUDA(cudaGetLastError());
@@ -2315,14 +2329,16 @@ class GroupbyState {
             double ta = now();
             d_bucket.ensure(device, (size_t)n_vo * bucket_cap * 16);
             if (v_nullable) d_nbucket.ensure(device, (size_t)spg_owners * bucket_cap * 8);
-            d_retry2[0].ensure(device, ((size_t)rows + (size_t)spg_owners * (spgg_ns[mm] + SPG_STASH) * passes) * GEN_RETRY_WORDS * 8);
+            // one entry per row at most (bucket overflow, carry, no room in the shared table), plus one per occupied slot per pass
+            const int64_t retry_cap = rows + (int64_t)spg_owners * (spgg_ns[mm] + SPG_STASH) * passes;
+            d_retry2[0].ensure(device, (size_t)retry_cap * GEN_RETRY_WORDS * 8);
             t_alloc += now() - ta;
             B200_CUDA(cudaMemsetAsync(d_bucket_cnt.p, 0, (size_t)(n_vo + spg_owners) * SPG_CNT_STRIDE * 8, stream));
             auto make_args = [&]() {
                 SpgGenArgs g{};
                 g.s.n_rows = rows; g.s.n_owners = spg_owners;
                 g.s.tkeys = d_keys.as<long long>(); g.s.cap = cap; g.s.counters = d_counters.as<long long>(); g.s.group_limit = (long long)(cap / 2);
-                g.s.retry_ctr = d_counters.as<long long>() + CTR_FAIL; g.s.retry = d_retry2[0].as<unsigned long long>();
+                g.s.retry_ctr = d_counters.as<long long>() + CTR_FAIL; g.s.retry = d_retry2[0].as<unsigned long long>(); g.s.retry_cap = retry_cap;
                 g.s.bucket = d_bucket.as<longlong2>(); g.s.bucket_cnt = d_bucket_cnt.as<unsigned long long>(); g.s.bucket_cap = bucket_cap;
                 g.s.ns = spgg_ns[mm]; g.s.n_pass = passes;
                 g.nbucket = v_nullable ? d_nbucket.as<long long>() : nullptr; g.n_vo = n_vo;
@@ -3043,6 +3059,8 @@ int64_t b200_groupby_get_metric(void* state, int32_t which) {
         case 11: return s->co_batches;
         case 12: return s->spgg_launches;
         case 14: return s->spgn_launches;
+        case 15: return s->spg16_launches;
+        case 16: return s->spg_n_hot;
         case 13: { cudaSetDevice(s->device); s->read_counters(); return s->n_groups + s->untracked_groups; }  // exact (synchronises the stream)
         case 100: s->profiling = true; return 0;
         default: return -1;

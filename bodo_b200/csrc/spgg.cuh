@@ -43,10 +43,12 @@ struct SpgGenArgs {
     int dropna;
     GenFlush fl;
 };
-constexpr int GEN_RETRY_WORDS = 8;  // [key][sum][cnt][nnull][min][max][-][-]
+constexpr int GEN_RETRY_WORDS = 8;  // [key][sum][cnt][nnull][min][max][msum (double bits)][-]
 
-// one partial aggregate (sum / cnt / min / max over `cnt` non-NA values, plus `nnull` rows whose value was NA) -> slot `sl`
-__device__ __forceinline__ void gen_apply_slot(const GenFlush& f, uint64_t sl, unsigned long long sum, unsigned long long cnt,
+// one partial aggregate (sum / cnt / min / max over `cnt` non-NA values, plus `nnull` rows whose value was NA) -> slot `sl`.
+// `sum` is the partial sum mod 2^64 (SUM); `msum` is the same partial as a double (MEAN), given separately because a partial
+// need not fit a signed 64-bit word: a high-word piece can be +2^63, an NA-key partial any 128-bit value.
+__device__ __forceinline__ void gen_apply_slot(const GenFlush& f, uint64_t sl, unsigned long long sum, double msum, unsigned long long cnt,
                                                unsigned long long nnull, long long mn, long long mx) {
 #pragma unroll 1
     for (int j = 0; j < f.n; j++) {
@@ -55,7 +57,7 @@ __device__ __forceinline__ void gen_apply_slot(const GenFlush& f, uint64_t sl, u
             case K_COUNT: if (cnt) atomicAdd(f.a0[j] + sl, cnt); break;
             case K_SIZE: if (cnt + nnull) atomicAdd(f.a0[j] + sl, cnt + nnull); break;
             case K_MEAN:
-                if (sum) atomicAdd((double*)f.a0[j] + sl, (double)(long long)sum);
+                if (msum != 0.0) atomicAdd((double*)f.a0[j] + sl, msum);
                 if (cnt) atomicAdd(f.a1[j] + sl, cnt);
                 break;
             case K_MIN_I64:
@@ -68,7 +70,7 @@ __device__ __forceinline__ void gen_apply_slot(const GenFlush& f, uint64_t sl, u
     }
 }
 
-__device__ __forceinline__ void gen_direct_apply(const SpgGenArgs& g, long long key, unsigned long long sum, unsigned long long cnt,
+__device__ __forceinline__ void gen_direct_apply(const SpgGenArgs& g, long long key, unsigned long long sum, double msum, unsigned long long cnt,
                                               unsigned long long nnull, long long mn, long long mx) {
     const SpgArgs& a = g.s;
     uint64_t sl;
@@ -77,23 +79,25 @@ __device__ __forceinline__ void gen_direct_apply(const SpgGenArgs& g, long long 
         sl = find_or_insert(a.tkeys, a.cap, key, a.counters, a.group_limit);
         if (sl == ~0ull) {  // global table at its limit: park the partial, the host grows the table and replays it
             unsigned long long f = atomicAdd((unsigned long long*)a.retry_ctr, 1ull);
+            if (f >= (unsigned long long)a.retry_cap) { a.counters[CTR_RETRY_OVERFLOW] = 1; return; }
             unsigned long long* r = a.retry + f * GEN_RETRY_WORDS;
             r[0] = (unsigned long long)key; r[1] = sum; r[2] = cnt; r[3] = nnull; r[4] = (unsigned long long)mn; r[5] = (unsigned long long)mx;
+            r[6] = (unsigned long long)__double_as_longlong(msum);
             return;
         }
     }
-    gen_apply_slot(g.fl, sl, sum, cnt, nnull, mn, mx);
+    gen_apply_slot(g.fl, sl, sum, msum, cnt, nnull, mn, mx);
 }
 
 __global__ void spgg_replay_kernel(const __grid_constant__ SpgGenArgs g, const unsigned long long* rows, long long n) {
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         const unsigned long long* r = rows + i * GEN_RETRY_WORDS;
-        gen_direct_apply(g, (long long)r[0], r[1], r[2], r[3], (long long)r[4], (long long)r[5]);
+        gen_direct_apply(g, (long long)r[0], r[1], __longlong_as_double((long long)r[6]), r[2], r[3], (long long)r[4], (long long)r[5]);
     }
 }
 
 constexpr int GEN_CLS = 448;  // counting-sort classes of K1g: n_vo buckets of valued rows + n_owners buckets of NA-value rows
-constexpr size_t GEN_K1_SMEM = (size_t)SPG_TILE * 32 + GEN_CLS * 8 + 16 + 32 + GEN_CLS * 4 + (GEN_CLS + 4) * 4 + 2 * (SPG_TILE / 8 + 16) + 64;
+constexpr size_t GEN_K1_SMEM = (size_t)SPG_TILE * 32 + GEN_CLS * 8 + 16 + 48 + GEN_CLS * 4 + (GEN_CLS + 4) * 4 + 2 * (SPG_TILE / 8 + 16) + 64;
 
 template <int BYTES>
 __device__ __forceinline__ long long gen_widen(const void* raw, int j, int is_signed) {
@@ -115,7 +119,8 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPG_TCTAS) spgg_partition_kernel
     unsigned long long* na_sum = (unsigned long long*)(mbar + 2);                 // NA-key group, this CTA's partial aggregate
     long long* na_min = (long long*)(na_sum + 1);
     long long* na_max = na_min + 1;
-    unsigned int* na_cnt = (unsigned int*)(na_max + 1);                           // [0] non-NA values, [1] NA values
+    long long* na_hi = na_max + 1;                                                // high word of the 128-bit sum (MEAN); 8 bytes pad
+    unsigned int* na_cnt = (unsigned int*)(na_hi + 2);                            // [0] non-NA values, [1] NA values
     unsigned int* hist = na_cnt + 2;                                              // GEN_CLS
     unsigned int* lbase = hist + GEN_CLS;                                         // GEN_CLS + 4
     unsigned char* kvb = (unsigned char*)(lbase + GEN_CLS + 4);                   // 256 + 16 validity bytes of the tile's keys
@@ -127,7 +132,7 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPG_TCTAS) spgg_partition_kernel
     if (tid == 0) {
         mbar_init(&mbar[0], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        *na_sum = 0; *na_min = INT64_MAX; *na_max = INT64_MIN; na_cnt[0] = 0; na_cnt[1] = 0;
+        *na_sum = 0; *na_hi = 0; *na_min = INT64_MAX; *na_max = INT64_MIN; na_cnt[0] = 0; na_cnt[1] = 0;
     }
     for (int j = tid; j < C; j += SPG_TTHREADS) hist[j] = 0;
     __syncthreads();
@@ -172,7 +177,10 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPG_TCTAS) spgg_partition_kernel
             if (!kok) {  // NA key: dropped, or this CTA's share of the NA group
                 if (!g.dropna) {
                     if (vok) {
-                        atomicAdd(na_sum, (unsigned long long)v);
+                        // na_sum alone may wrap (SUM is mod 2^64); MEAN gets the exact 128-bit sum: sign extension + carry
+                        const unsigned long long old = atomicAdd(na_sum, (unsigned long long)v);
+                        const long long dh = (v < 0 ? -1ll : 0ll) + (old + (unsigned long long)v < old ? 1ll : 0ll);
+                        if (dh) atomicAdd((unsigned long long*)na_hi, (unsigned long long)dh);
                         atomicAdd(&na_cnt[0], 1u);
                         if (v < *na_min) atomicMin(na_min, v);
                         if (v > *na_max) atomicMax(na_max, v);
@@ -180,7 +188,7 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPG_TCTAS) spgg_partition_kernel
                 }
                 continue;
             }
-            if (k == EMPTY_KEY) { gen_direct_apply(g, k, vok ? (unsigned long long)v : 0ull, vok ? 1ull : 0ull, vok ? 0ull : 1ull, v, v); continue; }
+            if (k == EMPTY_KEY) { gen_direct_apply(g, k, vok ? (unsigned long long)v : 0ull, vok ? (double)v : 0.0, vok ? 1ull : 0ull, vok ? 0ull : 1ull, v, v); continue; }
             cls[r] = vok ? (int)spg_owner(spg_hash(k), NVO) : NVO + (int)spg_owner(spg_hash(k), G);
             rk[r] = atomicAdd(&hist[cls[r]], 1u);
         }
@@ -219,12 +227,12 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPG_TCTAS) spgg_partition_kernel
                 const unsigned int c = spg_owner(h, NVO);
                 const unsigned long long off = gbase[c] + p;
                 if (off < (unsigned long long)a.bucket_cap) a.bucket[(size_t)c * a.bucket_cap + off] = row;
-                else gen_direct_apply(g, row.x, (unsigned long long)row.y, 1ull, 0ull, row.y, row.y);  // bucket full (skew)
+                else gen_direct_apply(g, row.x, (unsigned long long)row.y, (double)row.y, 1ull, 0ull, row.y, row.y);  // bucket full (skew)
             } else {
                 const unsigned int o = spg_owner(h, G);
                 const unsigned long long off = gbase[NVO + o] + p;
                 if (off < (unsigned long long)a.bucket_cap) g.nbucket[(size_t)o * a.bucket_cap + off] = row.x;
-                else gen_direct_apply(g, row.x, 0ull, 0ull, 1ull, 0, 0);
+                else gen_direct_apply(g, row.x, 0ull, 0.0, 0ull, 1ull, 0, 0);
             }
         }
         for (int j = tid; j < C; j += SPG_TTHREADS) hist[j] = 0;
@@ -232,7 +240,8 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPG_TCTAS) spgg_partition_kernel
     }
     if (tid == 0 && (na_cnt[0] | na_cnt[1])) {  // NA-key group (slot cap of the state's table)
         a.counters[CTR_NA] = 1;
-        gen_apply_slot(g.fl, a.cap, *na_sum, (unsigned long long)na_cnt[0], (unsigned long long)na_cnt[1], *na_min, *na_max);
+        const double msum = (double)*na_hi * 18446744073709551616.0 + (double)*na_sum;  // na_hi * 2^64 + the unsigned low word
+        gen_apply_slot(g.fl, a.cap, *na_sum, msum, (unsigned long long)na_cnt[0], (unsigned long long)na_cnt[1], *na_min, *na_max);
     }
 }
 
@@ -263,8 +272,11 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgg_aggregate_kernel(const __
         if (HAS_SUM) {
             unsigned int lo = (unsigned int)(unsigned long long)val, hi = (unsigned int)((unsigned long long)val >> 32);
             unsigned int old = atomicAdd(&slo[s], lo);
-            hi += (old + lo < old) ? 1u : 0u;
-            if (hi) gen_direct_apply(g, key, (unsigned long long)hi << 32, 0ull, 0ull, 0, 0);
+            const unsigned int carry = (old + lo < old) ? 1u : 0u;
+            hi += carry;
+            // the piece is (val >> 32) + carry in units of 2^32: +2^63 when the high word is 0x7FFFFFFF and the low word carries,
+            // which the 64-bit word reads as -2^63, so MEAN takes the signed value
+            if (hi) gen_direct_apply(g, key, (unsigned long long)hi << 32, (double)((val >> 32) + carry) * 4294967296.0, 0ull, 0ull, 0, 0);
         }
         atomicAdd(&scnt[s], 1u);
         if (HAS_MM) {
@@ -308,7 +320,7 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgg_aggregate_kernel(const __
     };
     auto slow_upsert = [&](long long key, long long val) {
         const int s = slow_slot(key);
-        if (s < 0) { gen_direct_apply(g, key, (unsigned long long)val, 1ull, 0ull, val, val); return; }
+        if (s < 0) { gen_direct_apply(g, key, (unsigned long long)val, (double)val, 1ull, 0ull, val, val); return; }
         add(s, key, val);
     };
 
@@ -370,7 +382,7 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgg_aggregate_kernel(const __
             const long long key = __ldcs(nsrc + p);
             if (NP > 1 && __umulhi((unsigned int)(spg_hash(key) >> 32), GP) - (unsigned int)me * NP != pass) continue;
             const int s = slow_slot(key);  // looks the four candidates up first
-            if (s < 0) gen_direct_apply(g, key, 0ull, 0ull, 1ull, 0, 0);
+            if (s < 0) gen_direct_apply(g, key, 0ull, 0.0, 0ull, 1ull, 0, 0);
             else if (HAS_NN) atomicAdd(&snull[s], 1u);
         }
         __syncthreads();
@@ -378,7 +390,7 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgg_aggregate_kernel(const __
             long long key = skeys[s];
             if (key == EMPTY_KEY) continue;
             unsigned long long sum = HAS_SUM ? (unsigned long long)slo[s] - 0x80000000ull : 0ull;
-            gen_direct_apply(g, key, sum, (unsigned long long)scnt[s], HAS_NN ? (unsigned long long)snull[s] : 0ull, HAS_MM ? smin[s] : 0, HAS_MM ? smax[s] : 0);
+            gen_direct_apply(g, key, sum, (double)(long long)sum, (unsigned long long)scnt[s], HAS_NN ? (unsigned long long)snull[s] : 0ull, HAS_MM ? smin[s] : 0, HAS_MM ? smax[s] : 0);
         }
         __syncthreads();
     }

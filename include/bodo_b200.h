@@ -129,7 +129,9 @@ void b200_delete_groupby_state(void* state);
  * (SPG) launches, 9 rows/partials replayed from the SPG retry lists, 10 low-cardinality (LC) launches, 11 small batches
  * that were coalesced on the device before a fast-path launch, 12 SPG launches of the generic signature (SPG-G: nullable /
  * 4-byte keys or values, mean / min / max; included in 8), 13 groups in the table right now (exact: reads the device counter,
- * synchronises the state's stream), 14 SPG launches with narrow (int32 key, int32 value) bucket rows (SPG-N; included in 8). */
+ * synchronises the state's stream), 14 SPG launches with narrow (int32 key, int32 value) bucket rows (SPG-N; included in 8),
+ * 15 SPG launches with 16-byte (int64 key, int64 value) bucket rows (included in 8), 16 heavy-hitter keys admitted to the
+ * partition kernel's hot table (0 when there are none or the table is disabled). */
 /* nunique keeps one nested distinct state over (key, value) per value column (owned by `state`).  A sharded caller exchanges every
  * nested state (b200_groupby_exchange_fused_pack / _combine + b200_groupby_finalize on the handle returned here — a key's pairs are
  * owned where the key is owned) BEFORE it exchanges and finalizes the outer state; single-GPU callers never need these. */

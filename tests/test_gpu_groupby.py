@@ -157,14 +157,16 @@ def test_sm_partitioned_path_vs_oracle(gpu_lib, oracle, n_groups, hint, funcs):
                             expected_groups=hint, output_batch_size=1 << 30)
     dt = table_to_device(t)
     groupby_build_consume_batch(st, dt, True, True)
-    used_spg = get_metric(st, 8)
+    used = {m: get_metric(st, m) for m in (8, 10, 14, 15)}
     out, last = groupby_produce_output_batch(st, True)
     got = out.to_pandas()
     delete_groupby_state(st)
     exp = oracle_groupby_frame(oracle, t, 0, list(funcs), [None if f == "size" else 1 for f in funcs])
     assert_frames_equal(positional(got), exp)
-    if n_groups <= 1_000_000:
-        assert used_spg >= 1, "the SM-partitioned kernel was expected to run for this shape"
+    # synth_fill keys and values fit 32 bits: an estimate of at most 1024 groups (the 1000-group prefix, the hint 16) takes the
+    # low-cardinality kernel (metric 10), any other the narrow-row pair (metric 14); the 16-byte pair (metric 15) never runs
+    lowcard = (hint or n_groups) <= 1024
+    assert used[10 if lowcard else 14] >= 1 and used[15] == 0, f"expected the {'low-cardinality' if lowcard else 'narrow-row'} kernels, metrics {used}"
 
 
 @pytest.mark.timeout(300)
@@ -542,9 +544,9 @@ def test_narrow_row_sm_partitioned_path_exact_with_wide_stragglers(gpu_lib, orac
     st = init_groupby_state(-1, (0,), funcs, tuple(range(nf + 1)) if "size" not in funcs else (0, 0), (1,) * (0 if funcs == ("size",) else nf),
                             expected_groups=ng, output_batch_size=1 << 30)
     groupby_build_consume_batch(st, table_to_device(t), True, True)
-    used = get_metric(st, 14)
+    used, wide = get_metric(st, 14), get_metric(st, 15)
     out, _ = groupby_produce_output_batch(st, True)
     got = out.to_pandas()
     delete_groupby_state(st)
-    assert used >= 1, "the narrow-row kernels were expected to run for this shape"
+    assert used >= 1 and wide == 0, "the narrow-row kernels (and not the 16-byte ones) were expected to run for this shape"
     assert_frames_equal(positional(got), oracle_groupby_frame(oracle, t, 0, list(funcs), [None if f == "size" else 1 for f in funcs]))
