@@ -35,8 +35,21 @@ constexpr int EX_MAX_COLS = 32;
 
 struct ExprInstr { int32_t op; int32_t pad; int64_t arg; };
 
-struct ExprVal { int64_t bits; bool is_f; bool valid; };
-__device__ __forceinline__ double ev_f(const ExprVal& v) { return v.is_f ? __longlong_as_double(v.bits) : (double)v.bits; }
+// is_u: the value came straight from a UINT64 column, so `bits` holds it as uint64 (values >= 2^63 read as negative int64).
+// Comparisons and conversions to double honour it; arithmetic, negation and casts clear it (uint64 arithmetic wraps as int64).
+struct ExprVal { int64_t bits; bool is_f; bool valid; bool is_u; };
+__device__ __forceinline__ double ev_f(const ExprVal& v) {
+    return v.is_f ? __longlong_as_double(v.bits) : v.is_u ? (double)(unsigned long long)v.bits : (double)v.bits;
+}
+// Truthiness of a value (and / or / not, the predicate, BOOL stores): value != 0, so a float -0.0 is false and NaN is true.
+__device__ __forceinline__ bool ev_true(const ExprVal& v) { return v.is_f ? __longlong_as_double(v.bits) != 0.0 : v.bits != 0; }
+// Three-way order of two integer values, exact when either is a uint64 >= 2^63: such a value is above every int64, and two of
+// them order like their (top-bit-set) int64 bit patterns.
+__device__ __forceinline__ int ev_cmp_int(const ExprVal& x, const ExprVal& y) {
+    const bool xbig = x.is_u && x.bits < 0, ybig = y.is_u && y.bits < 0;
+    if (xbig != ybig) return xbig ? 1 : -1;
+    return x.bits < y.bits ? -1 : x.bits > y.bits ? 1 : 0;
+}
 
 struct FilterProjectArgs {
     int64_t n_rows;
@@ -67,17 +80,19 @@ __device__ __forceinline__ ExprVal expr_eval(const FilterProjectArgs& a, int pc,
                 ExprVal v;
                 v.valid = bit_valid(a.in_valid[c], row);
                 v.is_f = ctype_is_float(ct);
+                v.is_u = ct == CT_UINT64;
                 v.bits = v.is_f ? __double_as_longlong(load_as_f64(a.in_data[c], ct, row)) : load_int_as_i64(a.in_data[c], ct, row);
                 if (v.is_f && isnan(__longlong_as_double(v.bits))) v.valid = false;  // NaN is NA for float columns (isnan_alltype)
                 st[sp++] = v;
                 break;
             }
-            case EX_CONST_I64: st[sp++] = ExprVal{in.arg, false, true}; break;
-            case EX_CONST_F64: st[sp++] = ExprVal{in.arg, true, true}; break;
+            case EX_CONST_I64: st[sp++] = ExprVal{in.arg, false, true, false}; break;
+            case EX_CONST_F64: st[sp++] = ExprVal{in.arg, true, true, false}; break;
             case EX_ADD: case EX_SUB: case EX_MUL: case EX_DIV: {
                 const ExprVal b = st[--sp], x = st[--sp];
                 ExprVal r;
                 r.valid = x.valid && b.valid;
+                r.is_u = false;
                 r.is_f = x.is_f || b.is_f || in.op == EX_DIV;  // true division, as pandas' `/`
                 if (r.is_f) {
                     const double p = ev_f(x), q = ev_f(b);
@@ -97,41 +112,48 @@ __device__ __forceinline__ ExprVal expr_eval(const FilterProjectArgs& a, int pc,
                     const double p = ev_f(x), q = ev_f(b);
                     t = in.op == EX_LT ? p < q : in.op == EX_LE ? p <= q : in.op == EX_GT ? p > q : in.op == EX_GE ? p >= q : in.op == EX_EQ ? p == q : p != q;
                 } else {
-                    const int64_t p = x.bits, q = b.bits;
-                    t = in.op == EX_LT ? p < q : in.op == EX_LE ? p <= q : in.op == EX_GT ? p > q : in.op == EX_GE ? p >= q : in.op == EX_EQ ? p == q : p != q;
+                    const int c = ev_cmp_int(x, b);
+                    t = in.op == EX_LT ? c < 0 : in.op == EX_LE ? c <= 0 : in.op == EX_GT ? c > 0 : in.op == EX_GE ? c >= 0 : in.op == EX_EQ ? c == 0 : c != 0;
                 }
-                st[sp++] = ExprVal{t ? 1 : 0, false, x.valid && b.valid};
+                st[sp++] = ExprVal{t ? 1 : 0, false, x.valid && b.valid, false};
                 break;
             }
             case EX_AND: case EX_OR: {  // Kleene logic
                 const ExprVal b = st[--sp], x = st[--sp];
-                const bool xt = x.valid && x.bits != 0, xf = x.valid && x.bits == 0, bt = b.valid && b.bits != 0, bf = b.valid && b.bits == 0;
+                const bool xt = x.valid && ev_true(x), xf = x.valid && !ev_true(x), bt = b.valid && ev_true(b), bf = b.valid && !ev_true(b);
                 ExprVal r;
-                r.is_f = false;
+                r.is_f = false; r.is_u = false;
                 if (in.op == EX_AND) { r.valid = (xf || bf) || (x.valid && b.valid); r.bits = (xt && bt) ? 1 : 0; }
                 else { r.valid = (xt || bt) || (x.valid && b.valid); r.bits = (xt || bt) ? 1 : 0; }
                 st[sp++] = r;
                 break;
             }
-            case EX_NOT: { ExprVal& x = st[sp - 1]; x.bits = x.bits == 0 ? 1 : 0; x.is_f = false; break; }
-            case EX_NEG: { ExprVal& x = st[sp - 1]; x.bits = x.is_f ? __double_as_longlong(-__longlong_as_double(x.bits)) : (int64_t)(0ull - (unsigned long long)x.bits); break; }
-            case EX_TO_F64: { ExprVal& x = st[sp - 1]; if (!x.is_f) { x.bits = __double_as_longlong((double)x.bits); x.is_f = true; } break; }
-            case EX_TO_I64: { ExprVal& x = st[sp - 1]; if (x.is_f) { x.bits = (int64_t)__longlong_as_double(x.bits); x.is_f = false; } break; }
-            case EX_IS_NULL: { ExprVal& x = st[sp - 1]; x.bits = x.valid ? 0 : 1; x.is_f = false; x.valid = true; break; }
+            case EX_NOT: { ExprVal& x = st[sp - 1]; x.bits = ev_true(x) ? 0 : 1; x.is_f = false; x.is_u = false; break; }
+            case EX_NEG: { ExprVal& x = st[sp - 1]; x.bits = x.is_f ? __double_as_longlong(-__longlong_as_double(x.bits)) : (int64_t)(0ull - (unsigned long long)x.bits); x.is_u = false; break; }
+            case EX_TO_F64: { ExprVal& x = st[sp - 1]; if (!x.is_f) { x.bits = __double_as_longlong(ev_f(x)); x.is_f = true; x.is_u = false; } break; }
+            // float -> int truncates toward zero; NaN and values outside int64 saturate (numpy leaves those undefined)
+            case EX_TO_I64: { ExprVal& x = st[sp - 1]; if (x.is_f) { x.bits = (int64_t)__longlong_as_double(x.bits); x.is_f = false; } x.is_u = false; break; }
+            case EX_IS_NULL: { ExprVal& x = st[sp - 1]; x.bits = x.valid ? 0 : 1; x.is_f = false; x.is_u = false; x.valid = true; break; }
             default: break;
         }
     }
     return st[sp - 1];
 }
 
+// Stores a value as the output's CType the way numpy's astype converts it (for values the type can hold): a float becomes an
+// integer of any width by truncation toward zero (through int64, or uint64 for a UINT64 output), an integer keeps its low
+// bytes, an integer becomes FLOAT32 in one rounding, and BOOL stores value != 0.
 __device__ __forceinline__ void store_val(void* out, int ct, int64_t i, const ExprVal& v) {
+    const double d = __longlong_as_double(v.bits);
+    const int64_t iv = !v.is_f ? v.bits : ct == CT_UINT64 ? (int64_t)(unsigned long long)d : (int64_t)d;
     switch (ct) {
         case CT_FLOAT64: ((double*)out)[i] = ev_f(v); break;
-        case CT_FLOAT32: ((float*)out)[i] = (float)ev_f(v); break;
-        case CT_INT64: case CT_UINT64: case CT_DATETIME: case CT_TIMEDELTA: ((int64_t*)out)[i] = v.is_f ? (int64_t)__longlong_as_double(v.bits) : v.bits; break;
-        case CT_INT32: case CT_UINT32: case CT_DATE: ((int32_t*)out)[i] = (int32_t)(v.is_f ? (int64_t)__longlong_as_double(v.bits) : v.bits); break;
-        case CT_INT16: case CT_UINT16: ((int16_t*)out)[i] = (int16_t)v.bits; break;
-        default: ((int8_t*)out)[i] = (int8_t)v.bits; break;
+        case CT_FLOAT32: ((float*)out)[i] = v.is_f ? (float)d : v.is_u ? (float)(unsigned long long)v.bits : (float)v.bits; break;
+        case CT_BOOL: ((uint8_t*)out)[i] = ev_true(v) ? 1 : 0; break;
+        case CT_INT64: case CT_UINT64: case CT_DATETIME: case CT_TIMEDELTA: ((int64_t*)out)[i] = iv; break;
+        case CT_INT32: case CT_UINT32: case CT_DATE: ((int32_t*)out)[i] = (int32_t)iv; break;
+        case CT_INT16: case CT_UINT16: ((int16_t*)out)[i] = (int16_t)iv; break;
+        default: ((int8_t*)out)[i] = (int8_t)iv; break;
     }
 }
 
@@ -151,7 +173,7 @@ __global__ void __launch_bounds__(FP_THREADS) filter_project_kernel(const __grid
             keep[r] = row < a.n_rows;
             if (keep[r] && a.pred_start >= 0) {
                 const ExprVal p = expr_eval(a, a.pred_start, row);
-                keep[r] = p.valid && p.bits != 0;
+                keep[r] = p.valid && ev_true(p);
             }
             const unsigned m = __ballot_sync(0xffffffffu, keep[r]);
             rank[r] = __popc(m & ((1u << lane) - 1));
@@ -200,7 +222,9 @@ int64_t b200_filter_project(const b200_table* in_table, const void* program, int
         using namespace b200;
         B200_REQUIRE(in_table && program && out && out->cols && (n_out == 0 || out_starts), "b200_filter_project: null argument");
         B200_REQUIRE(in_table->device >= 0, "b200_filter_project: the table must be device resident (this path has no CPU fallback)");
-        B200_REQUIRE(in_table->n_cols <= EX_MAX_COLS && n_out <= EX_MAX_OUT && n_instr <= EX_MAX_INSTR && n_instr >= 1, "b200_filter_project: too many columns / outputs / instructions");
+        B200_REQUIRE(in_table->n_cols <= EX_MAX_COLS, "b200_filter_project: the input table has more than 32 columns");
+        B200_REQUIRE(n_out >= 0 && n_out <= EX_MAX_OUT, "b200_filter_project: more than 16 output columns");
+        B200_REQUIRE(n_instr >= 1 && n_instr <= EX_MAX_INSTR, "b200_filter_project: the program needs 1 to 64 instructions");
         cudaStream_t st = (cudaStream_t)stream;
         B200_CUDA(cudaSetDevice(in_table->device)); scratch_set_stream(st);
         FilterProjectArgs a{};
@@ -226,6 +250,11 @@ int64_t b200_filter_project(const b200_table* in_table, const void* program, int
             max_depth = std::max(max_depth, depth);
         }
         B200_REQUIRE(max_depth <= EX_MAX_STACK && prog[n_instr - 1].op == EX_END, "b200_filter_project: program too deep or not terminated");
+        // an expression starts at instruction 0 or right after an END; any other start would run the VM off its checked depth
+        auto starts_expr = [&](int32_t s) { return s == 0 || (s > 0 && s < n_instr && prog[s - 1].op == EX_END); };
+        B200_REQUIRE(pred_start == -1 || starts_expr(pred_start), "b200_filter_project: pred_start does not start an expression");
+        for (int j = 0; j < n_out; j++)
+            B200_REQUIRE(starts_expr(out_starts[j]), "b200_filter_project: out_starts[j] does not start an expression");
         a.pred_start = pred_start;
         a.n_out = n_out;
         DevBuf cursor;

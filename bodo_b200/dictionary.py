@@ -6,7 +6,8 @@ Every batch arrives with its own dictionary (Arrow DictionaryArray, or a plain s
 batch).  The builder keeps ONE growing dictionary per key column; a batch's dictionary is matched against it on the host
 (dictionaries are small: distinct strings, not rows) and the batch's index column is rewritten to global ids on the device
 (b200_remap_i32: the `transpose` step of UnifyDictionaryArray).  The operators then see an ordinary int32 key column; output
-ids are decoded back through the same dictionary.  NA stays NA (validity bitmap of the index column).
+ids are decoded back through the same dictionary.  NA stays NA: a null index and an index to a null dictionary entry both
+become a NA row (validity bitmap of the id column).
 """
 
 from __future__ import annotations
@@ -29,6 +30,9 @@ class DictionaryBuilder:
         """global ids of a batch dictionary (pyarrow string array); new strings are appended (InsertIfNotExists)."""
         ids = np.empty(len(batch_dictionary), dtype=np.int32)
         for j, s in enumerate(batch_dictionary.to_pylist()):
+            if s is None:  # null entries get no global id: the rows that use them are NA (unify)
+                ids[j] = 0
+                continue
             g = self.index.get(s)
             if g is None:
                 g = len(self.values)
@@ -43,6 +47,9 @@ class DictionaryBuilder:
         import torch
 
         if isinstance(arr, pa.ChunkedArray):
+            if pa.types.is_dictionary(arr.type) and arr.num_chunks > 1 and any(c.dictionary.null_count for c in arr.chunks):
+                # Arrow cannot concatenate dictionaries with null entries: decode the chunks (those entries become null rows)
+                arr = pa.chunked_array([c.cast(arr.type.value_type) for c in arr.chunks])
             arr = arr.combine_chunks()
         if not pa.types.is_dictionary(arr.type):
             arr = arr.dictionary_encode()
@@ -55,8 +62,10 @@ class DictionaryBuilder:
         host_idx = np.frombuffer(bufs[1], dtype=np.int32)[off: off + n] if n else np.empty(0, np.int32)
         d_idx = torch.from_numpy(np.ascontiguousarray(host_idx)).to(dev)
         validity = None
-        if idx.null_count > 0:
-            mask = np.asarray(idx.is_valid())
+        mask = np.asarray(idx.is_valid())
+        if arr.dictionary.null_count > 0:  # a row whose dictionary entry is null is NA too
+            mask = mask & np.asarray(arr.dictionary.is_valid())[np.where(mask, host_idx, 0)]
+        if not mask.all():
             vb = np.packbits(mask, bitorder="little")
             pad = np.zeros((len(vb) + 15) // 8 * 8, dtype=np.uint8)
             pad[: len(vb)] = vb

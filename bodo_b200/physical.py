@@ -121,6 +121,8 @@ class PhysicalFilterProject:
     def __init__(self, predicate, outputs, device: int | None = None, stream: int = 0):
         self.predicate = predicate
         self.outputs = list(outputs)
+        if not self.outputs:  # a batch is a list of columns: without one it could not say how many rows were kept
+            raise ValueError("PhysicalFilterProject needs at least one output column")
         self.device = device
         self.stream = stream
         self._compiled = None
@@ -173,7 +175,8 @@ class PhysicalFilterProject:
 
 def filter_project_table(table: Table, keep) -> Table:
     """Rows of a device-resident `table` whose entry in `keep` (uint8 device tensor, one byte per row) is non-zero, through the
-    fused filter kernel (used by streaming.join.runtime_join_filter)."""
+    fused filter kernel (used by streaming.join.runtime_join_filter).  Every column is one output of the kernel, so a table of
+    more than 16 columns raises B200Error."""
     from .expr import col
     from .table import ArrTypes, Column, CTypes
 

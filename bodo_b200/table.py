@@ -281,8 +281,12 @@ def column_from_pandas(s) -> Column:
     if a.dtype.kind in "Mm":
         # DATETIME / TIMEDELTA columns are int64 NANOSECONDS (Bodo_CTypes, _bodo_common.h:331-359): pandas >= 3 hands out
         # datetime64[us] (and [s]/[ms] on request), so the unit is normalised before the storage is reinterpreted
+        # NaT is NA (the reference converts every pandas slice to Arrow first, read_pandas.h, and Arrow makes NaT null)
         ct = CTypes.DATETIME if a.dtype.kind == "M" else CTypes.TIMEDELTA
         a = a.astype("datetime64[ns]" if a.dtype.kind == "M" else "timedelta64[ns]", copy=False)
+        nat = np.isnat(a)
+        if nat.any():
+            return Column(np.ascontiguousarray(a.view("int64")), np.packbits(~nat, bitorder="little"), ct, ArrTypes.NULLABLE_INT_BOOL)
         return Column(np.ascontiguousarray(a.view("int64")), None, ct)
     if a.dtype == object:
         raise TypeError(f"bodo_b200: column '{s.name}' has object dtype (strings are a 'next' row, SURVEY.md §8f)")
@@ -340,6 +344,9 @@ def column_to_pandas(c: Column, stream: int = 0):
     if vals.dtype.kind in "Mm" and mask is not None and not mask.all():
         vals = vals.copy()
         vals[~mask] = np.datetime64("NaT") if vals.dtype.kind == "M" else np.timedelta64("NaT")
+    if c.arr_type == ArrTypes.NULLABLE_INT_BOOL and c.c_type == CTypes.BOOL:
+        m = ~mask if mask is not None else np.zeros(len(vals), dtype=bool)
+        return pd.array(pd.arrays.BooleanArray(vals.astype(bool), m), dtype="boolean")
     if c.arr_type == ArrTypes.NULLABLE_INT_BOOL and vals.dtype.kind in "iuf":
         name = {"i": "Int", "u": "UInt", "f": "Float"}[vals.dtype.kind] + str(vals.dtype.itemsize * 8)
         m = ~mask if mask is not None else np.zeros(len(vals), dtype=bool)

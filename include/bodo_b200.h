@@ -253,13 +253,15 @@ int b200_merge_segment_bitmaps(const uint8_t* segments, const int64_t* counts, i
 /* One postfix instruction: op (EX_* below) + 64-bit argument (column index, or the bits of an int64 / double constant).
  * EX_COL=0 CONST_I64=1 CONST_F64=2 ADD=3 SUB=4 MUL=5 DIV=6 LT=7 LE=8 GT=9 GE=10 EQ=11 NE=12 AND=13 OR=14 NOT=15
  * TO_F64=16 TO_I64=17 IS_NULL=18 NEG=19 END=20.  A program is a sequence of expressions, each terminated by END and
- * leaving one value; arithmetic / comparisons propagate NA, AND / OR are Kleene, a NA predicate drops the row. */
+ * leaving one value; arithmetic / comparisons propagate NA, AND / OR are Kleene, a NA predicate drops the row.  AND / OR /
+ * NOT and the predicate take value != 0 as true (a float -0.0 is false, NaN read from a float column is NA). */
 typedef struct b200_expr_instr { int32_t op; int32_t pad; int64_t arg; } b200_expr_instr;
 
 /* Evaluates the predicate (expression starting at instruction pred_start; -1 = keep every row) and the n_out output
  * expressions (starting at out_starts[j]) of every row of a device-resident table in ONE kernel, compacting the surviving
  * rows: out->cols[j] (device buffers of in_table->n_rows items provided by the caller, c_type = storage type, validity =
- * bitmap buffer or NULL) receive the rows that pass.  Returns the number of output rows (< 0 on error). */
+ * bitmap buffer or NULL) receive the rows that pass, in an unspecified order (each 1024-row tile claims its place with an
+ * atomic cursor).  Every start must be 0 or follow an END.  Returns the number of output rows (< 0 on error). */
 int64_t b200_filter_project(const b200_table* in_table, const void* program, int32_t n_instr, int32_t pred_start,
                             const int32_t* out_starts, int32_t n_out, b200_table* out, void* stream);
 
