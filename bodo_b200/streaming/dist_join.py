@@ -239,7 +239,6 @@ class DistJoinState:
         dist.all_reduce(tot, group=self.group)
         n_blocks = int(tot.item()) // 32 + 1
         words, bounds = J.build_runtime_filter(self.local, n_blocks)
-        bounds = [bounds] if len(self.build_keys) == 1 else bounds
         gathered = torch.empty(self.n_pes * words.numel(), dtype=words.dtype, device=dev)
         dist.all_gather_into_tensor(gathered, words, group=self.group)  # NCCL has no bitwise-or reduction
         acc = gathered.view(self.n_pes, -1)[0].clone()

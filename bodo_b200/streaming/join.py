@@ -178,8 +178,8 @@ def delete_join_state(join_state: JoinState) -> None:
 
 def build_runtime_filter(join_state, n_bloom_blocks: int = 0):
     """Build the bloom filter + key bounds of a finished build side; returns (bloom words as a device tensor aliasing the
-    state's memory, (key_min, key_max)), or for a multi-column key [(min, max) of each key column].  Sharded joins OR / min / max
-    these across ranks (dist_join.DistJoinState does)."""
+    state's memory, [(min, max) of each key column]).  Sharded joins OR / min / max these across ranks (dist_join.DistJoinState
+    does)."""
     import torch
 
     st = getattr(join_state, "local", join_state)
@@ -192,8 +192,7 @@ def build_runtime_filter(join_state, n_bloom_blocks: int = 0):
     from ..table import DeviceArray
 
     words = torch.as_tensor(DeviceArray(int(ffi.cast("uintptr_t", ptr[0])), int(nb[0]) * 8, "int32", st.device, owner=st), device=torch.device("cuda", st.device))
-    bounds = [(int(mm[2 * j]), int(mm[2 * j + 1])) for j in range(nk)]
-    return words, (bounds[0] if nk == 1 else bounds)
+    return words, [(int(mm[2 * j]), int(mm[2 * j + 1])) for j in range(nk)]
 
 
 def runtime_join_filter(join_states, table: Table, join_keys_idxs, process_col_bitmasks=None) -> Table:

@@ -238,7 +238,7 @@ def test_runtime_join_filter_has_no_false_negatives(gpu_lib):
     probe.loc[::1000, "k"] = pd.NA
     st = init_join_state(-1, (0,), (1,), tuple(build.columns), tuple(probe.columns), False, False)
     join_build_consume_batch(st, table_to_device(Table.from_pandas(build)), True)
-    words, (mn, mx) = build_runtime_filter(st)
+    words, [(mn, mx)] = build_runtime_filter(st)
     assert (mn, mx) == (int(bk.min()), int(bk.max())) and words.numel() == (nb // 32 + 1) * 8
     kept = runtime_join_filter((st,), table_to_device(Table.from_pandas(probe)), ((1,),)).to_pandas()
     partner = probe.k.isin(bk).fillna(False).to_numpy()

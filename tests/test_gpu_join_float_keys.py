@@ -257,7 +257,7 @@ def test_runtime_filter(gpu_lib):
     probe = pd.DataFrame({"p0": rng.random(npr), "k": pk})
     st = init_join_state(-1, (0,), (1,), tuple(build.columns), tuple(probe.columns), False, False)
     join_build_consume_batch(st, table_to_device(Table.from_pandas(build)), True)
-    _, (mn, mx) = build_runtime_filter(st)
+    _, [(mn, mx)] = build_runtime_filter(st)
     assert decode_bound(mn) == np.nanmin(bk) == -INF and decode_bound(mx) == np.nanmax(bk)
     kept = runtime_join_filter((st,), table_to_device(Table.from_pandas(probe)), ((1,),)).to_pandas()
     bck, bcv = canon_keys(build.k)
@@ -351,7 +351,9 @@ def _sharded_worker(rank, world, port, q):
 def test_sharded_join_two_gpus(gpu_lib):
     """Shuffle, shuffle-outer and broadcast joins over the ranks: -0.0 build rows on rank 0 meet 0.0 probe rows on the last rank
     (both hash to one rank), and the union of the ranks' outputs equals the oracle's join of the global tables.  The inner case
-    runs with is_na_equal=False: its runtime filter drops NA-key probe rows."""
+    runs with is_na_equal=False, so its NaN probe rows match nothing and the runtime filter drops them before the shuffle; the
+    filter's handling of NA keys under is_na_equal=True is checked on one GPU (test_gpu_join_multi_keys.py,
+    test_runtime_filter_has_no_false_negatives)."""
     import socket
 
     import torch
