@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbodo_b200.so")
-SOURCES = ["misc.cu", "groupby.cu", "shuffle.cu", "join.cu", "expr.cu"]
+SOURCES = ["misc.cu", "groupby.cu", "shuffle.cu", "join.cu", "expr.cu", "sort.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper); the kernels use sm_90a TMA / mbarrier PTX
 NVCC_FLAGS = [
     *GENCODE, "-O3", "-lineinfo", "-std=c++17",

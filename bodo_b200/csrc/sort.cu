@@ -1,0 +1,503 @@
+// sort.cu — streaming top-k: ORDER BY k_0 .. k_{n-1} LIMIT limit OFFSET offset over a stream of batches (sm_90a).
+//
+// Replaces the LIMIT form of the reference's streaming sort state (bodo/libs/streaming/_sort.cpp: stream_sort_state_init_py_entry,
+// the build-consume and produce-output entries, delete_stream_sort_state), which DuckDB's TopN lowers to (PhysicalSort,
+// bodo/pandas/physical/sort.h).  Only the first K = limit + offset rows of the stable sort are ever needed, so the state keeps at
+// most K "held" rows and a device-resident cutoff, the key tuple of the K-th held row:
+//
+//   topk_filter_kernel   one pass per batch over the key columns only: a row survives iff its key tuple is strictly below the
+//                        cutoff (a row that ties the cutoff sorts after the held row, its arrival index is larger).  Survivors are
+//                        compacted (warp ballot -> tile scan -> one cursor atomic per tile) into the candidate store together with
+//                        their encoded keys, arrival index and every column; payload bytes are read for survivors only.
+//   reduce               held rows + candidates are sorted by (encoded keys, arrival index): topk_block_sort_kernel (bitonic sort
+//                        of 1024-row tiles in shared memory) then topk_merge_kernel passes (merge path over pairs of sorted runs,
+//                        every run cut to its first K rows); topk_gather_kernel moves the first K rows into the other store buffer
+//                        and writes the new cutoff.
+//
+// Key encoding: each key becomes one uint64 whose unsigned order is the key order (sign bit flipped for signed integers and
+// temporals; floats widened to double, -0.0 folded onto +0.0, then the order-preserving form; complemented for a descending
+// key) plus one NA-class bit (NA and NaN keys: word 0, class 1 for na_position="last", 0 for "first"; other keys the opposite
+// class).  Rows compare lexicographically over (class_0, word_0, class_1, word_1, ..., arrival index): no two rows are equal,
+// so the (unstable) bitonic sort still yields the stable order.
+#include <algorithm>
+#include <vector>
+
+#include "common.cuh"
+
+namespace b200 {
+
+constexpr int TK_MAX_KEYS = 4;
+constexpr int TK_MAX_COLS = 32;
+// K = limit + offset is capped so that store row ids (uint32, the sort permutation) and the two store buffers of max(2K, 4 Mi)
+// rows stay within reach: 2^26 rows is 2 x 128 Mi rows of store, about 5 GB per 8-byte column.
+constexpr int64_t TK_MAX_K = 1ll << 26;
+// Store capacity: max(2K, 4 Mi rows).  At least 2K so that a reduce (down to K rows) always frees at least K rows for the next
+// slice of a batch; at least 4 Mi rows so that, once a cutoff exists and few rows survive, the host needs to read the candidate
+// count only about once per 4 Mi consumed rows (it keeps an upper bound and reads only when that bound could overflow).
+constexpr int64_t TK_MIN_CAP = 1ll << 22;
+constexpr int TK_THREADS = 256, TK_ROWS = 4, TK_TILE = TK_THREADS * TK_ROWS;
+constexpr int TK_SORT_TILE = 1024, TK_SORT_THREADS = 512, TK_MERGE_ITEMS = 8;
+constexpr uint32_t TK_SENTINEL = 0xFFFFFFFFu;
+constexpr uint64_t TK_SIGN = 0x8000000000000000ull;
+
+struct TkCutoff { uint32_t has; uint32_t cls; uint64_t w[TK_MAX_KEYS]; };
+
+// One buffer of rows, structure of arrays: encoded key words, NA-class bits (bit j = key j), arrival index, every column's values
+// and, for nullable columns, one validity byte per row.
+struct TkStore {
+    uint64_t* w[TK_MAX_KEYS];
+    uint8_t* cls;
+    int64_t* seq;
+    void* data[TK_MAX_COLS];
+    uint8_t* vb[TK_MAX_COLS];
+};
+
+struct TkSchema {
+    int n_keys, n_cols;
+    int ctype[TK_MAX_COLS];
+    uint32_t desc_mask, na_last_mask;
+};
+
+struct TkFilterArgs {
+    TkSchema sc;
+    int64_t row0, row1;      // rows [row0, row1) of the batch
+    int64_t seq_base;        // arrival index of batch row 0
+    const void* in_data[TK_MAX_COLS];
+    const uint8_t* in_valid[TK_MAX_COLS];
+    const TkCutoff* cutoff;
+    TkStore st;
+    unsigned long long* cursor;  // rows in the store
+};
+
+__device__ __forceinline__ bool tk_signed(int ct) {
+    return ct == CT_INT8 || ct == CT_INT16 || ct == CT_INT32 || ct == CT_INT64 || ct == CT_DATE || ct == CT_DATETIME || ct == CT_TIMEDELTA;
+}
+
+// Encoded word of key column j at row i; *cls receives its NA-class bit.
+__device__ __forceinline__ uint64_t tk_encode(const TkSchema& sc, int j, const void* p, const uint8_t* valid, int64_t i, uint32_t* cls) {
+    const int ct = sc.ctype[j];
+    uint64_t w;
+    bool na = !bit_valid(valid, i);
+    if (ctype_is_float(ct)) {
+        const double d = load_as_f64(p, ct, i);
+        na = na || isnan(d);
+        w = (uint64_t)canon_float_ordered(canon_float_key(d)) ^ TK_SIGN;
+    } else {
+        const uint64_t v = (uint64_t)load_int_as_i64(p, ct, i);
+        w = tk_signed(ct) ? v ^ TK_SIGN : v;
+    }
+    const uint32_t na_last = (sc.na_last_mask >> j) & 1;
+    *cls = na ? na_last : na_last ^ 1;
+    if (na) return 0;
+    return ((sc.desc_mask >> j) & 1) ? ~w : w;
+}
+
+// The row's key tuple is strictly below the cutoff's.
+__device__ __forceinline__ bool tk_below_cutoff(const TkFilterArgs& a, const TkCutoff& c, int64_t row) {
+#pragma unroll
+    for (int j = 0; j < TK_MAX_KEYS; j++) {
+        if (j < a.sc.n_keys) {
+            uint32_t cl;
+            const uint64_t w = tk_encode(a.sc, j, a.in_data[j], a.in_valid[j], row, &cl);
+            const uint32_t cc = (c.cls >> j) & 1;
+            if (cl != cc) return cl < cc;
+            if (w != c.w[j]) return w < c.w[j];
+        }
+    }
+    return false;
+}
+
+__device__ __forceinline__ void tk_copy_cell(const void* src, int64_t si, void* dst, int64_t di, int size) {
+    switch (size) {
+        case 8: ((uint64_t*)dst)[di] = ((const uint64_t*)src)[si]; break;
+        case 4: ((uint32_t*)dst)[di] = ((const uint32_t*)src)[si]; break;
+        case 2: ((uint16_t*)dst)[di] = ((const uint16_t*)src)[si]; break;
+        default: ((uint8_t*)dst)[di] = ((const uint8_t*)src)[si]; break;
+    }
+}
+
+__global__ void __launch_bounds__(TK_THREADS, 4) topk_filter_kernel(const __grid_constant__ TkFilterArgs a) {
+    __shared__ unsigned int wsum[TK_ROWS][TK_THREADS / 32];
+    __shared__ unsigned long long tile_base;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const TkCutoff cut = *a.cutoff;
+    const int64_t n = a.row1 - a.row0;
+    const int64_t n_tiles = (n + TK_TILE - 1) / TK_TILE;
+    for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        bool keep[TK_ROWS];
+        unsigned int rank[TK_ROWS];
+#pragma unroll
+        for (int r = 0; r < TK_ROWS; r++) {
+            const int64_t row = a.row0 + t * TK_TILE + r * TK_THREADS + threadIdx.x;
+            keep[r] = row < a.row1 && (!cut.has || tk_below_cutoff(a, cut, row));
+            const unsigned m = __ballot_sync(0xffffffffu, keep[r]);
+            rank[r] = __popc(m & ((1u << lane) - 1));
+            if (lane == 0) wsum[r][warp] = __popc(m);
+        }
+        __syncthreads();
+        if (threadIdx.x < 32) {  // exclusive scan of the 32 (row slot, warp) counts; one cursor atomic per tile
+            const int r = threadIdx.x >> 3, w = threadIdx.x & 7;
+            unsigned int x = wsum[r][w], inc = x;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += y; }
+            wsum[r][w] = inc - x;
+            if (lane == 31) tile_base = inc ? atomicAdd(a.cursor, (unsigned long long)inc) : 0ull;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int r = 0; r < TK_ROWS; r++) {
+            if (!keep[r]) continue;
+            const int64_t row = a.row0 + t * TK_TILE + r * TK_THREADS + threadIdx.x;
+            const int64_t o = (int64_t)(tile_base + wsum[r][warp] + rank[r]);
+            uint32_t cls = 0;
+            for (int j = 0; j < a.sc.n_keys; j++) {  // survivors are rare once a cutoff exists: encode again instead of holding it
+                uint32_t cl;
+                a.st.w[j][o] = tk_encode(a.sc, j, a.in_data[j], a.in_valid[j], row, &cl);
+                cls |= cl << j;
+            }
+            a.st.cls[o] = (uint8_t)cls;
+            a.st.seq[o] = a.seq_base + row;
+            for (int c = 0; c < a.sc.n_cols; c++) {
+                tk_copy_cell(a.in_data[c], row, a.st.data[c], o, ctype_size(a.sc.ctype[c]));
+                if (a.st.vb[c]) a.st.vb[c][o] = bit_valid(a.in_valid[c], row) ? 1 : 0;
+            }
+        }
+        __syncthreads();
+    }
+}
+
+// Order of two store rows: (class_0, word_0, ..., arrival index).  Never equal for two different rows.
+__device__ __forceinline__ bool tk_less(const TkStore& s, int nk, uint32_t a, uint32_t b) {
+    const uint32_t ca = s.cls[a], cb = s.cls[b];
+#pragma unroll
+    for (int j = 0; j < TK_MAX_KEYS; j++) {
+        if (j < nk) {
+            const uint32_t x = (ca >> j) & 1, y = (cb >> j) & 1;
+            if (x != y) return x < y;
+            const uint64_t wa = s.w[j][a], wb = s.w[j][b];
+            if (wa != wb) return wa < wb;
+        }
+    }
+    return s.seq[a] < s.seq[b];
+}
+__device__ __forceinline__ bool tk_less_sent(const TkStore& s, int nk, uint32_t a, uint32_t b) {
+    if (a == TK_SENTINEL) return false;
+    if (b == TK_SENTINEL) return true;
+    return tk_less(s, nk, a, b);
+}
+
+// Row ids of a sorted run starting at o of width w, cut to its first K rows.
+__host__ __device__ __forceinline__ int64_t tk_run_len(int64_t o, int64_t w, int64_t n, int64_t K) {
+    if (o >= n) return 0;
+    const int64_t l = n - o < w ? n - o : w;
+    return l < K ? l : K;
+}
+
+// Bitonic sort of the row ids of one TK_SORT_TILE-row tile; writes the tile's first min(K, rows) ids.
+__global__ void __launch_bounds__(TK_SORT_THREADS) topk_block_sort_kernel(const TkStore s, int nk, int64_t n, int64_t K, uint32_t* out) {
+    __shared__ uint32_t v[TK_SORT_TILE];
+    const int64_t o = (int64_t)blockIdx.x * TK_SORT_TILE;
+    const int len = (int)(n - o < TK_SORT_TILE ? n - o : TK_SORT_TILE);
+    for (int i = threadIdx.x; i < TK_SORT_TILE; i += TK_SORT_THREADS) v[i] = i < len ? (uint32_t)(o + i) : TK_SENTINEL;
+    __syncthreads();
+    for (int k = 2; k <= TK_SORT_TILE; k <<= 1) {
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int i = threadIdx.x; i < TK_SORT_TILE; i += TK_SORT_THREADS) {
+                const int p = i ^ j;
+                if (p > i) {
+                    const uint32_t x = v[i], y = v[p];
+                    const bool up = (i & k) == 0;
+                    if (up ? tk_less_sent(s, nk, y, x) : tk_less_sent(s, nk, x, y)) { v[i] = y; v[p] = x; }
+                }
+            }
+            __syncthreads();
+        }
+    }
+    const int64_t keep = tk_run_len(o, TK_SORT_TILE, n, K);
+    for (int i = threadIdx.x; i < keep; i += TK_SORT_THREADS) out[o + i] = v[i];
+}
+
+// One merge pass: runs of width w at offsets 2pw and 2pw + w become one run of width 2w (cut to K rows).  Each thread finds the
+// start of its TK_MERGE_ITEMS outputs on the merge path by binary search, then merges them sequentially.
+__global__ void topk_merge_kernel(const TkStore s, int nk, int64_t n, int64_t K, int64_t w, int64_t chunks_per_pair, int64_t n_pairs,
+                                  const uint32_t* __restrict__ in, uint32_t* __restrict__ out) {
+    const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= n_pairs * chunks_per_pair) return;
+    const int64_t p = gid / chunks_per_pair, d0 = (gid % chunks_per_pair) * TK_MERGE_ITEMS;
+    const int64_t ao = 2 * p * w, bo = ao + w;
+    const int64_t la = tk_run_len(ao, w, n, K), lb = tk_run_len(bo, w, n, K);
+    const int64_t m = la + lb < K ? la + lb : K;
+    if (d0 >= m) return;
+    const uint32_t* A = in + ao;
+    const uint32_t* B = in + bo;
+    int64_t lo = d0 - lb > 0 ? d0 - lb : 0, hi = d0 < la ? d0 : la;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (tk_less(s, nk, B[d0 - mid - 1], A[mid])) hi = mid; else lo = mid + 1;
+    }
+    int64_t i = lo, j = d0 - lo;
+    for (int t = 0; t < TK_MERGE_ITEMS && d0 + t < m; t++) {
+        const bool take_a = j >= lb || (i < la && tk_less(s, nk, A[i], B[j]));
+        out[ao + d0 + t] = take_a ? A[i++] : B[j++];
+    }
+}
+
+// dst row i = src row perm[i] for i < m; the K-th row becomes the cutoff; the store count becomes m.
+__global__ void topk_gather_kernel(const TkStore src, const TkStore dst, const TkSchema sc, const uint32_t* __restrict__ perm, int64_t m,
+                                   int64_t K, TkCutoff* cutoff, unsigned long long* cursor) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid == 0) *cursor = (unsigned long long)m;
+    for (int64_t i = gid; i < m; i += stride) {
+        const uint32_t si = perm[i];
+        for (int j = 0; j < sc.n_keys; j++) dst.w[j][i] = src.w[j][si];
+        dst.cls[i] = src.cls[si];
+        dst.seq[i] = src.seq[si];
+        for (int c = 0; c < sc.n_cols; c++) {
+            tk_copy_cell(src.data[c], si, dst.data[c], i, ctype_size(sc.ctype[c]));
+            if (dst.vb[c]) dst.vb[c][i] = src.vb[c][si];
+        }
+        if (i == K - 1) {
+            for (int j = 0; j < sc.n_keys; j++) cutoff->w[j] = src.w[j][si];
+            cutoff->cls = src.cls[si];
+            cutoff->has = 1;
+        }
+    }
+}
+
+struct SortState {
+    int device;
+    cudaStream_t stream;
+    TkSchema sc{};
+    int arr_type[TK_MAX_COLS];
+    int64_t limit, offset, K, cap, output_batch_size;
+    // two store buffers (cur = the one the filter appends to) and their memory
+    std::vector<DevBuf> mem[2];
+    TkStore store[2]{};
+    int cur = 0;
+    DevBuf perm[2], d_cursor, d_cutoff, d_bitmaps;
+    std::vector<uint32_t*> out_bitmap;
+    unsigned long long* h_count = nullptr;
+    int64_t held = 0;         // sorted rows at the front of the current store (<= K)
+    int64_t count_bound = 0;  // upper bound on the store count: last count read + rows launched since
+    bool has_cutoff = false, finished = false;
+    int64_t n_out = 0, out_cursor = 0;
+    // metrics
+    int64_t rows_consumed = 0, rows_admitted = 0, admitted_after_cutoff = 0, reduce_steps = 0, count_reads = 0, filter_launches = 0;
+
+    SortState(int64_t limit_, int64_t offset_, const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_keys, const int32_t* asc,
+              const int32_t* na_last, int64_t obs, int dev, cudaStream_t st)
+        : device(dev), stream(st), limit(limit_), offset(offset_), output_batch_size(obs) {
+        B200_REQUIRE(limit >= 0 && offset >= 0, "b200 sort: limit and offset must be non-negative");
+        B200_REQUIRE(limit <= TK_MAX_K && offset <= TK_MAX_K - limit, "b200 sort: limit + offset exceeds the top-k cap of 2^26 rows");
+        B200_REQUIRE(n_keys >= 1 && n_keys <= TK_MAX_KEYS, "b200 sort: 1 to 4 sort keys");
+        B200_REQUIRE(n_arrs >= n_keys && n_arrs <= TK_MAX_COLS, "b200 sort: keys are the first n_keys of at most 32 columns");
+        B200_REQUIRE(c_types && arr_types && asc && na_last, "b200 sort: null argument");
+        K = limit + offset;
+        sc.n_keys = n_keys; sc.n_cols = n_arrs;
+        for (int c = 0; c < n_arrs; c++) {
+            B200_REQUIRE(ctype_size(c_types[c]) > 0, "b200 sort: unsupported column dtype (fixed-width numeric, bool and temporal columns only)");
+            B200_REQUIRE(arr_types[c] == ARR_NUMPY || arr_types[c] == ARR_NULLABLE, "b200 sort: unsupported array type");
+            sc.ctype[c] = c_types[c]; arr_type[c] = arr_types[c];
+        }
+        for (int j = 0; j < n_keys; j++) {
+            if (!asc[j]) sc.desc_mask |= 1u << j;
+            if (na_last[j]) sc.na_last_mask |= 1u << j;
+        }
+        cap = std::max<int64_t>(2 * K, TK_MIN_CAP);
+        B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
+        h_count = (unsigned long long*)pinned_acquire(8);
+        d_cursor.alloc(8); d_cutoff.alloc(sizeof(TkCutoff));
+        B200_CUDA(cudaMemsetAsync(d_cursor.p, 0, 8, stream));
+        B200_CUDA(cudaMemsetAsync(d_cutoff.p, 0, sizeof(TkCutoff), stream));
+        if (K == 0) return;  // nothing is ever kept: no store
+        for (int b = 0; b < 2; b++) {
+            auto take = [&](size_t bytes) { mem[b].emplace_back(); mem[b].back().alloc(bytes); return mem[b].back().p; };
+            TkStore& s = store[b];
+            for (int j = 0; j < n_keys; j++) s.w[j] = (uint64_t*)take(cap * 8);
+            s.cls = (uint8_t*)take(cap);
+            s.seq = (int64_t*)take(cap * 8);
+            for (int c = 0; c < n_arrs; c++) {
+                s.data[c] = take(cap * ctype_size(sc.ctype[c]));
+                s.vb[c] = arr_type[c] == ARR_NULLABLE ? (uint8_t*)take(cap) : nullptr;
+            }
+            perm[b].alloc(cap * 4);
+        }
+    }
+    ~SortState() {
+        cudaSetDevice(device); scratch_set_stream(stream);
+        pinned_release(h_count, 8);
+    }
+
+    int grid_for(int64_t items, int per_block) const { return (int)std::max<int64_t>(1, std::min<int64_t>((items + per_block - 1) / per_block, (int64_t)num_sms(device) * 8)); }
+
+    int64_t read_count() {
+        B200_CUDA(cudaMemcpyAsync(h_count, d_cursor.p, 8, cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaStreamSynchronize(stream));
+        count_reads++;
+        count_bound = (int64_t)*h_count;
+        return count_bound;
+    }
+
+    // Sorts held rows + candidates, keeps the first K in the other buffer and writes the cutoff.  n: the store count, if known.
+    void reduce(int64_t n = -1) {
+        if (n < 0) n = read_count();
+        reduce_steps++;
+        rows_admitted += n - held;
+        if (has_cutoff) admitted_after_cutoff += n - held;
+        if (n > held) {
+            uint32_t* a = perm[0].as<uint32_t>();
+            uint32_t* b = perm[1].as<uint32_t>();
+            const TkStore& s = store[cur];
+            topk_block_sort_kernel<<<(unsigned)((n + TK_SORT_TILE - 1) / TK_SORT_TILE), TK_SORT_THREADS, 0, stream>>>(s, sc.n_keys, n, K, a);
+            B200_CUDA(cudaGetLastError());
+            for (int64_t w = TK_SORT_TILE; w < n; w *= 2) {
+                const int64_t n_pairs = (n + 2 * w - 1) / (2 * w);
+                const int64_t chunks = (std::min(2 * w, K) + TK_MERGE_ITEMS - 1) / TK_MERGE_ITEMS;
+                const int64_t threads = n_pairs * chunks;
+                topk_merge_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(s, sc.n_keys, n, K, w, chunks, n_pairs, a, b);
+                B200_CUDA(cudaGetLastError());
+                std::swap(a, b);
+            }
+            const int64_t m = std::min(n, K);
+            topk_gather_kernel<<<grid_for(m, 256), 256, 0, stream>>>(s, store[cur ^ 1], sc, a, m, K, d_cutoff.as<TkCutoff>(),
+                                                                    d_cursor.as<unsigned long long>());
+            B200_CUDA(cudaGetLastError());
+            cur ^= 1;
+            held = m;
+        }
+        count_bound = held;
+        if (held == K) has_cutoff = true;
+    }
+
+    void consume(const b200_table* t) {
+        B200_REQUIRE(!finished, "b200 sort: batch consumed after is_last");
+        B200_REQUIRE(t->n_cols == sc.n_cols, "b200 sort: the batch's column count differs from the state's schema");
+        for (int c = 0; c < sc.n_cols; c++)
+            B200_REQUIRE(t->cols[c].c_type == sc.ctype[c] && t->cols[c].arr_type == arr_type[c],
+                         "b200 sort: a batch's column types differ from the state's schema");
+        const int64_t n = t->n_rows;
+        if (n > 0) B200_REQUIRE(t->device == device, "b200 sort: batches must be resident on the state's device (stage host batches first)");
+        B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
+        const int64_t seq_base = rows_consumed;
+        rows_consumed += n;
+        if (K == 0 || n == 0) return;
+        TkFilterArgs a{};
+        a.sc = sc;
+        a.seq_base = seq_base;
+        for (int c = 0; c < sc.n_cols; c++) { a.in_data[c] = t->cols[c].data; a.in_valid[c] = t->cols[c].validity; }
+        a.cutoff = d_cutoff.as<TkCutoff>();
+        a.cursor = d_cursor.as<unsigned long long>();
+        for (int64_t r0 = 0; r0 < n;) {
+            int64_t r = n - r0;
+            if (count_bound + r > cap) {
+                read_count();
+                if (count_bound + r > cap && count_bound > held) reduce(count_bound);
+                r = std::min(r, cap - count_bound);
+            }
+            a.row0 = r0; a.row1 = r0 + r;
+            a.st = store[cur];
+            topk_filter_kernel<<<grid_for(r, TK_TILE), TK_THREADS, 0, stream>>>(a);
+            B200_CUDA(cudaGetLastError());
+            filter_launches++;
+            count_bound += r;
+            r0 += r;
+            if (!has_cutoff && count_bound >= K) reduce();  // before a cutoff every row is admitted: the count is exactly count_bound
+        }
+    }
+
+    void finish() {
+        B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
+        if (K > 0) reduce();
+        finished = true;
+        n_out = std::max<int64_t>(0, held - offset);
+        int n_nullable = 0;
+        for (int c = 0; c < sc.n_cols; c++) n_nullable += arr_type[c] == ARR_NULLABLE;
+        const int64_t words = (n_out + 31) / 32 + 2;
+        d_bitmaps.alloc((size_t)std::max(1, n_nullable) * words * 4);
+        B200_CUDA(cudaMemsetAsync(d_bitmaps.p, 0, d_bitmaps.bytes, stream));
+        out_bitmap.assign(sc.n_cols, nullptr);
+        for (int c = 0, k = 0; c < sc.n_cols; c++) {
+            if (arr_type[c] != ARR_NULLABLE) continue;
+            out_bitmap[c] = d_bitmaps.as<uint32_t>() + (k++) * words;
+            if (n_out > 0) launch_pack_bitmap(store[cur].vb[c] + offset, n_out, out_bitmap[c], grid_for(n_out, 256), stream);
+        }
+        B200_CUDA(cudaGetLastError());
+        B200_CUDA(cudaStreamSynchronize(stream));
+    }
+
+    int produce(b200_table* out, int32_t* out_is_last, bool produce_output) {
+        B200_REQUIRE(finished, "b200 sort: output requested before the last batch was consumed");
+        B200_REQUIRE(out->cols != nullptr, "b200 sort: out->cols must point to one descriptor per column");
+        int64_t bs = output_batch_size > 0 ? output_batch_size : n_out;
+        if (bs % 32 != 0 && bs < n_out) bs = (bs + 31) & ~31ll;  // validity bitmaps are sliced at word granularity
+        const int64_t rows = produce_output ? std::min(bs, n_out - out_cursor) : 0;
+        out->n_rows = rows; out->n_cols = sc.n_cols; out->device = device;
+        const int64_t base = offset + out_cursor;
+        for (int c = 0; c < sc.n_cols; c++) {
+            b200_column& col = out->cols[c];
+            col.data = K == 0 ? d_cutoff.p : (char*)store[cur].data[c] + base * ctype_size(sc.ctype[c]);
+            col.validity = out_bitmap[c] ? (uint8_t*)out_bitmap[c] + out_cursor / 8 : nullptr;
+            col.length = rows; col.c_type = sc.ctype[c]; col.arr_type = arr_type[c];
+        }
+        out_cursor += rows;
+        *out_is_last = out_cursor >= n_out ? 1 : 0;
+        return 0;
+    }
+};
+
+}  // namespace b200
+
+using b200::SortState;
+
+extern "C" {
+
+void* b200_sort_state_init(int64_t operator_id, int64_t limit, int64_t offset, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                           int32_t n_keys, const int32_t* ascending, const int32_t* na_last, int64_t output_batch_size, int32_t device,
+                           void* stream) {
+    (void)operator_id;
+    try {
+        int ndev = 0;
+        if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+            throw b200::Error("b200 sort: no CUDA device available (this path has no CPU fallback)");
+        B200_REQUIRE(device >= 0 && device < ndev, "b200 sort: bad device ordinal");
+        return new SortState(limit, offset, c_types, arr_types, n_arrs, n_keys, ascending, na_last, output_batch_size, device,
+                             (cudaStream_t)stream);
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
+}
+
+int b200_sort_build_consume_batch(void* state, const b200_table* in_table, int32_t is_last, int32_t* request_input) {
+    try {
+        B200_REQUIRE(state && in_table, "b200 sort: null state or table");
+        auto* s = (SortState*)state;
+        s->consume(in_table);
+        if (is_last) s->finish();
+        if (request_input) *request_input = 1;
+        return is_last ? 1 : 0;
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
+}
+
+int b200_sort_produce_output_batch(void* state, b200_table* out, int32_t* out_is_last, int32_t produce_output) {
+    try {
+        B200_REQUIRE(state && out && out_is_last, "b200 sort: null argument");
+        return ((SortState*)state)->produce(out, out_is_last, produce_output != 0);
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
+}
+
+void b200_delete_sort_state(void* state) { delete (SortState*)state; }
+
+int64_t b200_sort_get_metric(void* state, int32_t which) {
+    auto* s = (SortState*)state;
+    switch (which) {
+        case 0: return s->rows_consumed;
+        case 1: return s->rows_admitted;
+        case 2: return s->reduce_steps;
+        case 3: return s->count_reads;
+        case 4: return s->filter_launches;
+        case 5: return s->admitted_after_cutoff;
+        case 6: return s->cap;
+        default: return -1;
+    }
+}
+
+}  // extern "C"

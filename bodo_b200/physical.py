@@ -5,6 +5,7 @@ bodo/pandas/physical/operator.h:46-50,247-458; aggregate.h:65-365; join.h:58-744
     PhysicalReadPandas / PhysicalReadArrow / PhysicalReadParquet : sources (batches of host columns)
     PhysicalAggregate : sink of one pipeline (ConsumeBatch) and source of the next (ProduceBatch)
     PhysicalJoin      : sink for the build side, ProcessBatch for the probe side
+    PhysicalSort      : ORDER BY ... LIMIT ... OFFSET; sink of one pipeline and source of the next
     Pipeline          : while not finished: batch = source.ProduceBatch(); ... sink.ConsumeBatch(batch)
 
 plus two helpers that run those pipelines over pandas frames the way bodo.pandas does for
@@ -20,6 +21,7 @@ from typing import Iterable, Sequence
 
 from .streaming import groupby as G
 from .streaming import join as J
+from .streaming import sort as S
 from .table import Table
 
 STREAMING_BATCH_SIZE = 32768  # bodo/libs/streaming/_shuffle.h:27-31
@@ -273,6 +275,35 @@ class PhysicalJoin:
         J.delete_join_state(self.state)
 
 
+class PhysicalSort:
+    """Top-k sink/source (the reference's PhysicalSort, bodo/pandas/physical/sort.h, which DuckDB's TopN lowers to): rows
+    [offset, offset + limit) of the input sorted stably by `by` (column names; ascending / na_position per key or one for all).
+    The column names are taken from the first batch."""
+
+    def __init__(self, by, ascending=True, na_position="last", limit=None, offset=0, parallel: bool = False, **kw):
+        self.args = (by, ascending, na_position, limit, offset, parallel)
+        self.kw = kw
+        self.state = None
+        if limit is None:
+            raise S._lib.B200Error("PhysicalSort: a limit is required (a full sort without LIMIT is not supported)")
+
+    def ConsumeBatch(self, batch: Table, prev: OperatorResult) -> OperatorResult:
+        if self.state is None:
+            by, asc, nap, limit, offset, parallel = self.args
+            self.state = S.init_stream_sort_state(-1, limit, offset, by, asc, nap, batch.names, parallel, **self.kw)
+        is_last = prev == OperatorResult.FINISHED
+        S.sort_build_consume_batch(self.state, batch, is_last)
+        return OperatorResult.FINISHED if is_last else OperatorResult.NEED_MORE_INPUT
+
+    def ProduceBatch(self):
+        out, last = S.produce_output_batch(self.state, True)
+        return out, (OperatorResult.FINISHED if last else OperatorResult.HAVE_MORE_OUTPUT)
+
+    def Finalize(self):
+        if self.state is not None:
+            S.delete_stream_sort_state(self.state)
+
+
 class ResultCollector:
     """PhysicalResultCollector: concatenates output batches into one pandas frame."""
 
@@ -346,6 +377,17 @@ def groupby_agg_parquet(path: str, by, aggs: Sequence[tuple], dropna: bool = Tru
     out = coll.result()
     out.columns = by + [name for name, _, _ in aggs]
     return out
+
+
+def sort_values_head(df, by, ascending=True, na_position="last", n: int = 5, offset: int = 0, batch_size: int = STREAMING_BATCH_SIZE, **kw):
+    """df.sort_values(by, ascending=..., na_position=..., kind="stable").iloc[offset:offset + n] through PhysicalSort.  ascending and
+    na_position may be one value or one per key.  Returns a pandas DataFrame with a fresh index."""
+    op = PhysicalSort(by, ascending, na_position, limit=n, offset=offset, **kw)
+    run_pipeline(PhysicalReadPandas(df, batch_size), [], op)
+    coll = ResultCollector()
+    run_pipeline(op, [], coll)
+    op.Finalize()
+    return coll.result()
 
 
 def merge(left, right, left_on, right_on, how: str = "inner", batch_size: int = STREAMING_BATCH_SIZE, **kw):

@@ -209,6 +209,33 @@ int b200_join_runtime_filter_n(void* state, const b200_table* in_table, const in
  * inline-payload kernel (key + payload in one 32-byte slot), 7 inline-payload table builds. */
 int64_t b200_join_get_metric(void* state, int32_t which);
 
+/* ---- streaming top-k: ORDER BY ... LIMIT ... OFFSET (reference: bodo/libs/streaming/_sort.cpp) ---- */
+
+/* stream_sort_state_init_py_entry (_sort.cpp), LIMIT form only.  The result is rows [offset, offset + limit) of the input
+ * sorted stably (ties keep arrival order: batch order, then row order) by the first n_keys (1..4) of the n_arrs (<= 32) columns;
+ * every column is fixed width (integer, float, bool, date, datetime, timedelta; numpy or nullable).  ascending[j] and na_last[j]
+ * (na_position "last" = 1, "first" = 0) are per key; a nullable NA and a float NaN are both NA; -0.0 and 0.0 tie.  0 <= limit,
+ * 0 <= offset and limit + offset <= 2^26 (the store's uint32 row ids and its two buffers of max(2 (limit + offset), 4 Mi) rows).
+ * A dictionary-id key column sorts by id, not by string. */
+void* b200_sort_state_init(int64_t operator_id, int64_t limit, int64_t offset, const int8_t* c_types, const int8_t* arr_types,
+                           int32_t n_arrs, int32_t n_keys, const int32_t* ascending, const int32_t* na_last,
+                           int64_t output_batch_size, int32_t device, void* stream);
+
+/* The build-consume entry of _sort.cpp: filters a DEVICE-resident batch (same schema as the state) against the current cutoff on
+ * the device; on is_last reduces to the final rows.  Returns 1 after is_last, 0 otherwise, < 0 on error; *request_input = 1. */
+int b200_sort_build_consume_batch(void* state, const b200_table* in_table, int32_t is_last, int32_t* request_input);
+
+/* The produce-output entry of _sort.cpp: fills `out` (out->cols with room for n_arrs descriptors) with library-owned device
+ * columns of the next <= output_batch_size result rows, in order; valid until delete.  Sets *out_is_last. */
+int b200_sort_produce_output_batch(void* state, b200_table* out, int32_t* out_is_last, int32_t produce_output);
+
+/* delete_stream_sort_state (_sort.cpp). */
+void b200_delete_sort_state(void* state);
+
+/* Metrics: 0 rows consumed, 1 rows admitted as candidates, 2 reduce steps, 3 host reads of the candidate count, 4 filter
+ * launches, 5 rows admitted while a cutoff existed, 6 store capacity in rows. */
+int64_t b200_sort_get_metric(void* state, int32_t which);
+
 /* ---- row -> rank shuffle (reference: bodo/libs/_shuffle.cpp) ---- */
 
 /* hash_keys_table(SEED_HASH_PARTITION) + hash_to_rank (bodo/libs/_array_hash.cpp:76-109,
