@@ -147,12 +147,8 @@ class GroupbyState:
         return out
 
     def _exchange(self):
-        """Hash-partition exchange of the partial aggregates after the last local batch, then finalize.
-
-        Fused form (default): ONE kernel packs every partial row another rank owns straight into that rank's receive slab over
-        NVLink (symmetric memory, streaming/exchange.py), a device-side barrier, one combine kernel — no count exchange, no
-        send buffer, no host synchronisation before finalize.  Falls back to the NCCL all-to-all-v (`_exchange_nccl`) when
-        symmetric memory is unavailable or a rank's share did not fit its slab segment (finalize reports that: -2)."""
+        """Hash-partition exchange of the partial aggregates after the last local batch: first every nested nunique state (a
+        key's (key, value) pairs are owned where the key is owned), then the outer state, each finalized after its exchange."""
         import os
         import time
 
@@ -162,99 +158,69 @@ class GroupbyState:
 
         L = _lib.lib()
         h = self.handle
-        trace = os.environ.get("B200_TRACE") and self.rank == 0
         t0 = time.perf_counter()
         slabs = X.get_slabs(self.process_group, self.device)
-        done = False
-        # nunique: the nested (key, value) distinct states are exchanged first (fused form only: their partial rows are multi-key)
         for i in range(int(L.b200_groupby_num_inner_states(h))):
-            hi = _lib.check_ptr(L.b200_groupby_inner_state(h, i), "groupby nunique")
-            if slabs is None:
-                raise _lib.B200Error("groupby nunique on the sharded path needs the fused exchange (torch symmetric memory)")
-            row_bytes = int(L.b200_groupby_exchange_row_bytes(hi))
-            cap_rows = (slabs.slab_bytes - X.HDR_BYTES) // (self.n_pes * row_bytes)
-            peers_dev, my_slab, hdl = slabs.next()
-            stream = torch.cuda.ExternalStream(self.stream) if self.stream else torch.cuda.default_stream(self.device)
-            with torch.cuda.stream(stream):
-                _lib.check(L.b200_groupby_exchange_fused_pack(hi, ffi.cast("void* const*", peers_dev), cap_rows), "groupby nunique exchange (pack)")
-                hdl.barrier(channel=0)
-                _lib.check(L.b200_groupby_exchange_fused_combine(hi, ffi.cast("void*", my_slab), cap_rows), "groupby nunique exchange (combine)")
-            if int(L.b200_groupby_finalize(hi)) < 0:
-                raise _lib.B200Error("groupby nunique: the distinct (key, value) pairs did not fit the exchange slab "
-                                     "(raise B200_XCHG_SLAB_BYTES)")
-        if slabs is not None:
-            row_bytes = int(L.b200_groupby_exchange_row_bytes(h))
-            cap_rows = (slabs.slab_bytes - X.HDR_BYTES) // (self.n_pes * row_bytes)
-            peers_dev, my_slab, hdl = slabs.next()
-            stream = torch.cuda.ExternalStream(self.stream) if self.stream else torch.cuda.default_stream(self.device)
-            with torch.cuda.stream(stream):
-                _lib.check(L.b200_groupby_exchange_fused_pack(h, ffi.cast("void* const*", peers_dev), cap_rows), "groupby fused exchange (pack)")
-                hdl.barrier(channel=0)
-                _lib.check(L.b200_groupby_exchange_fused_combine(h, ffi.cast("void*", my_slab), cap_rows), "groupby fused exchange (combine)")
-            rc = int(L.b200_groupby_finalize(h))
-            if rc == -1:
-                _lib.check(-1, "groupby finalize")
-            done = rc != -2
-            self.shuffle_bytes = None
-        if not done:
-            self._exchange_nccl()
-            _lib.check(int(L.b200_groupby_finalize(h)), "groupby finalize")
+            self._exchange_state(_lib.check_ptr(L.b200_groupby_inner_state(h, i), "groupby nunique"), slabs)
+        self.exchange_path, self.shuffle_bytes = self._exchange_state(h, slabs)
         self.exchanged = True
-        self.exchange_path = "fused" if done else "nccl"
-        if trace:
+        if os.environ.get("B200_TRACE") and self.rank == 0:
             torch.cuda.synchronize()
-            print(f"[b200 exchange ms] {'fused' if done else 'nccl'} exchange + finalize = {(time.perf_counter() - t0) * 1e3:.3f}", flush=True)
+            print(f"[b200 exchange ms] {self.exchange_path} exchange + finalize = {(time.perf_counter() - t0) * 1e3:.3f}", flush=True)
 
-    def _exchange_nccl(self):
-        """The same exchange through NCCL: count all-gather + one all-to-all-v of the packed partial rows, then combine."""
-        import os
-        import time
+    def _exchange_state(self, h, slabs):
+        """Exchanges and finalizes one C state; returns (path, bytes sent through NCCL or None).
 
+        Fused form (when symmetric memory is available): ONE kernel packs every partial row another rank owns straight into that
+        rank's receive slab over NVLink (streaming/exchange.py), a device-side barrier, one combine kernel — no count exchange, no
+        send buffer, no host synchronisation before finalize.  NCCL form (no slabs, or finalize reported -2: a rank's share did
+        not fit its slab segment): count all-gather + one all-to-all-v of the packed rows, then the same combine."""
         import torch
         import torch.distributed as dist
 
-        trace = os.environ.get("B200_TRACE") and self.rank == 0
-        t = [time.perf_counter()]
-
-        def mark():
-            if trace:
-                torch.cuda.synchronize()
-                t.append(time.perf_counter())
+        from . import exchange as X
 
         L = _lib.lib()
-        h = self.handle
+        null = ffi.NULL
+        row_bytes = int(L.b200_groupby_exchange_row_bytes(h))
+        if slabs is not None:
+            cap_rows = (slabs.slab_bytes - X.HDR_BYTES) // (self.n_pes * row_bytes)
+            peers_dev, my_slab, hdl = slabs.next()
+            stream = torch.cuda.ExternalStream(self.stream) if self.stream else torch.cuda.default_stream(self.device)
+            with torch.cuda.stream(stream):
+                _lib.check(L.b200_groupby_exchange_pack(h, ffi.cast("void* const*", peers_dev), cap_rows, null), "groupby exchange (pack)")
+                hdl.barrier(channel=0)
+                _lib.check(L.b200_groupby_exchange_combine(h, ffi.cast("void*", my_slab), cap_rows, null), "groupby exchange (combine)")
+            rc = int(L.b200_groupby_finalize(h))
+            if rc != -2:
+                _lib.check(rc, "groupby finalize")
+                return "fused", None
+            # (the fused pack counted every destination's rows exactly)
+        else:
+            _lib.check(L.b200_groupby_exchange_pack(h, null, 0, null), "groupby exchange (count)")
         counts = ffi.new("int64_t[]", self.n_pes)
-        row_bytes = _lib.check(L.b200_groupby_shuffle_prepare(h, counts), "groupby shuffle prepare")
-        mark()
-        send_counts = [int(counts[i]) for i in range(self.n_pes)]
+        _lib.check(L.b200_groupby_exchange_counts(h, counts), "groupby exchange (counts)")
+        send_counts = list(counts)
         dev = torch.device("cuda", self.device)
         words = row_bytes // 8
         n_send = sum(send_counts)
         # counts travel as one small all-gather of the n_pes x n_pes matrix (mpi_comm_info's MPI_Alltoall,
         # _shuffle.cpp:210-213), issued asynchronously so it overlaps the pack kernel
-        sc = torch.tensor(send_counts, dtype=torch.int64, device=dev)
         allc = torch.empty(self.n_pes * self.n_pes, dtype=torch.int64, device=dev)
-        work = dist.all_gather_into_tensor(allc, sc, group=self.process_group, async_op=True)
+        work = dist.all_gather_into_tensor(allc, torch.tensor(send_counts, dtype=torch.int64, device=dev), group=self.process_group, async_op=True)
         send = torch.empty((max(n_send, 1), words), dtype=torch.int64, device=dev)
-        _lib.check(L.b200_groupby_shuffle_pack(h, ffi.cast("void*", send.data_ptr())), "groupby shuffle pack")
-        mark()
+        _lib.check(L.b200_groupby_exchange_pack(h, null, 0, ffi.cast("void*", send.data_ptr())), "groupby exchange (pack)")
         work.wait()
         recv_counts = allc.view(self.n_pes, self.n_pes)[:, self.rank].tolist()
-        mark()
         n_recv = sum(recv_counts)
         recv = torch.empty((max(n_recv, 1), words), dtype=torch.int64, device=dev)
         dist.all_to_all_single(recv[:n_recv], send[:n_send], output_split_sizes=recv_counts,
                                input_split_sizes=send_counts, group=self.process_group)
         torch.cuda.current_stream(dev).synchronize()
-        mark()
-        _lib.check(L.b200_groupby_shuffle_combine(h, ffi.cast("void*", recv.data_ptr()), n_recv),
-                   "groupby shuffle combine")
-        L.b200_stream_synchronize(ffi.cast("void*", self.stream))
-        mark()
-        self.shuffle_bytes = n_send * row_bytes
-        if trace:
-            names = ["prepare", "pack", "counts", "alltoall", "combine"]
-            print("[b200 exchange ms] " + " ".join(f"{n}={(b - a) * 1e3:.3f}" for n, a, b in zip(names, t, t[1:])), flush=True)
+        _lib.check(L.b200_groupby_exchange_combine(h, ffi.cast("void*", recv.data_ptr()), 0, ffi.new("int64_t[]", recv_counts)),
+                   "groupby exchange (combine)")
+        _lib.check(int(L.b200_groupby_finalize(h)), "groupby finalize")  # (reads `recv`: rows that found the table full)
+        return "nccl", n_send * row_bytes
 
 
 def _current_device() -> int:

@@ -268,8 +268,7 @@ def _worker(rank, world, port, q):
             w = np.random.default_rng(23).integers(-9, 9, n).astype(np.int64)
             c = (n + world - 1) // world
             mine = pd.DataFrame({"k": keys[rank * c:(rank + 1) * c], "w": w[rank * c:(rank + 1) * c]})
-            # (nunique exchanges its nested states through the slab: the fused exchange only)
-            fn = ("sum", "count", "nunique") if name == "fused" else ("sum", "count")
+            fn = ("sum", "count", "nunique")
             st = init_groupby_state(-1, (0,), fn, tuple(range(len(fn) + 1)), (1,) * len(fn), parallel=True, dropna=False,
                                     device=rank, output_batch_size=1 << 30)
             nb = 6
