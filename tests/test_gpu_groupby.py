@@ -330,8 +330,9 @@ def test_var_std_skew_against_pandas_and_reference_formulas(gpu_lib, nullable):
     """var / std / var_pop / std_pop / skew (Bodo_FTypes 24 / 25 / 22 / 23 / 27; the reference's GPU test matrix,
     bodo/tests/test_df_lib/test_gpu/test_gpu_end_to_end.py:68-110).  Reference: Welford (count, mean, M2) for var / std
     (groupby/_groupby_agg_funcs.h:694-719), power sums for skew (:723-745), eval in _groupby_eval.h:71-137.  The device carries
-    power sums for all of them; tolerance = the reference's test tolerance (rtol 1e-5), valid while |mean| / std <~ 1e5
-    (cancellation in sum x^2 - (sum x)^2 / n loses about 2 log10(|mean| / std) digits of the 16 a double has)."""
+    power sums about a per-group shift for all of them; tolerance = the reference's test tolerance (rtol 1e-5).  The shift keeps
+    the error independent of |mean| / std (tests/test_gpu_groupby_float_values.py states the bound and checks it up to offsets
+    of 1e12)."""
     rng = np.random.default_rng(23)
     n, ng = 60_000, 211
     k = rng.integers(0, ng, n).astype(np.int64)
