@@ -265,6 +265,300 @@ __global__ void topk_gather_kernel(const TkStore src, const TkStore dst, const T
     }
 }
 
+// ---- full sort (ORDER BY without LIMIT): append-only chunk store, LSD radix sort at is_last ----
+//
+//   fsort_append_kernel  per consume call: the batch's columns, plus one validity byte per nullable column, are copied into the
+//                        chunk store at rows [rows_consumed, rows_consumed + n).  Arrival order is storage order.
+//   fsort_hist_kernel    at is_last: one read of the key columns builds the 256-bin histogram of every byte digit of every key's
+//                        radix word and each key's NA count.  The host reads them back once and skips every pass whose digit takes
+//                        a single value over all rows.
+//   fsort_pass_kernel    one onesweep pass per digit that is not skipped, least significant key first: a stable in-tile rank
+//                        (warp multisplit), a decoupled look-back over per-tile digit counts seeded by the global histogram, and a
+//                        staged, coalesced copy-out of (radix word, row id) pairs.  The first pass of a key computes its words from
+//                        the column: in row order for the first key sorted, through the current permutation for the others.
+//   fsort_gather_kernel  every column and validity byte through the final permutation into the output store.
+//
+// Radix word: an unsigned integer of the key's own width whose order is the key order (sign bit flipped for signed integers and
+// temporals; float32 and float64 in their ordered forms with -0.0 folded onto 0.0; complemented for a descending key); an NA or NaN
+// key has word 0 and its NA-class bit set by na_position.  A key that can hold NAs gets one more pass on that class bit after its
+// byte passes; the bit rides in bit 31 of the row id, which is why the store holds at most 2^31 rows.
+constexpr int FS_CHUNK_LOG = 24;
+constexpr int64_t FS_CHUNK = 1ll << FS_CHUNK_LOG;
+constexpr int FS_MAX_CHUNKS = 128;
+constexpr int64_t FS_MAX_ROWS = (int64_t)FS_MAX_CHUNKS * FS_CHUNK;  // 2^31
+constexpr int FS_THREADS = 256, FS_WARPS = FS_THREADS / 32, FS_ITEMS = 16, FS_TILE = FS_THREADS * FS_ITEMS;
+constexpr uint32_t FS_ID_MASK = 0x7FFFFFFFu;
+constexpr int FS_HIST_WORDS = TK_MAX_KEYS * 8 * 256 + TK_MAX_KEYS;  // [key][byte][digit] counts, then one NA count per key
+// look-back word: pass epoch (bits 34..63), AGGREGATE / INCLUSIVE flag (bits 32..33), count (bits 0..31)
+constexpr unsigned long long FS_AGG = 1ull << 32, FS_INCL = 2ull << 32;
+enum { FS_IN_PAIRS = 0, FS_IN_COLUMN = 1, FS_IN_GATHER = 2 };
+
+// One chunk is one allocation: FS_CHUNK values of every column, then FS_CHUNK validity bytes of every nullable column.
+struct FsLayout {
+    int n_cols;
+    int ctype[TK_MAX_COLS];
+    int64_t coff[TK_MAX_COLS];  // byte offset of column c's values in a chunk
+    int64_t voff[TK_MAX_COLS];  // byte offset of its validity bytes, -1 for a numpy column
+};
+struct FsChunks { const char* p[FS_MAX_CHUNKS]; };
+struct FsKey { int ct, desc, na_last; int64_t coff, voff; };
+
+// Radix word of the key cell at row `off` of `chunk`; *na: the cell is NA or NaN.
+__device__ __forceinline__ uint64_t fs_word(const FsKey& k, const char* chunk, int64_t off, bool* na) {
+    const char* p = chunk + k.coff;
+    bool isna = k.voff >= 0 && chunk[k.voff + off] == 0;
+    uint64_t w;
+    int bits;
+    if (k.ct == CT_FLOAT64) {
+        const double d = ((const double*)p)[off];
+        isna = isna || isnan(d);
+        w = (uint64_t)canon_float_ordered(canon_float_key(d)) ^ TK_SIGN;
+        bits = 64;
+    } else if (k.ct == CT_FLOAT32) {
+        const float f = ((const float*)p)[off];
+        isna = isna || isnan(f);
+        const uint32_t b = f == 0.0f ? 0u : __float_as_uint(f);
+        w = b ^ ((b >> 31) ? 0xFFFFFFFFu : 0x80000000u);
+        bits = 32;
+    } else {
+        const int sz = ctype_size(k.ct);
+        switch (sz) {
+            case 8: w = ((const uint64_t*)p)[off]; break;
+            case 4: w = ((const uint32_t*)p)[off]; break;
+            case 2: w = ((const uint16_t*)p)[off]; break;
+            default: w = ((const uint8_t*)p)[off]; break;
+        }
+        bits = 8 * sz;
+        if (tk_signed(k.ct)) w ^= 1ull << (bits - 1);
+    }
+    if (k.desc) w = ~w & (bits == 64 ? ~0ull : (1ull << bits) - 1);
+    *na = isna;
+    return isna ? 0 : w;
+}
+
+template <typename W>
+__device__ __forceinline__ uint32_t fs_digit(W w, uint32_t id, int shift) {
+    return shift < 0 ? id >> 31 : (uint32_t)(w >> shift) & 0xFFu;
+}
+
+struct FsAppendArgs {
+    int64_t src0, n, dst0;  // batch rows [src0, src0 + n) go to rows [dst0, dst0 + n) of `chunk`
+    FsLayout lay;
+    char* chunk;
+    const void* in_data[TK_MAX_COLS];
+    const uint8_t* in_valid[TK_MAX_COLS];
+};
+
+__global__ void __launch_bounds__(256) fsort_append_kernel(const __grid_constant__ FsAppendArgs a) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += stride) {
+        const int64_t s = a.src0 + i, o = a.dst0 + i;
+        for (int c = 0; c < a.lay.n_cols; c++) {
+            tk_copy_cell(a.in_data[c], s, a.chunk + a.lay.coff[c], o, ctype_size(a.lay.ctype[c]));
+            if (a.lay.voff[c] >= 0) a.chunk[a.lay.voff[c] + o] = bit_valid(a.in_valid[c], s) ? 1 : 0;
+        }
+    }
+}
+
+struct FsHistArgs {
+    int64_t n;
+    int n_keys;
+    FsKey key[TK_MAX_KEYS];
+    uint32_t* hist;  // FS_HIST_WORDS
+    FsChunks ch;
+};
+
+// Block-private histograms of every (key, byte) digit, merged into `hist` once per block.  Equal digits within a warp are
+// counted by one shared atomic (match.any), so a constant byte costs one atomic per warp, not 32.
+__global__ void __launch_bounds__(FS_THREADS) fsort_hist_kernel(const __grid_constant__ FsHistArgs a) {
+    __shared__ uint32_t h[TK_MAX_KEYS * 8 * 256];
+    __shared__ uint32_t s_na[TK_MAX_KEYS];
+    const int lane = threadIdx.x & 31;
+    for (int i = threadIdx.x; i < a.n_keys * 8 * 256; i += FS_THREADS) h[i] = 0;
+    if (threadIdx.x < TK_MAX_KEYS) s_na[threadIdx.x] = 0;
+    __syncthreads();
+    const int64_t stride = (int64_t)gridDim.x * FS_THREADS;
+    for (int64_t r0 = (int64_t)blockIdx.x * FS_THREADS; r0 < a.n; r0 += stride) {
+        const int64_t r = r0 + threadIdx.x;
+        const unsigned act = __ballot_sync(0xffffffffu, r < a.n);
+        if (r >= a.n) continue;
+        const char* chunk = a.ch.p[r >> FS_CHUNK_LOG];
+        const int64_t off = r & (FS_CHUNK - 1);
+        const int leader = __ffs(act) - 1;
+        for (int j = 0; j < a.n_keys; j++) {
+            bool na;
+            const uint64_t w = fs_word(a.key[j], chunk, off, &na);
+            const unsigned nam = __ballot_sync(act, na);
+            if (lane == leader && nam) atomicAdd(&s_na[j], (uint32_t)__popc(nam));
+            const int nb = ctype_size(a.key[j].ct);
+            for (int b = 0; b < nb; b++) {
+                const uint32_t d = (uint32_t)(w >> (8 * b)) & 0xFFu;
+                const unsigned peers = __match_any_sync(act, d);
+                if (lane == __ffs(peers) - 1) atomicAdd(&h[(j * 8 + b) * 256 + d], (uint32_t)__popc(peers));
+            }
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < a.n_keys * 8 * 256; i += FS_THREADS)
+        if (h[i]) atomicAdd(&a.hist[i], h[i]);
+    if (threadIdx.x < a.n_keys && s_na[threadIdx.x]) atomicAdd(&a.hist[TK_MAX_KEYS * 8 * 256 + threadIdx.x], s_na[threadIdx.x]);
+}
+
+struct FsPassArgs {
+    int64_t n;
+    int shift;       // digit = (word >> shift) & 255; -1: the NA-class bit (bit 31 of the row id)
+    uint32_t epoch;  // this pass's tag in the look-back words (1, 2, ...; the words start at 0)
+    FsKey key;       // FS_IN_COLUMN / FS_IN_GATHER: the column the words are computed from
+    const void* w_in;
+    const uint32_t* id_in;
+    void* w_out;
+    uint32_t* id_out;
+    unsigned long long* status;  // [tile][digit] look-back words
+    unsigned int* tile_counter;  // tiles are numbered in the order their blocks start
+    uint32_t base[256];          // first output row of each digit: exclusive scan of the pass's global histogram
+    FsChunks ch;
+};
+
+// One LSD pass over FS_TILE-row tiles.  Warp w of a tile owns its rows [w * 32 * FS_ITEMS, (w + 1) * 32 * FS_ITEMS), item k of
+// lane l is row 32 k + l of that range, and items are ranked in row order, so the in-tile rank is stable.  Row ids are 32-bit;
+// words are W (uint32_t for keys of <= 4 bytes, uint64_t otherwise).
+template <typename W, int MODE>
+__global__ void __launch_bounds__(FS_THREADS) fsort_pass_kernel(const __grid_constant__ FsPassArgs a) {
+    __shared__ uint32_t s_hist[FS_WARPS][256];  // per-warp digit counts, then each warp's offset inside the digit's tile run
+    __shared__ uint32_t s_start[256];           // tile-local first position of each digit
+    __shared__ uint32_t s_gofs[256];            // output row of tile-local position p of digit d: s_gofs[d] + p
+    __shared__ uint32_t s_wsum[FS_WARPS];
+    __shared__ W s_stage[FS_TILE];
+    __shared__ uint8_t s_dig[FS_TILE];
+    __shared__ uint32_t s_tile;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) s_tile = atomicAdd(a.tile_counter, 1u);
+    for (int i = threadIdx.x; i < FS_WARPS * 256; i += FS_THREADS) (&s_hist[0][0])[i] = 0;
+    __syncthreads();
+    const uint32_t t = s_tile;
+    const int64_t tile0 = (int64_t)t * FS_TILE;
+    const int tile_n = (int)(a.n - tile0 < FS_TILE ? a.n - tile0 : FS_TILE);
+    const int64_t row0 = tile0 + warp * (32 * FS_ITEMS) + lane;
+    const unsigned lt = (1u << lane) - 1;
+    W w[FS_ITEMS];
+    uint32_t id[FS_ITEMS], rk[FS_ITEMS];
+#pragma unroll
+    for (int k = 0; k < FS_ITEMS; k++) {
+        const int64_t i = row0 + 32 * k;
+        const bool valid = i < a.n;
+        uint32_t d = 0;
+        w[k] = 0; id[k] = 0;
+        if (valid) {
+            if (MODE == FS_IN_PAIRS) {
+                w[k] = ((const W*)a.w_in)[i];
+                id[k] = a.id_in[i];
+            } else {
+                const uint32_t r = MODE == FS_IN_COLUMN ? (uint32_t)i : (a.id_in[i] & FS_ID_MASK);
+                bool na;
+                w[k] = (W)fs_word(a.key, a.ch.p[r >> FS_CHUNK_LOG], r & (FS_CHUNK - 1), &na);
+                id[k] = r | ((uint32_t)(na ? a.key.na_last : !a.key.na_last) << 31);
+            }
+            d = fs_digit(w[k], id[k], a.shift);
+        }
+        // warp multisplit: m = the valid lanes whose digit equals this lane's
+        unsigned m = __ballot_sync(0xffffffffu, valid);
+#pragma unroll
+        for (int b = 0; b < 8; b++) {
+            const unsigned bal = __ballot_sync(0xffffffffu, (d >> b) & 1);
+            m &= ((d >> b) & 1) ? bal : ~bal;
+        }
+        const uint32_t before = valid ? s_hist[warp][d] : 0;
+        __syncwarp();
+        if (valid && (m & lt) == 0) s_hist[warp][d] = before + __popc(m);
+        __syncwarp();
+        rk[k] = before + __popc(m & lt);
+    }
+    __syncthreads();
+    // thread d: digit d's warp offsets, tile count, tile-local start and look-back
+    const int d = threadIdx.x;
+    uint32_t cnt = 0;
+#pragma unroll
+    for (int q = 0; q < FS_WARPS; q++) { const uint32_t x = s_hist[q][d]; s_hist[q][d] = cnt; cnt += x; }
+    uint32_t inc = cnt;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
+    if (lane == 31) s_wsum[warp] = inc;
+    volatile unsigned long long* status = a.status;
+    const unsigned long long tag = (unsigned long long)a.epoch << 34;
+    uint32_t excl = 0;
+    if (t == 0) {
+        status[d] = tag | FS_INCL | cnt;
+    } else {
+        status[(int64_t)t * 256 + d] = tag | FS_AGG | cnt;
+        // Tile j < t drew its number before this one, so its block is running and publishes its aggregate without waiting.
+        for (int64_t j = (int64_t)t - 1;;) {
+            const unsigned long long s = status[j * 256 + d];
+            if ((s >> 34) != a.epoch) continue;
+            excl += (uint32_t)s;
+            if (s & FS_INCL) break;
+            j--;
+        }
+        status[(int64_t)t * 256 + d] = tag | FS_INCL | (excl + cnt);
+    }
+    __syncthreads();
+    uint32_t wpre = 0;
+    for (int q = 0; q < warp; q++) wpre += s_wsum[q];
+    const uint32_t start = wpre + inc - cnt;
+    s_start[d] = start;
+    s_gofs[d] = a.base[d] + excl - start;
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < FS_ITEMS; k++) {
+        if (row0 + 32 * k < a.n) {
+            const uint32_t dk = fs_digit(w[k], id[k], a.shift);
+            rk[k] += s_start[dk] + s_hist[warp][dk];
+            s_stage[rk[k]] = w[k];
+            s_dig[rk[k]] = (uint8_t)dk;
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < tile_n; i += FS_THREADS) ((W*)a.w_out)[s_gofs[s_dig[i]] + (uint32_t)i] = s_stage[i];
+    __syncthreads();
+    uint32_t* s_id = (uint32_t*)s_stage;
+#pragma unroll
+    for (int k = 0; k < FS_ITEMS; k++)
+        if (row0 + 32 * k < a.n) s_id[rk[k]] = id[k];
+    __syncthreads();
+    for (int i = threadIdx.x; i < tile_n; i += FS_THREADS) a.id_out[s_gofs[s_dig[i]] + (uint32_t)i] = s_id[i];
+}
+
+struct FsGatherArgs {
+    int64_t n;
+    const uint32_t* ids;  // the permutation (bit 31 ignored); nullptr: identity
+    FsLayout lay;
+    void* out[TK_MAX_COLS];
+    uint8_t* out_vb[TK_MAX_COLS];
+    FsChunks ch;
+};
+
+__global__ void __launch_bounds__(256) fsort_gather_kernel(const __grid_constant__ FsGatherArgs a) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += stride) {
+        const uint32_t r = a.ids ? (a.ids[i] & FS_ID_MASK) : (uint32_t)i;
+        const char* chunk = a.ch.p[r >> FS_CHUNK_LOG];
+        const int64_t off = r & (FS_CHUNK - 1);
+        for (int c = 0; c < a.lay.n_cols; c++) {
+            tk_copy_cell(chunk + a.lay.coff[c], off, a.out[c], i, ctype_size(a.lay.ctype[c]));
+            if (a.lay.voff[c] >= 0) a.out_vb[c][i] = (uint8_t)chunk[a.lay.voff[c] + off];
+        }
+    }
+}
+
+static_assert(FS_THREADS == 256, "fsort_pass_kernel: one thread per digit");
+
+template <typename W>
+void launch_fsort_pass(int mode, int64_t n_tiles, const FsPassArgs& a, cudaStream_t st) {
+    const unsigned g = (unsigned)n_tiles;
+    if (mode == FS_IN_PAIRS) fsort_pass_kernel<W, FS_IN_PAIRS><<<g, FS_THREADS, 0, st>>>(a);
+    else if (mode == FS_IN_COLUMN) fsort_pass_kernel<W, FS_IN_COLUMN><<<g, FS_THREADS, 0, st>>>(a);
+    else fsort_pass_kernel<W, FS_IN_GATHER><<<g, FS_THREADS, 0, st>>>(a);
+}
+
 struct SortState {
     int device;
     cudaStream_t stream;
@@ -284,12 +578,19 @@ struct SortState {
     int64_t n_out = 0, out_cursor = 0;
     // metrics
     int64_t rows_consumed = 0, rows_admitted = 0, admitted_after_cutoff = 0, reduce_steps = 0, count_reads = 0, filter_launches = 0;
+    // full sort (no limit): the chunk store, the output store and its validity bytes
+    bool full = false;
+    FsLayout lay{};
+    int64_t chunk_bytes = 0, n_chunks = 0, passes_run = 0, passes_skipped = 0;
+    std::vector<DevBuf> chunks, out_mem;
 
-    SortState(int64_t limit_, int64_t offset_, const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_keys, const int32_t* asc,
-              const int32_t* na_last, int64_t obs, int dev, cudaStream_t st)
-        : device(dev), stream(st), limit(limit_), offset(offset_), output_batch_size(obs) {
-        B200_REQUIRE(limit >= 0 && offset >= 0, "b200 sort: limit and offset must be non-negative");
-        B200_REQUIRE(limit <= TK_MAX_K && offset <= TK_MAX_K - limit, "b200 sort: limit + offset exceeds the top-k cap of 2^26 rows");
+    SortState(bool full_, int64_t limit_, int64_t offset_, const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_keys,
+              const int32_t* asc, const int32_t* na_last, int64_t obs, int dev, cudaStream_t st)
+        : device(dev), stream(st), limit(limit_), offset(offset_), output_batch_size(obs), full(full_) {
+        if (!full) {
+            B200_REQUIRE(limit >= 0 && offset >= 0, "b200 sort: limit and offset must be non-negative");
+            B200_REQUIRE(limit <= TK_MAX_K && offset <= TK_MAX_K - limit, "b200 sort: limit + offset exceeds the top-k cap of 2^26 rows");
+        }
         B200_REQUIRE(n_keys >= 1 && n_keys <= TK_MAX_KEYS, "b200 sort: 1 to 4 sort keys");
         B200_REQUIRE(n_arrs >= n_keys && n_arrs <= TK_MAX_COLS, "b200 sort: keys are the first n_keys of at most 32 columns");
         B200_REQUIRE(c_types && arr_types && asc && na_last, "b200 sort: null argument");
@@ -304,12 +605,26 @@ struct SortState {
             if (!asc[j]) sc.desc_mask |= 1u << j;
             if (na_last[j]) sc.na_last_mask |= 1u << j;
         }
-        cap = std::max<int64_t>(2 * K, TK_MIN_CAP);
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
         h_count = (unsigned long long*)pinned_acquire(8);
         d_cursor.alloc(8); d_cutoff.alloc(sizeof(TkCutoff));
         B200_CUDA(cudaMemsetAsync(d_cursor.p, 0, 8, stream));
         B200_CUDA(cudaMemsetAsync(d_cutoff.p, 0, sizeof(TkCutoff), stream));
+        if (full) {
+            cap = 0;
+            lay.n_cols = n_arrs;
+            for (int c = 0; c < n_arrs; c++) {
+                lay.ctype[c] = sc.ctype[c];
+                lay.coff[c] = chunk_bytes;
+                chunk_bytes += FS_CHUNK * ctype_size(sc.ctype[c]);
+            }
+            for (int c = 0; c < n_arrs; c++) {
+                lay.voff[c] = arr_type[c] == ARR_NULLABLE ? chunk_bytes : -1;
+                if (arr_type[c] == ARR_NULLABLE) chunk_bytes += FS_CHUNK;
+            }
+            return;
+        }
+        cap = std::max<int64_t>(2 * K, TK_MIN_CAP);
         if (K == 0) return;  // nothing is ever kept: no store
         for (int b = 0; b < 2; b++) {
             auto take = [&](size_t bytes) { mem[b].emplace_back(); mem[b].back().alloc(bytes); return mem[b].back().p; };
@@ -378,9 +693,11 @@ struct SortState {
                          "b200 sort: a batch's column types differ from the state's schema");
         const int64_t n = t->n_rows;
         if (n > 0) B200_REQUIRE(t->device == device, "b200 sort: batches must be resident on the state's device (stage host batches first)");
+        if (full) B200_REQUIRE(n <= FS_MAX_ROWS - rows_consumed, "b200 sort: a full sort holds at most 2^31 rows (32-bit row ids)");
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
         const int64_t seq_base = rows_consumed;
         rows_consumed += n;
+        if (full) return append(t, seq_base, n);
         if (K == 0 || n == 0) return;
         TkFilterArgs a{};
         a.sc = sc;
@@ -406,11 +723,121 @@ struct SortState {
         }
     }
 
+    // Full sort: rows [0, n) of the batch go to rows [g0, g0 + n) of the chunk store.
+    void append(const b200_table* t, int64_t g0, int64_t n) {
+        FsAppendArgs a{};
+        a.lay = lay;
+        for (int c = 0; c < sc.n_cols; c++) { a.in_data[c] = t->cols[c].data; a.in_valid[c] = t->cols[c].validity; }
+        for (int64_t i = 0; i < n;) {
+            const int64_t g = g0 + i, k = g >> FS_CHUNK_LOG, off = g & (FS_CHUNK - 1);
+            const int64_t r = std::min(n - i, FS_CHUNK - off);
+            if (k == (int64_t)chunks.size()) {
+                chunks.emplace_back();
+                chunks.back().alloc((size_t)chunk_bytes);
+                n_chunks++;
+            }
+            a.src0 = i; a.n = r; a.dst0 = off; a.chunk = chunks[k].as<char>();
+            fsort_append_kernel<<<grid_for(r, 256), 256, 0, stream>>>(a);
+            B200_CUDA(cudaGetLastError());
+            i += r;
+        }
+    }
+
+    // Full sort at is_last: digit histograms, the pass plan, the digit passes and the gather into the output store (out_mem);
+    // the validity bytes of nullable column c go to out_vb[c].  Pair buffers and look-back words are freed on return.
+    void sort_full(std::vector<DevBuf>& out_vb) {
+        const int64_t n = rows_consumed;
+        const int nk = sc.n_keys;
+        FsChunks ch{};
+        for (size_t k = 0; k < chunks.size(); k++) ch.p[k] = chunks[k].as<char>();
+        FsKey key[TK_MAX_KEYS]{};
+        for (int j = 0; j < nk; j++)
+            key[j] = FsKey{sc.ctype[j], (int)((sc.desc_mask >> j) & 1), (int)((sc.na_last_mask >> j) & 1), lay.coff[j], lay.voff[j]};
+        DevBuf wbuf[2], ibuf[2], status, counters;
+        const uint32_t* ids = nullptr;  // the permutation so far; nullptr: identity
+        if (n > 0) {
+            DevBuf d_hist;
+            d_hist.alloc(FS_HIST_WORDS * 4);
+            B200_CUDA(cudaMemsetAsync(d_hist.p, 0, FS_HIST_WORDS * 4, stream));
+            FsHistArgs ha{};
+            ha.n = n; ha.n_keys = nk; ha.hist = d_hist.as<uint32_t>(); ha.ch = ch;
+            for (int j = 0; j < nk; j++) ha.key[j] = key[j];
+            fsort_hist_kernel<<<grid_for(n, FS_THREADS), FS_THREADS, 0, stream>>>(ha);
+            B200_CUDA(cudaGetLastError());
+            auto* h = (uint32_t*)pinned_acquire(FS_HIST_WORDS * 4);
+            B200_CUDA(cudaMemcpyAsync(h, d_hist.p, FS_HIST_WORDS * 4, cudaMemcpyDeviceToHost, stream));
+            B200_CUDA(cudaStreamSynchronize(stream));
+            // LSD plan: least significant key first; per key its byte digits from the lowest, then its NA class.  A digit that
+            // takes one value on every row leaves the order as it is: that pass is skipped.
+            struct Pass { int key, shift; uint32_t base[256]; };
+            std::vector<Pass> plan;
+            for (int j = nk - 1; j >= 0; j--) {
+                for (int b = 0; b < ctype_size(sc.ctype[j]); b++) {
+                    const uint32_t* c = h + (j * 8 + b) * 256;
+                    if (std::any_of(c, c + 256, [&](uint32_t x) { return (int64_t)x == n; })) { passes_skipped++; continue; }
+                    Pass p{j, 8 * b, {}};
+                    for (uint32_t d = 0, s = 0; d < 256; s += c[d], d++) p.base[d] = s;
+                    plan.push_back(p);
+                }
+                if (arr_type[j] == ARR_NULLABLE || ctype_is_float(sc.ctype[j])) {
+                    const int64_t na = h[TK_MAX_KEYS * 8 * 256 + j];
+                    if (na == 0 || na == n) { passes_skipped++; continue; }
+                    const int64_t class0 = key[j].na_last ? n - na : na;  // rows whose class bit is 0
+                    Pass p{j, -1, {}};
+                    for (int d = 1; d < 256; d++) p.base[d] = (uint32_t)class0;
+                    plan.push_back(p);
+                }
+            }
+            pinned_release(h, FS_HIST_WORDS * 4);
+            passes_run = (int64_t)plan.size();
+            if (!plan.empty()) {
+                size_t wb = 4;
+                for (const Pass& p : plan) if (ctype_size(sc.ctype[p.key]) > 4) wb = 8;
+                for (int b = 0; b < 2; b++) { wbuf[b].alloc((size_t)n * wb); ibuf[b].alloc((size_t)n * 4); }
+                const int64_t n_tiles = (n + FS_TILE - 1) / FS_TILE;
+                status.alloc((size_t)n_tiles * 256 * 8);
+                counters.alloc(plan.size() * 4);
+                B200_CUDA(cudaMemsetAsync(status.p, 0, (size_t)n_tiles * 256 * 8, stream));
+                B200_CUDA(cudaMemsetAsync(counters.p, 0, plan.size() * 4, stream));
+                int cur_buf = -1, prev_key = -1;
+                for (size_t q = 0; q < plan.size(); q++) {
+                    const Pass& p = plan[q];
+                    const int mode = p.key == prev_key ? FS_IN_PAIRS : ids ? FS_IN_GATHER : FS_IN_COLUMN;
+                    const int ob = cur_buf == 0 ? 1 : 0;
+                    FsPassArgs a{};
+                    a.n = n; a.shift = p.shift; a.epoch = (uint32_t)q + 1; a.key = key[p.key];
+                    a.w_in = cur_buf >= 0 ? wbuf[cur_buf].p : nullptr; a.id_in = ids;
+                    a.w_out = wbuf[ob].p; a.id_out = ibuf[ob].as<uint32_t>();
+                    a.status = status.as<unsigned long long>(); a.tile_counter = counters.as<unsigned int>() + q;
+                    std::copy(p.base, p.base + 256, a.base);
+                    a.ch = ch;
+                    if (ctype_size(sc.ctype[p.key]) > 4) launch_fsort_pass<uint64_t>(mode, n_tiles, a, stream);
+                    else launch_fsort_pass<uint32_t>(mode, n_tiles, a, stream);
+                    B200_CUDA(cudaGetLastError());
+                    cur_buf = ob; ids = ibuf[ob].as<uint32_t>(); prev_key = p.key;
+                }
+            }
+        }
+        FsGatherArgs ga{};
+        ga.n = n; ga.ids = ids; ga.lay = lay; ga.ch = ch;
+        out_mem.resize(sc.n_cols);
+        for (int c = 0; c < sc.n_cols; c++) {
+            out_mem[c].alloc((size_t)n * ctype_size(sc.ctype[c]));
+            ga.out[c] = out_mem[c].p;
+            if (arr_type[c] == ARR_NULLABLE) { out_vb[c].alloc((size_t)n); ga.out_vb[c] = out_vb[c].as<uint8_t>(); }
+        }
+        if (n > 0) fsort_gather_kernel<<<grid_for(n, 256), 256, 0, stream>>>(ga);
+        B200_CUDA(cudaGetLastError());
+    }
+
     void finish() {
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
-        if (K > 0) reduce();
+        std::vector<DevBuf> out_vb(sc.n_cols);  // full sort: the output's validity bytes, until they are packed
+        if (full) sort_full(out_vb);
+        else if (K > 0) reduce();
         finished = true;
-        n_out = std::max<int64_t>(0, held - offset);
+        n_out = full ? rows_consumed : std::max<int64_t>(0, held - offset);
+        auto vb_of = [&](int c) { return full ? out_vb[c].as<uint8_t>() : store[cur].vb[c] + offset; };
         int n_nullable = 0;
         for (int c = 0; c < sc.n_cols; c++) n_nullable += arr_type[c] == ARR_NULLABLE;
         const int64_t words = (n_out + 31) / 32 + 2;
@@ -420,9 +847,11 @@ struct SortState {
         for (int c = 0, k = 0; c < sc.n_cols; c++) {
             if (arr_type[c] != ARR_NULLABLE) continue;
             out_bitmap[c] = d_bitmaps.as<uint32_t>() + (k++) * words;
-            if (n_out > 0) launch_pack_bitmap(store[cur].vb[c] + offset, n_out, out_bitmap[c], grid_for(n_out, 256), stream);
+            if (n_out > 0) launch_pack_bitmap(vb_of(c), n_out, out_bitmap[c], grid_for(n_out, 256), stream);
         }
         B200_CUDA(cudaGetLastError());
+        chunks.clear();  // full sort: the rows now live in the output store
+        out_vb.clear();
         B200_CUDA(cudaStreamSynchronize(stream));
     }
 
@@ -433,10 +862,11 @@ struct SortState {
         if (bs % 32 != 0 && bs < n_out) bs = (bs + 31) & ~31ll;  // validity bitmaps are sliced at word granularity
         const int64_t rows = produce_output ? std::min(bs, n_out - out_cursor) : 0;
         out->n_rows = rows; out->n_cols = sc.n_cols; out->device = device;
-        const int64_t base = offset + out_cursor;
+        const int64_t base = full ? out_cursor : offset + out_cursor;
         for (int c = 0; c < sc.n_cols; c++) {
             b200_column& col = out->cols[c];
-            col.data = K == 0 ? d_cutoff.p : (char*)store[cur].data[c] + base * ctype_size(sc.ctype[c]);
+            if (full) col.data = out_mem[c].as<char>() + base * ctype_size(sc.ctype[c]);
+            else col.data = K == 0 ? d_cutoff.p : (char*)store[cur].data[c] + base * ctype_size(sc.ctype[c]);
             col.validity = out_bitmap[c] ? (uint8_t*)out_bitmap[c] + out_cursor / 8 : nullptr;
             col.length = rows; col.c_type = sc.ctype[c]; col.arr_type = arr_type[c];
         }
@@ -452,18 +882,30 @@ using b200::SortState;
 
 extern "C" {
 
-void* b200_sort_state_init(int64_t operator_id, int64_t limit, int64_t offset, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                           int32_t n_keys, const int32_t* ascending, const int32_t* na_last, int64_t output_batch_size, int32_t device,
-                           void* stream) {
-    (void)operator_id;
+static void* sort_state_new(bool full, int64_t limit, int64_t offset, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                            int32_t n_keys, const int32_t* ascending, const int32_t* na_last, int64_t output_batch_size, int32_t device,
+                            void* stream) {
     try {
         int ndev = 0;
         if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
             throw b200::Error("b200 sort: no CUDA device available (this path has no CPU fallback)");
         B200_REQUIRE(device >= 0 && device < ndev, "b200 sort: bad device ordinal");
-        return new SortState(limit, offset, c_types, arr_types, n_arrs, n_keys, ascending, na_last, output_batch_size, device,
+        return new SortState(full, limit, offset, c_types, arr_types, n_arrs, n_keys, ascending, na_last, output_batch_size, device,
                              (cudaStream_t)stream);
     } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
+}
+
+void* b200_sort_state_init(int64_t operator_id, int64_t limit, int64_t offset, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                           int32_t n_keys, const int32_t* ascending, const int32_t* na_last, int64_t output_batch_size, int32_t device,
+                           void* stream) {
+    (void)operator_id;
+    return sort_state_new(false, limit, offset, c_types, arr_types, n_arrs, n_keys, ascending, na_last, output_batch_size, device, stream);
+}
+
+void* b200_sort_state_init_full(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs, int32_t n_keys,
+                                const int32_t* ascending, const int32_t* na_last, int64_t output_batch_size, int32_t device, void* stream) {
+    (void)operator_id;
+    return sort_state_new(true, 0, 0, c_types, arr_types, n_arrs, n_keys, ascending, na_last, output_batch_size, device, stream);
 }
 
 int b200_sort_build_consume_batch(void* state, const b200_table* in_table, int32_t is_last, int32_t* request_input) {
@@ -495,7 +937,9 @@ int64_t b200_sort_get_metric(void* state, int32_t which) {
         case 3: return s->count_reads;
         case 4: return s->filter_launches;
         case 5: return s->admitted_after_cutoff;
-        case 6: return s->cap;
+        case 6: return s->full ? s->n_chunks * b200::FS_CHUNK : s->cap;
+        case 7: return s->passes_run;
+        case 8: return s->passes_skipped;
         default: return -1;
     }
 }

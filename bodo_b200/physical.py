@@ -5,7 +5,8 @@ bodo/pandas/physical/operator.h:46-50,247-458; aggregate.h:65-365; join.h:58-744
     PhysicalReadPandas / PhysicalReadArrow / PhysicalReadParquet : sources (batches of host columns)
     PhysicalAggregate : sink of one pipeline (ConsumeBatch) and source of the next (ProduceBatch)
     PhysicalJoin      : sink for the build side, ProcessBatch for the probe side
-    PhysicalSort      : ORDER BY ... LIMIT ... OFFSET; sink of one pipeline and source of the next
+    PhysicalSort      : ORDER BY ... LIMIT ... OFFSET, or ORDER BY without LIMIT (full=True); sink of one pipeline and source
+                        of the next
     Pipeline          : while not finished: batch = source.ProduceBatch(); ... sink.ConsumeBatch(batch)
 
 plus two helpers that run those pipelines over pandas frames the way bodo.pandas does for
@@ -276,21 +277,27 @@ class PhysicalJoin:
 
 
 class PhysicalSort:
-    """Top-k sink/source (the reference's PhysicalSort, bodo/pandas/physical/sort.h, which DuckDB's TopN lowers to): rows
+    """Sort sink/source (the reference's PhysicalSort, bodo/pandas/physical/sort.h, which DuckDB's TopN lowers to): rows
     [offset, offset + limit) of the input sorted stably by `by` (column names; ascending / na_position per key or one for all).
-    The column names are taken from the first batch."""
+    With full=True (no limit, no offset) every row, sorted: an ORDER BY without LIMIT.  The column names are taken from the
+    first batch."""
 
-    def __init__(self, by, ascending=True, na_position="last", limit=None, offset=0, parallel: bool = False, **kw):
+    def __init__(self, by, ascending=True, na_position="last", limit=None, offset=0, parallel: bool = False, full: bool = False, **kw):
         self.args = (by, ascending, na_position, limit, offset, parallel)
+        self.full = bool(full)
         self.kw = kw
         self.state = None
-        if limit is None:
+        if self.full:
+            if limit is not None or offset not in (None, 0):
+                raise S._lib.B200Error(f"PhysicalSort: a full sort takes no limit or offset (got limit={limit}, offset={offset})")
+        elif limit is None:
             raise S._lib.B200Error("PhysicalSort: a limit is required (a full sort without LIMIT is not supported)")
 
     def ConsumeBatch(self, batch: Table, prev: OperatorResult) -> OperatorResult:
         if self.state is None:
             by, asc, nap, limit, offset, parallel = self.args
-            self.state = S.init_stream_sort_state(-1, limit, offset, by, asc, nap, batch.names, parallel, **self.kw)
+            kw = dict(self.kw, full=True) if self.full else self.kw
+            self.state = S.init_stream_sort_state(-1, limit, offset, by, asc, nap, batch.names, parallel, **kw)
         is_last = prev == OperatorResult.FINISHED
         S.sort_build_consume_batch(self.state, batch, is_last)
         return OperatorResult.FINISHED if is_last else OperatorResult.NEED_MORE_INPUT
@@ -383,6 +390,17 @@ def sort_values_head(df, by, ascending=True, na_position="last", n: int = 5, off
     """df.sort_values(by, ascending=..., na_position=..., kind="stable").iloc[offset:offset + n] through PhysicalSort.  ascending and
     na_position may be one value or one per key.  Returns a pandas DataFrame with a fresh index."""
     op = PhysicalSort(by, ascending, na_position, limit=n, offset=offset, **kw)
+    run_pipeline(PhysicalReadPandas(df, batch_size), [], op)
+    coll = ResultCollector()
+    run_pipeline(op, [], coll)
+    op.Finalize()
+    return coll.result()
+
+
+def sort_values(df, by, ascending=True, na_position="last", batch_size: int = STREAMING_BATCH_SIZE, **kw):
+    """df.sort_values(by, ascending=..., na_position=..., kind="stable").reset_index(drop=True) through PhysicalSort(full=True).
+    ascending and na_position may be one value or one per key.  Returns a pandas DataFrame with a fresh index."""
+    op = PhysicalSort(by, ascending, na_position, full=True, **kw)
     run_pipeline(PhysicalReadPandas(df, batch_size), [], op)
     coll = ResultCollector()
     run_pipeline(op, [], coll)

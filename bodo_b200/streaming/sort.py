@@ -1,18 +1,24 @@
-"""Streaming top-k operator API (ORDER BY ... LIMIT ... OFFSET) — the host-side mirror of bodo/libs/streaming/sort.py.
+"""Streaming sort operator API (ORDER BY ... LIMIT ... OFFSET, and ORDER BY without LIMIT) — the host-side mirror of
+bodo/libs/streaming/sort.py.
 
 Same verbs as the reference's streaming sort (init_stream_sort_state, sort_build_consume_batch, produce_output_batch,
-delete_stream_sort_state), LIMIT form only: the result is rows [offset, offset + limit) of the input sorted stably by the `by`
+delete_stream_sort_state).  LIMIT form: the result is rows [offset, offset + limit) of the input sorted stably by the `by`
 columns, equal to
 
     df.assign(_seq=range(len(df))).sort_values([*by, "_seq"], ascending=[*asc, True], na_position=...).iloc[offset:offset + limit]
 
 with one na_position per key.  The work happens in libbodo_b200.so (sort.cu): one filter kernel per batch against a
-device-resident cutoff, and a device sort of the few surviving candidates.  A full sort without a limit is not provided.
+device-resident cutoff, and a device sort of the few surviving candidates.
+
+Full form (full=True, no limit, no offset): every row, equal to df.sort_values(by, kind="stable").reset_index(drop=True).  Each
+batch is appended to a device-resident chunk store, and is_last runs an LSD radix sort over it (sort.cu).  It is opt-in rather
+than limit=None: the state holds the entire input in device memory, so a query that lost its LIMIT fails instead.
 
 With parallel=True the state is one shard of a torch.distributed process group (one process per GPU): every rank reduces its
 own stream to at most limit + offset rows, the ranks all-gather those rows at is_last, every rank runs them (rank-major) through
 a fresh state, and rank 0 produces the result while the other ranks produce one empty batch.  The answer is the stable top-k
-of the rank inputs concatenated in rank order.
+of the rank inputs concatenated in rank order.  A sharded full sort is not supported: such a state raises at its first consume
+call when the process group has more than one rank (with one rank it sorts locally).
 """
 
 from __future__ import annotations
@@ -24,14 +30,21 @@ from ..table import CTable, Table, table_from_ctable, to_device
 MAX_KEYS = 4
 # limit + offset cap: the store addresses rows with uint32 ids and keeps two buffers of max(2 (limit + offset), 4 Mi) rows
 MAX_LIMIT_PLUS_OFFSET = 1 << 26
+# full sort: rows per state (32-bit row ids whose top bit carries a key's NA class during its class pass)
+MAX_FULL_SORT_ROWS = 1 << 31
 
 
 class SortState:
     """Python handle of the C sort state (created lazily at the first consume call)."""
 
     def __init__(self, operator_id, limit, offset, by, asc, na_position, col_names, parallel, output_batch_size, device, stream,
-                 process_group):
-        if limit is None:
+                 process_group, full=False):
+        self.full = bool(full)
+        if self.full:
+            if limit is not None or offset not in (None, 0):
+                raise _lib.B200Error(f"Streaming Sort: a full sort takes no limit or offset (got limit={limit}, offset={offset})")
+            limit = offset = 0
+        elif limit is None:
             raise _lib.B200Error("Streaming Sort: a limit is required (a full sort without LIMIT is not supported)")
         limit, offset = int(limit), int(offset or 0)
         if limit < 0 or offset < 0:
@@ -84,8 +97,12 @@ class SortState:
         nal = ffi.new("int32_t[]", [int(x) for x in self.na_last])
         lim = self.limit if limit is None else limit
         off = self.offset if offset is None else offset
-        h = L.b200_sort_state_init(self.operator_id, lim, off, c_types, a_types, len(cols), len(self.by), asc, nal,
-                                   self.output_batch_size, self.device, ffi.cast("void*", self.stream))
+        if self.full:
+            h = L.b200_sort_state_init_full(self.operator_id, c_types, a_types, len(cols), len(self.by), asc, nal, self.output_batch_size,
+                                            self.device, ffi.cast("void*", self.stream))
+        else:
+            h = L.b200_sort_state_init(self.operator_id, lim, off, c_types, a_types, len(cols), len(self.by), asc, nal,
+                                       self.output_batch_size, self.device, ffi.cast("void*", self.stream))
         self.handle = _lib.check_ptr(h, "init_stream_sort_state")
 
     def _consume(self, table: Table, is_last: bool):
@@ -133,13 +150,15 @@ def _current_device() -> int:
 
 
 def init_stream_sort_state(operator_id, limit, offset, by, asc, na_position, col_names, parallel=False, *, output_batch_size=32768,
-                           device=None, stream=0, process_group=None) -> SortState:
-    """Mirror of bodo.libs.streaming.sort.init_stream_sort_state, LIMIT form.
+                           device=None, stream=0, process_group=None, full=False) -> SortState:
+    """Mirror of bodo.libs.streaming.sort.init_stream_sort_state.
 
     by: sort key column names (1..4); asc / na_position: one value or one per key; col_names: the input columns, in order.
-    Raises B200Error without a limit, for a negative limit or offset, or when limit + offset exceeds MAX_LIMIT_PLUS_OFFSET."""
+    LIMIT form (full=False): raises B200Error without a limit, for a negative limit or offset, or when limit + offset exceeds
+    MAX_LIMIT_PLUS_OFFSET.  Full sort (full=True): every row in sorted order; limit must be None and offset None or 0, and the
+    state holds at most MAX_FULL_SORT_ROWS rows."""
     return SortState(operator_id, limit, offset, by, asc, na_position, col_names, parallel, output_batch_size, device, stream,
-                     process_group)
+                     process_group, full)
 
 
 def sort_build_consume_batch(state: SortState, table: Table, is_last: bool):
@@ -153,6 +172,8 @@ def sort_build_consume_batch(state: SortState, table: Table, is_last: bool):
         sharded = dist.is_initialized() and dist.get_world_size(state.process_group) > 1
     else:
         sharded = False
+    if sharded and state.full:
+        raise _lib.B200Error("Streaming Sort: a sharded full sort is not supported (process group of more than one rank)")
     # a sharded rank keeps its first limit + offset rows: the offset applies to the gathered result only
     state._ensure(table, *((state.limit + state.offset, 0) if sharded else (None, None)))
     req = state._consume(table, is_last)
@@ -185,5 +206,6 @@ def delete_stream_sort_state(state: SortState) -> None:
 
 def get_metric(state: SortState, which: int) -> int:
     """0 rows consumed, 1 rows admitted as candidates, 2 reduce steps, 3 host reads of the candidate count, 4 filter launches,
-    5 rows admitted while a cutoff existed, 6 store capacity in rows."""
+    5 rows admitted while a cutoff existed, 6 store capacity in rows, 7 digit passes run (full sort), 8 digit passes skipped
+    because their digit is constant over all rows (full sort).  Metrics 1-5 read 0 in a full sort, 7 and 8 in a top-k."""
     return int(_lib.lib().b200_sort_get_metric(state.handle, which))

@@ -219,8 +219,18 @@ void* b200_sort_state_init(int64_t operator_id, int64_t limit, int64_t offset, c
                            int32_t n_arrs, int32_t n_keys, const int32_t* ascending, const int32_t* na_last,
                            int64_t output_batch_size, int32_t device, void* stream);
 
+/* stream_sort_state_init_py_entry (_sort.cpp), the form without LIMIT: a full sort.  The result is every input row, sorted
+ * stably by the same key, type and NA rules as b200_sort_state_init; it equals df.sort_values(by, kind="stable").  The state
+ * holds the whole input in device memory (fixed 2^24-row chunks) and sorts it at is_last with an LSD radix sort; at most 2^31
+ * rows (32-bit row ids), a consume call past that fails before it launches anything.  The build-consume, produce, delete and
+ * metric entries below serve both forms. */
+void* b200_sort_state_init_full(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs, int32_t n_keys,
+                                const int32_t* ascending, const int32_t* na_last, int64_t output_batch_size, int32_t device,
+                                void* stream);
+
 /* The build-consume entry of _sort.cpp: filters a DEVICE-resident batch (same schema as the state) against the current cutoff on
- * the device; on is_last reduces to the final rows.  Returns 1 after is_last, 0 otherwise, < 0 on error; *request_input = 1. */
+ * the device (full sort: appends it to the chunk store); on is_last reduces to the final rows (full sort: sorts every row).
+ * Returns 1 after is_last, 0 otherwise, < 0 on error; *request_input = 1. */
 int b200_sort_build_consume_batch(void* state, const b200_table* in_table, int32_t is_last, int32_t* request_input);
 
 /* The produce-output entry of _sort.cpp: fills `out` (out->cols with room for n_arrs descriptors) with library-owned device
@@ -231,7 +241,9 @@ int b200_sort_produce_output_batch(void* state, b200_table* out, int32_t* out_is
 void b200_delete_sort_state(void* state);
 
 /* Metrics: 0 rows consumed, 1 rows admitted as candidates, 2 reduce steps, 3 host reads of the candidate count, 4 filter
- * launches, 5 rows admitted while a cutoff existed, 6 store capacity in rows. */
+ * launches, 5 rows admitted while a cutoff existed, 6 store capacity in rows, 7 digit passes run (full sort), 8 digit passes
+ * skipped because their digit is constant over all rows (full sort).  A full sort reads 0 for metrics 1-5; top-k reads 0 for
+ * 7 and 8.  Full-sort passes: per key one per byte of its width, plus one NA-class pass for a nullable or float key. */
 int64_t b200_sort_get_metric(void* state, int32_t which);
 
 /* ---- row -> rank shuffle (reference: bodo/libs/_shuffle.cpp) ---- */
