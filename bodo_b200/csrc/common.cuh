@@ -53,7 +53,7 @@ __host__ __device__ inline int ctype_size(int ct) {
     }
 }
 __host__ __device__ inline bool ctype_is_float(int ct) { return ct == CT_FLOAT32 || ct == CT_FLOAT64; }
-inline bool ctype_is_signed_int(int ct) {
+__host__ __device__ inline bool ctype_is_signed_int(int ct) {
     return ct == CT_INT8 || ct == CT_INT16 || ct == CT_INT32 || ct == CT_INT64 || ct == CT_DATE || ct == CT_DATETIME ||
            ct == CT_TIMEDELTA;
 }
@@ -176,6 +176,24 @@ __device__ __forceinline__ double load_as_f64(const void* __restrict__ p, int ct
         case CT_FLOAT64: return ((const double*)p)[i];
         case CT_FLOAT32: return (double)((const float*)p)[i];
         default: return (double)load_int_as_i64(p, ct, i);
+    }
+}
+// The bits of the `size`-byte cell i, zero-extended.
+__device__ __forceinline__ uint64_t load_bits(const void* __restrict__ p, int size, int64_t i) {
+    switch (size) {
+        case 8: return ((const uint64_t*)p)[i];
+        case 4: return ((const uint32_t*)p)[i];
+        case 2: return ((const uint16_t*)p)[i];
+        default: return ((const uint8_t*)p)[i];
+    }
+}
+// dst[di] = src[si] for cells of `size` bytes.
+__device__ __forceinline__ void copy_cell(void* dst, int64_t di, const void* src, int64_t si, int size) {
+    switch (size) {
+        case 8: ((uint64_t*)dst)[di] = ((const uint64_t*)src)[si]; break;
+        case 4: ((uint32_t*)dst)[di] = ((const uint32_t*)src)[si]; break;
+        case 2: ((uint16_t*)dst)[di] = ((const uint16_t*)src)[si]; break;
+        default: ((uint8_t*)dst)[di] = ((const uint8_t*)src)[si]; break;
     }
 }
 

@@ -230,14 +230,6 @@ struct GatherArgs {
     void* ob_data[J_MAX_COLS]; uint8_t* ob_valid[J_MAX_COLS];  // output columns (validity: one byte per row or nullptr)
     void* op_data[J_MAX_COLS]; uint8_t* op_valid[J_MAX_COLS];
 };
-__device__ __forceinline__ void copy_item(void* dst, int64_t d, const void* src, int64_t s, int size) {
-    switch (size) {
-        case 8: ((uint64_t*)dst)[d] = ((const uint64_t*)src)[s]; break;
-        case 4: ((uint32_t*)dst)[d] = ((const uint32_t*)src)[s]; break;
-        case 2: ((uint16_t*)dst)[d] = ((const uint16_t*)src)[s]; break;
-        default: ((uint8_t*)dst)[d] = ((const uint8_t*)src)[s]; break;
-    }
-}
 __device__ __forceinline__ void zero_item(void* dst, int64_t d, int size) {
     switch (size) {
         case 8: ((uint64_t*)dst)[d] = 0; break;
@@ -260,14 +252,14 @@ __global__ void __launch_bounds__(256) join_probe_gather_kernel(const __grid_con
                 uint32_t brow = c == 1 ? a.info[s].first : a.groups[a.goffs[s] + q];
                 if (a.bmatched) a.bmatched[brow] = 1;
                 for (int k = 0; k < a.n_b; k++) {
-                    copy_item(a.ob_data[k], orow, a.b_data[k], brow, a.b_size[k]);
+                    copy_cell(a.ob_data[k], orow, a.b_data[k], brow, a.b_size[k]);
                     if (a.ob_valid[k]) a.ob_valid[k][orow] = a.b_valid[k] ? a.b_valid[k][brow] : 1;
                 }
             } else {
                 for (int k = 0; k < a.n_b; k++) { zero_item(a.ob_data[k], orow, a.b_size[k]); a.ob_valid[k][orow] = 0; }
             }
             for (int k = 0; k < a.n_p; k++) {
-                copy_item(a.op_data[k], orow, a.p_data[k], i, a.p_size[k]);
+                copy_cell(a.op_data[k], orow, a.p_data[k], i, a.p_size[k]);
                 if (a.op_valid[k]) a.op_valid[k][orow] = bit_valid(a.p_valid[k], i) ? 1 : 0;
             }
         }
@@ -295,7 +287,7 @@ __global__ void join_unmatched_emit_kernel(const __grid_constant__ TailArgs a) {
         if (!a.flags[i]) continue;
         int64_t orow = (int64_t)a.off[i];
         for (int k = 0; k < a.n_b; k++) {
-            copy_item(a.ob_data[k], orow, a.b_data[k], i, a.b_size[k]);
+            copy_cell(a.ob_data[k], orow, a.b_data[k], i, a.b_size[k]);
             if (a.ob_valid[k]) a.ob_valid[k][orow] = a.b_valid[k] ? a.b_valid[k][i] : 1;
         }
         for (int k = 0; k < a.n_p; k++) { zero_item(a.op_data[k], orow, a.p_size[k]); a.op_valid[k][orow] = 0; }
@@ -432,7 +424,7 @@ __global__ void __launch_bounds__(256) join_probe_fast_kernel(const __grid_const
                 if (a.ob_valid[k2]) a.ob_valid[k2][orow] = f < 0 ? (kvalid[r] ? 1 : 0) : (a.b_valid[k2] ? a.b_valid[k2][brow[r]] : 1);
             }
             for (int k2 = 0; k2 < a.n_p; k2++) {
-                copy_item(a.op_data[k2], orow, a.p_data[k2], i, a.p_size[k2]);
+                copy_cell(a.op_data[k2], orow, a.p_data[k2], i, a.p_size[k2]);
                 if (a.op_valid[k2]) a.op_valid[k2][orow] = bit_valid(a.p_valid[k2], i) ? 1 : 0;
             }
         }

@@ -1,24 +1,19 @@
-// sort.cu — streaming top-k: ORDER BY k_0 .. k_{n-1} LIMIT limit OFFSET offset over a stream of batches (sm_90a).
+// sort.cu — streaming sort over a stream of batches (sm_90a): ORDER BY k_0 .. k_{n-1} [LIMIT limit OFFSET offset].
 //
-// Replaces the LIMIT form of the reference's streaming sort state (bodo/libs/streaming/_sort.cpp: stream_sort_state_init_py_entry,
-// the build-consume and produce-output entries, delete_stream_sort_state), which DuckDB's TopN lowers to (PhysicalSort,
-// bodo/pandas/physical/sort.h).  Only the first K = limit + offset rows of the stable sort are ever needed, so the state keeps at
-// most K "held" rows and a device-resident cutoff, the key tuple of the K-th held row:
+// Replaces the reference's streaming sort state (bodo/libs/streaming/_sort.cpp: stream_sort_state_init_py_entry, the
+// build-consume and produce-output entries, delete_stream_sort_state), which DuckDB's ORDER BY and TopN lower to (PhysicalSort,
+// bodo/pandas/physical/sort.h).  Two forms share the schema, the batch checks, the key encoding and the output side (SortState);
+// each keeps its own rows:
 //
-//   topk_filter_kernel   one pass per batch over the key columns only: a row survives iff its key tuple is strictly below the
-//                        cutoff (a row that ties the cutoff sorts after the held row, its arrival index is larger).  Survivors are
-//                        compacted (warp ballot -> tile scan -> one cursor atomic per tile) into the candidate store together with
-//                        their encoded keys, arrival index and every column; payload bytes are read for survivors only.
-//   reduce               held rows + candidates are sorted by (encoded keys, arrival index): topk_block_sort_kernel (bitonic sort
-//                        of 1024-row tiles in shared memory) then topk_merge_kernel passes (merge path over pairs of sorted runs,
-//                        every run cut to its first K rows); topk_gather_kernel moves the first K rows into the other store buffer
-//                        and writes the new cutoff.
+//   TopkState      ORDER BY ... LIMIT: only the first K = limit + offset rows of the stable sort are ever needed, so the state
+//                  keeps at most K "held" rows and a device-resident cutoff, the key tuple of the K-th held row (topk_* kernels).
+//   FullSortState  ORDER BY without LIMIT: every row is appended to a chunk store and radix-sorted at is_last (fsort_* kernels).
 //
-// Key encoding: each key becomes one uint64 whose unsigned order is the key order (sign bit flipped for signed integers and
-// temporals; floats widened to double, -0.0 folded onto +0.0, then the order-preserving form; complemented for a descending
-// key) plus one NA-class bit (NA and NaN keys: word 0, class 1 for na_position="last", 0 for "first"; other keys the opposite
-// class).  Rows compare lexicographically over (class_0, word_0, class_1, word_1, ..., arrival index): no two rows are equal,
-// so the (unstable) bitonic sort still yields the stable order.
+// Key encoding (sort_word): each key cell becomes an unsigned integer of the key's own width whose unsigned order is the key
+// order (sign bit flipped for signed integers and temporals; float32 and float64 in their ordered forms with -0.0 folded onto
+// +0.0; complemented for a descending key), plus one NA-class bit: NA and NaN keys get word 0 and class 1 for
+// na_position="last", 0 for "first"; other keys the opposite class.  Rows compare lexicographically over (class_0, word_0,
+// class_1, word_1, ..., arrival index), so no two rows are equal.
 #include <algorithm>
 #include <vector>
 
@@ -26,8 +21,59 @@
 
 namespace b200 {
 
-constexpr int TK_MAX_KEYS = 4;
-constexpr int TK_MAX_COLS = 32;
+constexpr int SORT_MAX_KEYS = 4;
+constexpr int SORT_MAX_COLS = 32;
+
+// The schema both forms sort by: one descriptor per key (the first n_keys columns) and every column's type.  A key's width in
+// bytes is held beside its c-type: the kernels' raw loads read it rather than derive it from the c-type, which keeps the inlined
+// encoder from being specialised once per load width (smaller, faster filter and pass code).
+struct SortKey { int ct, size, desc, na_last; };
+struct SortSchema {
+    int n_keys, n_cols;
+    SortKey key[SORT_MAX_KEYS];
+    int ctype[SORT_MAX_COLS];
+};
+
+// Radix word of a key cell whose bits are `raw` (zero-extended).  `na` comes in true for a null cell and leaves true for a null
+// or NaN cell, whose word is 0.
+__device__ __forceinline__ uint64_t sort_word(const SortKey& k, uint64_t raw, bool& na) {
+    uint64_t w;
+    int bits;
+    if (k.ct == CT_FLOAT64) {
+        const double d = __longlong_as_double((long long)raw);
+        na = na || isnan(d);
+        w = (uint64_t)canon_float_ordered(canon_float_key(d)) ^ 0x8000000000000000ull;
+        bits = 64;
+    } else if (k.ct == CT_FLOAT32) {
+        const float f = __uint_as_float((uint32_t)raw);
+        na = na || isnan(f);
+        const uint32_t b = f == 0.0f ? 0u : (uint32_t)raw;
+        w = b ^ ((b >> 31) ? 0xFFFFFFFFu : 0x80000000u);
+        bits = 32;
+    } else {
+        bits = 8 * k.size;
+        w = ctype_is_signed_int(k.ct) ? raw ^ (1ull << (bits - 1)) : raw;
+    }
+    if (k.desc) w = ~w & (bits == 64 ? ~0ull : (1ull << bits) - 1);
+    return na ? 0 : w;
+}
+// NA-class bit of a key cell (`na`: null or NaN).
+__device__ __forceinline__ uint32_t sort_class(const SortKey& k, bool na) { return na ? k.na_last : !k.na_last; }
+
+// ---- top-k (ORDER BY ... LIMIT): candidate filter, bitonic sort + merge reduce ----
+//
+//   topk_filter_kernel   one pass per batch over the key columns only: a row survives iff its key tuple is strictly below the
+//                        cutoff (a row that ties the cutoff sorts after the held row, its arrival index is larger).  Survivors are
+//                        compacted (warp ballot -> tile scan -> one cursor atomic per tile) into the candidate store together with
+//                        their key words, arrival index and every column; payload bytes are read for survivors only.
+//   reduce               held rows + candidates are sorted by (key words, arrival index): topk_block_sort_kernel (bitonic sort of
+//                        1024-row tiles in shared memory) then topk_merge_kernel passes (merge path over pairs of sorted runs,
+//                        every run cut to its first K rows); topk_gather_kernel moves the first K rows into the other store buffer
+//                        and writes the new cutoff.
+//
+// The store keeps each key's word zero-extended to 64 bits; words of one key all have that key's width, so they compare as they
+// would at it.  No two rows are equal, so the (unstable) bitonic sort still yields the stable order.
+//
 // K = limit + offset is capped so that store row ids (uint32, the sort permutation) and the two store buffers of max(2K, 4 Mi)
 // rows stay within reach: 2^26 rows is 2 x 128 Mi rows of store, about 5 GB per 8-byte column.
 constexpr int64_t TK_MAX_K = 1ll << 26;
@@ -38,82 +84,52 @@ constexpr int64_t TK_MIN_CAP = 1ll << 22;
 constexpr int TK_THREADS = 256, TK_ROWS = 4, TK_TILE = TK_THREADS * TK_ROWS;
 constexpr int TK_SORT_TILE = 1024, TK_SORT_THREADS = 512, TK_MERGE_ITEMS = 8;
 constexpr uint32_t TK_SENTINEL = 0xFFFFFFFFu;
-constexpr uint64_t TK_SIGN = 0x8000000000000000ull;
 
-struct TkCutoff { uint32_t has; uint32_t cls; uint64_t w[TK_MAX_KEYS]; };
+struct TkCutoff { uint32_t has; uint32_t cls; uint64_t w[SORT_MAX_KEYS]; };
 
-// One buffer of rows, structure of arrays: encoded key words, NA-class bits (bit j = key j), arrival index, every column's values
-// and, for nullable columns, one validity byte per row.
+// One buffer of rows, structure of arrays: key words, NA-class bits (bit j = key j), arrival index, every column's values and,
+// for nullable columns, one validity byte per row.
 struct TkStore {
-    uint64_t* w[TK_MAX_KEYS];
+    uint64_t* w[SORT_MAX_KEYS];
     uint8_t* cls;
     int64_t* seq;
-    void* data[TK_MAX_COLS];
-    uint8_t* vb[TK_MAX_COLS];
-};
-
-struct TkSchema {
-    int n_keys, n_cols;
-    int ctype[TK_MAX_COLS];
-    uint32_t desc_mask, na_last_mask;
+    void* data[SORT_MAX_COLS];
+    uint8_t* vb[SORT_MAX_COLS];
 };
 
 struct TkFilterArgs {
-    TkSchema sc;
+    SortSchema sc;
     int64_t row0, row1;      // rows [row0, row1) of the batch
     int64_t seq_base;        // arrival index of batch row 0
-    const void* in_data[TK_MAX_COLS];
-    const uint8_t* in_valid[TK_MAX_COLS];
+    const void* in_data[SORT_MAX_COLS];
+    const uint8_t* in_valid[SORT_MAX_COLS];
     const TkCutoff* cutoff;
     TkStore st;
     unsigned long long* cursor;  // rows in the store
 };
 
-__device__ __forceinline__ bool tk_signed(int ct) {
-    return ct == CT_INT8 || ct == CT_INT16 || ct == CT_INT32 || ct == CT_INT64 || ct == CT_DATE || ct == CT_DATETIME || ct == CT_TIMEDELTA;
-}
-
-// Encoded word of key column j at row i; *cls receives its NA-class bit.
-__device__ __forceinline__ uint64_t tk_encode(const TkSchema& sc, int j, const void* p, const uint8_t* valid, int64_t i, uint32_t* cls) {
-    const int ct = sc.ctype[j];
-    uint64_t w;
-    bool na = !bit_valid(valid, i);
-    if (ctype_is_float(ct)) {
-        const double d = load_as_f64(p, ct, i);
-        na = na || isnan(d);
-        w = (uint64_t)canon_float_ordered(canon_float_key(d)) ^ TK_SIGN;
-    } else {
-        const uint64_t v = (uint64_t)load_int_as_i64(p, ct, i);
-        w = tk_signed(ct) ? v ^ TK_SIGN : v;
-    }
-    const uint32_t na_last = (sc.na_last_mask >> j) & 1;
-    *cls = na ? na_last : na_last ^ 1;
-    if (na) return 0;
-    return ((sc.desc_mask >> j) & 1) ? ~w : w;
+// Radix word of key j at batch row i; *cls receives its NA-class bit.
+__device__ __forceinline__ uint64_t tk_word(const TkFilterArgs& a, int j, int64_t i, uint32_t* cls) {
+    const SortKey& k = a.sc.key[j];
+    bool na = !bit_valid(a.in_valid[j], i);
+    const uint64_t w = sort_word(k, load_bits(a.in_data[j], k.size, i), na);
+    *cls = sort_class(k, na);
+    return w;
 }
 
 // The row's key tuple is strictly below the cutoff's.
 __device__ __forceinline__ bool tk_below_cutoff(const TkFilterArgs& a, const TkCutoff& c, int64_t row) {
 #pragma unroll
-    for (int j = 0; j < TK_MAX_KEYS; j++) {
+    for (int j = 0; j < SORT_MAX_KEYS; j++) {
         if (j < a.sc.n_keys) {
             uint32_t cl;
-            const uint64_t w = tk_encode(a.sc, j, a.in_data[j], a.in_valid[j], row, &cl);
+            const uint64_t w = tk_word(a, j, row, &cl);
             const uint32_t cc = (c.cls >> j) & 1;
             if (cl != cc) return cl < cc;
             if (w != c.w[j]) return w < c.w[j];
         }
     }
     return false;
-}
-
-__device__ __forceinline__ void tk_copy_cell(const void* src, int64_t si, void* dst, int64_t di, int size) {
-    switch (size) {
-        case 8: ((uint64_t*)dst)[di] = ((const uint64_t*)src)[si]; break;
-        case 4: ((uint32_t*)dst)[di] = ((const uint32_t*)src)[si]; break;
-        case 2: ((uint16_t*)dst)[di] = ((const uint16_t*)src)[si]; break;
-        default: ((uint8_t*)dst)[di] = ((const uint8_t*)src)[si]; break;
-    }
 }
 
 __global__ void __launch_bounds__(TK_THREADS, 4) topk_filter_kernel(const __grid_constant__ TkFilterArgs a) {
@@ -152,13 +168,13 @@ __global__ void __launch_bounds__(TK_THREADS, 4) topk_filter_kernel(const __grid
             uint32_t cls = 0;
             for (int j = 0; j < a.sc.n_keys; j++) {  // survivors are rare once a cutoff exists: encode again instead of holding it
                 uint32_t cl;
-                a.st.w[j][o] = tk_encode(a.sc, j, a.in_data[j], a.in_valid[j], row, &cl);
+                a.st.w[j][o] = tk_word(a, j, row, &cl);
                 cls |= cl << j;
             }
             a.st.cls[o] = (uint8_t)cls;
             a.st.seq[o] = a.seq_base + row;
             for (int c = 0; c < a.sc.n_cols; c++) {
-                tk_copy_cell(a.in_data[c], row, a.st.data[c], o, ctype_size(a.sc.ctype[c]));
+                copy_cell(a.st.data[c], o, a.in_data[c], row, ctype_size(a.sc.ctype[c]));
                 if (a.st.vb[c]) a.st.vb[c][o] = bit_valid(a.in_valid[c], row) ? 1 : 0;
             }
         }
@@ -170,7 +186,7 @@ __global__ void __launch_bounds__(TK_THREADS, 4) topk_filter_kernel(const __grid
 __device__ __forceinline__ bool tk_less(const TkStore& s, int nk, uint32_t a, uint32_t b) {
     const uint32_t ca = s.cls[a], cb = s.cls[b];
 #pragma unroll
-    for (int j = 0; j < TK_MAX_KEYS; j++) {
+    for (int j = 0; j < SORT_MAX_KEYS; j++) {
         if (j < nk) {
             const uint32_t x = (ca >> j) & 1, y = (cb >> j) & 1;
             if (x != y) return x < y;
@@ -243,7 +259,7 @@ __global__ void topk_merge_kernel(const TkStore s, int nk, int64_t n, int64_t K,
 }
 
 // dst row i = src row perm[i] for i < m; the K-th row becomes the cutoff; the store count becomes m.
-__global__ void topk_gather_kernel(const TkStore src, const TkStore dst, const TkSchema sc, const uint32_t* __restrict__ perm, int64_t m,
+__global__ void topk_gather_kernel(const TkStore src, const TkStore dst, const SortSchema sc, const uint32_t* __restrict__ perm, int64_t m,
                                    int64_t K, TkCutoff* cutoff, unsigned long long* cursor) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -254,7 +270,7 @@ __global__ void topk_gather_kernel(const TkStore src, const TkStore dst, const T
         dst.cls[i] = src.cls[si];
         dst.seq[i] = src.seq[si];
         for (int c = 0; c < sc.n_cols; c++) {
-            tk_copy_cell(src.data[c], si, dst.data[c], i, ctype_size(sc.ctype[c]));
+            copy_cell(dst.data[c], i, src.data[c], si, ctype_size(sc.ctype[c]));
             if (dst.vb[c]) dst.vb[c][i] = src.vb[c][si];
         }
         if (i == K - 1) {
@@ -278,62 +294,32 @@ __global__ void topk_gather_kernel(const TkStore src, const TkStore dst, const T
 //                        the column: in row order for the first key sorted, through the current permutation for the others.
 //   fsort_gather_kernel  every column and validity byte through the final permutation into the output store.
 //
-// Radix word: an unsigned integer of the key's own width whose order is the key order (sign bit flipped for signed integers and
-// temporals; float32 and float64 in their ordered forms with -0.0 folded onto 0.0; complemented for a descending key); an NA or NaN
-// key has word 0 and its NA-class bit set by na_position.  A key that can hold NAs gets one more pass on that class bit after its
-// byte passes; the bit rides in bit 31 of the row id, which is why the store holds at most 2^31 rows.
+// A key that can hold NAs gets one more pass on its NA-class bit after its byte passes; the bit rides in bit 31 of the row id,
+// which is why the store holds at most 2^31 rows.
 constexpr int FS_CHUNK_LOG = 24;
 constexpr int64_t FS_CHUNK = 1ll << FS_CHUNK_LOG;
 constexpr int FS_MAX_CHUNKS = 128;
 constexpr int64_t FS_MAX_ROWS = (int64_t)FS_MAX_CHUNKS * FS_CHUNK;  // 2^31
 constexpr int FS_THREADS = 256, FS_WARPS = FS_THREADS / 32, FS_ITEMS = 16, FS_TILE = FS_THREADS * FS_ITEMS;
 constexpr uint32_t FS_ID_MASK = 0x7FFFFFFFu;
-constexpr int FS_HIST_WORDS = TK_MAX_KEYS * 8 * 256 + TK_MAX_KEYS;  // [key][byte][digit] counts, then one NA count per key
+constexpr int FS_HIST_WORDS = SORT_MAX_KEYS * 8 * 256 + SORT_MAX_KEYS;  // [key][byte][digit] counts, then one NA count per key
 // look-back word: pass epoch (bits 34..63), AGGREGATE / INCLUSIVE flag (bits 32..33), count (bits 0..31)
 constexpr unsigned long long FS_AGG = 1ull << 32, FS_INCL = 2ull << 32;
 enum { FS_IN_PAIRS = 0, FS_IN_COLUMN = 1, FS_IN_GATHER = 2 };
 
 // One chunk is one allocation: FS_CHUNK values of every column, then FS_CHUNK validity bytes of every nullable column.
 struct FsLayout {
-    int n_cols;
-    int ctype[TK_MAX_COLS];
-    int64_t coff[TK_MAX_COLS];  // byte offset of column c's values in a chunk
-    int64_t voff[TK_MAX_COLS];  // byte offset of its validity bytes, -1 for a numpy column
+    SortSchema sc;
+    int64_t coff[SORT_MAX_COLS];  // byte offset of column c's values in a chunk
+    int64_t voff[SORT_MAX_COLS];  // byte offset of its validity bytes, -1 for a numpy column
 };
 struct FsChunks { const char* p[FS_MAX_CHUNKS]; };
-struct FsKey { int ct, desc, na_last; int64_t coff, voff; };
 
-// Radix word of the key cell at row `off` of `chunk`; *na: the cell is NA or NaN.
-__device__ __forceinline__ uint64_t fs_word(const FsKey& k, const char* chunk, int64_t off, bool* na) {
-    const char* p = chunk + k.coff;
-    bool isna = k.voff >= 0 && chunk[k.voff + off] == 0;
-    uint64_t w;
-    int bits;
-    if (k.ct == CT_FLOAT64) {
-        const double d = ((const double*)p)[off];
-        isna = isna || isnan(d);
-        w = (uint64_t)canon_float_ordered(canon_float_key(d)) ^ TK_SIGN;
-        bits = 64;
-    } else if (k.ct == CT_FLOAT32) {
-        const float f = ((const float*)p)[off];
-        isna = isna || isnan(f);
-        const uint32_t b = f == 0.0f ? 0u : __float_as_uint(f);
-        w = b ^ ((b >> 31) ? 0xFFFFFFFFu : 0x80000000u);
-        bits = 32;
-    } else {
-        const int sz = ctype_size(k.ct);
-        switch (sz) {
-            case 8: w = ((const uint64_t*)p)[off]; break;
-            case 4: w = ((const uint32_t*)p)[off]; break;
-            case 2: w = ((const uint16_t*)p)[off]; break;
-            default: w = ((const uint8_t*)p)[off]; break;
-        }
-        bits = 8 * sz;
-        if (tk_signed(k.ct)) w ^= 1ull << (bits - 1);
-    }
-    if (k.desc) w = ~w & (bits == 64 ? ~0ull : (1ull << bits) - 1);
-    *na = isna;
-    return isna ? 0 : w;
+// Radix word of the key cell at row `off` of `chunk`, the key's values at byte offset coff and its validity bytes at voff;
+// na: the cell is NA or NaN.
+__device__ __forceinline__ uint64_t fs_word(const SortKey& k, int64_t coff, int64_t voff, const char* chunk, int64_t off, bool& na) {
+    na = voff >= 0 && chunk[voff + off] == 0;
+    return sort_word(k, load_bits(chunk + coff, k.size, off), na);
 }
 
 template <typename W>
@@ -345,16 +331,16 @@ struct FsAppendArgs {
     int64_t src0, n, dst0;  // batch rows [src0, src0 + n) go to rows [dst0, dst0 + n) of `chunk`
     FsLayout lay;
     char* chunk;
-    const void* in_data[TK_MAX_COLS];
-    const uint8_t* in_valid[TK_MAX_COLS];
+    const void* in_data[SORT_MAX_COLS];
+    const uint8_t* in_valid[SORT_MAX_COLS];
 };
 
 __global__ void __launch_bounds__(256) fsort_append_kernel(const __grid_constant__ FsAppendArgs a) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += stride) {
         const int64_t s = a.src0 + i, o = a.dst0 + i;
-        for (int c = 0; c < a.lay.n_cols; c++) {
-            tk_copy_cell(a.in_data[c], s, a.chunk + a.lay.coff[c], o, ctype_size(a.lay.ctype[c]));
+        for (int c = 0; c < a.lay.sc.n_cols; c++) {
+            copy_cell(a.chunk + a.lay.coff[c], o, a.in_data[c], s, ctype_size(a.lay.sc.ctype[c]));
             if (a.lay.voff[c] >= 0) a.chunk[a.lay.voff[c] + o] = bit_valid(a.in_valid[c], s) ? 1 : 0;
         }
     }
@@ -362,8 +348,7 @@ __global__ void __launch_bounds__(256) fsort_append_kernel(const __grid_constant
 
 struct FsHistArgs {
     int64_t n;
-    int n_keys;
-    FsKey key[TK_MAX_KEYS];
+    FsLayout lay;
     uint32_t* hist;  // FS_HIST_WORDS
     FsChunks ch;
 };
@@ -371,11 +356,12 @@ struct FsHistArgs {
 // Block-private histograms of every (key, byte) digit, merged into `hist` once per block.  Equal digits within a warp are
 // counted by one shared atomic (match.any), so a constant byte costs one atomic per warp, not 32.
 __global__ void __launch_bounds__(FS_THREADS) fsort_hist_kernel(const __grid_constant__ FsHistArgs a) {
-    __shared__ uint32_t h[TK_MAX_KEYS * 8 * 256];
-    __shared__ uint32_t s_na[TK_MAX_KEYS];
+    __shared__ uint32_t h[SORT_MAX_KEYS * 8 * 256];
+    __shared__ uint32_t s_na[SORT_MAX_KEYS];
     const int lane = threadIdx.x & 31;
-    for (int i = threadIdx.x; i < a.n_keys * 8 * 256; i += FS_THREADS) h[i] = 0;
-    if (threadIdx.x < TK_MAX_KEYS) s_na[threadIdx.x] = 0;
+    const int nk = a.lay.sc.n_keys;
+    for (int i = threadIdx.x; i < nk * 8 * 256; i += FS_THREADS) h[i] = 0;
+    if (threadIdx.x < SORT_MAX_KEYS) s_na[threadIdx.x] = 0;
     __syncthreads();
     const int64_t stride = (int64_t)gridDim.x * FS_THREADS;
     for (int64_t r0 = (int64_t)blockIdx.x * FS_THREADS; r0 < a.n; r0 += stride) {
@@ -385,12 +371,12 @@ __global__ void __launch_bounds__(FS_THREADS) fsort_hist_kernel(const __grid_con
         const char* chunk = a.ch.p[r >> FS_CHUNK_LOG];
         const int64_t off = r & (FS_CHUNK - 1);
         const int leader = __ffs(act) - 1;
-        for (int j = 0; j < a.n_keys; j++) {
+        for (int j = 0; j < nk; j++) {
             bool na;
-            const uint64_t w = fs_word(a.key[j], chunk, off, &na);
+            const uint64_t w = fs_word(a.lay.sc.key[j], a.lay.coff[j], a.lay.voff[j], chunk, off, na);
             const unsigned nam = __ballot_sync(act, na);
             if (lane == leader && nam) atomicAdd(&s_na[j], (uint32_t)__popc(nam));
-            const int nb = ctype_size(a.key[j].ct);
+            const int nb = a.lay.sc.key[j].size;
             for (int b = 0; b < nb; b++) {
                 const uint32_t d = (uint32_t)(w >> (8 * b)) & 0xFFu;
                 const unsigned peers = __match_any_sync(act, d);
@@ -399,16 +385,17 @@ __global__ void __launch_bounds__(FS_THREADS) fsort_hist_kernel(const __grid_con
         }
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < a.n_keys * 8 * 256; i += FS_THREADS)
+    for (int i = threadIdx.x; i < nk * 8 * 256; i += FS_THREADS)
         if (h[i]) atomicAdd(&a.hist[i], h[i]);
-    if (threadIdx.x < a.n_keys && s_na[threadIdx.x]) atomicAdd(&a.hist[TK_MAX_KEYS * 8 * 256 + threadIdx.x], s_na[threadIdx.x]);
+    if (threadIdx.x < nk && s_na[threadIdx.x]) atomicAdd(&a.hist[SORT_MAX_KEYS * 8 * 256 + threadIdx.x], s_na[threadIdx.x]);
 }
 
 struct FsPassArgs {
     int64_t n;
     int shift;       // digit = (word >> shift) & 255; -1: the NA-class bit (bit 31 of the row id)
     uint32_t epoch;  // this pass's tag in the look-back words (1, 2, ...; the words start at 0)
-    FsKey key;       // FS_IN_COLUMN / FS_IN_GATHER: the column the words are computed from
+    SortKey key;     // FS_IN_COLUMN / FS_IN_GATHER: the column the words are computed from, at chunk offsets coff / voff
+    int64_t coff, voff;
     const void* w_in;
     const uint32_t* id_in;
     void* w_out;
@@ -455,8 +442,8 @@ __global__ void __launch_bounds__(FS_THREADS) fsort_pass_kernel(const __grid_con
             } else {
                 const uint32_t r = MODE == FS_IN_COLUMN ? (uint32_t)i : (a.id_in[i] & FS_ID_MASK);
                 bool na;
-                w[k] = (W)fs_word(a.key, a.ch.p[r >> FS_CHUNK_LOG], r & (FS_CHUNK - 1), &na);
-                id[k] = r | ((uint32_t)(na ? a.key.na_last : !a.key.na_last) << 31);
+                w[k] = (W)fs_word(a.key, a.coff, a.voff, a.ch.p[r >> FS_CHUNK_LOG], r & (FS_CHUNK - 1), na);
+                id[k] = r | (sort_class(a.key, na) << 31);
             }
             d = fs_digit(w[k], id[k], a.shift);
         }
@@ -531,8 +518,8 @@ struct FsGatherArgs {
     int64_t n;
     const uint32_t* ids;  // the permutation (bit 31 ignored); nullptr: identity
     FsLayout lay;
-    void* out[TK_MAX_COLS];
-    uint8_t* out_vb[TK_MAX_COLS];
+    void* out[SORT_MAX_COLS];
+    uint8_t* out_vb[SORT_MAX_COLS];
     FsChunks ch;
 };
 
@@ -542,8 +529,8 @@ __global__ void __launch_bounds__(256) fsort_gather_kernel(const __grid_constant
         const uint32_t r = a.ids ? (a.ids[i] & FS_ID_MASK) : (uint32_t)i;
         const char* chunk = a.ch.p[r >> FS_CHUNK_LOG];
         const int64_t off = r & (FS_CHUNK - 1);
-        for (int c = 0; c < a.lay.n_cols; c++) {
-            tk_copy_cell(chunk + a.lay.coff[c], off, a.out[c], i, ctype_size(a.lay.ctype[c]));
+        for (int c = 0; c < a.lay.sc.n_cols; c++) {
+            copy_cell(a.out[c], i, chunk + a.lay.coff[c], off, ctype_size(a.lay.sc.ctype[c]));
             if (a.lay.voff[c] >= 0) a.out_vb[c][i] = (uint8_t)chunk[a.lay.voff[c] + off];
         }
     }
@@ -559,72 +546,128 @@ void launch_fsort_pass(int mode, int64_t n_tiles, const FsPassArgs& a, cudaStrea
     else fsort_pass_kernel<W, FS_IN_GATHER><<<g, FS_THREADS, 0, st>>>(a);
 }
 
+// ---- host state: a form consumes rows and at is_last points the output views at its sorted rows; the base checks batches,
+// packs the output's validity bitmaps and hands out output batches ----
 struct SortState {
-    int device;
+    int device, sms;
     cudaStream_t stream;
-    TkSchema sc{};
-    int arr_type[TK_MAX_COLS];
-    int64_t limit, offset, K, cap, output_batch_size;
-    // two store buffers (cur = the one the filter appends to) and their memory
-    std::vector<DevBuf> mem[2];
-    TkStore store[2]{};
-    int cur = 0;
-    DevBuf perm[2], d_cursor, d_cutoff, d_bitmaps;
-    std::vector<uint32_t*> out_bitmap;
-    unsigned long long* h_count = nullptr;
-    int64_t held = 0;         // sorted rows at the front of the current store (<= K)
-    int64_t count_bound = 0;  // upper bound on the store count: last count read + rows launched since
-    bool has_cutoff = false, finished = false;
+    SortSchema sc{};
+    int arr_type[SORT_MAX_COLS];
+    int64_t output_batch_size;
+    int64_t rows_consumed = 0;  // metric 0
+    bool finished = false;
+    // output views, set by the form's finish_rows: rows [0, n_out) of column c at out_data[c], for a nullable column one validity
+    // byte per row at out_vb[c]
+    char* out_data[SORT_MAX_COLS]{};
+    uint8_t* out_vb[SORT_MAX_COLS]{};
     int64_t n_out = 0, out_cursor = 0;
-    // metrics
-    int64_t rows_consumed = 0, rows_admitted = 0, admitted_after_cutoff = 0, reduce_steps = 0, count_reads = 0, filter_launches = 0;
-    // full sort (no limit): the chunk store, the output store and its validity bytes
-    bool full = false;
-    FsLayout lay{};
-    int64_t chunk_bytes = 0, n_chunks = 0, passes_run = 0, passes_skipped = 0;
-    std::vector<DevBuf> chunks, out_mem;
+    DevBuf d_bitmaps;
+    std::vector<uint32_t*> out_bitmap;
 
-    SortState(bool full_, int64_t limit_, int64_t offset_, const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_keys,
-              const int32_t* asc, const int32_t* na_last, int64_t obs, int dev, cudaStream_t st)
-        : device(dev), stream(st), limit(limit_), offset(offset_), output_batch_size(obs), full(full_) {
-        if (!full) {
-            B200_REQUIRE(limit >= 0 && offset >= 0, "b200 sort: limit and offset must be non-negative");
-            B200_REQUIRE(limit <= TK_MAX_K && offset <= TK_MAX_K - limit, "b200 sort: limit + offset exceeds the top-k cap of 2^26 rows");
-        }
-        B200_REQUIRE(n_keys >= 1 && n_keys <= TK_MAX_KEYS, "b200 sort: 1 to 4 sort keys");
-        B200_REQUIRE(n_arrs >= n_keys && n_arrs <= TK_MAX_COLS, "b200 sort: keys are the first n_keys of at most 32 columns");
+    SortState(const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_keys, const int32_t* asc, const int32_t* na_last,
+              int64_t obs, int dev, cudaStream_t st)
+        : device(dev), stream(st), output_batch_size(obs) {
+        B200_REQUIRE(n_keys >= 1 && n_keys <= SORT_MAX_KEYS, "b200 sort: 1 to 4 sort keys");
+        B200_REQUIRE(n_arrs >= n_keys && n_arrs <= SORT_MAX_COLS, "b200 sort: keys are the first n_keys of at most 32 columns");
         B200_REQUIRE(c_types && arr_types && asc && na_last, "b200 sort: null argument");
-        K = limit + offset;
         sc.n_keys = n_keys; sc.n_cols = n_arrs;
         for (int c = 0; c < n_arrs; c++) {
             B200_REQUIRE(ctype_size(c_types[c]) > 0, "b200 sort: unsupported column dtype (fixed-width numeric, bool and temporal columns only)");
             B200_REQUIRE(arr_types[c] == ARR_NUMPY || arr_types[c] == ARR_NULLABLE, "b200 sort: unsupported array type");
             sc.ctype[c] = c_types[c]; arr_type[c] = arr_types[c];
         }
-        for (int j = 0; j < n_keys; j++) {
-            if (!asc[j]) sc.desc_mask |= 1u << j;
-            if (na_last[j]) sc.na_last_mask |= 1u << j;
-        }
+        for (int j = 0; j < n_keys; j++) sc.key[j] = SortKey{sc.ctype[j], ctype_size(sc.ctype[j]), asc[j] ? 0 : 1, na_last[j] ? 1 : 0};
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
+        sms = num_sms(device);
+    }
+    // The caller selects the state's device and stream first (b200_delete_sort_state): both forms' buffers go back to its pool.
+    virtual ~SortState() = default;
+
+    // Rows [0, n) of a checked batch, arriving with indices rows_consumed, rows_consumed + 1, ...
+    virtual void consume_rows(const b200_table* t, int64_t n) = 0;
+    // At is_last: sort, then set n_out, out_data and out_vb.  Validity bytes the form allocates for its output go in vbytes (one
+    // slot per column), which is freed once the bitmaps are packed.
+    virtual void finish_rows(std::vector<DevBuf>& vbytes) = 0;
+    // Metric 0 to 8; a metric the form does not keep reads 0.
+    virtual int64_t metric(int which) const = 0;
+
+    int grid_for(int64_t items, int per_block) const { return (int)std::max<int64_t>(1, std::min<int64_t>((items + per_block - 1) / per_block, (int64_t)sms * 8)); }
+
+    void consume(const b200_table* t) {
+        B200_REQUIRE(!finished, "b200 sort: batch consumed after is_last");
+        B200_REQUIRE(t->n_cols == sc.n_cols, "b200 sort: the batch's column count differs from the state's schema");
+        for (int c = 0; c < sc.n_cols; c++)
+            B200_REQUIRE(t->cols[c].c_type == sc.ctype[c] && t->cols[c].arr_type == arr_type[c],
+                         "b200 sort: a batch's column types differ from the state's schema");
+        const int64_t n = t->n_rows;
+        if (n > 0) B200_REQUIRE(t->device == device, "b200 sort: batches must be resident on the state's device (stage host batches first)");
+        B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
+        consume_rows(t, n);
+        rows_consumed += n;
+    }
+
+    void finish() {
+        B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
+        std::vector<DevBuf> vbytes(sc.n_cols);
+        finish_rows(vbytes);
+        finished = true;
+        int n_nullable = 0;
+        for (int c = 0; c < sc.n_cols; c++) n_nullable += arr_type[c] == ARR_NULLABLE;
+        const int64_t words = (n_out + 31) / 32 + 2;
+        d_bitmaps.alloc((size_t)std::max(1, n_nullable) * words * 4);
+        B200_CUDA(cudaMemsetAsync(d_bitmaps.p, 0, d_bitmaps.bytes, stream));
+        out_bitmap.assign(sc.n_cols, nullptr);
+        for (int c = 0, k = 0; c < sc.n_cols; c++) {
+            if (arr_type[c] != ARR_NULLABLE) continue;
+            out_bitmap[c] = d_bitmaps.as<uint32_t>() + (k++) * words;
+            if (n_out > 0) launch_pack_bitmap(out_vb[c], n_out, out_bitmap[c], grid_for(n_out, 256), stream);
+        }
+        B200_CUDA(cudaGetLastError());
+        vbytes.clear();
+        B200_CUDA(cudaStreamSynchronize(stream));
+    }
+
+    int produce(b200_table* out, int32_t* out_is_last, bool produce_output) {
+        B200_REQUIRE(finished, "b200 sort: output requested before the last batch was consumed");
+        B200_REQUIRE(out->cols != nullptr, "b200 sort: out->cols must point to one descriptor per column");
+        int64_t bs = output_batch_size > 0 ? output_batch_size : n_out;
+        if (bs % 32 != 0 && bs < n_out) bs = (bs + 31) & ~31ll;  // validity bitmaps are sliced at word granularity
+        const int64_t rows = produce_output ? std::min(bs, n_out - out_cursor) : 0;
+        out->n_rows = rows; out->n_cols = sc.n_cols; out->device = device;
+        for (int c = 0; c < sc.n_cols; c++) {
+            b200_column& col = out->cols[c];
+            col.data = out_data[c] + out_cursor * ctype_size(sc.ctype[c]);
+            col.validity = out_bitmap[c] ? (uint8_t*)out_bitmap[c] + out_cursor / 8 : nullptr;
+            col.length = rows; col.c_type = sc.ctype[c]; col.arr_type = arr_type[c];
+        }
+        out_cursor += rows;
+        *out_is_last = out_cursor >= n_out ? 1 : 0;
+        return 0;
+    }
+};
+
+// ORDER BY ... LIMIT limit OFFSET offset.
+struct TopkState : SortState {
+    int64_t offset, K, cap;
+    // two store buffers (cur = the one the filter appends to) and their memory
+    std::vector<DevBuf> mem[2];
+    TkStore store[2]{};
+    int cur = 0;
+    DevBuf perm[2], d_cursor, d_cutoff;
+    unsigned long long* h_count = nullptr;
+    int64_t held = 0;         // sorted rows at the front of the current store (<= K)
+    int64_t count_bound = 0;  // upper bound on the store count: last count read + rows launched since
+    bool has_cutoff = false;
+    int64_t rows_admitted = 0, admitted_after_cutoff = 0, reduce_steps = 0, count_reads = 0, filter_launches = 0;
+
+    TopkState(int64_t limit, int64_t offset_, const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_keys,
+              const int32_t* asc, const int32_t* na_last, int64_t obs, int dev, cudaStream_t st)
+        : SortState(c_types, arr_types, n_arrs, n_keys, asc, na_last, obs, dev, st), offset(offset_), K(limit + offset_),
+          cap(std::max<int64_t>(2 * K, TK_MIN_CAP)) {
         h_count = (unsigned long long*)pinned_acquire(8);
         d_cursor.alloc(8); d_cutoff.alloc(sizeof(TkCutoff));
         B200_CUDA(cudaMemsetAsync(d_cursor.p, 0, 8, stream));
         B200_CUDA(cudaMemsetAsync(d_cutoff.p, 0, sizeof(TkCutoff), stream));
-        if (full) {
-            cap = 0;
-            lay.n_cols = n_arrs;
-            for (int c = 0; c < n_arrs; c++) {
-                lay.ctype[c] = sc.ctype[c];
-                lay.coff[c] = chunk_bytes;
-                chunk_bytes += FS_CHUNK * ctype_size(sc.ctype[c]);
-            }
-            for (int c = 0; c < n_arrs; c++) {
-                lay.voff[c] = arr_type[c] == ARR_NULLABLE ? chunk_bytes : -1;
-                if (arr_type[c] == ARR_NULLABLE) chunk_bytes += FS_CHUNK;
-            }
-            return;
-        }
-        cap = std::max<int64_t>(2 * K, TK_MIN_CAP);
         if (K == 0) return;  // nothing is ever kept: no store
         for (int b = 0; b < 2; b++) {
             auto take = [&](size_t bytes) { mem[b].emplace_back(); mem[b].back().alloc(bytes); return mem[b].back().p; };
@@ -639,12 +682,7 @@ struct SortState {
             perm[b].alloc(cap * 4);
         }
     }
-    ~SortState() {
-        cudaSetDevice(device); scratch_set_stream(stream);
-        pinned_release(h_count, 8);
-    }
-
-    int grid_for(int64_t items, int per_block) const { return (int)std::max<int64_t>(1, std::min<int64_t>((items + per_block - 1) / per_block, (int64_t)num_sms(device) * 8)); }
+    ~TopkState() override { pinned_release(h_count, 8); }
 
     int64_t read_count() {
         B200_CUDA(cudaMemcpyAsync(h_count, d_cursor.p, 8, cudaMemcpyDeviceToHost, stream));
@@ -685,23 +723,11 @@ struct SortState {
         if (held == K) has_cutoff = true;
     }
 
-    void consume(const b200_table* t) {
-        B200_REQUIRE(!finished, "b200 sort: batch consumed after is_last");
-        B200_REQUIRE(t->n_cols == sc.n_cols, "b200 sort: the batch's column count differs from the state's schema");
-        for (int c = 0; c < sc.n_cols; c++)
-            B200_REQUIRE(t->cols[c].c_type == sc.ctype[c] && t->cols[c].arr_type == arr_type[c],
-                         "b200 sort: a batch's column types differ from the state's schema");
-        const int64_t n = t->n_rows;
-        if (n > 0) B200_REQUIRE(t->device == device, "b200 sort: batches must be resident on the state's device (stage host batches first)");
-        if (full) B200_REQUIRE(n <= FS_MAX_ROWS - rows_consumed, "b200 sort: a full sort holds at most 2^31 rows (32-bit row ids)");
-        B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
-        const int64_t seq_base = rows_consumed;
-        rows_consumed += n;
-        if (full) return append(t, seq_base, n);
+    void consume_rows(const b200_table* t, int64_t n) override {
         if (K == 0 || n == 0) return;
         TkFilterArgs a{};
         a.sc = sc;
-        a.seq_base = seq_base;
+        a.seq_base = rows_consumed;
         for (int c = 0; c < sc.n_cols; c++) { a.in_data[c] = t->cols[c].data; a.in_valid[c] = t->cols[c].validity; }
         a.cutoff = d_cutoff.as<TkCutoff>();
         a.cursor = d_cursor.as<unsigned long long>();
@@ -723,13 +749,51 @@ struct SortState {
         }
     }
 
-    // Full sort: rows [0, n) of the batch go to rows [g0, g0 + n) of the chunk store.
-    void append(const b200_table* t, int64_t g0, int64_t n) {
+    void finish_rows(std::vector<DevBuf>&) override {
+        if (K > 0) reduce();
+        n_out = std::max<int64_t>(0, held - offset);
+        const TkStore& s = store[cur];
+        for (int c = 0; c < sc.n_cols; c++) {
+            // K = 0 has no store: its zero output rows still carry a non-null data pointer
+            out_data[c] = K == 0 ? d_cutoff.as<char>() : (char*)s.data[c] + offset * ctype_size(sc.ctype[c]);
+            out_vb[c] = s.vb[c] ? s.vb[c] + offset : nullptr;
+        }
+    }
+
+    int64_t metric(int which) const override {
+        const int64_t m[9] = {rows_consumed, rows_admitted, reduce_steps, count_reads, filter_launches, admitted_after_cutoff, cap, 0, 0};
+        return m[which];
+    }
+};
+
+// ORDER BY without LIMIT.
+struct FullSortState : SortState {
+    FsLayout lay{};
+    int64_t chunk_bytes = 0, n_chunks = 0, passes_run = 0, passes_skipped = 0;
+    std::vector<DevBuf> chunks, out_mem;
+
+    FullSortState(const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_keys, const int32_t* asc, const int32_t* na_last,
+                  int64_t obs, int dev, cudaStream_t st)
+        : SortState(c_types, arr_types, n_arrs, n_keys, asc, na_last, obs, dev, st) {
+        lay.sc = sc;
+        for (int c = 0; c < n_arrs; c++) {
+            lay.coff[c] = chunk_bytes;
+            chunk_bytes += FS_CHUNK * ctype_size(sc.ctype[c]);
+        }
+        for (int c = 0; c < n_arrs; c++) {
+            lay.voff[c] = arr_type[c] == ARR_NULLABLE ? chunk_bytes : -1;
+            if (arr_type[c] == ARR_NULLABLE) chunk_bytes += FS_CHUNK;
+        }
+    }
+
+    // Rows [0, n) of the batch go to rows [rows_consumed, rows_consumed + n) of the chunk store.
+    void consume_rows(const b200_table* t, int64_t n) override {
+        B200_REQUIRE(n <= FS_MAX_ROWS - rows_consumed, "b200 sort: a full sort holds at most 2^31 rows (32-bit row ids)");
         FsAppendArgs a{};
         a.lay = lay;
         for (int c = 0; c < sc.n_cols; c++) { a.in_data[c] = t->cols[c].data; a.in_valid[c] = t->cols[c].validity; }
         for (int64_t i = 0; i < n;) {
-            const int64_t g = g0 + i, k = g >> FS_CHUNK_LOG, off = g & (FS_CHUNK - 1);
+            const int64_t g = rows_consumed + i, k = g >> FS_CHUNK_LOG, off = g & (FS_CHUNK - 1);
             const int64_t r = std::min(n - i, FS_CHUNK - off);
             if (k == (int64_t)chunks.size()) {
                 chunks.emplace_back();
@@ -743,16 +807,13 @@ struct SortState {
         }
     }
 
-    // Full sort at is_last: digit histograms, the pass plan, the digit passes and the gather into the output store (out_mem);
-    // the validity bytes of nullable column c go to out_vb[c].  Pair buffers and look-back words are freed on return.
-    void sort_full(std::vector<DevBuf>& out_vb) {
+    // Digit histograms, the pass plan, the digit passes and the gather into the output store (out_mem; the validity bytes of
+    // nullable column c go to vbytes[c]).  Chunks, pair buffers and look-back words are freed on return.
+    void finish_rows(std::vector<DevBuf>& vbytes) override {
         const int64_t n = rows_consumed;
         const int nk = sc.n_keys;
         FsChunks ch{};
         for (size_t k = 0; k < chunks.size(); k++) ch.p[k] = chunks[k].as<char>();
-        FsKey key[TK_MAX_KEYS]{};
-        for (int j = 0; j < nk; j++)
-            key[j] = FsKey{sc.ctype[j], (int)((sc.desc_mask >> j) & 1), (int)((sc.na_last_mask >> j) & 1), lay.coff[j], lay.voff[j]};
         DevBuf wbuf[2], ibuf[2], status, counters;
         const uint32_t* ids = nullptr;  // the permutation so far; nullptr: identity
         if (n > 0) {
@@ -760,8 +821,7 @@ struct SortState {
             d_hist.alloc(FS_HIST_WORDS * 4);
             B200_CUDA(cudaMemsetAsync(d_hist.p, 0, FS_HIST_WORDS * 4, stream));
             FsHistArgs ha{};
-            ha.n = n; ha.n_keys = nk; ha.hist = d_hist.as<uint32_t>(); ha.ch = ch;
-            for (int j = 0; j < nk; j++) ha.key[j] = key[j];
+            ha.n = n; ha.lay = lay; ha.hist = d_hist.as<uint32_t>(); ha.ch = ch;
             fsort_hist_kernel<<<grid_for(n, FS_THREADS), FS_THREADS, 0, stream>>>(ha);
             B200_CUDA(cudaGetLastError());
             auto* h = (uint32_t*)pinned_acquire(FS_HIST_WORDS * 4);
@@ -780,9 +840,9 @@ struct SortState {
                     plan.push_back(p);
                 }
                 if (arr_type[j] == ARR_NULLABLE || ctype_is_float(sc.ctype[j])) {
-                    const int64_t na = h[TK_MAX_KEYS * 8 * 256 + j];
+                    const int64_t na = h[SORT_MAX_KEYS * 8 * 256 + j];
                     if (na == 0 || na == n) { passes_skipped++; continue; }
-                    const int64_t class0 = key[j].na_last ? n - na : na;  // rows whose class bit is 0
+                    const int64_t class0 = sc.key[j].na_last ? n - na : na;  // rows whose class bit is 0
                     Pass p{j, -1, {}};
                     for (int d = 1; d < 256; d++) p.base[d] = (uint32_t)class0;
                     plan.push_back(p);
@@ -805,7 +865,8 @@ struct SortState {
                     const int mode = p.key == prev_key ? FS_IN_PAIRS : ids ? FS_IN_GATHER : FS_IN_COLUMN;
                     const int ob = cur_buf == 0 ? 1 : 0;
                     FsPassArgs a{};
-                    a.n = n; a.shift = p.shift; a.epoch = (uint32_t)q + 1; a.key = key[p.key];
+                    a.n = n; a.shift = p.shift; a.epoch = (uint32_t)q + 1;
+                    a.key = sc.key[p.key]; a.coff = lay.coff[p.key]; a.voff = lay.voff[p.key];
                     a.w_in = cur_buf >= 0 ? wbuf[cur_buf].p : nullptr; a.id_in = ids;
                     a.w_out = wbuf[ob].p; a.id_out = ibuf[ob].as<uint32_t>();
                     a.status = status.as<unsigned long long>(); a.tile_counter = counters.as<unsigned int>() + q;
@@ -823,58 +884,32 @@ struct SortState {
         out_mem.resize(sc.n_cols);
         for (int c = 0; c < sc.n_cols; c++) {
             out_mem[c].alloc((size_t)n * ctype_size(sc.ctype[c]));
-            ga.out[c] = out_mem[c].p;
-            if (arr_type[c] == ARR_NULLABLE) { out_vb[c].alloc((size_t)n); ga.out_vb[c] = out_vb[c].as<uint8_t>(); }
+            ga.out[c] = out_data[c] = out_mem[c].as<char>();
+            if (arr_type[c] == ARR_NULLABLE) { vbytes[c].alloc((size_t)n); ga.out_vb[c] = out_vb[c] = vbytes[c].as<uint8_t>(); }
         }
         if (n > 0) fsort_gather_kernel<<<grid_for(n, 256), 256, 0, stream>>>(ga);
         B200_CUDA(cudaGetLastError());
+        n_out = n;
+        chunks.clear();  // the rows now live in the output store
     }
 
-    void finish() {
-        B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
-        std::vector<DevBuf> out_vb(sc.n_cols);  // full sort: the output's validity bytes, until they are packed
-        if (full) sort_full(out_vb);
-        else if (K > 0) reduce();
-        finished = true;
-        n_out = full ? rows_consumed : std::max<int64_t>(0, held - offset);
-        auto vb_of = [&](int c) { return full ? out_vb[c].as<uint8_t>() : store[cur].vb[c] + offset; };
-        int n_nullable = 0;
-        for (int c = 0; c < sc.n_cols; c++) n_nullable += arr_type[c] == ARR_NULLABLE;
-        const int64_t words = (n_out + 31) / 32 + 2;
-        d_bitmaps.alloc((size_t)std::max(1, n_nullable) * words * 4);
-        B200_CUDA(cudaMemsetAsync(d_bitmaps.p, 0, d_bitmaps.bytes, stream));
-        out_bitmap.assign(sc.n_cols, nullptr);
-        for (int c = 0, k = 0; c < sc.n_cols; c++) {
-            if (arr_type[c] != ARR_NULLABLE) continue;
-            out_bitmap[c] = d_bitmaps.as<uint32_t>() + (k++) * words;
-            if (n_out > 0) launch_pack_bitmap(vb_of(c), n_out, out_bitmap[c], grid_for(n_out, 256), stream);
-        }
-        B200_CUDA(cudaGetLastError());
-        chunks.clear();  // full sort: the rows now live in the output store
-        out_vb.clear();
-        B200_CUDA(cudaStreamSynchronize(stream));
-    }
-
-    int produce(b200_table* out, int32_t* out_is_last, bool produce_output) {
-        B200_REQUIRE(finished, "b200 sort: output requested before the last batch was consumed");
-        B200_REQUIRE(out->cols != nullptr, "b200 sort: out->cols must point to one descriptor per column");
-        int64_t bs = output_batch_size > 0 ? output_batch_size : n_out;
-        if (bs % 32 != 0 && bs < n_out) bs = (bs + 31) & ~31ll;  // validity bitmaps are sliced at word granularity
-        const int64_t rows = produce_output ? std::min(bs, n_out - out_cursor) : 0;
-        out->n_rows = rows; out->n_cols = sc.n_cols; out->device = device;
-        const int64_t base = full ? out_cursor : offset + out_cursor;
-        for (int c = 0; c < sc.n_cols; c++) {
-            b200_column& col = out->cols[c];
-            if (full) col.data = out_mem[c].as<char>() + base * ctype_size(sc.ctype[c]);
-            else col.data = K == 0 ? d_cutoff.p : (char*)store[cur].data[c] + base * ctype_size(sc.ctype[c]);
-            col.validity = out_bitmap[c] ? (uint8_t*)out_bitmap[c] + out_cursor / 8 : nullptr;
-            col.length = rows; col.c_type = sc.ctype[c]; col.arr_type = arr_type[c];
-        }
-        out_cursor += rows;
-        *out_is_last = out_cursor >= n_out ? 1 : 0;
-        return 0;
+    int64_t metric(int which) const override {
+        const int64_t m[9] = {rows_consumed, 0, 0, 0, 0, 0, n_chunks * FS_CHUNK, passes_run, passes_skipped};
+        return m[which];
     }
 };
+
+// A new state from make() once the device is known to exist; nullptr and the last error on failure.
+template <typename Make>
+static void* sort_state_new(int32_t device, Make make) {
+    try {
+        int ndev = 0;
+        if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+            throw Error("b200 sort: no CUDA device available (this path has no CPU fallback)");
+        B200_REQUIRE(device >= 0 && device < ndev, "b200 sort: bad device ordinal");
+        return make();
+    } catch (const std::exception& e) { set_last_error(e.what()); return nullptr; }
+}
 
 }  // namespace b200
 
@@ -882,30 +917,25 @@ using b200::SortState;
 
 extern "C" {
 
-static void* sort_state_new(bool full, int64_t limit, int64_t offset, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                            int32_t n_keys, const int32_t* ascending, const int32_t* na_last, int64_t output_batch_size, int32_t device,
-                            void* stream) {
-    try {
-        int ndev = 0;
-        if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-            throw b200::Error("b200 sort: no CUDA device available (this path has no CPU fallback)");
-        B200_REQUIRE(device >= 0 && device < ndev, "b200 sort: bad device ordinal");
-        return new SortState(full, limit, offset, c_types, arr_types, n_arrs, n_keys, ascending, na_last, output_batch_size, device,
-                             (cudaStream_t)stream);
-    } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
-}
-
 void* b200_sort_state_init(int64_t operator_id, int64_t limit, int64_t offset, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
                            int32_t n_keys, const int32_t* ascending, const int32_t* na_last, int64_t output_batch_size, int32_t device,
                            void* stream) {
     (void)operator_id;
-    return sort_state_new(false, limit, offset, c_types, arr_types, n_arrs, n_keys, ascending, na_last, output_batch_size, device, stream);
+    return b200::sort_state_new(device, [&]() -> SortState* {
+        B200_REQUIRE(limit >= 0 && offset >= 0, "b200 sort: limit and offset must be non-negative");
+        B200_REQUIRE(limit <= b200::TK_MAX_K && offset <= b200::TK_MAX_K - limit, "b200 sort: limit + offset exceeds the top-k cap of 2^26 rows");
+        return new b200::TopkState(limit, offset, c_types, arr_types, n_arrs, n_keys, ascending, na_last, output_batch_size, device,
+                                   (cudaStream_t)stream);
+    });
 }
 
 void* b200_sort_state_init_full(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs, int32_t n_keys,
                                 const int32_t* ascending, const int32_t* na_last, int64_t output_batch_size, int32_t device, void* stream) {
     (void)operator_id;
-    return sort_state_new(true, 0, 0, c_types, arr_types, n_arrs, n_keys, ascending, na_last, output_batch_size, device, stream);
+    return b200::sort_state_new(device, [&]() -> SortState* {
+        return new b200::FullSortState(c_types, arr_types, n_arrs, n_keys, ascending, na_last, output_batch_size, device,
+                                       (cudaStream_t)stream);
+    });
 }
 
 int b200_sort_build_consume_batch(void* state, const b200_table* in_table, int32_t is_last, int32_t* request_input) {
@@ -926,22 +956,14 @@ int b200_sort_produce_output_batch(void* state, b200_table* out, int32_t* out_is
     } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
 }
 
-void b200_delete_sort_state(void* state) { delete (SortState*)state; }
+void b200_delete_sort_state(void* state) {
+    auto* s = (SortState*)state;
+    if (s) { cudaSetDevice(s->device); b200::scratch_set_stream(s->stream); }  // the form's buffers go back to this pool
+    delete s;
+}
 
 int64_t b200_sort_get_metric(void* state, int32_t which) {
-    auto* s = (SortState*)state;
-    switch (which) {
-        case 0: return s->rows_consumed;
-        case 1: return s->rows_admitted;
-        case 2: return s->reduce_steps;
-        case 3: return s->count_reads;
-        case 4: return s->filter_launches;
-        case 5: return s->admitted_after_cutoff;
-        case 6: return s->full ? s->n_chunks * b200::FS_CHUNK : s->cap;
-        case 7: return s->passes_run;
-        case 8: return s->passes_skipped;
-        default: return -1;
-    }
+    return which >= 0 && which <= 8 ? ((SortState*)state)->metric(which) : -1;
 }
 
 }  // extern "C"
