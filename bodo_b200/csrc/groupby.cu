@@ -66,7 +66,8 @@ enum CounterSlot : int {
     CTR_RETRY1 = 6,         // rows in the slot-1 retry list (SPG)
     CTR_XCHG_OVERFLOW = 7,  // fused exchange: some rank's share overflowed its slab segment, nobody combined
     CTR_RETRY_OVERFLOW = 8, // SPG / SPG-G: an entry did not fit its retry list and was dropped (the host raises an error)
-    N_COUNTERS = 9
+    CTR_DENSE_WIDE = 9,     // SPG-N dense form: rows whose key or value offset did not fit its window
+    N_COUNTERS = 10
 };
 
 struct ConsumeArgs {
@@ -1073,6 +1074,14 @@ struct SpgArgs {
     const int* n_hot;           // number of keys in hot_tab (device memory: K1 reads it, the host never waits for it)
     int reserve_tickets;  // K2n flush: the global table is empty — a CTA reserves the group tickets of all its slots with one atomic
 };
+// SPG-N dense form (spgn.cuh): key window [kbase, kbase + 2^d_kb), value offsets of d_vb bits above vbase
+struct SpgDenseArgs : SpgArgs {
+    long long kbase, vbase;
+    unsigned int d_kb, d_vb;
+    unsigned int d_mul, d_inv;  // odd multiplier of the key scramble, and its inverse mod 2^32
+    unsigned int d_gmagic;      // ceil(2^32 / n_owners): x div n_owners = umulhi(x, d_gmagic) for x < 2^21
+    int d_slots;                // K2d table slots per owner: ceil(2^d_kb / n_owners)
+};
 
 // cheap in-kernel hash for owner / shared-table slot (placement inside one GPU is free to choose; the rank
 // placement that must match the reference uses xxh3, see shuffle.cu)
@@ -1116,16 +1125,21 @@ constexpr int SPG_HOT_TAB = 8192;        // counting-table slots of the sample k
 constexpr size_t SPG_HOT_SAMPLE_SMEM = (size_t)SPG_HOT_TAB * 12 + SPG_HOT_SLOTS * 8;
 __device__ __forceinline__ unsigned int spg_hot_bucket(uint64_t h) { return (unsigned int)(h >> 8) & (SPG_HOT_BUCKETS - 1); }
 
-__global__ void __launch_bounds__(1024, 1) spg_hot_sample_kernel(const long long* keys, const long long* vals, int64_t n_rows, long long* hot_tab, int* n_hot) {
+// Also the SPG-N verdicts: n_hot[1] = sampled rows that do not fit an (int32, int32) bucket row, and range = {min key, max key,
+// min value, max value} of the sampled rows (the window of the dense form).
+__global__ void __launch_bounds__(1024, 1) spg_hot_sample_kernel(const long long* keys, const long long* vals, int64_t n_rows, long long* hot_tab, int* n_hot,
+                                                                 long long* range) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     long long* tk = (long long*)smem_raw;                  // SPG_HOT_TAB keys
     unsigned int* tc = (unsigned int*)(tk + SPG_HOT_TAB);  // their sample counts
     long long* hk = (long long*)(tc + SPG_HOT_TAB);        // SPG_HOT_SLOTS: the hot table being built
     __shared__ unsigned int fill, nh, nwide;
+    __shared__ long long rng[4];
     const int tid = threadIdx.x;
     for (int s = tid; s < SPG_HOT_TAB; s += 1024) { tk[s] = EMPTY_KEY; tc[s] = 0; }
     for (int s = tid; s < SPG_HOT_SLOTS; s += 1024) hk[s] = EMPTY_KEY;
-    if (tid == 0) { fill = 0; nh = 0; nwide = 0; }
+    if (tid == 0) { fill = 0; nh = 0; nwide = 0; rng[0] = rng[2] = LLONG_MAX; rng[1] = rng[3] = LLONG_MIN; }
+    long long kmin = LLONG_MAX, kmax = LLONG_MIN, vmin = LLONG_MAX, vmax = LLONG_MIN;
     __syncthreads();
     // the sample = 32 evenly spaced blocks of 1024 contiguous rows (one coalesced 8 KB read per block and column: a row-strided
     // sample touched a different DRAM page and TLB entry with every load and took 0.26 ms for 32 Ki rows)
@@ -1143,6 +1157,7 @@ __global__ void __launch_bounds__(1024, 1) spg_hot_sample_kernel(const long long
             if (i < S) {
                 const long long v = vals ? vals[row] : 0;
                 if (kv[u] != (long long)(int)kv[u] || (int)kv[u] == (int)0x80000000 || v != (long long)(int)v) atomicAdd(&nwide, 1u);
+                kmin = min(kmin, kv[u]); kmax = max(kmax, kv[u]); vmin = min(vmin, v); vmax = max(vmax, v);
             }
         }
 #pragma unroll
@@ -1163,7 +1178,13 @@ __global__ void __launch_bounds__(1024, 1) spg_hot_sample_kernel(const long long
             }
         }
     }
+    for (int d = 16; d; d >>= 1) {
+        kmin = min(kmin, __shfl_xor_sync(0xffffffffu, kmin, d)); kmax = max(kmax, __shfl_xor_sync(0xffffffffu, kmax, d));
+        vmin = min(vmin, __shfl_xor_sync(0xffffffffu, vmin, d)); vmax = max(vmax, __shfl_xor_sync(0xffffffffu, vmax, d));
+    }
+    if ((tid & 31) == 0) { atomicMin(&rng[0], kmin); atomicMax(&rng[1], kmax); atomicMin(&rng[2], vmin); atomicMax(&rng[3], vmax); }
     __syncthreads();
+    if (tid < 4) range[tid] = rng[tid];
     const unsigned int T = S >= (16 << 10) ? (unsigned int)(S >> 10) : 16u;  // hot = at least 1/1024 of the sample
     // admit candidates heaviest first (four count bands); a candidate whose two-slot bucket is taken stays an ordinary key
     for (int band = 3; band >= 0; band--) {
@@ -2050,12 +2071,17 @@ class GroupbyState {
             spgn_ns = ((int)(((size_t)max_smem - 256 - SPGN_QUEUE_BYTES) / 12) - SPG_STASH) & ~1;  // (K2n also has a few static shared words)
             spgn_smem = (size_t)(spgn_ns + SPG_STASH) * 12 + SPGN_QUEUE_BYTES + 16;
             spgn_enabled = true;
+            spgd_max_smem = (size_t)max_smem - 256;  // (K2d's flush has a few static shared words)
             for_each_sum_cnt([&](auto s, auto c) {
                 if (!set_smem_limit((const void*)spgn_partition_kernel<s, c>, spgn_part_smem())) spgn_enabled = false;
                 if (!set_smem_limit((const void*)spgn_aggregate_kernel<s, c>, spgn_smem)) spgn_enabled = false;
+                if (!set_smem_limit((const void*)spgn_partition_kernel<s, c, true>, spgn_part_smem())) spgd_max_smem = 0;
+                if (!set_smem_limit((const void*)spgn_aggregate_kernel<s, c, true>, spgd_max_smem)) spgd_max_smem = 0;
             });
             const char* e8 = getenv("B200_SPG_NARROW");
             if (e8 && e8[0] == '0') spgn_enabled = false;
+            const char* e9 = getenv("B200_SPG_DENSE");
+            if ((e9 && e9[0] == '0') || !spgn_enabled || sms < 2) spgd_max_smem = 0;  // (the slot division needs >= 2 owners)
         }
         {   // SPG-G (spgg.cuh): generic signatures
             spgg_enabled = 2 * sms <= GEN_CLS;  // classes of K1g's counting sort: at least owners + owners
@@ -2075,7 +2101,7 @@ class GroupbyState {
         }
         if (!set_smem_limit((const void*)spg_hot_sample_kernel, SPG_HOT_SAMPLE_SMEM)) return false;
         { const char* e4 = getenv("B200_SPG_HOT"); spg_hot_enabled = !(e4 && e4[0] == '0'); }
-        d_hot.alloc((size_t)SPG_HOT_SLOTS * 8 + 16);
+        d_hot.alloc((size_t)SPG_HOT_SLOTS * 8 + 48);
         { const char* e3 = getenv("B200_LC"); lc_enabled = !(e3 && e3[0] == '0'); }
         spg_owners = sms;  // one owner (bucket + shared table) per SM
         // SPG-G: one counter per class of K1g.  consume_spg_gen clears n_vo + owners counters, and n_vo (owners x passes) may
@@ -2091,8 +2117,52 @@ class GroupbyState {
     size_t spgn_smem = 0;
     bool spgn_enabled = false;
     int spg_sample_wide = -1;  // sampled rows of the first launch that do NOT fit (int32 key, int32 value); -1 = not sampled
-    int64_t spgn_launches = 0, spg16_launches = 0;  // launches of the narrow-row pair, of the 16-byte pair
+    int64_t spgn_launches = 0, spg16_launches = 0;  // launches of the narrow-row pair (either form), of the 16-byte pair
     static size_t spgn_part_smem() { return (size_t)SPGN_TILE * (16 + 8 + 1) + SPG_MAX_OWNERS * 16 + 16 + (2 * SPG_MAX_OWNERS + 4) * 4 + 256; }
+    // SPG-N dense form (spgn.cuh): chosen once per state from the sample's key and value range
+    size_t spgd_max_smem = 0;  // shared memory K2d may use; 0 = the dense form is off (B200_SPG_DENSE=0 or unavailable)
+    bool spgd_ok = false;      // the sample fits a dense window: the fields below hold it
+    long long spgd_kbase = 0, spgd_vbase = 0;
+    unsigned int spgd_kb = 0, spgd_vb = 0;
+    int spgd_slots = 0;
+    int64_t spgd_wide_rows = 0, spgd_launches = 0;  // rows outside the window so far (counters[CTR_DENSE_WIDE]); dense pairs
+    static constexpr unsigned int SPGD_MUL = 0x9E3779B1u;  // odd: the key scramble's multiplier
+    static unsigned int odd_inverse(unsigned int m) {       // m^-1 mod 2^32 (Newton: each step doubles the correct low bits)
+        unsigned int x = m;                                  // correct to 3 bits for any odd m
+        for (int i = 0; i < 4; i++) x *= 2u - m * x;
+        return x;
+    }
+    // The dense window for sampled keys in [kmin, kmax] and values in [vmin, vmax] (DESIGN §3): 1/32 of the key range of head
+    // room below and above (none below when the keys start near 0), a power-of-two window of at most 2^21 keys whose K2d table
+    // fits the shared memory, and a value window of the bits the slot leaves, centred on the sampled values.
+    void spgd_plan(long long kmin, long long kmax, long long vmin, long long vmax, bool has_vals) {
+        spgd_ok = false;
+        if (spgd_max_smem == 0 || kmin > kmax) return;
+        const uint64_t range = (uint64_t)kmax - (uint64_t)kmin;
+        if (range >= (1ull << 21)) return;
+        const uint64_t pad = range / 32;
+        long long kbase;
+        if (kmin >= 0 && (uint64_t)kmin <= pad) kbase = 0;
+        else if (kmin < LLONG_MIN + (long long)pad + 1) return;  // (the window must not hold EMPTY_KEY, the marker key)
+        else kbase = kmin - (long long)pad;
+        const uint64_t span = (uint64_t)kmax - (uint64_t)kbase + 1, need = span + span / 32;
+        unsigned int kb = 1;
+        while ((1ull << kb) < need) kb++;
+        if (kb > 21 || kbase > LLONG_MAX - (long long)((1ull << kb) - 1)) return;  // (nor wrap past INT64_MAX)
+        const uint64_t slots = ((1ull << kb) + spg_owners - 1) / spg_owners;
+        if (slots * 8 > spgd_max_smem) return;
+        unsigned int sb = 0;
+        while ((1ull << sb) < slots) sb++;
+        const unsigned int vb = std::min(32u - sb, 31u);
+        long long vbase = 0;
+        if (has_vals) {
+            const uint64_t vspan = (uint64_t)vmax - (uint64_t)vmin + 1;  // (0 when the sample spans all of int64)
+            if (vspan == 0 || vspan > (1ull << vb)) return;
+            vbase = (long long)((uint64_t)vmin - ((1ull << vb) - vspan) / 2);
+        }
+        spgd_ok = true;
+        spgd_kbase = kbase; spgd_vbase = vbase; spgd_kb = kb; spgd_vb = vb; spgd_slots = (int)slots;
+    }
     int64_t spgn_group_capacity() const { return (int64_t)spg_owners * (spgn_ns * 7 / 10); }
     int spgg_ns[4] = {0, 0, 0, 0};  // K2g table slots, by slot layout v = (min/max fields) + 2 * (NA-value counter)
     size_t spgg_smem[4] = {0, 0, 0, 0};
@@ -2116,8 +2186,8 @@ class GroupbyState {
     // One SPG launch pair in flight while the host inspects the previous one (two retry lists / counter slots), so
     // the GPU never idles on the host's counter read-back.
     PooledBuf d_retry2[2];
-    static constexpr int H_SPG_WORDS = 2 * N_COUNTERS + 1;
-    long long* h_spg = nullptr;  // pinned: [slot][N_COUNTERS] counter snapshots, then the two ints of the sample verdict
+    static constexpr int H_SPG_WORDS = 2 * N_COUNTERS + 5;
+    long long* h_spg = nullptr;  // pinned: [slot][N_COUNTERS] counter snapshots, then the two ints of the sample verdict and its key / value range
     cudaEvent_t spg_ev[2] = {nullptr, nullptr};
 
     int64_t spgn_wide_rows = 0;  // rows that did not fit the narrow format so far (counters[CTR_WIDE])
@@ -2127,6 +2197,7 @@ class GroupbyState {
         const long long* hc = h_spg + slot * N_COUNTERS;
         n_groups = hc[CTR_GROUPS];
         spgn_wide_rows = hc[CTR_WIDE];
+        spgd_wide_rows = hc[CTR_DENSE_WIDE];
         const int64_t nr = hc[spg_retry_slot(slot)];  // retry rows of that launch
         if (nr == 0) return;
         // rows / partials that found the global table full: grow, then merge them like received partial rows
@@ -2174,17 +2245,21 @@ class GroupbyState {
             // once per state: count a sample of this call's keys (heavy hitters) and test the sampled rows against the narrow-row
             // format; the host reads back both verdicts
             int* d_nhot = (int*)(d_hot.as<long long>() + SPG_HOT_SLOTS);
-            spg_hot_sample_kernel<<<1, 1024, SPG_HOT_SAMPLE_SMEM, stream>>>(keys, vals, n, d_hot.as<long long>(), d_nhot);
-            B200_CUDA(cudaMemcpyAsync(h_spg + 2 * N_COUNTERS, d_nhot, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+            spg_hot_sample_kernel<<<1, 1024, SPG_HOT_SAMPLE_SMEM, stream>>>(keys, vals, n, d_hot.as<long long>(), d_nhot, d_hot.as<long long>() + SPG_HOT_SLOTS + 1);
+            B200_CUDA(cudaMemcpyAsync(h_spg + 2 * N_COUNTERS, d_nhot, 5 * sizeof(long long), cudaMemcpyDeviceToHost, stream));
             B200_CUDA(cudaStreamSynchronize(stream));
             spg_n_hot = spg_hot_enabled ? ((int*)(h_spg + 2 * N_COUNTERS))[0] : 0;
             spg_sample_wide = ((int*)(h_spg + 2 * N_COUNTERS))[1];
+            const long long* rng = h_spg + 2 * N_COUNTERS + 1;
+            spgd_plan(rng[0], rng[1], rng[2], rng[3], vals != nullptr);
             spg_hot_sampled = true;
             launches++;
         }
+        // SPG-N: no heavy hitters, and the sample found only rows that fit (int32 key, int32 value) — for either form: keys far
+        // beyond int32 (2^40 + id) keep the 16-byte pair, whose rare paths tests/test_gpu_spg_row_path.py exercises with them
+        const bool narrow_sig = spgn_enabled && !lowcard && spg_n_hot == 0 && spg_sample_wide == 0;
         // narrow bucket rows are half the bytes: twice the rows per launch for the same scratch, half the per-launch flushes
-        const bool narrow_call = spgn_enabled && !lowcard && spg_n_hot == 0 && spg_sample_wide == 0;
-        const int64_t launch_rows = narrow_call ? 2 * SPG_LAUNCH_ROWS : SPG_LAUNCH_ROWS;
+        const int64_t launch_rows = narrow_sig ? 2 * SPG_LAUNCH_ROWS : SPG_LAUNCH_ROWS;
         int64_t li = 0;
         for (int64_t r0 = 0; r0 < n; r0 += launch_rows, li++) {
             int slot = (int)(li & 1);
@@ -2198,10 +2273,12 @@ class GroupbyState {
             const int gl = (int)std::min<int64_t>((int64_t)sms * (small ? 3 : 2), (rows + LC_THREADS * 2 - 1) / (LC_THREADS * 2));
             const int g2 = (int)std::min<int64_t>((int64_t)sms * SPG_TCTAS, (rows + SPG_TILE - 1) / SPG_TILE);
             const bool hot = !lowcard && spg_hot_enabled && spg_n_hot > 0;
-            // SPG-N: the sample found only rows that fit (int32 key, int32 value), and the rows that did not so far are rare
-            const bool narrow = !lowcard && spgn_enabled && !hot && spg_sample_wide == 0 && spgn_wide_rows * 64 <= rows_consumed;
+            // SPG-N: dense when the sample found a window and the rows outside it so far are rare; else the hash form when the rows
+            // that did not fit (int32 key, int32 value) so far are rare
+            const bool dense = narrow_sig && spgd_ok && spgd_wide_rows * 64 <= rows_consumed;
+            const bool narrow = dense || (narrow_sig && spgn_wide_rows * 64 <= rows_consumed);
             const int64_t est_n = std::max<int64_t>(est_groups, 1);
-            const int n_pass = narrow ? (int)std::min<int64_t>(SPG_MAX_PASSES, std::max<int64_t>(1, (est_n + spgn_group_capacity() - 1) / spgn_group_capacity()))
+            const int n_pass = dense ? 1 : narrow ? (int)std::min<int64_t>(SPG_MAX_PASSES, std::max<int64_t>(1, (est_n + spgn_group_capacity() - 1) / spgn_group_capacity()))
                                       : spg_passes;
             // retry entries: at most one per row (K1's direct rows; in K2 a carry or a row without a slot), plus one per partial of
             // the per-CTA tables: LC's slots, or every occupied K2 slot (buckets and stash) in every pass and K1's heavy hitters
@@ -2244,10 +2321,26 @@ class GroupbyState {
                     a.bucket_cap = bucket_cap & ~1ll;
                     const size_t nsm = spgn_part_smem();
                     const int gn = (int)std::min<int64_t>((int64_t)sms * SPGN_CTAS, (rows + SPGN_TILE - 1) / SPGN_TILE);
-                    with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
-                        spgn_partition_kernel<s, c><<<gn, SPG_TTHREADS, nsm, stream>>>(a);
-                        spgn_aggregate_kernel<s, c><<<spg_owners, SPG_THREADS, spgn_smem, stream>>>(a);
-                    });
+                    if (dense) {
+                        a.bucket_cap = bucket_cap & ~3ll;  // 4-byte rows: every owner's bucket starts 16-byte aligned
+                        SpgDenseArgs da{};
+                        static_cast<SpgArgs&>(da) = a;
+                        da.kbase = spgd_kbase; da.vbase = spgd_vbase; da.d_kb = spgd_kb; da.d_vb = spgd_vb;
+                        da.d_mul = SPGD_MUL; da.d_inv = odd_inverse(SPGD_MUL);
+                        da.d_gmagic = (unsigned int)((0xffffffffull + spg_owners) / spg_owners);  // ceil(2^32 / owners)
+                        da.d_slots = spgd_slots;
+                        const size_t dsm = (size_t)spgd_slots * 8;
+                        with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
+                            spgn_partition_kernel<s, c, true><<<gn, SPG_TTHREADS, nsm, stream>>>(da);
+                            spgn_aggregate_kernel<s, c, true><<<spg_owners, SPG_THREADS, dsm, stream>>>(da);
+                        });
+                        spgd_launches++;
+                    } else {
+                        with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
+                            spgn_partition_kernel<s, c><<<gn, SPG_TTHREADS, nsm, stream>>>(a);
+                            spgn_aggregate_kernel<s, c><<<spg_owners, SPG_THREADS, spgn_smem, stream>>>(a);
+                        });
+                    }
                     spgn_launches++;
                 } else {
                     with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
@@ -3019,6 +3112,7 @@ int64_t b200_groupby_get_metric(void* state, int32_t which) {
         case 14: return s->spgn_launches;
         case 15: return s->spg16_launches;
         case 16: return s->spg_n_hot;
+        case 17: return s->spgd_launches;
         case 13: { cudaSetDevice(s->device); s->read_counters(); return s->n_groups; }  // exact (synchronises the stream)
         case 100: s->profiling = true; return 0;
         default: return -1;

@@ -9,6 +9,13 @@
 // int32, or the key INT32_MIN, which marks a free slot) take the direct global path inside K1n, so the result is exact for any
 // input; a.counters[CTR_WIDE] counts them and the host drops back to the 16-byte kernels when they are not rare.
 // Sums stay exact mod 2^64: the sign-extended value is added as (low word, high word + carry) exactly as in spg_aggregate_kernel.
+//
+// The DENSE form (template flag DENSE, DESIGN §3) is for keys that lie in a small window [kbase, kbase + 2^KB), KB <= 21, chosen
+// from the state's sample.  A row's key offset d = key - kbase is scrambled by a bijection sigma on KB bits and split into
+// (owner, slot) = (sigma(d) mod G, sigma(d) div G): the owner's shared table is direct-mapped, so the bucket row needs no key.  It
+// is ONE 4-byte word, slot << VB | (value - vbase), and K2 does one load and two 32-bit shared atomics per row with no key
+// compare and no insertion: 16 + 4 + 4 = 24 B/row of HBM traffic.  A row whose key or value offset does not fit takes the
+// direct path in K1 and counts in counters[CTR_DENSE_WIDE]; the host goes back to the hash form when such rows are not rare.
 #pragma once
 
 constexpr int SPGN_EMPTY = (int)0x80000000;
@@ -37,23 +44,39 @@ __device__ __forceinline__ uint64_t spgn_insert_ticketed(long long* __restrict__
     }
 }
 
-template <bool HAS_SUM, bool HAS_CNT>
-__global__ void __launch_bounds__(SPG_TTHREADS, SPGN_CTAS) spgn_partition_kernel(const __grid_constant__ SpgArgs a) {
+// The dense form's key map.  sigma(d) = xorshift(d * mul mod 2^KB) is a bijection on KB bits: an odd multiplier is invertible mod
+// 2^KB, and x ^ (x >> s) with 2s >= KB is its own inverse.  It spreads keys that share a stride (all multiples of G, of 128, of
+// 2^k) or a sub-range of the window over all owners.  q = umulhi(x, gmagic) with gmagic = ceil(2^32 / G) is x div G exactly for
+// x < 2^21 and 2 <= G <= 256 (the error x * (gmagic * G - 2^32) / 2^32 stays below 2^29 / 2^32).  tests/test_spgn_dense_map.py
+// checks all of it over every window size and owner count.
+__device__ __forceinline__ unsigned int spgd_scramble(unsigned int d, unsigned int kb, unsigned int mul) {
+    const unsigned int x = (d * mul) & ((1u << kb) - 1u);
+    return x ^ (x >> ((kb + 1) / 2));
+}
+__device__ __forceinline__ long long spgd_key(const SpgDenseArgs& a, unsigned int slot, unsigned int owner) {
+    unsigned int x = slot * (unsigned int)a.n_owners + owner;
+    x ^= x >> ((a.d_kb + 1) / 2);
+    return (long long)((unsigned long long)a.kbase + ((x * a.d_inv) & ((1u << a.d_kb) - 1u)));
+}
+
+template <bool HAS_SUM, bool HAS_CNT, bool DENSE = false>
+__global__ void __launch_bounds__(SPG_TTHREADS, SPGN_CTAS) spgn_partition_kernel(const __grid_constant__ std::conditional_t<DENSE, SpgDenseArgs, SpgArgs> a) {
+    using Row = std::conditional_t<DENSE, unsigned int, int2>;  // bucket row: slot << VB | value offset, or (int32 key, int32 value)
     extern __shared__ __align__(128) unsigned char smem_n_raw[];
     long long* raw_k = (long long*)smem_n_raw;                                 // [SPGN_TILE] keys
     long long* raw_v = raw_k + SPGN_TILE;                                       // [SPGN_TILE] values
-    int2* stage = (int2*)(raw_v + SPGN_TILE);                                   // SPGN_TILE x 8
+    Row* stage = (Row*)(raw_v + SPGN_TILE);                                     // SPGN_TILE rows
     unsigned long long* gbase = (unsigned long long*)(stage + SPGN_TILE);      // SPG_MAX_OWNERS x 8
     uint64_t* mbar = (uint64_t*)(gbase + SPG_MAX_OWNERS);                      // 2 mbarriers (one used)
     unsigned int* hist = (unsigned int*)(mbar + 2);                            // SPG_MAX_OWNERS
     unsigned int* lbase = hist + SPG_MAX_OWNERS;                               // SPG_MAX_OWNERS + 1
     unsigned char* stage_owner = (unsigned char*)(lbase + SPG_MAX_OWNERS + 4);  // SPGN_TILE
-    int2** dptr = (int2**)(stage_owner + SPGN_TILE);                            // SPG_MAX_OWNERS: run start - local start, as an address
+    Row** dptr = (Row**)(stage_owner + SPGN_TILE);                              // SPG_MAX_OWNERS: run start - local start, as an address
     unsigned int* tile_over = (unsigned int*)(dptr + SPG_MAX_OWNERS);           // some run of this tile does not fit its bucket
     const int G = a.n_owners, tid = threadIdx.x;
     constexpr int ROWS = SPGN_TILE / SPG_TTHREADS;
     const int64_t n_tiles = (a.n_rows + SPGN_TILE - 1) / SPGN_TILE;
-    int2* bucket = reinterpret_cast<int2*>(a.bucket);
+    Row* bucket = reinterpret_cast<Row*>(a.bucket);
     unsigned int wide = 0;
     if (tid == 0) {
         mbar_init(&mbar[0], 1);
@@ -90,6 +113,7 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPGN_CTAS) spgn_partition_kernel
         }
         int o[ROWS];
         unsigned int rk[ROWS];
+        [[maybe_unused]] unsigned int w[ROWS];  // DENSE: the row's bucket word
 #pragma unroll
         for (int r = 0; r < ROWS; r++) {
             const int j = r * SPG_TTHREADS + tid;
@@ -97,11 +121,21 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPGN_CTAS) spgn_partition_kernel
             if (!full && r0 + j >= a.n_rows) continue;
             const long long k = raw_k[j];
             const long long v = HAS_SUM ? raw_v[j] : 0;
-            // both values inside int32 <=> the high words of (x + 2^31) are zero; the key INT32_MIN (low word of k + 2^31 zero) is excluded
-            const unsigned long long kb = (unsigned long long)k + 0x80000000ull, vb = (unsigned long long)v + 0x80000000ull;
-            const bool narrow = ((kb | vb) >> 32) == 0 && (unsigned int)kb != 0u;
-            if (!narrow) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, k, (unsigned long long)v, 1ull); wide++; continue; }
-            o[r] = (int)spg_owner(spg_hash(k), G);
+            if constexpr (DENSE) {
+                // key and value offsets inside their windows (unsigned: below the base wraps to a large offset)
+                const unsigned long long d = (unsigned long long)k - (unsigned long long)a.kbase;
+                const unsigned long long e = HAS_SUM ? (unsigned long long)v - (unsigned long long)a.vbase : 0ull;
+                if ((d >> a.d_kb) != 0 || (e >> a.d_vb) != 0) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, k, (unsigned long long)v, 1ull); wide++; continue; }
+                const unsigned int x = spgd_scramble((unsigned int)d, a.d_kb, a.d_mul), q = __umulhi(x, a.d_gmagic);
+                o[r] = (int)(x - q * (unsigned int)G);
+                w[r] = q << a.d_vb | (unsigned int)e;
+            } else {
+                // both values inside int32 <=> the high words of (x + 2^31) are zero; the key INT32_MIN (low word of k + 2^31 zero) is excluded
+                const unsigned long long kb = (unsigned long long)k + 0x80000000ull, vb = (unsigned long long)v + 0x80000000ull;
+                const bool narrow = ((kb | vb) >> 32) == 0 && (unsigned int)kb != 0u;
+                if (!narrow) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, k, (unsigned long long)v, 1ull); wide++; continue; }
+                o[r] = (int)spg_owner(spg_hash(k), G);
+            }
             rk[r] = atomicAdd(&hist[o[r]], 1u);
         }
         __syncthreads();
@@ -126,7 +160,8 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPGN_CTAS) spgn_partition_kernel
             if (o[r] < 0) continue;
             const int j = r * SPG_TTHREADS + tid;
             const unsigned int p = lbase[o[r]] + rk[r];
-            stage[p] = make_int2((int)raw_k[j], HAS_SUM ? (int)raw_v[j] : 0);
+            if constexpr (DENSE) stage[p] = w[r];
+            else stage[p] = make_int2((int)raw_k[j], HAS_SUM ? (int)raw_v[j] : 0);
             stage_owner[p] = (unsigned char)o[r];
         }
         if (tid >= SPG_TTHREADS - G) {
@@ -142,7 +177,7 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPGN_CTAS) spgn_partition_kernel
             unsigned int p = tid;
             for (; p + SPG_TTHREADS < n_tile; p += 2 * SPG_TTHREADS) {
                 const unsigned int o0 = stage_owner[p], o1 = stage_owner[p + SPG_TTHREADS];
-                const int2 r0v = stage[p], r1v = stage[p + SPG_TTHREADS];
+                const Row r0v = stage[p], r1v = stage[p + SPG_TTHREADS];
                 dptr[o0][p] = r0v;
                 dptr[o1][p + SPG_TTHREADS] = r1v;
             }
@@ -151,8 +186,11 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPGN_CTAS) spgn_partition_kernel
             for (unsigned int p = tid; p < n_tile; p += SPG_TTHREADS) {
                 const unsigned int ow = stage_owner[p];
                 const unsigned long long off = gbase[ow] + p;
-                const int2 row = stage[p];
+                const Row row = stage[p];
                 if (off < (unsigned long long)a.bucket_cap) bucket[(size_t)ow * a.bucket_cap + off] = row;
+                else if constexpr (DENSE)  // bucket full (skew): the row back from its word and owner
+                    spg_direct_apply<HAS_SUM, HAS_CNT>(a, spgd_key(a, row >> a.d_vb, ow),
+                                                       (unsigned long long)a.vbase + (row & ((1u << a.d_vb) - 1u)), 1ull);
                 else spg_direct_apply<HAS_SUM, HAS_CNT>(a, (long long)row.x, (unsigned long long)(long long)row.y, 1ull);  // bucket full (skew)
             }
         }
@@ -161,7 +199,7 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPGN_CTAS) spgn_partition_kernel
         if (tid == 0) *tile_over = 0;
         __syncthreads();
     }
-    if (wide) atomicAdd((unsigned long long*)&a.counters[CTR_WIDE], (unsigned long long)wide);
+    if (wide) atomicAdd((unsigned long long*)&a.counters[DENSE ? CTR_DENSE_WIDE : CTR_WIDE], (unsigned long long)wide);
 }
 
 // K2n's two candidate buckets of a key (two slots each) among the NB buckets of the shared table
@@ -239,9 +277,55 @@ __device__ unsigned long long spgn_phase_clocks[SPG_MAX_OWNERS * 4];  // per CTA
 #define SPGN_PHASE(i) do {} while (0)
 #endif
 
+// K2d's flush of one owner's table into the state's global table: K2n's flush (below) for a table whose slot s holds a group
+// when occupied(s), read by entry(s, key, sum, cnt).  (K2n keeps its own copy, whose code is tuned to its slot layout.)
+template <bool HAS_SUM, bool HAS_CNT, typename Occupied, typename Entry>
+__device__ __forceinline__ void spgd_flush(const SpgArgs& a, int n_slots, Occupied occupied, Entry entry) {
+    const int tid = threadIdx.x;
+    __shared__ unsigned int fl_occ, fl_dup;
+    __shared__ int fl_reserved;
+    if (tid == 0) { fl_occ = 0; fl_dup = 0; fl_reserved = 0; }
+    __syncthreads();
+    if (a.reserve_tickets && a.group_limit >= 0) {
+        unsigned int mine = 0;
+        for (int s = tid; s < n_slots; s += SPG_THREADS) mine += occupied(s);
+        for (int d = 16; d; d >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, d);
+        if ((tid & 31) == 0 && mine) atomicAdd(&fl_occ, mine);
+        __syncthreads();
+        if (tid == 0 && fl_occ) {
+            const long long t = (long long)atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], (unsigned long long)fl_occ);
+            if (t + (long long)fl_occ <= a.group_limit) fl_reserved = 1;
+            else atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], (unsigned long long)(-(long long)fl_occ));  // no room: per-insert tickets
+        }
+        __syncthreads();
+    }
+    const bool reserved = fl_reserved != 0;
+    unsigned int dup = 0;
+    for (int s = tid; s < n_slots; s += SPG_THREADS) {
+        if (!occupied(s)) continue;
+        long long key;
+        unsigned long long sum, cnt;
+        entry(s, key, sum, cnt);
+        if (!reserved) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, key, sum, cnt); continue; }
+        // ticket already held: insert without the limit; a key that was there already gives its ticket back
+        bool inserted;
+        const uint64_t sl = spgn_insert_ticketed(a.tkeys, a.cap, key, inserted);
+        if (!inserted) dup++;
+        if (HAS_SUM && sum) atomicAdd(a.acc_sum + sl, sum);
+        if (HAS_CNT && cnt) atomicAdd(a.acc_cnt + sl, cnt);
+    }
+    if (reserved) {
+        for (int d = 16; d; d >>= 1) dup += __shfl_xor_sync(0xffffffffu, dup, d);
+        if ((tid & 31) == 0 && dup) atomicAdd(&fl_dup, dup);
+        __syncthreads();
+        if (tid == 0 && fl_dup) atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], (unsigned long long)(-(long long)fl_dup));
+    }
+    __syncthreads();
+}
+
 // K2n: slot = int32 key, low sum word (biased by 2^31), count.
 template <bool HAS_SUM, bool HAS_CNT>
-__global__ void __launch_bounds__(SPG_THREADS, 1) spgn_aggregate_kernel(const __grid_constant__ SpgArgs a) {
+__device__ __forceinline__ void spgn_hash_aggregate(const SpgArgs& a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SPGN_PHASE(-1);
     const int NS = a.ns, NT = a.ns + SPG_STASH, tid = threadIdx.x, me = blockIdx.x;
@@ -407,4 +491,68 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgn_aggregate_kernel(const __
         __syncthreads();
         SPGN_PHASE(2);
     }
+}
+
+// K2d, the dense form of K2n (spgn_aggregate_kernel<., ., true>): slot s of owner `me` is the key kbase + sigma^-1(s * G + me).
+// A slot is {low word of the sum of value offsets, count}; the count is kept for a sum-only signature too, it marks the slots
+// the flush visits.  The row loop has no rare path but a wrap of the sum word, which sends its 2^32 to the global table.
+template <bool HAS_SUM, bool HAS_CNT>
+__device__ __noinline__ void spgd_carry(const SpgDenseArgs& a, unsigned int slot) {
+    spg_direct_apply<HAS_SUM, HAS_CNT>(a, spgd_key(a, slot, blockIdx.x), 1ull << 32, 0ull);
+}
+
+template <bool HAS_SUM, bool HAS_CNT>
+__device__ __forceinline__ void spgd_aggregate(const SpgDenseArgs& a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int NS = a.d_slots, tid = threadIdx.x, me = blockIdx.x;
+    unsigned int* ssum = (unsigned int*)smem_raw;  // NS: sum of (value - vbase) mod 2^32
+    unsigned int* scnt = ssum + NS;                // NS: rows
+    for (int s = tid; s < NS; s += SPG_THREADS) { ssum[s] = 0; scnt[s] = 0; }
+    __syncthreads();
+    unsigned long long n_in = a.bucket_cnt[me * SPG_CNT_STRIDE];
+    if (n_in > (unsigned long long)a.bucket_cap) n_in = (unsigned long long)a.bucket_cap;
+    const unsigned int* src = reinterpret_cast<const unsigned int*>(a.bucket) + (size_t)me * a.bucket_cap;  // bucket_cap % 4 == 0: 16-byte aligned
+    const unsigned int vb = a.d_vb, vmask = (1u << vb) - 1u;
+    auto add = [&](unsigned int w) {
+        const unsigned int s = w >> vb;
+        if (HAS_SUM) {
+            const unsigned int e = w & vmask, old = atomicAdd(&ssum[s], e);
+            if (old + e < old) spgd_carry<HAS_SUM, HAS_CNT>(a, s);
+        }
+        atomicAdd(&scnt[s], 1u);
+    };
+    // software pipeline: V 16-byte loads (4 rows each) per thread in flight while the previous V are aggregated
+    constexpr int V = 2;
+    const uint4* src4 = reinterpret_cast<const uint4*>(src);
+    const unsigned long long n4 = n_in / 4, step = (unsigned long long)V * SPG_THREADS, full = n4 / step * step;
+    if (full > 0) {
+        uint4 cur[V], nxt[V];
+#pragma unroll
+        for (int j = 0; j < V; j++) cur[j] = __ldcs(src4 + tid + j * SPG_THREADS);
+        for (unsigned long long ub = 0; ub < full; ub += step) {
+            if (ub + step < full) {
+#pragma unroll
+                for (int j = 0; j < V; j++) nxt[j] = __ldcs(src4 + ub + step + tid + j * SPG_THREADS);
+            }
+#pragma unroll
+            for (int j = 0; j < V; j++) { add(cur[j].x); add(cur[j].y); add(cur[j].z); add(cur[j].w); }
+#pragma unroll
+            for (int j = 0; j < V; j++) cur[j] = nxt[j];
+        }
+    }
+    for (unsigned long long i = 4 * full + tid; i < n_in; i += SPG_THREADS) add(__ldcs(src + i));
+    __syncthreads();
+    const unsigned long long vbase = (unsigned long long)a.vbase;
+    spgd_flush<HAS_SUM, HAS_CNT>(a, NS, [&](int s) { return scnt[s] != 0; },
+                                 [&](int s, long long& key, unsigned long long& sum, unsigned long long& cnt) {
+                                     cnt = (unsigned long long)scnt[s];
+                                     key = spgd_key(a, (unsigned int)s, (unsigned int)me);
+                                     sum = (unsigned long long)ssum[s] + cnt * vbase;  // exact mod 2^64
+                                 });
+}
+
+template <bool HAS_SUM, bool HAS_CNT, bool DENSE = false>
+__global__ void __launch_bounds__(SPG_THREADS, 1) spgn_aggregate_kernel(const __grid_constant__ std::conditional_t<DENSE, SpgDenseArgs, SpgArgs> a) {
+    if constexpr (DENSE) spgd_aggregate<HAS_SUM, HAS_CNT>(a);
+    else spgn_hash_aggregate<HAS_SUM, HAS_CNT>(a);
 }
