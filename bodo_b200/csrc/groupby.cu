@@ -1045,6 +1045,7 @@ constexpr int SPG_MAX_OWNERS = 256;
 // slower after an unrelated allocation moved it), so every counter gets its own line.
 constexpr int SPG_CNT_STRIDE = 16;
 constexpr int SPG_STASH = 1024;     // K2: linear-probing stash slots for keys whose two buckets are full
+constexpr int SPGN_EMPTY = (int)0x80000000;  // free slot of a shared table with int32 keys (spgn.cuh)
 
 struct SpgArgs {
     const long long* keys;
@@ -1211,9 +1212,10 @@ __global__ void __launch_bounds__(1024, 1) spg_hot_sample_kernel(const long long
 // Each tile is counting-sorted by owner in shared memory: hash, shared-memory histogram atomic (a row's rank in its owner's
 // run), exclusive scan of the histogram by warp 0, staging of the rows at their sorted positions.  One global atomic per
 // (tile, owner) on the owner's row counter reserves a run in its bucket, and the runs are copied out with coalesced 16-byte
-// stores; rows past the end of a bucket (skew) take the direct path.
+// stores; rows past the end of a bucket (skew) take the direct path.  spg_partition_tiles below is this loop for every K1
+// form (K1, K1n in spgn.cuh, K1g in spgg.cuh); a form supplies only what it loads, how it classifies and stages a row, and
+// how it copies the staged rows out.
 constexpr int SPG_TTHREADS = 512;  // threads per CTA of K1 (4 rows per thread per tile)
-constexpr int SPG_TBUFS = 1;       // raw tile buffers per CTA (1: next tile streams in during copy-out; 2: full double buffering)
 constexpr int SPG_TCTAS = 3;       // CTAs per SM
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -1234,85 +1236,161 @@ __device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gsrc, ui
                  ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
+// The shared memory of one K1 shape, as byte offsets: the raw tile (TMA destination: TILE 8-byte keys, TILE 8-byte values),
+// TILE staged rows of ROW_BYTES, per class the published run start (gbase), the tile's mbarrier, the class histogram and its
+// exclusive scan (lbase), then TAIL bytes the form lays out itself.  Every region is a multiple of 16 bytes (TMA destinations).
+// The kernel takes its pointers and the host its launch size (`bytes`) from here.
+template <int TILE, int MAX_C, int ROW_BYTES, int TAIL>
+struct SpgTileSmem {
+    static constexpr size_t raw_k = 0, raw_v = raw_k + (size_t)TILE * 8, stage = raw_v + (size_t)TILE * 8;
+    static constexpr size_t gbase = stage + (size_t)TILE * ROW_BYTES, mbar = gbase + (size_t)MAX_C * 8, hist = mbar + 16;
+    static constexpr size_t lbase = hist + (size_t)MAX_C * 4, tail = lbase + (size_t)(MAX_C + 4) * 4, bytes = tail + TAIL;
+    static_assert(stage % 16 == 0 && gbase % 16 == 0 && lbase % 16 == 0 && tail % 16 == 0, "K1 shared regions stay 16-byte aligned");
+};
+
+// The K1 tile loop shared by every form.  C classes (at most the shape's MAX_C, and at most THREADS: the last C threads
+// reserve the runs); class c's bucket row counter is cls_cnt[c * SPG_CNT_STRIDE].  The form's part, as callables:
+//   load_tma(r0, mbar)    thread 0, full tile at row r0: expect_tx on mbar and the tile's bulk copies
+//   load_partial(r0)      every thread, the trailing partial tile: the same slabs with ordinary loads
+//   init()                thread 0, once, after the mbarrier's init: the form's own shared state
+//   classify(j, w)        tile row j (in range): its class, or -1 when the row was handled here; w is handed on to stage
+//   stage(p, j, c, w)     store tile row j of class c at staged position p
+//   on_run(c, g0, n)      the run thread of class c, after gbase[c] is published: the run starts at g0 and holds n rows
+//   copy_out(n_tile)      copy the n_tile staged rows out: staged row p of class c goes to offset gbase[c] + p of c's bucket
+template <int TILE, int THREADS, typename Smem, typename LoadTma, typename LoadPartial, typename Init, typename Classify,
+          typename Stage, typename OnRun, typename CopyOut>
+__device__ __forceinline__ void spg_partition_tiles(unsigned char* smem, int64_t n_rows, int C, unsigned long long* cls_cnt,
+                                                    LoadTma load_tma, LoadPartial load_partial, Init init, Classify classify,
+                                                    Stage stage, OnRun on_run, CopyOut copy_out) {
+    unsigned long long* gbase = (unsigned long long*)(smem + Smem::gbase);
+    uint64_t* mbar = (uint64_t*)(smem + Smem::mbar);
+    unsigned int* hist = (unsigned int*)(smem + Smem::hist);
+    unsigned int* lbase = (unsigned int*)(smem + Smem::lbase);
+    const int tid = threadIdx.x;
+    constexpr int ROWS = TILE / THREADS;
+    const int64_t n_tiles = (n_rows + TILE - 1) / TILE;
+    if (tid == 0) {
+        mbar_init(mbar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        init();
+    }
+    for (int j = tid; j < C; j += THREADS) hist[j] = 0;
+    __syncthreads();
+    // full tiles come in through TMA; a trailing partial tile is loaded with ordinary loads
+    auto issue = [&](int64_t t) {
+        const int64_t r0 = t * TILE;
+        if (r0 + TILE <= n_rows && tid == 0) load_tma(r0, mbar);
+    };
+    uint32_t phase = 0;
+    int64_t t = blockIdx.x;
+    if (t < n_tiles) issue(t);
+    for (; t < n_tiles; t += gridDim.x) {
+        const int64_t r0 = t * TILE;
+        const int64_t tn = t + gridDim.x;
+        const bool full = r0 + TILE <= n_rows;
+        if (full) {
+            while (!mbar_try_wait(mbar, phase)) {}
+            phase ^= 1;
+        } else {
+            load_partial(r0);
+            __syncthreads();
+        }
+        int c[ROWS];
+        unsigned int rk[ROWS];
+        [[maybe_unused]] unsigned int w[ROWS];
+#pragma unroll
+        for (int r = 0; r < ROWS; r++) {
+            const int j = r * THREADS + tid;
+            c[r] = -1;
+            if (r0 + j >= n_rows) continue;
+            c[r] = classify(j, w[r]);
+            if (c[r] >= 0) rk[r] = atomicAdd(&hist[c[r]], 1u);
+        }
+        __syncthreads();
+        // reserve one run per class: the global atomic's round trip (~1 us) is kept in a register and only waited for
+        // after the staging pass, which needs the local prefix sums but not the global run start
+        unsigned long long my_gbase = 0;
+        unsigned int my_cnt = 0;
+        if (tid >= THREADS - C) { const int cl = tid - (THREADS - C); my_cnt = hist[cl]; if (my_cnt) my_gbase = atomicAdd(&cls_cnt[cl * SPG_CNT_STRIDE], (unsigned long long)my_cnt); }
+        if (tid < 32) {
+            unsigned int carry = 0;
+            for (int base = 0; base < C; base += 32) {
+                int j = base + tid;
+                unsigned int x = j < C ? hist[j] : 0u, inc = x;
+#pragma unroll
+                for (int d = 1; d < 32; d <<= 1) { unsigned int y = __shfl_up_sync(0xffffffffu, inc, d); if (tid >= d) inc += y; }
+                if (j < C) lbase[j] = carry + inc - x;
+                carry += __shfl_sync(0xffffffffu, inc, 31);
+            }
+            if (tid == 0) lbase[C] = carry;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int r = 0; r < ROWS; r++) {
+            if (c[r] < 0) continue;
+            stage(lbase[c[r]] + rk[r], r * THREADS + tid, c[r], w[r]);
+        }
+        // publish run start minus local start, so the copy-out computes its destination with one add
+        if (tid >= THREADS - C) {
+            const int cl = tid - (THREADS - C);
+            gbase[cl] = my_gbase - lbase[cl];
+            on_run(cl, my_gbase, my_cnt);
+        }
+        __syncthreads();  // the raw tile is free from here on
+        if (tn < n_tiles) issue(tn);  // the next tile streams in during the copy-out
+        copy_out(lbase[C]);
+        for (int j = tid; j < C; j += THREADS) hist[j] = 0;
+        __syncthreads();
+    }
+}
+
+// K1 (16-byte rows): class = owner.  The marker key takes the direct path; with HOT the heavy hitters are aggregated here.
+template <bool HOT>
+using SpgK1Smem = SpgTileSmem<SPG_TILE, SPG_MAX_OWNERS, 16, SPG_TILE + (HOT ? SPG_HOT_SLOTS * 20 : 0)>;
+
 template <bool HAS_SUM, bool HAS_CNT, bool HOT = false>
 __global__ void __launch_bounds__(SPG_TTHREADS, SPG_TCTAS) spg_partition_tma_kernel(const __grid_constant__ SpgArgs a) {
     extern __shared__ __align__(128) unsigned char smem_tma_raw[];  // own name: the other kernels declare smem_raw with 16-byte alignment
-    long long* raw_k = (long long*)smem_tma_raw;                                   // [NB][SPG_TILE] keys
-    long long* raw_v = raw_k + SPG_TBUFS * SPG_TILE;                           // [NB][SPG_TILE] values
-    longlong2* stage = (longlong2*)(raw_v + SPG_TBUFS * SPG_TILE);             // SPG_TILE x 16
-    unsigned long long* gbase = (unsigned long long*)(stage + SPG_TILE);      // SPG_MAX_OWNERS x 8
-    uint64_t* mbar = (uint64_t*)(gbase + SPG_MAX_OWNERS);                      // 2 mbarriers
-    unsigned int* hist = (unsigned int*)(mbar + 2);                            // SPG_MAX_OWNERS
-    unsigned int* lbase = hist + SPG_MAX_OWNERS;                               // SPG_MAX_OWNERS + 1
-    unsigned char* stage_owner = (unsigned char*)(lbase + SPG_MAX_OWNERS + 4);  // SPG_TILE
+    using L = SpgK1Smem<HOT>;
+    long long* raw_k = (long long*)(smem_tma_raw + L::raw_k);
+    long long* raw_v = (long long*)(smem_tma_raw + L::raw_v);
+    longlong2* stage = (longlong2*)(smem_tma_raw + L::stage);
+    const unsigned long long* gbase = (const unsigned long long*)(smem_tma_raw + L::gbase);
+    unsigned char* stage_owner = smem_tma_raw + L::tail;                       // SPG_TILE
     long long* hkeys = (long long*)(stage_owner + SPG_TILE);                   // SPG_HOT_SLOTS heavy-hitter keys ...
     unsigned int* hlo = (unsigned int*)(hkeys + SPG_HOT_SLOTS);                // ... and this CTA's partial sums / row counts
     unsigned int* hhi = hlo + SPG_HOT_SLOTS;
     unsigned int* hcnt = hhi + SPG_HOT_SLOTS;
     const int G = a.n_owners, tid = threadIdx.x;
-    constexpr bool hot_on = HOT;  // separate instantiation: the uniform-key kernel carries none of this (its SASS is the
-                                  // kernel tuned before heavy hitters existed)
-    if (hot_on)
+    // HOT is a separate instantiation: the uniform-key kernel carries none of this
+    if (HOT)
         for (int s = tid; s < SPG_HOT_SLOTS; s += SPG_TTHREADS) { hkeys[s] = a.hot_tab[s]; hlo[s] = 0; hhi[s] = 0; hcnt[s] = 0; }
-    constexpr int ROWS = SPG_TILE / SPG_TTHREADS;
-    const int64_t n_tiles = (a.n_rows + SPG_TILE - 1) / SPG_TILE;
-    if (tid == 0) {
-        mbar_init(&mbar[0], 1);
-        mbar_init(&mbar[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    for (int j = tid; j < G; j += SPG_TTHREADS) hist[j] = 0;
-    __syncthreads();
-    // full tiles come in through TMA; a trailing partial tile is loaded with ordinary loads
-    auto issue = [&](int64_t t, int b) {
-        const int64_t r0 = t * SPG_TILE;
-        if (r0 + SPG_TILE <= a.n_rows) {
-            if (tid == 0) {
-                mbar_expect_tx(&mbar[b], (HAS_SUM ? 2u : 1u) * SPG_TILE * 8u);
-                tma_load_1d(raw_k + b * SPG_TILE, a.keys + r0, SPG_TILE * 8u, &mbar[b]);
-                if (HAS_SUM) tma_load_1d(raw_v + b * SPG_TILE, a.vals + r0, SPG_TILE * 8u, &mbar[b]);
-            }
-        }
-    };
-    uint32_t phase[2] = {0, 0};
-    int64_t t = blockIdx.x;
-    int b = 0;
-    if (t < n_tiles) issue(t, 0);
-    for (; t < n_tiles; t += gridDim.x, b ^= (SPG_TBUFS - 1)) {
-        const int64_t r0 = t * SPG_TILE;
-        const int64_t tn = t + gridDim.x;
-        if (SPG_TBUFS == 2 && tn < n_tiles) issue(tn, b ^ 1);  // prefetch the next tile of this CTA while this one is sorted
-        const bool full = r0 + SPG_TILE <= a.n_rows;
-        long long* kb = raw_k + b * SPG_TILE;
-        long long* vb = raw_v + b * SPG_TILE;
-        if (full) {
-            while (!mbar_try_wait(&mbar[b], phase[b])) {}
-            phase[b] ^= 1;
-        } else {
+    spg_partition_tiles<SPG_TILE, SPG_TTHREADS, L>(
+        smem_tma_raw, a.n_rows, G, a.bucket_cnt,
+        [&](int64_t r0, uint64_t* mbar) {
+            mbar_expect_tx(mbar, (HAS_SUM ? 2u : 1u) * SPG_TILE * 8u);
+            tma_load_1d(raw_k, a.keys + r0, SPG_TILE * 8u, mbar);
+            if (HAS_SUM) tma_load_1d(raw_v, a.vals + r0, SPG_TILE * 8u, mbar);
+        },
+        [&](int64_t r0) {
             for (int j = tid; j < SPG_TILE; j += SPG_TTHREADS) {
-                int64_t i = r0 + j;
-                kb[j] = i < a.n_rows ? a.keys[i] : 0;
-                vb[j] = (HAS_SUM && i < a.n_rows) ? a.vals[i] : 0;
+                const int64_t i = r0 + j;
+                raw_k[j] = i < a.n_rows ? a.keys[i] : 0;
+                raw_v[j] = (HAS_SUM && i < a.n_rows) ? a.vals[i] : 0;
             }
-            __syncthreads();
-        }
-        int o[ROWS];
-        unsigned int rk[ROWS];
-#pragma unroll
-        for (int r = 0; r < ROWS; r++) {
-            const int j = r * SPG_TTHREADS + tid;
-            o[r] = -1;
-            if (r0 + j >= a.n_rows) continue;
-            const long long k = kb[j];
-            if (k == EMPTY_KEY) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, k, HAS_SUM ? (unsigned long long)vb[j] : 0ull, 1ull); continue; }
+        },
+        [] {},
+        [&](int j, unsigned int&) -> int {
+            const long long k = raw_k[j];
+            if (k == EMPTY_KEY) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, k, HAS_SUM ? (unsigned long long)raw_v[j] : 0ull, 1ull); return -1; }
             const uint64_t h = spg_hash(k);
-            if (hot_on) {  // heavy hitter: aggregate here, the row never reaches an owner bucket
+            if (HOT) {  // heavy hitter: aggregate here, the row never reaches an owner bucket
                 const unsigned int hb = spg_hot_bucket(h);
                 const ulonglong2 hk2 = *reinterpret_cast<const ulonglong2*>(hkeys + 2 * hb);
                 const int hs = hk2.x == (unsigned long long)k ? (int)(2 * hb) : hk2.y == (unsigned long long)k ? (int)(2 * hb + 1) : -1;
                 if (hs >= 0) {
                     if (HAS_SUM) {
-                        const unsigned long long v = (unsigned long long)vb[j];
+                        const unsigned long long v = (unsigned long long)raw_v[j];
                         const unsigned int lo = (unsigned int)v;
                         unsigned int hi = (unsigned int)(v >> 32);
                         const unsigned int old = atomicAdd(&hlo[hs], lo);
@@ -1320,64 +1398,110 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPG_TCTAS) spg_partition_tma_ker
                         if (hi) atomicAdd(&hhi[hs], hi);
                     }
                     atomicAdd(&hcnt[hs], 1u);  // rows, also when only SUM is asked for: the group has to exist
-                    continue;
+                    return -1;
                 }
             }
-            o[r] = (int)spg_owner(h, G);
-            rk[r] = atomicAdd(&hist[o[r]], 1u);
-        }
-        __syncthreads();
-        // reserve one run per owner: the global atomic's round trip (~1 us) is kept in a register and only waited for
-        // after the staging pass, which needs the local prefix sums but not the global run start
-        unsigned long long my_gbase = 0;
-        if (tid >= SPG_TTHREADS - G) { int ow = tid - (SPG_TTHREADS - G); unsigned int cnt = hist[ow]; if (cnt) my_gbase = atomicAdd(&a.bucket_cnt[ow * SPG_CNT_STRIDE], (unsigned long long)cnt); }
-        if (tid < 32) {
-            unsigned int carry = 0;
-            for (int base = 0; base < G; base += 32) {
-                int j = base + tid;
-                unsigned int x = j < G ? hist[j] : 0u, inc = x;
-#pragma unroll
-                for (int d = 1; d < 32; d <<= 1) { unsigned int y = __shfl_up_sync(0xffffffffu, inc, d); if (tid >= d) inc += y; }
-                if (j < G) lbase[j] = carry + inc - x;
-                carry += __shfl_sync(0xffffffffu, inc, 31);
+            return (int)spg_owner(h, G);
+        },
+        [&](unsigned int p, int j, int o, unsigned int) {
+            stage[p] = make_longlong2(raw_k[j], HAS_SUM ? raw_v[j] : 0);
+            stage_owner[p] = (unsigned char)o;
+        },
+        [](int, unsigned long long, unsigned int) {},
+        [&](unsigned int n_tile) {
+            for (unsigned int p = tid; p < n_tile; p += SPG_TTHREADS) {
+                unsigned int ow = stage_owner[p];
+                unsigned long long off = gbase[ow] + p;
+                longlong2 row = stage[p];
+                if (off < (unsigned long long)a.bucket_cap) a.bucket[(size_t)ow * a.bucket_cap + off] = row;
+                else spg_direct_apply<HAS_SUM, HAS_CNT>(a, row.x, (unsigned long long)row.y, 1ull);
             }
-            if (tid == 0) lbase[G] = carry;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int r = 0; r < ROWS; r++) {
-            if (o[r] < 0) continue;
-            const int j = r * SPG_TTHREADS + tid;
-            unsigned int p = lbase[o[r]] + rk[r];
-            stage[p] = make_longlong2(kb[j], HAS_SUM ? vb[j] : 0);
-            stage_owner[p] = (unsigned char)o[r];
-        }
-        // publish run start minus local start, so the copy-out computes its destination with one add
-        if (tid >= SPG_TTHREADS - G) { int ow = tid - (SPG_TTHREADS - G); gbase[ow] = my_gbase - lbase[ow]; }
-        __syncthreads();  // raw buffer b is free from here on
-        if (SPG_TBUFS == 1 && tn < n_tiles) issue(tn, 0);  // single buffer: the next tile streams in during the copy-out
-        const unsigned int n_tile = lbase[G];
-        for (unsigned int p = tid; p < n_tile; p += SPG_TTHREADS) {
-            unsigned int ow = stage_owner[p];
-            unsigned long long off = gbase[ow] + p;
-            longlong2 row = stage[p];
-            if (off < (unsigned long long)a.bucket_cap) a.bucket[(size_t)ow * a.bucket_cap + off] = row;
-            else spg_direct_apply<HAS_SUM, HAS_CNT>(a, row.x, (unsigned long long)row.y, 1ull);
-        }
-        for (int j = tid; j < G; j += SPG_TTHREADS) hist[j] = 0;
-        __syncthreads();
-    }
-    if (hot_on) {  // this CTA's heavy-hitter partials -> global table (n_hot atomics per CTA)
+        });
+    if (HOT) {  // this CTA's heavy-hitter partials -> global table (n_hot atomics per CTA)
         __syncthreads();
         for (int s = tid; s < SPG_HOT_SLOTS; s += SPG_TTHREADS)
             if (hcnt[s]) spg_direct_apply<HAS_SUM, HAS_CNT>(a, hkeys[s], (unsigned long long)hlo[s] | ((unsigned long long)hhi[s] << 32), (unsigned long long)hcnt[s]);
     }
 }
 
+// The two-choice shared table of K2, K2n and K2g: every key has two candidate buckets of two slots (one shared load each);
+// slots [2 NB, 2 NB + SPG_STASH) are a linear-probing stash.  K is the slot's key word: long long (free = EMPTY_KEY) or int
+// (free = SPGN_EMPTY).
+template <typename K>
+using SpgKeyPair = std::conditional_t<sizeof(K) == 8, longlong2, int2>;
+template <typename K>
+__device__ __forceinline__ constexpr K spg_free_key() {
+    if constexpr (sizeof(K) == 8) return EMPTY_KEY;
+    else return SPGN_EMPTY;
+}
+__device__ __forceinline__ long long spg_cas(long long* p, long long cmp, long long val) {
+    return (long long)atomicCAS((unsigned long long*)p, (unsigned long long)cmp, (unsigned long long)val);
+}
+__device__ __forceinline__ int spg_cas(int* p, int cmp, int val) { return atomicCAS(p, cmp, val); }
+
+// the two candidate buckets of a key with hash h among the NB buckets
+__device__ __forceinline__ void spg_buckets(uint64_t h, unsigned int NB, unsigned int& b1, unsigned int& b2) {
+    b1 = __umulhi((unsigned int)(h >> 20), NB);
+    b2 = __umulhi(((unsigned int)h ^ (unsigned int)(h >> 44)) * 0x9E3779B1u, NB);  // low word of h remixed: independent of b1's bits 20..51 enough
+    b2 = b2 == b1 ? (b1 + 1 == NB ? 0u : b1 + 1) : b2;
+}
+
+// the slot of `key` among the four candidates, the keys c1 of bucket b1 and c2 of bucket b2, or -1
+template <typename K>
+__device__ __forceinline__ int spg_match(SpgKeyPair<K> c1, SpgKeyPair<K> c2, unsigned int b1, unsigned int b2, K key) {
+    return c1.x == key ? (int)(2 * b1) : c1.y == key ? (int)(2 * b1 + 1) : c2.x == key ? (int)(2 * b2) : c2.y == key ? (int)(2 * b2 + 1) : -1;
+}
+// the hot lookup: two loads and four compares, no branch
+template <typename K>
+__device__ __forceinline__ int spg_find(const K* skeys, unsigned int b1, unsigned int b2, K key) {
+    return spg_match<K>(*reinterpret_cast<const SpgKeyPair<K>*>(skeys + 2 * b1), *reinterpret_cast<const SpgKeyPair<K>*>(skeys + 2 * b2), b1, b2, key);
+}
+
+// The slow path of a key with hash h in a table of NS bucket slots: its slot if one of the four candidates holds it, else a free candidate slot it claims,
+// else its find-or-insert slot in the stash; -1 when the stash is full too (the caller takes the direct path).
+// Balanced allocation: a new key goes to the EMPTIER of its two buckets (0.9 % of the keys overflow into the stash at 50 %
+// load where first-fit left 2.2 % there — every row of a stash-resident key comes through here), and the four CAS attempts
+// are skipped when both buckets are full (buckets never lose keys), so a stash-resident key costs two loads and one stash
+// probe instead of four failed CAS round trips.
+template <typename K>
+__device__ __forceinline__ int spg_claim(K* skeys, unsigned int NS, uint64_t h, K key) {
+    constexpr K FREE = spg_free_key<K>();
+    const unsigned int NB = NS / 2;
+    unsigned int b1, b2;
+    spg_buckets(h, NB, b1, b2);
+    const SpgKeyPair<K> c1 = *reinterpret_cast<const SpgKeyPair<K>*>(skeys + 2 * b1);
+    const SpgKeyPair<K> c2 = *reinterpret_cast<const SpgKeyPair<K>*>(skeys + 2 * b2);
+    const int f1 = (c1.x == FREE) + (c1.y == FREE), f2 = (c2.x == FREE) + (c2.y == FREE);
+    int s = spg_match<K>(c1, c2, b1, b2, key);
+    if (s < 0 && f1 + f2 > 0) {
+        const unsigned int first = f2 > f1 ? b2 : b1, second = f2 > f1 ? b1 : b2;
+        const unsigned int cand[4] = {2 * first, 2 * first + 1, 2 * second, 2 * second + 1};
+#pragma unroll
+        for (int c = 0; c < 4 && s < 0; c++) {
+            const K prev = spg_cas(&skeys[cand[c]], FREE, key);
+            if (prev == FREE || prev == key) s = (int)cand[c];
+        }
+    }
+    if (s < 0) {
+        unsigned int st = NS + ((unsigned int)(h >> 12) & (SPG_STASH - 1));
+        for (int probes = 0; probes < SPG_STASH && s < 0; probes++) {
+            K kk = skeys[st];
+            if (kk == FREE) {
+                const K prev = spg_cas(&skeys[st], FREE, key);
+                if (prev == FREE) { s = (int)st; break; }
+                kk = prev;
+            }
+            if (kk == key) { s = (int)st; break; }
+            st = st + 1 == NS + SPG_STASH ? NS : st + 1;
+        }
+    }
+    return s;
+}
+
 // K2: one CTA per owner aggregates its bucket in shared memory, then flushes into the global table.
 //
-// Shared table = two-choice bucketed hash table + stash: every key has two candidate buckets of two slots (one 16-byte
-// shared load each), so the hot lookup is two unconditional loads + four compares, no probe loop and no divergence
+// Shared table = the two-choice bucketed hash table + stash above (spg_find / spg_claim) with 16-byte candidate loads, so
+// the hot lookup is two unconditional loads + four compares, no probe loop and no divergence
 // (a linear-probing table spends much of its issue slots on loop control with about half the lanes active; compare a
 // collision-free key set with scratch/ubench3.cu).
 // Everything else — first appearance of a key (CAS into a free candidate slot), keys whose four candidates are taken
@@ -1397,12 +1521,6 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spg_aggregate_kernel(const __g
     const unsigned int NB = (unsigned int)NS / 2;
     const unsigned int NP = (unsigned int)a.n_pass, GP = (unsigned int)gridDim.x * NP;
 
-    auto buckets = [&](long long key, unsigned int& b1, unsigned int& b2) {
-        const uint64_t h = spg_hash(key);
-        b1 = __umulhi((unsigned int)(h >> 20), NB);
-        b2 = __umulhi(((unsigned int)h ^ (unsigned int)(h >> 44)) * 0x9E3779B1u, NB);  // low word of h remixed: independent of b1's bits 20..51 enough
-        b2 = b2 == b1 ? (b1 + 1 == NB ? 0u : b1 + 1) : b2;
-    };
     auto add = [&](int s, long long key, long long val) {
         if (HAS_SUM) {
             unsigned int lo = (unsigned int)(unsigned long long)val, hi = (unsigned int)((unsigned long long)val >> 32);
@@ -1412,42 +1530,9 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spg_aggregate_kernel(const __g
         }
         if (HAS_CNT) atomicAdd(&scnt[s], 1u);
     };
-    // slow path: claim a free candidate slot, else find-or-insert in the stash, else the direct global path.
-    // Balanced allocation: a new key goes to the EMPTIER of its two buckets (0.9 % of the keys overflow into the stash
-    // at 50 % load where first-fit left 2.2 % there — every row of a stash-resident key comes through here), and the four
-    // CAS attempts are skipped when both buckets are full (buckets never lose keys), so a stash-resident key costs two
-    // loads and one stash probe instead of four failed CAS round trips.
+    // slow path: the key's slot, a free candidate slot or a stash slot, else the direct global path
     auto slow_upsert = [&](long long key, long long val) {
-        unsigned int b1, b2;
-        buckets(key, b1, b2);
-        const unsigned long long uk = (unsigned long long)key;
-        const ulonglong2 c1 = *reinterpret_cast<const ulonglong2*>(skeys + 2 * b1);
-        const ulonglong2 c2 = *reinterpret_cast<const ulonglong2*>(skeys + 2 * b2);
-        const int f1 = (c1.x == (unsigned long long)EMPTY_KEY) + (c1.y == (unsigned long long)EMPTY_KEY);
-        const int f2 = (c2.x == (unsigned long long)EMPTY_KEY) + (c2.y == (unsigned long long)EMPTY_KEY);
-        int s = c1.x == uk ? (int)(2 * b1) : c1.y == uk ? (int)(2 * b1 + 1) : c2.x == uk ? (int)(2 * b2) : c2.y == uk ? (int)(2 * b2 + 1) : -1;
-        if (s < 0 && f1 + f2 > 0) {
-            const unsigned int first = f2 > f1 ? b2 : b1, second = f2 > f1 ? b1 : b2;
-            const unsigned int cand[4] = {2 * first, 2 * first + 1, 2 * second, 2 * second + 1};
-#pragma unroll
-            for (int c = 0; c < 4 && s < 0; c++) {
-                unsigned long long old = atomicCAS((unsigned long long*)&skeys[cand[c]], (unsigned long long)EMPTY_KEY, uk);
-                if (old == (unsigned long long)EMPTY_KEY || old == uk) s = (int)cand[c];
-            }
-        }
-        if (s < 0) {
-            unsigned int st = (unsigned int)NS + ((unsigned int)(spg_hash(key) >> 12) & (SPG_STASH - 1));
-            for (int probes = 0; probes < SPG_STASH && s < 0; probes++) {
-                unsigned long long kk = (unsigned long long)skeys[st];
-                if (kk == (unsigned long long)EMPTY_KEY) {
-                    unsigned long long old = atomicCAS((unsigned long long*)&skeys[st], (unsigned long long)EMPTY_KEY, uk);
-                    if (old == (unsigned long long)EMPTY_KEY) { s = (int)st; break; }
-                    kk = old;
-                }
-                if (kk == uk) { s = (int)st; break; }
-                st = st + 1 == (unsigned int)NS + SPG_STASH ? (unsigned int)NS : st + 1;
-            }
-        }
+        const int s = spg_claim(skeys, (unsigned int)NS, spg_hash(key), key);
         if (s < 0) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, key, (unsigned long long)val, 1ull); return; }
         add(s, key, val);
     };
@@ -1469,11 +1554,8 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spg_aggregate_kernel(const __g
 #pragma unroll
         for (int u = 0; u < U; u++) {  // hot lookups: branch-free
             unsigned int b1, b2;
-            buckets(row[u].x, b1, b2);
-            const ulonglong2 k1 = *reinterpret_cast<const ulonglong2*>(skeys + 2 * b1);
-            const ulonglong2 k2 = *reinterpret_cast<const ulonglong2*>(skeys + 2 * b2);
-            const unsigned long long uk = (unsigned long long)row[u].x;
-            sl[u] = k1.x == uk ? (int)(2 * b1) : k1.y == uk ? (int)(2 * b1 + 1) : k2.x == uk ? (int)(2 * b2) : k2.y == uk ? (int)(2 * b2 + 1) : -1;
+            spg_buckets(spg_hash(row[u].x), NB, b1, b2);
+            sl[u] = spg_find(skeys, b1, b2, row[u].x);
             if (!FULL && row[u].x == EMPTY_KEY) sl[u] = -2;  // padding lane
             // multi-pass: owner = mulhi(hash_hi, G) = mulhi(hash_hi, G * NP) / NP; this pass keeps sub-range `pass` only
             if (NP > 1 && __umulhi((unsigned int)(spg_hash(row[u].x) >> 32), GP) - (unsigned int)me * NP != pass) sl[u] = -2;
@@ -2062,8 +2144,8 @@ class GroupbyState {
         bool ok = true;
         for_each_sum_cnt([&](auto s, auto c) {
             ok = ok && set_smem_limit((const void*)spg_aggregate_kernel<s, c>, spg_smem)
-                    && set_smem_limit((const void*)spg_partition_tma_kernel<s, c>, spg_tma_smem())
-                    && set_smem_limit((const void*)spg_partition_tma_kernel<s, c, true>, spg_tma_smem(true))
+                    && set_smem_limit((const void*)spg_partition_tma_kernel<s, c>, SpgK1Smem<false>::bytes)
+                    && set_smem_limit((const void*)spg_partition_tma_kernel<s, c, true>, SpgK1Smem<true>::bytes)
                     && set_smem_limit((const void*)groupby_lowcard_kernel<s, c, LC_SLOTS_BIG, 2>, (size_t)LC_SLOTS_BIG * 20 + 64);
         });
         if (!ok) return false;
@@ -2073,9 +2155,9 @@ class GroupbyState {
             spgn_enabled = true;
             spgd_max_smem = (size_t)max_smem - 256;  // (K2d's flush has a few static shared words)
             for_each_sum_cnt([&](auto s, auto c) {
-                if (!set_smem_limit((const void*)spgn_partition_kernel<s, c>, spgn_part_smem())) spgn_enabled = false;
+                if (!set_smem_limit((const void*)spgn_partition_kernel<s, c>, SpgnK1Smem<false>::bytes)) spgn_enabled = false;
                 if (!set_smem_limit((const void*)spgn_aggregate_kernel<s, c>, spgn_smem)) spgn_enabled = false;
-                if (!set_smem_limit((const void*)spgn_partition_kernel<s, c, true>, spgn_part_smem())) spgd_max_smem = 0;
+                if (!set_smem_limit((const void*)spgn_partition_kernel<s, c, true>, SpgnK1Smem<true>::bytes)) spgd_max_smem = 0;
                 if (!set_smem_limit((const void*)spgn_aggregate_kernel<s, c, true>, spgd_max_smem)) spgd_max_smem = 0;
             });
             const char* e8 = getenv("B200_SPG_NARROW");
@@ -2086,7 +2168,7 @@ class GroupbyState {
         {   // SPG-G (spgg.cuh): generic signatures
             spgg_enabled = 2 * sms <= GEN_CLS;  // classes of K1g's counting sort: at least owners + owners
             for_each_spgg_part([&](auto ks, auto vs) {
-                if (!set_smem_limit((const void*)spgg_partition_kernel<ks, vs>, GEN_K1_SMEM)) spgg_enabled = false;
+                if (!set_smem_limit((const void*)spgg_partition_kernel<ks, vs>, SpggK1Smem::bytes)) spgg_enabled = false;
             });
             for (int v = 0; v < 4; v++) {  // v = mm + 2 * nn
                 const int sb = 16 + ((v & 1) ? 16 : 0) + ((v & 2) ? 4 : 0);
@@ -2118,7 +2200,6 @@ class GroupbyState {
     bool spgn_enabled = false;
     int spg_sample_wide = -1;  // sampled rows of the first launch that do NOT fit (int32 key, int32 value); -1 = not sampled
     int64_t spgn_launches = 0, spg16_launches = 0;  // launches of the narrow-row pair (either form), of the 16-byte pair
-    static size_t spgn_part_smem() { return (size_t)SPGN_TILE * (16 + 8 + 1) + SPG_MAX_OWNERS * 16 + 16 + (2 * SPG_MAX_OWNERS + 4) * 4 + 256; }
     // SPG-N dense form (spgn.cuh): chosen once per state from the sample's key and value range
     size_t spgd_max_smem = 0;  // shared memory K2d may use; 0 = the dense form is off (B200_SPG_DENSE=0 or unavailable)
     bool spgd_ok = false;      // the sample fits a dense window: the fields below hold it
@@ -2178,7 +2259,6 @@ class GroupbyState {
         int64_t p = (est + spg_group_capacity() - 1) / spg_group_capacity();
         return p <= 1 ? 1 : (p <= SPG_MAX_PASSES ? (int)p : 0);
     }
-    static size_t spg_tma_smem(bool hot = false) { return (size_t)SPG_TILE * (16 * SPG_TBUFS + 16 + 1) + SPG_MAX_OWNERS * 8 + 16 + (2 * SPG_MAX_OWNERS + 4) * 4 + (hot ? SPG_HOT_SLOTS * 20 : 0) + 256; }
     bool lc_pick(int64_t est) { lowcard_small = est <= LC_SLOTS_SMALL / 4; return lc_enabled && est <= LC_SLOTS_BIG / 4; }
     // groups the shared-memory tables of all owners are expected to hold together (two-choice buckets work well up to ~70 %)
     int64_t spg_group_capacity() const { return (int64_t)spg_owners * (spg_ns * 7 / 10); }
@@ -2310,7 +2390,6 @@ class GroupbyState {
                 lc_launches++;
             } else {
                 if (hot) { a.hot_tab = d_hot.as<long long>(); a.n_hot = (const int*)(d_hot.as<long long>() + SPG_HOT_SLOTS); }
-                const size_t tsm = spg_tma_smem(hot);
                 if (narrow) {
                     a.ns = spgn_ns;
                     // first flush into an empty table: per-CTA ticket reservation, but only with >= 25 % head room under the group
@@ -2319,7 +2398,6 @@ class GroupbyState {
                     // 8 GPUs: 1 M groups against a limit of 2^20 cost 1.4 ms per state in some runs)
                     a.reserve_tickets = (n_groups_bound == 0 && li == 0 && est_groups > 0 && est_groups + est_groups / 4 <= (int64_t)(cap / 2)) ? 1 : 0;
                     a.bucket_cap = bucket_cap & ~1ll;
-                    const size_t nsm = spgn_part_smem();
                     const int gn = (int)std::min<int64_t>((int64_t)sms * SPGN_CTAS, (rows + SPGN_TILE - 1) / SPGN_TILE);
                     if (dense) {
                         a.bucket_cap = bucket_cap & ~3ll;  // 4-byte rows: every owner's bucket starts 16-byte aligned
@@ -2331,21 +2409,21 @@ class GroupbyState {
                         da.d_slots = spgd_slots;
                         const size_t dsm = (size_t)spgd_slots * 8;
                         with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
-                            spgn_partition_kernel<s, c, true><<<gn, SPG_TTHREADS, nsm, stream>>>(da);
+                            spgn_partition_kernel<s, c, true><<<gn, SPG_TTHREADS, SpgnK1Smem<true>::bytes, stream>>>(da);
                             spgn_aggregate_kernel<s, c, true><<<spg_owners, SPG_THREADS, dsm, stream>>>(da);
                         });
                         spgd_launches++;
                     } else {
                         with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
-                            spgn_partition_kernel<s, c><<<gn, SPG_TTHREADS, nsm, stream>>>(a);
+                            spgn_partition_kernel<s, c><<<gn, SPG_TTHREADS, SpgnK1Smem<false>::bytes, stream>>>(a);
                             spgn_aggregate_kernel<s, c><<<spg_owners, SPG_THREADS, spgn_smem, stream>>>(a);
                         });
                     }
                     spgn_launches++;
                 } else {
                     with_sum_cnt(sum_j >= 0, cnt_j >= 0, [&](auto s, auto c) {
-                        if (hot) spg_partition_tma_kernel<s, c, true><<<g2, SPG_TTHREADS, tsm, stream>>>(a);
-                        else spg_partition_tma_kernel<s, c><<<g2, SPG_TTHREADS, tsm, stream>>>(a);
+                        if (hot) spg_partition_tma_kernel<s, c, true><<<g2, SPG_TTHREADS, SpgK1Smem<true>::bytes, stream>>>(a);
+                        else spg_partition_tma_kernel<s, c><<<g2, SPG_TTHREADS, SpgK1Smem<false>::bytes, stream>>>(a);
                         spg_aggregate_kernel<s, c><<<spg_owners, SPG_THREADS, spg_smem, stream>>>(a);
                     });
                     spg16_launches++;
@@ -2440,7 +2518,7 @@ class GroupbyState {
             const SpgGenArgs g = make_args();
             const ProfEvents prof = prof_begin(profiling);
             const int g1 = (int)std::min<int64_t>((int64_t)sms * SPG_TCTAS, (rows + SPG_TILE - 1) / SPG_TILE);
-            with_spgg_part(ks, vs, [&](auto k, auto v) { spgg_partition_kernel<k, v><<<g1, SPG_TTHREADS, GEN_K1_SMEM, stream>>>(g); });
+            with_spgg_part(ks, vs, [&](auto k, auto v) { spgg_partition_kernel<k, v><<<g1, SPG_TTHREADS, SpggK1Smem::bytes, stream>>>(g); });
             with_spgg_agg(gs.has_sum, gs.has_mm, gs.has_nn, [&](auto s, auto m, auto nn) {
                 spgg_aggregate_kernel<s, m, nn><<<spg_owners, SPG_THREADS, spgg_smem[mm], stream>>>(g);
             });

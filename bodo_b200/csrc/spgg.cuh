@@ -8,13 +8,13 @@
 //           per launch and owner and folds it into the state's double accumulator at the flush; the reference adds doubles row
 //           by row, _groupby_agg_funcs.h:673-689 — same value up to the rounding of the partial sums)
 //
-// K1g is spg_partition_tma_kernel generalised: the tile's raw key / value bytes AND its two validity-bitmap slices (256 B per
-// 2048-row tile) come in through TMA (cp.async.bulk + mbarrier), rows are widened to (int64 key, int64 value) when they are
+// K1g runs K1's tile loop (spg_partition_tiles in groupby.cu): the tile's raw key / value bytes AND its two validity-bitmap
+// slices (256 B per 2048-row tile) come in through TMA (cp.async.bulk + mbarrier), rows are widened to (int64 key, int64 value) when they are
 // read from the staging tile.  Rows whose VALUE is NA must still create their group (and count for `size`): they are
 // partitioned too, into a second, key-only bucket per owner (class index owner + G in the same counting sort), so no row
 // takes a global-memory probe inside K1g.  NA-KEY rows are dropped (dropna) or pre-aggregated per CTA in shared memory and
 // added to the NA slot of the state's table once per CTA.  Only rows with the marker key and bucket overflow (skew) take the
-// direct path.  K2g is spg_aggregate_kernel's hot loop over a wider slot when min / max are asked for (key, low sum word,
+// direct path.  K2g is spg_aggregate_kernel's hot loop (the shared two-choice table: spg_buckets, spg_find, spg_claim) over a wider slot when min / max are asked for (key, low sum word,
 // count, min, max = 32 B instead of 16 B, so the owners hold half as many groups per pass), plus a pass over the owner's
 // key-only bucket.  min / max read the slot first and only issue the (CAS-emulated, SASS ATOMS.CAST.SPIN.64) 64-bit shared
 // atomic when the row improves the extremum: ~ln(rows per group) times per group.
@@ -97,7 +97,9 @@ __global__ void spgg_replay_kernel(const __grid_constant__ SpgGenArgs g, const u
 }
 
 constexpr int GEN_CLS = 448;  // counting-sort classes of K1g: n_vo buckets of valued rows + n_owners buckets of NA-value rows
-constexpr size_t GEN_K1_SMEM = (size_t)SPG_TILE * 32 + GEN_CLS * 8 + 16 + 48 + GEN_CLS * 4 + (GEN_CLS + 4) * 4 + 2 * (SPG_TILE / 8 + 16) + 64;
+// K1g's shared memory: spg_partition_tiles' regions (raw keys / values of up to 8 bytes), then the tile's two validity slices
+// (SPG_TILE / 8 + 16 bytes each) and the CTA's NA-key group (48 bytes)
+using SpggK1Smem = SpgTileSmem<SPG_TILE, GEN_CLS, 16, 2 * (SPG_TILE / 8 + 16) + 48>;
 
 template <int BYTES>
 __device__ __forceinline__ long long gen_widen(const void* raw, int j, int is_signed) {
@@ -106,70 +108,44 @@ __device__ __forceinline__ long long gen_widen(const void* raw, int j, int is_si
     return is_signed ? (long long)t : (long long)(unsigned int)t;
 }
 
-// K1g: KS / VS = bytes per key / value element (VS = 0: no value column).
+// K1g: KS / VS = bytes per key / value element (VS = 0: no value column).  Class = valued bucket (owner, or virtual owner), or
+// n_vo + owner for the key-only bucket of a row whose value is NA.
 template <int KS, int VS>
 __global__ void __launch_bounds__(SPG_TTHREADS, SPG_TCTAS) spgg_partition_kernel(const __grid_constant__ SpgGenArgs g) {
     extern __shared__ __align__(128) unsigned char smem_gen_raw[];
+    using L = SpggK1Smem;
     const SpgArgs& a = g.s;
-    unsigned char* raw_k = smem_gen_raw;                                          // SPG_TILE x 8 (raw bytes: SPG_TILE x KS used)
-    unsigned char* raw_v = raw_k + SPG_TILE * 8;                                  // SPG_TILE x 8
-    longlong2* stage = (longlong2*)(raw_v + SPG_TILE * 8);                        // SPG_TILE x 16
-    unsigned long long* gbase = (unsigned long long*)(stage + SPG_TILE);         // GEN_CLS x 8
-    uint64_t* mbar = (uint64_t*)(gbase + GEN_CLS);                                // 2 mbarriers (one used)
-    unsigned long long* na_sum = (unsigned long long*)(mbar + 2);                 // NA-key group, this CTA's partial aggregate
+    unsigned char* raw_k = smem_gen_raw + L::raw_k;                               // SPG_TILE x 8 (raw bytes: SPG_TILE x KS used)
+    unsigned char* raw_v = smem_gen_raw + L::raw_v;                               // SPG_TILE x 8
+    longlong2* stage = (longlong2*)(smem_gen_raw + L::stage);                     // SPG_TILE x 16
+    const unsigned long long* gbase = (const unsigned long long*)(smem_gen_raw + L::gbase);
+    unsigned char* kvb = smem_gen_raw + L::tail;                                  // 256 + 16 validity bytes of the tile's keys
+    unsigned char* vvb = kvb + SPG_TILE / 8 + 16;                                 // ... and values
+    unsigned long long* na_sum = (unsigned long long*)(vvb + SPG_TILE / 8 + 16);  // NA-key group, this CTA's partial aggregate
     long long* na_min = (long long*)(na_sum + 1);
     long long* na_max = na_min + 1;
     long long* na_hi = na_max + 1;                                                // high word of the 128-bit sum (MEAN); 8 bytes pad
     unsigned int* na_cnt = (unsigned int*)(na_hi + 2);                            // [0] non-NA values, [1] NA values
-    unsigned int* hist = na_cnt + 2;                                              // GEN_CLS
-    unsigned int* lbase = hist + GEN_CLS;                                         // GEN_CLS + 4
-    unsigned char* kvb = (unsigned char*)(lbase + GEN_CLS + 4);                   // 256 + 16 validity bytes of the tile's keys
-    unsigned char* vvb = kvb + SPG_TILE / 8 + 16;                                 // ... and values
     const bool k_nullable = g.kvalid != nullptr, v_nullable = VS && g.vvalid != nullptr;
     const int G = a.n_owners, NVO = g.n_vo, C = NVO + (v_nullable ? G : 0), tid = threadIdx.x;
-    constexpr int ROWS = SPG_TILE / SPG_TTHREADS;
-    const int64_t n_tiles = (a.n_rows + SPG_TILE - 1) / SPG_TILE;
-    if (tid == 0) {
-        mbar_init(&mbar[0], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        *na_sum = 0; *na_hi = 0; *na_min = INT64_MAX; *na_max = INT64_MIN; na_cnt[0] = 0; na_cnt[1] = 0;
-    }
-    for (int j = tid; j < C; j += SPG_TTHREADS) hist[j] = 0;
-    __syncthreads();
-    auto issue = [&](int64_t t) {
-        const int64_t r0 = t * SPG_TILE;
-        if (r0 + SPG_TILE <= a.n_rows && tid == 0) {
-            mbar_expect_tx(&mbar[0], (uint32_t)(SPG_TILE * (KS + VS) + (k_nullable ? SPG_TILE / 8 : 0) + (v_nullable ? SPG_TILE / 8 : 0)));
-            tma_load_1d(raw_k, (const char*)g.kdata + r0 * KS, SPG_TILE * KS, &mbar[0]);
-            if (VS) tma_load_1d(raw_v, (const char*)g.vdata + r0 * VS, SPG_TILE * VS, &mbar[0]);
-            if (k_nullable) tma_load_1d(kvb, g.kvalid + r0 / 8, SPG_TILE / 8, &mbar[0]);
-            if (v_nullable) tma_load_1d(vvb, g.vvalid + r0 / 8, SPG_TILE / 8, &mbar[0]);
-        }
-    };
-    uint32_t phase = 0;
-    int64_t t = blockIdx.x;
-    if (t < n_tiles) issue(t);
-    for (; t < n_tiles; t += gridDim.x) {
-        const int64_t r0 = t * SPG_TILE;
-        const int64_t tn = t + gridDim.x;
-        if (r0 + SPG_TILE <= a.n_rows) {
-            while (!mbar_try_wait(&mbar[0], phase)) {}
-            phase ^= 1;
-        } else {  // trailing partial tile: ordinary loads of the raw bytes
+    spg_partition_tiles<SPG_TILE, SPG_TTHREADS, L>(
+        smem_gen_raw, a.n_rows, C, a.bucket_cnt,
+        [&](int64_t r0, uint64_t* mbar) {
+            mbar_expect_tx(mbar, (uint32_t)(SPG_TILE * (KS + VS) + (k_nullable ? SPG_TILE / 8 : 0) + (v_nullable ? SPG_TILE / 8 : 0)));
+            tma_load_1d(raw_k, (const char*)g.kdata + r0 * KS, SPG_TILE * KS, mbar);
+            if (VS) tma_load_1d(raw_v, (const char*)g.vdata + r0 * VS, SPG_TILE * VS, mbar);
+            if (k_nullable) tma_load_1d(kvb, g.kvalid + r0 / 8, SPG_TILE / 8, mbar);
+            if (v_nullable) tma_load_1d(vvb, g.vvalid + r0 / 8, SPG_TILE / 8, mbar);
+        },
+        [&](int64_t r0) {  // the raw bytes
             const int64_t left = a.n_rows - r0;
             for (int64_t j = tid; j < left * KS; j += SPG_TTHREADS) raw_k[j] = ((const unsigned char*)g.kdata)[r0 * KS + j];
             if (VS) for (int64_t j = tid; j < left * VS; j += SPG_TTHREADS) raw_v[j] = ((const unsigned char*)g.vdata)[r0 * VS + j];
             if (k_nullable) for (int64_t j = tid; j < (left + 7) / 8; j += SPG_TTHREADS) kvb[j] = g.kvalid[r0 / 8 + j];
             if (v_nullable) for (int64_t j = tid; j < (left + 7) / 8; j += SPG_TTHREADS) vvb[j] = g.vvalid[r0 / 8 + j];
-            __syncthreads();
-        }
-        int cls[ROWS];
-        unsigned int rk[ROWS];
-#pragma unroll
-        for (int r = 0; r < ROWS; r++) {
-            const int j = r * SPG_TTHREADS + tid;
-            cls[r] = -1;
-            if (r0 + j >= a.n_rows) continue;
+        },
+        [&] { *na_sum = 0; *na_hi = 0; *na_min = INT64_MAX; *na_max = INT64_MIN; na_cnt[0] = 0; na_cnt[1] = 0; },
+        [&](int j, unsigned int&) -> int {
             const bool kok = !k_nullable || ((kvb[j >> 3] >> (j & 7)) & 1);
             const bool vok = !v_nullable || ((vvb[j >> 3] >> (j & 7)) & 1);
             const long long k = gen_widen<KS>(raw_k, j, g.k_signed);
@@ -186,58 +162,34 @@ __global__ void __launch_bounds__(SPG_TTHREADS, SPG_TCTAS) spgg_partition_kernel
                         if (v > *na_max) atomicMax(na_max, v);
                     } else atomicAdd(&na_cnt[1], 1u);
                 }
-                continue;
+                return -1;
             }
-            if (k == EMPTY_KEY) { gen_direct_apply(g, k, vok ? (unsigned long long)v : 0ull, vok ? (double)v : 0.0, vok ? 1ull : 0ull, vok ? 0ull : 1ull, v, v); continue; }
-            cls[r] = vok ? (int)spg_owner(spg_hash(k), NVO) : NVO + (int)spg_owner(spg_hash(k), G);
-            rk[r] = atomicAdd(&hist[cls[r]], 1u);
-        }
-        __syncthreads();
-        unsigned long long my_gbase = 0;
-        if (tid >= SPG_TTHREADS - C) { int c = tid - (SPG_TTHREADS - C); unsigned int cnt = hist[c]; if (cnt) my_gbase = atomicAdd(&a.bucket_cnt[c * SPG_CNT_STRIDE], (unsigned long long)cnt); }
-        if (tid < 32) {
-            unsigned int carry = 0;
-            for (int base = 0; base < C; base += 32) {
-                int j = base + tid;
-                unsigned int x = j < C ? hist[j] : 0u, inc = x;
-#pragma unroll
-                for (int d = 1; d < 32; d <<= 1) { unsigned int y = __shfl_up_sync(0xffffffffu, inc, d); if (tid >= d) inc += y; }
-                if (j < C) lbase[j] = carry + inc - x;
-                carry += __shfl_sync(0xffffffffu, inc, 31);
-            }
-            if (tid == 0) lbase[C] = carry;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int r = 0; r < ROWS; r++) {
-            if (cls[r] < 0) continue;
-            const int j = r * SPG_TTHREADS + tid;
-            const unsigned int p = lbase[cls[r]] + rk[r];
+            if (k == EMPTY_KEY) { gen_direct_apply(g, k, vok ? (unsigned long long)v : 0ull, vok ? (double)v : 0.0, vok ? 1ull : 0ull, vok ? 0ull : 1ull, v, v); return -1; }
+            return vok ? (int)spg_owner(spg_hash(k), NVO) : NVO + (int)spg_owner(spg_hash(k), G);
+        },
+        [&](unsigned int p, int j, int, unsigned int) {
             stage[p] = make_longlong2(gen_widen<KS>(raw_k, j, g.k_signed), VS ? gen_widen<VS ? VS : 8>(raw_v, j, g.v_signed) : 0);
-        }
-        if (tid >= SPG_TTHREADS - C) { int c = tid - (SPG_TTHREADS - C); gbase[c] = my_gbase - lbase[c]; }
-        __syncthreads();  // the raw tile is free from here on
-        if (tn < n_tiles) issue(tn);  // the next tile streams in during the copy-out
-        // the staged rows are sorted by class, valued rows first: a row's class follows from its key and its position
-        const unsigned int n_tile = lbase[C], n_valued = lbase[NVO];
-        for (unsigned int p = tid; p < n_tile; p += SPG_TTHREADS) {
-            const longlong2 row = stage[p];
-            const uint64_t h = spg_hash(row.x);
-            if (p < n_valued) {
-                const unsigned int c = spg_owner(h, NVO);
-                const unsigned long long off = gbase[c] + p;
-                if (off < (unsigned long long)a.bucket_cap) a.bucket[(size_t)c * a.bucket_cap + off] = row;
-                else gen_direct_apply(g, row.x, (unsigned long long)row.y, (double)row.y, 1ull, 0ull, row.y, row.y);  // bucket full (skew)
-            } else {
-                const unsigned int o = spg_owner(h, G);
-                const unsigned long long off = gbase[NVO + o] + p;
-                if (off < (unsigned long long)a.bucket_cap) g.nbucket[(size_t)o * a.bucket_cap + off] = row.x;
-                else gen_direct_apply(g, row.x, 0ull, 0.0, 0ull, 1ull, 0, 0);
+        },
+        [](int, unsigned long long, unsigned int) {},
+        [&](unsigned int n_tile) {
+            // the staged rows are sorted by class, valued rows first: a row's class follows from its key and its position
+            const unsigned int n_valued = ((const unsigned int*)(smem_gen_raw + L::lbase))[NVO];
+            for (unsigned int p = tid; p < n_tile; p += SPG_TTHREADS) {
+                const longlong2 row = stage[p];
+                const uint64_t h = spg_hash(row.x);
+                if (p < n_valued) {
+                    const unsigned int c = spg_owner(h, NVO);
+                    const unsigned long long off = gbase[c] + p;
+                    if (off < (unsigned long long)a.bucket_cap) a.bucket[(size_t)c * a.bucket_cap + off] = row;
+                    else gen_direct_apply(g, row.x, (unsigned long long)row.y, (double)row.y, 1ull, 0ull, row.y, row.y);  // bucket full (skew)
+                } else {
+                    const unsigned int o = spg_owner(h, G);
+                    const unsigned long long off = gbase[NVO + o] + p;
+                    if (off < (unsigned long long)a.bucket_cap) g.nbucket[(size_t)o * a.bucket_cap + off] = row.x;
+                    else gen_direct_apply(g, row.x, 0ull, 0.0, 0ull, 1ull, 0, 0);
+                }
             }
-        }
-        for (int j = tid; j < C; j += SPG_TTHREADS) hist[j] = 0;
-        __syncthreads();
-    }
+        });
     if (tid == 0 && (na_cnt[0] | na_cnt[1])) {  // NA-key group (slot cap of the state's table)
         a.counters[CTR_NA] = 1;
         const double msum = (double)*na_hi * 18446744073709551616.0 + (double)*na_sum;  // na_hi * 2^64 + the unsigned low word
@@ -262,12 +214,6 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgg_aggregate_kernel(const __
     const bool VO = g.n_vo != a.n_owners;  // bucket me * NP + pass holds exactly this pass's rows
     const bool CHK = NP > 1 && !VO;        // else every row of the owner's bucket is tested against the pass
 
-    auto buckets = [&](long long key, unsigned int& b1, unsigned int& b2) {
-        const uint64_t h = spg_hash(key);
-        b1 = __umulhi((unsigned int)(h >> 20), NB);
-        b2 = __umulhi(((unsigned int)h ^ (unsigned int)(h >> 44)) * 0x9E3779B1u, NB);
-        b2 = b2 == b1 ? (b1 + 1 == NB ? 0u : b1 + 1) : b2;
-    };
     auto add = [&](int s, long long key, long long val) {
         if (HAS_SUM) {
             unsigned int lo = (unsigned int)(unsigned long long)val, hi = (unsigned int)((unsigned long long)val >> 32);
@@ -284,40 +230,8 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgg_aggregate_kernel(const __
             if (val > smax[s]) atomicMax(&smax[s], val);
         }
     };
-    // slow path: claim a free candidate slot, else find-or-insert in the stash; -1 = no room (the row goes the direct way)
-    auto slow_slot = [&](long long key) -> int {
-        unsigned int b1, b2;
-        buckets(key, b1, b2);
-        const unsigned long long uk = (unsigned long long)key;
-        const ulonglong2 c1 = *reinterpret_cast<const ulonglong2*>(skeys + 2 * b1);
-        const ulonglong2 c2 = *reinterpret_cast<const ulonglong2*>(skeys + 2 * b2);
-        const int f1 = (c1.x == (unsigned long long)EMPTY_KEY) + (c1.y == (unsigned long long)EMPTY_KEY);
-        const int f2 = (c2.x == (unsigned long long)EMPTY_KEY) + (c2.y == (unsigned long long)EMPTY_KEY);
-        int s = c1.x == uk ? (int)(2 * b1) : c1.y == uk ? (int)(2 * b1 + 1) : c2.x == uk ? (int)(2 * b2) : c2.y == uk ? (int)(2 * b2 + 1) : -1;
-        if (s < 0 && f1 + f2 > 0) {
-            const unsigned int first = f2 > f1 ? b2 : b1, second = f2 > f1 ? b1 : b2;
-            const unsigned int cand[4] = {2 * first, 2 * first + 1, 2 * second, 2 * second + 1};
-#pragma unroll
-            for (int c = 0; c < 4 && s < 0; c++) {
-                unsigned long long old = atomicCAS((unsigned long long*)&skeys[cand[c]], (unsigned long long)EMPTY_KEY, uk);
-                if (old == (unsigned long long)EMPTY_KEY || old == uk) s = (int)cand[c];
-            }
-        }
-        if (s < 0) {
-            unsigned int st = (unsigned int)NS + ((unsigned int)(spg_hash(key) >> 12) & (SPG_STASH - 1));
-            for (int probes = 0; probes < SPG_STASH && s < 0; probes++) {
-                unsigned long long kk = (unsigned long long)skeys[st];
-                if (kk == (unsigned long long)EMPTY_KEY) {
-                    unsigned long long old = atomicCAS((unsigned long long*)&skeys[st], (unsigned long long)EMPTY_KEY, uk);
-                    if (old == (unsigned long long)EMPTY_KEY) { s = (int)st; break; }
-                    kk = old;
-                }
-                if (kk == uk) { s = (int)st; break; }
-                st = st + 1 == (unsigned int)NS + SPG_STASH ? (unsigned int)NS : st + 1;
-            }
-        }
-        return s;
-    };
+    // slow path: the key's slot, a free candidate slot or a stash slot; -1 = no room (the row goes the direct way)
+    auto slow_slot = [&](long long key) { return spg_claim(skeys, (unsigned int)NS, spg_hash(key), key); };
     auto slow_upsert = [&](long long key, long long val) {
         const int s = slow_slot(key);
         if (s < 0) { gen_direct_apply(g, key, (unsigned long long)val, (double)val, 1ull, 0ull, val, val); return; }
@@ -342,11 +256,8 @@ __global__ void __launch_bounds__(SPG_THREADS, 1) spgg_aggregate_kernel(const __
 #pragma unroll
         for (int u = 0; u < U; u++) {
             unsigned int b1, b2;
-            buckets(row[u].x, b1, b2);
-            const ulonglong2 k1 = *reinterpret_cast<const ulonglong2*>(skeys + 2 * b1);
-            const ulonglong2 k2 = *reinterpret_cast<const ulonglong2*>(skeys + 2 * b2);
-            const unsigned long long uk = (unsigned long long)row[u].x;
-            sl[u] = k1.x == uk ? (int)(2 * b1) : k1.y == uk ? (int)(2 * b1 + 1) : k2.x == uk ? (int)(2 * b2) : k2.y == uk ? (int)(2 * b2 + 1) : -1;
+            spg_buckets(spg_hash(row[u].x), NB, b1, b2);
+            sl[u] = spg_find(skeys, b1, b2, row[u].x);
             if (!FULL && row[u].x == EMPTY_KEY) sl[u] = -2;
             if (CHK && __umulhi((unsigned int)(spg_hash(row[u].x) >> 32), GP) - (unsigned int)me * NP != pass) sl[u] = -2;
         }

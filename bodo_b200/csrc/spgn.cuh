@@ -9,6 +9,8 @@
 // int32, or the key INT32_MIN, which marks a free slot) take the direct global path inside K1n, so the result is exact for any
 // input; a.counters[CTR_WIDE] counts them and the host drops back to the 16-byte kernels when they are not rare.
 // Sums stay exact mod 2^64: the sign-extended value is added as (low word, high word + carry) exactly as in spg_aggregate_kernel.
+// K1n is K1's tile loop (spg_partition_tiles in groupby.cu) with its own classify / stage / copy-out; K2n's table is the shared
+// two-choice table (spg_find, and spg_claim in spgn_cold_row) with int32 keys, and K2n and K2d flush through spg_flush_ticketed.
 //
 // The DENSE form (template flag DENSE, DESIGN §3) is for keys that lie in a small window [kbase, kbase + 2^KB), KB <= 21, chosen
 // from the state's sample.  A row's key offset d = key - kbase is scrambled by a bijection sigma on KB bits and split into
@@ -18,7 +20,6 @@
 // direct path in K1 and counts in counters[CTR_DENSE_WIDE]; the host goes back to the hash form when such rows are not rare.
 #pragma once
 
-constexpr int SPGN_EMPTY = (int)0x80000000;
 #ifndef SPGN_TILE_ROWS
 #define SPGN_TILE_ROWS 4096
 #endif
@@ -59,158 +60,100 @@ __device__ __forceinline__ long long spgd_key(const SpgDenseArgs& a, unsigned in
     return (long long)((unsigned long long)a.kbase + ((x * a.d_inv) & ((1u << a.d_kb) - 1u)));
 }
 
+// K1n's shared memory: spg_partition_tiles' regions with 8-byte (hash) or 4-byte (dense) staged rows, then the staged rows'
+// owners (SPGN_TILE), per owner its run's destination (SPG_MAX_OWNERS pointers) and the tile_over flag
+template <bool DENSE>
+using SpgnK1Smem = SpgTileSmem<SPGN_TILE, SPG_MAX_OWNERS, DENSE ? 4 : 8, SPGN_TILE + SPG_MAX_OWNERS * 8 + 16>;
+
 template <bool HAS_SUM, bool HAS_CNT, bool DENSE = false>
 __global__ void __launch_bounds__(SPG_TTHREADS, SPGN_CTAS) spgn_partition_kernel(const __grid_constant__ std::conditional_t<DENSE, SpgDenseArgs, SpgArgs> a) {
     using Row = std::conditional_t<DENSE, unsigned int, int2>;  // bucket row: slot << VB | value offset, or (int32 key, int32 value)
+    using L = SpgnK1Smem<DENSE>;
     extern __shared__ __align__(128) unsigned char smem_n_raw[];
-    long long* raw_k = (long long*)smem_n_raw;                                 // [SPGN_TILE] keys
-    long long* raw_v = raw_k + SPGN_TILE;                                       // [SPGN_TILE] values
-    Row* stage = (Row*)(raw_v + SPGN_TILE);                                     // SPGN_TILE rows
-    unsigned long long* gbase = (unsigned long long*)(stage + SPGN_TILE);      // SPG_MAX_OWNERS x 8
-    uint64_t* mbar = (uint64_t*)(gbase + SPG_MAX_OWNERS);                      // 2 mbarriers (one used)
-    unsigned int* hist = (unsigned int*)(mbar + 2);                            // SPG_MAX_OWNERS
-    unsigned int* lbase = hist + SPG_MAX_OWNERS;                               // SPG_MAX_OWNERS + 1
-    unsigned char* stage_owner = (unsigned char*)(lbase + SPG_MAX_OWNERS + 4);  // SPGN_TILE
+    long long* raw_k = (long long*)(smem_n_raw + L::raw_k);
+    long long* raw_v = (long long*)(smem_n_raw + L::raw_v);
+    Row* stage = (Row*)(smem_n_raw + L::stage);
+    const unsigned long long* gbase = (const unsigned long long*)(smem_n_raw + L::gbase);
+    unsigned char* stage_owner = smem_n_raw + L::tail;                          // SPGN_TILE
     Row** dptr = (Row**)(stage_owner + SPGN_TILE);                              // SPG_MAX_OWNERS: run start - local start, as an address
     unsigned int* tile_over = (unsigned int*)(dptr + SPG_MAX_OWNERS);           // some run of this tile does not fit its bucket
     const int G = a.n_owners, tid = threadIdx.x;
-    constexpr int ROWS = SPGN_TILE / SPG_TTHREADS;
-    const int64_t n_tiles = (a.n_rows + SPGN_TILE - 1) / SPGN_TILE;
     Row* bucket = reinterpret_cast<Row*>(a.bucket);
     unsigned int wide = 0;
-    if (tid == 0) {
-        mbar_init(&mbar[0], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        *tile_over = 0;
-    }
-    for (int j = tid; j < G; j += SPG_TTHREADS) hist[j] = 0;
-    __syncthreads();
-    auto issue = [&](int64_t t) {
-        const int64_t r0 = t * SPGN_TILE;
-        if (r0 + SPGN_TILE <= a.n_rows && tid == 0) {
-            mbar_expect_tx(&mbar[0], (HAS_SUM ? 2u : 1u) * SPGN_TILE * 8u);
-            tma_load_1d(raw_k, a.keys + r0, SPGN_TILE * 8u, &mbar[0]);
-            if (HAS_SUM) tma_load_1d(raw_v, a.vals + r0, SPGN_TILE * 8u, &mbar[0]);
-        }
-    };
-    uint32_t phase = 0;
-    int64_t t = blockIdx.x;
-    if (t < n_tiles) issue(t);
-    for (; t < n_tiles; t += gridDim.x) {
-        const int64_t r0 = t * SPGN_TILE;
-        const int64_t tn = t + gridDim.x;
-        const bool full = r0 + SPGN_TILE <= a.n_rows;
-        if (full) {
-            while (!mbar_try_wait(&mbar[0], phase)) {}
-            phase ^= 1;
-        } else {
+    spg_partition_tiles<SPGN_TILE, SPG_TTHREADS, L>(
+        smem_n_raw, a.n_rows, G, a.bucket_cnt,
+        [&](int64_t r0, uint64_t* mbar) {
+            mbar_expect_tx(mbar, (HAS_SUM ? 2u : 1u) * SPGN_TILE * 8u);
+            tma_load_1d(raw_k, a.keys + r0, SPGN_TILE * 8u, mbar);
+            if (HAS_SUM) tma_load_1d(raw_v, a.vals + r0, SPGN_TILE * 8u, mbar);
+        },
+        [&](int64_t r0) {
             for (int j = tid; j < SPGN_TILE; j += SPG_TTHREADS) {
                 int64_t i = r0 + j;
                 raw_k[j] = i < a.n_rows ? a.keys[i] : 0;
                 raw_v[j] = (HAS_SUM && i < a.n_rows) ? a.vals[i] : 0;
             }
-            __syncthreads();
-        }
-        int o[ROWS];
-        unsigned int rk[ROWS];
-        [[maybe_unused]] unsigned int w[ROWS];  // DENSE: the row's bucket word
-#pragma unroll
-        for (int r = 0; r < ROWS; r++) {
-            const int j = r * SPG_TTHREADS + tid;
-            o[r] = -1;
-            if (!full && r0 + j >= a.n_rows) continue;
+        },
+        [&] { *tile_over = 0; },
+        [&](int j, [[maybe_unused]] unsigned int& w) -> int {  // DENSE: w = the row's bucket word
             const long long k = raw_k[j];
             const long long v = HAS_SUM ? raw_v[j] : 0;
             if constexpr (DENSE) {
                 // key and value offsets inside their windows (unsigned: below the base wraps to a large offset)
                 const unsigned long long d = (unsigned long long)k - (unsigned long long)a.kbase;
                 const unsigned long long e = HAS_SUM ? (unsigned long long)v - (unsigned long long)a.vbase : 0ull;
-                if ((d >> a.d_kb) != 0 || (e >> a.d_vb) != 0) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, k, (unsigned long long)v, 1ull); wide++; continue; }
+                if ((d >> a.d_kb) != 0 || (e >> a.d_vb) != 0) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, k, (unsigned long long)v, 1ull); wide++; return -1; }
                 const unsigned int x = spgd_scramble((unsigned int)d, a.d_kb, a.d_mul), q = __umulhi(x, a.d_gmagic);
-                o[r] = (int)(x - q * (unsigned int)G);
-                w[r] = q << a.d_vb | (unsigned int)e;
+                w = q << a.d_vb | (unsigned int)e;
+                return (int)(x - q * (unsigned int)G);
             } else {
                 // both values inside int32 <=> the high words of (x + 2^31) are zero; the key INT32_MIN (low word of k + 2^31 zero) is excluded
                 const unsigned long long kb = (unsigned long long)k + 0x80000000ull, vb = (unsigned long long)v + 0x80000000ull;
                 const bool narrow = ((kb | vb) >> 32) == 0 && (unsigned int)kb != 0u;
-                if (!narrow) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, k, (unsigned long long)v, 1ull); wide++; continue; }
-                o[r] = (int)spg_owner(spg_hash(k), G);
+                if (!narrow) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, k, (unsigned long long)v, 1ull); wide++; return -1; }
+                return (int)spg_owner(spg_hash(k), G);
             }
-            rk[r] = atomicAdd(&hist[o[r]], 1u);
-        }
-        __syncthreads();
-        unsigned long long my_gbase = 0;
-        unsigned int my_cnt = 0;
-        if (tid >= SPG_TTHREADS - G) { int ow = tid - (SPG_TTHREADS - G); my_cnt = hist[ow]; if (my_cnt) my_gbase = atomicAdd(&a.bucket_cnt[ow * SPG_CNT_STRIDE], (unsigned long long)my_cnt); }
-        if (tid < 32) {
-            unsigned int carry = 0;
-            for (int base = 0; base < G; base += 32) {
-                int j = base + tid;
-                unsigned int x = j < G ? hist[j] : 0u, inc = x;
-#pragma unroll
-                for (int d = 1; d < 32; d <<= 1) { unsigned int y = __shfl_up_sync(0xffffffffu, inc, d); if (tid >= d) inc += y; }
-                if (j < G) lbase[j] = carry + inc - x;
-                carry += __shfl_sync(0xffffffffu, inc, 31);
-            }
-            if (tid == 0) lbase[G] = carry;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int r = 0; r < ROWS; r++) {
-            if (o[r] < 0) continue;
-            const int j = r * SPG_TTHREADS + tid;
-            const unsigned int p = lbase[o[r]] + rk[r];
-            if constexpr (DENSE) stage[p] = w[r];
+        },
+        [&](unsigned int p, int j, int o, [[maybe_unused]] unsigned int w) {
+            if constexpr (DENSE) stage[p] = w;
             else stage[p] = make_int2((int)raw_k[j], HAS_SUM ? (int)raw_v[j] : 0);
-            stage_owner[p] = (unsigned char)o[r];
-        }
-        if (tid >= SPG_TTHREADS - G) {
-            const int ow = tid - (SPG_TTHREADS - G);
-            gbase[ow] = my_gbase - lbase[ow];
+            stage_owner[p] = (unsigned char)o;
+        },
+        [&](int ow, unsigned long long my_gbase, unsigned int my_cnt) {
+            const unsigned int* lbase = (const unsigned int*)(smem_n_raw + L::lbase);
             dptr[ow] = bucket + ((size_t)ow * a.bucket_cap + my_gbase - lbase[ow]);  // staged position p of this owner's run goes to dptr[ow][p]
             if (my_gbase + my_cnt > (unsigned long long)a.bucket_cap) *tile_over = 1;
-        }
-        __syncthreads();  // the raw tile is free from here on
-        if (tn < n_tiles) issue(tn);
-        const unsigned int n_tile = lbase[G];
-        if (*tile_over == 0) {  // every run fits (the common case): one owner byte, one address and one 8-byte store per row
-            unsigned int p = tid;
-            for (; p + SPG_TTHREADS < n_tile; p += 2 * SPG_TTHREADS) {
-                const unsigned int o0 = stage_owner[p], o1 = stage_owner[p + SPG_TTHREADS];
-                const Row r0v = stage[p], r1v = stage[p + SPG_TTHREADS];
-                dptr[o0][p] = r0v;
-                dptr[o1][p + SPG_TTHREADS] = r1v;
+        },
+        [&](unsigned int n_tile) {
+            if (*tile_over == 0) {  // every run fits (the common case): one owner byte, one address and one 8-byte store per row
+                unsigned int p = tid;
+                for (; p + SPG_TTHREADS < n_tile; p += 2 * SPG_TTHREADS) {
+                    const unsigned int o0 = stage_owner[p], o1 = stage_owner[p + SPG_TTHREADS];
+                    const Row r0v = stage[p], r1v = stage[p + SPG_TTHREADS];
+                    dptr[o0][p] = r0v;
+                    dptr[o1][p + SPG_TTHREADS] = r1v;
+                }
+                if (p < n_tile) dptr[stage_owner[p]][p] = stage[p];
+            } else {
+                for (unsigned int p = tid; p < n_tile; p += SPG_TTHREADS) {
+                    const unsigned int ow = stage_owner[p];
+                    const unsigned long long off = gbase[ow] + p;
+                    const Row row = stage[p];
+                    if (off < (unsigned long long)a.bucket_cap) bucket[(size_t)ow * a.bucket_cap + off] = row;
+                    else if constexpr (DENSE)  // bucket full (skew): the row back from its word and owner
+                        spg_direct_apply<HAS_SUM, HAS_CNT>(a, spgd_key(a, row >> a.d_vb, ow),
+                                                           (unsigned long long)a.vbase + (row & ((1u << a.d_vb) - 1u)), 1ull);
+                    else spg_direct_apply<HAS_SUM, HAS_CNT>(a, (long long)row.x, (unsigned long long)(long long)row.y, 1ull);  // bucket full (skew)
+                }
             }
-            if (p < n_tile) dptr[stage_owner[p]][p] = stage[p];
-        } else {
-            for (unsigned int p = tid; p < n_tile; p += SPG_TTHREADS) {
-                const unsigned int ow = stage_owner[p];
-                const unsigned long long off = gbase[ow] + p;
-                const Row row = stage[p];
-                if (off < (unsigned long long)a.bucket_cap) bucket[(size_t)ow * a.bucket_cap + off] = row;
-                else if constexpr (DENSE)  // bucket full (skew): the row back from its word and owner
-                    spg_direct_apply<HAS_SUM, HAS_CNT>(a, spgd_key(a, row >> a.d_vb, ow),
-                                                       (unsigned long long)a.vbase + (row & ((1u << a.d_vb) - 1u)), 1ull);
-                else spg_direct_apply<HAS_SUM, HAS_CNT>(a, (long long)row.x, (unsigned long long)(long long)row.y, 1ull);  // bucket full (skew)
-            }
-        }
-        __syncthreads();  // (tile_over is read above, cleared below)
-        for (int j = tid; j < G; j += SPG_TTHREADS) hist[j] = 0;
-        if (tid == 0) *tile_over = 0;
-        __syncthreads();
-    }
+            __syncthreads();  // every thread has read tile_over
+            if (tid == 0) *tile_over = 0;
+        });
     if (wide) atomicAdd((unsigned long long*)&a.counters[DENSE ? CTR_DENSE_WIDE : CTR_WIDE], (unsigned long long)wide);
 }
 
-// K2n's two candidate buckets of a key (two slots each) among the NB buckets of the shared table
-__device__ __forceinline__ void spgn_buckets(uint64_t h, unsigned int NB, unsigned int& b1, unsigned int& b2) {
-    b1 = __umulhi((unsigned int)(h >> 20), NB);
-    b2 = __umulhi(((unsigned int)h ^ (unsigned int)(h >> 44)) * 0x9E3779B1u, NB);
-    b2 = b2 == b1 ? (b1 + 1 == NB ? 0u : b1 + 1) : b2;
-}
-
-// K2n's rare per-row work, for one queued row.  !added: the key is not in its two buckets (first appearance: CAS into the emptier
-// bucket, else the stash, else the direct path), then the row is added.  added: the row was added already and the low sum word
+// K2n's rare per-row work, for one queued row.  !added: the key is not in its two buckets (spg_claim: a free candidate slot, else
+// the stash; else the direct path), then the row is added.  added: the row was added already and the low sum word
 // wrapped, so the high sum word takes the sign extension plus the carry: +1 for a value >= 0, -1 for a negative one.  Either way
 // a carry into the high sum word goes to the global table.
 // Out of line on purpose: inlined into the row loop it made K2n slower per 2^28 rows on an H100 (scratch/spg_harness.cu): at
@@ -220,35 +163,7 @@ __device__ __noinline__ void spgn_cold_row(const SpgArgs& a, int* skeys, unsigne
                                            bool added) {
     unsigned int old = 0;
     if (!added) {
-        const unsigned int NS = 2 * NB;
-        unsigned int b1, b2;
-        spgn_buckets(spg_hash((long long)key), NB, b1, b2);
-        const int2 c1 = *reinterpret_cast<const int2*>(skeys + 2 * b1);
-        const int2 c2 = *reinterpret_cast<const int2*>(skeys + 2 * b2);
-        const int f1 = (c1.x == SPGN_EMPTY) + (c1.y == SPGN_EMPTY), f2 = (c2.x == SPGN_EMPTY) + (c2.y == SPGN_EMPTY);
-        int s = c1.x == key ? (int)(2 * b1) : c1.y == key ? (int)(2 * b1 + 1) : c2.x == key ? (int)(2 * b2) : c2.y == key ? (int)(2 * b2 + 1) : -1;
-        if (s < 0 && f1 + f2 > 0) {
-            const unsigned int first = f2 > f1 ? b2 : b1, second = f2 > f1 ? b1 : b2;
-            const unsigned int cand[4] = {2 * first, 2 * first + 1, 2 * second, 2 * second + 1};
-#pragma unroll
-            for (int c = 0; c < 4 && s < 0; c++) {
-                const int prev = atomicCAS(&skeys[cand[c]], SPGN_EMPTY, key);
-                if (prev == SPGN_EMPTY || prev == key) s = (int)cand[c];
-            }
-        }
-        if (s < 0) {
-            unsigned int st = NS + ((unsigned int)(spg_hash((long long)key) >> 12) & (SPG_STASH - 1));
-            for (int probes = 0; probes < SPG_STASH && s < 0; probes++) {
-                int kk = skeys[st];
-                if (kk == SPGN_EMPTY) {
-                    const int prev = atomicCAS(&skeys[st], SPGN_EMPTY, key);
-                    if (prev == SPGN_EMPTY) { s = (int)st; break; }
-                    kk = prev;
-                }
-                if (kk == key) { s = (int)st; break; }
-                st = st + 1 == NS + SPG_STASH ? NS : st + 1;
-            }
-        }
+        const int s = spg_claim(skeys, 2 * NB, spg_hash((long long)key), key);
         if (s < 0) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, (long long)key, (unsigned long long)(long long)val, 1ull); return; }
         if (HAS_SUM) old = atomicAdd(&slo[s], (unsigned int)val);
         if (HAS_CNT) atomicAdd(&scnt[s], 1u);
@@ -277,10 +192,13 @@ __device__ unsigned long long spgn_phase_clocks[SPG_MAX_OWNERS * 4];  // per CTA
 #define SPGN_PHASE(i) do {} while (0)
 #endif
 
-// K2d's flush of one owner's table into the state's global table: K2n's flush (below) for a table whose slot s holds a group
-// when occupied(s), read by entry(s, key, sum, cnt).  (K2n keeps its own copy, whose code is tuned to its slot layout.)
+// The flush of K2n and K2d: one owner's n_slots-slot table, whose slot s holds a group when occupied(s), read by
+// entry(s, key, sum, cnt), into the state's global table.  First flush of a state (empty global table, a.reserve_tickets):
+// every occupied slot is a NEW group, and 10^6 per-insert tickets on one counter cost ~0.2 ms — the CTA takes the tickets of
+// all its slots with ONE atomic and returns the few it did not need (a key that sits in two slots, or that the direct path
+// inserted meanwhile).
 template <bool HAS_SUM, bool HAS_CNT, typename Occupied, typename Entry>
-__device__ __forceinline__ void spgd_flush(const SpgArgs& a, int n_slots, Occupied occupied, Entry entry) {
+__device__ __forceinline__ void spg_flush_ticketed(const SpgArgs& a, int n_slots, Occupied occupied, Entry entry) {
     const int tid = threadIdx.x;
     __shared__ unsigned int fl_occ, fl_dup;
     __shared__ int fl_reserved;
@@ -379,11 +297,9 @@ __device__ __forceinline__ void spgn_hash_aggregate(const SpgArgs& a) {
         for (int u = 0; u < U; u++) {
             const uint64_t h = spg_hash((long long)row[u].x);
             unsigned int b1, b2;
-            spgn_buckets(h, NB, b1, b2);
-            const int2 k1 = *reinterpret_cast<const int2*>(skeys + 2 * b1);
-            const int2 k2 = *reinterpret_cast<const int2*>(skeys + 2 * b2);
+            spg_buckets(h, NB, b1, b2);
             const int key = row[u].x;
-            sl[u] = k1.x == key ? (int)(2 * b1) : k1.y == key ? (int)(2 * b1 + 1) : k2.x == key ? (int)(2 * b2) : k2.y == key ? (int)(2 * b2 + 1) : -1;
+            sl[u] = spg_find(skeys, b1, b2, key);
             if (!FULL && key == SPGN_EMPTY) sl[u] = -2;  // padding lane (INT32_MIN never reaches a bucket)
             if (NP > 1 && __umulhi((unsigned int)(h >> 32), GP) - (unsigned int)me * NP != pass) sl[u] = -2;
         }
@@ -448,47 +364,12 @@ __device__ __forceinline__ void spgn_hash_aggregate(const SpgArgs& a) {
 #ifdef SPGN_SKIP_FLUSH
         continue;
 #endif
-        // flush.  First flush of a state (empty global table, a.reserve_tickets): every occupied slot is a NEW group, and 10^6
-        // per-insert tickets on one counter cost ~0.2 ms — the CTA takes the tickets of all its slots with ONE atomic and returns
-        // the few it did not need (a key that sits in two slots, or that the direct path inserted meanwhile).
-        __shared__ unsigned int fl_occ, fl_dup;
-        __shared__ int fl_reserved;
-        if (tid == 0) { fl_occ = 0; fl_dup = 0; fl_reserved = 0; }
-        __syncthreads();
-        if (a.reserve_tickets && a.group_limit >= 0) {
-            unsigned int mine = 0;
-            for (int s = tid; s < NT; s += SPG_THREADS) mine += skeys[s] != SPGN_EMPTY;
-            for (int d = 16; d; d >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, d);
-            if ((tid & 31) == 0 && mine) atomicAdd(&fl_occ, mine);
-            __syncthreads();
-            if (tid == 0 && fl_occ) {
-                const long long t = (long long)atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], (unsigned long long)fl_occ);
-                if (t + (long long)fl_occ <= a.group_limit) fl_reserved = 1;
-                else atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], (unsigned long long)(-(long long)fl_occ));  // no room: per-insert tickets
-            }
-            __syncthreads();
-        }
-        const bool reserved = fl_reserved != 0;
-        unsigned int dup = 0;
-        for (int s = tid; s < NT; s += SPG_THREADS) {
-            const int key = skeys[s];
-            if (key == SPGN_EMPTY) continue;
-            const unsigned long long sum = (unsigned long long)slo[s] - 0x80000000ull;  // remove the bias (wraps mod 2^64)
-            if (!reserved) { spg_direct_apply<HAS_SUM, HAS_CNT>(a, (long long)key, sum, (unsigned long long)scnt[s]); continue; }
-            // ticket already held: insert without the limit; a key that was there already gives its ticket back
-            bool inserted;
-            const uint64_t sl = spgn_insert_ticketed(a.tkeys, a.cap, (long long)key, inserted);
-            if (!inserted) dup++;
-            if (HAS_SUM && sum) atomicAdd(a.acc_sum + sl, sum);
-            if (HAS_CNT && scnt[s]) atomicAdd(a.acc_cnt + sl, (unsigned long long)scnt[s]);
-        }
-        if (reserved) {
-            for (int d = 16; d; d >>= 1) dup += __shfl_xor_sync(0xffffffffu, dup, d);
-            if ((tid & 31) == 0 && dup) atomicAdd(&fl_dup, dup);
-            __syncthreads();
-            if (tid == 0 && fl_dup) atomicAdd((unsigned long long*)&a.counters[CTR_GROUPS], (unsigned long long)(-(long long)fl_dup));
-        }
-        __syncthreads();
+        spg_flush_ticketed<HAS_SUM, HAS_CNT>(a, NT, [&](int s) { return skeys[s] != SPGN_EMPTY; },
+                                             [&](int s, long long& key, unsigned long long& sum, unsigned long long& cnt) {
+                                                 key = (long long)skeys[s];
+                                                 sum = (unsigned long long)slo[s] - 0x80000000ull;  // remove the bias (wraps mod 2^64)
+                                                 cnt = (unsigned long long)scnt[s];
+                                             });
         SPGN_PHASE(2);
     }
 }
@@ -543,7 +424,7 @@ __device__ __forceinline__ void spgd_aggregate(const SpgDenseArgs& a) {
     for (unsigned long long i = 4 * full + tid; i < n_in; i += SPG_THREADS) add(__ldcs(src + i));
     __syncthreads();
     const unsigned long long vbase = (unsigned long long)a.vbase;
-    spgd_flush<HAS_SUM, HAS_CNT>(a, NS, [&](int s) { return scnt[s] != 0; },
+    spg_flush_ticketed<HAS_SUM, HAS_CNT>(a, NS, [&](int s) { return scnt[s] != 0; },
                                  [&](int s, long long& key, unsigned long long& sum, unsigned long long& cnt) {
                                      cnt = (unsigned long long)scnt[s];
                                      key = spgd_key(a, (unsigned int)s, (unsigned int)me);

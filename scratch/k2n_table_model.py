@@ -1,6 +1,6 @@
 """Usage: python scratch/k2n_table_model.py GROUPS {balanced|firstfit} [r = scrambled keys]
 CPU model of K2n's shared table (spgn_aggregate_kernel, bodo_b200/csrc/spgn.cuh) at the flagship shape: the keys of
-bodo_b200/synth.py inserted one by one, in order of first appearance, with the kernel's spg_hash, spg_owner and spgn_buckets,
+bodo_b200/synth.py inserted one by one, in order of first appearance, with the kernel's spg_hash, spg_owner and spg_buckets,
 132 owners (the SMs of an H100), and K2n's bucket slots.  Prints which keys live in their second bucket and which miss both
 buckets (the stash, so the cold path on every one of their rows).  Sequential insertion: it does not model insert races."""
 import numpy as np, sys

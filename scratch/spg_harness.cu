@@ -76,7 +76,7 @@ int main(int argc, char** argv) {
     const int spgn_ns = ((int)(((size_t)max_smem - 256 - SPGN_QUEUE_BYTES) / 12) - SPG_STASH) & ~1;
     const int ns = narrow ? spgn_ns : spg_ns;
     const size_t k2_smem = narrow ? (size_t)(spgn_ns + SPG_STASH) * 12 + SPGN_QUEUE_BYTES + 16 : (size_t)(spg_ns + SPG_STASH) * 16 + 16;
-    const size_t k1_smem = narrow ? GroupbyState::spgn_part_smem() : GroupbyState::spg_tma_smem();
+    const size_t k1_smem = narrow ? SpgnK1Smem<false>::bytes : SpgK1Smem<false>::bytes;
     const int tile = narrow ? SPGN_TILE : SPG_TILE, k1_threads = SPG_TTHREADS, k1_ctas = narrow ? SPGN_CTAS : SPG_TCTAS;
     const int g1 = (int)std::min<int64_t>((int64_t)sms * k1_ctas, (rows + tile - 1) / tile);
     const int64_t group_cap = (int64_t)owners * (narrow ? spgn_ns * 7 / 10 : spg_ns * 7 / 10);
