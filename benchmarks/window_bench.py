@@ -1,0 +1,204 @@
+"""Streaming window operator (ranking functions OVER (PARTITION BY p ORDER BY o)), 1 x H100.
+
+    python benchmarks/window_bench.py [--rows 268435456] [--batch 16777216] [--reps 3] [--cases rn_rank_dense,all6,no_partition]
+
+Data, resident in HBM: `--rows` rows of an int64 partition key p in [0, 10^6), a float64 order key o (synth.device_fill's uniform
+doubles in [0, 1)) and an int64 row id r, fed in `--batch`-row batches.  Cases:
+  rn_rank_dense  row_number, rank, dense_rank OVER (PARTITION BY p ORDER BY o)
+  all6           all six functions (ntile(4)) over the same window
+  no_partition   row_number, rank, dense_rank OVER (ORDER BY o): one partition
+One step = init -> consume every batch (is_last on the last) -> produce -> delete, timed with CUDA events on the operator's stream;
+the median of `--reps` steps after one warm-up.  Every window step alternates with a full sort of the same keys and columns in
+the same process (sort_ms), so the window's cost above the sort is a measured difference (extra_ms).
+Reported per case: ms_per_step, rows_per_s, bytes (the sort's design bytes from benchmarks/sort_bench.py plus the window
+kernels' bytes, see window_bytes) and gbps as a share of the data sheet's 3350 GB/s, metric 9 (partitions), the card's name and
+power limit, and result_check: the output equals a torch recomputation (two stable torch.sorts, then diff, cummax and cumsum).
+The process exits non-zero on a mismatch.
+"""
+
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+from benchmarks.sort_bench import PEAK_GBPS, card, moved_bytes, plan  # noqa: E402
+
+FUNCS3 = [("rn", "row_number"), ("rk", "rank"), ("dr", "dense_rank")]
+FUNCS6 = FUNCS3 + [("pr", "percent_rank"), ("cd", "cume_dist"), ("nt", "ntile", 4)]
+
+
+def window_bytes(n, key_bytes, n_funcs, n_parts, n_peers):
+    """bounds: read each key column once (the row above is the one-row halo, in cache) and write a flag byte; ends: read the flags,
+    write D and the size at each partition start and the end at each peer-group start; eval: read the flags and those three
+    words once per partition / peer group, write 8 bytes per function and row."""
+    ends = 4 * (2 * n_parts + n_peers)
+    return int(n * (key_bytes + 1) + (n + ends) + (n + ends) + 8 * n * n_funcs)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rows", type=int, default=1 << 28)
+    ap.add_argument("--batch", type=int, default=1 << 24)
+    ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--cases", type=str, default="rn_rank_dense,all6,no_partition")
+    args = ap.parse_args()
+
+    import torch
+
+    from bodo_b200 import _lib, synth
+    from bodo_b200.streaming import sort as S
+    from bodo_b200.streaming import window as W
+    from bodo_b200.table import Column, Table
+
+    _lib.require_gpu()
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    stream = torch.cuda.current_stream(dev)
+    sp = stream.cuda_stream
+    n = args.rows
+    print(json.dumps({"card": card(), "torch_device": torch.cuda.get_device_name(dev)}), flush=True)
+
+    g = torch.Generator(device=dev).manual_seed(61)
+    pk = torch.randint(0, 10**6, (n,), generator=g, device=dev, dtype=torch.int64)
+    ok = torch.empty(n, dtype=torch.float64, device=dev)
+    synth.device_fill(None, ok, 0, 1, 62, sp)
+    rid = torch.arange(n, dtype=torch.int64, device=dev)
+    names = ["p", "o", "r"]
+    torch.cuda.synchronize(dev)
+    cases = {"rn_rank_dense": (["p"], FUNCS3), "all6": (["p"], FUNCS6), "no_partition": ([], FUNCS3)}
+
+    def batches():
+        for r0 in range(0, n, args.batch):
+            r1 = min(n, r0 + args.batch)
+            yield Table([Column(pk[r0:r1]), Column(ok[r0:r1]), Column(rid[r0:r1])], names), r1 == n
+
+    def window_step(part, funcs, keep=False):
+        st = W.init_window_state(-1, part, ["o"], True, "last", funcs, names, output_batch_size=1 << 30, device=0, stream=sp)
+        for t, last in batches():
+            W.window_build_consume_batch(st, t, last)
+        out, _ = W.window_produce_output_batch(st)
+        res = [torch.as_tensor(c.data, device=dev).clone() for c in out.columns] if keep else None
+        m9 = W.get_metric(st, 9)
+        W.delete_window_state(st)
+        return res, m9
+
+    def sort_step(part):
+        st = S.init_stream_sort_state(-1, None, 0, part + ["o"], [True] * (len(part) + 1), ["last"] * (len(part) + 1), names,
+                                      output_batch_size=1 << 30, device=0, stream=sp, full=True)
+        for t, last in batches():
+            S.sort_build_consume_batch(st, t, last)
+        S.produce_output_batch(st)
+        m = [S.get_metric(st, w) for w in range(9)]
+        S.delete_stream_sort_state(st)
+        return m
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        r = fn()
+        e1.record(stream)
+        torch.cuda.synchronize(dev)
+        return e0.elapsed_time(e1), r
+
+    def check(part, funcs, res):
+        """res: the window's output columns (p, o, r, then one per function).  Expected columns are built one at a time, so the
+        recomputation fits next to the inputs and the output on an 80 GB card."""
+        idx = torch.sort(ok, stable=True).indices
+        if part:
+            idx = idx[torch.sort(pk[idx], stable=True).indices]
+        if not (torch.equal(res[2], idx) and torch.equal(res[0], pk[idx]) and torch.equal(res[1].view(torch.int64), ok[idx].view(torch.int64))):
+            return "MISMATCH: an input column differs from the stable sort", 0, 0
+        i = torch.arange(n, device=dev, dtype=torch.int64)
+        ps = torch.zeros(n, dtype=torch.bool, device=dev)
+        ps[0] = True
+        if part:
+            ps[1:] = torch.diff(pk[idx]) != 0
+        qs = ps.clone()
+        qs[1:] |= torch.diff(ok[idx]) != 0
+        del idx
+        P = torch.cummax(torch.where(ps, i, 0), 0).values
+        Q = torch.cummax(torch.where(qs, i, 0), 0).values
+        D = torch.cumsum(qs.to(torch.int64), 0)
+        pid = torch.cumsum(ps.to(torch.int64), 0) - 1
+        s = torch.bincount(pid)[pid]
+        del pid
+        qid = torch.cumsum(qs.to(torch.int64), 0) - 1
+        qend = torch.cat([torch.nonzero(qs).flatten()[1:], torch.tensor([n], device=dev)])[qid]
+        del qid
+
+        def expected(f):
+            if f == "rn":
+                return i - P + 1
+            if f == "rk":
+                return Q - P + 1
+            if f == "dr":
+                return D - D[P] + 1
+            if f == "pr":
+                return torch.where(s == 1, 0.0, (Q - P).to(torch.float64) / torch.clamp(s - 1, min=1).to(torch.float64))
+            if f == "cd":
+                return (qend - P).to(torch.float64) / s.to(torch.float64)
+            pos = i - P
+            q, r = s // 4, s % 4
+            big = r * (q + 1)
+            return torch.where(pos < big, pos // (q + 1) + 1, r + (pos - big) // torch.clamp(q, min=1) + 1)
+
+        for j, f in enumerate(funcs):
+            if not torch.equal(res[3 + j].view(torch.int64), expected(f[0]).view(torch.int64)):
+                return f"MISMATCH: {f[0]}", 0, 0
+        return "ok", int(ps.sum()), int(qs.sum())
+
+    def free():
+        torch.cuda.empty_cache()
+        _lib.lib().b200_pool_trim(0, 0)
+
+    ok_all = True
+    for name in args.cases.split(","):
+        part, funcs = cases[name]
+        window_step(part, funcs)  # warm-up
+        sort_step(part)
+        wt, st_ = [], []
+        for _ in range(args.reps):
+            ms, (_, m9) = timed(lambda: window_step(part, funcs))
+            wt.append(ms)
+            ms, sm = timed(lambda: sort_step(part))
+            st_.append(ms)
+        w_ms, s_ms = sorted(wt)[len(wt) // 2], sorted(st_)[len(st_) // 2]
+        free()
+        # check
+        res, _ = window_step(part, funcs, keep=True)
+        free()
+        chk, n_parts, n_peers = check(part, funcs, res)
+        if chk == "ok" and m9 != n_parts:
+            chk = f"MISMATCH: metric 9 = {m9}, partitions = {n_parts}"
+        del res
+        free()
+        # design bytes: the sort of the keys (passes from the data, as sort_bench predicts them), then the window kernels
+        f64w = lambda x: torch.where(x < 0, x.view(torch.int64) ^ 0x7FFFFFFFFFFFFFFF, x.view(torch.int64))  # noqa: E731
+        words = [f64w(ok)] + ([pk ^ (-(2 ** 63))] if part else [])
+        kp = plan(torch, words, [8] * len(words), [True] + [False] * len(part), [0] * len(words))
+        del words
+        free()
+        key_bytes = 8 * (1 + len(part))
+        sort_bytes = moved_bytes(n, 24, 0, key_bytes, kp)
+        total = sort_bytes + window_bytes(n, key_bytes, len(funcs), n_parts, n_peers)
+        out = {"case": name, "rows": n, "batch": args.batch, "funcs": [f[1] for f in funcs], "ms_per_step": round(w_ms, 3),
+               "runs_ms": [round(x, 3) for x in wt], "sort_ms": round(s_ms, 3), "sort_runs_ms": [round(x, 3) for x in st_],
+               "extra_ms": round(w_ms - s_ms, 3), "extra_share_of_sort": round((w_ms - s_ms) / s_ms, 4),
+               "rows_per_s": round(n / (w_ms * 1e-3), 1), "bytes": total, "gbps": round(total / (w_ms * 1e-3) / 1e9, 1),
+               "share_of_3350_gbps": round(total / (w_ms * 1e-3) / 1e9 / PEAK_GBPS, 4), "metric9_partitions": m9,
+               "sort_passes_run_skipped": sm[7:9], "result_check": chk, "card": card()}
+        print(json.dumps(out), flush=True)
+        print(f"result_check: {chk}", flush=True)
+        ok_all &= chk == "ok"
+    if not ok_all:
+        sys.exit(3)
+
+
+if __name__ == "__main__":
+    main()

@@ -556,6 +556,9 @@ struct SortState {
     int64_t output_batch_size;
     int64_t rows_consumed = 0;  // metric 0
     bool finished = false;
+    // Output columns: the n_cols input columns, then any columns a form computes (numpy, of type sc.ctype[c]; the window's
+    // function columns).
+    int n_out_cols;
     // output views, set by the form's finish_rows: rows [0, n_out) of column c at out_data[c], for a nullable column one validity
     // byte per row at out_vb[c]
     char* out_data[SORT_MAX_COLS]{};
@@ -566,7 +569,7 @@ struct SortState {
 
     SortState(const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_keys, const int32_t* asc, const int32_t* na_last,
               int64_t obs, int dev, cudaStream_t st)
-        : device(dev), stream(st), output_batch_size(obs) {
+        : device(dev), stream(st), output_batch_size(obs), n_out_cols(n_arrs) {
         B200_REQUIRE(n_keys >= 1 && n_keys <= SORT_MAX_KEYS, "b200 sort: 1 to 4 sort keys");
         B200_REQUIRE(n_arrs >= n_keys && n_arrs <= SORT_MAX_COLS, "b200 sort: keys are the first n_keys of at most 32 columns");
         B200_REQUIRE(c_types && arr_types && asc && na_last, "b200 sort: null argument");
@@ -588,7 +591,7 @@ struct SortState {
     // At is_last: sort, then set n_out, out_data and out_vb.  Validity bytes the form allocates for its output go in vbytes (one
     // slot per column), which is freed once the bitmaps are packed.
     virtual void finish_rows(std::vector<DevBuf>& vbytes) = 0;
-    // Metric 0 to 8; a metric the form does not keep reads 0.
+    // Metric 0 to 9; a metric the form does not keep reads 0.
     virtual int64_t metric(int which) const = 0;
 
     int grid_for(int64_t items, int per_block) const { return (int)std::max<int64_t>(1, std::min<int64_t>((items + per_block - 1) / per_block, (int64_t)sms * 8)); }
@@ -616,7 +619,7 @@ struct SortState {
         const int64_t words = (n_out + 31) / 32 + 2;
         d_bitmaps.alloc((size_t)std::max(1, n_nullable) * words * 4);
         B200_CUDA(cudaMemsetAsync(d_bitmaps.p, 0, d_bitmaps.bytes, stream));
-        out_bitmap.assign(sc.n_cols, nullptr);
+        out_bitmap.assign(n_out_cols, nullptr);
         for (int c = 0, k = 0; c < sc.n_cols; c++) {
             if (arr_type[c] != ARR_NULLABLE) continue;
             out_bitmap[c] = d_bitmaps.as<uint32_t>() + (k++) * words;
@@ -633,8 +636,8 @@ struct SortState {
         int64_t bs = output_batch_size > 0 ? output_batch_size : n_out;
         if (bs % 32 != 0 && bs < n_out) bs = (bs + 31) & ~31ll;  // validity bitmaps are sliced at word granularity
         const int64_t rows = produce_output ? std::min(bs, n_out - out_cursor) : 0;
-        out->n_rows = rows; out->n_cols = sc.n_cols; out->device = device;
-        for (int c = 0; c < sc.n_cols; c++) {
+        out->n_rows = rows; out->n_cols = n_out_cols; out->device = device;
+        for (int c = 0; c < n_out_cols; c++) {
             b200_column& col = out->cols[c];
             col.data = out_data[c] + out_cursor * ctype_size(sc.ctype[c]);
             col.validity = out_bitmap[c] ? (uint8_t*)out_bitmap[c] + out_cursor / 8 : nullptr;
@@ -761,7 +764,7 @@ struct TopkState : SortState {
     }
 
     int64_t metric(int which) const override {
-        const int64_t m[9] = {rows_consumed, rows_admitted, reduce_steps, count_reads, filter_launches, admitted_after_cutoff, cap, 0, 0};
+        const int64_t m[10] = {rows_consumed, rows_admitted, reduce_steps, count_reads, filter_launches, admitted_after_cutoff, cap, 0, 0, 0};
         return m[which];
     }
 };
@@ -894,9 +897,287 @@ struct FullSortState : SortState {
     }
 
     int64_t metric(int which) const override {
-        const int64_t m[9] = {rows_consumed, 0, 0, 0, 0, 0, n_chunks * FS_CHUNK, passes_run, passes_skipped};
+        const int64_t m[10] = {rows_consumed, 0, 0, 0, 0, 0, n_chunks * FS_CHUNK, passes_run, passes_skipped, 0};
         return m[which];
     }
+};
+
+// ---- window (ranking functions OVER (PARTITION BY p ... ORDER BY o ...)): a full sort by (p ascending NA last, o), then scans
+// over the sorted key columns ----
+//
+//   window_bounds_kernel  one pass over the sorted key columns: position i starts a partition when a partition key's (NA class,
+//                         radix word) differs from position i - 1's, and a peer group when any key does (i = 0 starts both).
+//                         The row at i - 1 is the tile's one-row halo.  Writes one flag byte per position and per WN_TILE-row
+//                         tile the reduction of the scan values below, plus the tile's partition-start count.
+//   window_tiles_kernel   one block: the exclusive scan of the tile values, and the partition and peer-group totals.
+//   window_ends_kernel    scan of the flags seeded by the tile prefix: per position the partition start P (a max-scan of the
+//                         start positions), the peer start Q (a max-scan) and D, the number of peer starts up to the position.
+//                         The last row of a partition writes its size into slot P and the last row of a peer group its end into
+//                         slot Q; a partition's first row writes D into slot P.  No reverse scan is needed.
+//   window_eval_kernel    the same scan again, then every requested function per position.
+// Row positions are below 2^31 (the full sort's limit), so positions, sizes and counts are uint32.
+enum { WN_ROW_NUMBER = 0, WN_RANK = 1, WN_DENSE_RANK = 2, WN_PERCENT_RANK = 3, WN_CUME_DIST = 4, WN_NTILE = 5 };
+constexpr int WN_THREADS = 256, WN_WARPS = WN_THREADS / 32, WN_ITEMS = 8, WN_TILE = WN_THREADS * WN_ITEMS;
+constexpr uint8_t WN_PART = 1, WN_PEER = 2;  // a partition start is also a peer-group start
+
+// Scan value of a position: (partition start, peer start, peer starts so far) under (max, max, +).
+struct WnAgg { uint32_t p, q, d; };
+__device__ __forceinline__ WnAgg wn_combine(WnAgg a, WnAgg b) { return {max(a.p, b.p), max(a.q, b.q), a.d + b.d}; }
+
+struct WnArgs {
+    int64_t n;
+    int n_part, n_keys;
+    SortKey key[SORT_MAX_KEYS];
+    const char* data[SORT_MAX_KEYS];   // sorted key columns
+    const uint8_t* vb[SORT_MAX_KEYS];  // their validity bytes, nullptr for a numpy column
+    uint8_t* flags;
+    WnAgg* tile;          // per tile: its reduction (bounds), then its exclusive prefix (tiles)
+    uint32_t* tile_parts; // per tile: partition starts
+    uint32_t* totals;     // [0] partitions, [1] peer groups
+    uint32_t *psize, *pend, *pdense;  // slot P: partition size, slot Q: peer-group end, slot P: D at the partition start
+    int n_funcs;
+    int func[SORT_MAX_COLS];
+    int64_t farg[SORT_MAX_COLS];
+    void* out[SORT_MAX_COLS];
+};
+
+// Position of item k of thread (warp, lane) in tile t: items are warp-strided, so every load and store is coalesced.
+__device__ __forceinline__ int64_t wn_row(int64_t t, int k, int warp, int lane) {
+    return t * WN_TILE + (k * WN_WARPS + warp) * 32 + lane;
+}
+
+__device__ __forceinline__ bool wn_key_differs(const WnArgs& a, int j, int64_t i) {
+    const SortKey& k = a.key[j];
+    bool na0 = a.vb[j] && a.vb[j][i - 1] == 0, na1 = a.vb[j] && a.vb[j][i] == 0;
+    const uint64_t w0 = sort_word(k, load_bits(a.data[j], k.size, i - 1), na0);
+    const uint64_t w1 = sort_word(k, load_bits(a.data[j], k.size, i), na1);
+    return na0 != na1 || w0 != w1;
+}
+
+__global__ void __launch_bounds__(WN_THREADS) window_bounds_kernel(const __grid_constant__ WnArgs a) {
+    __shared__ WnAgg s_agg[WN_WARPS];
+    __shared__ uint32_t s_parts[WN_WARPS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t t = blockIdx.x;
+    WnAgg acc{0, 0, 0};
+    uint32_t parts = 0;
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        if (i >= a.n) break;
+        uint8_t f = WN_PART | WN_PEER;
+        if (i > 0) {
+            f = 0;
+            for (int j = 0; j < a.n_keys && !f; j++)
+                if (wn_key_differs(a, j, i)) f = j < a.n_part ? (WN_PART | WN_PEER) : WN_PEER;
+        }
+        a.flags[i] = f;
+        if (f & WN_PART) { acc.p = (uint32_t)i; parts++; }
+        if (f & WN_PEER) { acc.q = (uint32_t)i; acc.d++; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        acc = wn_combine(acc, WnAgg{__shfl_xor_sync(0xffffffffu, acc.p, o), __shfl_xor_sync(0xffffffffu, acc.q, o),
+                                    __shfl_xor_sync(0xffffffffu, acc.d, o)});
+        parts += __shfl_xor_sync(0xffffffffu, parts, o);
+    }
+    if (lane == 0) { s_agg[warp] = acc; s_parts[warp] = parts; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < WN_WARPS; w++) { acc = wn_combine(acc, s_agg[w]); parts += s_parts[w]; }
+        a.tile[t] = acc;
+        a.tile_parts[t] = parts;
+    }
+}
+
+// One block of 1024 threads; thread x scans a contiguous run of tiles.
+__global__ void __launch_bounds__(1024) window_tiles_kernel(const __grid_constant__ WnArgs a, int64_t n_tiles) {
+    __shared__ WnAgg s_agg[32];
+    __shared__ uint32_t s_parts[32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t per = (n_tiles + 1023) / 1024, t0 = threadIdx.x * per, t1 = min(n_tiles, t0 + per);
+    WnAgg acc{0, 0, 0};
+    uint32_t parts = 0;
+    for (int64_t t = t0; t < t1; t++) { acc = wn_combine(acc, a.tile[t]); parts += a.tile_parts[t]; }
+    WnAgg inc = acc;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const WnAgg y{__shfl_up_sync(0xffffffffu, inc.p, o), __shfl_up_sync(0xffffffffu, inc.q, o), __shfl_up_sync(0xffffffffu, inc.d, o)};
+        if (lane >= o) inc = wn_combine(y, inc);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) parts += __shfl_xor_sync(0xffffffffu, parts, o);
+    if (lane == 31) s_agg[warp] = inc;
+    if (lane == 0) s_parts[warp] = parts;
+    __syncthreads();
+    WnAgg run{0, 0, 0};
+    for (int w = 0; w < warp; w++) run = wn_combine(run, s_agg[w]);
+    // exclusive prefix of this thread's first tile: the earlier warps, then the earlier lanes of this warp
+    WnAgg ex{__shfl_up_sync(0xffffffffu, inc.p, 1), __shfl_up_sync(0xffffffffu, inc.q, 1), __shfl_up_sync(0xffffffffu, inc.d, 1)};
+    if (lane > 0) run = wn_combine(run, ex);
+    for (int64_t t = t0; t < t1; t++) {
+        const WnAgg v = a.tile[t];
+        a.tile[t] = run;
+        run = wn_combine(run, v);
+    }
+    if (threadIdx.x == 1023) {
+        uint32_t total_parts = 0;
+        for (int w = 0; w < 32; w++) total_parts += s_parts[w];
+        a.totals[0] = total_parts;
+        a.totals[1] = run.d;
+    }
+}
+
+// Inclusive scan values of this thread's WN_ITEMS positions of tile t, seeded by the tile's exclusive prefix.
+__device__ __forceinline__ void wn_scan_tile(const WnArgs& a, int64_t t, uint8_t (&f)[WN_ITEMS], WnAgg (&v)[WN_ITEMS]) {
+    __shared__ WnAgg s_seg[WN_ITEMS * WN_WARPS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        f[k] = i < a.n ? a.flags[i] : 0;
+        v[k] = WnAgg{(f[k] & WN_PART) ? (uint32_t)i : 0u, (f[k] & WN_PEER) ? (uint32_t)i : 0u, (f[k] & WN_PEER) ? 1u : 0u};
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const WnAgg y{__shfl_up_sync(0xffffffffu, v[k].p, o), __shfl_up_sync(0xffffffffu, v[k].q, o),
+                          __shfl_up_sync(0xffffffffu, v[k].d, o)};
+            if (lane >= o) v[k] = wn_combine(y, v[k]);
+        }
+        if (lane == 31) s_seg[k * WN_WARPS + warp] = v[k];
+    }
+    __syncthreads();
+    if (warp == 0) {  // exclusive scan of the 64 (item, warp) segments in row order, seeded by the tile prefix: 2 per lane
+        static_assert(WN_ITEMS * WN_WARPS == 64, "two segments per lane");
+        const WnAgg x0 = s_seg[2 * lane], x1 = s_seg[2 * lane + 1];
+        const WnAgg pair = wn_combine(x0, x1);
+        WnAgg inc = pair;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const WnAgg y{__shfl_up_sync(0xffffffffu, inc.p, o), __shfl_up_sync(0xffffffffu, inc.q, o), __shfl_up_sync(0xffffffffu, inc.d, o)};
+            if (lane >= o) inc = wn_combine(y, inc);
+        }
+        WnAgg ex{__shfl_up_sync(0xffffffffu, inc.p, 1), __shfl_up_sync(0xffffffffu, inc.q, 1), __shfl_up_sync(0xffffffffu, inc.d, 1)};
+        WnAgg base = a.tile[t];
+        if (lane > 0) base = wn_combine(base, ex);
+        s_seg[2 * lane] = base;
+        s_seg[2 * lane + 1] = wn_combine(base, x0);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) v[k] = wn_combine(s_seg[k * WN_WARPS + warp], v[k]);
+}
+
+__global__ void __launch_bounds__(WN_THREADS) window_ends_kernel(const __grid_constant__ WnArgs a) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t t = blockIdx.x;
+    uint8_t f[WN_ITEMS];
+    WnAgg v[WN_ITEMS];
+    wn_scan_tile(a, t, f, v);
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        if (i >= a.n) break;
+        const uint8_t next = i + 1 < a.n ? a.flags[i + 1] : (WN_PART | WN_PEER);
+        if (f[k] & WN_PART) a.pdense[i] = v[k].d;
+        if (next & WN_PART) a.psize[v[k].p] = (uint32_t)(i + 1) - v[k].p;
+        if (next & WN_PEER) a.pend[v[k].q] = (uint32_t)(i + 1);
+    }
+}
+
+__global__ void __launch_bounds__(WN_THREADS) window_eval_kernel(const __grid_constant__ WnArgs a) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t t = blockIdx.x;
+    uint8_t f[WN_ITEMS];
+    WnAgg v[WN_ITEMS];
+    wn_scan_tile(a, t, f, v);
+    // The divisions below have out-of-line slow paths: holding every item's scan values in registers across them spills, so
+    // each thread parks its own values in shared memory and the item loop is not unrolled.
+    __shared__ WnAgg s_v[WN_ITEMS][WN_THREADS];
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) s_v[k][threadIdx.x] = v[k];
+#pragma unroll 1
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        if (i >= a.n) break;
+        const WnAgg vk = s_v[k][threadIdx.x];
+        const uint32_t P = vk.p, s = a.psize[P], pos = (uint32_t)i - P, rank = vk.q - P + 1;
+        for (int fn = 0; fn < a.n_funcs; fn++) {
+            int64_t r = 0;
+            double x = 0.0;
+            switch (a.func[fn]) {
+                case WN_ROW_NUMBER: r = pos + 1; break;
+                case WN_RANK: r = rank; break;
+                case WN_DENSE_RANK: r = vk.d - a.pdense[P] + 1; break;
+                case WN_PERCENT_RANK: x = s == 1 ? 0.0 : (double)(rank - 1) / (double)(s - 1); break;
+                case WN_CUME_DIST: x = (double)(a.pend[vk.q] - P) / (double)s; break;
+                default: {  // WN_NTILE: the first s % n buckets hold s / n + 1 rows, the others s / n.  n > s gives buckets 1..s, as
+                            // n = s does, so n is capped at s and the arithmetic stays in 32 bits.
+                    const uint32_t nb = (uint32_t)min(a.farg[fn], (int64_t)s), q = s / nb, rem = s % nb, big = rem * (q + 1);
+                    r = pos < big ? pos / (q + 1) + 1 : rem + (pos - big) / q + 1;
+                }
+            }
+            if (a.func[fn] == WN_PERCENT_RANK || a.func[fn] == WN_CUME_DIST) ((double*)a.out[fn])[i] = x;
+            else ((int64_t*)a.out[fn])[i] = r;
+        }
+    }
+}
+
+// ROW_NUMBER / RANK / DENSE_RANK / PERCENT_RANK / CUME_DIST / NTILE over (PARTITION BY the first n_part keys ORDER BY the rest).
+// The output is the full sort's, plus one numpy column per function after the input columns.
+struct WindowState : FullSortState {
+    int n_part, n_funcs;
+    int func[SORT_MAX_COLS];
+    int64_t farg[SORT_MAX_COLS];
+    std::vector<DevBuf> fout;
+    int64_t n_partitions = 0;  // metric 9
+
+    WindowState(const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_part_, int n_keys, const int32_t* asc,
+                const int32_t* na_last, const int32_t* funcs, const int64_t* fargs, int n_funcs_, int64_t obs, int dev, cudaStream_t st)
+        : FullSortState(c_types, arr_types, n_arrs, n_keys, asc, na_last, obs, dev, st), n_part(n_part_), n_funcs(n_funcs_) {
+        for (int f = 0; f < n_funcs; f++) {
+            func[f] = funcs[f]; farg[f] = fargs ? fargs[f] : 0;
+            const bool real = func[f] == WN_PERCENT_RANK || func[f] == WN_CUME_DIST;
+            sc.ctype[n_out_cols] = real ? CT_FLOAT64 : CT_INT64;
+            arr_type[n_out_cols++] = ARR_NUMPY;
+        }
+    }
+
+    // The sort first (its chunks and pair buffers are freed on return), then the window scratch and function columns.
+    void finish_rows(std::vector<DevBuf>& vbytes) override {
+        FullSortState::finish_rows(vbytes);
+        const int64_t n = n_out;
+        fout.resize(n_funcs);
+        WnArgs a{};
+        a.n = n; a.n_part = n_part; a.n_keys = sc.n_keys; a.n_funcs = n_funcs;
+        for (int j = 0; j < sc.n_keys; j++) { a.key[j] = sc.key[j]; a.data[j] = out_data[j]; a.vb[j] = out_vb[j]; }
+        for (int f = 0; f < n_funcs; f++) {
+            fout[f].alloc((size_t)n * 8);
+            a.out[f] = out_data[sc.n_cols + f] = fout[f].as<char>();
+            a.func[f] = func[f]; a.farg[f] = farg[f];
+        }
+        if (n == 0) return;
+        const int64_t n_tiles = (n + WN_TILE - 1) / WN_TILE;
+        DevBuf flags, tiles, tile_parts, totals, ends;
+        flags.alloc((size_t)n);
+        tiles.alloc((size_t)n_tiles * sizeof(WnAgg));
+        tile_parts.alloc((size_t)n_tiles * 4);
+        totals.alloc(8);
+        ends.alloc((size_t)n * 12);
+        a.flags = flags.as<uint8_t>(); a.tile = tiles.as<WnAgg>(); a.tile_parts = tile_parts.as<uint32_t>(); a.totals = totals.as<uint32_t>();
+        a.psize = ends.as<uint32_t>(); a.pend = a.psize + n; a.pdense = a.pend + n;
+        window_bounds_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
+        window_tiles_kernel<<<1, 1024, 0, stream>>>(a, n_tiles);
+        window_ends_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
+        window_eval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
+        B200_CUDA(cudaGetLastError());
+        auto* h = (uint32_t*)pinned_acquire(8);
+        B200_CUDA(cudaMemcpyAsync(h, totals.p, 8, cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaStreamSynchronize(stream));
+        n_partitions = h[0];
+        pinned_release(h, 8);
+    }
+
+    int64_t metric(int which) const override { return which == 9 ? n_partitions : FullSortState::metric(which); }
 };
 
 // A new state from make() once the device is known to exist; nullptr and the last error on failure.
@@ -938,6 +1219,32 @@ void* b200_sort_state_init_full(int64_t operator_id, const int8_t* c_types, cons
     });
 }
 
+void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs, int32_t n_partition_keys,
+                             int32_t n_order_keys, const int32_t* order_ascending, const int32_t* order_na_last, const int32_t* funcs,
+                             const int64_t* func_args, int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream) {
+    (void)operator_id;
+    return b200::sort_state_new(device, [&]() -> SortState* {
+        const int np = n_partition_keys, no = n_order_keys;
+        B200_REQUIRE(np >= 0 && no >= 0 && np + no >= 1 && np + no <= b200::SORT_MAX_KEYS,
+                     "b200 window: 1 to 4 keys (PARTITION BY plus ORDER BY), neither count negative");
+        B200_REQUIRE(no == 0 || (order_ascending && order_na_last), "b200 window: null ORDER BY direction or NA placement");
+        B200_REQUIRE(funcs && n_funcs >= 1, "b200 window: at least one function");
+        B200_REQUIRE(n_arrs >= np + no && n_arrs + n_funcs <= b200::SORT_MAX_COLS,
+                     "b200 window: the keys are the first n_partition_keys + n_order_keys columns, and input plus function columns are at most 32");
+        for (int f = 0; f < n_funcs; f++) {
+            B200_REQUIRE(funcs[f] >= b200::WN_ROW_NUMBER && funcs[f] <= b200::WN_NTILE, "b200 window: unknown function code");
+            if (funcs[f] == b200::WN_NTILE) B200_REQUIRE(func_args && func_args[f] >= 1, "b200 window: ntile needs n >= 1");
+        }
+        int32_t asc[b200::SORT_MAX_KEYS], na_last[b200::SORT_MAX_KEYS];
+        for (int j = 0; j < np + no; j++) {  // PARTITION BY keys: ascending, NA last
+            asc[j] = j < np ? 1 : order_ascending[j - np];
+            na_last[j] = j < np ? 1 : order_na_last[j - np];
+        }
+        return new b200::WindowState(c_types, arr_types, n_arrs, np, np + no, asc, na_last, funcs, func_args, n_funcs, output_batch_size,
+                                     device, (cudaStream_t)stream);
+    });
+}
+
 int b200_sort_build_consume_batch(void* state, const b200_table* in_table, int32_t is_last, int32_t* request_input) {
     try {
         B200_REQUIRE(state && in_table, "b200 sort: null state or table");
@@ -963,7 +1270,7 @@ void b200_delete_sort_state(void* state) {
 }
 
 int64_t b200_sort_get_metric(void* state, int32_t which) {
-    return which >= 0 && which <= 8 ? ((SortState*)state)->metric(which) : -1;
+    return which >= 0 && which <= 9 ? ((SortState*)state)->metric(which) : -1;
 }
 
 }  // extern "C"

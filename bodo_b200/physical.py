@@ -7,6 +7,7 @@ bodo/pandas/physical/operator.h:46-50,247-458; aggregate.h:65-365; join.h:58-744
     PhysicalJoin      : sink for the build side, ProcessBatch for the probe side
     PhysicalSort      : ORDER BY ... LIMIT ... OFFSET, or ORDER BY without LIMIT (full=True); sink of one pipeline and source
                         of the next
+    PhysicalWindow    : ranking window functions OVER (PARTITION BY ... ORDER BY ...); sink of one pipeline and source of the next
     Pipeline          : while not finished: batch = source.ProduceBatch(); ... sink.ConsumeBatch(batch)
 
 plus two helpers that run those pipelines over pandas frames the way bodo.pandas does for
@@ -23,6 +24,7 @@ from typing import Iterable, Sequence
 from .streaming import groupby as G
 from .streaming import join as J
 from .streaming import sort as S
+from .streaming import window as W
 from .table import Table
 
 STREAMING_BATCH_SIZE = 32768  # bodo/libs/streaming/_shuffle.h:27-31
@@ -311,6 +313,34 @@ class PhysicalSort:
             S.delete_stream_sort_state(self.state)
 
 
+class PhysicalWindow:
+    """Window sink/source: every input row once, in the stable order by (partition_by ascending NA last, order_by), with one
+    column per function after the input columns.  funcs: [(out_name, fname)] or (out_name, "ntile", n), fname one of
+    streaming.window.FUNCS; ascending / na_position: one value or one per ORDER BY key.  The column names are taken from the first
+    batch."""
+
+    def __init__(self, partition_by, order_by, funcs, ascending=True, na_position="last", parallel: bool = False, **kw):
+        self.args = (partition_by, order_by, ascending, na_position, list(funcs), parallel)
+        self.kw = kw
+        self.state = None
+
+    def ConsumeBatch(self, batch: Table, prev: OperatorResult) -> OperatorResult:
+        if self.state is None:
+            part, order, asc, nap, funcs, parallel = self.args
+            self.state = W.init_window_state(-1, part, order, asc, nap, funcs, batch.names, parallel, **self.kw)
+        is_last = prev == OperatorResult.FINISHED
+        W.window_build_consume_batch(self.state, batch, is_last)
+        return OperatorResult.FINISHED if is_last else OperatorResult.NEED_MORE_INPUT
+
+    def ProduceBatch(self):
+        out, last = W.window_produce_output_batch(self.state, True)
+        return out, (OperatorResult.FINISHED if last else OperatorResult.HAVE_MORE_OUTPUT)
+
+    def Finalize(self):
+        if self.state is not None:
+            W.delete_window_state(self.state)
+
+
 class ResultCollector:
     """PhysicalResultCollector: concatenates output batches into one pandas frame."""
 
@@ -401,6 +431,18 @@ def sort_values(df, by, ascending=True, na_position="last", batch_size: int = ST
     """df.sort_values(by, ascending=..., na_position=..., kind="stable").reset_index(drop=True) through PhysicalSort(full=True).
     ascending and na_position may be one value or one per key.  Returns a pandas DataFrame with a fresh index."""
     op = PhysicalSort(by, ascending, na_position, full=True, **kw)
+    run_pipeline(PhysicalReadPandas(df, batch_size), [], op)
+    coll = ResultCollector()
+    run_pipeline(op, [], coll)
+    op.Finalize()
+    return coll.result()
+
+
+def window(df, partition_by, order_by, funcs, ascending=True, na_position="last", batch_size: int = STREAMING_BATCH_SIZE, **kw):
+    """Ranking window functions OVER (PARTITION BY partition_by ORDER BY order_by) through PhysicalWindow.  Returns a pandas
+    DataFrame in the operator's output order (stably sorted by partition keys, then order keys) with a fresh index: df's columns,
+    then one column per function."""
+    op = PhysicalWindow(partition_by, order_by, funcs, ascending, na_position, **kw)
     run_pipeline(PhysicalReadPandas(df, batch_size), [], op)
     coll = ResultCollector()
     run_pipeline(op, [], coll)

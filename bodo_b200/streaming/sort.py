@@ -72,6 +72,7 @@ class SortState:
         self.key_inds = [col_names.index(k) for k in by]
         self.phys = self.key_inds + [i for i in range(len(col_names)) if i not in self.key_inds]
         self.out_order = [self.phys.index(i) for i in range(len(col_names))]
+        self.out_names = [col_names[i] for i in self.phys]  # the produced columns, in physical order
         self.parallel = bool(parallel)
         self.output_batch_size = int(output_batch_size)
         self.device = device
@@ -97,13 +98,16 @@ class SortState:
         nal = ffi.new("int32_t[]", [int(x) for x in self.na_last])
         lim = self.limit if limit is None else limit
         off = self.offset if offset is None else offset
+        self.handle = self._new_handle(L, c_types, a_types, len(cols), asc, nal, lim, off)
+
+    def _new_handle(self, L, c_types, a_types, n_cols, asc, nal, limit, offset):
         if self.full:
-            h = L.b200_sort_state_init_full(self.operator_id, c_types, a_types, len(cols), len(self.by), asc, nal, self.output_batch_size,
+            h = L.b200_sort_state_init_full(self.operator_id, c_types, a_types, n_cols, len(self.by), asc, nal, self.output_batch_size,
                                             self.device, ffi.cast("void*", self.stream))
         else:
-            h = L.b200_sort_state_init(self.operator_id, lim, off, c_types, a_types, len(cols), len(self.by), asc, nal,
+            h = L.b200_sort_state_init(self.operator_id, limit, offset, c_types, a_types, n_cols, len(self.by), asc, nal,
                                        self.output_batch_size, self.device, ffi.cast("void*", self.stream))
-        self.handle = _lib.check_ptr(h, "init_stream_sort_state")
+        return _lib.check_ptr(h, "init_stream_sort_state")
 
     def _consume(self, table: Table, is_last: bool):
         L = _lib.lib()
@@ -115,13 +119,13 @@ class SortState:
 
     def _produce(self, produce_output: bool):
         L = _lib.lib()
-        ncols = len(self.phys)
+        ncols = len(self.out_names)
         self._out_cols = ffi.new("b200_column[]", ncols)
         self._out_tab = ffi.new("b200_table*")
         self._out_tab.cols = self._out_cols
         last = ffi.new("int32_t*")
         _lib.check(L.b200_sort_produce_output_batch(self.handle, self._out_tab, last, int(bool(produce_output))), "sort produce_output_batch")
-        phys = table_from_ctable(self._out_tab, ncols, [self.col_names[i] for i in self.phys], owner=self)
+        phys = table_from_ctable(self._out_tab, ncols, self.out_names, owner=self)
         return phys.select(self.out_order), bool(last[0])
 
     def _gather_and_reduce(self):
@@ -207,5 +211,6 @@ def delete_stream_sort_state(state: SortState) -> None:
 def get_metric(state: SortState, which: int) -> int:
     """0 rows consumed, 1 rows admitted as candidates, 2 reduce steps, 3 host reads of the candidate count, 4 filter launches,
     5 rows admitted while a cutoff existed, 6 store capacity in rows, 7 digit passes run (full sort), 8 digit passes skipped
-    because their digit is constant over all rows (full sort).  Metrics 1-5 read 0 in a full sort, 7 and 8 in a top-k."""
+    because their digit is constant over all rows (full sort), 9 partitions (window, streaming/window.py).  Metrics 1-5 read 0 in
+    a full sort, 7-9 in a top-k and 9 in a full sort."""
     return int(_lib.lib().b200_sort_get_metric(state.handle, which))

@@ -228,12 +228,34 @@ void* b200_sort_state_init_full(int64_t operator_id, const int8_t* c_types, cons
                                 const int32_t* ascending, const int32_t* na_last, int64_t output_batch_size, int32_t device,
                                 void* stream);
 
+/* Ranking window functions, ROW_NUMBER / RANK / DENSE_RANK / PERCENT_RANK / CUME_DIST / NTILE(n) OVER (PARTITION BY p ORDER BY o),
+ * as a third form of the sort state (the reference plans these through its window / MRNF arguments, which the groupby ABI above
+ * drops).  The keys are the first n_partition_keys + n_order_keys (0 <= each, 1 <= sum <= 4) of the n_arrs columns, partition keys
+ * first; key columns are distinct and of the sort's key types.  PARTITION BY keys sort ascending with NA last; ORDER BY key j takes
+ * order_ascending[j] and order_na_last[j].  Two cells of a key are equal when both are NA (a float NaN is NA) or both are valid with
+ * equal radix words (-0.0 equals 0.0).  Rows with equal partition keys are a partition; rows of a partition with equal order keys
+ * are peers (without ORDER BY every row of a partition is a peer of every other).
+ * funcs[i] uses codes local to this library: 0 row_number, 1 rank, 2 dense_rank, 3 percent_rank, 4 cume_dist, 5 ntile;
+ * func_args[i] is ntile's n (>= 1) and is ignored for the others (func_args may be NULL without an ntile).  With s the partition
+ * size and k the row's 0-based position in it: row_number = k + 1 (ties in arrival order); rank = 1 + rows before the row's first
+ * peer; dense_rank = 1 + peer groups before the row's; percent_rank = (rank - 1) / (s - 1), 0.0 when s = 1; cume_dist = rows up to
+ * and including the row's last peer / s; ntile: with q = s / n and r = s % n the first r buckets hold q + 1 rows and the others q
+ * (buckets 1..s when n > s).  row_number, rank, dense_rank and ntile are INT64, percent_rank and cume_dist FLOAT64 (one IEEE double
+ * division of the two integers); all numpy arrays.  The output is every input row once, in the stable sort's order by (partition
+ * keys, order keys, arrival): the n_arrs input columns, then one column per function, so `out->cols` of a produce call holds
+ * n_arrs + n_funcs descriptors (at most 32).  At most 2^31 rows, as the full sort.  The build-consume, produce, delete and metric
+ * entries below serve this form too; metric 9 is the number of partitions. */
+void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                             int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                             const int32_t* order_na_last, const int32_t* funcs, const int64_t* func_args, int32_t n_funcs,
+                             int64_t output_batch_size, int32_t device, void* stream);
+
 /* The build-consume entry of _sort.cpp: filters a DEVICE-resident batch (same schema as the state) against the current cutoff on
  * the device (full sort: appends it to the chunk store); on is_last reduces to the final rows (full sort: sorts every row).
  * Returns 1 after is_last, 0 otherwise, < 0 on error; *request_input = 1. */
 int b200_sort_build_consume_batch(void* state, const b200_table* in_table, int32_t is_last, int32_t* request_input);
 
-/* The produce-output entry of _sort.cpp: fills `out` (out->cols with room for n_arrs descriptors) with library-owned device
+/* The produce-output entry of _sort.cpp: fills `out` (out->cols with room for n_arrs descriptors, n_arrs + n_funcs for a window) with library-owned device
  * columns of the next <= output_batch_size result rows, in order; valid until delete.  Sets *out_is_last. */
 int b200_sort_produce_output_batch(void* state, b200_table* out, int32_t* out_is_last, int32_t produce_output);
 
@@ -242,8 +264,8 @@ void b200_delete_sort_state(void* state);
 
 /* Metrics: 0 rows consumed, 1 rows admitted as candidates, 2 reduce steps, 3 host reads of the candidate count, 4 filter
  * launches, 5 rows admitted while a cutoff existed, 6 store capacity in rows, 7 digit passes run (full sort), 8 digit passes
- * skipped because their digit is constant over all rows (full sort).  A full sort reads 0 for metrics 1-5; top-k reads 0 for
- * 7 and 8.  Full-sort passes: per key one per byte of its width, plus one NA-class pass for a nullable or float key. */
+ * skipped because their digit is constant over all rows (full sort), 9 partitions (window).  A full sort or window reads 0 for
+ * metrics 1-5; top-k reads 0 for 7 to 9 and a full sort for 9.  Full-sort passes: per key one per byte of its width, plus one NA-class pass for a nullable or float key. */
 int64_t b200_sort_get_metric(void* state, int32_t which);
 
 /* ---- row -> rank shuffle (reference: bodo/libs/_shuffle.cpp) ---- */
