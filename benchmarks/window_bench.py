@@ -7,6 +7,11 @@ doubles in [0, 1)) and an int64 row id r, fed in `--batch`-row batches.  Cases:
   rn_rank_dense  row_number, rank, dense_rank OVER (PARTITION BY p ORDER BY o)
   all6           all six functions (ntile(4)) over the same window
   no_partition   row_number, rank, dense_rank OVER (ORDER BY o): one partition
+  running        SUM(r) ROWS, MAX(r) RANGE and COUNT(*) over the partition, OVER (PARTITION BY p ORDER BY o)
+  partition_aggs SUM / MEAN / MIN / MAX(o) over the whole partition
+  lag_lead       LAG(r, 1) and LEAD(o, 1, 0.0)
+The value cases (the last three) also alternate with rn_rank_dense (rn_rank_dense_ms), so their cost above the ranking kernels
+is measured too; their result check covers the validity of the nullable columns.
 One step = init -> consume every batch (is_last on the last) -> produce -> delete, timed with CUDA events on the operator's stream;
 the median of `--reps` steps after one warm-up.  Every window step alternates with a full sort of the same keys and columns in
 the same process (sort_ms), so the window's cost above the sort is a measured difference (extra_ms).
@@ -31,6 +36,10 @@ from benchmarks.sort_bench import PEAK_GBPS, card, moved_bytes, plan  # noqa: E4
 
 FUNCS3 = [("rn", "row_number"), ("rk", "rank"), ("dr", "dense_rank")]
 FUNCS6 = FUNCS3 + [("pr", "percent_rank"), ("cd", "cume_dist"), ("nt", "ntile", 4)]
+RUNNING = [("sr", "sum", "r", "rows"), ("mr", "max", "r", "range"), ("cz", "count", None, "partition")]
+PARTITION_AGGS = [(f"{f}o", f, "o", "partition") for f in ("sum", "mean", "min", "max")]
+LAG_LEAD = [("lg", "lag", "r", 1), ("ld", "lead", "o", 1, 0.0)]
+VALUE_CASES = ("running", "partition_aggs", "lag_lead")
 
 
 def window_bytes(n, key_bytes, n_funcs, n_parts, n_peers):
@@ -39,6 +48,31 @@ def window_bytes(n, key_bytes, n_funcs, n_parts, n_peers):
     words once per partition / peer group, write 8 bytes per function and row."""
     ends = 4 * (2 * n_parts + n_peers)
     return int(n * (key_bytes + 1) + (n + ends) + (n + ends) + 8 * n * n_funcs)
+
+
+def value_bytes(n, funcs, n_parts, n_peers):
+    """The value kernels after bounds / tiles / ends (every value column here is 8 bytes wide, numpy).  A scan function (sum,
+    count of a column, mean, min, max) reads its column and the flags twice (reduce, then rescan) and writes its 8-byte cell, plus
+    a validity byte when nullable, at each frame end (min / max also read the chosen cell there); the eval pass reads the flags
+    and the partition / peer-group words once, and per function writes 8 bytes (+1 validity) per row, reading the frame end's
+    cell for a scan function whose frame ends elsewhere and the source cell for first / last / lag / lead."""
+    ends = {"rows": n, "range": n_peers, "partition": n_parts}
+    total, evals = 0, False
+    for f in funcs:
+        fname, col = f[1], f[2]
+        vb = 0 if fname == "count" else 1
+        frame = f[3] if len(f) > 3 and fname not in ("lag", "lead") else "range"
+        if fname in ("lag", "lead", "first_value", "last_value") or col is None:
+            evals = True
+            total += n * (8 + vb) + (n * 8 if col is not None else 0)
+            continue
+        total += 2 * n * 9 + ends[frame] * (8 + vb) + (ends[frame] * 8 if fname in ("min", "max") else 0)
+        if frame != "rows":
+            evals = True
+            total += n * (8 + vb) + ends[frame] * (8 + vb)
+    if evals:
+        total += n + 4 * (n_parts + n_peers)
+    return int(total)
 
 
 def main():
@@ -71,7 +105,8 @@ def main():
     rid = torch.arange(n, dtype=torch.int64, device=dev)
     names = ["p", "o", "r"]
     torch.cuda.synchronize(dev)
-    cases = {"rn_rank_dense": (["p"], FUNCS3), "all6": (["p"], FUNCS6), "no_partition": ([], FUNCS3)}
+    cases = {"rn_rank_dense": (["p"], FUNCS3), "all6": (["p"], FUNCS6), "no_partition": ([], FUNCS3), "running": (["p"], RUNNING),
+             "partition_aggs": (["p"], PARTITION_AGGS), "lag_lead": (["p"], LAG_LEAD)}
 
     def batches():
         for r0 in range(0, n, args.batch):
@@ -83,7 +118,12 @@ def main():
         for t, last in batches():
             W.window_build_consume_batch(st, t, last)
         out, _ = W.window_produce_output_batch(st)
-        res = [torch.as_tensor(c.data, device=dev).clone() for c in out.columns] if keep else None
+        res = None
+        if keep:  # each column's data, and for a nullable function column its validity as one bool per row
+            res = [torch.as_tensor(c.data, device=dev).clone() for c in out.columns]
+            bit = torch.arange(8, device=dev, dtype=torch.uint8)
+            res += [None if c.validity is None else
+                    ((torch.as_tensor(c.validity, device=dev).unsqueeze(1) >> bit) & 1).flatten()[:n].bool() for c in out.columns[3:]]
         m9 = W.get_metric(st, 9)
         W.delete_window_state(st)
         return res, m9
@@ -148,8 +188,40 @@ def main():
             big = r * (q + 1)
             return torch.where(pos < big, pos // (q + 1) + 1, r + (pos - big) // torch.clamp(q, min=1) + 1)
 
+        sr, so, nf = res[2], res[1], len(funcs)
+        pid = torch.cumsum(ps.to(torch.int64), 0) - 1
+        n_p = int(pid[-1]) + 1
+
+        def value_ok(j, f):
+            """The value cases: integer results exactly; partition sums and means of o (>= 0) within 4 (m + 1) u of the exact value
+            for a partition of m rows, which covers the device's and torch's summation orders."""
+            got, valid = res[3 + j], res[3 + nf + j]
+            if f[1] == "count":
+                return torch.equal(got, s)
+            if f[1] == "lag":
+                return torch.equal(valid, ~ps) and torch.equal(torch.where(ps, 0, got), torch.where(ps, 0, torch.roll(sr, 1)))
+            if f[1] == "lead":
+                last = torch.roll(ps, -1)
+                last[-1] = True
+                return bool(valid.all()) and torch.equal(got.view(torch.int64), torch.where(last, 0.0, torch.roll(so, -1)).view(torch.int64))
+            if not bool(valid.all()):
+                return False
+            if f[2] == "r" and f[1] == "sum":  # ROWS frame: a segmented cumsum through the offsets at P
+                cs = torch.cumsum(sr, 0)
+                return torch.equal(got, cs - torch.where(P > 0, cs[(P - 1).clamp(min=0)], 0))
+            if f[2] == "r":  # MAX over RANGE: the running max at the peer group's last row
+                return torch.equal(got, (torch.cummax((pid << 32) | sr, 0).values & 0xFFFFFFFF)[qend - 1])
+            if f[1] in ("min", "max"):
+                init = torch.full((n_p,), float("inf") if f[1] == "min" else float("-inf"), dtype=torch.float64, device=dev)
+                red = init.scatter_reduce(0, pid, so, "amin" if f[1] == "min" else "amax", include_self=False)
+                return torch.equal(got.view(torch.int64), red[pid].view(torch.int64))
+            tot = torch.zeros(n_p, dtype=torch.float64, device=dev).index_add_(0, pid, so)[pid]
+            exp = tot if f[1] == "sum" else tot / s.to(torch.float64)
+            return bool(((got - exp).abs() <= 4 * (s + 1).to(torch.float64) * 2.0 ** -53 * exp.abs()).all())
+
         for j, f in enumerate(funcs):
-            if not torch.equal(res[3 + j].view(torch.int64), expected(f[0]).view(torch.int64)):
+            good = value_ok(j, f) if f[1] in W.VALUE_FUNCS else torch.equal(res[3 + j].view(torch.int64), expected(f[0]).view(torch.int64))
+            if not good:
                 return f"MISMATCH: {f[0]}", 0, 0
         return "ok", int(ps.sum()), int(qs.sum())
 
@@ -162,12 +234,17 @@ def main():
         part, funcs = cases[name]
         window_step(part, funcs)  # warm-up
         sort_step(part)
-        wt, st_ = [], []
+        value_case = name in VALUE_CASES
+        if value_case:
+            window_step(part, FUNCS3)
+        wt, st_, rt = [], [], []
         for _ in range(args.reps):
             ms, (_, m9) = timed(lambda: window_step(part, funcs))
             wt.append(ms)
             ms, sm = timed(lambda: sort_step(part))
             st_.append(ms)
+            if value_case:  # the value kernels' cost next to the ranking kernels', in the same process
+                rt.append(timed(lambda: window_step(part, FUNCS3))[0])
         w_ms, s_ms = sorted(wt)[len(wt) // 2], sorted(st_)[len(st_) // 2]
         free()
         # check
@@ -186,13 +263,20 @@ def main():
         free()
         key_bytes = 8 * (1 + len(part))
         sort_bytes = moved_bytes(n, 24, 0, key_bytes, kp)
-        total = sort_bytes + window_bytes(n, key_bytes, len(funcs), n_parts, n_peers)
+        if value_case:  # bounds and ends as the ranking cases (no ranking eval pass), then the value kernels
+            ends4 = 4 * (2 * n_parts + n_peers)
+            total = sort_bytes + window_bytes(n, key_bytes, 0, n_parts, n_peers) - (n + ends4) + value_bytes(n, funcs, n_parts, n_peers)
+        else:
+            total = sort_bytes + window_bytes(n, key_bytes, len(funcs), n_parts, n_peers)
         out = {"case": name, "rows": n, "batch": args.batch, "funcs": [f[1] for f in funcs], "ms_per_step": round(w_ms, 3),
                "runs_ms": [round(x, 3) for x in wt], "sort_ms": round(s_ms, 3), "sort_runs_ms": [round(x, 3) for x in st_],
                "extra_ms": round(w_ms - s_ms, 3), "extra_share_of_sort": round((w_ms - s_ms) / s_ms, 4),
                "rows_per_s": round(n / (w_ms * 1e-3), 1), "bytes": total, "gbps": round(total / (w_ms * 1e-3) / 1e9, 1),
                "share_of_3350_gbps": round(total / (w_ms * 1e-3) / 1e9 / PEAK_GBPS, 4), "metric9_partitions": m9,
                "sort_passes_run_skipped": sm[7:9], "result_check": chk, "card": card()}
+        if value_case:
+            r_ms = sorted(rt)[len(rt) // 2]
+            out.update(rn_rank_dense_ms=round(r_ms, 3), rn_rank_dense_runs_ms=[round(x, 3) for x in rt], extra_over_rn_rank_dense_ms=round(w_ms - r_ms, 3))
         print(json.dumps(out), flush=True)
         print(f"result_check: {chk}", flush=True)
         ok_all &= chk == "ok"

@@ -556,8 +556,8 @@ struct SortState {
     int64_t output_batch_size;
     int64_t rows_consumed = 0;  // metric 0
     bool finished = false;
-    // Output columns: the n_cols input columns, then any columns a form computes (numpy, of type sc.ctype[c]; the window's
-    // function columns).
+    // Output columns: the n_cols input columns, then any columns a form computes (of type sc.ctype[c] and array type
+    // arr_type[c]; the window's function columns).
     int n_out_cols;
     // output views, set by the form's finish_rows: rows [0, n_out) of column c at out_data[c], for a nullable column one validity
     // byte per row at out_vb[c]
@@ -589,7 +589,7 @@ struct SortState {
     // Rows [0, n) of a checked batch, arriving with indices rows_consumed, rows_consumed + 1, ...
     virtual void consume_rows(const b200_table* t, int64_t n) = 0;
     // At is_last: sort, then set n_out, out_data and out_vb.  Validity bytes the form allocates for its output go in vbytes (one
-    // slot per column), which is freed once the bitmaps are packed.
+    // slot per output column), which is freed once the bitmaps are packed.
     virtual void finish_rows(std::vector<DevBuf>& vbytes) = 0;
     // Metric 0 to 9; a metric the form does not keep reads 0.
     virtual int64_t metric(int which) const = 0;
@@ -611,16 +611,16 @@ struct SortState {
 
     void finish() {
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
-        std::vector<DevBuf> vbytes(sc.n_cols);
+        std::vector<DevBuf> vbytes(n_out_cols);
         finish_rows(vbytes);
         finished = true;
         int n_nullable = 0;
-        for (int c = 0; c < sc.n_cols; c++) n_nullable += arr_type[c] == ARR_NULLABLE;
+        for (int c = 0; c < n_out_cols; c++) n_nullable += arr_type[c] == ARR_NULLABLE;
         const int64_t words = (n_out + 31) / 32 + 2;
         d_bitmaps.alloc((size_t)std::max(1, n_nullable) * words * 4);
         B200_CUDA(cudaMemsetAsync(d_bitmaps.p, 0, d_bitmaps.bytes, stream));
         out_bitmap.assign(n_out_cols, nullptr);
-        for (int c = 0, k = 0; c < sc.n_cols; c++) {
+        for (int c = 0, k = 0; c < n_out_cols; c++) {
             if (arr_type[c] != ARR_NULLABLE) continue;
             out_bitmap[c] = d_bitmaps.as<uint32_t>() + (k++) * words;
             if (n_out > 0) launch_pack_bitmap(out_vb[c], n_out, out_bitmap[c], grid_for(n_out, 256), stream);
@@ -1122,23 +1122,305 @@ __global__ void __launch_bounds__(WN_THREADS) window_eval_kernel(const __grid_co
     }
 }
 
-// ROW_NUMBER / RANK / DENSE_RANK / PERCENT_RANK / CUME_DIST / NTILE over (PARTITION BY the first n_part keys ORDER BY the rest).
-// The output is the full sort's, plus one numpy column per function after the input columns.
+// ---- value window functions: SUM / COUNT / MEAN / MIN / MAX / FIRST_VALUE / LAST_VALUE over a frame [P, e], LAG / LEAD ----
+//
+// They run after window_ends_kernel, over the sorted columns the gather wrote.  A frame starts at the partition start P and ends
+// at e = i (WF_ROWS), the row's last peer pend[Q] - 1 (WF_RANGE) or the partition's last row P + psize[P] - 1 (WF_PARTITION).
+//   window_vscan_kernel<K, false>  per scan function (sum, count of a column, mean, min, max): the segmented reduction of each
+//                                  WN_TILE-row tile, reset at partition starts (the WN_PART flags).
+//   window_vtiles_kernel<K>        one block: the exclusive scan of the tile carries.
+//   window_vscan_kernel<K, true>   the tile's scan again, seeded by its carry; every position that ends a frame of the function
+//                                  writes the function's final cell and validity byte there.
+//   window_veval_kernel            the ranking scan of the flags (P, Q) again, then per position and value function: a scan
+//                                  function whose frame ends elsewhere copies out[e] to out[i] (race-free: e(e(i)) = e(i), so only
+//                                  frame ends are read and they are not written); count(*) is e - P + 1; first_value, last_value,
+//                                  lag and lead gather the cell at P, e, i - k or i + k (or take the default) from the sorted column.
+// A min / max scan carries (radix word, position) with ties kept on the left and resolves to that position's cell.  Float sums
+// are combined in double in the scan's fixed order, which depends only on the row count: they are bit-identical across runs and
+// batch splits.
+enum { WN_SUM = 6, WN_COUNT = 7, WN_MEAN = 8, WN_MIN = 9, WN_MAX = 10, WN_FIRST_VALUE = 11, WN_LAST_VALUE = 12, WN_LAG = 13, WN_LEAD = 14 };
+enum { WF_NONE = 0, WF_RANGE = 1, WF_ROWS = 2, WF_PARTITION = 3 };
+enum { WV_ISUM = 0, WV_FSUM = 1, WV_MIN = 2, WV_MAX = 3 };  // scan kinds: 64-bit wrapping sum (and count), double sum, min, max
+constexpr uint32_t WV_NONE = 0xFFFFFFFFu;                    // a min / max scan that has seen no valid cell
+constexpr uint64_t WV_NEG_ZERO = 0x8000000000000000ull;      // -0.0, the identity of a double sum (x + -0.0 == x for every x)
+
+// Scan value: x the sum (int64 bits or double bits) or the radix word; c the count of valid cells or the position of the min /
+// max; f set when the segment holds a partition start.
+struct WvAgg { uint64_t x; uint32_t c, f; };
+
+// One value function as the kernels see it.
+struct WvFunc {
+    int code, frame, ct, size, out_size, dflt_valid;  // ct / size: the value column's c-type and cell bytes (size 0: count(*))
+    int64_t k;                                        // lag / lead offset
+    uint64_t dflt;                                    // lag / lead default bits
+    const char* data;                                 // the sorted value column and its validity bytes (nullptr: numpy)
+    const uint8_t* vb;
+    char* out;                                        // the output column and its validity bytes (nullptr: count, numpy)
+    uint8_t* out_vb;
+};
+
+struct WvArgs {
+    int64_t n;
+    const uint8_t* flags;
+    const uint32_t *psize, *pend;
+    WvAgg* carry;  // per tile: its reduction, then its exclusive prefix
+    WvFunc s;      // window_vscan_kernel / window_vtiles_kernel: the function being scanned
+    int n_funcs;   // window_veval_kernel: the value functions with work there
+    WvFunc f[SORT_MAX_COLS];
+};
+
+template <int K>
+__device__ __forceinline__ WvAgg wv_identity() { return WvAgg{K == WV_FSUM ? WV_NEG_ZERO : 0ull, (K == WV_MIN || K == WV_MAX) ? WV_NONE : 0u, 0u}; }
+
+template <int K>
+__device__ __forceinline__ WvAgg wv_combine(WvAgg a, WvAgg b) {
+    if (b.f) return b;
+    WvAgg r{b.x, b.c, a.f};
+    if (K == WV_ISUM) { r.x = a.x + b.x; r.c = a.c + b.c; }
+    else if (K == WV_FSUM) { r.x = (uint64_t)__double_as_longlong(__longlong_as_double((long long)a.x) + __longlong_as_double((long long)b.x)); r.c = a.c + b.c; }
+    else {
+        const bool take_b = a.c == WV_NONE || (b.c != WV_NONE && (K == WV_MIN ? b.x < a.x : b.x > a.x));  // ties keep the left row
+        if (!take_b) { r.x = a.x; r.c = a.c; }
+    }
+    return r;
+}
+
+__device__ __forceinline__ WvAgg wv_shfl_up(WvAgg v, int o) {
+    return WvAgg{__shfl_up_sync(0xffffffffu, (unsigned long long)v.x, o), __shfl_up_sync(0xffffffffu, v.c, o), __shfl_up_sync(0xffffffffu, v.f, o)};
+}
+
+// Scan value of position i of the scanned function; `part`: i starts a partition.
+template <int K>
+__device__ __forceinline__ WvAgg wv_value(const WvFunc& s, int64_t i, bool part) {
+    WvAgg r = wv_identity<K>();
+    r.f = part;
+    bool na = s.vb && s.vb[i] == 0;
+    if (K == WV_ISUM && s.code == WN_COUNT && !ctype_is_float(s.ct)) { r.c = !na; return r; }  // only NaN needs the values
+    const uint64_t raw = load_bits(s.data, s.size, i);
+    if (K == WV_ISUM) {
+        uint64_t x = raw;
+        if (s.ct == CT_FLOAT64) na = na || isnan(__longlong_as_double((long long)raw));
+        else if (s.ct == CT_FLOAT32) na = na || isnan(__uint_as_float((uint32_t)raw));
+        else if (ctype_is_signed_int(s.ct)) x = (uint64_t)((int64_t)(raw << (64 - 8 * s.size)) >> (64 - 8 * s.size));
+        if (!na) { r.x = x; r.c = 1; }
+    } else if (K == WV_FSUM) {
+        const double d = s.ct == CT_FLOAT64 ? __longlong_as_double((long long)raw) : (double)__uint_as_float((uint32_t)raw);
+        if (!(na || isnan(d))) { r.x = (uint64_t)__double_as_longlong(d); r.c = 1; }
+    } else {
+        const uint64_t w = sort_word(SortKey{s.ct, s.size, 0, 1}, raw, na);
+        if (!na) { r.x = w; r.c = (uint32_t)i; }
+    }
+    return r;
+}
+
+// Inclusive scan of this thread's WN_ITEMS values of a tile (warp-strided, as wn_row), seeded by `seed`.
+template <int K>
+__device__ __forceinline__ void wv_scan_tile(WvAgg seed, WvAgg (&v)[WN_ITEMS]) {
+    __shared__ WvAgg s_seg[WN_ITEMS * WN_WARPS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) {
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const WvAgg y = wv_shfl_up(v[k], o);
+            if (lane >= o) v[k] = wv_combine<K>(y, v[k]);
+        }
+        if (lane == 31) s_seg[k * WN_WARPS + warp] = v[k];
+    }
+    __syncthreads();
+    if (warp == 0) {  // exclusive scan of the 64 (item, warp) segments in row order, seeded: 2 per lane
+        const WvAgg x0 = s_seg[2 * lane], x1 = s_seg[2 * lane + 1];
+        WvAgg inc = wv_combine<K>(x0, x1);
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const WvAgg y = wv_shfl_up(inc, o);
+            if (lane >= o) inc = wv_combine<K>(y, inc);
+        }
+        const WvAgg ex = wv_shfl_up(inc, 1);
+        const WvAgg base = lane > 0 ? wv_combine<K>(seed, ex) : seed;
+        s_seg[2 * lane] = base;
+        s_seg[2 * lane + 1] = wv_combine<K>(base, x0);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) v[k] = wv_combine<K>(s_seg[k * WN_WARPS + warp], v[k]);
+}
+
+// dst[i] = the low `size` bytes of bits.
+__device__ __forceinline__ void wv_store_bits(void* dst, int64_t i, uint64_t bits, int size) {
+    switch (size) {
+        case 8: ((uint64_t*)dst)[i] = bits; break;
+        case 4: ((uint32_t*)dst)[i] = (uint32_t)bits; break;
+        case 2: ((uint16_t*)dst)[i] = (uint16_t)bits; break;
+        default: ((uint8_t*)dst)[i] = (uint8_t)bits; break;
+    }
+}
+
+// The function's result at a frame end i whose frame's scan value is v.
+template <int K>
+__device__ __forceinline__ void wv_write(const WvFunc& s, int64_t i, WvAgg v) {
+    if (s.code == WN_COUNT) { ((int64_t*)s.out)[i] = v.c; return; }
+    if (K == WV_MIN || K == WV_MAX) {
+        const bool ok = v.c != WV_NONE;
+        if (ok) copy_cell(s.out, i, s.data, v.c, s.size);
+        else wv_store_bits(s.out, i, 0, s.size);
+        s.out_vb[i] = ok;
+        return;
+    }
+    const bool ok = v.c > 0;
+    if (s.code == WN_MEAN) {
+        const double sum = K == WV_FSUM ? __longlong_as_double((long long)v.x)
+                                        : ctype_is_signed_int(s.ct) || s.ct == CT_BOOL ? (double)(int64_t)v.x : (double)v.x;
+        ((double*)s.out)[i] = ok ? sum / (double)v.c : 0.0;
+    } else if (s.ct == CT_FLOAT32) {
+        ((float*)s.out)[i] = ok ? (float)__longlong_as_double((long long)v.x) : 0.0f;
+    } else {
+        ((uint64_t*)s.out)[i] = ok ? v.x : 0ull;
+    }
+    s.out_vb[i] = ok;
+}
+
+template <int K, bool FINAL>
+__global__ void __launch_bounds__(WN_THREADS) window_vscan_kernel(const __grid_constant__ WvArgs a) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t t = blockIdx.x;
+    WvAgg v[WN_ITEMS];
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        v[k] = i < a.n ? wv_value<K>(a.s, i, a.flags[i] & WN_PART) : wv_identity<K>();
+    }
+    wv_scan_tile<K>(FINAL ? a.carry[t] : wv_identity<K>(), v);
+    if (!FINAL) {  // padding rows hold the identity, so the tile's last slot holds its reduction
+        if (threadIdx.x == WN_THREADS - 1) a.carry[t] = v[WN_ITEMS - 1];
+        return;
+    }
+    const uint8_t end_flag = a.s.frame == WF_RANGE ? WN_PEER : WN_PART;
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        if (i >= a.n) break;
+        if (a.s.frame == WF_ROWS || i + 1 == a.n || (a.flags[i + 1] & end_flag)) wv_write<K>(a.s, i, v[k]);
+    }
+}
+
+// One block of 1024 threads; thread x scans a contiguous run of tiles (as window_tiles_kernel).
+template <int K>
+__global__ void __launch_bounds__(1024) window_vtiles_kernel(const __grid_constant__ WvArgs a, int64_t n_tiles) {
+    __shared__ WvAgg s_agg[32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t per = (n_tiles + 1023) / 1024, t0 = threadIdx.x * per, t1 = min(n_tiles, t0 + per);
+    WvAgg acc = wv_identity<K>();
+    for (int64_t t = t0; t < t1; t++) acc = wv_combine<K>(acc, a.carry[t]);
+    WvAgg inc = acc;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const WvAgg y = wv_shfl_up(inc, o);
+        if (lane >= o) inc = wv_combine<K>(y, inc);
+    }
+    if (lane == 31) s_agg[warp] = inc;
+    __syncthreads();
+    WvAgg run = wv_identity<K>();
+    for (int w = 0; w < warp; w++) run = wv_combine<K>(run, s_agg[w]);
+    const WvAgg ex = wv_shfl_up(inc, 1);
+    if (lane > 0) run = wv_combine<K>(run, ex);
+    for (int64_t t = t0; t < t1; t++) {
+        const WvAgg v = a.carry[t];
+        a.carry[t] = run;
+        run = wv_combine<K>(run, v);
+    }
+}
+
+__global__ void __launch_bounds__(WN_THREADS) window_veval_kernel(const __grid_constant__ WnArgs w, const __grid_constant__ WvArgs a) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t t = blockIdx.x;
+    uint8_t f[WN_ITEMS];
+    WnAgg v[WN_ITEMS];
+    wn_scan_tile(w, t, f, v);
+    __shared__ WnAgg s_v[WN_ITEMS][WN_THREADS];  // parked as in window_eval_kernel: the item loop is not unrolled
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) s_v[k][threadIdx.x] = v[k];
+#pragma unroll 1
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        if (i >= a.n) break;
+        const WnAgg vk = s_v[k][threadIdx.x];
+        const int64_t P = vk.p, pe = P + w.psize[vk.p];  // the partition is [P, pe)
+        for (int fn = 0; fn < a.n_funcs; fn++) {
+            const WvFunc& g = a.f[fn];
+            const int64_t e = g.frame == WF_ROWS ? i : g.frame == WF_RANGE ? (int64_t)w.pend[vk.q] - 1 : pe - 1;
+            int64_t src;
+            switch (g.code) {
+                case WN_FIRST_VALUE: src = P; break;
+                case WN_LAST_VALUE: src = e; break;
+                case WN_LAG: src = i - g.k >= P ? i - g.k : -1; break;
+                case WN_LEAD: src = i + g.k < pe ? i + g.k : -1; break;
+                default:
+                    if (g.size == 0) { ((int64_t*)g.out)[i] = e - P + 1; continue; }  // count(*)
+                    src = e;  // a scan function: its frame end holds the result
+            }
+            const bool scanned = g.code <= WN_MAX;
+            if (scanned && e == i) continue;
+            const char* from = scanned ? g.out : g.data;
+            const int sz = scanned ? g.out_size : g.size;
+            if (src >= 0) {
+                copy_cell(g.out, i, from, src, sz);
+                if (g.out_vb) g.out_vb[i] = scanned ? g.out_vb[src] : g.vb ? g.vb[src] : 1;
+            } else {
+                wv_store_bits(g.out, i, g.dflt, sz);
+                g.out_vb[i] = (uint8_t)g.dflt_valid;
+            }
+        }
+    }
+}
+
+template <int K>
+void launch_wv_scan(const WvArgs& a, int64_t n_tiles, cudaStream_t st) {
+    window_vscan_kernel<K, false><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
+    window_vtiles_kernel<K><<<1, 1024, 0, st>>>(a, n_tiles);
+    window_vscan_kernel<K, true><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
+}
+
+// Ranking and value window functions over (PARTITION BY the first n_part keys ORDER BY the rest).  The output is the full sort's,
+// plus one column per function after the input columns: numpy for the ranking functions and count, nullable for the others.
 struct WindowState : FullSortState {
     int n_part, n_funcs;
-    int func[SORT_MAX_COLS];
-    int64_t farg[SORT_MAX_COLS];
+    b200_window_func fn[SORT_MAX_COLS];
     std::vector<DevBuf> fout;
     int64_t n_partitions = 0;  // metric 9
 
     WindowState(const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_part_, int n_keys, const int32_t* asc,
-                const int32_t* na_last, const int32_t* funcs, const int64_t* fargs, int n_funcs_, int64_t obs, int dev, cudaStream_t st)
+                const int32_t* na_last, const b200_window_func* funcs, int n_funcs_, int64_t obs, int dev, cudaStream_t st)
         : FullSortState(c_types, arr_types, n_arrs, n_keys, asc, na_last, obs, dev, st), n_part(n_part_), n_funcs(n_funcs_) {
         for (int f = 0; f < n_funcs; f++) {
-            func[f] = funcs[f]; farg[f] = fargs ? fargs[f] : 0;
-            const bool real = func[f] == WN_PERCENT_RANK || func[f] == WN_CUME_DIST;
-            sc.ctype[n_out_cols] = real ? CT_FLOAT64 : CT_INT64;
-            arr_type[n_out_cols++] = ARR_NUMPY;
+            const b200_window_func& d = fn[f] = funcs[f];
+            B200_REQUIRE(d.code >= WN_ROW_NUMBER && d.code <= WN_LEAD, "b200 window: unknown function code");
+            int ct = CT_INT64, at = ARR_NUMPY;
+            if (d.code <= WN_NTILE) {
+                B200_REQUIRE(d.col == -1 && d.frame == WF_NONE, "b200 window: a ranking function takes no column and no frame");
+                if (d.code == WN_NTILE) B200_REQUIRE(d.arg >= 1, "b200 window: ntile needs n >= 1");
+                if (d.code == WN_PERCENT_RANK || d.code == WN_CUME_DIST) ct = CT_FLOAT64;
+            } else {
+                B200_REQUIRE((d.col >= 0 && d.col < n_arrs) || (d.code == WN_COUNT && d.col == -1),
+                             "b200 window: value column index out of range (-1, count(*), is for count only)");
+                if (d.code == WN_LAG || d.code == WN_LEAD) {
+                    B200_REQUIRE(d.frame == WF_NONE, "b200 window: lag and lead take no frame");
+                    B200_REQUIRE(d.arg >= 0 && d.arg <= 0x7FFFFFFF, "b200 window: lag / lead offset k must be in [0, 2^31)");
+                    B200_REQUIRE(d.default_valid == 0 || d.default_valid == 1, "b200 window: default_valid must be 0 or 1");
+                } else {
+                    B200_REQUIRE(d.frame >= WF_RANGE && d.frame <= WF_PARTITION, "b200 window: unknown frame (1 range, 2 rows, 3 partition)");
+                }
+                const int vct = d.col >= 0 ? sc.ctype[d.col] : CT_INT64;
+                const bool temporal = vct == CT_DATE || vct == CT_DATETIME || vct == CT_TIMEDELTA;
+                if (d.code == WN_SUM || d.code == WN_MEAN)
+                    B200_REQUIRE(!temporal, "b200 window: sum and mean need an integer, bool or float column");
+                if (d.code == WN_SUM) ct = ctype_is_float(vct) ? vct : ctype_is_signed_int(vct) || vct == CT_BOOL ? CT_INT64 : CT_UINT64;
+                else if (d.code == WN_MEAN) ct = CT_FLOAT64;
+                else if (d.code != WN_COUNT) ct = vct;
+                if (d.code != WN_COUNT) at = ARR_NULLABLE;
+            }
+            sc.ctype[n_out_cols] = ct;
+            arr_type[n_out_cols++] = at;
         }
     }
 
@@ -1148,12 +1430,28 @@ struct WindowState : FullSortState {
         const int64_t n = n_out;
         fout.resize(n_funcs);
         WnArgs a{};
-        a.n = n; a.n_part = n_part; a.n_keys = sc.n_keys; a.n_funcs = n_funcs;
+        a.n = n; a.n_part = n_part; a.n_keys = sc.n_keys;
         for (int j = 0; j < sc.n_keys; j++) { a.key[j] = sc.key[j]; a.data[j] = out_data[j]; a.vb[j] = out_vb[j]; }
+        WvArgs va{};
+        std::vector<WvFunc> scans;
+        bool eval = false;
         for (int f = 0; f < n_funcs; f++) {
+            const int c = sc.n_cols + f;
             fout[f].alloc((size_t)n * 8);
-            a.out[f] = out_data[sc.n_cols + f] = fout[f].as<char>();
-            a.func[f] = func[f]; a.farg[f] = farg[f];
+            out_data[c] = fout[f].as<char>();
+            if (arr_type[c] == ARR_NULLABLE) { vbytes[c].alloc((size_t)n); out_vb[c] = vbytes[c].as<uint8_t>(); }
+            const b200_window_func& d = fn[f];
+            if (d.code <= WN_NTILE) {
+                a.out[a.n_funcs] = out_data[c];
+                a.func[a.n_funcs] = d.code; a.farg[a.n_funcs++] = d.arg;
+                continue;
+            }
+            WvFunc g{d.code, d.frame, d.col >= 0 ? sc.ctype[d.col] : CT_INT64, d.col >= 0 ? ctype_size(sc.ctype[d.col]) : 0,
+                     ctype_size(sc.ctype[c]), d.default_valid, d.arg, d.default_bits, d.col >= 0 ? out_data[d.col] : nullptr,
+                     d.col >= 0 ? out_vb[d.col] : nullptr, out_data[c], out_vb[c]};
+            const bool scanned = d.code <= WN_MAX && d.col >= 0;
+            if (scanned) scans.push_back(g);
+            if (!scanned || d.frame != WF_ROWS) { va.f[va.n_funcs++] = g; eval = true; }
         }
         if (n == 0) return;
         const int64_t n_tiles = (n + WN_TILE - 1) / WN_TILE;
@@ -1168,7 +1466,19 @@ struct WindowState : FullSortState {
         window_bounds_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
         window_tiles_kernel<<<1, 1024, 0, stream>>>(a, n_tiles);
         window_ends_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
-        window_eval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
+        if (a.n_funcs > 0) window_eval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
+        B200_CUDA(cudaGetLastError());
+        DevBuf carry;
+        if (!scans.empty()) carry.alloc((size_t)n_tiles * sizeof(WvAgg));
+        va.n = n; va.flags = a.flags; va.psize = a.psize; va.pend = a.pend; va.carry = carry.as<WvAgg>();
+        for (const WvFunc& g : scans) {
+            va.s = g;
+            if (g.code == WN_MIN) launch_wv_scan<WV_MIN>(va, n_tiles, stream);
+            else if (g.code == WN_MAX) launch_wv_scan<WV_MAX>(va, n_tiles, stream);
+            else if (g.code != WN_COUNT && ctype_is_float(g.ct)) launch_wv_scan<WV_FSUM>(va, n_tiles, stream);
+            else launch_wv_scan<WV_ISUM>(va, n_tiles, stream);
+        }
+        if (eval) window_veval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a, va);
         B200_CUDA(cudaGetLastError());
         auto* h = (uint32_t*)pinned_acquire(8);
         B200_CUDA(cudaMemcpyAsync(h, totals.p, 8, cudaMemcpyDeviceToHost, stream));
@@ -1219,9 +1529,10 @@ void* b200_sort_state_init_full(int64_t operator_id, const int8_t* c_types, cons
     });
 }
 
-void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs, int32_t n_partition_keys,
-                             int32_t n_order_keys, const int32_t* order_ascending, const int32_t* order_na_last, const int32_t* funcs,
-                             const int64_t* func_args, int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream) {
+void* b200_window_state_init_funcs(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                                   int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                                   const int32_t* order_na_last, const b200_window_func* funcs, int32_t n_funcs, int64_t output_batch_size,
+                                   int32_t device, void* stream) {
     (void)operator_id;
     return b200::sort_state_new(device, [&]() -> SortState* {
         const int np = n_partition_keys, no = n_order_keys;
@@ -1231,18 +1542,30 @@ void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const i
         B200_REQUIRE(funcs && n_funcs >= 1, "b200 window: at least one function");
         B200_REQUIRE(n_arrs >= np + no && n_arrs + n_funcs <= b200::SORT_MAX_COLS,
                      "b200 window: the keys are the first n_partition_keys + n_order_keys columns, and input plus function columns are at most 32");
-        for (int f = 0; f < n_funcs; f++) {
-            B200_REQUIRE(funcs[f] >= b200::WN_ROW_NUMBER && funcs[f] <= b200::WN_NTILE, "b200 window: unknown function code");
-            if (funcs[f] == b200::WN_NTILE) B200_REQUIRE(func_args && func_args[f] >= 1, "b200 window: ntile needs n >= 1");
-        }
         int32_t asc[b200::SORT_MAX_KEYS], na_last[b200::SORT_MAX_KEYS];
         for (int j = 0; j < np + no; j++) {  // PARTITION BY keys: ascending, NA last
             asc[j] = j < np ? 1 : order_ascending[j - np];
             na_last[j] = j < np ? 1 : order_na_last[j - np];
         }
-        return new b200::WindowState(c_types, arr_types, n_arrs, np, np + no, asc, na_last, funcs, func_args, n_funcs, output_batch_size,
-                                     device, (cudaStream_t)stream);
+        return new b200::WindowState(c_types, arr_types, n_arrs, np, np + no, asc, na_last, funcs, n_funcs, output_batch_size, device,
+                                     (cudaStream_t)stream);
     });
+}
+
+void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs, int32_t n_partition_keys,
+                             int32_t n_order_keys, const int32_t* order_ascending, const int32_t* order_na_last, const int32_t* funcs,
+                             const int64_t* func_args, int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream) {
+    b200_window_func d[b200::SORT_MAX_COLS] = {};
+    try {
+        B200_REQUIRE(funcs && n_funcs >= 1 && n_funcs <= b200::SORT_MAX_COLS, "b200 window: 1 to 32 functions");
+        for (int f = 0; f < n_funcs; f++) {
+            B200_REQUIRE(funcs[f] >= b200::WN_ROW_NUMBER && funcs[f] <= b200::WN_NTILE, "b200 window: unknown function code");
+            if (funcs[f] == b200::WN_NTILE) B200_REQUIRE(func_args, "b200 window: ntile needs n >= 1");
+            d[f] = b200_window_func{funcs[f], -1, b200::WF_NONE, 0, func_args ? func_args[f] : 0, 0};
+        }
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
+    return b200_window_state_init_funcs(operator_id, c_types, arr_types, n_arrs, n_partition_keys, n_order_keys, order_ascending,
+                                        order_na_last, d, n_funcs, output_batch_size, device, stream);
 }
 
 int b200_sort_build_consume_batch(void* state, const b200_table* in_table, int32_t is_last, int32_t* request_input) {

@@ -1,11 +1,16 @@
-"""Streaming window operator: ranking functions OVER (PARTITION BY p ... ORDER BY o ...).
+"""Streaming window operator: ranking, aggregate and navigation functions OVER (PARTITION BY p ... ORDER BY o ...).
 
     ROW_NUMBER() / RANK() / DENSE_RANK() / PERCENT_RANK() / CUME_DIST() / NTILE(n) OVER (PARTITION BY p ORDER BY o)
+    SUM / COUNT / AVG / MIN / MAX / FIRST_VALUE / LAST_VALUE (x) OVER (PARTITION BY p ORDER BY o [frame])
+    LAG / LEAD (x, k, default) OVER (PARTITION BY p ORDER BY o)
 
-pandas equivalents: groupby(p).cumcount() + 1 and groupby(p)[o].rank(method="min" / "dense" / "max", pct=...).  The state is a
-third form of the streaming sort (streaming/sort.py's SortState, sort.cu's WindowState): batches are appended to the full sort's
-device chunk store, is_last sorts every row by (partition keys ascending NA last, order keys, arrival index) and then scans the
-sorted key columns on the device for partition and peer-group boundaries.
+pandas equivalents: groupby(p).cumcount() + 1, groupby(p)[o].rank(method="min" / "dense" / "max", pct=...),
+groupby(p)[x].cumsum() / cummin() / cummax() (the "rows" frame), groupby(p)[x].transform("sum" / "mean" / "min" / "max" /
+"count" / "size" / "first" / "last") (the "partition" frame) and groupby(p)[x].shift(k, fill_value=default) (lag; lead is
+shift(-k)).  The state is a third form of the streaming sort (streaming/sort.py's SortState, sort.cu's WindowState): batches are
+appended to the full sort's device chunk store, is_last sorts every row by (partition keys ascending NA last, order keys, arrival
+index), scans the sorted key columns on the device for partition and peer-group boundaries and then scans or gathers the value
+columns.
 
 Semantics:
   - keys: 0..4 PARTITION BY columns and 0..4 ORDER BY columns, 1..4 in all, distinct, of the sort's key types (fixed-width
@@ -19,6 +24,28 @@ Semantics:
     s // n + 1 rows, the others s // n; buckets 1..s when n > s).
   - row_number, rank, dense_rank and ntile are int64 columns, percent_rank and cume_dist float64 (one IEEE double division of two
     integers, so bit-identical to numpy's).
+  - value functions read one input column (any column, keys included).  Frames start at the row's partition's first row P and
+    end at e: "range" (the default; SQL's default frame RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW) at the row's last peer,
+    which is the partition's last row without ORDER BY; "rows" (ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW) at the row
+    itself, ties in arrival order; "partition" (ROWS BETWEEN UNBOUNDED PRECEDING AND UNBOUNDED FOLLOWING) at the partition's last
+    row.  Bounded frames (k PRECEDING / FOLLOWING) are not supported.  Over [P, e], with a float NaN counted as NA:
+      count(x): non-NA cells, count(None): COUNT(*) = e - P + 1; int64 numpy.
+      sum(x): the sum of the non-NA cells, NA when there are none; integers and bool wrap in 64 bits (int64 for signed and bool,
+        uint64 for unsigned), floats accumulate in double (float32 narrowed once at the end); nullable.
+      mean(x): sum / count in double ((double) of the exact 64-bit sum for integers and bool), NA when count = 0; float64,
+        nullable.  sum and mean of a temporal column raise.
+      min(x) / max(x): the cell of the earliest row holding the least / greatest non-NA value, compared in the sort's key order
+        (so every key type works; -0.0 ties 0.0 and the earlier row's bits are returned); NA when no cell is valid; x's type,
+        nullable.
+      first_value(x) / last_value(x): the cell at P / e as it is, bits and validity (a NaN stays a valid NaN, SQL RESPECT NULLS);
+        x's type, nullable.
+      lag(x, k=1, default=None) / lead(...): the cell at i - k / i + k if that row is in the row's partition, else default (NA
+        when None); 0 <= k < 2^31, k = 0 is the row itself; no frame; x's type, nullable.  default is converted to x's numpy
+        dtype and must round-trip exactly.
+    These follow SQL where pandas differs: groupby().cumsum() / cummin() / cummax() give NA at NA rows where the "rows" frame
+    gives the aggregate so far; transform("sum") of an all-NA partition gives 0 where sum gives NA; float sums are combined in
+    the scan's order, not sequentially.  Results depend only on the sorted positions: every row that shares a frame end gets a
+    bit-identical result, and float sums are bit-identical across runs and across any split of the rows into batches.
   - output: every input row once, in the stable sort's order by (partition keys, order keys, arrival); every input column in
     input order, then one column per function under the caller's name.  SQL leaves the order open; fixing it makes every column
     comparable bit for bit.
@@ -28,15 +55,28 @@ Semantics:
 
 from __future__ import annotations
 
+import warnings
+
+import numpy as np
+
 from .. import _lib
 from .._lib import ffi
-from ..table import Table
+from ..table import CTypes, Table, np_dtype_of
 from .sort import MAX_FULL_SORT_ROWS, MAX_KEYS, SortState
 
-# Function codes of b200_window_state_init (include/bodo_b200.h).
+# Function codes of b200_window_func (include/bodo_b200.h): the ranking functions, then the value functions.
 FUNCS = {"row_number": 0, "rank": 1, "dense_rank": 2, "percent_rank": 3, "cume_dist": 4, "ntile": 5}
+VALUE_FUNCS = {"sum": 6, "count": 7, "mean": 8, "min": 9, "max": 10, "first_value": 11, "last_value": 12, "lag": 13, "lead": 14}
+FRAMES = {"range": 1, "rows": 2, "partition": 3}
+_VALUE_NAMES = {c: f for f, c in VALUE_FUNCS.items()}
+_FRAME_NAMES = {c: f for f, c in FRAMES.items()}
 MAX_COLS = 32
 MAX_WINDOW_ROWS = MAX_FULL_SORT_ROWS
+MAX_LAG = (1 << 31) - 1
+_TEMPORAL = (CTypes.DATE, CTypes.DATETIME, CTypes.TIMEDELTA)
+_FORMS = (f"ranking: (out_name, fname) with fname in {sorted(FUNCS)}, or (out_name, 'ntile', n); value: (out_name, fname, column"
+          f"[, frame]) with fname in {sorted(set(VALUE_FUNCS) - {'lag', 'lead'})}, frame in {sorted(FRAMES)}, column None for "
+          "count(*) only, or (out_name, 'lag' | 'lead', column[, k[, default]])")
 
 
 def _names(x):
@@ -45,15 +85,56 @@ def _names(x):
     return [x] if isinstance(x, str) else list(x)
 
 
+def _parse_value(f, col_names):
+    """(out_name, fname, column[, frame]) or (out_name, 'lag' | 'lead', column[, k[, default]]) -> (out_name, code, k, column,
+    frame code, default); frame code 0 for lag and lead."""
+    name, fname, column = f[0], f[1], f[2]
+    if not (column is None and fname == "count") and not (isinstance(column, str) and column in col_names):
+        raise _lib.B200Error(f"Streaming Window: {f!r}: unknown column {column!r} (one of {col_names}; None for count only)")
+    if fname in ("lag", "lead"):
+        if len(f) > 5:
+            raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} takes (out_name, {fname!r}, column[, k[, default]])")
+        k = f[3] if len(f) > 3 else 1
+        if isinstance(k, str) and k in FRAMES:
+            raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} takes no frame")
+        if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or not 0 <= k <= MAX_LAG:
+            raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} needs an integer k with 0 <= k < 2^31")
+        return (name, VALUE_FUNCS[fname], int(k), column, 0, f[4] if len(f) > 4 else None)
+    frame = f[3] if len(f) > 3 else "range"
+    if len(f) > 4 or not isinstance(frame, str) or frame not in FRAMES:
+        raise _lib.B200Error(f"Streaming Window: {f!r}: bad frame (one of {sorted(FRAMES)}, as (out_name, {fname!r}, column[, frame]))")
+    return (name, VALUE_FUNCS[fname], 0, column, FRAMES[frame], None)
+
+
+def _default_bits(f, ct):
+    """Bits of lag / lead's default in the column's numpy dtype; raises unless it round-trips exactly."""
+    default, dt = f[5], np_dtype_of(ct)
+    entry = (f[0], _VALUE_NAMES[f[1]], f[3], f[2], default)
+    try:
+        with warnings.catch_warnings(), np.errstate(all="ignore"):
+            warnings.simplefilter("ignore")
+            y = np.array([default]).astype(dt)
+        back = y[0].item()
+        ok = back == default or (isinstance(back, float) and back != back and default != default)
+    except (TypeError, ValueError, OverflowError):
+        ok = False
+    if not ok:
+        raise _lib.B200Error(f"Streaming Window: {entry!r}: default {default!r} is not exactly representable as {dt}")
+    return int(y.view(f"u{dt.itemsize}")[0])
+
+
 def _parse_funcs(funcs, col_names):
-    """[(out_name, fname)] or (out_name, "ntile", n) entries -> [(out_name, code, n)]."""
+    """Ranking entries -> (out_name, code, n); value entries -> (out_name, code, k, column, frame code, default)."""
     out = []
     for f in funcs:
         f = tuple(f)
-        if len(f) < 2 or not isinstance(f[0], str) or f[1] not in FUNCS:
-            raise _lib.B200Error(f"Streaming Window: unknown window function {f!r} (one of {sorted(FUNCS)}, as (out_name, fname) or "
-                                 "(out_name, 'ntile', n))")
+        if (len(f) < 2 or not isinstance(f[0], str) or not isinstance(f[1], str) or f[1] not in FUNCS and f[1] not in VALUE_FUNCS
+                or f[1] in VALUE_FUNCS and len(f) < 3):
+            raise _lib.B200Error(f"Streaming Window: unknown window function {f!r} ({_FORMS})")
         name, fname = f[0], f[1]
+        if fname in VALUE_FUNCS:
+            out.append(_parse_value(f, col_names))
+            continue
         if fname == "ntile":
             if len(f) != 3 or isinstance(f[2], bool) or not isinstance(f[2], int) or f[2] < 1:
                 raise _lib.B200Error(f"Streaming Window: ntile needs an integer n >= 1, as (out_name, 'ntile', n) (got {f!r})")
@@ -65,7 +146,7 @@ def _parse_funcs(funcs, col_names):
         out.append((name, FUNCS[fname], arg))
     if not out:
         raise _lib.B200Error("Streaming Window: at least one window function")
-    names = [n for n, _, _ in out]
+    names = [f[0] for f in out]
     dup = sorted({n for n in names if names.count(n) > 1})
     if dup:
         raise _lib.B200Error(f"Streaming Window: duplicate output names {dup}")
@@ -103,17 +184,45 @@ class WindowState(SortState):
                          output_batch_size, device, stream, process_group, full=True)
         self.partition_by, self.order_by = part, order
         self.funcs = parsed
-        self.out_names += [n for n, _, _ in parsed]
+        self.out_names += [f[0] for f in parsed]
         self.out_order += list(range(len(self.phys), len(self.phys) + len(parsed)))
+        self.descs = None
+
+    def descriptors(self, c_types):
+        """The b200_window_func fields (code, col, frame, default_valid, arg, default_bits) of every function, given the c-types
+        of the input columns in input order.  Raises B200Error for sum or mean of a temporal column and for a lag / lead default
+        that does not round-trip through the column's dtype."""
+        out = []
+        for f in self.funcs:
+            if len(f) == 3:
+                out.append((f[1], -1, 0, 0, f[2], 0))
+                continue
+            name, code, arg, column, frame, default = f
+            if column is None:
+                out.append((code, -1, frame, 0, arg, 0))
+                continue
+            ct = c_types[self.col_names.index(column)]
+            if code in (VALUE_FUNCS["sum"], VALUE_FUNCS["mean"]) and ct in _TEMPORAL:
+                entry = (name, _VALUE_NAMES[code], column, _FRAME_NAMES[frame])
+                raise _lib.B200Error(f"Streaming Window: {entry!r}: sum and mean need an integer, bool or float column, not a temporal one")
+            valid = default is not None
+            out.append((code, self.phys.index(self.col_names.index(column)), frame, int(valid), arg, _default_bits(f, ct) if valid else 0))
+        return out
+
+    def _ensure(self, table: Table, limit=None, offset=None):
+        if self.handle is None and table.n_cols == len(self.col_names):
+            self.descs = self.descriptors([c.c_type for c in table.columns])
+        super()._ensure(table, limit, offset)
 
     def _new_handle(self, L, c_types, a_types, n_cols, asc, nal, limit, offset):
         np_ = len(self.partition_by)
         oasc = ffi.new("int32_t[]", [int(a) for a in self.asc[np_:]] or [0])
         onal = ffi.new("int32_t[]", [int(x) for x in self.na_last[np_:]] or [0])
-        codes = ffi.new("int32_t[]", [c for _, c, _ in self.funcs])
-        args = ffi.new("int64_t[]", [a for _, _, a in self.funcs])
-        h = L.b200_window_state_init(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, codes, args,
-                                     len(self.funcs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
+        fs = ffi.new("b200_window_func[]", len(self.descs))
+        for d, (code, col, frame, valid, arg, bits) in zip(fs, self.descs):
+            d.code, d.col, d.frame, d.default_valid, d.arg, d.default_bits = code, col, frame, valid, arg, bits
+        h = L.b200_window_state_init_funcs(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs,
+                                           len(self.descs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
         return _lib.check_ptr(h, "init_window_state")
 
 
@@ -122,9 +231,14 @@ def init_window_state(operator_id, partition_by, order_by, ascending, na_positio
     """A window state over batches with columns `col_names`.
 
     partition_by / order_by: a column name or a list of names (either may be empty, 1..4 in all); ascending / na_position: one
-    value or one per ORDER BY key; funcs: [(out_name, fname)] with fname in FUNCS, or (out_name, "ntile", n) with n >= 1.
+    value or one per ORDER BY key; funcs: ranking entries (out_name, fname) with fname in FUNCS, or (out_name, "ntile", n) with
+    n >= 1; value entries (out_name, fname, column[, frame]) with fname in VALUE_FUNCS other than lag / lead, frame one of FRAMES
+    (default "range") and column None for count(*) only, or (out_name, "lag" | "lead", column[, k[, default]]) (k = 1 and
+    default None, NA, by default).
     Raises B200Error for an unknown function, duplicate output names or names that clash with an input column, keys that are
-    missing or not distinct, a key count outside 1..4, a bad na_position, or ntile n < 1."""
+    missing or not distinct, a key count outside 1..4, a bad na_position, ntile n < 1, an unknown value column, a bad frame, a
+    frame on lag or lead, k outside [0, 2^31); and at the first consume call for sum or mean of a temporal column or a lag / lead
+    default that the column's dtype cannot hold exactly."""
     return WindowState(operator_id, partition_by, order_by, ascending, na_position, funcs, col_names, parallel, output_batch_size,
                        device, stream, process_group)
 

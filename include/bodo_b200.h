@@ -244,11 +244,50 @@ void* b200_sort_state_init_full(int64_t operator_id, const int8_t* c_types, cons
  * division of the two integers); all numpy arrays.  The output is every input row once, in the stable sort's order by (partition
  * keys, order keys, arrival): the n_arrs input columns, then one column per function, so `out->cols` of a produce call holds
  * n_arrs + n_funcs descriptors (at most 32).  At most 2^31 rows, as the full sort.  The build-consume, produce, delete and metric
- * entries below serve this form too; metric 9 is the number of partitions. */
+ * entries below serve this form too; metric 9 is the number of partitions.  This entry takes ranking functions only; it is
+ * b200_window_state_init_funcs with one descriptor {funcs[i], -1, 0, 0, func_args[i], 0} per function. */
 void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
                              int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
                              const int32_t* order_na_last, const int32_t* funcs, const int64_t* func_args, int32_t n_funcs,
                              int64_t output_batch_size, int32_t device, void* stream);
+
+/* One window function of b200_window_state_init_funcs.
+ *   code: 0 row_number, 1 rank, 2 dense_rank, 3 percent_rank, 4 cume_dist, 5 ntile (the ranking functions above), then the value
+ *         functions 6 sum, 7 count, 8 mean, 9 min, 10 max, 11 first_value, 12 last_value, 13 lag, 14 lead.
+ *   col: the input column (0 <= col < n_arrs) a value function reads, any column including a key; -1 for a ranking function and
+ *        for count(*).
+ *   frame: 0 for a ranking function, lag and lead; for the others 1 range (RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW: up
+ *          to the row's last peer; the whole partition without ORDER BY), 2 rows (ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT
+ *          ROW: up to the row itself, ties in arrival order), 3 partition (the whole partition).  Every frame starts at the
+ *          partition's first row.
+ *   arg: ntile's n (>= 1); lag / lead's offset k (0 <= k < 2^31; k = 0 is the row itself).
+ *   default_valid, default_bits: lag / lead's value when row i - k / i + k is outside the row's partition: the low bytes of
+ *          default_bits in the column's type if default_valid, else NA.
+ * Over a frame [P, e] (a float NaN is NA for the aggregates):
+ *   count     non-NA cells, or e - P + 1 for count(*); INT64, numpy.
+ *   sum       sum of the non-NA cells, NA when there are none; integers and bool wrap in 64 bits (INT64 for signed and bool,
+ *             UINT64 for unsigned), floats accumulate in double (float32 narrowed once at the end) in an order fixed by the row
+ *             count; nullable.  Not for temporal columns.
+ *   mean      sum / count in double ((double) of the exact 64-bit sum for integers and bool), NA when count = 0; FLOAT64, nullable.
+ *             Not for temporal columns.
+ *   min, max  the cell of the earliest row holding the least / greatest non-NA value, compared by the sort's ascending radix
+ *             word (-0.0 ties 0.0); NA when the frame has no valid cell; the column's type, nullable.
+ *   first_value, last_value  the cell at P / e as it is (bits and validity: a NaN stays a valid NaN); the column's type, nullable.
+ *   lag, lead the cell at i - k / i + k when that row is in the row's partition, else the default; the column's type, nullable.
+ * Every row that shares a frame end gets a bit-identical result. */
+typedef struct b200_window_func {
+    int32_t code, col, frame, default_valid;
+    int64_t arg;
+    uint64_t default_bits;
+} b200_window_func;
+
+/* The window state of b200_window_state_init with ranking and value functions, one descriptor each (n_arrs + n_funcs <= 32).  A
+ * bad code, column index, frame, ntile n or lag / lead k, a frame on a ranking function, lag or lead, or sum / mean of a temporal
+ * column fails here (NULL, last error set).  Function columns follow the input columns in the output, in descriptor order. */
+void* b200_window_state_init_funcs(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                                   int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                                   const int32_t* order_na_last, const b200_window_func* funcs, int32_t n_funcs,
+                                   int64_t output_batch_size, int32_t device, void* stream);
 
 /* The build-consume entry of _sort.cpp: filters a DEVICE-resident batch (same schema as the state) against the current cutoff on
  * the device (full sort: appends it to the chunk store); on is_last reduces to the final rows (full sort: sorts every row).
