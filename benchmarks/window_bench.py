@@ -10,7 +10,10 @@ doubles in [0, 1)) and an int64 row id r, fed in `--batch`-row batches.  Cases:
   running        SUM(r) ROWS, MAX(r) RANGE and COUNT(*) over the partition, OVER (PARTITION BY p ORDER BY o)
   partition_aggs SUM / MEAN / MIN / MAX(o) over the whole partition
   lag_lead       LAG(r, 1) and LEAD(o, 1, 0.0)
-The value cases (the last three) also alternate with rn_rank_dense (rn_rank_dense_ms), so their cost above the ranking kernels
+  moving         AVG(o) and MAX(o) ROWS BETWEEN 6 PRECEDING AND CURRENT ROW, SUM(r) ROWS BETWEEN 3 PRECEDING AND 3 FOLLOWING
+                 and NTH_VALUE(r, 2), OVER (PARTITION BY p ORDER BY o)
+  moving_wide    SUM(r) and MIN(o) ROWS BETWEEN 65535 PRECEDING AND CURRENT ROW OVER (ORDER BY o): one partition, a deep tree
+The value cases (running to moving_wide) also alternate with rn_rank_dense (rn_rank_dense_ms), so their cost above the ranking kernels
 is measured too; their result check covers the validity of the nullable columns.
 One step = init -> consume every batch (is_last on the last) -> produce -> delete, timed with CUDA events on the operator's stream;
 the median of `--reps` steps after one warm-up.  Every window step alternates with a full sort of the same keys and columns in
@@ -39,7 +42,10 @@ FUNCS6 = FUNCS3 + [("pr", "percent_rank"), ("cd", "cume_dist"), ("nt", "ntile", 
 RUNNING = [("sr", "sum", "r", "rows"), ("mr", "max", "r", "range"), ("cz", "count", None, "partition")]
 PARTITION_AGGS = [(f"{f}o", f, "o", "partition") for f in ("sum", "mean", "min", "max")]
 LAG_LEAD = [("lg", "lag", "r", 1), ("ld", "lead", "o", 1, 0.0)]
-VALUE_CASES = ("running", "partition_aggs", "lag_lead")
+MOVING = [("ma", "mean", "o", ("rows", -6, 0)), ("sc", "sum", "r", ("rows", -3, 3)), ("mx", "max", "o", ("rows", -6, 0)),
+          ("n2", "nth_value", "r", 2)]
+MOVING_WIDE = [("sw", "sum", "r", ("rows", -65535, 0)), ("nw", "min", "o", ("rows", -65535, 0))]
+VALUE_CASES = ("running", "partition_aggs", "lag_lead", "moving", "moving_wide")
 
 
 def window_bytes(n, key_bytes, n_funcs, n_parts, n_peers):
@@ -75,6 +81,30 @@ def value_bytes(n, funcs, n_parts, n_peers):
     return int(total)
 
 
+def in_frame_path(f):
+    """Functions over a ("rows", start, end) frame and nth_value run in the frame kernels, not in the scans."""
+    return f[1] == "nth_value" or (len(f) > 3 and isinstance(f[3], tuple))
+
+
+def frame_bytes(n, funcs, n_parts, n_peers):
+    """The frame kernels (8-byte numpy value columns, as value_bytes).  An aggregate over a bounded frame: the tree build reads
+    its column once and writes 4 bytes per row of nodes (16-byte nodes of the levels >= 3); the query pass reads the flags and
+    the partition / peer-group words, the column once more (edge leaves; the nodes and the leaves that neighbouring frames share
+    are counted once) and writes 8 + 1 bytes per row.  The gather pass (count(*), first_value, last_value, nth_value) reads the
+    flags and words once, and per function and row the source cell and its 8 + 1 output bytes (count(*): 8)."""
+    words = n + 4 * (n_parts + n_peers)
+    total, gathers = 0, False
+    for f in funcs:
+        if f[1] == "nth_value" or f[2] is None or f[1] in ("first_value", "last_value"):
+            gathers = True
+            total += n * (8 if f[2] is None else 8 + 8 + 1)
+        else:
+            total += n * (8 + 4) + words + n * (8 + 8 + 1)
+    if gathers:
+        total += words
+    return int(total)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=1 << 28)
@@ -106,7 +136,8 @@ def main():
     names = ["p", "o", "r"]
     torch.cuda.synchronize(dev)
     cases = {"rn_rank_dense": (["p"], FUNCS3), "all6": (["p"], FUNCS6), "no_partition": ([], FUNCS3), "running": (["p"], RUNNING),
-             "partition_aggs": (["p"], PARTITION_AGGS), "lag_lead": (["p"], LAG_LEAD)}
+             "partition_aggs": (["p"], PARTITION_AGGS), "lag_lead": (["p"], LAG_LEAD), "moving": (["p"], MOVING),
+             "moving_wide": ([], MOVING_WIDE)}
 
     def batches():
         for r0 in range(0, n, args.batch):
@@ -219,8 +250,42 @@ def main():
             exp = tot if f[1] == "sum" else tot / s.to(torch.float64)
             return bool(((got - exp).abs() <= 4 * (s + 1).to(torch.float64) * 2.0 ** -53 * exp.abs()).all())
 
+        def frame_ok(j, f):
+            """Bounded frames and nth_value: sums of r as cumsum differences over [lo, hi] (exact); min / max of o over the
+            trailing frame [max(P, i - w + 1), i] from maxima / minima of 2^k rows doubled within the partition (bit for bit);
+            means of o (>= 0) from w shifted terms, within 4 (w + 1) u; nth_value(r, n) over "range" as the cell at P + n - 1
+            when that row is at most the row's last peer, else NA."""
+            got, valid = res[3 + j], res[3 + nf + j]
+            pe = P + s
+            if f[1] == "nth_value":
+                src = P + f[3] - 1
+                inside = src <= qend - 1
+                return torch.equal(valid, inside) and torch.equal(torch.where(inside, got, 0), torch.where(inside, sr[src.clamp(max=n - 1)], 0))
+            _, a, b = f[3]
+            if not bool(valid.all()):  # every frame here holds its own row
+                return False
+            lo, hi = torch.maximum(P, i + a), torch.minimum(pe - 1, i + b)
+            if f[1] == "sum":
+                cs = torch.cat([torch.zeros(1, dtype=torch.int64, device=dev), torch.cumsum(sr, 0)])
+                return torch.equal(got, cs[hi + 1] - cs[lo])
+            w = 1 - a  # trailing frames (b == 0) of w rows
+            if f[1] == "mean":
+                tot = torch.zeros(n, dtype=torch.float64, device=dev)
+                for k in range(w):
+                    tot += torch.where(i - k >= P, torch.roll(so, k), 0.0)
+                exp = tot / (i - lo + 1).to(torch.float64)
+                return bool(((got - exp).abs() <= 4 * (w + 1) * 2.0 ** -53 * exp).all())
+            op, ident = (torch.maximum, float("-inf")) if f[1] == "max" else (torch.minimum, float("inf"))
+            m, K = so.clone(), 0  # m[i]: op over [i - 2^K + 1, i] within the row's partition
+            while (2 << K) <= w:
+                m = op(m, torch.where(i - (1 << K) >= P, torch.roll(m, 1 << K), ident))
+                K += 1
+            j2 = i - w + (1 << K)
+            exp = op(m, torch.where(j2 >= P, m[j2.clamp(min=0)], ident))
+            return torch.equal(got.view(torch.int64), exp.view(torch.int64))
+
         for j, f in enumerate(funcs):
-            good = value_ok(j, f) if f[1] in W.VALUE_FUNCS else torch.equal(res[3 + j].view(torch.int64), expected(f[0]).view(torch.int64))
+            good = frame_ok(j, f) if in_frame_path(f) else value_ok(j, f) if f[1] in W.VALUE_FUNCS else torch.equal(res[3 + j].view(torch.int64), expected(f[0]).view(torch.int64))
             if not good:
                 return f"MISMATCH: {f[0]}", 0, 0
         return "ok", int(ps.sum()), int(qs.sum())
@@ -265,7 +330,9 @@ def main():
         sort_bytes = moved_bytes(n, 24, 0, key_bytes, kp)
         if value_case:  # bounds and ends as the ranking cases (no ranking eval pass), then the value kernels
             ends4 = 4 * (2 * n_parts + n_peers)
-            total = sort_bytes + window_bytes(n, key_bytes, 0, n_parts, n_peers) - (n + ends4) + value_bytes(n, funcs, n_parts, n_peers)
+            scans = [f for f in funcs if not in_frame_path(f)]
+            total = (sort_bytes + window_bytes(n, key_bytes, 0, n_parts, n_peers) - (n + ends4) + value_bytes(n, scans, n_parts, n_peers)
+                     + frame_bytes(n, [f for f in funcs if in_frame_path(f)], n_parts, n_peers))
         else:
             total = sort_bytes + window_bytes(n, key_bytes, len(funcs), n_parts, n_peers)
         out = {"case": name, "rows": n, "batch": args.batch, "funcs": [f[1] for f in funcs], "ms_per_step": round(w_ms, 3),

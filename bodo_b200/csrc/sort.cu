@@ -1381,20 +1381,170 @@ void launch_wv_scan(const WvArgs& a, int64_t n_tiles, cudaStream_t st) {
     window_vscan_kernel<K, true><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
 }
 
+// ---- bounded ROWS frames (k PRECEDING / k FOLLOWING) and NTH_VALUE ----
+//
+// They run after the scans and window_veval_kernel, and only for functions routed here: every function over a bounded frame
+// (frame WF_BOUNDED) and NTH_VALUE over any frame.  A row's frame is [lo, hi] (empty when lo > hi), from wf_bounds only.
+//   window_tree_kernel<K>     per aggregate over a bounded frame (sum, count of a column, mean, min, max): a dyadic block tree over
+//                             the sorted positions, with no partition reset.  Level l holds the combine of each aligned block
+//                             [b 2^l, (b + 1) 2^l) that lies inside [0, n), for l >= 3; levels 0..2 are not stored (the query
+//                             reads them from the sorted column).  A launch takes 2048 inputs per block at level `base` (the
+//                             sorted column for base 0) and builds levels base + 1 .. base + 11, so n < 2^31 takes at most 3.
+//   window_frame_kernel<K>    the ranking scan of the flags (P, Q) again, then per row: the aggregate over [lo, hi] from the tree
+//                             (K a scan kind), or every gather function (K = WV_GATHER): count(*) = max(0, hi - lo + 1),
+//                             first_value / last_value / nth_value(n) = the cell at lo / hi / lo + n - 1 when that lies in [lo, hi].
+// A query combines, left to right, the leaves from lo up to the next multiple of 8 (at most 7), then the largest aligned stored
+// block that starts at the current position and ends by the last multiple of 8 in the frame, repeatedly, then the leaves up to hi
+// (at most 7).  The order depends only on (lo, hi); a frame of W rows takes at most 14 leaves and 2 log2(W) nodes.
+enum { WN_NTH_VALUE = 15 };
+enum { WF_BOUNDED = 4 };
+constexpr int64_t WF_UNBOUNDED_START = INT64_MIN, WF_UNBOUNDED_END = INT64_MAX;
+constexpr int WV_GATHER = 4;            // window_frame_kernel's gather pass (the scan kinds are 0..3)
+constexpr int WT_LOW = 3, WT_LEVELS = 32;  // levels below WT_LOW are not stored; level l < WT_LEVELS
+
+// A function of this path: the value function, its frame bounds (read for WF_BOUNDED only; the unbounded sentinels above) and,
+// in g.k, nth_value's n.
+struct WfFunc {
+    WvFunc g;
+    int64_t start, end;
+};
+
+struct WfArgs {
+    int64_t n;
+    const uint8_t* flags;
+    const WnAgg* tile;              // the ranking scan's tile prefixes
+    const uint32_t *psize, *pend;
+    WvAgg* tree;
+    int64_t off[WT_LEVELS];         // level l's first node in `tree` (l >= WT_LOW); level l holds n >> l nodes
+    WfFunc s;                       // window_tree_kernel / window_frame_kernel<K != WV_GATHER>: the aggregate
+    int n_funcs;                    // window_frame_kernel<WV_GATHER>: the gather functions
+    WfFunc f[SORT_MAX_COLS];
+};
+
+// Row i's frame [lo, hi] in its partition [P, pe), with qe one past its last peer.
+__device__ __forceinline__ void wf_bounds(const WfFunc& g, int64_t i, int64_t P, int64_t pe, int64_t qe, int64_t& lo, int64_t& hi) {
+    lo = P;
+    hi = g.g.frame == WF_ROWS ? i : g.g.frame == WF_RANGE ? qe - 1 : pe - 1;
+    if (g.g.frame == WF_BOUNDED) {
+        if (g.start != WF_UNBOUNDED_START) lo = max(P, i + g.start);
+        if (g.end != WF_UNBOUNDED_END) hi = min(pe - 1, i + g.end);
+    }
+}
+
+__device__ __forceinline__ void wt_store(const WfArgs& a, int l, int64_t b, WvAgg v) {
+    if (l >= WT_LOW && l < WT_LEVELS && b < (a.n >> l)) a.tree[a.off[l] + b] = v;
+}
+
+template <int K>
+__global__ void __launch_bounds__(WN_THREADS) window_tree_kernel(const __grid_constant__ WfArgs a, int base) {
+    __shared__ WvAgg s_node[WN_THREADS];
+    const int64_t n_in = a.n >> base, j0 = (int64_t)blockIdx.x * WN_TILE + threadIdx.x * WN_ITEMS;
+    WvAgg x[WN_ITEMS];
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t j = j0 + k;
+        x[k] = j >= n_in ? wv_identity<K>() : base == 0 ? wv_value<K>(a.s.g, j, false) : a.tree[a.off[base] + j];
+    }
+#pragma unroll
+    for (int h = 1, m = WN_ITEMS / 2; m >= 1; h++, m >>= 1) {  // levels base + 1 .. base + 3 in registers
+#pragma unroll
+        for (int k = 0; k < m; k++) {
+            x[k] = wv_combine<K>(x[2 * k], x[2 * k + 1]);
+            wt_store(a, base + h, (j0 >> h) + k, x[k]);
+        }
+    }
+    s_node[threadIdx.x] = x[0];
+    __syncthreads();
+    for (int h = 4, m = WN_THREADS / 2; m >= 1; h++, m >>= 1) {  // levels base + 4 .. base + 11 in shared memory
+        WvAgg y = x[0];
+        if (threadIdx.x < m) y = wv_combine<K>(s_node[2 * threadIdx.x], s_node[2 * threadIdx.x + 1]);
+        __syncthreads();
+        if (threadIdx.x < m) {
+            s_node[threadIdx.x] = y;
+            wt_store(a, base + h, (int64_t)blockIdx.x * m + threadIdx.x, y);
+        }
+        __syncthreads();
+    }
+}
+
+// The aggregate of the scanned function over [lo, hi]: edge leaves from the sorted column, aligned blocks from the tree.
+template <int K>
+__device__ __forceinline__ WvAgg wt_query(const WfArgs& a, int64_t lo, int64_t hi) {
+    WvAgg acc = wv_identity<K>();
+    const int64_t r = hi + 1, a8 = min(r, (lo + 7) & ~(int64_t)7);
+    int64_t j = lo;
+    for (; j < a8; j++) acc = wv_combine<K>(acc, wv_value<K>(a.s.g, j, false));
+    const int64_t b8 = max(j, r & ~(int64_t)7);
+    while (j < b8) {  // j and b8 are multiples of 8, so l >= 3
+        const int l = min(j == 0 ? 62 : __ffsll(j) - 1, 63 - __clzll(b8 - j));
+        acc = wv_combine<K>(acc, a.tree[a.off[l] + (j >> l)]);
+        j += (int64_t)1 << l;
+    }
+    for (; j < r; j++) acc = wv_combine<K>(acc, wv_value<K>(a.s.g, j, false));
+    return acc;
+}
+
+template <int K>
+__global__ void __launch_bounds__(WN_THREADS) window_frame_kernel(const __grid_constant__ WfArgs a) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    constexpr int KQ = K == WV_GATHER ? WV_ISUM : K;  // the scan kind of the aggregate pass
+    const int64_t t = blockIdx.x;
+    WnArgs w;  // wn_scan_tile reads n, flags and the tile prefixes only
+    w.n = a.n; w.flags = const_cast<uint8_t*>(a.flags); w.tile = const_cast<WnAgg*>(a.tile);
+    uint8_t f[WN_ITEMS];
+    WnAgg v[WN_ITEMS];
+    wn_scan_tile(w, t, f, v);
+    __shared__ WnAgg s_v[WN_ITEMS][WN_THREADS];  // parked as in window_eval_kernel: the item loop is not unrolled
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) s_v[k][threadIdx.x] = v[k];
+#pragma unroll 1
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        if (i >= a.n) break;
+        const WnAgg vk = s_v[k][threadIdx.x];
+        const int64_t P = vk.p, pe = P + a.psize[vk.p], qe = a.pend[vk.q];
+        int64_t lo, hi;
+        if (K != WV_GATHER) {
+            wf_bounds(a.s, i, P, pe, qe, lo, hi);
+            wv_write<KQ>(a.s.g, i, wt_query<KQ>(a, lo, hi));
+        } else for (int fn = 0; fn < a.n_funcs; fn++) {
+            const WfFunc& g = a.f[fn];
+            wf_bounds(g, i, P, pe, qe, lo, hi);
+            if (g.g.size == 0) { ((int64_t*)g.g.out)[i] = max(hi - lo + 1, (int64_t)0); continue; }  // count(*)
+            const int64_t src = g.g.code == WN_FIRST_VALUE ? lo : g.g.code == WN_LAST_VALUE ? hi : lo + g.g.k - 1;
+            const bool in = lo <= hi && src <= hi;
+            if (in) copy_cell(g.g.out, i, g.g.data, src, g.g.size);
+            else wv_store_bits(g.g.out, i, 0, g.g.size);
+            g.g.out_vb[i] = in && (!g.g.vb || g.g.vb[src]);
+        }
+    }
+}
+
+// Build the tree of the aggregate a.s (levels WT_LOW.. up to log2 n), then evaluate it at every row.
+template <int K>
+void launch_wf_tree(const WfArgs& a, int64_t n_tiles, cudaStream_t st) {
+    for (int base = 0; (a.n >> max(base + 1, WT_LOW)) > 0; base += 11)
+        window_tree_kernel<K><<<(unsigned)(((a.n >> base) + WN_TILE - 1) / WN_TILE), WN_THREADS, 0, st>>>(a, base);
+    window_frame_kernel<K><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
+}
+
 // Ranking and value window functions over (PARTITION BY the first n_part keys ORDER BY the rest).  The output is the full sort's,
 // plus one column per function after the input columns: numpy for the ranking functions and count, nullable for the others.
 struct WindowState : FullSortState {
     int n_part, n_funcs;
     b200_window_func fn[SORT_MAX_COLS];
+    b200_window_frame bound[SORT_MAX_COLS];  // a WF_BOUNDED function's frame
     std::vector<DevBuf> fout;
     int64_t n_partitions = 0;  // metric 9
 
     WindowState(const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_part_, int n_keys, const int32_t* asc,
-                const int32_t* na_last, const b200_window_func* funcs, int n_funcs_, int64_t obs, int dev, cudaStream_t st)
+                const int32_t* na_last, const b200_window_func* funcs, const b200_window_frame* frames, int n_funcs_, int64_t obs,
+                int dev, cudaStream_t st)
         : FullSortState(c_types, arr_types, n_arrs, n_keys, asc, na_last, obs, dev, st), n_part(n_part_), n_funcs(n_funcs_) {
         for (int f = 0; f < n_funcs; f++) {
-            const b200_window_func& d = fn[f] = funcs[f];
-            B200_REQUIRE(d.code >= WN_ROW_NUMBER && d.code <= WN_LEAD, "b200 window: unknown function code");
+            b200_window_func& d = fn[f] = funcs[f];
+            bound[f] = b200_window_frame{WF_UNBOUNDED_START, WF_UNBOUNDED_END};
+            B200_REQUIRE(d.code >= WN_ROW_NUMBER && d.code <= WN_NTH_VALUE, "b200 window: unknown function code");
             int ct = CT_INT64, at = ARR_NUMPY;
             if (d.code <= WN_NTILE) {
                 B200_REQUIRE(d.col == -1 && d.frame == WF_NONE, "b200 window: a ranking function takes no column and no frame");
@@ -1408,7 +1558,23 @@ struct WindowState : FullSortState {
                     B200_REQUIRE(d.arg >= 0 && d.arg <= 0x7FFFFFFF, "b200 window: lag / lead offset k must be in [0, 2^31)");
                     B200_REQUIRE(d.default_valid == 0 || d.default_valid == 1, "b200 window: default_valid must be 0 or 1");
                 } else {
-                    B200_REQUIRE(d.frame >= WF_RANGE && d.frame <= WF_PARTITION, "b200 window: unknown frame (1 range, 2 rows, 3 partition)");
+                    B200_REQUIRE(d.frame >= WF_RANGE && d.frame <= WF_BOUNDED,
+                                 "b200 window: unknown frame (1 range, 2 rows, 3 partition, 4 rows between)");
+                }
+                if (d.code == WN_NTH_VALUE) B200_REQUIRE(d.arg >= 1 && d.arg <= 0x7FFFFFFF, "b200 window: nth_value needs n in [1, 2^31)");
+                if (d.frame == WF_BOUNDED) {
+                    B200_REQUIRE(frames, "b200 window: frame 4 (rows between) needs frames[i]");
+                    const b200_window_frame b = frames[f];
+                    const int64_t lim = 0x7FFFFFFF;
+                    B200_REQUIRE((b.start == WF_UNBOUNDED_START || (b.start >= -lim && b.start <= lim)) &&
+                                 (b.end == WF_UNBOUNDED_END || (b.end >= -lim && b.end <= lim)),
+                                 "b200 window: a frame bound is UNBOUNDED or a row offset in (-2^31, 2^31)");
+                    B200_REQUIRE(b.start == WF_UNBOUNDED_START || b.end == WF_UNBOUNDED_END || b.start <= b.end,
+                                 "b200 window: frame start after frame end");
+                    bound[f] = b;
+                    // the spellings of the unbounded frames: the same frame gives the same bits however it is written
+                    if (b.start == WF_UNBOUNDED_START && b.end == 0) d.frame = WF_ROWS;
+                    else if (b.start == WF_UNBOUNDED_START && b.end == WF_UNBOUNDED_END) d.frame = WF_PARTITION;
                 }
                 const int vct = d.col >= 0 ? sc.ctype[d.col] : CT_INT64;
                 const bool temporal = vct == CT_DATE || vct == CT_DATETIME || vct == CT_TIMEDELTA;
@@ -1434,6 +1600,8 @@ struct WindowState : FullSortState {
         for (int j = 0; j < sc.n_keys; j++) { a.key[j] = sc.key[j]; a.data[j] = out_data[j]; a.vb[j] = out_vb[j]; }
         WvArgs va{};
         std::vector<WvFunc> scans;
+        WfArgs fa{};
+        std::vector<WfFunc> trees;
         bool eval = false;
         for (int f = 0; f < n_funcs; f++) {
             const int c = sc.n_cols + f;
@@ -1449,6 +1617,12 @@ struct WindowState : FullSortState {
             WvFunc g{d.code, d.frame, d.col >= 0 ? sc.ctype[d.col] : CT_INT64, d.col >= 0 ? ctype_size(sc.ctype[d.col]) : 0,
                      ctype_size(sc.ctype[c]), d.default_valid, d.arg, d.default_bits, d.col >= 0 ? out_data[d.col] : nullptr,
                      d.col >= 0 ? out_vb[d.col] : nullptr, out_data[c], out_vb[c]};
+            if (d.frame == WF_BOUNDED || d.code == WN_NTH_VALUE) {  // the frame path only
+                const WfFunc h{g, bound[f].start, bound[f].end};
+                if (d.code <= WN_MAX && d.col >= 0) trees.push_back(h);
+                else fa.f[fa.n_funcs++] = h;
+                continue;
+            }
             const bool scanned = d.code <= WN_MAX && d.col >= 0;
             if (scanned) scans.push_back(g);
             if (!scanned || d.frame != WF_ROWS) { va.f[va.n_funcs++] = g; eval = true; }
@@ -1480,6 +1654,23 @@ struct WindowState : FullSortState {
         }
         if (eval) window_veval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a, va);
         B200_CUDA(cudaGetLastError());
+        DevBuf tree;  // one tree buffer, reused by every aggregate over a bounded frame: n / 8 + n / 16 + ... nodes, <= 4 B per row
+        if (!trees.empty() || fa.n_funcs > 0) {
+            fa.n = n; fa.flags = a.flags; fa.tile = a.tile; fa.psize = a.psize; fa.pend = a.pend;
+            int64_t nodes = 0;
+            for (int l = WT_LOW; l < WT_LEVELS; l++) { fa.off[l] = nodes; nodes += n >> l; }
+            if (!trees.empty()) tree.alloc((size_t)std::max<int64_t>(nodes, 1) * sizeof(WvAgg));
+            fa.tree = tree.as<WvAgg>();
+            for (const WfFunc& h : trees) {
+                fa.s = h;
+                if (h.g.code == WN_MIN) launch_wf_tree<WV_MIN>(fa, n_tiles, stream);
+                else if (h.g.code == WN_MAX) launch_wf_tree<WV_MAX>(fa, n_tiles, stream);
+                else if (h.g.code != WN_COUNT && ctype_is_float(h.g.ct)) launch_wf_tree<WV_FSUM>(fa, n_tiles, stream);
+                else launch_wf_tree<WV_ISUM>(fa, n_tiles, stream);
+            }
+            if (fa.n_funcs > 0) window_frame_kernel<WV_GATHER><<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(fa);
+            B200_CUDA(cudaGetLastError());
+        }
         auto* h = (uint32_t*)pinned_acquire(8);
         B200_CUDA(cudaMemcpyAsync(h, totals.p, 8, cudaMemcpyDeviceToHost, stream));
         B200_CUDA(cudaStreamSynchronize(stream));
@@ -1533,6 +1724,22 @@ void* b200_window_state_init_funcs(int64_t operator_id, const int8_t* c_types, c
                                    int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
                                    const int32_t* order_na_last, const b200_window_func* funcs, int32_t n_funcs, int64_t output_batch_size,
                                    int32_t device, void* stream) {
+    try {  // this entry's domain: codes 0..14, frames 0..3 (the frame entry adds nth_value and bounded frames)
+        for (int f = 0; funcs && f < n_funcs && f < b200::SORT_MAX_COLS; f++) {
+            B200_REQUIRE(funcs[f].code >= b200::WN_ROW_NUMBER && funcs[f].code <= b200::WN_LEAD, "b200 window: unknown function code");
+            if (funcs[f].code >= b200::WN_SUM && funcs[f].code <= b200::WN_LAST_VALUE)
+                B200_REQUIRE(funcs[f].frame >= b200::WF_RANGE && funcs[f].frame <= b200::WF_PARTITION,
+                             "b200 window: unknown frame (1 range, 2 rows, 3 partition)");
+        }
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
+    return b200_window_state_init_frames(operator_id, c_types, arr_types, n_arrs, n_partition_keys, n_order_keys, order_ascending,
+                                         order_na_last, funcs, nullptr, n_funcs, output_batch_size, device, stream);
+}
+
+void* b200_window_state_init_frames(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                                    int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                                    const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
+                                    int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream) {
     (void)operator_id;
     return b200::sort_state_new(device, [&]() -> SortState* {
         const int np = n_partition_keys, no = n_order_keys;
@@ -1547,8 +1754,8 @@ void* b200_window_state_init_funcs(int64_t operator_id, const int8_t* c_types, c
             asc[j] = j < np ? 1 : order_ascending[j - np];
             na_last[j] = j < np ? 1 : order_na_last[j - np];
         }
-        return new b200::WindowState(c_types, arr_types, n_arrs, np, np + no, asc, na_last, funcs, n_funcs, output_batch_size, device,
-                                     (cudaStream_t)stream);
+        return new b200::WindowState(c_types, arr_types, n_arrs, np, np + no, asc, na_last, funcs, frames, n_funcs, output_batch_size,
+                                     device, (cudaStream_t)stream);
     });
 }
 

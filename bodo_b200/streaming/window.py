@@ -3,6 +3,7 @@
     ROW_NUMBER() / RANK() / DENSE_RANK() / PERCENT_RANK() / CUME_DIST() / NTILE(n) OVER (PARTITION BY p ORDER BY o)
     SUM / COUNT / AVG / MIN / MAX / FIRST_VALUE / LAST_VALUE (x) OVER (PARTITION BY p ORDER BY o [frame])
     LAG / LEAD (x, k, default) OVER (PARTITION BY p ORDER BY o)
+    NTH_VALUE (x, n) OVER (PARTITION BY p ORDER BY o [frame]), and every frame function over ROWS BETWEEN k PRECEDING AND k FOLLOWING
 
 pandas equivalents: groupby(p).cumcount() + 1, groupby(p)[o].rank(method="min" / "dense" / "max", pct=...),
 groupby(p)[x].cumsum() / cummin() / cummax() (the "rows" frame), groupby(p)[x].transform("sum" / "mean" / "min" / "max" /
@@ -28,7 +29,12 @@ Semantics:
     end at e: "range" (the default; SQL's default frame RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW) at the row's last peer,
     which is the partition's last row without ORDER BY; "rows" (ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW) at the row
     itself, ties in arrival order; "partition" (ROWS BETWEEN UNBOUNDED PRECEDING AND UNBOUNDED FOLLOWING) at the partition's last
-    row.  Bounded frames (k PRECEDING / FOLLOWING) are not supported.  Over [P, e], with a float NaN counted as NA:
+    row.  ("rows", start, end) is ROWS BETWEEN start AND end, each None (UNBOUNDED) or an integer row offset in (-2^31, 2^31)
+    (negative PRECEDING, 0 CURRENT ROW, positive FOLLOWING; start <= end when both are offsets): for row i of the partition
+    [P, pe) the frame is [lo, hi] with lo = P (start None) or max(P, i + start), hi = pe - 1 (end None) or min(pe - 1, i + end),
+    empty when lo > hi.  ("rows", None, 0) is "rows" and ("rows", None, None) is "partition".  It takes sum, count, mean, min,
+    max, first_value, last_value and nth_value, which are then defined as below with [lo, hi] in place of [P, e]; an empty frame
+    gives NA (count 0).  Over [P, e], with a float NaN counted as NA:
       count(x): non-NA cells, count(None): COUNT(*) = e - P + 1; int64 numpy.
       sum(x): the sum of the non-NA cells, NA when there are none; integers and bool wrap in 64 bits (int64 for signed and bool,
         uint64 for unsigned), floats accumulate in double (float32 narrowed once at the end); nullable.
@@ -39,12 +45,16 @@ Semantics:
         nullable.
       first_value(x) / last_value(x): the cell at P / e as it is, bits and validity (a NaN stays a valid NaN, SQL RESPECT NULLS);
         x's type, nullable.
+      nth_value(x, n): the cell at P + n - 1 as first_value gives it when that row is in the frame, else NA; 1 <= n < 2^31;
+        frame "range" by default; x's type, nullable.
       lag(x, k=1, default=None) / lead(...): the cell at i - k / i + k if that row is in the row's partition, else default (NA
         when None); 0 <= k < 2^31, k = 0 is the row itself; no frame; x's type, nullable.  default is converted to x's numpy
         dtype and must round-trip exactly.
     These follow SQL where pandas differs: groupby().cumsum() / cummin() / cummax() give NA at NA rows where the "rows" frame
     gives the aggregate so far; transform("sum") of an all-NA partition gives 0 where sum gives NA; float sums are combined in
-    the scan's order, not sequentially.  Results depend only on the sorted positions: every row that shares a frame end gets a
+    the scan's order, not sequentially.  Over ("rows", start, end) the results are pandas' groupby(p)[x].rolling(w,
+    min_periods=1) ones (count: min_periods=0), with float sums combined in an order that depends only on the frame's bounds.
+    Results depend only on the sorted positions: every row that shares a frame end (a bounded frame: both bounds) gets a
     bit-identical result, and float sums are bit-identical across runs and across any split of the rows into batches.
   - output: every input row once, in the stable sort's order by (partition keys, order keys, arrival); every input column in
     input order, then one column per function under the caller's name.  SQL leaves the order open; fixing it makes every column
@@ -68,15 +78,22 @@ from .sort import MAX_FULL_SORT_ROWS, MAX_KEYS, SortState
 FUNCS = {"row_number": 0, "rank": 1, "dense_rank": 2, "percent_rank": 3, "cume_dist": 4, "ntile": 5}
 VALUE_FUNCS = {"sum": 6, "count": 7, "mean": 8, "min": 9, "max": 10, "first_value": 11, "last_value": 12, "lag": 13, "lead": 14}
 FRAMES = {"range": 1, "rows": 2, "partition": 3}
-_VALUE_NAMES = {c: f for f, c in VALUE_FUNCS.items()}
+# The frame entry's codes (b200_window_state_init_frames): nth_value, and ROWS BETWEEN start AND end with its UNBOUNDED sentinels.
+FRAME_FUNCS = {"nth_value": 15}
+ROWS_BETWEEN = 4
+UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING = -(1 << 63), (1 << 63) - 1
+BOUNDED_FUNCS = ("sum", "count", "mean", "min", "max", "first_value", "last_value", "nth_value")
+_VALUE_NAMES = {c: f for f, c in {**VALUE_FUNCS, **FRAME_FUNCS}.items()}
 _FRAME_NAMES = {c: f for f, c in FRAMES.items()}
 MAX_COLS = 32
 MAX_WINDOW_ROWS = MAX_FULL_SORT_ROWS
 MAX_LAG = (1 << 31) - 1
+MAX_FRAME_OFFSET = MAX_LAG
 _TEMPORAL = (CTypes.DATE, CTypes.DATETIME, CTypes.TIMEDELTA)
 _FORMS = (f"ranking: (out_name, fname) with fname in {sorted(FUNCS)}, or (out_name, 'ntile', n); value: (out_name, fname, column"
-          f"[, frame]) with fname in {sorted(set(VALUE_FUNCS) - {'lag', 'lead'})}, frame in {sorted(FRAMES)}, column None for "
-          "count(*) only, or (out_name, 'lag' | 'lead', column[, k[, default]])")
+          f"[, frame]) with fname in {sorted(set(VALUE_FUNCS) - {'lag', 'lead'})}, frame in {sorted(FRAMES)} or ('rows', start, end), "
+          "column None for count(*) only, or (out_name, 'lag' | 'lead', column[, k[, default]]), or (out_name, 'nth_value', column, "
+          "n[, frame])")
 
 
 def _names(x):
@@ -86,8 +103,9 @@ def _names(x):
 
 
 def _parse_value(f, col_names):
-    """(out_name, fname, column[, frame]) or (out_name, 'lag' | 'lead', column[, k[, default]]) -> (out_name, code, k, column,
-    frame code, default); frame code 0 for lag and lead."""
+    """(out_name, fname, column[, frame]), (out_name, 'lag' | 'lead', column[, k[, default]]) or (out_name, 'nth_value', column,
+    n[, frame]) -> (out_name, code, k, column, frame code, default[, (start, end)]); frame code 0 for lag and lead, k = n for
+    nth_value, (start, end) for a ROWS_BETWEEN frame only."""
     name, fname, column = f[0], f[1], f[2]
     if not (column is None and fname == "count") and not (isinstance(column, str) and column in col_names):
         raise _lib.B200Error(f"Streaming Window: {f!r}: unknown column {column!r} (one of {col_names}; None for count only)")
@@ -100,10 +118,42 @@ def _parse_value(f, col_names):
         if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or not 0 <= k <= MAX_LAG:
             raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} needs an integer k with 0 <= k < 2^31")
         return (name, VALUE_FUNCS[fname], int(k), column, 0, f[4] if len(f) > 4 else None)
-    frame = f[3] if len(f) > 3 else "range"
-    if len(f) > 4 or not isinstance(frame, str) or frame not in FRAMES:
-        raise _lib.B200Error(f"Streaming Window: {f!r}: bad frame (one of {sorted(FRAMES)}, as (out_name, {fname!r}, column[, frame]))")
-    return (name, VALUE_FUNCS[fname], 0, column, FRAMES[frame], None)
+    if fname == "nth_value":
+        nth = f[3] if len(f) > 3 else None
+        if len(f) > 5 or isinstance(nth, (bool, np.bool_)) or not isinstance(nth, (int, np.integer)) or not 1 <= nth <= MAX_LAG:
+            raise _lib.B200Error(f"Streaming Window: {f!r}: nth_value takes (out_name, 'nth_value', column, n[, frame]) with an integer "
+                                 "1 <= n < 2^31")
+        return (name, FRAME_FUNCS[fname], int(nth), column, *_parse_frame(f, f[4] if len(f) > 4 else "range"))
+    if len(f) > 4:
+        raise _lib.B200Error(f"Streaming Window: {f!r}: bad frame (one of {sorted(FRAMES)} or ('rows', start, end), as (out_name, "
+                             f"{fname!r}, column[, frame]))")
+    return (name, VALUE_FUNCS[fname], 0, column, *_parse_frame(f, f[3] if len(f) > 3 else "range"))
+
+
+def _parse_frame(f, frame):
+    """A frame name, or ("rows", start, end) with start / end None (UNBOUNDED) or a row offset (negative PRECEDING, 0 CURRENT ROW,
+    positive FOLLOWING) -> (frame code, default None[, (start, end)]).  ("rows", None, 0) is "rows" and ("rows", None, None) is
+    "partition", so a frame gives the same results however it is spelled."""
+    if isinstance(frame, str) and frame in FRAMES:
+        return FRAMES[frame], None
+    if not (isinstance(frame, (tuple, list)) and len(frame) == 3 and frame[0] == "rows"):
+        raise _lib.B200Error(f"Streaming Window: {f!r}: bad frame (one of {sorted(FRAMES)} or ('rows', start, end), as (out_name, "
+                             f"{f[1]!r}, column[, frame]))")
+    start, end = frame[1], frame[2]
+    for b in (start, end):
+        if b is not None and (isinstance(b, (bool, np.bool_)) or not isinstance(b, (int, np.integer))
+                              or not -MAX_FRAME_OFFSET <= b <= MAX_FRAME_OFFSET):
+            raise _lib.B200Error(f"Streaming Window: {f!r}: bad frame bound {b!r} (None for UNBOUNDED or an integer row offset in "
+                                 "(-2^31, 2^31))")
+    if start is not None and end is not None and start > end:
+        raise _lib.B200Error(f"Streaming Window: {f!r}: frame start {start} is after frame end {end}")
+    if f[1] not in BOUNDED_FUNCS:
+        raise _lib.B200Error(f"Streaming Window: {f!r}: a ('rows', start, end) frame takes one of {list(BOUNDED_FUNCS)}")
+    if start is None and end == 0:
+        return FRAMES["rows"], None
+    if start is None and end is None:
+        return FRAMES["partition"], None
+    return (ROWS_BETWEEN, None, (UNBOUNDED_PRECEDING if start is None else int(start), UNBOUNDED_FOLLOWING if end is None else int(end)))
 
 
 def _default_bits(f, ct):
@@ -124,15 +174,17 @@ def _default_bits(f, ct):
 
 
 def _parse_funcs(funcs, col_names):
-    """Ranking entries -> (out_name, code, n); value entries -> (out_name, code, k, column, frame code, default)."""
+    """Ranking entries -> (out_name, code, n); value entries -> (out_name, code, k, column, frame code, default), with a
+    seventh field (start, end) for a ROWS_BETWEEN frame."""
     out = []
     for f in funcs:
         f = tuple(f)
-        if (len(f) < 2 or not isinstance(f[0], str) or not isinstance(f[1], str) or f[1] not in FUNCS and f[1] not in VALUE_FUNCS
-                or f[1] in VALUE_FUNCS and len(f) < 3):
+        value = isinstance(f[1] if len(f) > 1 else None, str) and (f[1] in VALUE_FUNCS or f[1] in FRAME_FUNCS)
+        if (len(f) < 2 or not isinstance(f[0], str) or not isinstance(f[1], str) or f[1] not in FUNCS and not value
+                or value and len(f) < 3):
             raise _lib.B200Error(f"Streaming Window: unknown window function {f!r} ({_FORMS})")
         name, fname = f[0], f[1]
-        if fname in VALUE_FUNCS:
+        if value:
             out.append(_parse_value(f, col_names))
             continue
         if fname == "ntile":
@@ -197,17 +249,23 @@ class WindowState(SortState):
             if len(f) == 3:
                 out.append((f[1], -1, 0, 0, f[2], 0))
                 continue
-            name, code, arg, column, frame, default = f
+            name, code, arg, column, frame, default = f[:6]
             if column is None:
                 out.append((code, -1, frame, 0, arg, 0))
                 continue
             ct = c_types[self.col_names.index(column)]
             if code in (VALUE_FUNCS["sum"], VALUE_FUNCS["mean"]) and ct in _TEMPORAL:
-                entry = (name, _VALUE_NAMES[code], column, _FRAME_NAMES[frame])
+                bounds = [None if b in (UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING) else b for b in f[6]] if len(f) > 6 else None
+                entry = (name, _VALUE_NAMES[code], column, _FRAME_NAMES[frame] if bounds is None else ("rows", *bounds))
                 raise _lib.B200Error(f"Streaming Window: {entry!r}: sum and mean need an integer, bool or float column, not a temporal one")
             valid = default is not None
             out.append((code, self.phys.index(self.col_names.index(column)), frame, int(valid), arg, _default_bits(f, ct) if valid else 0))
         return out
+
+    def frames(self):
+        """The b200_window_frame (start, end) of every function: its bounds for a ('rows', start, end) frame (code ROWS_BETWEEN),
+        else (UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING), which the library does not read."""
+        return [f[6] if len(f) > 6 else (UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING) for f in self.funcs]
 
     def _ensure(self, table: Table, limit=None, offset=None):
         if self.handle is None and table.n_cols == len(self.col_names):
@@ -221,8 +279,11 @@ class WindowState(SortState):
         fs = ffi.new("b200_window_func[]", len(self.descs))
         for d, (code, col, frame, valid, arg, bits) in zip(fs, self.descs):
             d.code, d.col, d.frame, d.default_valid, d.arg, d.default_bits = code, col, frame, valid, arg, bits
-        h = L.b200_window_state_init_funcs(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs,
-                                           len(self.descs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
+        frs = ffi.new("b200_window_frame[]", len(self.descs))
+        for d, (start, end) in zip(frs, self.frames()):
+            d.start, d.end = start, end
+        h = L.b200_window_state_init_frames(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs, frs,
+                                            len(self.descs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
         return _lib.check_ptr(h, "init_window_state")
 
 
@@ -233,11 +294,12 @@ def init_window_state(operator_id, partition_by, order_by, ascending, na_positio
     partition_by / order_by: a column name or a list of names (either may be empty, 1..4 in all); ascending / na_position: one
     value or one per ORDER BY key; funcs: ranking entries (out_name, fname) with fname in FUNCS, or (out_name, "ntile", n) with
     n >= 1; value entries (out_name, fname, column[, frame]) with fname in VALUE_FUNCS other than lag / lead, frame one of FRAMES
-    (default "range") and column None for count(*) only, or (out_name, "lag" | "lead", column[, k[, default]]) (k = 1 and
-    default None, NA, by default).
+    (default "range") or ("rows", start, end) and column None for count(*) only, (out_name, "lag" | "lead", column[, k[,
+    default]]) (k = 1 and default None, NA, by default), or (out_name, "nth_value", column, n[, frame]).
+    Example, a 7-row moving average: ("ma7", "mean", "x", ("rows", -6, 0)).
     Raises B200Error for an unknown function, duplicate output names or names that clash with an input column, keys that are
-    missing or not distinct, a key count outside 1..4, a bad na_position, ntile n < 1, an unknown value column, a bad frame, a
-    frame on lag or lead, k outside [0, 2^31); and at the first consume call for sum or mean of a temporal column or a lag / lead
+    missing or not distinct, a key count outside 1..4, a bad na_position, ntile n < 1, an unknown value column, a bad frame or
+    frame bound, a frame on lag or lead, k outside [0, 2^31), nth_value n outside [1, 2^31); and at the first consume call for sum or mean of a temporal column or a lag / lead
     default that the column's dtype cannot hold exactly."""
     return WindowState(operator_id, partition_by, order_by, ascending, na_position, funcs, col_names, parallel, output_batch_size,
                        device, stream, process_group)

@@ -253,14 +253,17 @@ void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const i
 
 /* One window function of b200_window_state_init_funcs.
  *   code: 0 row_number, 1 rank, 2 dense_rank, 3 percent_rank, 4 cume_dist, 5 ntile (the ranking functions above), then the value
- *         functions 6 sum, 7 count, 8 mean, 9 min, 10 max, 11 first_value, 12 last_value, 13 lag, 14 lead.
+ *         functions 6 sum, 7 count, 8 mean, 9 min, 10 max, 11 first_value, 12 last_value, 13 lag, 14 lead, 15 nth_value
+ *         (b200_window_state_init_frames only).
  *   col: the input column (0 <= col < n_arrs) a value function reads, any column including a key; -1 for a ranking function and
  *        for count(*).
  *   frame: 0 for a ranking function, lag and lead; for the others 1 range (RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW: up
  *          to the row's last peer; the whole partition without ORDER BY), 2 rows (ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT
- *          ROW: up to the row itself, ties in arrival order), 3 partition (the whole partition).  Every frame starts at the
- *          partition's first row.
- *   arg: ntile's n (>= 1); lag / lead's offset k (0 <= k < 2^31; k = 0 is the row itself).
+ *          ROW: up to the row itself, ties in arrival order), 3 partition (the whole partition).  Frames 1..3 start at the
+ *          partition's first row.  4 rows between (b200_window_state_init_frames only): ROWS BETWEEN start AND end of the
+ *          function's b200_window_frame, for sum, count (of a column or count(*)), mean, min, max, first_value, last_value and
+ *          nth_value.
+ *   arg: ntile's n (>= 1); lag / lead's offset k (0 <= k < 2^31; k = 0 is the row itself); nth_value's n (1 <= n < 2^31).
  *   default_valid, default_bits: lag / lead's value when row i - k / i + k is outside the row's partition: the low bytes of
  *          default_bits in the column's type if default_valid, else NA.
  * Over a frame [P, e] (a float NaN is NA for the aggregates):
@@ -274,12 +277,27 @@ void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const i
  *             word (-0.0 ties 0.0); NA when the frame has no valid cell; the column's type, nullable.
  *   first_value, last_value  the cell at P / e as it is (bits and validity: a NaN stays a valid NaN); the column's type, nullable.
  *   lag, lead the cell at i - k / i + k when that row is in the row's partition, else the default; the column's type, nullable.
- * Every row that shares a frame end gets a bit-identical result. */
+ *   nth_value the cell at P + n - 1 as it is when that row is in the frame, else NA; the column's type, nullable.
+ * Every row that shares a frame end gets a bit-identical result.
+ * Over a frame 4 [lo, hi] (below) the same definitions hold with lo in place of P and hi in place of e; an empty frame (lo > hi)
+ * gives NA, and count 0.  Float sums there are combined in an order fixed by (lo, hi) alone, so rows with the same bounds get the
+ * same bits, across runs and batch splits. */
 typedef struct b200_window_func {
     int32_t code, col, frame, default_valid;
     int64_t arg;
     uint64_t default_bits;
 } b200_window_func;
+
+/* The bounds of a frame 4 (ROWS BETWEEN start AND end): each UNBOUNDED (the sentinels below) or a signed row offset from the
+ * current row, -2^31 < offset < 2^31: negative PRECEDING, 0 CURRENT ROW, positive FOLLOWING; start <= end when both are offsets.
+ * For row i of the partition [P, pe) (sorted positions) the frame is [lo, hi] with lo = P for an unbounded start, else
+ * max(P, i + start), and hi = pe - 1 for an unbounded end, else min(pe - 1, i + end); it is empty when lo > hi.
+ * (UNBOUNDED, 0) is frame 2 and (UNBOUNDED, UNBOUNDED) frame 3, with the same results. */
+#define B200_WINDOW_UNBOUNDED_PRECEDING INT64_MIN
+#define B200_WINDOW_UNBOUNDED_FOLLOWING INT64_MAX
+typedef struct b200_window_frame {
+    int64_t start, end;
+} b200_window_frame;
 
 /* The window state of b200_window_state_init with ranking and value functions, one descriptor each (n_arrs + n_funcs <= 32).  A
  * bad code, column index, frame, ntile n or lag / lead k, a frame on a ranking function, lag or lead, or sum / mean of a temporal
@@ -288,6 +306,15 @@ void* b200_window_state_init_funcs(int64_t operator_id, const int8_t* c_types, c
                                    int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
                                    const int32_t* order_na_last, const b200_window_func* funcs, int32_t n_funcs,
                                    int64_t output_batch_size, int32_t device, void* stream);
+
+/* b200_window_state_init_funcs with codes 0..15 and frames 0..4: frames[i] is read only when funcs[i].frame == 4 (frames may be
+ * NULL when no function uses frame 4).  A bound outside the domain above, start > end, frame 4 on a function other than sum,
+ * count, mean, min, max, first_value, last_value and nth_value, or nth_value's n outside [1, 2^31) fails here (NULL, last error
+ * set).  b200_window_state_init_funcs is this entry with frames NULL, restricted to codes 0..14 and frames 0..3. */
+void* b200_window_state_init_frames(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                                    int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                                    const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
+                                    int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream);
 
 /* The build-consume entry of _sort.cpp: filters a DEVICE-resident batch (same schema as the state) against the current cutoff on
  * the device (full sort: appends it to the chunk store); on is_last reduces to the final rows (full sort: sorts every row).
