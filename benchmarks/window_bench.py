@@ -13,7 +13,9 @@ doubles in [0, 1)) and an int64 row id r, fed in `--batch`-row batches.  Cases:
   moving         AVG(o) and MAX(o) ROWS BETWEEN 6 PRECEDING AND CURRENT ROW, SUM(r) ROWS BETWEEN 3 PRECEDING AND 3 FOLLOWING
                  and NTH_VALUE(r, 2), OVER (PARTITION BY p ORDER BY o)
   moving_wide    SUM(r) and MIN(o) ROWS BETWEEN 65535 PRECEDING AND CURRENT ROW OVER (ORDER BY o): one partition, a deep tree
-The value cases (running to moving_wide) also alternate with rn_rank_dense (rn_rank_dense_ms), so their cost above the ranking kernels
+  moments        STDDEV(o) ROWS BETWEEN 19 PRECEDING AND CURRENT ROW (a Bollinger band's width), VAR(o) ROWS (running) and
+                 STDDEV_POP(o) over the partition, OVER (PARTITION BY p ORDER BY o)
+The value cases (running to moments) also alternate with rn_rank_dense (rn_rank_dense_ms), so their cost above the ranking kernels
 is measured too; their result check covers the validity of the nullable columns.
 One step = init -> consume every batch (is_last on the last) -> produce -> delete, timed with CUDA events on the operator's stream;
 the median of `--reps` steps after one warm-up.  Every window step alternates with a full sort of the same keys and columns in
@@ -45,7 +47,9 @@ LAG_LEAD = [("lg", "lag", "r", 1), ("ld", "lead", "o", 1, 0.0)]
 MOVING = [("ma", "mean", "o", ("rows", -6, 0)), ("sc", "sum", "r", ("rows", -3, 3)), ("mx", "max", "o", ("rows", -6, 0)),
           ("n2", "nth_value", "r", 2)]
 MOVING_WIDE = [("sw", "sum", "r", ("rows", -65535, 0)), ("nw", "min", "o", ("rows", -65535, 0))]
-VALUE_CASES = ("running", "partition_aggs", "lag_lead", "moving", "moving_wide")
+MOMENTS = [("sd20", "std", "o", ("rows", -19, 0)), ("vr", "var", "o", "rows"), ("spp", "std_pop", "o", "partition")]
+MOMENT_NAMES = ("var", "std", "var_pop", "std_pop")
+VALUE_CASES = ("running", "partition_aggs", "lag_lead", "moving", "moving_wide", "moments")
 
 
 def window_bytes(n, key_bytes, n_funcs, n_parts, n_peers):
@@ -58,7 +62,7 @@ def window_bytes(n, key_bytes, n_funcs, n_parts, n_peers):
 
 def value_bytes(n, funcs, n_parts, n_peers):
     """The value kernels after bounds / tiles / ends (every value column here is 8 bytes wide, numpy).  A scan function (sum,
-    count of a column, mean, min, max) reads its column and the flags twice (reduce, then rescan) and writes its 8-byte cell, plus
+    count of a column, mean, min, max, var, std, var_pop, std_pop) reads its column and the flags twice (reduce, then rescan) and writes its 8-byte cell, plus
     a validity byte when nullable, at each frame end (min / max also read the chosen cell there); the eval pass reads the flags
     and the partition / peer-group words once, and per function writes 8 bytes (+1 validity) per row, reading the frame end's
     cell for a scan function whose frame ends elsewhere and the source cell for first / last / lag / lead."""
@@ -88,7 +92,8 @@ def in_frame_path(f):
 
 def frame_bytes(n, funcs, n_parts, n_peers):
     """The frame kernels (8-byte numpy value columns, as value_bytes).  An aggregate over a bounded frame: the tree build reads
-    its column once and writes 4 bytes per row of nodes (16-byte nodes of the levels >= 3); the query pass reads the flags and
+    its column once and writes 4 bytes per row of nodes (16-byte nodes of the levels >= 3; 6 bytes per row of 24-byte nodes for
+    var / std / var_pop / std_pop); the query pass reads the flags and
     the partition / peer-group words, the column once more (edge leaves; the nodes and the leaves that neighbouring frames share
     are counted once) and writes 8 + 1 bytes per row.  The gather pass (count(*), first_value, last_value, nth_value) reads the
     flags and words once, and per function and row the source cell and its 8 + 1 output bytes (count(*): 8)."""
@@ -99,7 +104,7 @@ def frame_bytes(n, funcs, n_parts, n_peers):
             gathers = True
             total += n * (8 if f[2] is None else 8 + 8 + 1)
         else:
-            total += n * (8 + 4) + words + n * (8 + 8 + 1)
+            total += n * (8 + (6 if f[1] in MOMENT_NAMES else 4)) + words + n * (8 + 8 + 1)
     if gathers:
         total += words
     return int(total)
@@ -137,7 +142,7 @@ def main():
     torch.cuda.synchronize(dev)
     cases = {"rn_rank_dense": (["p"], FUNCS3), "all6": (["p"], FUNCS6), "no_partition": ([], FUNCS3), "running": (["p"], RUNNING),
              "partition_aggs": (["p"], PARTITION_AGGS), "lag_lead": (["p"], LAG_LEAD), "moving": (["p"], MOVING),
-             "moving_wide": ([], MOVING_WIDE)}
+             "moving_wide": ([], MOVING_WIDE), "moments": (["p"], MOMENTS)}
 
     def batches():
         for r0 in range(0, n, args.batch):
@@ -284,7 +289,64 @@ def main():
             exp = op(m, torch.where(j2 >= P, m[j2.clamp(min=0)], ident))
             return torch.equal(got.view(torch.int64), exp.view(torch.int64))
 
+        def moment_ok(j, f):
+            """var / std of o against torch float64 two-pass computations (the frame's mean, then the sum of squared deviations
+            from it): the partition's std_pop through index_add; the trailing 20-row frame's over its 20 shifted terms; the
+            running var over a (partition, position) matrix, one prefix length at a time.  Each within DESIGN §3c's bound for
+            the device plus 8 m u (M2 + |mean| sqrt(m M2)) for the recomputation's own rounding; validity exactly."""
+            got, valid = res[3 + j], res[3 + nf + j]
+            u = 2.0 ** -53
+            if f[3] == "partition":
+                cnt = s.to(torch.float64)
+                mu = torch.zeros(n_p, dtype=torch.float64, device=dev).index_add_(0, pid, so)[pid] / cnt
+                M2 = torch.zeros(n_p, dtype=torch.float64, device=dev).index_add_(0, pid, (so - mu) ** 2)[pid]
+                h = cnt - 1
+            elif f[3] == "rows":
+                pos = i - P
+                L = int(s.max())
+                X = torch.zeros(n_p, L, dtype=torch.float64, device=dev)
+                X[pid, pos] = so
+                means = torch.cumsum(X, 1) / torch.arange(1, L + 1, device=dev, dtype=torch.float64)
+                M2s = torch.empty(n_p, L, dtype=torch.float64, device=dev)
+                for k in range(L):  # prefix k + 1 of every partition (longer than the partition: unused)
+                    M2s[:, k] = ((X[:, :k + 1] - means[:, k:k + 1]) ** 2).sum(1)
+                mu, M2 = means[pid, pos], M2s[pid, pos]
+                cnt = (pos + 1).to(torch.float64)
+                h = cnt - 1
+                del X, means, M2s, pos
+            else:
+                w = -f[3][1] + 1
+                lo = torch.maximum(P, i - w + 1)
+                cnt = (i - lo + 1).to(torch.float64)
+                tot = torch.zeros(n, dtype=torch.float64, device=dev)
+                for k in range(w):
+                    tot += torch.where(i - k >= P, torch.roll(so, k), 0.0)
+                mu = tot / cnt
+                M2 = torch.zeros(n, dtype=torch.float64, device=dev)
+                for k in range(w):
+                    M2 += torch.where(i - k >= P, (torch.roll(so, k) - mu) ** 2, 0.0)
+                h = torch.minimum(cnt - 1, 10 + 3 * torch.floor(torch.log2(cnt)))
+                del tot, lo
+            pop = f[1] in ("var_pop", "std_pop")
+            if not torch.equal(valid, cnt >= (1 if pop else 2)):
+                return False
+            gam = lambda k: k * u / (1 - k * u)  # noqa: E731
+            spread = mu.abs() * torch.sqrt(cnt * M2)
+            tol = torch.sqrt(h) * (gam(21 * h) * M2 + gam(8 * h) * spread) + 8 * cnt * u * (M2 + spread)
+            div = (cnt - (0 if pop else 1)).clamp(min=1)
+            var, tv = M2 / div, tol / div
+            tv = tv + 2 * u * var
+            exp, t = var, tv
+            if f[1] in ("std", "std_pop"):
+                exp = torch.sqrt(var)
+                t = torch.minimum(torch.sqrt(tv), tv / exp.clamp(min=1e-300)) + 2 * u * exp
+            return bool(((got - exp).abs() <= t)[valid].all())
+
         for j, f in enumerate(funcs):
+            if f[1] in MOMENT_NAMES:
+                if not moment_ok(j, f):
+                    return f"MISMATCH: {f[0]}", 0, 0
+                continue
             good = frame_ok(j, f) if in_frame_path(f) else value_ok(j, f) if f[1] in W.VALUE_FUNCS else torch.equal(res[3 + j].view(torch.int64), expected(f[0]).view(torch.int64))
             if not good:
                 return f"MISMATCH: {f[0]}", 0, 0

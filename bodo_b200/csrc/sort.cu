@@ -1148,6 +1148,23 @@ constexpr uint64_t WV_NEG_ZERO = 0x8000000000000000ull;      // -0.0, the identi
 // max; f set when the segment holds a partition start.
 struct WvAgg { uint64_t x; uint32_t c, f; };
 
+// VAR / STDDEV / VAR_POP / STDDEV_POP (codes 16..19) scan kind WV_MOM: c the count of valid cells, f as WvAgg's, mean their
+// mean and m2 = sum (x - mean)^2, combined by Chan's pairwise merge (wv_combine<WV_MOM>).  wv_t<K> is kind K's scan value.
+enum { WN_VAR = 16, WN_STD = 17, WN_VAR_POP = 18, WN_STD_POP = 19 };
+enum { WV_MOM = 5 };
+struct WvMom { uint32_t c, f; double mean, m2; };
+template <int K> struct WvKind { using T = WvAgg; };
+template <> struct WvKind<WV_MOM> { using T = WvMom; };
+template <int K> using wv_t = typename WvKind<K>::T;
+
+// The carry and tree buffers hold kind K's scan values.
+template <int K>
+__device__ __forceinline__ wv_t<K>* wv_buf(void* p) { return (wv_t<K>*)p; }
+
+// A function whose result comes from a scan or a tree of its scan values: sum, count, mean, min, max and the moments (the ranking
+// codes are routed before this is asked).
+__host__ __device__ constexpr bool wv_aggregate(int code) { return code <= WN_MAX || code >= WN_VAR; }
+
 // One value function as the kernels see it.
 struct WvFunc {
     int code, frame, ct, size, out_size, dflt_valid;  // ct / size: the value column's c-type and cell bytes (size 0: count(*))
@@ -1163,17 +1180,19 @@ struct WvArgs {
     int64_t n;
     const uint8_t* flags;
     const uint32_t *psize, *pend;
-    WvAgg* carry;  // per tile: its reduction, then its exclusive prefix
+    void* carry;   // per tile: its reduction, then its exclusive prefix (wv_t<K>)
     WvFunc s;      // window_vscan_kernel / window_vtiles_kernel: the function being scanned
     int n_funcs;   // window_veval_kernel: the value functions with work there
     WvFunc f[SORT_MAX_COLS];
 };
 
 template <int K>
-__device__ __forceinline__ WvAgg wv_identity() { return WvAgg{K == WV_FSUM ? WV_NEG_ZERO : 0ull, (K == WV_MIN || K == WV_MAX) ? WV_NONE : 0u, 0u}; }
+__device__ __forceinline__ wv_t<K> wv_identity() { return WvAgg{K == WV_FSUM ? WV_NEG_ZERO : 0ull, (K == WV_MIN || K == WV_MAX) ? WV_NONE : 0u, 0u}; }
+template <>
+__device__ __forceinline__ WvMom wv_identity<WV_MOM>() { return WvMom{0u, 0u, 0.0, 0.0}; }
 
 template <int K>
-__device__ __forceinline__ WvAgg wv_combine(WvAgg a, WvAgg b) {
+__device__ __forceinline__ wv_t<K> wv_combine(wv_t<K> a, wv_t<K> b) {
     if (b.f) return b;
     WvAgg r{b.x, b.c, a.f};
     if (K == WV_ISUM) { r.x = a.x + b.x; r.c = a.c + b.c; }
@@ -1184,14 +1203,30 @@ __device__ __forceinline__ WvAgg wv_combine(WvAgg a, WvAgg b) {
     }
     return r;
 }
+// Chan's merge of (n_a, mean_a, M2_a) and (n_b, mean_b, M2_b): with d = mean_b - mean_a and n = n_a + n_b, mean = mean_a +
+// d n_b / n and M2 = M2_a + M2_b + d^2 n_a n_b / n.  An empty side gives the other side's values exactly (no 0 / 0); every term
+// of M2 is >= 0, and equal means give d = 0, so a frame of equal values has M2 = 0 exactly.
+template <>
+__device__ __forceinline__ WvMom wv_combine<WV_MOM>(WvMom a, WvMom b) {
+    if (b.f) return b;
+    if (b.c == 0) return a;
+    if (a.c == 0) { b.f = a.f; return b; }
+    const uint32_t n = a.c + b.c;
+    const double w = (double)b.c / (double)n, d = b.mean - a.mean;
+    return WvMom{n, a.f, a.mean + d * w, a.m2 + b.m2 + d * (d * ((double)a.c * w))};
+}
 
 __device__ __forceinline__ WvAgg wv_shfl_up(WvAgg v, int o) {
     return WvAgg{__shfl_up_sync(0xffffffffu, (unsigned long long)v.x, o), __shfl_up_sync(0xffffffffu, v.c, o), __shfl_up_sync(0xffffffffu, v.f, o)};
 }
+__device__ __forceinline__ WvMom wv_shfl_up(WvMom v, int o) {
+    return WvMom{__shfl_up_sync(0xffffffffu, v.c, o), __shfl_up_sync(0xffffffffu, v.f, o), __shfl_up_sync(0xffffffffu, v.mean, o),
+                 __shfl_up_sync(0xffffffffu, v.m2, o)};
+}
 
 // Scan value of position i of the scanned function; `part`: i starts a partition.
 template <int K>
-__device__ __forceinline__ WvAgg wv_value(const WvFunc& s, int64_t i, bool part) {
+__device__ __forceinline__ wv_t<K> wv_value(const WvFunc& s, int64_t i, bool part) {
     WvAgg r = wv_identity<K>();
     r.f = part;
     bool na = s.vb && s.vb[i] == 0;
@@ -1212,32 +1247,45 @@ __device__ __forceinline__ WvAgg wv_value(const WvFunc& s, int64_t i, bool part)
     }
     return r;
 }
+// (1, x, 0) for a valid, non-NaN cell x converted to double (integers and bool exactly up to 2^53); the identity otherwise.
+template <>
+__device__ __forceinline__ WvMom wv_value<WV_MOM>(const WvFunc& s, int64_t i, bool part) {
+    WvMom r = wv_identity<WV_MOM>();
+    r.f = part;
+    const uint64_t raw = load_bits(s.data, s.size, i);
+    const double x = s.ct == CT_FLOAT64 ? __longlong_as_double((long long)raw)
+                   : s.ct == CT_FLOAT32 ? (double)__uint_as_float((uint32_t)raw)
+                   : ctype_is_signed_int(s.ct) ? (double)((int64_t)(raw << (64 - 8 * s.size)) >> (64 - 8 * s.size))
+                                               : (double)raw;
+    if (!(s.vb && s.vb[i] == 0) && !isnan(x)) { r.c = 1; r.mean = x; }
+    return r;
+}
 
 // Inclusive scan of this thread's WN_ITEMS values of a tile (warp-strided, as wn_row), seeded by `seed`.
 template <int K>
-__device__ __forceinline__ void wv_scan_tile(WvAgg seed, WvAgg (&v)[WN_ITEMS]) {
-    __shared__ WvAgg s_seg[WN_ITEMS * WN_WARPS];
+__device__ __forceinline__ void wv_scan_tile(wv_t<K> seed, wv_t<K> (&v)[WN_ITEMS]) {
+    __shared__ wv_t<K> s_seg[WN_ITEMS * WN_WARPS];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
     for (int k = 0; k < WN_ITEMS; k++) {
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
-            const WvAgg y = wv_shfl_up(v[k], o);
+            const wv_t<K> y = wv_shfl_up(v[k], o);
             if (lane >= o) v[k] = wv_combine<K>(y, v[k]);
         }
         if (lane == 31) s_seg[k * WN_WARPS + warp] = v[k];
     }
     __syncthreads();
     if (warp == 0) {  // exclusive scan of the 64 (item, warp) segments in row order, seeded: 2 per lane
-        const WvAgg x0 = s_seg[2 * lane], x1 = s_seg[2 * lane + 1];
-        WvAgg inc = wv_combine<K>(x0, x1);
+        const wv_t<K> x0 = s_seg[2 * lane], x1 = s_seg[2 * lane + 1];
+        wv_t<K> inc = wv_combine<K>(x0, x1);
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
-            const WvAgg y = wv_shfl_up(inc, o);
+            const wv_t<K> y = wv_shfl_up(inc, o);
             if (lane >= o) inc = wv_combine<K>(y, inc);
         }
-        const WvAgg ex = wv_shfl_up(inc, 1);
-        const WvAgg base = lane > 0 ? wv_combine<K>(seed, ex) : seed;
+        const wv_t<K> ex = wv_shfl_up(inc, 1);
+        const wv_t<K> base = lane > 0 ? wv_combine<K>(seed, ex) : seed;
         s_seg[2 * lane] = base;
         s_seg[2 * lane + 1] = wv_combine<K>(base, x0);
     }
@@ -1258,7 +1306,7 @@ __device__ __forceinline__ void wv_store_bits(void* dst, int64_t i, uint64_t bit
 
 // The function's result at a frame end i whose frame's scan value is v.
 template <int K>
-__device__ __forceinline__ void wv_write(const WvFunc& s, int64_t i, WvAgg v) {
+__device__ __forceinline__ void wv_write(const WvFunc& s, int64_t i, wv_t<K> v) {
     if (s.code == WN_COUNT) { ((int64_t*)s.out)[i] = v.c; return; }
     if (K == WV_MIN || K == WV_MAX) {
         const bool ok = v.c != WV_NONE;
@@ -1279,20 +1327,30 @@ __device__ __forceinline__ void wv_write(const WvFunc& s, int64_t i, WvAgg v) {
     }
     s.out_vb[i] = ok;
 }
+// var = M2 / (m - 1) (NA when m < 2), var_pop = M2 / m (NA when m = 0), std / std_pop their IEEE sqrt; FLOAT64.  A frame holding
+// +-inf has a non-finite mean and gives a valid NaN.
+template <>
+__device__ __forceinline__ void wv_write<WV_MOM>(const WvFunc& s, int64_t i, WvMom v) {
+    const bool pop = s.code == WN_VAR_POP || s.code == WN_STD_POP, ok = v.c > (pop ? 0u : 1u);
+    double r = isfinite(v.mean) ? v.m2 / ((double)v.c - (pop ? 0.0 : 1.0)) : __longlong_as_double(0x7FF8000000000000ll);
+    if (s.code == WN_STD || s.code == WN_STD_POP) r = sqrt(r);
+    ((double*)s.out)[i] = ok ? r : 0.0;
+    s.out_vb[i] = ok;
+}
 
 template <int K, bool FINAL>
 __global__ void __launch_bounds__(WN_THREADS) window_vscan_kernel(const __grid_constant__ WvArgs a) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t t = blockIdx.x;
-    WvAgg v[WN_ITEMS];
+    wv_t<K> v[WN_ITEMS];
 #pragma unroll
     for (int k = 0; k < WN_ITEMS; k++) {
         const int64_t i = wn_row(t, k, warp, lane);
         v[k] = i < a.n ? wv_value<K>(a.s, i, a.flags[i] & WN_PART) : wv_identity<K>();
     }
-    wv_scan_tile<K>(FINAL ? a.carry[t] : wv_identity<K>(), v);
+    wv_scan_tile<K>(FINAL ? wv_buf<K>(a.carry)[t] : wv_identity<K>(), v);
     if (!FINAL) {  // padding rows hold the identity, so the tile's last slot holds its reduction
-        if (threadIdx.x == WN_THREADS - 1) a.carry[t] = v[WN_ITEMS - 1];
+        if (threadIdx.x == WN_THREADS - 1) wv_buf<K>(a.carry)[t] = v[WN_ITEMS - 1];
         return;
     }
     const uint8_t end_flag = a.s.frame == WF_RANGE ? WN_PEER : WN_PART;
@@ -1307,26 +1365,26 @@ __global__ void __launch_bounds__(WN_THREADS) window_vscan_kernel(const __grid_c
 // One block of 1024 threads; thread x scans a contiguous run of tiles (as window_tiles_kernel).
 template <int K>
 __global__ void __launch_bounds__(1024) window_vtiles_kernel(const __grid_constant__ WvArgs a, int64_t n_tiles) {
-    __shared__ WvAgg s_agg[32];
+    __shared__ wv_t<K> s_agg[32];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t per = (n_tiles + 1023) / 1024, t0 = threadIdx.x * per, t1 = min(n_tiles, t0 + per);
-    WvAgg acc = wv_identity<K>();
-    for (int64_t t = t0; t < t1; t++) acc = wv_combine<K>(acc, a.carry[t]);
-    WvAgg inc = acc;
+    wv_t<K> acc = wv_identity<K>();
+    for (int64_t t = t0; t < t1; t++) acc = wv_combine<K>(acc, wv_buf<K>(a.carry)[t]);
+    wv_t<K> inc = acc;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
-        const WvAgg y = wv_shfl_up(inc, o);
+        const wv_t<K> y = wv_shfl_up(inc, o);
         if (lane >= o) inc = wv_combine<K>(y, inc);
     }
     if (lane == 31) s_agg[warp] = inc;
     __syncthreads();
-    WvAgg run = wv_identity<K>();
+    wv_t<K> run = wv_identity<K>();
     for (int w = 0; w < warp; w++) run = wv_combine<K>(run, s_agg[w]);
-    const WvAgg ex = wv_shfl_up(inc, 1);
+    const wv_t<K> ex = wv_shfl_up(inc, 1);
     if (lane > 0) run = wv_combine<K>(run, ex);
     for (int64_t t = t0; t < t1; t++) {
-        const WvAgg v = a.carry[t];
-        a.carry[t] = run;
+        const wv_t<K> v = wv_buf<K>(a.carry)[t];
+        wv_buf<K>(a.carry)[t] = run;
         run = wv_combine<K>(run, v);
     }
 }
@@ -1359,7 +1417,7 @@ __global__ void __launch_bounds__(WN_THREADS) window_veval_kernel(const __grid_c
                     if (g.size == 0) { ((int64_t*)g.out)[i] = e - P + 1; continue; }  // count(*)
                     src = e;  // a scan function: its frame end holds the result
             }
-            const bool scanned = g.code <= WN_MAX;
+            const bool scanned = wv_aggregate(g.code);
             if (scanned && e == i) continue;
             const char* from = scanned ? g.out : g.data;
             const int sz = scanned ? g.out_size : g.size;
@@ -1399,7 +1457,7 @@ void launch_wv_scan(const WvArgs& a, int64_t n_tiles, cudaStream_t st) {
 enum { WN_NTH_VALUE = 15 };
 enum { WF_BOUNDED = 4 };
 constexpr int64_t WF_UNBOUNDED_START = INT64_MIN, WF_UNBOUNDED_END = INT64_MAX;
-constexpr int WV_GATHER = 4;            // window_frame_kernel's gather pass (the scan kinds are 0..3)
+constexpr int WV_GATHER = 4;            // window_frame_kernel's gather pass (the scan kinds are 0..3 and WV_MOM)
 constexpr int WT_LOW = 3, WT_LEVELS = 32;  // levels below WT_LOW are not stored; level l < WT_LEVELS
 
 // A function of this path: the value function, its frame bounds (read for WF_BOUNDED only; the unbounded sentinels above) and,
@@ -1414,7 +1472,7 @@ struct WfArgs {
     const uint8_t* flags;
     const WnAgg* tile;              // the ranking scan's tile prefixes
     const uint32_t *psize, *pend;
-    WvAgg* tree;
+    void* tree;                     // wv_t<K> nodes
     int64_t off[WT_LEVELS];         // level l's first node in `tree` (l >= WT_LOW); level l holds n >> l nodes
     WfFunc s;                       // window_tree_kernel / window_frame_kernel<K != WV_GATHER>: the aggregate
     int n_funcs;                    // window_frame_kernel<WV_GATHER>: the gather functions
@@ -1431,37 +1489,58 @@ __device__ __forceinline__ void wf_bounds(const WfFunc& g, int64_t i, int64_t P,
     }
 }
 
-__device__ __forceinline__ void wt_store(const WfArgs& a, int l, int64_t b, WvAgg v) {
-    if (l >= WT_LOW && l < WT_LEVELS && b < (a.n >> l)) a.tree[a.off[l] + b] = v;
+template <int K>
+__device__ __forceinline__ void wt_store(const WfArgs& a, int l, int64_t b, wv_t<K> v) {
+    if (l >= WT_LOW && l < WT_LEVELS && b < (a.n >> l)) wv_buf<K>(a.tree)[a.off[l] + b] = v;
+}
+
+// Levels base + 1 .. base + 3 of a thread's WN_ITEMS inputs x, in registers; x[0] ends as their combine.
+template <int K>
+__device__ __forceinline__ void wt_levels3(const WfArgs& a, int base, int64_t j0, wv_t<K> (&x)[WN_ITEMS]) {
+#pragma unroll
+    for (int h = 1, m = WN_ITEMS / 2; m >= 1; h++, m >>= 1) {
+#pragma unroll
+        for (int k = 0; k < m; k++) {
+            x[k] = wv_combine<K>(x[2 * k], x[2 * k + 1]);
+            wt_store<K>(a, base + h, (j0 >> h) + k, x[k]);
+        }
+    }
+}
+// The same with constant trip counts: the loop above leaves the moments' larger combine partly rolled, and x in local memory.
+template <>
+__device__ __forceinline__ void wt_levels3<WV_MOM>(const WfArgs& a, int base, int64_t j0, WvMom (&x)[WN_ITEMS]) {
+#pragma unroll
+    for (int h = 1; h <= 3; h++) {
+#pragma unroll
+        for (int k = 0; k < WN_ITEMS / 2; k++) {
+            if (k < (WN_ITEMS >> h)) {
+                x[k] = wv_combine<WV_MOM>(x[2 * k], x[2 * k + 1]);
+                wt_store<WV_MOM>(a, base + h, (j0 >> h) + k, x[k]);
+            }
+        }
+    }
 }
 
 template <int K>
 __global__ void __launch_bounds__(WN_THREADS) window_tree_kernel(const __grid_constant__ WfArgs a, int base) {
-    __shared__ WvAgg s_node[WN_THREADS];
+    __shared__ wv_t<K> s_node[WN_THREADS];
     const int64_t n_in = a.n >> base, j0 = (int64_t)blockIdx.x * WN_TILE + threadIdx.x * WN_ITEMS;
-    WvAgg x[WN_ITEMS];
+    wv_t<K> x[WN_ITEMS];
 #pragma unroll
     for (int k = 0; k < WN_ITEMS; k++) {
         const int64_t j = j0 + k;
-        x[k] = j >= n_in ? wv_identity<K>() : base == 0 ? wv_value<K>(a.s.g, j, false) : a.tree[a.off[base] + j];
+        x[k] = j >= n_in ? wv_identity<K>() : base == 0 ? wv_value<K>(a.s.g, j, false) : wv_buf<K>(a.tree)[a.off[base] + j];
     }
-#pragma unroll
-    for (int h = 1, m = WN_ITEMS / 2; m >= 1; h++, m >>= 1) {  // levels base + 1 .. base + 3 in registers
-#pragma unroll
-        for (int k = 0; k < m; k++) {
-            x[k] = wv_combine<K>(x[2 * k], x[2 * k + 1]);
-            wt_store(a, base + h, (j0 >> h) + k, x[k]);
-        }
-    }
+    wt_levels3<K>(a, base, j0, x);  // levels base + 1 .. base + 3 in registers
     s_node[threadIdx.x] = x[0];
     __syncthreads();
     for (int h = 4, m = WN_THREADS / 2; m >= 1; h++, m >>= 1) {  // levels base + 4 .. base + 11 in shared memory
-        WvAgg y = x[0];
+        wv_t<K> y = x[0];
         if (threadIdx.x < m) y = wv_combine<K>(s_node[2 * threadIdx.x], s_node[2 * threadIdx.x + 1]);
         __syncthreads();
         if (threadIdx.x < m) {
             s_node[threadIdx.x] = y;
-            wt_store(a, base + h, (int64_t)blockIdx.x * m + threadIdx.x, y);
+            wt_store<K>(a, base + h, (int64_t)blockIdx.x * m + threadIdx.x, y);
         }
         __syncthreads();
     }
@@ -1469,15 +1548,15 @@ __global__ void __launch_bounds__(WN_THREADS) window_tree_kernel(const __grid_co
 
 // The aggregate of the scanned function over [lo, hi]: edge leaves from the sorted column, aligned blocks from the tree.
 template <int K>
-__device__ __forceinline__ WvAgg wt_query(const WfArgs& a, int64_t lo, int64_t hi) {
-    WvAgg acc = wv_identity<K>();
+__device__ __forceinline__ wv_t<K> wt_query(const WfArgs& a, int64_t lo, int64_t hi) {
+    wv_t<K> acc = wv_identity<K>();
     const int64_t r = hi + 1, a8 = min(r, (lo + 7) & ~(int64_t)7);
     int64_t j = lo;
     for (; j < a8; j++) acc = wv_combine<K>(acc, wv_value<K>(a.s.g, j, false));
     const int64_t b8 = max(j, r & ~(int64_t)7);
     while (j < b8) {  // j and b8 are multiples of 8, so l >= 3
         const int l = min(j == 0 ? 62 : __ffsll(j) - 1, 63 - __clzll(b8 - j));
-        acc = wv_combine<K>(acc, a.tree[a.off[l] + (j >> l)]);
+        acc = wv_combine<K>(acc, wv_buf<K>(a.tree)[a.off[l] + (j >> l)]);
         j += (int64_t)1 << l;
     }
     for (; j < r; j++) acc = wv_combine<K>(acc, wv_value<K>(a.s.g, j, false));
@@ -1544,7 +1623,7 @@ struct WindowState : FullSortState {
         for (int f = 0; f < n_funcs; f++) {
             b200_window_func& d = fn[f] = funcs[f];
             bound[f] = b200_window_frame{WF_UNBOUNDED_START, WF_UNBOUNDED_END};
-            B200_REQUIRE(d.code >= WN_ROW_NUMBER && d.code <= WN_NTH_VALUE, "b200 window: unknown function code");
+            B200_REQUIRE(d.code >= WN_ROW_NUMBER && d.code <= WN_STD_POP, "b200 window: unknown function code");
             int ct = CT_INT64, at = ARR_NUMPY;
             if (d.code <= WN_NTILE) {
                 B200_REQUIRE(d.col == -1 && d.frame == WF_NONE, "b200 window: a ranking function takes no column and no frame");
@@ -1580,8 +1659,9 @@ struct WindowState : FullSortState {
                 const bool temporal = vct == CT_DATE || vct == CT_DATETIME || vct == CT_TIMEDELTA;
                 if (d.code == WN_SUM || d.code == WN_MEAN)
                     B200_REQUIRE(!temporal, "b200 window: sum and mean need an integer, bool or float column");
+                if (d.code >= WN_VAR) B200_REQUIRE(!temporal, "b200 window: var and std need an integer, bool or float column");
                 if (d.code == WN_SUM) ct = ctype_is_float(vct) ? vct : ctype_is_signed_int(vct) || vct == CT_BOOL ? CT_INT64 : CT_UINT64;
-                else if (d.code == WN_MEAN) ct = CT_FLOAT64;
+                else if (d.code == WN_MEAN || d.code >= WN_VAR) ct = CT_FLOAT64;
                 else if (d.code != WN_COUNT) ct = vct;
                 if (d.code != WN_COUNT) at = ARR_NULLABLE;
             }
@@ -1619,11 +1699,11 @@ struct WindowState : FullSortState {
                      d.col >= 0 ? out_vb[d.col] : nullptr, out_data[c], out_vb[c]};
             if (d.frame == WF_BOUNDED || d.code == WN_NTH_VALUE) {  // the frame path only
                 const WfFunc h{g, bound[f].start, bound[f].end};
-                if (d.code <= WN_MAX && d.col >= 0) trees.push_back(h);
+                if (wv_aggregate(d.code) && d.col >= 0) trees.push_back(h);
                 else fa.f[fa.n_funcs++] = h;
                 continue;
             }
-            const bool scanned = d.code <= WN_MAX && d.col >= 0;
+            const bool scanned = wv_aggregate(d.code) && d.col >= 0;
             if (scanned) scans.push_back(g);
             if (!scanned || d.frame != WF_ROWS) { va.f[va.n_funcs++] = g; eval = true; }
         }
@@ -1642,28 +1722,35 @@ struct WindowState : FullSortState {
         window_ends_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
         if (a.n_funcs > 0) window_eval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
         B200_CUDA(cudaGetLastError());
-        DevBuf carry;
-        if (!scans.empty()) carry.alloc((size_t)n_tiles * sizeof(WvAgg));
-        va.n = n; va.flags = a.flags; va.psize = a.psize; va.pend = a.pend; va.carry = carry.as<WvAgg>();
+        DevBuf carry;  // sized for the largest scan value among the scans
+        const auto moments = [](int code) { return code >= WN_VAR; };
+        const bool mom_scan = std::any_of(scans.begin(), scans.end(), [&](const WvFunc& g) { return moments(g.code); });
+        if (!scans.empty()) carry.alloc((size_t)n_tiles * (mom_scan ? sizeof(WvMom) : sizeof(WvAgg)));
+        va.n = n; va.flags = a.flags; va.psize = a.psize; va.pend = a.pend; va.carry = carry.p;
         for (const WvFunc& g : scans) {
             va.s = g;
-            if (g.code == WN_MIN) launch_wv_scan<WV_MIN>(va, n_tiles, stream);
+            if (moments(g.code)) launch_wv_scan<WV_MOM>(va, n_tiles, stream);
+            else if (g.code == WN_MIN) launch_wv_scan<WV_MIN>(va, n_tiles, stream);
             else if (g.code == WN_MAX) launch_wv_scan<WV_MAX>(va, n_tiles, stream);
             else if (g.code != WN_COUNT && ctype_is_float(g.ct)) launch_wv_scan<WV_FSUM>(va, n_tiles, stream);
             else launch_wv_scan<WV_ISUM>(va, n_tiles, stream);
         }
         if (eval) window_veval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a, va);
         B200_CUDA(cudaGetLastError());
-        DevBuf tree;  // one tree buffer, reused by every aggregate over a bounded frame: n / 8 + n / 16 + ... nodes, <= 4 B per row
+        // one tree buffer, reused by every aggregate over a bounded frame: n / 8 + n / 16 + ... nodes of the largest scan value
+        // among them, <= 4 B per row (<= 6 B per row with a moment)
+        DevBuf tree;
         if (!trees.empty() || fa.n_funcs > 0) {
             fa.n = n; fa.flags = a.flags; fa.tile = a.tile; fa.psize = a.psize; fa.pend = a.pend;
             int64_t nodes = 0;
             for (int l = WT_LOW; l < WT_LEVELS; l++) { fa.off[l] = nodes; nodes += n >> l; }
-            if (!trees.empty()) tree.alloc((size_t)std::max<int64_t>(nodes, 1) * sizeof(WvAgg));
-            fa.tree = tree.as<WvAgg>();
+            const bool mom_tree = std::any_of(trees.begin(), trees.end(), [&](const WfFunc& h) { return moments(h.g.code); });
+            if (!trees.empty()) tree.alloc((size_t)std::max<int64_t>(nodes, 1) * (mom_tree ? sizeof(WvMom) : sizeof(WvAgg)));
+            fa.tree = tree.p;
             for (const WfFunc& h : trees) {
                 fa.s = h;
-                if (h.g.code == WN_MIN) launch_wf_tree<WV_MIN>(fa, n_tiles, stream);
+                if (moments(h.g.code)) launch_wf_tree<WV_MOM>(fa, n_tiles, stream);
+                else if (h.g.code == WN_MIN) launch_wf_tree<WV_MIN>(fa, n_tiles, stream);
                 else if (h.g.code == WN_MAX) launch_wf_tree<WV_MAX>(fa, n_tiles, stream);
                 else if (h.g.code != WN_COUNT && ctype_is_float(h.g.ct)) launch_wf_tree<WV_FSUM>(fa, n_tiles, stream);
                 else launch_wf_tree<WV_ISUM>(fa, n_tiles, stream);
@@ -1740,6 +1827,18 @@ void* b200_window_state_init_frames(int64_t operator_id, const int8_t* c_types, 
                                     int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
                                     const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
                                     int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream) {
+    try {  // this entry's domain: codes 0..15 (the moments entry adds var, std, var_pop and std_pop)
+        for (int f = 0; funcs && f < n_funcs && f < b200::SORT_MAX_COLS; f++)
+            B200_REQUIRE(funcs[f].code >= b200::WN_ROW_NUMBER && funcs[f].code <= b200::WN_NTH_VALUE, "b200 window: unknown function code");
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
+    return b200_window_state_init_moments(operator_id, c_types, arr_types, n_arrs, n_partition_keys, n_order_keys, order_ascending,
+                                          order_na_last, funcs, frames, n_funcs, output_batch_size, device, stream);
+}
+
+void* b200_window_state_init_moments(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                                     int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                                     const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
+                                     int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream) {
     (void)operator_id;
     return b200::sort_state_new(device, [&]() -> SortState* {
         const int np = n_partition_keys, no = n_order_keys;

@@ -316,8 +316,8 @@ class PhysicalSort:
 class PhysicalWindow:
     """Window sink/source: every input row once, in the stable order by (partition_by ascending NA last, order_by), with one
     column per function after the input columns.  funcs: ranking entries (out_name, fname) or (out_name, "ntile", n), fname one
-    of streaming.window.FUNCS; value entries (out_name, fname, column[, frame]), fname one of streaming.window.VALUE_FUNCS and
-    frame one of "range" (default), "rows", "partition" or ("rows", start, end) (ROWS BETWEEN start AND end, None for UNBOUNDED,
+    of streaming.window.FUNCS; value entries (out_name, fname, column[, frame]), fname one of streaming.window.VALUE_FUNCS or
+    MOMENT_FUNCS (var, std, var_pop, std_pop) and frame one of "range" (default), "rows", "partition" or ("rows", start, end) (ROWS BETWEEN start AND end, None for UNBOUNDED,
     negative offsets PRECEDING, positive FOLLOWING), (out_name, "lag" | "lead", column[, k[, default]]) or (out_name,
     "nth_value", column, n[, frame]);
     ascending / na_position: one value or one per ORDER BY key.  The column names are taken from the first batch."""
@@ -444,7 +444,7 @@ def sort_values(df, by, ascending=True, na_position="last", batch_size: int = ST
 def window(df, partition_by, order_by, funcs, ascending=True, na_position="last", batch_size: int = STREAMING_BATCH_SIZE, **kw):
     """Ranking, aggregate and navigation window functions OVER (PARTITION BY partition_by ORDER BY order_by) through
     PhysicalWindow (funcs as PhysicalWindow takes them, e.g. [("run", "sum", "x", "rows"), ("prev", "lag", "x", 1, 0),
-    ("ma7", "mean", "x", ("rows", -6, 0))]).  Returns a pandas
+    ("ma7", "mean", "x", ("rows", -6, 0)), ("sd20", "std", "x", ("rows", -19, 0))]).  Returns a pandas
     DataFrame in the operator's output order (stably sorted by partition keys, then order keys) with a fresh index: df's columns,
     then one column per function."""
     op = PhysicalWindow(partition_by, order_by, funcs, ascending, na_position, **kw)

@@ -4,11 +4,13 @@
     SUM / COUNT / AVG / MIN / MAX / FIRST_VALUE / LAST_VALUE (x) OVER (PARTITION BY p ORDER BY o [frame])
     LAG / LEAD (x, k, default) OVER (PARTITION BY p ORDER BY o)
     NTH_VALUE (x, n) OVER (PARTITION BY p ORDER BY o [frame]), and every frame function over ROWS BETWEEN k PRECEDING AND k FOLLOWING
+    VAR_SAMP / STDDEV_SAMP / VAR_POP / STDDEV_POP (x) OVER (PARTITION BY p ORDER BY o [frame])
 
 pandas equivalents: groupby(p).cumcount() + 1, groupby(p)[o].rank(method="min" / "dense" / "max", pct=...),
 groupby(p)[x].cumsum() / cummin() / cummax() (the "rows" frame), groupby(p)[x].transform("sum" / "mean" / "min" / "max" /
-"count" / "size" / "first" / "last") (the "partition" frame) and groupby(p)[x].shift(k, fill_value=default) (lag; lead is
-shift(-k)).  The state is a third form of the streaming sort (streaming/sort.py's SortState, sort.cu's WindowState): batches are
+"count" / "size" / "first" / "last" / "var" / "std") (the "partition" frame), groupby(p)[x].expanding().var() / .std() (the
+"rows" frame), groupby(p)[x].rolling(w).var() / .std() (a bounded frame) and groupby(p)[x].shift(k, fill_value=default) (lag;
+lead is shift(-k)).  The state is a third form of the streaming sort (streaming/sort.py's SortState, sort.cu's WindowState): batches are
 appended to the full sort's device chunk store, is_last sorts every row by (partition keys ascending NA last, order keys, arrival
 index), scans the sorted key columns on the device for partition and peer-group boundaries and then scans or gathers the value
 columns.
@@ -33,8 +35,8 @@ Semantics:
     (negative PRECEDING, 0 CURRENT ROW, positive FOLLOWING; start <= end when both are offsets): for row i of the partition
     [P, pe) the frame is [lo, hi] with lo = P (start None) or max(P, i + start), hi = pe - 1 (end None) or min(pe - 1, i + end),
     empty when lo > hi.  ("rows", None, 0) is "rows" and ("rows", None, None) is "partition".  It takes sum, count, mean, min,
-    max, first_value, last_value and nth_value, which are then defined as below with [lo, hi] in place of [P, e]; an empty frame
-    gives NA (count 0).  Over [P, e], with a float NaN counted as NA:
+    max, first_value, last_value, nth_value, var, std, var_pop and std_pop, which are then defined as below with [lo, hi] in
+    place of [P, e]; an empty frame gives NA (count 0).  Over [P, e], with a float NaN counted as NA:
       count(x): non-NA cells, count(None): COUNT(*) = e - P + 1; int64 numpy.
       sum(x): the sum of the non-NA cells, NA when there are none; integers and bool wrap in 64 bits (int64 for signed and bool,
         uint64 for unsigned), floats accumulate in double (float32 narrowed once at the end); nullable.
@@ -47,6 +49,12 @@ Semantics:
         x's type, nullable.
       nth_value(x, n): the cell at P + n - 1 as first_value gives it when that row is in the frame, else NA; 1 <= n < 2^31;
         frame "range" by default; x's type, nullable.
+      var(x) / std(x) / var_pop(x) / std_pop(x): with m the non-NA cells (integers and bool converted to double, exact up to
+        2^53) and M2 = sum (x - mean)^2 over them: var = M2 / (m - 1), NA when m < 2 (SQL VAR_SAMP, pandas ddof=1); var_pop =
+        M2 / m, NA when m = 0 and 0.0 when m = 1 (VAR_POP, ddof=0); std / std_pop their IEEE sqrt.  M2 is combined from (count,
+        mean, M2) by Chan's pairwise merge, with no sum of squares, so it keeps its digits when |mean| >> the spread (DESIGN
+        §3c gives the bound); it is never negative and is exactly 0.0 over equal values.  A frame holding +-inf gives a valid
+        NaN, as pandas does.  float64, nullable; a temporal column raises.
       lag(x, k=1, default=None) / lead(...): the cell at i - k / i + k if that row is in the row's partition, else default (NA
         when None); 0 <= k < 2^31, k = 0 is the row itself; no frame; x's type, nullable.  default is converted to x's numpy
         dtype and must round-trip exactly.
@@ -55,7 +63,8 @@ Semantics:
     the scan's order, not sequentially.  Over ("rows", start, end) the results are pandas' groupby(p)[x].rolling(w,
     min_periods=1) ones (count: min_periods=0), with float sums combined in an order that depends only on the frame's bounds.
     Results depend only on the sorted positions: every row that shares a frame end (a bounded frame: both bounds) gets a
-    bit-identical result, and float sums are bit-identical across runs and across any split of the rows into batches.
+    bit-identical result, and float sums and the moments are bit-identical across runs and across any split of the rows into
+    batches.
   - output: every input row once, in the stable sort's order by (partition keys, order keys, arrival); every input column in
     input order, then one column per function under the caller's name.  SQL leaves the order open; fixing it makes every column
     comparable bit for bit.
@@ -82,8 +91,10 @@ FRAMES = {"range": 1, "rows": 2, "partition": 3}
 FRAME_FUNCS = {"nth_value": 15}
 ROWS_BETWEEN = 4
 UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING = -(1 << 63), (1 << 63) - 1
-BOUNDED_FUNCS = ("sum", "count", "mean", "min", "max", "first_value", "last_value", "nth_value")
-_VALUE_NAMES = {c: f for f, c in {**VALUE_FUNCS, **FRAME_FUNCS}.items()}
+# The moments entry's codes (b200_window_state_init_moments): VAR_SAMP, STDDEV_SAMP, VAR_POP and STDDEV_POP.
+MOMENT_FUNCS = {"var": 16, "std": 17, "var_pop": 18, "std_pop": 19}
+BOUNDED_FUNCS = ("sum", "count", "mean", "min", "max", "first_value", "last_value", "nth_value", "var", "std", "var_pop", "std_pop")
+_VALUE_NAMES = {c: f for f, c in {**VALUE_FUNCS, **FRAME_FUNCS, **MOMENT_FUNCS}.items()}
 _FRAME_NAMES = {c: f for f, c in FRAMES.items()}
 MAX_COLS = 32
 MAX_WINDOW_ROWS = MAX_FULL_SORT_ROWS
@@ -91,7 +102,7 @@ MAX_LAG = (1 << 31) - 1
 MAX_FRAME_OFFSET = MAX_LAG
 _TEMPORAL = (CTypes.DATE, CTypes.DATETIME, CTypes.TIMEDELTA)
 _FORMS = (f"ranking: (out_name, fname) with fname in {sorted(FUNCS)}, or (out_name, 'ntile', n); value: (out_name, fname, column"
-          f"[, frame]) with fname in {sorted(set(VALUE_FUNCS) - {'lag', 'lead'})}, frame in {sorted(FRAMES)} or ('rows', start, end), "
+          f"[, frame]) with fname in {sorted(set(VALUE_FUNCS) - {'lag', 'lead'} | set(MOMENT_FUNCS))}, frame in {sorted(FRAMES)} or ('rows', start, end), "
           "column None for count(*) only, or (out_name, 'lag' | 'lead', column[, k[, default]]), or (out_name, 'nth_value', column, "
           "n[, frame])")
 
@@ -127,7 +138,7 @@ def _parse_value(f, col_names):
     if len(f) > 4:
         raise _lib.B200Error(f"Streaming Window: {f!r}: bad frame (one of {sorted(FRAMES)} or ('rows', start, end), as (out_name, "
                              f"{fname!r}, column[, frame]))")
-    return (name, VALUE_FUNCS[fname], 0, column, *_parse_frame(f, f[3] if len(f) > 3 else "range"))
+    return (name, {**VALUE_FUNCS, **MOMENT_FUNCS}[fname], 0, column, *_parse_frame(f, f[3] if len(f) > 3 else "range"))
 
 
 def _parse_frame(f, frame):
@@ -179,7 +190,7 @@ def _parse_funcs(funcs, col_names):
     out = []
     for f in funcs:
         f = tuple(f)
-        value = isinstance(f[1] if len(f) > 1 else None, str) and (f[1] in VALUE_FUNCS or f[1] in FRAME_FUNCS)
+        value = isinstance(f[1] if len(f) > 1 else None, str) and (f[1] in VALUE_FUNCS or f[1] in FRAME_FUNCS or f[1] in MOMENT_FUNCS)
         if (len(f) < 2 or not isinstance(f[0], str) or not isinstance(f[1], str) or f[1] not in FUNCS and not value
                 or value and len(f) < 3):
             raise _lib.B200Error(f"Streaming Window: unknown window function {f!r} ({_FORMS})")
@@ -242,7 +253,7 @@ class WindowState(SortState):
 
     def descriptors(self, c_types):
         """The b200_window_func fields (code, col, frame, default_valid, arg, default_bits) of every function, given the c-types
-        of the input columns in input order.  Raises B200Error for sum or mean of a temporal column and for a lag / lead default
+        of the input columns in input order.  Raises B200Error for sum, mean, var or std of a temporal column and for a lag / lead default
         that does not round-trip through the column's dtype."""
         out = []
         for f in self.funcs:
@@ -254,10 +265,12 @@ class WindowState(SortState):
                 out.append((code, -1, frame, 0, arg, 0))
                 continue
             ct = c_types[self.col_names.index(column)]
-            if code in (VALUE_FUNCS["sum"], VALUE_FUNCS["mean"]) and ct in _TEMPORAL:
+            moment = code in MOMENT_FUNCS.values()
+            if (code in (VALUE_FUNCS["sum"], VALUE_FUNCS["mean"]) or moment) and ct in _TEMPORAL:
                 bounds = [None if b in (UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING) else b for b in f[6]] if len(f) > 6 else None
                 entry = (name, _VALUE_NAMES[code], column, _FRAME_NAMES[frame] if bounds is None else ("rows", *bounds))
-                raise _lib.B200Error(f"Streaming Window: {entry!r}: sum and mean need an integer, bool or float column, not a temporal one")
+                what = "var and std" if moment else "sum and mean"
+                raise _lib.B200Error(f"Streaming Window: {entry!r}: {what} need an integer, bool or float column, not a temporal one")
             valid = default is not None
             out.append((code, self.phys.index(self.col_names.index(column)), frame, int(valid), arg, _default_bits(f, ct) if valid else 0))
         return out
@@ -282,8 +295,8 @@ class WindowState(SortState):
         frs = ffi.new("b200_window_frame[]", len(self.descs))
         for d, (start, end) in zip(frs, self.frames()):
             d.start, d.end = start, end
-        h = L.b200_window_state_init_frames(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs, frs,
-                                            len(self.descs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
+        h = L.b200_window_state_init_moments(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs, frs,
+                                             len(self.descs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
         return _lib.check_ptr(h, "init_window_state")
 
 
@@ -295,11 +308,14 @@ def init_window_state(operator_id, partition_by, order_by, ascending, na_positio
     value or one per ORDER BY key; funcs: ranking entries (out_name, fname) with fname in FUNCS, or (out_name, "ntile", n) with
     n >= 1; value entries (out_name, fname, column[, frame]) with fname in VALUE_FUNCS other than lag / lead, frame one of FRAMES
     (default "range") or ("rows", start, end) and column None for count(*) only, (out_name, "lag" | "lead", column[, k[,
-    default]]) (k = 1 and default None, NA, by default), or (out_name, "nth_value", column, n[, frame]).
-    Example, a 7-row moving average: ("ma7", "mean", "x", ("rows", -6, 0)).
+    default]]) (k = 1 and default None, NA, by default), (out_name, "nth_value", column, n[, frame]), or (out_name, fname,
+    column[, frame]) with fname in MOMENT_FUNCS (var, std, var_pop, std_pop) and any frame sum takes.
+    Examples, a 7-row moving average: ("ma7", "mean", "x", ("rows", -6, 0)); a 20-row rolling standard deviation (a Bollinger
+    band's width): ("sd20", "std", "x", ("rows", -19, 0)); the population variance of the partition: ("vp", "var_pop", "x",
+    "partition").
     Raises B200Error for an unknown function, duplicate output names or names that clash with an input column, keys that are
     missing or not distinct, a key count outside 1..4, a bad na_position, ntile n < 1, an unknown value column, a bad frame or
-    frame bound, a frame on lag or lead, k outside [0, 2^31), nth_value n outside [1, 2^31); and at the first consume call for sum or mean of a temporal column or a lag / lead
+    frame bound, a frame on lag or lead, k outside [0, 2^31), nth_value n outside [1, 2^31); and at the first consume call for sum, mean, var or std of a temporal column or a lag / lead
     default that the column's dtype cannot hold exactly."""
     return WindowState(operator_id, partition_by, order_by, ascending, na_position, funcs, col_names, parallel, output_batch_size,
                        device, stream, process_group)

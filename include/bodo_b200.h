@@ -254,15 +254,15 @@ void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const i
 /* One window function of b200_window_state_init_funcs.
  *   code: 0 row_number, 1 rank, 2 dense_rank, 3 percent_rank, 4 cume_dist, 5 ntile (the ranking functions above), then the value
  *         functions 6 sum, 7 count, 8 mean, 9 min, 10 max, 11 first_value, 12 last_value, 13 lag, 14 lead, 15 nth_value
- *         (b200_window_state_init_frames only).
+ *         (b200_window_state_init_frames only), 16 var, 17 std, 18 var_pop, 19 std_pop (b200_window_state_init_moments only).
  *   col: the input column (0 <= col < n_arrs) a value function reads, any column including a key; -1 for a ranking function and
  *        for count(*).
  *   frame: 0 for a ranking function, lag and lead; for the others 1 range (RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW: up
  *          to the row's last peer; the whole partition without ORDER BY), 2 rows (ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT
  *          ROW: up to the row itself, ties in arrival order), 3 partition (the whole partition).  Frames 1..3 start at the
  *          partition's first row.  4 rows between (b200_window_state_init_frames only): ROWS BETWEEN start AND end of the
- *          function's b200_window_frame, for sum, count (of a column or count(*)), mean, min, max, first_value, last_value and
- *          nth_value.
+ *          function's b200_window_frame, for sum, count (of a column or count(*)), mean, min, max, first_value, last_value,
+ *          nth_value, var, std, var_pop and std_pop.
  *   arg: ntile's n (>= 1); lag / lead's offset k (0 <= k < 2^31; k = 0 is the row itself); nth_value's n (1 <= n < 2^31).
  *   default_valid, default_bits: lag / lead's value when row i - k / i + k is outside the row's partition: the low bytes of
  *          default_bits in the column's type if default_valid, else NA.
@@ -278,6 +278,12 @@ void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const i
  *   first_value, last_value  the cell at P / e as it is (bits and validity: a NaN stays a valid NaN); the column's type, nullable.
  *   lag, lead the cell at i - k / i + k when that row is in the row's partition, else the default; the column's type, nullable.
  *   nth_value the cell at P + n - 1 as it is when that row is in the frame, else NA; the column's type, nullable.
+ *   var, std, var_pop, std_pop  with m the frame's non-NA cells (integers and bool converted to double, exact up to 2^53) and
+ *             M2 = sum (x - mean)^2 over them: 16 var = M2 / (m - 1), NA when m < 2 (VAR_SAMP); 17 std = sqrt(var) (STDDEV_SAMP);
+ *             18 var_pop = M2 / m, NA when m = 0, 0.0 when m = 1 (VAR_POP); 19 std_pop = sqrt(var_pop) (STDDEV_POP).  M2 is
+ *             combined from (count, mean, M2) triples by Chan's pairwise merge in the scan's or the frame tree's order: never
+ *             negative, exactly 0.0 over equal values, a valid NaN when the frame holds +-inf.  FLOAT64, nullable.  Not for
+ *             temporal columns.
  * Every row that shares a frame end gets a bit-identical result.
  * Over a frame 4 [lo, hi] (below) the same definitions hold with lo in place of P and hi in place of e; an empty frame (lo > hi)
  * gives NA, and count 0.  Float sums there are combined in an order fixed by (lo, hi) alone, so rows with the same bounds get the
@@ -310,11 +316,19 @@ void* b200_window_state_init_funcs(int64_t operator_id, const int8_t* c_types, c
 /* b200_window_state_init_funcs with codes 0..15 and frames 0..4: frames[i] is read only when funcs[i].frame == 4 (frames may be
  * NULL when no function uses frame 4).  A bound outside the domain above, start > end, frame 4 on a function other than sum,
  * count, mean, min, max, first_value, last_value and nth_value, or nth_value's n outside [1, 2^31) fails here (NULL, last error
- * set).  b200_window_state_init_funcs is this entry with frames NULL, restricted to codes 0..14 and frames 0..3. */
+ * set).  b200_window_state_init_funcs is this entry with frames NULL, restricted to codes 0..14 and frames 0..3.  This entry is
+ * b200_window_state_init_moments restricted to codes 0..15. */
 void* b200_window_state_init_frames(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
                                     int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
                                     const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
                                     int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream);
+
+/* b200_window_state_init_frames with codes 0..19: 16 var, 17 std, 18 var_pop and 19 std_pop (defined above) take a column and
+ * frames 1..4, as sum does.  A temporal column fails here (NULL, last error set). */
+void* b200_window_state_init_moments(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                                     int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                                     const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
+                                     int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream);
 
 /* The build-consume entry of _sort.cpp: filters a DEVICE-resident batch (same schema as the state) against the current cutoff on
  * the device (full sort: appends it to the chunk store); on is_last reduces to the final rows (full sort: sorts every row).
