@@ -15,7 +15,14 @@ doubles in [0, 1)) and an int64 row id r, fed in `--batch`-row batches.  Cases:
   moving_wide    SUM(r) and MIN(o) ROWS BETWEEN 65535 PRECEDING AND CURRENT ROW OVER (ORDER BY o): one partition, a deep tree
   moments        STDDEV(o) ROWS BETWEEN 19 PRECEDING AND CURRENT ROW (a Bollinger band's width), VAR(o) ROWS (running) and
                  STDDEV_POP(o) over the partition, OVER (PARTITION BY p ORDER BY o)
-The value cases (running to moments) also alternate with rn_rank_dense (rn_rank_dense_ms), so their cost above the ranking kernels
+  range_moving   AVG(o) and MAX(o) RANGE BETWEEN 2^35 ns PRECEDING AND CURRENT ROW, SUM(r) and COUNT(*) RANGE BETWEEN 2^34 ns
+                 PRECEDING AND 2^34 ns FOLLOWING, OVER (PARTITION BY p ORDER BY t): about 8 rows per frame, as in moving
+  range_wide     SUM(r) and MIN(o) RANGE BETWEEN 2^28 ns PRECEDING AND CURRENT ROW OVER (ORDER BY t): one partition, about 65 536
+                 rows per frame, as in moving_wide
+The range cases add a fourth column t, an int64 DATETIME key uniform in [0, 2^40) ns, and order by it; the other cases keep
+their three columns.  `--profile` runs one more step per case under torch.profiler (separately from the timed steps) and
+reports the window kernels' device times; with it, nothing is timed (run it separately from the timed run).
+The value cases (running to moments, and the range cases) also alternate with rn_rank_dense (rn_rank_dense_ms), so their cost above the ranking kernels
 is measured too; their result check covers the validity of the nullable columns.
 One step = init -> consume every batch (is_last on the last) -> produce -> delete, timed with CUDA events on the operator's stream;
 the median of `--reps` steps after one warm-up.  Every window step alternates with a full sort of the same keys and columns in
@@ -49,7 +56,18 @@ MOVING = [("ma", "mean", "o", ("rows", -6, 0)), ("sc", "sum", "r", ("rows", -3, 
 MOVING_WIDE = [("sw", "sum", "r", ("rows", -65535, 0)), ("nw", "min", "o", ("rows", -65535, 0))]
 MOMENTS = [("sd20", "std", "o", ("rows", -19, 0)), ("vr", "var", "o", "rows"), ("spp", "std_pop", "o", "partition")]
 MOMENT_NAMES = ("var", "std", "var_pop", "std_pop")
-VALUE_CASES = ("running", "partition_aggs", "lag_lead", "moving", "moving_wide", "moments")
+def _ns(k):
+    import numpy as np
+
+    return np.timedelta64(k, "ns")
+
+
+RANGE_MOVING = [("ra", "mean", "o", ("range_between", -_ns(1 << 35), 0)), ("rx", "max", "o", ("range_between", -_ns(1 << 35), 0)),
+                ("rs", "sum", "r", ("range_between", -_ns(1 << 34), _ns(1 << 34))),
+                ("rc", "count", None, ("range_between", -_ns(1 << 34), _ns(1 << 34)))]
+RANGE_WIDE = [("ws", "sum", "r", ("range_between", -_ns(1 << 28), 0)), ("wn", "min", "o", ("range_between", -_ns(1 << 28), 0))]
+RANGE_CASES = ("range_moving", "range_wide")
+VALUE_CASES = ("running", "partition_aggs", "lag_lead", "moving", "moving_wide", "moments") + RANGE_CASES
 
 
 def window_bytes(n, key_bytes, n_funcs, n_parts, n_peers):
@@ -85,6 +103,14 @@ def value_bytes(n, funcs, n_parts, n_peers):
     return int(total)
 
 
+def range_bytes(n, funcs, n_parts, n_peers):
+    """The bounds pass of each distinct RANGE frame with value offsets (design bytes, not measured): the flags byte, the partition
+    and peer-group words (4 bytes each per partition / peer group), the 8-byte key once (the searches' probes stay near the row
+    and are counted once) and the 8-byte (lo, hi) per row."""
+    frames = {f[-1] for f in funcs if len(f) > 3 and isinstance(f[-1], tuple) and f[-1][0] == "range_between"}
+    return int(len(frames) * (n * (1 + 8 + 8) + 4 * (n_parts + n_peers)))
+
+
 def in_frame_path(f):
     """Functions over a ("rows", start, end) frame and nth_value run in the frame kernels, not in the scans."""
     return f[1] == "nth_value" or (len(f) > 3 and isinstance(f[3], tuple))
@@ -96,18 +122,20 @@ def frame_bytes(n, funcs, n_parts, n_peers):
     var / std / var_pop / std_pop); the query pass reads the flags and
     the partition / peer-group words, the column once more (edge leaves; the nodes and the leaves that neighbouring frames share
     are counted once) and writes 8 + 1 bytes per row.  The gather pass (count(*), first_value, last_value, nth_value) reads the
-    flags and words once, and per function and row the source cell and its 8 + 1 output bytes (count(*): 8)."""
+    flags and words once per launch, and per function and row the source cell and its 8 + 1 output bytes (count(*): 8).  Every
+    RANGE frame with value offsets has its own gather launch, and each of its functions reads the 8-byte (lo, hi) per row."""
     words = n + 4 * (n_parts + n_peers)
-    total, gathers = 0, False
+    total, gather_launches = 0, set()
     for f in funcs:
+        fr = f[-1] if len(f) > 3 and isinstance(f[-1], tuple) and f[-1][0] == "range_between" else None
+        if fr is not None:
+            total += 8 * n
         if f[1] == "nth_value" or f[2] is None or f[1] in ("first_value", "last_value"):
-            gathers = True
+            gather_launches.add(fr)
             total += n * (8 if f[2] is None else 8 + 8 + 1)
         else:
             total += n * (8 + (6 if f[1] in MOMENT_NAMES else 4)) + words + n * (8 + 8 + 1)
-    if gathers:
-        total += words
-    return int(total)
+    return int(total + len(gather_launches) * words)
 
 
 def main():
@@ -116,6 +144,7 @@ def main():
     ap.add_argument("--batch", type=int, default=1 << 24)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--cases", type=str, default="rn_rank_dense,all6,no_partition")
+    ap.add_argument("--profile", action="store_true")
     args = ap.parse_args()
 
     import torch
@@ -123,7 +152,7 @@ def main():
     from bodo_b200 import _lib, synth
     from bodo_b200.streaming import sort as S
     from bodo_b200.streaming import window as W
-    from bodo_b200.table import Column, Table
+    from bodo_b200.table import ArrTypes, Column, CTypes, Table
 
     _lib.require_gpu()
     dev = torch.device("cuda", 0)
@@ -138,19 +167,24 @@ def main():
     ok = torch.empty(n, dtype=torch.float64, device=dev)
     synth.device_fill(None, ok, 0, 1, 62, sp)
     rid = torch.arange(n, dtype=torch.int64, device=dev)
-    names = ["p", "o", "r"]
+    tk = None  # the range cases' DATETIME key, made on first use
     torch.cuda.synchronize(dev)
     cases = {"rn_rank_dense": (["p"], FUNCS3), "all6": (["p"], FUNCS6), "no_partition": ([], FUNCS3), "running": (["p"], RUNNING),
              "partition_aggs": (["p"], PARTITION_AGGS), "lag_lead": (["p"], LAG_LEAD), "moving": (["p"], MOVING),
-             "moving_wide": ([], MOVING_WIDE), "moments": (["p"], MOMENTS)}
+             "moving_wide": ([], MOVING_WIDE), "moments": (["p"], MOMENTS), "range_moving": (["p"], RANGE_MOVING),
+             "range_wide": ([], RANGE_WIDE)}
+    names, order = ["p", "o", "r"], "o"
 
     def batches():
         for r0 in range(0, n, args.batch):
             r1 = min(n, r0 + args.batch)
-            yield Table([Column(pk[r0:r1]), Column(ok[r0:r1]), Column(rid[r0:r1])], names), r1 == n
+            cols = [Column(pk[r0:r1]), Column(ok[r0:r1]), Column(rid[r0:r1])]
+            if len(names) > 3:
+                cols.append(Column(tk[r0:r1], None, CTypes.DATETIME, ArrTypes.NUMPY, r1 - r0))
+            yield Table(cols, names), r1 == n
 
     def window_step(part, funcs, keep=False):
-        st = W.init_window_state(-1, part, ["o"], True, "last", funcs, names, output_batch_size=1 << 30, device=0, stream=sp)
+        st = W.init_window_state(-1, part, [order], True, "last", funcs, names, output_batch_size=1 << 30, device=0, stream=sp)
         for t, last in batches():
             W.window_build_consume_batch(st, t, last)
         out, _ = W.window_produce_output_batch(st)
@@ -159,13 +193,13 @@ def main():
             res = [torch.as_tensor(c.data, device=dev).clone() for c in out.columns]
             bit = torch.arange(8, device=dev, dtype=torch.uint8)
             res += [None if c.validity is None else
-                    ((torch.as_tensor(c.validity, device=dev).unsqueeze(1) >> bit) & 1).flatten()[:n].bool() for c in out.columns[3:]]
+                    ((torch.as_tensor(c.validity, device=dev).unsqueeze(1) >> bit) & 1).flatten()[:n].bool() for c in out.columns[len(names):]]
         m9 = W.get_metric(st, 9)
         W.delete_window_state(st)
         return res, m9
 
     def sort_step(part):
-        st = S.init_stream_sort_state(-1, None, 0, part + ["o"], [True] * (len(part) + 1), ["last"] * (len(part) + 1), names,
+        st = S.init_stream_sort_state(-1, None, 0, part + [order], [True] * (len(part) + 1), ["last"] * (len(part) + 1), names,
                                       output_batch_size=1 << 30, device=0, stream=sp, full=True)
         for t, last in batches():
             S.sort_build_consume_batch(st, t, last)
@@ -352,13 +386,103 @@ def main():
                 return f"MISMATCH: {f[0]}", 0, 0
         return "ok", int(ps.sum()), int(qs.sum())
 
+    def range_check(part, funcs, res):
+        """The range cases: every row's [lo, hi] from torch.searchsorted over the exact composite (p << 40) | t of the sorted
+        rows (CURRENT ROW ends at the row's last peer); sums of r as int64 cumsum differences and COUNT(*) as hi - lo + 1, bit
+        for bit; AVG(o) (o >= 0) from the frame's shifted terms within 4 (m + 1) u; MIN / MAX(o) from minima / maxima of 2^k
+        rows doubled, bit for bit."""
+        idx = torch.sort(tk, stable=True).indices
+        if part:
+            idx = idx[torch.sort(pk[idx], stable=True).indices]
+        if not (torch.equal(res[2], idx) and torch.equal(res[3], tk[idx])):
+            return "MISMATCH: an input column differs from the stable sort", 0, 0
+        del idx
+        sp_ = res[0] if part else torch.zeros(n, dtype=torch.int64, device=dev)
+        so, sr, st_k = res[1], res[2], res[3]
+        comp = (sp_ << 40) | st_k
+        base = sp_ << 40
+        ps = torch.ones(n, dtype=torch.bool, device=dev)
+        ps[1:] = torch.diff(sp_) != 0
+        qs = ps.clone()
+        qs[1:] |= torch.diff(st_k) != 0
+        n_parts, n_peers = int(ps.sum()), int(qs.sum())
+        del ps, qs
+        i = torch.arange(n, device=dev, dtype=torch.int64)
+        nf = len(funcs)
+        for j, f in enumerate(funcs):
+            got, valid = res[4 + j], res[4 + nf + j]
+            a, b = (int(x) for x in f[3][1:])  # ns
+            lo = torch.searchsorted(comp, base + (st_k + a).clamp(min=0))
+            hi = torch.searchsorted(comp, comp if b == 0 else base + (st_k + b).clamp(max=(1 << 40) - 1), right=True) - 1
+            if valid is not None and not bool(valid.all()):  # every frame here holds its own row
+                return f"MISMATCH: {f[0]} validity", 0, 0
+            if f[1] == "count":
+                good = torch.equal(got, hi - lo + 1)
+            elif f[1] == "sum":
+                cs = torch.cat([torch.zeros(1, dtype=torch.int64, device=dev), torch.cumsum(sr, 0)])
+                good = torch.equal(got, cs[hi + 1] - cs[lo])
+                del cs
+            elif f[1] == "mean":
+                cnt = hi - lo + 1
+                tot = torch.zeros(n, dtype=torch.float64, device=dev)
+                for k in range(int(cnt.max())):
+                    tot += torch.where(lo + k <= hi, so[(lo + k).clamp(max=n - 1)], 0.0)
+                exp = tot / cnt.to(torch.float64)
+                good = bool(((got - exp).abs() <= 4 * (cnt + 1).to(torch.float64) * 2.0 ** -53 * exp).all())
+                del tot, exp, cnt
+            else:
+                op = torch.maximum if f[1] == "max" else torch.minimum
+                w = hi - lo + 1
+                K = torch.frexp(w.to(torch.float64))[1].to(torch.int64) - 1
+                m, exp, k = so.clone(), torch.empty_like(so), 0
+                while True:  # m[x] = op over [x, x + 2^k) (clipped at n)
+                    s_ = K == k
+                    if bool(s_.any()):
+                        exp[s_] = op(m[lo[s_]], m[hi[s_] - (1 << k) + 1])
+                    if (2 << k) > int(w.max()):
+                        break
+                    m = op(m, torch.cat([m[1 << k:], m[-(1 << k):]]))
+                    k += 1
+                good = torch.equal(got.view(torch.int64), exp.view(torch.int64))
+                del m, exp, K, w
+            del lo, hi
+            if not good:
+                return f"MISMATCH: {f[0]}", 0, 0
+        return "ok", n_parts, n_peers
+
     def free():
         torch.cuda.empty_cache()
         _lib.lib().b200_pool_trim(0, 0)
 
+    def profile_case(name, part, funcs):
+        """One warm-up step, then one step under torch.profiler: the window kernels' device times (no timing, no check)."""
+        from torch.profiler import ProfilerActivity, profile
+
+        window_step(part, funcs)
+        torch.cuda.synchronize(dev)
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            window_step(part, funcs)
+            torch.cuda.synchronize(dev)
+        kern = {}
+        for ev in prof.events():
+            if str(ev.device_type).endswith("CUDA") and "window_" in ev.name:
+                key = ev.name.split("(")[0].replace("void b200::", "")
+                kern[key] = kern.get(key, 0.0) + getattr(ev, "device_time", getattr(ev, "cuda_time", 0.0)) / 1e3
+        print(json.dumps({"case": name, "profile_kernel_ms": {k: round(v, 3) for k, v in sorted(kern.items())}, "card": card()}), flush=True)
+        free()
+
     ok_all = True
     for name in args.cases.split(","):
         part, funcs = cases[name]
+        if name in RANGE_CASES:
+            if tk is None:
+                tk = torch.randint(0, 1 << 40, (n,), generator=g, device=dev, dtype=torch.int64)
+            names, order = ["p", "o", "r", "t"], "t"
+        else:
+            names, order = ["p", "o", "r"], "o"
+        if args.profile:
+            profile_case(name, part, funcs)
+            continue
         window_step(part, funcs)  # warm-up
         sort_step(part)
         value_case = name in VALUE_CASES
@@ -377,24 +501,24 @@ def main():
         # check
         res, _ = window_step(part, funcs, keep=True)
         free()
-        chk, n_parts, n_peers = check(part, funcs, res)
+        chk, n_parts, n_peers = (range_check if name in RANGE_CASES else check)(part, funcs, res)
         if chk == "ok" and m9 != n_parts:
             chk = f"MISMATCH: metric 9 = {m9}, partitions = {n_parts}"
         del res
         free()
         # design bytes: the sort of the keys (passes from the data, as sort_bench predicts them), then the window kernels
         f64w = lambda x: torch.where(x < 0, x.view(torch.int64) ^ 0x7FFFFFFFFFFFFFFF, x.view(torch.int64))  # noqa: E731
-        words = [f64w(ok)] + ([pk ^ (-(2 ** 63))] if part else [])
+        words = [tk ^ (-(2 ** 63)) if name in RANGE_CASES else f64w(ok)] + ([pk ^ (-(2 ** 63))] if part else [])
         kp = plan(torch, words, [8] * len(words), [True] + [False] * len(part), [0] * len(words))
         del words
         free()
         key_bytes = 8 * (1 + len(part))
-        sort_bytes = moved_bytes(n, 24, 0, key_bytes, kp)
+        sort_bytes = moved_bytes(n, 8 * len(names), 0, key_bytes, kp)
         if value_case:  # bounds and ends as the ranking cases (no ranking eval pass), then the value kernels
             ends4 = 4 * (2 * n_parts + n_peers)
             scans = [f for f in funcs if not in_frame_path(f)]
             total = (sort_bytes + window_bytes(n, key_bytes, 0, n_parts, n_peers) - (n + ends4) + value_bytes(n, scans, n_parts, n_peers)
-                     + frame_bytes(n, [f for f in funcs if in_frame_path(f)], n_parts, n_peers))
+                     + frame_bytes(n, [f for f in funcs if in_frame_path(f)], n_parts, n_peers) + range_bytes(n, funcs, n_parts, n_peers))
         else:
             total = sort_bytes + window_bytes(n, key_bytes, len(funcs), n_parts, n_peers)
         out = {"case": name, "rows": n, "batch": args.batch, "funcs": [f[1] for f in funcs], "ms_per_step": round(w_ms, 3),

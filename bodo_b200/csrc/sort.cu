@@ -1442,7 +1442,8 @@ void launch_wv_scan(const WvArgs& a, int64_t n_tiles, cudaStream_t st) {
 // ---- bounded ROWS frames (k PRECEDING / k FOLLOWING) and NTH_VALUE ----
 //
 // They run after the scans and window_veval_kernel, and only for functions routed here: every function over a bounded frame
-// (frame WF_BOUNDED) and NTH_VALUE over any frame.  A row's frame is [lo, hi] (empty when lo > hi), from wf_bounds only.
+// (frame WF_BOUNDED or WF_RANGE_BETWEEN) and NTH_VALUE over any frame.  A row's frame is [lo, hi] (empty when lo > hi), from wf_bounds
+// only (frame 5: from its bounds buffer, read by window_range_frame_kernel<K>, the same per-row evaluation without the scan).
 //   window_tree_kernel<K>     per aggregate over a bounded frame (sum, count of a column, mean, min, max): a dyadic block tree over
 //                             the sorted positions, with no partition reset.  Level l holds the combine of each aligned block
 //                             [b 2^l, (b + 1) 2^l) that lies inside [0, n), for l >= 3; levels 0..2 are not stored (the query
@@ -1455,16 +1456,19 @@ void launch_wv_scan(const WvArgs& a, int64_t n_tiles, cudaStream_t st) {
 // block that starts at the current position and ends by the last multiple of 8 in the frame, repeatedly, then the leaves up to hi
 // (at most 7).  The order depends only on (lo, hi); a frame of W rows takes at most 14 leaves and 2 log2(W) nodes.
 enum { WN_NTH_VALUE = 15 };
-enum { WF_BOUNDED = 4 };
+enum { WF_BOUNDED = 4, WF_RANGE_BETWEEN = 5 };  // frame 5: bounds per row from window_range_bounds_kernel (below)
 constexpr int64_t WF_UNBOUNDED_START = INT64_MIN, WF_UNBOUNDED_END = INT64_MAX;
 constexpr int WV_GATHER = 4;            // window_frame_kernel's gather pass (the scan kinds are 0..3 and WV_MOM)
 constexpr int WT_LOW = 3, WT_LEVELS = 32;  // levels below WT_LOW are not stored; level l < WT_LEVELS
 
-// A function of this path: the value function, its frame bounds (read for WF_BOUNDED only; the unbounded sentinels above) and,
-// in g.k, nth_value's n.
+// A function of this path: the value function, its frame bounds (WF_BOUNDED: row offsets or the unbounded sentinels above;
+// WF_RANGE_BETWEEN: the bounds buffer of its frame) and, in g.k, nth_value's n.
 struct WfFunc {
     WvFunc g;
-    int64_t start, end;
+    union {
+        struct { int64_t start, end; };
+        const int2* range;  // per row (lo, hi), from window_range_bounds_kernel (below)
+    };
 };
 
 struct WfArgs {
@@ -1563,10 +1567,30 @@ __device__ __forceinline__ wv_t<K> wt_query(const WfArgs& a, int64_t lo, int64_t
     return acc;
 }
 
+// Row i's frame functions: the aggregate a.s over its [lo, hi] from the tree (K a scan kind), or every gather function (K =
+// WV_GATHER); bounds(g, lo, hi) gives function g's frame.
+template <int K, typename Bounds>
+__device__ __forceinline__ void wf_eval_row(const WfArgs& a, int64_t i, Bounds bounds) {
+    constexpr int KQ = K == WV_GATHER ? WV_ISUM : K;  // the scan kind of the aggregate pass
+    int64_t lo, hi;
+    if (K != WV_GATHER) {
+        bounds(a.s, lo, hi);
+        wv_write<KQ>(a.s.g, i, wt_query<KQ>(a, lo, hi));
+    } else for (int fn = 0; fn < a.n_funcs; fn++) {
+        const WfFunc& g = a.f[fn];
+        bounds(g, lo, hi);
+        if (g.g.size == 0) { ((int64_t*)g.g.out)[i] = max(hi - lo + 1, (int64_t)0); continue; }  // count(*)
+        const int64_t src = g.g.code == WN_FIRST_VALUE ? lo : g.g.code == WN_LAST_VALUE ? hi : lo + g.g.k - 1;
+        const bool in = lo <= hi && src <= hi;
+        if (in) copy_cell(g.g.out, i, g.g.data, src, g.g.size);
+        else wv_store_bits(g.g.out, i, 0, g.g.size);
+        g.g.out_vb[i] = in && (!g.g.vb || g.g.vb[src]);
+    }
+}
+
 template <int K>
 __global__ void __launch_bounds__(WN_THREADS) window_frame_kernel(const __grid_constant__ WfArgs a) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    constexpr int KQ = K == WV_GATHER ? WV_ISUM : K;  // the scan kind of the aggregate pass
     const int64_t t = blockIdx.x;
     WnArgs w;  // wn_scan_tile reads n, flags and the tile prefixes only
     w.n = a.n; w.flags = const_cast<uint8_t*>(a.flags); w.tile = const_cast<WnAgg*>(a.tile);
@@ -1582,21 +1606,21 @@ __global__ void __launch_bounds__(WN_THREADS) window_frame_kernel(const __grid_c
         if (i >= a.n) break;
         const WnAgg vk = s_v[k][threadIdx.x];
         const int64_t P = vk.p, pe = P + a.psize[vk.p], qe = a.pend[vk.q];
-        int64_t lo, hi;
-        if (K != WV_GATHER) {
-            wf_bounds(a.s, i, P, pe, qe, lo, hi);
-            wv_write<KQ>(a.s.g, i, wt_query<KQ>(a, lo, hi));
-        } else for (int fn = 0; fn < a.n_funcs; fn++) {
-            const WfFunc& g = a.f[fn];
-            wf_bounds(g, i, P, pe, qe, lo, hi);
-            if (g.g.size == 0) { ((int64_t*)g.g.out)[i] = max(hi - lo + 1, (int64_t)0); continue; }  // count(*)
-            const int64_t src = g.g.code == WN_FIRST_VALUE ? lo : g.g.code == WN_LAST_VALUE ? hi : lo + g.g.k - 1;
-            const bool in = lo <= hi && src <= hi;
-            if (in) copy_cell(g.g.out, i, g.g.data, src, g.g.size);
-            else wv_store_bits(g.g.out, i, 0, g.g.size);
-            g.g.out_vb[i] = in && (!g.g.vb || g.g.vb[src]);
-        }
+        wf_eval_row<K>(a, i, [&](const WfFunc& g, int64_t& lo, int64_t& hi) { wf_bounds(g, i, P, pe, qe, lo, hi); });
     }
+}
+
+// The same over frame-5 functions, whose bounds window_range_bounds_kernel wrote: no scan of the flags is needed, so one thread
+// per row.  48 registers: at the default budget the compiler holds the double sum in 32 and spills.
+template <int K>
+__global__ void __maxnreg__(48) window_range_frame_kernel(const __grid_constant__ WfArgs a) {
+    const int64_t i = (int64_t)blockIdx.x * WN_THREADS + threadIdx.x;
+    if (i >= a.n) return;
+    wf_eval_row<K>(a, i, [i](const WfFunc& g, int64_t& lo, int64_t& hi) {
+        const int2 b = __ldg(g.range + i);
+        lo = b.x;
+        hi = b.y;
+    });
 }
 
 // Build the tree of the aggregate a.s (levels WT_LOW.. up to log2 n), then evaluate it at every row.
@@ -1604,7 +1628,156 @@ template <int K>
 void launch_wf_tree(const WfArgs& a, int64_t n_tiles, cudaStream_t st) {
     for (int base = 0; (a.n >> max(base + 1, WT_LOW)) > 0; base += 11)
         window_tree_kernel<K><<<(unsigned)(((a.n >> base) + WN_TILE - 1) / WN_TILE), WN_THREADS, 0, st>>>(a, base);
-    window_frame_kernel<K><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
+    if (a.s.g.frame == WF_RANGE_BETWEEN) window_range_frame_kernel<K><<<(unsigned)(n_tiles * WN_ITEMS), WN_THREADS, 0, st>>>(a);
+    else window_frame_kernel<K><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
+}
+
+// ---- RANGE frames with value offsets (RANGE BETWEEN x PRECEDING AND y FOLLOWING): frame 5 ----
+//
+// A frame-5 function's bounds are a b200_window_range: per side UNBOUNDED, CURRENT ROW (the row's peer group: its first peer Q or
+// its last peer qe - 1) or an offset k measured in the single ORDER BY key x.  With the key ascending, a k PRECEDING start is the
+// first row of the partition's non-NA run with x_j >= x_i - k and a k FOLLOWING end the last row with x_j <= x_i + k (a PRECEDING
+// end and a FOLLOWING start mirror these); descending swaps the signs.  An offset bound at an NA row (null or NaN) is its peer
+// group's boundary; at a non-NA row it never reaches an NA row, and one that no row satisfies leaves the frame empty.
+//   window_range_bounds_kernel  one launch per distinct frame-5 frame, before that frame's trees and gathers: the ranking scan of
+//                               the flags (P, Q) again, psize / pend for pe and qe, then per row and offset side one search of
+//                               the sorted key column.  Writes (lo, hi) per row; window_range_frame_kernel<K> reads them.
+// Every comparison is exact in an ascending 64-bit order word: integers (DATE in days, DATETIME / TIMEDELTA in ns) as x + 2^63
+// (signed) or x (unsigned), so x -+ k is the word -+ k and a carry out of 64 bits means the bound lies past every value of the
+// type; floats widened to double and compared against fl(x -+ k) through the sort's double order (-0.0 equals 0.0).
+// A state holds at most FS_MAX_ROWS rows: the positions of a non-empty frame fit int32, an empty frame is stored as (0, -1).
+static_assert(FS_MAX_ROWS <= (int64_t)INT32_MAX + 1, "window_range_bounds_kernel stores non-empty bounds as int32");
+enum { WR_UNBOUNDED_PRECEDING = 0, WR_PRECEDING = 1, WR_CURRENT_ROW = 2, WR_FOLLOWING = 3, WR_UNBOUNDED_FOLLOWING = 4 };
+
+struct WrArgs {
+    int64_t n;
+    const uint8_t* flags;
+    const WnAgg* tile;             // the ranking scan's tile prefixes
+    const uint32_t *psize, *pend;
+    SortKey key;                   // the ORDER BY key (read for offset bounds only)
+    const char* data;              // its sorted column and validity bytes (nullptr: numpy)
+    const uint8_t* vb;
+    int start_kind, end_kind;
+    uint64_t start_bits, end_bits; // offset magnitudes: a non-negative integer, or a finite non-negative double's bits
+    int2* out;                     // per row: (lo, hi)
+};
+
+// Ascending order word of key cell j (load_bits at the key's width, as the sort's encoder reads it); na: null or NaN.
+__device__ __forceinline__ uint64_t wr_word(const WrArgs& a, int64_t j, bool& na) {
+    const SortKey& k = a.key;
+    const uint64_t raw = load_bits(a.data, k.size, j);
+    na = a.vb && a.vb[j] == 0;
+    if (ctype_is_float(k.ct)) {
+        const double d = k.ct == CT_FLOAT64 ? __longlong_as_double((long long)raw) : (double)__uint_as_float((uint32_t)raw);
+        na = na || isnan(d);
+        return (uint64_t)canon_float_ordered(canon_float_key(d)) ^ 0x8000000000000000ull;
+    }
+    if (!ctype_is_signed_int(k.ct)) return raw;
+    return (uint64_t)((int64_t)(raw << (64 - 8 * k.size)) >> (64 - 8 * k.size)) ^ 0x8000000000000000ull;
+}
+
+// Order word of x - k (neg) or x + k for the cell whose word is w; sat = -1 / +1 when an integer result lies below / above every
+// word (it then bounds nothing on that side), else 0.
+__device__ __forceinline__ uint64_t wr_target(int ct, uint64_t w, bool neg, uint64_t k, int& sat) {
+    sat = 0;
+    if (ctype_is_float(ct)) {
+        const double x = ordered_to_f64(w), d = __longlong_as_double((long long)k), t = neg ? x - d : x + d;
+        return (uint64_t)canon_float_ordered(canon_float_key(t)) ^ 0x8000000000000000ull;
+    }
+    if (neg) { sat = w < k ? -1 : 0; return w - k; }
+    sat = w > ~0ull - k ? 1 : 0;
+    return w + k;
+}
+
+// The first j in [P, pe) with p(j), pe if none, for p false then true over [P, pe): gallop from h in [P, pe) by 1, 2, 4, ...
+// rows, then bisect.  O(log d) probes for an answer d rows from h, all near h.
+template <typename Pred>
+__device__ __forceinline__ int64_t wr_first(int64_t P, int64_t pe, int64_t h, Pred p) {
+    int64_t lo, hi;  // p(lo) false or lo = P - 1; p(hi) true or hi = pe
+    if (p(h)) {
+        hi = h;
+        for (int64_t s = 1;; s <<= 1) {
+            lo = hi - s;
+            if (lo < P) { lo = P - 1; break; }
+            if (!p(lo)) break;
+            hi = lo;
+        }
+    } else {
+        lo = h;
+        for (int64_t s = 1;; s <<= 1) {
+            hi = lo + s;
+            if (hi >= pe) { hi = pe; break; }
+            if (p(hi)) break;
+            lo = hi;
+        }
+    }
+    while (hi - lo > 1) {
+        const int64_t m = lo + ((hi - lo) >> 1);
+        if (p(m)) hi = m;
+        else lo = m;
+    }
+    return hi;
+}
+
+// Row i's start (end = false) or end bound of one side.  wi / na: row i's order word and NA flag (read for the offset kinds only).
+__device__ __forceinline__ int64_t wr_bound(const WrArgs& a, int kind, uint64_t k, bool end, int64_t P, int64_t pe, int64_t Q,
+                                            int64_t qe, uint64_t wi, bool na) {
+    if (kind == WR_UNBOUNDED_PRECEDING) return P;
+    if (kind == WR_UNBOUNDED_FOLLOWING) return pe - 1;
+    if (kind == WR_CURRENT_ROW || na) return end ? qe - 1 : Q;
+    // In y = word (ascending) or ~word (descending), y grows with the position over the non-NA run: a start is the first row
+    // with y >= Y, an end the last row with y <= Y, i.e. one before the first with y >= Y + 1.  NA rows stand below (NA first)
+    // or above (NA last) every y, so the search never needs the run's ends.
+    const bool desc = a.key.desc, nl = a.key.na_last;
+    int sat;
+    uint64_t Y = wr_target(a.key.ct, wi, (kind == WR_PRECEDING) != desc, k, sat);
+    if (desc) { Y = ~Y; sat = -sat; }
+    if (end) {
+        if (sat == 0 && Y == ~0ull) sat = 1;
+        Y++;
+    }
+    const auto p = [&](int64_t j) {
+        bool nj;
+        const uint64_t wj = wr_word(a, j, nj);
+        return nj ? nl : sat < 0 || (sat == 0 && (desc ? ~wj : wj) >= Y);
+    };
+    const int64_t j = wr_first(P, pe, kind == WR_PRECEDING ? Q : qe - 1, p);
+    bool nj = false;
+    if (!end) {
+        if (j < pe) wr_word(a, j, nj);
+        return nj ? pe : j;  // only NA rows satisfy it: empty
+    }
+    if (j - 1 >= P) wr_word(a, j - 1, nj);
+    return nj ? P - 1 : j - 1;
+}
+
+__global__ void __launch_bounds__(WN_THREADS) window_range_bounds_kernel(const __grid_constant__ WrArgs a) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t t = blockIdx.x;
+    WnArgs w;  // wn_scan_tile reads n, flags and the tile prefixes only
+    w.n = a.n; w.flags = const_cast<uint8_t*>(a.flags); w.tile = const_cast<WnAgg*>(a.tile);
+    uint8_t f[WN_ITEMS];
+    WnAgg v[WN_ITEMS];
+    wn_scan_tile(w, t, f, v);
+    __shared__ WnAgg s_v[WN_ITEMS][WN_THREADS];  // parked as in window_eval_kernel: the item loop is not unrolled
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) s_v[k][threadIdx.x] = v[k];
+    const bool offsets = a.start_kind == WR_PRECEDING || a.start_kind == WR_FOLLOWING || a.end_kind == WR_PRECEDING ||
+                         a.end_kind == WR_FOLLOWING;
+#pragma unroll 1
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        if (i >= a.n) break;
+        const WnAgg vk = s_v[k][threadIdx.x];
+        const int64_t P = vk.p, pe = P + a.psize[vk.p], Q = vk.q, qe = a.pend[vk.q];
+        bool na = false;
+        const uint64_t wi = offsets ? wr_word(a, i, na) : 0;
+        const int64_t lo = wr_bound(a, a.start_kind, a.start_bits, false, P, pe, Q, qe, wi, na);
+        const int64_t hi = wr_bound(a, a.end_kind, a.end_bits, true, P, pe, Q, qe, wi, na);
+        // A non-empty frame lies in [0, n) with n <= 2^31, so both bounds fit int32.  An empty one may carry lo = pe = 2^31 (a
+        // state of exactly 2^31 rows), so every empty frame is stored as (0, -1): its consumers read nothing for lo > hi.
+        a.out[i] = lo <= hi ? make_int2((int)lo, (int)hi) : make_int2(0, -1);
+    }
 }
 
 // Ranking and value window functions over (PARTITION BY the first n_part keys ORDER BY the rest).  The output is the full sort's,
@@ -1613,16 +1786,18 @@ struct WindowState : FullSortState {
     int n_part, n_funcs;
     b200_window_func fn[SORT_MAX_COLS];
     b200_window_frame bound[SORT_MAX_COLS];  // a WF_BOUNDED function's frame
+    b200_window_range range[SORT_MAX_COLS];  // a WF_RANGE_BETWEEN function's frame
     std::vector<DevBuf> fout;
     int64_t n_partitions = 0;  // metric 9
 
     WindowState(const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_part_, int n_keys, const int32_t* asc,
-                const int32_t* na_last, const b200_window_func* funcs, const b200_window_frame* frames, int n_funcs_, int64_t obs,
-                int dev, cudaStream_t st)
+                const int32_t* na_last, const b200_window_func* funcs, const b200_window_frame* frames, const b200_window_range* ranges,
+                int n_funcs_, int64_t obs, int dev, cudaStream_t st)
         : FullSortState(c_types, arr_types, n_arrs, n_keys, asc, na_last, obs, dev, st), n_part(n_part_), n_funcs(n_funcs_) {
         for (int f = 0; f < n_funcs; f++) {
             b200_window_func& d = fn[f] = funcs[f];
             bound[f] = b200_window_frame{WF_UNBOUNDED_START, WF_UNBOUNDED_END};
+            range[f] = b200_window_range{WR_UNBOUNDED_PRECEDING, WR_UNBOUNDED_FOLLOWING, 0, 0};
             B200_REQUIRE(d.code >= WN_ROW_NUMBER && d.code <= WN_STD_POP, "b200 window: unknown function code");
             int ct = CT_INT64, at = ARR_NUMPY;
             if (d.code <= WN_NTILE) {
@@ -1637,9 +1812,10 @@ struct WindowState : FullSortState {
                     B200_REQUIRE(d.arg >= 0 && d.arg <= 0x7FFFFFFF, "b200 window: lag / lead offset k must be in [0, 2^31)");
                     B200_REQUIRE(d.default_valid == 0 || d.default_valid == 1, "b200 window: default_valid must be 0 or 1");
                 } else {
-                    B200_REQUIRE(d.frame >= WF_RANGE && d.frame <= WF_BOUNDED,
-                                 "b200 window: unknown frame (1 range, 2 rows, 3 partition, 4 rows between)");
+                    B200_REQUIRE(d.frame >= WF_RANGE && d.frame <= WF_RANGE_BETWEEN,
+                                 "b200 window: unknown frame (1 range, 2 rows, 3 partition, 4 rows between, 5 range between)");
                 }
+                if (d.frame == WF_RANGE_BETWEEN) check_range(f, d, ranges, n_keys);
                 if (d.code == WN_NTH_VALUE) B200_REQUIRE(d.arg >= 1 && d.arg <= 0x7FFFFFFF, "b200 window: nth_value needs n in [1, 2^31)");
                 if (d.frame == WF_BOUNDED) {
                     B200_REQUIRE(frames, "b200 window: frame 4 (rows between) needs frames[i]");
@@ -1670,6 +1846,38 @@ struct WindowState : FullSortState {
         }
     }
 
+    // Validates function f's b200_window_range (frame 5) against the keys and stores it; the unbounded-start spellings become
+    // frames 1 and 3, so a frame gives the same bits however it is written.
+    void check_range(int f, b200_window_func& d, const b200_window_range* ranges, int n_keys) {
+        B200_REQUIRE(ranges, "b200 window: frame 5 (range between) needs ranges[i]");
+        b200_window_range r = ranges[f];
+        B200_REQUIRE(r.start_kind >= WR_UNBOUNDED_PRECEDING && r.start_kind <= r.end_kind && r.end_kind <= WR_UNBOUNDED_FOLLOWING &&
+                     r.start_kind != WR_UNBOUNDED_FOLLOWING && r.end_kind != WR_UNBOUNDED_PRECEDING,
+                     "b200 window: range bound kinds are 0..4 with start_kind <= end_kind, start_kind != 4 and end_kind != 0");
+        const auto offset = [](int kind) { return kind == WR_PRECEDING || kind == WR_FOLLOWING; };
+        if (offset(r.start_kind) || offset(r.end_kind)) {
+            B200_REQUIRE(n_keys - n_part == 1, "b200 window: a range offset (k PRECEDING / FOLLOWING) needs exactly one ORDER BY key");
+            const int kct = sc.ctype[n_part];
+            const bool flt = ctype_is_float(kct);
+            B200_REQUIRE(flt || ctype_is_signed_int(kct) || kct == CT_UINT8 || kct == CT_UINT16 || kct == CT_UINT32 || kct == CT_UINT64,
+                         "b200 window: a range offset needs an integer, float or temporal ORDER BY key (not bool)");
+            for (const uint64_t k : {offset(r.start_kind) ? r.start_bits : 0ull, offset(r.end_kind) ? r.end_bits : 0ull})
+                B200_REQUIRE(flt ? k < 0x7FF0000000000000ull : (int64_t)k >= 0,
+                             "b200 window: a range offset is a non-negative int64 (integer keys, DATE days, DATETIME / TIMEDELTA ns) or "
+                             "the bits of a finite, non-negative double (float keys)");
+            // both offsets on one side: PRECEDING starts at least as far back as it ends, FOLLOWING the other way round (finite,
+            // non-negative doubles order as their bits)
+            if (r.start_kind == r.end_kind)
+                B200_REQUIRE(r.start_kind == WR_PRECEDING ? r.start_bits >= r.end_bits : r.start_bits <= r.end_bits,
+                             "b200 window: frame start after frame end");
+        }
+        if (!offset(r.start_kind)) r.start_bits = 0;  // unread: equal frames then compare equal
+        if (!offset(r.end_kind)) r.end_bits = 0;
+        range[f] = r;
+        if (r.start_kind == WR_UNBOUNDED_PRECEDING && r.end_kind == WR_CURRENT_ROW) d.frame = WF_RANGE;
+        else if (r.start_kind == WR_UNBOUNDED_PRECEDING && r.end_kind == WR_UNBOUNDED_FOLLOWING) d.frame = WF_PARTITION;
+    }
+
     // The sort first (its chunks and pair buffers are freed on return), then the window scratch and function columns.
     void finish_rows(std::vector<DevBuf>& vbytes) override {
         FullSortState::finish_rows(vbytes);
@@ -1682,6 +1890,8 @@ struct WindowState : FullSortState {
         std::vector<WvFunc> scans;
         WfArgs fa{};
         std::vector<WfFunc> trees;
+        struct RangeFrame { b200_window_range r; std::vector<WfFunc> trees, gathers; };  // the functions of one distinct frame 5
+        std::vector<RangeFrame> ranged;
         bool eval = false;
         for (int f = 0; f < n_funcs; f++) {
             const int c = sc.n_cols + f;
@@ -1697,10 +1907,25 @@ struct WindowState : FullSortState {
             WvFunc g{d.code, d.frame, d.col >= 0 ? sc.ctype[d.col] : CT_INT64, d.col >= 0 ? ctype_size(sc.ctype[d.col]) : 0,
                      ctype_size(sc.ctype[c]), d.default_valid, d.arg, d.default_bits, d.col >= 0 ? out_data[d.col] : nullptr,
                      d.col >= 0 ? out_vb[d.col] : nullptr, out_data[c], out_vb[c]};
-            if (d.frame == WF_BOUNDED || d.code == WN_NTH_VALUE) {  // the frame path only
-                const WfFunc h{g, bound[f].start, bound[f].end};
-                if (wv_aggregate(d.code) && d.col >= 0) trees.push_back(h);
-                else fa.f[fa.n_funcs++] = h;
+            if (d.frame == WF_BOUNDED || d.frame == WF_RANGE_BETWEEN || d.code == WN_NTH_VALUE) {  // the frame path only
+                WfFunc h{};
+                h.g = g;
+                h.start = bound[f].start;
+                h.end = bound[f].end;
+                const bool agg = wv_aggregate(d.code) && d.col >= 0;
+                if (d.frame == WF_RANGE_BETWEEN) {
+                    const b200_window_range& r = range[f];
+                    auto it = std::find_if(ranged.begin(), ranged.end(), [&](const RangeFrame& x) {
+                        return x.r.start_kind == r.start_kind && x.r.end_kind == r.end_kind && x.r.start_bits == r.start_bits &&
+                               x.r.end_bits == r.end_bits;
+                    });
+                    if (it == ranged.end()) it = ranged.insert(ranged.end(), RangeFrame{r, {}, {}});
+                    (agg ? it->trees : it->gathers).push_back(h);
+                } else if (agg) {
+                    trees.push_back(h);
+                } else {
+                    fa.f[fa.n_funcs++] = h;
+                }
                 continue;
             }
             const bool scanned = wv_aggregate(d.code) && d.col >= 0;
@@ -1739,24 +1964,43 @@ struct WindowState : FullSortState {
         B200_CUDA(cudaGetLastError());
         // one tree buffer, reused by every aggregate over a bounded frame: n / 8 + n / 16 + ... nodes of the largest scan value
         // among them, <= 4 B per row (<= 6 B per row with a moment)
-        DevBuf tree;
-        if (!trees.empty() || fa.n_funcs > 0) {
+        DevBuf tree, rb;
+        if (!trees.empty() || fa.n_funcs > 0 || !ranged.empty()) {
             fa.n = n; fa.flags = a.flags; fa.tile = a.tile; fa.psize = a.psize; fa.pend = a.pend;
             int64_t nodes = 0;
             for (int l = WT_LOW; l < WT_LEVELS; l++) { fa.off[l] = nodes; nodes += n >> l; }
-            const bool mom_tree = std::any_of(trees.begin(), trees.end(), [&](const WfFunc& h) { return moments(h.g.code); });
-            if (!trees.empty()) tree.alloc((size_t)std::max<int64_t>(nodes, 1) * (mom_tree ? sizeof(WvMom) : sizeof(WvAgg)));
+            bool mom_tree = std::any_of(trees.begin(), trees.end(), [&](const WfFunc& h) { return moments(h.g.code); });
+            bool any_tree = !trees.empty();
+            for (const RangeFrame& rf : ranged) {
+                any_tree = any_tree || !rf.trees.empty();
+                mom_tree = mom_tree || std::any_of(rf.trees.begin(), rf.trees.end(), [&](const WfFunc& h) { return moments(h.g.code); });
+            }
+            if (any_tree) tree.alloc((size_t)std::max<int64_t>(nodes, 1) * (mom_tree ? sizeof(WvMom) : sizeof(WvAgg)));
             fa.tree = tree.p;
-            for (const WfFunc& h : trees) {
+            const auto launch_tree = [&](const WfFunc& h) {
                 fa.s = h;
                 if (moments(h.g.code)) launch_wf_tree<WV_MOM>(fa, n_tiles, stream);
                 else if (h.g.code == WN_MIN) launch_wf_tree<WV_MIN>(fa, n_tiles, stream);
                 else if (h.g.code == WN_MAX) launch_wf_tree<WV_MAX>(fa, n_tiles, stream);
                 else if (h.g.code != WN_COUNT && ctype_is_float(h.g.ct)) launch_wf_tree<WV_FSUM>(fa, n_tiles, stream);
                 else launch_wf_tree<WV_ISUM>(fa, n_tiles, stream);
-            }
+            };
+            for (const WfFunc& h : trees) launch_tree(h);
             if (fa.n_funcs > 0) window_frame_kernel<WV_GATHER><<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(fa);
             B200_CUDA(cudaGetLastError());
+            // frame 5: one 8 B/row bounds buffer, reused frame by frame (its bounds, then its trees, then its gathers)
+            if (!ranged.empty()) rb.alloc((size_t)n * sizeof(int2));
+            const int ok = std::min(n_part, sc.n_keys - 1);  // the ORDER BY key when there is one (offsets need it)
+            WrArgs ra{n, a.flags, a.tile, a.psize, a.pend, sc.key[ok], out_data[ok], out_vb[ok], 0, 0, 0, 0, rb.as<int2>()};
+            for (RangeFrame& rf : ranged) {
+                ra.start_kind = rf.r.start_kind; ra.end_kind = rf.r.end_kind; ra.start_bits = rf.r.start_bits; ra.end_bits = rf.r.end_bits;
+                window_range_bounds_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(ra);
+                for (WfFunc& h : rf.trees) { h.range = ra.out; launch_tree(h); }
+                fa.n_funcs = 0;
+                for (WfFunc& h : rf.gathers) { h.range = ra.out; fa.f[fa.n_funcs++] = h; }
+                if (fa.n_funcs > 0) window_range_frame_kernel<WV_GATHER><<<(unsigned)(n_tiles * WN_ITEMS), WN_THREADS, 0, stream>>>(fa);
+                B200_CUDA(cudaGetLastError());
+            }
         }
         auto* h = (uint32_t*)pinned_acquire(8);
         B200_CUDA(cudaMemcpyAsync(h, totals.p, 8, cudaMemcpyDeviceToHost, stream));
@@ -1839,6 +2083,21 @@ void* b200_window_state_init_moments(int64_t operator_id, const int8_t* c_types,
                                      int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
                                      const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
                                      int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream) {
+    try {  // this entry's domain: frames 0..4 (the ranges entry adds frame 5); a ranking function, lag or lead with a frame keeps the
+           // constructor's message
+        for (int f = 0; funcs && f < n_funcs && f < b200::SORT_MAX_COLS; f++)
+            if (funcs[f].code >= b200::WN_SUM && funcs[f].code != b200::WN_LAG && funcs[f].code != b200::WN_LEAD)
+                B200_REQUIRE(funcs[f].frame != b200::WF_RANGE_BETWEEN, "b200 window: unknown frame (1 range, 2 rows, 3 partition, 4 rows between)");
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
+    return b200_window_state_init_ranges(operator_id, c_types, arr_types, n_arrs, n_partition_keys, n_order_keys, order_ascending,
+                                         order_na_last, funcs, frames, nullptr, n_funcs, output_batch_size, device, stream);
+}
+
+void* b200_window_state_init_ranges(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                                    int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                                    const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
+                                    const b200_window_range* ranges, int32_t n_funcs, int64_t output_batch_size, int32_t device,
+                                    void* stream) {
     (void)operator_id;
     return b200::sort_state_new(device, [&]() -> SortState* {
         const int np = n_partition_keys, no = n_order_keys;
@@ -1853,8 +2112,8 @@ void* b200_window_state_init_moments(int64_t operator_id, const int8_t* c_types,
             asc[j] = j < np ? 1 : order_ascending[j - np];
             na_last[j] = j < np ? 1 : order_na_last[j - np];
         }
-        return new b200::WindowState(c_types, arr_types, n_arrs, np, np + no, asc, na_last, funcs, frames, n_funcs, output_batch_size,
-                                     device, (cudaStream_t)stream);
+        return new b200::WindowState(c_types, arr_types, n_arrs, np, np + no, asc, na_last, funcs, frames, ranges, n_funcs,
+                                     output_batch_size, device, (cudaStream_t)stream);
     });
 }
 

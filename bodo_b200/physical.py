@@ -317,8 +317,10 @@ class PhysicalWindow:
     """Window sink/source: every input row once, in the stable order by (partition_by ascending NA last, order_by), with one
     column per function after the input columns.  funcs: ranking entries (out_name, fname) or (out_name, "ntile", n), fname one
     of streaming.window.FUNCS; value entries (out_name, fname, column[, frame]), fname one of streaming.window.VALUE_FUNCS or
-    MOMENT_FUNCS (var, std, var_pop, std_pop) and frame one of "range" (default), "rows", "partition" or ("rows", start, end) (ROWS BETWEEN start AND end, None for UNBOUNDED,
-    negative offsets PRECEDING, positive FOLLOWING), (out_name, "lag" | "lead", column[, k[, default]]) or (out_name,
+    MOMENT_FUNCS (var, std, var_pop, std_pop) and frame one of "range" (default), "rows", "partition", ("rows", start, end) (ROWS BETWEEN start AND end, None for UNBOUNDED,
+    negative offsets PRECEDING, positive FOLLOWING) or ("range_between", start, end) (RANGE BETWEEN start AND end, the same
+    spelling with offsets measured in the single ORDER BY key, e.g. -pd.Timedelta("1h")), (out_name, "lag" | "lead", column[, k[,
+    default]]) or (out_name,
     "nth_value", column, n[, frame]);
     ascending / na_position: one value or one per ORDER BY key.  The column names are taken from the first batch."""
 

@@ -5,11 +5,12 @@
     LAG / LEAD (x, k, default) OVER (PARTITION BY p ORDER BY o)
     NTH_VALUE (x, n) OVER (PARTITION BY p ORDER BY o [frame]), and every frame function over ROWS BETWEEN k PRECEDING AND k FOLLOWING
     VAR_SAMP / STDDEV_SAMP / VAR_POP / STDDEV_POP (x) OVER (PARTITION BY p ORDER BY o [frame])
+    every frame function over RANGE BETWEEN x PRECEDING AND y FOLLOWING, an offset measured in the ORDER BY value
 
 pandas equivalents: groupby(p).cumcount() + 1, groupby(p)[o].rank(method="min" / "dense" / "max", pct=...),
 groupby(p)[x].cumsum() / cummin() / cummax() (the "rows" frame), groupby(p)[x].transform("sum" / "mean" / "min" / "max" /
 "count" / "size" / "first" / "last" / "var" / "std") (the "partition" frame), groupby(p)[x].expanding().var() / .std() (the
-"rows" frame), groupby(p)[x].rolling(w).var() / .std() (a bounded frame) and groupby(p)[x].shift(k, fill_value=default) (lag;
+"rows" frame), groupby(p)[x].rolling(w).var() / .std() (a bounded frame), groupby(p).rolling("1h", on=t) (a RANGE frame) and groupby(p)[x].shift(k, fill_value=default) (lag;
 lead is shift(-k)).  The state is a third form of the streaming sort (streaming/sort.py's SortState, sort.cu's WindowState): batches are
 appended to the full sort's device chunk store, is_last sorts every row by (partition keys ascending NA last, order keys, arrival
 index), scans the sorted key columns on the device for partition and peer-group boundaries and then scans or gathers the value
@@ -36,7 +37,18 @@ Semantics:
     [P, pe) the frame is [lo, hi] with lo = P (start None) or max(P, i + start), hi = pe - 1 (end None) or min(pe - 1, i + end),
     empty when lo > hi.  ("rows", None, 0) is "rows" and ("rows", None, None) is "partition".  It takes sum, count, mean, min,
     max, first_value, last_value, nth_value, var, std, var_pop and std_pop, which are then defined as below with [lo, hi] in
-    place of [P, e]; an empty frame gives NA (count 0).  Over [P, e], with a float NaN counted as NA:
+    place of [P, e]; an empty frame gives NA (count 0).  ("range_between", start, end) is RANGE BETWEEN start AND end with the
+    same spelling: None is UNBOUNDED, zero CURRENT ROW (the row's peer group: from its first peer / to its last peer; any ORDER
+    BY), a negative offset PRECEDING and a positive one FOLLOWING, measured in the single ORDER BY key x.  With x ascending a
+    k PRECEDING start is the first row of the partition's non-NA run with x_j >= x_i - k and a k FOLLOWING end the last row
+    with x_j <= x_i + k (a PRECEDING end and a FOLLOWING start mirror these); descending swaps the signs.  Integer and temporal
+    keys compare exactly (no wrap), float keys against fl(x_i -+ k) in double.  An integer key takes an integer offset, a float
+    key an int or float, DATETIME / TIMEDELTA a numpy.timedelta64, datetime.timedelta or pandas.Timedelta, DATE a timedelta of
+    whole days.  A dictionary-encoded string key arrives as its INT32 ids, which the window cannot tell from integers: an
+    offset over it measures distances between ids, so range offsets are meant for numeric and temporal keys only.  At an NA
+    row an offset bound is the NA peer group's boundary; at a non-NA row it never reaches an NA row, and
+    one that no row satisfies leaves the frame empty.  It takes the functions ("rows", start, end) takes;
+    ("range_between", None, 0) is "range" and ("range_between", None, None) is "partition".  Over [P, e], with a float NaN counted as NA:
       count(x): non-NA cells, count(None): COUNT(*) = e - P + 1; int64 numpy.
       sum(x): the sum of the non-NA cells, NA when there are none; integers and bool wrap in 64 bits (int64 for signed and bool,
         uint64 for unsigned), floats accumulate in double (float32 narrowed once at the end); nullable.
@@ -74,6 +86,8 @@ Semantics:
 
 from __future__ import annotations
 
+import datetime
+import struct
 import warnings
 
 import numpy as np
@@ -93,6 +107,9 @@ ROWS_BETWEEN = 4
 UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING = -(1 << 63), (1 << 63) - 1
 # The moments entry's codes (b200_window_state_init_moments): VAR_SAMP, STDDEV_SAMP, VAR_POP and STDDEV_POP.
 MOMENT_FUNCS = {"var": 16, "std": 17, "var_pop": 18, "std_pop": 19}
+# The ranges entry's frame (b200_window_state_init_ranges): RANGE BETWEEN start AND end, with the kinds of b200_window_range.
+RANGE_BETWEEN = 5
+RANGE_KINDS = {"unbounded_preceding": 0, "preceding": 1, "current_row": 2, "following": 3, "unbounded_following": 4}
 BOUNDED_FUNCS = ("sum", "count", "mean", "min", "max", "first_value", "last_value", "nth_value", "var", "std", "var_pop", "std_pop")
 _VALUE_NAMES = {c: f for f, c in {**VALUE_FUNCS, **FRAME_FUNCS, **MOMENT_FUNCS}.items()}
 _FRAME_NAMES = {c: f for f, c in FRAMES.items()}
@@ -101,8 +118,13 @@ MAX_WINDOW_ROWS = MAX_FULL_SORT_ROWS
 MAX_LAG = (1 << 31) - 1
 MAX_FRAME_OFFSET = MAX_LAG
 _TEMPORAL = (CTypes.DATE, CTypes.DATETIME, CTypes.TIMEDELTA)
+_INTEGER = (CTypes.INT8, CTypes.INT16, CTypes.INT32, CTypes.INT64, CTypes.UINT8, CTypes.UINT16, CTypes.UINT32, CTypes.UINT64)
+_NS_PER_UNIT = {"W": 604_800 * 10**9, "D": 86_400 * 10**9, "h": 3_600 * 10**9, "m": 60 * 10**9, "s": 10**9, "ms": 10**6, "us": 10**3,
+                "ns": 1}
+_DAY_NS = 86_400 * 10**9
+_CT_NAMES = {v: k for k, v in vars(CTypes).items() if k.isupper() and isinstance(v, int)}
 _FORMS = (f"ranking: (out_name, fname) with fname in {sorted(FUNCS)}, or (out_name, 'ntile', n); value: (out_name, fname, column"
-          f"[, frame]) with fname in {sorted(set(VALUE_FUNCS) - {'lag', 'lead'} | set(MOMENT_FUNCS))}, frame in {sorted(FRAMES)} or ('rows', start, end), "
+          f"[, frame]) with fname in {sorted(set(VALUE_FUNCS) - {'lag', 'lead'} | set(MOMENT_FUNCS))}, frame in {sorted(FRAMES)}, ('rows', start, end) or ('range_between', start, end), "
           "column None for count(*) only, or (out_name, 'lag' | 'lead', column[, k[, default]]), or (out_name, 'nth_value', column, "
           "n[, frame])")
 
@@ -116,7 +138,7 @@ def _names(x):
 def _parse_value(f, col_names):
     """(out_name, fname, column[, frame]), (out_name, 'lag' | 'lead', column[, k[, default]]) or (out_name, 'nth_value', column,
     n[, frame]) -> (out_name, code, k, column, frame code, default[, (start, end)]); frame code 0 for lag and lead, k = n for
-    nth_value, (start, end) for a ROWS_BETWEEN frame only."""
+    nth_value, (start, end) for a ROWS_BETWEEN or RANGE_BETWEEN frame only."""
     name, fname, column = f[0], f[1], f[2]
     if not (column is None and fname == "count") and not (isinstance(column, str) and column in col_names):
         raise _lib.B200Error(f"Streaming Window: {f!r}: unknown column {column!r} (one of {col_names}; None for count only)")
@@ -124,7 +146,7 @@ def _parse_value(f, col_names):
         if len(f) > 5:
             raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} takes (out_name, {fname!r}, column[, k[, default]])")
         k = f[3] if len(f) > 3 else 1
-        if isinstance(k, str) and k in FRAMES:
+        if isinstance(k, str) and k in FRAMES or isinstance(k, (tuple, list)) and len(k) == 3 and k[0] == "range_between":
             raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} takes no frame")
         if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or not 0 <= k <= MAX_LAG:
             raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} needs an integer k with 0 <= k < 2^31")
@@ -136,7 +158,7 @@ def _parse_value(f, col_names):
                                  "1 <= n < 2^31")
         return (name, FRAME_FUNCS[fname], int(nth), column, *_parse_frame(f, f[4] if len(f) > 4 else "range"))
     if len(f) > 4:
-        raise _lib.B200Error(f"Streaming Window: {f!r}: bad frame (one of {sorted(FRAMES)} or ('rows', start, end), as (out_name, "
+        raise _lib.B200Error(f"Streaming Window: {f!r}: bad frame (one of {sorted(FRAMES)}, ('rows', start, end) or ('range_between', start, end), as (out_name, "
                              f"{fname!r}, column[, frame]))")
     return (name, {**VALUE_FUNCS, **MOMENT_FUNCS}[fname], 0, column, *_parse_frame(f, f[3] if len(f) > 3 else "range"))
 
@@ -147,8 +169,10 @@ def _parse_frame(f, frame):
     "partition", so a frame gives the same results however it is spelled."""
     if isinstance(frame, str) and frame in FRAMES:
         return FRAMES[frame], None
+    if isinstance(frame, (tuple, list)) and len(frame) == 3 and frame[0] == "range_between":
+        return _parse_range(f, frame[1], frame[2])
     if not (isinstance(frame, (tuple, list)) and len(frame) == 3 and frame[0] == "rows"):
-        raise _lib.B200Error(f"Streaming Window: {f!r}: bad frame (one of {sorted(FRAMES)} or ('rows', start, end), as (out_name, "
+        raise _lib.B200Error(f"Streaming Window: {f!r}: bad frame (one of {sorted(FRAMES)}, ('rows', start, end) or ('range_between', start, end), as (out_name, "
                              f"{f[1]!r}, column[, frame]))")
     start, end = frame[1], frame[2]
     for b in (start, end):
@@ -165,6 +189,88 @@ def _parse_frame(f, frame):
     if start is None and end is None:
         return FRAMES["partition"], None
     return (ROWS_BETWEEN, None, (UNBOUNDED_PRECEDING if start is None else int(start), UNBOUNDED_FOLLOWING if end is None else int(end)))
+
+
+def _offset(b):
+    """A RANGE offset -> (family, signed value): ("int", int) for a Python or numpy integer (not bool) with |k| < 2^63,
+    ("float", float) for a finite float that a double holds exactly, ("ns", int) for a numpy.timedelta64 (not NaT, exact in ns),
+    datetime.timedelta or pandas.Timedelta.  None for anything else."""
+    if isinstance(b, (bool, np.bool_)):
+        return None
+    if hasattr(b, "asm8") and isinstance(b, datetime.timedelta):  # pandas.Timedelta, in its own unit
+        b = b.asm8
+    if isinstance(b, np.timedelta64):
+        unit, count = np.datetime_data(b.dtype)
+        if np.isnat(b) or unit not in _NS_PER_UNIT and unit not in ("ps", "fs", "as"):
+            return None
+        v = int(b.astype(np.int64)) * count
+        if unit in _NS_PER_UNIT:
+            ns = v * _NS_PER_UNIT[unit]
+        else:
+            per = {"ps": 10**3, "fs": 10**6, "as": 10**9}[unit]
+            if v % per:
+                return None
+            ns = v // per
+        return ("ns", ns) if abs(ns) < 1 << 63 else None
+    if isinstance(b, datetime.timedelta):
+        ns = ((b.days * 86_400 + b.seconds) * 10**6 + b.microseconds) * 1000
+        return ("ns", ns) if abs(ns) < 1 << 63 else None
+    if isinstance(b, (int, np.integer)):  # numpy.timedelta64 is a numpy integer: handled above
+        return ("int", int(b)) if abs(int(b)) < 1 << 63 else None
+    if isinstance(b, (float, np.floating)):
+        x = float(b)
+        return ("float", x) if np.isfinite(x) and x == b else None
+    return None
+
+
+def _parse_range(f, start, end):
+    """("range_between", start, end), each None (UNBOUNDED), zero (CURRENT ROW) or a signed offset (negative PRECEDING, positive
+    FOLLOWING) -> (RANGE_BETWEEN, None, (start, end)) with zero offsets made 0; (None, 0) is "range" and (None, None) is
+    "partition", so a frame gives the same results however it is spelled.  Offsets are checked against the ORDER BY key's type
+    at the first consume call (WindowState.ranges)."""
+    bounds = []
+    for b in (start, end):
+        if b is None:
+            bounds.append(None)
+            continue
+        o = _offset(b)
+        if o is None:
+            raise _lib.B200Error(f"Streaming Window: {f!r}: bad frame bound {b!r} (None for UNBOUNDED, or an offset: an integer with "
+                                 "|k| < 2^63, a finite float, or a numpy.timedelta64 / datetime.timedelta / pandas.Timedelta exact in "
+                                 "ns; negative PRECEDING, 0 CURRENT ROW, positive FOLLOWING)")
+        bounds.append(0 if o[1] == 0 else b)
+    start, end = bounds
+    if start is not None and end is not None:
+        (fs, s), (fe, e) = _offset(start) or ("int", 0), _offset(end) or ("int", 0)
+        if (fs == "ns") == (fe == "ns") or s == 0 or e == 0:
+            if s > e:
+                raise _lib.B200Error(f"Streaming Window: {f!r}: frame start {start!r} is after frame end {end!r}")
+    if f[1] not in BOUNDED_FUNCS:
+        raise _lib.B200Error(f"Streaming Window: {f!r}: a ('range_between', start, end) frame takes one of {list(BOUNDED_FUNCS)}")
+    if start is None and end is None:
+        return FRAMES["partition"], None
+    if start is None and isinstance(end, int) and end == 0:
+        return FRAMES["range"], None
+    return RANGE_BETWEEN, None, (start, end)
+
+
+def _range_kind(b, end):
+    if b is None:
+        return RANGE_KINDS["unbounded_following" if end else "unbounded_preceding"]
+    if isinstance(b, int) and not isinstance(b, bool) and b == 0:
+        return RANGE_KINDS["current_row"]
+    return RANGE_KINDS["preceding" if _offset(b)[1] < 0 else "following"]
+
+
+def _entry(f):
+    """A parsed value entry as the caller wrote it, with its frame spelled out (for error messages)."""
+    name, code, arg, column, frame = f[:5]
+    fr = _FRAME_NAMES.get(frame)
+    if len(f) > 6 and frame == ROWS_BETWEEN:
+        fr = ("rows", *[None if b in (UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING) else b for b in f[6]])
+    elif len(f) > 6:
+        fr = ("range_between", *f[6])
+    return (name, _VALUE_NAMES[code], column, fr) if code != FRAME_FUNCS["nth_value"] else (name, "nth_value", column, arg, fr)
 
 
 def _default_bits(f, ct):
@@ -186,7 +292,7 @@ def _default_bits(f, ct):
 
 def _parse_funcs(funcs, col_names):
     """Ranking entries -> (out_name, code, n); value entries -> (out_name, code, k, column, frame code, default), with a
-    seventh field (start, end) for a ROWS_BETWEEN frame."""
+    seventh field (start, end) for a ROWS_BETWEEN or RANGE_BETWEEN frame."""
     out = []
     for f in funcs:
         f = tuple(f)
@@ -243,6 +349,10 @@ class WindowState(SortState):
         if any(p not in ("first", "last") for p in nap):
             raise _lib.B200Error(f"Streaming Window: na_position must be 'first' or 'last' (got {nap})")
         parsed = _parse_funcs(funcs, col_names)
+        for f in parsed:
+            if len(f) > 6 and f[4] == RANGE_BETWEEN and len(order) != 1 and any(b not in (None, 0) for b in f[6]):
+                raise _lib.B200Error(f"Streaming Window: {_entry(f)!r}: a range offset (k PRECEDING / FOLLOWING) needs exactly one ORDER "
+                                     f"BY key (got {order})")
         super().__init__(operator_id, None, 0, keys, [True] * len(part) + asc, ["last"] * len(part) + nap, col_names, parallel,
                          output_batch_size, device, stream, process_group, full=True)
         self.partition_by, self.order_by = part, order
@@ -267,8 +377,7 @@ class WindowState(SortState):
             ct = c_types[self.col_names.index(column)]
             moment = code in MOMENT_FUNCS.values()
             if (code in (VALUE_FUNCS["sum"], VALUE_FUNCS["mean"]) or moment) and ct in _TEMPORAL:
-                bounds = [None if b in (UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING) else b for b in f[6]] if len(f) > 6 else None
-                entry = (name, _VALUE_NAMES[code], column, _FRAME_NAMES[frame] if bounds is None else ("rows", *bounds))
+                entry = _entry(f)
                 what = "var and std" if moment else "sum and mean"
                 raise _lib.B200Error(f"Streaming Window: {entry!r}: {what} need an integer, bool or float column, not a temporal one")
             valid = default is not None
@@ -278,11 +387,49 @@ class WindowState(SortState):
     def frames(self):
         """The b200_window_frame (start, end) of every function: its bounds for a ('rows', start, end) frame (code ROWS_BETWEEN),
         else (UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING), which the library does not read."""
-        return [f[6] if len(f) > 6 else (UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING) for f in self.funcs]
+        return [f[6] if len(f) > 6 and f[4] == ROWS_BETWEEN else (UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING) for f in self.funcs]
+
+    def ranges(self, c_types):
+        """The b200_window_range (start_kind, end_kind, start_bits, end_bits) of every function, given the c-types of the input
+        columns in input order: its kinds and offset magnitudes in the ORDER BY key's arithmetic (integers as they are, DATE in
+        days, DATETIME / TIMEDELTA in ns, float keys as the bits of a double) for a ('range_between', start, end) frame (code
+        RANGE_BETWEEN), else (0, 4, 0, 0), which the library does not read.  Raises B200Error for an offset whose type does not fit
+        the key: integers take an integer, floats an integer or float that a double holds exactly, DATETIME / TIMEDELTA a
+        timedelta, DATE a timedelta of whole days; a bool key takes none."""
+        out = []
+        for f in self.funcs:
+            if not (len(f) > 6 and f[4] == RANGE_BETWEEN):
+                out.append((RANGE_KINDS["unbounded_preceding"], RANGE_KINDS["unbounded_following"], 0, 0))
+                continue
+            kinds, bits = [_range_kind(f[6][0], False), _range_kind(f[6][1], True)], [0, 0]
+            for j, b in enumerate(f[6]):
+                if kinds[j] not in (RANGE_KINDS["preceding"], RANGE_KINDS["following"]):
+                    continue
+                key = self.order_by[0]
+                ct = c_types[self.col_names.index(key)]
+                fam, v = _offset(b)
+                k = abs(v)
+                if ct in _INTEGER and fam == "int":
+                    bits[j] = k
+                elif ct in (CTypes.FLOAT32, CTypes.FLOAT64) and fam in ("int", "float") and float(k) == k:
+                    bits[j] = struct.unpack("<Q", struct.pack("<d", float(k)))[0]
+                elif ct in (CTypes.DATETIME, CTypes.TIMEDELTA) and fam == "ns":
+                    bits[j] = k
+                elif ct == CTypes.DATE and fam == "ns" and k % _DAY_NS == 0:
+                    bits[j] = k // _DAY_NS
+                else:
+                    want = ("an integer" if ct in _INTEGER else "an int or float exactly representable as a double"
+                            if ct in (CTypes.FLOAT32, CTypes.FLOAT64) else "a timedelta" if ct in (CTypes.DATETIME, CTypes.TIMEDELTA)
+                            else "a timedelta of whole days" if ct == CTypes.DATE else "no offset (an integer, float or temporal key is needed)")
+                    raise _lib.B200Error(f"Streaming Window: {_entry(f)!r}: range offset {b!r} does not fit ORDER BY key {key!r} of "
+                                         f"type {_CT_NAMES.get(ct, ct)}: it takes {want}")
+            out.append((kinds[0], kinds[1], bits[0], bits[1]))
+        return out
 
     def _ensure(self, table: Table, limit=None, offset=None):
         if self.handle is None and table.n_cols == len(self.col_names):
             self.descs = self.descriptors([c.c_type for c in table.columns])
+            self.rdescs = self.ranges([c.c_type for c in table.columns])
         super()._ensure(table, limit, offset)
 
     def _new_handle(self, L, c_types, a_types, n_cols, asc, nal, limit, offset):
@@ -295,8 +442,11 @@ class WindowState(SortState):
         frs = ffi.new("b200_window_frame[]", len(self.descs))
         for d, (start, end) in zip(frs, self.frames()):
             d.start, d.end = start, end
-        h = L.b200_window_state_init_moments(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs, frs,
-                                             len(self.descs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
+        rs = ffi.new("b200_window_range[]", len(self.descs))
+        for d, (sk, ek, sb, eb) in zip(rs, self.rdescs):
+            d.start_kind, d.end_kind, d.start_bits, d.end_bits = sk, ek, sb, eb
+        h = L.b200_window_state_init_ranges(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs, frs,
+                                            rs, len(self.descs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
         return _lib.check_ptr(h, "init_window_state")
 
 
@@ -310,13 +460,15 @@ def init_window_state(operator_id, partition_by, order_by, ascending, na_positio
     (default "range") or ("rows", start, end) and column None for count(*) only, (out_name, "lag" | "lead", column[, k[,
     default]]) (k = 1 and default None, NA, by default), (out_name, "nth_value", column, n[, frame]), or (out_name, fname,
     column[, frame]) with fname in MOMENT_FUNCS (var, std, var_pop, std_pop) and any frame sum takes.
-    Examples, a 7-row moving average: ("ma7", "mean", "x", ("rows", -6, 0)); a 20-row rolling standard deviation (a Bollinger
+    Examples, a 7-row moving average: ("ma7", "mean", "x", ("rows", -6, 0)); a one-hour time window over a DATETIME ORDER BY
+    key: ("s1h", "sum", "amount", ("range_between", -pd.Timedelta("1h"), 0)); a 20-row rolling standard deviation (a Bollinger
     band's width): ("sd20", "std", "x", ("rows", -19, 0)); the population variance of the partition: ("vp", "var_pop", "x",
     "partition").
     Raises B200Error for an unknown function, duplicate output names or names that clash with an input column, keys that are
     missing or not distinct, a key count outside 1..4, a bad na_position, ntile n < 1, an unknown value column, a bad frame or
-    frame bound, a frame on lag or lead, k outside [0, 2^31), nth_value n outside [1, 2^31); and at the first consume call for sum, mean, var or std of a temporal column or a lag / lead
-    default that the column's dtype cannot hold exactly."""
+    frame bound, a frame on lag or lead, k outside [0, 2^31), nth_value n outside [1, 2^31), a range offset without exactly one
+    ORDER BY key; and at the first consume call for sum, mean, var or std of a temporal column, a lag / lead default that the
+    column's dtype cannot hold exactly or a range offset whose type does not fit the ORDER BY key."""
     return WindowState(operator_id, partition_by, order_by, ascending, na_position, funcs, col_names, parallel, output_batch_size,
                        device, stream, process_group)
 

@@ -262,7 +262,8 @@ void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const i
  *          ROW: up to the row itself, ties in arrival order), 3 partition (the whole partition).  Frames 1..3 start at the
  *          partition's first row.  4 rows between (b200_window_state_init_frames only): ROWS BETWEEN start AND end of the
  *          function's b200_window_frame, for sum, count (of a column or count(*)), mean, min, max, first_value, last_value,
- *          nth_value, var, std, var_pop and std_pop.
+ *          nth_value, var, std, var_pop and std_pop.  5 range between (b200_window_state_init_ranges only): RANGE BETWEEN start
+ *          AND end of the function's b200_window_range, for the same functions.
  *   arg: ntile's n (>= 1); lag / lead's offset k (0 <= k < 2^31; k = 0 is the row itself); nth_value's n (1 <= n < 2^31).
  *   default_valid, default_bits: lag / lead's value when row i - k / i + k is outside the row's partition: the low bytes of
  *          default_bits in the column's type if default_valid, else NA.
@@ -329,6 +330,41 @@ void* b200_window_state_init_moments(int64_t operator_id, const int8_t* c_types,
                                      int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
                                      const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
                                      int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream);
+
+/* The bounds of a frame 5 (RANGE BETWEEN start AND end), measured in ORDER BY values.  Kinds: 0 UNBOUNDED PRECEDING,
+ * 1 PRECEDING, 2 CURRENT ROW, 3 FOLLOWING, 4 UNBOUNDED FOLLOWING, with start_kind <= end_kind, start_kind != 4 and end_kind != 0.
+ * The bits of kinds 1 and 3 hold the offset's magnitude k in the key's arithmetic: a non-negative int64 for an integer key, days
+ * for DATE, ns for DATETIME and TIMEDELTA, the bits of a finite, non-negative double for a FLOAT32 / FLOAT64 key; the other kinds'
+ * bits are not read.  For row i of the partition [P, pe) (sorted positions):
+ *   UNBOUNDED is P (start) or pe - 1 (end).  CURRENT ROW is the row's peer group: its first peer (start) or its last peer (end);
+ *   it takes any ORDER BY, including none and several keys.
+ *   k PRECEDING / k FOLLOWING need exactly one ORDER BY key x, an integer (8 to 64 bits, signed or unsigned), FLOAT32, FLOAT64,
+ *   DATE, DATETIME or TIMEDELTA, numpy or nullable (not BOOL).  With x ascending, a k PRECEDING start is the first row of the
+ *   partition's non-NA run with x_j >= x_i - k, a k FOLLOWING end the last row with x_j <= x_i + k, a k PRECEDING end the last row
+ *   with x_j <= x_i - k and a k FOLLOWING start the first row with x_j >= x_i + k; with x descending PRECEDING means larger
+ *   values, so the signs swap.  Integer and temporal keys compare exactly, with no wrap: a bound beyond the type's range reaches
+ *   the end of the non-NA run.  Float keys compare against fl(x_i -+ k) in IEEE double (FLOAT32 widened exactly first), so -0.0
+ *   equals 0.0 and at x_i = +inf a k PRECEDING start is the first +inf row.
+ *   NA and NaN cells are one peer group at one end of the partition (order_na_last).  At an NA row an offset bound is that peer
+ *   group's first (start) or last (end) row; at a non-NA row an offset bound never reaches an NA row, and an offset bound that no
+ *   non-NA row satisfies leaves the frame empty.
+ * The frame is [lo, hi], empty when lo > hi; the definitions of frame 4 over [lo, hi] apply. */
+typedef struct b200_window_range {
+    int32_t start_kind, end_kind;
+    uint64_t start_bits, end_bits;
+} b200_window_range;
+
+/* b200_window_state_init_moments with frame 5 (range between, code 5): ranges[i] is read only when funcs[i].frame == 5 (ranges
+ * may be NULL when no function uses frame 5).  Frame 5 takes sum, count (of a column or count(*)), mean, min, max, first_value,
+ * last_value, nth_value, var, std, var_pop and std_pop.  Bad kinds, an offset without exactly one ORDER BY key, an offset on a
+ * BOOL key, a negative or non-finite offset, or start after end fails here (NULL, last error set).  (UNBOUNDED PRECEDING, CURRENT
+ * ROW) is frame 1 and (UNBOUNDED PRECEDING, UNBOUNDED FOLLOWING) frame 3, with the same results.
+ * b200_window_state_init_moments is this entry with ranges NULL, restricted to frames 0..4. */
+void* b200_window_state_init_ranges(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                                    int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                                    const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
+                                    const b200_window_range* ranges, int32_t n_funcs, int64_t output_batch_size, int32_t device,
+                                    void* stream);
 
 /* The build-consume entry of _sort.cpp: filters a DEVICE-resident batch (same schema as the state) against the current cutoff on
  * the device (full sort: appends it to the chunk store); on is_last reduces to the final rows (full sort: sorts every row).
