@@ -43,7 +43,8 @@ enum OpKind : int { K_SUM_I64 = 0, K_SUM_F64, K_COUNT, K_SIZE, K_MEAN, K_MIN_I64
                     K_NUNIQUE,  // number of distinct non-NA values: filled at finalize from a nested (key, value) distinct state
                     // evaluation-only kinds of composite functions (accumulators: K_MOM1 + K_MOM2 (+ K_MOM3))
                     E_VAR, E_STD, E_VAR_POP, E_STD_POP, E_SKEW,
-                    K_SHIFT, K_MOM1 };
+                    K_SHIFT, K_MOM1,
+                    K_MRNF };  // one word of a min_row_number_filter winner record (see mrnf_merge_kernel); no consume kernel applies it
 constexpr unsigned long long SHIFT_UNSET = 0x7ff8000000000000ull;  // K_SHIFT's initial value (quiet NaN; NaN values are skipped)
 
 struct OpDesc {
@@ -1019,6 +1020,199 @@ __global__ void eval_mk_keys_kernel(const __grid_constant__ EvalMkKeysArgs a) {
     }
 }
 
+// ---- min_row_number_filter (MRNF): QUALIFY ROW_NUMBER() OVER (PARTITION BY keys ORDER BY sort columns) = 1 ----
+// Every group keeps the first row of the stable order by (sort columns, arrival).  A row's rank is the tuple (class_0, word_0,
+// ..., class_{n-1}, word_{n-1}, seq) of the sort's key encoding (sort_word / sort_class) and its arrival number seq = rows
+// consumed before it + 1.  The tuple is one bit string (fields in that order, each at its own width, seq in MRNF_SEQ_BITS bits)
+// cut into big-endian digits of 63 bits; a digit's top bit is always 0, so no digit of a row is all-ones, the value a free
+// scratch digit holds.  Comparing digit strings lexicographically is comparing the tuples, and seq makes every row's distinct.
+// Per slot the table carries the winner record W (n_digits digits, a validity word with bit j = kept column j valid, one 8-byte
+// word per kept column: K_MRNF accumulators, moved by the rehash as any other) and the batch scratch B (n_digits words, all-ones
+// between batches).  Per batch, once every row is in the table: digit pass d = 0 .. n_digits-1 (mrnf_min_kernel) takes the
+// minimum of digit d over the rows whose digits 0..d-1 equal B's, so B ends as the batch's least tuple per slot; then
+// mrnf_merge_kernel lets the one row equal to B compare itself against W, replace it when smaller and reset B.
+constexpr int MRNF_MAX_DIGITS = 5;           // 4 keys x (1 + 64) bits + MRNF_SEQ_BITS <= 5 x 63
+constexpr int MRNF_SEQ_BITS = 48;
+constexpr int MRNF_FIELDS = 2 * MAX_KEYS + 1;  // class and word per sort key, then seq
+constexpr int MRNF_MAX_KEEP = 2 * MAX_OPS - MRNF_MAX_DIGITS - 1;  // what the rehash carries besides the digits and validity word
+constexpr unsigned long long MRNF_DIGIT_MASK = 0x7FFFFFFFFFFFFFFFull;
+
+struct MrnfArgs {
+    int64_t n_rows;
+    unsigned long long seq_base;  // rows consumed before this batch
+    // the table (single-column: tkeys; multi-column: tags / mk / mkmask) and the batch's key columns (float keys canonical)
+    int nk, dropna;
+    const void* key_data[MAX_KEYS];
+    const uint8_t* key_valid[MAX_KEYS];
+    int key_ctype[MAX_KEYS];
+    const long long* tkeys;
+    const unsigned long long* tags;
+    const long long* mk[MAX_KEYS];
+    const unsigned char* mkmask;
+    uint64_t cap;
+    uint64_t* slot;  // per batch row: its slot (pass 0 writes it, later passes read it), ~0 = dropped (NA key, dropna)
+    // the order
+    int n_sort, n_digits;
+    SortKey key[MAX_KEYS];
+    const void* sort_data[MAX_KEYS];
+    const uint8_t* sort_valid[MAX_KEYS];
+    int f_end[MRNF_FIELDS];  // bit position just past each field in the tuple's bit string (fields of absent keys are 0)
+    unsigned long long* b;   // B: digit d of slot s at b[d * (cap + 2) + s]
+    unsigned long long* w[MRNF_MAX_DIGITS];
+    unsigned long long* w_valid;
+    // the kept columns as the batch holds them (a kept key column is read here, not from its canonical column)
+    int n_keep;
+    const void* keep_data[MRNF_MAX_KEEP];
+    const uint8_t* keep_valid[MRNF_MAX_KEEP];
+    int keep_size[MRNF_MAX_KEEP];
+    unsigned long long* keep_w[MRNF_MAX_KEEP];
+};
+
+// lookup only in the multi-column table (the key tuple of batch row `row`, NK columns); ~0 when the row was dropped (dropna) or
+// its tuple is not in the table.  NK is a template argument so that the tuple stays in registers.
+template <int NK>
+__device__ __forceinline__ uint64_t find_only_mk(const MrnfArgs& a, int64_t row) {
+    long long keys[NK];
+    unsigned int mask = 0;
+#pragma unroll
+    for (int j = 0; j < NK; j++) {
+        const bool v = bit_valid(a.key_valid[j], row);
+        keys[j] = v ? (long long)load_int_as_i64(a.key_data[j], a.key_ctype[j], row) : 0;
+        mask |= v ? (1u << j) : 0u;
+    }
+    if (a.dropna && mask != (1u << NK) - 1u) return ~0ull;
+    const unsigned long long tag = mk_tag(keys, mask, NK);
+    const uint64_t m = a.cap - 1;
+    uint64_t s = (tag >> 20) & m;
+    for (uint64_t probes = 0; probes <= m; probes++) {
+        const unsigned long long t = __ldcg(a.tags + s);
+        if (t == tag) {
+            bool eq = __ldcg(a.mkmask + s) == (unsigned char)mask;
+#pragma unroll
+            for (int j = 0; j < NK; j++) eq = eq && __ldcg(a.mk[j] + s) == keys[j];
+            if (eq) return s;
+        } else if (t == TAG_EMPTY) {
+            return ~0ull;
+        }
+        s = (s + 1) & m;
+    }
+    return ~0ull;
+}
+// the slot of batch row `row` (every row is in the table), as the consume kernels placed it; ~0 for a row they dropped
+__device__ __forceinline__ uint64_t mrnf_find_slot(const MrnfArgs& a, int64_t row) {
+    switch (a.nk) {
+        case 1: {
+            if (!bit_valid(a.key_valid[0], row)) return a.dropna ? ~0ull : a.cap;
+            const long long key = load_int_as_i64(a.key_data[0], a.key_ctype[0], row);
+            return key == EMPTY_KEY ? a.cap + 1 : find_only(a.tkeys, a.cap, key);
+        }
+        case 2: return find_only_mk<2>(a, row);
+        case 3: return find_only_mk<3>(a, row);
+        default: return find_only_mk<4>(a, row);
+    }
+}
+// the tuple's fields of batch row `row`
+__device__ __forceinline__ void mrnf_fields(const MrnfArgs& a, int64_t row, unsigned long long* v) {
+#pragma unroll
+    for (int j = 0; j < MAX_KEYS; j++) {
+        v[2 * j] = v[2 * j + 1] = 0;
+        if (j < a.n_sort) {
+            bool na = !bit_valid(a.sort_valid[j], row);
+            v[2 * j + 1] = sort_word(a.key[j], load_bits(a.sort_data[j], a.key[j].size, row), na);
+            v[2 * j] = sort_class(a.key[j], na);
+        }
+    }
+    v[2 * MAX_KEYS] = a.seq_base + (unsigned long long)row + 1ull;
+}
+// digit d: bits [63 d, 63 d + 63) of the bit string; bit i of field f lands at bit i + 63 d + 63 - f_end[f] of the digit
+__device__ __forceinline__ unsigned long long mrnf_digit(const MrnfArgs& a, const unsigned long long* v, int d) {
+    unsigned long long r = 0;
+#pragma unroll
+    for (int f = 0; f < MRNF_FIELDS; f++) {
+        const int sh = 63 * d + 63 - a.f_end[f];
+        if (sh >= 0 && sh < 64) r |= v[f] << sh;
+        else if (sh < 0 && sh > -64) r |= v[f] >> -sh;
+    }
+    return r & MRNF_DIGIT_MASK;
+}
+
+// digit pass d: B[d] = min of digit d over the slot's rows whose digits 0..d-1 equal B[0..d-1]
+__global__ void __launch_bounds__(256) mrnf_min_kernel(const __grid_constant__ MrnfArgs a, int d) {
+    const uint64_t stride_b = a.cap + 2;
+    for (int64_t row = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; row < a.n_rows; row += (int64_t)gridDim.x * blockDim.x) {
+        uint64_t slot;
+        if (d == 0) { slot = mrnf_find_slot(a, row); a.slot[row] = slot; }
+        else slot = a.slot[row];
+        if (slot == ~0ull) continue;
+        unsigned long long v[MRNF_FIELDS];
+        mrnf_fields(a, row, v);
+        bool in = true;
+        for (int e = 0; e < d && in; e++) in = mrnf_digit(a, v, e) == a.b[e * stride_b + slot];
+        if (!in) continue;
+        unsigned long long* bp = a.b + d * stride_b + slot;
+        const unsigned long long x = mrnf_digit(a, v, d);
+        if (x < __ldcg(bp)) atomicMin(bp, x);  // (read first: with few groups most rows lose without an atomic)
+    }
+}
+// The row equal to B (one per touched slot: seq differs between rows) replaces W when its tuple is smaller, then resets B.
+// Another row of the slot may read B while it is being reset; it sees each digit either as the winner's or as all-ones, which
+// no digit of a row equals, so it cannot match.
+__global__ void __launch_bounds__(256) mrnf_merge_kernel(const __grid_constant__ MrnfArgs a) {
+    const uint64_t stride_b = a.cap + 2;
+    for (int64_t row = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; row < a.n_rows; row += (int64_t)gridDim.x * blockDim.x) {
+        const uint64_t slot = a.slot[row];
+        if (slot == ~0ull) continue;
+        unsigned long long v[MRNF_FIELDS];
+        mrnf_fields(a, row, v);
+        bool win = true;
+        for (int e = 0; e < a.n_digits && win; e++) win = mrnf_digit(a, v, e) == __ldcg(a.b + e * stride_b + slot);
+        if (!win) continue;
+        bool smaller = false;
+        for (int e = 0; e < a.n_digits; e++) {
+            const unsigned long long x = mrnf_digit(a, v, e), y = a.w[e][slot];
+            if (x != y) { smaller = x < y; break; }
+        }
+        if (smaller) {
+            for (int e = 0; e < a.n_digits; e++) a.w[e][slot] = mrnf_digit(a, v, e);
+            unsigned long long vw = 0;
+            for (int j = 0; j < a.n_keep; j++) {
+                a.keep_w[j][slot] = load_bits(a.keep_data[j], a.keep_size[j], row);
+                vw |= bit_valid(a.keep_valid[j], row) ? 1ull << j : 0ull;
+            }
+            a.w_valid[slot] = vw;
+        }
+        for (int e = 0; e < a.n_digits; e++) a.b[e * stride_b + slot] = ~0ull;
+    }
+}
+
+struct MrnfOutArgs {
+    const uint64_t* slot_of_out;
+    const long long* n_out_ptr;
+    const unsigned long long* w_valid;
+    int n_keep;
+    const unsigned long long* keep_w[MRNF_MAX_KEEP];
+    int keep_size[MRNF_MAX_KEEP];
+    void* out[MRNF_MAX_KEEP];
+    uint32_t* out_valid[MRNF_MAX_KEEP];  // validity bitmap as 32-bit words (nullable kept columns), else nullptr
+};
+// finalize: the winner's cells of every kept column, at the column's width, for the compacted slots
+__global__ void mrnf_gather_kernel(const __grid_constant__ MrnfOutArgs a) {
+    const int64_t n_out = *a.n_out_ptr;
+    const int64_t n_round = (n_out + 31) & ~31ll;
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < n_round; p += (int64_t)gridDim.x * blockDim.x) {
+        const bool in = p < n_out;
+        const uint64_t s = in ? a.slot_of_out[p] : 0;
+        const unsigned long long vw = in ? a.w_valid[s] : 0ull;
+        for (int j = 0; j < a.n_keep; j++) {
+            if (in) copy_cell(a.out[j], p, a.keep_w[j] + s, 0, a.keep_size[j]);
+            if (a.out_valid[j]) {
+                const unsigned m = __ballot_sync(0xffffffffu, (vw >> j) & 1ull);
+                if ((threadIdx.x & 31) == 0) a.out_valid[j][p >> 5] = m;
+            }
+        }
+    }
+}
+
 // ================================================================================================
 // SM-partitioned groupby (SPG): the fast path for cardinalities whose accumulators fit the chip's
 // aggregate shared memory (≈ SMs x 10k groups).  Motivation (scratch/ubench*.cu): two global `red`s per
@@ -1760,6 +1954,15 @@ static bool set_smem_limit(const void* fn, size_t bytes) {
     return false;
 }
 
+// The arguments of a min_row_number_filter state (b200_groupby_state_init_mrnf), checked by GroupbyState::setup_mrnf.
+struct MrnfSpec {
+    int n_sort;
+    const int32_t* sort_cols;
+    const int32_t* ascending;
+    const int32_t* na_last;
+    const int32_t* keep;  // one flag per column
+};
+
 class GroupbyState {
    public:
     int device;
@@ -1840,7 +2043,7 @@ class GroupbyState {
 
     GroupbyState(const int8_t* ct, const int8_t* at, int n_arrs, const int32_t* ftypes, const int32_t* f_in_offsets,
                  const int32_t* f_in_cols, int n_funcs_, uint64_t n_keys, int64_t out_bs, bool parallel_, bool dropna_,
-                 int device_, int n_pes_, int rank_, int64_t expected_groups, cudaStream_t stream_)
+                 int device_, int n_pes_, int rank_, int64_t expected_groups, cudaStream_t stream_, const MrnfSpec* mrnf = nullptr)
         : device(device_), stream(stream_), n_cols(n_arrs), n_funcs(0), n_outs(n_funcs_), dropna(dropna_), parallel(parallel_),
           n_pes(n_pes_), rank(rank_), output_batch_size(out_bs) {
         B200_REQUIRE(n_keys >= 1 && n_keys <= (uint64_t)MAX_KEYS, "b200 groupby: between 1 and 4 key columns are supported");
@@ -1945,8 +2148,9 @@ class GroupbyState {
             outs.push_back(o);
             funcs.push_back(f);
         }
+        if (mrnf) setup_mrnf(*mrnf);
         n_funcs = (int)funcs.size();
-        B200_REQUIRE(n_funcs <= MAX_OPS, "b200 groupby: too many aggregate functions (composite ones count their accumulator columns)");
+        B200_REQUIRE(mr.on || n_funcs <= MAX_OPS, "b200 groupby: too many aggregate functions (composite ones count their accumulator columns)");
         d_a0.resize(n_funcs); d_a1.resize(n_funcs);
         d_out_data.resize(n_outs); d_out_valid.resize(n_outs);
         d_counters.alloc(N_COUNTERS * sizeof(long long));
@@ -2090,7 +2294,7 @@ class GroupbyState {
             MkArgs a = mk_table_args();
             a.dropna = dropna ? 1 : 0; a.n_rows = rows; a.index_list = index_list;
             for (int j = 0; j < nk; j++) { a.key_data[j] = data[j]; a.key_valid[j] = valid[j]; a.key_ctype[j] = c_types[j]; }
-            a.n_ops = n_funcs;
+            a.n_ops = n_apply();
             fill_ops(a.ops, data, valid);
             groupby_consume_mk_kernel<<<grid_for(rows), 256, 0, stream>>>(a);
             launches++; consume_launches += index_list == nullptr;
@@ -2633,15 +2837,17 @@ class GroupbyState {
         ConsumeArgs a{};
         a.key_data = data[0]; a.key_valid = valid[0]; a.key_ctype = c_types[0]; a.dropna = dropna ? 1 : 0;
         a.n_rows = rows; a.index_list = index_list; a.tkeys = d_keys.as<long long>(); a.cap = cap;
-        a.counters = d_counters.as<long long>(); a.group_limit = (long long)(cap / 2); a.fail_list = d_fail.as<uint32_t>(); a.n_ops = n_funcs;
+        a.counters = d_counters.as<long long>(); a.group_limit = (long long)(cap / 2); a.fail_list = d_fail.as<uint32_t>(); a.n_ops = n_apply();
         // rank-major sequence numbers: rows of a lower rank come first (the reference's row-block distribution), then row order
         a.seq_base = ((unsigned long long)rank << 44) + (unsigned long long)rows_consumed;
         fill_ops(a.ops, data, valid);
         return a;
     }
-    // the n_funcs aggregate updates of a consume launch (ConsumeArgs / MkArgs)
+    // the aggregate updates a consume launch applies per row: every function's, none for MRNF (its passes run after the launch)
+    int n_apply() const { return mr.on ? 0 : n_funcs; }
+    // the n_apply() aggregate updates of a consume launch (ConsumeArgs / MkArgs)
     void fill_ops(OpDesc* ops, const std::vector<const void*>& data, const std::vector<const uint8_t*>& valid) const {
-        for (int j = 0; j < n_funcs; j++) {
+        for (int j = 0; j < n_apply(); j++) {
             const FuncSpec& f = funcs[j];
             ops[j].kind = f.kind; ops[j].in_ctype = f.in_ctype;
             ops[j].in_data = f.in_col >= 0 ? data[f.in_col] : nullptr;
@@ -2673,6 +2879,131 @@ class GroupbyState {
             data[kc] = d_canon[kc].p;
         }
     }
+    // one device-resident chunk of a batch: keys canonicalised, then aggregated (MRNF also reads the batch's own cells)
+    void consume_chunk(std::vector<const void*>& data, const std::vector<const uint8_t*>& valid, int64_t n) {
+        const std::vector<const void*> raw = data;
+        canon_keys(data, n);
+        if (mr.on) consume_mrnf(data, raw, valid, n);
+        else consume_device_chunk(data, valid, n);
+    }
+
+    // ---- min_row_number_filter (see mrnf_min_kernel) ----
+    struct Mrnf {
+        bool on = false;
+        int n_sort = 0, n_digits = 0;
+        int sort_col[MAX_KEYS] = {};
+        SortKey key[MAX_KEYS] = {};
+        int f_end[MRNF_FIELDS] = {};
+        std::vector<int> keep;  // kept columns, in column order
+        int w0 = 0;             // funcs[w0 ..): the winner's digits, its validity word, one word per kept column
+        DevBuf b, slot;         // B (n_digits x (b_cap + 2) words) and the batch's slot cache
+        uint64_t b_cap = 0;
+    } mr;
+
+    void setup_mrnf(const MrnfSpec& s) {
+        B200_REQUIRE(n_outs == 0, "b200 groupby: min_row_number_filter takes no other aggregate function");
+        B200_REQUIRE(s.n_sort >= 1 && s.n_sort <= MAX_KEYS, "b200 groupby: min_row_number_filter takes 1 to 4 sort columns");
+        mr.on = true;
+        mr.n_sort = s.n_sort;
+        int bits = 0;
+        for (int j = 0; j < s.n_sort; j++) {
+            const int c = s.sort_cols[j];
+            const std::string what = "b200 groupby: min_row_number_filter sort column " + std::to_string(j) + " (column " + std::to_string(c) + ")";
+            B200_REQUIRE(c >= 0 && c < n_cols, what + " is out of range");
+            for (int q = 0; q < j; q++) B200_REQUIRE(s.sort_cols[q] != c, what + " is listed twice");
+            B200_REQUIRE(ctype_size(in_types[c]) > 0, what + " is not a fixed-width column");
+            B200_REQUIRE(arr_types[c] == ARR_NUMPY || arr_types[c] == ARR_NULLABLE, what + " has an unsupported array type");
+            mr.sort_col[j] = c;
+            mr.key[j] = SortKey{in_types[c], ctype_size(in_types[c]), s.ascending[j] ? 0 : 1, s.na_last[j] ? 1 : 0};
+            mr.f_end[2 * j] = bits += 1;
+            mr.f_end[2 * j + 1] = bits += 8 * ctype_size(in_types[c]);
+        }
+        mr.f_end[2 * MAX_KEYS] = bits += MRNF_SEQ_BITS;
+        mr.n_digits = (bits + 62) / 63;
+        for (int c = 0; c < n_cols; c++) {
+            if (!s.keep[c]) continue;
+            const std::string what = "b200 groupby: min_row_number_filter kept column " + std::to_string(c);
+            B200_REQUIRE(ctype_size(in_types[c]) > 0, what + " is not a fixed-width column");
+            B200_REQUIRE(arr_types[c] == ARR_NUMPY || arr_types[c] == ARR_NULLABLE, what + " has an unsupported array type");
+            mr.keep.push_back(c);
+        }
+        B200_REQUIRE(!mr.keep.empty(), "b200 groupby: min_row_number_filter keeps no column");
+        B200_REQUIRE((int)mr.keep.size() <= MRNF_MAX_KEEP, "b200 groupby: min_row_number_filter keeps at most " + std::to_string(MRNF_MAX_KEEP) + " columns");
+        // the winner record: digits all-ones (above every row's tuple), validity and payload zero
+        mr.w0 = (int)funcs.size();
+        FuncSpec w{};
+        w.in_col = -1; w.in_ctype = CT_INT64; w.in_arrtype = ARR_NUMPY; w.kind = K_MRNF; w.out_ctype = CT_INT64; w.out_arrtype = ARR_NUMPY;
+        for (int e = 0; e < mr.n_digits + 1 + (int)mr.keep.size(); e++) {
+            w.init0 = e < mr.n_digits ? ~0ull : 0ull;
+            funcs.push_back(w);
+        }
+    }
+
+    void consume_mrnf(const std::vector<const void*>& keys, const std::vector<const void*>& raw, const std::vector<const uint8_t*>& valid, int64_t n) {
+        if (n == 0) return;
+        B200_REQUIRE(rows_consumed + n < (1ll << MRNF_SEQ_BITS), "b200 groupby: min_row_number_filter takes fewer than 2^48 rows");
+        const unsigned long long seq_base = (unsigned long long)rows_consumed;
+        // insert the keys (no aggregate: n_apply() is 0); the table grows and the failed rows are replayed until all are in
+        if (nk > 1) consume_mk(keys, valid, n);
+        else consume_direct(keys, valid, n, false, -1, -1, -1, false);
+        if (mr.b_cap != cap) {  // (B is all-ones whenever the table grows: a fresh B for the new capacity)
+            mr.b.alloc((size_t)mr.n_digits * (cap + 2) * 8);
+            fill(mr.b.p, (uint64_t)mr.n_digits * (cap + 2), ~0ull);
+            mr.b_cap = cap;
+        }
+        mr.slot.ensure((size_t)n * 8);
+        MrnfArgs a{};
+        a.n_rows = n; a.seq_base = seq_base; a.nk = nk; a.dropna = dropna ? 1 : 0; a.cap = cap;
+        for (int j = 0; j < nk; j++) { a.key_data[j] = keys[j]; a.key_valid[j] = valid[j]; a.key_ctype[j] = c_types[j]; }
+        if (nk == 1) a.tkeys = d_keys.as<long long>();
+        else {
+            a.tags = d_tags.as<unsigned long long>(); a.mkmask = d_mkmask.as<unsigned char>();
+            for (int j = 0; j < nk; j++) a.mk[j] = d_mk[j].as<long long>();
+        }
+        a.slot = mr.slot.as<uint64_t>();
+        a.n_sort = mr.n_sort; a.n_digits = mr.n_digits;
+        for (int j = 0; j < mr.n_sort; j++) { a.key[j] = mr.key[j]; a.sort_data[j] = raw[mr.sort_col[j]]; a.sort_valid[j] = valid[mr.sort_col[j]]; }
+        std::copy(mr.f_end, mr.f_end + MRNF_FIELDS, a.f_end);
+        a.b = mr.b.as<unsigned long long>();
+        for (int e = 0; e < mr.n_digits; e++) a.w[e] = d_a0[mr.w0 + e].as<unsigned long long>();
+        a.w_valid = d_a0[mr.w0 + mr.n_digits].as<unsigned long long>();
+        a.n_keep = (int)mr.keep.size();
+        for (int j = 0; j < a.n_keep; j++) {
+            const int c = mr.keep[j];
+            a.keep_data[j] = raw[c]; a.keep_valid[j] = valid[c]; a.keep_size[j] = ctype_size(in_types[c]);
+            a.keep_w[j] = d_a0[mr.w0 + mr.n_digits + 1 + j].as<unsigned long long>();
+        }
+        for (int d = 0; d < mr.n_digits; d++) mrnf_min_kernel<<<grid_for(n), 256, 0, stream>>>(a, d);
+        mrnf_merge_kernel<<<grid_for(n), 256, 0, stream>>>(a);
+        launches += mr.n_digits + 1;
+        B200_CUDA(cudaGetLastError());
+    }
+
+    int64_t finalize_mrnf() {
+        compact();
+        const int64_t max_out = max_out_bound();
+        const size_t words = (size_t)((max_out + 31) / 32 + 1);
+        const int n_keep = (int)mr.keep.size();
+        d_out_data.resize(n_keep); d_out_valid.resize(n_keep);
+        MrnfOutArgs o{};
+        o.slot_of_out = d_slot_of_out.as<uint64_t>(); o.n_out_ptr = d_counters.as<long long>() + CTR_OUT;
+        o.w_valid = d_a0[mr.w0 + mr.n_digits].as<unsigned long long>(); o.n_keep = n_keep;
+        for (int j = 0; j < n_keep; j++) {
+            const int c = mr.keep[j];
+            o.keep_w[j] = d_a0[mr.w0 + mr.n_digits + 1 + j].as<unsigned long long>(); o.keep_size[j] = ctype_size(in_types[c]);
+            d_out_data[j].ensure((size_t)(max_out + 32) * 8);
+            o.out[j] = d_out_data[j].p;
+            if (arr_types[c] == ARR_NULLABLE) { d_out_valid[j].ensure(words * 4); o.out_valid[j] = d_out_valid[j].as<uint32_t>(); }
+        }
+        mrnf_gather_kernel<<<grid_for(max_out), 256, 0, stream>>>(o);
+        launches++;
+        B200_CUDA(cudaGetLastError());
+        read_counters();
+        n_out = h_counters[CTR_OUT];
+        finalized = true;
+        out_cursor = 0;
+        return n_out;
+    }
 
     void consume(const b200_table* t) {
         B200_REQUIRE(!build_done, "b200 groupby: consume after the build was finished");
@@ -2682,6 +3013,11 @@ class GroupbyState {
         std::vector<bool> used(n_cols, false);
         for (int kc = 0; kc < nk; kc++) used[kc] = true;
         for (auto& f : funcs) if (f.in_col >= 0) used[f.in_col] = true;
+        if (mr.on) {
+            B200_REQUIRE(n_pes == 1, "b200 groupby: a sharded min_row_number_filter is not supported (n_pes > 1); run it on one rank");
+            for (int j = 0; j < mr.n_sort; j++) used[mr.sort_col[j]] = true;
+            for (int c : mr.keep) used[c] = true;
+        }
         for (int c = 0; c < n_cols; c++) {
             if (!used[c]) continue;
             B200_REQUIRE(t->cols[c].c_type == in_types[c], "b200 groupby: batch column dtype differs from the build schema");
@@ -2708,8 +3044,7 @@ class GroupbyState {
                     data[c] = (const char*)t->cols[c].data + r0 * ctype_size(in_types[c]);
                     valid[c] = t->cols[c].validity ? t->cols[c].validity + r0 / 8 : nullptr;
                 }
-                canon_keys(data, rows);
-                consume_device_chunk(data, valid, rows);
+                consume_chunk(data, valid, rows);
             }
             return;
         }
@@ -2746,8 +3081,7 @@ class GroupbyState {
             }
             B200_CUDA(cudaEventRecord(stage_ready[b], copy_stream));
             B200_CUDA(cudaStreamWaitEvent(stream, stage_ready[b], 0));
-            canon_keys(data, rows);
-            consume_device_chunk(data, valid, rows);
+            consume_chunk(data, valid, rows);
             B200_CUDA(cudaEventRecord(stage_free[b], stream));
             stage_recorded[b] = true;
         }
@@ -2763,6 +3097,7 @@ class GroupbyState {
     int64_t co_n = 0, co_batches = 0;
     int co_vcol = -1;
     bool coalesce(const b200_table* t, int64_t n) {
+        if (mr.on) return false;
         if (n == 0 || n >= CO_MIN_BATCH || nk != 1 || n_funcs < 1 || c_types[0] != CT_INT64 || t->cols[0].validity != nullptr) return false;
         { const char* e = getenv("B200_COALESCE"); if (e && e[0] == '0') return false; }
         int vcol = -1;
@@ -2858,6 +3193,7 @@ class GroupbyState {
         if (finalized) return n_out;
         ScopedTimer timer{t_finalize};
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
+        if (mr.on) return finalize_mrnf();
         flush_coalesced();
         // the exchange settles first, so that nunique also counts into the groups it brought
         if (exchanged && !settle_exchange()) return -2;
@@ -2965,6 +3301,7 @@ class GroupbyState {
     // (send_buf) the rows of destination d at the exclusive prefix of the counts of the previous pack; neither: count only.
     void exchange_pack(void* const* peer_slabs_dev, int64_t cap_rows, void* send_buf) {
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
+        B200_REQUIRE(!mr.on, "b200 groupby: a sharded min_row_number_filter is not supported (no exchange of winner records)");
         flush_coalesced();
         build_done = true;
         const size_t cursor_bytes = (size_t)std::max(n_pes, 32) * 8;
@@ -3065,6 +3402,19 @@ class GroupbyState {
         B200_REQUIRE(out->cols != nullptr, "b200 groupby: out->cols must point to n_keys + n_funcs descriptors");
         out->n_rows = rows; out->n_cols = nk + n_outs; out->device = device;
         int64_t off = out_cursor;
+        if (mr.on) {  // the kept columns only
+            out->n_cols = (int32_t)mr.keep.size();
+            for (size_t j = 0; j < mr.keep.size(); j++) {
+                const int c = mr.keep[j];
+                b200_column& k = out->cols[j];
+                k.data = (char*)d_out_data[j].p + off * ctype_size(in_types[c]);
+                k.validity = arr_types[c] == ARR_NULLABLE ? d_out_valid[j].as<uint8_t>() + off / 8 : nullptr;
+                k.length = rows; k.c_type = in_types[c]; k.arr_type = arr_types[c];
+            }
+            out_cursor += rows;
+            *out_is_last = out_cursor >= n_out ? 1 : 0;
+            return 0;
+        }
         for (int kc = 0; kc < nk; kc++) {
             b200_column& k = out->cols[kc];
             const DevBuf& kd = nk == 1 ? d_out_keys : d_out_mk[kc];
@@ -3113,6 +3463,27 @@ void* b200_groupby_state_init(int64_t operator_id, const int8_t* build_arr_c_typ
     return new GroupbyState(build_arr_c_types, build_arr_array_types, n_build_arrs, ftypes, f_in_offsets, f_in_cols, n_funcs,
                             n_keys, output_batch_size, parallel != 0, pandas_drop_na != 0, device, n_pes, myrank,
                             expected_groups, (cudaStream_t)stream);
+    B200_CATCH(nullptr)
+}
+
+void* b200_groupby_state_init_mrnf(int64_t operator_id, const int8_t* build_arr_c_types, const int8_t* build_arr_array_types,
+                                   int32_t n_build_arrs, uint64_t n_keys, const int32_t* sort_cols, const int32_t* sort_ascending,
+                                   const int32_t* sort_na_last, int32_t n_sort, const int32_t* keep, int64_t output_batch_size,
+                                   int32_t parallel, int32_t pandas_drop_na, int32_t device, int32_t n_pes, int32_t myrank,
+                                   int64_t expected_groups, void* stream) {
+    (void)operator_id;
+    B200_TRY
+    B200_REQUIRE(build_arr_c_types && build_arr_array_types && keep && (n_sort <= 0 || (sort_cols && sort_ascending && sort_na_last)),
+                 "b200 groupby: null min_row_number_filter argument");
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+        throw b200::Error("b200 groupby: no CUDA device available (this path has no CPU fallback)");
+    B200_REQUIRE(device >= 0 && device < ndev, "b200 groupby: bad device ordinal");
+    const int32_t no_off[1] = {0};
+    const b200::MrnfSpec spec{n_sort, sort_cols, sort_ascending, sort_na_last, keep};
+    return new GroupbyState(build_arr_c_types, build_arr_array_types, n_build_arrs, nullptr, no_off, nullptr, 0, n_keys,
+                            output_batch_size, parallel != 0, pandas_drop_na != 0, device, n_pes, myrank, expected_groups,
+                            (cudaStream_t)stream, &spec);
     B200_CATCH(nullptr)
 }
 

@@ -24,41 +24,13 @@ namespace b200 {
 constexpr int SORT_MAX_KEYS = 4;
 constexpr int SORT_MAX_COLS = 32;
 
-// The schema both forms sort by: one descriptor per key (the first n_keys columns) and every column's type.  A key's width in
-// bytes is held beside its c-type: the kernels' raw loads read it rather than derive it from the c-type, which keeps the inlined
-// encoder from being specialised once per load width (smaller, faster filter and pass code).
-struct SortKey { int ct, size, desc, na_last; };
+// The schema both forms sort by: one descriptor per key (the first n_keys columns, SortKey in common.cuh) and every column's
+// type.
 struct SortSchema {
     int n_keys, n_cols;
     SortKey key[SORT_MAX_KEYS];
     int ctype[SORT_MAX_COLS];
 };
-
-// Radix word of a key cell whose bits are `raw` (zero-extended).  `na` comes in true for a null cell and leaves true for a null
-// or NaN cell, whose word is 0.
-__device__ __forceinline__ uint64_t sort_word(const SortKey& k, uint64_t raw, bool& na) {
-    uint64_t w;
-    int bits;
-    if (k.ct == CT_FLOAT64) {
-        const double d = __longlong_as_double((long long)raw);
-        na = na || isnan(d);
-        w = (uint64_t)canon_float_ordered(canon_float_key(d)) ^ 0x8000000000000000ull;
-        bits = 64;
-    } else if (k.ct == CT_FLOAT32) {
-        const float f = __uint_as_float((uint32_t)raw);
-        na = na || isnan(f);
-        const uint32_t b = f == 0.0f ? 0u : (uint32_t)raw;
-        w = b ^ ((b >> 31) ? 0xFFFFFFFFu : 0x80000000u);
-        bits = 32;
-    } else {
-        bits = 8 * k.size;
-        w = ctype_is_signed_int(k.ct) ? raw ^ (1ull << (bits - 1)) : raw;
-    }
-    if (k.desc) w = ~w & (bits == 64 ? ~0ull : (1ull << bits) - 1);
-    return na ? 0 : w;
-}
-// NA-class bit of a key cell (`na`: null or NaN).
-__device__ __forceinline__ uint32_t sort_class(const SortKey& k, bool na) { return na ? k.na_last : !k.na_last; }
 
 // ---- top-k (ORDER BY ... LIMIT): candidate filter, bitonic sort + merge reduce ----
 //

@@ -10,6 +10,27 @@ Differences: the reference types the state at Numba compile time; here the build
 from the first consumed batch.  With parallel=True the state is one shard of a torch.distributed process
 group (one process per GPU): the last consume call runs the hash-partition exchange that replaces the
 reference's MPI shuffle (streaming/_shuffle.cpp:687-804).
+
+min_row_number_filter (MRNF): fnames == ("min_row_number_filter",) with the four mrnf_* arguments keeps one row per group,
+QUALIFY ROW_NUMBER() OVER (PARTITION BY keys ORDER BY sort columns) = 1, i.e.
+df.sort_values(sort columns, kind="stable").drop_duplicates(keys, keep="first")[kept columns]:
+  - keys: 1..4 columns (key_inds) with the groupby's key types and equality (float keys: -0.0 equals 0.0, NaN is the NA key);
+    dropna=True drops rows with an NA key, dropna=False puts all NA keys in one group.
+  - mrnf_sort_col_inds: 1..4 distinct columns (a key column too) of the sort's key types (fixed-width integer, float, bool,
+    DATE, DATETIME, TIMEDELTA; numpy or nullable); mrnf_sort_col_asc[j]: ascending; mrnf_sort_col_na[j]: True puts NA last.  A
+    float NaN is NA and -0.0 ties with 0.0, as in the sort.
+  - winner: the first row of the stable order by (sort columns, arrival), arrival being batch order, then row order: of rows
+    that tie on every sort column the earliest wins, even across batches.  The result is bit-identical across runs, batch
+    splits and table growth.
+  - mrnf_col_inds_keep: the output columns (logical indices, keys allowed, at most 26), in input order under their input
+    names, each holding the winner's own cell (bits and validity: a kept float key shows the winner's -0.0), with the input's
+    type and array kind.  One row per group; group order unspecified.
+  - f_in_offsets / f_in_cols list the function's input columns: f_in_offsets == (0, len(f_in_cols)), f_in_cols non-key
+    columns; the operator reads only the keys, the sort columns and the kept columns.
+  - every key, sort and kept column is fixed width (anything else raises, naming the column); a parallel state on a process
+    group of more than one rank raises at its first consume call (sharded MRNF is not supported), with one rank it runs locally.
+The state streams every batch into the groupby's hash table and keeps one winner record per group (DESIGN.md §3d), so it holds
+O(groups) device memory whatever the row count.
 """
 
 from __future__ import annotations
@@ -22,10 +43,57 @@ from ..table import CTable, Table, table_from_ctable
 
 # names must match supported_agg_funcs positions / Bodo_FTypes (groupby/_groupby_ftypes.h:17-110)
 FTYPES = {"size": 4, "sum": 6, "count": 7, "nunique": 8, "mean": 14, "min": 15, "max": 16, "first": 18, "last": 19, "var_pop": 22, "std_pop": 23, "var": 24, "std": 25, "skew": 27}
+MRNF = "min_row_number_filter"
+MRNF_MAX_SORT, MRNF_MAX_KEEP = 4, 26
+_FIXED_WIDTH = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 11, 13, 15, 16}  # CTypes with a fixed-width cell (integers, floats, bool, temporals)
+
+
+def _mrnf_spec(key_inds, fnames, f_in_offsets, f_in_cols, sort_inds, asc, na, keep):
+    """The validated MRNF arguments as (sort_inds, asc, na, keep), or None for an ordinary aggregation."""
+    args = {"mrnf_sort_col_inds": sort_inds, "mrnf_sort_col_asc": asc, "mrnf_sort_col_na": na, "mrnf_col_inds_keep": keep}
+    given = [k for k, v in args.items() if v is not None]
+    if MRNF not in fnames:
+        if given:
+            raise _lib.B200Error(f"Streaming Groupby: {', '.join(given)} belong to min_row_number_filter, which must then be the only "
+                                 f"function (fnames={tuple(fnames)})")
+        return None
+    if tuple(fnames) != (MRNF,):
+        raise _lib.B200Error(f"Streaming Groupby: min_row_number_filter cannot be combined with other functions (fnames={tuple(fnames)})")
+    missing = [k for k, v in args.items() if v is None]
+    if missing:
+        raise _lib.B200Error(f"Streaming Groupby: min_row_number_filter needs {', '.join(missing)}")
+
+    def indices(name, v, lo, hi):
+        v = tuple(v)
+        if not lo <= len(v) <= hi:
+            raise _lib.B200Error(f"Streaming Groupby: {name} must have {lo} to {hi} entries (got {len(v)})")
+        if any(isinstance(x, bool) or int(x) != x or x < 0 for x in v):
+            raise _lib.B200Error(f"Streaming Groupby: {name} must hold non-negative column indices (got {v})")
+        v = tuple(int(x) for x in v)
+        if len(set(v)) != len(v):
+            raise _lib.B200Error(f"Streaming Groupby: {name} lists a column twice (got {v})")
+        return v
+
+    sort = indices("mrnf_sort_col_inds", sort_inds, 1, MRNF_MAX_SORT)
+    flags = []
+    for name, v in (("mrnf_sort_col_asc", asc), ("mrnf_sort_col_na", na)):
+        v = tuple(v)
+        if len(v) != len(sort):
+            raise _lib.B200Error(f"Streaming Groupby: {name} must have one entry per sort column ({len(sort)}, got {len(v)})")
+        flags.append(tuple(bool(x) for x in v))
+    kept = indices("mrnf_col_inds_keep", keep, 1, MRNF_MAX_KEEP)
+    f_in_offsets, f_in_cols = tuple(f_in_offsets), tuple(f_in_cols)
+    if f_in_offsets != (0, len(f_in_cols)):
+        raise _lib.B200Error(f"Streaming Groupby: min_row_number_filter needs f_in_offsets == (0, len(f_in_cols)) (got {f_in_offsets})")
+    if any(int(c) in key_inds or c < 0 for c in f_in_cols):
+        raise _lib.B200Error(f"Streaming Groupby: min_row_number_filter's f_in_cols must be non-key columns (got {f_in_cols})")
+    return sort, flags[0], flags[1], kept
 
 
 class GroupbyState:
     """Python handle of the C GroupbyState (created lazily at the first consume call)."""
+
+    mrnf = None  # (sort_inds, asc, na_last, keep) of a min_row_number_filter state
 
     def __init__(self, operator_id, key_inds, fnames, f_in_offsets, f_in_cols, parallel, dropna, output_batch_size,
                  expected_groups, device, stream, process_group):
@@ -64,15 +132,18 @@ class GroupbyState:
         others = [i for i in range(n) if i not in self.key_inds]
         self.build_indices = list(self.key_inds) + others
         remap = {logical: phys for phys, logical in enumerate(self.build_indices)}
-        phys_f_in_cols = [remap[c] for c in self.f_in_cols]
         cols = [table.columns[i] for i in self.build_indices]
         c_types = ffi.new("int8_t[]", [c.c_type for c in cols])
         a_types = ffi.new("int8_t[]", [c.arr_type for c in cols])
+        if self.device is None:
+            self.device = table.device if table.device >= 0 else _current_device()
+        if self.mrnf is not None:
+            self._init_mrnf(table, remap, c_types, a_types)
+            return
+        phys_f_in_cols = [remap[c] for c in self.f_in_cols]
         ftypes = ffi.new("int32_t[]", [FTYPES[f] for f in self.fnames] or [0])
         offs = ffi.new("int32_t[]", list(self.f_in_offsets))
         fcols = ffi.new("int32_t[]", phys_f_in_cols or [0])
-        if self.device is None:
-            self.device = table.device if table.device >= 0 else _current_device()
         n_pes, rank = 1, 0
         if self.parallel:
             import torch.distributed as dist
@@ -100,6 +171,36 @@ class GroupbyState:
             seen.add(cand)
             uniq.append(cand)
         self.out_names = key_names + uniq
+
+    def _init_mrnf(self, table: Table, remap, c_types, a_types):
+        """Creates the C state of a min_row_number_filter once the schema is known (the sharded case was refused before)."""
+        L = _lib.lib()
+        sort, asc, na_last, keep = self.mrnf
+        n = table.n_cols
+        for name, inds in (("key_inds", self.key_inds), ("mrnf_sort_col_inds", sort), ("mrnf_col_inds_keep", keep),
+                           ("f_in_cols", self.f_in_cols)):
+            bad = [i for i in inds if i >= n]
+            if bad:
+                raise _lib.B200Error(f"Streaming Groupby: {name} {bad} out of range for a batch of {n} columns")
+        for what, inds in (("key", self.key_inds), ("sort", sort), ("kept", keep)):
+            for i in inds:
+                if table.columns[i].c_type not in _FIXED_WIDTH:
+                    raise _lib.B200Error(f"Streaming Groupby: min_row_number_filter {what} column '{table.names[i]}' is not a fixed-width "
+                                         f"column (c_type {table.columns[i].c_type})")
+        self.n_pes, self.rank = 1, 0
+        keep_mask = [0] * n
+        for i in keep:
+            keep_mask[remap[i]] = 1
+        h = L.b200_groupby_state_init_mrnf(self.operator_id, c_types, a_types, n, len(self.key_inds),
+                                           ffi.new("int32_t[]", [remap[i] for i in sort]), ffi.new("int32_t[]", [int(x) for x in asc]),
+                                           ffi.new("int32_t[]", [int(x) for x in na_last]), len(sort), ffi.new("int32_t[]", keep_mask),
+                                           self.output_batch_size, 0, int(self.dropna), self.device, 1, 0, self.expected_groups,
+                                           ffi.cast("void*", self.stream))
+        self.handle = _lib.check_ptr(h, "init_groupby_state (min_row_number_filter)")
+        # the library returns the kept columns in physical order (keys first); the output lists them in input order
+        phys = sorted(remap[i] for i in keep)
+        self._mrnf_order = [phys.index(remap[i]) for i in sorted(keep)]
+        self.out_names = [table.names[self.build_indices[p]] for p in phys]
 
     # ---- reduce-or-shuffle (reference: GroupbyIncrementalShuffleState::ShouldShuffleAfterProcessing,
     # bodo/libs/streaming/_groupby.cpp:1655-1711: an HLL estimate of how many NEW groups the pending rows hold decides whether they are
@@ -235,20 +336,27 @@ def init_groupby_state(operator_id, key_inds, fnames, f_in_offsets, f_in_cols, m
                        stream=0, process_group=None) -> GroupbyState:
     """Mirror of bodo.libs.streaming.groupby.init_groupby_state (groupby.py:702-715).
 
-    key_inds / f_in_cols index the logical input table; fnames are names from supported_agg_funcs.
-    The MRNF arguments must be None (min_row_number_filter is out of scope) and op_pool_size_bytes is
-    ignored (the table is sized in HBM, there is no host operator pool).
+    key_inds / f_in_cols index the logical input table; fnames are names from supported_agg_funcs, or
+    ("min_row_number_filter",) with the four mrnf_* arguments (see the module docstring; a bad length, index, duplicate, an empty
+    keep list, MRNF arguments beside other functions or min_row_number_filter without them raise B200Error naming the argument).
+    op_pool_size_bytes is ignored (the table is sized in HBM, there is no host operator pool).
     Keyword-only extras: dropna (pandas_drop_na of the C++ ctor), output_batch_size, expected_groups
     (sizing hint), device, stream (cudaStream_t as int), process_group (torch.distributed).
     """
-    if any(x is not None for x in (mrnf_sort_col_inds, mrnf_sort_col_asc, mrnf_sort_col_na, mrnf_col_inds_keep)):
-        raise _lib.B200Error("Streaming Groupby: min_row_number_filter is not supported by bodo_b200")
     key_inds = getattr(key_inds, "meta", key_inds)
-    fnames = getattr(fnames, "meta", fnames)
+    fnames = tuple(getattr(fnames, "meta", fnames))
     f_in_offsets = getattr(f_in_offsets, "meta", f_in_offsets)
     f_in_cols = getattr(f_in_cols, "meta", f_in_cols)
-    return GroupbyState(operator_id, key_inds, fnames, f_in_offsets, f_in_cols, parallel, dropna, output_batch_size,
-                        expected_groups, device, stream, process_group)
+    mrnf = [getattr(x, "meta", x) for x in (mrnf_sort_col_inds, mrnf_sort_col_asc, mrnf_sort_col_na, mrnf_col_inds_keep)]
+    spec = _mrnf_spec(tuple(int(k) for k in key_inds), fnames, f_in_offsets, f_in_cols, *mrnf)
+    if spec is None:
+        return GroupbyState(operator_id, key_inds, fnames, f_in_offsets, f_in_cols, parallel, dropna, output_batch_size,
+                            expected_groups, device, stream, process_group)
+    st = GroupbyState(operator_id, key_inds, (), (0,), (), parallel, dropna, output_batch_size, expected_groups, device, stream,
+                      process_group)
+    st.mrnf = spec
+    st.f_in_cols = tuple(int(c) for c in f_in_cols)
+    return st
 
 
 def groupby_build_consume_batch(groupby_state: GroupbyState, table: Table, is_last: bool, is_final_pipeline: bool = True):
@@ -258,6 +366,12 @@ def groupby_build_consume_batch(groupby_state: GroupbyState, table: Table, is_la
     ran out of input keep calling with empty batches, as in the reference's pipeline loop,
     bodo/pandas/_pipeline.cpp:453-457)."""
     st = groupby_state
+    if st.mrnf is not None and st.parallel and st.handle is None:
+        import torch.distributed as dist
+
+        if dist.is_initialized() and dist.get_world_size(st.process_group) > 1:
+            raise _lib.B200Error("Streaming Groupby: a sharded min_row_number_filter is not supported (process group of more than one "
+                                 "rank)")
     st._ensure(table)
     L = _lib.lib()
     phys = table.select(st.build_indices)
@@ -282,7 +396,7 @@ def groupby_produce_output_batch(groupby_state: GroupbyState, produce_output: bo
     if st.handle is None:
         raise _lib.B200Error("groupby_produce_output_batch called before any build batch was consumed")
     L = _lib.lib()
-    ncols = len(st.key_inds) + len(st.fnames)
+    ncols = len(st.out_names)
     st._out_cols = ffi.new("b200_column[]", ncols)
     st._out_tab = ffi.new("b200_table*")
     st._out_tab.cols = st._out_cols
@@ -290,6 +404,8 @@ def groupby_produce_output_batch(groupby_state: GroupbyState, produce_output: bo
     _lib.check(L.b200_groupby_produce_output_batch(st.handle, st._out_tab, last, int(bool(produce_output))),
                "groupby_produce_output_batch")
     out = table_from_ctable(st._out_tab, ncols, st.out_names, owner=st)
+    if st.mrnf is not None:
+        out = out.select(st._mrnf_order)
     return out, bool(last[0])
 
 

@@ -58,7 +58,7 @@ int b200_device_count(void);
  * distinct / drop_duplicates, reference: physical/aggregate.h:198-227); ftypes are Bodo_FTypes (groupby/_groupby_ftypes.h:17-110: size=4 sum=6 count=7 mean=14
  * min=15 max=16); f_in_offsets/f_in_cols is the CSR map function -> physical input column
  * (streaming/_groupby.h:1059-1070). Arguments of the reference that only concern window functions,
- * MRNF, sort keys and the host operator pool are dropped. `pandas_drop_na`: drop rows with NA keys
+ * MRNF, sort keys and the host operator pool are dropped (MRNF has its own entry, b200_groupby_state_init_mrnf). `pandas_drop_na`: drop rows with NA keys
  * (filter_na_keys, _groupby.cpp:4278-4309). `parallel`: state is one shard of n_pes; ownership
  * is hash_to_rank(key) (bodo/libs/_shuffle.h:5-7). `expected_groups` is a sizing hint (0 = unknown).
  * `stream` is a cudaStream_t all work is enqueued on (NULL = legacy default stream). */
@@ -69,6 +69,31 @@ void* b200_groupby_state_init(int64_t operator_id, const int8_t* build_arr_c_typ
                               int64_t output_batch_size, int32_t parallel, int32_t pandas_drop_na,
                               int32_t device, int32_t n_pes, int32_t myrank,
                               int64_t expected_groups, void* stream);
+
+/* groupby_state_init_py_entry (_groupby.cpp:4917-4970) with its MRNF arguments (sort_asc / sort_na / n_sort_keys / cols_to_keep):
+ * a min_row_number_filter state, QUALIFY ROW_NUMBER() OVER (PARTITION BY keys ORDER BY sort columns) = 1, i.e.
+ * df.sort_values(sort columns, kind="stable").drop_duplicates(keys, keep="first")[kept columns].
+ *   Keys: the first n_keys (1..4) columns, of the key types and with the key equality of b200_groupby_state_init (float keys:
+ *     -0.0 equals 0.0 and NaN is the NA key).  pandas_drop_na drops rows with an NA key; otherwise all NA keys form one group.
+ *   Sort columns: sort_cols[0 .. n_sort) (1 <= n_sort <= 4, distinct, any column including a key): fixed-width integer, float,
+ *     bool, DATE, DATETIME or TIMEDELTA, numpy or nullable.  sort_ascending[j] and sort_na_last[j] (NA last = 1, first = 0) per
+ *     column.  A float NaN is NA and -0.0 ties with 0.0: the rules of b200_sort_state_init.
+ *   Winner: per group the first row of the stable order by (sort columns, arrival), arrival being batch order, then row order, so
+ *     a row that ties on every sort column with an earlier row (of this batch or an earlier one) never wins.  The result is
+ *     bit-identical across runs, batch splits and table growth.
+ *   Output: one row per group (group order unspecified): the columns c with keep[c] != 0 (keep: one flag per column, at least
+ *     one and at most 26 set), in column order, each with the winning row's own cell (bits and validity; a kept float key shows
+ *     the winner's -0.0), type and array kind, so `out->cols` of a produce call holds one descriptor per kept column.
+ *   Columns that are neither keys, sort columns nor kept are never read.  Every key, sort and kept column is fixed width;
+ *   anything else fails here, naming the column.  A state with parallel set and n_pes > 1 fails at its first consume call
+ *   (sharded MRNF is not supported); with n_pes == 1 it runs locally.
+ * Build-consume, finalize, produce, delete and the metrics are the entries of the ordinary state (metric 0: groups); the exchange
+ * entries refuse an MRNF state. */
+void* b200_groupby_state_init_mrnf(int64_t operator_id, const int8_t* build_arr_c_types, const int8_t* build_arr_array_types,
+                                   int32_t n_build_arrs, uint64_t n_keys, const int32_t* sort_cols, const int32_t* sort_ascending,
+                                   const int32_t* sort_na_last, int32_t n_sort, const int32_t* keep, int64_t output_batch_size,
+                                   int32_t parallel, int32_t pandas_drop_na, int32_t device, int32_t n_pes, int32_t myrank,
+                                   int64_t expected_groups, void* stream);
 
 /* groupby_build_consume_batch_py_entry (_groupby.cpp:4663-4676). Returns 1 when the build is globally
  * finished (is_last was passed), 0 otherwise, <0 on error. *request_input is always set to 1 (the GPU
