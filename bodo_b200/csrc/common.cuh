@@ -175,6 +175,7 @@ __device__ __forceinline__ double load_as_f64(const void* __restrict__ p, int ct
     switch (ct) {
         case CT_FLOAT64: return ((const double*)p)[i];
         case CT_FLOAT32: return (double)((const float*)p)[i];
+        case CT_UINT64: return (double)((const uint64_t*)p)[i];  // (its int64 pattern would read 2^63 and above as negative)
         default: return (double)load_int_as_i64(p, ct, i);
     }
 }
