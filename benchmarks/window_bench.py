@@ -15,6 +15,8 @@ doubles in [0, 1)) and an int64 row id r, fed in `--batch`-row batches.  Cases:
   moving_wide    SUM(r) and MIN(o) ROWS BETWEEN 65535 PRECEDING AND CURRENT ROW OVER (ORDER BY o): one partition, a deep tree
   moments        STDDEV(o) ROWS BETWEEN 19 PRECEDING AND CURRENT ROW (a Bollinger band's width), VAR(o) ROWS (running) and
                  STDDEV_POP(o) over the partition, OVER (PARTITION BY p ORDER BY o)
+  bivariate      CORR(o, r) ROWS BETWEEN 19 PRECEDING AND CURRENT ROW (a rolling correlation), COVAR_SAMP(o, r) ROWS (running)
+                 and REGR_SLOPE(o, r) over the partition (a beta), OVER (PARTITION BY p ORDER BY o)
   range_moving   AVG(o) and MAX(o) RANGE BETWEEN 2^35 ns PRECEDING AND CURRENT ROW, SUM(r) and COUNT(*) RANGE BETWEEN 2^34 ns
                  PRECEDING AND 2^34 ns FOLLOWING, OVER (PARTITION BY p ORDER BY t): about 8 rows per frame, as in moving
   range_wide     SUM(r) and MIN(o) RANGE BETWEEN 2^28 ns PRECEDING AND CURRENT ROW OVER (ORDER BY t): one partition, about 65 536
@@ -22,8 +24,9 @@ doubles in [0, 1)) and an int64 row id r, fed in `--batch`-row batches.  Cases:
 The range cases add a fourth column t, an int64 DATETIME key uniform in [0, 2^40) ns, and order by it; the other cases keep
 their three columns.  `--profile` runs one more step per case under torch.profiler (separately from the timed steps) and
 reports the window kernels' device times; with it, nothing is timed (run it separately from the timed run).
-The value cases (running to moments, and the range cases) also alternate with rn_rank_dense (rn_rank_dense_ms), so their cost above the ranking kernels
-is measured too; their result check covers the validity of the nullable columns.
+The value cases (running to bivariate, and the range cases) also alternate with rn_rank_dense (rn_rank_dense_ms), so their cost above the ranking kernels
+is measured too; their result check covers the validity of the nullable columns.  bivariate also alternates with moments
+(moments_ms): its scan value is twice the moments' and it reads a second column.
 One step = init -> consume every batch (is_last on the last) -> produce -> delete, timed with CUDA events on the operator's stream;
 the median of `--reps` steps after one warm-up.  Every window step alternates with a full sort of the same keys and columns in
 the same process (sort_ms), so the window's cost above the sort is a measured difference (extra_ms).
@@ -56,6 +59,8 @@ MOVING = [("ma", "mean", "o", ("rows", -6, 0)), ("sc", "sum", "r", ("rows", -3, 
 MOVING_WIDE = [("sw", "sum", "r", ("rows", -65535, 0)), ("nw", "min", "o", ("rows", -65535, 0))]
 MOMENTS = [("sd20", "std", "o", ("rows", -19, 0)), ("vr", "var", "o", "rows"), ("spp", "std_pop", "o", "partition")]
 MOMENT_NAMES = ("var", "std", "var_pop", "std_pop")
+BIVARIATE = [("rho20", "corr", "o", "r", ("rows", -19, 0)), ("cv", "covar_samp", "o", "r", "rows"), ("beta", "regr_slope", "o", "r", "partition")]
+BIVARIATE_NAMES = ("covar_samp", "covar_pop", "corr", "regr_slope", "regr_intercept")
 def _ns(k):
     import numpy as np
 
@@ -67,7 +72,19 @@ RANGE_MOVING = [("ra", "mean", "o", ("range_between", -_ns(1 << 35), 0)), ("rx",
                 ("rc", "count", None, ("range_between", -_ns(1 << 34), _ns(1 << 34)))]
 RANGE_WIDE = [("ws", "sum", "r", ("range_between", -_ns(1 << 28), 0)), ("wn", "min", "o", ("range_between", -_ns(1 << 28), 0))]
 RANGE_CASES = ("range_moving", "range_wide")
-VALUE_CASES = ("running", "partition_aggs", "lag_lead", "moving", "moving_wide", "moments") + RANGE_CASES
+VALUE_CASES = ("running", "partition_aggs", "lag_lead", "moving", "moving_wide", "moments", "bivariate") + RANGE_CASES
+
+
+def frame_of(f):
+    """A value entry's frame: (out, fname, column[, frame]), (out, fname, y, x[, frame]) for the bivariate functions; lag and
+    lead have none (their cost is counted as the "range" frame's)."""
+    k = 4 if f[1] in BIVARIATE_NAMES else 3
+    return f[k] if len(f) > k and f[1] not in ("lag", "lead") else "range"
+
+
+def n_cols(f):
+    """The 8-byte value columns a function reads: two for the bivariate functions."""
+    return 2 if f[1] in BIVARIATE_NAMES else 1
 
 
 def window_bytes(n, key_bytes, n_funcs, n_parts, n_peers):
@@ -80,7 +97,8 @@ def window_bytes(n, key_bytes, n_funcs, n_parts, n_peers):
 
 def value_bytes(n, funcs, n_parts, n_peers):
     """The value kernels after bounds / tiles / ends (every value column here is 8 bytes wide, numpy).  A scan function (sum,
-    count of a column, mean, min, max, var, std, var_pop, std_pop) reads its column and the flags twice (reduce, then rescan) and writes its 8-byte cell, plus
+    count of a column, mean, min, max, var, std, var_pop, std_pop, and the bivariate functions, which read two columns) reads its
+    columns and the flags twice (reduce, then rescan) and writes its 8-byte cell, plus
     a validity byte when nullable, at each frame end (min / max also read the chosen cell there); the eval pass reads the flags
     and the partition / peer-group words once, and per function writes 8 bytes (+1 validity) per row, reading the frame end's
     cell for a scan function whose frame ends elsewhere and the source cell for first / last / lag / lead."""
@@ -89,12 +107,12 @@ def value_bytes(n, funcs, n_parts, n_peers):
     for f in funcs:
         fname, col = f[1], f[2]
         vb = 0 if fname == "count" else 1
-        frame = f[3] if len(f) > 3 and fname not in ("lag", "lead") else "range"
+        frame = frame_of(f)
         if fname in ("lag", "lead", "first_value", "last_value") or col is None:
             evals = True
             total += n * (8 + vb) + (n * 8 if col is not None else 0)
             continue
-        total += 2 * n * 9 + ends[frame] * (8 + vb) + (ends[frame] * 8 if fname in ("min", "max") else 0)
+        total += 2 * n * (1 + 8 * n_cols(f)) + ends[frame] * (8 + vb) + (ends[frame] * 8 if fname in ("min", "max") else 0)
         if frame != "rows":
             evals = True
             total += n * (8 + vb) + ends[frame] * (8 + vb)
@@ -113,13 +131,14 @@ def range_bytes(n, funcs, n_parts, n_peers):
 
 def in_frame_path(f):
     """Functions over a ("rows", start, end) frame and nth_value run in the frame kernels, not in the scans."""
-    return f[1] == "nth_value" or (len(f) > 3 and isinstance(f[3], tuple))
+    return f[1] == "nth_value" or isinstance(frame_of(f), tuple)
 
 
 def frame_bytes(n, funcs, n_parts, n_peers):
     """The frame kernels (8-byte numpy value columns, as value_bytes).  An aggregate over a bounded frame: the tree build reads
     its column once and writes 4 bytes per row of nodes (16-byte nodes of the levels >= 3; 6 bytes per row of 24-byte nodes for
-    var / std / var_pop / std_pop); the query pass reads the flags and
+    var / std / var_pop / std_pop, 12 bytes per row of 48-byte nodes for the bivariate functions, which read both columns at each
+    step); the query pass reads the flags and
     the partition / peer-group words, the column once more (edge leaves; the nodes and the leaves that neighbouring frames share
     are counted once) and writes 8 + 1 bytes per row.  The gather pass (count(*), first_value, last_value, nth_value) reads the
     flags and words once per launch, and per function and row the source cell and its 8 + 1 output bytes (count(*): 8).  Every
@@ -134,7 +153,8 @@ def frame_bytes(n, funcs, n_parts, n_peers):
             gather_launches.add(fr)
             total += n * (8 if f[2] is None else 8 + 8 + 1)
         else:
-            total += n * (8 + (6 if f[1] in MOMENT_NAMES else 4)) + words + n * (8 + 8 + 1)
+            nodes = 12 if f[1] in BIVARIATE_NAMES else 6 if f[1] in MOMENT_NAMES else 4
+            total += n * (8 * n_cols(f) + nodes) + words + n * (8 * n_cols(f) + 8 + 1)
     return int(total + len(gather_launches) * words)
 
 
@@ -171,7 +191,7 @@ def main():
     torch.cuda.synchronize(dev)
     cases = {"rn_rank_dense": (["p"], FUNCS3), "all6": (["p"], FUNCS6), "no_partition": ([], FUNCS3), "running": (["p"], RUNNING),
              "partition_aggs": (["p"], PARTITION_AGGS), "lag_lead": (["p"], LAG_LEAD), "moving": (["p"], MOVING),
-             "moving_wide": ([], MOVING_WIDE), "moments": (["p"], MOMENTS), "range_moving": (["p"], RANGE_MOVING),
+             "moving_wide": ([], MOVING_WIDE), "moments": (["p"], MOMENTS), "bivariate": (["p"], BIVARIATE), "range_moving": (["p"], RANGE_MOVING),
              "range_wide": ([], RANGE_WIDE)}
     names, order = ["p", "o", "r"], "o"
 
@@ -376,7 +396,91 @@ def main():
                 t = torch.minimum(torch.sqrt(tv), tv / exp.clamp(min=1e-300)) + 2 * u * exp
             return bool(((got - exp).abs() <= t)[valid].all())
 
+        def frame_sums(f, x, y):
+            """Per row over f's frame (the partition, the running prefix or a trailing frame): (count, Sxx, Syy, Sxy, the means of
+            x and y), two-pass in torch float64, and h, the merge height of §3c's bound."""
+            fr = frame_of(f)
+            z = lambda: torch.zeros(n_p, dtype=torch.float64, device=dev)  # noqa: E731
+            if fr == "partition":
+                cnt = s.to(torch.float64)
+                mx, my = z().index_add_(0, pid, x)[pid] / cnt, z().index_add_(0, pid, y)[pid] / cnt
+                dx, dy = x - mx, y - my
+                sums = [z().index_add_(0, pid, a * b)[pid] for a, b in ((dx, dx), (dy, dy), (dx, dy))]
+                return cnt, *sums, mx, my, cnt - 1
+            if fr == "rows":  # a (partition, position) matrix; per prefix length k + 1, the rows at position k
+                pos = i - P
+                L = int(s.max())
+                X, Y = torch.zeros(n_p, L, dtype=torch.float64, device=dev), torch.zeros(n_p, L, dtype=torch.float64, device=dev)
+                X[pid, pos], Y[pid, pos] = x, y
+                ar = torch.arange(1, L + 1, device=dev, dtype=torch.float64)
+                mxs, mys = torch.cumsum(X, 1) / ar, torch.cumsum(Y, 1) / ar
+                by_pos = torch.argsort(pos)
+                ends_k = torch.cumsum(torch.bincount(pos, minlength=L), 0).tolist()
+                sums = [torch.empty(n, dtype=torch.float64, device=dev) for _ in range(3)]
+                for k in range(L):
+                    rows = by_pos[(ends_k[k - 1] if k else 0):ends_k[k]]
+                    pr = pid[rows]
+                    dx, dy = X[pr, :k + 1] - mxs[pr, k:k + 1], Y[pr, :k + 1] - mys[pr, k:k + 1]
+                    for out_, a, b in zip(sums, (dx, dy, dx), (dx, dy, dy)):
+                        out_[rows] = (a * b).sum(1)
+                cnt = (pos + 1).to(torch.float64)
+                mx, my = mxs[pid, pos], mys[pid, pos]
+                del X, Y, mxs, mys, by_pos, pos
+                return cnt, *sums, mx, my, cnt - 1
+            w = -fr[1] + 1
+            cnt = (i - torch.maximum(P, i - w + 1) + 1).to(torch.float64)
+            sx, sy = torch.zeros(n, dtype=torch.float64, device=dev), torch.zeros(n, dtype=torch.float64, device=dev)
+            for k in range(w):
+                inside = i - k >= P
+                sx += torch.where(inside, torch.roll(x, k), 0.0)
+                sy += torch.where(inside, torch.roll(y, k), 0.0)
+            mx, my = sx / cnt, sy / cnt
+            del sx, sy
+            sums = [torch.zeros(n, dtype=torch.float64, device=dev) for _ in range(3)]
+            for k in range(w):
+                inside = i - k >= P
+                dx, dy = torch.where(inside, torch.roll(x, k) - mx, 0.0), torch.where(inside, torch.roll(y, k) - my, 0.0)
+                for out_, a, b in zip(sums, (dx, dy, dx), (dx, dy, dy)):
+                    out_ += a * b
+            return cnt, *sums, mx, my, torch.minimum(cnt - 1, 10 + 3 * torch.floor(torch.log2(cnt)))
+
+        def bivariate_ok(j, f):
+            """covar_samp / corr / regr_slope(y, x) against torch float64 two-pass co-moments (as moment_ok): each of Sxx, Syy
+            and Sxy within DESIGN §3c's bound for the device plus 8 m u times the same terms for the recomputation's own rounding,
+            then corr and slope within what those bounds give them (first order, doubled); validity exactly."""
+            got, valid = res[3 + j], res[3 + nf + j]
+            u = 2.0 ** -53
+            y, x = (so if c == "o" else sr.to(torch.float64) for c in (f[2], f[3]))
+            cnt, sxx, syy, sxy, mx, my, h = frame_sums(f, x, y)
+            gam = lambda k: k * u / (1 - k * u)  # noqa: E731
+            sq = lambda v: torch.sqrt(v.clamp(min=0))  # noqa: E731
+
+            def tol(a, b, ma, mb):  # |S_ab - S_ab*| (§3c), with a = b giving S_aa's
+                t = sq(a * b) + ma.abs() * sq(cnt * b) + mb.abs() * sq(cnt * a)
+                return torch.sqrt(h) * (gam(21 * h) * sq(a * b) + gam(8 * h) * (t - sq(a * b))) + 8 * cnt * u * t
+
+            exy, exx, eyy = tol(sxx, syy, mx, my), tol(sxx, sxx, mx, mx), tol(syy, syy, my, my)
+            if f[1] == "covar_samp":
+                want, div = cnt >= 2, (cnt - 1).clamp(min=1)
+                exp, t = sxy / div, exy / div + 2 * u * (sxy / div).abs()
+            elif f[1] == "corr":
+                want = (cnt >= 2) & (sxx > 0) & (syy > 0)
+                d = sq(sxx * syy).clamp(min=1e-300)
+                exp = (sxy / d).clamp(-1, 1)
+                t = 2 * (exy / d + exp.abs() * 0.5 * (exx / sxx.clamp(min=1e-300) + eyy / syy.clamp(min=1e-300))) + 4 * u
+            else:
+                want = sxx > 0
+                sl = sxy / sxx.clamp(min=1e-300)
+                exp, t = sl, 2 * (exy + sl.abs() * exx) / (sxx - exx).clamp(min=1e-300) + 2 * u * sl.abs()
+            if not torch.equal(valid, want):
+                return False
+            return bool(((got - exp).abs() <= t)[valid].all())
+
         for j, f in enumerate(funcs):
+            if f[1] in BIVARIATE_NAMES:
+                if not bivariate_ok(j, f):
+                    return f"MISMATCH: {f[0]}", 0, 0
+                continue
             if f[1] in MOMENT_NAMES:
                 if not moment_ok(j, f):
                     return f"MISMATCH: {f[0]}", 0, 0
@@ -488,7 +592,9 @@ def main():
         value_case = name in VALUE_CASES
         if value_case:
             window_step(part, FUNCS3)
-        wt, st_, rt = [], [], []
+        if name == "bivariate":
+            window_step(part, MOMENTS)
+        wt, st_, rt, mt = [], [], [], []
         for _ in range(args.reps):
             ms, (_, m9) = timed(lambda: window_step(part, funcs))
             wt.append(ms)
@@ -496,6 +602,8 @@ def main():
             st_.append(ms)
             if value_case:  # the value kernels' cost next to the ranking kernels', in the same process
                 rt.append(timed(lambda: window_step(part, FUNCS3))[0])
+            if name == "bivariate":  # next to the moments, whose scan value is half as wide
+                mt.append(timed(lambda: window_step(part, MOMENTS))[0])
         w_ms, s_ms = sorted(wt)[len(wt) // 2], sorted(st_)[len(st_) // 2]
         free()
         # check
@@ -530,6 +638,9 @@ def main():
         if value_case:
             r_ms = sorted(rt)[len(rt) // 2]
             out.update(rn_rank_dense_ms=round(r_ms, 3), rn_rank_dense_runs_ms=[round(x, 3) for x in rt], extra_over_rn_rank_dense_ms=round(w_ms - r_ms, 3))
+        if mt:
+            m_ms = sorted(mt)[len(mt) // 2]
+            out.update(moments_ms=round(m_ms, 3), moments_runs_ms=[round(x, 3) for x in mt], extra_over_moments_ms=round(w_ms - m_ms, 3))
         print(json.dumps(out), flush=True)
         print(f"result_check: {chk}", flush=True)
         ok_all &= chk == "ok"

@@ -15,6 +15,7 @@
 // na_position="last", 0 for "first"; other keys the opposite class.  Rows compare lexicographically over (class_0, word_0,
 // class_1, word_1, ..., arrival index), so no two rows are equal.
 #include <algorithm>
+#include <cfloat>
 #include <vector>
 
 #include "common.cuh"
@@ -1125,8 +1126,15 @@ struct WvAgg { uint64_t x; uint32_t c, f; };
 enum { WN_VAR = 16, WN_STD = 17, WN_VAR_POP = 18, WN_STD_POP = 19 };
 enum { WV_MOM = 5 };
 struct WvMom { uint32_t c, f; double mean, m2; };
+// COVAR_SAMP / COVAR_POP / CORR / REGR_SLOPE / REGR_INTERCEPT (codes 20..24, y = the function's column, x = its second column)
+// scan kind WV_CO: c the count of rows where both cells are valid and non-NaN, f as WvAgg's, mx / my their means and sxx / syy /
+// sxy = sum (x - mx)^2, sum (y - my)^2, sum (x - mx)(y - my), combined by the bivariate form of Chan's merge (wv_combine<WV_CO>).
+enum { WN_COVAR_SAMP = 20, WN_COVAR_POP = 21, WN_CORR = 22, WN_REGR_SLOPE = 23, WN_REGR_INTERCEPT = 24 };
+enum { WV_CO = 6 };
+struct WvCo { uint32_t c, f; double mx, my, sxx, syy, sxy; };
 template <int K> struct WvKind { using T = WvAgg; };
 template <> struct WvKind<WV_MOM> { using T = WvMom; };
+template <> struct WvKind<WV_CO> { using T = WvCo; };
 template <int K> using wv_t = typename WvKind<K>::T;
 
 // The carry and tree buffers hold kind K's scan values.
@@ -1148,6 +1156,15 @@ struct WvFunc {
     uint8_t* out_vb;
 };
 
+// A bivariate function's second column (x): the sorted cells and validity bytes (nullptr: numpy), c-type and cell bytes.  The
+// scan, tree and frame kernels take it as a last parameter of their own (read by WV_CO only), so the argument structs and every
+// other kernel parameter keep their offsets.
+struct WvCol {
+    const char* data;
+    const uint8_t* vb;
+    int ct, size;
+};
+
 struct WvArgs {
     int64_t n;
     const uint8_t* flags;
@@ -1162,6 +1179,8 @@ template <int K>
 __device__ __forceinline__ wv_t<K> wv_identity() { return WvAgg{K == WV_FSUM ? WV_NEG_ZERO : 0ull, (K == WV_MIN || K == WV_MAX) ? WV_NONE : 0u, 0u}; }
 template <>
 __device__ __forceinline__ WvMom wv_identity<WV_MOM>() { return WvMom{0u, 0u, 0.0, 0.0}; }
+template <>
+__device__ __forceinline__ WvCo wv_identity<WV_CO>() { return WvCo{0u, 0u, 0.0, 0.0, 0.0, 0.0, 0.0}; }
 
 template <int K>
 __device__ __forceinline__ wv_t<K> wv_combine(wv_t<K> a, wv_t<K> b) {
@@ -1187,6 +1206,19 @@ __device__ __forceinline__ WvMom wv_combine<WV_MOM>(WvMom a, WvMom b) {
     const double w = (double)b.c / (double)n, d = b.mean - a.mean;
     return WvMom{n, a.f, a.mean + d * w, a.m2 + b.m2 + d * (d * ((double)a.c * w))};
 }
+// The bivariate merge: the means as WV_MOM's, and with t = n_a n_b / n, sxx += (dx dx) t, syy += (dy dy) t, sxy += (dx dy) t.
+// The three terms are formed alike, so swapping x and y swaps sxx and syy and leaves sxy's bits (dx dy = dy dx), and x = y gives
+// sxx, syy and sxy the same bits; a frame of equal x has dx = 0 at every merge, so sxx = 0 exactly.
+template <>
+__device__ __forceinline__ WvCo wv_combine<WV_CO>(WvCo a, WvCo b) {
+    if (b.f) return b;
+    if (b.c == 0) return a;
+    if (a.c == 0) { b.f = a.f; return b; }
+    const uint32_t n = a.c + b.c;
+    const double w = (double)b.c / (double)n, dx = b.mx - a.mx, dy = b.my - a.my, t = (double)a.c * w;
+    return WvCo{n, a.f, a.mx + dx * w, a.my + dy * w, a.sxx + b.sxx + (dx * dx) * t, a.syy + b.syy + (dy * dy) * t,
+                a.sxy + b.sxy + (dx * dy) * t};
+}
 
 __device__ __forceinline__ WvAgg wv_shfl_up(WvAgg v, int o) {
     return WvAgg{__shfl_up_sync(0xffffffffu, (unsigned long long)v.x, o), __shfl_up_sync(0xffffffffu, v.c, o), __shfl_up_sync(0xffffffffu, v.f, o)};
@@ -1195,10 +1227,25 @@ __device__ __forceinline__ WvMom wv_shfl_up(WvMom v, int o) {
     return WvMom{__shfl_up_sync(0xffffffffu, v.c, o), __shfl_up_sync(0xffffffffu, v.f, o), __shfl_up_sync(0xffffffffu, v.mean, o),
                  __shfl_up_sync(0xffffffffu, v.m2, o)};
 }
+__device__ __forceinline__ WvCo wv_shfl_up(WvCo v, int o) {
+    return WvCo{__shfl_up_sync(0xffffffffu, v.c, o), __shfl_up_sync(0xffffffffu, v.f, o), __shfl_up_sync(0xffffffffu, v.mx, o),
+                __shfl_up_sync(0xffffffffu, v.my, o), __shfl_up_sync(0xffffffffu, v.sxx, o), __shfl_up_sync(0xffffffffu, v.syy, o),
+                __shfl_up_sync(0xffffffffu, v.sxy, o)};
+}
 
-// Scan value of position i of the scanned function; `part`: i starts a partition.
+// Cell i of a column of c-type ct and `size` bytes as a double (integers and bool exactly up to 2^53), as wv_value<WV_MOM>
+// converts its cells (which keeps its own copy, so the moments' kernels compile as before).
+__device__ __forceinline__ double wv_double(const char* data, int ct, int size, int64_t i) {
+    const uint64_t raw = load_bits(data, size, i);
+    return ct == CT_FLOAT64 ? __longlong_as_double((long long)raw)
+         : ct == CT_FLOAT32 ? (double)__uint_as_float((uint32_t)raw)
+         : ctype_is_signed_int(ct) ? (double)((int64_t)(raw << (64 - 8 * size)) >> (64 - 8 * size))
+                                   : (double)raw;
+}
+
+// Scan value of position i of the scanned function (x: its second column, read by WV_CO only); `part`: i starts a partition.
 template <int K>
-__device__ __forceinline__ wv_t<K> wv_value(const WvFunc& s, int64_t i, bool part) {
+__device__ __forceinline__ wv_t<K> wv_value(const WvFunc& s, const WvCol& x, int64_t i, bool part) {
     WvAgg r = wv_identity<K>();
     r.f = part;
     bool na = s.vb && s.vb[i] == 0;
@@ -1221,7 +1268,7 @@ __device__ __forceinline__ wv_t<K> wv_value(const WvFunc& s, int64_t i, bool par
 }
 // (1, x, 0) for a valid, non-NaN cell x converted to double (integers and bool exactly up to 2^53); the identity otherwise.
 template <>
-__device__ __forceinline__ WvMom wv_value<WV_MOM>(const WvFunc& s, int64_t i, bool part) {
+__device__ __forceinline__ WvMom wv_value<WV_MOM>(const WvFunc& s, const WvCol&, int64_t i, bool part) {
     WvMom r = wv_identity<WV_MOM>();
     r.f = part;
     const uint64_t raw = load_bits(s.data, s.size, i);
@@ -1230,6 +1277,15 @@ __device__ __forceinline__ WvMom wv_value<WV_MOM>(const WvFunc& s, int64_t i, bo
                    : ctype_is_signed_int(s.ct) ? (double)((int64_t)(raw << (64 - 8 * s.size)) >> (64 - 8 * s.size))
                                                : (double)raw;
     if (!(s.vb && s.vb[i] == 0) && !isnan(x)) { r.c = 1; r.mean = x; }
+    return r;
+}
+// (1, x, y, 0, 0, 0) when both cells are valid and non-NaN (pairwise deletion); the identity otherwise.
+template <>
+__device__ __forceinline__ WvCo wv_value<WV_CO>(const WvFunc& s, const WvCol& x, int64_t i, bool part) {
+    WvCo r = wv_identity<WV_CO>();
+    r.f = part;
+    const double yv = wv_double(s.data, s.ct, s.size, i), xv = wv_double(x.data, x.ct, x.size, i);
+    if (!(s.vb && s.vb[i] == 0) && !(x.vb && x.vb[i] == 0) && !isnan(xv) && !isnan(yv)) { r.c = 1; r.mx = xv; r.my = yv; }
     return r;
 }
 
@@ -1309,16 +1365,43 @@ __device__ __forceinline__ void wv_write<WV_MOM>(const WvFunc& s, int64_t i, WvM
     ((double*)s.out)[i] = ok ? r : 0.0;
     s.out_vb[i] = ok;
 }
+// covar_samp = sxy / (m - 1) (NA when m < 2), covar_pop = sxy / m (NA when m = 0), corr = sxy / sqrt(sxx syy) (NA when m < 2,
+// sxx = 0 or syy = 0; sxy / (sqrt(sxx) sqrt(syy)) when sxx syy overflows or is subnormal; clamped to [-1, 1]), regr_slope =
+// sxy / sxx and regr_intercept = my - slope mx (NA when sxx = 0, which covers m <= 1); FLOAT64.  A frame whose counted pairs hold
+// +-inf has a non-finite mean and gives a valid NaN.
+template <>
+__device__ __forceinline__ void wv_write<WV_CO>(const WvFunc& s, int64_t i, WvCo v) {
+    const double m = (double)v.c;
+    bool ok;
+    double r;
+    if (s.code == WN_COVAR_SAMP || s.code == WN_COVAR_POP) {
+        const bool pop = s.code == WN_COVAR_POP;
+        ok = v.c > (pop ? 0u : 1u);
+        r = v.sxy / (m - (pop ? 0.0 : 1.0));
+    } else if (s.code == WN_CORR) {
+        ok = v.c > 1u && v.sxx != 0.0 && v.syy != 0.0;
+        const double p = v.sxx * v.syy;
+        r = v.sxy / (p >= DBL_MIN && p <= DBL_MAX ? sqrt(p) : sqrt(v.sxx) * sqrt(v.syy));
+        r = r > 1.0 ? 1.0 : r < -1.0 ? -1.0 : r;  // NaN passes
+    } else {
+        ok = v.sxx != 0.0;
+        const double slope = v.sxy / v.sxx;
+        r = s.code == WN_REGR_SLOPE ? slope : v.my - slope * v.mx;
+    }
+    if (!(isfinite(v.mx) && isfinite(v.my))) r = __longlong_as_double(0x7FF8000000000000ll);
+    ((double*)s.out)[i] = ok ? r : 0.0;
+    s.out_vb[i] = ok;
+}
 
 template <int K, bool FINAL>
-__global__ void __launch_bounds__(WN_THREADS) window_vscan_kernel(const __grid_constant__ WvArgs a) {
+__global__ void __launch_bounds__(WN_THREADS) window_vscan_kernel(const __grid_constant__ WvArgs a, const __grid_constant__ WvCol x) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t t = blockIdx.x;
     wv_t<K> v[WN_ITEMS];
 #pragma unroll
     for (int k = 0; k < WN_ITEMS; k++) {
         const int64_t i = wn_row(t, k, warp, lane);
-        v[k] = i < a.n ? wv_value<K>(a.s, i, a.flags[i] & WN_PART) : wv_identity<K>();
+        v[k] = i < a.n ? wv_value<K>(a.s, x, i, a.flags[i] & WN_PART) : wv_identity<K>();
     }
     wv_scan_tile<K>(FINAL ? wv_buf<K>(a.carry)[t] : wv_identity<K>(), v);
     if (!FINAL) {  // padding rows hold the identity, so the tile's last slot holds its reduction
@@ -1405,10 +1488,10 @@ __global__ void __launch_bounds__(WN_THREADS) window_veval_kernel(const __grid_c
 }
 
 template <int K>
-void launch_wv_scan(const WvArgs& a, int64_t n_tiles, cudaStream_t st) {
-    window_vscan_kernel<K, false><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
+void launch_wv_scan(const WvArgs& a, const WvCol& x, int64_t n_tiles, cudaStream_t st) {
+    window_vscan_kernel<K, false><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a, x);
     window_vtiles_kernel<K><<<1, 1024, 0, st>>>(a, n_tiles);
-    window_vscan_kernel<K, true><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
+    window_vscan_kernel<K, true><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a, x);
 }
 
 // ---- bounded ROWS frames (k PRECEDING / k FOLLOWING) and NTH_VALUE ----
@@ -1430,7 +1513,7 @@ void launch_wv_scan(const WvArgs& a, int64_t n_tiles, cudaStream_t st) {
 enum { WN_NTH_VALUE = 15 };
 enum { WF_BOUNDED = 4, WF_RANGE_BETWEEN = 5 };  // frame 5: bounds per row from window_range_bounds_kernel (below)
 constexpr int64_t WF_UNBOUNDED_START = INT64_MIN, WF_UNBOUNDED_END = INT64_MAX;
-constexpr int WV_GATHER = 4;            // window_frame_kernel's gather pass (the scan kinds are 0..3 and WV_MOM)
+constexpr int WV_GATHER = 4;            // window_frame_kernel's gather pass (the scan kinds are 0..3, WV_MOM and WV_CO)
 constexpr int WT_LOW = 3, WT_LEVELS = 32;  // levels below WT_LOW are not stored; level l < WT_LEVELS
 
 // A function of this path: the value function, its frame bounds (WF_BOUNDED: row offsets or the unbounded sentinels above;
@@ -1482,30 +1565,39 @@ __device__ __forceinline__ void wt_levels3(const WfArgs& a, int base, int64_t j0
         }
     }
 }
-// The same with constant trip counts: the loop above leaves the moments' larger combine partly rolled, and x in local memory.
-template <>
-__device__ __forceinline__ void wt_levels3<WV_MOM>(const WfArgs& a, int base, int64_t j0, WvMom (&x)[WN_ITEMS]) {
+// The same with constant trip counts: the loop above leaves the moments' and co-moments' larger combines partly rolled, and x in
+// local memory.
+template <int K>
+__device__ __forceinline__ void wt_levels3_unrolled(const WfArgs& a, int base, int64_t j0, wv_t<K> (&x)[WN_ITEMS]) {
 #pragma unroll
     for (int h = 1; h <= 3; h++) {
 #pragma unroll
         for (int k = 0; k < WN_ITEMS / 2; k++) {
             if (k < (WN_ITEMS >> h)) {
-                x[k] = wv_combine<WV_MOM>(x[2 * k], x[2 * k + 1]);
-                wt_store<WV_MOM>(a, base + h, (j0 >> h) + k, x[k]);
+                x[k] = wv_combine<K>(x[2 * k], x[2 * k + 1]);
+                wt_store<K>(a, base + h, (j0 >> h) + k, x[k]);
             }
         }
     }
 }
+template <>
+__device__ __forceinline__ void wt_levels3<WV_MOM>(const WfArgs& a, int base, int64_t j0, WvMom (&x)[WN_ITEMS]) {
+    wt_levels3_unrolled<WV_MOM>(a, base, j0, x);
+}
+template <>
+__device__ __forceinline__ void wt_levels3<WV_CO>(const WfArgs& a, int base, int64_t j0, WvCo (&x)[WN_ITEMS]) {
+    wt_levels3_unrolled<WV_CO>(a, base, j0, x);
+}
 
 template <int K>
-__global__ void __launch_bounds__(WN_THREADS) window_tree_kernel(const __grid_constant__ WfArgs a, int base) {
+__global__ void __launch_bounds__(WN_THREADS) window_tree_kernel(const __grid_constant__ WfArgs a, int base, const __grid_constant__ WvCol x2) {
     __shared__ wv_t<K> s_node[WN_THREADS];
     const int64_t n_in = a.n >> base, j0 = (int64_t)blockIdx.x * WN_TILE + threadIdx.x * WN_ITEMS;
     wv_t<K> x[WN_ITEMS];
 #pragma unroll
     for (int k = 0; k < WN_ITEMS; k++) {
         const int64_t j = j0 + k;
-        x[k] = j >= n_in ? wv_identity<K>() : base == 0 ? wv_value<K>(a.s.g, j, false) : wv_buf<K>(a.tree)[a.off[base] + j];
+        x[k] = j >= n_in ? wv_identity<K>() : base == 0 ? wv_value<K>(a.s.g, x2, j, false) : wv_buf<K>(a.tree)[a.off[base] + j];
     }
     wt_levels3<K>(a, base, j0, x);  // levels base + 1 .. base + 3 in registers
     s_node[threadIdx.x] = x[0];
@@ -1524,30 +1616,30 @@ __global__ void __launch_bounds__(WN_THREADS) window_tree_kernel(const __grid_co
 
 // The aggregate of the scanned function over [lo, hi]: edge leaves from the sorted column, aligned blocks from the tree.
 template <int K>
-__device__ __forceinline__ wv_t<K> wt_query(const WfArgs& a, int64_t lo, int64_t hi) {
+__device__ __forceinline__ wv_t<K> wt_query(const WfArgs& a, const WvCol& x, int64_t lo, int64_t hi) {
     wv_t<K> acc = wv_identity<K>();
     const int64_t r = hi + 1, a8 = min(r, (lo + 7) & ~(int64_t)7);
     int64_t j = lo;
-    for (; j < a8; j++) acc = wv_combine<K>(acc, wv_value<K>(a.s.g, j, false));
+    for (; j < a8; j++) acc = wv_combine<K>(acc, wv_value<K>(a.s.g, x, j, false));
     const int64_t b8 = max(j, r & ~(int64_t)7);
     while (j < b8) {  // j and b8 are multiples of 8, so l >= 3
         const int l = min(j == 0 ? 62 : __ffsll(j) - 1, 63 - __clzll(b8 - j));
         acc = wv_combine<K>(acc, wv_buf<K>(a.tree)[a.off[l] + (j >> l)]);
         j += (int64_t)1 << l;
     }
-    for (; j < r; j++) acc = wv_combine<K>(acc, wv_value<K>(a.s.g, j, false));
+    for (; j < r; j++) acc = wv_combine<K>(acc, wv_value<K>(a.s.g, x, j, false));
     return acc;
 }
 
 // Row i's frame functions: the aggregate a.s over its [lo, hi] from the tree (K a scan kind), or every gather function (K =
 // WV_GATHER); bounds(g, lo, hi) gives function g's frame.
 template <int K, typename Bounds>
-__device__ __forceinline__ void wf_eval_row(const WfArgs& a, int64_t i, Bounds bounds) {
+__device__ __forceinline__ void wf_eval_row(const WfArgs& a, const WvCol& x, int64_t i, Bounds bounds) {
     constexpr int KQ = K == WV_GATHER ? WV_ISUM : K;  // the scan kind of the aggregate pass
     int64_t lo, hi;
     if (K != WV_GATHER) {
         bounds(a.s, lo, hi);
-        wv_write<KQ>(a.s.g, i, wt_query<KQ>(a, lo, hi));
+        wv_write<KQ>(a.s.g, i, wt_query<KQ>(a, x, lo, hi));
     } else for (int fn = 0; fn < a.n_funcs; fn++) {
         const WfFunc& g = a.f[fn];
         bounds(g, lo, hi);
@@ -1561,7 +1653,7 @@ __device__ __forceinline__ void wf_eval_row(const WfArgs& a, int64_t i, Bounds b
 }
 
 template <int K>
-__global__ void __launch_bounds__(WN_THREADS) window_frame_kernel(const __grid_constant__ WfArgs a) {
+__global__ void __launch_bounds__(WN_THREADS) window_frame_kernel(const __grid_constant__ WfArgs a, const __grid_constant__ WvCol x) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t t = blockIdx.x;
     WnArgs w;  // wn_scan_tile reads n, flags and the tile prefixes only
@@ -1578,17 +1670,18 @@ __global__ void __launch_bounds__(WN_THREADS) window_frame_kernel(const __grid_c
         if (i >= a.n) break;
         const WnAgg vk = s_v[k][threadIdx.x];
         const int64_t P = vk.p, pe = P + a.psize[vk.p], qe = a.pend[vk.q];
-        wf_eval_row<K>(a, i, [&](const WfFunc& g, int64_t& lo, int64_t& hi) { wf_bounds(g, i, P, pe, qe, lo, hi); });
+        wf_eval_row<K>(a, x, i, [&](const WfFunc& g, int64_t& lo, int64_t& hi) { wf_bounds(g, i, P, pe, qe, lo, hi); });
     }
 }
 
 // The same over frame-5 functions, whose bounds window_range_bounds_kernel wrote: no scan of the flags is needed, so one thread
-// per row.  48 registers: at the default budget the compiler holds the double sum in 32 and spills.
+// per row.  48 registers: at the default budget the compiler holds the double sum in 32 and spills.  The co-moments' 48-byte
+// accumulator and leaf spill at 48, so WV_CO takes up to 80 (it uses 68).
 template <int K>
-__global__ void __maxnreg__(48) window_range_frame_kernel(const __grid_constant__ WfArgs a) {
+__global__ void __maxnreg__(K == WV_CO ? 80 : 48) window_range_frame_kernel(const __grid_constant__ WfArgs a, const __grid_constant__ WvCol x) {
     const int64_t i = (int64_t)blockIdx.x * WN_THREADS + threadIdx.x;
     if (i >= a.n) return;
-    wf_eval_row<K>(a, i, [i](const WfFunc& g, int64_t& lo, int64_t& hi) {
+    wf_eval_row<K>(a, x, i, [i](const WfFunc& g, int64_t& lo, int64_t& hi) {
         const int2 b = __ldg(g.range + i);
         lo = b.x;
         hi = b.y;
@@ -1597,11 +1690,11 @@ __global__ void __maxnreg__(48) window_range_frame_kernel(const __grid_constant_
 
 // Build the tree of the aggregate a.s (levels WT_LOW.. up to log2 n), then evaluate it at every row.
 template <int K>
-void launch_wf_tree(const WfArgs& a, int64_t n_tiles, cudaStream_t st) {
+void launch_wf_tree(const WfArgs& a, const WvCol& x, int64_t n_tiles, cudaStream_t st) {
     for (int base = 0; (a.n >> max(base + 1, WT_LOW)) > 0; base += 11)
-        window_tree_kernel<K><<<(unsigned)(((a.n >> base) + WN_TILE - 1) / WN_TILE), WN_THREADS, 0, st>>>(a, base);
-    if (a.s.g.frame == WF_RANGE_BETWEEN) window_range_frame_kernel<K><<<(unsigned)(n_tiles * WN_ITEMS), WN_THREADS, 0, st>>>(a);
-    else window_frame_kernel<K><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
+        window_tree_kernel<K><<<(unsigned)(((a.n >> base) + WN_TILE - 1) / WN_TILE), WN_THREADS, 0, st>>>(a, base, x);
+    if (a.s.g.frame == WF_RANGE_BETWEEN) window_range_frame_kernel<K><<<(unsigned)(n_tiles * WN_ITEMS), WN_THREADS, 0, st>>>(a, x);
+    else window_frame_kernel<K><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a, x);
 }
 
 // ---- RANGE frames with value offsets (RANGE BETWEEN x PRECEDING AND y FOLLOWING): frame 5 ----
@@ -1770,7 +1863,7 @@ struct WindowState : FullSortState {
             b200_window_func& d = fn[f] = funcs[f];
             bound[f] = b200_window_frame{WF_UNBOUNDED_START, WF_UNBOUNDED_END};
             range[f] = b200_window_range{WR_UNBOUNDED_PRECEDING, WR_UNBOUNDED_FOLLOWING, 0, 0};
-            B200_REQUIRE(d.code >= WN_ROW_NUMBER && d.code <= WN_STD_POP, "b200 window: unknown function code");
+            B200_REQUIRE(d.code >= WN_ROW_NUMBER && d.code <= WN_REGR_INTERCEPT, "b200 window: unknown function code");
             int ct = CT_INT64, at = ARR_NUMPY;
             if (d.code <= WN_NTILE) {
                 B200_REQUIRE(d.col == -1 && d.frame == WF_NONE, "b200 window: a ranking function takes no column and no frame");
@@ -1804,10 +1897,17 @@ struct WindowState : FullSortState {
                     else if (b.start == WF_UNBOUNDED_START && b.end == WF_UNBOUNDED_END) d.frame = WF_PARTITION;
                 }
                 const int vct = d.col >= 0 ? sc.ctype[d.col] : CT_INT64;
-                const bool temporal = vct == CT_DATE || vct == CT_DATETIME || vct == CT_TIMEDELTA;
+                const auto is_temporal = [](int t) { return t == CT_DATE || t == CT_DATETIME || t == CT_TIMEDELTA; };
+                const bool temporal = is_temporal(vct);
                 if (d.code == WN_SUM || d.code == WN_MEAN)
                     B200_REQUIRE(!temporal, "b200 window: sum and mean need an integer, bool or float column");
-                if (d.code >= WN_VAR) B200_REQUIRE(!temporal, "b200 window: var and std need an integer, bool or float column");
+                if (d.code >= WN_VAR && d.code <= WN_STD_POP)
+                    B200_REQUIRE(!temporal, "b200 window: var and std need an integer, bool or float column");
+                if (d.code >= WN_COVAR_SAMP) {  // arg: the second column (x); frame 0 failed above
+                    B200_REQUIRE(d.arg >= 0 && d.arg < n_arrs, "b200 window: covar / corr / regr second column index (arg) out of range");
+                    B200_REQUIRE(!temporal && !is_temporal(sc.ctype[d.arg]),
+                                 "b200 window: covar, corr and regr need integer, bool or float columns");
+                }
                 if (d.code == WN_SUM) ct = ctype_is_float(vct) ? vct : ctype_is_signed_int(vct) || vct == CT_BOOL ? CT_INT64 : CT_UINT64;
                 else if (d.code == WN_MEAN || d.code >= WN_VAR) ct = CT_FLOAT64;
                 else if (d.code != WN_COUNT) ct = vct;
@@ -1919,46 +2019,55 @@ struct WindowState : FullSortState {
         window_ends_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
         if (a.n_funcs > 0) window_eval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
         B200_CUDA(cudaGetLastError());
+        const auto moments = [](int code) { return code >= WN_VAR && code <= WN_STD_POP; };
+        const auto bivariate = [](int code) { return code >= WN_COVAR_SAMP; };
+        const auto value_bytes = [&](int code) { return bivariate(code) ? sizeof(WvCo) : moments(code) ? sizeof(WvMom) : sizeof(WvAgg); };
+        const auto col2 = [&](const WvFunc& g) {  // a bivariate function's second column: its index is in arg (g.k)
+            const int j = (int)g.k;
+            return WvCol{out_data[j], out_vb[j], sc.ctype[j], ctype_size(sc.ctype[j])};
+        };
         DevBuf carry;  // sized for the largest scan value among the scans
-        const auto moments = [](int code) { return code >= WN_VAR; };
-        const bool mom_scan = std::any_of(scans.begin(), scans.end(), [&](const WvFunc& g) { return moments(g.code); });
-        if (!scans.empty()) carry.alloc((size_t)n_tiles * (mom_scan ? sizeof(WvMom) : sizeof(WvAgg)));
+        size_t carry_bytes = 0;
+        for (const WvFunc& g : scans) carry_bytes = std::max(carry_bytes, value_bytes(g.code));
+        if (!scans.empty()) carry.alloc((size_t)n_tiles * carry_bytes);
         va.n = n; va.flags = a.flags; va.psize = a.psize; va.pend = a.pend; va.carry = carry.p;
         for (const WvFunc& g : scans) {
             va.s = g;
-            if (moments(g.code)) launch_wv_scan<WV_MOM>(va, n_tiles, stream);
-            else if (g.code == WN_MIN) launch_wv_scan<WV_MIN>(va, n_tiles, stream);
-            else if (g.code == WN_MAX) launch_wv_scan<WV_MAX>(va, n_tiles, stream);
-            else if (g.code != WN_COUNT && ctype_is_float(g.ct)) launch_wv_scan<WV_FSUM>(va, n_tiles, stream);
-            else launch_wv_scan<WV_ISUM>(va, n_tiles, stream);
+            const WvCol x = bivariate(g.code) ? col2(g) : WvCol{};
+            if (bivariate(g.code)) launch_wv_scan<WV_CO>(va, x, n_tiles, stream);
+            else if (moments(g.code)) launch_wv_scan<WV_MOM>(va, x, n_tiles, stream);
+            else if (g.code == WN_MIN) launch_wv_scan<WV_MIN>(va, x, n_tiles, stream);
+            else if (g.code == WN_MAX) launch_wv_scan<WV_MAX>(va, x, n_tiles, stream);
+            else if (g.code != WN_COUNT && ctype_is_float(g.ct)) launch_wv_scan<WV_FSUM>(va, x, n_tiles, stream);
+            else launch_wv_scan<WV_ISUM>(va, x, n_tiles, stream);
         }
         if (eval) window_veval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a, va);
         B200_CUDA(cudaGetLastError());
         // one tree buffer, reused by every aggregate over a bounded frame: n / 8 + n / 16 + ... nodes of the largest scan value
-        // among them, <= 4 B per row (<= 6 B per row with a moment)
+        // among them, <= 4 B per row (<= 6 B per row with a moment, <= 12 B per row with a bivariate function)
         DevBuf tree, rb;
         if (!trees.empty() || fa.n_funcs > 0 || !ranged.empty()) {
             fa.n = n; fa.flags = a.flags; fa.tile = a.tile; fa.psize = a.psize; fa.pend = a.pend;
             int64_t nodes = 0;
             for (int l = WT_LOW; l < WT_LEVELS; l++) { fa.off[l] = nodes; nodes += n >> l; }
-            bool mom_tree = std::any_of(trees.begin(), trees.end(), [&](const WfFunc& h) { return moments(h.g.code); });
-            bool any_tree = !trees.empty();
-            for (const RangeFrame& rf : ranged) {
-                any_tree = any_tree || !rf.trees.empty();
-                mom_tree = mom_tree || std::any_of(rf.trees.begin(), rf.trees.end(), [&](const WfFunc& h) { return moments(h.g.code); });
-            }
-            if (any_tree) tree.alloc((size_t)std::max<int64_t>(nodes, 1) * (mom_tree ? sizeof(WvMom) : sizeof(WvAgg)));
+            size_t tree_bytes = 0;  // 0: no tree
+            for (const WfFunc& h : trees) tree_bytes = std::max(tree_bytes, value_bytes(h.g.code));
+            for (const RangeFrame& rf : ranged)
+                for (const WfFunc& h : rf.trees) tree_bytes = std::max(tree_bytes, value_bytes(h.g.code));
+            if (tree_bytes > 0) tree.alloc((size_t)std::max<int64_t>(nodes, 1) * tree_bytes);
             fa.tree = tree.p;
             const auto launch_tree = [&](const WfFunc& h) {
                 fa.s = h;
-                if (moments(h.g.code)) launch_wf_tree<WV_MOM>(fa, n_tiles, stream);
-                else if (h.g.code == WN_MIN) launch_wf_tree<WV_MIN>(fa, n_tiles, stream);
-                else if (h.g.code == WN_MAX) launch_wf_tree<WV_MAX>(fa, n_tiles, stream);
-                else if (h.g.code != WN_COUNT && ctype_is_float(h.g.ct)) launch_wf_tree<WV_FSUM>(fa, n_tiles, stream);
-                else launch_wf_tree<WV_ISUM>(fa, n_tiles, stream);
+                const WvCol x = bivariate(h.g.code) ? col2(h.g) : WvCol{};
+                if (bivariate(h.g.code)) launch_wf_tree<WV_CO>(fa, x, n_tiles, stream);
+                else if (moments(h.g.code)) launch_wf_tree<WV_MOM>(fa, x, n_tiles, stream);
+                else if (h.g.code == WN_MIN) launch_wf_tree<WV_MIN>(fa, x, n_tiles, stream);
+                else if (h.g.code == WN_MAX) launch_wf_tree<WV_MAX>(fa, x, n_tiles, stream);
+                else if (h.g.code != WN_COUNT && ctype_is_float(h.g.ct)) launch_wf_tree<WV_FSUM>(fa, x, n_tiles, stream);
+                else launch_wf_tree<WV_ISUM>(fa, x, n_tiles, stream);
             };
             for (const WfFunc& h : trees) launch_tree(h);
-            if (fa.n_funcs > 0) window_frame_kernel<WV_GATHER><<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(fa);
+            if (fa.n_funcs > 0) window_frame_kernel<WV_GATHER><<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(fa, WvCol{});
             B200_CUDA(cudaGetLastError());
             // frame 5: one 8 B/row bounds buffer, reused frame by frame (its bounds, then its trees, then its gathers)
             if (!ranged.empty()) rb.alloc((size_t)n * sizeof(int2));
@@ -1970,7 +2079,7 @@ struct WindowState : FullSortState {
                 for (WfFunc& h : rf.trees) { h.range = ra.out; launch_tree(h); }
                 fa.n_funcs = 0;
                 for (WfFunc& h : rf.gathers) { h.range = ra.out; fa.f[fa.n_funcs++] = h; }
-                if (fa.n_funcs > 0) window_range_frame_kernel<WV_GATHER><<<(unsigned)(n_tiles * WN_ITEMS), WN_THREADS, 0, stream>>>(fa);
+                if (fa.n_funcs > 0) window_range_frame_kernel<WV_GATHER><<<(unsigned)(n_tiles * WN_ITEMS), WN_THREADS, 0, stream>>>(fa, WvCol{});
                 B200_CUDA(cudaGetLastError());
             }
         }
@@ -2070,6 +2179,19 @@ void* b200_window_state_init_ranges(int64_t operator_id, const int8_t* c_types, 
                                     const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
                                     const b200_window_range* ranges, int32_t n_funcs, int64_t output_batch_size, int32_t device,
                                     void* stream) {
+    try {  // this entry's domain: codes 0..19 (the bivariate entry adds covar_samp, covar_pop, corr, regr_slope and regr_intercept)
+        for (int f = 0; funcs && f < n_funcs && f < b200::SORT_MAX_COLS; f++)
+            B200_REQUIRE(funcs[f].code >= b200::WN_ROW_NUMBER && funcs[f].code <= b200::WN_STD_POP, "b200 window: unknown function code");
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
+    return b200_window_state_init_bivariate(operator_id, c_types, arr_types, n_arrs, n_partition_keys, n_order_keys, order_ascending,
+                                            order_na_last, funcs, frames, ranges, n_funcs, output_batch_size, device, stream);
+}
+
+void* b200_window_state_init_bivariate(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                                       int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                                       const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
+                                       const b200_window_range* ranges, int32_t n_funcs, int64_t output_batch_size, int32_t device,
+                                       void* stream) {
     (void)operator_id;
     return b200::sort_state_new(device, [&]() -> SortState* {
         const int np = n_partition_keys, no = n_order_keys;

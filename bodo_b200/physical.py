@@ -326,8 +326,9 @@ class PhysicalWindow:
     MOMENT_FUNCS (var, std, var_pop, std_pop) and frame one of "range" (default), "rows", "partition", ("rows", start, end) (ROWS BETWEEN start AND end, None for UNBOUNDED,
     negative offsets PRECEDING, positive FOLLOWING) or ("range_between", start, end) (RANGE BETWEEN start AND end, the same
     spelling with offsets measured in the single ORDER BY key, e.g. -pd.Timedelta("1h")), (out_name, "lag" | "lead", column[, k[,
-    default]]) or (out_name,
-    "nth_value", column, n[, frame]);
+    default]]), (out_name,
+    "nth_value", column, n[, frame]) or (out_name, fname, y, x[, frame]), fname one of streaming.window.BIVARIATE_FUNCS
+    (covar_samp, covar_pop, corr, regr_slope, regr_intercept, over any frame sum takes);
     ascending / na_position: one value or one per ORDER BY key.  The column names are taken from the first batch."""
 
     def __init__(self, partition_by, order_by, funcs, ascending=True, na_position="last", parallel: bool = False, **kw):
@@ -476,7 +477,8 @@ def sort_values(df, by, ascending=True, na_position="last", batch_size: int = ST
 def window(df, partition_by, order_by, funcs, ascending=True, na_position="last", batch_size: int = STREAMING_BATCH_SIZE, **kw):
     """Ranking, aggregate and navigation window functions OVER (PARTITION BY partition_by ORDER BY order_by) through
     PhysicalWindow (funcs as PhysicalWindow takes them, e.g. [("run", "sum", "x", "rows"), ("prev", "lag", "x", 1, 0),
-    ("ma7", "mean", "x", ("rows", -6, 0)), ("sd20", "std", "x", ("rows", -19, 0))]).  Returns a pandas
+    ("ma7", "mean", "x", ("rows", -6, 0)), ("sd20", "std", "x", ("rows", -19, 0)), ("beta", "regr_slope", "y", "x", ("rows", -59,
+    0))]).  Returns a pandas
     DataFrame in the operator's output order (stably sorted by partition keys, then order keys) with a fresh index: df's columns,
     then one column per function."""
     op = PhysicalWindow(partition_by, order_by, funcs, ascending, na_position, **kw)

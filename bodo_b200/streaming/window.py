@@ -6,11 +6,13 @@
     NTH_VALUE (x, n) OVER (PARTITION BY p ORDER BY o [frame]), and every frame function over ROWS BETWEEN k PRECEDING AND k FOLLOWING
     VAR_SAMP / STDDEV_SAMP / VAR_POP / STDDEV_POP (x) OVER (PARTITION BY p ORDER BY o [frame])
     every frame function over RANGE BETWEEN x PRECEDING AND y FOLLOWING, an offset measured in the ORDER BY value
+    COVAR_SAMP / COVAR_POP / CORR / REGR_SLOPE / REGR_INTERCEPT (y, x) OVER (PARTITION BY p ORDER BY o [frame])
 
 pandas equivalents: groupby(p).cumcount() + 1, groupby(p)[o].rank(method="min" / "dense" / "max", pct=...),
 groupby(p)[x].cumsum() / cummin() / cummax() (the "rows" frame), groupby(p)[x].transform("sum" / "mean" / "min" / "max" /
 "count" / "size" / "first" / "last" / "var" / "std") (the "partition" frame), groupby(p)[x].expanding().var() / .std() (the
-"rows" frame), groupby(p)[x].rolling(w).var() / .std() (a bounded frame), groupby(p).rolling("1h", on=t) (a RANGE frame) and groupby(p)[x].shift(k, fill_value=default) (lag;
+"rows" frame), groupby(p)[x].rolling(w).var() / .std() (a bounded frame), groupby(p).rolling("1h", on=t) (a RANGE frame),
+groupby(p)[y].rolling(w).cov(x) / .corr(x) (a bounded frame) and groupby(p)[x].shift(k, fill_value=default) (lag;
 lead is shift(-k)).  The state is a third form of the streaming sort (streaming/sort.py's SortState, sort.cu's WindowState): batches are
 appended to the full sort's device chunk store, is_last sorts every row by (partition keys ascending NA last, order keys, arrival
 index), scans the sorted key columns on the device for partition and peer-group boundaries and then scans or gathers the value
@@ -28,7 +30,8 @@ Semantics:
     s // n + 1 rows, the others s // n; buckets 1..s when n > s).
   - row_number, rank, dense_rank and ntile are int64 columns, percent_rank and cume_dist float64 (one IEEE double division of two
     integers, so bit-identical to numpy's).
-  - value functions read one input column (any column, keys included).  Frames start at the row's partition's first row P and
+  - value functions read one input column (any column, keys included); covar_samp, covar_pop, corr, regr_slope and
+    regr_intercept read two, (y, x), which may be the same column.  Frames start at the row's partition's first row P and
     end at e: "range" (the default; SQL's default frame RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW) at the row's last peer,
     which is the partition's last row without ORDER BY; "rows" (ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW) at the row
     itself, ties in arrival order; "partition" (ROWS BETWEEN UNBOUNDED PRECEDING AND UNBOUNDED FOLLOWING) at the partition's last
@@ -37,7 +40,7 @@ Semantics:
     [P, pe) the frame is [lo, hi] with lo = P (start None) or max(P, i + start), hi = pe - 1 (end None) or min(pe - 1, i + end),
     empty when lo > hi.  ("rows", None, 0) is "rows" and ("rows", None, None) is "partition".  It takes sum, count, mean, min,
     max, first_value, last_value, nth_value, var, std, var_pop and std_pop, which are then defined as below with [lo, hi] in
-    place of [P, e]; an empty frame gives NA (count 0).  ("range_between", start, end) is RANGE BETWEEN start AND end with the
+    place of [P, e], as are the five functions of two columns below; an empty frame gives NA (count 0).  ("range_between", start, end) is RANGE BETWEEN start AND end with the
     same spelling: None is UNBOUNDED, zero CURRENT ROW (the row's peer group: from its first peer / to its last peer; any ORDER
     BY), a negative offset PRECEDING and a positive one FOLLOWING, measured in the single ORDER BY key x.  With x ascending a
     k PRECEDING start is the first row of the partition's non-NA run with x_j >= x_i - k and a k FOLLOWING end the last row
@@ -67,6 +70,16 @@ Semantics:
         mean, M2) by Chan's pairwise merge, with no sum of squares, so it keeps its digits when |mean| >> the spread (DESIGN
         §3c gives the bound); it is never negative and is exactly 0.0 over equal values.  A frame holding +-inf gives a valid
         NaN, as pandas does.  float64, nullable; a temporal column raises.
+      covar_samp(y, x) / covar_pop(y, x) / corr(y, x) / regr_slope(y, x) / regr_intercept(y, x), written (out_name, fname,
+        y, x[, frame]) in SQL's argument order: over the m rows where both cells are non-NA (pairwise deletion, as SQL and
+        pandas; integers and bool converted to double, exact up to 2^53), with means mx, my and Sxx = sum (x - mx)^2, Syy =
+        sum (y - my)^2, Sxy = sum (x - mx)(y - my): covar_samp = Sxy / (m - 1), NA when m < 2; covar_pop = Sxy / m, NA when
+        m = 0; corr = Sxy / sqrt(Sxx Syy), clamped to [-1, 1], NA when m < 2, Sxx = 0 or Syy = 0 (SQL NULL where pandas gives
+        NaN); regr_slope = Sxy / Sxx and regr_intercept = my - regr_slope mx, NA when Sxx = 0.  (count, mx, my, Sxx, Syy, Sxy)
+        is combined by the bivariate form of Chan's merge, with no sum of products (DESIGN §3c gives the bound): covar and
+        corr are bit-for-bit symmetric in (y, x), corr(x, x) is exactly 1.0 where Sxx > 0, and equal x values give Sxx = 0
+        exactly.  A frame whose counted pairs hold +-inf gives a valid NaN.  float64, nullable; a temporal column in either
+        position raises.
       lag(x, k=1, default=None) / lead(...): the cell at i - k / i + k if that row is in the row's partition, else default (NA
         when None); 0 <= k < 2^31, k = 0 is the row itself; no frame; x's type, nullable.  default is converted to x's numpy
         dtype and must round-trip exactly.
@@ -75,8 +88,8 @@ Semantics:
     the scan's order, not sequentially.  Over ("rows", start, end) the results are pandas' groupby(p)[x].rolling(w,
     min_periods=1) ones (count: min_periods=0), with float sums combined in an order that depends only on the frame's bounds.
     Results depend only on the sorted positions: every row that shares a frame end (a bounded frame: both bounds) gets a
-    bit-identical result, and float sums and the moments are bit-identical across runs and across any split of the rows into
-    batches.
+    bit-identical result, and float sums, the moments and the co-moments are bit-identical across runs and across any split of
+    the rows into batches.
   - output: every input row once, in the stable sort's order by (partition keys, order keys, arrival); every input column in
     input order, then one column per function under the caller's name.  SQL leaves the order open; fixing it makes every column
     comparable bit for bit.
@@ -111,7 +124,10 @@ MOMENT_FUNCS = {"var": 16, "std": 17, "var_pop": 18, "std_pop": 19}
 RANGE_BETWEEN = 5
 RANGE_KINDS = {"unbounded_preceding": 0, "preceding": 1, "current_row": 2, "following": 3, "unbounded_following": 4}
 BOUNDED_FUNCS = ("sum", "count", "mean", "min", "max", "first_value", "last_value", "nth_value", "var", "std", "var_pop", "std_pop")
-_VALUE_NAMES = {c: f for f, c in {**VALUE_FUNCS, **FRAME_FUNCS, **MOMENT_FUNCS}.items()}
+# The bivariate entry's codes (b200_window_state_init_bivariate): functions of two columns (y, x), x's index in arg.  They take
+# every frame BOUNDED_FUNCS take.
+BIVARIATE_FUNCS = {"covar_samp": 20, "covar_pop": 21, "corr": 22, "regr_slope": 23, "regr_intercept": 24}
+_VALUE_NAMES = {c: f for f, c in {**VALUE_FUNCS, **FRAME_FUNCS, **MOMENT_FUNCS, **BIVARIATE_FUNCS}.items()}
 _FRAME_NAMES = {c: f for f, c in FRAMES.items()}
 MAX_COLS = 32
 MAX_WINDOW_ROWS = MAX_FULL_SORT_ROWS
@@ -126,7 +142,7 @@ _CT_NAMES = {v: k for k, v in vars(CTypes).items() if k.isupper() and isinstance
 _FORMS = (f"ranking: (out_name, fname) with fname in {sorted(FUNCS)}, or (out_name, 'ntile', n); value: (out_name, fname, column"
           f"[, frame]) with fname in {sorted(set(VALUE_FUNCS) - {'lag', 'lead'} | set(MOMENT_FUNCS))}, frame in {sorted(FRAMES)}, ('rows', start, end) or ('range_between', start, end), "
           "column None for count(*) only, or (out_name, 'lag' | 'lead', column[, k[, default]]), or (out_name, 'nth_value', column, "
-          "n[, frame])")
+          f"n[, frame]), or (out_name, fname, column1, column2[, frame]) with fname in {sorted(BIVARIATE_FUNCS)}")
 
 
 def _names(x):
@@ -151,6 +167,13 @@ def _parse_value(f, col_names):
         if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or not 0 <= k <= MAX_LAG:
             raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} needs an integer k with 0 <= k < 2^31")
         return (name, VALUE_FUNCS[fname], int(k), column, 0, f[4] if len(f) > 4 else None)
+    if fname in BIVARIATE_FUNCS:
+        if len(f) < 4 or not (isinstance(f[3], str) and f[3] in col_names):
+            raise _lib.B200Error(f"Streaming Window: {f!r}: unknown second column {f[3] if len(f) > 3 else None!r} (one of {col_names}), as "
+                                 f"(out_name, {fname!r}, column1, column2[, frame])")
+        if len(f) > 5:
+            raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} takes (out_name, {fname!r}, column1, column2[, frame])")
+        return (name, BIVARIATE_FUNCS[fname], f[3], column, *_parse_frame(f, f[4] if len(f) > 4 else "range"))
     if fname == "nth_value":
         nth = f[3] if len(f) > 3 else None
         if len(f) > 5 or isinstance(nth, (bool, np.bool_)) or not isinstance(nth, (int, np.integer)) or not 1 <= nth <= MAX_LAG:
@@ -182,7 +205,7 @@ def _parse_frame(f, frame):
                                  "(-2^31, 2^31))")
     if start is not None and end is not None and start > end:
         raise _lib.B200Error(f"Streaming Window: {f!r}: frame start {start} is after frame end {end}")
-    if f[1] not in BOUNDED_FUNCS:
+    if f[1] not in BOUNDED_FUNCS and f[1] not in BIVARIATE_FUNCS:
         raise _lib.B200Error(f"Streaming Window: {f!r}: a ('rows', start, end) frame takes one of {list(BOUNDED_FUNCS)}")
     if start is None and end == 0:
         return FRAMES["rows"], None
@@ -245,7 +268,7 @@ def _parse_range(f, start, end):
         if (fs == "ns") == (fe == "ns") or s == 0 or e == 0:
             if s > e:
                 raise _lib.B200Error(f"Streaming Window: {f!r}: frame start {start!r} is after frame end {end!r}")
-    if f[1] not in BOUNDED_FUNCS:
+    if f[1] not in BOUNDED_FUNCS and f[1] not in BIVARIATE_FUNCS:
         raise _lib.B200Error(f"Streaming Window: {f!r}: a ('range_between', start, end) frame takes one of {list(BOUNDED_FUNCS)}")
     if start is None and end is None:
         return FRAMES["partition"], None
@@ -270,6 +293,8 @@ def _entry(f):
         fr = ("rows", *[None if b in (UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING) else b for b in f[6]])
     elif len(f) > 6:
         fr = ("range_between", *f[6])
+    if code in BIVARIATE_FUNCS.values():
+        return (name, _VALUE_NAMES[code], column, arg, fr)
     return (name, _VALUE_NAMES[code], column, fr) if code != FRAME_FUNCS["nth_value"] else (name, "nth_value", column, arg, fr)
 
 
@@ -296,7 +321,8 @@ def _parse_funcs(funcs, col_names):
     out = []
     for f in funcs:
         f = tuple(f)
-        value = isinstance(f[1] if len(f) > 1 else None, str) and (f[1] in VALUE_FUNCS or f[1] in FRAME_FUNCS or f[1] in MOMENT_FUNCS)
+        value = isinstance(f[1] if len(f) > 1 else None, str) and (f[1] in VALUE_FUNCS or f[1] in FRAME_FUNCS or f[1] in MOMENT_FUNCS
+                                                                   or f[1] in BIVARIATE_FUNCS)
         if (len(f) < 2 or not isinstance(f[0], str) or not isinstance(f[1], str) or f[1] not in FUNCS and not value
                 or value and len(f) < 3):
             raise _lib.B200Error(f"Streaming Window: unknown window function {f!r} ({_FORMS})")
@@ -363,8 +389,9 @@ class WindowState(SortState):
 
     def descriptors(self, c_types):
         """The b200_window_func fields (code, col, frame, default_valid, arg, default_bits) of every function, given the c-types
-        of the input columns in input order.  Raises B200Error for sum, mean, var or std of a temporal column and for a lag / lead default
-        that does not round-trip through the column's dtype."""
+        of the input columns in input order; a bivariate function's arg is its second column's physical index.  Raises B200Error
+        for sum, mean, var or std of a temporal column, a bivariate function with a temporal column in either position and a lag /
+        lead default that does not round-trip through the column's dtype."""
         out = []
         for f in self.funcs:
             if len(f) == 3:
@@ -375,6 +402,12 @@ class WindowState(SortState):
                 out.append((code, -1, frame, 0, arg, 0))
                 continue
             ct = c_types[self.col_names.index(column)]
+            if code in BIVARIATE_FUNCS.values():
+                if ct in _TEMPORAL or c_types[self.col_names.index(arg)] in _TEMPORAL:
+                    raise _lib.B200Error(f"Streaming Window: {_entry(f)!r}: covar, corr and regr need integer, bool or float columns, "
+                                         "not temporal ones")
+                out.append((code, self.phys.index(self.col_names.index(column)), frame, 0, self.phys.index(self.col_names.index(arg)), 0))
+                continue
             moment = code in MOMENT_FUNCS.values()
             if (code in (VALUE_FUNCS["sum"], VALUE_FUNCS["mean"]) or moment) and ct in _TEMPORAL:
                 entry = _entry(f)
@@ -445,8 +478,8 @@ class WindowState(SortState):
         rs = ffi.new("b200_window_range[]", len(self.descs))
         for d, (sk, ek, sb, eb) in zip(rs, self.rdescs):
             d.start_kind, d.end_kind, d.start_bits, d.end_bits = sk, ek, sb, eb
-        h = L.b200_window_state_init_ranges(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs, frs,
-                                            rs, len(self.descs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
+        h = L.b200_window_state_init_bivariate(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs,
+                                               frs, rs, len(self.descs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
         return _lib.check_ptr(h, "init_window_state")
 
 
@@ -459,15 +492,19 @@ def init_window_state(operator_id, partition_by, order_by, ascending, na_positio
     n >= 1; value entries (out_name, fname, column[, frame]) with fname in VALUE_FUNCS other than lag / lead, frame one of FRAMES
     (default "range") or ("rows", start, end) and column None for count(*) only, (out_name, "lag" | "lead", column[, k[,
     default]]) (k = 1 and default None, NA, by default), (out_name, "nth_value", column, n[, frame]), or (out_name, fname,
-    column[, frame]) with fname in MOMENT_FUNCS (var, std, var_pop, std_pop) and any frame sum takes.
+    column[, frame]) with fname in MOMENT_FUNCS (var, std, var_pop, std_pop) and any frame sum takes, or (out_name, fname, y, x[,
+    frame]) with fname in BIVARIATE_FUNCS (covar_samp, covar_pop, corr, regr_slope, regr_intercept; SQL's argument order) and
+    any frame sum takes.
     Examples, a 7-row moving average: ("ma7", "mean", "x", ("rows", -6, 0)); a one-hour time window over a DATETIME ORDER BY
     key: ("s1h", "sum", "amount", ("range_between", -pd.Timedelta("1h"), 0)); a 20-row rolling standard deviation (a Bollinger
     band's width): ("sd20", "std", "x", ("rows", -19, 0)); the population variance of the partition: ("vp", "var_pop", "x",
-    "partition").
+    "partition"); a 60-row rolling beta of r on the market return mr and their correlation: ("beta", "regr_slope", "r", "mr",
+    ("rows", -59, 0)), ("rho", "corr", "r", "mr", ("rows", -59, 0)).
     Raises B200Error for an unknown function, duplicate output names or names that clash with an input column, keys that are
     missing or not distinct, a key count outside 1..4, a bad na_position, ntile n < 1, an unknown value column, a bad frame or
     frame bound, a frame on lag or lead, k outside [0, 2^31), nth_value n outside [1, 2^31), a range offset without exactly one
-    ORDER BY key; and at the first consume call for sum, mean, var or std of a temporal column, a lag / lead default that the
+    ORDER BY key, a missing or unknown second column of a bivariate function; and at the first consume call for sum, mean, var
+    or std of a temporal column, a bivariate function with a temporal column in either position, a lag / lead default that the
     column's dtype cannot hold exactly or a range offset whose type does not fit the ORDER BY key."""
     return WindowState(operator_id, partition_by, order_by, ascending, na_position, funcs, col_names, parallel, output_batch_size,
                        device, stream, process_group)

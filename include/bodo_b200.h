@@ -279,7 +279,8 @@ void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const i
 /* One window function of b200_window_state_init_funcs.
  *   code: 0 row_number, 1 rank, 2 dense_rank, 3 percent_rank, 4 cume_dist, 5 ntile (the ranking functions above), then the value
  *         functions 6 sum, 7 count, 8 mean, 9 min, 10 max, 11 first_value, 12 last_value, 13 lag, 14 lead, 15 nth_value
- *         (b200_window_state_init_frames only), 16 var, 17 std, 18 var_pop, 19 std_pop (b200_window_state_init_moments only).
+ *         (b200_window_state_init_frames only), 16 var, 17 std, 18 var_pop, 19 std_pop (b200_window_state_init_moments only),
+ *         20 covar_samp, 21 covar_pop, 22 corr, 23 regr_slope, 24 regr_intercept (b200_window_state_init_bivariate only).
  *   col: the input column (0 <= col < n_arrs) a value function reads, any column including a key; -1 for a ranking function and
  *        for count(*).
  *   frame: 0 for a ranking function, lag and lead; for the others 1 range (RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW: up
@@ -289,7 +290,8 @@ void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const i
  *          function's b200_window_frame, for sum, count (of a column or count(*)), mean, min, max, first_value, last_value,
  *          nth_value, var, std, var_pop and std_pop.  5 range between (b200_window_state_init_ranges only): RANGE BETWEEN start
  *          AND end of the function's b200_window_range, for the same functions.
- *   arg: ntile's n (>= 1); lag / lead's offset k (0 <= k < 2^31; k = 0 is the row itself); nth_value's n (1 <= n < 2^31).
+ *   arg: ntile's n (>= 1); lag / lead's offset k (0 <= k < 2^31; k = 0 is the row itself); nth_value's n (1 <= n < 2^31); the
+ *        second column (x, 0 <= arg < n_arrs) of codes 20..24, whose first column (y) is col.
  *   default_valid, default_bits: lag / lead's value when row i - k / i + k is outside the row's partition: the low bytes of
  *          default_bits in the column's type if default_valid, else NA.
  * Over a frame [P, e] (a float NaN is NA for the aggregates):
@@ -310,6 +312,16 @@ void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const i
  *             combined from (count, mean, M2) triples by Chan's pairwise merge in the scan's or the frame tree's order: never
  *             negative, exactly 0.0 over equal values, a valid NaN when the frame holds +-inf.  FLOAT64, nullable.  Not for
  *             temporal columns.
+ *   covar_samp, covar_pop, corr, regr_slope, regr_intercept  with y = col and x = arg, m the frame's rows where both cells are
+ *             non-NA (pairwise deletion; integers and bool converted to double, exact up to 2^53), and over them the means
+ *             mx, my and Sxx = sum (x - mx)^2, Syy = sum (y - my)^2, Sxy = sum (x - mx)(y - my): 20 covar_samp = Sxy / (m - 1),
+ *             NA when m < 2 (COVAR_SAMP(y, x)); 21 covar_pop = Sxy / m, NA when m = 0 (COVAR_POP); 22 corr = Sxy / sqrt(Sxx Syy),
+ *             NA when m < 2, Sxx = 0 or Syy = 0, Sxy / (sqrt(Sxx) sqrt(Syy)) when Sxx Syy overflows or is subnormal, clamped
+ *             to [-1, 1] (CORR); 23 regr_slope = Sxy / Sxx, NA when Sxx = 0 (REGR_SLOPE(y, x)); 24 regr_intercept =
+ *             my - regr_slope mx, NA when Sxx = 0 (REGR_INTERCEPT(y, x)).  (count, mx, my, Sxx, Syy, Sxy) is combined by the
+ *             bivariate form of Chan's merge, with no sum of products: covar and corr are bit-symmetric in (x, y), x = y gives
+ *             corr 1.0 exactly where Sxx > 0 (and Sxx^2 is normal), equal x gives Sxx = 0 exactly; a valid NaN when the
+ *             frame's counted pairs hold +-inf.  FLOAT64, nullable.  Not for temporal columns.
  * Every row that shares a frame end gets a bit-identical result.
  * Over a frame 4 [lo, hi] (below) the same definitions hold with lo in place of P and hi in place of e; an empty frame (lo > hi)
  * gives NA, and count 0.  Float sums there are combined in an order fixed by (lo, hi) alone, so rows with the same bounds get the
@@ -384,12 +396,23 @@ typedef struct b200_window_range {
  * last_value, nth_value, var, std, var_pop and std_pop.  Bad kinds, an offset without exactly one ORDER BY key, an offset on a
  * BOOL key, a negative or non-finite offset, or start after end fails here (NULL, last error set).  (UNBOUNDED PRECEDING, CURRENT
  * ROW) is frame 1 and (UNBOUNDED PRECEDING, UNBOUNDED FOLLOWING) frame 3, with the same results.
- * b200_window_state_init_moments is this entry with ranges NULL, restricted to frames 0..4. */
+ * b200_window_state_init_moments is this entry with ranges NULL, restricted to frames 0..4.  This entry is
+ * b200_window_state_init_bivariate restricted to codes 0..19. */
 void* b200_window_state_init_ranges(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
                                     int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
                                     const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
                                     const b200_window_range* ranges, int32_t n_funcs, int64_t output_batch_size, int32_t device,
                                     void* stream);
+
+/* b200_window_state_init_ranges with codes 0..24: 20 covar_samp, 21 covar_pop, 22 corr, 23 regr_slope and 24 regr_intercept
+ * (defined above) read two columns, y = col and x = arg (0 <= arg < n_arrs; any column including a key, and the two may be the
+ * same), and take frames 1..5, as sum does.  A bad arg or a temporal column in either position fails here (NULL, last error
+ * set). */
+void* b200_window_state_init_bivariate(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                                       int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                                       const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
+                                       const b200_window_range* ranges, int32_t n_funcs, int64_t output_batch_size, int32_t device,
+                                       void* stream);
 
 /* The build-consume entry of _sort.cpp: filters a DEVICE-resident batch (same schema as the state) against the current cutoff on
  * the device (full sort: appends it to the chunk store); on is_last reduces to the final rows (full sort: sorts every row).
