@@ -21,8 +21,12 @@ doubles in [0, 1)) and an int64 row id r, fed in `--batch`-row batches.  Cases:
                  PRECEDING AND 2^34 ns FOLLOWING, OVER (PARTITION BY p ORDER BY t): about 8 rows per frame, as in moving
   range_wide     SUM(r) and MIN(o) RANGE BETWEEN 2^28 ns PRECEDING AND CURRENT ROW OVER (ORDER BY t): one partition, about 65 536
                  rows per frame, as in moving_wide
-The range cases add a fourth column t, an int64 DATETIME key uniform in [0, 2^40) ns, and order by it; the other cases keep
-their three columns.  `--profile` runs one more step per case under torch.profiler (separately from the timed steps) and
+  ignore_nulls   a per-group ffill and bfill and a LAG that skips missing readings: LAST_VALUE(x IGNORE NULLS) ROWS, FIRST_VALUE(x
+                 IGNORE NULLS) ROWS BETWEEN CURRENT ROW AND UNBOUNDED FOLLOWING and LAG(x, 1) IGNORE NULLS, OVER (PARTITION BY p
+                 ORDER BY o)
+The range cases add a fourth column t, an int64 DATETIME key uniform in [0, 2^40) ns, and order by it; ignore_nulls adds a
+fourth column x, float64 normal values with about 30 % NaN placed by a hash of the row id; the other cases keep their three
+columns.  ignore_nulls alternates with lag_lead (lag_lead_ms), so its cost above RESPECT NULLS navigation is measured too.  `--profile` runs one more step per case under torch.profiler (separately from the timed steps) and
 reports the window kernels' device times; with it, nothing is timed (run it separately from the timed run).
 The value cases (running to bivariate, and the range cases) also alternate with rn_rank_dense (rn_rank_dense_ms), so their cost above the ranking kernels
 is measured too; their result check covers the validity of the nullable columns.  bivariate also alternates with moments
@@ -72,6 +76,8 @@ RANGE_MOVING = [("ra", "mean", "o", ("range_between", -_ns(1 << 35), 0)), ("rx",
                 ("rc", "count", None, ("range_between", -_ns(1 << 34), _ns(1 << 34)))]
 RANGE_WIDE = [("ws", "sum", "r", ("range_between", -_ns(1 << 28), 0)), ("wn", "min", "o", ("range_between", -_ns(1 << 28), 0))]
 RANGE_CASES = ("range_moving", "range_wide")
+IGNORE_NULLS = [("ff", "last_value", "x", "rows", "ignore_nulls"), ("bf", "first_value", "x", ("rows", 0, None), "ignore_nulls"),
+                ("lgx", "lag", "x", 1, None, "ignore_nulls")]
 VALUE_CASES = ("running", "partition_aggs", "lag_lead", "moving", "moving_wide", "moments", "bivariate") + RANGE_CASES
 
 
@@ -127,6 +133,15 @@ def range_bytes(n, funcs, n_parts, n_peers):
     and are counted once) and the 8-byte (lo, hi) per row."""
     frames = {f[-1] for f in funcs if len(f) > 3 and isinstance(f[-1], tuple) and f[-1][0] == "range_between"}
     return int(len(frames) * (n * (1 + 8 + 8) + 4 * (n_parts + n_peers)))
+
+
+def nulls_bytes(n, n_funcs, n_cols, n_valid, n_parts, n_peers):
+    """The IGNORE NULLS kernels per distinct value column (8-byte numpy cells, design bytes): the count pass reads the column,
+    the compaction pass reads it again and writes c (4 bytes per row) and pos (4 bytes per non-null row); the eval pass reads
+    the flags and the partition / peer-group words once, and per function and row two words of c, one of pos, the chosen 8-byte
+    cell and writes 8 + 1 bytes (the reads of c and pos that neighbouring rows share are counted once each)."""
+    build = n * 8 + n * 8 + 4 * n + 4 * n_valid
+    return int(n_cols * (build + n + 4 * (n_parts + n_peers)) + n_funcs * n * (4 + 4 + 8 + 8 + 1))
 
 
 def in_frame_path(f):
@@ -188,19 +203,22 @@ def main():
     synth.device_fill(None, ok, 0, 1, 62, sp)
     rid = torch.arange(n, dtype=torch.int64, device=dev)
     tk = None  # the range cases' DATETIME key, made on first use
+    xk = None  # ignore_nulls' value column, made on first use
     torch.cuda.synchronize(dev)
     cases = {"rn_rank_dense": (["p"], FUNCS3), "all6": (["p"], FUNCS6), "no_partition": ([], FUNCS3), "running": (["p"], RUNNING),
              "partition_aggs": (["p"], PARTITION_AGGS), "lag_lead": (["p"], LAG_LEAD), "moving": (["p"], MOVING),
              "moving_wide": ([], MOVING_WIDE), "moments": (["p"], MOMENTS), "bivariate": (["p"], BIVARIATE), "range_moving": (["p"], RANGE_MOVING),
-             "range_wide": ([], RANGE_WIDE)}
+             "range_wide": ([], RANGE_WIDE), "ignore_nulls": (["p"], IGNORE_NULLS)}
     names, order = ["p", "o", "r"], "o"
 
     def batches():
         for r0 in range(0, n, args.batch):
             r1 = min(n, r0 + args.batch)
             cols = [Column(pk[r0:r1]), Column(ok[r0:r1]), Column(rid[r0:r1])]
-            if len(names) > 3:
+            if names[3:] == ["t"]:
                 cols.append(Column(tk[r0:r1], None, CTypes.DATETIME, ArrTypes.NUMPY, r1 - r0))
+            elif names[3:] == ["x"]:
+                cols.append(Column(xk[r0:r1]))
             yield Table(cols, names), r1 == n
 
     def window_step(part, funcs, keep=False):
@@ -554,6 +572,37 @@ def main():
                 return f"MISMATCH: {f[0]}", 0, 0
         return "ok", n_parts, n_peers
 
+    def nulls_check(part, funcs, res):
+        """ignore_nulls: the sorted columns against two stable torch.sorts, then per row the last non-null row at or before it
+        (a cummax of the non-null positions), the first at or after it (a reversed cummin) and the last before it, each valid when
+        it lies in the row's partition; the chosen cells bit for bit."""
+        idx = torch.sort(ok, stable=True).indices
+        idx = idx[torch.sort(pk[idx], stable=True).indices]
+        if not (torch.equal(res[2], idx) and torch.equal(res[3].view(torch.int64), xk[idx].view(torch.int64))):
+            return "MISMATCH: an input column differs from the stable sort", 0, 0
+        del idx
+        sp_, sx = res[0], res[3]
+        i = torch.arange(n, device=dev, dtype=torch.int64)
+        ps = torch.ones(n, dtype=torch.bool, device=dev)
+        ps[1:] = torch.diff(sp_) != 0
+        qs = ps.clone()
+        qs[1:] |= torch.diff(res[1]) != 0
+        P = torch.cummax(torch.where(ps, i, 0), 0).values
+        last = torch.roll(ps, -1)
+        last[-1] = True
+        pe = torch.flip(torch.cummin(torch.flip(torch.where(last, i + 1, n), [0]), 0).values, [0])
+        nn = ~torch.isnan(sx)
+        prev = torch.cummax(torch.where(nn, i, -1), 0).values
+        nxt = torch.flip(torch.cummin(torch.flip(torch.where(nn, i, n), [0]), 0).values, [0])
+        before = torch.cat([torch.full((1,), -1, dtype=torch.int64, device=dev), prev[:-1]])
+        nf = len(funcs)
+        for j, (src, good) in enumerate(((prev, prev >= P), (nxt, nxt < pe), (before, before >= P))):
+            got, valid = res[4 + j], res[4 + nf + j]
+            exp = sx[src.clamp(0, n - 1)].view(torch.int64)
+            if not (torch.equal(valid, good) and torch.equal(torch.where(good, got.view(torch.int64), 0), torch.where(good, exp, 0))):
+                return f"MISMATCH: {funcs[j][0]}", 0, 0
+        return "ok", int(ps.sum()), int(qs.sum())
+
     def free():
         torch.cuda.empty_cache()
         _lib.lib().b200_pool_trim(0, 0)
@@ -582,6 +631,13 @@ def main():
             if tk is None:
                 tk = torch.randint(0, 1 << 40, (n,), generator=g, device=dev, dtype=torch.int64)
             names, order = ["p", "o", "r", "t"], "t"
+        elif name == "ignore_nulls":
+            if xk is None:  # NaN where a multiplicative hash of the row id falls in the lowest 30 % of [0, 2^10)
+                xk = torch.randn(n, generator=g, device=dev, dtype=torch.float64)
+                h = ((rid * -7046029254386353131) >> 54) & 1023
+                xk[h < 307] = float("nan")
+                del h
+            names, order = ["p", "o", "r", "x"], "o"
         else:
             names, order = ["p", "o", "r"], "o"
         if args.profile:
@@ -594,7 +650,9 @@ def main():
             window_step(part, FUNCS3)
         if name == "bivariate":
             window_step(part, MOMENTS)
-        wt, st_, rt, mt = [], [], [], []
+        if name == "ignore_nulls":
+            window_step(part, LAG_LEAD)
+        wt, st_, rt, mt, lt = [], [], [], [], []
         for _ in range(args.reps):
             ms, (_, m9) = timed(lambda: window_step(part, funcs))
             wt.append(ms)
@@ -604,12 +662,14 @@ def main():
                 rt.append(timed(lambda: window_step(part, FUNCS3))[0])
             if name == "bivariate":  # next to the moments, whose scan value is half as wide
                 mt.append(timed(lambda: window_step(part, MOMENTS))[0])
+            if name == "ignore_nulls":  # next to RESPECT NULLS navigation over the same four columns
+                lt.append(timed(lambda: window_step(part, LAG_LEAD))[0])
         w_ms, s_ms = sorted(wt)[len(wt) // 2], sorted(st_)[len(st_) // 2]
         free()
         # check
         res, _ = window_step(part, funcs, keep=True)
         free()
-        chk, n_parts, n_peers = (range_check if name in RANGE_CASES else check)(part, funcs, res)
+        chk, n_parts, n_peers = (range_check if name in RANGE_CASES else nulls_check if name == "ignore_nulls" else check)(part, funcs, res)
         if chk == "ok" and m9 != n_parts:
             chk = f"MISMATCH: metric 9 = {m9}, partitions = {n_parts}"
         del res
@@ -617,6 +677,7 @@ def main():
         # design bytes: the sort of the keys (passes from the data, as sort_bench predicts them), then the window kernels
         f64w = lambda x: torch.where(x < 0, x.view(torch.int64) ^ 0x7FFFFFFFFFFFFFFF, x.view(torch.int64))  # noqa: E731
         words = [tk ^ (-(2 ** 63)) if name in RANGE_CASES else f64w(ok)] + ([pk ^ (-(2 ** 63))] if part else [])
+        n_valid = int((~torch.isnan(xk)).sum()) if name == "ignore_nulls" else 0
         kp = plan(torch, words, [8] * len(words), [True] + [False] * len(part), [0] * len(words))
         del words
         free()
@@ -627,6 +688,9 @@ def main():
             scans = [f for f in funcs if not in_frame_path(f)]
             total = (sort_bytes + window_bytes(n, key_bytes, 0, n_parts, n_peers) - (n + ends4) + value_bytes(n, scans, n_parts, n_peers)
                      + frame_bytes(n, [f for f in funcs if in_frame_path(f)], n_parts, n_peers) + range_bytes(n, funcs, n_parts, n_peers))
+        elif name == "ignore_nulls":  # bounds and ends as the ranking cases, then one (c, pos) build and one eval pass
+            total = (sort_bytes + window_bytes(n, key_bytes, 0, n_parts, n_peers) - (n + 4 * (2 * n_parts + n_peers))
+                     + nulls_bytes(n, len(funcs), 1, n_valid, n_parts, n_peers))
         else:
             total = sort_bytes + window_bytes(n, key_bytes, len(funcs), n_parts, n_peers)
         out = {"case": name, "rows": n, "batch": args.batch, "funcs": [f[1] for f in funcs], "ms_per_step": round(w_ms, 3),
@@ -638,6 +702,9 @@ def main():
         if value_case:
             r_ms = sorted(rt)[len(rt) // 2]
             out.update(rn_rank_dense_ms=round(r_ms, 3), rn_rank_dense_runs_ms=[round(x, 3) for x in rt], extra_over_rn_rank_dense_ms=round(w_ms - r_ms, 3))
+        if lt:
+            l_ms = sorted(lt)[len(lt) // 2]
+            out.update(lag_lead_ms=round(l_ms, 3), lag_lead_runs_ms=[round(x, 3) for x in lt], extra_over_lag_lead_ms=round(w_ms - l_ms, 3))
         if mt:
             m_ms = sorted(mt)[len(mt) // 2]
             out.update(moments_ms=round(m_ms, 3), moments_runs_ms=[round(x, 3) for x in mt], extra_over_moments_ms=round(w_ms - m_ms, 3))

@@ -1845,6 +1845,201 @@ __global__ void __launch_bounds__(WN_THREADS) window_range_bounds_kernel(const _
     }
 }
 
+// ---- IGNORE NULLS: FIRST_VALUE / LAST_VALUE / NTH_VALUE over every frame, LAG / LEAD ----
+//
+// A cell is null when count(x) does not count it: its validity byte is 0 or it is a float NaN (RESPECT NULLS first_value keeps
+// a NaN as a valid cell; IGNORE NULLS skips it, as pandas' ffill / bfill do).  With v[j] = 1 at the non-null sorted rows, one
+// value column gets c[0..n], the exclusive prefix count of v (c[n] = m, the non-null rows), and pos[0..m), their positions:
+//   window_nulls_count_kernel    per WN_TILE-row tile: its non-null count.
+//   window_nulls_tiles_kernel    one block: the exclusive scan of the tile counts, and c[n].
+//   window_nulls_compact_kernel  per tile again: c[i] from the tile prefix and a ballot per 32 rows; pos[c[i]] = i at non-null i.
+// Then each function is index arithmetic on (c, pos) over the frame [lo, hi] or the partition [P, pe) of its RESPECT NULLS form:
+//   first_value  j = c[lo], valid iff lo <= hi and j < c[hi + 1]      nth_value(n)  j = c[lo] + n - 1, valid iff j < c[hi + 1]
+//   last_value   j = c[hi + 1] - 1, valid iff j >= c[lo]              lag(k)        j = c[i] - k, valid iff j >= c[P]
+//   lead(k)      j = c[i + 1] + k - 1, valid iff j < c[pe]            (lo <= hi is tested before c is read: an empty bounded
+// frame's lo may lie past n).  The result is the cell at pos[j]; else NA, or lag / lead's default.  lag / lead with k = 0 is the
+// row itself, as in RESPECT NULLS.  No arithmetic on the values: the results are exact and depend only on sorted positions.
+//   window_nulls_eval_kernel     frames 1..4, lag and lead: the ranking scan of the flags (P, Q) again, then per row every
+//                                IGNORE NULLS function of the column whose (c, pos) is built.
+//   window_nulls_range_kernel    frame 5: the same, one thread per row, from the bounds window_range_bounds_kernel wrote.
+// c and pos are uint32 (n <= 2^31); one buffer of 8 B per row holds them and is rebuilt for each value column.
+struct WnlArgs {
+    int64_t n;
+    const uint8_t* flags;
+    const WnAgg* tile;              // the ranking scan's tile prefixes
+    const uint32_t *psize, *pend;
+    WvCol x;                        // the value column of every function below
+    uint32_t* tcount;               // per tile: its non-null count, then its exclusive prefix
+    uint32_t *c, *pos;
+    int n_funcs;
+    WfFunc f[SORT_MAX_COLS];        // g.k: nth_value's n or lag / lead's k; frame 5: range
+};
+
+__device__ __forceinline__ bool wnl_null(const WvCol& x, int64_t i) {
+    if (x.vb && x.vb[i] == 0) return true;
+    if (x.ct == CT_FLOAT64) return isnan(__longlong_as_double((long long)load_bits(x.data, 8, i)));
+    if (x.ct == CT_FLOAT32) return isnan(__uint_as_float((uint32_t)load_bits(x.data, 4, i)));
+    return false;
+}
+
+__global__ void __launch_bounds__(WN_THREADS) window_nulls_count_kernel(const __grid_constant__ WnlArgs a) {
+    __shared__ uint32_t s_cnt[WN_WARPS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t t = blockIdx.x;
+    uint32_t cnt = 0;
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        cnt += i < a.n && !wnl_null(a.x, i);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if (lane == 0) s_cnt[warp] = cnt;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < WN_WARPS; w++) cnt += s_cnt[w];
+        a.tcount[t] = cnt;
+    }
+}
+
+// One block of 1024 threads; thread x scans a contiguous run of tiles (as window_tiles_kernel).
+__global__ void __launch_bounds__(1024) window_nulls_tiles_kernel(const __grid_constant__ WnlArgs a, int64_t n_tiles) {
+    __shared__ uint32_t s_sum[32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t per = (n_tiles + 1023) / 1024, t0 = threadIdx.x * per, t1 = min(n_tiles, t0 + per);
+    uint32_t acc = 0;
+    for (int64_t t = t0; t < t1; t++) acc += a.tcount[t];
+    uint32_t inc = acc;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += y;
+    }
+    if (lane == 31) s_sum[warp] = inc;
+    __syncthreads();
+    uint32_t run = inc - acc;
+    for (int w = 0; w < warp; w++) run += s_sum[w];
+    for (int64_t t = t0; t < t1; t++) {
+        const uint32_t v = a.tcount[t];
+        a.tcount[t] = run;
+        run += v;
+    }
+    if (threadIdx.x == 1023) a.c[a.n] = run;
+}
+
+__global__ void __launch_bounds__(WN_THREADS) window_nulls_compact_kernel(const __grid_constant__ WnlArgs a) {
+    __shared__ uint32_t s_seg[WN_ITEMS * WN_WARPS];  // per (item, warp) segment of 32 rows: its count, then its exclusive prefix
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t t = blockIdx.x;
+    uint32_t ball[WN_ITEMS];
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        ball[k] = __ballot_sync(0xffffffffu, i < a.n && !wnl_null(a.x, i));
+        if (lane == 0) s_seg[k * WN_WARPS + warp] = __popc(ball[k]);
+    }
+    __syncthreads();
+    if (warp == 0) {  // exclusive scan of the 64 segments in row order, seeded by the tile prefix: 2 per lane
+        const uint32_t x0 = s_seg[2 * lane], x1 = s_seg[2 * lane + 1];
+        uint32_t inc = x0 + x1;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += y;
+        }
+        const uint32_t base = a.tcount[t] + inc - x0 - x1;
+        s_seg[2 * lane] = base;
+        s_seg[2 * lane + 1] = base + x0;
+    }
+    __syncthreads();
+    const uint32_t below = (1u << lane) - 1u;
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        if (i >= a.n) break;
+        const uint32_t ci = s_seg[k * WN_WARPS + warp] + __popc(ball[k] & below);
+        a.c[i] = ci;
+        if ((ball[k] >> lane) & 1u) a.pos[ci] = (uint32_t)i;
+    }
+}
+
+// Row i's IGNORE NULLS functions; bounds(g, lo, hi) gives a frame function's [lo, hi], and [P, pe) is the row's partition (read
+// by lag and lead only).
+template <typename Bounds>
+__device__ __forceinline__ void wnl_eval_row(const WnlArgs& a, int64_t i, int64_t P, int64_t pe, Bounds bounds) {
+    for (int fn = 0; fn < a.n_funcs; fn++) {
+        const WfFunc& h = a.f[fn];
+        const WvFunc& g = h.g;
+        int64_t j = -1;  // the chosen non-null row's index in pos, -1: none
+        bool self = false;
+        if (g.code == WN_LAG || g.code == WN_LEAD) {
+            if (g.k == 0) self = true;
+            else if (g.code == WN_LAG) { const int64_t r = (int64_t)a.c[i] - g.k; if (r >= (int64_t)a.c[P]) j = r; }
+            else { const int64_t r = (int64_t)a.c[i + 1] + g.k - 1; if (r < (int64_t)a.c[pe]) j = r; }
+        } else {
+            int64_t lo, hi;
+            bounds(h, lo, hi);
+            if (lo <= hi) {
+                const int64_t c0 = a.c[lo], c1 = a.c[hi + 1];
+                const int64_t r = g.code == WN_FIRST_VALUE ? c0 : g.code == WN_LAST_VALUE ? c1 - 1 : c0 + g.k - 1;
+                if (r >= c0 && r < c1) j = r;
+            }
+        }
+        if (self) {
+            copy_cell(g.out, i, g.data, i, g.size);
+            g.out_vb[i] = !g.vb || g.vb[i];
+        } else if (j >= 0) {
+            copy_cell(g.out, i, g.data, a.pos[j], g.size);
+            g.out_vb[i] = 1;
+        } else {
+            const bool nav = g.code == WN_LAG || g.code == WN_LEAD;
+            wv_store_bits(g.out, i, nav ? g.dflt : 0ull, g.size);
+            g.out_vb[i] = nav ? (uint8_t)g.dflt_valid : 0;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(WN_THREADS) window_nulls_eval_kernel(const __grid_constant__ WnlArgs a) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t t = blockIdx.x;
+    WnArgs w;  // wn_scan_tile reads n, flags and the tile prefixes only
+    w.n = a.n; w.flags = const_cast<uint8_t*>(a.flags); w.tile = const_cast<WnAgg*>(a.tile);
+    uint8_t f[WN_ITEMS];
+    WnAgg v[WN_ITEMS];
+    wn_scan_tile(w, t, f, v);
+    __shared__ WnAgg s_v[WN_ITEMS][WN_THREADS];  // parked as in window_eval_kernel: the item loop is not unrolled
+#pragma unroll
+    for (int k = 0; k < WN_ITEMS; k++) s_v[k][threadIdx.x] = v[k];
+#pragma unroll 1
+    for (int k = 0; k < WN_ITEMS; k++) {
+        const int64_t i = wn_row(t, k, warp, lane);
+        if (i >= a.n) break;
+        const WnAgg vk = s_v[k][threadIdx.x];
+        const int64_t P = vk.p, pe = P + a.psize[vk.p], qe = a.pend[vk.q];
+        wnl_eval_row(a, i, P, pe, [&](const WfFunc& g, int64_t& lo, int64_t& hi) { wf_bounds(g, i, P, pe, qe, lo, hi); });
+    }
+}
+
+__global__ void __launch_bounds__(WN_THREADS) window_nulls_range_kernel(const __grid_constant__ WnlArgs a) {
+    const int64_t i = (int64_t)blockIdx.x * WN_THREADS + threadIdx.x;
+    if (i >= a.n) return;
+    wnl_eval_row(a, i, 0, 0, [i](const WfFunc& g, int64_t& lo, int64_t& hi) {
+        const int2 b = __ldg(g.range + i);
+        lo = b.x;
+        hi = b.y;
+    });
+}
+
+// (c, pos) of value column x, then `eval` over a.f (frames 1..4, lag and lead) or `range` (frame 5).
+static void launch_wnl(WnlArgs& a, const WvCol& x, int64_t n_tiles, bool range, cudaStream_t st) {
+    a.x = x;
+    window_nulls_count_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
+    window_nulls_tiles_kernel<<<1, 1024, 0, st>>>(a, n_tiles);
+    window_nulls_compact_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
+    if (range) window_nulls_range_kernel<<<(unsigned)(n_tiles * WN_ITEMS), WN_THREADS, 0, st>>>(a);
+    else window_nulls_eval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
+}
+
 // Ranking and value window functions over (PARTITION BY the first n_part keys ORDER BY the rest).  The output is the full sort's,
 // plus one column per function after the input columns: numpy for the ranking functions and count, nullable for the others.
 struct WindowState : FullSortState {
@@ -1852,18 +2047,22 @@ struct WindowState : FullSortState {
     b200_window_func fn[SORT_MAX_COLS];
     b200_window_frame bound[SORT_MAX_COLS];  // a WF_BOUNDED function's frame
     b200_window_range range[SORT_MAX_COLS];  // a WF_RANGE_BETWEEN function's frame
+    bool ignore_nulls[SORT_MAX_COLS];        // first_value, last_value, lag, lead or nth_value with IGNORE NULLS
     std::vector<DevBuf> fout;
     int64_t n_partitions = 0;  // metric 9
 
     WindowState(const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_part_, int n_keys, const int32_t* asc,
                 const int32_t* na_last, const b200_window_func* funcs, const b200_window_frame* frames, const b200_window_range* ranges,
-                int n_funcs_, int64_t obs, int dev, cudaStream_t st)
+                const int32_t* nulls, int n_funcs_, int64_t obs, int dev, cudaStream_t st)
         : FullSortState(c_types, arr_types, n_arrs, n_keys, asc, na_last, obs, dev, st), n_part(n_part_), n_funcs(n_funcs_) {
         for (int f = 0; f < n_funcs; f++) {
             b200_window_func& d = fn[f] = funcs[f];
             bound[f] = b200_window_frame{WF_UNBOUNDED_START, WF_UNBOUNDED_END};
             range[f] = b200_window_range{WR_UNBOUNDED_PRECEDING, WR_UNBOUNDED_FOLLOWING, 0, 0};
             B200_REQUIRE(d.code >= WN_ROW_NUMBER && d.code <= WN_REGR_INTERCEPT, "b200 window: unknown function code");
+            ignore_nulls[f] = nulls && nulls[f] != 0;
+            B200_REQUIRE(!ignore_nulls[f] || (d.code >= WN_FIRST_VALUE && d.code <= WN_NTH_VALUE),
+                         "b200 window: IGNORE NULLS takes first_value, last_value, lag, lead and nth_value only (codes 11..15)");
             int ct = CT_INT64, at = ARR_NUMPY;
             if (d.code <= WN_NTILE) {
                 B200_REQUIRE(d.col == -1 && d.frame == WF_NONE, "b200 window: a ranking function takes no column and no frame");
@@ -1962,8 +2161,19 @@ struct WindowState : FullSortState {
         std::vector<WvFunc> scans;
         WfArgs fa{};
         std::vector<WfFunc> trees;
-        struct RangeFrame { b200_window_range r; std::vector<WfFunc> trees, gathers; };  // the functions of one distinct frame 5
+        // the functions of one distinct frame 5 (nulls: its IGNORE NULLS functions)
+        struct RangeFrame { b200_window_range r; std::vector<WfFunc> trees, gathers, nulls; };
         std::vector<RangeFrame> ranged;
+        const auto range_frame = [&](int f) {
+            const b200_window_range& r = range[f];
+            auto it = std::find_if(ranged.begin(), ranged.end(), [&](const RangeFrame& x) {
+                return x.r.start_kind == r.start_kind && x.r.end_kind == r.end_kind && x.r.start_bits == r.start_bits &&
+                       x.r.end_bits == r.end_bits;
+            });
+            return it == ranged.end() ? ranged.insert(ranged.end(), RangeFrame{r, {}, {}, {}}) : it;
+        };
+        std::vector<WfFunc> nulls;  // IGNORE NULLS functions over frames 1..4, lag and lead
+        bool any_nulls = false;
         bool eval = false;
         for (int f = 0; f < n_funcs; f++) {
             const int c = sc.n_cols + f;
@@ -1979,6 +2189,15 @@ struct WindowState : FullSortState {
             WvFunc g{d.code, d.frame, d.col >= 0 ? sc.ctype[d.col] : CT_INT64, d.col >= 0 ? ctype_size(sc.ctype[d.col]) : 0,
                      ctype_size(sc.ctype[c]), d.default_valid, d.arg, d.default_bits, d.col >= 0 ? out_data[d.col] : nullptr,
                      d.col >= 0 ? out_vb[d.col] : nullptr, out_data[c], out_vb[c]};
+            if (ignore_nulls[f]) {  // the IGNORE NULLS kernels only, never a scan, tree or gather
+                WfFunc h{};
+                h.g = g;
+                h.start = bound[f].start;
+                h.end = bound[f].end;
+                (d.frame == WF_RANGE_BETWEEN ? range_frame(f)->nulls : nulls).push_back(h);
+                any_nulls = true;
+                continue;
+            }
             if (d.frame == WF_BOUNDED || d.frame == WF_RANGE_BETWEEN || d.code == WN_NTH_VALUE) {  // the frame path only
                 WfFunc h{};
                 h.g = g;
@@ -1986,13 +2205,7 @@ struct WindowState : FullSortState {
                 h.end = bound[f].end;
                 const bool agg = wv_aggregate(d.code) && d.col >= 0;
                 if (d.frame == WF_RANGE_BETWEEN) {
-                    const b200_window_range& r = range[f];
-                    auto it = std::find_if(ranged.begin(), ranged.end(), [&](const RangeFrame& x) {
-                        return x.r.start_kind == r.start_kind && x.r.end_kind == r.end_kind && x.r.start_bits == r.start_bits &&
-                               x.r.end_bits == r.end_bits;
-                    });
-                    if (it == ranged.end()) it = ranged.insert(ranged.end(), RangeFrame{r, {}, {}});
-                    (agg ? it->trees : it->gathers).push_back(h);
+                    (agg ? range_frame(f)->trees : range_frame(f)->gathers).push_back(h);
                 } else if (agg) {
                     trees.push_back(h);
                 } else {
@@ -2043,6 +2256,30 @@ struct WindowState : FullSortState {
         }
         if (eval) window_veval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a, va);
         B200_CUDA(cudaGetLastError());
+        // IGNORE NULLS: one (c, pos) buffer of 8 B per row (plus a word per tile), rebuilt for each value column.  It is built once
+        // per distinct column of the frame 1..4 / lag / lead functions, then once per distinct (frame 5, column) in the frame
+        // loop below, after that frame's bounds.
+        DevBuf nb;
+        WnlArgs na{};
+        const auto launch_nulls = [&](const std::vector<WfFunc>& fs, bool range) {
+            for (size_t j = 0; j < fs.size(); j++) {
+                const WvFunc& g = fs[j].g;
+                bool seen = false;
+                for (size_t k = 0; k < j; k++) seen = seen || fs[k].g.data == g.data;
+                if (seen) continue;
+                na.n_funcs = 0;
+                for (size_t k = j; k < fs.size(); k++)
+                    if (fs[k].g.data == g.data) na.f[na.n_funcs++] = fs[k];
+                launch_wnl(na, WvCol{g.data, g.vb, g.ct, g.size}, n_tiles, range, stream);
+            }
+            B200_CUDA(cudaGetLastError());
+        };
+        if (any_nulls) {
+            nb.alloc((size_t)(2 * n + 1 + n_tiles) * 4);
+            na.n = n; na.flags = a.flags; na.tile = a.tile; na.psize = a.psize; na.pend = a.pend;
+            na.c = nb.as<uint32_t>(); na.pos = na.c + n + 1; na.tcount = na.pos + n;
+            launch_nulls(nulls, false);
+        }
         // one tree buffer, reused by every aggregate over a bounded frame: n / 8 + n / 16 + ... nodes of the largest scan value
         // among them, <= 4 B per row (<= 6 B per row with a moment, <= 12 B per row with a bivariate function)
         DevBuf tree, rb;
@@ -2081,6 +2318,8 @@ struct WindowState : FullSortState {
                 for (WfFunc& h : rf.gathers) { h.range = ra.out; fa.f[fa.n_funcs++] = h; }
                 if (fa.n_funcs > 0) window_range_frame_kernel<WV_GATHER><<<(unsigned)(n_tiles * WN_ITEMS), WN_THREADS, 0, stream>>>(fa, WvCol{});
                 B200_CUDA(cudaGetLastError());
+                for (WfFunc& h : rf.nulls) h.range = ra.out;
+                launch_nulls(rf.nulls, true);
             }
         }
         auto* h = (uint32_t*)pinned_acquire(8);
@@ -2192,6 +2431,15 @@ void* b200_window_state_init_bivariate(int64_t operator_id, const int8_t* c_type
                                        const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
                                        const b200_window_range* ranges, int32_t n_funcs, int64_t output_batch_size, int32_t device,
                                        void* stream) {
+    return b200_window_state_init_nulls(operator_id, c_types, arr_types, n_arrs, n_partition_keys, n_order_keys, order_ascending,
+                                        order_na_last, funcs, frames, ranges, nullptr, n_funcs, output_batch_size, device, stream);
+}
+
+void* b200_window_state_init_nulls(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                                   int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                                   const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
+                                   const b200_window_range* ranges, const int32_t* ignore_nulls, int32_t n_funcs,
+                                   int64_t output_batch_size, int32_t device, void* stream) {
     (void)operator_id;
     return b200::sort_state_new(device, [&]() -> SortState* {
         const int np = n_partition_keys, no = n_order_keys;
@@ -2206,8 +2454,8 @@ void* b200_window_state_init_bivariate(int64_t operator_id, const int8_t* c_type
             asc[j] = j < np ? 1 : order_ascending[j - np];
             na_last[j] = j < np ? 1 : order_na_last[j - np];
         }
-        return new b200::WindowState(c_types, arr_types, n_arrs, np, np + no, asc, na_last, funcs, frames, ranges, n_funcs,
-                                     output_batch_size, device, (cudaStream_t)stream);
+        return new b200::WindowState(c_types, arr_types, n_arrs, np, np + no, asc, na_last, funcs, frames, ranges, ignore_nulls,
+                                     n_funcs, output_batch_size, device, (cudaStream_t)stream);
     });
 }
 

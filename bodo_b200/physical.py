@@ -328,7 +328,8 @@ class PhysicalWindow:
     spelling with offsets measured in the single ORDER BY key, e.g. -pd.Timedelta("1h")), (out_name, "lag" | "lead", column[, k[,
     default]]), (out_name,
     "nth_value", column, n[, frame]) or (out_name, fname, y, x[, frame]), fname one of streaming.window.BIVARIATE_FUNCS
-    (covar_samp, covar_pop, corr, regr_slope, regr_intercept, over any frame sum takes);
+    (covar_samp, covar_pop, corr, regr_slope, regr_intercept, over any frame sum takes); an entry of first_value, last_value,
+    nth_value, lag or lead may end with "ignore_nulls" (IGNORE NULLS) or "respect_nulls" (the default);
     ascending / na_position: one value or one per ORDER BY key.  The column names are taken from the first batch."""
 
     def __init__(self, partition_by, order_by, funcs, ascending=True, na_position="last", parallel: bool = False, **kw):
@@ -478,7 +479,7 @@ def window(df, partition_by, order_by, funcs, ascending=True, na_position="last"
     """Ranking, aggregate and navigation window functions OVER (PARTITION BY partition_by ORDER BY order_by) through
     PhysicalWindow (funcs as PhysicalWindow takes them, e.g. [("run", "sum", "x", "rows"), ("prev", "lag", "x", 1, 0),
     ("ma7", "mean", "x", ("rows", -6, 0)), ("sd20", "std", "x", ("rows", -19, 0)), ("beta", "regr_slope", "y", "x", ("rows", -59,
-    0))]).  Returns a pandas
+    0)), ("ffill", "last_value", "x", "rows", "ignore_nulls")]).  Returns a pandas
     DataFrame in the operator's output order (stably sorted by partition keys, then order keys) with a fresh index: df's columns,
     then one column per function."""
     op = PhysicalWindow(partition_by, order_by, funcs, ascending, na_position, **kw)

@@ -7,13 +7,15 @@
     VAR_SAMP / STDDEV_SAMP / VAR_POP / STDDEV_POP (x) OVER (PARTITION BY p ORDER BY o [frame])
     every frame function over RANGE BETWEEN x PRECEDING AND y FOLLOWING, an offset measured in the ORDER BY value
     COVAR_SAMP / COVAR_POP / CORR / REGR_SLOPE / REGR_INTERCEPT (y, x) OVER (PARTITION BY p ORDER BY o [frame])
+    FIRST_VALUE / LAST_VALUE / NTH_VALUE / LAG / LEAD with IGNORE NULLS (a trailing "ignore_nulls" in the entry)
 
 pandas equivalents: groupby(p).cumcount() + 1, groupby(p)[o].rank(method="min" / "dense" / "max", pct=...),
 groupby(p)[x].cumsum() / cummin() / cummax() (the "rows" frame), groupby(p)[x].transform("sum" / "mean" / "min" / "max" /
 "count" / "size" / "first" / "last" / "var" / "std") (the "partition" frame), groupby(p)[x].expanding().var() / .std() (the
 "rows" frame), groupby(p)[x].rolling(w).var() / .std() (a bounded frame), groupby(p).rolling("1h", on=t) (a RANGE frame),
-groupby(p)[y].rolling(w).cov(x) / .corr(x) (a bounded frame) and groupby(p)[x].shift(k, fill_value=default) (lag;
-lead is shift(-k)).  The state is a third form of the streaming sort (streaming/sort.py's SortState, sort.cu's WindowState): batches are
+groupby(p)[y].rolling(w).cov(x) / .corr(x) (a bounded frame), groupby(p)[x].shift(k, fill_value=default) (lag;
+lead is shift(-k)) and, ordered by a row id, groupby(p)[x].ffill() / ffill(limit=n) / bfill() / bfill(limit=n) (last_value
+IGNORE NULLS over "rows" / ("rows", -n, 0), first_value IGNORE NULLS over ("rows", 0, None) / ("rows", 0, n)).  The state is a third form of the streaming sort (streaming/sort.py's SortState, sort.cu's WindowState): batches are
 appended to the full sort's device chunk store, is_last sorts every row by (partition keys ascending NA last, order keys, arrival
 index), scans the sorted key columns on the device for partition and peer-group boundaries and then scans or gathers the value
 columns.
@@ -83,6 +85,16 @@ Semantics:
       lag(x, k=1, default=None) / lead(...): the cell at i - k / i + k if that row is in the row's partition, else default (NA
         when None); 0 <= k < 2^31, k = 0 is the row itself; no frame; x's type, nullable.  default is converted to x's numpy
         dtype and must round-trip exactly.
+    IGNORE NULLS: an entry of first_value, last_value, nth_value, lag or lead may end with "ignore_nulls" or "respect_nulls"
+    (the default, the definitions above), recognised only as the last element at index 3 or later (so a column named
+    "ignore_nulls" is still a column) and removed before the rest is parsed; on any other function it raises.  A cell is null
+    exactly when count(x) does not count it: invalid or a float NaN.  This differs from RESPECT NULLS first_value, which returns
+    a NaN as a valid cell: IGNORE NULLS skips it, as pandas' ffill / bfill do, so it works on numpy float columns too.  With row
+    i's frame [lo, hi] and partition [P, pe) as the RESPECT NULLS function computes them (every frame, the same empty-frame rule):
+      first_value(x) / last_value(x): the first / last non-null cell in [lo, hi], NA if none; nth_value(x, n): the n-th non-null
+        cell in [lo, hi], NA if there are fewer than n; lag(x, k, default) / lead(...): the k-th non-null cell before row i in
+        [P, i) / after it in (i, pe), default if there are fewer than k (k = 0 is the row itself, as above).
+      The result is the chosen cell's bits (-0.0 stays -0.0); x's type, nullable; bit-identical across runs and batch splits.
     These follow SQL where pandas differs: groupby().cumsum() / cummin() / cummax() give NA at NA rows where the "rows" frame
     gives the aggregate so far; transform("sum") of an all-NA partition gives 0 where sum gives NA; float sums are combined in
     the scan's order, not sequentially.  Over ("rows", start, end) the results are pandas' groupby(p)[x].rolling(w,
@@ -127,6 +139,9 @@ BOUNDED_FUNCS = ("sum", "count", "mean", "min", "max", "first_value", "last_valu
 # The bivariate entry's codes (b200_window_state_init_bivariate): functions of two columns (y, x), x's index in arg.  They take
 # every frame BOUNDED_FUNCS take.
 BIVARIATE_FUNCS = {"covar_samp": 20, "covar_pop": 21, "corr": 22, "regr_slope": 23, "regr_intercept": 24}
+# The navigation functions that take a trailing "ignore_nulls" / "respect_nulls" marker (b200_window_state_init_nulls).
+NULLS_FUNCS = ("first_value", "last_value", "nth_value", "lag", "lead")
+NULLS_MARKERS = ("ignore_nulls", "respect_nulls")
 _VALUE_NAMES = {c: f for f, c in {**VALUE_FUNCS, **FRAME_FUNCS, **MOMENT_FUNCS, **BIVARIATE_FUNCS}.items()}
 _FRAME_NAMES = {c: f for f, c in FRAMES.items()}
 MAX_COLS = 32
@@ -142,7 +157,8 @@ _CT_NAMES = {v: k for k, v in vars(CTypes).items() if k.isupper() and isinstance
 _FORMS = (f"ranking: (out_name, fname) with fname in {sorted(FUNCS)}, or (out_name, 'ntile', n); value: (out_name, fname, column"
           f"[, frame]) with fname in {sorted(set(VALUE_FUNCS) - {'lag', 'lead'} | set(MOMENT_FUNCS))}, frame in {sorted(FRAMES)}, ('rows', start, end) or ('range_between', start, end), "
           "column None for count(*) only, or (out_name, 'lag' | 'lead', column[, k[, default]]), or (out_name, 'nth_value', column, "
-          f"n[, frame]), or (out_name, fname, column1, column2[, frame]) with fname in {sorted(BIVARIATE_FUNCS)}")
+          f"n[, frame]), or (out_name, fname, column1, column2[, frame]) with fname in {sorted(BIVARIATE_FUNCS)}; an entry of "
+          f"{', '.join(NULLS_FUNCS)} may end with 'ignore_nulls' or 'respect_nulls' (the default)")
 
 
 def _names(x):
@@ -151,39 +167,40 @@ def _names(x):
     return [x] if isinstance(x, str) else list(x)
 
 
-def _parse_value(f, col_names):
+def _parse_value(f, col_names, entry):
     """(out_name, fname, column[, frame]), (out_name, 'lag' | 'lead', column[, k[, default]]) or (out_name, 'nth_value', column,
     n[, frame]) -> (out_name, code, k, column, frame code, default[, (start, end)]); frame code 0 for lag and lead, k = n for
-    nth_value, (start, end) for a ROWS_BETWEEN or RANGE_BETWEEN frame only."""
+    nth_value, (start, end) for a ROWS_BETWEEN or RANGE_BETWEEN frame only.  f is the entry without its nulls marker, entry the
+    entry as written (named in errors)."""
     name, fname, column = f[0], f[1], f[2]
     if not (column is None and fname == "count") and not (isinstance(column, str) and column in col_names):
-        raise _lib.B200Error(f"Streaming Window: {f!r}: unknown column {column!r} (one of {col_names}; None for count only)")
+        raise _lib.B200Error(f"Streaming Window: {entry!r}: unknown column {column!r} (one of {col_names}; None for count only)")
     if fname in ("lag", "lead"):
         if len(f) > 5:
-            raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} takes (out_name, {fname!r}, column[, k[, default]])")
+            raise _lib.B200Error(f"Streaming Window: {entry!r}: {fname} takes (out_name, {fname!r}, column[, k[, default]])")
         k = f[3] if len(f) > 3 else 1
         if isinstance(k, str) and k in FRAMES or isinstance(k, (tuple, list)) and len(k) == 3 and k[0] == "range_between":
-            raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} takes no frame")
+            raise _lib.B200Error(f"Streaming Window: {entry!r}: {fname} takes no frame")
         if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or not 0 <= k <= MAX_LAG:
-            raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} needs an integer k with 0 <= k < 2^31")
+            raise _lib.B200Error(f"Streaming Window: {entry!r}: {fname} needs an integer k with 0 <= k < 2^31")
         return (name, VALUE_FUNCS[fname], int(k), column, 0, f[4] if len(f) > 4 else None)
     if fname in BIVARIATE_FUNCS:
         if len(f) < 4 or not (isinstance(f[3], str) and f[3] in col_names):
-            raise _lib.B200Error(f"Streaming Window: {f!r}: unknown second column {f[3] if len(f) > 3 else None!r} (one of {col_names}), as "
+            raise _lib.B200Error(f"Streaming Window: {entry!r}: unknown second column {f[3] if len(f) > 3 else None!r} (one of {col_names}), as "
                                  f"(out_name, {fname!r}, column1, column2[, frame])")
         if len(f) > 5:
-            raise _lib.B200Error(f"Streaming Window: {f!r}: {fname} takes (out_name, {fname!r}, column1, column2[, frame])")
-        return (name, BIVARIATE_FUNCS[fname], f[3], column, *_parse_frame(f, f[4] if len(f) > 4 else "range"))
+            raise _lib.B200Error(f"Streaming Window: {entry!r}: {fname} takes (out_name, {fname!r}, column1, column2[, frame])")
+        return (name, BIVARIATE_FUNCS[fname], f[3], column, *_parse_frame(entry, f[4] if len(f) > 4 else "range"))
     if fname == "nth_value":
         nth = f[3] if len(f) > 3 else None
         if len(f) > 5 or isinstance(nth, (bool, np.bool_)) or not isinstance(nth, (int, np.integer)) or not 1 <= nth <= MAX_LAG:
-            raise _lib.B200Error(f"Streaming Window: {f!r}: nth_value takes (out_name, 'nth_value', column, n[, frame]) with an integer "
+            raise _lib.B200Error(f"Streaming Window: {entry!r}: nth_value takes (out_name, 'nth_value', column, n[, frame]) with an integer "
                                  "1 <= n < 2^31")
-        return (name, FRAME_FUNCS[fname], int(nth), column, *_parse_frame(f, f[4] if len(f) > 4 else "range"))
+        return (name, FRAME_FUNCS[fname], int(nth), column, *_parse_frame(entry, f[4] if len(f) > 4 else "range"))
     if len(f) > 4:
-        raise _lib.B200Error(f"Streaming Window: {f!r}: bad frame (one of {sorted(FRAMES)}, ('rows', start, end) or ('range_between', start, end), as (out_name, "
+        raise _lib.B200Error(f"Streaming Window: {entry!r}: bad frame (one of {sorted(FRAMES)}, ('rows', start, end) or ('range_between', start, end), as (out_name, "
                              f"{fname!r}, column[, frame]))")
-    return (name, {**VALUE_FUNCS, **MOMENT_FUNCS}[fname], 0, column, *_parse_frame(f, f[3] if len(f) > 3 else "range"))
+    return (name, {**VALUE_FUNCS, **MOMENT_FUNCS}[fname], 0, column, *_parse_frame(entry, f[3] if len(f) > 3 else "range"))
 
 
 def _parse_frame(f, frame):
@@ -285,9 +302,10 @@ def _range_kind(b, end):
     return RANGE_KINDS["preceding" if _offset(b)[1] < 0 else "following"]
 
 
-def _entry(f):
-    """A parsed value entry as the caller wrote it, with its frame spelled out (for error messages)."""
+def _entry(f, ignore_nulls=False):
+    """A parsed value entry as the caller wrote it, with its frame spelled out and its IGNORE NULLS marker (for error messages)."""
     name, code, arg, column, frame = f[:5]
+    mark = ("ignore_nulls",) if ignore_nulls else ()
     fr = _FRAME_NAMES.get(frame)
     if len(f) > 6 and frame == ROWS_BETWEEN:
         fr = ("rows", *[None if b in (UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING) else b for b in f[6]])
@@ -295,13 +313,15 @@ def _entry(f):
         fr = ("range_between", *f[6])
     if code in BIVARIATE_FUNCS.values():
         return (name, _VALUE_NAMES[code], column, arg, fr)
-    return (name, _VALUE_NAMES[code], column, fr) if code != FRAME_FUNCS["nth_value"] else (name, "nth_value", column, arg, fr)
+    if code in (VALUE_FUNCS["lag"], VALUE_FUNCS["lead"]):
+        return (name, _VALUE_NAMES[code], column, arg, f[5], *mark)
+    return (name, _VALUE_NAMES[code], column, fr, *mark) if code != FRAME_FUNCS["nth_value"] else (name, "nth_value", column, arg, fr, *mark)
 
 
-def _default_bits(f, ct):
+def _default_bits(f, ct, ignore_nulls=False):
     """Bits of lag / lead's default in the column's numpy dtype; raises unless it round-trips exactly."""
     default, dt = f[5], np_dtype_of(ct)
-    entry = (f[0], _VALUE_NAMES[f[1]], f[3], f[2], default)
+    entry = _entry(f, ignore_nulls)
     try:
         with warnings.catch_warnings(), np.errstate(all="ignore"):
             warnings.simplefilter("ignore")
@@ -317,18 +337,23 @@ def _default_bits(f, ct):
 
 def _parse_funcs(funcs, col_names):
     """Ranking entries -> (out_name, code, n); value entries -> (out_name, code, k, column, frame code, default), with a
-    seventh field (start, end) for a ROWS_BETWEEN or RANGE_BETWEEN frame."""
-    out = []
+    seventh field (start, end) for a ROWS_BETWEEN or RANGE_BETWEEN frame.  Returns those and one IGNORE NULLS flag per entry: a
+    trailing "ignore_nulls" / "respect_nulls" (the last element, at index 3 or later) is removed before the entry is parsed."""
+    out, nulls = [], []
     for f in funcs:
         f = tuple(f)
+        marker = f[-1] if len(f) > 3 and isinstance(f[-1], str) and f[-1] in NULLS_MARKERS else None
         value = isinstance(f[1] if len(f) > 1 else None, str) and (f[1] in VALUE_FUNCS or f[1] in FRAME_FUNCS or f[1] in MOMENT_FUNCS
                                                                    or f[1] in BIVARIATE_FUNCS)
         if (len(f) < 2 or not isinstance(f[0], str) or not isinstance(f[1], str) or f[1] not in FUNCS and not value
                 or value and len(f) < 3):
             raise _lib.B200Error(f"Streaming Window: unknown window function {f!r} ({_FORMS})")
         name, fname = f[0], f[1]
+        if marker is not None and fname not in NULLS_FUNCS:
+            raise _lib.B200Error(f"Streaming Window: {f!r}: {marker!r} takes one of {list(NULLS_FUNCS)}")
+        nulls.append(marker == "ignore_nulls")
         if value:
-            out.append(_parse_value(f, col_names))
+            out.append(_parse_value(f[:-1] if marker is not None else f, col_names, f))
             continue
         if fname == "ntile":
             if len(f) != 3 or isinstance(f[2], bool) or not isinstance(f[2], int) or f[2] < 1:
@@ -350,7 +375,7 @@ def _parse_funcs(funcs, col_names):
         raise _lib.B200Error(f"Streaming Window: output names {clash} clash with input columns")
     if len(col_names) + len(out) > MAX_COLS:
         raise _lib.B200Error(f"Streaming Window: {len(col_names)} input columns and {len(out)} functions exceed {MAX_COLS} output columns")
-    return out
+    return out, nulls
 
 
 class WindowState(SortState):
@@ -374,15 +399,16 @@ class WindowState(SortState):
             raise _lib.B200Error("Streaming Window: ascending and na_position need one value or one entry per ORDER BY key")
         if any(p not in ("first", "last") for p in nap):
             raise _lib.B200Error(f"Streaming Window: na_position must be 'first' or 'last' (got {nap})")
-        parsed = _parse_funcs(funcs, col_names)
-        for f in parsed:
+        parsed, nulls = _parse_funcs(funcs, col_names)
+        for f, ign in zip(parsed, nulls):
             if len(f) > 6 and f[4] == RANGE_BETWEEN and len(order) != 1 and any(b not in (None, 0) for b in f[6]):
-                raise _lib.B200Error(f"Streaming Window: {_entry(f)!r}: a range offset (k PRECEDING / FOLLOWING) needs exactly one ORDER "
+                raise _lib.B200Error(f"Streaming Window: {_entry(f, ign)!r}: a range offset (k PRECEDING / FOLLOWING) needs exactly one ORDER "
                                      f"BY key (got {order})")
         super().__init__(operator_id, None, 0, keys, [True] * len(part) + asc, ["last"] * len(part) + nap, col_names, parallel,
                          output_batch_size, device, stream, process_group, full=True)
         self.partition_by, self.order_by = part, order
         self.funcs = parsed
+        self.ignore_nulls = nulls  # per function: IGNORE NULLS
         self.out_names += [f[0] for f in parsed]
         self.out_order += list(range(len(self.phys), len(self.phys) + len(parsed)))
         self.descs = None
@@ -393,7 +419,7 @@ class WindowState(SortState):
         for sum, mean, var or std of a temporal column, a bivariate function with a temporal column in either position and a lag /
         lead default that does not round-trip through the column's dtype."""
         out = []
-        for f in self.funcs:
+        for f, ign in zip(self.funcs, self.ignore_nulls):
             if len(f) == 3:
                 out.append((f[1], -1, 0, 0, f[2], 0))
                 continue
@@ -414,7 +440,7 @@ class WindowState(SortState):
                 what = "var and std" if moment else "sum and mean"
                 raise _lib.B200Error(f"Streaming Window: {entry!r}: {what} need an integer, bool or float column, not a temporal one")
             valid = default is not None
-            out.append((code, self.phys.index(self.col_names.index(column)), frame, int(valid), arg, _default_bits(f, ct) if valid else 0))
+            out.append((code, self.phys.index(self.col_names.index(column)), frame, int(valid), arg, _default_bits(f, ct, ign) if valid else 0))
         return out
 
     def frames(self):
@@ -430,7 +456,7 @@ class WindowState(SortState):
         the key: integers take an integer, floats an integer or float that a double holds exactly, DATETIME / TIMEDELTA a
         timedelta, DATE a timedelta of whole days; a bool key takes none."""
         out = []
-        for f in self.funcs:
+        for f, ign in zip(self.funcs, self.ignore_nulls):
             if not (len(f) > 6 and f[4] == RANGE_BETWEEN):
                 out.append((RANGE_KINDS["unbounded_preceding"], RANGE_KINDS["unbounded_following"], 0, 0))
                 continue
@@ -454,7 +480,7 @@ class WindowState(SortState):
                     want = ("an integer" if ct in _INTEGER else "an int or float exactly representable as a double"
                             if ct in (CTypes.FLOAT32, CTypes.FLOAT64) else "a timedelta" if ct in (CTypes.DATETIME, CTypes.TIMEDELTA)
                             else "a timedelta of whole days" if ct == CTypes.DATE else "no offset (an integer, float or temporal key is needed)")
-                    raise _lib.B200Error(f"Streaming Window: {_entry(f)!r}: range offset {b!r} does not fit ORDER BY key {key!r} of "
+                    raise _lib.B200Error(f"Streaming Window: {_entry(f, ign)!r}: range offset {b!r} does not fit ORDER BY key {key!r} of "
                                          f"type {_CT_NAMES.get(ct, ct)}: it takes {want}")
             out.append((kinds[0], kinds[1], bits[0], bits[1]))
         return out
@@ -478,8 +504,9 @@ class WindowState(SortState):
         rs = ffi.new("b200_window_range[]", len(self.descs))
         for d, (sk, ek, sb, eb) in zip(rs, self.rdescs):
             d.start_kind, d.end_kind, d.start_bits, d.end_bits = sk, ek, sb, eb
-        h = L.b200_window_state_init_bivariate(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs,
-                                               frs, rs, len(self.descs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
+        nulls = ffi.new("int32_t[]", [int(x) for x in self.ignore_nulls])
+        h = L.b200_window_state_init_nulls(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs, frs, rs,
+                                           nulls, len(self.descs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
         return _lib.check_ptr(h, "init_window_state")
 
 
@@ -494,16 +521,20 @@ def init_window_state(operator_id, partition_by, order_by, ascending, na_positio
     default]]) (k = 1 and default None, NA, by default), (out_name, "nth_value", column, n[, frame]), or (out_name, fname,
     column[, frame]) with fname in MOMENT_FUNCS (var, std, var_pop, std_pop) and any frame sum takes, or (out_name, fname, y, x[,
     frame]) with fname in BIVARIATE_FUNCS (covar_samp, covar_pop, corr, regr_slope, regr_intercept; SQL's argument order) and
-    any frame sum takes.
+    any frame sum takes.  An entry of first_value, last_value, nth_value, lag or lead may end with "ignore_nulls" (IGNORE NULLS)
+    or "respect_nulls" (the default).
     Examples, a 7-row moving average: ("ma7", "mean", "x", ("rows", -6, 0)); a one-hour time window over a DATETIME ORDER BY
     key: ("s1h", "sum", "amount", ("range_between", -pd.Timedelta("1h"), 0)); a 20-row rolling standard deviation (a Bollinger
     band's width): ("sd20", "std", "x", ("rows", -19, 0)); the population variance of the partition: ("vp", "var_pop", "x",
     "partition"); a 60-row rolling beta of r on the market return mr and their correlation: ("beta", "regr_slope", "r", "mr",
-    ("rows", -59, 0)), ("rho", "corr", "r", "mr", ("rows", -59, 0)).
+    ("rows", -59, 0)), ("rho", "corr", "r", "mr", ("rows", -59, 0)); the last known reading per sensor (a per-group ffill, ordered
+    by time): ("last", "last_value", "x", "rows", "ignore_nulls"); the previous reading that is not missing: ("prev", "lag", "x",
+    1, None, "ignore_nulls").
     Raises B200Error for an unknown function, duplicate output names or names that clash with an input column, keys that are
     missing or not distinct, a key count outside 1..4, a bad na_position, ntile n < 1, an unknown value column, a bad frame or
     frame bound, a frame on lag or lead, k outside [0, 2^31), nth_value n outside [1, 2^31), a range offset without exactly one
-    ORDER BY key, a missing or unknown second column of a bivariate function; and at the first consume call for sum, mean, var
+    ORDER BY key, a missing or unknown second column of a bivariate function, an "ignore_nulls" / "respect_nulls" marker on
+    another function; and at the first consume call for sum, mean, var
     or std of a temporal column, a bivariate function with a temporal column in either position, a lag / lead default that the
     column's dtype cannot hold exactly or a range offset whose type does not fit the ORDER BY key."""
     return WindowState(operator_id, partition_by, order_by, ascending, na_position, funcs, col_names, parallel, output_batch_size,

@@ -414,6 +414,26 @@ void* b200_window_state_init_bivariate(int64_t operator_id, const int8_t* c_type
                                        const b200_window_range* ranges, int32_t n_funcs, int64_t output_batch_size, int32_t device,
                                        void* stream);
 
+/* b200_window_state_init_bivariate plus one IGNORE NULLS flag per function: ignore_nulls[i] != 0 marks funcs[i] IGNORE NULLS,
+ * 0 RESPECT NULLS (the definitions above); ignore_nulls may be NULL, all RESPECT NULLS.  A non-zero flag is accepted for codes
+ * 11 first_value, 12 last_value, 13 lag, 14 lead and 15 nth_value only; on any other code it fails here (NULL, last error set).
+ * Under IGNORE NULLS a cell is null exactly when count does not count it: its validity is clear or it is a float NaN (RESPECT
+ * NULLS first_value returns a NaN as a valid cell; IGNORE NULLS skips it, as pandas' ffill / bfill do).  With row i's frame
+ * [lo, hi] and partition [P, pe) as RESPECT NULLS computes them (every frame 1..5, the same empty-frame rule):
+ *   first_value  the first non-null cell in [lo, hi]; NA if none.
+ *   last_value   the last non-null cell in [lo, hi]; NA if none.
+ *   nth_value    the n-th non-null cell in [lo, hi] (FROM FIRST); NA if there are fewer than n.
+ *   lag          the k-th non-null cell before row i within [P, i); the default if there are fewer than k.
+ *   lead         the k-th non-null cell after row i within (i, pe); the default if there are fewer than k.
+ * lag / lead with k = 0 are the row itself, as under RESPECT NULLS.  The result keeps the chosen cell's bits (-0.0 stays -0.0);
+ * the column's type, nullable.  Results depend only on the sorted positions: bit-identical across runs and batch splits.
+ * b200_window_state_init_bivariate is this entry with ignore_nulls NULL. */
+void* b200_window_state_init_nulls(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                                   int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                                   const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
+                                   const b200_window_range* ranges, const int32_t* ignore_nulls, int32_t n_funcs,
+                                   int64_t output_batch_size, int32_t device, void* stream);
+
 /* The build-consume entry of _sort.cpp: filters a DEVICE-resident batch (same schema as the state) against the current cutoff on
  * the device (full sort: appends it to the chunk store); on is_last reduces to the final rows (full sort: sorts every row).
  * Returns 1 after is_last, 0 otherwise, < 0 on error; *request_input = 1. */
