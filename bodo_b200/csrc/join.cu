@@ -197,15 +197,18 @@ __global__ void join_fill_groups_kernel(const uint32_t* row_slot, int64_t n, con
 // mode 0: inner / outer join; 1: anti join (a probe row goes out, once and with NULL build columns, iff it has NO match:
 // the is_anti_join template of the reference's probe, _join.cpp:763-767); 2: mark join (every probe row goes out once, without
 // build columns; mark[i] says whether it has a match, _join.cpp:3668-3693)
+// key_reject: the probe key is int64 / DATETIME / TIMEDELTA and the build key UINT64, or the other way round.  Keys join by value, so
+// a valid probe key with its top bit set (a negative value, or a uint64 of at least 2^63) has no partner; it is not an NA key.
 template <bool FK>
 __global__ void join_probe_count_kernel(const void* key_data, int key_ctype, const uint8_t* key_valid, int64_t n,
                                         const long long* tkeys, uint64_t cap, const SlotInfo* info, int probe_outer,
-                                        uint32_t* pslot, uint32_t* pcnt, int na_equal, int mode, uint8_t* mark) {
+                                        uint32_t* pslot, uint32_t* pcnt, int na_equal, int mode, uint8_t* mark, int key_reject) {
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
         uint32_t s;
         const JoinKey jk = load_join_key<FK>(key_data, key_ctype, i, bit_valid(key_valid, i));
         if (jk.na) s = na_equal ? (uint32_t)cap : J_NONE;
+        else if (!FK && key_reject && jk.key < 0) s = J_NONE;
         else s = jk.key == J_EMPTY ? (uint32_t)cap + 1 : j_find(tkeys, cap, jk.key);
         uint32_t c = s == J_NONE ? 0 : info[s].cnt;
         if (c == 0) s = J_NONE;
@@ -342,6 +345,7 @@ struct FastProbeArgs {
     unsigned long long* cursor;
     int n_b, n_p;
     int na_equal;
+    int key_reject;                        // as in join_probe_count_kernel
     int b_field[J_MAX_COLS];               // kept build col -> payload field index, -1 = the key column
     const uint8_t* b_valid[J_MAX_COLS]; int b_size[J_MAX_COLS];
     const void* p_data[J_MAX_COLS]; const uint8_t* p_valid[J_MAX_COLS]; int p_size[J_MAX_COLS];
@@ -382,6 +386,7 @@ __global__ void __launch_bounds__(256) join_probe_fast_kernel(const __grid_const
                 const JoinKey jk = load_join_key<FK>(a.key_data, a.key_ctype, i, true);  // bits under a NULL too: the output's validity hides them
                 key[r] = jk.key; bits[r] = jk.bits;
                 if (!kvalid[r] || jk.na) { if (a.na_equal) { Slot16 e = a.slots[a.cap]; match[r] = e.cnt > 0; brow[r] = e.first; } }
+                else if (!FK && a.key_reject && key[r] < 0) {}  // a value the build key's type cannot hold: no partner
                 else if (key[r] == J_EMPTY) { Slot16 e = a.slots[a.cap + 1]; match[r] = e.cnt > 0; brow[r] = e.first; }
                 else {
                     uint64_t s = j_hash_slot(key[r], mask);
@@ -647,6 +652,14 @@ __device__ __forceinline__ bool mk_equal_build(const KeySet& bk, uint32_t row, c
     for (int j = 0; j < MAX_HASH_KEYS; j++) eq = eq && (j >= bk.n_keys || o.key[j] == r.key[j]);
     return eq;
 }
+// Bit j of `key_reject`: key position j compares an int64 / DATETIME / TIMEDELTA column with a UINT64 one.  A valid key there with
+// its top bit set is a value the other column's type cannot hold, so the row has no partner (NA columns read as 0).
+__device__ __forceinline__ bool mk_rejected(const MKRow& r, uint32_t key_reject) {
+    bool x = false;
+#pragma unroll
+    for (int j = 0; j < MAX_HASH_KEYS; j++) x = x || ((key_reject >> j & 1) && r.key[j] < 0);
+    return x;
+}
 __device__ __forceinline__ uint64_t mk_slot(uint64_t h, uint64_t mask) { return (h >> 32) & mask; }
 __device__ __forceinline__ uint32_t mk_tag(uint64_t h) { return (uint32_t)h; }
 
@@ -678,13 +691,13 @@ __global__ void join_insert_count_mk_kernel(const KeySet bk, int64_t n, unsigned
 // join_probe_count_kernel for a multi-column key: same outputs (pslot, pcnt, mark) in modes 0, 1 and 2
 __global__ void join_probe_count_mk_kernel(const KeySet pk, const KeySet bk, int64_t n, const unsigned long long* __restrict__ table,
                                            uint64_t cap, const SlotInfo* info, int probe_outer, uint32_t* pslot, uint32_t* pcnt,
-                                           int na_equal, int mode, uint8_t* mark) {
+                                           int na_equal, int mode, uint8_t* mark, uint32_t key_reject) {
     const uint64_t mask = cap - 1;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
         const MKRow r = mk_row<false>(pk, i);
         uint32_t s = J_NONE;
-        if (!r.na || na_equal) {
+        if ((!r.na || na_equal) && !mk_rejected(r, key_reject)) {
             const uint64_t h = mk_hash(r, pk.n_keys);
             for (uint64_t t = mk_slot(h, mask);; t = (t + 1) & mask) {
                 const unsigned long long w = __ldg(table + t);
@@ -747,11 +760,11 @@ struct MKBounds { long long v[2 * MAX_HASH_KEYS]; };
 // clears its use_minmax bit and use_bloom.  An NA column drops the row unless NA joins NA; then it skips the bounds and is hashed
 // into the bloom test as the build side hashes it.
 __global__ void join_runtime_filter_kernel(const KeySet pk, int64_t n, int na_equal, const uint32_t* bloom, uint64_t n_blocks,
-                                           const MKBounds b, uint32_t use_minmax, int use_bloom, uint8_t* keep) {
+                                           const MKBounds b, uint32_t use_minmax, int use_bloom, uint8_t* keep, uint32_t key_reject) {
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
         const MKRow r = mk_row<false>(pk, i);
-        bool k = !r.na || na_equal;
+        bool k = (!r.na || na_equal) && !mk_rejected(r, key_reject);
 #pragma unroll
         for (int j = 0; j < MAX_HASH_KEYS; j++) {
             if (j >= pk.n_keys || !(use_minmax >> j & 1) || (r.na >> j & 1)) continue;
@@ -820,6 +833,7 @@ class JoinState {
     bool na_equal = false;  // is_na_equal of the reference's HashJoinState
     int n_keys = 1;         // key columns: the first n_keys of each side; more than one always takes the CSR form (the _mk kernels)
     bool float_key = false; // float64 or float32 key column (n_keys == 1): every FK-templated key kernel runs its FK instantiation
+    uint32_t key_reject = 0;  // bit j: probe key position j differs from the build key in signedness at 8 bytes (signedness_differs)
     int64_t output_batch_size;
     // build side
     std::vector<GrowCol> bcol, bvalid;  // data; validity as one byte per row (empty when the column has none so far)
@@ -881,6 +895,8 @@ class JoinState {
         B200_REQUIRE(np >= n_keys, "b200 join: fewer columns than key columns");
         for (int j = 0; j < n_keys; j++) require_key_type(j, p_ct[j], "probe");
         B200_REQUIRE(ctype_size(b_ct[0]) == ctype_size(p_ct[0]), "b200 join: build and probe key widths differ");
+        key_reject = 0;
+        for (int j = 0; j < n_keys; j++) key_reject |= signedness_differs(p_ct[j], b_ct[j]) ? 1u << j : 0u;
         out_data.resize(n_b + np); out_vbytes.resize(n_b + np); out_bitmap.resize(n_b + np);
         if ((int)stage_data.size() < std::max(n_b, np)) { stage_data.resize(std::max(n_b, np)); stage_valid.resize(std::max(n_b, np)); }
     }
@@ -894,6 +910,13 @@ class JoinState {
         if (ctype_is_float(b_ct[j]) || ctype_is_float(ct))
             B200_REQUIRE(ct == b_ct[j], "b200 join: " + pos + types + "; float keys join float keys of the same type");
         if (n_keys > 1) B200_REQUIRE(ctype_size(ct) == ctype_size(b_ct[j]), "b200 join: " + pos + types + "; integer keys join integer keys of the same width");
+    }
+    // Integer keys join by value, as pandas merge does.  Up to 4 bytes the key load sign- or zero-extends each side to int64, which
+    // is the value.  At 8 bytes an int64 / DATETIME / TIMEDELTA key and a UINT64 key are the same value exactly when their bits are
+    // equal and the top bit is clear, so the probe side rejects a key with that bit set (key_reject) and any build key with it is
+    // then unreachable.
+    static bool signedness_differs(int probe_ct, int build_ct) {
+        return ctype_size(probe_ct) == 8 && !ctype_is_float(probe_ct) && !ctype_is_float(build_ct) && (probe_ct == CT_UINT64) != (build_ct == CT_UINT64);
     }
     KeySet build_keys() const {
         KeySet k{};
@@ -962,7 +985,7 @@ class JoinState {
         B200_REQUIRE(t->device == device, "b200 join: runtime_filter takes a device-resident table on the state's device");
         KeySet pk{};
         pk.n_keys = n_keys;
-        uint32_t mm = 0;
+        uint32_t mm = 0, reject = 0;
         bool all = true, any = false;
         for (int j = 0; j < n_keys; j++) {
             const int c = key_cols[j];
@@ -973,6 +996,7 @@ class JoinState {
             B200_REQUIRE(ctype_size(t->cols[c].c_type) == ctype_size(b_ct[j]), "b200 join: runtime_filter: key column type differs from the build key");
             pk.data[j] = t->cols[c].data; pk.valid[j] = t->cols[c].validity; pk.ctype[j] = t->cols[c].c_type;
             if (use_minmax[j]) mm |= 1u << j;
+            if (signedness_differs(pk.ctype[j], b_ct[j])) reject |= 1u << j;
         }
         B200_CUDA(cudaSetDevice(device));
         const int64_t n = t->n_rows;
@@ -985,7 +1009,7 @@ class JoinState {
         MKBounds b;
         std::copy(key_bounds, key_bounds + 2 * MAX_HASH_KEYS, b.v);
         join_runtime_filter_kernel<<<grid_for(n), 256, 0, stream>>>(pk, n, na_equal ? 1 : 0, d_bloom.as<uint32_t>(), bloom_blocks, b, mm,
-                                                                    use_bloom && all ? 1 : 0, keep);
+                                                                    use_bloom && all ? 1 : 0, keep, reject);
         launches++;
         B200_CUDA(cudaGetLastError());
         filter_rows_in += n;
@@ -1190,8 +1214,9 @@ class JoinState {
         d_cursor.ensure(8);
         B200_CUDA(cudaMemsetAsync(d_cursor.p, 0, 8, stream));
         // inline-payload variant: every column of this batch 8 bytes wide and bitmap-free, 1..4 kept probe columns
-        // (a nullable-typed column without a bitmap still gets one)
-        bool inl = form == TableForm::SLOT32 && valid[0] == nullptr && nkp >= 1 && nkp <= J_INL_MAX_P && nkb <= 4;
+        // (a nullable-typed column without a bitmap still gets one); the inline kernel compares key bits, so a probe key of the
+        // other signedness takes the fast kernel
+        bool inl = form == TableForm::SLOT32 && valid[0] == nullptr && nkp >= 1 && nkp <= J_INL_MAX_P && nkb <= 4 && !key_reject;
         for (const OutCol& c : cols) inl = inl && c.size == 8 && !c.nullable;
         const int gridp = (int)std::min<int64_t>((int64_t)sms * 8, (n + 1023) / 1024);
         if (inl) {
@@ -1214,7 +1239,7 @@ class JoinState {
             FastProbeArgs f{};
             f.n_probe = n; f.key_data = data[0]; f.key_ctype = p_ct[0]; f.key_valid = valid[0];
             f.slots = d_slots16.as<Slot16>(); f.cap = cap; f.bpack = d_bpack.as<unsigned long long>(); f.n_fields = std::max(n_b - 1, 1);
-            f.cursor = d_cursor.as<unsigned long long>(); f.n_b = nkb; f.n_p = nkp; f.na_equal = na_equal ? 1 : 0;
+            f.cursor = d_cursor.as<unsigned long long>(); f.n_b = nkb; f.n_p = nkp; f.na_equal = na_equal ? 1 : 0; f.key_reject = (int)key_reject;
             for (int k = 0; k < (int)cols.size(); k++) {
                 const OutCol& c = cols[k];
                 if (c.is_b) {
@@ -1245,12 +1270,13 @@ class JoinState {
             if (n_keys > 1)
                 join_probe_count_mk_kernel<<<grid_for(n), 256, 0, stream>>>(probe_keys(data, valid), build_keys(), n, d_tkeys.as<unsigned long long>(), cap,
                                                                             d_info.as<SlotInfo>(), probe_outer ? 1 : 0, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(),
-                                                                            na_equal ? 1 : 0, anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr);
+                                                                            na_equal ? 1 : 0, anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr,
+                                                                            key_reject);
             else
                 with_key([&](auto fk) {
                     join_probe_count_kernel<fk><<<grid_for(n), 256, 0, stream>>>(data[0], p_ct[0], valid[0], n, d_tkeys.as<long long>(), cap, d_info.as<SlotInfo>(),
                                                                                  probe_outer ? 1 : 0, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(), na_equal ? 1 : 0,
-                                                                                 anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr);
+                                                                                 anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr, (int)key_reject);
                 });
             launches++;
             B200_CUDA(cudaMemsetAsync(d_pcnt.as<uint32_t>() + n, 0, 4, stream));

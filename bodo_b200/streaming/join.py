@@ -145,6 +145,9 @@ def join_probe_consume_batch(join_state: JoinState, table: Table, is_last: bool,
         kb_logical = []  # a mark join does not output build table columns
     kb = [st.build_indices.index(i) for i in kb_logical]
     kp = [st.probe_indices.index(i) for i in kp_logical]
+    if not st.is_mark_join and not kb and not kp:  # a batch is a list of columns: without one it could not say how many rows it has
+        raise _lib.B200Error(f"join_probe_consume_batch: used_cols={used_cols!r} keeps no column; keep at least one build or probe "
+                             "column (a mark join always has its mark column)")
     names = [st.build_names[j] for j in kb] + [phys.names[j] for j in kp]
     # unique output names (a key named the same on both sides appears twice, like pandas' _x/_y without renaming)
     seen, uniq = set(), []
