@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "expr.cuh"
 
 namespace b200 {
 
@@ -783,6 +784,85 @@ __global__ void join_runtime_filter_kernel(const KeySet pk, int64_t n, int na_eq
     }
 }
 
+// ---- non-equi condition (the reference's cond_func: join.py:991-1100, join_state_init_py_entry; cuDF's filter_join_indices) ----
+// A candidate pair (probe row p, build row b of p's key group) passes when the condition program (expr.cuh) evaluates to a valid,
+// true value.  The program's column argument c < J_MAX_COLS reads build column c at row b (validity one byte per row, nullptr =
+// all valid), J_MAX_COLS + c reads probe column c at row p (Arrow bitmap).  A state with a condition always takes the CSR form:
+// join_probe_count_kernel / _mk in mode 0 without probe_outer give each probe row its slot, then the two kernels below evaluate
+// the condition on every candidate, once to count and once to gather.
+struct CondArgs {
+    ExprInstr prog[EX_MAX_INSTR];
+    const void* b_data[J_MAX_COLS]; const uint8_t* b_valid[J_MAX_COLS]; int b_ct[J_MAX_COLS];
+    const void* p_data[J_MAX_COLS]; const uint8_t* p_valid[J_MAX_COLS]; int p_ct[J_MAX_COLS];
+};
+__device__ __forceinline__ bool cond_pass(const CondArgs& a, int64_t p, uint32_t b) {
+    const ExprVal v = expr_run(a.prog, 0, [&](int64_t arg) {
+        const int c = (int)arg;
+        if (c < J_MAX_COLS) return expr_load(a.b_data[c], a.b_ct[c], b, !a.b_valid[c] || a.b_valid[c][b]);
+        const int q = c - J_MAX_COLS;
+        return expr_load(a.p_data[q], a.p_ct[q], p, bit_valid(a.p_valid[q], p));
+    });
+    return v.valid && ev_true(v);
+}
+// build row of candidate q (0 <= q < c) of key group s, which has c rows
+__device__ __forceinline__ uint32_t cand_row(const SlotInfo* info, const unsigned long long* goffs, const uint32_t* groups, uint32_t s,
+                                             uint32_t c, uint32_t q) {
+    return c == 1 ? info[s].first : groups[goffs[s] + q];
+}
+// condition pass A: each probe row's output count for the join kind.  mode 0 (inner / outer): its passing pairs, or one NULL-build
+// row for a probe_outer row without one; 1 (anti): one row iff no pair passes; 2 (mark): one row, mark[i] = some pair passes.
+// pairs[0] += candidate pairs evaluated, pairs[1] += pairs that passed.
+__global__ void __launch_bounds__(256) join_cond_count_kernel(const __grid_constant__ CondArgs a, int64_t n, const uint32_t* pslot,
+                                                              const SlotInfo* info, const unsigned long long* goffs, const uint32_t* groups,
+                                                              int probe_outer, int mode, uint32_t* pcnt, uint8_t* mark, unsigned long long* pairs) {
+    unsigned long long n_eval = 0, n_pass = 0;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
+        const uint32_t s = pslot[i];
+        const uint32_t c = s == J_NONE ? 0 : info[s].cnt;
+        uint32_t k = 0;
+        for (uint32_t q = 0; q < c; q++) k += cond_pass(a, i, cand_row(info, goffs, groups, s, c, q)) ? 1 : 0;
+        n_eval += c; n_pass += k;
+        if (mode == 1) pcnt[i] = k ? 0u : 1u;
+        else if (mode == 2) { pcnt[i] = 1u; mark[i] = k ? 1 : 0; }
+        else pcnt[i] = k ? k : (probe_outer ? 1u : 0u);
+    }
+    for (int d = 16; d; d >>= 1) { n_eval += __shfl_xor_sync(0xffffffffu, n_eval, d); n_pass += __shfl_xor_sync(0xffffffffu, n_pass, d); }
+    if ((threadIdx.x & 31) == 0 && n_eval) { atomicAdd(pairs, n_eval); atomicAdd(pairs + 1, n_pass); }
+}
+// condition pass B: the passing pairs of a probe row go to its output rows in candidate order (build_outer: they mark their build
+// row matched); a row the count gave an output row without a passing pair (probe_outer, anti, mark) goes out NULL-extended.
+__global__ void __launch_bounds__(256) join_cond_gather_kernel(const __grid_constant__ GatherArgs g, const __grid_constant__ CondArgs a, int mode) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < g.n_probe; i += stride) {
+        const unsigned long long o = g.poff[i];
+        if (g.poff[i + 1] == o) continue;
+        uint32_t k = 0;
+        const uint32_t s = g.pslot[i];
+        const uint32_t c = mode != 0 || s == J_NONE ? 0 : g.info[s].cnt;
+        for (uint32_t q = 0; q < c; q++) {
+            const uint32_t brow = cand_row(g.info, g.goffs, g.groups, s, c, q);
+            if (!cond_pass(a, i, brow)) continue;
+            const int64_t orow = (int64_t)(o + k++);
+            if (g.bmatched) g.bmatched[brow] = 1;
+            for (int j = 0; j < g.n_b; j++) {
+                copy_cell(g.ob_data[j], orow, g.b_data[j], brow, g.b_size[j]);
+                if (g.ob_valid[j]) g.ob_valid[j][orow] = g.b_valid[j] ? g.b_valid[j][brow] : 1;
+            }
+            for (int j = 0; j < g.n_p; j++) {
+                copy_cell(g.op_data[j], orow, g.p_data[j], i, g.p_size[j]);
+                if (g.op_valid[j]) g.op_valid[j][orow] = bit_valid(g.p_valid[j], i) ? 1 : 0;
+            }
+        }
+        if (k) continue;
+        for (int j = 0; j < g.n_b; j++) { zero_item(g.ob_data[j], (int64_t)o, g.b_size[j]); g.ob_valid[j][o] = 0; }
+        for (int j = 0; j < g.n_p; j++) {
+            copy_cell(g.op_data[j], (int64_t)o, g.p_data[j], i, g.p_size[j]);
+            if (g.op_valid[j]) g.op_valid[j][o] = bit_valid(g.p_valid[j], i) ? 1 : 0;
+        }
+    }
+}
+
 // ================================================================================================
 // When `buf` holds fewer than `need` bytes, replaces it by a buffer of max(need, alloc) bytes that keeps its first `keep` bytes.
 static void grow_keep(DevBuf& buf, size_t need, size_t keep, cudaStream_t st, size_t alloc = 0) {
@@ -852,6 +932,12 @@ class JoinState {
     // is_anti_join template argument of the probe)
     bool mark = false, anti = false;
     DevBuf d_mark, d_mark_valid;
+    // non-equi condition (set_condition, before the first build batch): one expression over build column c (arg c) and probe
+    // column c (arg J_MAX_COLS + c); empty = none.  d_cond_pairs: candidate pairs evaluated, pairs passed (metrics 8, 9)
+    std::vector<ExprInstr> cond;
+    DevBuf d_cond_pairs;
+    unsigned long long* h_cond_pairs = nullptr;
+    int64_t cond_evaluated = 0, cond_passed = 0;
     // runtime join filter, built on demand from the build keys
     DevBuf d_bloom, d_minmax;
     uint64_t bloom_blocks = 0;
@@ -897,10 +983,14 @@ class JoinState {
         B200_REQUIRE(ctype_size(b_ct[0]) == ctype_size(p_ct[0]), "b200 join: build and probe key widths differ");
         key_reject = 0;
         for (int j = 0; j < n_keys; j++) key_reject |= signedness_differs(p_ct[j], b_ct[j]) ? 1u << j : 0u;
+        for (const ExprInstr& in : cond)
+            B200_REQUIRE(in.op != EX_COL || in.arg < J_MAX_COLS || in.arg - J_MAX_COLS < np,
+                         "b200 join: the condition reads probe column " + std::to_string(in.arg - J_MAX_COLS) + " and the probe table has " +
+                             std::to_string(np) + " columns");
         out_data.resize(n_b + np); out_vbytes.resize(n_b + np); out_bitmap.resize(n_b + np);
         if ((int)stage_data.size() < std::max(n_b, np)) { stage_data.resize(std::max(n_b, np)); stage_valid.resize(std::max(n_b, np)); }
     }
-    ~JoinState() { cudaSetDevice(device); scratch_set_stream(stream); cudaStreamSynchronize(stream); pinned_release(h_word, 8); }
+    ~JoinState() { cudaSetDevice(device); scratch_set_stream(stream); cudaStreamSynchronize(stream); pinned_release(h_word, 8); pinned_release(h_cond_pairs, 16); }
 
     // Key position j: a float key joins a float key of the same type only; integer keys join integer keys of the same width (for
     // one key column the callers check the width with their own message)
@@ -952,6 +1042,17 @@ class JoinState {
         B200_REQUIRE(!(is_mark && is_anti), "b200 join: a join is a mark join or an anti join, not both");
         B200_REQUIRE(!(is_mark || is_anti) || !build_outer, "b200 join: mark / anti joins do not emit build rows (build_table_outer must be false)");
         mark = is_mark; anti = is_anti;
+    }
+    // The non-equi condition: one expression (ending in EX_END) over the columns of both sides.  Build columns are checked here,
+    // probe columns here when the probe schema is known and otherwise when the first probe batch brings it.
+    void set_condition(const ExprInstr* prog, int n_instr) {
+        B200_REQUIRE(n_build == 0 && !build_final, "b200 join: the condition must be set before the first build batch");
+        const std::string who = "b200 join: set_condition";
+        expr_validate(prog, n_instr, [&](int64_t c) {
+            return (c >= 0 && c < n_b) || (c >= J_MAX_COLS && c < 2 * J_MAX_COLS && (n_p == 0 || c - J_MAX_COLS < n_p));
+        }, who);
+        for (int i = 0; i + 1 < n_instr; i++) B200_REQUIRE(prog[i].op != EX_END, who + ": the condition is one expression (one END, at the end)");
+        cond.assign(prog, prog + n_instr);
     }
 
     // ---- runtime join filter ----
@@ -1117,7 +1218,7 @@ class JoinState {
         while (cap < 2ull * (uint64_t)n_build) cap <<= 1;
         uint64_t n_slots = cap + 2;
         // the unique-key tables (Slot32, Slot16) hold one int64 key: a multi-column key always takes the CSR form
-        if (n_keys == 1 && !mark && !anti && try_inline_build(n_slots)) {
+        if (n_keys == 1 && !mark && !anti && cond.empty() && try_inline_build(n_slots)) {
             form = TableForm::SLOT32; inline_builds++;
             build_final = true;
             return;
@@ -1151,12 +1252,17 @@ class JoinState {
                 launches++;
             }
             d_cnt_multi.release(); d_fill.release(); d_row_slot.release();
-            if (n_keys == 1 && n_multi == 0 && !build_outer && !probe_outer && !mark && !anti) {
+            if (n_keys == 1 && n_multi == 0 && !build_outer && !probe_outer && !mark && !anti && cond.empty()) {
                 // every key (incl. the NA / marker groups) has exactly one build row: set up the fused probe path
                 form = TableForm::SLOT16;
                 setup_slot16();
                 d_tkeys.release(); d_info.release();  // the general-path table is not needed any more
             }
+        }
+        if (!cond.empty()) {
+            d_cond_pairs.alloc(16);
+            B200_CUDA(cudaMemsetAsync(d_cond_pairs.p, 0, 16, stream));
+            h_cond_pairs = (unsigned long long*)pinned_acquire(16);
         }
         if (build_outer) { d_bmatched.alloc((size_t)std::max<int64_t>(n_build, 1)); B200_CUDA(cudaMemsetAsync(d_bmatched.p, 0, (size_t)std::max<int64_t>(n_build, 1), stream)); }
         B200_CUDA(cudaGetLastError());
@@ -1262,23 +1368,38 @@ class JoinState {
     // build rows of a build-outer join follow the last probe batch
     int64_t probe_general(int64_t n, const std::vector<OutCol>& cols, int nkb, const std::vector<const void*>& data,
                           const std::vector<const uint8_t*>& valid, bool is_last) {
-        // pass A + scan
+        // pass A + scan; with a condition pass A gives the slot (mode 0, no probe_outer row) and the condition count kernel the counts
+        const bool has_cond = !cond.empty();
+        const int mode = anti ? 1 : (mark ? 2 : 0), count_mode = has_cond ? 0 : mode, count_po = probe_outer && !has_cond ? 1 : 0;
+        CondArgs ca{};
+        if (has_cond) {
+            std::copy(cond.begin(), cond.end(), ca.prog);
+            for (int c = 0; c < n_b; c++) { ca.b_data[c] = bcol[c].buf.p; ca.b_valid[c] = build_valid(c); ca.b_ct[c] = b_ct[c]; }
+            for (int c = 0; c < n_p; c++) { ca.p_data[c] = data[c]; ca.p_valid[c] = valid[c]; ca.p_ct[c] = p_ct[c]; }
+        }
         unsigned long long n_match = 0;
         d_pslot.ensure((size_t)(n + 1) * 4); d_pcnt.ensure((size_t)(n + 1) * 4); d_poff.ensure((size_t)(n + 2) * 8);
         if (n > 0) {
             if (mark) { d_mark.ensure((size_t)n + 32); d_mark_valid.ensure((size_t)(n + 7) / 8 + 32); B200_CUDA(cudaMemsetAsync(d_mark_valid.p, 0xff, (size_t)(n + 7) / 8 + 8, stream)); }
             if (n_keys > 1)
                 join_probe_count_mk_kernel<<<grid_for(n), 256, 0, stream>>>(probe_keys(data, valid), build_keys(), n, d_tkeys.as<unsigned long long>(), cap,
-                                                                            d_info.as<SlotInfo>(), probe_outer ? 1 : 0, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(),
-                                                                            na_equal ? 1 : 0, anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr,
+                                                                            d_info.as<SlotInfo>(), count_po, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(),
+                                                                            na_equal ? 1 : 0, count_mode, mark ? d_mark.as<uint8_t>() : nullptr,
                                                                             key_reject);
             else
                 with_key([&](auto fk) {
                     join_probe_count_kernel<fk><<<grid_for(n), 256, 0, stream>>>(data[0], p_ct[0], valid[0], n, d_tkeys.as<long long>(), cap, d_info.as<SlotInfo>(),
-                                                                                 probe_outer ? 1 : 0, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(), na_equal ? 1 : 0,
-                                                                                 anti ? 1 : (mark ? 2 : 0), mark ? d_mark.as<uint8_t>() : nullptr, (int)key_reject);
+                                                                                 count_po, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>(), na_equal ? 1 : 0,
+                                                                                 count_mode, mark ? d_mark.as<uint8_t>() : nullptr, (int)key_reject);
                 });
             launches++;
+            if (has_cond) {
+                join_cond_count_kernel<<<grid_for(n), 256, 0, stream>>>(ca, n, d_pslot.as<uint32_t>(), d_info.as<SlotInfo>(), d_goffs.as<unsigned long long>(),
+                                                                        d_groups.as<uint32_t>(), probe_outer ? 1 : 0, mode, d_pcnt.as<uint32_t>(),
+                                                                        mark ? d_mark.as<uint8_t>() : nullptr, d_cond_pairs.as<unsigned long long>());
+                launches++;
+                B200_CUDA(cudaGetLastError());
+            }
             B200_CUDA(cudaMemsetAsync(d_pcnt.as<uint32_t>() + n, 0, 4, stream));
             n_match = scan.run(d_pcnt.as<uint32_t>(), n + 1, d_poff.as<unsigned long long>(), stream, &launches);
         }
@@ -1305,7 +1426,12 @@ class JoinState {
                 g.op_data[j] = out_data[k].p; g.op_valid[j] = out_valid(cols, k);
             }
         }
-        if (n > 0 && n_match > 0) { join_probe_gather_kernel<<<grid_for(n), 256, 0, stream>>>(g); launches++; B200_CUDA(cudaGetLastError()); }
+        if (n > 0 && n_match > 0) {
+            if (has_cond) join_cond_gather_kernel<<<grid_for(n), 256, 0, stream>>>(g, ca, mode);
+            else join_probe_gather_kernel<<<grid_for(n), 256, 0, stream>>>(g);
+            launches++;
+            B200_CUDA(cudaGetLastError());
+        }
         if (tail_flags.p) {
             join_unmatched_flags_kernel<<<grid_for(n_build), 256, 0, stream>>>(d_bmatched.as<uint8_t>(), n_build, tail_flags.as<uint32_t>());
             B200_CUDA(cudaMemsetAsync(tail_flags.as<uint32_t>() + n_build, 0, 4, stream));
@@ -1365,7 +1491,9 @@ class JoinState {
         for (int k = 0; k < n_out_cols; k++)
             if (cols[k].nullable && rows > 0) { launch_pack_bitmap(out_vbytes[k].as<uint8_t>(), rows, out_bitmap[k].as<uint32_t>(), grid_for(rows), stream); launches++; }
         B200_CUDA(cudaGetLastError());
+        if (h_cond_pairs) B200_CUDA(cudaMemcpyAsync(h_cond_pairs, d_cond_pairs.p, 16, cudaMemcpyDeviceToHost, stream));
         B200_CUDA(cudaStreamSynchronize(stream));
+        if (h_cond_pairs) { cond_evaluated = (int64_t)h_cond_pairs[0]; cond_passed = (int64_t)h_cond_pairs[1]; }
         describe_out(out, cols, rows);
         if (mark) {  // the mark column: BOOL, nullable array type, every row valid; output row i is probe row i
             b200_column& c = out->cols[n_out_cols];
@@ -1428,6 +1556,14 @@ int b200_join_set_kind(void* state, int32_t is_mark_join, int32_t is_anti_join) 
     } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
 }
 
+int b200_join_set_condition(void* state, const void* program, int32_t n_instr) {
+    try {
+        B200_REQUIRE(state && program, "b200 join: null argument");
+        ((JoinState*)state)->set_condition((const b200::ExprInstr*)program, n_instr);
+        return 0;
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
+}
+
 int b200_join_build_filter(void* state, int64_t n_bloom_blocks, void** bloom_words_dev, int64_t* n_blocks_out, int64_t* key_min_max) {
     try {
         B200_REQUIRE(state && n_bloom_blocks >= 0, "b200 join: bad arguments");
@@ -1471,6 +1607,8 @@ int64_t b200_join_get_metric(void* state, int32_t which) {
         case 5: return s->fast_probes;
         case 6: return s->inline_probes;
         case 7: return s->inline_builds;
+        case 8: return s->cond_evaluated;
+        case 9: return s->cond_passed;
         default: return -1;
     }
 }

@@ -4,6 +4,10 @@ conjunction, cast, null test), compiled to the postfix program b200_filter_proje
 
     e = (col("L_SHIPDATE") <= lit(datetime.date(1998, 9, 2))) & ~col("L_DISCOUNT").isnull()
     p = col("L_EXTENDEDPRICE") * (lit(1.0) - col("L_DISCOUNT"))
+
+A join's non-equi condition names the side of each column (streaming.join.init_join_state, non_equi_condition):
+
+    c = (probe_col("ts") >= build_col("start")) & (probe_col("ts") < build_col("end"))
 """
 
 from __future__ import annotations
@@ -60,6 +64,16 @@ class Expr:
 
 def col(name) -> Expr:
     return Expr("col", value=name)
+
+
+def build_col(name) -> Expr:
+    """Column `name` of a join's build side (the right table of merge), for a join's non_equi_condition."""
+    return Expr("col", value=("build", name))
+
+
+def probe_col(name) -> Expr:
+    """Column `name` of a join's probe side (the left table of merge), for a join's non_equi_condition."""
+    return Expr("col", value=("probe", name))
 
 
 def lit(v) -> Expr:

@@ -493,7 +493,10 @@ def window(df, partition_by, order_by, funcs, ascending=True, na_position="last"
 def merge(left, right, left_on, right_on, how: str = "inner", batch_size: int = STREAMING_BATCH_SIZE, **kw):
     """left.merge(right, left_on=..., right_on=..., how=...) through the streaming join (right = build side).  left_on / right_on:
     a column name, or equal-length lists of 1..4 names (a multi-column key).
-    Output columns: right's columns then left's columns (the reference's build-then-probe order), renamed on clashes."""
+    Output columns: right's columns then left's columns (the reference's build-then-probe order), renamed on clashes.
+    `non_equi_condition=` joins only the key-equal pairs that also satisfy a condition (an Expr; left is the probe side, right
+    the build side), e.g. `merge(events, windows, "acct", "acct", how="left",
+    non_equi_condition=(probe_col("ts") >= build_col("start")) & (probe_col("ts") < build_col("end")))`."""
     rcols, lcols = list(right.columns), list(left.columns)
     lo = [left_on] if isinstance(left_on, str) else list(left_on)
     ro = [right_on] if isinstance(right_on, str) else list(right_on)

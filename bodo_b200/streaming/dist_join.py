@@ -129,7 +129,7 @@ class DistJoinState:
 
     def __init__(self, operator_id, build_key_inds, probe_key_inds, build_colnames, probe_colnames, build_outer, probe_outer,
                  output_batch_size, expected_build_rows, device, stream, is_na_equal=False, build_parallel=False, probe_parallel=False,
-                 force_broadcast=False, process_group=None, is_mark_join=False, is_anti_join=False):
+                 force_broadcast=False, process_group=None, is_mark_join=False, is_anti_join=False, non_equi_condition=None):
         import torch
         import torch.distributed as dist
 
@@ -145,7 +145,7 @@ class DistJoinState:
         self.device = device if device is not None else torch.cuda.current_device()
         self.local = J.JoinState(operator_id, build_key_inds, probe_key_inds, build_colnames, probe_colnames, build_outer, probe_outer,
                                  output_batch_size, expected_build_rows, self.device, stream, is_na_equal=is_na_equal,
-                                 is_mark_join=is_mark_join, is_anti_join=is_anti_join)
+                                 is_mark_join=is_mark_join, is_anti_join=is_anti_join, non_equi_condition=non_equi_condition)
         self.probe_outer = bool(probe_outer)
         # bloom filter + key bounds over the build keys of ALL ranks, applied to probe rows before they are shuffled (the
         # reference's use_bloom_filter probe path, _join.cpp:3460-3600); B200_JOIN_BLOOM=0 disables it

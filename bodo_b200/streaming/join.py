@@ -12,13 +12,14 @@ from __future__ import annotations
 
 from .. import _lib
 from .._lib import ffi
+from ..expr import OPS, Expr, compile_program
 from ..table import CTable, Table, table_from_ctable
 
 
 class JoinState:
     def __init__(self, operator_id, build_key_inds, probe_key_inds, build_colnames, probe_colnames, build_outer, probe_outer,
                  output_batch_size, expected_build_rows, device, stream, is_na_equal=False, build_parallel=False, probe_parallel=False,
-                 is_mark_join=False, is_anti_join=False):
+                 is_mark_join=False, is_anti_join=False, non_equi_condition=None):
         self.operator_id = int(operator_id)
         self.is_mark_join = bool(is_mark_join)
         self.is_anti_join = bool(is_anti_join)
@@ -44,6 +45,10 @@ class JoinState:
         self.probe_indices = None
         self.build_names = None
         self._out = None
+        self.condition = None  # [(op, arg)] of the non-equi condition, resolved to physical columns
+        if non_equi_condition is not None:
+            self.condition = compile_condition(non_equi_condition, self.build_key_inds, self.probe_key_inds, self.build_colnames,
+                                               self.probe_colnames)
 
     def _physical(self, table: Table, key_inds):
         others = [i for i in range(table.n_cols) if i not in key_inds]
@@ -65,14 +70,72 @@ class JoinState:
         self.handle = _lib.check_ptr(h, "init_join_state")
         if self.is_mark_join or self.is_anti_join:
             _lib.check(L.b200_join_set_kind(self.handle, int(self.is_mark_join), int(self.is_anti_join)), "init_join_state")
+        if self.condition is not None:
+            prog = ffi.new("b200_expr_instr[]", len(self.condition))
+            for i, (op, arg) in enumerate(self.condition):
+                prog[i].op = op
+                prog[i].arg = arg
+            _lib.check(L.b200_join_set_condition(self.handle, prog, len(self.condition)), "init_join_state")
+
+
+J_MAX_COLS = 32        # columns per side (join.cu); a probe column c is program column J_MAX_COLS + c
+EX_MAX_INSTR = 64      # instructions of one program (expr.cuh)
+EX_MAX_STACK = 8       # values live at once while it runs
+
+
+def compile_condition(cond, build_key_inds, probe_key_inds, build_colnames, probe_colnames):
+    """The non-equi condition as the postfix program b200_join_set_condition takes: [(op, arg)] ending in END.  Column references
+    are build_col(name) / probe_col(name); a name resolves against that side's colnames to its physical column (keys first, then
+    the other columns in input order), a probe column c becoming J_MAX_COLS + c.  Runs on the host only."""
+    if not isinstance(cond, Expr):
+        raise _lib.B200Error(f"Streaming Join: non_equi_condition must be a bodo_b200.expr.Expr built from build_col / probe_col, not "
+                             f"{type(cond).__name__} (string conditions are not supported)")
+    sides = {"build": (build_colnames, build_key_inds, 0), "probe": (probe_colnames, probe_key_inds, J_MAX_COLS)}
+    col_index = {}
+    for ref in cond.columns():
+        if not (isinstance(ref, tuple) and len(ref) == 2 and ref[0] in sides):
+            raise _lib.B200Error(f"Streaming Join: non_equi_condition column {ref!r} names no join side: use build_col({ref!r}) or "
+                                 f"probe_col({ref!r})")
+        side, name = ref
+        names, keys, base = sides[side]
+        if names is None:
+            raise _lib.B200Error(f"Streaming Join: non_equi_condition reads {side} column {name!r}, but {side}_colnames is None: the "
+                                 "condition's names resolve against the column names given at init")
+        hits = [i for i, nm in enumerate(names) if nm == name]
+        if len(hits) != 1:
+            raise _lib.B200Error(f"Streaming Join: non_equi_condition: the {side} side has {'no' if not hits else 'more than one'} column "
+                                 f"{name!r} ({side} columns: {list(names)})")
+        physical = list(keys) + [i for i in range(len(names)) if i not in keys]
+        col_index[ref] = base + physical.index(hits[0])
+    prog, _ = compile_program([cond], col_index)
+    if len(prog) > EX_MAX_INSTR:
+        raise _lib.B200Error(f"Streaming Join: non_equi_condition compiles to {len(prog)} instructions; the limit is {EX_MAX_INSTR}")
+    unary = {OPS[o] for o in ("not", "neg", "to_f64", "to_i64", "is_null")}
+    depth = max_depth = 0
+    for op, _ in prog:
+        depth += 1 if op in (OPS["col"], OPS["const_i64"], OPS["const_f64"]) else 0 if op in unary or op == OPS["end"] else -1
+        max_depth = max(max_depth, depth)
+    if max_depth > EX_MAX_STACK:
+        raise _lib.B200Error(f"Streaming Join: non_equi_condition needs a stack of {max_depth} values while it runs; the limit is "
+                             f"{EX_MAX_STACK} (split deep nesting, e.g. ((a + b) + c) rather than a + (b + (c + d)))")
+    return prog
 
 
 def init_join_state(operator_id, build_key_inds, probe_key_inds, build_colnames, probe_colnames, build_outer, probe_outer,
                     interval_build_columns=None, force_broadcast=False, op_pool_size_bytes=-1, non_equi_condition=None,
                     build_parallel=False, probe_parallel=False, *, output_batch_size=32768, expected_build_rows=0, device=None,
                     stream=0, is_na_equal=False, is_mark_join=False, is_anti_join=False) -> JoinState:
-    """Mirror of bodo.libs.streaming.join.init_join_state (join.py:991-1100).  Interval joins and non-equi conditions are
-    out of scope (SURVEY.md §2.1 row 3) and must be left at their defaults.
+    """Mirror of bodo.libs.streaming.join.init_join_state (join.py:991-1100).  Interval joins (`interval_build_columns`) are out
+    of scope (SURVEY.md §2.1 row 3) and must be left at the default.
+
+    `non_equi_condition` joins on the equi-join keys AND a condition between the two sides.  The reference takes a string
+    ("left.`A` < right.`B`") and compiles it to a cond_func; here it is a bodo_b200.expr.Expr whose columns are
+    build_col(name) / probe_col(name), resolved against build_colnames / probe_colnames at init, e.g.
+    `(probe_col("ts") >= build_col("start")) & (probe_col("ts") < build_col("end"))`.  A pair of rows with equal keys joins when the
+    condition is valid and true (b200_filter_project's semantics: NA and NaN cells are NA, arithmetic and comparisons propagate
+    NA, `&` / `|` are Kleene, DATE is days and DATETIME nanoseconds); the outer, anti and mark kinds then apply to the pairs that
+    pass.  The condition may read any column, also one used_cols drops, and adds no output column.  At least one equi-join key
+    is required: a condition-only (nested-loop) join is not supported.
 
     `is_na_equal` is HashJoinState's option: False is what this door constructs in the reference (join_state_init_py_entry,
     _join.cpp:4087-4136: NA keys never match); the pandas door (bodo/pandas/physical/join.h:267, here PhysicalJoin / merge)
@@ -85,19 +148,22 @@ def init_join_state(operator_id, build_key_inds, probe_key_inds, build_colnames,
     reference's planner for LEFT ANTI joins, bodo/pandas/physical/join.h:151): a mark join emits every probe row once, without
     build columns, plus a trailing boolean column that says whether the row has a match; an anti join emits the probe rows
     that have none."""
-    if interval_build_columns not in (None, (), []) or non_equi_condition is not None:
-        raise _lib.B200Error("Streaming Join: interval / non-equi joins are not supported by bodo_b200")
+    if interval_build_columns not in (None, (), []):
+        raise _lib.B200Error("Streaming Join: interval joins (interval_build_columns) are not supported by bodo_b200")
     g = lambda x: getattr(x, "meta", x)
+    if non_equi_condition is not None and (len(tuple(g(build_key_inds))) == 0 or len(tuple(g(probe_key_inds))) == 0):
+        raise _lib.B200Error("Streaming Join: a non_equi_condition without an equi-join key (a nested-loop join) is not supported by "
+                             "bodo_b200; give at least one key column per side")
     if build_parallel or probe_parallel:
         from .dist_join import DistJoinState
 
         return DistJoinState(operator_id, g(build_key_inds), g(probe_key_inds), g(build_colnames), g(probe_colnames), build_outer,
                              probe_outer, output_batch_size, expected_build_rows, device, stream, is_na_equal=is_na_equal,
                              build_parallel=build_parallel, probe_parallel=probe_parallel, force_broadcast=force_broadcast,
-                             is_mark_join=is_mark_join, is_anti_join=is_anti_join)
+                             is_mark_join=is_mark_join, is_anti_join=is_anti_join, non_equi_condition=non_equi_condition)
     return JoinState(operator_id, g(build_key_inds), g(probe_key_inds), g(build_colnames), g(probe_colnames), build_outer,
                      probe_outer, output_batch_size, expected_build_rows, device, stream, is_na_equal=is_na_equal,
-                     is_mark_join=is_mark_join, is_anti_join=is_anti_join)
+                     is_mark_join=is_mark_join, is_anti_join=is_anti_join, non_equi_condition=non_equi_condition)
 
 
 def join_build_consume_batch(join_state: JoinState, table: Table, is_last: bool):

@@ -205,6 +205,16 @@ void b200_delete_join_state(void* state);
  * descriptors) or probe-side anti join (the is_anti_join template argument of the reference's probe, _join.cpp:763-767 — a probe
  * row goes out, with NULL build columns, iff no build row matches).  build_table_outer must be false for both. */
 int b200_join_set_kind(void* state, int32_t is_mark_join, int32_t is_anti_join);
+/* Non-equi condition (the cond_func argument of join_state_init_py_entry, _join.cpp:4087-4136; bodo/libs/streaming/join.py:991-1100
+ * builds it from the `non_equi_condition` string; the GPU path runs cudf::filter_join_indices after the hash join), to be called
+ * between init and the first build batch: `program` is n_instr b200_expr_instr (below) forming ONE expression that ends in END.
+ * An EX_COL argument c < 32 reads build column c, 32 + c probe column c (physical, keys-first column order of each side).  Build
+ * columns are checked here, probe columns when the probe schema is known (here, or at the first probe batch).  A candidate pair
+ * (a probe row and a build row with an equal key) joins when the condition is valid and true (b200_filter_project's semantics);
+ * the join kinds then apply to the passing pairs: a probe row with none is NULL-extended (probe_table_outer), kept by an anti
+ * join, marked false by a mark join; a build row is matched (build_table_outer) only through a passing pair.  The state always
+ * takes the general (CSR) table, never the unique-key tables of metrics 5-7. */
+int b200_join_set_condition(void* state, const void* program, int32_t n_instr);
 
 /* Runtime join filter (HashJoinState::RuntimeFilter, _join.h:1060-1095; bloom filter bodo/libs/gpu_bloom_filter.cu:60-201; key
  * min / max _join.cpp:3199-3238), available once the build side is complete.  The reference keeps one bloom filter over the whole
@@ -229,7 +239,8 @@ int b200_join_runtime_filter_n(void* state, const b200_table* in_table, const in
 
 /* Operator metrics (the reference's JoinMetrics, bodo/libs/streaming/_join.h): 0 build rows, 1 hash-table slots, 2 probe rows,
  * 3 output rows, 4 kernel launches, 5 probe batches through a fused (unique-build-key) probe kernel, 6 of those through the
- * inline-payload kernel (key + payload in one 32-byte slot), 7 inline-payload table builds. */
+ * inline-payload kernel (key + payload in one 32-byte slot), 7 inline-payload table builds, 8 candidate pairs the non-equi
+ * condition evaluated, 9 of those that passed (8 and 9 stay 0 without a condition). */
 int64_t b200_join_get_metric(void* state, int32_t which);
 
 /* ---- streaming top-k: ORDER BY ... LIMIT ... OFFSET (reference: bodo/libs/streaming/_sort.cpp) ---- */
