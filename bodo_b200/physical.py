@@ -181,15 +181,24 @@ class PhysicalFilterProject:
 
 def filter_project_table(table: Table, keep) -> Table:
     """Rows of a device-resident `table` whose entry in `keep` (uint8 device tensor, one byte per row) is non-zero, through the
-    fused filter kernel (used by streaming.join.runtime_join_filter).  Every column is one output of the kernel, so a table of
-    more than 16 columns raises B200Error."""
-    from .expr import col
-    from .table import ArrTypes, Column, CTypes
+    fused filter kernel (used by streaming.join.runtime_join_filter).  The kept rows are the input's: same c-types, array types,
+    bitmap presence and bits.  Each column passes through the kernel as the signed integer of its width, so a float NaN stays a
+    valid NaN (the kernel reads NaN as NA), and a column without a bitmap comes back without one.  Every column is one output of
+    the kernel, so a table of more than 16 columns raises B200Error."""
+    import torch
 
-    ext = Table(list(table.columns) + [Column(keep, None, CTypes.BOOL, ArrTypes.NUMPY, table.n_rows)], list(table.names) + ["__keep"])
-    op = PhysicalFilterProject(col("__keep"), [(n, col(n)) for n in table.names], device=table.device)
+    from .expr import col
+    from .table import ArrTypes, Column, CTypes, np_dtype_of
+
+    as_int = {1: CTypes.INT8, 2: CTypes.INT16, 4: CTypes.INT32, 8: CTypes.INT64}
+    names = [f"c{j}" for j in range(table.n_cols)]
+    ins = [Column(c.data, c.validity, as_int[np_dtype_of(c.c_type).itemsize], c.arr_type, c.length) for c in table.columns]
+    ext = Table(ins + [Column(keep, None, CTypes.BOOL, ArrTypes.NUMPY, table.n_rows)], names + ["__keep"])
+    op = PhysicalFilterProject(col("__keep"), [(nm, col(nm)) for nm in names], device=table.device)
     out, _ = op.ProcessBatch(ext, OperatorResult.NEED_MORE_INPUT)
-    return out
+    cols = [Column(o.data.view(getattr(torch, str(np_dtype_of(c.c_type)))), o.validity if c.validity is not None else None, c.c_type,
+                   c.arr_type, o.length) for c, o in zip(table.columns, out.columns)]
+    return Table(cols, list(table.names))
 
 
 class PhysicalReadArrowDevice:

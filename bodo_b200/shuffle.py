@@ -124,6 +124,8 @@ def merge_segment_bitmaps(bitmap, counts: Sequence[int]):
         raise _lib.B200Error("merge_segment_bitmaps: device tensors only (this package has no CPU path)")
     n = int(sum(counts))
     out = torch.zeros(((n + 31) // 32 + 2) * 4, dtype=torch.uint8, device=bitmap.device)
+    if n == 0:  # a rank that receives no row gets an empty segment buffer, whose null pointer the entry point refuses
+        return out
     cnt = ffi.new("int64_t[]", [int(c) for c in counts])
     _lib.check(_lib.lib().b200_merge_segment_bitmaps(ffi.cast("uint8_t*", bitmap.data_ptr()), cnt, len(counts),
                                                      ffi.cast("uint8_t*", out.data_ptr()), bitmap.device.index,

@@ -16,6 +16,12 @@ Here, per rank (one process per GPU, torch.distributed / NCCL for the plumbing):
            side against a partitioned build keeps only the rows whose key this rank owns (no exchange); against a replicated
            (or broadcast) build side the batch is probed as it is.
 
+A REPLICATED build side with a build-outer tail (build_outer / full outer) against a partitioned probe side is made partitioned
+instead: each rank keeps the build rows whose key it owns (no exchange) and the probe batches are exchanged.  Probed where it
+was fed, every rank would emit the build rows IT did not match, so an unmatched row would come out once per rank and a row
+matched on one rank NULL-extended from the others.  (The broadcast decision keeps a build-outer join partitioned for the same
+reason.)  The hash partition takes key columns of 4 and 8 bytes: a placement that partitions refuses 1- and 2-byte keys.
+
 The calls are collective, as in the reference: every rank calls build / probe the same number of times (ranks that ran out of
 input keep calling with empty batches until the is_last call, bodo/pandas/_pipeline.cpp:453-457).
 Placement is the reference's: (uint32) XXH3_64(key, SEED_HASH_PARTITION) % n_pes, and for a multi-column key hash_keys over the
@@ -138,10 +144,12 @@ class DistJoinState:
         self.group = process_group
         self.n_pes = dist.get_world_size(process_group)
         self.rank = dist.get_rank(process_group)
-        self.build_parallel = bool(build_parallel) and self.n_pes > 1
         self.probe_parallel = bool(probe_parallel) and self.n_pes > 1
         self.force_broadcast = bool(force_broadcast)
         self.build_outer = bool(build_outer)
+        # a replicated build side with a build-outer tail against a partitioned probe side: keep the owned build rows (see above)
+        self.owned_build = not build_parallel and self.probe_parallel and self.build_outer
+        self.build_parallel = (bool(build_parallel) and self.n_pes > 1) or self.owned_build
         self.device = device if device is not None else torch.cuda.current_device()
         self.local = J.JoinState(operator_id, build_key_inds, probe_key_inds, build_colnames, probe_colnames, build_outer, probe_outer,
                                  output_batch_size, expected_build_rows, self.device, stream, is_na_equal=is_na_equal,
@@ -219,6 +227,8 @@ class DistJoinState:
             mine = all_gather_table(whole, self.device, self.group)
             self.is_broadcast = True
             self.metrics["broadcast"] = 1
+        elif self.owned_build:
+            mine = self._owned_only(whole, self.build_keys)
         else:
             mine = self._shuffle(whole, self.build_keys)
         self.metrics["build_rows_local"] = mine.n_rows
@@ -258,7 +268,7 @@ class DistJoinState:
         self.metrics["probe_rows_in"] += table.n_rows
         partitioned_build = self.build_parallel and not self.is_broadcast
         if partitioned_build and self.probe_parallel:
-            if self.filter_ready and table.n_rows:
+            if self.filter_ready and table.n_rows and table.n_cols <= J.EX_MAX_OUT:  # (a wider probe side goes unfiltered)
                 table = J.runtime_join_filter((self,), to_device(table, self.device), (self.probe_keys,))
                 self.metrics["probe_rows_after_filter"] = self.metrics.get("probe_rows_after_filter", 0) + table.n_rows
             table = self._shuffle(table, self.probe_keys)

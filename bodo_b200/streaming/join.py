@@ -81,6 +81,7 @@ class JoinState:
 J_MAX_COLS = 32        # columns per side (join.cu); a probe column c is program column J_MAX_COLS + c
 EX_MAX_INSTR = 64      # instructions of one program (expr.cuh)
 EX_MAX_STACK = 8       # values live at once while it runs
+EX_MAX_OUT = 16        # output columns of one filter-projection call: the widest table runtime_join_filter takes
 
 
 def compile_condition(cond, build_key_inds, probe_key_inds, build_colnames, probe_colnames):

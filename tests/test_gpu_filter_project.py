@@ -665,9 +665,10 @@ def test_multiple_batches_through_one_operator(gpu_lib):
 
 
 @pytest.mark.gpu
-def test_filter_project_table_passthrough(gpu_lib):
+def test_filter_project_table_keeps_rows_bit_for_bit(gpu_lib):
     """The runtime join filter's compaction: every column of a mixed-dtype table with nulls passes through unchanged for the
-    rows whose keep byte is non-zero (any non-zero byte keeps)."""
+    rows whose keep byte is non-zero (any non-zero byte keeps): c-type, array type, bitmap presence, validity and bits, so a
+    float NaN stays a valid NaN with its payload."""
     import torch
 
     spec = [(f"c_{dt}", dt, "nullable" if dt != "date32" else "arrow_offset", 0.15) for dt in DTYPES]
@@ -679,13 +680,12 @@ def test_filter_project_table_passthrough(gpu_lib):
     assert out.names == dt.names and out.n_rows == int((keep != 0).sum())
     order = np.argsort(out.columns[0].values_numpy())
     np.testing.assert_array_equal(out.columns[0].values_numpy()[order], np.flatnonzero(keep))
-    for nm, c in zip(out.names[1:], out.columns[1:]):
+    as_bits = lambda x: x.view(np.uint8) if x.dtype == bool else x.view(f"i{x.dtype.itemsize}") if x.dtype.kind == "f" else x  # noqa: E731
+    for nm, c, inc in zip(out.names[1:], out.columns[1:], dt.columns[1:]):
         ct, v, valid = cols[nm]
-        exp = v.view(np.uint8) if v.dtype == bool else v
-        valid = valid & ~np.isnan(v) if ct in FLOATS else valid    # a passthrough reads NaN as NA too
+        assert (c.c_type, c.arr_type, c.validity is not None) == (inc.c_type, inc.arr_type, inc.validity is not None), nm
         got = c.values_numpy()[order]
-        _assert_column(nm, got.view(np.uint8) if got.dtype == bool else got, c.valid_mask_numpy()[order], exp[keep != 0],
-                       valid[keep != 0])
+        _assert_column(nm, as_bits(got), c.valid_mask_numpy()[order], as_bits(v)[keep != 0], valid[keep != 0])
 
 
 @pytest.mark.gpu
