@@ -16,6 +16,7 @@
 // class_1, word_1, ..., arrival index), so no two rows are equal.
 #include <algorithm>
 #include <cfloat>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -2040,28 +2041,35 @@ static void launch_wnl(WnlArgs& a, const WvCol& x, int64_t n_tiles, bool range, 
     else window_nulls_eval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
 }
 
+// Calls launch(std::integral_constant<int, K>) with aggregate g's scan kind K, which its scan and its frame tree share.
+template <typename Launch>
+static void with_wv_kind(const WvFunc& g, Launch launch) {
+    if (g.code >= WN_COVAR_SAMP) launch(std::integral_constant<int, WV_CO>());
+    else if (g.code >= WN_VAR) launch(std::integral_constant<int, WV_MOM>());
+    else if (g.code == WN_MIN) launch(std::integral_constant<int, WV_MIN>());
+    else if (g.code == WN_MAX) launch(std::integral_constant<int, WV_MAX>());
+    else if (g.code != WN_COUNT && ctype_is_float(g.ct)) launch(std::integral_constant<int, WV_FSUM>());
+    else launch(std::integral_constant<int, WV_ISUM>());
+}
+
 // Ranking and value window functions over (PARTITION BY the first n_part keys ORDER BY the rest).  The output is the full sort's,
 // plus one column per function after the input columns: numpy for the ranking functions and count, nullable for the others.
 struct WindowState : FullSortState {
     int n_part, n_funcs;
-    b200_window_func fn[SORT_MAX_COLS];
-    b200_window_frame bound[SORT_MAX_COLS];  // a WF_BOUNDED function's frame
-    b200_window_range range[SORT_MAX_COLS];  // a WF_RANGE_BETWEEN function's frame
-    bool ignore_nulls[SORT_MAX_COLS];        // first_value, last_value, lag, lead or nth_value with IGNORE NULLS
+    b200_window_func fn[SORT_MAX_COLS];  // rows / range hold the unbounded frame unless the function came with frame 4 / 5
     std::vector<DevBuf> fout;
     int64_t n_partitions = 0;  // metric 9
 
     WindowState(const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_part_, int n_keys, const int32_t* asc,
-                const int32_t* na_last, const b200_window_func* funcs, const b200_window_frame* frames, const b200_window_range* ranges,
-                const int32_t* nulls, int n_funcs_, int64_t obs, int dev, cudaStream_t st)
+                const int32_t* na_last, const b200_window_func* funcs, int n_funcs_, int64_t obs, int dev, cudaStream_t st)
         : FullSortState(c_types, arr_types, n_arrs, n_keys, asc, na_last, obs, dev, st), n_part(n_part_), n_funcs(n_funcs_) {
         for (int f = 0; f < n_funcs; f++) {
             b200_window_func& d = fn[f] = funcs[f];
-            bound[f] = b200_window_frame{WF_UNBOUNDED_START, WF_UNBOUNDED_END};
-            range[f] = b200_window_range{WR_UNBOUNDED_PRECEDING, WR_UNBOUNDED_FOLLOWING, 0, 0};
+            // the bounds a function's frame does not read: equal functions then reach the kernels as equal bits
+            if (d.frame != WF_BOUNDED) d.rows = b200_window_frame{WF_UNBOUNDED_START, WF_UNBOUNDED_END};
+            if (d.frame != WF_RANGE_BETWEEN) d.range = b200_window_range{WR_UNBOUNDED_PRECEDING, WR_UNBOUNDED_FOLLOWING, 0, 0};
             B200_REQUIRE(d.code >= WN_ROW_NUMBER && d.code <= WN_REGR_INTERCEPT, "b200 window: unknown function code");
-            ignore_nulls[f] = nulls && nulls[f] != 0;
-            B200_REQUIRE(!ignore_nulls[f] || (d.code >= WN_FIRST_VALUE && d.code <= WN_NTH_VALUE),
+            B200_REQUIRE(!d.ignore_nulls || (d.code >= WN_FIRST_VALUE && d.code <= WN_NTH_VALUE),
                          "b200 window: IGNORE NULLS takes first_value, last_value, lag, lead and nth_value only (codes 11..15)");
             int ct = CT_INT64, at = ARR_NUMPY;
             if (d.code <= WN_NTILE) {
@@ -2079,18 +2087,16 @@ struct WindowState : FullSortState {
                     B200_REQUIRE(d.frame >= WF_RANGE && d.frame <= WF_RANGE_BETWEEN,
                                  "b200 window: unknown frame (1 range, 2 rows, 3 partition, 4 rows between, 5 range between)");
                 }
-                if (d.frame == WF_RANGE_BETWEEN) check_range(f, d, ranges, n_keys);
+                if (d.frame == WF_RANGE_BETWEEN) check_range(d, n_keys);
                 if (d.code == WN_NTH_VALUE) B200_REQUIRE(d.arg >= 1 && d.arg <= 0x7FFFFFFF, "b200 window: nth_value needs n in [1, 2^31)");
                 if (d.frame == WF_BOUNDED) {
-                    B200_REQUIRE(frames, "b200 window: frame 4 (rows between) needs frames[i]");
-                    const b200_window_frame b = frames[f];
+                    const b200_window_frame b = d.rows;
                     const int64_t lim = 0x7FFFFFFF;
                     B200_REQUIRE((b.start == WF_UNBOUNDED_START || (b.start >= -lim && b.start <= lim)) &&
                                  (b.end == WF_UNBOUNDED_END || (b.end >= -lim && b.end <= lim)),
                                  "b200 window: a frame bound is UNBOUNDED or a row offset in (-2^31, 2^31)");
                     B200_REQUIRE(b.start == WF_UNBOUNDED_START || b.end == WF_UNBOUNDED_END || b.start <= b.end,
                                  "b200 window: frame start after frame end");
-                    bound[f] = b;
                     // the spellings of the unbounded frames: the same frame gives the same bits however it is written
                     if (b.start == WF_UNBOUNDED_START && b.end == 0) d.frame = WF_ROWS;
                     else if (b.start == WF_UNBOUNDED_START && b.end == WF_UNBOUNDED_END) d.frame = WF_PARTITION;
@@ -2117,11 +2123,10 @@ struct WindowState : FullSortState {
         }
     }
 
-    // Validates function f's b200_window_range (frame 5) against the keys and stores it; the unbounded-start spellings become
+    // Validates function d's range (frame 5) against the keys and zeroes its unread bits; the unbounded-start spellings become
     // frames 1 and 3, so a frame gives the same bits however it is written.
-    void check_range(int f, b200_window_func& d, const b200_window_range* ranges, int n_keys) {
-        B200_REQUIRE(ranges, "b200 window: frame 5 (range between) needs ranges[i]");
-        b200_window_range r = ranges[f];
+    void check_range(b200_window_func& d, int n_keys) {
+        b200_window_range& r = d.range;
         B200_REQUIRE(r.start_kind >= WR_UNBOUNDED_PRECEDING && r.start_kind <= r.end_kind && r.end_kind <= WR_UNBOUNDED_FOLLOWING &&
                      r.start_kind != WR_UNBOUNDED_FOLLOWING && r.end_kind != WR_UNBOUNDED_PRECEDING,
                      "b200 window: range bound kinds are 0..4 with start_kind <= end_kind, start_kind != 4 and end_kind != 0");
@@ -2144,7 +2149,6 @@ struct WindowState : FullSortState {
         }
         if (!offset(r.start_kind)) r.start_bits = 0;  // unread: equal frames then compare equal
         if (!offset(r.end_kind)) r.end_bits = 0;
-        range[f] = r;
         if (r.start_kind == WR_UNBOUNDED_PRECEDING && r.end_kind == WR_CURRENT_ROW) d.frame = WF_RANGE;
         else if (r.start_kind == WR_UNBOUNDED_PRECEDING && r.end_kind == WR_UNBOUNDED_FOLLOWING) d.frame = WF_PARTITION;
     }
@@ -2165,7 +2169,7 @@ struct WindowState : FullSortState {
         struct RangeFrame { b200_window_range r; std::vector<WfFunc> trees, gathers, nulls; };
         std::vector<RangeFrame> ranged;
         const auto range_frame = [&](int f) {
-            const b200_window_range& r = range[f];
+            const b200_window_range& r = fn[f].range;
             auto it = std::find_if(ranged.begin(), ranged.end(), [&](const RangeFrame& x) {
                 return x.r.start_kind == r.start_kind && x.r.end_kind == r.end_kind && x.r.start_bits == r.start_bits &&
                        x.r.end_bits == r.end_bits;
@@ -2189,20 +2193,16 @@ struct WindowState : FullSortState {
             WvFunc g{d.code, d.frame, d.col >= 0 ? sc.ctype[d.col] : CT_INT64, d.col >= 0 ? ctype_size(sc.ctype[d.col]) : 0,
                      ctype_size(sc.ctype[c]), d.default_valid, d.arg, d.default_bits, d.col >= 0 ? out_data[d.col] : nullptr,
                      d.col >= 0 ? out_vb[d.col] : nullptr, out_data[c], out_vb[c]};
-            if (ignore_nulls[f]) {  // the IGNORE NULLS kernels only, never a scan, tree or gather
-                WfFunc h{};
-                h.g = g;
-                h.start = bound[f].start;
-                h.end = bound[f].end;
+            WfFunc h{};
+            h.g = g;
+            h.start = d.rows.start;
+            h.end = d.rows.end;
+            if (d.ignore_nulls) {  // the IGNORE NULLS kernels only, never a scan, tree or gather
                 (d.frame == WF_RANGE_BETWEEN ? range_frame(f)->nulls : nulls).push_back(h);
                 any_nulls = true;
                 continue;
             }
             if (d.frame == WF_BOUNDED || d.frame == WF_RANGE_BETWEEN || d.code == WN_NTH_VALUE) {  // the frame path only
-                WfFunc h{};
-                h.g = g;
-                h.start = bound[f].start;
-                h.end = bound[f].end;
                 const bool agg = wv_aggregate(d.code) && d.col >= 0;
                 if (d.frame == WF_RANGE_BETWEEN) {
                     (agg ? range_frame(f)->trees : range_frame(f)->gathers).push_back(h);
@@ -2247,12 +2247,7 @@ struct WindowState : FullSortState {
         for (const WvFunc& g : scans) {
             va.s = g;
             const WvCol x = bivariate(g.code) ? col2(g) : WvCol{};
-            if (bivariate(g.code)) launch_wv_scan<WV_CO>(va, x, n_tiles, stream);
-            else if (moments(g.code)) launch_wv_scan<WV_MOM>(va, x, n_tiles, stream);
-            else if (g.code == WN_MIN) launch_wv_scan<WV_MIN>(va, x, n_tiles, stream);
-            else if (g.code == WN_MAX) launch_wv_scan<WV_MAX>(va, x, n_tiles, stream);
-            else if (g.code != WN_COUNT && ctype_is_float(g.ct)) launch_wv_scan<WV_FSUM>(va, x, n_tiles, stream);
-            else launch_wv_scan<WV_ISUM>(va, x, n_tiles, stream);
+            with_wv_kind(g, [&](auto k) { launch_wv_scan<decltype(k)::value>(va, x, n_tiles, stream); });
         }
         if (eval) window_veval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a, va);
         B200_CUDA(cudaGetLastError());
@@ -2296,12 +2291,7 @@ struct WindowState : FullSortState {
             const auto launch_tree = [&](const WfFunc& h) {
                 fa.s = h;
                 const WvCol x = bivariate(h.g.code) ? col2(h.g) : WvCol{};
-                if (bivariate(h.g.code)) launch_wf_tree<WV_CO>(fa, x, n_tiles, stream);
-                else if (moments(h.g.code)) launch_wf_tree<WV_MOM>(fa, x, n_tiles, stream);
-                else if (h.g.code == WN_MIN) launch_wf_tree<WV_MIN>(fa, x, n_tiles, stream);
-                else if (h.g.code == WN_MAX) launch_wf_tree<WV_MAX>(fa, x, n_tiles, stream);
-                else if (h.g.code != WN_COUNT && ctype_is_float(h.g.ct)) launch_wf_tree<WV_FSUM>(fa, x, n_tiles, stream);
-                else launch_wf_tree<WV_ISUM>(fa, x, n_tiles, stream);
+                with_wv_kind(h.g, [&](auto k) { launch_wf_tree<decltype(k)::value>(fa, x, n_tiles, stream); });
             };
             for (const WfFunc& h : trees) launch_tree(h);
             if (fa.n_funcs > 0) window_frame_kernel<WV_GATHER><<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(fa, WvCol{});
@@ -2371,75 +2361,9 @@ void* b200_sort_state_init_full(int64_t operator_id, const int8_t* c_types, cons
     });
 }
 
-void* b200_window_state_init_funcs(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                                   int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                                   const int32_t* order_na_last, const b200_window_func* funcs, int32_t n_funcs, int64_t output_batch_size,
-                                   int32_t device, void* stream) {
-    try {  // this entry's domain: codes 0..14, frames 0..3 (the frame entry adds nth_value and bounded frames)
-        for (int f = 0; funcs && f < n_funcs && f < b200::SORT_MAX_COLS; f++) {
-            B200_REQUIRE(funcs[f].code >= b200::WN_ROW_NUMBER && funcs[f].code <= b200::WN_LEAD, "b200 window: unknown function code");
-            if (funcs[f].code >= b200::WN_SUM && funcs[f].code <= b200::WN_LAST_VALUE)
-                B200_REQUIRE(funcs[f].frame >= b200::WF_RANGE && funcs[f].frame <= b200::WF_PARTITION,
-                             "b200 window: unknown frame (1 range, 2 rows, 3 partition)");
-        }
-    } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
-    return b200_window_state_init_frames(operator_id, c_types, arr_types, n_arrs, n_partition_keys, n_order_keys, order_ascending,
-                                         order_na_last, funcs, nullptr, n_funcs, output_batch_size, device, stream);
-}
-
-void* b200_window_state_init_frames(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                                    int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                                    const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
-                                    int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream) {
-    try {  // this entry's domain: codes 0..15 (the moments entry adds var, std, var_pop and std_pop)
-        for (int f = 0; funcs && f < n_funcs && f < b200::SORT_MAX_COLS; f++)
-            B200_REQUIRE(funcs[f].code >= b200::WN_ROW_NUMBER && funcs[f].code <= b200::WN_NTH_VALUE, "b200 window: unknown function code");
-    } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
-    return b200_window_state_init_moments(operator_id, c_types, arr_types, n_arrs, n_partition_keys, n_order_keys, order_ascending,
-                                          order_na_last, funcs, frames, n_funcs, output_batch_size, device, stream);
-}
-
-void* b200_window_state_init_moments(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                                     int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                                     const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
-                                     int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream) {
-    try {  // this entry's domain: frames 0..4 (the ranges entry adds frame 5); a ranking function, lag or lead with a frame keeps the
-           // constructor's message
-        for (int f = 0; funcs && f < n_funcs && f < b200::SORT_MAX_COLS; f++)
-            if (funcs[f].code >= b200::WN_SUM && funcs[f].code != b200::WN_LAG && funcs[f].code != b200::WN_LEAD)
-                B200_REQUIRE(funcs[f].frame != b200::WF_RANGE_BETWEEN, "b200 window: unknown frame (1 range, 2 rows, 3 partition, 4 rows between)");
-    } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
-    return b200_window_state_init_ranges(operator_id, c_types, arr_types, n_arrs, n_partition_keys, n_order_keys, order_ascending,
-                                         order_na_last, funcs, frames, nullptr, n_funcs, output_batch_size, device, stream);
-}
-
-void* b200_window_state_init_ranges(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                                    int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                                    const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
-                                    const b200_window_range* ranges, int32_t n_funcs, int64_t output_batch_size, int32_t device,
-                                    void* stream) {
-    try {  // this entry's domain: codes 0..19 (the bivariate entry adds covar_samp, covar_pop, corr, regr_slope and regr_intercept)
-        for (int f = 0; funcs && f < n_funcs && f < b200::SORT_MAX_COLS; f++)
-            B200_REQUIRE(funcs[f].code >= b200::WN_ROW_NUMBER && funcs[f].code <= b200::WN_STD_POP, "b200 window: unknown function code");
-    } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
-    return b200_window_state_init_bivariate(operator_id, c_types, arr_types, n_arrs, n_partition_keys, n_order_keys, order_ascending,
-                                            order_na_last, funcs, frames, ranges, n_funcs, output_batch_size, device, stream);
-}
-
-void* b200_window_state_init_bivariate(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                                       int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                                       const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
-                                       const b200_window_range* ranges, int32_t n_funcs, int64_t output_batch_size, int32_t device,
-                                       void* stream) {
-    return b200_window_state_init_nulls(operator_id, c_types, arr_types, n_arrs, n_partition_keys, n_order_keys, order_ascending,
-                                        order_na_last, funcs, frames, ranges, nullptr, n_funcs, output_batch_size, device, stream);
-}
-
-void* b200_window_state_init_nulls(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                                   int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                                   const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
-                                   const b200_window_range* ranges, const int32_t* ignore_nulls, int32_t n_funcs,
-                                   int64_t output_batch_size, int32_t device, void* stream) {
+void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs, int32_t n_partition_keys,
+                             int32_t n_order_keys, const int32_t* order_ascending, const int32_t* order_na_last,
+                             const b200_window_func* funcs, int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream) {
     (void)operator_id;
     return b200::sort_state_new(device, [&]() -> SortState* {
         const int np = n_partition_keys, no = n_order_keys;
@@ -2454,25 +2378,9 @@ void* b200_window_state_init_nulls(int64_t operator_id, const int8_t* c_types, c
             asc[j] = j < np ? 1 : order_ascending[j - np];
             na_last[j] = j < np ? 1 : order_na_last[j - np];
         }
-        return new b200::WindowState(c_types, arr_types, n_arrs, np, np + no, asc, na_last, funcs, frames, ranges, ignore_nulls,
-                                     n_funcs, output_batch_size, device, (cudaStream_t)stream);
+        return new b200::WindowState(c_types, arr_types, n_arrs, np, np + no, asc, na_last, funcs, n_funcs, output_batch_size, device,
+                                     (cudaStream_t)stream);
     });
-}
-
-void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs, int32_t n_partition_keys,
-                             int32_t n_order_keys, const int32_t* order_ascending, const int32_t* order_na_last, const int32_t* funcs,
-                             const int64_t* func_args, int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream) {
-    b200_window_func d[b200::SORT_MAX_COLS] = {};
-    try {
-        B200_REQUIRE(funcs && n_funcs >= 1 && n_funcs <= b200::SORT_MAX_COLS, "b200 window: 1 to 32 functions");
-        for (int f = 0; f < n_funcs; f++) {
-            B200_REQUIRE(funcs[f] >= b200::WN_ROW_NUMBER && funcs[f] <= b200::WN_NTILE, "b200 window: unknown function code");
-            if (funcs[f] == b200::WN_NTILE) B200_REQUIRE(func_args, "b200 window: ntile needs n >= 1");
-            d[f] = b200_window_func{funcs[f], -1, b200::WF_NONE, 0, func_args ? func_args[f] : 0, 0};
-        }
-    } catch (const std::exception& e) { b200::set_last_error(e.what()); return nullptr; }
-    return b200_window_state_init_funcs(operator_id, c_types, arr_types, n_arrs, n_partition_keys, n_order_keys, order_ascending,
-                                        order_na_last, d, n_funcs, output_batch_size, device, stream);
 }
 
 int b200_sort_build_consume_batch(void* state, const b200_table* in_table, int32_t is_last, int32_t* request_input) {

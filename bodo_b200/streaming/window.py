@@ -126,20 +126,20 @@ from .sort import MAX_FULL_SORT_ROWS, MAX_KEYS, SortState
 FUNCS = {"row_number": 0, "rank": 1, "dense_rank": 2, "percent_rank": 3, "cume_dist": 4, "ntile": 5}
 VALUE_FUNCS = {"sum": 6, "count": 7, "mean": 8, "min": 9, "max": 10, "first_value": 11, "last_value": 12, "lag": 13, "lead": 14}
 FRAMES = {"range": 1, "rows": 2, "partition": 3}
-# The frame entry's codes (b200_window_state_init_frames): nth_value, and ROWS BETWEEN start AND end with its UNBOUNDED sentinels.
+# nth_value, and frame 4, ROWS BETWEEN start AND end (b200_window_func.rows), with its UNBOUNDED sentinels.
 FRAME_FUNCS = {"nth_value": 15}
 ROWS_BETWEEN = 4
 UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING = -(1 << 63), (1 << 63) - 1
-# The moments entry's codes (b200_window_state_init_moments): VAR_SAMP, STDDEV_SAMP, VAR_POP and STDDEV_POP.
+# VAR_SAMP, STDDEV_SAMP, VAR_POP and STDDEV_POP.
 MOMENT_FUNCS = {"var": 16, "std": 17, "var_pop": 18, "std_pop": 19}
-# The ranges entry's frame (b200_window_state_init_ranges): RANGE BETWEEN start AND end, with the kinds of b200_window_range.
+# Frame 5, RANGE BETWEEN start AND end (b200_window_func.range), with the kinds of b200_window_range.
 RANGE_BETWEEN = 5
 RANGE_KINDS = {"unbounded_preceding": 0, "preceding": 1, "current_row": 2, "following": 3, "unbounded_following": 4}
 BOUNDED_FUNCS = ("sum", "count", "mean", "min", "max", "first_value", "last_value", "nth_value", "var", "std", "var_pop", "std_pop")
-# The bivariate entry's codes (b200_window_state_init_bivariate): functions of two columns (y, x), x's index in arg.  They take
+# Functions of two columns (y, x), x's index in arg.  They take
 # every frame BOUNDED_FUNCS take.
 BIVARIATE_FUNCS = {"covar_samp": 20, "covar_pop": 21, "corr": 22, "regr_slope": 23, "regr_intercept": 24}
-# The navigation functions that take a trailing "ignore_nulls" / "respect_nulls" marker (b200_window_state_init_nulls).
+# The navigation functions that take a trailing "ignore_nulls" / "respect_nulls" marker (b200_window_func.ignore_nulls).
 NULLS_FUNCS = ("first_value", "last_value", "nth_value", "lag", "lead")
 NULLS_MARKERS = ("ignore_nulls", "respect_nulls")
 _VALUE_NAMES = {c: f for f, c in {**VALUE_FUNCS, **FRAME_FUNCS, **MOMENT_FUNCS, **BIVARIATE_FUNCS}.items()}
@@ -495,18 +495,10 @@ class WindowState(SortState):
         np_ = len(self.partition_by)
         oasc = ffi.new("int32_t[]", [int(a) for a in self.asc[np_:]] or [0])
         onal = ffi.new("int32_t[]", [int(x) for x in self.na_last[np_:]] or [0])
-        fs = ffi.new("b200_window_func[]", len(self.descs))
-        for d, (code, col, frame, valid, arg, bits) in zip(fs, self.descs):
-            d.code, d.col, d.frame, d.default_valid, d.arg, d.default_bits = code, col, frame, valid, arg, bits
-        frs = ffi.new("b200_window_frame[]", len(self.descs))
-        for d, (start, end) in zip(frs, self.frames()):
-            d.start, d.end = start, end
-        rs = ffi.new("b200_window_range[]", len(self.descs))
-        for d, (sk, ek, sb, eb) in zip(rs, self.rdescs):
-            d.start_kind, d.end_kind, d.start_bits, d.end_bits = sk, ek, sb, eb
-        nulls = ffi.new("int32_t[]", [int(x) for x in self.ignore_nulls])
-        h = L.b200_window_state_init_nulls(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs, frs, rs,
-                                           nulls, len(self.descs), self.output_batch_size, self.device, ffi.cast("void*", self.stream))
+        funcs = zip(self.descs, self.frames(), self.rdescs, self.ignore_nulls)
+        fs = ffi.new("b200_window_func[]", [(*d, rows, rng, int(ign)) for d, rows, rng, ign in funcs])
+        h = L.b200_window_state_init(self.operator_id, c_types, a_types, n_cols, np_, len(self.order_by), oasc, onal, fs, len(self.descs),
+                                     self.output_batch_size, self.device, ffi.cast("void*", self.stream))
         return _lib.check_ptr(h, "init_window_state")
 
 

@@ -264,47 +264,75 @@ void* b200_sort_state_init_full(int64_t operator_id, const int8_t* c_types, cons
                                 const int32_t* ascending, const int32_t* na_last, int64_t output_batch_size, int32_t device,
                                 void* stream);
 
-/* Ranking window functions, ROW_NUMBER / RANK / DENSE_RANK / PERCENT_RANK / CUME_DIST / NTILE(n) OVER (PARTITION BY p ORDER BY o),
- * as a third form of the sort state (the reference plans these through its window / MRNF arguments, which the groupby ABI above
- * drops).  The keys are the first n_partition_keys + n_order_keys (0 <= each, 1 <= sum <= 4) of the n_arrs columns, partition keys
- * first; key columns are distinct and of the sort's key types.  PARTITION BY keys sort ascending with NA last; ORDER BY key j takes
- * order_ascending[j] and order_na_last[j].  Two cells of a key are equal when both are NA (a float NaN is NA) or both are valid with
- * equal radix words (-0.0 equals 0.0).  Rows with equal partition keys are a partition; rows of a partition with equal order keys
- * are peers (without ORDER BY every row of a partition is a peer of every other).
- * funcs[i] uses codes local to this library: 0 row_number, 1 rank, 2 dense_rank, 3 percent_rank, 4 cume_dist, 5 ntile;
- * func_args[i] is ntile's n (>= 1) and is ignored for the others (func_args may be NULL without an ntile).  With s the partition
- * size and k the row's 0-based position in it: row_number = k + 1 (ties in arrival order); rank = 1 + rows before the row's first
- * peer; dense_rank = 1 + peer groups before the row's; percent_rank = (rank - 1) / (s - 1), 0.0 when s = 1; cume_dist = rows up to
- * and including the row's last peer / s; ntile: with q = s / n and r = s % n the first r buckets hold q + 1 rows and the others q
- * (buckets 1..s when n > s).  row_number, rank, dense_rank and ntile are INT64, percent_rank and cume_dist FLOAT64 (one IEEE double
- * division of the two integers); all numpy arrays.  The output is every input row once, in the stable sort's order by (partition
- * keys, order keys, arrival): the n_arrs input columns, then one column per function, so `out->cols` of a produce call holds
- * n_arrs + n_funcs descriptors (at most 32).  At most 2^31 rows, as the full sort.  The build-consume, produce, delete and metric
- * entries below serve this form too; metric 9 is the number of partitions.  This entry takes ranking functions only; it is
- * b200_window_state_init_funcs with one descriptor {funcs[i], -1, 0, 0, func_args[i], 0} per function. */
-void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                             int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                             const int32_t* order_na_last, const int32_t* funcs, const int64_t* func_args, int32_t n_funcs,
-                             int64_t output_batch_size, int32_t device, void* stream);
+/* Window functions over (PARTITION BY p ORDER BY o), as a third form of the sort state (the reference plans these through its
+ * window / MRNF arguments, which the groupby ABI above drops).  The keys are the first n_partition_keys + n_order_keys (0 <= each,
+ * 1 <= sum <= 4) of the n_arrs columns, partition keys first; key columns are distinct and of the sort's key types.  PARTITION BY
+ * keys sort ascending with NA last; ORDER BY key j takes order_ascending[j] and order_na_last[j].  Two cells of a key are equal
+ * when both are NA (a float NaN is NA) or both are valid with equal radix words (-0.0 equals 0.0).  Rows with equal partition
+ * keys are a partition; rows of a partition with equal order keys are peers (without ORDER BY every row of a partition is a peer
+ * of every other).
+ * The ranking functions use codes local to this library: 0 row_number, 1 rank, 2 dense_rank, 3 percent_rank, 4 cume_dist, 5 ntile.
+ * With s the partition size and k the row's 0-based position in it: row_number = k + 1 (ties in arrival order); rank = 1 + rows
+ * before the row's first peer; dense_rank = 1 + peer groups before the row's; percent_rank = (rank - 1) / (s - 1), 0.0 when
+ * s = 1; cume_dist = rows up to and including the row's last peer / s; ntile(n): with q = s / n and r = s % n the first r buckets
+ * hold q + 1 rows and the others q (buckets 1..s when n > s).  row_number, rank, dense_rank and ntile are INT64, percent_rank and
+ * cume_dist FLOAT64 (one IEEE double division of the two integers); all numpy arrays. */
 
-/* One window function of b200_window_state_init_funcs.
+/* The bounds of a frame 4 (ROWS BETWEEN start AND end): each UNBOUNDED (the sentinels below) or a signed row offset from the
+ * current row, -2^31 < offset < 2^31: negative PRECEDING, 0 CURRENT ROW, positive FOLLOWING; start <= end when both are offsets.
+ * For row i of the partition [P, pe) (sorted positions) the frame is [lo, hi] with lo = P for an unbounded start, else
+ * max(P, i + start), and hi = pe - 1 for an unbounded end, else min(pe - 1, i + end); it is empty when lo > hi.
+ * (UNBOUNDED, 0) is frame 2 and (UNBOUNDED, UNBOUNDED) frame 3, with the same results. */
+#define B200_WINDOW_UNBOUNDED_PRECEDING INT64_MIN
+#define B200_WINDOW_UNBOUNDED_FOLLOWING INT64_MAX
+typedef struct b200_window_frame {
+    int64_t start, end;
+} b200_window_frame;
+
+/* The bounds of a frame 5 (RANGE BETWEEN start AND end), measured in ORDER BY values.  Kinds: 0 UNBOUNDED PRECEDING,
+ * 1 PRECEDING, 2 CURRENT ROW, 3 FOLLOWING, 4 UNBOUNDED FOLLOWING, with start_kind <= end_kind, start_kind != 4 and end_kind != 0.
+ * The bits of kinds 1 and 3 hold the offset's magnitude k in the key's arithmetic: a non-negative int64 for an integer key, days
+ * for DATE, ns for DATETIME and TIMEDELTA, the bits of a finite, non-negative double for a FLOAT32 / FLOAT64 key; the other kinds'
+ * bits are not read.  For row i of the partition [P, pe) (sorted positions):
+ *   UNBOUNDED is P (start) or pe - 1 (end).  CURRENT ROW is the row's peer group: its first peer (start) or its last peer (end);
+ *   it takes any ORDER BY, including none and several keys.
+ *   k PRECEDING / k FOLLOWING need exactly one ORDER BY key x, an integer (8 to 64 bits, signed or unsigned), FLOAT32, FLOAT64,
+ *   DATE, DATETIME or TIMEDELTA, numpy or nullable (not BOOL).  With x ascending, a k PRECEDING start is the first row of the
+ *   partition's non-NA run with x_j >= x_i - k, a k FOLLOWING end the last row with x_j <= x_i + k, a k PRECEDING end the last row
+ *   with x_j <= x_i - k and a k FOLLOWING start the first row with x_j >= x_i + k; with x descending PRECEDING means larger
+ *   values, so the signs swap.  Integer and temporal keys compare exactly, with no wrap: a bound beyond the type's range reaches
+ *   the end of the non-NA run.  Float keys compare against fl(x_i -+ k) in IEEE double (FLOAT32 widened exactly first), so -0.0
+ *   equals 0.0 and at x_i = +inf a k PRECEDING start is the first +inf row.
+ *   NA and NaN cells are one peer group at one end of the partition (order_na_last).  At an NA row an offset bound is that peer
+ *   group's first (start) or last (end) row; at a non-NA row an offset bound never reaches an NA row, and an offset bound that no
+ *   non-NA row satisfies leaves the frame empty.
+ * The frame is [lo, hi], empty when lo > hi; the definitions of frame 4 over [lo, hi] apply.  (UNBOUNDED PRECEDING, CURRENT ROW)
+ * is frame 1 and (UNBOUNDED PRECEDING, UNBOUNDED FOLLOWING) frame 3, with the same results. */
+typedef struct b200_window_range {
+    int32_t start_kind, end_kind;
+    uint64_t start_bits, end_bits;
+} b200_window_range;
+
+/* One window function of b200_window_state_init.
  *   code: 0 row_number, 1 rank, 2 dense_rank, 3 percent_rank, 4 cume_dist, 5 ntile (the ranking functions above), then the value
- *         functions 6 sum, 7 count, 8 mean, 9 min, 10 max, 11 first_value, 12 last_value, 13 lag, 14 lead, 15 nth_value
- *         (b200_window_state_init_frames only), 16 var, 17 std, 18 var_pop, 19 std_pop (b200_window_state_init_moments only),
- *         20 covar_samp, 21 covar_pop, 22 corr, 23 regr_slope, 24 regr_intercept (b200_window_state_init_bivariate only).
+ *         functions 6 sum, 7 count, 8 mean, 9 min, 10 max, 11 first_value, 12 last_value, 13 lag, 14 lead, 15 nth_value,
+ *         16 var, 17 std, 18 var_pop, 19 std_pop, 20 covar_samp, 21 covar_pop, 22 corr, 23 regr_slope, 24 regr_intercept.
  *   col: the input column (0 <= col < n_arrs) a value function reads, any column including a key; -1 for a ranking function and
  *        for count(*).
  *   frame: 0 for a ranking function, lag and lead; for the others 1 range (RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW: up
  *          to the row's last peer; the whole partition without ORDER BY), 2 rows (ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT
  *          ROW: up to the row itself, ties in arrival order), 3 partition (the whole partition).  Frames 1..3 start at the
- *          partition's first row.  4 rows between (b200_window_state_init_frames only): ROWS BETWEEN start AND end of the
- *          function's b200_window_frame, for sum, count (of a column or count(*)), mean, min, max, first_value, last_value,
- *          nth_value, var, std, var_pop and std_pop.  5 range between (b200_window_state_init_ranges only): RANGE BETWEEN start
- *          AND end of the function's b200_window_range, for the same functions.
+ *          partition's first row.  4 rows between: ROWS BETWEEN start AND end of the function's rows.  5 range between: RANGE
+ *          BETWEEN start AND end of the function's range.  Every value function other than lag and lead takes frames 1..5.
  *   arg: ntile's n (>= 1); lag / lead's offset k (0 <= k < 2^31; k = 0 is the row itself); nth_value's n (1 <= n < 2^31); the
- *        second column (x, 0 <= arg < n_arrs) of codes 20..24, whose first column (y) is col.
+ *        second column (x, 0 <= arg < n_arrs; any column including a key, and the two may be the same) of codes 20..24, whose
+ *        first column (y) is col.  Not read by the other codes.
  *   default_valid, default_bits: lag / lead's value when row i - k / i + k is outside the row's partition: the low bytes of
  *          default_bits in the column's type if default_valid, else NA.
+ *   rows: the bounds of frame 4, read only when frame == 4.
+ *   range: the bounds of frame 5, read only when frame == 5.
+ *   ignore_nulls: non-zero marks the function IGNORE NULLS, 0 RESPECT NULLS; a non-zero flag is accepted for codes 11 first_value,
+ *          12 last_value, 13 lag, 14 lead and 15 nth_value only.
  * Over a frame [P, e] (a float NaN is NA for the aggregates):
  *   count     non-NA cells, or e - P + 1 for count(*); INT64, numpy.
  *   sum       sum of the non-NA cells, NA when there are none; integers and bool wrap in 64 bits (INT64 for signed and bool,
@@ -334,116 +362,41 @@ void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const i
  *             corr 1.0 exactly where Sxx > 0 (and Sxx^2 is normal), equal x gives Sxx = 0 exactly; a valid NaN when the
  *             frame's counted pairs hold +-inf.  FLOAT64, nullable.  Not for temporal columns.
  * Every row that shares a frame end gets a bit-identical result.
- * Over a frame 4 [lo, hi] (below) the same definitions hold with lo in place of P and hi in place of e; an empty frame (lo > hi)
+ * Over a frame 4 or 5 [lo, hi] the same definitions hold with lo in place of P and hi in place of e; an empty frame (lo > hi)
  * gives NA, and count 0.  Float sums there are combined in an order fixed by (lo, hi) alone, so rows with the same bounds get the
- * same bits, across runs and batch splits. */
-typedef struct b200_window_func {
-    int32_t code, col, frame, default_valid;
-    int64_t arg;
-    uint64_t default_bits;
-} b200_window_func;
-
-/* The bounds of a frame 4 (ROWS BETWEEN start AND end): each UNBOUNDED (the sentinels below) or a signed row offset from the
- * current row, -2^31 < offset < 2^31: negative PRECEDING, 0 CURRENT ROW, positive FOLLOWING; start <= end when both are offsets.
- * For row i of the partition [P, pe) (sorted positions) the frame is [lo, hi] with lo = P for an unbounded start, else
- * max(P, i + start), and hi = pe - 1 for an unbounded end, else min(pe - 1, i + end); it is empty when lo > hi.
- * (UNBOUNDED, 0) is frame 2 and (UNBOUNDED, UNBOUNDED) frame 3, with the same results. */
-#define B200_WINDOW_UNBOUNDED_PRECEDING INT64_MIN
-#define B200_WINDOW_UNBOUNDED_FOLLOWING INT64_MAX
-typedef struct b200_window_frame {
-    int64_t start, end;
-} b200_window_frame;
-
-/* The window state of b200_window_state_init with ranking and value functions, one descriptor each (n_arrs + n_funcs <= 32).  A
- * bad code, column index, frame, ntile n or lag / lead k, a frame on a ranking function, lag or lead, or sum / mean of a temporal
- * column fails here (NULL, last error set).  Function columns follow the input columns in the output, in descriptor order. */
-void* b200_window_state_init_funcs(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                                   int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                                   const int32_t* order_na_last, const b200_window_func* funcs, int32_t n_funcs,
-                                   int64_t output_batch_size, int32_t device, void* stream);
-
-/* b200_window_state_init_funcs with codes 0..15 and frames 0..4: frames[i] is read only when funcs[i].frame == 4 (frames may be
- * NULL when no function uses frame 4).  A bound outside the domain above, start > end, frame 4 on a function other than sum,
- * count, mean, min, max, first_value, last_value and nth_value, or nth_value's n outside [1, 2^31) fails here (NULL, last error
- * set).  b200_window_state_init_funcs is this entry with frames NULL, restricted to codes 0..14 and frames 0..3.  This entry is
- * b200_window_state_init_moments restricted to codes 0..15. */
-void* b200_window_state_init_frames(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                                    int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                                    const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
-                                    int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream);
-
-/* b200_window_state_init_frames with codes 0..19: 16 var, 17 std, 18 var_pop and 19 std_pop (defined above) take a column and
- * frames 1..4, as sum does.  A temporal column fails here (NULL, last error set). */
-void* b200_window_state_init_moments(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                                     int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                                     const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
-                                     int32_t n_funcs, int64_t output_batch_size, int32_t device, void* stream);
-
-/* The bounds of a frame 5 (RANGE BETWEEN start AND end), measured in ORDER BY values.  Kinds: 0 UNBOUNDED PRECEDING,
- * 1 PRECEDING, 2 CURRENT ROW, 3 FOLLOWING, 4 UNBOUNDED FOLLOWING, with start_kind <= end_kind, start_kind != 4 and end_kind != 0.
- * The bits of kinds 1 and 3 hold the offset's magnitude k in the key's arithmetic: a non-negative int64 for an integer key, days
- * for DATE, ns for DATETIME and TIMEDELTA, the bits of a finite, non-negative double for a FLOAT32 / FLOAT64 key; the other kinds'
- * bits are not read.  For row i of the partition [P, pe) (sorted positions):
- *   UNBOUNDED is P (start) or pe - 1 (end).  CURRENT ROW is the row's peer group: its first peer (start) or its last peer (end);
- *   it takes any ORDER BY, including none and several keys.
- *   k PRECEDING / k FOLLOWING need exactly one ORDER BY key x, an integer (8 to 64 bits, signed or unsigned), FLOAT32, FLOAT64,
- *   DATE, DATETIME or TIMEDELTA, numpy or nullable (not BOOL).  With x ascending, a k PRECEDING start is the first row of the
- *   partition's non-NA run with x_j >= x_i - k, a k FOLLOWING end the last row with x_j <= x_i + k, a k PRECEDING end the last row
- *   with x_j <= x_i - k and a k FOLLOWING start the first row with x_j >= x_i + k; with x descending PRECEDING means larger
- *   values, so the signs swap.  Integer and temporal keys compare exactly, with no wrap: a bound beyond the type's range reaches
- *   the end of the non-NA run.  Float keys compare against fl(x_i -+ k) in IEEE double (FLOAT32 widened exactly first), so -0.0
- *   equals 0.0 and at x_i = +inf a k PRECEDING start is the first +inf row.
- *   NA and NaN cells are one peer group at one end of the partition (order_na_last).  At an NA row an offset bound is that peer
- *   group's first (start) or last (end) row; at a non-NA row an offset bound never reaches an NA row, and an offset bound that no
- *   non-NA row satisfies leaves the frame empty.
- * The frame is [lo, hi], empty when lo > hi; the definitions of frame 4 over [lo, hi] apply. */
-typedef struct b200_window_range {
-    int32_t start_kind, end_kind;
-    uint64_t start_bits, end_bits;
-} b200_window_range;
-
-/* b200_window_state_init_moments with frame 5 (range between, code 5): ranges[i] is read only when funcs[i].frame == 5 (ranges
- * may be NULL when no function uses frame 5).  Frame 5 takes sum, count (of a column or count(*)), mean, min, max, first_value,
- * last_value, nth_value, var, std, var_pop and std_pop.  Bad kinds, an offset without exactly one ORDER BY key, an offset on a
- * BOOL key, a negative or non-finite offset, or start after end fails here (NULL, last error set).  (UNBOUNDED PRECEDING, CURRENT
- * ROW) is frame 1 and (UNBOUNDED PRECEDING, UNBOUNDED FOLLOWING) frame 3, with the same results.
- * b200_window_state_init_moments is this entry with ranges NULL, restricted to frames 0..4.  This entry is
- * b200_window_state_init_bivariate restricted to codes 0..19. */
-void* b200_window_state_init_ranges(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                                    int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                                    const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
-                                    const b200_window_range* ranges, int32_t n_funcs, int64_t output_batch_size, int32_t device,
-                                    void* stream);
-
-/* b200_window_state_init_ranges with codes 0..24: 20 covar_samp, 21 covar_pop, 22 corr, 23 regr_slope and 24 regr_intercept
- * (defined above) read two columns, y = col and x = arg (0 <= arg < n_arrs; any column including a key, and the two may be the
- * same), and take frames 1..5, as sum does.  A bad arg or a temporal column in either position fails here (NULL, last error
- * set). */
-void* b200_window_state_init_bivariate(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                                       int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                                       const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
-                                       const b200_window_range* ranges, int32_t n_funcs, int64_t output_batch_size, int32_t device,
-                                       void* stream);
-
-/* b200_window_state_init_bivariate plus one IGNORE NULLS flag per function: ignore_nulls[i] != 0 marks funcs[i] IGNORE NULLS,
- * 0 RESPECT NULLS (the definitions above); ignore_nulls may be NULL, all RESPECT NULLS.  A non-zero flag is accepted for codes
- * 11 first_value, 12 last_value, 13 lag, 14 lead and 15 nth_value only; on any other code it fails here (NULL, last error set).
- * Under IGNORE NULLS a cell is null exactly when count does not count it: its validity is clear or it is a float NaN (RESPECT
- * NULLS first_value returns a NaN as a valid cell; IGNORE NULLS skips it, as pandas' ffill / bfill do).  With row i's frame
- * [lo, hi] and partition [P, pe) as RESPECT NULLS computes them (every frame 1..5, the same empty-frame rule):
+ * same bits, across runs and batch splits.
+ * IGNORE NULLS: a cell is null exactly when count does not count it: its validity is clear or it is a float NaN (RESPECT NULLS
+ * first_value returns a NaN as a valid cell; IGNORE NULLS skips it, as pandas' ffill / bfill do).  With row i's frame [lo, hi]
+ * and partition [P, pe) as RESPECT NULLS computes them (every frame 1..5, the same empty-frame rule):
  *   first_value  the first non-null cell in [lo, hi]; NA if none.
  *   last_value   the last non-null cell in [lo, hi]; NA if none.
  *   nth_value    the n-th non-null cell in [lo, hi] (FROM FIRST); NA if there are fewer than n.
  *   lag          the k-th non-null cell before row i within [P, i); the default if there are fewer than k.
  *   lead         the k-th non-null cell after row i within (i, pe); the default if there are fewer than k.
  * lag / lead with k = 0 are the row itself, as under RESPECT NULLS.  The result keeps the chosen cell's bits (-0.0 stays -0.0);
- * the column's type, nullable.  Results depend only on the sorted positions: bit-identical across runs and batch splits.
- * b200_window_state_init_bivariate is this entry with ignore_nulls NULL. */
-void* b200_window_state_init_nulls(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
-                                   int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
-                                   const int32_t* order_na_last, const b200_window_func* funcs, const b200_window_frame* frames,
-                                   const b200_window_range* ranges, const int32_t* ignore_nulls, int32_t n_funcs,
-                                   int64_t output_batch_size, int32_t device, void* stream);
+ * the column's type, nullable.  Results depend only on the sorted positions: bit-identical across runs and batch splits. */
+typedef struct b200_window_func {
+    int32_t code, col, frame, default_valid;
+    int64_t arg;
+    uint64_t default_bits;
+    b200_window_frame rows;  /* read only when frame == 4 */
+    b200_window_range range; /* read only when frame == 5 */
+    int32_t ignore_nulls;    /* non-zero: IGNORE NULLS; codes 11..15 only */
+} b200_window_func;
+
+/* The window state with n_funcs functions, one descriptor each (n_arrs + n_funcs <= 32).  The output is every input row once,
+ * in the stable sort's order by (partition keys, order keys, arrival): the n_arrs input columns, then one column per function
+ * in descriptor order, so `out->cols` of a produce call holds n_arrs + n_funcs descriptors.  At most 2^31 rows, as the full
+ * sort.  The build-consume, produce, delete and metric entries below serve this form too; metric 9 is the number of partitions.
+ * Fails here (NULL, last error set) on: a bad code, column index, frame, ntile n, lag / lead k or nth_value n (outside
+ * [1, 2^31)); a frame on a ranking function, lag or lead; a frame 4 bound outside the domain above, or start > end; bad frame 5
+ * kinds, an offset without exactly one ORDER BY key, an offset on a BOOL key, a negative or non-finite offset, or start after
+ * end; a bad arg of codes 20..24; sum, mean, var, std, var_pop, std_pop or codes 20..24 over a temporal column (either column
+ * for 20..24); a non-zero ignore_nulls on a code other than 11..15. */
+void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs,
+                             int32_t n_partition_keys, int32_t n_order_keys, const int32_t* order_ascending,
+                             const int32_t* order_na_last, const b200_window_func* funcs, int32_t n_funcs,
+                             int64_t output_batch_size, int32_t device, void* stream);
 
 /* The build-consume entry of _sort.cpp: filters a DEVICE-resident batch (same schema as the state) against the current cutoff on
  * the device (full sort: appends it to the chunk store); on is_last reduces to the final rows (full sort: sorts every row).

@@ -496,7 +496,7 @@ def test_pandas_rolling_cov_corr(gpu_lib, with_na):
 
 
 # ---- the C ABI ----
-def _init(L, entry, cts, descs, n_order=1):
+def _init(L, cts, descs, n_order=1):
     n = len(cts)
     c_types = ffi.new("int8_t[]", cts)
     a_types = ffi.new("int8_t[]", [ArrTypes.NUMPY] * n)
@@ -504,29 +504,25 @@ def _init(L, entry, cts, descs, n_order=1):
     fs = ffi.new("b200_window_func[]", len(descs))
     for d, (code, col, frame, arg) in zip(fs, descs):
         d.code, d.col, d.frame, d.default_valid, d.arg, d.default_bits = code, col, frame, 0, arg, 0
-    frs = ffi.new("b200_window_frame[]", [(W.UNBOUNDED_PRECEDING, W.UNBOUNDED_FOLLOWING)] * len(descs))
-    rs = ffi.new("b200_window_range[]", len(descs))
-    return getattr(L, entry)(-1, c_types, a_types, n, 1, n_order, one, one, fs, frs, rs, len(descs), 1024, 0, ffi.NULL)
+    return L.b200_window_state_init(-1, c_types, a_types, n, 1, n_order, one, one, fs, len(descs), 1024, 0, ffi.NULL)
 
 
 def test_abi_codes_and_validation(gpu_lib):
     L = _lib.lib()
     cts = [CTypes.INT64, CTypes.INT64, CTypes.FLOAT64, CTypes.INT32, CTypes.DATETIME]
     for code in range(20, 25):
-        h = _init(L, "b200_window_state_init_bivariate", cts, [(code, 2, 2, 3)])
+        h = _init(L, cts, [(code, 2, 2, 3)])
         assert h != ffi.NULL, ffi.string(L.b200_last_error()).decode()
         L.b200_delete_sort_state(h)
-        assert _init(L, "b200_window_state_init_ranges", cts, [(code, 2, 2, 3)]) == ffi.NULL
-        assert "unknown function code" in ffi.string(L.b200_last_error()).decode()
     for arg, msg in ((5, "second column index"), (-1, "second column index")):
-        assert _init(L, "b200_window_state_init_bivariate", cts, [(22, 2, 2, arg)]) == ffi.NULL
+        assert _init(L, cts, [(22, 2, 2, arg)]) == ffi.NULL
         assert msg in ffi.string(L.b200_last_error()).decode()
     for col, arg in ((4, 2), (2, 4)):
-        assert _init(L, "b200_window_state_init_bivariate", cts, [(20, col, 1, arg)]) == ffi.NULL
+        assert _init(L, cts, [(20, col, 1, arg)]) == ffi.NULL
         assert "covar, corr and regr need integer, bool or float columns" in ffi.string(L.b200_last_error()).decode()
-    assert _init(L, "b200_window_state_init_bivariate", cts, [(23, 2, 0, 3)]) == ffi.NULL
+    assert _init(L, cts, [(23, 2, 0, 3)]) == ffi.NULL
     assert "unknown frame" in ffi.string(L.b200_last_error()).decode()
-    assert _init(L, "b200_window_state_init_bivariate", cts, [(25, 2, 2, 3)]) == ffi.NULL
+    assert _init(L, cts, [(25, 2, 2, 3)]) == ffi.NULL
     assert "unknown function code" in ffi.string(L.b200_last_error()).decode()
 
 

@@ -389,24 +389,21 @@ def test_device_side_validation(gpu_lib):
     one = ffi.new("int32_t[]", [1])
     UP, UF = W.UNBOUNDED_PRECEDING, W.UNBOUNDED_FOLLOWING
 
-    def init(code, col, frame, arg=0, start=UP, end=UF, frames=True):
+    def init(code, col, frame, arg=0, start=UP, end=UF):
         fs = ffi.new("b200_window_func[]", 1)
         fs[0].code, fs[0].col, fs[0].frame, fs[0].arg = code, col, frame, arg
-        frs = ffi.new("b200_window_frame[]", 1)
-        frs[0].start, frs[0].end = start, end
-        h = L.b200_window_state_init_frames(-1, c_types, a_types, 2, 1, 0, one, one, fs, frs if frames else ffi.NULL, 1, 1024, 0,
-                                            ffi.NULL)
+        fs[0].rows.start, fs[0].rows.end = start, end
+        h = L.b200_window_state_init(-1, c_types, a_types, 2, 1, 0, one, one, fs, 1, 1024, 0, ffi.NULL)
         if h != ffi.NULL:
             L.b200_delete_sort_state(h)
             return None
         return ffi.string(L.b200_last_error()).decode()
 
-    assert init(6, 0, 4, 0, -3, 0) is None and init(15, 1, 1, 2) is None and init(7, -1, 4, 0, 0, 0, True) is None
-    assert init(15, 0, 4, 1, UP, 5) is None and init(11, 0, 2, frames=False) is None and init(9, 0, 4, 0, -(2 ** 31 - 1), 2 ** 31 - 1) is None
+    assert init(6, 0, 4, 0, -3, 0) is None and init(15, 1, 1, 2) is None and init(7, -1, 4, 0, 0, 0) is None
+    assert init(15, 0, 4, 1, UP, 5) is None and init(11, 0, 2) is None and init(9, 0, 4, 0, -(2 ** 31 - 1), 2 ** 31 - 1) is None
     assert "nth_value needs n" in init(15, 0, 1, 0)
     assert "nth_value needs n" in init(15, 0, 1, 1 << 31)
     assert "column index out of range" in init(15, -1, 1, 1)
-    assert "needs frames" in init(6, 0, 4, frames=False)
     assert "row offset" in init(6, 0, 4, 0, -(1 << 31), 0)
     assert "row offset" in init(6, 0, 4, 0, 0, 1 << 31)
     assert "row offset" in init(6, 0, 4, 0, UF, UF)
@@ -414,6 +411,6 @@ def test_device_side_validation(gpu_lib):
     assert "start after frame end" in init(6, 0, 4, 0, 2, 1)
     assert "lag and lead take no frame" in init(13, 0, 4, 1)
     assert "no column and no frame" in init(0, -1, 4)
-    assert "unknown frame" in init(6, 0, 5)
-    assert "unknown function code" in init(16, 0, 1)
+    assert "unknown frame" in init(6, 0, 6)
+    assert "unknown function code" in init(25, 0, 1)
     assert "sum and mean need" in init(8, 1, 4, 0, -1, 1)

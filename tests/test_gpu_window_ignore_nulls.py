@@ -17,7 +17,6 @@ from bodo_b200.streaming import window as W
 from bodo_b200.table import ArrTypes, Column, CTypes, Table
 from tests import test_gpu_window_frames as F
 from tests import test_gpu_window_ranges as R
-from tests.helpers import table_to_device
 from tests.test_gpu_sort import KEY_TYPES, col_mask, make_column
 from tests.test_gpu_window_values import TILE, _default_for, _sorted_col, bounds, run
 
@@ -410,28 +409,23 @@ def test_pandas_ffill_bfill(gpu_lib, dtype):
 
 
 # ---- the C ABI ----
-def _init(L, entry, cts, descs, nulls=None):
+def _init(L, cts, descs, nulls=None):
     n = len(cts)
     c_types = ffi.new("int8_t[]", cts)
     a_types = ffi.new("int8_t[]", [ArrTypes.NUMPY] * n)
     one = ffi.new("int32_t[]", [1])
     fs = ffi.new("b200_window_func[]", len(descs))
-    for d, (code, col, frame, arg) in zip(fs, descs):
-        d.code, d.col, d.frame, d.default_valid, d.arg, d.default_bits = code, col, frame, 0, arg, 0
-    frs = ffi.new("b200_window_frame[]", [(W.UNBOUNDED_PRECEDING, W.UNBOUNDED_FOLLOWING)] * len(descs))
-    rs = ffi.new("b200_window_range[]", len(descs))
-    args = [-1, c_types, a_types, n, 1, 1, one, one, fs, frs, rs]
-    if entry == "b200_window_state_init_nulls":
-        args.append(ffi.NULL if nulls is None else ffi.new("int32_t[]", nulls))
-    return getattr(L, entry)(*args, len(descs), 1024, 0, ffi.NULL)
+    for d, (code, col, frame, arg), ign in zip(fs, descs, nulls or [0] * len(descs)):
+        d.code, d.col, d.frame, d.default_valid, d.arg, d.default_bits, d.ignore_nulls = code, col, frame, 0, arg, 0, ign
+    return L.b200_window_state_init(-1, c_types, a_types, n, 1, 1, one, one, fs, len(descs), 1024, 0, ffi.NULL)
 
 
 def test_abi_flags_and_validation(gpu_lib):
     L = _lib.lib()
     cts = [CTypes.INT64, CTypes.INT64, CTypes.FLOAT64, CTypes.INT32]
     descs = [(0, -1, 0, 0), (11, 2, 2, 0), (12, 2, 3, 0), (13, 2, 0, 1), (14, 3, 0, 2), (15, 2, 1, 2), (6, 2, 2, 0), (22, 2, 2, 3)]
-    for nulls in (None, [0] * 8, [0, 1, 1, 1, 1, 1, 0, 0], [0, 7, -1, 1, 1, 1, 0, 0]):
-        h = _init(L, "b200_window_state_init_nulls", cts, descs, nulls)
+    for nulls in ([0] * 8, [0, 1, 1, 1, 1, 1, 0, 0], [0, 7, -1, 1, 1, 1, 0, 0]):
+        h = _init(L, cts, descs, nulls)
         assert h != ffi.NULL, ffi.string(L.b200_last_error()).decode()
         L.b200_delete_sort_state(h)
     for j, (code, *_rest) in enumerate(descs):
@@ -439,47 +433,9 @@ def test_abi_flags_and_validation(gpu_lib):
             continue
         flags = [0] * len(descs)
         flags[j] = 1
-        assert _init(L, "b200_window_state_init_nulls", cts, descs, flags) == ffi.NULL
+        assert _init(L, cts, descs, flags) == ffi.NULL
         assert "IGNORE NULLS takes first_value, last_value, lag, lead and nth_value only" in ffi.string(L.b200_last_error()).decode()
-    for entry in ("b200_window_state_init_nulls", "b200_window_state_init_bivariate"):
-        assert _init(L, entry, cts, [(25, 2, 2, 3)]) == ffi.NULL
-        assert "unknown function code" in ffi.string(L.b200_last_error()).decode()
+    assert _init(L, cts, [(25, 2, 2, 3)]) == ffi.NULL
+    assert "unknown function code" in ffi.string(L.b200_last_error()).decode()
 
 
-class _Entry:
-    """The library with b200_window_state_init_nulls routed to `how`: "null" (ignore_nulls NULL), "zeros" (an all-zero array) or
-    "bivariate" (b200_window_state_init_bivariate, which has no ignore_nulls parameter)."""
-
-    def __init__(self, L, how):
-        self.L, self.how = L, how
-
-    def __getattr__(self, a):
-        return getattr(self.L, a)
-
-    def b200_window_state_init_nulls(self, *args):
-        head, flags, tail = args[:11], args[11], args[12:]
-        if self.how == "bivariate":
-            return self.L.b200_window_state_init_bivariate(*head, *tail)
-        return self.L.b200_window_state_init_nulls(*head, ffi.NULL if self.how == "null" else ffi.new("int32_t[]", [0] * tail[0]), *tail)
-
-
-def test_abi_null_flags_equal_the_bivariate_entry(gpu_lib):
-    """A NULL ignore_nulls, an all-zero one and the bivariate entry give the same bits."""
-    rng = np.random.default_rng(3000)
-    n = 5000
-    t = Table([make_column(CTypes.INT16, n, rng, False), make_column(CTypes.INT32, n, rng, True),
-               value_column(CTypes.FLOAT64, n, rng, True, 0.5)], ["g", "o", "x"])
-    fs = [("f", "first_value", "x", "rows"), ("l", "last_value", "x", ("rows", -2, 0)), ("lg", "lag", "x", 2), ("n", "nth_value", "x", 2),
-          ("k", "corr", "x", "o", "partition"), ("r", "first_value", "x", ("range_between", -3, 0))]
-    outs = {}
-    for how in ("null", "zeros", "bivariate"):
-        st = W.init_window_state(-1, ["g"], ["o"], True, "last", fs, t.names)
-        st._new_handle = lambda L, *a, st=st, how=how: W.WindowState._new_handle(st, _Entry(L, how), *a)
-        W.window_build_consume_batch(st, table_to_device(t), True)
-        out, _ = W.window_produce_output_batch(st)
-        outs[how] = [(c.values_numpy().copy(), col_mask(c).copy()) for c in out.columns]
-        W.delete_window_state(st)
-    for how in ("zeros", "bivariate"):
-        for a, b in zip(outs["null"], outs[how]):
-            np.testing.assert_array_equal(a[0].view(np.uint8), b[0].view(np.uint8))
-            np.testing.assert_array_equal(a[1], b[1])

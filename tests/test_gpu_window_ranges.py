@@ -382,25 +382,14 @@ def test_device_side_validation(gpu_lib):
     L = _lib.lib()
     one = ffi.new("int32_t[]", [1, 1])
 
-    def init(code, col, frame, kinds=(1, 2), bits=(1, 0), cts=(CTypes.INT64, CTypes.INT64), n_order=1, entry="ranges", ranges=True):
+    def init(code, col, frame, kinds=(1, 2), bits=(1, 0), cts=(CTypes.INT64, CTypes.INT64), n_order=1):
         c_types = ffi.new("int8_t[]", list(cts) + [CTypes.INT64])
         a_types = ffi.new("int8_t[]", [ArrTypes.NUMPY] * (len(cts) + 1))
         fs = ffi.new("b200_window_func[]", 1)
         fs[0].code, fs[0].col, fs[0].frame, fs[0].arg = code, col, frame, 1
-        frs = ffi.new("b200_window_frame[]", 1)
-        frs[0].start, frs[0].end = W.UNBOUNDED_PRECEDING, W.UNBOUNDED_FOLLOWING
-        rs = ffi.new("b200_window_range[]", 1)
-        rs[0].start_kind, rs[0].end_kind, rs[0].start_bits, rs[0].end_bits = kinds[0], kinds[1], bits[0], bits[1]
+        fs[0].range.start_kind, fs[0].range.end_kind, fs[0].range.start_bits, fs[0].range.end_bits = kinds[0], kinds[1], bits[0], bits[1]
         np_ = len(cts) - n_order
-        if entry == "ranges":
-            h = L.b200_window_state_init_ranges(-1, c_types, a_types, len(cts) + 1, np_, n_order, one, one, fs, frs,
-                                                rs if ranges else ffi.NULL, 1, 1024, 0, ffi.NULL)
-        elif entry == "moments":
-            h = L.b200_window_state_init_moments(-1, c_types, a_types, len(cts) + 1, np_, n_order, one, one, fs, frs, 1, 1024, 0, ffi.NULL)
-        elif entry == "frames":
-            h = L.b200_window_state_init_frames(-1, c_types, a_types, len(cts) + 1, np_, n_order, one, one, fs, frs, 1, 1024, 0, ffi.NULL)
-        else:
-            h = L.b200_window_state_init_funcs(-1, c_types, a_types, len(cts) + 1, np_, n_order, one, one, fs, 1, 1024, 0, ffi.NULL)
+        h = L.b200_window_state_init(-1, c_types, a_types, len(cts) + 1, np_, n_order, one, one, fs, 1, 1024, 0, ffi.NULL)
         if h != ffi.NULL:
             L.b200_delete_sort_state(h)
             return None
@@ -408,10 +397,9 @@ def test_device_side_validation(gpu_lib):
 
     dbl = int(np.float64(0.5).view(np.uint64))
     assert init(6, 2, 5) is None and init(15, 2, 5) is None and init(16, 2, 5, (0, 3), (0, 9)) is None
-    assert init(7, -1, 5, (2, 4), ranges=True, cts=(CTypes.INT64, CTypes.BOOL)) is None  # no offset: any key
+    assert init(7, -1, 5, (2, 4), cts=(CTypes.INT64, CTypes.BOOL)) is None  # no offset: any key
     assert init(6, 2, 5, (1, 3), (dbl, dbl), cts=(CTypes.INT64, CTypes.FLOAT32)) is None
     assert init(6, 2, 5, (1, 1), (5, 5)) is None and init(6, 2, 5, (3, 3), (2, 2)) is None
-    assert "needs ranges" in init(6, 2, 5, ranges=False)
     for kinds in ((4, 4), (0, 0), (3, 1), (-1, 2), (2, 5)):
         assert "range bound kinds" in init(6, 2, 5, kinds)
     assert "exactly one ORDER BY key" in init(6, 2, 5, n_order=2)
@@ -424,11 +412,6 @@ def test_device_side_validation(gpu_lib):
     assert "start after frame end" in init(6, 2, 5, (3, 3), (5, 2))
     assert "lag and lead take no frame" in init(13, 2, 5)
     assert "no column and no frame" in init(0, -1, 5)
-    for entry in ("moments", "frames", "funcs"):  # the older entries keep refusing frame 5
-        assert "unknown frame" in init(6, 2, 5, entry=entry)
-        # and keep their messages for a frame on lag / lead or a ranking function
-        assert "lag and lead take no frame" in init(13, 2, 5, entry=entry)
-        assert "no column and no frame" in init(0, -1, 5, entry=entry)
     assert "unknown frame (1 range, 2 rows, 3 partition, 4 rows between, 5 range between)" in init(6, 2, 6)
 
 

@@ -518,7 +518,7 @@ def test_device_side_validation(gpu_lib):
         fs = ffi.new("b200_window_func[]", max(1, n_funcs))
         for d in fs:
             d.code, d.col, d.frame, d.arg, d.default_valid = code, col, frame, arg, valid
-        h = L.b200_window_state_init_funcs(-1, c_types, a_types, 2, 1, 0, one, one, fs, n_funcs, 1024, 0, ffi.NULL)
+        h = L.b200_window_state_init(-1, c_types, a_types, 2, 1, 0, one, one, fs, n_funcs, 1024, 0, ffi.NULL)
         if h != ffi.NULL:
             L.b200_delete_sort_state(h)
             return None
@@ -530,11 +530,11 @@ def test_device_side_validation(gpu_lib):
     assert "lag and lead take no frame" in init(14, 0, 1)
     assert "no column and no frame" in init(1, -1, 2)
     assert "unknown frame" in init(6, 0, 0)
-    assert "unknown frame" in init(11, 0, 4)
+    assert "unknown frame" in init(11, 0, 6)
     assert "sum and mean need" in init(8, 1, 1)
     assert "offset k" in init(13, 0, 0, 1 << 31)
     assert "offset k" in init(14, 0, 0, -1)
-    assert "unknown function code" in init(15, 0, 1)
+    assert "unknown function code" in init(25, 0, 1)
     assert "at most 32" in init(7, 0, 1, n_funcs=31)
 
 

@@ -105,8 +105,7 @@ def test_header_documents_the_codes_and_declares_the_entry():
     assert "16 var, 17 std, 18 var_pop, 19 std_pop" in header
     assert "16 var = M2 / (m - 1), NA when m < 2" in header and "18 var_pop = M2 / m, NA when m = 0" in header
     assert "17 std = sqrt(var)" in header and "19 std_pop = sqrt(var_pop)" in header
-    assert "b200_window_state_init_moments restricted to codes 0..15" in header
-    assert "b200_window_state_init_moments" in set(_lib.declared_symbols())
+    assert [s for s in _lib.declared_symbols() if s.startswith("b200_window_state_init")] == ["b200_window_state_init"]
     assert "13 lag, 14 lead, 15 nth_value" in header
 
 

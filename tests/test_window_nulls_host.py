@@ -7,7 +7,7 @@ import re
 import pytest
 
 from bodo_b200 import _lib
-from bodo_b200._lib import B200Error
+from bodo_b200._lib import B200Error, ffi
 from bodo_b200.physical import PhysicalWindow
 from bodo_b200.streaming import window as W
 from bodo_b200.table import CTypes
@@ -135,19 +135,18 @@ def test_header_defines_ignore_nulls_and_declares_the_entry():
     with open(_lib.HEADER) as f:
         text = f.read()
     header = " ".join(re.sub(r"\n\s*\*", " ", text).split())
-    assert "b200_window_state_init_nulls" in set(_lib.declared_symbols())
-    assert "b200_window_state_init_bivariate is this entry with ignore_nulls NULL" in header
+    assert [s for s in _lib.declared_symbols() if s.startswith("b200_window_state_init")] == ["b200_window_state_init"]
     assert "codes 11 first_value, 12 last_value, 13 lag, 14 lead and 15 nth_value only" in header
     assert "its validity is clear or it is a float NaN" in header
     for d in ("first_value the first non-null cell in [lo, hi]; NA if none", "last_value the last non-null cell in [lo, hi]; NA if none",
               "nth_value the n-th non-null cell in [lo, hi] (FROM FIRST)", "lag the k-th non-null cell before row i within [P, i)",
               "lead the k-th non-null cell after row i within (i, pe)"):
         assert d in header, d
-    decl = re.search(r"void\* b200_window_state_init_nulls\(([^;]*)\);", text).group(1)
-    assert "const b200_window_range* ranges, const int32_t* ignore_nulls, int32_t n_funcs" in " ".join(decl.split())
+    decl = re.search(r"void\* b200_window_state_init\(([^;]*)\);", text).group(1)
+    assert "const b200_window_func* funcs, int32_t n_funcs" in " ".join(decl.split())
+    assert dict(ffi.typeof("b200_window_func").fields)["ignore_nulls"].type is ffi.typeof("int32_t")
     # the RESPECT NULLS sentences stay as they were
     assert "first_value, last_value the cell at P / e as it is (bits and validity: a NaN stays a valid NaN)" in header
-    assert "b200_window_state_init_ranges with codes 0..24" in header
 
 
 def test_physical_window_passes_the_marker_through():
