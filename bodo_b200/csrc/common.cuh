@@ -17,8 +17,12 @@ enum CType : int { CT_INT8 = 0, CT_UINT8 = 1, CT_INT32 = 2, CT_UINT32 = 3, CT_IN
                    CT_TIMEDELTA = 16 };
 enum ArrType : int { ARR_NUMPY = 0, ARR_NULLABLE = 2 };
 // Bodo_FTypes (reference: bodo/libs/groupby/_groupby_ftypes.h:17-110)
-enum FType : int { FT_SIZE = 4, FT_SUM = 6, FT_COUNT = 7, FT_NUNIQUE = 8, FT_MEAN = 14, FT_MIN = 15, FT_MAX = 16, FT_FIRST = 18, FT_LAST = 19,
-                   FT_VAR_POP = 22, FT_STD_POP = 23, FT_VAR = 24, FT_STD = 25, FT_SKEW = 27 };
+// 28..34 continue the enum after skew in the reference's order; they are recalled, not read from a reference checkout (17 and 26
+// are fixed by their neighbours).
+enum FType : int { FT_SIZE = 4, FT_SUM = 6, FT_COUNT = 7, FT_NUNIQUE = 8, FT_MEAN = 14, FT_MIN = 15, FT_MAX = 16, FT_PROD = 17, FT_FIRST = 18,
+                   FT_LAST = 19, FT_VAR_POP = 22, FT_STD_POP = 23, FT_VAR = 24, FT_STD = 25, FT_KURTOSIS = 26, FT_SKEW = 27,
+                   FT_BOOLOR_AGG = 28, FT_BOOLAND_AGG = 29, FT_BOOLXOR_AGG = 30, FT_BITOR_AGG = 31, FT_BITAND_AGG = 32, FT_BITXOR_AGG = 33,
+                   FT_COUNT_IF = 34 };
 
 // hash seeds (reference: bodo/libs/_array_hash.h:8-14)
 constexpr uint32_t SEED_HASH_PARTITION = 0xb0d01289u;
@@ -52,7 +56,16 @@ __host__ __device__ inline int ctype_size(int ct) {
         default: return 0;
     }
 }
+inline const char* ctype_name(int ct) {
+    switch (ct) {
+        case CT_INT8: return "int8"; case CT_UINT8: return "uint8"; case CT_INT16: return "int16"; case CT_UINT16: return "uint16";
+        case CT_INT32: return "int32"; case CT_UINT32: return "uint32"; case CT_INT64: return "int64"; case CT_UINT64: return "uint64";
+        case CT_FLOAT32: return "float32"; case CT_FLOAT64: return "float64"; case CT_BOOL: return "bool"; case CT_DATE: return "date";
+        case CT_DATETIME: return "datetime"; case CT_TIMEDELTA: return "timedelta"; default: return "unknown";
+    }
+}
 __host__ __device__ inline bool ctype_is_float(int ct) { return ct == CT_FLOAT32 || ct == CT_FLOAT64; }
+__host__ __device__ inline bool ctype_is_temporal(int ct) { return ct == CT_DATE || ct == CT_DATETIME || ct == CT_TIMEDELTA; }
 __host__ __device__ inline bool ctype_is_signed_int(int ct) {
     return ct == CT_INT8 || ct == CT_INT16 || ct == CT_INT32 || ct == CT_INT64 || ct == CT_DATE || ct == CT_DATETIME ||
            ct == CT_TIMEDELTA;

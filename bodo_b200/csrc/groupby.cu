@@ -21,6 +21,7 @@
 #include <vector>
 
 #include <cooperative_groups.h>
+#include <cooperative_groups/reduce.h>
 
 #include "common.cuh"
 
@@ -30,10 +31,10 @@ constexpr long long EMPTY_KEY = (long long)0x8000000000000000ULL;  // INT64_MIN 
 constexpr int MAX_OPS = 16;
 constexpr int64_t CHUNK_ROWS = 1ll << 28;  // rows per consume chunk (bounds the fail list of the direct path at 1 GiB)
 
-// var / std / var_pop / std_pop / skew accumulate the moments of d = x - c about a per-group shift c: K_SHIFT holds c (NaN until
-// the group's first non-NA value CASes itself in; c never changes after that), K_MOM1 holds sum d (a0) and the count (a1), K_MOM2
-// sum d^2, K_MOM3 sum d^3.  The four are consecutive primitives, K_SHIFT first: apply_ops and combine_apply carry d (or the
-// partial's shift difference) in registers from K_SHIFT to the sums after it.  When the values lie within a factor of 2 of c,
+// var / std / var_pop / std_pop / skew / kurtosis accumulate the moments of d = x - c about a per-group shift c: K_SHIFT holds c
+// (NaN until the group's first non-NA value CASes itself in; c never changes after that), K_MOM1 holds sum d (a0) and the count
+// (a1), K_MOM2 sum d^2, K_MOM3 sum d^3, K_MOM4 sum d^4.  They are consecutive primitives, K_SHIFT first: apply_ops and
+// combine_apply carry d (or the partial's shift difference) in registers from K_SHIFT to the sums after it.  When the values lie within a factor of 2 of c,
 // x - c is exact (Sterbenz), so a large common offset (epoch seconds, prices in cents) costs no digits.
 enum OpKind : int { K_SUM_I64 = 0, K_SUM_F64, K_COUNT, K_SIZE, K_MEAN, K_MIN_I64, K_MAX_I64, K_MIN_F64, K_MAX_F64,
                     K_MOM2, K_MOM3,
@@ -44,7 +45,16 @@ enum OpKind : int { K_SUM_I64 = 0, K_SUM_F64, K_COUNT, K_SIZE, K_MEAN, K_MIN_I64
                     // evaluation-only kinds of composite functions (accumulators: K_MOM1 + K_MOM2 (+ K_MOM3))
                     E_VAR, E_STD, E_VAR_POP, E_STD_POP, E_SKEW,
                     K_SHIFT, K_MOM1,
-                    K_MRNF };  // one word of a min_row_number_filter winner record (see mrnf_merge_kernel); no consume kernel applies it
+                    K_MRNF,  // one word of a min_row_number_filter winner record (see mrnf_merge_kernel); no consume kernel applies it
+                    // prod: a0 = product (uint64 mod 2^64 / double bits), starts at 1; no native atomic (see prod_update)
+                    K_PROD_I64, K_PROD_F64,
+                    K_MOM4,  // sum d^4 of a moment group (kurtosis), after K_MOM3
+                    // 64-bit word ops: bitor / bitand / bitxor of the integer value (AND starts all-ones) and boolor / booland of its
+                    // truth (0 or all-ones); a1 (when present) counts the non-NA rows
+                    K_OR, K_AND, K_XOR, K_LOR, K_LAND,
+                    K_COUNT_IF,  // a0 = rows whose value is true (nonzero); a1 (when present) counts the non-NA rows
+                    // evaluation-only kinds: kurtosis (accumulators K_MOM1 .. K_MOM4), boolxor (K_COUNT_IF: exactly one true)
+                    E_KURT, E_BOOLXOR };
 constexpr unsigned long long SHIFT_UNSET = 0x7ff8000000000000ull;  // K_SHIFT's initial value (quiet NaN; NaN values are skipped)
 
 struct OpDesc {
@@ -155,8 +165,147 @@ __device__ __forceinline__ double group_shift(double* c, double v) {
     return prev == SHIFT_UNSET ? v : __longlong_as_double((long long)prev);
 }
 
+// prod has no native atomic, and a CAS loop on one word completes about one update per round trip to L2, however many warps wait.
+// So a batch into few groups is multiplied together on chip first: the lanes of the warp that update the same word multiply their
+// values (labeled_partition on the word's address: lanes of different aggregates can run this code together), then the warp's
+// leader multiplies that into the CTA's entry for the word (ProdCache, shared memory), and the consume kernel multiplies every
+// entry into its word once, at its end (prod_flush).  A word that finds no entry (more distinct words than the cache holds near
+// its hash) takes the CAS loop on its global word directly, as the exchange's combine does.  Integers multiply as uint64 (exact
+// mod 2^64 in any order), floats as doubles (the order is the only difference from a serial product).
+constexpr int PC_SLOTS = 128, PC_PROBES = 8;
+constexpr unsigned long long PC_FREE = 0, PC_BUSY = 2;  // entry keys: free, being filled, or word address | 1 for a float word
+struct ProdCache {
+    unsigned long long key[PC_SLOTS];
+    unsigned long long val[PC_SLOTS];
+};
+template <bool F>
+__device__ __forceinline__ unsigned long long prod_mul(unsigned long long a, unsigned long long b) {
+    return F ? (unsigned long long)__double_as_longlong(__longlong_as_double((long long)a) * __longlong_as_double((long long)b)) : a * b;
+}
+// *p *= v by CAS; a failed CAS backs off before it retries, so that a word many CTAs flush into at once is not flooded with CASes
+// that carry a stale value
+template <bool F>
+__device__ __forceinline__ void prod_cas(unsigned long long* p, unsigned long long v, bool shared_word) {
+    unsigned long long old = shared_word ? *(volatile unsigned long long*)p : __ldcg(p), seen;
+    unsigned int pause = 32;
+    for (;;) {
+        seen = old;
+        const unsigned long long next = prod_mul<F>(seen, v);
+        if (next == seen) return;
+        old = atomicCAS(p, seen, next);
+        if (old == seen) return;
+        if (!shared_word) {
+            __nanosleep(pause);
+            pause = pause < 4096 ? 2 * pause : pause;
+        }
+    }
+}
+template <bool F>
+__device__ __forceinline__ void prod_update(unsigned long long* p, unsigned long long v, ProdCache* pc) {
+    namespace cg = cooperative_groups;
+    const cg::coalesced_group same = cg::labeled_partition(cg::coalesced_threads(), (unsigned long long)p);
+    if constexpr (F) v = (unsigned long long)__double_as_longlong(cg::reduce(same, __longlong_as_double((long long)v), [](double x, double y) { return x * y; }));
+    else v = cg::reduce(same, v, [](unsigned long long x, unsigned long long y) { return x * y; });
+    if (same.thread_rank() != 0) return;
+    if (pc) {
+        const unsigned long long key = (unsigned long long)p | (F ? 1ull : 0ull);
+        unsigned int h = (unsigned int)(key_hash((long long)key) >> 32) & (PC_SLOTS - 1);
+        for (int probe = 0; probe < PC_PROBES;) {
+            const unsigned long long k = *(volatile unsigned long long*)&pc->key[h];
+            if (k == key) { prod_cas<F>(&pc->val[h], v, true); return; }
+            if (k == PC_BUSY) continue;  // being filled: look again
+            if (k == PC_FREE) {
+                if (atomicCAS(&pc->key[h], PC_FREE, PC_BUSY) == PC_FREE) {  // the entry starts at this warp's product
+                    pc->val[h] = v;
+                    __threadfence_block();
+                    atomicExch(&pc->key[h], key);
+                    return;
+                }
+                continue;  // somebody else took it: look at it again
+            }
+            h = (h + 1) & (PC_SLOTS - 1);
+            probe++;
+        }
+    }
+    prod_cas<F>(p, v, false);
+}
+// A consume kernel's cache around its row loop: `on` (some op is a prod; uniform over the CTA) clears it before the loop, then
+// multiplies every entry into its word after the loop.
+__device__ __forceinline__ void prod_cache_clear(ProdCache& pc, bool on) {
+    if (!on) return;
+    for (int i = threadIdx.x; i < PC_SLOTS; i += blockDim.x) pc.key[i] = PC_FREE;
+    __syncthreads();
+}
+__device__ __forceinline__ void prod_flush(ProdCache& pc, bool on) {
+    if (!on) return;
+    __syncthreads();
+    for (int i = threadIdx.x; i < PC_SLOTS; i += blockDim.x) {
+        const unsigned long long k = pc.key[i];
+        if (k == PC_FREE) continue;
+        if (k & 1ull) prod_cas<true>((unsigned long long*)(k & ~7ull), pc.val[i], false);
+        else prod_cas<false>((unsigned long long*)k, pc.val[i], false);
+    }
+}
 template <typename A>
-__device__ __forceinline__ void apply_ops(const A& a, uint64_t slot, int64_t row) {
+__host__ __device__ __forceinline__ bool has_prod(const A& a) {
+    for (int j = 0; j < a.n_ops; j++) if (a.ops[j].kind == K_PROD_I64 || a.ops[j].kind == K_PROD_F64) return true;
+    return false;
+}
+// the dynamic shared memory of a consume launch: the ProdCache only when it applies a prod, so that other signatures keep the
+// whole L1 / shared split they had
+template <typename A> size_t prod_smem_bytes(const A& a) { return has_prod(a) ? sizeof(ProdCache) : 0; }
+template <typename A> bool has_reduction_kinds(const A& a) {
+    for (int j = 0; j < a.n_ops; j++) if (a.ops[j].kind > K_MRNF) return true;
+    return false;
+}
+// The operand of a word op (K_OR .. K_COUNT_IF): the integer for bitor / bitand / bitxor, else the value's truth as 0 or all-ones
+// (nonzero is true).  False for an NA value (NaN).
+__device__ __forceinline__ bool word_operand(const OpDesc& op, int64_t row, unsigned long long& w) {
+    if (ctype_is_float(op.in_ctype)) {
+        const double v = load_as_f64(op.in_data, op.in_ctype, row);
+        w = v != 0.0 ? ~0ull : 0ull;
+        return !isnan(v);
+    }
+    w = (unsigned long long)load_int_as_i64(op.in_data, op.in_ctype, row);
+    if (op.kind != K_OR && op.kind != K_AND && op.kind != K_XOR) w = w ? ~0ull : 0ull;
+    return true;
+}
+// One row's word op on `p`.  An OR / XOR with 0 and an AND with all-ones cannot change the word, so those rows only count.
+__device__ __forceinline__ void word_update(int kind, unsigned long long* p, unsigned long long w) {
+    switch (kind) {
+        case K_AND: case K_LAND: if (w != ~0ull) atomicAnd(p, w); break;
+        case K_COUNT_IF: if (w) atomicAdd(p, 1ull); break;
+        case K_XOR: if (w) atomicXor(p, w); break;
+        default: if (w) atomicOr(p, w); break;  // K_OR, K_LOR
+    }
+}
+
+// One row's update of prod, a word op or count_if.
+__device__ __forceinline__ void apply_reduction_op(const OpDesc& op, uint64_t slot, int64_t row, ProdCache* pc) {
+    switch (op.kind) {
+        case K_PROD_I64:
+            prod_update<false>((unsigned long long*)op.a0 + slot, (unsigned long long)load_int_as_i64(op.in_data, op.in_ctype, row), pc);
+            break;
+        case K_PROD_F64: {
+            const double v = load_as_f64(op.in_data, op.in_ctype, row);
+            if (!isnan(v)) prod_update<true>((unsigned long long*)op.a0 + slot, (unsigned long long)__double_as_longlong(v), pc);
+            break;
+        }
+        case K_OR: case K_AND: case K_XOR: case K_LOR: case K_LAND: case K_COUNT_IF: {
+            unsigned long long w;
+            if (!word_operand(op, row, w)) break;
+            word_update(op.kind, (unsigned long long*)op.a0 + slot, w);
+            if (op.a1) atomicAdd((unsigned long long*)op.a1 + slot, 1ull);
+            break;
+        }
+    }
+}
+
+// RED: the launch applies some kind appended after K_MRNF (prod, kurtosis's K_MOM4, the word ops, count_if).  The consume kernels
+// are instantiated for both values and the host picks one per state (has_reduction_kinds), so the other signatures run the row
+// loop they ran before these kinds existed.
+template <bool RED, typename A>
+__device__ __forceinline__ void apply_ops(const A& a, uint64_t slot, int64_t row, ProdCache* pc) {
     double d = 0.0;  // K_SHIFT -> K_MOM*: the row's value minus its group's shift
     bool has_d = false;
 #pragma unroll 1
@@ -205,6 +354,12 @@ __device__ __forceinline__ void apply_ops(const A& a, uint64_t slot, int64_t row
             case K_MOM2: case K_MOM3:
                 if (has_d) atomicAdd((double*)op.a0 + slot, op.kind == K_MOM2 ? d * d : d * d * d);
                 break;
+            default:
+                if constexpr (RED) {
+                    if (op.kind == K_MOM4) { if (has_d) atomicAdd((double*)op.a0 + slot, (d * d) * (d * d)); }
+                    else apply_reduction_op(op, slot, row, pc);  // prod, the word ops, count_if
+                }
+                break;
             case K_FIRST: case K_LAST: {  // phase 1: which row supplies the value (phase 2 writes it, groupby_firstlast_fix_kernel)
                 unsigned long long bits;
                 if (firstlast_value(op, row, bits)) {
@@ -243,7 +398,12 @@ __device__ __forceinline__ void apply_ops(const A& a, uint64_t slot, int64_t row
 }
 
 // Generic fused consume kernel: any key/value types, any mix of aggregates, nullable columns.
+template <bool RED>
 __global__ void __launch_bounds__(256) groupby_consume_kernel(const __grid_constant__ ConsumeArgs a) {
+    extern __shared__ __align__(8) unsigned char prod_smem[];  // a ProdCache when some op is a prod (prod_smem_bytes), else empty
+    ProdCache& pc = *reinterpret_cast<ProdCache*>(prod_smem);
+    const bool prod = RED && has_prod(a);
+    prod_cache_clear(pc, prod);
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < a.n_rows; i += stride) {
         int64_t row = a.index_list ? (int64_t)a.index_list[i] : i;
@@ -267,8 +427,9 @@ __global__ void __launch_bounds__(256) groupby_consume_kernel(const __grid_const
                 }
             }
         }
-        apply_ops(a, slot, row);
+        apply_ops<RED>(a, slot, row, &pc);
     }
+    prod_flush(pc, prod);
 }
 
 // first / last, phase 2 (after every row of the launch — replays included — has been applied): the row whose sequence number
@@ -421,6 +582,7 @@ struct OutDesc {
     const void* a1;
     const void* b0;  // composite functions: sum of squares
     const void* c0;  //                      sum of cubes
+    const void* d0;  //                      sum of fourth powers
     void* out_data;
     uint32_t* out_valid;  // validity bitmap as 32-bit words, or nullptr when the column has no nulls
 };
@@ -519,6 +681,41 @@ __global__ void eval_output_kernel(const __grid_constant__ EvalArgs a) {
                         store_f_typed(op.out_data, op.out_ctype, p, r);
                         break;
                     }
+                    case E_KURT: {  // pandas' nankurt (Fisher's excess kurtosis, bias-corrected) on the power sums of d = x - c
+                        const unsigned long long cnt = ((const unsigned long long*)op.a1)[s];
+                        const double n = (double)cnt, s1 = ((const double*)op.a0)[s], s2 = ((const double*)op.b0)[s];
+                        const double s3 = ((const double*)op.c0)[s], s4 = ((const double*)op.d0)[s];
+                        valid = cnt >= 4;
+                        double r = __longlong_as_double(0x7ff8000000000000ll);
+                        if (valid && isfinite(s1) && isfinite(s2) && isfinite(s3) && isfinite(s4)) {  // (a group holding ±inf: NaN)
+                            const double mean = s1 / n;  // central moments, in which c cancels
+                            const double m2 = s2 - s1 * mean;
+                            const double m4 = s4 - 4.0 * s3 * mean + 6.0 * s2 * mean * mean - 3.0 * s1 * mean * mean * mean;
+                            double num = n * (n + 1.0) * (n - 1.0) * m4, den = (n - 2.0) * (n - 3.0) * m2 * m2;
+                            if (fabs(num) < 1e-14) num = 0.0;
+                            if (fabs(den) < 1e-14) den = 0.0;
+                            r = den == 0.0 ? 0.0 : num / den - 3.0 * (n - 1.0) * (n - 1.0) / ((n - 2.0) * (n - 3.0));
+                        }
+                        store_f_typed(op.out_data, op.out_ctype, p, r);
+                        break;
+                    }
+                    case K_PROD_I64: case K_OR: case K_AND: case K_XOR: {  // (prod: every group valid, 1 when it saw no value)
+                        if (op.a1) valid = ((const unsigned long long*)op.a1)[s] > 0;
+                        store_int_typed(op.out_data, op.out_ctype, p, ((const long long*)op.a0)[s]);
+                        break;
+                    }
+                    case K_PROD_F64:
+                        store_f_typed(op.out_data, op.out_ctype, p, ((const double*)op.a0)[s]);
+                        break;
+                    case K_LOR: case K_LAND: case E_BOOLXOR: {
+                        const unsigned long long w = ((const unsigned long long*)op.a0)[s];
+                        if (op.a1) valid = ((const unsigned long long*)op.a1)[s] > 0;
+                        store_int_typed(op.out_data, CT_BOOL, p, op.kind == E_BOOLXOR ? w == 1 : w != 0);
+                        break;
+                    }
+                    case K_COUNT_IF:
+                        store_int_typed(op.out_data, CT_INT64, p, ((const long long*)op.a0)[s]);
+                        break;
                     case K_FIRST: case K_LAST: {  // NA when the group never saw a non-NA value (nullable / float outputs)
                         const unsigned long long q = ((const unsigned long long*)op.a1)[s];
                         const bool seen = op.kind == K_FIRST ? q != ~0ull : q != 0ull;
@@ -624,7 +821,12 @@ __device__ __forceinline__ uint64_t find_or_insert_mk(const A& a, const long lon
     return ~0ull;
 }
 
+template <bool RED>
 __global__ void __launch_bounds__(256) groupby_consume_mk_kernel(const __grid_constant__ MkArgs a) {
+    extern __shared__ __align__(8) unsigned char prod_smem[];  // a ProdCache when some op is a prod (prod_smem_bytes), else empty
+    ProdCache& pc = *reinterpret_cast<ProdCache*>(prod_smem);
+    const bool prod = RED && has_prod(a);
+    prod_cache_clear(pc, prod);
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < a.n_rows; i += stride) {
         int64_t row = a.index_list ? (int64_t)a.index_list[i] : i;
@@ -642,8 +844,9 @@ __global__ void __launch_bounds__(256) groupby_consume_mk_kernel(const __grid_co
             a.fail_list[f] = (uint32_t)row;
             continue;
         }
-        apply_ops(a, slot, row);
+        apply_ops<RED>(a, slot, row, &pc);
     }
+    prod_flush(pc, prod);
 }
 
 struct RehashMkArgs {
@@ -907,13 +1110,14 @@ __device__ __forceinline__ bool for_each_source_row(const XchgSource& src, F&& f
 // combine step (get_combine_func, groupby/_groupby_update.cpp:41-57): count/size/mean -> sum, min -> min, max -> max
 // merges the accumulator words r[0 ...] of one partial row into `slot`
 // A moment group (K_SHIFT ...) re-centres the partial's sums about its own shift c_s on the slot's shift c_t: with delta = c_s - c_t,
-// sum (d + delta)^k expands to S1 + n delta, S2 + 2 delta S1 + n delta^2, S3 + 3 delta S2 + 3 delta^2 S1 + n delta^3.  A slot without a
+// sum (d + delta)^k expands to S1 + n delta, S2 + 2 delta S1 + n delta^2, S3 + 3 delta S2 + 3 delta^2 S1 + n delta^3,
+// S4 + 4 delta S3 + 6 delta^2 S2 + 4 delta^3 S1 + n delta^4.  A slot without a
 // shift takes c_s (delta = 0); a partial without one (every row of the group was NA on that rank) adds nothing.
 __device__ __forceinline__ void combine_apply(const CombineArgs& a, uint64_t slot, const unsigned long long* r) {
     {
         int w = 0;
         bool mom = false;
-        double delta = 0.0, n_s = 0.0, s1 = 0.0, s2 = 0.0;  // K_SHIFT -> K_MOM*: the partial's moments seen so far
+        double delta = 0.0, n_s = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;  // K_SHIFT -> K_MOM*: the partial's moments seen so far
         for (int j = 0; j < a.n_ops; j++) {
             unsigned long long v0 = r[w++];
             unsigned long long v1 = a.a1[j] ? r[w++] : 0;
@@ -937,8 +1141,21 @@ __device__ __forceinline__ void combine_apply(const CombineArgs& a, uint64_t slo
                     atomicAdd((double*)a.a0[j] + slot, s2 + 2.0 * delta * s1 + n_s * delta * delta);
                     break;
                 case K_MOM3:
-                    if (mom) atomicAdd((double*)a.a0[j] + slot, f0 + 3.0 * delta * s2 + 3.0 * delta * delta * s1 + n_s * delta * delta * delta);
+                    if (!mom) break;
+                    s3 = f0;
+                    atomicAdd((double*)a.a0[j] + slot, s3 + 3.0 * delta * s2 + 3.0 * delta * delta * s1 + n_s * delta * delta * delta);
                     break;
+                case K_MOM4:
+                    if (mom) {
+                        const double d2 = delta * delta;
+                        atomicAdd((double*)a.a0[j] + slot, f0 + 4.0 * delta * s3 + 6.0 * d2 * s2 + 4.0 * d2 * delta * s1 + n_s * d2 * d2);
+                    }
+                    break;
+                case K_PROD_I64: prod_update<false>((unsigned long long*)a.a0[j] + slot, v0, nullptr); break;
+                case K_PROD_F64: prod_update<true>((unsigned long long*)a.a0[j] + slot, v0, nullptr); break;
+                // word ops: the partial's word is itself an operand (0 / all-ones for the truth ops); true-counts add
+                case K_OR: case K_AND: case K_XOR: case K_LOR: case K_LAND: word_update(a.kinds[j], (unsigned long long*)a.a0[j] + slot, v0); break;
+                case K_COUNT_IF: atomicAdd((unsigned long long*)a.a0[j] + slot, v0); break;
                 case K_MEAN:
                     atomicAdd((double*)a.a0[j] + slot, __longlong_as_double((long long)v0));
                     atomicAdd((unsigned long long*)a.a1[j] + slot, v1);
@@ -1897,7 +2114,7 @@ __global__ void __launch_bounds__(LC_THREADS, MIN_CTAS) groupby_lowcard_kernel(c
 struct OutSpec {
     int ftype;
     int kind;        // OpKind used by eval_output_kernel
-    int prim[3];
+    int prim[4];
     int n_prim;
     int out_ctype, out_arrtype;
 };
@@ -2076,14 +2293,47 @@ class GroupbyState {
             bool isf = ctype_is_float(f.in_ctype);
             f.has_a1 = false;
             f.init0 = 0;
+            // a refusal of the input column's type by the function `name`, which takes `takes`
+            auto refuse_type = [&](bool ok, const char* name, const char* takes) {
+                B200_REQUIRE(ok, std::string("b200 groupby: ") + name + " does not take a " + ctype_name(f.in_ctype) + " column (column " +
+                                     std::to_string(f.in_col) + "; it takes " + takes + ")");
+            };
             // output typing: get_groupby_output_dtype (groupby/_groupby_common.cpp:561-668)
             switch (f.ftype) {
                 case FT_SIZE: f.kind = K_SIZE; f.out_ctype = CT_INT64; f.out_arrtype = ARR_NUMPY; break;
                 case FT_COUNT: f.kind = K_COUNT; f.out_ctype = CT_INT64; f.out_arrtype = ARR_NUMPY; break;
-                case FT_SUM:
-                    f.kind = isf ? K_SUM_F64 : K_SUM_I64;
+                case FT_SUM: case FT_PROD:
+                    if (f.ftype == FT_PROD) refuse_type(!ctype_is_temporal(f.in_ctype), "prod", "integer, bool and float columns");
+                    f.kind = f.ftype == FT_SUM ? (isf ? K_SUM_F64 : K_SUM_I64) : (isf ? K_PROD_F64 : K_PROD_I64);
                     f.out_ctype = isf ? f.in_ctype : (ctype_is_signed_int(f.in_ctype) || f.in_ctype == CT_BOOL ? CT_INT64 : CT_UINT64);
                     f.out_arrtype = f.in_ctype == CT_BOOL ? ARR_NULLABLE : f.in_arrtype;
+                    if (f.ftype == FT_PROD) f.init0 = isf ? 0x3FF0000000000000ull : 1ull;  // 1.0 / 1: an empty product
+                    break;
+                case FT_BOOLOR_AGG: case FT_BOOLAND_AGG: case FT_BOOLXOR_AGG: {
+                    // nonzero is true; NA (and NaN) rows are skipped; a group without a non-NA value is NA.  boolxor counts the
+                    // true values: true iff exactly one is
+                    const bool band = f.ftype == FT_BOOLAND_AGG;
+                    refuse_type(!ctype_is_temporal(f.in_ctype), band ? "booland_agg" : f.ftype == FT_BOOLOR_AGG ? "boolor_agg" : "boolxor_agg",
+                                "bool, integer and float columns");
+                    f.kind = band ? K_LAND : f.ftype == FT_BOOLOR_AGG ? K_LOR : K_COUNT_IF;
+                    f.out_ctype = CT_BOOL; f.out_arrtype = ARR_NULLABLE;
+                    f.has_a1 = f.in_arrtype == ARR_NULLABLE || isf;
+                    f.init0 = band ? ~0ull : 0ull;
+                    break;
+                }
+                case FT_BITOR_AGG: case FT_BITAND_AGG: case FT_BITXOR_AGG: {
+                    const bool band = f.ftype == FT_BITAND_AGG;
+                    refuse_type(!isf && f.in_ctype != CT_BOOL && !ctype_is_temporal(f.in_ctype),
+                                band ? "bitand_agg" : f.ftype == FT_BITOR_AGG ? "bitor_agg" : "bitxor_agg", "integer columns");
+                    f.kind = band ? K_AND : f.ftype == FT_BITOR_AGG ? K_OR : K_XOR;
+                    f.out_ctype = f.in_ctype; f.out_arrtype = ARR_NULLABLE;
+                    f.has_a1 = f.in_arrtype == ARR_NULLABLE;
+                    f.init0 = band ? ~0ull : 0ull;
+                    break;
+                }
+                case FT_COUNT_IF:
+                    refuse_type(f.in_ctype == CT_BOOL, "count_if", "bool columns");
+                    f.kind = K_COUNT_IF; f.out_ctype = CT_INT64; f.out_arrtype = ARR_NUMPY;
                     break;
                 case FT_MEAN: f.kind = K_MEAN; f.out_ctype = CT_FLOAT64; f.out_arrtype = ARR_NULLABLE; f.has_a1 = true; break;
                 case FT_MIN: case FT_MAX: {
@@ -2113,38 +2363,43 @@ class GroupbyState {
                     f.has_a1 = true; f.init1 = f.ftype == FT_FIRST ? ~0ull : 0ull;
                     has_firstlast = true;
                     break;
-                case FT_VAR: case FT_STD: case FT_VAR_POP: case FT_STD_POP: case FT_SKEW: {
-                    // composite: the moment group of its input column (K_SHIFT, K_MOM1, K_MOM2 (, K_MOM3 when some skew reads
-                    // the column)), shared by every composite over that column
+                case FT_VAR: case FT_STD: case FT_VAR_POP: case FT_STD_POP: case FT_SKEW: case FT_KURTOSIS: {
+                    // composite: the moment group of its input column (K_SHIFT, K_MOM1, K_MOM2 (, K_MOM3 when some skew or kurtosis
+                    // reads the column (, K_MOM4 when some kurtosis does))), shared by every composite over that column
                     OutSpec o{};
                     o.ftype = f.ftype;
-                    o.kind = f.ftype == FT_VAR ? E_VAR : f.ftype == FT_STD ? E_STD : f.ftype == FT_VAR_POP ? E_VAR_POP : f.ftype == FT_STD_POP ? E_STD_POP : E_SKEW;
+                    o.kind = f.ftype == FT_VAR ? E_VAR : f.ftype == FT_STD ? E_STD : f.ftype == FT_VAR_POP ? E_VAR_POP : f.ftype == FT_STD_POP ? E_STD_POP
+                           : f.ftype == FT_SKEW ? E_SKEW : E_KURT;
                     o.out_ctype = CT_FLOAT64; o.out_arrtype = ARR_NULLABLE;
                     int g = 0;
                     while (g < (int)funcs.size() && !(funcs[g].kind == K_SHIFT && funcs[g].in_col == f.in_col)) g++;
                     if (g == (int)funcs.size()) {
-                        bool skew = false;
-                        for (int q = 0; q < n_outs; q++)
-                            skew |= ftypes[q] == FT_SKEW && f_in_offsets[q + 1] > f_in_offsets[q] && f_in_cols[f_in_offsets[q]] == f.in_col;
-                        const int kinds[4] = {K_SHIFT, K_MOM1, K_MOM2, K_MOM3};
-                        for (int q = 0; q < (skew ? 4 : 3); q++) {
+                        bool skew = false, kurt = false;
+                        for (int q = 0; q < n_outs; q++) {
+                            if (f_in_offsets[q + 1] == f_in_offsets[q] || f_in_cols[f_in_offsets[q]] != f.in_col) continue;
+                            skew |= ftypes[q] == FT_SKEW;
+                            kurt |= ftypes[q] == FT_KURTOSIS;
+                        }
+                        const int kinds[5] = {K_SHIFT, K_MOM1, K_MOM2, K_MOM3, K_MOM4};
+                        for (int q = 0; q < (kurt ? 5 : skew ? 4 : 3); q++) {
                             FuncSpec pf = f;
                             pf.kind = kinds[q]; pf.has_a1 = kinds[q] == K_MOM1; pf.out_ctype = CT_FLOAT64; pf.out_arrtype = ARR_NULLABLE;
                             pf.init0 = kinds[q] == K_SHIFT ? SHIFT_UNSET : 0ull;
                             funcs.push_back(pf);
                         }
                     }
-                    o.n_prim = f.ftype == FT_SKEW ? 3 : 2;
-                    for (int q = 0; q < o.n_prim; q++) o.prim[q] = g + 1 + q;  // eval reads K_MOM1 (sum, count), K_MOM2 (, K_MOM3)
+                    o.n_prim = f.ftype == FT_KURTOSIS ? 4 : f.ftype == FT_SKEW ? 3 : 2;
+                    for (int q = 0; q < o.n_prim; q++) o.prim[q] = g + 1 + q;  // eval reads K_MOM1 (sum, count), K_MOM2 (, K_MOM3 (, K_MOM4))
                     outs.push_back(o);
                     continue;
                 }
                 default:
                     throw Error("b200 groupby: unsupported aggregate function ftype=" + std::to_string(f.ftype) +
-                                " (supported: size, sum, count, nunique, mean, min, max, first, last, var, std, var_pop, std_pop, skew)");
+                                " (supported: size, sum, count, nunique, mean, min, max, prod, first, last, var, std, var_pop, std_pop, "
+                                "kurtosis, skew, boolor_agg, booland_agg, boolxor_agg, bitor_agg, bitand_agg, bitxor_agg, count_if)");
             }
             OutSpec o{};
-            o.ftype = f.ftype; o.kind = f.kind; o.prim[0] = (int)funcs.size(); o.n_prim = 1; o.out_ctype = f.out_ctype; o.out_arrtype = f.out_arrtype;
+            o.ftype = f.ftype; o.kind = f.ftype == FT_BOOLXOR_AGG ? E_BOOLXOR : f.kind; o.prim[0] = (int)funcs.size(); o.n_prim = 1; o.out_ctype = f.out_ctype; o.out_arrtype = f.out_arrtype;
             outs.push_back(o);
             funcs.push_back(f);
         }
@@ -2296,7 +2551,8 @@ class GroupbyState {
             for (int j = 0; j < nk; j++) { a.key_data[j] = data[j]; a.key_valid[j] = valid[j]; a.key_ctype[j] = c_types[j]; }
             a.n_ops = n_apply();
             fill_ops(a.ops, data, valid);
-            groupby_consume_mk_kernel<<<grid_for(rows), 256, 0, stream>>>(a);
+            if (has_reduction_kinds(a)) groupby_consume_mk_kernel<true><<<grid_for(rows), 256, prod_smem_bytes(a), stream>>>(a);
+            else groupby_consume_mk_kernel<false><<<grid_for(rows), 256, 0, stream>>>(a);
             launches++; consume_launches += index_list == nullptr;
             B200_CUDA(cudaGetLastError());
         };
@@ -2815,7 +3071,8 @@ class GroupbyState {
                 });
             } else {
                 ConsumeArgs a = generic_args(data, valid, index_list, rows);
-                groupby_consume_kernel<<<grid_for(rows), 256, 0, stream>>>(a);
+                if (has_reduction_kinds(a)) groupby_consume_kernel<true><<<grid_for(rows), 256, prod_smem_bytes(a), stream>>>(a);
+                else groupby_consume_kernel<false><<<grid_for(rows), 256, 0, stream>>>(a);
             }
             launches++;
             if (index_list == nullptr) consume_launches++;
@@ -3230,6 +3487,7 @@ class GroupbyState {
             e.ops[j].a1 = funcs[p0].has_a1 ? d_a1[p0].p : nullptr; e.ops[j].out_data = d_out_data[j].p;
             e.ops[j].b0 = o.n_prim > 1 ? d_a0[o.prim[1]].p : nullptr;
             e.ops[j].c0 = o.n_prim > 2 ? d_a0[o.prim[2]].p : nullptr;
+            e.ops[j].d0 = o.n_prim > 3 ? d_a0[o.prim[3]].p : nullptr;
             if (o.out_arrtype == ARR_NULLABLE) { d_out_valid[j].ensure(words * 4); e.ops[j].out_valid = d_out_valid[j].as<uint32_t>(); }
         }
         eval_output_kernel<<<grid_for(max_out), 256, 0, stream>>>(e);

@@ -887,14 +887,6 @@ struct GrowCol {  // growable device column (geometric growth, copy on grow)
     void reserve(size_t n) { if (n > buf.bytes) { B200_REQUIRE(used == 0, "internal: reserve after append"); buf.alloc(n); } }
 };
 
-static const char* ctype_name(int ct) {
-    switch (ct) {
-        case CT_INT8: return "int8"; case CT_UINT8: return "uint8"; case CT_INT16: return "int16"; case CT_UINT16: return "uint16";
-        case CT_INT32: return "int32"; case CT_UINT32: return "uint32"; case CT_INT64: return "int64"; case CT_UINT64: return "uint64";
-        case CT_FLOAT32: return "float32"; case CT_FLOAT64: return "float64"; case CT_BOOL: return "bool"; case CT_DATE: return "date";
-        case CT_DATETIME: return "datetime"; case CT_TIMEDELTA: return "timedelta"; default: return "unknown";
-    }
-}
 // f(std::integral_constant<int, v>) for the one v in [0, N) equal to `v`: the kernel instantiation a runtime argument selects
 template <typename F, int... I> void with_int_seq(int v, F&& f, std::integer_sequence<int, I...>) {
     ((v == I ? f(std::integral_constant<int, I>{}) : void()), ...);

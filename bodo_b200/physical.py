@@ -396,7 +396,10 @@ def run_pipeline(source, between: Iterable, sink) -> None:
 def groupby_agg(df, by, aggs: Sequence[tuple], dropna: bool = True, batch_size: int = STREAMING_BATCH_SIZE, **kw):
     """df.groupby(by, as_index=False, dropna=dropna).agg(...) through the streaming operators.
 
-    aggs: [(out_name, column, func)] with func in {'sum','count','mean','min','max','size'}.
+    aggs: [(out_name, column, func)] with func one of streaming.groupby.FTYPES: 'size', 'sum', 'count', 'nunique', 'mean', 'min',
+    'max', 'prod', 'first', 'last', 'var', 'std', 'var_pop', 'std_pop', 'skew', 'kurtosis', 'boolor_agg', 'booland_agg',
+    'boolxor_agg', 'bitor_agg', 'bitand_agg', 'bitxor_agg', 'count_if' (no pandas aliases: 'any' / 'all' give False for an all-NA
+    group, where boolor_agg / booland_agg give NA).
     Returns a pandas DataFrame (group order unspecified, as in the reference)."""
     by = [by] if isinstance(by, str) else list(by)
     cols = list(df.columns)
