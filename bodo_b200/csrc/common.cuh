@@ -348,4 +348,9 @@ struct DevBuf {
 };
 using PooledBuf = DevBuf;
 
+// Stable ascending radix sort of rows [0, n) by n_keys (1..4) plain device columns without NAs, key j at data[j] encoded by
+// keys[j] (sort_word), through the full sort's histogram and pass kernels (sort.cu), on stream `st`.  Returns the permutation in
+// ids[0] or ids[1] (mask each entry with 0x7FFFFFFF), or nullptr for the identity (every digit constant, or n == 0).
+const uint32_t* radix_sort_columns(int n_keys, const void* const* data, const SortKey* keys, int64_t n, DevBuf (&ids)[2], cudaStream_t st);
+
 }  // namespace b200

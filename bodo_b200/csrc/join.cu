@@ -20,6 +20,7 @@
 // Keys: the first n_keys (1..4) columns of each side.  One key column can take the unique-key tables (Slot16 / Slot32); a
 // multi-column key always takes the CSR form, whose key table holds (tuple-hash tag, first build row) words (the _mk kernels).
 #include <algorithm>
+#include <cmath>
 #include <type_traits>
 #include <utility>
 #include <vector>
@@ -157,13 +158,28 @@ __device__ __forceinline__ JoinKey load_join_key(const void* __restrict__ p, int
     }
 }
 
-// BuildHashTable: slot per distinct key, num_rows_in_group, build_row_to_group_map (= row_slot)
-template <bool FK>
+// The as-of join's `on` column of one side: a build column (validity one byte per row, nullptr = none) or a probe column (Arrow
+// bitmap).  A null cell and a NaN are NA: such a row takes part in no match.
+struct AsofOn { const void* data; const uint8_t* valid; SortKey key; };
+template <bool BYTES>
+__device__ __forceinline__ uint64_t asof_word(const AsofOn& o, int64_t i, bool& na) {
+    na = BYTES ? (o.valid && !o.valid[i]) : !bit_valid(o.valid, i);
+    return sort_word(o.key, load_bits(o.data, o.key.size, i), na);
+}
+
+// BuildHashTable: slot per distinct key, num_rows_in_group, build_row_to_group_map (= row_slot).  ASOF: a row whose `on` cell is
+// NA belongs to no group either.
+template <bool FK, bool ASOF>
 __global__ void join_insert_count_kernel(const void* key_data, int key_ctype, const uint8_t* key_valid_bytes, int64_t n,
-                                         long long* tkeys, uint64_t cap, SlotInfo* info, uint32_t* row_slot, int na_equal) {
+                                         long long* tkeys, uint64_t cap, SlotInfo* info, uint32_t* row_slot, int na_equal, const AsofOn on) {
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
         uint32_t s;
+        if constexpr (ASOF) {
+            bool na;
+            asof_word<true>(on, i, na);
+            if (na) { row_slot[i] = J_NONE; continue; }
+        }
         const JoinKey jk = load_join_key<FK>(key_data, key_ctype, i, !key_valid_bytes || key_valid_bytes[i]);
         if (jk.na) {
             if (!na_equal) { row_slot[i] = J_NONE; continue; }  // never matches: belongs to no group
@@ -176,12 +192,13 @@ __global__ void join_insert_count_kernel(const void* key_data, int key_ctype, co
         info[s].first = (uint32_t)i;  // any row of the group; exact when cnt == 1
     }
 }
-__global__ void join_slot_counts_kernel(const SlotInfo* info, uint64_t n_slots, uint32_t* cnt_multi) {
-    // CSR only holds groups with more than one row
+__global__ void join_slot_counts_kernel(const SlotInfo* info, uint64_t n_slots, uint32_t* cnt_multi, uint32_t min_rows) {
+    // the CSR holds the groups of at least min_rows rows: 2 for the equi-join (a group of one keeps its row in the slot), 1 for
+    // the as-of join
     uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
     for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < n_slots; s += stride) {
         uint32_t c = info[s].cnt;
-        cnt_multi[s] = c > 1 ? c : 0;
+        cnt_multi[s] = c >= min_rows ? c : 0;
     }
 }
 // FinalizeGroups: groups[offs[slot] + k] = k-th build row of the slot's key
@@ -200,17 +217,22 @@ __global__ void join_fill_groups_kernel(const uint32_t* row_slot, int64_t n, con
 // build columns; mark[i] says whether it has a match, _join.cpp:3668-3693)
 // key_reject: the probe key is int64 / DATETIME / TIMEDELTA and the build key UINT64, or the other way round.  Keys join by value, so
 // a valid probe key with its top bit set (a negative value, or a uint64 of at least 2^63) has no partner; it is not an NA key.
+// The slot of probe row i's key in the single-key table (J_NONE: no such key).
+template <bool FK>
+__device__ __forceinline__ uint32_t probe_slot(const void* key_data, int key_ctype, const uint8_t* key_valid, int64_t i, const long long* tkeys,
+                                               uint64_t cap, int na_equal, int key_reject) {
+    const JoinKey jk = load_join_key<FK>(key_data, key_ctype, i, bit_valid(key_valid, i));
+    if (jk.na) return na_equal ? (uint32_t)cap : J_NONE;
+    if (!FK && key_reject && jk.key < 0) return J_NONE;
+    return jk.key == J_EMPTY ? (uint32_t)cap + 1 : j_find(tkeys, cap, jk.key);
+}
 template <bool FK>
 __global__ void join_probe_count_kernel(const void* key_data, int key_ctype, const uint8_t* key_valid, int64_t n,
                                         const long long* tkeys, uint64_t cap, const SlotInfo* info, int probe_outer,
                                         uint32_t* pslot, uint32_t* pcnt, int na_equal, int mode, uint8_t* mark, int key_reject) {
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
-        uint32_t s;
-        const JoinKey jk = load_join_key<FK>(key_data, key_ctype, i, bit_valid(key_valid, i));
-        if (jk.na) s = na_equal ? (uint32_t)cap : J_NONE;
-        else if (!FK && key_reject && jk.key < 0) s = J_NONE;
-        else s = jk.key == J_EMPTY ? (uint32_t)cap + 1 : j_find(tkeys, cap, jk.key);
+        uint32_t s = probe_slot<FK>(key_data, key_ctype, key_valid, i, tkeys, cap, na_equal, key_reject);
         uint32_t c = s == J_NONE ? 0 : info[s].cnt;
         if (c == 0) s = J_NONE;
         if (mode == 1) { pslot[i] = J_NONE; pcnt[i] = c ? 0u : 1u; continue; }
@@ -665,11 +687,17 @@ __device__ __forceinline__ uint64_t mk_slot(uint64_t h, uint64_t mask) { return 
 __device__ __forceinline__ uint32_t mk_tag(uint64_t h) { return (uint32_t)h; }
 
 // join_insert_count_kernel for a multi-column key: same outputs (row_slot, info[s].cnt, info[s].first)
+template <bool ASOF>
 __global__ void join_insert_count_mk_kernel(const KeySet bk, int64_t n, unsigned long long* table, uint64_t cap, SlotInfo* info,
-                                            uint32_t* row_slot, int na_equal) {
+                                            uint32_t* row_slot, int na_equal, const AsofOn on) {
     const uint64_t mask = cap - 1;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
+        if constexpr (ASOF) {
+            bool na;
+            asof_word<true>(on, i, na);
+            if (na) { row_slot[i] = J_NONE; continue; }
+        }
         const MKRow r = mk_row<true>(bk, i);
         if (r.na && !na_equal) { row_slot[i] = J_NONE; continue; }  // never matches: belongs to no group
         const uint64_t h = mk_hash(r, bk.n_keys);
@@ -689,23 +717,28 @@ __global__ void join_insert_count_mk_kernel(const KeySet bk, int64_t n, unsigned
         info[s].first = (uint32_t)i;  // any row of the group; exact when cnt == 1
     }
 }
+// The slot of probe row i's key tuple in the multi-column key table (J_NONE: no such key).
+__device__ __forceinline__ uint32_t probe_slot_mk(const KeySet& pk, const KeySet& bk, int64_t i, const unsigned long long* __restrict__ table,
+                                                  uint64_t cap, int na_equal, uint32_t key_reject) {
+    const uint64_t mask = cap - 1;
+    const MKRow r = mk_row<false>(pk, i);
+    if ((!r.na || na_equal) && !mk_rejected(r, key_reject)) {
+        const uint64_t h = mk_hash(r, pk.n_keys);
+        for (uint64_t t = mk_slot(h, mask);; t = (t + 1) & mask) {
+            const unsigned long long w = __ldg(table + t);
+            if (w == MK_EMPTY) break;
+            if ((uint32_t)(w >> 32) == mk_tag(h) && mk_equal_build(bk, (uint32_t)w, r)) return (uint32_t)t;
+        }
+    }
+    return J_NONE;
+}
 // join_probe_count_kernel for a multi-column key: same outputs (pslot, pcnt, mark) in modes 0, 1 and 2
 __global__ void join_probe_count_mk_kernel(const KeySet pk, const KeySet bk, int64_t n, const unsigned long long* __restrict__ table,
                                            uint64_t cap, const SlotInfo* info, int probe_outer, uint32_t* pslot, uint32_t* pcnt,
                                            int na_equal, int mode, uint8_t* mark, uint32_t key_reject) {
-    const uint64_t mask = cap - 1;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
-        const MKRow r = mk_row<false>(pk, i);
-        uint32_t s = J_NONE;
-        if ((!r.na || na_equal) && !mk_rejected(r, key_reject)) {
-            const uint64_t h = mk_hash(r, pk.n_keys);
-            for (uint64_t t = mk_slot(h, mask);; t = (t + 1) & mask) {
-                const unsigned long long w = __ldg(table + t);
-                if (w == MK_EMPTY) break;
-                if ((uint32_t)(w >> 32) == mk_tag(h) && mk_equal_build(bk, (uint32_t)w, r)) { s = (uint32_t)t; break; }
-            }
-        }
+        uint32_t s = probe_slot_mk(pk, bk, i, table, cap, na_equal, key_reject);
         uint32_t c = s == J_NONE ? 0 : info[s].cnt;
         if (c == 0) s = J_NONE;
         if (mode == 1) { pslot[i] = J_NONE; pcnt[i] = c ? 0u : 1u; continue; }
@@ -863,6 +896,121 @@ __global__ void __launch_bounds__(256) join_cond_gather_kernel(const __grid_cons
     }
 }
 
+// ---- as-of join (pandas.merge_asof; SQL ASOF JOIN ... MATCH_CONDITION) ----
+// Build: every key group goes into the CSR, groups of one row included (join_slot_counts_kernel with min_rows 1), and a row with
+// an NA `on` cell belongs to no group (the ASOF instantiations of the insert kernels).  radix_sort_columns sorts the build row ids
+// stably by (slot, on word), so groups[goffs[s] ..] lists group s's rows by ascending `on`, ties in arrival order, and
+// join_asof_groups_kernel stores the rows' words beside them (gwords): a probe's binary search reads words, not `on` cells through
+// row ids.  Probe: the key lookup of the equi-join (probe_slot / probe_slot_mk), a binary search of the probe's `on` word in its
+// group's words, the tolerance check, then the gather.  Words order as the values do (sort_word, -0.0 equal to 0.0), and for an
+// integer or temporal column the difference of two words is the exact difference of the values as a uint64.
+enum { ASOF_BACKWARD = 0, ASOF_FORWARD = 1, ASOF_NEAREST = 2 };
+struct AsofArgs {
+    const void* key_data; int key_ctype; const uint8_t* key_valid;  // one key column
+    KeySet pk, bk;                                                   // a multi-column key
+    const void* table;  // the key table: int64 keys, or the multi-column key table's (tag, row) words
+    uint64_t cap; int na_equal; uint32_t key_reject;
+    const SlotInfo* info; const unsigned long long* goffs; const uint32_t* groups; const uint64_t* gwords;
+    AsofOn on;  // the probe's `on` column
+    int direction, allow_exact, has_tol;
+    unsigned long long tol_w;  // integer / temporal column: the tolerance, in word (= value) units
+    double tol_f;              // float column
+};
+// The value of a float column's word (sort_word inverted), as float64.
+__device__ __forceinline__ double asof_float(int ct, uint64_t w) {
+    if (ct == CT_FLOAT64) return __longlong_as_double(canon_float_ordered((long long)(w ^ 0x8000000000000000ull)));
+    const uint32_t x = (uint32_t)w;
+    return (double)__uint_as_float(x >> 31 ? x ^ 0x80000000u : ~x);
+}
+// First position k < c with w[k] > v (strict) or w[k] >= v, else c.
+__device__ __forceinline__ uint32_t asof_first_above(const uint64_t* __restrict__ w, uint32_t c, uint64_t v, bool strict) {
+    uint32_t lo = 0, hi = c;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        const uint64_t x = __ldg(w + mid);
+        if (strict ? x > v : x >= v) hi = mid;
+        else lo = mid + 1;
+    }
+    return lo;
+}
+// The build row probe row i matches, or J_NONE.  KT: 0 one integer key column, 1 one float key column, 2 a multi-column key.
+template <int KT>
+__device__ __forceinline__ uint32_t asof_match(const AsofArgs& a, int64_t i) {
+    uint32_t s;
+    if constexpr (KT == 2) s = probe_slot_mk(a.pk, a.bk, i, (const unsigned long long*)a.table, a.cap, a.na_equal, a.key_reject);
+    else s = probe_slot<KT == 1>(a.key_data, a.key_ctype, a.key_valid, i, (const long long*)a.table, a.cap, a.na_equal, (int)a.key_reject);
+    const uint32_t c = s == J_NONE ? 0 : a.info[s].cnt;
+    if (c == 0) return J_NONE;
+    bool na;
+    const uint64_t v = asof_word<false>(a.on, i, na);
+    if (na) return J_NONE;
+    const unsigned long long g0 = a.goffs[s];
+    const uint64_t* w = a.gwords + g0;
+    // backward candidate: position kb - 1, the last w <= v (w < v without exact matches); forward candidate: kf, the first w >= v
+    // (w > v).  Equal words keep arrival order, so these are the last and the first of a run of ties.
+    const uint32_t kb = a.direction != ASOF_FORWARD ? asof_first_above(w, c, v, a.allow_exact) : 0;
+    const uint32_t kf = a.direction != ASOF_BACKWARD ? asof_first_above(w, c, v, !a.allow_exact) : c;
+    const bool hb = kb > 0, hf = kf < c;
+    if (!hb && !hf) return J_NONE;
+    bool fwd;  // the forward candidate wins: the nearer one, the backward one on a tie (pandas: bdiff <= fdiff keeps backward)
+    if (ctype_is_float(a.on.key.ct)) {
+        const double x = asof_float(a.on.key.ct, v);
+        const double db = hb ? x - asof_float(a.on.key.ct, __ldg(w + kb - 1)) : 0.0, df = hf ? asof_float(a.on.key.ct, __ldg(w + kf)) - x : 0.0;
+        fwd = !hb || (hf && !(db <= df));
+        if (a.has_tol && (fwd ? df : db) > a.tol_f) return J_NONE;
+    } else {
+        const uint64_t db = hb ? v - __ldg(w + kb - 1) : 0, df = hf ? __ldg(w + kf) - v : 0;
+        fwd = !hb || (hf && df < db);
+        if (a.has_tol && (fwd ? df : db) > a.tol_w) return J_NONE;
+    }
+    return a.groups[g0 + (fwd ? kf : kb - 1)];
+}
+// Output row o from probe row i and build row brow, or NULL build cells when brow is J_NONE.
+__device__ __forceinline__ void asof_emit(const GatherArgs& g, int64_t o, int64_t i, uint32_t brow) {
+    for (int k = 0; k < g.n_b; k++) {
+        if (brow == J_NONE) { zero_item(g.ob_data[k], o, g.b_size[k]); g.ob_valid[k][o] = 0; continue; }
+        copy_cell(g.ob_data[k], o, g.b_data[k], brow, g.b_size[k]);
+        if (g.ob_valid[k]) g.ob_valid[k][o] = g.b_valid[k] ? g.b_valid[k][brow] : 1;
+    }
+    for (int k = 0; k < g.n_p; k++) {
+        copy_cell(g.op_data[k], o, g.p_data[k], i, g.p_size[k]);
+        if (g.op_valid[k]) g.op_valid[k][o] = bit_valid(g.p_valid[k], i) ? 1 : 0;
+    }
+}
+// left as-of: output row i is probe row i, in one kernel.  (256, 1): with the block size alone ptxas keeps the multi-column key
+// instantiation at 32 registers and spills.
+template <int KT>
+__global__ void __launch_bounds__(256, 1) join_asof_left_kernel(const __grid_constant__ GatherArgs g, const __grid_constant__ AsofArgs a) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < g.n_probe; i += stride) asof_emit(g, i, i, asof_match<KT>(a, i));
+}
+// inner as-of: the matched build row (J_NONE: none) and a 0 / 1 output count per probe row; the scan, then join_asof_gather_kernel
+template <int KT>
+__global__ void __launch_bounds__(256) join_asof_match_kernel(const __grid_constant__ AsofArgs a, int64_t n, uint32_t* brow, uint32_t* cnt) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
+        const uint32_t b = asof_match<KT>(a, i);
+        brow[i] = b;
+        cnt[i] = b != J_NONE ? 1u : 0u;
+    }
+}
+// g.pslot holds the matched build rows, g.poff the output offsets
+__global__ void __launch_bounds__(256) join_asof_gather_kernel(const __grid_constant__ GatherArgs g) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < g.n_probe; i += stride)
+        if (g.poff[i + 1] != g.poff[i]) asof_emit(g, (int64_t)g.poff[i], i, g.pslot[i]);
+}
+// groups[p] = the p-th build row of the sorted order (ids: the permutation, nullptr = identity), gwords[p] its `on` word
+__global__ void join_asof_groups_kernel(const uint32_t* ids, int64_t n, const AsofOn on, uint32_t* groups, uint64_t* gwords) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < n; p += stride) {
+        const uint32_t r = ids ? ids[p] & 0x7FFFFFFFu : (uint32_t)p;
+        bool na;
+        groups[p] = r;
+        gwords[p] = asof_word<true>(on, r, na);
+    }
+}
+
 // ================================================================================================
 // When `buf` holds fewer than `need` bytes, replaces it by a buffer of max(need, alloc) bytes that keeps its first `keep` bytes.
 static void grow_keep(DevBuf& buf, size_t need, size_t keep, cudaStream_t st, size_t alloc = 0) {
@@ -927,6 +1075,14 @@ class JoinState {
     // non-equi condition (set_condition, before the first build batch): one expression over build column c (arg c) and probe
     // column c (arg J_MAX_COLS + c); empty = none.  d_cond_pairs: candidate pairs evaluated, pairs passed (metrics 8, 9)
     std::vector<ExprInstr> cond;
+    // as-of join (set_asof, before the first build batch): the `on` column of each side, direction, exact matches, tolerance.  The
+    // build keeps every key group in the CSR, sorted by `on`; d_gwords holds the `on` words of the groups' rows.
+    bool asof = false;
+    int asof_b_on = -1, asof_p_on = -1, asof_dir = 0;
+    bool asof_exact = true, asof_has_tol = false;
+    long long asof_tol_i = 0;
+    double asof_tol_f = 0;
+    DevBuf d_gwords;
     DevBuf d_cond_pairs;
     unsigned long long* h_cond_pairs = nullptr;
     int64_t cond_evaluated = 0, cond_passed = 0;
@@ -975,6 +1131,7 @@ class JoinState {
         B200_REQUIRE(ctype_size(b_ct[0]) == ctype_size(p_ct[0]), "b200 join: build and probe key widths differ");
         key_reject = 0;
         for (int j = 0; j < n_keys; j++) key_reject |= signedness_differs(p_ct[j], b_ct[j]) ? 1u << j : 0u;
+        if (asof) check_asof_probe();
         for (const ExprInstr& in : cond)
             B200_REQUIRE(in.op != EX_COL || in.arg < J_MAX_COLS || in.arg - J_MAX_COLS < np,
                          "b200 join: the condition reads probe column " + std::to_string(in.arg - J_MAX_COLS) + " and the probe table has " +
@@ -1033,18 +1190,60 @@ class JoinState {
         B200_REQUIRE(n_build == 0 && !build_final, "b200 join: the join kind must be set before the first build batch");
         B200_REQUIRE(!(is_mark && is_anti), "b200 join: a join is a mark join or an anti join, not both");
         B200_REQUIRE(!(is_mark || is_anti) || !build_outer, "b200 join: mark / anti joins do not emit build rows (build_table_outer must be false)");
+        B200_REQUIRE(!(is_mark || is_anti) || !asof, "b200 join: an as-of join is not a mark or anti join");
         mark = is_mark; anti = is_anti;
     }
     // The non-equi condition: one expression (ending in EX_END) over the columns of both sides.  Build columns are checked here,
     // probe columns here when the probe schema is known and otherwise when the first probe batch brings it.
     void set_condition(const ExprInstr* prog, int n_instr) {
         B200_REQUIRE(n_build == 0 && !build_final, "b200 join: the condition must be set before the first build batch");
+        B200_REQUIRE(!asof, "b200 join: an as-of join takes no non-equi condition");
         const std::string who = "b200 join: set_condition";
         expr_validate(prog, n_instr, [&](int64_t c) {
             return (c >= 0 && c < n_b) || (c >= J_MAX_COLS && c < 2 * J_MAX_COLS && (n_p == 0 || c - J_MAX_COLS < n_p));
         }, who);
         for (int i = 0; i + 1 < n_instr; i++) B200_REQUIRE(prog[i].op != EX_END, who + ": the condition is one expression (one END, at the end)");
         cond.assign(prog, prog + n_instr);
+    }
+    // The as-of join (pandas.merge_asof): each probe row matches at most the one build row of its key group whose `on` value is the
+    // latest at or before its own (backward), the earliest at or after it (forward) or the nearer of those two (nearest).
+    void set_asof(int b_on, int p_on, int dir, bool exact, bool has_tol, long long tol_i, double tol_f) {
+        const std::string who = "b200 join: set_asof: ";
+        B200_REQUIRE(n_build == 0 && !build_final, who + "the as-of join must be set before the first build batch");
+        B200_REQUIRE(!build_outer, who + "a build-outer as-of join is not supported");
+        B200_REQUIRE(!mark && !anti && cond.empty(), who + "an as-of join is not a mark, anti or condition join");
+        B200_REQUIRE(dir >= ASOF_BACKWARD && dir <= ASOF_NEAREST, who + "direction is 0 (backward), 1 (forward) or 2 (nearest)");
+        B200_REQUIRE(b_on >= n_keys && b_on < n_b, who + "the build `on` column must be a non-key column of the build table (got " + std::to_string(b_on) +
+                                                       "; the key columns are 0.." + std::to_string(n_keys - 1) + " of " + std::to_string(n_b) + ")");
+        B200_REQUIRE(p_on >= n_keys && p_on < J_MAX_COLS, who + "the probe `on` column must be a non-key column of the probe table (got " + std::to_string(p_on) + ")");
+        const int ct = b_ct[b_on];
+        B200_REQUIRE(ct != CT_BOOL, who + "the `on` column is " + ctype_name(ct) + "; it must be an integer, float, date, datetime or timedelta column");
+        if (has_tol && ctype_is_float(ct)) B200_REQUIRE(std::isfinite(tol_f) && tol_f >= 0, who + "the tolerance must be finite and >= 0");
+        if (has_tol && !ctype_is_float(ct)) B200_REQUIRE(tol_i >= 0, who + "the tolerance must be >= 0");
+        asof_b_on = b_on; asof_p_on = p_on; asof_dir = dir; asof_exact = exact; asof_has_tol = has_tol; asof_tol_i = tol_i; asof_tol_f = tol_f;
+        if (n_p) check_asof_probe();  // the probe schema is known: check it now, else when the first probe batch brings it
+        asof = true;
+    }
+    void check_asof_probe() const {
+        B200_REQUIRE(asof_p_on < n_p, "b200 join: set_asof: the probe `on` column " + std::to_string(asof_p_on) + " is out of range (the probe table has " +
+                                          std::to_string(n_p) + " columns)");
+        B200_REQUIRE(p_ct[asof_p_on] == b_ct[asof_b_on], std::string("b200 join: set_asof: the probe `on` column is ") + ctype_name(p_ct[asof_p_on]) +
+                                                              " and the build `on` column " + ctype_name(b_ct[asof_b_on]) + "; both sides need the same type");
+    }
+    SortKey asof_key() const { return SortKey{b_ct[asof_b_on], ctype_size(b_ct[asof_b_on]), 0, 1}; }
+    AsofOn asof_build_on() const { return AsofOn{bcol[asof_b_on].buf.p, build_valid(asof_b_on), asof_key()}; }
+    // groups (the CSR of every key group, `total` rows) sorted by `on`, and their words
+    void build_asof_groups(unsigned long long total) {
+        d_gwords.alloc((size_t)std::max<unsigned long long>(total, 1) * 8);
+        if (total == 0) return;
+        const void* cols[2] = {d_row_slot.p, bcol[asof_b_on].buf.p};
+        const SortKey keys[2] = {SortKey{CT_UINT32, 4, 0, 1}, asof_key()};
+        DevBuf ids[2];
+        const uint32_t* perm = radix_sort_columns(2, cols, keys, n_build, ids, stream);
+        join_asof_groups_kernel<<<grid_for((int64_t)total), 256, 0, stream>>>(perm, (int64_t)total, asof_build_on(), d_groups.as<uint32_t>(),
+                                                                              d_gwords.as<uint64_t>());
+        launches++;
+        B200_CUDA(cudaGetLastError());
     }
 
     // ---- runtime join filter ----
@@ -1210,7 +1409,7 @@ class JoinState {
         while (cap < 2ull * (uint64_t)n_build) cap <<= 1;
         uint64_t n_slots = cap + 2;
         // the unique-key tables (Slot32, Slot16) hold one int64 key: a multi-column key always takes the CSR form
-        if (n_keys == 1 && !mark && !anti && cond.empty() && try_inline_build(n_slots)) {
+        if (n_keys == 1 && !mark && !anti && cond.empty() && !asof && try_inline_build(n_slots)) {
             form = TableForm::SLOT32; inline_builds++;
             build_final = true;
             return;
@@ -1222,21 +1421,25 @@ class JoinState {
         d_row_slot.alloc((size_t)std::max<int64_t>(n_build, 1) * 4);
         launches++;
         if (n_build > 0) {
-            if (n_keys > 1)
-                join_insert_count_mk_kernel<<<grid_for(n_build), 256, 0, stream>>>(build_keys(), n_build, d_tkeys.as<unsigned long long>(), cap,
-                                                                                   d_info.as<SlotInfo>(), d_row_slot.as<uint32_t>(), na_equal ? 1 : 0);
-            else
-                with_key([&](auto fk) {
-                    join_insert_count_kernel<fk><<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], build_valid(0), n_build, d_tkeys.as<long long>(), cap,
-                                                                                       d_info.as<SlotInfo>(), d_row_slot.as<uint32_t>(), na_equal ? 1 : 0);
-                });
+            const AsofOn on = asof ? asof_build_on() : AsofOn{};
+            with_int<2>(asof ? 1 : 0, [&](auto as) {
+                if (n_keys > 1)
+                    join_insert_count_mk_kernel<decltype(as)::value == 1><<<grid_for(n_build), 256, 0, stream>>>(build_keys(), n_build, d_tkeys.as<unsigned long long>(), cap,
+                                                                                           d_info.as<SlotInfo>(), d_row_slot.as<uint32_t>(), na_equal ? 1 : 0, on);
+                else
+                    with_key([&](auto fk) {
+                        join_insert_count_kernel<fk, decltype(as)::value == 1><<<grid_for(n_build), 256, 0, stream>>>(bcol[0].buf.p, b_ct[0], build_valid(0), n_build, d_tkeys.as<long long>(),
+                                                                                               cap, d_info.as<SlotInfo>(), d_row_slot.as<uint32_t>(), na_equal ? 1 : 0, on);
+                    });
+            });
             d_cnt_multi.alloc(n_slots * 4);
-            join_slot_counts_kernel<<<grid_for((int64_t)n_slots), 256, 0, stream>>>(d_info.as<SlotInfo>(), n_slots, d_cnt_multi.as<uint32_t>());
+            join_slot_counts_kernel<<<grid_for((int64_t)n_slots), 256, 0, stream>>>(d_info.as<SlotInfo>(), n_slots, d_cnt_multi.as<uint32_t>(), asof ? 1u : 2u);
             launches += 2;
             d_goffs.alloc((n_slots + 1) * 8);
             unsigned long long n_multi = scan.run(d_cnt_multi.as<uint32_t>(), (int64_t)n_slots, d_goffs.as<unsigned long long>(), stream, &launches);
             d_groups.alloc((size_t)std::max<unsigned long long>(n_multi, 1) * 4);
-            if (n_multi > 0) {
+            if (asof) build_asof_groups(n_multi);
+            else if (n_multi > 0) {
                 d_fill.alloc(n_slots * 4);
                 B200_CUDA(cudaMemsetAsync(d_fill.p, 0, n_slots * 4, stream));
                 join_fill_groups_kernel<<<grid_for(n_build), 256, 0, stream>>>(d_row_slot.as<uint32_t>(), n_build, d_info.as<SlotInfo>(), d_goffs.as<unsigned long long>(),
@@ -1244,7 +1447,7 @@ class JoinState {
                 launches++;
             }
             d_cnt_multi.release(); d_fill.release(); d_row_slot.release();
-            if (n_keys == 1 && n_multi == 0 && !build_outer && !probe_outer && !mark && !anti && cond.empty()) {
+            if (n_keys == 1 && n_multi == 0 && !build_outer && !probe_outer && !mark && !anti && cond.empty() && !asof) {
                 // every key (incl. the NA / marker groups) has exactly one build row: set up the fused probe path
                 form = TableForm::SLOT16;
                 setup_slot16();
@@ -1356,6 +1559,66 @@ class JoinState {
         return (int64_t)read_word(d_cursor.as<unsigned long long>());
     }
 
+    // The gather kernels' arguments for a probe batch of n rows: the general path's per-row slots and output offsets, the CSR, and
+    // the kept columns of both sides with their output columns (size_outputs first: it may move them).
+    GatherArgs gather_args(int64_t n, const std::vector<OutCol>& cols, int nkb, const std::vector<const void*>& data,
+                           const std::vector<const uint8_t*>& valid) const {
+        GatherArgs g{};
+        g.n_probe = n; g.pslot = d_pslot.as<uint32_t>(); g.poff = d_poff.as<unsigned long long>(); g.info = d_info.as<SlotInfo>();
+        g.goffs = d_goffs.as<unsigned long long>(); g.groups = d_groups.as<uint32_t>(); g.bmatched = build_outer ? d_bmatched.as<uint8_t>() : nullptr;
+        g.n_b = nkb; g.n_p = (int)cols.size() - nkb;
+        for (int k = 0; k < (int)cols.size(); k++) {
+            const OutCol& c = cols[k];
+            if (c.is_b) {
+                g.b_data[k] = bcol[c.src].buf.p; g.b_valid[k] = build_valid(c.src); g.b_size[k] = c.size;
+                g.ob_data[k] = out_data[k].p; g.ob_valid[k] = out_valid(cols, k);
+            } else {
+                const int j = k - nkb;
+                g.p_data[j] = data[c.src]; g.p_valid[j] = valid[c.src]; g.p_size[j] = c.size;
+                g.op_data[j] = out_data[k].p; g.op_valid[j] = out_valid(cols, k);
+            }
+        }
+        return g;
+    }
+
+    // as-of join: a left as-of batch is one kernel (output row i = probe row i); an inner one the match kernel, the scan and a
+    // one-row gather
+    int64_t probe_asof(int64_t n, const std::vector<OutCol>& cols, int nkb, const std::vector<const void*>& data,
+                       const std::vector<const uint8_t*>& valid) {
+        AsofArgs a{};
+        if (n_keys > 1) { a.pk = probe_keys(data, valid); a.bk = build_keys(); }
+        else { a.key_data = data[0]; a.key_ctype = p_ct[0]; a.key_valid = valid[0]; }
+        a.table = d_tkeys.p; a.cap = cap; a.na_equal = na_equal ? 1 : 0; a.key_reject = key_reject;
+        a.info = d_info.as<SlotInfo>(); a.goffs = d_goffs.as<unsigned long long>(); a.groups = d_groups.as<uint32_t>(); a.gwords = d_gwords.as<uint64_t>();
+        a.on = AsofOn{data[asof_p_on], valid[asof_p_on], asof_key()};
+        a.direction = asof_dir; a.allow_exact = asof_exact ? 1 : 0; a.has_tol = asof_has_tol ? 1 : 0;
+        a.tol_w = (unsigned long long)asof_tol_i; a.tol_f = asof_tol_f;
+        const int kt = n_keys > 1 ? 2 : float_key ? 1 : 0;
+        unsigned long long rows = (unsigned long long)n;
+        if (probe_outer) {
+            size_outputs(cols, n);
+            const GatherArgs g = gather_args(n, cols, nkb, data, valid);
+            if (n > 0) with_int<3>(kt, [&](auto k) { join_asof_left_kernel<k><<<grid_for(n), 256, 0, stream>>>(g, a); });
+        } else {
+            d_pslot.ensure((size_t)(n + 1) * 4); d_pcnt.ensure((size_t)(n + 1) * 4); d_poff.ensure((size_t)(n + 2) * 8);
+            rows = 0;
+            if (n > 0) {
+                with_int<3>(kt, [&](auto k) {
+                    join_asof_match_kernel<k><<<grid_for(n), 256, 0, stream>>>(a, n, d_pslot.as<uint32_t>(), d_pcnt.as<uint32_t>());
+                });
+                launches++;
+                B200_CUDA(cudaMemsetAsync(d_pcnt.as<uint32_t>() + n, 0, 4, stream));
+                rows = scan.run(d_pcnt.as<uint32_t>(), n + 1, d_poff.as<unsigned long long>(), stream, &launches);
+            }
+            size_outputs(cols, (int64_t)rows);
+            const GatherArgs g = gather_args(n, cols, nkb, data, valid);
+            if (rows > 0) join_asof_gather_kernel<<<grid_for(n), 256, 0, stream>>>(g);
+        }
+        if (n > 0) launches++;
+        B200_CUDA(cudaGetLastError());
+        return (int64_t)rows;
+    }
+
     // general path (CSR groups: duplicate keys, outer, anti and mark joins): count + scan, then expand and gather; the unmatched
     // build rows of a build-outer join follow the last probe batch
     int64_t probe_general(int64_t n, const std::vector<OutCol>& cols, int nkb, const std::vector<const void*>& data,
@@ -1403,21 +1666,7 @@ class JoinState {
         }
         // pass B needs bmatched complete before the tail is computed, so: gather first, then the tail
         size_outputs(cols, (int64_t)n_match);
-        GatherArgs g{};
-        g.n_probe = n; g.pslot = d_pslot.as<uint32_t>(); g.poff = d_poff.as<unsigned long long>(); g.info = d_info.as<SlotInfo>();
-        g.goffs = d_goffs.as<unsigned long long>(); g.groups = d_groups.as<uint32_t>(); g.bmatched = build_outer ? d_bmatched.as<uint8_t>() : nullptr;
-        g.n_b = nkb; g.n_p = (int)cols.size() - nkb;
-        for (int k = 0; k < (int)cols.size(); k++) {
-            const OutCol& c = cols[k];
-            if (c.is_b) {
-                g.b_data[k] = bcol[c.src].buf.p; g.b_valid[k] = build_valid(c.src); g.b_size[k] = c.size;
-                g.ob_data[k] = out_data[k].p; g.ob_valid[k] = out_valid(cols, k);
-            } else {
-                const int j = k - nkb;
-                g.p_data[j] = data[c.src]; g.p_valid[j] = valid[c.src]; g.p_size[j] = c.size;
-                g.op_data[j] = out_data[k].p; g.op_valid[j] = out_valid(cols, k);
-            }
-        }
+        const GatherArgs g = gather_args(n, cols, nkb, data, valid);
         if (n > 0 && n_match > 0) {
             if (has_cond) join_cond_gather_kernel<<<grid_for(n), 256, 0, stream>>>(g, ca, mode);
             else join_probe_gather_kernel<<<grid_for(n), 256, 0, stream>>>(g);
@@ -1478,8 +1727,9 @@ class JoinState {
         std::vector<const void*> data; std::vector<const uint8_t*> valid;
         stage_batch(t, n_p, p_ct, data, valid);
         const std::vector<OutCol> cols = plan_out(kb, kp, valid);
-        const int64_t rows = form == TableForm::CSR ? probe_general(n, cols, (int)kb.size(), data, valid, is_last)
-                                                    : probe_unique(n, cols, (int)kb.size(), data, valid);
+        const int64_t rows = asof                     ? probe_asof(n, cols, (int)kb.size(), data, valid)
+                             : form == TableForm::CSR ? probe_general(n, cols, (int)kb.size(), data, valid, is_last)
+                                                      : probe_unique(n, cols, (int)kb.size(), data, valid);
         for (int k = 0; k < n_out_cols; k++)
             if (cols[k].nullable && rows > 0) { launch_pack_bitmap(out_vbytes[k].as<uint8_t>(), rows, out_bitmap[k].as<uint32_t>(), grid_for(rows), stream); launches++; }
         B200_CUDA(cudaGetLastError());
@@ -1552,6 +1802,15 @@ int b200_join_set_condition(void* state, const void* program, int32_t n_instr) {
     try {
         B200_REQUIRE(state && program, "b200 join: null argument");
         ((JoinState*)state)->set_condition((const b200::ExprInstr*)program, n_instr);
+        return 0;
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
+}
+
+int b200_join_set_asof(void* state, int32_t build_on_col, int32_t probe_on_col, int32_t direction, int32_t allow_exact_matches,
+                        int32_t has_tolerance, int64_t tolerance_i64, double tolerance_f64) {
+    try {
+        B200_REQUIRE(state, "b200 join: null state");
+        ((JoinState*)state)->set_asof(build_on_col, probe_on_col, direction, allow_exact_matches != 0, has_tolerance != 0, tolerance_i64, tolerance_f64);
         return 0;
     } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
 }

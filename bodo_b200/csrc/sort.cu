@@ -320,20 +320,45 @@ __global__ void __launch_bounds__(256) fsort_append_kernel(const __grid_constant
     }
 }
 
+// Where the radix words come from: word(k, j, r, na) is the radix word of key j's cell at row r (key j described by k), na as
+// fs_word's.  FsChunkSrc reads the full sort's chunk store; FsArraySrc plain device columns (validity one byte per row,
+// nullptr = none), which is how the join's as-of build hands over its (slot, on) keys.  A pass reads one key: the host hands
+// it the source of that key as key 0 (for_key), so the pass kernel indexes no parameter array.
+struct FsChunkSrc {
+    FsChunks ch;
+    int64_t coff[SORT_MAX_KEYS], voff[SORT_MAX_KEYS];
+    __device__ __forceinline__ uint64_t word(const SortKey& k, int j, uint32_t r, bool& na) const {
+        return fs_word(k, coff[j], voff[j], ch.p[r >> FS_CHUNK_LOG], r & (FS_CHUNK - 1), na);
+    }
+    FsChunkSrc for_key(int j) const { FsChunkSrc s = *this; s.coff[0] = coff[j]; s.voff[0] = voff[j]; return s; }
+};
+struct FsArraySrc {
+    const void* data[SORT_MAX_KEYS];
+    const uint8_t* valid[SORT_MAX_KEYS];
+    __device__ __forceinline__ uint64_t word(const SortKey& k, int j, uint32_t r, bool& na) const {
+        na = valid[j] && !valid[j][r];
+        return sort_word(k, load_bits(data[j], k.size, r), na);
+    }
+    FsArraySrc for_key(int j) const { FsArraySrc s = *this; s.data[0] = data[j]; s.valid[0] = valid[j]; return s; }
+};
+
+template <typename Src>
 struct FsHistArgs {
     int64_t n;
-    FsLayout lay;
+    int nk;
+    SortKey key[SORT_MAX_KEYS];
     uint32_t* hist;  // FS_HIST_WORDS
-    FsChunks ch;
+    Src src;
 };
 
 // Block-private histograms of every (key, byte) digit, merged into `hist` once per block.  Equal digits within a warp are
 // counted by one shared atomic (match.any), so a constant byte costs one atomic per warp, not 32.
-__global__ void __launch_bounds__(FS_THREADS) fsort_hist_kernel(const __grid_constant__ FsHistArgs a) {
+template <typename Src>
+__global__ void __launch_bounds__(FS_THREADS) fsort_hist_kernel(const __grid_constant__ FsHistArgs<Src> a) {
     __shared__ uint32_t h[SORT_MAX_KEYS * 8 * 256];
     __shared__ uint32_t s_na[SORT_MAX_KEYS];
     const int lane = threadIdx.x & 31;
-    const int nk = a.lay.sc.n_keys;
+    const int nk = a.nk;
     for (int i = threadIdx.x; i < nk * 8 * 256; i += FS_THREADS) h[i] = 0;
     if (threadIdx.x < SORT_MAX_KEYS) s_na[threadIdx.x] = 0;
     __syncthreads();
@@ -342,15 +367,13 @@ __global__ void __launch_bounds__(FS_THREADS) fsort_hist_kernel(const __grid_con
         const int64_t r = r0 + threadIdx.x;
         const unsigned act = __ballot_sync(0xffffffffu, r < a.n);
         if (r >= a.n) continue;
-        const char* chunk = a.ch.p[r >> FS_CHUNK_LOG];
-        const int64_t off = r & (FS_CHUNK - 1);
         const int leader = __ffs(act) - 1;
         for (int j = 0; j < nk; j++) {
             bool na;
-            const uint64_t w = fs_word(a.lay.sc.key[j], a.lay.coff[j], a.lay.voff[j], chunk, off, na);
+            const uint64_t w = a.src.word(a.key[j], j, (uint32_t)r, na);
             const unsigned nam = __ballot_sync(act, na);
             if (lane == leader && nam) atomicAdd(&s_na[j], (uint32_t)__popc(nam));
-            const int nb = a.lay.sc.key[j].size;
+            const int nb = a.key[j].size;
             for (int b = 0; b < nb; b++) {
                 const uint32_t d = (uint32_t)(w >> (8 * b)) & 0xFFu;
                 const unsigned peers = __match_any_sync(act, d);
@@ -364,12 +387,12 @@ __global__ void __launch_bounds__(FS_THREADS) fsort_hist_kernel(const __grid_con
     if (threadIdx.x < nk && s_na[threadIdx.x]) atomicAdd(&a.hist[SORT_MAX_KEYS * 8 * 256 + threadIdx.x], s_na[threadIdx.x]);
 }
 
+template <typename Src>
 struct FsPassArgs {
     int64_t n;
     int shift;       // digit = (word >> shift) & 255; -1: the NA-class bit (bit 31 of the row id)
     uint32_t epoch;  // this pass's tag in the look-back words (1, 2, ...; the words start at 0)
-    SortKey key;     // FS_IN_COLUMN / FS_IN_GATHER: the column the words are computed from, at chunk offsets coff / voff
-    int64_t coff, voff;
+    SortKey key;     // FS_IN_COLUMN / FS_IN_GATHER: the key the words are computed from, key 0 of `src`
     const void* w_in;
     const uint32_t* id_in;
     void* w_out;
@@ -377,14 +400,14 @@ struct FsPassArgs {
     unsigned long long* status;  // [tile][digit] look-back words
     unsigned int* tile_counter;  // tiles are numbered in the order their blocks start
     uint32_t base[256];          // first output row of each digit: exclusive scan of the pass's global histogram
-    FsChunks ch;
+    Src src;
 };
 
 // One LSD pass over FS_TILE-row tiles.  Warp w of a tile owns its rows [w * 32 * FS_ITEMS, (w + 1) * 32 * FS_ITEMS), item k of
 // lane l is row 32 k + l of that range, and items are ranked in row order, so the in-tile rank is stable.  Row ids are 32-bit;
 // words are W (uint32_t for keys of <= 4 bytes, uint64_t otherwise).
-template <typename W, int MODE>
-__global__ void __launch_bounds__(FS_THREADS) fsort_pass_kernel(const __grid_constant__ FsPassArgs a) {
+template <typename W, int MODE, typename Src>
+__global__ void __launch_bounds__(FS_THREADS) fsort_pass_kernel(const __grid_constant__ FsPassArgs<Src> a) {
     __shared__ uint32_t s_hist[FS_WARPS][256];  // per-warp digit counts, then each warp's offset inside the digit's tile run
     __shared__ uint32_t s_start[256];           // tile-local first position of each digit
     __shared__ uint32_t s_gofs[256];            // output row of tile-local position p of digit d: s_gofs[d] + p
@@ -416,7 +439,7 @@ __global__ void __launch_bounds__(FS_THREADS) fsort_pass_kernel(const __grid_con
             } else {
                 const uint32_t r = MODE == FS_IN_COLUMN ? (uint32_t)i : (a.id_in[i] & FS_ID_MASK);
                 bool na;
-                w[k] = (W)fs_word(a.key, a.coff, a.voff, a.ch.p[r >> FS_CHUNK_LOG], r & (FS_CHUNK - 1), na);
+                w[k] = (W)a.src.word(a.key, 0, r, na);
                 id[k] = r | (sort_class(a.key, na) << 31);
             }
             d = fs_digit(w[k], id[k], a.shift);
@@ -512,12 +535,96 @@ __global__ void __launch_bounds__(256) fsort_gather_kernel(const __grid_constant
 
 static_assert(FS_THREADS == 256, "fsort_pass_kernel: one thread per digit");
 
-template <typename W>
-void launch_fsort_pass(int mode, int64_t n_tiles, const FsPassArgs& a, cudaStream_t st) {
+template <typename W, typename Src>
+void launch_fsort_pass(int mode, int64_t n_tiles, const FsPassArgs<Src>& a, cudaStream_t st) {
     const unsigned g = (unsigned)n_tiles;
     if (mode == FS_IN_PAIRS) fsort_pass_kernel<W, FS_IN_PAIRS><<<g, FS_THREADS, 0, st>>>(a);
     else if (mode == FS_IN_COLUMN) fsort_pass_kernel<W, FS_IN_COLUMN><<<g, FS_THREADS, 0, st>>>(a);
     else fsort_pass_kernel<W, FS_IN_GATHER><<<g, FS_THREADS, 0, st>>>(a);
+}
+
+// The LSD radix sort of rows [0, n) by nk keys read from `src`: the digit histograms (one kernel), the pass plan, then one
+// fsort_pass_kernel per planned digit.  Plan: least significant key first; per key its byte digits from the lowest, then its
+// NA class when may_na[j].  A digit that takes one value on every row leaves the order as it is: that pass is skipped.
+// Returns the permutation in ibuf[0] or ibuf[1] (bit 31 of an entry is the NA-class bit, not part of the row id), or nullptr
+// when no pass ran (the identity).  Word buffers and look-back words are freed on return.
+template <typename Src>
+const uint32_t* fsort_rows(const Src& src, const SortKey* keys, const bool* may_na, int nk, int64_t n, DevBuf (&ibuf)[2], int hist_grid,
+                           cudaStream_t stream, int64_t& passes_run, int64_t& passes_skipped) {
+    DevBuf d_hist;
+    d_hist.alloc(FS_HIST_WORDS * 4);
+    B200_CUDA(cudaMemsetAsync(d_hist.p, 0, FS_HIST_WORDS * 4, stream));
+    FsHistArgs<Src> ha{};
+    ha.n = n; ha.nk = nk; ha.hist = d_hist.as<uint32_t>(); ha.src = src;
+    std::copy(keys, keys + nk, ha.key);
+    fsort_hist_kernel<<<hist_grid, FS_THREADS, 0, stream>>>(ha);
+    B200_CUDA(cudaGetLastError());
+    auto* h = (uint32_t*)pinned_acquire(FS_HIST_WORDS * 4);
+    B200_CUDA(cudaMemcpyAsync(h, d_hist.p, FS_HIST_WORDS * 4, cudaMemcpyDeviceToHost, stream));
+    B200_CUDA(cudaStreamSynchronize(stream));
+    struct Pass { int key, shift; uint32_t base[256]; };
+    std::vector<Pass> plan;
+    for (int j = nk - 1; j >= 0; j--) {
+        for (int b = 0; b < keys[j].size; b++) {
+            const uint32_t* c = h + (j * 8 + b) * 256;
+            if (std::any_of(c, c + 256, [&](uint32_t x) { return (int64_t)x == n; })) { passes_skipped++; continue; }
+            Pass p{j, 8 * b, {}};
+            for (uint32_t d = 0, s = 0; d < 256; s += c[d], d++) p.base[d] = s;
+            plan.push_back(p);
+        }
+        if (may_na[j]) {
+            const int64_t na = h[SORT_MAX_KEYS * 8 * 256 + j];
+            if (na == 0 || na == n) { passes_skipped++; continue; }
+            const int64_t class0 = keys[j].na_last ? n - na : na;  // rows whose class bit is 0
+            Pass p{j, -1, {}};
+            for (int d = 1; d < 256; d++) p.base[d] = (uint32_t)class0;
+            plan.push_back(p);
+        }
+    }
+    pinned_release(h, FS_HIST_WORDS * 4);
+    passes_run += (int64_t)plan.size();
+    if (plan.empty()) return nullptr;
+    DevBuf wbuf[2], status, counters;
+    size_t wb = 4;
+    for (const Pass& p : plan) if (keys[p.key].size > 4) wb = 8;
+    for (int b = 0; b < 2; b++) { wbuf[b].alloc((size_t)n * wb); ibuf[b].alloc((size_t)n * 4); }
+    const int64_t n_tiles = (n + FS_TILE - 1) / FS_TILE;
+    status.alloc((size_t)n_tiles * 256 * 8);
+    counters.alloc(plan.size() * 4);
+    B200_CUDA(cudaMemsetAsync(status.p, 0, (size_t)n_tiles * 256 * 8, stream));
+    B200_CUDA(cudaMemsetAsync(counters.p, 0, plan.size() * 4, stream));
+    const uint32_t* ids = nullptr;
+    int cur_buf = -1, prev_key = -1;
+    for (size_t q = 0; q < plan.size(); q++) {
+        const Pass& p = plan[q];
+        const int mode = p.key == prev_key ? FS_IN_PAIRS : ids ? FS_IN_GATHER : FS_IN_COLUMN;
+        const int ob = cur_buf == 0 ? 1 : 0;
+        FsPassArgs<Src> a{};
+        a.n = n; a.shift = p.shift; a.epoch = (uint32_t)q + 1;
+        a.key = keys[p.key]; a.src = src.for_key(p.key);
+        a.w_in = cur_buf >= 0 ? wbuf[cur_buf].p : nullptr; a.id_in = ids;
+        a.w_out = wbuf[ob].p; a.id_out = ibuf[ob].as<uint32_t>();
+        a.status = status.as<unsigned long long>(); a.tile_counter = counters.as<unsigned int>() + q;
+        std::copy(p.base, p.base + 256, a.base);
+        if (keys[p.key].size > 4) launch_fsort_pass<uint64_t>(mode, n_tiles, a, stream);
+        else launch_fsort_pass<uint32_t>(mode, n_tiles, a, stream);
+        B200_CUDA(cudaGetLastError());
+        cur_buf = ob; ids = ibuf[ob].as<uint32_t>(); prev_key = p.key;
+    }
+    return ids;
+}
+
+const uint32_t* radix_sort_columns(int n_keys, const void* const* data, const SortKey* keys, int64_t n, DevBuf (&ids)[2], cudaStream_t st) {
+    B200_REQUIRE(n_keys >= 1 && n_keys <= SORT_MAX_KEYS && n <= FS_MAX_ROWS, "internal: radix_sort_columns: 1 to 4 keys, at most 2^31 rows");
+    if (n == 0) return nullptr;
+    FsArraySrc src{};
+    bool may_na[SORT_MAX_KEYS] = {};
+    for (int j = 0; j < n_keys; j++) src.data[j] = data[j];
+    int dev = 0;
+    B200_CUDA(cudaGetDevice(&dev));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + FS_THREADS - 1) / FS_THREADS, (int64_t)num_sms(dev) * 8));
+    int64_t run = 0, skipped = 0;
+    return fsort_rows(src, keys, may_na, n_keys, n, ids, grid, st, run, skipped);
 }
 
 // ---- host state: a form consumes rows and at is_last points the output views at its sorted rows; the base checks batches,
@@ -791,70 +898,17 @@ struct FullSortState : SortState {
         const int nk = sc.n_keys;
         FsChunks ch{};
         for (size_t k = 0; k < chunks.size(); k++) ch.p[k] = chunks[k].as<char>();
-        DevBuf wbuf[2], ibuf[2], status, counters;
-        const uint32_t* ids = nullptr;  // the permutation so far; nullptr: identity
+        DevBuf ibuf[2];
+        const uint32_t* ids = nullptr;  // the permutation; nullptr: identity
         if (n > 0) {
-            DevBuf d_hist;
-            d_hist.alloc(FS_HIST_WORDS * 4);
-            B200_CUDA(cudaMemsetAsync(d_hist.p, 0, FS_HIST_WORDS * 4, stream));
-            FsHistArgs ha{};
-            ha.n = n; ha.lay = lay; ha.hist = d_hist.as<uint32_t>(); ha.ch = ch;
-            fsort_hist_kernel<<<grid_for(n, FS_THREADS), FS_THREADS, 0, stream>>>(ha);
-            B200_CUDA(cudaGetLastError());
-            auto* h = (uint32_t*)pinned_acquire(FS_HIST_WORDS * 4);
-            B200_CUDA(cudaMemcpyAsync(h, d_hist.p, FS_HIST_WORDS * 4, cudaMemcpyDeviceToHost, stream));
-            B200_CUDA(cudaStreamSynchronize(stream));
-            // LSD plan: least significant key first; per key its byte digits from the lowest, then its NA class.  A digit that
-            // takes one value on every row leaves the order as it is: that pass is skipped.
-            struct Pass { int key, shift; uint32_t base[256]; };
-            std::vector<Pass> plan;
-            for (int j = nk - 1; j >= 0; j--) {
-                for (int b = 0; b < ctype_size(sc.ctype[j]); b++) {
-                    const uint32_t* c = h + (j * 8 + b) * 256;
-                    if (std::any_of(c, c + 256, [&](uint32_t x) { return (int64_t)x == n; })) { passes_skipped++; continue; }
-                    Pass p{j, 8 * b, {}};
-                    for (uint32_t d = 0, s = 0; d < 256; s += c[d], d++) p.base[d] = s;
-                    plan.push_back(p);
-                }
-                if (arr_type[j] == ARR_NULLABLE || ctype_is_float(sc.ctype[j])) {
-                    const int64_t na = h[SORT_MAX_KEYS * 8 * 256 + j];
-                    if (na == 0 || na == n) { passes_skipped++; continue; }
-                    const int64_t class0 = sc.key[j].na_last ? n - na : na;  // rows whose class bit is 0
-                    Pass p{j, -1, {}};
-                    for (int d = 1; d < 256; d++) p.base[d] = (uint32_t)class0;
-                    plan.push_back(p);
-                }
+            FsChunkSrc src{};
+            src.ch = ch;
+            bool may_na[SORT_MAX_KEYS] = {};
+            for (int j = 0; j < nk; j++) {
+                src.coff[j] = lay.coff[j]; src.voff[j] = lay.voff[j];
+                may_na[j] = arr_type[j] == ARR_NULLABLE || ctype_is_float(sc.ctype[j]);
             }
-            pinned_release(h, FS_HIST_WORDS * 4);
-            passes_run = (int64_t)plan.size();
-            if (!plan.empty()) {
-                size_t wb = 4;
-                for (const Pass& p : plan) if (ctype_size(sc.ctype[p.key]) > 4) wb = 8;
-                for (int b = 0; b < 2; b++) { wbuf[b].alloc((size_t)n * wb); ibuf[b].alloc((size_t)n * 4); }
-                const int64_t n_tiles = (n + FS_TILE - 1) / FS_TILE;
-                status.alloc((size_t)n_tiles * 256 * 8);
-                counters.alloc(plan.size() * 4);
-                B200_CUDA(cudaMemsetAsync(status.p, 0, (size_t)n_tiles * 256 * 8, stream));
-                B200_CUDA(cudaMemsetAsync(counters.p, 0, plan.size() * 4, stream));
-                int cur_buf = -1, prev_key = -1;
-                for (size_t q = 0; q < plan.size(); q++) {
-                    const Pass& p = plan[q];
-                    const int mode = p.key == prev_key ? FS_IN_PAIRS : ids ? FS_IN_GATHER : FS_IN_COLUMN;
-                    const int ob = cur_buf == 0 ? 1 : 0;
-                    FsPassArgs a{};
-                    a.n = n; a.shift = p.shift; a.epoch = (uint32_t)q + 1;
-                    a.key = sc.key[p.key]; a.coff = lay.coff[p.key]; a.voff = lay.voff[p.key];
-                    a.w_in = cur_buf >= 0 ? wbuf[cur_buf].p : nullptr; a.id_in = ids;
-                    a.w_out = wbuf[ob].p; a.id_out = ibuf[ob].as<uint32_t>();
-                    a.status = status.as<unsigned long long>(); a.tile_counter = counters.as<unsigned int>() + q;
-                    std::copy(p.base, p.base + 256, a.base);
-                    a.ch = ch;
-                    if (ctype_size(sc.ctype[p.key]) > 4) launch_fsort_pass<uint64_t>(mode, n_tiles, a, stream);
-                    else launch_fsort_pass<uint32_t>(mode, n_tiles, a, stream);
-                    B200_CUDA(cudaGetLastError());
-                    cur_buf = ob; ids = ibuf[ob].as<uint32_t>(); prev_key = p.key;
-                }
-            }
+            ids = fsort_rows(src, sc.key, may_na, nk, n, ibuf, grid_for(n, FS_THREADS), stream, passes_run, passes_skipped);
         }
         FsGatherArgs ga{};
         ga.n = n; ga.ids = ids; ga.lay = lay; ga.ch = ch;

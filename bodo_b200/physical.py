@@ -268,8 +268,11 @@ class PhysicalJoin:
     """Hash join: sink for build batches, ProcessBatch for probe batches (join.h:58-744)."""
 
     def __init__(self, build_key, probe_key, build_names, probe_names, how: str = "inner", **kw):
-        """build_key / probe_key: a column index, or a sequence of 1..4 indices (a multi-column key, in key order)."""
+        """build_key / probe_key: a column index, or a sequence of 1..4 indices (a multi-column key, in key order).  With asof_on=...
+        (an as-of join, see streaming.join.init_join_state) how is "left" or "inner" and the key sequences may be empty."""
         keys = lambda k: tuple(k) if isinstance(k, (list, tuple)) else (k,)
+        if kw.get("asof_on") is not None and how not in ("left", "inner"):
+            raise J._lib.B200Error(f"PhysicalJoin: an as-of join (asof_on) is how='left' or how='inner', not {how!r}")
         build_outer = how in ("right", "outer")   # the build side is the RIGHT table (reference convention)
         probe_outer = how in ("left", "outer")
         if how == "anti":   # LEFT ANTI: probe rows without a partner (physical/join.h:151: no build columns in the output)
@@ -500,6 +503,58 @@ def window(df, partition_by, order_by, funcs, ascending=True, na_position="last"
     run_pipeline(op, [], coll)
     op.Finalize()
     return coll.result()
+
+
+def _names(x):
+    return [] if x is None else [x] if isinstance(x, str) else list(x)
+
+
+def asof_output_layout(left_cols, right_cols, on=None, left_on=None, right_on=None, by=None, left_by=None, right_by=None, suffixes=("_x", "_y")):
+    """The column layout of pandas.merge_asof(left, right, ...): (left on, right on, left by, right by, right's output columns,
+    output names).  The output is left's columns, then right's without each `on` / `by` column that has the same name as its left
+    partner (on=, by=); a name left and right both still have gets the suffixes.  Runs on the host only."""
+    if (on is None) == (left_on is None or right_on is None) or (on is not None and (left_on is not None or right_on is not None)):
+        raise ValueError("merge_asof: give on=, or both left_on= and right_on=")
+    lon, ron = (on, on) if on is not None else (left_on, right_on)
+    if not (isinstance(lon, str) and isinstance(ron, str)):
+        raise ValueError("merge_asof: one `on` column per side")
+    if by is not None and (left_by is not None or right_by is not None):
+        raise ValueError("merge_asof: give by=, or left_by= and right_by=, not both")
+    lby, rby = (_names(by), _names(by)) if by is not None else (_names(left_by), _names(right_by))
+    if len(lby) != len(rby) or len(lby) > 4:
+        raise ValueError(f"merge_asof: left_by and right_by need the same number of columns, at most 4 (got {lby} and {rby})")
+    for side, names, cols in (("left", [lon] + lby, left_cols), ("right", [ron] + rby, right_cols)):
+        missing = [c for c in names if c not in cols]
+        if missing:
+            raise ValueError(f"merge_asof: the {side} frame has no column {missing[0]!r}")
+    merged = {r for l, r in zip([lon] + lby, [ron] + rby) if l == r}
+    right_keep = [c for c in right_cols if c not in merged]
+    clash = set(left_cols) & set(right_keep)
+    names = [c + suffixes[0] if c in clash else c for c in left_cols] + [c + suffixes[1] if c in clash else c for c in right_keep]
+    return lon, ron, lby, rby, right_keep, names
+
+
+def merge_asof(left, right, on=None, *, left_on=None, right_on=None, by=None, left_by=None, right_by=None, suffixes=("_x", "_y"),
+               tolerance=None, allow_exact_matches=True, direction="backward", batch_size: int = STREAMING_BATCH_SIZE, **kw):
+    """pandas.merge_asof(left, right, ...) through the streaming join's as-of form (left = probe side, right = build side, how="left"):
+    each left row once, in left's order, with the right row of equal `by` keys whose `on` value is the latest at or before its own
+    (direction="backward"), the earliest at or after it ("forward") or the nearer one ("nearest"), NULL right columns without one.
+    Neither frame needs to be sorted.  NA `by` keys match each other, as in pandas; NA `on` cells match nothing.  Same column layout
+    and names as pandas (asof_output_layout).  how="inner" in kw keeps only the matched left rows."""
+    import pandas as pd
+
+    lcols, rcols = list(left.columns), list(right.columns)
+    lon, ron, lby, rby, right_keep, names = asof_output_layout(lcols, rcols, on, left_on, right_on, by, left_by, right_by, suffixes)
+    how = kw.pop("how", "left")
+    op = PhysicalJoin([rcols.index(c) for c in rby], [lcols.index(c) for c in lby], rcols, lcols, how=how, asof_on=(ron, lon),
+                      asof_direction=direction, asof_allow_exact_matches=allow_exact_matches, asof_tolerance=tolerance, **kw)
+    run_pipeline(PhysicalReadPandas(right, batch_size), [], op)
+    coll = ResultCollector()
+    run_pipeline(PhysicalReadPandas(left, batch_size), [op], coll)
+    op.Finalize()
+    res = coll.result()  # right's columns, then left's
+    cols = [res.iloc[:, len(rcols) + j] for j in range(len(lcols))] + [res.iloc[:, rcols.index(c)] for c in right_keep]
+    return pd.concat(cols, axis=1, keys=range(len(cols))).set_axis(names, axis=1) if cols else res
 
 
 def merge(left, right, left_on, right_on, how: str = "inner", batch_size: int = STREAMING_BATCH_SIZE, **kw):

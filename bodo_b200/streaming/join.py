@@ -10,21 +10,39 @@ Output column order is the reference's: kept build-table columns first, then kep
 
 from __future__ import annotations
 
+import math
+from datetime import timedelta
+
+import numpy as np
+
 from .. import _lib
 from .._lib import ffi
 from ..expr import OPS, Expr, compile_program
-from ..table import CTable, Table, table_from_ctable
+from ..table import Column, CTable, CTypes, Table, table_from_ctable
+
+ASOF_DIRECTIONS = {"backward": 0, "forward": 1, "nearest": 2}
 
 
 class JoinState:
     def __init__(self, operator_id, build_key_inds, probe_key_inds, build_colnames, probe_colnames, build_outer, probe_outer,
                  output_batch_size, expected_build_rows, device, stream, is_na_equal=False, build_parallel=False, probe_parallel=False,
-                 is_mark_join=False, is_anti_join=False, non_equi_condition=None):
+                 is_mark_join=False, is_anti_join=False, non_equi_condition=None, asof=None):
         self.operator_id = int(operator_id)
         self.is_mark_join = bool(is_mark_join)
         self.is_anti_join = bool(is_anti_join)
         self.build_key_inds = tuple(int(k) for k in build_key_inds)
         self.probe_key_inds = tuple(int(k) for k in probe_key_inds)
+        # as-of join: (build on, probe on, direction, allow_exact_matches, tolerance), `on` as physical columns.  Without equi-join
+        # keys both sides get one constant INT8 key column appended (const_key), so every build row is in one group.
+        self.asof = None
+        self.const_key = False
+        if asof is not None:
+            on, direction, exact, tolerance = asof
+            if not self.build_key_inds and not self.probe_key_inds:
+                self.const_key = True
+                self.build_key_inds, self.probe_key_inds = (len(build_colnames),), (len(probe_colnames),)
+            b_on, p_on = resolve_asof_on(on, self.build_key_inds, self.probe_key_inds, build_colnames, probe_colnames)
+            self.asof = (b_on, p_on, ASOF_DIRECTIONS[direction], bool(exact), tolerance)
         if not 1 <= len(self.build_key_inds) <= 4 or len(self.probe_key_inds) != len(self.build_key_inds):
             raise _lib.B200Error("Streaming Join: 1 to 4 equi-join keys per side, the same number on both sides "
                                  f"(got {len(self.build_key_inds)} build and {len(self.probe_key_inds)} probe keys)")
@@ -76,6 +94,23 @@ class JoinState:
                 prog[i].op = op
                 prog[i].arg = arg
             _lib.check(L.b200_join_set_condition(self.handle, prog, len(self.condition)), "init_join_state")
+        if self.asof is not None:
+            b_on, p_on, direction, exact, tolerance = self.asof
+            has, tol_i, tol_f = asof_tolerance_units(tolerance, bct[b_on])
+            _lib.check(L.b200_join_set_asof(self.handle, b_on, p_on, direction, int(exact), has, tol_i, tol_f), "init_join_state")
+
+    def _with_const_key(self, table: Table) -> Table:
+        """`table` with the constant INT8 key column of an as-of join without equi-join keys appended."""
+        if not self.const_key:
+            return table
+        n = table.n_rows
+        if table.device >= 0:
+            import torch
+
+            key = torch.zeros(max(n, 1), dtype=torch.int8, device=torch.device("cuda", table.device))
+        else:
+            key = np.zeros(max(n, 1), dtype=np.int8)
+        return Table(list(table.columns) + [Column(key, None, CTypes.INT8, length=n)], list(table.names) + ["__asof_key"])
 
 
 J_MAX_COLS = 32        # columns per side (join.cu); a probe column c is program column J_MAX_COLS + c
@@ -122,10 +157,80 @@ def compile_condition(cond, build_key_inds, probe_key_inds, build_colnames, prob
     return prog
 
 
+def resolve_asof_on(on, build_key_inds, probe_key_inds, build_colnames, probe_colnames):
+    """asof_on = (build column name, probe column name) as (build, probe) physical columns (keys first, then the other columns in
+    input order), resolved against the colnames as the non-equi condition's names are.  Runs on the host only."""
+    if not (isinstance(on, (tuple, list)) and len(on) == 2):
+        raise _lib.B200Error(f"Streaming Join: asof_on must be (build column name, probe column name), got {on!r}")
+    out = []
+    for side, name, names, keys in (("build", on[0], build_colnames, build_key_inds), ("probe", on[1], probe_colnames, probe_key_inds)):
+        if names is None:
+            raise _lib.B200Error(f"Streaming Join: asof_on names {side} column {name!r}, but {side}_colnames is None: the as-of join's "
+                                 "names resolve against the column names given at init")
+        hits = [i for i, nm in enumerate(names) if nm == name]
+        if len(hits) != 1:
+            raise _lib.B200Error(f"Streaming Join: asof_on: the {side} side has {'no' if not hits else 'more than one'} column {name!r} "
+                                 f"({side} columns: {list(names)})")
+        if hits[0] in keys:
+            raise _lib.B200Error(f"Streaming Join: asof_on: {side} column {name!r} is an equi-join key; the `on` column is not a key column")
+        physical = list(keys) + [i for i in range(max(len(names), max(keys) + 1)) if i not in keys]  # (+ the constant key)
+        out.append(physical.index(hits[0]))
+    return tuple(out)
+
+
+def _is_timedelta(x) -> bool:
+    import pandas as pd
+
+    return isinstance(x, (pd.Timedelta, timedelta, np.timedelta64))
+
+
+def check_asof_tolerance(tolerance):
+    """Refuse a tolerance that is not an int, a float or a Timedelta, or that is negative or not finite."""
+    if tolerance is None:
+        return
+    import pandas as pd
+
+    if _is_timedelta(tolerance):
+        td = pd.Timedelta(tolerance)
+        if td is pd.NaT or td < pd.Timedelta(0):
+            raise _lib.B200Error(f"Streaming Join: asof_tolerance must be >= 0 (got {tolerance!r})")
+        return
+    if isinstance(tolerance, (bool, np.bool_)) or not isinstance(tolerance, (int, float, np.integer, np.floating)):
+        raise _lib.B200Error(f"Streaming Join: asof_tolerance must be an int, a float or a pd.Timedelta (got {type(tolerance).__name__})")
+    if not math.isfinite(float(tolerance)) or tolerance < 0:
+        raise _lib.B200Error(f"Streaming Join: asof_tolerance must be finite and >= 0 (got {tolerance!r})")
+
+
+def asof_tolerance_units(tolerance, c_type):
+    """(has_tolerance, tolerance_i64, tolerance_f64) of b200_join_set_asof for an `on` column of `c_type`: an integer in the
+    column's units for integer and temporal columns (a Timedelta becomes ns for DATETIME / TIMEDELTA and whole days for DATE), a
+    float for float columns."""
+    if tolerance is None:
+        return 0, 0, 0.0
+    import pandas as pd
+
+    if _is_timedelta(tolerance):
+        ns = pd.Timedelta(tolerance).value
+        if c_type in (CTypes.DATETIME, CTypes.TIMEDELTA):
+            return 1, int(ns), 0.0
+        if c_type == CTypes.DATE:
+            days, rest = divmod(ns, 86_400 * 10**9)
+            if rest:
+                raise _lib.B200Error(f"Streaming Join: asof_tolerance {tolerance!r} is not a whole number of days (the `on` column is a date)")
+            return 1, int(days), 0.0
+        raise _lib.B200Error("Streaming Join: a Timedelta asof_tolerance needs a date, datetime or timedelta `on` column")
+    if c_type in (CTypes.FLOAT32, CTypes.FLOAT64):
+        return 1, 0, float(tolerance)
+    if not isinstance(tolerance, (int, np.integer)) and float(tolerance) != int(tolerance):
+        raise _lib.B200Error(f"Streaming Join: asof_tolerance {tolerance!r} is not an integer (the `on` column is an integer or temporal column)")
+    return 1, int(tolerance), 0.0
+
+
 def init_join_state(operator_id, build_key_inds, probe_key_inds, build_colnames, probe_colnames, build_outer, probe_outer,
                     interval_build_columns=None, force_broadcast=False, op_pool_size_bytes=-1, non_equi_condition=None,
                     build_parallel=False, probe_parallel=False, *, output_batch_size=32768, expected_build_rows=0, device=None,
-                    stream=0, is_na_equal=False, is_mark_join=False, is_anti_join=False) -> JoinState:
+                    stream=0, is_na_equal=False, is_mark_join=False, is_anti_join=False, asof_on=None, asof_direction="backward",
+                    asof_allow_exact_matches=True, asof_tolerance=None) -> JoinState:
     """Mirror of bodo.libs.streaming.join.init_join_state (join.py:991-1100).  Interval joins (`interval_build_columns`) are out
     of scope (SURVEY.md §2.1 row 3) and must be left at the default.
 
@@ -148,10 +253,32 @@ def init_join_state(operator_id, build_key_inds, probe_key_inds, build_colnames,
     `is_mark_join` (HashJoinState's ctor argument, _join.h:287) / `is_anti_join` (the probe's template argument, selected by the
     reference's planner for LEFT ANTI joins, bodo/pandas/physical/join.h:151): a mark join emits every probe row once, without
     build columns, plus a trailing boolean column that says whether the row has a match; an anti join emits the probe rows
-    that have none."""
+    that have none.
+
+    `asof_on=(build column name, probe column name)` makes an as-of join, the contract of pandas.merge_asof (SQL: ASOF JOIN ...
+    MATCH_CONDITION): each probe row matches at most one build row with equal keys (0 to 4 keys; none puts every build row in one
+    group), the one whose `on` value is the latest at or before the probe's (`asof_direction="backward"`), the earliest at or
+    after it ("forward") or the nearer of those two ("nearest", a tie going to the backward one); among equal `on` values the
+    last build row in arrival order for backward, the first for forward.  `asof_allow_exact_matches=False` makes the bounds
+    strict; `asof_tolerance` (an int, a float or a pd.Timedelta, in the column's units) drops a match further away than it.
+    NA `on` cells never match.  probe_outer=True is the left as-of join (pandas' form: every probe row once), False the inner
+    one.  The `on` columns are one per side, of the same type: an integer, float, date, datetime or timedelta column.  Not with
+    build_outer, the mark / anti kinds, a non_equi_condition or a sharded join."""
     if interval_build_columns not in (None, (), []):
         raise _lib.B200Error("Streaming Join: interval joins (interval_build_columns) are not supported by bodo_b200")
     g = lambda x: getattr(x, "meta", x)
+    asof = None
+    if asof_on is not None:
+        if build_parallel or probe_parallel:
+            raise _lib.B200Error("Streaming Join: a sharded asof join is not supported (build_parallel / probe_parallel)")
+        if build_outer:
+            raise _lib.B200Error("Streaming Join: a build-outer asof join is not supported (build_outer must be False)")
+        if is_mark_join or is_anti_join or non_equi_condition is not None:
+            raise _lib.B200Error("Streaming Join: an asof join is not a mark, anti or non_equi_condition join")
+        if asof_direction not in ASOF_DIRECTIONS:
+            raise _lib.B200Error(f"Streaming Join: asof_direction must be one of {list(ASOF_DIRECTIONS)} (got {asof_direction!r})")
+        check_asof_tolerance(asof_tolerance)
+        asof = (g(asof_on), asof_direction, asof_allow_exact_matches, asof_tolerance)
     if non_equi_condition is not None and (len(tuple(g(build_key_inds))) == 0 or len(tuple(g(probe_key_inds))) == 0):
         raise _lib.B200Error("Streaming Join: a non_equi_condition without an equi-join key (a nested-loop join) is not supported by "
                              "bodo_b200; give at least one key column per side")
@@ -164,7 +291,7 @@ def init_join_state(operator_id, build_key_inds, probe_key_inds, build_colnames,
                              is_mark_join=is_mark_join, is_anti_join=is_anti_join, non_equi_condition=non_equi_condition)
     return JoinState(operator_id, g(build_key_inds), g(probe_key_inds), g(build_colnames), g(probe_colnames), build_outer,
                      probe_outer, output_batch_size, expected_build_rows, device, stream, is_na_equal=is_na_equal,
-                     is_mark_join=is_mark_join, is_anti_join=is_anti_join, non_equi_condition=non_equi_condition)
+                     is_mark_join=is_mark_join, is_anti_join=is_anti_join, non_equi_condition=non_equi_condition, asof=asof)
 
 
 def join_build_consume_batch(join_state: JoinState, table: Table, is_last: bool):
@@ -172,6 +299,7 @@ def join_build_consume_batch(join_state: JoinState, table: Table, is_last: bool)
     if hasattr(join_state, "build_consume"):  # sharded state (build_parallel / probe_parallel): dist_join.DistJoinState
         return join_state.build_consume(table, is_last)
     st = join_state
+    table = st._with_const_key(table)
     if st.build_indices is None:
         st.build_indices = st._physical(table, st.build_key_inds)
         cols = [table.columns[i] for i in st.build_indices]
@@ -200,12 +328,13 @@ def join_probe_consume_batch(join_state: JoinState, table: Table, is_last: bool,
     L = _lib.lib()
     if st.build_indices is None or st.handle is None:
         raise _lib.B200Error("join_probe_consume_batch called before any build batch was consumed")
+    table = st._with_const_key(table)
     if st.probe_indices is None:
         st.probe_indices = st._physical(table, st.probe_key_inds)
     phys = table.select(st.probe_indices)
-    if used_cols is None:
-        kb_logical = sorted(st.build_indices)
-        kp_logical = sorted(st.probe_indices)
+    if used_cols is None:  # every column but the constant key of an as-of join without keys
+        kb_logical = [i for i in sorted(st.build_indices) if not (st.const_key and i in st.build_key_inds)]
+        kp_logical = [i for i in sorted(st.probe_indices) if not (st.const_key and i in st.probe_key_inds)]
     else:
         kb_logical, kp_logical = list(used_cols[0]), list(used_cols[1])
     if st.is_mark_join:

@@ -217,6 +217,24 @@ int b200_join_set_kind(void* state, int32_t is_mark_join, int32_t is_anti_join);
  * takes the general (CSR) table, never the unique-key tables of metrics 5-7. */
 int b200_join_set_condition(void* state, const void* program, int32_t n_instr);
 
+/* As-of join, the contract of pandas.merge_asof (the reference's streaming join has no counterpart); call it before the first
+ * build batch, like b200_join_set_condition.  build_on_col / probe_on_col are physical, non-key columns of the same c-type: any
+ * integer width, FLOAT32, FLOAT64, DATE, DATETIME or TIMEDELTA (not BOOL); the probe side is checked when its schema arrives.
+ * For probe row p the candidates are the build rows with equal keys (NA keys as is_na_equal says); with v = p's `on` value and w
+ * a candidate's:
+ *   direction 0 (backward): the largest w <= v (w < v when allow_exact_matches is 0); among equal w the last in build arrival
+ *   order (batch order, then row order).  1 (forward): the smallest w >= v (w > v); among equal w the first.  2 (nearest): the
+ *   backward and forward candidates, the one with the smaller |v - w|; a tie goes to the backward one.
+ * With has_tolerance the match is dropped when |v - w| > tolerance, in the column's units (ns for DATETIME / TIMEDELTA, days for
+ * DATE): tolerance_i64 (>= 0) for integer and temporal columns, where the difference is exact, tolerance_f64 (finite, >= 0) for
+ * float columns, where it is computed in float64.  An NA `on` cell (null, or NaN) never matches, on either side; -0.0 equals 0.0.
+ * probe_table_outer (the left as-of join, pandas' only form) emits every probe row once, NULL-extended without a match; without
+ * it (inner as-of) only matched probe rows go out.  Output rows are in probe order; the probe side need not be sorted.  Fails
+ * on a key or out-of-range column, a BOOL or mismatched `on` type, a negative or non-finite tolerance, a build_table_outer
+ * state, and a mark, anti or condition join. */
+int b200_join_set_asof(void* state, int32_t build_on_col, int32_t probe_on_col, int32_t direction, int32_t allow_exact_matches,
+                       int32_t has_tolerance, int64_t tolerance_i64, double tolerance_f64);
+
 /* Runtime join filter (HashJoinState::RuntimeFilter, _join.h:1060-1095; bloom filter bodo/libs/gpu_bloom_filter.cu:60-201; key
  * min / max _join.cpp:3199-3238), available once the build side is complete.  The reference keeps one bloom filter over the whole
  * key and bounds per key column; so does this, for any key count (1..4).
