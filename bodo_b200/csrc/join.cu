@@ -34,59 +34,83 @@ constexpr long long J_EMPTY = (long long)0x8000000000000000ULL;
 constexpr int J_MAX_COLS = 32;
 constexpr uint32_t J_NONE = 0xffffffffu;
 
-// ---- exclusive scan u32 -> u64 (reduce / scan-of-sums / scan), tile = 2048 elements per CTA ----
-constexpr int SCAN_TILE = 2048;
-__global__ void __launch_bounds__(256) scan_reduce_kernel(const uint32_t* in, int64_t n, unsigned long long* block_sums) {
-    __shared__ unsigned long long sh[256];
-    int64_t base = (int64_t)blockIdx.x * SCAN_TILE;
-    unsigned long long s = 0;
-    for (int k = threadIdx.x; k < SCAN_TILE; k += 256) { int64_t i = base + k; if (i < n) s += in[i]; }
-    sh[threadIdx.x] = s;
-    __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) { if (threadIdx.x < o) sh[threadIdx.x] += sh[threadIdx.x + o]; __syncthreads(); }
-    if (threadIdx.x == 0) block_sums[blockIdx.x] = sh[0];
-}
-__global__ void __launch_bounds__(1024) scan_sums_kernel(unsigned long long* block_sums, int64_t nb, unsigned long long* total) {
-    // single CTA: each thread owns a contiguous run of block sums
-    __shared__ unsigned long long sh[1024];
-    int64_t per = (nb + 1023) / 1024;
-    int64_t b0 = threadIdx.x * per, b1 = b0 + per < nb ? b0 + per : nb;
-    unsigned long long s = 0;
-    for (int64_t b = b0; b < b1; b++) s += block_sums[b];
-    sh[threadIdx.x] = s;
-    __syncthreads();
-    // inclusive Hillis-Steele over 1024 partials
-    for (int o = 1; o < 1024; o <<= 1) {
-        unsigned long long v = threadIdx.x >= o ? sh[threadIdx.x - o] : 0;
-        __syncthreads();
-        sh[threadIdx.x] += v;
-        __syncthreads();
-    }
-    unsigned long long run = threadIdx.x ? sh[threadIdx.x - 1] : 0;
-    for (int64_t b = b0; b < b1; b++) { unsigned long long v = block_sums[b]; block_sums[b] = run; run += v; }
-    if (threadIdx.x == 1023) *total = sh[1023];
-}
-__global__ void __launch_bounds__(256) scan_apply_kernel(const uint32_t* in, int64_t n, const unsigned long long* block_sums,
-                                                         unsigned long long* out) {
-    __shared__ unsigned long long sh[256];
-    int64_t base = (int64_t)blockIdx.x * SCAN_TILE;
-    constexpr int PER = SCAN_TILE / 256;
-    uint32_t v[PER];
-    unsigned long long s = 0;
-    int64_t i0 = base + (int64_t)threadIdx.x * PER;
+// ---- exclusive scan u32 -> u64 in three launches over 2048-row tiles (256 threads x 8 rows, row k * 256 + thread of a
+// tile, so every load and store is coalesced): each tile's sum, one block's exclusive scan of the tile sums, each tile's scan
+// seeded by its prefix ----
+constexpr int OFS_THREADS = 256, OFS_WARPS = OFS_THREADS / 32, OFS_ITEMS = 8, OFS_TILE = OFS_THREADS * OFS_ITEMS;
+__device__ __forceinline__ int64_t ofs_row(int64_t t, int k) { return t * OFS_TILE + k * OFS_THREADS + threadIdx.x; }
+__device__ __forceinline__ unsigned long long ofs_warp_inclusive(unsigned long long v) {
+    const int lane = threadIdx.x & 31;
 #pragma unroll
-    for (int k = 0; k < PER; k++) { v[k] = (i0 + k < n) ? in[i0 + k] : 0; s += v[k]; }
-    sh[threadIdx.x] = s;
-    __syncthreads();
-    for (int o = 1; o < 256; o <<= 1) {
-        unsigned long long t = threadIdx.x >= o ? sh[threadIdx.x - o] : 0;
-        __syncthreads();
-        sh[threadIdx.x] += t;
-        __syncthreads();
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long y = __shfl_up_sync(0xffffffffu, v, o);
+        if (lane >= o) v += y;
     }
-    unsigned long long run = block_sums[blockIdx.x] + (threadIdx.x ? sh[threadIdx.x - 1] : 0);
+    return v;
+}
+__global__ void __launch_bounds__(OFS_THREADS) offsets_tile_sum_kernel(const uint32_t* in, int64_t n, unsigned long long* sums) {
+    __shared__ unsigned long long s_warp[OFS_WARPS];
+    unsigned long long s = 0;
 #pragma unroll
-    for (int k = 0; k < PER; k++) { if (i0 + k < n) out[i0 + k] = run; run += v[k]; }
+    for (int k = 0; k < OFS_ITEMS; k++) {
+        const int64_t i = ofs_row(blockIdx.x, k);
+        if (i < n) s += in[i];
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < OFS_WARPS; w++) s += s_warp[w];
+        sums[blockIdx.x] = s;
+    }
+}
+// One block of 1024 threads, each a contiguous run of tile sums: c becomes its exclusive scan, *total the sum of all.
+__global__ void __launch_bounds__(1024) offsets_carry_kernel(unsigned long long* c, int64_t nb, unsigned long long* total) {
+    __shared__ unsigned long long s_warp[32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t per = (nb + 1023) / 1024, b0 = threadIdx.x * per, b1 = min(nb, b0 + per);
+    unsigned long long acc = 0;
+    for (int64_t b = b0; b < b1; b++) acc += c[b];
+    const unsigned long long inc = ofs_warp_inclusive(acc);
+    if (lane == 31) s_warp[warp] = inc;
+    __syncthreads();
+    unsigned long long run = inc - acc;  // the earlier lanes of this warp, then the earlier warps
+    for (int w = 0; w < warp; w++) run += s_warp[w];
+    for (int64_t b = b0; b < b1; b++) {
+        const unsigned long long v = c[b];
+        c[b] = run;
+        run += v;
+    }
+    if (threadIdx.x == 1023) *total = run;
+}
+__global__ void __launch_bounds__(OFS_THREADS) offsets_tile_scan_kernel(const uint32_t* in, int64_t n, const unsigned long long* carry,
+                                                                        unsigned long long* out) {
+    __shared__ unsigned long long s_seg[OFS_ITEMS * OFS_WARPS];  // per (item, warp) segment of 32 rows: its sum, then its prefix
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t x[OFS_ITEMS];
+    unsigned long long v[OFS_ITEMS];
+#pragma unroll
+    for (int k = 0; k < OFS_ITEMS; k++) {
+        const int64_t i = ofs_row(blockIdx.x, k);
+        x[k] = i < n ? in[i] : 0;
+        v[k] = ofs_warp_inclusive(x[k]);
+        if (lane == 31) s_seg[k * OFS_WARPS + warp] = v[k];
+    }
+    __syncthreads();
+    if (warp == 0) {  // the 64 segments in row order, two per lane, seeded by the tile's prefix
+        static_assert(OFS_ITEMS * OFS_WARPS == 64, "two segments per lane");
+        const unsigned long long x0 = s_seg[2 * lane], x1 = s_seg[2 * lane + 1];
+        const unsigned long long base = carry[blockIdx.x] + ofs_warp_inclusive(x0 + x1) - x0 - x1;
+        s_seg[2 * lane] = base;
+        s_seg[2 * lane + 1] = base + x0;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < OFS_ITEMS; k++) {
+        const int64_t i = ofs_row(blockIdx.x, k);
+        if (i < n) out[i] = s_seg[k * OFS_WARPS + warp] + v[k] - x[k];
+    }
 }
 
 struct Scanner {
@@ -97,12 +121,12 @@ struct Scanner {
     unsigned long long run(const uint32_t* in, int64_t n, unsigned long long* out, cudaStream_t st, int64_t* launches) {
         if (!h_total) h_total = (unsigned long long*)pinned_acquire(8);
         if (n == 0) return 0;
-        int64_t nb = (n + SCAN_TILE - 1) / SCAN_TILE;
+        int64_t nb = (n + OFS_TILE - 1) / OFS_TILE;
         sums.ensure((size_t)nb * 8);
         total.ensure(8);
-        scan_reduce_kernel<<<(unsigned)nb, 256, 0, st>>>(in, n, sums.as<unsigned long long>());
-        scan_sums_kernel<<<1, 1024, 0, st>>>(sums.as<unsigned long long>(), nb, total.as<unsigned long long>());
-        scan_apply_kernel<<<(unsigned)nb, 256, 0, st>>>(in, n, sums.as<unsigned long long>(), out);
+        offsets_tile_sum_kernel<<<(unsigned)nb, OFS_THREADS, 0, st>>>(in, n, sums.as<unsigned long long>());
+        offsets_carry_kernel<<<1, 1024, 0, st>>>(sums.as<unsigned long long>(), nb, total.as<unsigned long long>());
+        offsets_tile_scan_kernel<<<(unsigned)nb, OFS_THREADS, 0, st>>>(in, n, sums.as<unsigned long long>(), out);
         *launches += 3;
         B200_CUDA(cudaGetLastError());
         B200_CUDA(cudaMemcpyAsync(h_total, total.p, 8, cudaMemcpyDeviceToHost, st));

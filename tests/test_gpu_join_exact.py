@@ -735,7 +735,7 @@ def test_fast_probe_past_one_grid_on_slot16(gpu_lib):
 
 @gpu
 def test_general_probe_and_build_outer_tail_past_2_21_scan_elements(gpu_lib):
-    """The single-CTA scan_sums_kernel gives each thread more than one block only past 2^21 elements: a general-path probe batch of
+    """The single-CTA offsets_carry_kernel gives each thread more than one tile only past 2^21 elements: a general-path probe batch of
     more than 2^21 rows, and a build-outer tail over more than 2^21 build rows."""
     n_probe = (1 << 21) + 5 + 1000
     n_build = (1 << 21) + 3
