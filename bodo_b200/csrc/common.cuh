@@ -353,4 +353,13 @@ using PooledBuf = DevBuf;
 // ids[0] or ids[1] (mask each entry with 0x7FFFFFFF), or nullptr for the identity (every digit constant, or n == 0).
 const uint32_t* radix_sort_columns(int n_keys, const void* const* data, const SortKey* keys, int64_t n, DevBuf (&ids)[2], cudaStream_t st);
 
+// Exclusive scan u32 -> u64 over 2048-row tiles (join.cu: offsets_tile_sum / offsets_carry / offsets_tile_scan kernels).
+struct Scanner {
+    DevBuf sums, total;
+    unsigned long long* h_total = nullptr;
+    ~Scanner();
+    // out[i] = sum_{j<i} in[j] on stream st; returns the grand total (synchronises the stream); adds its launches to *launches
+    unsigned long long run(const uint32_t* in, int64_t n, unsigned long long* out, cudaStream_t st, int64_t* launches);
+};
+
 }  // namespace b200

@@ -1430,6 +1430,112 @@ __global__ void mrnf_gather_kernel(const __grid_constant__ MrnfOutArgs a) {
     }
 }
 
+// ---- min_row_number_filter with a limit n > 1: QUALIFY ROW_NUMBER() OVER (PARTITION BY keys ORDER BY sort columns) <= n ----
+// Each group keeps its n least rank tuples (the digit strings above).  The table carries one word per slot, the group's dense id
+// (a K_MRNF accumulator, all-ones until the group's first candidate claims one), so ids survive growth while slots move.  Per id
+// the cutoff C holds the digits of the group's n-th survivor as of the last reduce (all-ones while it had fewer than n).  Per
+// batch, once every row is in the table, mrnf_top_filter_kernel appends each row whose digits are below its group's cutoff to the
+// candidate store.  A reduce (host-triggered) sorts the store by (id, digits), keeps the first n rows of every id and lowers C.
+// Store row layout, one 8-byte column each: id, digits 0 .. n_digits-1, validity word (bit j = kept column j), kept cells.
+struct MrnfTopArgs {
+    MrnfArgs m;                        // the table, the order and the kept columns (b, w, w_valid, keep_w and slot are unused)
+    unsigned long long* gid;           // per slot: the group's id, ~0 = none yet
+    unsigned long long* ctr;           // [0] store rows (the append cursor), [1] ids handed out
+    const unsigned long long* cutoff;  // digit e of id g at cutoff[g * n_digits + e], for g < n_cut
+    unsigned long long n_cut;
+    unsigned drop_nan;                 // dropna: key columns (float) whose NaN marker group is dropped, as compact_* drop it
+    unsigned long long* store;         // column c of store row r at store[c * store_cap + r]
+    unsigned long long store_cap;
+};
+__global__ void __launch_bounds__(256) mrnf_top_filter_kernel(const __grid_constant__ MrnfTopArgs a) {
+    const MrnfArgs& m = a.m;
+    const int64_t n_round = (m.n_rows + 31) & ~31ll;
+    const int lane = threadIdx.x & 31;
+    for (int64_t row = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; row < n_round; row += (int64_t)gridDim.x * blockDim.x) {
+        const uint64_t slot = row < m.n_rows ? mrnf_find_slot(m, row) : ~0ull;
+        bool in = slot != ~0ull;
+        for (int j = 0; j < m.nk && in; j++)
+            if (((a.drop_nan >> j) & 1u) && bit_valid(m.key_valid[j], row)) in = load_int_as_i64(m.key_data[j], m.key_ctype[j], row) != EMPTY_KEY;
+        unsigned long long v[MRNF_FIELDS];
+        unsigned long long id = ~0ull;
+        if (in) {
+            mrnf_fields(m, row, v);
+            id = __ldcg(a.gid + slot);
+            if (id < a.n_cut) {  // below the cutoff (a row never equals it: seq differs)
+                const unsigned long long* c = a.cutoff + id * m.n_digits;
+                for (int e = 0; e < m.n_digits; e++) {
+                    const unsigned long long x = mrnf_digit(m, v, e), y = c[e];
+                    if (x != y) { in = x < y; break; }
+                }
+            }
+            if (in && id == ~0ull) {  // the group's first candidate: claim an id; a thread that loses the race takes the winner's
+                const unsigned long long mine = atomicAdd(a.ctr + 1, 1ull);
+                const unsigned long long old = atomicCAS(a.gid + slot, ~0ull, mine);
+                id = old == ~0ull ? mine : old;
+            }
+        }
+        const unsigned ball = __ballot_sync(0xffffffffu, in);
+        unsigned long long base = 0;
+        if (lane == 0 && ball) base = atomicAdd(a.ctr, (unsigned long long)__popc(ball));
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if (!in) continue;
+        unsigned long long* p = a.store + base + __popc(ball & ((1u << lane) - 1));
+        p[0] = id;
+        for (int e = 0; e < m.n_digits; e++) p[(e + 1) * a.store_cap] = mrnf_digit(m, v, e);
+        unsigned long long vw = 0;
+        for (int j = 0; j < m.n_keep; j++) {
+            p[(m.n_digits + 2 + j) * a.store_cap] = load_bits(m.keep_data[j], m.keep_size[j], row);
+            vw |= bit_valid(m.keep_valid[j], row) ? 1ull << j : 0ull;
+        }
+        p[(m.n_digits + 1) * a.store_cap] = vw;
+    }
+}
+
+// reduce, on the store sorted by (id, digits) through perm (nullptr: the identity): head[id] = position of the id's first row
+__global__ void mrnf_top_head_kernel(const unsigned long long* gid, const uint32_t* perm, int64_t n, uint32_t* head) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const unsigned long long g = gid[perm ? perm[i] & 0x7FFFFFFFu : i];
+        if (i == 0 || gid[perm ? perm[i - 1] & 0x7FFFFFFFu : i - 1] != g) head[g] = (uint32_t)i;
+    }
+}
+// keep[i] = the row at sorted position i ranks below `limit` in its id; the row of rank limit - 1 writes its digits as the cutoff
+__global__ void mrnf_top_rank_kernel(const unsigned long long* store, uint64_t store_cap, int n_digits, const uint32_t* perm,
+                                     int64_t n, const uint32_t* head, long long limit, uint32_t* keep, unsigned long long* cutoff) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = perm ? perm[i] & 0x7FFFFFFFu : i;
+        const unsigned long long g = store[r];
+        const long long rank = i - (int64_t)head[g];
+        keep[i] = rank < limit;
+        if (rank == limit - 1)
+            for (int e = 0; e < n_digits; e++) cutoff[g * n_digits + e] = store[(e + 1) * store_cap + r];
+    }
+}
+// store row perm[i] (every column) to dst row pos[i], for the rows with keep[i] (all rows when keep is nullptr)
+__global__ void mrnf_top_move_kernel(const unsigned long long* src, unsigned long long* dst, uint64_t store_cap, int n_words,
+                                     const uint32_t* perm, int64_t n, const uint32_t* keep, const unsigned long long* pos) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        if (keep && !keep[i]) continue;
+        const int64_t r = perm ? perm[i] & 0x7FFFFFFFu : i, d = pos ? (int64_t)pos[i] : i;
+        for (int c = 0; c < n_words; c++) dst[c * store_cap + d] = src[c * store_cap + r];
+    }
+}
+// finalize: store rows [0, n_out) (the survivors in (id, rank) order) to the kept columns at their widths
+__global__ void mrnf_top_gather_kernel(const unsigned long long* store, uint64_t store_cap, int n_digits, int64_t n_out,
+                                       const __grid_constant__ MrnfOutArgs a) {
+    const int64_t n_round = (n_out + 31) & ~31ll;
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < n_round; p += (int64_t)gridDim.x * blockDim.x) {
+        const bool in = p < n_out;
+        const unsigned long long vw = in ? store[(n_digits + 1) * store_cap + p] : 0ull;
+        for (int j = 0; j < a.n_keep; j++) {
+            if (in) copy_cell(a.out[j], p, store + (n_digits + 2 + j) * store_cap + p, 0, a.keep_size[j]);
+            if (a.out_valid[j]) {
+                const unsigned m = __ballot_sync(0xffffffffu, (vw >> j) & 1ull);
+                if ((threadIdx.x & 31) == 0) a.out_valid[j][p >> 5] = m;
+            }
+        }
+    }
+}
+
 // ================================================================================================
 // SM-partitioned groupby (SPG): the fast path for cardinalities whose accumulators fit the chip's
 // aggregate shared memory (≈ SMs x 10k groups).  Motivation (scratch/ubench*.cu): two global `red`s per
@@ -2178,6 +2284,7 @@ struct MrnfSpec {
     const int32_t* ascending;
     const int32_t* na_last;
     const int32_t* keep;  // one flag per column
+    int64_t limit;        // rows kept per group (b200_groupby_state_init_mrnf_limit)
 };
 
 class GroupbyState {
@@ -2439,6 +2546,7 @@ class GroupbyState {
         if (copy_stream) { cudaStreamSynchronize(copy_stream); cudaStreamDestroy(copy_stream); }
         for (int b = 0; b < 2; b++) { if (stage_free[b]) cudaEventDestroy(stage_free[b]); if (stage_ready[b]) cudaEventDestroy(stage_ready[b]); }
         pinned_release(h_counters, N_COUNTERS * sizeof(long long));
+        if (mt.h_ctr) pinned_release(mt.h_ctr, 16);
         pinned_release(h_spg, H_SPG_WORDS * sizeof(long long));
         for (int b = 0; b < 2; b++) if (spg_ev[b]) cudaEventDestroy(spg_ev[b]);
         for (auto& pr : prof_events) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
@@ -3155,7 +3263,25 @@ class GroupbyState {
         int w0 = 0;             // funcs[w0 ..): the winner's digits, its validity word, one word per kept column
         DevBuf b, slot;         // B (n_digits x (b_cap + 2) words) and the batch's slot cache
         uint64_t b_cap = 0;
+        int64_t limit = 1;      // rows kept per group; > 1: funcs[w0] is the group id word and the rows go through the store
     } mr;
+
+    // ---- limit > 1 (see mrnf_top_filter_kernel) ----
+    static constexpr int64_t MRNF_CAND_MAX = 1ll << 31;      // rows radix_sort_columns sorts at once
+    static constexpr int64_t MRNF_REDUCE_MIN = 1ll << 22;    // admitted rows that make a reduce worth its sort
+    struct MrnfTop {
+        DevBuf store[2];        // the candidate store and the reduce's destination, store_words() columns of cap rows each
+        int64_t cap = 0;
+        int64_t survivors = 0;  // store rows after the last reduce (every id's first `limit` rows, in (id, rank) order)
+        int64_t bound = 0;      // upper bound on the store's rows (survivors + rows filtered since)
+        int64_t admitted = 0, reduces = 0;  // metrics 18 and 19: candidate rows admitted, reduces run
+        DevBuf ctr;             // [0] store rows, [1] ids handed out
+        unsigned long long* h_ctr = nullptr;  // pinned mirror of ctr
+        DevBuf cutoff, head, keep, pos, ids[2];
+        int64_t n_cut = 0;      // ids with a cutoff row (ids handed out at the last reduce)
+        Scanner scan;
+    } mt;
+    int store_words() const { return 2 + mr.n_digits + (int)mr.keep.size(); }
 
     void setup_mrnf(const MrnfSpec& s) {
         B200_REQUIRE(n_outs == 0, "b200 groupby: min_row_number_filter takes no other aggregate function");
@@ -3186,8 +3312,20 @@ class GroupbyState {
         }
         B200_REQUIRE(!mr.keep.empty(), "b200 groupby: min_row_number_filter keeps no column");
         B200_REQUIRE((int)mr.keep.size() <= MRNF_MAX_KEEP, "b200 groupby: min_row_number_filter keeps at most " + std::to_string(MRNF_MAX_KEEP) + " columns");
-        // the winner record: digits all-ones (above every row's tuple), validity and payload zero
+        B200_REQUIRE(s.limit >= 1 && s.limit < MRNF_CAND_MAX, "b200 groupby: min_row_number_filter rows_per_group must be in [1, 2^31)");
+        mr.limit = s.limit;
         mr.w0 = (int)funcs.size();
+        if (mr.limit > 1) {  // the group id word, all-ones until claimed
+            FuncSpec g{};
+            g.in_col = -1; g.in_ctype = CT_INT64; g.in_arrtype = ARR_NUMPY; g.kind = K_MRNF; g.out_ctype = CT_INT64; g.out_arrtype = ARR_NUMPY;
+            g.init0 = ~0ull;
+            funcs.push_back(g);
+            mt.ctr.alloc(16);
+            B200_CUDA(cudaMemsetAsync(mt.ctr.p, 0, 16, stream));
+            mt.h_ctr = (unsigned long long*)pinned_acquire(16);
+            return;
+        }
+        // the winner record: digits all-ones (above every row's tuple), validity and payload zero
         FuncSpec w{};
         w.in_col = -1; w.in_ctype = CT_INT64; w.in_arrtype = ARR_NUMPY; w.kind = K_MRNF; w.out_ctype = CT_INT64; w.out_arrtype = ARR_NUMPY;
         for (int e = 0; e < mr.n_digits + 1 + (int)mr.keep.size(); e++) {
@@ -3203,12 +3341,12 @@ class GroupbyState {
         // insert the keys (no aggregate: n_apply() is 0); the table grows and the failed rows are replayed until all are in
         if (nk > 1) consume_mk(keys, valid, n);
         else consume_direct(keys, valid, n, false, -1, -1, -1, false);
-        if (mr.b_cap != cap) {  // (B is all-ones whenever the table grows: a fresh B for the new capacity)
+        if (mr.limit == 1 && mr.b_cap != cap) {  // (B is all-ones whenever the table grows: a fresh B for the new capacity)
             mr.b.alloc((size_t)mr.n_digits * (cap + 2) * 8);
             fill(mr.b.p, (uint64_t)mr.n_digits * (cap + 2), ~0ull);
             mr.b_cap = cap;
         }
-        mr.slot.ensure((size_t)n * 8);
+        if (mr.limit == 1) mr.slot.ensure((size_t)n * 8);
         MrnfArgs a{};
         a.n_rows = n; a.seq_base = seq_base; a.nk = nk; a.dropna = dropna ? 1 : 0; a.cap = cap;
         for (int j = 0; j < nk; j++) { a.key_data[j] = keys[j]; a.key_valid[j] = valid[j]; a.key_ctype[j] = c_types[j]; }
@@ -3217,26 +3355,160 @@ class GroupbyState {
             a.tags = d_tags.as<unsigned long long>(); a.mkmask = d_mkmask.as<unsigned char>();
             for (int j = 0; j < nk; j++) a.mk[j] = d_mk[j].as<long long>();
         }
-        a.slot = mr.slot.as<uint64_t>();
+        a.slot = mr.slot.as<uint64_t>();  // (limit > 1: unused)
         a.n_sort = mr.n_sort; a.n_digits = mr.n_digits;
         for (int j = 0; j < mr.n_sort; j++) { a.key[j] = mr.key[j]; a.sort_data[j] = raw[mr.sort_col[j]]; a.sort_valid[j] = valid[mr.sort_col[j]]; }
         std::copy(mr.f_end, mr.f_end + MRNF_FIELDS, a.f_end);
-        a.b = mr.b.as<unsigned long long>();
-        for (int e = 0; e < mr.n_digits; e++) a.w[e] = d_a0[mr.w0 + e].as<unsigned long long>();
-        a.w_valid = d_a0[mr.w0 + mr.n_digits].as<unsigned long long>();
         a.n_keep = (int)mr.keep.size();
         for (int j = 0; j < a.n_keep; j++) {
             const int c = mr.keep[j];
             a.keep_data[j] = raw[c]; a.keep_valid[j] = valid[c]; a.keep_size[j] = ctype_size(in_types[c]);
-            a.keep_w[j] = d_a0[mr.w0 + mr.n_digits + 1 + j].as<unsigned long long>();
         }
+        if (mr.limit > 1) { filter_top(a); return; }
+        a.b = mr.b.as<unsigned long long>();
+        for (int e = 0; e < mr.n_digits; e++) a.w[e] = d_a0[mr.w0 + e].as<unsigned long long>();
+        a.w_valid = d_a0[mr.w0 + mr.n_digits].as<unsigned long long>();
+        for (int j = 0; j < a.n_keep; j++) a.keep_w[j] = d_a0[mr.w0 + mr.n_digits + 1 + j].as<unsigned long long>();
         for (int d = 0; d < mr.n_digits; d++) mrnf_min_kernel<<<grid_for(n), 256, 0, stream>>>(a, d);
         mrnf_merge_kernel<<<grid_for(n), 256, 0, stream>>>(a);
         launches += mr.n_digits + 1;
         B200_CUDA(cudaGetLastError());
     }
 
+    // ---- limit > 1: the candidate store (see mrnf_top_filter_kernel) ----
+    // Filters one chunk (every row is in the table).  Before the launch the host makes room for every row of the chunk in the
+    // store, so the kernel never overflows; the store's row count stays on the device, the host keeps an upper bound.
+    void filter_top(const MrnfArgs& m) {
+        const int64_t n = m.n_rows;
+        ensure_candidate_room(n);
+        // amortised reduce: once the rows admitted since the last reduce may have reached max(survivors, MRNF_REDUCE_MIN), count them
+        const int64_t due = std::max(mt.survivors, MRNF_REDUCE_MIN);
+        if (mt.bound - mt.survivors >= due) {
+            read_top_counts();
+            if (mt.bound - mt.survivors >= due) reduce_top();
+        }
+        if (mt.bound + n > mt.cap) {  // a larger store, keeping its rows
+            const int64_t nc = std::min(MRNF_CAND_MAX, std::max(mt.bound + n, mt.cap + mt.cap / 2));
+            const int w = store_words();
+            DevBuf g;
+            g.alloc((size_t)w * nc * 8);
+            if (mt.bound > 0) B200_CUDA(cudaMemcpy2DAsync(g.p, (size_t)nc * 8, mt.store[0].p, (size_t)mt.cap * 8, (size_t)mt.bound * 8, w, cudaMemcpyDeviceToDevice, stream));
+            mt.store[0] = std::move(g);
+            mt.store[1].alloc((size_t)w * nc * 8);
+            mt.cap = nc;
+        }
+        MrnfTopArgs t{};
+        t.m = m;
+        t.gid = d_a0[mr.w0].as<unsigned long long>();
+        t.ctr = mt.ctr.as<unsigned long long>();
+        t.cutoff = mt.cutoff.as<unsigned long long>(); t.n_cut = (unsigned long long)mt.n_cut;
+        for (int j = 0; j < nk; j++) if (dropna && float_key(j)) t.drop_nan |= 1u << j;
+        t.store = mt.store[0].as<unsigned long long>(); t.store_cap = (unsigned long long)mt.cap;
+        mrnf_top_filter_kernel<<<grid_for(n), 256, 0, stream>>>(t);
+        launches++;
+        B200_CUDA(cudaGetLastError());
+        mt.bound += n;
+    }
+    // Refuses n more rows when the store could pass MRNF_CAND_MAX rows even right after a reduce.
+    void ensure_candidate_room(int64_t n) {
+        if (mr.limit == 1 || mt.bound + n <= MRNF_CAND_MAX) return;
+        read_top_counts();
+        reduce_top();
+        B200_REQUIRE(mt.survivors + n <= MRNF_CAND_MAX,
+                     "b200 groupby: min_row_number_filter with rows_per_group = " + std::to_string(mr.limit) + " sorts its candidates (the " +
+                         std::to_string(mt.survivors) + " survivors, at most groups x rows_per_group, plus a batch of " + std::to_string(n) +
+                         " rows) in one radix sort of at most 2^31 rows; keep groups x rows_per_group + batch rows below 2^31");
+    }
+    // the store's exact row count into mt.bound (synchronises the stream)
+    void read_top_counts() {
+        B200_CUDA(cudaMemcpyAsync(mt.h_ctr, mt.ctr.p, 16, cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaStreamSynchronize(stream));
+        mt.bound = (int64_t)mt.h_ctr[0];
+    }
+    // After read_top_counts: sorts the store by (id, digits), keeps each id's first mr.limit rows, in that order, and writes the
+    // cutoff of every id that has mr.limit of them.  Nothing to do when no row came since the last reduce.
+    void reduce_top() {
+        const int64_t m = mt.bound, n_ids = (int64_t)mt.h_ctr[1];
+        if (m == mt.survivors) return;
+        mt.admitted += m - mt.survivors;
+        mt.reduces++;
+        const int nd = mr.n_digits, w = store_words();
+        if (n_ids > mt.n_cut) {  // cutoffs for the ids handed out since: all-ones (fewer than limit survivors)
+            DevBuf c;
+            c.alloc((size_t)n_ids * nd * 8);
+            if (mt.n_cut > 0) B200_CUDA(cudaMemcpyAsync(c.p, mt.cutoff.p, (size_t)mt.n_cut * nd * 8, cudaMemcpyDeviceToDevice, stream));
+            fill(c.as<unsigned long long>() + mt.n_cut * nd, (uint64_t)(n_ids - mt.n_cut) * nd, ~0ull);
+            mt.cutoff = std::move(c);
+            mt.n_cut = n_ids;
+        }
+        const uint64_t sc = (uint64_t)mt.cap;
+        const SortKey u64{CT_UINT64, 8, 0, 0};
+        const SortKey keys[4] = {u64, u64, u64, u64};
+        const void* cols[4];
+        auto col = [&](int c) { return (const void*)(mt.store[0].as<unsigned long long>() + c * sc); };
+        const uint32_t* perm;
+        if (1 + nd > 4) {  // at most four columns per sort: digits 3.. first, then a stable sort by (id, digits 0..2) of that order
+            for (int e = 3; e < nd; e++) cols[e - 3] = col(1 + e);
+            perm = radix_sort_columns(nd - 3, cols, keys, m, mt.ids, stream);
+            if (perm) {
+                mrnf_top_move_kernel<<<grid_for(m), 256, 0, stream>>>(mt.store[0].as<unsigned long long>(), mt.store[1].as<unsigned long long>(), sc, w,
+                                                                    perm, m, nullptr, nullptr);
+                launches++;
+                std::swap(mt.store[0], mt.store[1]);
+            }
+            for (int c = 0; c < 4; c++) cols[c] = col(c);
+            perm = radix_sort_columns(4, cols, keys, m, mt.ids, stream);
+        } else {
+            for (int c = 0; c < 1 + nd; c++) cols[c] = col(c);
+            perm = radix_sort_columns(1 + nd, cols, keys, m, mt.ids, stream);
+        }
+        mt.head.ensure((size_t)n_ids * 4);
+        mt.keep.ensure((size_t)m * 4);
+        mt.pos.ensure((size_t)m * 8);
+        const unsigned long long* st = mt.store[0].as<unsigned long long>();
+        mrnf_top_head_kernel<<<grid_for(m), 256, 0, stream>>>(st, perm, m, mt.head.as<uint32_t>());
+        mrnf_top_rank_kernel<<<grid_for(m), 256, 0, stream>>>(st, sc, nd, perm, m, mt.head.as<uint32_t>(), (long long)mr.limit,
+                                                              mt.keep.as<uint32_t>(), mt.cutoff.as<unsigned long long>());
+        launches += 2;
+        B200_CUDA(cudaGetLastError());
+        const int64_t kept = (int64_t)mt.scan.run(mt.keep.as<uint32_t>(), m, mt.pos.as<unsigned long long>(), stream, &launches);
+        mrnf_top_move_kernel<<<grid_for(m), 256, 0, stream>>>(st, mt.store[1].as<unsigned long long>(), sc, w, perm, m, mt.keep.as<uint32_t>(),
+                                                            mt.pos.as<unsigned long long>());
+        launches++;
+        B200_CUDA(cudaGetLastError());
+        std::swap(mt.store[0], mt.store[1]);
+        mt.survivors = mt.bound = kept;
+        fill(mt.ctr.p, 1, (unsigned long long)kept);  // the append cursor
+    }
+    int64_t finalize_mrnf_top() {
+        read_top_counts();
+        reduce_top();
+        const int64_t max_out = mt.survivors;
+        const size_t words = (size_t)((max_out + 31) / 32 + 1);
+        const int n_keep = (int)mr.keep.size();
+        d_out_data.resize(n_keep); d_out_valid.resize(n_keep);
+        MrnfOutArgs o{};
+        o.n_keep = n_keep;
+        for (int j = 0; j < n_keep; j++) {
+            const int c = mr.keep[j];
+            o.keep_size[j] = ctype_size(in_types[c]);
+            d_out_data[j].ensure((size_t)(max_out + 32) * 8);
+            o.out[j] = d_out_data[j].p;
+            if (arr_types[c] == ARR_NULLABLE) { d_out_valid[j].ensure(words * 4); o.out_valid[j] = d_out_valid[j].as<uint32_t>(); }
+        }
+        mrnf_top_gather_kernel<<<grid_for(std::max<int64_t>(max_out, 1)), 256, 0, stream>>>(mt.store[0].as<unsigned long long>(), (uint64_t)mt.cap,
+                                                                                            mr.n_digits, max_out, o);
+        launches++;
+        B200_CUDA(cudaGetLastError());
+        B200_CUDA(cudaStreamSynchronize(stream));
+        n_out = max_out;
+        finalized = true;
+        out_cursor = 0;
+        return n_out;
+    }
+
     int64_t finalize_mrnf() {
+        if (mr.limit > 1) return finalize_mrnf_top();
         compact();
         const int64_t max_out = max_out_bound();
         const size_t words = (size_t)((max_out + 31) / 32 + 1);
@@ -3272,6 +3544,7 @@ class GroupbyState {
         for (auto& f : funcs) if (f.in_col >= 0) used[f.in_col] = true;
         if (mr.on) {
             B200_REQUIRE(n_pes == 1, "b200 groupby: a sharded min_row_number_filter is not supported (n_pes > 1); run it on one rank");
+            ensure_candidate_room(n);  // (before anything reads the batch)
             for (int j = 0; j < mr.n_sort; j++) used[mr.sort_col[j]] = true;
             for (int c : mr.keep) used[c] = true;
         }
@@ -3729,6 +4002,16 @@ void* b200_groupby_state_init_mrnf(int64_t operator_id, const int8_t* build_arr_
                                    const int32_t* sort_na_last, int32_t n_sort, const int32_t* keep, int64_t output_batch_size,
                                    int32_t parallel, int32_t pandas_drop_na, int32_t device, int32_t n_pes, int32_t myrank,
                                    int64_t expected_groups, void* stream) {
+    return b200_groupby_state_init_mrnf_limit(operator_id, build_arr_c_types, build_arr_array_types, n_build_arrs, n_keys, sort_cols, sort_ascending,
+                                              sort_na_last, n_sort, keep, output_batch_size, parallel, pandas_drop_na, device, n_pes, myrank,
+                                              expected_groups, stream, 1);
+}
+
+void* b200_groupby_state_init_mrnf_limit(int64_t operator_id, const int8_t* build_arr_c_types, const int8_t* build_arr_array_types,
+                                         int32_t n_build_arrs, uint64_t n_keys, const int32_t* sort_cols, const int32_t* sort_ascending,
+                                         const int32_t* sort_na_last, int32_t n_sort, const int32_t* keep, int64_t output_batch_size,
+                                         int32_t parallel, int32_t pandas_drop_na, int32_t device, int32_t n_pes, int32_t myrank,
+                                         int64_t expected_groups, void* stream, int64_t rows_per_group) {
     (void)operator_id;
     B200_TRY
     B200_REQUIRE(build_arr_c_types && build_arr_array_types && keep && (n_sort <= 0 || (sort_cols && sort_ascending && sort_na_last)),
@@ -3738,7 +4021,7 @@ void* b200_groupby_state_init_mrnf(int64_t operator_id, const int8_t* build_arr_
         throw b200::Error("b200 groupby: no CUDA device available (this path has no CPU fallback)");
     B200_REQUIRE(device >= 0 && device < ndev, "b200 groupby: bad device ordinal");
     const int32_t no_off[1] = {0};
-    const b200::MrnfSpec spec{n_sort, sort_cols, sort_ascending, sort_na_last, keep};
+    const b200::MrnfSpec spec{n_sort, sort_cols, sort_ascending, sort_na_last, keep, rows_per_group};
     return new GroupbyState(build_arr_c_types, build_arr_array_types, n_build_arrs, nullptr, no_off, nullptr, 0, n_keys,
                             output_batch_size, parallel != 0, pandas_drop_na != 0, device, n_pes, myrank, expected_groups,
                             (cudaStream_t)stream, &spec);
@@ -3820,6 +4103,8 @@ int64_t b200_groupby_get_metric(void* state, int32_t which) {
         case 15: return s->spg16_launches;
         case 16: return s->spg_n_hot;
         case 17: return s->spgd_launches;
+        case 18: return s->mt.admitted;
+        case 19: return s->mt.reduces;
         case 13: { cudaSetDevice(s->device); s->read_counters(); return s->n_groups; }  // exact (synchronises the stream)
         case 100: s->profiling = true; return 0;
         default: return -1;

@@ -113,27 +113,22 @@ __global__ void __launch_bounds__(OFS_THREADS) offsets_tile_scan_kernel(const ui
     }
 }
 
-struct Scanner {
-    DevBuf sums, total;
-    unsigned long long* h_total = nullptr;
-    ~Scanner() { pinned_release(h_total, 8); }
-    // out[i] = sum_{j<i} in[j]; returns the grand total (synchronises the stream)
-    unsigned long long run(const uint32_t* in, int64_t n, unsigned long long* out, cudaStream_t st, int64_t* launches) {
-        if (!h_total) h_total = (unsigned long long*)pinned_acquire(8);
-        if (n == 0) return 0;
-        int64_t nb = (n + OFS_TILE - 1) / OFS_TILE;
-        sums.ensure((size_t)nb * 8);
-        total.ensure(8);
-        offsets_tile_sum_kernel<<<(unsigned)nb, OFS_THREADS, 0, st>>>(in, n, sums.as<unsigned long long>());
-        offsets_carry_kernel<<<1, 1024, 0, st>>>(sums.as<unsigned long long>(), nb, total.as<unsigned long long>());
-        offsets_tile_scan_kernel<<<(unsigned)nb, OFS_THREADS, 0, st>>>(in, n, sums.as<unsigned long long>(), out);
-        *launches += 3;
-        B200_CUDA(cudaGetLastError());
-        B200_CUDA(cudaMemcpyAsync(h_total, total.p, 8, cudaMemcpyDeviceToHost, st));
-        B200_CUDA(cudaStreamSynchronize(st));
-        return *h_total;
-    }
-};
+Scanner::~Scanner() { pinned_release(h_total, 8); }
+unsigned long long Scanner::run(const uint32_t* in, int64_t n, unsigned long long* out, cudaStream_t st, int64_t* launches) {
+    if (!h_total) h_total = (unsigned long long*)pinned_acquire(8);
+    if (n == 0) return 0;
+    int64_t nb = (n + OFS_TILE - 1) / OFS_TILE;
+    sums.ensure((size_t)nb * 8);
+    total.ensure(8);
+    offsets_tile_sum_kernel<<<(unsigned)nb, OFS_THREADS, 0, st>>>(in, n, sums.as<unsigned long long>());
+    offsets_carry_kernel<<<1, 1024, 0, st>>>(sums.as<unsigned long long>(), nb, total.as<unsigned long long>());
+    offsets_tile_scan_kernel<<<(unsigned)nb, OFS_THREADS, 0, st>>>(in, n, sums.as<unsigned long long>(), out);
+    *launches += 3;
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaMemcpyAsync(h_total, total.p, 8, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    return *h_total;
+}
 
 // ---- hash table ----
 struct SlotInfo { uint32_t cnt; uint32_t first; };  // rows with this key; one of those rows (row id)

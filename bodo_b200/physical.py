@@ -234,7 +234,8 @@ class PhysicalReadArrowDevice:
 class PhysicalAggregate:
     """Groupby sink/source (aggregate.h:65-365). `aggs` = [(func_name, input_column_index or None for size)].
     mrnf = (sort_col_inds, ascending, na_last, keep_inds) with no aggs: a min_row_number_filter, one row per group, the first by
-    the sort columns (streaming.groupby's mrnf_* arguments)."""
+    the sort columns (streaming.groupby's mrnf_* arguments); mrnf_limit=n (forwarded to init_groupby_state with the other keywords)
+    keeps the first n rows per group."""
 
     def __init__(self, key_inds: Sequence[int], aggs: Sequence[tuple], dropna: bool = True, parallel: bool = False, mrnf=None, **kw):
         fnames = tuple(f for f, _ in aggs) + ((G.MRNF,) if mrnf is not None else ())
@@ -445,12 +446,13 @@ def groupby_agg_parquet(path: str, by, aggs: Sequence[tuple], dropna: bool = Tru
 
 
 def min_row_number_filter(df, by, order_by, ascending=True, na_position="last", keep=None, dropna: bool = False,
-                          batch_size: int = STREAMING_BATCH_SIZE, **kw):
-    """One row per group of `by`, the first by `order_by`: QUALIFY ROW_NUMBER() OVER (PARTITION BY by ORDER BY order_by) = 1, the
-    streaming equivalent of df.sort_values(order_by, ascending=..., na_position=..., kind="stable").drop_duplicates(by,
-    keep="first")[keep], through PhysicalAggregate(mrnf=...).  by, order_by: a column name or a list (1..4 each); ascending /
-    na_position: one value or one per order_by column; keep: the output columns (default: every column).  dropna=False (pandas'
-    drop_duplicates) makes all NA keys one group, dropna=True drops their rows.  Group order is unspecified."""
+                          batch_size: int = STREAMING_BATCH_SIZE, n: int = 1, **kw):
+    """The first n rows per group of `by` by `order_by` (default one): QUALIFY ROW_NUMBER() OVER (PARTITION BY by ORDER BY order_by)
+    <= n, the streaming equivalent of df.sort_values(order_by, ascending=..., na_position=..., kind="stable").groupby(by, sort=False,
+    dropna=dropna).head(n)[keep] (for n = 1, .drop_duplicates(by, keep="first")[keep]), through PhysicalAggregate(mrnf=...,
+    mrnf_limit=n).  by, order_by: a column name or a list (1..4 each); ascending / na_position: one value or one per order_by
+    column; keep: the output columns (default: every column).  dropna=False (pandas' drop_duplicates) makes all NA keys one group,
+    dropna=True drops their rows.  Group order is unspecified; a group's rows are consecutive, in rank order."""
     cols = list(df.columns)
     by = [by] if isinstance(by, str) else list(by)
     order_by = [order_by] if isinstance(order_by, str) else list(order_by)
@@ -460,7 +462,7 @@ def min_row_number_filter(df, by, order_by, ascending=True, na_position="last", 
     if any(p not in ("first", "last") for p in nap):
         raise ValueError(f"min_row_number_filter: na_position must be 'first' or 'last' (got {na_position!r})")
     mrnf = ([cols.index(c) for c in order_by], asc, [p == "last" for p in nap], [cols.index(c) for c in keep])
-    op = PhysicalAggregate([cols.index(k) for k in by], [], dropna=dropna, mrnf=mrnf, **kw)
+    op = PhysicalAggregate([cols.index(k) for k in by], [], dropna=dropna, mrnf=mrnf, mrnf_limit=n, **kw)
     run_pipeline(PhysicalReadPandas(df, batch_size), [], op)
     coll = ResultCollector()
     run_pipeline(op, [], coll)

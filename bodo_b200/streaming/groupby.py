@@ -31,11 +31,21 @@ df.sort_values(sort columns, kind="stable").drop_duplicates(keys, keep="first")[
     group of more than one rank raises at its first consume call (sharded MRNF is not supported), with one rank it runs locally.
 The state streams every batch into the groupby's hash table and keeps one winner record per group (DESIGN.md §3d), so it holds
 O(groups) device memory whatever the row count.
+
+mrnf_limit=n (keyword-only, an int, 1 <= n < 2^31, default 1; only with min_row_number_filter) keeps the first n rows per group,
+QUALIFY ROW_NUMBER() OVER (PARTITION BY keys ORDER BY sort columns) <= n, i.e.
+df.sort_values(sort columns, kind="stable").groupby(keys, sort=False, dropna=dropna).head(n)[kept columns] as a multiset of rows:
+  - everything above holds; of rows that tie on every sort column the earlier arrival ranks first, even across batches, and a
+    group with fewer than n rows keeps all of them.
+  - a group's rows are consecutive and in rank order in the output, also when the group spans two output batches (group order
+    is unspecified), so a cumulative count numbers them.
+  - n > 1 keeps candidate rows in a device store reduced by a radix sort of at most 2^31 rows: a batch whose rows, added to the
+    survivors (at most groups x n), would pass that raises.  Its memory is O(groups x n + rows admitted between reduces).
 """
 
 from __future__ import annotations
 
-
+import numbers
 
 from .. import _lib
 from .._lib import ffi
@@ -48,6 +58,7 @@ FTYPES = {"size": 4, "sum": 6, "count": 7, "nunique": 8, "mean": 14, "min": 15, 
           "boolxor_agg": 30, "bitor_agg": 31, "bitand_agg": 32, "bitxor_agg": 33, "count_if": 34}
 MRNF = "min_row_number_filter"
 MRNF_MAX_SORT, MRNF_MAX_KEEP = 4, 26
+MRNF_MAX_LIMIT = 1 << 31  # mrnf_limit < 2^31 (the candidate store's sort holds at most 2^31 rows)
 _FIXED_WIDTH = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 11, 13, 15, 16}  # CTypes with a fixed-width cell (integers, floats, bool, temporals)
 
 
@@ -97,6 +108,7 @@ class GroupbyState:
     """Python handle of the C GroupbyState (created lazily at the first consume call)."""
 
     mrnf = None  # (sort_inds, asc, na_last, keep) of a min_row_number_filter state
+    mrnf_limit = 1  # rows kept per group by a min_row_number_filter state
 
     def __init__(self, operator_id, key_inds, fnames, f_in_offsets, f_in_cols, parallel, dropna, output_batch_size,
                  expected_groups, device, stream, process_group):
@@ -194,11 +206,11 @@ class GroupbyState:
         keep_mask = [0] * n
         for i in keep:
             keep_mask[remap[i]] = 1
-        h = L.b200_groupby_state_init_mrnf(self.operator_id, c_types, a_types, n, len(self.key_inds),
-                                           ffi.new("int32_t[]", [remap[i] for i in sort]), ffi.new("int32_t[]", [int(x) for x in asc]),
-                                           ffi.new("int32_t[]", [int(x) for x in na_last]), len(sort), ffi.new("int32_t[]", keep_mask),
-                                           self.output_batch_size, 0, int(self.dropna), self.device, 1, 0, self.expected_groups,
-                                           ffi.cast("void*", self.stream))
+        h = L.b200_groupby_state_init_mrnf_limit(self.operator_id, c_types, a_types, n, len(self.key_inds),
+                                                 ffi.new("int32_t[]", [remap[i] for i in sort]), ffi.new("int32_t[]", [int(x) for x in asc]),
+                                                 ffi.new("int32_t[]", [int(x) for x in na_last]), len(sort), ffi.new("int32_t[]", keep_mask),
+                                                 self.output_batch_size, 0, int(self.dropna), self.device, 1, 0, self.expected_groups,
+                                                 ffi.cast("void*", self.stream), self.mrnf_limit)
         self.handle = _lib.check_ptr(h, "init_groupby_state (min_row_number_filter)")
         # the library returns the kept columns in physical order (keys first); the output lists them in input order
         phys = sorted(remap[i] for i in keep)
@@ -336,7 +348,7 @@ def _current_device() -> int:
 def init_groupby_state(operator_id, key_inds, fnames, f_in_offsets, f_in_cols, mrnf_sort_col_inds=None,
                        mrnf_sort_col_asc=None, mrnf_sort_col_na=None, mrnf_col_inds_keep=None, op_pool_size_bytes=-1,
                        parallel=False, *, dropna=True, output_batch_size=32768, expected_groups=0, device=None,
-                       stream=0, process_group=None) -> GroupbyState:
+                       stream=0, process_group=None, mrnf_limit=1) -> GroupbyState:
     """Mirror of bodo.libs.streaming.groupby.init_groupby_state (groupby.py:702-715).
 
     key_inds / f_in_cols index the logical input table; fnames are names from supported_agg_funcs, or
@@ -344,7 +356,9 @@ def init_groupby_state(operator_id, key_inds, fnames, f_in_offsets, f_in_cols, m
     keep list, MRNF arguments beside other functions or min_row_number_filter without them raise B200Error naming the argument).
     op_pool_size_bytes is ignored (the table is sized in HBM, there is no host operator pool).
     Keyword-only extras: dropna (pandas_drop_na of the C++ ctor), output_batch_size, expected_groups
-    (sizing hint), device, stream (cudaStream_t as int), process_group (torch.distributed).
+    (sizing hint), device, stream (cudaStream_t as int), process_group (torch.distributed), mrnf_limit (rows kept per group by
+    min_row_number_filter, see the module docstring; a bool, a non-integer, a value < 1 or >= 2^31, or a value other than 1
+    without min_row_number_filter raise B200Error naming mrnf_limit).
     """
     key_inds = getattr(key_inds, "meta", key_inds)
     fnames = tuple(getattr(fnames, "meta", fnames))
@@ -352,12 +366,17 @@ def init_groupby_state(operator_id, key_inds, fnames, f_in_offsets, f_in_cols, m
     f_in_cols = getattr(f_in_cols, "meta", f_in_cols)
     mrnf = [getattr(x, "meta", x) for x in (mrnf_sort_col_inds, mrnf_sort_col_asc, mrnf_sort_col_na, mrnf_col_inds_keep)]
     spec = _mrnf_spec(tuple(int(k) for k in key_inds), fnames, f_in_offsets, f_in_cols, *mrnf)
+    if isinstance(mrnf_limit, bool) or not isinstance(mrnf_limit, numbers.Integral) or not 1 <= mrnf_limit < MRNF_MAX_LIMIT:
+        raise _lib.B200Error(f"Streaming Groupby: mrnf_limit must be an integer in [1, 2^31) (got {mrnf_limit!r})")
+    if spec is None and mrnf_limit != 1:
+        raise _lib.B200Error(f"Streaming Groupby: mrnf_limit={mrnf_limit} needs min_row_number_filter (fnames={fnames})")
     if spec is None:
         return GroupbyState(operator_id, key_inds, fnames, f_in_offsets, f_in_cols, parallel, dropna, output_batch_size,
                             expected_groups, device, stream, process_group)
     st = GroupbyState(operator_id, key_inds, (), (0,), (), parallel, dropna, output_batch_size, expected_groups, device, stream,
                       process_group)
     st.mrnf = spec
+    st.mrnf_limit = int(mrnf_limit)
     st.f_in_cols = tuple(int(c) for c in f_in_cols)
     return st
 

@@ -96,6 +96,28 @@ void* b200_groupby_state_init_mrnf(int64_t operator_id, const int8_t* build_arr_
                                    int32_t parallel, int32_t pandas_drop_na, int32_t device, int32_t n_pes, int32_t myrank,
                                    int64_t expected_groups, void* stream);
 
+/* b200_groupby_state_init_mrnf with a limit: QUALIFY ROW_NUMBER() OVER (PARTITION BY keys ORDER BY sort columns) <= rows_per_group,
+ * i.e. df.sort_values(sort columns, kind="stable").groupby(keys, sort=False, dropna=...).head(rows_per_group)[kept columns].  The
+ * reference's MRNF keeps one row per group; rows_per_group > 1 goes beyond it.
+ *   Arguments, keys, sort columns, kept columns (at most 26), dropna and the sharded refusal: as b200_groupby_state_init_mrnf.
+ *   rows_per_group: 1 <= rows_per_group < 2^31.  1 is b200_groupby_state_init_mrnf itself (one winner record per group, no store).
+ *   Rows: every group keeps the first rows_per_group rows of the stable order by (sort columns, arrival), arrival being batch
+ *     order, then row order, so of rows that tie on every sort column the earlier arrival ranks first, even across batches; a group
+ *     with fewer rows keeps all of them.  Each row holds its own cells (bits and validity) of the kept columns.
+ *   Output order: groups in an unspecified order; a group's rows are consecutive and in rank order, also when the group spans two
+ *     output batches, so a cumulative count numbers them.  The rows of every group are bit-identical across runs, batch splits and
+ *     table growth.
+ *   Limit: rows_per_group > 1 keeps candidate rows in a store that a radix sort of at most 2^31 rows reduces.  A consume call whose
+ *     rows, added to the survivors of every group (at most groups x rows_per_group), would pass 2^31 fails, naming the limit;
+ *     nothing is truncated.  Fewer than 2^48 rows in all.
+ *   Metrics: 0 is the groups while consuming and the output rows after finalize (the groups when rows_per_group == 1); 18 the
+ *     candidate rows admitted to the store, 19 the reduces of the store (both 0 when rows_per_group == 1). */
+void* b200_groupby_state_init_mrnf_limit(int64_t operator_id, const int8_t* build_arr_c_types, const int8_t* build_arr_array_types,
+                                         int32_t n_build_arrs, uint64_t n_keys, const int32_t* sort_cols, const int32_t* sort_ascending,
+                                         const int32_t* sort_na_last, int32_t n_sort, const int32_t* keep, int64_t output_batch_size,
+                                         int32_t parallel, int32_t pandas_drop_na, int32_t device, int32_t n_pes, int32_t myrank,
+                                         int64_t expected_groups, void* stream, int64_t rows_per_group);
+
 /* groupby_build_consume_batch_py_entry (_groupby.cpp:4663-4676). Returns 1 when the build is globally
  * finished (is_last was passed), 0 otherwise, <0 on error. *request_input is always set to 1 (the GPU
  * state sizes its table up front and never back-pressures). */
@@ -155,7 +177,8 @@ void b200_delete_groupby_state(void* state);
  * 4-byte keys or values, mean / min / max; included in 8), 13 groups in the table right now (exact: reads the device counter,
  * synchronises the state's stream), 14 SPG launches with narrow (int32 key, int32 value) bucket rows (SPG-N; included in 8),
  * 15 SPG launches with 16-byte (int64 key, int64 value) bucket rows (included in 8), 16 heavy-hitter keys admitted to the
- * partition kernel's hot table (0 when there are none or the table is disabled). */
+ * partition kernel's hot table (0 when there are none or the table is disabled), 18 / 19 candidate rows admitted / store reduces
+ * of a b200_groupby_state_init_mrnf_limit state (0 otherwise). */
 /* nunique keeps one nested distinct state over (key, value) per value column (owned by `state`).  A sharded caller exchanges every
  * nested state (the exchange above + b200_groupby_finalize on the handle returned here — a key's pairs are owned where the key is
  * owned) BEFORE it exchanges and finalizes the outer state; single-GPU callers never need these. */
