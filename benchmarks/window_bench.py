@@ -618,7 +618,7 @@ def main():
             torch.cuda.synchronize(dev)
         kern = {}
         for ev in prof.events():
-            if str(ev.device_type).endswith("CUDA") and "window_" in ev.name:
+            if str(ev.device_type).endswith("CUDA") and ("window_" in ev.name or "tile_carry_kernel" in ev.name):
                 key = ev.name.split("(")[0].replace("void b200::", "")
                 kern[key] = kern.get(key, 0.0) + getattr(ev, "device_time", getattr(ev, "cuda_time", 0.0)) / 1e3
         print(json.dumps({"case": name, "profile_kernel_ms": {k: round(v, 3) for k, v in sorted(kern.items())}, "card": card()}), flush=True)

@@ -353,7 +353,126 @@ using PooledBuf = DevBuf;
 // ids[0] or ids[1] (mask each entry with 0x7FFFFFFF), or nullptr for the identity (every digit constant, or n == 0).
 const uint32_t* radix_sort_columns(int n_keys, const void* const* data, const SortKey* keys, int64_t n, DevBuf (&ids)[2], cudaStream_t st);
 
-// Exclusive scan u32 -> u64 over 2048-row tiles (join.cu: offsets_tile_sum / offsets_carry / offsets_tile_scan kernels).
+// ---- tile scans (join.cu's offsets, sort.cu's window): a tile of 2048 rows, 256 threads x 8 items ----
+// A scan runs in three launches: each tile's reduction, tile_carry_kernel over the tile values, then each tile's scan seeded by
+// its prefix (tile_scan).  A scan value is a monoid M: M::T the value, M::identity(), and M::combine(a, b) with a covering the
+// earlier rows.  Values move between lanes word by word (shfl_up / shfl_xor), so M::T is trivially copyable and 4-byte aligned.
+// A value type may supply its own shfl_up(T, int) next to it: the helpers call shfl_up unqualified, so argument-dependent lookup
+// at instantiation picks that overload over the word-wise one (sort.cu does so for the window's scan values).
+constexpr int TILE_THREADS = 256, TILE_WARPS = TILE_THREADS / 32, TILE_ITEMS = 8, TILE_ROWS = TILE_THREADS * TILE_ITEMS;
+// Row of this thread's item k in tile t: items are warp-strided, so every load and store is coalesced.  tile_row(t, k) is
+// tile_row(t, 0) + k * TILE_THREADS; a kernel whose item loop only indexes rows takes that form and holds fewer registers.
+__device__ __forceinline__ int64_t tile_row(int64_t t, int k) {
+    return t * TILE_ROWS + (k * TILE_WARPS + (threadIdx.x >> 5)) * 32 + (threadIdx.x & 31);
+}
+
+template <typename U>
+struct SumOf {
+    using T = U;
+    __device__ __forceinline__ static T identity() { return 0; }
+    __device__ __forceinline__ static T combine(T a, T b) { return a + b; }
+};
+
+template <bool UP, typename T>
+__device__ __forceinline__ T shfl_words(T v, int o) {
+    static_assert(sizeof(T) % 4 == 0, "a scan value is whole 32-bit words");
+    uint32_t w[sizeof(T) / 4];
+    memcpy(w, &v, sizeof(T));
+#pragma unroll
+    for (int j = 0; j < (int)(sizeof(T) / 4); j++) w[j] = UP ? __shfl_up_sync(0xffffffffu, w[j], o) : __shfl_xor_sync(0xffffffffu, w[j], o);
+    memcpy(&v, w, sizeof(T));
+    return v;
+}
+template <typename T> __device__ __forceinline__ T shfl_up(T v, int o) { return shfl_words<true>(v, o); }
+template <typename T> __device__ __forceinline__ T shfl_xor(T v, int o) { return shfl_words<false>(v, o); }
+
+template <typename M>
+__device__ __forceinline__ typename M::T warp_inclusive_scan(typename M::T v) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const typename M::T y = shfl_up(v, o);
+        if (lane >= o) v = M::combine(y, v);
+    }
+    return v;
+}
+
+// The combine of every thread's v in the tile, in thread 0, for a commutative M: a warp butterfly, then the warps in order.
+template <typename M>
+__device__ __forceinline__ typename M::T block_reduce(typename M::T v) {
+    __shared__ typename M::T s_warp[TILE_WARPS];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = M::combine(v, shfl_xor(v, o));
+    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x == 0)
+        for (int w = 1; w < TILE_WARPS; w++) v = M::combine(v, s_warp[w]);
+    return v;
+}
+
+// s_seg[k * TILE_WARPS + warp] holds the total of segment (item k, warp), 32 rows; each becomes its exclusive prefix seeded by
+// `seed`.  Warp 0 scans the 64 segments in row order, two per lane.  Every thread of the tile calls it.  The seed is a reference,
+// so a tile prefix in memory is read by warp 0 only, after the barrier, and not held in every thread's registers.
+template <typename M>
+__device__ __forceinline__ void tile_segment_scan(typename M::T* s_seg, const typename M::T& seed) {
+    using T = typename M::T;
+    static_assert(TILE_ITEMS * TILE_WARPS == 64, "two segments per lane");
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    __syncthreads();
+    if (warp == 0) {
+        const T x0 = s_seg[2 * lane], x1 = s_seg[2 * lane + 1];
+        const T ex = shfl_up(warp_inclusive_scan<M>(M::combine(x0, x1)), 1);
+        T base = seed;
+        if (lane > 0) base = M::combine(base, ex);
+        s_seg[2 * lane] = base;
+        s_seg[2 * lane + 1] = M::combine(base, x0);
+    }
+    __syncthreads();
+}
+
+// Inclusive scan of this thread's TILE_ITEMS values of a tile (v[k] at tile_row(t, k)), seeded by `seed`: a warp scan per item,
+// the segment scan, then each segment's prefix combined in.
+template <typename M>
+__device__ __forceinline__ void tile_scan(const typename M::T& seed, typename M::T (&v)[TILE_ITEMS]) {
+    __shared__ typename M::T s_seg[TILE_ITEMS * TILE_WARPS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        v[k] = warp_inclusive_scan<M>(v[k]);
+        if (lane == 31) s_seg[k * TILE_WARPS + warp] = v[k];
+    }
+    tile_segment_scan<M>(s_seg, seed);
+#pragma unroll
+    for (int k = 0; k < TILE_ITEMS; k++) v[k] = M::combine(s_seg[k * TILE_WARPS + warp], v[k]);
+}
+
+// One block of 1024 threads, each a contiguous run of the n tile values c: c becomes their exclusive scan and *total (unless
+// nullptr) their combine.  A run's prefix starts from the identity, takes the earlier warps in order, then the earlier lanes of
+// its warp; the runs are then walked left to right.  The order depends on n only, so float scans are reproducible.
+template <typename M>
+__global__ void __launch_bounds__(1024) tile_carry_kernel(typename M::T* c, int64_t n, typename M::T* total) {
+    using T = typename M::T;
+    __shared__ T s_agg[32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t per = (n + 1023) / 1024, t0 = threadIdx.x * per, t1 = min(n, t0 + per);
+    T acc = M::identity();
+    for (int64_t t = t0; t < t1; t++) acc = M::combine(acc, c[t]);
+    const T inc = warp_inclusive_scan<M>(acc);
+    if (lane == 31) s_agg[warp] = inc;
+    __syncthreads();
+    T run = M::identity();
+    for (int w = 0; w < warp; w++) run = M::combine(run, s_agg[w]);
+    const T ex = shfl_up(inc, 1);
+    if (lane > 0) run = M::combine(run, ex);
+    for (int64_t t = t0; t < t1; t++) {
+        const T v = c[t];
+        c[t] = run;
+        run = M::combine(run, v);
+    }
+    if (total && threadIdx.x == 1023) *total = run;
+}
+
+// Exclusive scan u32 -> u64 (join.cu: offsets_tile_sum_kernel, tile_carry_kernel, offsets_tile_scan_kernel).
 struct Scanner {
     DevBuf sums, total;
     unsigned long long* h_total = nullptr;

@@ -34,82 +34,34 @@ constexpr long long J_EMPTY = (long long)0x8000000000000000ULL;
 constexpr int J_MAX_COLS = 32;
 constexpr uint32_t J_NONE = 0xffffffffu;
 
-// ---- exclusive scan u32 -> u64 in three launches over 2048-row tiles (256 threads x 8 rows, row k * 256 + thread of a
-// tile, so every load and store is coalesced): each tile's sum, one block's exclusive scan of the tile sums, each tile's scan
-// seeded by its prefix ----
-constexpr int OFS_THREADS = 256, OFS_WARPS = OFS_THREADS / 32, OFS_ITEMS = 8, OFS_TILE = OFS_THREADS * OFS_ITEMS;
-__device__ __forceinline__ int64_t ofs_row(int64_t t, int k) { return t * OFS_TILE + k * OFS_THREADS + threadIdx.x; }
-__device__ __forceinline__ unsigned long long ofs_warp_inclusive(unsigned long long v) {
-    const int lane = threadIdx.x & 31;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long y = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += y;
-    }
-    return v;
-}
-__global__ void __launch_bounds__(OFS_THREADS) offsets_tile_sum_kernel(const uint32_t* in, int64_t n, unsigned long long* sums) {
-    __shared__ unsigned long long s_warp[OFS_WARPS];
+// ---- exclusive scan u32 -> u64 in three launches over 2048-row tiles (common.cuh): each tile's sum, tile_carry_kernel over the
+// tile sums, each tile's scan seeded by its prefix ----
+__global__ void __launch_bounds__(TILE_THREADS) offsets_tile_sum_kernel(const uint32_t* in, int64_t n, unsigned long long* sums) {
     unsigned long long s = 0;
+    const int64_t i0 = tile_row(blockIdx.x, 0);
 #pragma unroll
-    for (int k = 0; k < OFS_ITEMS; k++) {
-        const int64_t i = ofs_row(blockIdx.x, k);
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        const int64_t i = i0 + k * TILE_THREADS;
         if (i < n) s += in[i];
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        for (int w = 1; w < OFS_WARPS; w++) s += s_warp[w];
-        sums[blockIdx.x] = s;
-    }
+    s = block_reduce<SumOf<unsigned long long>>(s);
+    if (threadIdx.x == 0) sums[blockIdx.x] = s;
 }
-// One block of 1024 threads, each a contiguous run of tile sums: c becomes its exclusive scan, *total the sum of all.
-__global__ void __launch_bounds__(1024) offsets_carry_kernel(unsigned long long* c, int64_t nb, unsigned long long* total) {
-    __shared__ unsigned long long s_warp[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t per = (nb + 1023) / 1024, b0 = threadIdx.x * per, b1 = min(nb, b0 + per);
-    unsigned long long acc = 0;
-    for (int64_t b = b0; b < b1; b++) acc += c[b];
-    const unsigned long long inc = ofs_warp_inclusive(acc);
-    if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();
-    unsigned long long run = inc - acc;  // the earlier lanes of this warp, then the earlier warps
-    for (int w = 0; w < warp; w++) run += s_warp[w];
-    for (int64_t b = b0; b < b1; b++) {
-        const unsigned long long v = c[b];
-        c[b] = run;
-        run += v;
-    }
-    if (threadIdx.x == 1023) *total = run;
-}
-__global__ void __launch_bounds__(OFS_THREADS) offsets_tile_scan_kernel(const uint32_t* in, int64_t n, const unsigned long long* carry,
-                                                                        unsigned long long* out) {
-    __shared__ unsigned long long s_seg[OFS_ITEMS * OFS_WARPS];  // per (item, warp) segment of 32 rows: its sum, then its prefix
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t x[OFS_ITEMS];
-    unsigned long long v[OFS_ITEMS];
+__global__ void __launch_bounds__(TILE_THREADS) offsets_tile_scan_kernel(const uint32_t* in, int64_t n, const unsigned long long* carry,
+                                                                         unsigned long long* out) {
+    uint32_t x[TILE_ITEMS];
+    unsigned long long v[TILE_ITEMS];
+    const int64_t i0 = tile_row(blockIdx.x, 0);
 #pragma unroll
-    for (int k = 0; k < OFS_ITEMS; k++) {
-        const int64_t i = ofs_row(blockIdx.x, k);
-        x[k] = i < n ? in[i] : 0;
-        v[k] = ofs_warp_inclusive(x[k]);
-        if (lane == 31) s_seg[k * OFS_WARPS + warp] = v[k];
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        const int64_t i = i0 + k * TILE_THREADS;
+        v[k] = x[k] = i < n ? in[i] : 0;
     }
-    __syncthreads();
-    if (warp == 0) {  // the 64 segments in row order, two per lane, seeded by the tile's prefix
-        static_assert(OFS_ITEMS * OFS_WARPS == 64, "two segments per lane");
-        const unsigned long long x0 = s_seg[2 * lane], x1 = s_seg[2 * lane + 1];
-        const unsigned long long base = carry[blockIdx.x] + ofs_warp_inclusive(x0 + x1) - x0 - x1;
-        s_seg[2 * lane] = base;
-        s_seg[2 * lane + 1] = base + x0;
-    }
-    __syncthreads();
+    tile_scan<SumOf<unsigned long long>>(carry[blockIdx.x], v);
 #pragma unroll
-    for (int k = 0; k < OFS_ITEMS; k++) {
-        const int64_t i = ofs_row(blockIdx.x, k);
-        if (i < n) out[i] = s_seg[k * OFS_WARPS + warp] + v[k] - x[k];
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        const int64_t i = i0 + k * TILE_THREADS;
+        if (i < n) out[i] = v[k] - x[k];
     }
 }
 
@@ -117,12 +69,12 @@ Scanner::~Scanner() { pinned_release(h_total, 8); }
 unsigned long long Scanner::run(const uint32_t* in, int64_t n, unsigned long long* out, cudaStream_t st, int64_t* launches) {
     if (!h_total) h_total = (unsigned long long*)pinned_acquire(8);
     if (n == 0) return 0;
-    int64_t nb = (n + OFS_TILE - 1) / OFS_TILE;
+    int64_t nb = (n + TILE_ROWS - 1) / TILE_ROWS;
     sums.ensure((size_t)nb * 8);
     total.ensure(8);
-    offsets_tile_sum_kernel<<<(unsigned)nb, OFS_THREADS, 0, st>>>(in, n, sums.as<unsigned long long>());
-    offsets_carry_kernel<<<1, 1024, 0, st>>>(sums.as<unsigned long long>(), nb, total.as<unsigned long long>());
-    offsets_tile_scan_kernel<<<(unsigned)nb, OFS_THREADS, 0, st>>>(in, n, sums.as<unsigned long long>(), out);
+    offsets_tile_sum_kernel<<<(unsigned)nb, TILE_THREADS, 0, st>>>(in, n, sums.as<unsigned long long>());
+    tile_carry_kernel<SumOf<unsigned long long>><<<1, 1024, 0, st>>>(sums.as<unsigned long long>(), nb, total.as<unsigned long long>());
+    offsets_tile_scan_kernel<<<(unsigned)nb, TILE_THREADS, 0, st>>>(in, n, sums.as<unsigned long long>(), out);
     *launches += 3;
     B200_CUDA(cudaGetLastError());
     B200_CUDA(cudaMemcpyAsync(h_total, total.p, 8, cudaMemcpyDeviceToHost, st));
@@ -450,9 +402,7 @@ __global__ void __launch_bounds__(256) join_probe_fast_kernel(const __grid_const
         }
         __syncthreads();
         if (warp == 0) {  // exclusive scan of the 32 (row-slot, warp) counts, one cursor atomic for the tile
-            unsigned int x = wcnt[lane], inc = x;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { unsigned int y = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += y; }
+            const unsigned int x = wcnt[lane], inc = warp_inclusive_scan<SumOf<unsigned int>>(x);
             woff[lane] = inc - x;
             if (lane == 31) tile_base = inc ? atomicAdd(a.cursor, (unsigned long long)inc) : 0ull;
         }
@@ -629,9 +579,7 @@ __global__ void __launch_bounds__(256) join_probe_inline_kernel(const __grid_con
         }
         __syncthreads();
         if (warp == 0) {
-            unsigned int x = wcnt[lane], inc = x;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { unsigned int y = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += y; }
+            const unsigned int x = wcnt[lane], inc = warp_inclusive_scan<SumOf<unsigned int>>(x);
             woff[lane] = inc - x;
             if (lane == 31) tile_base = inc ? atomicAdd(a.cursor, (unsigned long long)inc) : 0ull;
         }

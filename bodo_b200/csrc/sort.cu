@@ -127,9 +127,7 @@ __global__ void __launch_bounds__(TK_THREADS, 4) topk_filter_kernel(const __grid
         __syncthreads();
         if (threadIdx.x < 32) {  // exclusive scan of the 32 (row slot, warp) counts; one cursor atomic per tile
             const int r = threadIdx.x >> 3, w = threadIdx.x & 7;
-            unsigned int x = wsum[r][w], inc = x;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += y; }
+            const unsigned int x = wsum[r][w], inc = warp_inclusive_scan<SumOf<unsigned int>>(x);
             wsum[r][w] = inc - x;
             if (lane == 31) tile_base = inc ? atomicAdd(a.cursor, (unsigned long long)inc) : 0ull;
         }
@@ -463,9 +461,7 @@ __global__ void __launch_bounds__(FS_THREADS) fsort_pass_kernel(const __grid_con
     uint32_t cnt = 0;
 #pragma unroll
     for (int q = 0; q < FS_WARPS; q++) { const uint32_t x = s_hist[q][d]; s_hist[q][d] = cnt; cnt += x; }
-    uint32_t inc = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
+    const uint32_t inc = warp_inclusive_scan<SumOf<uint32_t>>(cnt);
     if (lane == 31) s_wsum[warp] = inc;
     volatile unsigned long long* status = a.status;
     const unsigned long long tag = (unsigned long long)a.epoch << 34;
@@ -935,9 +931,9 @@ struct FullSortState : SortState {
 //
 //   window_bounds_kernel  one pass over the sorted key columns: position i starts a partition when a partition key's (NA class,
 //                         radix word) differs from position i - 1's, and a peer group when any key does (i = 0 starts both).
-//                         The row at i - 1 is the tile's one-row halo.  Writes one flag byte per position and per WN_TILE-row
+//                         The row at i - 1 is the tile's one-row halo.  Writes one flag byte per position and per TILE_ROWS-row
 //                         tile the reduction of the scan values below, plus the tile's partition-start count.
-//   window_tiles_kernel   one block: the exclusive scan of the tile values, and the partition and peer-group totals.
+//   tile_carry_kernel     one block (common.cuh): the exclusive scan of the tile values, and their total (the partition count).
 //   window_ends_kernel    scan of the flags seeded by the tile prefix: per position the partition start P (a max-scan of the
 //                         start positions), the peer start Q (a max-scan) and D, the number of peer starts up to the position.
 //                         The last row of a partition writes its size into slot P and the last row of a peer group its end into
@@ -945,12 +941,27 @@ struct FullSortState : SortState {
 //   window_eval_kernel    the same scan again, then every requested function per position.
 // Row positions are below 2^31 (the full sort's limit), so positions, sizes and counts are uint32.
 enum { WN_ROW_NUMBER = 0, WN_RANK = 1, WN_DENSE_RANK = 2, WN_PERCENT_RANK = 3, WN_CUME_DIST = 4, WN_NTILE = 5 };
-constexpr int WN_THREADS = 256, WN_WARPS = WN_THREADS / 32, WN_ITEMS = 8, WN_TILE = WN_THREADS * WN_ITEMS;
 constexpr uint8_t WN_PART = 1, WN_PEER = 2;  // a partition start is also a peer-group start
 
 // Scan value of a position: (partition start, peer start, peer starts so far) under (max, max, +).
-struct WnAgg { uint32_t p, q, d; };
-__device__ __forceinline__ WnAgg wn_combine(WnAgg a, WnAgg b) { return {max(a.p, b.p), max(a.q, b.q), a.d + b.d}; }
+struct WnAgg {
+    using T = WnAgg;
+    uint32_t p, q, d;
+    __device__ __forceinline__ static WnAgg identity() { return {0, 0, 0}; }
+    __device__ __forceinline__ static WnAgg combine(WnAgg a, WnAgg b) { return {max(a.p, b.p), max(a.q, b.q), a.d + b.d}; }
+};
+// Field by field rather than common.cuh's word-wise shfl_up: the per-row kernels then keep their registers and code.
+__device__ __forceinline__ WnAgg shfl_up(WnAgg v, int o) {
+    return WnAgg{__shfl_up_sync(0xffffffffu, v.p, o), __shfl_up_sync(0xffffffffu, v.q, o), __shfl_up_sync(0xffffffffu, v.d, o)};
+}
+// A tile's value: its WnAgg and its partition starts, so the scan's total is the partition count.
+struct WnTile {
+    using T = WnTile;
+    WnAgg v;
+    uint32_t parts;
+    __device__ __forceinline__ static WnTile identity() { return {WnAgg::identity(), 0}; }
+    __device__ __forceinline__ static WnTile combine(WnTile a, WnTile b) { return {WnAgg::combine(a.v, b.v), a.parts + b.parts}; }
+};
 
 struct WnArgs {
     int64_t n;
@@ -959,20 +970,14 @@ struct WnArgs {
     const char* data[SORT_MAX_KEYS];   // sorted key columns
     const uint8_t* vb[SORT_MAX_KEYS];  // their validity bytes, nullptr for a numpy column
     uint8_t* flags;
-    WnAgg* tile;          // per tile: its reduction (bounds), then its exclusive prefix (tiles)
-    uint32_t* tile_parts; // per tile: partition starts
-    uint32_t* totals;     // [0] partitions, [1] peer groups
+    WnTile* tile;         // per tile: its reduction (bounds), then its exclusive prefix (tile_carry_kernel)
+    WnTile* total;        // the combine of every tile: .parts is the partition count
     uint32_t *psize, *pend, *pdense;  // slot P: partition size, slot Q: peer-group end, slot P: D at the partition start
     int n_funcs;
     int func[SORT_MAX_COLS];
     int64_t farg[SORT_MAX_COLS];
     void* out[SORT_MAX_COLS];
 };
-
-// Position of item k of thread (warp, lane) in tile t: items are warp-strided, so every load and store is coalesced.
-__device__ __forceinline__ int64_t wn_row(int64_t t, int k, int warp, int lane) {
-    return t * WN_TILE + (k * WN_WARPS + warp) * 32 + lane;
-}
 
 __device__ __forceinline__ bool wn_key_differs(const WnArgs& a, int j, int64_t i) {
     const SortKey& k = a.key[j];
@@ -982,16 +987,12 @@ __device__ __forceinline__ bool wn_key_differs(const WnArgs& a, int j, int64_t i
     return na0 != na1 || w0 != w1;
 }
 
-__global__ void __launch_bounds__(WN_THREADS) window_bounds_kernel(const __grid_constant__ WnArgs a) {
-    __shared__ WnAgg s_agg[WN_WARPS];
-    __shared__ uint32_t s_parts[WN_WARPS];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+__global__ void __launch_bounds__(TILE_THREADS) window_bounds_kernel(const __grid_constant__ WnArgs a) {
     const int64_t t = blockIdx.x;
-    WnAgg acc{0, 0, 0};
-    uint32_t parts = 0;
+    WnTile acc = WnTile::identity();
 #pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        const int64_t i = tile_row(t, k);
         if (i >= a.n) break;
         uint8_t f = WN_PART | WN_PEER;
         if (i > 0) {
@@ -1000,110 +1001,54 @@ __global__ void __launch_bounds__(WN_THREADS) window_bounds_kernel(const __grid_
                 if (wn_key_differs(a, j, i)) f = j < a.n_part ? (WN_PART | WN_PEER) : WN_PEER;
         }
         a.flags[i] = f;
-        if (f & WN_PART) { acc.p = (uint32_t)i; parts++; }
-        if (f & WN_PEER) { acc.q = (uint32_t)i; acc.d++; }
+        if (f & WN_PART) { acc.v.p = (uint32_t)i; acc.parts++; }
+        if (f & WN_PEER) { acc.v.q = (uint32_t)i; acc.v.d++; }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        acc = wn_combine(acc, WnAgg{__shfl_xor_sync(0xffffffffu, acc.p, o), __shfl_xor_sync(0xffffffffu, acc.q, o),
-                                    __shfl_xor_sync(0xffffffffu, acc.d, o)});
-        parts += __shfl_xor_sync(0xffffffffu, parts, o);
-    }
-    if (lane == 0) { s_agg[warp] = acc; s_parts[warp] = parts; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        for (int w = 1; w < WN_WARPS; w++) { acc = wn_combine(acc, s_agg[w]); parts += s_parts[w]; }
-        a.tile[t] = acc;
-        a.tile_parts[t] = parts;
-    }
+    acc = block_reduce<WnTile>(acc);
+    if (threadIdx.x == 0) a.tile[t] = acc;
 }
 
-// One block of 1024 threads; thread x scans a contiguous run of tiles.
-__global__ void __launch_bounds__(1024) window_tiles_kernel(const __grid_constant__ WnArgs a, int64_t n_tiles) {
-    __shared__ WnAgg s_agg[32];
-    __shared__ uint32_t s_parts[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t per = (n_tiles + 1023) / 1024, t0 = threadIdx.x * per, t1 = min(n_tiles, t0 + per);
-    WnAgg acc{0, 0, 0};
-    uint32_t parts = 0;
-    for (int64_t t = t0; t < t1; t++) { acc = wn_combine(acc, a.tile[t]); parts += a.tile_parts[t]; }
-    WnAgg inc = acc;
+// Inclusive scan values of this thread's TILE_ITEMS positions of tile t, seeded by the tile's exclusive prefix; f: their flags.
+__device__ __forceinline__ void wn_scan_tile(int64_t n, const uint8_t* flags, const WnTile* tile, int64_t t, uint8_t (&f)[TILE_ITEMS],
+                                             WnAgg (&v)[TILE_ITEMS]) {
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const WnAgg y{__shfl_up_sync(0xffffffffu, inc.p, o), __shfl_up_sync(0xffffffffu, inc.q, o), __shfl_up_sync(0xffffffffu, inc.d, o)};
-        if (lane >= o) inc = wn_combine(y, inc);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) parts += __shfl_xor_sync(0xffffffffu, parts, o);
-    if (lane == 31) s_agg[warp] = inc;
-    if (lane == 0) s_parts[warp] = parts;
-    __syncthreads();
-    WnAgg run{0, 0, 0};
-    for (int w = 0; w < warp; w++) run = wn_combine(run, s_agg[w]);
-    // exclusive prefix of this thread's first tile: the earlier warps, then the earlier lanes of this warp
-    WnAgg ex{__shfl_up_sync(0xffffffffu, inc.p, 1), __shfl_up_sync(0xffffffffu, inc.q, 1), __shfl_up_sync(0xffffffffu, inc.d, 1)};
-    if (lane > 0) run = wn_combine(run, ex);
-    for (int64_t t = t0; t < t1; t++) {
-        const WnAgg v = a.tile[t];
-        a.tile[t] = run;
-        run = wn_combine(run, v);
-    }
-    if (threadIdx.x == 1023) {
-        uint32_t total_parts = 0;
-        for (int w = 0; w < 32; w++) total_parts += s_parts[w];
-        a.totals[0] = total_parts;
-        a.totals[1] = run.d;
-    }
-}
-
-// Inclusive scan values of this thread's WN_ITEMS positions of tile t, seeded by the tile's exclusive prefix.
-__device__ __forceinline__ void wn_scan_tile(const WnArgs& a, int64_t t, uint8_t (&f)[WN_ITEMS], WnAgg (&v)[WN_ITEMS]) {
-    __shared__ WnAgg s_seg[WN_ITEMS * WN_WARPS];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
-        f[k] = i < a.n ? a.flags[i] : 0;
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        const int64_t i = tile_row(t, k);
+        f[k] = i < n ? flags[i] : 0;
         v[k] = WnAgg{(f[k] & WN_PART) ? (uint32_t)i : 0u, (f[k] & WN_PEER) ? (uint32_t)i : 0u, (f[k] & WN_PEER) ? 1u : 0u};
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const WnAgg y{__shfl_up_sync(0xffffffffu, v[k].p, o), __shfl_up_sync(0xffffffffu, v[k].q, o),
-                          __shfl_up_sync(0xffffffffu, v[k].d, o)};
-            if (lane >= o) v[k] = wn_combine(y, v[k]);
-        }
-        if (lane == 31) s_seg[k * WN_WARPS + warp] = v[k];
     }
-    __syncthreads();
-    if (warp == 0) {  // exclusive scan of the 64 (item, warp) segments in row order, seeded by the tile prefix: 2 per lane
-        static_assert(WN_ITEMS * WN_WARPS == 64, "two segments per lane");
-        const WnAgg x0 = s_seg[2 * lane], x1 = s_seg[2 * lane + 1];
-        const WnAgg pair = wn_combine(x0, x1);
-        WnAgg inc = pair;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const WnAgg y{__shfl_up_sync(0xffffffffu, inc.p, o), __shfl_up_sync(0xffffffffu, inc.q, o), __shfl_up_sync(0xffffffffu, inc.d, o)};
-            if (lane >= o) inc = wn_combine(y, inc);
-        }
-        WnAgg ex{__shfl_up_sync(0xffffffffu, inc.p, 1), __shfl_up_sync(0xffffffffu, inc.q, 1), __shfl_up_sync(0xffffffffu, inc.d, 1)};
-        WnAgg base = a.tile[t];
-        if (lane > 0) base = wn_combine(base, ex);
-        s_seg[2 * lane] = base;
-        s_seg[2 * lane + 1] = wn_combine(base, x0);
-    }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) v[k] = wn_combine(s_seg[k * WN_WARPS + warp], v[k]);
+    tile_scan<WnAgg>(tile[t].v, v);
 }
 
-__global__ void __launch_bounds__(WN_THREADS) window_ends_kernel(const __grid_constant__ WnArgs a) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+// The ranking scan of this block's tile, then body(i, v) for each of this thread's positions i < n, v its scan value.  The
+// bodies have out-of-line slow paths (divisions, searches): holding every item's scan values in registers across them spills,
+// so each thread parks its own values in shared memory and the item loop is not unrolled.
+template <typename Body>
+__device__ __forceinline__ void wn_for_rows(int64_t n, const uint8_t* flags, const WnTile* tile, Body body) {
     const int64_t t = blockIdx.x;
-    uint8_t f[WN_ITEMS];
-    WnAgg v[WN_ITEMS];
-    wn_scan_tile(a, t, f, v);
+    uint8_t f[TILE_ITEMS];
+    WnAgg v[TILE_ITEMS];
+    wn_scan_tile(n, flags, tile, t, f, v);
+    __shared__ WnAgg s_v[TILE_ITEMS][TILE_THREADS];
 #pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
+    for (int k = 0; k < TILE_ITEMS; k++) s_v[k][threadIdx.x] = v[k];
+#pragma unroll 1
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        const int64_t i = tile_row(t, k);
+        if (i >= n) break;
+        body(i, s_v[k][threadIdx.x]);
+    }
+}
+
+__global__ void __launch_bounds__(TILE_THREADS) window_ends_kernel(const __grid_constant__ WnArgs a) {
+    const int64_t t = blockIdx.x;
+    uint8_t f[TILE_ITEMS];
+    WnAgg v[TILE_ITEMS];
+    wn_scan_tile(a.n, a.flags, a.tile, t, f, v);
+    const int64_t i0 = tile_row(t, 0);
+#pragma unroll
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        const int64_t i = i0 + k * TILE_THREADS;
         if (i >= a.n) break;
         const uint8_t next = i + 1 < a.n ? a.flags[i + 1] : (WN_PART | WN_PEER);
         if (f[k] & WN_PART) a.pdense[i] = v[k].d;
@@ -1112,22 +1057,8 @@ __global__ void __launch_bounds__(WN_THREADS) window_ends_kernel(const __grid_co
     }
 }
 
-__global__ void __launch_bounds__(WN_THREADS) window_eval_kernel(const __grid_constant__ WnArgs a) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t t = blockIdx.x;
-    uint8_t f[WN_ITEMS];
-    WnAgg v[WN_ITEMS];
-    wn_scan_tile(a, t, f, v);
-    // The divisions below have out-of-line slow paths: holding every item's scan values in registers across them spills, so
-    // each thread parks its own values in shared memory and the item loop is not unrolled.
-    __shared__ WnAgg s_v[WN_ITEMS][WN_THREADS];
-#pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) s_v[k][threadIdx.x] = v[k];
-#pragma unroll 1
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
-        if (i >= a.n) break;
-        const WnAgg vk = s_v[k][threadIdx.x];
+__global__ void __launch_bounds__(TILE_THREADS) window_eval_kernel(const __grid_constant__ WnArgs a) {
+    wn_for_rows(a.n, a.flags, a.tile, [&](int64_t i, const WnAgg vk) {
         const uint32_t P = vk.p, s = a.psize[P], pos = (uint32_t)i - P, rank = vk.q - P + 1;
         for (int fn = 0; fn < a.n_funcs; fn++) {
             int64_t r = 0;
@@ -1147,7 +1078,7 @@ __global__ void __launch_bounds__(WN_THREADS) window_eval_kernel(const __grid_co
             if (a.func[fn] == WN_PERCENT_RANK || a.func[fn] == WN_CUME_DIST) ((double*)a.out[fn])[i] = x;
             else ((int64_t*)a.out[fn])[i] = r;
         }
-    }
+    });
 }
 
 // ---- value window functions: SUM / COUNT / MEAN / MIN / MAX / FIRST_VALUE / LAST_VALUE over a frame [P, e], LAG / LEAD ----
@@ -1155,8 +1086,8 @@ __global__ void __launch_bounds__(WN_THREADS) window_eval_kernel(const __grid_co
 // They run after window_ends_kernel, over the sorted columns the gather wrote.  A frame starts at the partition start P and ends
 // at e = i (WF_ROWS), the row's last peer pend[Q] - 1 (WF_RANGE) or the partition's last row P + psize[P] - 1 (WF_PARTITION).
 //   window_vscan_kernel<K, false>  per scan function (sum, count of a column, mean, min, max): the segmented reduction of each
-//                                  WN_TILE-row tile, reset at partition starts (the WN_PART flags).
-//   window_vtiles_kernel<K>        one block: the exclusive scan of the tile carries.
+//                                  TILE_ROWS-row tile, reset at partition starts (the WN_PART flags).
+//   tile_carry_kernel<Wv<K>>       one block: the exclusive scan of the tile carries.
 //   window_vscan_kernel<K, true>   the tile's scan again, seeded by its carry; every position that ends a frame of the function
 //                                  writes the function's final cell and validity byte there.
 //   window_veval_kernel            the ranking scan of the flags (P, Q) again, then per position and value function: a scan
@@ -1177,24 +1108,16 @@ constexpr uint64_t WV_NEG_ZERO = 0x8000000000000000ull;      // -0.0, the identi
 struct WvAgg { uint64_t x; uint32_t c, f; };
 
 // VAR / STDDEV / VAR_POP / STDDEV_POP (codes 16..19) scan kind WV_MOM: c the count of valid cells, f as WvAgg's, mean their
-// mean and m2 = sum (x - mean)^2, combined by Chan's pairwise merge (wv_combine<WV_MOM>).  wv_t<K> is kind K's scan value.
+// mean and m2 = sum (x - mean)^2, combined by Chan's pairwise merge (Wv<WV_MOM>::combine).  wv_t<K> is kind K's scan value.
 enum { WN_VAR = 16, WN_STD = 17, WN_VAR_POP = 18, WN_STD_POP = 19 };
 enum { WV_MOM = 5 };
 struct WvMom { uint32_t c, f; double mean, m2; };
 // COVAR_SAMP / COVAR_POP / CORR / REGR_SLOPE / REGR_INTERCEPT (codes 20..24, y = the function's column, x = its second column)
 // scan kind WV_CO: c the count of rows where both cells are valid and non-NaN, f as WvAgg's, mx / my their means and sxx / syy /
-// sxy = sum (x - mx)^2, sum (y - my)^2, sum (x - mx)(y - my), combined by the bivariate form of Chan's merge (wv_combine<WV_CO>).
+// sxy = sum (x - mx)^2, sum (y - my)^2, sum (x - mx)(y - my), combined by the bivariate form of Chan's merge (Wv<WV_CO>::combine).
 enum { WN_COVAR_SAMP = 20, WN_COVAR_POP = 21, WN_CORR = 22, WN_REGR_SLOPE = 23, WN_REGR_INTERCEPT = 24 };
 enum { WV_CO = 6 };
 struct WvCo { uint32_t c, f; double mx, my, sxx, syy, sxy; };
-template <int K> struct WvKind { using T = WvAgg; };
-template <> struct WvKind<WV_MOM> { using T = WvMom; };
-template <> struct WvKind<WV_CO> { using T = WvCo; };
-template <int K> using wv_t = typename WvKind<K>::T;
-
-// The carry and tree buffers hold kind K's scan values.
-template <int K>
-__device__ __forceinline__ wv_t<K>* wv_buf(void* p) { return (wv_t<K>*)p; }
 
 // A function whose result comes from a scan or a tree of its scan values: sum, count, mean, min, max and the moments (the ranking
 // codes are routed before this is asked).
@@ -1225,68 +1148,78 @@ struct WvArgs {
     const uint8_t* flags;
     const uint32_t *psize, *pend;
     void* carry;   // per tile: its reduction, then its exclusive prefix (wv_t<K>)
-    WvFunc s;      // window_vscan_kernel / window_vtiles_kernel: the function being scanned
+    WvFunc s;      // window_vscan_kernel: the function being scanned
     int n_funcs;   // window_veval_kernel: the value functions with work there
     WvFunc f[SORT_MAX_COLS];
 };
 
+// Kind K's scan value as a monoid (common.cuh): Wv<K>::T, identity() and combine(a, b).
 template <int K>
-__device__ __forceinline__ wv_t<K> wv_identity() { return WvAgg{K == WV_FSUM ? WV_NEG_ZERO : 0ull, (K == WV_MIN || K == WV_MAX) ? WV_NONE : 0u, 0u}; }
-template <>
-__device__ __forceinline__ WvMom wv_identity<WV_MOM>() { return WvMom{0u, 0u, 0.0, 0.0}; }
-template <>
-__device__ __forceinline__ WvCo wv_identity<WV_CO>() { return WvCo{0u, 0u, 0.0, 0.0, 0.0, 0.0, 0.0}; }
-
-template <int K>
-__device__ __forceinline__ wv_t<K> wv_combine(wv_t<K> a, wv_t<K> b) {
-    if (b.f) return b;
-    WvAgg r{b.x, b.c, a.f};
-    if (K == WV_ISUM) { r.x = a.x + b.x; r.c = a.c + b.c; }
-    else if (K == WV_FSUM) { r.x = (uint64_t)__double_as_longlong(__longlong_as_double((long long)a.x) + __longlong_as_double((long long)b.x)); r.c = a.c + b.c; }
-    else {
-        const bool take_b = a.c == WV_NONE || (b.c != WV_NONE && (K == WV_MIN ? b.x < a.x : b.x > a.x));  // ties keep the left row
-        if (!take_b) { r.x = a.x; r.c = a.c; }
+struct Wv {
+    using T = WvAgg;
+    __device__ __forceinline__ static WvAgg identity() { return WvAgg{K == WV_FSUM ? WV_NEG_ZERO : 0ull, (K == WV_MIN || K == WV_MAX) ? WV_NONE : 0u, 0u}; }
+    __device__ __forceinline__ static WvAgg combine(WvAgg a, WvAgg b) {
+        if (b.f) return b;
+        WvAgg r{b.x, b.c, a.f};
+        if (K == WV_ISUM) { r.x = a.x + b.x; r.c = a.c + b.c; }
+        else if (K == WV_FSUM) { r.x = (uint64_t)__double_as_longlong(__longlong_as_double((long long)a.x) + __longlong_as_double((long long)b.x)); r.c = a.c + b.c; }
+        else {
+            const bool take_b = a.c == WV_NONE || (b.c != WV_NONE && (K == WV_MIN ? b.x < a.x : b.x > a.x));  // ties keep the left row
+            if (!take_b) { r.x = a.x; r.c = a.c; }
+        }
+        return r;
     }
-    return r;
-}
+};
 // Chan's merge of (n_a, mean_a, M2_a) and (n_b, mean_b, M2_b): with d = mean_b - mean_a and n = n_a + n_b, mean = mean_a +
 // d n_b / n and M2 = M2_a + M2_b + d^2 n_a n_b / n.  An empty side gives the other side's values exactly (no 0 / 0); every term
 // of M2 is >= 0, and equal means give d = 0, so a frame of equal values has M2 = 0 exactly.
 template <>
-__device__ __forceinline__ WvMom wv_combine<WV_MOM>(WvMom a, WvMom b) {
-    if (b.f) return b;
-    if (b.c == 0) return a;
-    if (a.c == 0) { b.f = a.f; return b; }
-    const uint32_t n = a.c + b.c;
-    const double w = (double)b.c / (double)n, d = b.mean - a.mean;
-    return WvMom{n, a.f, a.mean + d * w, a.m2 + b.m2 + d * (d * ((double)a.c * w))};
-}
+struct Wv<WV_MOM> {
+    using T = WvMom;
+    __device__ __forceinline__ static WvMom identity() { return WvMom{0u, 0u, 0.0, 0.0}; }
+    __device__ __forceinline__ static WvMom combine(WvMom a, WvMom b) {
+        if (b.f) return b;
+        if (b.c == 0) return a;
+        if (a.c == 0) { b.f = a.f; return b; }
+        const uint32_t n = a.c + b.c;
+        const double w = (double)b.c / (double)n, d = b.mean - a.mean;
+        return WvMom{n, a.f, a.mean + d * w, a.m2 + b.m2 + d * (d * ((double)a.c * w))};
+    }
+};
 // The bivariate merge: the means as WV_MOM's, and with t = n_a n_b / n, sxx += (dx dx) t, syy += (dy dy) t, sxy += (dx dy) t.
 // The three terms are formed alike, so swapping x and y swaps sxx and syy and leaves sxy's bits (dx dy = dy dx), and x = y gives
 // sxx, syy and sxy the same bits; a frame of equal x has dx = 0 at every merge, so sxx = 0 exactly.
 template <>
-__device__ __forceinline__ WvCo wv_combine<WV_CO>(WvCo a, WvCo b) {
-    if (b.f) return b;
-    if (b.c == 0) return a;
-    if (a.c == 0) { b.f = a.f; return b; }
-    const uint32_t n = a.c + b.c;
-    const double w = (double)b.c / (double)n, dx = b.mx - a.mx, dy = b.my - a.my, t = (double)a.c * w;
-    return WvCo{n, a.f, a.mx + dx * w, a.my + dy * w, a.sxx + b.sxx + (dx * dx) * t, a.syy + b.syy + (dy * dy) * t,
-                a.sxy + b.sxy + (dx * dy) * t};
-}
-
-__device__ __forceinline__ WvAgg wv_shfl_up(WvAgg v, int o) {
+struct Wv<WV_CO> {
+    using T = WvCo;
+    __device__ __forceinline__ static WvCo identity() { return WvCo{0u, 0u, 0.0, 0.0, 0.0, 0.0, 0.0}; }
+    __device__ __forceinline__ static WvCo combine(WvCo a, WvCo b) {
+        if (b.f) return b;
+        if (b.c == 0) return a;
+        if (a.c == 0) { b.f = a.f; return b; }
+        const uint32_t n = a.c + b.c;
+        const double w = (double)b.c / (double)n, dx = b.mx - a.mx, dy = b.my - a.my, t = (double)a.c * w;
+        return WvCo{n, a.f, a.mx + dx * w, a.my + dy * w, a.sxx + b.sxx + (dx * dx) * t, a.syy + b.syy + (dy * dy) * t,
+                    a.sxy + b.sxy + (dx * dy) * t};
+    }
+};
+template <int K> using wv_t = typename Wv<K>::T;
+// Field-wise shuffles, as WnAgg's: the value scans then compile as with per-field shuffles of their own.
+__device__ __forceinline__ WvAgg shfl_up(WvAgg v, int o) {
     return WvAgg{__shfl_up_sync(0xffffffffu, (unsigned long long)v.x, o), __shfl_up_sync(0xffffffffu, v.c, o), __shfl_up_sync(0xffffffffu, v.f, o)};
 }
-__device__ __forceinline__ WvMom wv_shfl_up(WvMom v, int o) {
+__device__ __forceinline__ WvMom shfl_up(WvMom v, int o) {
     return WvMom{__shfl_up_sync(0xffffffffu, v.c, o), __shfl_up_sync(0xffffffffu, v.f, o), __shfl_up_sync(0xffffffffu, v.mean, o),
                  __shfl_up_sync(0xffffffffu, v.m2, o)};
 }
-__device__ __forceinline__ WvCo wv_shfl_up(WvCo v, int o) {
+__device__ __forceinline__ WvCo shfl_up(WvCo v, int o) {
     return WvCo{__shfl_up_sync(0xffffffffu, v.c, o), __shfl_up_sync(0xffffffffu, v.f, o), __shfl_up_sync(0xffffffffu, v.mx, o),
                 __shfl_up_sync(0xffffffffu, v.my, o), __shfl_up_sync(0xffffffffu, v.sxx, o), __shfl_up_sync(0xffffffffu, v.syy, o),
                 __shfl_up_sync(0xffffffffu, v.sxy, o)};
 }
+// The carry and tree buffers hold kind K's scan values.
+template <int K>
+__device__ __forceinline__ wv_t<K>* wv_buf(void* p) { return (wv_t<K>*)p; }
 
 // Cell i of a column of c-type ct and `size` bytes as a double (integers and bool exactly up to 2^53), as wv_value<WV_MOM>
 // converts its cells (which keeps its own copy, so the moments' kernels compile as before).
@@ -1301,7 +1234,7 @@ __device__ __forceinline__ double wv_double(const char* data, int ct, int size, 
 // Scan value of position i of the scanned function (x: its second column, read by WV_CO only); `part`: i starts a partition.
 template <int K>
 __device__ __forceinline__ wv_t<K> wv_value(const WvFunc& s, const WvCol& x, int64_t i, bool part) {
-    WvAgg r = wv_identity<K>();
+    WvAgg r = Wv<K>::identity();
     r.f = part;
     bool na = s.vb && s.vb[i] == 0;
     if (K == WV_ISUM && s.code == WN_COUNT && !ctype_is_float(s.ct)) { r.c = !na; return r; }  // only NaN needs the values
@@ -1324,7 +1257,7 @@ __device__ __forceinline__ wv_t<K> wv_value(const WvFunc& s, const WvCol& x, int
 // (1, x, 0) for a valid, non-NaN cell x converted to double (integers and bool exactly up to 2^53); the identity otherwise.
 template <>
 __device__ __forceinline__ WvMom wv_value<WV_MOM>(const WvFunc& s, const WvCol&, int64_t i, bool part) {
-    WvMom r = wv_identity<WV_MOM>();
+    WvMom r = Wv<WV_MOM>::identity();
     r.f = part;
     const uint64_t raw = load_bits(s.data, s.size, i);
     const double x = s.ct == CT_FLOAT64 ? __longlong_as_double((long long)raw)
@@ -1337,44 +1270,11 @@ __device__ __forceinline__ WvMom wv_value<WV_MOM>(const WvFunc& s, const WvCol&,
 // (1, x, y, 0, 0, 0) when both cells are valid and non-NaN (pairwise deletion); the identity otherwise.
 template <>
 __device__ __forceinline__ WvCo wv_value<WV_CO>(const WvFunc& s, const WvCol& x, int64_t i, bool part) {
-    WvCo r = wv_identity<WV_CO>();
+    WvCo r = Wv<WV_CO>::identity();
     r.f = part;
     const double yv = wv_double(s.data, s.ct, s.size, i), xv = wv_double(x.data, x.ct, x.size, i);
     if (!(s.vb && s.vb[i] == 0) && !(x.vb && x.vb[i] == 0) && !isnan(xv) && !isnan(yv)) { r.c = 1; r.mx = xv; r.my = yv; }
     return r;
-}
-
-// Inclusive scan of this thread's WN_ITEMS values of a tile (warp-strided, as wn_row), seeded by `seed`.
-template <int K>
-__device__ __forceinline__ void wv_scan_tile(wv_t<K> seed, wv_t<K> (&v)[WN_ITEMS]) {
-    __shared__ wv_t<K> s_seg[WN_ITEMS * WN_WARPS];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) {
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const wv_t<K> y = wv_shfl_up(v[k], o);
-            if (lane >= o) v[k] = wv_combine<K>(y, v[k]);
-        }
-        if (lane == 31) s_seg[k * WN_WARPS + warp] = v[k];
-    }
-    __syncthreads();
-    if (warp == 0) {  // exclusive scan of the 64 (item, warp) segments in row order, seeded: 2 per lane
-        const wv_t<K> x0 = s_seg[2 * lane], x1 = s_seg[2 * lane + 1];
-        wv_t<K> inc = wv_combine<K>(x0, x1);
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const wv_t<K> y = wv_shfl_up(inc, o);
-            if (lane >= o) inc = wv_combine<K>(y, inc);
-        }
-        const wv_t<K> ex = wv_shfl_up(inc, 1);
-        const wv_t<K> base = lane > 0 ? wv_combine<K>(seed, ex) : seed;
-        s_seg[2 * lane] = base;
-        s_seg[2 * lane + 1] = wv_combine<K>(base, x0);
-    }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) v[k] = wv_combine<K>(s_seg[k * WN_WARPS + warp], v[k]);
 }
 
 // dst[i] = the low `size` bytes of bits.
@@ -1415,7 +1315,8 @@ __device__ __forceinline__ void wv_write(const WvFunc& s, int64_t i, wv_t<K> v) 
 template <>
 __device__ __forceinline__ void wv_write<WV_MOM>(const WvFunc& s, int64_t i, WvMom v) {
     const bool pop = s.code == WN_VAR_POP || s.code == WN_STD_POP, ok = v.c > (pop ? 0u : 1u);
-    double r = isfinite(v.mean) ? v.m2 / ((double)v.c - (pop ? 0.0 : 1.0)) : __longlong_as_double(0x7FF8000000000000ll);
+    // Two branches rather than c - (pop ? 0.0 : 1.0): that constant would be hoisted and held across window_frame_kernel's row loop.
+    double r = isfinite(v.mean) ? v.m2 / (pop ? (double)v.c : (double)v.c - 1.0) : __longlong_as_double(0x7FF8000000000000ll);
     if (s.code == WN_STD || s.code == WN_STD_POP) r = sqrt(r);
     ((double*)s.out)[i] = ok ? r : 0.0;
     s.out_vb[i] = ok;
@@ -1449,70 +1350,30 @@ __device__ __forceinline__ void wv_write<WV_CO>(const WvFunc& s, int64_t i, WvCo
 }
 
 template <int K, bool FINAL>
-__global__ void __launch_bounds__(WN_THREADS) window_vscan_kernel(const __grid_constant__ WvArgs a, const __grid_constant__ WvCol x) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+__global__ void __launch_bounds__(TILE_THREADS) window_vscan_kernel(const __grid_constant__ WvArgs a, const __grid_constant__ WvCol x) {
     const int64_t t = blockIdx.x;
-    wv_t<K> v[WN_ITEMS];
+    wv_t<K> v[TILE_ITEMS];
 #pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
-        v[k] = i < a.n ? wv_value<K>(a.s, x, i, a.flags[i] & WN_PART) : wv_identity<K>();
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        const int64_t i = tile_row(t, k);
+        v[k] = i < a.n ? wv_value<K>(a.s, x, i, a.flags[i] & WN_PART) : Wv<K>::identity();
     }
-    wv_scan_tile<K>(FINAL ? wv_buf<K>(a.carry)[t] : wv_identity<K>(), v);
+    tile_scan<Wv<K>>(FINAL ? wv_buf<K>(a.carry)[t] : Wv<K>::identity(), v);
     if (!FINAL) {  // padding rows hold the identity, so the tile's last slot holds its reduction
-        if (threadIdx.x == WN_THREADS - 1) wv_buf<K>(a.carry)[t] = v[WN_ITEMS - 1];
+        if (threadIdx.x == TILE_THREADS - 1) wv_buf<K>(a.carry)[t] = v[TILE_ITEMS - 1];
         return;
     }
     const uint8_t end_flag = a.s.frame == WF_RANGE ? WN_PEER : WN_PART;
 #pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        const int64_t i = tile_row(t, k);
         if (i >= a.n) break;
         if (a.s.frame == WF_ROWS || i + 1 == a.n || (a.flags[i + 1] & end_flag)) wv_write<K>(a.s, i, v[k]);
     }
 }
 
-// One block of 1024 threads; thread x scans a contiguous run of tiles (as window_tiles_kernel).
-template <int K>
-__global__ void __launch_bounds__(1024) window_vtiles_kernel(const __grid_constant__ WvArgs a, int64_t n_tiles) {
-    __shared__ wv_t<K> s_agg[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t per = (n_tiles + 1023) / 1024, t0 = threadIdx.x * per, t1 = min(n_tiles, t0 + per);
-    wv_t<K> acc = wv_identity<K>();
-    for (int64_t t = t0; t < t1; t++) acc = wv_combine<K>(acc, wv_buf<K>(a.carry)[t]);
-    wv_t<K> inc = acc;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const wv_t<K> y = wv_shfl_up(inc, o);
-        if (lane >= o) inc = wv_combine<K>(y, inc);
-    }
-    if (lane == 31) s_agg[warp] = inc;
-    __syncthreads();
-    wv_t<K> run = wv_identity<K>();
-    for (int w = 0; w < warp; w++) run = wv_combine<K>(run, s_agg[w]);
-    const wv_t<K> ex = wv_shfl_up(inc, 1);
-    if (lane > 0) run = wv_combine<K>(run, ex);
-    for (int64_t t = t0; t < t1; t++) {
-        const wv_t<K> v = wv_buf<K>(a.carry)[t];
-        wv_buf<K>(a.carry)[t] = run;
-        run = wv_combine<K>(run, v);
-    }
-}
-
-__global__ void __launch_bounds__(WN_THREADS) window_veval_kernel(const __grid_constant__ WnArgs w, const __grid_constant__ WvArgs a) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t t = blockIdx.x;
-    uint8_t f[WN_ITEMS];
-    WnAgg v[WN_ITEMS];
-    wn_scan_tile(w, t, f, v);
-    __shared__ WnAgg s_v[WN_ITEMS][WN_THREADS];  // parked as in window_eval_kernel: the item loop is not unrolled
-#pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) s_v[k][threadIdx.x] = v[k];
-#pragma unroll 1
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
-        if (i >= a.n) break;
-        const WnAgg vk = s_v[k][threadIdx.x];
+__global__ void __launch_bounds__(TILE_THREADS) window_veval_kernel(const __grid_constant__ WnArgs w, const __grid_constant__ WvArgs a) {
+    wn_for_rows(w.n, w.flags, w.tile, [&](int64_t i, const WnAgg vk) {
         const int64_t P = vk.p, pe = P + w.psize[vk.p];  // the partition is [P, pe)
         for (int fn = 0; fn < a.n_funcs; fn++) {
             const WvFunc& g = a.f[fn];
@@ -1539,14 +1400,14 @@ __global__ void __launch_bounds__(WN_THREADS) window_veval_kernel(const __grid_c
                 g.out_vb[i] = (uint8_t)g.dflt_valid;
             }
         }
-    }
+    });
 }
 
 template <int K>
 void launch_wv_scan(const WvArgs& a, const WvCol& x, int64_t n_tiles, cudaStream_t st) {
-    window_vscan_kernel<K, false><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a, x);
-    window_vtiles_kernel<K><<<1, 1024, 0, st>>>(a, n_tiles);
-    window_vscan_kernel<K, true><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a, x);
+    window_vscan_kernel<K, false><<<(unsigned)n_tiles, TILE_THREADS, 0, st>>>(a, x);
+    tile_carry_kernel<Wv<K>><<<1, 1024, 0, st>>>((wv_t<K>*)a.carry, n_tiles, nullptr);
+    window_vscan_kernel<K, true><<<(unsigned)n_tiles, TILE_THREADS, 0, st>>>(a, x);
 }
 
 // ---- bounded ROWS frames (k PRECEDING / k FOLLOWING) and NTH_VALUE ----
@@ -1584,7 +1445,7 @@ struct WfFunc {
 struct WfArgs {
     int64_t n;
     const uint8_t* flags;
-    const WnAgg* tile;              // the ranking scan's tile prefixes
+    const WnTile* tile;             // the ranking scan's tile prefixes
     const uint32_t *psize, *pend;
     void* tree;                     // wv_t<K> nodes
     int64_t off[WT_LEVELS];         // level l's first node in `tree` (l >= WT_LOW); level l holds n >> l nodes
@@ -1608,14 +1469,14 @@ __device__ __forceinline__ void wt_store(const WfArgs& a, int l, int64_t b, wv_t
     if (l >= WT_LOW && l < WT_LEVELS && b < (a.n >> l)) wv_buf<K>(a.tree)[a.off[l] + b] = v;
 }
 
-// Levels base + 1 .. base + 3 of a thread's WN_ITEMS inputs x, in registers; x[0] ends as their combine.
+// Levels base + 1 .. base + 3 of a thread's TILE_ITEMS inputs x, in registers; x[0] ends as their combine.
 template <int K>
-__device__ __forceinline__ void wt_levels3(const WfArgs& a, int base, int64_t j0, wv_t<K> (&x)[WN_ITEMS]) {
+__device__ __forceinline__ void wt_levels3(const WfArgs& a, int base, int64_t j0, wv_t<K> (&x)[TILE_ITEMS]) {
 #pragma unroll
-    for (int h = 1, m = WN_ITEMS / 2; m >= 1; h++, m >>= 1) {
+    for (int h = 1, m = TILE_ITEMS / 2; m >= 1; h++, m >>= 1) {
 #pragma unroll
         for (int k = 0; k < m; k++) {
-            x[k] = wv_combine<K>(x[2 * k], x[2 * k + 1]);
+            x[k] = Wv<K>::combine(x[2 * k], x[2 * k + 1]);
             wt_store<K>(a, base + h, (j0 >> h) + k, x[k]);
         }
     }
@@ -1623,43 +1484,43 @@ __device__ __forceinline__ void wt_levels3(const WfArgs& a, int base, int64_t j0
 // The same with constant trip counts: the loop above leaves the moments' and co-moments' larger combines partly rolled, and x in
 // local memory.
 template <int K>
-__device__ __forceinline__ void wt_levels3_unrolled(const WfArgs& a, int base, int64_t j0, wv_t<K> (&x)[WN_ITEMS]) {
+__device__ __forceinline__ void wt_levels3_unrolled(const WfArgs& a, int base, int64_t j0, wv_t<K> (&x)[TILE_ITEMS]) {
 #pragma unroll
     for (int h = 1; h <= 3; h++) {
 #pragma unroll
-        for (int k = 0; k < WN_ITEMS / 2; k++) {
-            if (k < (WN_ITEMS >> h)) {
-                x[k] = wv_combine<K>(x[2 * k], x[2 * k + 1]);
+        for (int k = 0; k < TILE_ITEMS / 2; k++) {
+            if (k < (TILE_ITEMS >> h)) {
+                x[k] = Wv<K>::combine(x[2 * k], x[2 * k + 1]);
                 wt_store<K>(a, base + h, (j0 >> h) + k, x[k]);
             }
         }
     }
 }
 template <>
-__device__ __forceinline__ void wt_levels3<WV_MOM>(const WfArgs& a, int base, int64_t j0, WvMom (&x)[WN_ITEMS]) {
+__device__ __forceinline__ void wt_levels3<WV_MOM>(const WfArgs& a, int base, int64_t j0, WvMom (&x)[TILE_ITEMS]) {
     wt_levels3_unrolled<WV_MOM>(a, base, j0, x);
 }
 template <>
-__device__ __forceinline__ void wt_levels3<WV_CO>(const WfArgs& a, int base, int64_t j0, WvCo (&x)[WN_ITEMS]) {
+__device__ __forceinline__ void wt_levels3<WV_CO>(const WfArgs& a, int base, int64_t j0, WvCo (&x)[TILE_ITEMS]) {
     wt_levels3_unrolled<WV_CO>(a, base, j0, x);
 }
 
 template <int K>
-__global__ void __launch_bounds__(WN_THREADS) window_tree_kernel(const __grid_constant__ WfArgs a, int base, const __grid_constant__ WvCol x2) {
-    __shared__ wv_t<K> s_node[WN_THREADS];
-    const int64_t n_in = a.n >> base, j0 = (int64_t)blockIdx.x * WN_TILE + threadIdx.x * WN_ITEMS;
-    wv_t<K> x[WN_ITEMS];
+__global__ void __launch_bounds__(TILE_THREADS) window_tree_kernel(const __grid_constant__ WfArgs a, int base, const __grid_constant__ WvCol x2) {
+    __shared__ wv_t<K> s_node[TILE_THREADS];
+    const int64_t n_in = a.n >> base, j0 = (int64_t)blockIdx.x * TILE_ROWS + threadIdx.x * TILE_ITEMS;
+    wv_t<K> x[TILE_ITEMS];
 #pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) {
+    for (int k = 0; k < TILE_ITEMS; k++) {
         const int64_t j = j0 + k;
-        x[k] = j >= n_in ? wv_identity<K>() : base == 0 ? wv_value<K>(a.s.g, x2, j, false) : wv_buf<K>(a.tree)[a.off[base] + j];
+        x[k] = j >= n_in ? Wv<K>::identity() : base == 0 ? wv_value<K>(a.s.g, x2, j, false) : wv_buf<K>(a.tree)[a.off[base] + j];
     }
     wt_levels3<K>(a, base, j0, x);  // levels base + 1 .. base + 3 in registers
     s_node[threadIdx.x] = x[0];
     __syncthreads();
-    for (int h = 4, m = WN_THREADS / 2; m >= 1; h++, m >>= 1) {  // levels base + 4 .. base + 11 in shared memory
+    for (int h = 4, m = TILE_THREADS / 2; m >= 1; h++, m >>= 1) {  // levels base + 4 .. base + 11 in shared memory
         wv_t<K> y = x[0];
-        if (threadIdx.x < m) y = wv_combine<K>(s_node[2 * threadIdx.x], s_node[2 * threadIdx.x + 1]);
+        if (threadIdx.x < m) y = Wv<K>::combine(s_node[2 * threadIdx.x], s_node[2 * threadIdx.x + 1]);
         __syncthreads();
         if (threadIdx.x < m) {
             s_node[threadIdx.x] = y;
@@ -1672,17 +1533,17 @@ __global__ void __launch_bounds__(WN_THREADS) window_tree_kernel(const __grid_co
 // The aggregate of the scanned function over [lo, hi]: edge leaves from the sorted column, aligned blocks from the tree.
 template <int K>
 __device__ __forceinline__ wv_t<K> wt_query(const WfArgs& a, const WvCol& x, int64_t lo, int64_t hi) {
-    wv_t<K> acc = wv_identity<K>();
+    wv_t<K> acc = Wv<K>::identity();
     const int64_t r = hi + 1, a8 = min(r, (lo + 7) & ~(int64_t)7);
     int64_t j = lo;
-    for (; j < a8; j++) acc = wv_combine<K>(acc, wv_value<K>(a.s.g, x, j, false));
+    for (; j < a8; j++) acc = Wv<K>::combine(acc, wv_value<K>(a.s.g, x, j, false));
     const int64_t b8 = max(j, r & ~(int64_t)7);
     while (j < b8) {  // j and b8 are multiples of 8, so l >= 3
         const int l = min(j == 0 ? 62 : __ffsll(j) - 1, 63 - __clzll(b8 - j));
-        acc = wv_combine<K>(acc, wv_buf<K>(a.tree)[a.off[l] + (j >> l)]);
+        acc = Wv<K>::combine(acc, wv_buf<K>(a.tree)[a.off[l] + (j >> l)]);
         j += (int64_t)1 << l;
     }
-    for (; j < r; j++) acc = wv_combine<K>(acc, wv_value<K>(a.s.g, x, j, false));
+    for (; j < r; j++) acc = Wv<K>::combine(acc, wv_value<K>(a.s.g, x, j, false));
     return acc;
 }
 
@@ -1708,25 +1569,11 @@ __device__ __forceinline__ void wf_eval_row(const WfArgs& a, const WvCol& x, int
 }
 
 template <int K>
-__global__ void __launch_bounds__(WN_THREADS) window_frame_kernel(const __grid_constant__ WfArgs a, const __grid_constant__ WvCol x) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t t = blockIdx.x;
-    WnArgs w;  // wn_scan_tile reads n, flags and the tile prefixes only
-    w.n = a.n; w.flags = const_cast<uint8_t*>(a.flags); w.tile = const_cast<WnAgg*>(a.tile);
-    uint8_t f[WN_ITEMS];
-    WnAgg v[WN_ITEMS];
-    wn_scan_tile(w, t, f, v);
-    __shared__ WnAgg s_v[WN_ITEMS][WN_THREADS];  // parked as in window_eval_kernel: the item loop is not unrolled
-#pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) s_v[k][threadIdx.x] = v[k];
-#pragma unroll 1
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
-        if (i >= a.n) break;
-        const WnAgg vk = s_v[k][threadIdx.x];
+__global__ void __launch_bounds__(TILE_THREADS) window_frame_kernel(const __grid_constant__ WfArgs a, const __grid_constant__ WvCol x) {
+    wn_for_rows(a.n, a.flags, a.tile, [&](int64_t i, const WnAgg vk) {
         const int64_t P = vk.p, pe = P + a.psize[vk.p], qe = a.pend[vk.q];
         wf_eval_row<K>(a, x, i, [&](const WfFunc& g, int64_t& lo, int64_t& hi) { wf_bounds(g, i, P, pe, qe, lo, hi); });
-    }
+    });
 }
 
 // The same over frame-5 functions, whose bounds window_range_bounds_kernel wrote: no scan of the flags is needed, so one thread
@@ -1734,7 +1581,7 @@ __global__ void __launch_bounds__(WN_THREADS) window_frame_kernel(const __grid_c
 // accumulator and leaf spill at 48, so WV_CO takes up to 80 (it uses 68).
 template <int K>
 __global__ void __maxnreg__(K == WV_CO ? 80 : 48) window_range_frame_kernel(const __grid_constant__ WfArgs a, const __grid_constant__ WvCol x) {
-    const int64_t i = (int64_t)blockIdx.x * WN_THREADS + threadIdx.x;
+    const int64_t i = (int64_t)blockIdx.x * TILE_THREADS + threadIdx.x;
     if (i >= a.n) return;
     wf_eval_row<K>(a, x, i, [i](const WfFunc& g, int64_t& lo, int64_t& hi) {
         const int2 b = __ldg(g.range + i);
@@ -1747,9 +1594,9 @@ __global__ void __maxnreg__(K == WV_CO ? 80 : 48) window_range_frame_kernel(cons
 template <int K>
 void launch_wf_tree(const WfArgs& a, const WvCol& x, int64_t n_tiles, cudaStream_t st) {
     for (int base = 0; (a.n >> max(base + 1, WT_LOW)) > 0; base += 11)
-        window_tree_kernel<K><<<(unsigned)(((a.n >> base) + WN_TILE - 1) / WN_TILE), WN_THREADS, 0, st>>>(a, base, x);
-    if (a.s.g.frame == WF_RANGE_BETWEEN) window_range_frame_kernel<K><<<(unsigned)(n_tiles * WN_ITEMS), WN_THREADS, 0, st>>>(a, x);
-    else window_frame_kernel<K><<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a, x);
+        window_tree_kernel<K><<<(unsigned)(((a.n >> base) + TILE_ROWS - 1) / TILE_ROWS), TILE_THREADS, 0, st>>>(a, base, x);
+    if (a.s.g.frame == WF_RANGE_BETWEEN) window_range_frame_kernel<K><<<(unsigned)(n_tiles * TILE_ITEMS), TILE_THREADS, 0, st>>>(a, x);
+    else window_frame_kernel<K><<<(unsigned)n_tiles, TILE_THREADS, 0, st>>>(a, x);
 }
 
 // ---- RANGE frames with value offsets (RANGE BETWEEN x PRECEDING AND y FOLLOWING): frame 5 ----
@@ -1772,7 +1619,7 @@ enum { WR_UNBOUNDED_PRECEDING = 0, WR_PRECEDING = 1, WR_CURRENT_ROW = 2, WR_FOLL
 struct WrArgs {
     int64_t n;
     const uint8_t* flags;
-    const WnAgg* tile;             // the ranking scan's tile prefixes
+    const WnTile* tile;            // the ranking scan's tile prefixes
     const uint32_t *psize, *pend;
     SortKey key;                   // the ORDER BY key (read for offset bounds only)
     const char* data;              // its sorted column and validity bytes (nullptr: numpy)
@@ -1871,24 +1718,10 @@ __device__ __forceinline__ int64_t wr_bound(const WrArgs& a, int kind, uint64_t 
     return nj ? P - 1 : j - 1;
 }
 
-__global__ void __launch_bounds__(WN_THREADS) window_range_bounds_kernel(const __grid_constant__ WrArgs a) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t t = blockIdx.x;
-    WnArgs w;  // wn_scan_tile reads n, flags and the tile prefixes only
-    w.n = a.n; w.flags = const_cast<uint8_t*>(a.flags); w.tile = const_cast<WnAgg*>(a.tile);
-    uint8_t f[WN_ITEMS];
-    WnAgg v[WN_ITEMS];
-    wn_scan_tile(w, t, f, v);
-    __shared__ WnAgg s_v[WN_ITEMS][WN_THREADS];  // parked as in window_eval_kernel: the item loop is not unrolled
-#pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) s_v[k][threadIdx.x] = v[k];
+__global__ void __launch_bounds__(TILE_THREADS) window_range_bounds_kernel(const __grid_constant__ WrArgs a) {
     const bool offsets = a.start_kind == WR_PRECEDING || a.start_kind == WR_FOLLOWING || a.end_kind == WR_PRECEDING ||
                          a.end_kind == WR_FOLLOWING;
-#pragma unroll 1
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
-        if (i >= a.n) break;
-        const WnAgg vk = s_v[k][threadIdx.x];
+    wn_for_rows(a.n, a.flags, a.tile, [&](int64_t i, const WnAgg vk) {
         const int64_t P = vk.p, pe = P + a.psize[vk.p], Q = vk.q, qe = a.pend[vk.q];
         bool na = false;
         const uint64_t wi = offsets ? wr_word(a, i, na) : 0;
@@ -1897,7 +1730,7 @@ __global__ void __launch_bounds__(WN_THREADS) window_range_bounds_kernel(const _
         // A non-empty frame lies in [0, n) with n <= 2^31, so both bounds fit int32.  An empty one may carry lo = pe = 2^31 (a
         // state of exactly 2^31 rows), so every empty frame is stored as (0, -1): its consumers read nothing for lo > hi.
         a.out[i] = lo <= hi ? make_int2((int)lo, (int)hi) : make_int2(0, -1);
-    }
+    });
 }
 
 // ---- IGNORE NULLS: FIRST_VALUE / LAST_VALUE / NTH_VALUE over every frame, LAG / LEAD ----
@@ -1905,8 +1738,8 @@ __global__ void __launch_bounds__(WN_THREADS) window_range_bounds_kernel(const _
 // A cell is null when count(x) does not count it: its validity byte is 0 or it is a float NaN (RESPECT NULLS first_value keeps
 // a NaN as a valid cell; IGNORE NULLS skips it, as pandas' ffill / bfill do).  With v[j] = 1 at the non-null sorted rows, one
 // value column gets c[0..n], the exclusive prefix count of v (c[n] = m, the non-null rows), and pos[0..m), their positions:
-//   window_nulls_count_kernel    per WN_TILE-row tile: its non-null count.
-//   window_nulls_tiles_kernel    one block: the exclusive scan of the tile counts, and c[n].
+//   window_nulls_count_kernel    per TILE_ROWS-row tile: its non-null count.
+//   tile_carry_kernel            one block: the exclusive scan of the tile counts, and c[n].
 //   window_nulls_compact_kernel  per tile again: c[i] from the tile prefix and a ballot per 32 rows; pos[c[i]] = i at non-null i.
 // Then each function is index arithmetic on (c, pos) over the frame [lo, hi] or the partition [P, pe) of its RESPECT NULLS form:
 //   first_value  j = c[lo], valid iff lo <= hi and j < c[hi + 1]      nth_value(n)  j = c[lo] + n - 1, valid iff j < c[hi + 1]
@@ -1921,7 +1754,7 @@ __global__ void __launch_bounds__(WN_THREADS) window_range_bounds_kernel(const _
 struct WnlArgs {
     int64_t n;
     const uint8_t* flags;
-    const WnAgg* tile;              // the ranking scan's tile prefixes
+    const WnTile* tile;             // the ranking scan's tile prefixes
     const uint32_t *psize, *pend;
     WvCol x;                        // the value column of every function below
     uint32_t* tcount;               // per tile: its non-null count, then its exclusive prefix
@@ -1937,82 +1770,36 @@ __device__ __forceinline__ bool wnl_null(const WvCol& x, int64_t i) {
     return false;
 }
 
-__global__ void __launch_bounds__(WN_THREADS) window_nulls_count_kernel(const __grid_constant__ WnlArgs a) {
-    __shared__ uint32_t s_cnt[WN_WARPS];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+__global__ void __launch_bounds__(TILE_THREADS) window_nulls_count_kernel(const __grid_constant__ WnlArgs a) {
     const int64_t t = blockIdx.x;
     uint32_t cnt = 0;
 #pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        const int64_t i = tile_row(t, k);
         cnt += i < a.n && !wnl_null(a.x, i);
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    if (lane == 0) s_cnt[warp] = cnt;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        for (int w = 1; w < WN_WARPS; w++) cnt += s_cnt[w];
-        a.tcount[t] = cnt;
-    }
+    cnt = block_reduce<SumOf<uint32_t>>(cnt);
+    if (threadIdx.x == 0) a.tcount[t] = cnt;
 }
 
-// One block of 1024 threads; thread x scans a contiguous run of tiles (as window_tiles_kernel).
-__global__ void __launch_bounds__(1024) window_nulls_tiles_kernel(const __grid_constant__ WnlArgs a, int64_t n_tiles) {
-    __shared__ uint32_t s_sum[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t per = (n_tiles + 1023) / 1024, t0 = threadIdx.x * per, t1 = min(n_tiles, t0 + per);
-    uint32_t acc = 0;
-    for (int64_t t = t0; t < t1; t++) acc += a.tcount[t];
-    uint32_t inc = acc;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += y;
-    }
-    if (lane == 31) s_sum[warp] = inc;
-    __syncthreads();
-    uint32_t run = inc - acc;
-    for (int w = 0; w < warp; w++) run += s_sum[w];
-    for (int64_t t = t0; t < t1; t++) {
-        const uint32_t v = a.tcount[t];
-        a.tcount[t] = run;
-        run += v;
-    }
-    if (threadIdx.x == 1023) a.c[a.n] = run;
-}
-
-__global__ void __launch_bounds__(WN_THREADS) window_nulls_compact_kernel(const __grid_constant__ WnlArgs a) {
-    __shared__ uint32_t s_seg[WN_ITEMS * WN_WARPS];  // per (item, warp) segment of 32 rows: its count, then its exclusive prefix
+__global__ void __launch_bounds__(TILE_THREADS) window_nulls_compact_kernel(const __grid_constant__ WnlArgs a) {
+    __shared__ uint32_t s_seg[TILE_ITEMS * TILE_WARPS];  // per (item, warp) segment of 32 rows: its count, then its exclusive prefix
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t t = blockIdx.x;
-    uint32_t ball[WN_ITEMS];
+    uint32_t ball[TILE_ITEMS];
 #pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        const int64_t i = tile_row(t, k);
         ball[k] = __ballot_sync(0xffffffffu, i < a.n && !wnl_null(a.x, i));
-        if (lane == 0) s_seg[k * WN_WARPS + warp] = __popc(ball[k]);
+        if (lane == 0) s_seg[k * TILE_WARPS + warp] = __popc(ball[k]);
     }
-    __syncthreads();
-    if (warp == 0) {  // exclusive scan of the 64 segments in row order, seeded by the tile prefix: 2 per lane
-        const uint32_t x0 = s_seg[2 * lane], x1 = s_seg[2 * lane + 1];
-        uint32_t inc = x0 + x1;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += y;
-        }
-        const uint32_t base = a.tcount[t] + inc - x0 - x1;
-        s_seg[2 * lane] = base;
-        s_seg[2 * lane + 1] = base + x0;
-    }
-    __syncthreads();
+    tile_segment_scan<SumOf<uint32_t>>(s_seg, a.tcount[t]);
     const uint32_t below = (1u << lane) - 1u;
 #pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
+    for (int k = 0; k < TILE_ITEMS; k++) {
+        const int64_t i = tile_row(t, k);
         if (i >= a.n) break;
-        const uint32_t ci = s_seg[k * WN_WARPS + warp] + __popc(ball[k] & below);
+        const uint32_t ci = s_seg[k * TILE_WARPS + warp] + __popc(ball[k] & below);
         a.c[i] = ci;
         if ((ball[k] >> lane) & 1u) a.pos[ci] = (uint32_t)i;
     }
@@ -2054,29 +1841,15 @@ __device__ __forceinline__ void wnl_eval_row(const WnlArgs& a, int64_t i, int64_
     }
 }
 
-__global__ void __launch_bounds__(WN_THREADS) window_nulls_eval_kernel(const __grid_constant__ WnlArgs a) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t t = blockIdx.x;
-    WnArgs w;  // wn_scan_tile reads n, flags and the tile prefixes only
-    w.n = a.n; w.flags = const_cast<uint8_t*>(a.flags); w.tile = const_cast<WnAgg*>(a.tile);
-    uint8_t f[WN_ITEMS];
-    WnAgg v[WN_ITEMS];
-    wn_scan_tile(w, t, f, v);
-    __shared__ WnAgg s_v[WN_ITEMS][WN_THREADS];  // parked as in window_eval_kernel: the item loop is not unrolled
-#pragma unroll
-    for (int k = 0; k < WN_ITEMS; k++) s_v[k][threadIdx.x] = v[k];
-#pragma unroll 1
-    for (int k = 0; k < WN_ITEMS; k++) {
-        const int64_t i = wn_row(t, k, warp, lane);
-        if (i >= a.n) break;
-        const WnAgg vk = s_v[k][threadIdx.x];
+__global__ void __launch_bounds__(TILE_THREADS) window_nulls_eval_kernel(const __grid_constant__ WnlArgs a) {
+    wn_for_rows(a.n, a.flags, a.tile, [&](int64_t i, const WnAgg vk) {
         const int64_t P = vk.p, pe = P + a.psize[vk.p], qe = a.pend[vk.q];
         wnl_eval_row(a, i, P, pe, [&](const WfFunc& g, int64_t& lo, int64_t& hi) { wf_bounds(g, i, P, pe, qe, lo, hi); });
-    }
+    });
 }
 
-__global__ void __launch_bounds__(WN_THREADS) window_nulls_range_kernel(const __grid_constant__ WnlArgs a) {
-    const int64_t i = (int64_t)blockIdx.x * WN_THREADS + threadIdx.x;
+__global__ void __launch_bounds__(TILE_THREADS) window_nulls_range_kernel(const __grid_constant__ WnlArgs a) {
+    const int64_t i = (int64_t)blockIdx.x * TILE_THREADS + threadIdx.x;
     if (i >= a.n) return;
     wnl_eval_row(a, i, 0, 0, [i](const WfFunc& g, int64_t& lo, int64_t& hi) {
         const int2 b = __ldg(g.range + i);
@@ -2088,11 +1861,11 @@ __global__ void __launch_bounds__(WN_THREADS) window_nulls_range_kernel(const __
 // (c, pos) of value column x, then `eval` over a.f (frames 1..4, lag and lead) or `range` (frame 5).
 static void launch_wnl(WnlArgs& a, const WvCol& x, int64_t n_tiles, bool range, cudaStream_t st) {
     a.x = x;
-    window_nulls_count_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
-    window_nulls_tiles_kernel<<<1, 1024, 0, st>>>(a, n_tiles);
-    window_nulls_compact_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
-    if (range) window_nulls_range_kernel<<<(unsigned)(n_tiles * WN_ITEMS), WN_THREADS, 0, st>>>(a);
-    else window_nulls_eval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, st>>>(a);
+    window_nulls_count_kernel<<<(unsigned)n_tiles, TILE_THREADS, 0, st>>>(a);
+    tile_carry_kernel<SumOf<uint32_t>><<<1, 1024, 0, st>>>(a.tcount, n_tiles, a.c + a.n);
+    window_nulls_compact_kernel<<<(unsigned)n_tiles, TILE_THREADS, 0, st>>>(a);
+    if (range) window_nulls_range_kernel<<<(unsigned)(n_tiles * TILE_ITEMS), TILE_THREADS, 0, st>>>(a);
+    else window_nulls_eval_kernel<<<(unsigned)n_tiles, TILE_THREADS, 0, st>>>(a);
 }
 
 // Calls launch(std::integral_constant<int, K>) with aggregate g's scan kind K, which its scan and its frame tree share.
@@ -2272,19 +2045,18 @@ struct WindowState : FullSortState {
             if (!scanned || d.frame != WF_ROWS) { va.f[va.n_funcs++] = g; eval = true; }
         }
         if (n == 0) return;
-        const int64_t n_tiles = (n + WN_TILE - 1) / WN_TILE;
-        DevBuf flags, tiles, tile_parts, totals, ends;
+        const int64_t n_tiles = (n + TILE_ROWS - 1) / TILE_ROWS;
+        DevBuf flags, tiles, total, ends;
         flags.alloc((size_t)n);
-        tiles.alloc((size_t)n_tiles * sizeof(WnAgg));
-        tile_parts.alloc((size_t)n_tiles * 4);
-        totals.alloc(8);
+        tiles.alloc((size_t)n_tiles * sizeof(WnTile));
+        total.alloc(sizeof(WnTile));
         ends.alloc((size_t)n * 12);
-        a.flags = flags.as<uint8_t>(); a.tile = tiles.as<WnAgg>(); a.tile_parts = tile_parts.as<uint32_t>(); a.totals = totals.as<uint32_t>();
+        a.flags = flags.as<uint8_t>(); a.tile = tiles.as<WnTile>(); a.total = total.as<WnTile>();
         a.psize = ends.as<uint32_t>(); a.pend = a.psize + n; a.pdense = a.pend + n;
-        window_bounds_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
-        window_tiles_kernel<<<1, 1024, 0, stream>>>(a, n_tiles);
-        window_ends_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
-        if (a.n_funcs > 0) window_eval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a);
+        window_bounds_kernel<<<(unsigned)n_tiles, TILE_THREADS, 0, stream>>>(a);
+        tile_carry_kernel<WnTile><<<1, 1024, 0, stream>>>(a.tile, n_tiles, a.total);
+        window_ends_kernel<<<(unsigned)n_tiles, TILE_THREADS, 0, stream>>>(a);
+        if (a.n_funcs > 0) window_eval_kernel<<<(unsigned)n_tiles, TILE_THREADS, 0, stream>>>(a);
         B200_CUDA(cudaGetLastError());
         const auto moments = [](int code) { return code >= WN_VAR && code <= WN_STD_POP; };
         const auto bivariate = [](int code) { return code >= WN_COVAR_SAMP; };
@@ -2303,7 +2075,7 @@ struct WindowState : FullSortState {
             const WvCol x = bivariate(g.code) ? col2(g) : WvCol{};
             with_wv_kind(g, [&](auto k) { launch_wv_scan<decltype(k)::value>(va, x, n_tiles, stream); });
         }
-        if (eval) window_veval_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(a, va);
+        if (eval) window_veval_kernel<<<(unsigned)n_tiles, TILE_THREADS, 0, stream>>>(a, va);
         B200_CUDA(cudaGetLastError());
         // IGNORE NULLS: one (c, pos) buffer of 8 B per row (plus a word per tile), rebuilt for each value column.  It is built once
         // per distinct column of the frame 1..4 / lag / lead functions, then once per distinct (frame 5, column) in the frame
@@ -2348,7 +2120,7 @@ struct WindowState : FullSortState {
                 with_wv_kind(h.g, [&](auto k) { launch_wf_tree<decltype(k)::value>(fa, x, n_tiles, stream); });
             };
             for (const WfFunc& h : trees) launch_tree(h);
-            if (fa.n_funcs > 0) window_frame_kernel<WV_GATHER><<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(fa, WvCol{});
+            if (fa.n_funcs > 0) window_frame_kernel<WV_GATHER><<<(unsigned)n_tiles, TILE_THREADS, 0, stream>>>(fa, WvCol{});
             B200_CUDA(cudaGetLastError());
             // frame 5: one 8 B/row bounds buffer, reused frame by frame (its bounds, then its trees, then its gathers)
             if (!ranged.empty()) rb.alloc((size_t)n * sizeof(int2));
@@ -2356,21 +2128,21 @@ struct WindowState : FullSortState {
             WrArgs ra{n, a.flags, a.tile, a.psize, a.pend, sc.key[ok], out_data[ok], out_vb[ok], 0, 0, 0, 0, rb.as<int2>()};
             for (RangeFrame& rf : ranged) {
                 ra.start_kind = rf.r.start_kind; ra.end_kind = rf.r.end_kind; ra.start_bits = rf.r.start_bits; ra.end_bits = rf.r.end_bits;
-                window_range_bounds_kernel<<<(unsigned)n_tiles, WN_THREADS, 0, stream>>>(ra);
+                window_range_bounds_kernel<<<(unsigned)n_tiles, TILE_THREADS, 0, stream>>>(ra);
                 for (WfFunc& h : rf.trees) { h.range = ra.out; launch_tree(h); }
                 fa.n_funcs = 0;
                 for (WfFunc& h : rf.gathers) { h.range = ra.out; fa.f[fa.n_funcs++] = h; }
-                if (fa.n_funcs > 0) window_range_frame_kernel<WV_GATHER><<<(unsigned)(n_tiles * WN_ITEMS), WN_THREADS, 0, stream>>>(fa, WvCol{});
+                if (fa.n_funcs > 0) window_range_frame_kernel<WV_GATHER><<<(unsigned)(n_tiles * TILE_ITEMS), TILE_THREADS, 0, stream>>>(fa, WvCol{});
                 B200_CUDA(cudaGetLastError());
                 for (WfFunc& h : rf.nulls) h.range = ra.out;
                 launch_nulls(rf.nulls, true);
             }
         }
-        auto* h = (uint32_t*)pinned_acquire(8);
-        B200_CUDA(cudaMemcpyAsync(h, totals.p, 8, cudaMemcpyDeviceToHost, stream));
+        auto* h = (WnTile*)pinned_acquire(sizeof(WnTile));
+        B200_CUDA(cudaMemcpyAsync(h, total.p, sizeof(WnTile), cudaMemcpyDeviceToHost, stream));
         B200_CUDA(cudaStreamSynchronize(stream));
-        n_partitions = h[0];
-        pinned_release(h, 8);
+        n_partitions = h->parts;
+        pinned_release(h, sizeof(WnTile));
     }
 
     int64_t metric(int which) const override { return which == 9 ? n_partitions : FullSortState::metric(which); }

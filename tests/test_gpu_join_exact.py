@@ -735,8 +735,8 @@ def test_fast_probe_past_one_grid_on_slot16(gpu_lib):
 
 @gpu
 def test_general_probe_and_build_outer_tail_past_2_21_scan_elements(gpu_lib):
-    """The single-CTA offsets_carry_kernel gives each thread more than one tile only past 2^21 elements: a general-path probe batch of
-    more than 2^21 rows, and a build-outer tail over more than 2^21 build rows."""
+    """The offsets scan's single-CTA tile_carry_kernel gives each thread more than one tile only past 2^21 elements: a general-path
+    probe batch of more than 2^21 rows, and a build-outer tail over more than 2^21 build rows."""
     n_probe = (1 << 21) + 5 + 1000
     n_build = (1 << 21) + 3
     assert (n_probe - 1000 + 1 + 2047) // 2048 > 1024 and (n_build + 1 + 2047) // 2048 > 1024
