@@ -166,10 +166,13 @@ __host__ __device__ __forceinline__ int hash_to_rank_u32(uint32_t h, int n_pes) 
 // Table-slot hash: the same xxh3 value (one hash per row); ranks use the low 32 bits, slots the high 32
 // bits, so the two are independent (a rank's keys all share low32 % P).
 __device__ __forceinline__ uint64_t key_hash(int64_t key) { return xxh3_64_short((uint64_t)key, 8, SEED_HASH_PARTITION); }
-// Owner-rank hash of a valid table key: the hash shuffle_table gives its rows (hash_key_column).  A float key's encoding
-// (canon_float_key) goes through _Py_HashDouble of its value first; NaN hashes as 0, as a NaN row does there.
-__device__ __forceinline__ uint32_t owner_key_hash(int64_t key, bool is_float) {
-    return (uint32_t)(is_float ? xxh3_64_short((uint64_t)py_hash_double(canon_float_decode(key)), 8, SEED_HASH_PARTITION) : key_hash(key));
+// Owner-rank hash of a valid table key of input c-type ct: the hash shuffle_table gives its rows (hash_key_column).  A float key's
+// encoding (canon_float_key) goes through _Py_HashDouble of its value first; NaN hashes as 0, as a NaN row does there.  An integer,
+// bool or date key narrower than 8 bytes hashes the 4 low bytes of its widened value, as its column's raw bytes hash there.
+__device__ __forceinline__ uint32_t owner_key_hash(int64_t key, int ct) {
+    if (ct == CT_FLOAT64 || ct == CT_FLOAT32) return (uint32_t)xxh3_64_short((uint64_t)py_hash_double(canon_float_decode(key)), 8, SEED_HASH_PARTITION);
+    if (ctype_size(ct) == 8) return (uint32_t)key_hash(key);
+    return (uint32_t)xxh3_64_short((uint64_t)(uint32_t)key, 4, SEED_HASH_PARTITION);
 }
 
 __device__ __forceinline__ int64_t load_int_as_i64(const void* __restrict__ p, int ct, int64_t i) {

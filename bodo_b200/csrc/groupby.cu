@@ -550,11 +550,11 @@ __global__ void rehash_kernel(const __grid_constant__ RehashArgs a) {
 // ---- finalize: compact occupied slots, then evaluate output columns ----
 // n_pes > 1: only the groups this rank OWNS (hash_to_rank(key) == rank) are output — after the exchange the table still
 // holds the partial aggregates of groups that were sent to their owners (they are never touched again: received rows only
-// carry keys this rank owns).  key_float: the key is a float column (canon_float_key), so the marker group is the NaN group
+// carry keys this rank owns).  key_ctype: the key's input type; a float key (canon_float_key) has the NaN group in the marker slot
 // and dropna drops it.
 __global__ void compact_slots_kernel(const long long* __restrict__ tkeys, uint64_t cap, const long long* counters,
-                                     long long* cursor, uint64_t* slot_of_out, int n_pes, int rank, bool key_float, bool dropna) {
-    const bool na_present = counters[CTR_NA] != 0, empty_present = counters[CTR_MARKER] != 0 && !(key_float && dropna);
+                                     long long* cursor, uint64_t* slot_of_out, int n_pes, int rank, int key_ctype, bool dropna) {
+    const bool na_present = counters[CTR_NA] != 0, empty_present = counters[CTR_MARKER] != 0 && !(ctype_is_float(key_ctype) && dropna);
     const uint32_t na_hash = (uint32_t)xxh3_64_short(1ull, 8, SEED_HASH_PARTITION);  // hash_na_val (_array_hash.cpp:22-29)
     uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
     for (uint64_t s0 = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s0 < ((cap + 2 + 31) & ~31ull); s0 += stride) {
@@ -563,7 +563,7 @@ __global__ void compact_slots_kernel(const long long* __restrict__ tkeys, uint64
         else if (s0 == cap) occ = na_present;
         else if (s0 == cap + 1) occ = empty_present;
         if (occ && n_pes > 1) {
-            const uint32_t h = s0 == cap ? na_hash : owner_key_hash(s0 < cap ? tkeys[s0] : EMPTY_KEY, key_float);
+            const uint32_t h = s0 == cap ? na_hash : owner_key_hash(s0 < cap ? tkeys[s0] : EMPTY_KEY, key_ctype);
             occ = hash_to_rank_u32(h, n_pes) == rank;
         }
         unsigned m = __ballot_sync(0xffffffffu, occ);
@@ -886,7 +886,7 @@ __device__ __forceinline__ uint32_t mk_ref_hash(const long long* keys, unsigned 
     uint32_t h = 0;
     for (int j = 0; j < nk; j++) {
         const uint32_t hj = !((mask >> j) & 1u) ? na_hash
-                           : ctype_is_float(ctypes[j]) ? owner_key_hash(keys[j], true)
+                           : ctype_is_float(ctypes[j]) ? owner_key_hash(keys[j], ctypes[j])
                            : ctype_size(ctypes[j]) == 8 ? (uint32_t)xxh3_64_short((uint64_t)keys[j], 8, SEED_HASH_PARTITION)
                                                         : (uint32_t)xxh3_64_short((uint64_t)(uint32_t)keys[j], 4, SEED_HASH_PARTITION);
         h = j == 0 ? hj : hash_combine_boost(h, hj);
@@ -894,7 +894,7 @@ __device__ __forceinline__ uint32_t mk_ref_hash(const long long* keys, unsigned 
     return h;
 }
 __device__ __forceinline__ uint32_t mk_owner_hash(const MkOwner& ow, const long long* keys, unsigned int mask) {
-    if (ow.own_nk == 1) return (mask & 1u) ? owner_key_hash(keys[0], ctype_is_float(ow.key_ctype[0])) : (uint32_t)xxh3_64_short(1ull, 8, SEED_HASH_PARTITION);
+    if (ow.own_nk == 1) return (mask & 1u) ? owner_key_hash(keys[0], ow.key_ctype[0]) : (uint32_t)xxh3_64_short(1ull, 8, SEED_HASH_PARTITION);
     return mk_ref_hash(keys, mask, ow.nk, ow.key_ctype);
 }
 // nunique: one thread per distinct (key, value) pair of the nested state; pairs whose value is NA do not count, nor (float
@@ -970,7 +970,7 @@ struct SlotTable {
     uint64_t cap;
     long long* counters;
     long long group_limit;
-    bool key_float;  // owner_key_hash of a float key
+    int key_ctype;  // the key's input c-type (owner_key_hash)
     struct Key { long long k; bool valid; };
     __host__ __device__ uint64_t n_slots() const { return cap + 2; }
     __device__ int key_words() const { return 2; }
@@ -982,7 +982,7 @@ struct SlotTable {
         return s == cap + 1 && counters[CTR_MARKER] != 0;
     }
     __device__ uint32_t owner_hash(const Key& key) const {
-        return key.valid ? owner_key_hash(key.k, key_float) : (uint32_t)xxh3_64_short(1ull, 8, SEED_HASH_PARTITION);  // hash_na_val
+        return key.valid ? owner_key_hash(key.k, key_ctype) : (uint32_t)xxh3_64_short(1ull, 8, SEED_HASH_PARTITION);  // hash_na_val
     }
     __device__ void store(const Key& key, unsigned long long* o) const { o[0] = (unsigned long long)key.k; o[1] = key.valid ? 1ull : 0ull; }
     __device__ uint64_t insert(const unsigned long long* r) const {
@@ -3687,7 +3687,7 @@ class GroupbyState {
         else
             compact_slots_kernel<<<grid_for((int64_t)cap + 2), 256, 0, stream>>>(d_keys.as<long long>(), cap, d_counters.as<long long>(),
                                                                                       d_counters.as<long long>() + CTR_OUT, d_slot_of_out.as<uint64_t>(),
-                                                                                      n_pes, rank, float_key(0), dropna);
+                                                                                      n_pes, rank, in_types[0], dropna);
         launches++;
         B200_CUDA(cudaGetLastError());
         n_out = -1;  // known on the device (counters[CTR_OUT]); the host learns it with the next counter read-back
@@ -3799,7 +3799,7 @@ class GroupbyState {
     SlotTable slot_table() {
         SlotTable t{};
         t.tkeys = d_keys.as<long long>(); t.cap = cap; t.counters = d_counters.as<long long>(); t.group_limit = (long long)(cap / 2);
-        t.key_float = float_key(0);
+        t.key_ctype = in_types[0];
         return t;
     }
     TagTable tag_table() {

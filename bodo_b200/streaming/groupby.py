@@ -49,7 +49,7 @@ import numbers
 
 from .. import _lib
 from .._lib import ffi
-from ..table import CTable, Table, table_from_ctable
+from ..table import CTable, Table, np_dtype_of, table_from_ctable
 
 # names must match supported_agg_funcs positions / Bodo_FTypes (groupby/_groupby_ftypes.h:17-110).  28..34 continue the enum after
 # skew in the reference's order; they are recalled, not read from a reference checkout (17 and 26 are fixed by their neighbours).
@@ -165,6 +165,8 @@ class GroupbyState:
 
             n_pes, rank = dist.get_world_size(self.process_group), dist.get_rank(self.process_group)
         self.n_pes, self.rank = n_pes, rank
+        self.stays_partial = "first" in self.fnames or "last" in self.fnames or any(
+            np_dtype_of(c.c_type).itemsize < 4 for c in cols[:len(self.key_inds)])
         h = L.b200_groupby_state_init(self.operator_id, c_types, a_types, len(cols), ftypes, offs, fcols,
                                       len(self.fnames), len(self.key_inds), self.output_batch_size,
                                       int(self.parallel and n_pes > 1), int(self.dropna), self.device, n_pes, rank,
@@ -227,8 +229,13 @@ class GroupbyState:
     # state switches to the raw-row form: every further batch is hash-partitioned (b200_shuffle_partition) and exchanged right away
     # (all-to-all-v), each rank aggregates only rows of groups it owns, and the final exchange only carries what was aggregated
     # before the switch.  Collective: decided once, from the first >= B200_SHUFFLE_DECISION_ROWS rows, identically on every rank.
+    # A state that computes first or last never switches: a raw row is numbered by the rank that consumes it (its owner), not by
+    # the rank it came from, so after the switch first / last would no longer follow the rank-major order (rows of a lower rank
+    # first, then row order) that the partial-aggregate form keeps.  Nor does a state with a 1- or 2-byte key column (int8,
+    # uint8, int16, uint16, bool), which shuffle_table does not partition.
     raw_row_mode = False
     shuffle_decided = False
+    stays_partial = False
     raw_rows_shuffled = 0
 
     def _decide_reduce_or_shuffle(self):
@@ -237,6 +244,9 @@ class GroupbyState:
         import torch
         import torch.distributed as dist
 
+        if self.stays_partial:  # (the same on every rank: no collective needed)
+            self.shuffle_decided = True
+            return
         L = _lib.lib()
         dev = torch.device("cuda", self.device)
         t = torch.tensor([int(L.b200_groupby_get_metric(self.handle, 13)), int(L.b200_groupby_get_metric(self.handle, 2))], dtype=torch.int64, device=dev)

@@ -191,7 +191,9 @@ def test_float64_key_special_values(gpu_lib, oracle, R, transport):
 
 @pytest.mark.parametrize("transport", ["fused", "overflow", "nccl"])
 @pytest.mark.parametrize("R", [2, 3, 4])
-def test_nullable_int32_key_with_na(gpu_lib, oracle, R, transport):
+def test_nullable_int32_key_with_na_owned_where_shuffle_table_sends_it(gpu_lib, R, transport):
+    """An int32 key's owner is the hash of its 4 raw bytes (hash_keys_table, pinned against the oracle in test_gpu_shuffle.py),
+    as shuffle_table places its rows, not the hash of its widened 8-byte value."""
     rng = np.random.default_rng(300 + R)
     n = 80_000
     k = pd.array(rng.integers(-5000, 5000, n).astype(np.int32), dtype="Int32")
@@ -202,8 +204,10 @@ def test_nullable_int32_key_with_na(gpu_lib, oracle, R, transport):
     _check_union(outs, exp, 1, ("sum", "count", "max"), ())
 
     def owner(key):
-        valid = key.notna().to_numpy()
-        return oracle.hash_to_rank(key.to_numpy(dtype="int64", na_value=0), valid, R)
+        from bodo_b200.shuffle import hash_keys_table
+
+        _, dest = hash_keys_table(table_to_device(Table.from_pandas(key.to_frame())), 1, R)
+        return dest.cpu().numpy()
     _owned_single(outs, R, owner)
 
 

@@ -3,7 +3,9 @@ one GPU, with the ranks simulated as threads of this process.
 
 The lock-step process group.  R ranks run as R threads, each with a thread-local rank, and the torch.distributed functions the
 library calls (is_initialized, get_world_size, get_rank, all_reduce with SUM / MIN / MAX, all_gather_into_tensor and
-all_to_all_single with or without split sizes) are replaced through monkeypatch.  The ranks take turns: between two collectives
+all_to_all_single with or without split sizes, barrier) are replaced through monkeypatch.  A collective called with async_op=True
+runs at its barrier as any other and returns a completed handle whose wait() returns at once: a schedule more synchronous than
+the real one, never less.  The ranks take turns: between two collectives
 rank 0 runs, then rank 1, ..., so no two ranks are ever inside the library at once (the real system runs one process per GPU) and
 every run is deterministic.  A collective stores its input, hands the turn on and waits on a threading.Barrier(R) whose action
 runs the collective once for all ranks with torch ops on the ranks' tensors and gives the turn back to rank 0.  A rank that
@@ -56,6 +58,16 @@ class _Aborted(Exception):
     """Raised in a rank that stops because another rank failed."""
 
 
+class _Completed:
+    """The work handle of an async_op collective: it already ran."""
+
+    def wait(self, timeout=None):
+        return True
+
+    def is_completed(self):
+        return True
+
+
 class LockstepGroup:
     """R ranks as R threads that take turns (see the module docstring); `install` patches torch.distributed, `run` runs them."""
 
@@ -81,6 +93,7 @@ class LockstepGroup:
         monkeypatch.setattr(dist, "all_reduce", self.all_reduce)
         monkeypatch.setattr(dist, "all_gather_into_tensor", self.all_gather_into_tensor)
         monkeypatch.setattr(dist, "all_to_all_single", self.all_to_all_single)
+        monkeypatch.setattr(dist, "barrier", self.barrier_collective)
         return self
 
     @staticmethod
@@ -99,21 +112,24 @@ class LockstepGroup:
     def all_reduce(self, tensor, op=None, group=None, async_op=False):
         import torch.distributed as dist
 
-        self._enter("all_reduce", group, async_op, tensor=tensor, op=dist.ReduceOp.SUM if op is None else op)
+        return self._enter("all_reduce", group, async_op, tensor=tensor, op=dist.ReduceOp.SUM if op is None else op)
 
     def all_gather_into_tensor(self, output_tensor, input_tensor, group=None, async_op=False):
-        self._enter("all_gather_into_tensor", group, async_op, output=output_tensor, input=input_tensor)
+        return self._enter("all_gather_into_tensor", group, async_op, output=output_tensor, input=input_tensor)
 
     def all_to_all_single(self, output, input, output_split_sizes=None, input_split_sizes=None, group=None, async_op=False):
-        self._enter("all_to_all_single", group, async_op, output=output, input=input,
-                    out_splits=None if output_split_sizes is None else [int(x) for x in output_split_sizes],
-                    in_splits=None if input_split_sizes is None else [int(x) for x in input_split_sizes])
+        return self._enter("all_to_all_single", group, async_op, output=output, input=input,
+                           out_splits=None if output_split_sizes is None else [int(x) for x in output_split_sizes],
+                           in_splits=None if input_split_sizes is None else [int(x) for x in input_split_sizes])
+
+    def barrier_collective(self, group=None, async_op=False, device_ids=None):
+        """torch.distributed.barrier: every rank waits until all ranks arrived (also the device-side barrier of a stand-in for
+        the fused exchange's symmetric-memory handle)."""
+        return self._enter("barrier", group, async_op)
 
     # ---- turns and collectives
     def _enter(self, name, group, async_op, **args):
         self._check_group(group)
-        if async_op:
-            raise NotImplementedError(f"{name}: async_op")
         r = self.rank
         with self.cond:
             if self.finished:
@@ -126,6 +142,7 @@ class LockstepGroup:
         except threading.BrokenBarrierError:
             raise _Aborted(f"rank {r}: {name} was abandoned") from None
         self._wait_turn(r)
+        return _Completed() if async_op else None
 
     def _wait_turn(self, r):
         with self.cond:
@@ -153,6 +170,9 @@ class LockstepGroup:
         with self.cond:
             self.turn = 0
             self.cond.notify_all()
+
+    def _run_barrier(self, args):
+        pass
 
     def _run_all_reduce(self, args):
         import torch.distributed as dist
@@ -305,6 +325,69 @@ def test_collectives_match_hand_computed_results(lockstep, R):
         assert o["counts"] == [sc[s][r] for s in range(R)]
         assert o["v"] == [1000.0 * s + sum(sc[s][:r]) + i for s in range(R) for i in range(sc[s][r])]
     assert pg.calls == ["all_reduce"] * 4 + ["all_gather_into_tensor"] + ["all_to_all_single"] * 3
+
+
+@pytest.mark.parametrize("R", [2, 3, 5])
+def test_async_collectives_return_a_completed_handle(lockstep, R):
+    """async_op=True: the collective has run when the call returns (the output is already there), and wait() returns at once."""
+    import torch.distributed as dist
+
+    pg = lockstep(R)
+
+    def body(r):
+        x = torch.tensor([r + 1, 2 * r], dtype=torch.int64)
+        w1 = dist.all_reduce(x, async_op=True)
+        after_reduce = x.tolist()  # read before wait(): the collective ran already
+        g = torch.empty(2 * R, dtype=torch.int64)
+        w2 = dist.all_gather_into_tensor(g, torch.tensor([r, 7 * r], dtype=torch.int64), async_op=True)
+        after_gather = g.tolist()
+        y = torch.empty(R, dtype=torch.int64)
+        w3 = dist.all_to_all_single(y, torch.arange(R, dtype=torch.int64) + 10 * r, async_op=True)
+        t0 = time.monotonic()
+        for w in (w1, w2, w3):
+            w.wait()
+        assert time.monotonic() - t0 < 1.0
+        assert dist.all_reduce(torch.zeros(1)) is None  # (a synchronous call still returns None)
+        return after_reduce, after_gather, y.tolist(), all(w.is_completed() for w in (w1, w2, w3))
+
+    res = pg.run(body)
+    for r, (red, gat, a2a, done) in enumerate(res):
+        assert red == [R * (R + 1) // 2, R * (R - 1)]
+        assert gat == [v for s in range(R) for v in (s, 7 * s)]
+        assert a2a == [10 * s + r for s in range(R)] and done
+    assert pg.calls == ["all_reduce", "all_gather_into_tensor", "all_to_all_single", "all_reduce"]
+
+
+def test_barrier_waits_for_every_rank(lockstep):
+    """barrier(): no rank passes it before every rank arrived; a sync and an async barrier match one another."""
+    import torch.distributed as dist
+
+    R = 3
+    pg = lockstep(R)
+    log = []
+
+    def body(r):
+        log.append(("before", r))
+        dist.barrier()
+        log.append(("after", r))
+        w = dist.barrier(async_op=(r == 1))
+        if w is not None:
+            w.wait()
+        log.append(("end", r))
+
+    pg.run(body)
+    assert log == [(p, r) for p in ("before", "after", "end") for r in range(R)]
+    assert pg.calls == ["barrier", "barrier"]
+    mixed = lockstep(2)
+
+    def other(r):
+        if r == 0:
+            dist.barrier()
+        else:
+            dist.all_reduce(torch.zeros(1))
+
+    with pytest.raises(RankError, match="different collectives"):
+        mixed.run(other)
 
 
 def test_ranks_take_turns_in_rank_order(lockstep):
