@@ -17,12 +17,12 @@ enum CType : int { CT_INT8 = 0, CT_UINT8 = 1, CT_INT32 = 2, CT_UINT32 = 3, CT_IN
                    CT_TIMEDELTA = 16 };
 enum ArrType : int { ARR_NUMPY = 0, ARR_NULLABLE = 2 };
 // Bodo_FTypes (reference: bodo/libs/groupby/_groupby_ftypes.h:17-110)
-// 28..34 continue the enum after skew in the reference's order; they are recalled, not read from a reference checkout (17 and 26
-// are fixed by their neighbours).
+// 28..34 and 38..40 continue the enum after skew in the reference's order; they are recalled, not read from a reference checkout
+// (17 and 26 are fixed by their neighbours).
 enum FType : int { FT_SIZE = 4, FT_SUM = 6, FT_COUNT = 7, FT_NUNIQUE = 8, FT_MEAN = 14, FT_MIN = 15, FT_MAX = 16, FT_PROD = 17, FT_FIRST = 18,
                    FT_LAST = 19, FT_VAR_POP = 22, FT_STD_POP = 23, FT_VAR = 24, FT_STD = 25, FT_KURTOSIS = 26, FT_SKEW = 27,
                    FT_BOOLOR_AGG = 28, FT_BOOLAND_AGG = 29, FT_BOOLXOR_AGG = 30, FT_BITOR_AGG = 31, FT_BITAND_AGG = 32, FT_BITXOR_AGG = 33,
-                   FT_COUNT_IF = 34 };
+                   FT_COUNT_IF = 34, FT_MODE = 38, FT_PERCENTILE_CONT = 39, FT_PERCENTILE_DISC = 40 };
 
 // hash seeds (reference: bodo/libs/_array_hash.h:8-14)
 constexpr uint32_t SEED_HASH_PARTITION = 0xb0d01289u;
@@ -353,8 +353,10 @@ using PooledBuf = DevBuf;
 
 // Stable ascending radix sort of rows [0, n) by n_keys (1..4) plain device columns without NAs, key j at data[j] encoded by
 // keys[j] (sort_word), through the full sort's histogram and pass kernels (sort.cu), on stream `st`.  Returns the permutation in
-// ids[0] or ids[1] (mask each entry with 0x7FFFFFFF), or nullptr for the identity (every digit constant, or n == 0).
-const uint32_t* radix_sort_columns(int n_keys, const void* const* data, const SortKey* keys, int64_t n, DevBuf (&ids)[2], cudaStream_t st);
+// ids[0] or ids[1] (mask each entry with 0x7FFFFFFF), or nullptr for the identity (every digit constant, or n == 0).  Adds the
+// digit passes it ran to *passes_run unless that is nullptr.
+const uint32_t* radix_sort_columns(int n_keys, const void* const* data, const SortKey* keys, int64_t n, DevBuf (&ids)[2], cudaStream_t st,
+                                   int64_t* passes_run = nullptr);
 
 // ---- tile scans (join.cu's offsets, sort.cu's window): a tile of 2048 rows, 256 threads x 8 items ----
 // A scan runs in three launches: each tile's reduction, tile_carry_kernel over the tile values, then each tile's scan seeded by

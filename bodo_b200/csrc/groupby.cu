@@ -54,7 +54,11 @@ enum OpKind : int { K_SUM_I64 = 0, K_SUM_F64, K_COUNT, K_SIZE, K_MEAN, K_MIN_I64
                     K_OR, K_AND, K_XOR, K_LOR, K_LAND,
                     K_COUNT_IF,  // a0 = rows whose value is true (nonzero); a1 (when present) counts the non-NA rows
                     // evaluation-only kinds: kurtosis (accumulators K_MOM1 .. K_MOM4), boolxor (K_COUNT_IF: exactly one true)
-                    E_KURT, E_BOOLXOR };
+                    E_KURT, E_BOOLXOR,
+                    // holistic aggregates (see holistic_append_kernel): K_HID is the group's id word, all-ones until claimed; E_MODE,
+                    // E_PCONT and E_PDISC are their result words, written at finalize (a0 = the result's bits, a1 = 0 once it is
+                    // valid, all-ones before).  No consume kernel applies any of them: they lie past n_apply()
+                    K_HID, E_MODE, E_PCONT, E_PDISC };
 constexpr unsigned long long SHIFT_UNSET = 0x7ff8000000000000ull;  // K_SHIFT's initial value (quiet NaN; NaN values are skipped)
 
 struct OpDesc {
@@ -1536,6 +1540,178 @@ __global__ void mrnf_top_gather_kernel(const unsigned long long* store, uint64_t
     }
 }
 
+// ---- holistic aggregates: mode, percentile_cont, percentile_disc ----
+// They need the whole multiset of a group's non-NA values, so the state keeps it.  The table carries one K_HID word per slot, the
+// group's id (all-ones until the group's first row claims one; ids survive growth while slots move), and each distinct value
+// column has a store of (id, value) rows: a 4-byte id column and a column of the value's own width.  Per batch, once every row
+// is in the table, holistic_append_kernel appends each row's non-NA (and non-NaN) values.  Finalize sorts each store by (id,
+// sort_word(value)) with radix_sort_columns, marks each id's first and last sorted position (holistic_bounds_kernel) and writes
+// every result into its slot's result word (holistic_eval_kernel, one thread per slot): a percentile reads one or two sorted
+// positions; mode takes, per id, the longest run of equal values, found from the runs' starts (a flag, the tile scan,
+// holistic_run_start_kernel, holistic_run_best_kernel).  No thread walks a group's rows, so one group holding most rows costs
+// what a uniform input costs.
+struct HoAppendArgs {
+    MrnfArgs m;                // the table and the batch's key columns (n_rows, nk, dropna, key_*, tkeys / tags / mk / mkmask, cap)
+    unsigned drop_nan;         // dropna: key columns (float) whose NaN marker group is dropped, as compact_* drop it
+    unsigned long long* gid;   // per slot: the group's id, ~0 = none yet
+    unsigned long long* ctr;   // [0] ids handed out, [1 + i] rows of store i (its append cursor)
+    int n_st;
+    const void* val[MAX_OPS];  // the batch's value column of store i
+    const uint8_t* valid[MAX_OPS];
+    int ct[MAX_OPS];
+    uint32_t* st_id[MAX_OPS];
+    void* st_val[MAX_OPS];
+};
+__global__ void __launch_bounds__(256) holistic_append_kernel(const __grid_constant__ HoAppendArgs a) {
+    const MrnfArgs& m = a.m;
+    const int64_t n_round = (m.n_rows + 31) & ~31ll;
+    const int lane = threadIdx.x & 31;
+    for (int64_t row = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; row < n_round; row += (int64_t)gridDim.x * blockDim.x) {
+        const uint64_t slot = row < m.n_rows ? mrnf_find_slot(m, row) : ~0ull;
+        bool in = slot != ~0ull;
+        for (int j = 0; j < m.nk && in; j++)
+            if (((a.drop_nan >> j) & 1u) && bit_valid(m.key_valid[j], row)) in = load_int_as_i64(m.key_data[j], m.key_ctype[j], row) != EMPTY_KEY;
+        unsigned long long id = in ? __ldcg(a.gid + slot) : 0ull;
+        // a group without an id: of the warp's lanes that stand on its slot the lowest claims one (a thread that loses the race to
+        // another warp takes the winner's), the others take it from that lane
+        const bool claim = in && id == ~0ull;
+        const unsigned peers = __match_any_sync(0xffffffffu, claim ? slot : ~0ull);
+        const int leader = __ffs(peers) - 1;
+        if (claim && lane == leader) {
+            const unsigned long long mine = atomicAdd(a.ctr, 1ull);
+            const unsigned long long old = atomicCAS(a.gid + slot, ~0ull, mine);
+            id = old == ~0ull ? mine : old;
+        }
+        const unsigned long long lead_id = __shfl_sync(0xffffffffu, id, leader);
+        if (claim) id = lead_id;
+        for (int i = 0; i < a.n_st; i++) {
+            bool v = in && bit_valid(a.valid[i], row);
+            if (v && ctype_is_float(a.ct[i])) v = !isnan(load_as_f64(a.val[i], a.ct[i], row));
+            const unsigned ball = __ballot_sync(0xffffffffu, v);
+            unsigned long long base = 0;
+            if (lane == 0 && ball) base = atomicAdd(a.ctr + 1 + i, (unsigned long long)__popc(ball));
+            base = __shfl_sync(0xffffffffu, base, 0);
+            if (!v) continue;
+            const unsigned long long r = base + __popc(ball & ((1u << lane) - 1));
+            a.st_id[i][r] = (uint32_t)id;
+            copy_cell(a.st_val[i], (int64_t)r, a.val[i], row, ctype_size(a.ct[i]));
+        }
+    }
+}
+
+// One store after its sort: sorted position i holds store row row(i).
+struct HoSorted {
+    const uint32_t* id;
+    const void* val;
+    SortKey key;  // the value's encoding (ascending)
+    const uint32_t* perm;  // nullptr: the identity
+    int64_t n;
+    __device__ __forceinline__ int64_t row(int64_t i) const { return perm ? (int64_t)(perm[i] & 0x7FFFFFFFu) : i; }
+    __device__ __forceinline__ uint64_t word(int64_t r) const {
+        bool na = false;
+        return sort_word(key, load_bits(val, key.size, r), na);
+    }
+};
+// head[g] = the first sorted position of id g, tail[g] = one past its last (both stay 0 for an id without values); flag[i] = a run
+// of equal (id, value) starts at position i (flag nullptr: the store feeds no mode)
+__global__ void holistic_bounds_kernel(const __grid_constant__ HoSorted s, uint32_t* head, uint32_t* tail, uint32_t* flag) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < s.n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = s.row(i);
+        const uint32_t g = s.id[r];
+        const bool first = i == 0 || s.id[s.row(i - 1)] != g;
+        if (first) head[g] = (uint32_t)i;
+        if (i + 1 == s.n || s.id[s.row(i + 1)] != g) tail[g] = (uint32_t)(i + 1);
+        if (flag) flag[i] = first || s.word(s.row(i - 1)) != s.word(r);
+    }
+}
+// start[pos[i]] = i for every run start i (pos: the exclusive scan of flag)
+__global__ void holistic_run_start_kernel(const uint32_t* flag, const unsigned long long* pos, int64_t n, uint32_t* start) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        if (flag[i]) start[pos[i]] = (uint32_t)i;
+}
+// Run r covers sorted positions [start[r], start[r + 1]) (the last one ends at n).  best[g] = max over the runs of id g of
+// (length << 32 | ~start): the longest run, and of equally long ones the first, which holds the least value.
+__global__ void holistic_run_best_kernel(const __grid_constant__ HoSorted s, const uint32_t* start, int64_t n_runs, unsigned long long* best) {
+    for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n_runs; r += (int64_t)gridDim.x * blockDim.x) {
+        const uint32_t b = start[r];
+        const int64_t e = r + 1 < n_runs ? (int64_t)start[r + 1] : s.n;
+        atomicMax(best + s.id[s.row(b)], ((unsigned long long)(e - b) << 32) | (unsigned long long)(uint32_t)~b);
+    }
+}
+
+// A store value (raw bits of its width) as a double, -0.0 read as +0.0 (so a result depends on the multiset of sort words only).
+__device__ __forceinline__ double ho_f64(int ct, uint64_t raw) {
+    double d;
+    switch (ct) {
+        case CT_FLOAT64: d = __longlong_as_double((long long)raw); break;
+        case CT_FLOAT32: d = (double)__uint_as_float((uint32_t)raw); break;
+        case CT_UINT64: return (double)raw;
+        default: {
+            const int sh = 64 - 8 * ctype_size(ct);
+            return ctype_is_signed_int(ct) ? (double)((long long)(raw << sh) >> sh) : (double)raw;
+        }
+    }
+    return d == 0.0 ? 0.0 : d;
+}
+// The result word of a store value as eval_output_kernel's K_FIRST case reads it: a float as its double's bits (+0.0 for a zero),
+// an integer, bool or temporal sign- or zero-extended to 64 bits.
+__device__ __forceinline__ unsigned long long ho_bits(int ct, uint64_t raw) {
+    if (ctype_is_float(ct)) return (unsigned long long)__double_as_longlong(ho_f64(ct, raw));
+    const int sh = 64 - 8 * ctype_size(ct);
+    return ctype_is_signed_int(ct) ? (unsigned long long)((long long)(raw << sh) >> sh) : raw;
+}
+
+struct HoEvalArgs {
+    HoSorted s;
+    const unsigned long long* gid;  // per slot: the group's id
+    uint64_t n_slots;               // cap + 2
+    const uint32_t* head;
+    const uint32_t* tail;
+    const unsigned long long* best;  // mode: see holistic_run_best_kernel
+    int n_f;                         // the functions over this store
+    int kind[MAX_OPS];               // E_MODE, E_PCONT, E_PDISC
+    double q[MAX_OPS];
+    unsigned long long* res[MAX_OPS];   // the result word (a0) and its validity word (a1) per slot
+    unsigned long long* seen[MAX_OPS];
+};
+// One thread per slot (one per group: the id's bounds give its m values, v_0 .. v_{m-1} at sorted positions head .. tail - 1).
+// percentile_cont: h = q (m - 1), lo = floor(h), f = h - lo; v_lo when f == 0, else a + (b - a) f with a = v_lo and b = v_{lo+1}
+// as doubles (pandas' linear group_quantile).  Rounded operations without contraction: the host restatement of the formula gets
+// the same bits.  percentile_disc: v_i with i = clamp(ceil(q m) - 1, 0, m - 1).  mode: the value of the id's best run.
+__global__ void holistic_eval_kernel(const __grid_constant__ HoEvalArgs a) {
+    const HoSorted& s = a.s;
+    for (uint64_t slot = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; slot < a.n_slots; slot += (uint64_t)gridDim.x * blockDim.x) {
+        const unsigned long long g = a.gid[slot];
+        if (g == ~0ull) continue;
+        const int64_t h = a.head[g], m = (int64_t)a.tail[g] - h;
+        if (m <= 0) continue;
+        for (int f = 0; f < a.n_f; f++) {
+            unsigned long long bits;
+            if (a.kind[f] == E_PCONT) {
+                const double hq = __dmul_rn(a.q[f], (double)(m - 1)), lo = floor(hq), fr = __dsub_rn(hq, lo);
+                const int64_t i = (int64_t)lo;
+                double r = ho_f64(s.key.ct, load_bits(s.val, s.key.size, s.row(h + i)));
+                if (fr != 0.0) {
+                    const double b = ho_f64(s.key.ct, load_bits(s.val, s.key.size, s.row(h + i + 1)));
+                    r = __dadd_rn(r, __dmul_rn(__dsub_rn(b, r), fr));
+                }
+                bits = (unsigned long long)__double_as_longlong(r);
+            } else {
+                int64_t p;
+                if (a.kind[f] == E_PDISC) {
+                    const int64_t i = (int64_t)ceil(__dmul_rn(a.q[f], (double)m)) - 1;
+                    p = h + (i < 0 ? 0 : i >= m ? m - 1 : i);
+                } else {
+                    p = (uint32_t)~(uint32_t)a.best[g];
+                }
+                bits = ho_bits(s.key.ct, load_bits(s.val, s.key.size, s.row(p)));
+            }
+            a.res[f][slot] = bits;
+            a.seen[f][slot] = 0;
+        }
+    }
+}
+
 // ================================================================================================
 // SM-partitioned groupby (SPG): the fast path for cardinalities whose accumulators fit the chip's
 // aggregate shared memory (≈ SMs x 10k groups).  Motivation (scratch/ubench*.cu): two global `red`s per
@@ -2367,7 +2543,8 @@ class GroupbyState {
 
     GroupbyState(const int8_t* ct, const int8_t* at, int n_arrs, const int32_t* ftypes, const int32_t* f_in_offsets,
                  const int32_t* f_in_cols, int n_funcs_, uint64_t n_keys, int64_t out_bs, bool parallel_, bool dropna_,
-                 int device_, int n_pes_, int rank_, int64_t expected_groups, cudaStream_t stream_, const MrnfSpec* mrnf = nullptr)
+                 int device_, int n_pes_, int rank_, int64_t expected_groups, cudaStream_t stream_, const MrnfSpec* mrnf = nullptr,
+                 const double* fractions = nullptr)
         : device(device_), stream(stream_), n_cols(n_arrs), n_funcs(0), n_outs(n_funcs_), dropna(dropna_), parallel(parallel_),
           n_pes(n_pes_), rank(rank_), output_batch_size(out_bs) {
         B200_REQUIRE(n_keys >= 1 && n_keys <= (uint64_t)MAX_KEYS, "b200 groupby: between 1 and 4 key columns are supported");
@@ -2500,10 +2677,35 @@ class GroupbyState {
                     outs.push_back(o);
                     continue;
                 }
+                case FT_MODE: case FT_PERCENTILE_CONT: case FT_PERCENTILE_DISC: {
+                    // holistic: one store per value column; the result word is added after the loop (see Holistic)
+                    const bool cont = f.ftype == FT_PERCENTILE_CONT, disc = f.ftype == FT_PERCENTILE_DISC;
+                    B200_REQUIRE(n_in == 1, "b200 groupby: mode / percentile_cont / percentile_disc take one input column");
+                    if (cont) refuse_type(f.in_ctype != CT_BOOL && !ctype_is_temporal(f.in_ctype), "percentile_cont", "integer and float columns");
+                    if (disc) refuse_type(f.in_ctype != CT_BOOL, "percentile_disc", "integer, float, date, datetime and timedelta columns");
+                    double q = 0.0;
+                    if (cont || disc) {
+                        B200_REQUIRE(fractions != nullptr, "b200 groupby: percentile_cont / percentile_disc need a fraction (b200_groupby_state_init_percentiles)");
+                        q = fractions[j];
+                        B200_REQUIRE(q >= 0.0 && q <= 1.0, "b200 groupby: the fraction of percentile_cont / percentile_disc (function " + std::to_string(j) +
+                                                               ") must lie in [0, 1]");
+                    }
+                    size_t si = 0;
+                    while (si < ho.st.size() && ho.st[si].in_col != f.in_col) si++;
+                    if (si == ho.st.size()) { ho.st.emplace_back(); ho.st[si].in_col = f.in_col; }
+                    ho.on = true;
+                    ho.outs.push_back(HoOut{(int)outs.size(), (int)si, cont ? E_PCONT : disc ? E_PDISC : E_MODE, q});
+                    OutSpec o{};
+                    o.ftype = f.ftype; o.kind = K_FIRST; o.n_prim = 1;  // (prim[0]: the result word, set after the loop)
+                    o.out_ctype = cont ? CT_FLOAT64 : f.in_ctype; o.out_arrtype = ARR_NULLABLE;
+                    outs.push_back(o);
+                    continue;
+                }
                 default:
                     throw Error("b200 groupby: unsupported aggregate function ftype=" + std::to_string(f.ftype) +
                                 " (supported: size, sum, count, nunique, mean, min, max, prod, first, last, var, std, var_pop, std_pop, "
-                                "kurtosis, skew, boolor_agg, booland_agg, boolxor_agg, bitor_agg, bitand_agg, bitxor_agg, count_if)");
+                                "kurtosis, skew, boolor_agg, booland_agg, boolxor_agg, bitor_agg, bitand_agg, bitxor_agg, count_if, mode, "
+                                "percentile_cont, percentile_disc)");
             }
             OutSpec o{};
             o.ftype = f.ftype; o.kind = f.ftype == FT_BOOLXOR_AGG ? E_BOOLXOR : f.kind; o.prim[0] = (int)funcs.size(); o.n_prim = 1; o.out_ctype = f.out_ctype; o.out_arrtype = f.out_arrtype;
@@ -2511,6 +2713,7 @@ class GroupbyState {
             funcs.push_back(f);
         }
         if (mrnf) setup_mrnf(*mrnf);
+        if (ho.on) setup_holistic();
         n_funcs = (int)funcs.size();
         B200_REQUIRE(mr.on || n_funcs <= MAX_OPS, "b200 groupby: too many aggregate functions (composite ones count their accumulator columns)");
         d_a0.resize(n_funcs); d_a1.resize(n_funcs);
@@ -3208,8 +3411,9 @@ class GroupbyState {
         fill_ops(a.ops, data, valid);
         return a;
     }
-    // the aggregate updates a consume launch applies per row: every function's, none for MRNF (its passes run after the launch)
-    int n_apply() const { return mr.on ? 0 : n_funcs; }
+    // the aggregate updates a consume launch applies per row: every function's, none for MRNF (its passes run after the launch),
+    // none of the holistic words (holistic_append_kernel runs after the launch)
+    int n_apply() const { return mr.on ? 0 : ho.on ? ho.p0 : n_funcs; }
     // the n_apply() aggregate updates of a consume launch (ConsumeArgs / MkArgs)
     void fill_ops(OpDesc* ops, const std::vector<const void*>& data, const std::vector<const uint8_t*>& valid) const {
         for (int j = 0; j < n_apply(); j++) {
@@ -3249,6 +3453,7 @@ class GroupbyState {
         const std::vector<const void*> raw = data;
         canon_keys(data, n);
         if (mr.on) consume_mrnf(data, raw, valid, n);
+        else if (ho.on) consume_holistic(data, valid, n);
         else consume_device_chunk(data, valid, n);
     }
 
@@ -3534,6 +3739,169 @@ class GroupbyState {
         return n_out;
     }
 
+    // ---- holistic aggregates (see holistic_append_kernel) ----
+    static constexpr int64_t HO_STORE_MAX = 1ll << 31;  // rows radix_sort_columns sorts at once
+    static constexpr int64_t HO_MAX_IDS = 1ll << 32;    // store ids are 4 bytes
+    struct HoStore {
+        int in_col = -1;
+        DevBuf id, val;     // cap rows each: the group id (4 bytes) and the value (its width)
+        int64_t cap = 0;
+        int64_t bound = 0;  // upper bound on the rows (the device cursor ctr[1 + i] is exact)
+    };
+    struct HoOut { int out, store, kind; double q; };
+    struct Holistic {
+        bool on = false;
+        int p0 = 0;  // funcs[p0]: the group id word (K_HID); funcs[p0 + 1 + k]: the result word of outs[k]
+        std::vector<HoStore> st;
+        std::vector<HoOut> outs;
+        DevBuf ctr;  // [0] ids handed out, [1 + i] rows of store i
+        std::vector<unsigned long long> h_ctr;
+        int64_t id_bound = 0;  // upper bound on ctr[0]
+        int64_t passes = 0;    // metric 21: digit passes of the finalize sorts
+        DevBuf perm[2], head, tail, flag, pos, start, best;
+        Scanner scan;
+    } ho;
+
+    // the id word and one result word per holistic output, after every other accumulator (see n_apply)
+    void setup_holistic() {
+        B200_REQUIRE(ho.st.size() <= (size_t)MAX_OPS, "b200 groupby: too many value columns for mode / percentiles");
+        ho.p0 = (int)funcs.size();
+        FuncSpec g{};
+        g.in_col = -1; g.in_ctype = CT_INT64; g.in_arrtype = ARR_NUMPY; g.kind = K_HID; g.out_ctype = CT_INT64; g.out_arrtype = ARR_NUMPY;
+        g.init0 = ~0ull;
+        funcs.push_back(g);
+        for (const HoOut& h : ho.outs) {
+            FuncSpec r{};
+            r.in_col = ho.st[h.store].in_col; r.in_ctype = c_types[r.in_col]; r.in_arrtype = arr_types[r.in_col]; r.kind = h.kind;
+            r.out_ctype = outs[h.out].out_ctype; r.out_arrtype = ARR_NULLABLE; r.has_a1 = true; r.init1 = ~0ull;
+            outs[h.out].prim[0] = (int)funcs.size();
+            funcs.push_back(r);
+        }
+        ho.ctr.alloc((1 + ho.st.size()) * 8);
+        B200_CUDA(cudaMemsetAsync(ho.ctr.p, 0, (1 + ho.st.size()) * 8, stream));
+        ho.h_ctr.assign(1 + ho.st.size(), 0);
+    }
+    // the device counters into ho.h_ctr and the bounds (synchronises the stream)
+    void read_holistic_counts() {
+        B200_CUDA(cudaMemcpyAsync(ho.h_ctr.data(), ho.ctr.p, ho.h_ctr.size() * 8, cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaStreamSynchronize(stream));
+        ho.id_bound = (int64_t)ho.h_ctr[0];
+        for (size_t i = 0; i < ho.st.size(); i++) ho.st[i].bound = (int64_t)ho.h_ctr[1 + i];
+    }
+    int64_t holistic_rows() {  // metric 20: values appended to the stores
+        read_holistic_counts();
+        int64_t r = 0;
+        for (auto& s : ho.st) r += s.bound;
+        return r;
+    }
+    // Refuses a batch of n rows that could take a store past HO_STORE_MAX rows, or the ids past 4 bytes, before anything runs.
+    void ensure_holistic_room(int64_t n) {
+        bool over = ho.id_bound + n > HO_MAX_IDS;
+        for (auto& s : ho.st) over = over || s.bound + n > HO_STORE_MAX;
+        if (!over) return;
+        read_holistic_counts();
+        B200_REQUIRE(ho.id_bound + n <= HO_MAX_IDS, "b200 groupby: mode / percentiles number their groups with 4-byte ids; this batch could "
+                                                    "pass 2^32 groups");
+        for (auto& s : ho.st)
+            B200_REQUIRE(s.bound + n <= HO_STORE_MAX,
+                         "b200 groupby: mode / percentile_cont / percentile_disc keep the non-NA values of a column (column " + std::to_string(s.in_col) +
+                             ": " + std::to_string(s.bound) + " so far, plus a batch of " + std::to_string(n) +
+                             " rows) for one radix sort of at most 2^31 rows; keep them below 2^31 per column");
+    }
+    void consume_holistic(const std::vector<const void*>& data, const std::vector<const uint8_t*>& valid, int64_t n) {
+        if (n == 0) return;
+        // every row into the table first (the other aggregates are applied there: n_apply() stops before the holistic words)
+        if (nk > 1) consume_mk(data, valid, n);
+        else consume_direct(data, valid, n, false, -1, -1, -1, false);
+        HoAppendArgs a{};
+        MrnfArgs& m = a.m;
+        m.n_rows = n; m.nk = nk; m.dropna = dropna ? 1 : 0; m.cap = cap;
+        for (int j = 0; j < nk; j++) { m.key_data[j] = data[j]; m.key_valid[j] = valid[j]; m.key_ctype[j] = c_types[j]; }
+        if (nk == 1) m.tkeys = d_keys.as<long long>();
+        else {
+            m.tags = d_tags.as<unsigned long long>(); m.mkmask = d_mkmask.as<unsigned char>();
+            for (int j = 0; j < nk; j++) m.mk[j] = d_mk[j].as<long long>();
+        }
+        for (int j = 0; j < nk; j++) if (dropna && float_key(j)) a.drop_nan |= 1u << j;
+        a.gid = d_a0[ho.p0].as<unsigned long long>();
+        a.ctr = ho.ctr.as<unsigned long long>();
+        a.n_st = (int)ho.st.size();
+        for (int i = 0; i < a.n_st; i++) {
+            HoStore& s = ho.st[i];
+            const int c = s.in_col, w = ctype_size(in_types[c]);
+            if (s.bound + n > s.cap) {  // a larger store, keeping its rows (the host makes room: the kernel has no overflow path)
+                const int64_t nc = std::min(HO_STORE_MAX, std::max(s.bound + n, s.cap + s.cap / 2));
+                DevBuf id, val;
+                id.alloc((size_t)nc * 4);
+                val.alloc((size_t)nc * w);
+                if (s.bound > 0) {
+                    B200_CUDA(cudaMemcpyAsync(id.p, s.id.p, (size_t)s.bound * 4, cudaMemcpyDeviceToDevice, stream));
+                    B200_CUDA(cudaMemcpyAsync(val.p, s.val.p, (size_t)s.bound * w, cudaMemcpyDeviceToDevice, stream));
+                }
+                s.id = std::move(id); s.val = std::move(val); s.cap = nc;
+            }
+            a.val[i] = data[c]; a.valid[i] = valid[c]; a.ct[i] = in_types[c];
+            a.st_id[i] = s.id.as<uint32_t>(); a.st_val[i] = s.val.p;
+            s.bound += n;
+        }
+        holistic_append_kernel<<<grid_for(n), 256, 0, stream>>>(a);
+        launches++;
+        B200_CUDA(cudaGetLastError());
+        ho.id_bound += n;
+    }
+    // Writes every holistic result word (before compaction: eval_output_kernel reads them as first / last words).
+    void finalize_holistic() {
+        read_holistic_counts();
+        const int64_t n_ids = ho.id_bound;
+        if (n_ids == 0) return;
+        ho.head.ensure((size_t)n_ids * 4);
+        ho.tail.ensure((size_t)n_ids * 4);
+        for (size_t i = 0; i < ho.st.size(); i++) {
+            HoStore& s = ho.st[i];
+            const int64_t m = s.bound;
+            if (m == 0) continue;  // (every result over this column stays NA)
+            const int ct = in_types[s.in_col];
+            const SortKey keys[2] = {SortKey{CT_UINT32, 4, 0, 0}, SortKey{ct, ctype_size(ct), 0, 0}};
+            const void* cols[2] = {s.id.p, s.val.p};
+            HoSorted hs{};
+            hs.id = s.id.as<uint32_t>(); hs.val = s.val.p; hs.key = keys[1]; hs.n = m;
+            hs.perm = radix_sort_columns(2, cols, keys, m, ho.perm, stream, &ho.passes);
+            bool mode = false;
+            for (const HoOut& h : ho.outs) mode = mode || (h.store == (int)i && h.kind == E_MODE);
+            B200_CUDA(cudaMemsetAsync(ho.head.p, 0, (size_t)n_ids * 4, stream));
+            B200_CUDA(cudaMemsetAsync(ho.tail.p, 0, (size_t)n_ids * 4, stream));
+            if (mode) ho.flag.ensure((size_t)m * 4);
+            holistic_bounds_kernel<<<grid_for(m), 256, 0, stream>>>(hs, ho.head.as<uint32_t>(), ho.tail.as<uint32_t>(), mode ? ho.flag.as<uint32_t>() : nullptr);
+            launches++;
+            B200_CUDA(cudaGetLastError());
+            if (mode) {
+                ho.pos.ensure((size_t)m * 8);
+                ho.best.ensure((size_t)n_ids * 8);
+                B200_CUDA(cudaMemsetAsync(ho.best.p, 0, (size_t)n_ids * 8, stream));
+                const int64_t n_runs = (int64_t)ho.scan.run(ho.flag.as<uint32_t>(), m, ho.pos.as<unsigned long long>(), stream, &launches);
+                ho.start.ensure((size_t)n_runs * 4);
+                holistic_run_start_kernel<<<grid_for(m), 256, 0, stream>>>(ho.flag.as<uint32_t>(), ho.pos.as<unsigned long long>(), m, ho.start.as<uint32_t>());
+                holistic_run_best_kernel<<<grid_for(n_runs), 256, 0, stream>>>(hs, ho.start.as<uint32_t>(), n_runs, ho.best.as<unsigned long long>());
+                launches += 2;
+                B200_CUDA(cudaGetLastError());
+            }
+            HoEvalArgs e{};
+            e.s = hs; e.gid = d_a0[ho.p0].as<unsigned long long>(); e.n_slots = cap + 2;
+            e.head = ho.head.as<uint32_t>(); e.tail = ho.tail.as<uint32_t>(); e.best = mode ? ho.best.as<unsigned long long>() : nullptr;
+            for (size_t k = 0; k < ho.outs.size(); k++) {
+                const HoOut& h = ho.outs[k];
+                if (h.store != (int)i) continue;
+                const int p = ho.p0 + 1 + (int)k;
+                e.kind[e.n_f] = h.kind; e.q[e.n_f] = h.q;
+                e.res[e.n_f] = d_a0[p].as<unsigned long long>(); e.seen[e.n_f] = d_a1[p].as<unsigned long long>();
+                e.n_f++;
+            }
+            holistic_eval_kernel<<<grid_for((int64_t)cap + 2), 256, 0, stream>>>(e);
+            launches++;
+            B200_CUDA(cudaGetLastError());
+        }
+    }
+
     void consume(const b200_table* t) {
         B200_REQUIRE(!build_done, "b200 groupby: consume after the build was finished");
         B200_REQUIRE(t->n_cols == n_cols, "b200 groupby: batch has a different number of columns than the build schema");
@@ -3548,6 +3916,7 @@ class GroupbyState {
             for (int j = 0; j < mr.n_sort; j++) used[mr.sort_col[j]] = true;
             for (int c : mr.keep) used[c] = true;
         }
+        if (ho.on) ensure_holistic_room(n);  // (before anything reads the batch)
         for (int c = 0; c < n_cols; c++) {
             if (!used[c]) continue;
             B200_REQUIRE(t->cols[c].c_type == in_types[c], "b200 groupby: batch column dtype differs from the build schema");
@@ -3627,7 +3996,7 @@ class GroupbyState {
     int64_t co_n = 0, co_batches = 0;
     int co_vcol = -1;
     bool coalesce(const b200_table* t, int64_t n) {
-        if (mr.on) return false;
+        if (mr.on || ho.on) return false;
         if (n == 0 || n >= CO_MIN_BATCH || nk != 1 || n_funcs < 1 || c_types[0] != CT_INT64 || t->cols[0].validity != nullptr) return false;
         { const char* e = getenv("B200_COALESCE"); if (e && e[0] == '0') return false; }
         int vcol = -1;
@@ -3700,7 +4069,8 @@ class GroupbyState {
         if (nu_applied || nu_inner.empty()) return;
         for (auto& ni : nu_inner) {
             GroupbyState& in = *ni.st;
-            B200_REQUIRE(n_pes == 1 || in.exchanged, "b200 groupby: nunique on the sharded path: exchange the nested states (b200_groupby_inner_state) before the outer finalize");
+            // (a holistic state consumes only rows of groups it owns, so its nested states hold only pairs they own: no exchange)
+            B200_REQUIRE(n_pes == 1 || in.exchanged || ho.on, "b200 groupby: nunique on the sharded path: exchange the nested states (b200_groupby_inner_state) before the outer finalize");
             const int64_t n_pairs = in.finalize();
             B200_REQUIRE(n_pairs >= 0, "b200 groupby: nunique: the nested state's fused exchange overflowed its slab; exchange it in the NCCL form first");
             B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
@@ -3728,6 +4098,7 @@ class GroupbyState {
         // the exchange settles first, so that nunique also counts into the groups it brought
         if (exchanged && !settle_exchange()) return -2;
         apply_nunique();
+        if (ho.on) finalize_holistic();
         compact();
         const int64_t max_out = max_out_bound();
         EvalArgs e{};
@@ -3833,6 +4204,8 @@ class GroupbyState {
     void exchange_pack(void* const* peer_slabs_dev, int64_t cap_rows, void* send_buf) {
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
         B200_REQUIRE(!mr.on, "b200 groupby: a sharded min_row_number_filter is not supported (no exchange of winner records)");
+        B200_REQUIRE(!ho.on, "b200 groupby: mode / percentile_cont / percentile_disc do not combine as partial aggregates; a sharded state "
+                             "consumes rows hash-partitioned by key (each rank only its own groups) and finalizes without an exchange");
         flush_coalesced();
         build_done = true;
         const size_t cursor_bytes = (size_t)std::max(n_pes, 32) * 8;
@@ -3985,6 +4358,16 @@ void* b200_groupby_state_init(int64_t operator_id, const int8_t* build_arr_c_typ
                               const int32_t* f_in_cols, int32_t n_funcs, uint64_t n_keys, int64_t output_batch_size,
                               int32_t parallel, int32_t pandas_drop_na, int32_t device, int32_t n_pes, int32_t myrank,
                               int64_t expected_groups, void* stream) {
+    return b200_groupby_state_init_percentiles(operator_id, build_arr_c_types, build_arr_array_types, n_build_arrs, ftypes, f_in_offsets,
+                                               f_in_cols, n_funcs, n_keys, output_batch_size, parallel, pandas_drop_na, device, n_pes, myrank,
+                                               expected_groups, stream, nullptr);
+}
+
+void* b200_groupby_state_init_percentiles(int64_t operator_id, const int8_t* build_arr_c_types, const int8_t* build_arr_array_types,
+                                          int32_t n_build_arrs, const int32_t* ftypes, const int32_t* f_in_offsets,
+                                          const int32_t* f_in_cols, int32_t n_funcs, uint64_t n_keys, int64_t output_batch_size,
+                                          int32_t parallel, int32_t pandas_drop_na, int32_t device, int32_t n_pes, int32_t myrank,
+                                          int64_t expected_groups, void* stream, const double* fractions) {
     (void)operator_id;
     B200_TRY
     int ndev = 0;
@@ -3993,7 +4376,7 @@ void* b200_groupby_state_init(int64_t operator_id, const int8_t* build_arr_c_typ
     B200_REQUIRE(device >= 0 && device < ndev, "b200 groupby: bad device ordinal");
     return new GroupbyState(build_arr_c_types, build_arr_array_types, n_build_arrs, ftypes, f_in_offsets, f_in_cols, n_funcs,
                             n_keys, output_batch_size, parallel != 0, pandas_drop_na != 0, device, n_pes, myrank,
-                            expected_groups, (cudaStream_t)stream);
+                            expected_groups, (cudaStream_t)stream, nullptr, fractions);
     B200_CATCH(nullptr)
 }
 
@@ -4105,6 +4488,8 @@ int64_t b200_groupby_get_metric(void* state, int32_t which) {
         case 17: return s->spgd_launches;
         case 18: return s->mt.admitted;
         case 19: return s->mt.reduces;
+        case 20: { cudaSetDevice(s->device); return s->ho.on ? s->holistic_rows() : 0; }  // exact (synchronises the stream)
+        case 21: return s->ho.passes;
         case 13: { cudaSetDevice(s->device); s->read_counters(); return s->n_groups; }  // exact (synchronises the stream)
         case 100: s->profiling = true; return 0;
         default: return -1;

@@ -610,7 +610,8 @@ const uint32_t* fsort_rows(const Src& src, const SortKey* keys, const bool* may_
     return ids;
 }
 
-const uint32_t* radix_sort_columns(int n_keys, const void* const* data, const SortKey* keys, int64_t n, DevBuf (&ids)[2], cudaStream_t st) {
+const uint32_t* radix_sort_columns(int n_keys, const void* const* data, const SortKey* keys, int64_t n, DevBuf (&ids)[2], cudaStream_t st,
+                                   int64_t* passes_run) {
     B200_REQUIRE(n_keys >= 1 && n_keys <= SORT_MAX_KEYS && n <= FS_MAX_ROWS, "internal: radix_sort_columns: 1 to 4 keys, at most 2^31 rows");
     if (n == 0) return nullptr;
     FsArraySrc src{};
@@ -620,7 +621,9 @@ const uint32_t* radix_sort_columns(int n_keys, const void* const* data, const So
     B200_CUDA(cudaGetDevice(&dev));
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + FS_THREADS - 1) / FS_THREADS, (int64_t)num_sms(dev) * 8));
     int64_t run = 0, skipped = 0;
-    return fsort_rows(src, keys, may_na, n_keys, n, ids, grid, st, run, skipped);
+    const uint32_t* perm = fsort_rows(src, keys, may_na, n_keys, n, ids, grid, st, run, skipped);
+    if (passes_run) *passes_run += run;
+    return perm;
 }
 
 // ---- host state: a form consumes rows and at is_last points the output views at its sorted rows; the base checks batches,

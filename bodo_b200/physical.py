@@ -235,7 +235,8 @@ class PhysicalAggregate:
     """Groupby sink/source (aggregate.h:65-365). `aggs` = [(func_name, input_column_index or None for size)].
     mrnf = (sort_col_inds, ascending, na_last, keep_inds) with no aggs: a min_row_number_filter, one row per group, the first by
     the sort columns (streaming.groupby's mrnf_* arguments); mrnf_limit=n (forwarded to init_groupby_state with the other keywords)
-    keeps the first n rows per group."""
+    keeps the first n rows per group.  percentiles=(q, ...) (forwarded the same way) gives the fraction of every percentile_cont /
+    percentile_disc entry of aggs, in order."""
 
     def __init__(self, key_inds: Sequence[int], aggs: Sequence[tuple], dropna: bool = True, parallel: bool = False, mrnf=None, **kw):
         fnames = tuple(f for f, _ in aggs) + ((G.MRNF,) if mrnf is not None else ())
@@ -397,16 +398,39 @@ def run_pipeline(source, between: Iterable, sink) -> None:
         finished = res == OperatorResult.FINISHED
 
 
+def _percentile_aggs(aggs: Sequence[tuple], kw: dict):
+    """groupby_agg's aggs as (out_name, column, func) triples, and kw with percentiles= holding the q of every 4-tuple
+    (out_name, column, func, q) in order (forwarded by PhysicalAggregate to init_groupby_state)."""
+    triples, qs = [], []
+    for a in aggs:
+        a = tuple(a)
+        if len(a) == 4:
+            if a[2] not in G.PERCENTILES:
+                raise G._lib.B200Error(f"groupby_agg: only percentile_cont / percentile_disc take a fraction (got {a!r})")
+            qs.append(a[3])
+        elif len(a) != 3 or a[2] in G.PERCENTILES:
+            raise G._lib.B200Error(f"groupby_agg: an aggregate is (out_name, column, func), a percentile (out_name, column, func, q) "
+                                   f"(got {a!r})")
+        triples.append(a[:3])
+    if qs:
+        if kw.get("percentiles") is not None:
+            raise G._lib.B200Error("groupby_agg: give the fractions in the (out_name, column, func, q) tuples, not as percentiles=")
+        kw = dict(kw, percentiles=tuple(qs))
+    return triples, kw
+
+
 def groupby_agg(df, by, aggs: Sequence[tuple], dropna: bool = True, batch_size: int = STREAMING_BATCH_SIZE, **kw):
     """df.groupby(by, as_index=False, dropna=dropna).agg(...) through the streaming operators.
 
     aggs: [(out_name, column, func)] with func one of streaming.groupby.FTYPES: 'size', 'sum', 'count', 'nunique', 'mean', 'min',
     'max', 'prod', 'first', 'last', 'var', 'std', 'var_pop', 'std_pop', 'skew', 'kurtosis', 'boolor_agg', 'booland_agg',
-    'boolxor_agg', 'bitor_agg', 'bitand_agg', 'bitxor_agg', 'count_if' (no pandas aliases: 'any' / 'all' give False for an all-NA
-    group, where boolor_agg / booland_agg give NA).
+    'boolxor_agg', 'bitor_agg', 'bitand_agg', 'bitxor_agg', 'count_if', 'mode', 'percentile_cont', 'percentile_disc' (no pandas
+    aliases: 'any' / 'all' give False for an all-NA group, where boolor_agg / booland_agg give NA).  A percentile is the 4-tuple
+    (out_name, column, 'percentile_cont' or 'percentile_disc', q) with 0 <= q <= 1 (MEDIAN(x) is ('m', 'x', 'percentile_cont', 0.5)).
     Returns a pandas DataFrame (group order unspecified, as in the reference)."""
     by = [by] if isinstance(by, str) else list(by)
     cols = list(df.columns)
+    aggs, kw = _percentile_aggs(aggs, kw)
     used = list(by)
     for _, c, _ in aggs:
         if c is not None and c not in used:
@@ -429,6 +453,7 @@ def groupby_agg_parquet(path: str, by, aggs: Sequence[tuple], dropna: bool = Tru
     PhysicalAggregate.  Only the key and aggregated columns are decoded (column pruning, as the reference's planner does
     for ReadParquet under an aggregate).  Same `aggs` format and result shape as groupby_agg."""
     by = [by] if isinstance(by, str) else list(by)
+    aggs, kw = _percentile_aggs(aggs, kw)
     used = list(by)
     for _, c, _ in aggs:
         if c is not None and c not in used:

@@ -71,6 +71,38 @@ void* b200_groupby_state_init(int64_t operator_id, const int8_t* build_arr_c_typ
                               int32_t device, int32_t n_pes, int32_t myrank,
                               int64_t expected_groups, void* stream);
 
+/* b200_groupby_state_init with one fraction per function: the holistic aggregates mode=38, percentile_cont=39 and
+ * percentile_disc=40 (recalled enum values, not read from a reference checkout) beside any other function.
+ * b200_groupby_state_init is this entry with fractions = NULL.
+ *   fractions: n_funcs entries; entry j is the q of function j when it is percentile_cont or percentile_disc (0 <= q <= 1, not
+ *     NaN) and is ignored otherwise.  NULL is allowed when no function is a percentile.
+ *   Each of the three takes exactly one input column (a non-key column).  Per group, V is the multiset of that column's values
+ *     with NA cells (and NaN in a float column) skipped, m = |V|, and v_0 <= ... <= v_{m-1} is V in the order of the sort's key
+ *     encoding (ascending; -0.0 and 0.0 are one value).  A group with m = 0 gets NA; every output is nullable.
+ *   percentile_cont(q): h = q (m - 1), lo = floor(h), f = h - lo (float64); v_lo when f == 0, else a + (b - a) f with a = v_lo and
+ *     b = v_{lo+1} as float64, evaluated with rounded operations and no fused multiply-add (pandas' linear group_quantile;
+ *     MEDIAN(x) is q = 0.5).  Integer (uint64 included) and float columns; the output is FLOAT64.
+ *   percentile_disc(q): v_i with i = clamp(ceil(q m) - 1, 0, m - 1), q m in float64 (numpy's method="inverted_cdf").  Integer,
+ *     float, DATE, DATETIME and TIMEDELTA columns; the output has the input's type.
+ *   mode: the most frequent value of V, ties to the least value (Series.mode().iloc[0]).  Integer, float, bool, DATE, DATETIME and
+ *     TIMEDELTA columns; the output has the input's type.
+ *   A result is decoded from the value's encoding (a zero comes back as +0.0), so it depends only on V and is bit-identical across
+ *     runs, batch splits, empty batches, table growth and rank counts.
+ *   Memory: the state keeps a 4-byte group id and the value (its width) per non-NA value, one store per distinct value column,
+ *     sorted at finalize by a radix sort of at most 2^31 rows: a consume call that could take a store past 2^31 rows (or the state
+ *     past 2^32 groups) fails before it runs anything and leaves the state usable.
+ *   Such a state consumes on the direct (or multi-key) kernels only.  Sharded (parallel, n_pes > 1) it never exchanges partial
+ *     aggregates: the caller hash-partitions the rows by key before each consume call, every rank aggregates only the groups it
+ *     owns, and b200_groupby_finalize runs without an exchange (the exchange entries refuse the state).
+ *   Refused here, naming the argument: a percentile without fractions, a fraction outside [0, 1] or NaN, a function with other
+ *     than one input column, a column type the function does not take.
+ *   Metrics: 20 the values appended to the stores (exact: synchronises the stream), 21 the digit passes the finalize sorts ran. */
+void* b200_groupby_state_init_percentiles(int64_t operator_id, const int8_t* build_arr_c_types, const int8_t* build_arr_array_types,
+                                          int32_t n_build_arrs, const int32_t* ftypes, const int32_t* f_in_offsets,
+                                          const int32_t* f_in_cols, int32_t n_funcs, uint64_t n_keys, int64_t output_batch_size,
+                                          int32_t parallel, int32_t pandas_drop_na, int32_t device, int32_t n_pes, int32_t myrank,
+                                          int64_t expected_groups, void* stream, const double* fractions);
+
 /* groupby_state_init_py_entry (_groupby.cpp:4917-4970) with its MRNF arguments (sort_asc / sort_na / n_sort_keys / cols_to_keep):
  * a min_row_number_filter state, QUALIFY ROW_NUMBER() OVER (PARTITION BY keys ORDER BY sort columns) = 1, i.e.
  * df.sort_values(sort columns, kind="stable").drop_duplicates(keys, keep="first")[kept columns].
@@ -178,7 +210,8 @@ void b200_delete_groupby_state(void* state);
  * synchronises the state's stream), 14 SPG launches with narrow (int32 key, int32 value) bucket rows (SPG-N; included in 8),
  * 15 SPG launches with 16-byte (int64 key, int64 value) bucket rows (included in 8), 16 heavy-hitter keys admitted to the
  * partition kernel's hot table (0 when there are none or the table is disabled), 18 / 19 candidate rows admitted / store reduces
- * of a b200_groupby_state_init_mrnf_limit state (0 otherwise). */
+ * of a b200_groupby_state_init_mrnf_limit state (0 otherwise), 20 / 21 values appended to the stores / digit passes of the finalize
+ * sorts of a state with mode or a percentile (0 otherwise; 20 synchronises the stream). */
 /* nunique keeps one nested distinct state over (key, value) per value column (owned by `state`).  A sharded caller exchanges every
  * nested state (the exchange above + b200_groupby_finalize on the handle returned here — a key's pairs are owned where the key is
  * owned) BEFORE it exchanges and finalizes the outer state; single-GPU callers never need these. */
