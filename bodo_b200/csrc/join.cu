@@ -17,7 +17,7 @@
 // bodo/pandas/physical/join.h:267): NA joins NA.  false (the default of join_state_init_py_entry, SQL semantics): rows
 // with an NA key never match — they are filtered from the build table unless it is the outer side
 // (_join.cpp:3180 filter_na_values) and only survive as NULL-extended rows of an outer join.
-// Keys: the first n_keys (1..4) columns of each side.  One key column can take the unique-key tables (Slot16 / Slot32); a
+// Keys: the first n_keys (1..4) columns of each side; n_keys 0 is the nested-loop join (probe_nested, no table).  One key column can take the unique-key tables (Slot16 / Slot32); a
 // multi-column key always takes the CSR form, whose key table holds (tuple-hash tag, first build row) words (the _mk kernels).
 #include <algorithm>
 #include <cmath>
@@ -978,6 +978,179 @@ __global__ void join_asof_groups_kernel(const uint32_t* ids, int64_t n, const As
     }
 }
 
+// ---- nested-loop join: no equi-join key (the reference's NestedLoopJoinState, bodo/libs/streaming/_nested_loop_join.cpp) ----
+// Every (probe row, build row) pair is a candidate.  Output order is fixed: probe rows in batch order, each probe row's pairs in
+// build arrival order, a NULL-extended / anti / mark row in its probe row's place; a build-outer tail follows the last probe call.
+// With a condition, the work is a 2-D grid of probe tiles (NLJ_TILE_P rows: one warp per probe row at a time, NLJ_ROWS_PER_WARP
+// rows per warp) × build chunks (a multiple of NLJ_SUB rows).  The lanes of a warp take 32 consecutive build rows, so the
+// interpreter's control flow and the probe cells are warp-uniform; the build columns the program reads are staged per NLJ_SUB-row
+// sub-tile in shared memory (at most NLJ_MAX_STAGE columns, further ones read through L1).  Pass A writes the passing pairs of each
+// (probe row, chunk) into a count matrix n_probe × (chunks + 1), the last entry of a row being its NULL-extended / anti / mark row;
+// the Scanner turns it into output offsets and pass B writes the passing pairs at offset + running + popc(ballot & lanemask_lt).
+constexpr int NLJ_WARPS = 8, NLJ_ROWS_PER_WARP = 4, NLJ_TILE_P = NLJ_WARPS * NLJ_ROWS_PER_WARP, NLJ_SUB = 256, NLJ_MAX_STAGE = 8;
+constexpr int64_t NLJ_MAX_ROWS = 1ll << 31;  // output rows of one probe call
+struct NljArgs {
+    int64_t n_probe, n_build;
+    int64_t chunk;             // build rows per chunk (a multiple of NLJ_SUB); gridDim.y chunks
+    int n_stage;               // build columns staged in shared memory
+    int stage_col[NLJ_MAX_STAGE];
+    int8_t b_slot[J_MAX_COLS];  // build column -> its stage slot, -1: read from global memory
+};
+// Stages the NLJ_SUB build rows from s0 (up to `end`) of the staged columns: their expr_load bits, then their validity bytes.
+__device__ __forceinline__ void nlj_stage(const CondArgs& a, const NljArgs& na, int64_t s0, int64_t end, long long* sbits, uint8_t* svalid) {
+    const int64_t b = s0 + threadIdx.x;
+    if (b < end)
+        for (int s = 0; s < na.n_stage; s++) {
+            const int c = na.stage_col[s];
+            const ExprVal v = expr_load(a.b_data[c], a.b_ct[c], b, !a.b_valid[c] || a.b_valid[c][b]);
+            sbits[s * NLJ_SUB + threadIdx.x] = v.bits;
+            svalid[s * NLJ_SUB + threadIdx.x] = v.valid ? 1 : 0;
+        }
+}
+// The condition on probe row p and build row b, the j-th row of the staged sub-tile.
+__device__ __forceinline__ bool nlj_pass(const CondArgs& a, const NljArgs& na, const long long* sbits, const uint8_t* svalid, int j, int64_t p, int64_t b) {
+    const ExprVal v = expr_run(a.prog, 0, [&](int64_t arg) {
+        const int c = (int)arg;
+        if (c < J_MAX_COLS) {
+            const int s = na.b_slot[c];
+            if (s >= 0) return ExprVal{sbits[s * NLJ_SUB + j], ctype_is_float(a.b_ct[c]), svalid[s * NLJ_SUB + j] != 0, a.b_ct[c] == CT_UINT64};
+            return expr_load(a.b_data[c], a.b_ct[c], b, !a.b_valid[c] || a.b_valid[c][b]);
+        }
+        const int q = c - J_MAX_COLS;
+        return expr_load(a.p_data[q], a.p_ct[q], p, bit_valid(a.p_valid[q], p));
+    });
+    return v.valid && ev_true(v);
+}
+// condition pass A: cnt[p * (gridDim.y + 1) + chunk] = the passing pairs of probe row p in build chunk blockIdx.y.  pairs[0] += pairs
+// evaluated, pairs[1] += pairs passed (one atomic per warp).  Every pair is evaluated, for anti and mark joins too.
+__global__ void __launch_bounds__(NLJ_WARPS * 32) nlj_count_kernel(const __grid_constant__ CondArgs a, const __grid_constant__ NljArgs na, uint32_t* cnt,
+                                                                   unsigned long long* pairs) {
+    extern __shared__ long long nlj_smem[];
+    long long* sbits = nlj_smem;
+    uint8_t* svalid = (uint8_t*)(nlj_smem + na.n_stage * NLJ_SUB);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t b0 = (int64_t)blockIdx.y * na.chunk, end = min(b0 + na.chunk, na.n_build);
+    const int64_t p0 = (int64_t)blockIdx.x * NLJ_TILE_P + warp * NLJ_ROWS_PER_WARP;
+    uint32_t k[NLJ_ROWS_PER_WARP] = {};
+    unsigned long long n_eval = 0;
+    for (int64_t s0 = b0; s0 < end; s0 += NLJ_SUB) {
+        __syncthreads();
+        nlj_stage(a, na, s0, end, sbits, svalid);
+        __syncthreads();
+#pragma unroll
+        for (int r = 0; r < NLJ_ROWS_PER_WARP; r++) {
+            const int64_t p = p0 + r;
+            if (p >= na.n_probe) break;
+            for (int j = lane; j < NLJ_SUB && s0 + j - lane < end; j += 32) {
+                const int64_t b = s0 + j;
+                const bool in = b < end;
+                k[r] += __popc(__ballot_sync(0xffffffffu, in && nlj_pass(a, na, sbits, svalid, j, p, b)));
+                n_eval += in ? 1 : 0;
+            }
+        }
+    }
+    unsigned long long n_pass = 0;
+#pragma unroll
+    for (int r = 0; r < NLJ_ROWS_PER_WARP; r++) {
+        const int64_t p = p0 + r;
+        if (p < na.n_probe && lane == 0) cnt[p * (gridDim.y + 1) + blockIdx.y] = k[r];
+        n_pass += k[r];
+    }
+    for (int d = 16; d; d >>= 1) n_eval += __shfl_xor_sync(0xffffffffu, n_eval, d);
+    if (lane == 0 && n_eval) { atomicAdd(pairs, n_eval); atomicAdd(pairs + 1, n_pass); }
+}
+// After pass A, per probe row: the entry after its chunk counts, by kind.  mode 0: 1 for a probe_outer row without a passing pair;
+// 1 (anti): 1 without a passing pair, and the chunk counts zeroed; 2 (mark): 1, mark[p] = some pair passes, chunk counts zeroed.
+__global__ void nlj_rows_kernel(int64_t n, int n_chunks, uint32_t* cnt, int probe_outer, int mode, uint8_t* mark) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < n; p += stride) {
+        uint32_t* row = cnt + p * (n_chunks + 1);
+        bool any = false;
+        for (int c = 0; c < n_chunks; c++) any = any || row[c] != 0;
+        if (mode != 0)
+            for (int c = 0; c < n_chunks; c++) row[c] = 0;
+        row[n_chunks] = mode == 2 ? 1u : (!any && (mode == 1 || probe_outer)) ? 1u : 0u;
+        if (mode == 2) mark[p] = any ? 1 : 0;
+    }
+}
+// condition pass B: the passing pairs of (probe row, chunk) go to their output rows in build order (build_outer: they mark their
+// build row matched).  A block none of whose rows has output in its chunk skips it; so does a warp for each row without output.
+__global__ void __launch_bounds__(NLJ_WARPS * 32) nlj_gather_kernel(const __grid_constant__ GatherArgs g, const __grid_constant__ CondArgs a,
+                                                                    const __grid_constant__ NljArgs na) {
+    extern __shared__ long long nlj_smem[];
+    long long* sbits = nlj_smem;
+    uint8_t* svalid = (uint8_t*)(nlj_smem + na.n_stage * NLJ_SUB);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t b0 = (int64_t)blockIdx.y * na.chunk, end = min(b0 + na.chunk, na.n_build);
+    const int64_t p0 = (int64_t)blockIdx.x * NLJ_TILE_P + warp * NLJ_ROWS_PER_WARP;
+    unsigned long long o[NLJ_ROWS_PER_WARP];
+    bool need[NLJ_ROWS_PER_WARP], any = false;
+#pragma unroll
+    for (int r = 0; r < NLJ_ROWS_PER_WARP; r++) {
+        const int64_t p = p0 + r, e = p * (gridDim.y + 1) + blockIdx.y;
+        need[r] = p < na.n_probe && g.poff[e + 1] != g.poff[e];
+        o[r] = need[r] ? g.poff[e] : 0;
+        any = any || need[r];
+    }
+    if (!__syncthreads_or(any)) return;
+    const unsigned lt = (1u << lane) - 1;
+    for (int64_t s0 = b0; s0 < end; s0 += NLJ_SUB) {
+        __syncthreads();
+        nlj_stage(a, na, s0, end, sbits, svalid);
+        __syncthreads();
+#pragma unroll
+        for (int r = 0; r < NLJ_ROWS_PER_WARP; r++) {
+            if (!need[r]) continue;
+            const int64_t p = p0 + r;
+            for (int j = lane; j < NLJ_SUB && s0 + j - lane < end; j += 32) {
+                const int64_t b = s0 + j;
+                const bool ok = b < end && nlj_pass(a, na, sbits, svalid, j, p, b);
+                const unsigned m = __ballot_sync(0xffffffffu, ok);
+                if (ok) {
+                    const int64_t orow = (int64_t)(o[r] + __popc(m & lt));
+                    if (g.bmatched) g.bmatched[b] = 1;
+                    for (int q = 0; q < g.n_b; q++) {
+                        copy_cell(g.ob_data[q], orow, g.b_data[q], b, g.b_size[q]);
+                        if (g.ob_valid[q]) g.ob_valid[q][orow] = g.b_valid[q] ? g.b_valid[q][b] : 1;
+                    }
+                    for (int q = 0; q < g.n_p; q++) {
+                        copy_cell(g.op_data[q], orow, g.p_data[q], p, g.p_size[q]);
+                        if (g.op_valid[q]) g.op_valid[q][orow] = bit_valid(g.p_valid[q], p) ? 1 : 0;
+                    }
+                }
+                o[r] += __popc(m);
+            }
+        }
+    }
+}
+// The one-row entries: probe row p goes out NULL-extended (or as an anti / mark row, whose build columns are NULL or absent) at
+// g.poff[p * (n_chunks + 1) + n_chunks] when that entry is 1; without offsets (g.poff nullptr) every probe row goes out at row p.
+__global__ void nlj_probe_rows_kernel(const __grid_constant__ GatherArgs g, int n_chunks) {
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < g.n_probe; p += stride) {
+        if (!g.poff) { asof_emit(g, p, p, J_NONE); continue; }
+        const int64_t e = p * (n_chunks + 1) + n_chunks;
+        if (g.poff[e + 1] != g.poff[e]) asof_emit(g, (int64_t)g.poff[e], p, J_NONE);
+    }
+}
+// Cross join (no condition): output row o = (probe row o / n_build, build row o % n_build), o < rows <= NLJ_MAX_ROWS, so the
+// index arithmetic is 32-bit.  Consecutive threads write consecutive output rows and read consecutive build rows; the probe cell
+// of a run of n_build rows is one broadcast load.
+__global__ void __launch_bounds__(256) nlj_cross_kernel(const __grid_constant__ GatherArgs g, uint32_t n_build, uint32_t rows) {
+    const uint32_t stride = gridDim.x * blockDim.x;
+    for (uint32_t o = blockIdx.x * blockDim.x + threadIdx.x; o < rows; o += stride) {
+        const uint32_t p = o / n_build, b = o - p * n_build;
+        for (int q = 0; q < g.n_b; q++) {
+            copy_cell(g.ob_data[q], o, g.b_data[q], b, g.b_size[q]);
+            if (g.ob_valid[q]) g.ob_valid[q][o] = g.b_valid[q] ? g.b_valid[q][b] : 1;
+        }
+        for (int q = 0; q < g.n_p; q++) {
+            copy_cell(g.op_data[q], o, g.p_data[q], p, g.p_size[q]);
+            if (g.op_valid[q]) g.op_valid[q][o] = bit_valid(g.p_valid[q], p) ? 1 : 0;
+        }
+    }
+}
+
 // ================================================================================================
 // When `buf` holds fewer than `need` bytes, replaces it by a buffer of max(need, alloc) bytes that keeps its first `keep` bytes.
 static void grow_keep(DevBuf& buf, size_t need, size_t keep, cudaStream_t st, size_t alloc = 0) {
@@ -1071,7 +1244,7 @@ class JoinState {
     JoinState(const int8_t* bct, const int8_t* bat, int nb, const int8_t* pct, const int8_t* pat, int np, uint64_t nk,
               bool bo, bool po, bool na_eq, int64_t obs, int dev, int64_t expected_build_rows, cudaStream_t st)
         : device(dev), stream(st), n_b(nb), n_p(0), build_outer(bo), probe_outer(po), na_equal(na_eq), output_batch_size(obs) {
-        B200_REQUIRE(nk >= 1 && nk <= MAX_HASH_KEYS, "b200 join: between 1 and 4 key columns (n_keys) per side");
+        B200_REQUIRE(nk <= MAX_HASH_KEYS, "b200 join: between 0 (a nested-loop join) and 4 key columns (n_keys) per side");
         n_keys = (int)nk;
         for (int j = 0; j < 2 * MAX_HASH_KEYS; j++) key_bounds[j] = j % 2 ? INT64_MIN : INT64_MAX;
         B200_REQUIRE(nb >= 1 && np >= 0 && nb <= J_MAX_COLS && np <= J_MAX_COLS, "b200 join: between 1 and 32 columns per side");
@@ -1095,7 +1268,7 @@ class JoinState {
         for (int c = 0; c < np; c++) B200_REQUIRE(ctype_size(p_ct[c]) > 0, "b200 join: unsupported probe column dtype");
         B200_REQUIRE(np >= n_keys, "b200 join: fewer columns than key columns");
         for (int j = 0; j < n_keys; j++) require_key_type(j, p_ct[j], "probe");
-        B200_REQUIRE(ctype_size(b_ct[0]) == ctype_size(p_ct[0]), "b200 join: build and probe key widths differ");
+        if (n_keys > 0) B200_REQUIRE(ctype_size(b_ct[0]) == ctype_size(p_ct[0]), "b200 join: build and probe key widths differ");
         key_reject = 0;
         for (int j = 0; j < n_keys; j++) key_reject |= signedness_differs(p_ct[j], b_ct[j]) ? 1u << j : 0u;
         if (asof) check_asof_probe();
@@ -1177,6 +1350,7 @@ class JoinState {
     void set_asof(int b_on, int p_on, int dir, bool exact, bool has_tol, long long tol_i, double tol_f) {
         const std::string who = "b200 join: set_asof: ";
         B200_REQUIRE(n_build == 0 && !build_final, who + "the as-of join must be set before the first build batch");
+        B200_REQUIRE(n_keys > 0, who + "a nested-loop join (n_keys 0) has no as-of form; give one constant key column per side");
         B200_REQUIRE(!build_outer, who + "a build-outer as-of join is not supported");
         B200_REQUIRE(!mark && !anti && cond.empty(), who + "an as-of join is not a mark, anti or condition join");
         B200_REQUIRE(dir >= ASOF_BACKWARD && dir <= ASOF_NEAREST, who + "direction is 0 (backward), 1 (forward) or 2 (nearest)");
@@ -1218,6 +1392,7 @@ class JoinState {
     // pass the same value.  Also computes the min / max of the (non-NA) build keys, per key column.
     void build_filter(uint64_t n_blocks) {
         B200_REQUIRE(build_final, "b200 join: runtime filter before the build side was finished");
+        B200_REQUIRE(n_keys > 0, "b200 join: a nested-loop join (n_keys 0) has no key to build a runtime filter from");
         B200_CUDA(cudaSetDevice(device)); scratch_set_stream(stream);
         bloom_blocks = n_blocks ? n_blocks : (uint64_t)n_build / 32 + 1;
         d_bloom.alloc(bloom_blocks * 32);
@@ -1240,6 +1415,7 @@ class JoinState {
     // key_cols[j] < 0: key column j is absent from `t`; the bounds then apply to the present columns and the bloom filter only when
     // every column is present.  With no key column present every row is kept.
     void runtime_filter(const b200_table* t, const int32_t* key_cols, int nk, const int32_t* use_minmax, bool use_bloom, uint8_t* keep) {
+        B200_REQUIRE(n_keys > 0, "b200 join: runtime_filter_n: a nested-loop join (n_keys 0) has no key to filter probe rows by");
         B200_REQUIRE(nk == n_keys, "b200 join: runtime_filter_n: n_keys is " + std::to_string(nk) + " and this join has " + std::to_string(n_keys) + " key columns");
         B200_REQUIRE(t->device == device, "b200 join: runtime_filter takes a device-resident table on the state's device");
         KeySet pk{};
@@ -1372,6 +1548,10 @@ class JoinState {
     }
 
     void finalize_build() {
+        if (n_keys == 0) {  // a nested-loop join probes the build store itself: no hash table, bloom filter or CSR
+            finish_build();
+            return;
+        }
         cap = 1024;
         while (cap < 2ull * (uint64_t)n_build) cap <<= 1;
         uint64_t n_slots = cap + 2;
@@ -1421,6 +1601,10 @@ class JoinState {
                 d_tkeys.release(); d_info.release();  // the general-path table is not needed any more
             }
         }
+        finish_build();
+    }
+    // what every table form needs before the first probe: the condition's pair counters, the build-outer matched flags
+    void finish_build() {
         if (!cond.empty()) {
             d_cond_pairs.alloc(16);
             B200_CUDA(cudaMemsetAsync(d_cond_pairs.p, 0, 16, stream));
@@ -1586,6 +1770,135 @@ class JoinState {
         return (int64_t)rows;
     }
 
+    // the condition program and the columns it may read: the build store and probe batch `data` / `valid`
+    CondArgs cond_args(const std::vector<const void*>& data, const std::vector<const uint8_t*>& valid) const {
+        CondArgs ca{};
+        std::copy(cond.begin(), cond.end(), ca.prog);
+        for (int c = 0; c < n_b; c++) { ca.b_data[c] = bcol[c].buf.p; ca.b_valid[c] = build_valid(c); ca.b_ct[c] = b_ct[c]; }
+        for (int c = 0; c < n_p; c++) { ca.p_data[c] = data[c]; ca.p_valid[c] = valid[c]; ca.p_ct[c] = p_ct[c]; }
+        return ca;
+    }
+
+    // ---- nested-loop join (n_keys 0) ----
+    // The condition kernels' grid for a batch of n probe rows: build chunks of a multiple of NLJ_SUB rows, enough of them that the
+    // probe tiles × chunks fill the GPU about NLJ_BLOCKS_PER_SM times over, so a probe batch of a few rows still spreads over every
+    // SM; a large batch gets one chunk and a count matrix of 2 n entries.  The build columns the condition reads are staged.
+    static constexpr int NLJ_BLOCKS_PER_SM = 8;
+    NljArgs nlj_args(int64_t n) const {
+        NljArgs na{};
+        na.n_probe = n; na.n_build = n_build;
+        if (n > 0 && n_build > 0) {
+            const int64_t tiles = (n + NLJ_TILE_P - 1) / NLJ_TILE_P, subs = (n_build + NLJ_SUB - 1) / NLJ_SUB;
+            const int64_t chunks = std::min(std::max<int64_t>(1, ((int64_t)sms * NLJ_BLOCKS_PER_SM + tiles - 1) / tiles), subs);
+            na.chunk = (subs + chunks - 1) / chunks * NLJ_SUB;
+        }
+        std::fill(na.b_slot, na.b_slot + J_MAX_COLS, (int8_t)-1);
+        for (const ExprInstr& in : cond)
+            if (in.op == EX_COL && in.arg < J_MAX_COLS && na.b_slot[in.arg] < 0 && na.n_stage < NLJ_MAX_STAGE) {
+                na.b_slot[in.arg] = (int8_t)na.n_stage;
+                na.stage_col[na.n_stage++] = (int)in.arg;
+            }
+        return na;
+    }
+    static std::string nlj_too_many(unsigned long long rows, const std::string& how) {
+        return "b200 join: this nested-loop probe call would produce " + std::to_string(rows) + " output rows (" + how +
+               "); one probe call produces at most 2^31 rows: feed smaller probe batches";
+    }
+    // Every (probe row, build row) pair is a candidate.  Rows go out in probe order, each probe row's pairs in build arrival order, a
+    // NULL-extended / anti / mark row in its probe row's place; the build-outer tail follows the last probe call.
+    int64_t probe_nested(int64_t n, const std::vector<OutCol>& cols, int nkb, const std::vector<const void*>& data,
+                         const std::vector<const uint8_t*>& valid, bool is_last) {
+        const int mode = anti ? 1 : (mark ? 2 : 0);
+        if (mark && n > 0) { d_mark.ensure((size_t)n + 32); d_mark_valid.ensure((size_t)(n + 7) / 8 + 32); B200_CUDA(cudaMemsetAsync(d_mark_valid.p, 0xff, (size_t)(n + 7) / 8 + 8, stream)); }
+        int64_t rows = 0;
+        if (cond.empty()) {
+            // the counts are arithmetic: n × n_build pairs (inner / outer kinds), or one row per probe row: every one for a mark join,
+            // every one for an anti join against an empty build side and for a left / full join that NULL-extends them
+            const bool cross = mode == 0 && n_build > 0;
+            if (cross) {
+                B200_REQUIRE(n <= NLJ_MAX_ROWS / n_build, nlj_too_many((unsigned long long)n * (unsigned long long)n_build,
+                                                                       std::to_string(n) + " probe rows x " + std::to_string(n_build) + " build rows"));
+                rows = n * n_build;
+            } else if (mode == 2 || (n_build == 0 && (mode == 1 || probe_outer))) {
+                rows = n;
+            }
+            size_outputs(cols, rows);
+            GatherArgs g = gather_args(n, cols, nkb, data, valid);
+            g.poff = nullptr;
+            if (rows > 0) {
+                if (cross) nlj_cross_kernel<<<grid_for(rows), 256, 0, stream>>>(g, (uint32_t)n_build, (uint32_t)rows);
+                else nlj_probe_rows_kernel<<<grid_for(n), 256, 0, stream>>>(g, 0);
+                launches++;
+            }
+            if (mark && n > 0) B200_CUDA(cudaMemsetAsync(d_mark.p, n_build > 0 ? 1 : 0, (size_t)n, stream));
+            if (build_outer && n > 0 && n_build > 0) B200_CUDA(cudaMemsetAsync(d_bmatched.p, 1, (size_t)n_build, stream));  // every pair joins
+        } else {
+            const NljArgs na = nlj_args(n);
+            const CondArgs ca = cond_args(data, valid);
+            const int chunks = na.chunk ? (int)((n_build + na.chunk - 1) / na.chunk) : 0;
+            const int64_t entries = n * (chunks + 1);
+            const dim3 grid((unsigned)((n + NLJ_TILE_P - 1) / NLJ_TILE_P), (unsigned)chunks);
+            const size_t smem = (size_t)na.n_stage * NLJ_SUB * 9;  // bits (8 B), then validity (1 B), per staged column and row
+            d_pcnt.ensure((size_t)(entries + 1) * 4); d_poff.ensure((size_t)(entries + 2) * 8);
+            if (n > 0) {
+                if (chunks > 0) {
+                    nlj_count_kernel<<<grid, NLJ_WARPS * 32, smem, stream>>>(ca, na, d_pcnt.as<uint32_t>(), d_cond_pairs.as<unsigned long long>());
+                    launches++;
+                }
+                nlj_rows_kernel<<<grid_for(n), 256, 0, stream>>>(n, chunks, d_pcnt.as<uint32_t>(), probe_outer ? 1 : 0, mode, mark ? d_mark.as<uint8_t>() : nullptr);
+                launches++;
+                B200_CUDA(cudaGetLastError());
+                B200_CUDA(cudaMemsetAsync(d_pcnt.as<uint32_t>() + entries, 0, 4, stream));
+                rows = (int64_t)scan.run(d_pcnt.as<uint32_t>(), entries + 1, d_poff.as<unsigned long long>(), stream, &launches);
+            }
+            B200_REQUIRE(rows <= NLJ_MAX_ROWS, nlj_too_many((unsigned long long)rows, "pairs that pass the condition"));
+            size_outputs(cols, rows);
+            const GatherArgs g = gather_args(n, cols, nkb, data, valid);
+            if (rows > 0) {
+                if (mode == 0 && chunks > 0) { nlj_gather_kernel<<<grid, NLJ_WARPS * 32, smem, stream>>>(g, ca, na); launches++; }
+                if (mode != 0 || probe_outer) { nlj_probe_rows_kernel<<<grid_for(n), 256, 0, stream>>>(g, chunks); launches++; }
+            }
+        }
+        B200_CUDA(cudaGetLastError());
+        return rows + emit_build_tail(cols, nkb, rows, is_last);
+    }
+
+    // The unmatched build rows of a build-outer join, with NULL probe columns, after the `n_before` rows this call has written: once,
+    // with the last probe batch (bmatched must be complete).  Returns the rows added.
+    int64_t emit_build_tail(const std::vector<OutCol>& cols, int nkb, int64_t n_before, bool is_last) {
+        if (!(is_last && build_outer && !tail_emitted && n_build > 0)) return 0;
+        DevBuf tail_flags, tail_off;
+        tail_flags.alloc((size_t)(n_build + 1) * 4); tail_off.alloc((size_t)(n_build + 2) * 8);
+        join_unmatched_flags_kernel<<<grid_for(n_build), 256, 0, stream>>>(d_bmatched.as<uint8_t>(), n_build, tail_flags.as<uint32_t>());
+        B200_CUDA(cudaMemsetAsync(tail_flags.as<uint32_t>() + n_build, 0, 4, stream));
+        launches++;
+        const unsigned long long n_tail = scan.run(tail_flags.as<uint32_t>(), n_build + 1, tail_off.as<unsigned long long>(), stream, &launches);
+        tail_emitted = true;
+        if (n_tail > 0) {
+            // the tail size is only known after the gather: grow the outputs, keeping the gathered rows
+            size_outputs(cols, n_before + (int64_t)n_tail, n_before);
+            TailArgs ta{};
+            ta.n_build = n_build; ta.flags = tail_flags.as<uint32_t>(); ta.off = tail_off.as<unsigned long long>();
+            ta.n_b = nkb; ta.n_p = (int)cols.size() - nkb;
+            for (int k = 0; k < (int)cols.size(); k++) {
+                const OutCol& c = cols[k];
+                void* od = (char*)out_data[k].p + n_before * c.size;
+                uint8_t* ov = c.nullable ? out_vbytes[k].as<uint8_t>() + n_before : nullptr;
+                if (c.is_b) {
+                    ta.b_data[k] = bcol[c.src].buf.p; ta.b_valid[k] = build_valid(c.src); ta.b_size[k] = c.size;
+                    ta.ob_data[k] = od; ta.ob_valid[k] = ov;
+                } else {
+                    const int j = k - nkb;
+                    ta.p_size[j] = c.size; ta.op_data[j] = od; ta.op_valid[j] = ov;
+                }
+            }
+            join_unmatched_emit_kernel<<<grid_for(n_build), 256, 0, stream>>>(ta);
+            launches++;
+            B200_CUDA(cudaGetLastError());
+        }
+        return (int64_t)n_tail;
+    }
+
     // general path (CSR groups: duplicate keys, outer, anti and mark joins): count + scan, then expand and gather; the unmatched
     // build rows of a build-outer join follow the last probe batch
     int64_t probe_general(int64_t n, const std::vector<OutCol>& cols, int nkb, const std::vector<const void*>& data,
@@ -1593,12 +1906,7 @@ class JoinState {
         // pass A + scan; with a condition pass A gives the slot (mode 0, no probe_outer row) and the condition count kernel the counts
         const bool has_cond = !cond.empty();
         const int mode = anti ? 1 : (mark ? 2 : 0), count_mode = has_cond ? 0 : mode, count_po = probe_outer && !has_cond ? 1 : 0;
-        CondArgs ca{};
-        if (has_cond) {
-            std::copy(cond.begin(), cond.end(), ca.prog);
-            for (int c = 0; c < n_b; c++) { ca.b_data[c] = bcol[c].buf.p; ca.b_valid[c] = build_valid(c); ca.b_ct[c] = b_ct[c]; }
-            for (int c = 0; c < n_p; c++) { ca.p_data[c] = data[c]; ca.p_valid[c] = valid[c]; ca.p_ct[c] = p_ct[c]; }
-        }
+        const CondArgs ca = has_cond ? cond_args(data, valid) : CondArgs{};
         unsigned long long n_match = 0;
         d_pslot.ensure((size_t)(n + 1) * 4); d_pcnt.ensure((size_t)(n + 1) * 4); d_poff.ensure((size_t)(n + 2) * 8);
         if (n > 0) {
@@ -1625,12 +1933,6 @@ class JoinState {
             B200_CUDA(cudaMemsetAsync(d_pcnt.as<uint32_t>() + n, 0, 4, stream));
             n_match = scan.run(d_pcnt.as<uint32_t>(), n + 1, d_poff.as<unsigned long long>(), stream, &launches);
         }
-        // unmatched build rows go out with the last probe batch
-        unsigned long long n_tail = 0;
-        DevBuf tail_flags, tail_off;
-        if (is_last && build_outer && !tail_emitted && n_build > 0) {
-            tail_flags.alloc((size_t)(n_build + 1) * 4); tail_off.alloc((size_t)(n_build + 2) * 8);
-        }
         // pass B needs bmatched complete before the tail is computed, so: gather first, then the tail
         size_outputs(cols, (int64_t)n_match);
         const GatherArgs g = gather_args(n, cols, nkb, data, valid);
@@ -1640,36 +1942,7 @@ class JoinState {
             launches++;
             B200_CUDA(cudaGetLastError());
         }
-        if (tail_flags.p) {
-            join_unmatched_flags_kernel<<<grid_for(n_build), 256, 0, stream>>>(d_bmatched.as<uint8_t>(), n_build, tail_flags.as<uint32_t>());
-            B200_CUDA(cudaMemsetAsync(tail_flags.as<uint32_t>() + n_build, 0, 4, stream));
-            launches++;
-            n_tail = scan.run(tail_flags.as<uint32_t>(), n_build + 1, tail_off.as<unsigned long long>(), stream, &launches);
-            tail_emitted = true;
-            if (n_tail > 0) {
-                // the tail size is only known after the gather: grow the outputs, keeping the gathered rows
-                size_outputs(cols, (int64_t)(n_match + n_tail), (int64_t)n_match);
-                TailArgs ta{};
-                ta.n_build = n_build; ta.flags = tail_flags.as<uint32_t>(); ta.off = tail_off.as<unsigned long long>();
-                ta.n_b = nkb; ta.n_p = (int)cols.size() - nkb;
-                for (int k = 0; k < (int)cols.size(); k++) {
-                    const OutCol& c = cols[k];
-                    void* od = (char*)out_data[k].p + n_match * c.size;
-                    uint8_t* ov = c.nullable ? out_vbytes[k].as<uint8_t>() + n_match : nullptr;
-                    if (c.is_b) {
-                        ta.b_data[k] = bcol[c.src].buf.p; ta.b_valid[k] = build_valid(c.src); ta.b_size[k] = c.size;
-                        ta.ob_data[k] = od; ta.ob_valid[k] = ov;
-                    } else {
-                        const int j = k - nkb;
-                        ta.p_size[j] = c.size; ta.op_data[j] = od; ta.op_valid[j] = ov;
-                    }
-                }
-                join_unmatched_emit_kernel<<<grid_for(n_build), 256, 0, stream>>>(ta);
-                launches++;
-                B200_CUDA(cudaGetLastError());
-            }
-        }
-        return (int64_t)(n_match + n_tail);
+        return (int64_t)n_match + emit_build_tail(cols, nkb, (int64_t)n_match, is_last);
     }
 
     int64_t probe_consume(const b200_table* t, const uint64_t* kept_b, int64_t n_kb, const uint64_t* kept_p, int64_t n_kp,
@@ -1695,6 +1968,7 @@ class JoinState {
         stage_batch(t, n_p, p_ct, data, valid);
         const std::vector<OutCol> cols = plan_out(kb, kp, valid);
         const int64_t rows = asof                     ? probe_asof(n, cols, (int)kb.size(), data, valid)
+                             : n_keys == 0            ? probe_nested(n, cols, (int)kb.size(), data, valid, is_last)
                              : form == TableForm::CSR ? probe_general(n, cols, (int)kb.size(), data, valid, is_last)
                                                       : probe_unique(n, cols, (int)kb.size(), data, valid);
         for (int k = 0; k < n_out_cols; k++)

@@ -26,8 +26,9 @@ ASOF_DIRECTIONS = {"backward": 0, "forward": 1, "nearest": 2}
 class JoinState:
     def __init__(self, operator_id, build_key_inds, probe_key_inds, build_colnames, probe_colnames, build_outer, probe_outer,
                  output_batch_size, expected_build_rows, device, stream, is_na_equal=False, build_parallel=False, probe_parallel=False,
-                 is_mark_join=False, is_anti_join=False, non_equi_condition=None, asof=None):
+                 is_mark_join=False, is_anti_join=False, non_equi_condition=None, asof=None, nested_loop=False):
         self.operator_id = int(operator_id)
+        self.nested_loop = bool(nested_loop)  # no equi-join key: every (probe row, build row) pair is a candidate (n_keys 0)
         self.is_mark_join = bool(is_mark_join)
         self.is_anti_join = bool(is_anti_join)
         self.build_key_inds = tuple(int(k) for k in build_key_inds)
@@ -43,9 +44,13 @@ class JoinState:
                 self.build_key_inds, self.probe_key_inds = (len(build_colnames),), (len(probe_colnames),)
             b_on, p_on = resolve_asof_on(on, self.build_key_inds, self.probe_key_inds, build_colnames, probe_colnames)
             self.asof = (b_on, p_on, ASOF_DIRECTIONS[direction], bool(exact), tolerance)
-        if not 1 <= len(self.build_key_inds) <= 4 or len(self.probe_key_inds) != len(self.build_key_inds):
+        if self.nested_loop:
+            if self.build_key_inds or self.probe_key_inds:
+                raise _lib.B200Error("Streaming Join: a nested-loop join has no equi-join keys")
+        elif not 1 <= len(self.build_key_inds) <= 4 or len(self.probe_key_inds) != len(self.build_key_inds):
             raise _lib.B200Error("Streaming Join: 1 to 4 equi-join keys per side, the same number on both sides "
-                                 f"(got {len(self.build_key_inds)} build and {len(self.probe_key_inds)} probe keys)")
+                                 f"(got {len(self.build_key_inds)} build and {len(self.probe_key_inds)} probe keys; a join without keys is "
+                                 "init_nested_loop_join_state)")
         self.build_colnames = list(build_colnames) if build_colnames is not None else None
         self.probe_colnames = list(probe_colnames) if probe_colnames is not None else None
         self.build_outer = bool(build_outer)
@@ -241,7 +246,7 @@ def init_join_state(operator_id, build_key_inds, probe_key_inds, build_colnames,
     condition is valid and true (b200_filter_project's semantics: NA and NaN cells are NA, arithmetic and comparisons propagate
     NA, `&` / `|` are Kleene, DATE is days and DATETIME nanoseconds); the outer, anti and mark kinds then apply to the pairs that
     pass.  The condition may read any column, also one used_cols drops, and adds no output column.  At least one equi-join key
-    is required: a condition-only (nested-loop) join is not supported.
+    is required here: a join on a condition alone is init_nested_loop_join_state.
 
     `is_na_equal` is HashJoinState's option: False is what this door constructs in the reference (join_state_init_py_entry,
     _join.cpp:4087-4136: NA keys never match); the pandas door (bodo/pandas/physical/join.h:267, here PhysicalJoin / merge)
@@ -281,7 +286,7 @@ def init_join_state(operator_id, build_key_inds, probe_key_inds, build_colnames,
         asof = (g(asof_on), asof_direction, asof_allow_exact_matches, asof_tolerance)
     if non_equi_condition is not None and (len(tuple(g(build_key_inds))) == 0 or len(tuple(g(probe_key_inds))) == 0):
         raise _lib.B200Error("Streaming Join: a non_equi_condition without an equi-join key (a nested-loop join) is not supported by "
-                             "bodo_b200; give at least one key column per side")
+                             "init_join_state; use init_nested_loop_join_state")
     if build_parallel or probe_parallel:
         from .dist_join import DistJoinState
 
@@ -292,6 +297,42 @@ def init_join_state(operator_id, build_key_inds, probe_key_inds, build_colnames,
     return JoinState(operator_id, g(build_key_inds), g(probe_key_inds), g(build_colnames), g(probe_colnames), build_outer,
                      probe_outer, output_batch_size, expected_build_rows, device, stream, is_na_equal=is_na_equal,
                      is_mark_join=is_mark_join, is_anti_join=is_anti_join, non_equi_condition=non_equi_condition, asof=asof)
+
+
+def init_nested_loop_join_state(operator_id, build_colnames, probe_colnames, build_outer, probe_outer, non_equi_condition=None,
+                                build_parallel=False, probe_parallel=False, *, is_mark_join=False, is_anti_join=False,
+                                output_batch_size=32768, expected_build_rows=0, device=None, stream=0, asof_on=None,
+                                interval_build_columns=None) -> JoinState:
+    """A join without an equi-join key (the reference's NestedLoopJoinState, bodo/libs/streaming/_nested_loop_join.cpp): every
+    (probe row, build row) pair is a candidate.  Without `non_equi_condition` every pair joins: a cross join (SQL CROSS JOIN, pandas
+    how="cross").  With one (an Expr over build_col(name) / probe_col(name), as in init_join_state) the pairs whose condition is
+    valid and true join: band, range and threshold joins, `LEFT JOIN ... ON <inequality>`.  build_outer / probe_outer make the
+    right / left / full outer joins; is_anti_join keeps the probe rows without a passing pair (NOT EXISTS), is_mark_join emits
+    every probe row with a trailing boolean "has a passing pair" column (EXISTS).
+
+    The returned JoinState is driven by join_build_consume_batch / join_probe_consume_batch / delete_join_state / get_metric like a
+    hash join's (used_cols included).  Output order is guaranteed: within a probe call, rows follow the probe rows, and a probe
+    row's pairs follow the build arrival order (batch order, then row order); a NULL-extended, anti or mark row sits in its probe
+    row's place; the unmatched build rows of a right / full join follow the last probe call, in build order.  A cross join
+    therefore equals pandas' left.merge(right, how="cross") row for row (probe = left).  One probe call produces at most 2^31
+    rows; a bigger one raises B200Error before anything is allocated for the output: feed smaller probe batches.  Metrics 8 / 9
+    count the pairs evaluated and passed (0 without a condition).  Not sharded (build_parallel / probe_parallel), not as-of, not an
+    interval join, and mark / anti joins do not emit build rows (build_outer must be False)."""
+    if build_parallel or probe_parallel:
+        raise _lib.B200Error("Streaming Join: a sharded nested-loop join is not supported (build_parallel / probe_parallel)")
+    if asof_on is not None:
+        raise _lib.B200Error("Streaming Join: a nested-loop join has no as-of form (asof_on); init_join_state runs an as-of join "
+                             "without keys")
+    if interval_build_columns not in (None, (), []):
+        raise _lib.B200Error("Streaming Join: interval joins (interval_build_columns) are not supported by bodo_b200")
+    if is_mark_join and is_anti_join:
+        raise _lib.B200Error("Streaming Join: a join is a mark join or an anti join, not both")
+    if (is_mark_join or is_anti_join) and build_outer:
+        raise _lib.B200Error("Streaming Join: mark / anti joins do not emit build rows (build_outer must be False)")
+    g = lambda x: getattr(x, "meta", x)
+    return JoinState(operator_id, (), (), g(build_colnames), g(probe_colnames), build_outer, probe_outer, output_batch_size,
+                     expected_build_rows, device, stream, is_mark_join=is_mark_join, is_anti_join=is_anti_join,
+                     non_equi_condition=non_equi_condition, nested_loop=True)
 
 
 def join_build_consume_batch(join_state: JoinState, table: Table, is_last: bool):
