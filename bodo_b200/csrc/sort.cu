@@ -205,8 +205,25 @@ __global__ void __launch_bounds__(TK_SORT_THREADS) topk_block_sort_kernel(const 
     for (int i = threadIdx.x; i < keep; i += TK_SORT_THREADS) out[o + i] = v[i];
 }
 
-// One merge pass: runs of width w at offsets 2pw and 2pw + w become one run of width 2w (cut to K rows).  Each thread finds the
-// start of its TK_MERGE_ITEMS outputs on the merge path by binary search, then merges them sequentially.
+// Outputs [d0, min(d0 + ITEMS, m)) of the merge of two sorted runs of row ids, A(i) for i < la and B(j) for j < lb, go to out[d0 ..].
+// The thread finds where its outputs start on the merge path by binary search, then merges them sequentially.  b_first(b, a):
+// row b sorts strictly before row a; a row of A that ties a row of B comes first.
+template <int ITEMS, typename RunA, typename RunB, typename BFirst>
+__device__ __forceinline__ void merge_path_items(RunA A, int64_t la, RunB B, int64_t lb, int64_t d0, int64_t m, uint32_t* __restrict__ out,
+                                                 BFirst b_first) {
+    int64_t lo = d0 - lb > 0 ? d0 - lb : 0, hi = d0 < la ? d0 : la;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (b_first(B(d0 - mid - 1), A(mid))) hi = mid; else lo = mid + 1;
+    }
+    int64_t i = lo, j = d0 - lo;
+    for (int t = 0; t < ITEMS && d0 + t < m; t++) {
+        const bool take_a = j >= lb || (i < la && !b_first(B(j), A(i)));
+        out[d0 + t] = take_a ? A(i++) : B(j++);
+    }
+}
+
+// One merge pass: runs of width w at offsets 2pw and 2pw + w become one run of width 2w (cut to K rows).
 __global__ void topk_merge_kernel(const TkStore s, int nk, int64_t n, int64_t K, int64_t w, int64_t chunks_per_pair, int64_t n_pairs,
                                   const uint32_t* __restrict__ in, uint32_t* __restrict__ out) {
     const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -218,16 +235,8 @@ __global__ void topk_merge_kernel(const TkStore s, int nk, int64_t n, int64_t K,
     if (d0 >= m) return;
     const uint32_t* A = in + ao;
     const uint32_t* B = in + bo;
-    int64_t lo = d0 - lb > 0 ? d0 - lb : 0, hi = d0 < la ? d0 : la;
-    while (lo < hi) {
-        const int64_t mid = (lo + hi) >> 1;
-        if (tk_less(s, nk, B[d0 - mid - 1], A[mid])) hi = mid; else lo = mid + 1;
-    }
-    int64_t i = lo, j = d0 - lo;
-    for (int t = 0; t < TK_MERGE_ITEMS && d0 + t < m; t++) {
-        const bool take_a = j >= lb || (i < la && tk_less(s, nk, A[i], B[j]));
-        out[ao + d0 + t] = take_a ? A[i++] : B[j++];
-    }
+    merge_path_items<TK_MERGE_ITEMS>([&](int64_t i) { return A[i]; }, la, [&](int64_t j) { return B[j]; }, lb, d0, m, out + ao,
+                                     [&](uint32_t b, uint32_t a) { return tk_less(s, nk, b, a); });
 }
 
 // dst row i = src row perm[i] for i < m; the K-th row becomes the cutoff; the store count becomes m.
@@ -527,6 +536,115 @@ __global__ void __launch_bounds__(256) fsort_gather_kernel(const __grid_constant
             if (a.lay.voff[c] >= 0) a.out_vb[c][i] = (uint8_t)chunk[a.lay.voff[c] + off];
         }
     }
+}
+
+// ---- the full sort's sharded form (streaming/sort.py init_sharded_sort_state): every rank sorts its rows, samples them, counts
+// the rows below the chosen splitters and sends each rank its slice; the receiver's store holds the runs it got, one per source
+// rank, back to back, and merges them instead of sorting ----
+//
+//   fsort_sample_kernel       sample i of a finished sort is its output row q_i = floor(i n / s): per key (NA class, radix word),
+//                             then (rank, q_i), one uint64 each.
+//   fsort_count_below_kernel  per splitter (a sample record) the number of output rows whose (key, rank, row) tuple is below it,
+//                             by binary search over the sorted rows.
+//   fsort_merge_kernel        one pairwise merge-path round over runs of row ids (merge_path_items, as the top-k's reduce);
+//                             ceil(log2 P) rounds merge P runs.  Key words are read through FsChunkSrc; two rows that tie on
+//                             every key keep their store order, which is (source rank, position).
+constexpr int FS_MERGE_ITEMS = 16;
+
+// The key columns of a finished state's output: rows [0, n) of key j at data[j], its validity bitmap at bitmap[j] (nullptr: none).
+struct FsOutKeys {
+    int nk;
+    int64_t n, rank;
+    SortKey key[SORT_MAX_KEYS];
+    const void* data[SORT_MAX_KEYS];
+    const uint8_t* bitmap[SORT_MAX_KEYS];
+    __device__ __forceinline__ uint64_t word(int j, int64_t q, uint32_t& cls) const {
+        bool na = !bit_valid(bitmap[j], q);
+        const uint64_t w = sort_word(key[j], load_bits(data[j], key[j].size, q), na);
+        cls = sort_class(key[j], na);
+        return w;
+    }
+};
+
+__global__ void fsort_sample_kernel(const __grid_constant__ FsOutKeys a, int64_t s, uint64_t* __restrict__ rec) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= s) return;
+    const int64_t q = i * a.n / s;  // i n < 2^31 * 2^31
+    uint64_t* r = rec + i * (2 * a.nk + 2);
+    for (int j = 0; j < a.nk; j++) {
+        uint32_t cls;
+        r[2 * j + 1] = a.word(j, q, cls);
+        r[2 * j] = cls;
+    }
+    r[2 * a.nk] = (uint64_t)a.rank;
+    r[2 * a.nk + 1] = (uint64_t)q;
+}
+
+__global__ void fsort_count_below_kernel(const __grid_constant__ FsOutKeys a, const uint64_t* __restrict__ spl, int64_t n_spl,
+                                         int64_t* __restrict__ counts) {
+    const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n_spl) return;
+    const uint64_t* t = spl + k * (2 * a.nk + 2);
+    // row q is below the splitter: rows are sorted, so this holds for a prefix of [0, n)
+    auto below = [&](int64_t q) {
+        for (int j = 0; j < a.nk; j++) {
+            uint32_t cls;
+            const uint64_t w = a.word(j, q, cls);
+            if (cls != t[2 * j]) return cls < t[2 * j];
+            if (w != t[2 * j + 1]) return w < t[2 * j + 1];
+        }
+        if ((uint64_t)a.rank != t[2 * a.nk]) return (uint64_t)a.rank < t[2 * a.nk];
+        return (uint64_t)q < t[2 * a.nk + 1];
+    };
+    int64_t lo = 0, hi = a.n;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (below(mid)) lo = mid + 1; else hi = mid;
+    }
+    counts[k] = lo;
+}
+
+// Two adjacent runs of one merge round: A is rows [off, off + la) of the round's input, B the lb rows after it; they become rows
+// [off, off + la + lb) of its output, handled by threads chunk0 .. chunk0 + ceil((la + lb) / FS_MERGE_ITEMS) - 1.
+struct FsMergePair { int64_t off, la, lb, chunk0; };
+
+struct FsMergeArgs {
+    int nk;
+    SortKey key[SORT_MAX_KEYS];
+    FsChunkSrc src;
+    const FsMergePair* pair;
+    int64_t n_pairs, n_chunks;
+    const uint32_t* in;  // nullptr: the identity (the first round reads the store order)
+    uint32_t* out;
+};
+
+__global__ void __launch_bounds__(256) fsort_merge_kernel(const __grid_constant__ FsMergeArgs a) {
+    const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= a.n_chunks) return;
+    int64_t lo = 0, hi = a.n_pairs - 1;  // the last pair whose first chunk is <= c: a pair without rows owns no chunk
+    while (lo < hi) {
+        const int64_t mid = (lo + hi + 1) >> 1;
+        if (a.pair[mid].chunk0 <= c) lo = mid; else hi = mid - 1;
+    }
+    const FsMergePair p = a.pair[lo];
+    const int64_t d0 = (c - p.chunk0) * FS_MERGE_ITEMS, bo = p.off + p.la;
+    const uint32_t* in = a.in;
+    auto A = [&](int64_t i) { return in ? in[p.off + i] : (uint32_t)(p.off + i); };
+    auto B = [&](int64_t j) { return in ? in[bo + j] : (uint32_t)(bo + j); };
+    auto b_first = [&](uint32_t b, uint32_t x) {
+#pragma unroll
+        for (int j = 0; j < SORT_MAX_KEYS; j++) {
+            if (j < a.nk) {
+                bool nb, nx;
+                const uint64_t wb = a.src.word(a.key[j], j, b, nb), wx = a.src.word(a.key[j], j, x, nx);
+                const uint32_t cb = sort_class(a.key[j], nb), cx = sort_class(a.key[j], nx);
+                if (cb != cx) return cb < cx;
+                if (wb != wx) return wb < wx;
+            }
+        }
+        return false;
+    };
+    merge_path_items<FS_MERGE_ITEMS>(A, p.la, B, p.lb, d0, p.la + p.lb, a.out + p.off, b_first);
 }
 
 static_assert(FS_THREADS == 256, "fsort_pass_kernel: one thread per digit");
@@ -890,25 +1008,29 @@ struct FullSortState : SortState {
         }
     }
 
-    // Digit histograms, the pass plan, the digit passes and the gather into the output store (out_mem; the validity bytes of
-    // nullable column c go to vbytes[c]).  Chunks, pair buffers and look-back words are freed on return.
+    FsChunkSrc key_src(const FsChunks& ch) const {
+        FsChunkSrc src{};
+        src.ch = ch;
+        for (int j = 0; j < sc.n_keys; j++) { src.coff[j] = lay.coff[j]; src.voff[j] = lay.voff[j]; }
+        return src;
+    }
+
+    // The sorted order of the n > 0 stored rows: the digit histograms, the pass plan and the digit passes.  Returns the
+    // permutation in ibuf (bit 31 of an entry is not part of the row id), or nullptr for the identity.
+    virtual const uint32_t* sorted_ids(const FsChunks& ch, int64_t n, DevBuf (&ibuf)[2]) {
+        bool may_na[SORT_MAX_KEYS] = {};
+        for (int j = 0; j < sc.n_keys; j++) may_na[j] = arr_type[j] == ARR_NULLABLE || ctype_is_float(sc.ctype[j]);
+        return fsort_rows(key_src(ch), sc.key, may_na, sc.n_keys, n, ibuf, grid_for(n, FS_THREADS), stream, passes_run, passes_skipped);
+    }
+
+    // The sorted order, then the gather into the output store (out_mem; the validity bytes of nullable column c go to vbytes[c]).
+    // Chunks, pair buffers and look-back words are freed on return.
     void finish_rows(std::vector<DevBuf>& vbytes) override {
         const int64_t n = rows_consumed;
-        const int nk = sc.n_keys;
         FsChunks ch{};
         for (size_t k = 0; k < chunks.size(); k++) ch.p[k] = chunks[k].as<char>();
         DevBuf ibuf[2];
-        const uint32_t* ids = nullptr;  // the permutation; nullptr: identity
-        if (n > 0) {
-            FsChunkSrc src{};
-            src.ch = ch;
-            bool may_na[SORT_MAX_KEYS] = {};
-            for (int j = 0; j < nk; j++) {
-                src.coff[j] = lay.coff[j]; src.voff[j] = lay.voff[j];
-                may_na[j] = arr_type[j] == ARR_NULLABLE || ctype_is_float(sc.ctype[j]);
-            }
-            ids = fsort_rows(src, sc.key, may_na, nk, n, ibuf, grid_for(n, FS_THREADS), stream, passes_run, passes_skipped);
-        }
+        const uint32_t* ids = n > 0 ? sorted_ids(ch, n, ibuf) : nullptr;  // the permutation; nullptr: identity
         FsGatherArgs ga{};
         ga.n = n; ga.ids = ids; ga.lay = lay; ga.ch = ch;
         out_mem.resize(sc.n_cols);
@@ -926,6 +1048,103 @@ struct FullSortState : SortState {
     int64_t metric(int which) const override {
         const int64_t m[10] = {rows_consumed, 0, 0, 0, 0, 0, n_chunks * FS_CHUNK, passes_run, passes_skipped, 0};
         return m[which];
+    }
+
+    // The sorted key columns of a finished state, tagged with the caller's rank.
+    FsOutKeys out_keys(int64_t rank) const {
+        FsOutKeys k{};
+        k.nk = sc.n_keys; k.n = n_out; k.rank = rank;
+        for (int j = 0; j < sc.n_keys; j++) { k.key[j] = sc.key[j]; k.data[j] = out_data[j]; k.bitmap[j] = (const uint8_t*)out_bitmap[j]; }
+        return k;
+    }
+
+    // s sample records of the sorted rows (fsort_sample_kernel) into rec (host, s (2 n_keys + 2) words).
+    void sample(int64_t s, int64_t rank, uint64_t* rec) {
+        B200_REQUIRE(finished, "b200 sort: samples are taken after the last batch was consumed");
+        B200_REQUIRE(s >= 0 && s <= n_out && rec, "b200 sort: 0 <= samples <= rows, and a record buffer");
+        if (s == 0) return;
+        B200_CUDA(cudaSetDevice(device));
+        const size_t bytes = (size_t)s * (2 * sc.n_keys + 2) * 8;
+        DevBuf d; d.alloc(bytes);
+        fsort_sample_kernel<<<(unsigned)((s + 255) / 256), 256, 0, stream>>>(out_keys(rank), s, d.as<uint64_t>());
+        B200_CUDA(cudaGetLastError());
+        B200_CUDA(cudaMemcpyAsync(rec, d.p, bytes, cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaStreamSynchronize(stream));
+    }
+
+    // counts[k] = the sorted rows whose (key, rank, row) tuple is below splitter record k (fsort_count_below_kernel); host arrays.
+    void count_below(const uint64_t* spl, int64_t n_spl, int64_t rank, int64_t* counts) {
+        B200_REQUIRE(finished, "b200 sort: splitters are counted after the last batch was consumed");
+        B200_REQUIRE(n_spl >= 0 && (n_spl == 0 || (spl && counts)), "b200 sort: null splitter or count buffer");
+        if (n_spl == 0) return;
+        B200_CUDA(cudaSetDevice(device));
+        const size_t bytes = (size_t)n_spl * (2 * sc.n_keys + 2) * 8;
+        DevBuf d_spl, d_counts;
+        d_spl.alloc(bytes); d_counts.alloc((size_t)n_spl * 8);
+        B200_CUDA(cudaMemcpyAsync(d_spl.p, spl, bytes, cudaMemcpyHostToDevice, stream));
+        fsort_count_below_kernel<<<(unsigned)((n_spl + 127) / 128), 128, 0, stream>>>(out_keys(rank), d_spl.as<uint64_t>(), n_spl,
+                                                                                        d_counts.as<int64_t>());
+        B200_CUDA(cudaGetLastError());
+        B200_CUDA(cudaMemcpyAsync(counts, d_counts.p, (size_t)n_spl * 8, cudaMemcpyDeviceToHost, stream));
+        B200_CUDA(cudaStreamSynchronize(stream));
+    }
+};
+
+// A full sort whose input is n_runs runs of the given lengths, consumed back to back, each already in the state's sorted order:
+// is_last merges them (fsort_merge_kernel) instead of sorting.  Rows that tie on every key keep their store order.
+struct MergeSortState : FullSortState {
+    std::vector<int64_t> runs;
+
+    MergeSortState(const int64_t* run_lengths, int n_runs, const int8_t* c_types, const int8_t* arr_types, int n_arrs, int n_keys,
+                   const int32_t* asc, const int32_t* na_last, int64_t obs, int dev, cudaStream_t st)
+        : FullSortState(c_types, arr_types, n_arrs, n_keys, asc, na_last, obs, dev, st), runs(run_lengths, run_lengths + n_runs) {}
+
+    const uint32_t* sorted_ids(const FsChunks& ch, int64_t n, DevBuf (&ibuf)[2]) override {
+        int64_t total = 0;
+        std::vector<int64_t> len;
+        for (int64_t r : runs) { total += r; if (r > 0) len.push_back(r); }
+        B200_REQUIRE(total == n, "b200 sort: the rows consumed differ from the sum of the run lengths");
+        if (len.size() <= 1) return nullptr;
+        // every round's pairs, uploaded at once
+        std::vector<FsMergePair> pairs;
+        std::vector<size_t> first;
+        std::vector<int64_t> n_chunks;
+        while (len.size() > 1) {
+            first.push_back(pairs.size());
+            std::vector<int64_t> next;
+            int64_t off = 0, c = 0;
+            for (size_t p = 0; p < len.size(); p += 2) {
+                const int64_t la = len[p], lb = p + 1 < len.size() ? len[p + 1] : 0;
+                pairs.push_back(FsMergePair{off, la, lb, c});
+                c += (la + lb + FS_MERGE_ITEMS - 1) / FS_MERGE_ITEMS;
+                off += la + lb;
+                next.push_back(la + lb);
+            }
+            n_chunks.push_back(c);
+            len.swap(next);
+        }
+        first.push_back(pairs.size());
+        DevBuf d_pairs;
+        d_pairs.alloc(pairs.size() * sizeof(FsMergePair));
+        B200_CUDA(cudaMemcpyAsync(d_pairs.p, pairs.data(), pairs.size() * sizeof(FsMergePair), cudaMemcpyHostToDevice, stream));
+        for (int b = 0; b < 2; b++) ibuf[b].alloc((size_t)n * 4);
+        FsMergeArgs a{};
+        a.nk = sc.n_keys;
+        std::copy(sc.key, sc.key + sc.n_keys, a.key);
+        a.src = key_src(ch);
+        const uint32_t* ids = nullptr;
+        for (size_t r = 0; r + 1 < first.size(); r++) {
+            a.pair = d_pairs.as<FsMergePair>() + first[r];
+            a.n_pairs = (int64_t)(first[r + 1] - first[r]);
+            a.n_chunks = n_chunks[r];
+            a.in = ids;
+            a.out = ibuf[r & 1].as<uint32_t>();
+            fsort_merge_kernel<<<(unsigned)((a.n_chunks + 255) / 256), 256, 0, stream>>>(a);
+            B200_CUDA(cudaGetLastError());
+            ids = a.out;
+        }
+        B200_CUDA(cudaStreamSynchronize(stream));  // the pair list lives in host memory until its copy has run
+        return ids;
     }
 };
 
@@ -2188,6 +2407,43 @@ void* b200_sort_state_init_full(int64_t operator_id, const int8_t* c_types, cons
         return new b200::FullSortState(c_types, arr_types, n_arrs, n_keys, ascending, na_last, output_batch_size, device,
                                        (cudaStream_t)stream);
     });
+}
+
+void* b200_sort_state_init_runs(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs, int32_t n_keys,
+                                const int32_t* ascending, const int32_t* na_last, const int64_t* run_lengths, int32_t n_runs,
+                                int64_t output_batch_size, int32_t device, void* stream) {
+    (void)operator_id;
+    return b200::sort_state_new(device, [&]() -> SortState* {
+        B200_REQUIRE(run_lengths && n_runs >= 1, "b200 sort: at least one run length");
+        int64_t total = 0;
+        for (int32_t r = 0; r < n_runs; r++) {
+            B200_REQUIRE(run_lengths[r] >= 0, "b200 sort: run lengths must be non-negative");
+            total += run_lengths[r];
+            B200_REQUIRE(total <= b200::FS_MAX_ROWS, "b200 sort: a full sort holds at most 2^31 rows (32-bit row ids)");
+        }
+        return new b200::MergeSortState(run_lengths, n_runs, c_types, arr_types, n_arrs, n_keys, ascending, na_last, output_batch_size,
+                                        device, (cudaStream_t)stream);
+    });
+}
+
+int b200_sort_sample(void* state, int64_t n_samples, int64_t rank, uint64_t* records) {
+    try {
+        auto* s = dynamic_cast<b200::FullSortState*>((SortState*)state);
+        B200_REQUIRE(s, "b200 sort: samples are taken from a full-sort state");
+        b200::scratch_set_stream(s->stream);
+        s->sample(n_samples, rank, records);
+        return 0;
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
+}
+
+int b200_sort_count_below(void* state, const uint64_t* splitters, int64_t n_splitters, int64_t rank, int64_t* counts) {
+    try {
+        auto* s = dynamic_cast<b200::FullSortState*>((SortState*)state);
+        B200_REQUIRE(s, "b200 sort: splitters are counted in a full-sort state");
+        b200::scratch_set_stream(s->stream);
+        s->count_below(splitters, n_splitters, rank, counts);
+        return 0;
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
 }
 
 void* b200_window_state_init(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs, int32_t n_partition_keys,

@@ -318,8 +318,9 @@ class PhysicalJoin:
 class PhysicalSort:
     """Sort sink/source (the reference's PhysicalSort, bodo/pandas/physical/sort.h, which DuckDB's TopN lowers to): rows
     [offset, offset + limit) of the input sorted stably by `by` (column names; ascending / na_position per key or one for all).
-    With full=True (no limit, no offset) every row, sorted: an ORDER BY without LIMIT.  The column names are taken from the
-    first batch."""
+    With full=True (no limit, no offset) every row, sorted: an ORDER BY without LIMIT; with parallel=True as well, the sharded
+    full sort (streaming.sort.init_sharded_sort_state: each rank produces its key range of the result).  The column names are
+    taken from the first batch."""
 
     def __init__(self, by, ascending=True, na_position="last", limit=None, offset=0, parallel: bool = False, full: bool = False, **kw):
         self.args = (by, ascending, na_position, limit, offset, parallel)
@@ -335,8 +336,11 @@ class PhysicalSort:
     def ConsumeBatch(self, batch: Table, prev: OperatorResult) -> OperatorResult:
         if self.state is None:
             by, asc, nap, limit, offset, parallel = self.args
-            kw = dict(self.kw, full=True) if self.full else self.kw
-            self.state = S.init_stream_sort_state(-1, limit, offset, by, asc, nap, batch.names, parallel, **kw)
+            if self.full and parallel:
+                self.state = S.init_sharded_sort_state(-1, by, asc, nap, batch.names, **self.kw)
+            else:
+                kw = dict(self.kw, full=True) if self.full else self.kw
+                self.state = S.init_stream_sort_state(-1, limit, offset, by, asc, nap, batch.names, parallel, **kw)
         is_last = prev == OperatorResult.FINISHED
         S.sort_build_consume_batch(self.state, batch, is_last)
         return OperatorResult.FINISHED if is_last else OperatorResult.NEED_MORE_INPUT

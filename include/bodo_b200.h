@@ -346,6 +346,26 @@ void* b200_sort_state_init_full(int64_t operator_id, const int8_t* c_types, cons
                                 const int32_t* ascending, const int32_t* na_last, int64_t output_batch_size, int32_t device,
                                 void* stream);
 
+/* The sharded full sort's receive side: a full sort whose input is n_runs (>= 1) runs of run_lengths[r] (>= 0, summing to at
+ * most 2^31) rows, consumed back to back in run order, each already sorted by these keys.  is_last merges the runs (ceil(log2
+ * n_runs) merge-path rounds) instead of sorting; rows that tie on every key keep their input order, so runs from source ranks
+ * 0, 1, ... give the stable sort of the rank inputs concatenated in rank order.  is_last fails when the rows consumed differ
+ * from the sum of the lengths.  Unsorted runs give a permutation of the input in an unspecified order. */
+void* b200_sort_state_init_runs(int64_t operator_id, const int8_t* c_types, const int8_t* arr_types, int32_t n_arrs, int32_t n_keys,
+                                const int32_t* ascending, const int32_t* na_last, const int64_t* run_lengths, int32_t n_runs,
+                                int64_t output_batch_size, int32_t device, void* stream);
+
+/* Samples a finished full sort (b200_sort_state_init_full or _runs, after is_last): record i (0 <= i < n_samples <= rows) is
+ * output row q_i = floor(i * rows / n_samples) as 2 n_keys + 2 uint64 words: per key its NA class (0 or 1, the class that sorts
+ * first is 0) and radix word, the sort's own key encoding, then rank and q_i.  Records compare lexicographically word by word
+ * in the order of the rows.  `records` is host memory of n_samples * (2 n_keys + 2) words. */
+int b200_sort_sample(void* state, int64_t n_samples, int64_t rank, uint64_t* records);
+
+/* counts[k] (host) = the rows of a finished full sort whose record (the words b200_sort_sample would give them, with this rank)
+ * is below splitters[k] (host, records of the same layout), 0 <= k < n_splitters: a device binary search over the sorted rows.
+ * Rows [counts[k - 1], counts[k]) lie between two nondecreasing splitters. */
+int b200_sort_count_below(void* state, const uint64_t* splitters, int64_t n_splitters, int64_t rank, int64_t* counts);
+
 /* Window functions over (PARTITION BY p ORDER BY o), as a third form of the sort state (the reference plans these through its
  * window / MRNF arguments, which the groupby ABI above drops).  The keys are the first n_partition_keys + n_order_keys (0 <= each,
  * 1 <= sum <= 4) of the n_arrs columns, partition keys first; key columns are distinct and of the sort's key types.  PARTITION BY
