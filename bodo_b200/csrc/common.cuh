@@ -231,9 +231,26 @@ __device__ __forceinline__ uint32_t hash_key_column(const void* data, int ct, co
     if (ctype_size(ct) == 8) return (uint32_t)xxh3_64_short((uint64_t)load_int_as_i64(data, ct, i), 8, seed);
     return (uint32_t)xxh3_64_short((uint64_t)(uint32_t)load_int_as_i64(data, ct, i), 4, seed);  // 4-byte keys hash their 4 raw bytes
 }
+// Key hash policies of hash_keys_row.  ReferenceKeyHash is hash_key_column: the reference's placement, which hashes a valid
+// float NaN as a value.  KeyClassHash hashes every cell of one key class alike, equality being the window's, the sort's and the
+// groupby's: NA and a float NaN are one class (both hash as hash_na_val), -0.0 equals 0.0 (_Py_HashDouble gives both 0), and a
+// 1- or 2-byte integer or bool key hashes as the 4-byte integer of its value.  On keys without NaN it is hash_key_column.
+struct ReferenceKeyHash {
+    __device__ __forceinline__ static uint32_t column(const void* data, int ct, const uint8_t* valid, int64_t i, uint32_t seed) {
+        return hash_key_column(data, ct, valid, i, seed);
+    }
+};
+struct KeyClassHash {
+    __device__ __forceinline__ static uint32_t column(const void* data, int ct, const uint8_t* valid, int64_t i, uint32_t seed) {
+        if ((ct == CT_FLOAT64 || ct == CT_FLOAT32) && bit_valid(valid, i) && isnan(load_as_f64(data, ct, i)))
+            return (uint32_t)xxh3_64_short(1ull, 8, seed);
+        return hash_key_column(data, ct, valid, i, seed);  // (its narrow-integer path reads 1- and 2-byte cells as their value)
+    }
+};
+template <class H = ReferenceKeyHash>
 __device__ __forceinline__ uint32_t hash_keys_row(const KeySet& k, int64_t i, uint32_t seed) {
-    uint32_t h = hash_key_column(k.data[0], k.ctype[0], k.valid[0], i, seed);
-    for (int j = 1; j < k.n_keys; j++) h = hash_combine_boost(h, hash_key_column(k.data[j], k.ctype[j], k.valid[j], i, seed));
+    uint32_t h = H::column(k.data[0], k.ctype[0], k.valid[0], i, seed);
+    for (int j = 1; j < k.n_keys; j++) h = hash_combine_boost(h, H::column(k.data[j], k.ctype[j], k.valid[j], i, seed));
     return h;
 }
 

@@ -15,6 +15,10 @@
 //                    destination with byte padding, _shuffle.cpp:661-875).
 // Rows keep their input order inside a destination (fill_send_array is stable too), so the result is
 // bit-identical to the oracle's oracle_shuffle_partition.
+//
+// b200_shuffle_partition_classes runs the same pass with K1's key hash swapped for KeyClassHash (common.cuh): every row of
+// one key class (NA and NaN one class, -0.0 equal to 0.0, any fixed-width key type) goes to one rank, which is what the
+// sharded window and min_row_number_filter need.  K2-K4 only read dest8 and are shared.
 #include <vector>
 
 #include "common.cuh"
@@ -34,7 +38,9 @@ __global__ void hash_to_rank_kernel(const __grid_constant__ KeySet k, int64_t n,
     }
 }
 
-// K1: tile = contiguous rows [cta * tile_rows, ...). dest8 holds the destination of every row.
+// K1: tile = contiguous rows [cta * tile_rows, ...). dest8 holds the destination of every row.  H is the key hash policy
+// (common.cuh): ReferenceKeyHash places rows as the reference does, KeyClassHash sends every key class to one rank.
+template <class H>
 __global__ void __launch_bounds__(PART_THREADS) dest_hist_kernel(const __grid_constant__ KeySet k,
                                                                  int64_t n, int64_t tile_rows, int n_pes, uint8_t* dest8,
                                                                  unsigned int* hist /* [gridDim.x][n_pes] */) {
@@ -44,7 +50,7 @@ __global__ void __launch_bounds__(PART_THREADS) dest_hist_kernel(const __grid_co
     int64_t r0 = (int64_t)blockIdx.x * tile_rows;
     int64_t r1 = r0 + tile_rows < n ? r0 + tile_rows : n;
     for (int64_t i = r0 + threadIdx.x; i < r1; i += blockDim.x) {
-        int d = hash_to_rank_u32(hash_keys_row(k, i, SEED_HASH_PARTITION), n_pes);
+        int d = hash_to_rank_u32(hash_keys_row<H>(k, i, SEED_HASH_PARTITION), n_pes);
         dest8[i] = (uint8_t)d;
         atomicAdd(&sh[d], 1u);
     }
@@ -286,20 +292,25 @@ static int table_device(const b200_table* t) {
     B200_REQUIRE(t->device >= 0, "b200 shuffle: the table must be device resident");
     return t->device;
 }
-// the first n_keys columns as a KeySet (4- / 8-byte integer, date and float columns)
-static KeySet make_keyset(const b200_table* t, int n_keys) {
+// the first n_keys columns as a KeySet: 4- / 8-byte integer, date and float columns, and with narrow = true also 1- and 2-byte
+// integer and bool columns (the key-class placement)
+static KeySet make_keyset(const b200_table* t, int n_keys, bool narrow = false) {
     KeySet k{};
     k.n_keys = n_keys;
     for (int j = 0; j < n_keys; j++) {
         const b200_column& c = t->cols[j];
-        B200_REQUIRE(ctype_size(c.c_type) == 4 || ctype_size(c.c_type) == 8, "b200 shuffle: key columns must be 4- or 8-byte integer, date or float columns");
+        if (narrow)
+            B200_REQUIRE(ctype_size(c.c_type) >= 1 && ctype_size(c.c_type) <= 8, "b200 shuffle: key columns must be fixed-width integer, bool, date, time or float columns");
+        else
+            B200_REQUIRE(ctype_size(c.c_type) == 4 || ctype_size(c.c_type) == 8, "b200 shuffle: key columns must be 4- or 8-byte integer, date or float columns");
         k.data[j] = c.data; k.valid[j] = c.validity; k.ctype[j] = c.c_type;
     }
     return k;
 }
 
+// classes = false: the reference's placement (ReferenceKeyHash); true: one rank per key class (KeyClassHash).
 void shuffle_partition(const b200_table* in, int64_t n_keys, int n_pes, b200_table* out, int64_t* send_counts,
-                       long long* perm_out_dev, cudaStream_t st) {
+                       long long* perm_out_dev, cudaStream_t st, bool classes = false) {
     B200_REQUIRE(n_keys >= 1 && n_keys <= MAX_HASH_KEYS && n_keys <= in->n_cols, "b200 shuffle: between 1 and 4 key columns are supported");
     B200_REQUIRE(n_pes >= 1 && n_pes <= MAX_PES, "b200 shuffle: n_pes must be in [1, 256]");
     B200_REQUIRE(in->n_cols >= 1 && in->n_cols <= MAX_SHUFFLE_COLS, "b200 shuffle: between 1 and 32 columns are supported");
@@ -307,7 +318,7 @@ void shuffle_partition(const b200_table* in, int64_t n_keys, int n_pes, b200_tab
     int dev = table_device(in);
     B200_CUDA(cudaSetDevice(dev));
     int64_t n = in->n_rows;
-    KeySet ks = make_keyset(in, (int)n_keys);
+    KeySet ks = make_keyset(in, (int)n_keys, classes);
     for (int d = 0; d < n_pes; d++) send_counts[d] = 0;
     out->n_rows = n;
     if (n == 0) return;
@@ -317,7 +328,10 @@ void shuffle_partition(const b200_table* in, int64_t n_keys, int n_pes, b200_tab
     int64_t tile_rows = ((n + n_ctas - 1) / n_ctas + chunk - 1) / chunk * chunk;
     n_ctas = (int)((n + tile_rows - 1) / tile_rows);
     StreamBuf dest8((size_t)n, st), hist((size_t)n_ctas * n_pes * 4, st), offsets((size_t)n_ctas * n_pes * 8, st), totals((size_t)n_pes * 8, st);
-    dest_hist_kernel<<<n_ctas, PART_THREADS, 0, st>>>(ks, n, tile_rows, n_pes, dest8.as<uint8_t>(), hist.as<unsigned int>());
+    if (classes)
+        dest_hist_kernel<KeyClassHash><<<n_ctas, PART_THREADS, 0, st>>>(ks, n, tile_rows, n_pes, dest8.as<uint8_t>(), hist.as<unsigned int>());
+    else
+        dest_hist_kernel<ReferenceKeyHash><<<n_ctas, PART_THREADS, 0, st>>>(ks, n, tile_rows, n_pes, dest8.as<uint8_t>(), hist.as<unsigned int>());
     B200_CUDA(cudaGetLastError());
     scan_hist_kernel<<<1, 1024, 0, st>>>(hist.as<unsigned int>(), n_ctas, n_pes, offsets.as<long long>(), totals.as<long long>());
     B200_CUDA(cudaGetLastError());
@@ -419,6 +433,15 @@ int b200_shuffle_partition_perm(const b200_table* in_table, int64_t n_keys, int3
     try {
         B200_REQUIRE(in_table && out && send_counts, "b200_shuffle_partition_perm: null argument");
         b200::shuffle_partition(in_table, n_keys, n_pes, out, send_counts, (long long*)perm_out_dev, (cudaStream_t)stream);
+        return 0;
+    } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
+}
+
+int b200_shuffle_partition_classes(const b200_table* in_table, int64_t n_keys, int32_t n_pes, b200_table* out, int64_t* send_counts,
+                                   int64_t* perm_out_dev, void* stream) {
+    try {
+        B200_REQUIRE(in_table && out && send_counts, "b200_shuffle_partition_classes: null argument");
+        b200::shuffle_partition(in_table, n_keys, n_pes, out, send_counts, (long long*)perm_out_dev, (cudaStream_t)stream, true);
         return 0;
     } catch (const std::exception& e) { b200::set_last_error(e.what()); return -1; }
 }

@@ -236,9 +236,14 @@ class PhysicalAggregate:
     mrnf = (sort_col_inds, ascending, na_last, keep_inds) with no aggs: a min_row_number_filter, one row per group, the first by
     the sort columns (streaming.groupby's mrnf_* arguments); mrnf_limit=n (forwarded to init_groupby_state with the other keywords)
     keeps the first n rows per group.  percentiles=(q, ...) (forwarded the same way) gives the fraction of every percentile_cont /
-    percentile_disc entry of aggs, in order."""
+    percentile_disc entry of aggs, in order.  A min_row_number_filter with parallel=True is the sharded one
+    (streaming.groupby.init_sharded_mrnf_state: only each rank's winners are exchanged, at the last batch)."""
 
     def __init__(self, key_inds: Sequence[int], aggs: Sequence[tuple], dropna: bool = True, parallel: bool = False, mrnf=None, **kw):
+        if mrnf is not None and parallel and not aggs:
+            self.state = G.init_sharded_mrnf_state(-1, tuple(key_inds), *(tuple(x) for x in mrnf), dropna=dropna, **kw)
+            self.finished_build = False
+            return
         fnames = tuple(f for f, _ in aggs) + ((G.MRNF,) if mrnf is not None else ())
         f_in_offsets, f_in_cols = [0], []
         for _, c in aggs:
@@ -365,7 +370,9 @@ class PhysicalWindow:
     "nth_value", column, n[, frame]) or (out_name, fname, y, x[, frame]), fname one of streaming.window.BIVARIATE_FUNCS
     (covar_samp, covar_pop, corr, regr_slope, regr_intercept, over any frame sum takes); an entry of first_value, last_value,
     nth_value, lag or lead may end with "ignore_nulls" (IGNORE NULLS) or "respect_nulls" (the default);
-    ascending / na_position: one value or one per ORDER BY key.  The column names are taken from the first batch."""
+    ascending / na_position: one value or one per ORDER BY key.  The column names are taken from the first batch.  With
+    parallel=True the window is sharded (streaming.window.init_sharded_window_state: each rank produces the partitions it owns;
+    without PARTITION BY rank 0 produces every row)."""
 
     def __init__(self, partition_by, order_by, funcs, ascending=True, na_position="last", parallel: bool = False, **kw):
         self.args = (partition_by, order_by, ascending, na_position, list(funcs), parallel)
@@ -375,7 +382,10 @@ class PhysicalWindow:
     def ConsumeBatch(self, batch: Table, prev: OperatorResult) -> OperatorResult:
         if self.state is None:
             part, order, asc, nap, funcs, parallel = self.args
-            self.state = W.init_window_state(-1, part, order, asc, nap, funcs, batch.names, parallel, **self.kw)
+            if parallel:
+                self.state = W.init_sharded_window_state(-1, part, order, asc, nap, funcs, batch.names, **self.kw)
+            else:
+                self.state = W.init_window_state(-1, part, order, asc, nap, funcs, batch.names, False, **self.kw)
         is_last = prev == OperatorResult.FINISHED
         W.window_build_consume_batch(self.state, batch, is_last)
         return OperatorResult.FINISHED if is_last else OperatorResult.NEED_MORE_INPUT

@@ -24,8 +24,12 @@ from ._lib import ffi
 from .table import ArrTypes, Column, CTable, Table
 
 
-def partition_device(table: Table, n_keys: int, n_pes: int, stream: int = 0, want_perm: bool = False):
-    """Run the CUDA radix partition. Returns (partitioned Table of torch tensors, send_counts[, perm tensor])."""
+def partition_device(table: Table, n_keys: int, n_pes: int, stream: int = 0, want_perm: bool = False, by_class: bool = False):
+    """Run the CUDA radix partition. Returns (partitioned Table of torch tensors, send_counts[, perm tensor]).
+
+    by_class=False places rows as the reference's shuffle_table does (b200_shuffle_partition, 4- and 8-byte keys).  by_class=True
+    sends every key class to one rank (b200_shuffle_partition_classes): NA and a float NaN are one class, -0.0 equals 0.0, and
+    every fixed-width key type is accepted, 1- and 2-byte integers and bool included."""
     import torch
 
     L = _lib.lib()
@@ -46,6 +50,12 @@ def partition_device(table: Table, n_keys: int, n_pes: int, stream: int = 0, wan
     out = Table(out_cols, list(table.names))
     cin, cout = CTable(table), CTable(out)
     counts = ffi.new("int64_t[]", n_pes)
+    if by_class:
+        perm = torch.empty(n, dtype=torch.int64, device=dev) if want_perm else None
+        _lib.check(L.b200_shuffle_partition_classes(cin.ptr, n_keys, n_pes, cout.ptr, counts,
+                                                    ffi.cast("int64_t*", perm.data_ptr()) if want_perm else ffi.NULL,
+                                                    ffi.cast("void*", stream)), "shuffle partition by key class")
+        return (out, [int(counts[i]) for i in range(n_pes)]) + ((perm,) if want_perm else ())
     if want_perm:
         perm = torch.empty(n, dtype=torch.int64, device=dev)
         _lib.check(L.b200_shuffle_partition_perm(cin.ptr, n_keys, n_pes, cout.ptr, counts, ffi.cast("int64_t*", perm.data_ptr()),

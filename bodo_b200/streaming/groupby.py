@@ -32,6 +32,15 @@ df.sort_values(sort columns, kind="stable").drop_duplicates(keys, keep="first")[
 The state streams every batch into the groupby's hash table and keeps one winner record per group (DESIGN.md §3d), so it holds
 O(groups) device memory whatever the row count.
 
+Sharded min_row_number_filter (init_sharded_mrnf_state, one process per GPU of a torch.distributed process group): only winners
+move between ranks.  Consume calls before is_last are local and run no collective: each rank runs an ordinary MRNF that keeps the
+union of the keys, the sort columns and the caller's kept columns (at most 26).  The is_last call is collective: each rank
+produces its winners (at most groups x n rows), partitions them by key class on the keys (shuffle.partition_device(by_class=True):
+NA and NaN one class, -0.0 equal to 0.0, every key type), agrees the count matrix, exchanges them and consumes the rows it received
+in one call into a second MRNF with the same keys, sort and n that keeps the caller's columns.  The rows arrive in source-rank
+order and the partition is stable, so within a group each source's rows arrive in its own rank order: ties are broken by (rank,
+local arrival), and the top n of the union of every rank's top n is the MRNF of the rank inputs concatenated in rank order.
+
 mrnf_limit=n (keyword-only, an int, 1 <= n < 2^31, default 1; only with min_row_number_filter) keeps the first n rows per group,
 QUALIFY ROW_NUMBER() OVER (PARTITION BY keys ORDER BY sort columns) <= n, i.e.
 df.sort_values(sort columns, kind="stable").groupby(keys, sort=False, dropna=dropna).head(n)[kept columns] as a multiset of rows:
@@ -458,6 +467,105 @@ def init_groupby_state(operator_id, key_inds, fnames, f_in_offsets, f_in_cols, m
     return st
 
 
+MRNF_MAX_RECEIVE_ROWS = 1 << 31  # winners one rank may receive: the candidate store's sort holds at most 2^31 rows
+
+
+def _mrnf_state(operator_id, key_inds, spec, mrnf_limit, dropna, output_batch_size, device, stream):
+    """A local min_row_number_filter state of a validated spec (sort_inds, asc, na_last, keep)."""
+    st = GroupbyState(operator_id, key_inds, (), (0,), (), False, dropna, output_batch_size, 0, device, stream, None)
+    st.mrnf = spec
+    st.mrnf_limit = mrnf_limit
+    return st
+
+
+class ShardedMrnfState:
+    """Python handle of a sharded min_row_number_filter (init_sharded_mrnf_state).  `local` keeps this rank's winners over the union
+    of the key, sort and kept columns; at is_last the winners are exchanged by key and `final` keeps the winners of the groups this
+    rank owns (with one rank, `local` keeps the caller's columns and is the result)."""
+
+    def __init__(self, operator_id, key_inds, sort_inds, sort_asc, sort_na, keep_inds, dropna, mrnf_limit, output_batch_size, device,
+                 stream, process_group):
+        key_inds = tuple(int(k) for k in getattr(key_inds, "meta", key_inds))
+        sort, asc, na_last, keep = _mrnf_spec(key_inds, (MRNF,), (0, 0), (), sort_inds, sort_asc, sort_na, keep_inds)
+        if isinstance(mrnf_limit, bool) or not isinstance(mrnf_limit, numbers.Integral) or not 1 <= mrnf_limit < MRNF_MAX_LIMIT:
+            raise _lib.B200Error(f"Streaming Groupby: mrnf_limit must be an integer in [1, 2^31) (got {mrnf_limit!r})")
+        self.union = sorted(set(key_inds) | set(sort) | set(keep))
+        if len(self.union) > MRNF_MAX_KEEP:
+            raise _lib.B200Error(f"Streaming Groupby: a sharded min_row_number_filter keeps the union of the keys {list(key_inds)}, the sort "
+                                 f"columns {list(sort)} and the kept columns {list(keep)} until its exchange: {len(self.union)} columns "
+                                 f"{self.union}, more than {MRNF_MAX_KEEP}")
+        self.spec = (sort, asc, na_last, keep)
+        self.args = (operator_id, key_inds, int(mrnf_limit), bool(dropna))
+        self.output_batch_size = int(output_batch_size)
+        self.device, self.stream = device, int(stream)
+        self.process_group = process_group
+        # the winners leave `local` as one batch (output_batch_size 0)
+        self.local = _mrnf_state(operator_id, key_inds, (sort, asc, na_last, tuple(self.union)), int(mrnf_limit), dropna, 0, device, stream)
+        self.final = None
+        self.n_ranks = None
+
+    def consume(self, table: Table, is_last: bool):
+        if self.n_ranks is None:
+            from .sort import _world
+
+            self.n_ranks, self.rank = _world(self.process_group)
+            if self.n_ranks == 1:
+                self.local.mrnf, self.local.output_batch_size = self.spec, self.output_batch_size
+        res = groupby_build_consume_batch(self.local, table, is_last)
+        if is_last:
+            self.final = self.local if self.n_ranks == 1 else self._exchange()
+        return res
+
+    def _exchange(self):
+        """Partition the local winners by key class, exchange them and keep the winners of the groups this rank owns."""
+        import torch
+
+        from ..shuffle import exchange_table, partition_device, with_schema_validity
+        from ..table import Column
+        from .sort import agree_receive_rows
+
+        loc, union = self.local, self.union
+        operator_id, key_inds, limit, dropna = self.args
+        dev = torch.device("cuda", loc.device)
+        out, _ = groupby_produce_output_batch(loc, True)  # every winner, the union's columns in input order
+        n = out.n_rows
+        cols = []
+        for c in out.columns:  # library-owned device columns: wrapped, not copied (an empty one has no address to wrap)
+            data = torch.as_tensor(c.data, device=dev) if n else torch.empty(0, dtype=getattr(torch, str(np_dtype_of(c.c_type))), device=dev)
+            v = torch.as_tensor(c.validity, device=dev) if n and c.validity is not None else None
+            cols.append(Column(data, v, c.c_type, c.arr_type, n))
+        kp = [union.index(k) for k in key_inds]
+        order = kp + [j for j in range(len(union)) if j not in kp]  # the keys lead
+        part, send = partition_device(with_schema_validity(Table(cols, list(out.names)).select(order)), len(kp), self.n_ranks,
+                                      loc.stream, by_class=True)
+        agree_receive_rows(send, dev, self.process_group, cap=MRNF_MAX_RECEIVE_ROWS,
+                           what="Streaming Groupby: sharded min_row_number_filter", cap_name="the min_row_number_filter's cap")
+        got = exchange_table(part, send, self.process_group)
+        torch.cuda.synchronize(dev)
+        delete_groupby_state(loc)  # the winners have been sent
+        got = got.select([order.index(j) for j in range(len(union))])
+        sort, asc, na_last, keep = self.spec
+        spec = (tuple(union.index(i) for i in sort), asc, na_last, tuple(union.index(i) for i in keep))
+        fin = _mrnf_state(operator_id, tuple(kp), spec, limit, dropna, self.output_batch_size, loc.device, self.stream)
+        groupby_build_consume_batch(fin, got, True)
+        return fin
+
+
+def init_sharded_mrnf_state(operator_id, key_inds, mrnf_sort_col_inds, mrnf_sort_col_asc, mrnf_sort_col_na, mrnf_col_inds_keep, *,
+                            dropna=True, mrnf_limit=1, output_batch_size=32768, device=None, stream=0,
+                            process_group=None) -> ShardedMrnfState:
+    """A sharded min_row_number_filter over a torch.distributed process group (one process per GPU), driven by the groupby verbs:
+    the rows all ranks produce are, as a multiset, the MRNF (init_groupby_state's min_row_number_filter with these arguments) of the
+    rank inputs concatenated in rank order, bit for bit; of rows that tie on every sort column the lower rank wins.  Each group's
+    rows come out on one rank; with mrnf_limit > 1 they are consecutive and in rank order.  Consume calls before is_last are local;
+    the is_last call is collective (every rank passes is_last=True in the same call) and raises the same B200Error on every rank
+    when a rank would receive MRNF_MAX_RECEIVE_ROWS winners or more.  Raises B200Error for the arguments init_groupby_state refuses
+    and when the union of the key, sort and kept columns, which every rank keeps until the exchange, exceeds 26 columns.  Without
+    torch.distributed, or with one rank, it is the local min_row_number_filter."""
+    return ShardedMrnfState(operator_id, key_inds, mrnf_sort_col_inds, mrnf_sort_col_asc, mrnf_sort_col_na, mrnf_col_inds_keep, dropna,
+                            mrnf_limit, output_batch_size, device, stream, process_group)
+
+
 def groupby_build_consume_batch(groupby_state: GroupbyState, table: Table, is_last: bool, is_final_pipeline: bool = True):
     """Mirror of groupby_build_consume_batch (groupby.py:1295-1395): returns (is_last, request_input).
 
@@ -465,6 +573,10 @@ def groupby_build_consume_batch(groupby_state: GroupbyState, table: Table, is_la
     ran out of input keep calling with empty batches, as in the reference's pipeline loop,
     bodo/pandas/_pipeline.cpp:453-457)."""
     st = groupby_state
+    if isinstance(st, ShardedMrnfState):
+        if st.final is not None:
+            raise _lib.B200Error("groupby_build_consume_batch called after is_last")
+        return st.consume(table, is_last)
     if st.mrnf is not None and st.parallel and st.handle is None:
         import torch.distributed as dist
 
@@ -490,8 +602,13 @@ def groupby_build_consume_batch(groupby_state: GroupbyState, table: Table, is_la
 
 def groupby_produce_output_batch(groupby_state: GroupbyState, produce_output: bool = True):
     """Mirror of groupby_produce_output_batch (groupby.py:1502-1600): returns (out_table, is_last).
-    The returned Table wraps library-owned device columns that stay valid until the next produce call."""
+    The returned Table wraps library-owned device columns that stay valid until the next produce call.  A sharded
+    min_row_number_filter produces the winners of the groups this rank owns."""
     st = groupby_state
+    if isinstance(st, ShardedMrnfState):
+        if st.final is None:
+            raise _lib.B200Error("groupby_produce_output_batch called before the last batch was consumed")
+        st = st.final
     if st.handle is None:
         raise _lib.B200Error("groupby_produce_output_batch called before any build batch was consumed")
     L = _lib.lib()
@@ -509,10 +626,18 @@ def groupby_produce_output_batch(groupby_state: GroupbyState, produce_output: bo
 
 
 def delete_groupby_state(groupby_state: GroupbyState) -> None:
+    if isinstance(groupby_state, ShardedMrnfState):
+        for s in (groupby_state.local, groupby_state.final):
+            if s is not None:
+                delete_groupby_state(s)
+        return
     if groupby_state.handle is not None:
         _lib.lib().b200_delete_groupby_state(groupby_state.handle)
         groupby_state.handle = None
 
 
 def get_metric(groupby_state: GroupbyState, which: int) -> int:
+    """A sharded min_row_number_filter reports its local state before is_last and the state its output comes from after it."""
+    if isinstance(groupby_state, ShardedMrnfState):
+        groupby_state = groupby_state.final or groupby_state.local
     return int(_lib.lib().b200_groupby_get_metric(groupby_state.handle, which))

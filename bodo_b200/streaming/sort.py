@@ -205,23 +205,26 @@ def choose_splitters(records, weights, n_ranks):
     return recs[idx[idx < len(w)]]
 
 
-def agree_receive_rows(send_counts, device, group=None):
+def agree_receive_rows(send_counts, device, group=None, *, received=0, cap=None, what="Streaming Sort: sharded full sort",
+                       cap_name="the full sort's cap"):
     """Every rank's send counts to every rank, agreed through one all_reduce: returns the (P, P) matrix of rows rank i sends
-    rank j.  Raises the same B200Error on every rank when any rank would receive MAX_SHARDED_RECEIVE_ROWS rows or more (the
-    full sort's 32-bit row ids), before any row moves."""
+    rank j.  Raises the same B200Error on every rank when any rank would hold `cap` rows or more (default
+    MAX_SHARDED_RECEIVE_ROWS, the full sort's 32-bit row ids), counting `received` (a scalar or one entry per rank) rows it holds
+    already, before any row moves.  `what` and `cap_name` name the operator and its cap in the message."""
     import torch
     import torch.distributed as dist
 
+    cap = MAX_SHARDED_RECEIVE_ROWS if cap is None else cap
     n_ranks, rank = _world(group)
     m = torch.zeros((n_ranks, n_ranks), dtype=torch.int64, device=device)
     m[rank] = torch.as_tensor(np.asarray(send_counts, dtype=np.int64), device=device)
     dist.all_reduce(m, group=group)
     counts = m.cpu().numpy()
-    recv = counts.sum(axis=0)
-    over = np.flatnonzero(recv >= MAX_SHARDED_RECEIVE_ROWS)
+    recv = counts.sum(axis=0) + np.asarray(received, dtype=np.int64)
+    over = np.flatnonzero(recv >= cap)
     if len(over):
-        raise _lib.B200Error(f"Streaming Sort: sharded full sort: rank {int(over[0])} would receive {int(recv[over[0]])} rows, at or "
-                             f"above the full sort's cap of {MAX_SHARDED_RECEIVE_ROWS} rows per rank")
+        raise _lib.B200Error(f"{what}: rank {int(over[0])} would receive {int(recv[over[0]])} rows, at or above {cap_name} of {cap} "
+                             "rows per rank")
     return counts
 
 

@@ -105,8 +105,26 @@ Semantics:
   - output: every input row once, in the stable sort's order by (partition keys, order keys, arrival); every input column in
     input order, then one column per function under the caller's name.  SQL leaves the order open; fixing it makes every column
     comparable bit for bit.
-  - at most MAX_WINDOW_ROWS rows per state and MAX_COLS input plus function columns.  A sharded window is not supported: a
-    parallel state raises at its first consume call when the process group has more than one rank (with one rank it runs locally).
+  - at most MAX_WINDOW_ROWS rows per state and MAX_COLS input plus function columns.  A parallel state of init_window_state
+    raises at its first consume call when the process group has more than one rank (with one rank it runs locally): the sharded
+    window is init_sharded_window_state.
+
+Sharded window (init_sharded_window_state, one process per GPU of a torch.distributed process group).  Every consume call is
+collective.  It partitions the batch by key class on the PARTITION BY keys (shuffle.partition_device(by_class=True): NA and NaN
+are one class, -0.0 equals 0.0, every key type), agrees the P x P count matrix in one all_reduce and exchanges the rows
+(exchange_table); the rows a rank receives go into its own local window.  Every partition thus lives whole on one rank, and the
+local window, which is exact, computes it unchanged.  Without PARTITION BY the whole input is one partition: every row goes to
+rank 0, which produces the whole result while the other ranks produce one empty batch (correct, not scalable).
+  - arrival order: a rank receives rows in the order (consume call, source rank, source row), the arrival order that breaks
+    ties.
+  - result: rank r's output is the window of one state over the global input in that order, restricted to the partitions rank r
+    owns, in the same output order, bit for bit on every input and function column (every result depends only on sorted
+    positions within a partition).
+  - protocol: every rank calls consume the same number of times and passes is_last in the same call.  A call after which some
+    rank would hold MAX_WINDOW_ROWS rows or more raises the same B200Error on every rank before any row moves.  With one rank, or
+    without torch.distributed, the state is the local window.
+  - a dictionary-encoded string partition key is placed by its ids, which are only right when every rank uses the same
+    dictionary builder.
 """
 
 from __future__ import annotations
@@ -120,7 +138,7 @@ import numpy as np
 from .. import _lib
 from .._lib import ffi
 from ..table import CTypes, Table, np_dtype_of
-from .sort import MAX_FULL_SORT_ROWS, MAX_KEYS, SortState
+from .sort import MAX_FULL_SORT_ROWS, MAX_KEYS, SortState, _current_device, _world, agree_receive_rows
 
 # Function codes of b200_window_func (include/bodo_b200.h): the ranking functions, then the value functions.
 FUNCS = {"row_number": 0, "rank": 1, "dense_rank": 2, "percent_rank": 3, "cume_dist": 4, "ntile": 5}
@@ -502,6 +520,89 @@ class WindowState(SortState):
         return _lib.check_ptr(h, "init_window_state")
 
 
+class ShardedWindowState:
+    """Python handle of a sharded window (init_sharded_window_state): every consume call moves each row to the rank that owns its
+    partition, and `local` is the window over the rows this rank received."""
+
+    def __init__(self, operator_id, partition_by, order_by, ascending, na_position, funcs, col_names, output_batch_size, device, stream,
+                 process_group):
+        self.local = WindowState(operator_id, partition_by, order_by, ascending, na_position, funcs, col_names, False, output_batch_size,
+                                 device, stream, None)
+        self.process_group = process_group
+        self.n_ranks = None
+        self.received = None  # rows each rank has received so far, known alike on every rank
+        self.done = False
+
+    def consume(self, table: Table, is_last: bool):
+        loc = self.local
+        if self.n_ranks is None:
+            self.n_ranks, self.rank = _world(self.process_group)
+            self.received = np.zeros(self.n_ranks, dtype=np.int64)
+        if self.n_ranks > 1:
+            table = self._exchange(table)
+        loc._ensure(table)
+        req = loc._consume(table, is_last)
+        if is_last:
+            loc.done = self.done = True
+        return req
+
+    def _exchange(self, table: Table) -> Table:
+        """This call's rows of every rank that belong to this rank's partitions, in (source rank, source row) order."""
+        import torch
+
+        from ..shuffle import exchange_table, partition_device, with_schema_validity
+        from ..table import Column, to_device
+
+        loc, P = self.local, self.n_ranks
+        if table.n_cols != len(loc.col_names):
+            raise _lib.B200Error(f"Streaming Window: the batch has {table.n_cols} columns, the state {len(loc.col_names)}")
+        if loc.device is None:
+            loc.device = table.device if table.device >= 0 else _current_device()
+        dev = torch.device("cuda", loc.device)
+        phys = with_schema_validity(to_device(table, loc.device).select(loc.phys))  # the partition keys lead
+        n = phys.n_rows
+        if self.local.partition_by:
+            part, send = partition_device(phys, len(loc.partition_by), P, loc.stream, by_class=True)
+        else:  # one partition: every row to rank 0, the batch itself is the send buffer
+            part = Table([Column(_as_tensor(c.data, dev, n, c.c_type), None if c.validity is None else _as_tensor(c.validity, dev, (n + 7) // 8),
+                                 c.c_type, c.arr_type, n) for c in phys.columns], list(phys.names))
+            send = [n] + [0] * (P - 1)
+        counts = agree_receive_rows(send, dev, self.process_group, received=self.received, cap=MAX_WINDOW_ROWS,
+                                    what="Streaming Window: sharded window", cap_name="the window's cap")
+        self.received += counts.sum(axis=0)
+        got = exchange_table(part, send, self.process_group)
+        torch.cuda.synchronize(dev)
+        return got.select(loc.out_order[: len(loc.col_names)])  # back to input column order
+
+    def produce(self, produce_output: bool):
+        return self.local._produce(produce_output)
+
+
+def _as_tensor(x, dev, n, c_type=None):
+    """The first n cells of a device buffer (torch tensor or library-owned array) as a torch tensor."""
+    import torch
+
+    if n == 0:
+        dt = np.uint8 if c_type is None else np_dtype_of(c_type)
+        return torch.empty(0, dtype=getattr(torch, str(np.dtype(dt))), device=dev)
+    return (x if hasattr(x, "is_cuda") else torch.as_tensor(x, device=dev))[:n]
+
+
+def init_sharded_window_state(operator_id, partition_by, order_by, ascending, na_position, funcs, col_names, *,
+                              output_batch_size=32768, device=None, stream=0, process_group=None) -> ShardedWindowState:
+    """A sharded window over a torch.distributed process group (one process per GPU): init_window_state's arguments, validation
+    and errors, and the same verbs.  Every consume call is collective (every rank calls it the same number of times and passes
+    is_last in the same call) and moves each row to the rank that owns its partition (a hash of its PARTITION BY key class).  Rank
+    r's output is the window of one state over the global input in (consume call, source rank, source row) order, restricted to
+    the partitions rank r owns, in the same output order, bit for bit.  Without PARTITION BY every row goes to rank 0, which
+    produces the whole result while the other ranks produce one empty batch.  A call after which a rank would hold MAX_WINDOW_ROWS
+    rows or more raises the same B200Error on every rank before any row moves.  Without torch.distributed, or with one rank, it
+    is the local window.  A dictionary-encoded string partition key is placed by its ids: every rank must use the same
+    dictionary builder."""
+    return ShardedWindowState(operator_id, partition_by, order_by, ascending, na_position, funcs, col_names, output_batch_size, device,
+                              stream, process_group)
+
+
 def init_window_state(operator_id, partition_by, order_by, ascending, na_position, funcs, col_names, parallel=False, *,
                       output_batch_size=32768, device=None, stream=0, process_group=None) -> WindowState:
     """A window state over batches with columns `col_names`.
@@ -537,6 +638,8 @@ def window_build_consume_batch(state: WindowState, table: Table, is_last: bool):
     """Appends a batch (host batches are staged to the device); is_last sorts and evaluates.  Returns (is_last, request_input)."""
     if state.done:
         raise _lib.B200Error("window_build_consume_batch called after is_last")
+    if isinstance(state, ShardedWindowState):
+        return bool(is_last), state.consume(table, is_last)
     if state.parallel:
         import torch.distributed as dist
 
@@ -551,18 +654,25 @@ def window_build_consume_batch(state: WindowState, table: Table, is_last: bool):
 
 def window_produce_output_batch(state: WindowState, produce_output: bool = True):
     """Returns (table, is_last): the next <= output_batch_size output rows, as library-owned device columns that stay valid until
-    the state is deleted."""
+    the state is deleted.  A sharded window produces the rows of the partitions this rank owns."""
+    if isinstance(state, ShardedWindowState):
+        state = state.local
     if state.handle is None or not state.done:
         raise _lib.B200Error("window_produce_output_batch called before the last batch was consumed")
     return state._produce(produce_output)
 
 
 def delete_window_state(state: WindowState) -> None:
+    if isinstance(state, ShardedWindowState):
+        state = state.local
     if state.handle is not None:
         _lib.lib().b200_delete_sort_state(state.handle)
         state.handle = None
 
 
 def get_metric(state: WindowState, which: int) -> int:
-    """The sort's metrics (streaming/sort.py get_metric; 1-5 read 0) and 9, the number of partitions."""
+    """The sort's metrics (streaming/sort.py get_metric; 1-5 read 0) and 9, the number of partitions.  A sharded window reports
+    this rank's local window (metric 0 the rows it received, 9 the partitions it owns)."""
+    if isinstance(state, ShardedWindowState):
+        state = state.local
     return int(_lib.lib().b200_sort_get_metric(state.handle, which))

@@ -544,6 +544,14 @@ int b200_shuffle_partition(const b200_table* in_table, int64_t n_keys, int32_t n
 int b200_shuffle_partition_perm(const b200_table* in_table, int64_t n_keys, int32_t n_pes,
                                 b200_table* out, int64_t* send_counts, int64_t* perm_out_dev,
                                 void* stream);
+/* The same partition by key class: rows whose keys are equal as the window, the sort and the groupby compare them go to one
+ * rank.  NA and a float NaN are one class (both hash as hash_na_val), -0.0 equals 0.0, and every fixed-width key type is
+ * accepted: bool, 1-, 2-, 4- and 8-byte integers (a 1- or 2-byte key hashes as the 4-byte integer of its value), float32 /
+ * float64, DATE, DATETIME and TIMEDELTA, numpy or nullable.  On keys of 4 or 8 bytes without a valid NaN the placement is
+ * b200_shuffle_partition's.  perm_out_dev (device int64[n_rows]) may be NULL. */
+int b200_shuffle_partition_classes(const b200_table* in_table, int64_t n_keys, int32_t n_pes,
+                                   b200_table* out, int64_t* send_counts, int64_t* perm_out_dev,
+                                   void* stream);
 
 /* Receive side of shuffle_table: turns the n_src per-source validity segments (each ceil(counts[j]/8) bytes, back to
  * back, in source-rank order — what the all-to-all-v of the per-destination bitmaps delivers) into one contiguous Arrow
